@@ -48,6 +48,7 @@ struct DevBuf {
     template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+constexpr int KA_MAX_BLOCKS = 8;          // topic blocks of a pipelined solve
 constexpr int KA_MAX_CHAIN_BLOCKS = 8;    // slot-chain sub-blocks per staged block
 constexpr int KA_MAX_CHAIN_EVENTS = 64;   // per solve: 8 staged blocks x 8 sub-blocks
 
@@ -57,67 +58,85 @@ struct HostPinned {
     int4 tstatus;
 };
 
+struct Plan {
+    // kernel A
+    int a_warps, a_load_bytes, a_slab_bytes, a_cnt_bytes, a_load_kind;  // kind 0=u8 1=u16 2=u32
+    int a_levels;                                   // 1: some topic may hold a broker twice -> conflict levels + tables
+    int lv_owner_bytes, lv_last_bytes, lv_p_bytes;  // per-warp scratch of the level pass
+    size_t a_smem;
+    // leader order
+    int rec_kind, rec_bytes;  // 3: 16 B records (rows <= 3), 4 / 8: 32 B records (rows of 4 / 5..8)
+    int b_gctr;               // counters stay in global memory (table too large for shared memory)
+    int b_ring_log2;          // log2(records per TMA ring stage)
+    int b_threads;
+    size_t b_smem;
+};
+
+// One contiguous block of topics of a dense or ragged problem, with every device pointer already offset to the block.
+struct StageDesc {
+    int topic_base = 0, T = 0;
+    int64_t Q = 0;                  // partitions in the block
+    const int32_t* d_hash = nullptr;
+    const int64_t* d_part_off = nullptr;  // ragged only (block == whole problem)
+    const int64_t* d_rep_off = nullptr;
+    int P = 0, RF = 0;
+    const int32_t* d_cur = nullptr;
+    int desired_rf = -1, S = 1, Pmax = 0;
+    int64_t capmax = 0;
+    int64_t q0 = 0;                 // first partition row of the block inside the ctx scratch arrays
+    int blk = 0;                    // ordinal of the block inside a pipelined solve (its level tables: loff at topic_base + blk)
+    Plan pl;
+};
+
 }  // namespace
 
 struct ka_ctx {
     int device = 0;
     int sm_count = KA_SM_COUNT_FALLBACK;
     cudaStream_t stream = nullptr;  // used by the host-buffer entry points
+    cudaStream_t aux = nullptr;     // stage of the pipelined (super-chunk) solve
+    cudaStream_t sb1 = nullptr;     // slot-0 chains (the slot-1 chains + emit run on the caller's stream)
+    cudaStream_t sj = nullptr;      // device JSON emission, streamed copy-out
     // broker table
     int N = 0;
     std::vector<int32_t> broker_id;
-    std::vector<int32_t> broker_rack;
     int lut_mode = KA_LUT_SMEM;
     int min_id = 0;
     uint32_t range = 0;
-    int blob_bytes = 16;
+    int blob_bytes = 0;    // rack16 || lut16, staged whole into kernel A's shared memory (none before ka_ctx_set_brokers)
     int lut_off = 0;
-    int R = 0, roff_off = 0, memb_off = 0;
     DevBuf d_blob, d_glut, d_broker_id, d_ctr8;
     // counters of brokers not in the current table (Context.counter is keyed by broker id)
     std::unordered_map<int32_t, std::vector<int32_t>> parked;
+    int64_t launches = 0;
     // scratch
     DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len, d_tstatus, d_flags;
     DevBuf d_rec, d_perm, d_ntl, d_loff, d_lend, d_lvl_end;  // records, chosen positions, schedule permutation, level tables
+    DevBuf d_json, d_names, d_name_off, d_json_rowlen, d_json_blocksum, d_json_state;
     HostPinned* h_pin = nullptr;
-    // bookkeeping
+    unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_CHAIN_EVENTS][2]: {first byte, bytes} of every JSON fragment
+    // timing events (recorded only with timing on)
+    cudaEvent_t ev[6] = {};                                // solve: start, inputs in, kernel A done, stage done, chains done, end
+    cudaEvent_t ev_pipe[KA_MAX_BLOCKS][5] = {};            // pipelined block: stage start, kernel A done, stage done, chains start / done
+    cudaEvent_t ev_chain[KA_MAX_CHAIN_EVENTS][4] = {};     // chain sub-block: slot-0 chain start / done, slot-1 chain + emit start / done
+    // cross-stream events
+    cudaEvent_t ev_in = nullptr, ev_stage[KA_MAX_BLOCKS] = {}, ev_chain_in = nullptr, ev_b1[KA_MAX_CHAIN_EVENTS] = {};
+    cudaEvent_t ev_json_in[KA_MAX_CHAIN_EVENTS] = {}, ev_json_scan[KA_MAX_CHAIN_EVENTS] = {}, ev_out_done = nullptr;
+    // timing of the last solve
     bool timing = false;
-    cudaEvent_t ev[10] = {};
     float last_ms[8] = {};
     bool ev_valid = false;
-    cudaEvent_t ev_mark = nullptr;  // where enq_sticky_hist records 'kernel A done' (timing only)
-    int64_t launches = 0;
-    int topic_base = 0;       // ka_ctx_set_topic_base: index of the staged block's first topic in the whole (multi-GPU) run
-    bool last_was_staged = false;
-    int order_threads = 0;  // leader-order CTA size override (0 = heuristic from N); env KA_ORDER_THREADS wins
-    // second stream + events for the pipelined (super-chunk) solve
-    cudaStream_t aux = nullptr;
-    cudaStream_t sb1 = nullptr;             // slot-0 chain stream (the slot-1 chain + emit run on the caller's stream)
-    cudaEvent_t ev_chain_in = nullptr, ev_b1[KA_MAX_CHAIN_EVENTS] = {}, ev_chain[KA_MAX_CHAIN_EVENTS][4] = {};
-    int chain_ev_next = 0, chain_used = 0;
-    // device-side JSON emission (ka_solve_dense_json)
-    cudaStream_t sj = nullptr;
-    cudaEvent_t ev_json_in[KA_MAX_CHAIN_EVENTS] = {}, ev_json_scan[KA_MAX_CHAIN_EVENTS] = {};
-    DevBuf d_json, d_names, d_name_off, d_json_rowlen, d_json_blocksum, d_json_state;
-    unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_CHAIN_EVENTS][2]: {first byte, bytes} of every fragment
-    struct JsonJob* json_job = nullptr;
-    // host destination of a pipelined host-buffer solve: every chain sub-block is copied out on c->sj as soon as its emit is
-    // done, so that no D2H sits between two slot-1 chains on the caller's stream
-    int32_t* host_out = nullptr; int32_t* host_out_len = nullptr; int32_t* dev_out = nullptr; int32_t* dev_out_len = nullptr;
-    int out_copies = 0;
-    cudaEvent_t ev_out_done = nullptr;    // non-null while run_dense serves ka_solve_dense_json
-    bool slot_timed[2] = {false, false};   // ka_order_slot_device recorded ev_chain[slot][0..1]
-    cudaEvent_t ev_in = nullptr, ev_stage[8] = {};
-    cudaEvent_t ev_pipe[8][5] = {};
     int last_stages = 1;
+    int chain_used = 0;                    // ev_chain rows recorded
+    bool slot_timed[2] = {false, false};   // ka_order_slot_device recorded ev_chain[slot][0..1]
     // staged problem (between the context-free stage and the leader-order stage)
     bool staged = false;
-    struct StagedBlock* staged_block = nullptr;  // StageDesc of ka_stage_dense_device, consumed by ka_order_device
+    StageDesc staged_block;
+    int topic_base = 0;       // ka_ctx_set_topic_base: index of the staged block's first topic in the whole (multi-GPU) run
     // async status
+    bool last_was_staged = false;
     cudaStream_t last_stream = nullptr;
     bool pending_status = false;
-    const int32_t* last_part_id = nullptr;  // host pointer (ragged API) for status translation
-    const int64_t* last_part_off = nullptr;
     ka_status last{};
 };
 
@@ -144,7 +163,32 @@ int set_status(ka_status* st, int code, int topic = -1, int part = -1, int a = 0
     return code;
 }
 
+// An internal step failed with rc: report it in *st, unless *st already holds rc with its details (make_plan's limits).
+int failed(ka_status* st, int rc) {
+    if (st && st->code != rc) set_status(st, rc);
+    return rc;
+}
+
 inline size_t align16(size_t v) { return (v + 15) & ~size_t(15); }
+
+// Every event of the ctx, with whether it is timed.
+template <typename F>
+void for_each_event(ka_ctx* c, F f) {
+    const struct { cudaEvent_t* e; size_t n; bool timed; } pools[] = {
+        {c->ev, sizeof(c->ev) / sizeof(cudaEvent_t), true},
+        {&c->ev_pipe[0][0], sizeof(c->ev_pipe) / sizeof(cudaEvent_t), true},
+        {&c->ev_chain[0][0], sizeof(c->ev_chain) / sizeof(cudaEvent_t), true},
+        {&c->ev_in, 1, false},
+        {c->ev_stage, KA_MAX_BLOCKS, false},
+        {&c->ev_chain_in, 1, false},
+        {c->ev_b1, KA_MAX_CHAIN_EVENTS, false},
+        {c->ev_json_in, KA_MAX_CHAIN_EVENTS, false},
+        {c->ev_json_scan, KA_MAX_CHAIN_EVENTS, false},
+        {&c->ev_out_done, 1, false},
+    };
+    for (const auto& p : pools)
+        for (size_t i = 0; i < p.n; ++i) f(p.e[i], p.timed);
+}
 
 // download current device counters into ctx->parked keyed by id
 int park_counters(ka_ctx* c) {
@@ -161,21 +205,6 @@ int park_counters(ka_ctx* c) {
     return KA_OK;
 }
 
-struct Plan {
-    // kernel A
-    int a_warps, a_load_bytes, a_slab_bytes, a_cnt_bytes, a_load_kind;  // kind 0=u8 1=u16 2=u32
-    int a_rackptr, a_rp_bytes, a_blob_bytes;
-    int a_levels;                                   // 1: some topic may hold a broker twice -> conflict levels + tables
-    int lv_owner_bytes, lv_last_bytes, lv_p_bytes;  // per-warp scratch of the level pass
-    size_t a_smem;
-    // leader order
-    int rec_kind, rec_bytes;  // 3: 16 B records (rows <= 3), 4 / 8: 32 B records (rows of 4 / 5..8)
-    int b_gctr;               // counters stay in global memory (table too large for shared memory)
-    int b_ring_log2;          // log2(records per TMA ring stage)
-    int b_threads;
-    size_t b_smem;
-};
-
 constexpr size_t KA_ORDER_SMEM_BUDGET = 226 * 1024;
 
 int make_plan(ka_ctx* c, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged, Plan& pl, ka_status* st) {
@@ -187,24 +216,15 @@ int make_plan(ka_ctx* c, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged
     pl.a_load_bytes = (int)align16((size_t)std::max(N, 1) * lsz);
     pl.a_slab_bytes = (int)align16((size_t)std::max(Pmax, 1) * S * 2);
     pl.a_cnt_bytes = (int)align16((size_t)std::max(Pmax, 1));
-    // spread phase: window scan over the rotated order by default (measured faster on every BASELINE config: the
-    // monotone head finds a slot within ~1 window); KA_SPREAD_RACKPTR=1 selects the per-rack first-free-pointer
-    // variant (exact too; pays off only when walks are long: many full nodes AND tight rack constraints).
-    pl.a_rackptr = 0;
-    if (const char* e = std::getenv("KA_SPREAD_RACKPTR")) pl.a_rackptr = std::atoi(e) && c->R > 0 && c->R <= 4096;
-    pl.a_rp_bytes = pl.a_rackptr ? (int)align16((size_t)c->R * 2) : 0;
     // capacity 1 == every broker holds at most one partition of a topic == the topic is a single conflict level
     pl.a_levels = (capmax > 1 || ragged) ? 1 : 0;
-    if (const char* e = std::getenv("KA_FORCE_LEVELS")) pl.a_levels = pl.a_levels || std::atoi(e);
     if (pl.a_levels && Pmax > 32767) return set_status(st, KA_ERR_LIMIT, -1, -1, Pmax, N);  // level cursors are 15-bit
     pl.lv_owner_bytes = pl.a_levels ? (int)align16((size_t)std::max(N, 1) * 4) : 0;
     pl.lv_last_bytes = pl.a_levels ? (int)align16((size_t)std::max(N, 1) * 2) : 0;
     pl.lv_p_bytes = pl.a_levels ? (int)align16((size_t)(std::max(Pmax, 1) + 2) * 2) : 0;
-    const size_t per_warp = (size_t)pl.a_load_bytes + pl.a_slab_bytes + pl.a_cnt_bytes + 3 * (size_t)pl.a_rp_bytes +
-                            pl.lv_owner_bytes + pl.lv_last_bytes + 2 * (size_t)pl.lv_p_bytes;
-    // the rack member lists (last part of the blob) are only read by the opt-in rack-pointer spread: not staged otherwise
-    pl.a_blob_bytes = pl.a_rackptr ? c->blob_bytes : c->roff_off * 2;
-    const size_t shared = 16 + (size_t)pl.a_blob_bytes;
+    const size_t per_warp = (size_t)pl.a_load_bytes + pl.a_slab_bytes + pl.a_cnt_bytes + pl.lv_owner_bytes + pl.lv_last_bytes +
+                            2 * (size_t)pl.lv_p_bytes;
+    const size_t shared = 16 + (size_t)c->blob_bytes;
     if (shared + per_warp > KA_SMEM_BUDGET) return set_status(st, KA_ERR_LIMIT, -1, -1, Pmax, N);
     pl.a_warps = (int)std::min<size_t>(16, (KA_SMEM_BUDGET - shared) / per_warp);
     pl.a_smem = shared + per_warp * pl.a_warps;
@@ -235,7 +255,6 @@ int make_plan(ka_ctx* c, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged
     const int64_t cuts = (std::max<int64_t>(width, 1) + max_nt - 1) / max_nt;
     width = (std::max<int64_t>(width, 1) + cuts - 1) / cuts;
     int nt = (int)std::min<int64_t>(max_nt, ((width + 31) / 32) * 32);
-    if (c->order_threads > 0) nt = c->order_threads;
     if (const char* e = std::getenv("KA_ORDER_THREADS")) nt = std::atoi(e);
     nt = std::max(32, std::min(max_nt, (nt / 32) * 32));
     nt = std::min(nt, (KA_RING_STAGES - 1) << lg);
@@ -248,38 +267,75 @@ cudaError_t allow_smem(K kernel, size_t bytes) {
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
 }
 
-// One contiguous block of topics of a dense or ragged problem, with every device pointer already offset to the block.
-struct StageDesc {
-    int topic_base = 0, T = 0;
-    int64_t Q = 0;                  // partitions in the block
+// A whole problem with its inputs on the device: dense (P partitions of RF replicas per topic), or ragged (d_part_off /
+// d_rep_off set, with Q, R, Pmax and capmax from the host-side sizing scan; a ragged problem is always one block).
+struct Shape {
+    int T = 0, P = 0, RF = 0, desired_rf = -1, S = 1;
     const int32_t* d_hash = nullptr;
-    const int64_t* d_part_off = nullptr;  // ragged only (block == whole problem)
-    const int64_t* d_rep_off = nullptr;
-    int P = 0, RF = 0;
     const int32_t* d_cur = nullptr;
-    int desired_rf = -1, S = 1, Pmax = 0;
+    const int64_t* d_part_off = nullptr;
+    const int64_t* d_rep_off = nullptr;
+    int64_t Q = 0, R = 0;  // partitions, current replicas
+    int Pmax = 0;
     int64_t capmax = 0;
-    int64_t q0 = 0;                 // first partition row of the block inside the ctx scratch arrays
-    int blk = 0;                    // ordinal of the block inside a pipelined solve (its level tables: loff at topic_base + blk)
-    Plan pl;
 };
 
-}  // namespace
-struct StagedBlock { StageDesc d; };
-namespace {
+// The planned StageDesc of topics [t0, t1) of a problem, block `blk` of its solve.
+int describe_block(ka_ctx* c, const Shape& sh, int t0, int t1, int blk, StageDesc& d, ka_status* st) {
+    const bool ragged = sh.d_part_off != nullptr;
+    d = StageDesc();
+    d.topic_base = t0;
+    d.T = t1 - t0;
+    d.blk = blk;
+    d.q0 = (int64_t)t0 * sh.P;
+    d.Q = ragged ? sh.Q : (int64_t)d.T * sh.P;
+    d.d_hash = sh.d_hash + t0;
+    d.d_part_off = sh.d_part_off;
+    d.d_rep_off = sh.d_rep_off;
+    d.P = sh.P;
+    d.RF = sh.RF;
+    d.d_cur = sh.d_cur + d.q0 * sh.RF;
+    d.desired_rf = sh.desired_rf;
+    d.S = sh.S;
+    if (ragged) {
+        d.Pmax = sh.Pmax;
+        d.capmax = sh.capmax;
+    } else {
+        const int rf_t = sh.desired_rf >= 0 ? sh.desired_rf : sh.RF;
+        d.Pmax = sh.P;
+        d.capmax = c->N > 0 ? ((int64_t)sh.P * std::max(rf_t, 0) + c->N - 1) / c->N : 0;
+    }
+    return make_plan(c, d.Q, d.S, d.Pmax, d.capmax, ragged, d.pl, st);
+}
 
-int reserve_scratch(ka_ctx* c, int64_t Qtot, int rec_bytes, int Ttot, int blocks, bool levels) {
-    const size_t q = (size_t)std::max<int64_t>(Qtot, 1);
-    KA_CUDA(c->d_rec.reserve(q * rec_bytes + 256));
-    if (levels) {
+// Scratch of a solve of the blocks ds[0..K) (consecutive: the last one ends the problem).
+int reserve_scratch(ka_ctx* c, const StageDesc* ds, int K) {
+    const StageDesc& e = ds[K - 1];
+    const size_t q = (size_t)std::max<int64_t>(e.q0 + e.Q, 1);
+    const int T = e.topic_base + e.T;
+    KA_CUDA(c->d_rec.reserve(q * ds[0].pl.rec_bytes + 256));
+    if (ds[0].pl.a_levels) {
         KA_CUDA(c->d_perm.reserve(q * 2));
         KA_CUDA(c->d_lend.reserve(q * 4));
         KA_CUDA(c->d_lvl_end.reserve(q * 4));
-        KA_CUDA(c->d_ntl.reserve((size_t)std::max(Ttot, 1) * 4));
-        KA_CUDA(c->d_loff.reserve((size_t)(std::max(Ttot, 1) + blocks + 1) * 4));
+        KA_CUDA(c->d_ntl.reserve((size_t)std::max(T, 1) * 4));
+        KA_CUDA(c->d_loff.reserve((size_t)(std::max(T, 1) + K + 1) * 4));
     }
-    KA_CUDA(c->d_tstatus.reserve((size_t)std::max(Ttot, 1) * sizeof(int4)));
+    KA_CUDA(c->d_tstatus.reserve((size_t)std::max(T, 1) * sizeof(int4)));
     KA_CUDA(c->d_flags.reserve(64));
+    return KA_OK;
+}
+
+// Device copies of the inputs and rows of a host-buffer solve.
+int reserve_io(ka_ctx* c, int T, int64_t Q, int64_t R, int S, bool ragged) {
+    KA_CUDA(c->d_hash.reserve((size_t)std::max(T, 1) * 4));
+    if (ragged) {
+        KA_CUDA(c->d_part_off.reserve((size_t)(T + 1) * 8));
+        KA_CUDA(c->d_rep_off.reserve((size_t)(Q + 1) * 8));
+    }
+    KA_CUDA(c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4));
+    KA_CUDA(c->d_out.reserve((size_t)std::max<int64_t>(Q, 1) * S * 4));
+    KA_CUDA(c->d_out_len.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
     return KA_OK;
 }
 
@@ -287,7 +343,6 @@ int reserve_scratch(ka_ctx* c, int64_t Qtot, int rec_bytes, int Ttot, int blocks
 int reset_flags(ka_ctx* c, cudaStream_t s) {
     c->h_pin->err_topic = -1;
     c->h_pin->spin_flag = -1;
-    c->chain_ev_next = 0;
     c->chain_used = 0;
     c->slot_timed[0] = c->slot_timed[1] = false;
     KA_CUDA(cudaMemsetAsync(c->d_flags.p, 0xFF, 2 * sizeof(int), s));
@@ -315,7 +370,8 @@ cudaError_t launch_stage(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, cons
 }
 
 // Context-free part of a block (shards across GPUs): kernel A (records in schedule order) + the level tables.
-int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d) {
+// a_done is recorded at the end of kernel A when timing is on.
+int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done) {
     const int N = c->N, S = d.S;
     const Plan& pl = d.pl;
     if (d.T > 0) {
@@ -333,13 +389,8 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d) {
         p.Pmax = d.Pmax;
         p.N = N;
         p.blob = c->d_blob.as<uint16_t>();
-        p.blob_bytes = pl.a_blob_bytes;
+        p.blob_bytes = c->blob_bytes;
         p.lut_off = c->lut_off;
-        p.R = c->R;
-        p.rackptr = pl.a_rackptr;
-        p.roff_off = c->roff_off;
-        p.memb_off = c->memb_off;
-        p.rp_bytes = pl.a_rp_bytes;
         p.lut_mode = c->lut_mode;
         p.min_id = c->min_id;
         p.range = c->range;
@@ -366,7 +417,7 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d) {
         KA_CUDA(e);
         c->launches++;
     }
-    if (c->timing && c->ev_mark) KA_CUDA(cudaEventRecord(c->ev_mark, s));  // end of kernel A
+    if (c->timing) KA_CUDA(cudaEventRecord(a_done, s));
     if (pl.a_levels && d.T > 0) {
         int32_t* ntl = c->d_ntl.as<int32_t>() + d.topic_base;
         int32_t* loff = c->d_loff.as<int32_t>() + d.topic_base + d.blk;  // every block keeps T_k + 1 entries
@@ -423,32 +474,57 @@ int chain_subblocks(const StageDesc& d, int blocks_in_solve) {
     return std::min(n, KA_MAX_CHAIN_BLOCKS);
 }
 
-}  // namespace
-struct JsonJob {
-    int32_t* d_out;        // the solve's rows (device)
-    int32_t* d_out_len;
-    int S;
-    int blocks = 0;
+// Per-call state of one solve: where its inputs come from and its rows go, and how far its enqueue has got. Lives on the
+// stack of the entry point.
+struct SolveCall {
+    // host-buffer entry points: inputs of the whole problem in host memory, copied H2D block by block (null: on the device)
+    const int32_t* h_hash = nullptr;
+    const int32_t* h_cur = nullptr;
+    const int64_t* h_part_off = nullptr;  // ragged
+    const int64_t* h_rep_off = nullptr;
+    // rows of the whole problem on the device, and their host destination (null: they stay on the device)
+    int32_t* d_out = nullptr;
+    int32_t* d_out_len = nullptr;
+    int32_t* h_out = nullptr;
+    int32_t* h_out_len = nullptr;
+    bool json = false;        // ka_solve_dense_json: rows -> JSON text on c->sj as soon as they are final
+    // pipelined host-buffer solve, rows <= 3: every chain sub-block is copied out on c->sj as soon as its emit is done, so
+    // that no D2H sits between two slot-1 chains on the caller's stream
+    bool stream_out = false;
+    int out_copies = 0;       // sub-block copies handed to c->sj (ev_json_in)
+    int json_blocks = 0;      // JSON fragments enqueued (ev_json_in, ev_json_scan, h_frag)
+    int chains = 0;           // chain sub-blocks enqueued (ev_chain, ev_b1)
 };
-namespace {
 
-// KAG:169-186 for a finished range of rows (a chain sub-block): rows -> JSON text at the running offset of d_json, on c->sj.
-int enq_json_rows(ka_ctx* c, cudaStream_t s_done, int64_t row0, int64_t rows, int topic0, int P, bool first, bool last) {
-    JsonJob* jj = c->json_job;
-    const int k = jj->blocks;
+struct SubBlock { int t0, t1; int64_t r0, rq; };
+
+SubBlock sub_block(const StageDesc& d, int j, int nsub) {
+    SubBlock b;
+    b.t0 = (int)((int64_t)d.T * j / nsub);
+    b.t1 = (int)((int64_t)d.T * (j + 1) / nsub);
+    // ragged blocks are never cut (nsub == 1): sub-block rows follow from the dense shape
+    b.r0 = d.d_part_off ? 0 : (int64_t)b.t0 * d.P;
+    b.rq = d.d_part_off ? d.Q : (int64_t)(b.t1 - b.t0) * d.P;
+    return b;
+}
+
+// KAG:169-186 for a finished range of rows (sub-block b of block d): rows -> JSON text at the running offset of d_json, on c->sj.
+int enq_json_rows(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc& d, const SubBlock& b, bool first, bool last) {
+    const int k = io.json_blocks;
     if (k >= KA_MAX_CHAIN_EVENTS) return KA_ERR_LIMIT;
+    const int64_t row0 = d.q0 + b.r0, rows = b.rq;
     KA_CUDA(cudaEventRecord(c->ev_json_in[k], s_done));
     KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_json_in[k], 0));
     KaJsonParams p{};
     p.Q = (uint32_t)rows;
     p.row0 = (uint32_t)row0;
-    p.P = std::max(P, 1);
-    p.topic0 = topic0;
+    p.P = std::max(d.P, 1);
+    p.topic0 = d.topic_base + b.t0;
     p.name_off = c->d_name_off.as<int64_t>();
     p.names = c->d_names.as<char>();
-    p.out = jj->d_out + row0 * jj->S;
-    p.out_len = jj->d_out_len + row0;
-    p.S = jj->S;
+    p.out = io.d_out + row0 * d.S;
+    p.out_len = io.d_out_len + row0;
+    p.S = d.S;
     p.rowlen = c->d_json_rowlen.as<uint32_t>() + row0;
     p.blocksum = c->d_json_blocksum.as<uint32_t>() + (row0 / 256) + k;
     p.total = c->d_json_state.as<unsigned long long>();
@@ -466,27 +542,20 @@ int enq_json_rows(ka_ctx* c, cudaStream_t s_done, int64_t row0, int64_t rows, in
     KA_CUDA(cudaMemcpyAsync(c->h_frag + 2 * k, p.frag, 16, cudaMemcpyDeviceToHost, c->sj));
     KA_CUDA(cudaEventRecord(c->ev_json_scan[k], c->sj));
     c->launches += 3;
-    jj->blocks = k + 1;
+    io.json_blocks = k + 1;
     return KA_OK;
 }
 
-struct SubBlock { int t0, t1; int64_t r0, rq; };
-
-SubBlock sub_block(const StageDesc& d, int j, int nsub) {
-    SubBlock b;
-    b.t0 = (int)((int64_t)d.T * j / nsub);
-    b.t1 = (int)((int64_t)d.T * (j + 1) / nsub);
-    // ragged blocks are never cut (nsub == 1): sub-block rows follow from the dense shape
-    b.r0 = d.d_part_off ? 0 : (int64_t)b.t0 * d.P;
-    b.rq = d.d_part_off ? d.Q : (int64_t)(b.t1 - b.t0) * d.P;
-    return b;
+// D2H of rows [r0, r0 + rows) of a solve's output.
+int enq_copy_out(cudaStream_t s, const SolveCall& io, int S, int64_t r0, int64_t rows) {
+    KA_CUDA(cudaMemcpyAsync(io.h_out + r0 * S, io.d_out + r0 * S, (size_t)rows * S * 4, cudaMemcpyDeviceToHost, s));
+    if (io.h_out_len) KA_CUDA(cudaMemcpyAsync(io.h_out_len + r0, io.d_out_len + r0, (size_t)rows * 4, cudaMemcpyDeviceToHost, s));
+    return KA_OK;
 }
 
-// One slot chain (rows <= 3) over sub-block j of a staged block.
-int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int j, int nsub) {
+// Leader-order parameters of sub-block b of a staged block.
+KaOrderParams order_params(ka_ctx* c, const StageDesc& d, const SubBlock& b) {
     const Plan& pl = d.pl;
-    const SubBlock b = sub_block(d, j, nsub);
-    if (b.rq <= 0 || c->N <= 0) return KA_OK;
     KaOrderParams o{};
     o.N = c->N;
     o.S = d.S;
@@ -500,7 +569,15 @@ int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int 
     o.pos_base = (uint32_t)b.r0;
     o.chunk_lo_ptr = loff ? loff + b.t0 : nullptr;
     o.chunk_hi_ptr = loff ? loff + b.t1 : nullptr;
-    KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, pl) : launch_order<1, 1024>(s, o, pl)));
+    return o;
+}
+
+// One slot chain (rows <= 3) over sub-block j of a staged block.
+int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int j, int nsub) {
+    const SubBlock b = sub_block(d, j, nsub);
+    if (b.rq <= 0 || c->N <= 0) return KA_OK;
+    const KaOrderParams o = order_params(c, d, b);
+    KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, d.pl) : launch_order<1, 1024>(s, o, d.pl)));
     c->launches++;
     return KA_OK;
 }
@@ -519,39 +596,30 @@ int enq_emit_block(ka_ctx* c, cudaStream_t s, const StageDesc& d, int j, int nsu
     return KA_OK;
 }
 
-// The serial chains through Context.counter (KAS:202-239) for a staged block + the parallel emit. d_out/d_out_len: the
-// block's rows. Rows <= 3: slot-0 chain on c->sb1, slot-1 chain + emit on `s`; the caller has made c->sb1 wait for the
-// stage (c->ev_chain_in recorded after kernel A / the counter import). Everything is joined back into `s`.
-int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, int32_t* d_out, int32_t* d_out_len, int blocks_in_solve) {
-    const int N = c->N, S = d.S;
+// The serial chains through Context.counter (KAS:202-239) for a staged block + the parallel emit into the block's rows of
+// io.d_out. Rows <= 3: slot-0 chain on c->sb1, slot-1 chain + emit on `s`; the caller has made c->sb1 wait for the stage
+// (c->ev_chain_in recorded after kernel A / the counter import). Everything is joined back into `s`.
+int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io, int blocks_in_solve) {
+    const int S = d.S;
     const Plan& pl = d.pl;
-    if (d.Q <= 0 || N <= 0) return KA_OK;
-    KaOrderParams o{};
-    o.N = N;
-    o.S = S;
-    o.uniform_width = pl.a_levels ? 0u : (uint32_t)d.P;
-    o.chunk_end = pl.a_levels ? c->d_lvl_end.as<uint32_t>() + d.q0 : nullptr;
-    o.ctr8 = c->d_ctr8.as<int32_t>();
-    o.broker_id = c->d_broker_id.as<int32_t>();
-    o.ring_log2 = pl.b_ring_log2;
-    const int32_t* loff = pl.a_levels ? c->d_loff.as<int32_t>() + d.topic_base + d.blk : nullptr;
-    unsigned char* rec = c->d_rec.as<unsigned char>() + (size_t)d.q0 * pl.rec_bytes;
+    if (d.Q <= 0 || c->N <= 0) return KA_OK;
+    int32_t* d_out = io.d_out + d.q0 * S;
+    int32_t* d_out_len = io.d_out_len ? io.d_out_len + d.q0 : nullptr;
     if (pl.rec_kind != 3) {  // rows of 4..8: one fused chain over all slots, rows written by the kernel
-        o.Q = (uint32_t)d.Q;
-        o.rec = rec;
-        o.chunk_lo_ptr = loff;
-        o.chunk_hi_ptr = loff ? loff + d.T : nullptr;
+        const SubBlock b = sub_block(d, 0, 1);
+        KaOrderParams o = order_params(c, d, b);
+        o.broker_id = c->d_broker_id.as<int32_t>();
         o.out = d_out;
         o.out_len = d_out_len;
         KA_CUDA((pl.rec_kind == 4 ? launch_order<4, 512>(s, o, pl) : launch_order<8, 256>(s, o, pl)));
         c->launches++;
-        if (c->json_job) return enq_json_rows(c, s, d.q0, d.Q, d.topic_base, d.P, d.blk == 0, d.blk == blocks_in_solve - 1);
+        if (io.json) return enq_json_rows(c, s, io, d, b, d.blk == 0, d.blk == blocks_in_solve - 1);
         return KA_OK;
     }
     const int nsub = chain_subblocks(d, blocks_in_solve);
     cudaStream_t s1 = c->sb1;
     for (int j = 0; j < nsub; ++j) {
-        const int e = c->chain_ev_next++ % KA_MAX_CHAIN_EVENTS;
+        const int e = io.chains % KA_MAX_CHAIN_EVENTS;
         if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][0], s1));
         int rc = enq_slot_chain(c, s1, d, 0, j, nsub);                    // slot-0 chain
         if (rc != KA_OK) return rc;
@@ -562,25 +630,22 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, int32_t* d_out
         if ((rc = enq_slot_chain(c, s, d, 1, j, nsub)) != KA_OK) return rc;   // slot-1 chain
         if ((rc = enq_emit_block(c, s, d, j, nsub, d_out, d_out_len)) != KA_OK) return rc;
         if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][3], s));
-        if (c->host_out) {   // rows of this sub-block are final: copy them out on c->sj (on `s` itself once the events run out)
-            const SubBlock b = sub_block(d, j, nsub);
-            const int64_t r = d.q0 + b.r0;
+        const SubBlock b = sub_block(d, j, nsub);
+        if (io.stream_out) {   // rows of this sub-block are final: copy them out on c->sj (on `s` itself once the events run out)
             cudaStream_t so = s;
-            if (c->out_copies < KA_MAX_CHAIN_EVENTS) {
-                KA_CUDA(cudaEventRecord(c->ev_json_in[c->out_copies], s));
-                KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_json_in[c->out_copies], 0));
-                c->out_copies++;
+            if (io.out_copies < KA_MAX_CHAIN_EVENTS) {
+                KA_CUDA(cudaEventRecord(c->ev_json_in[io.out_copies], s));
+                KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_json_in[io.out_copies], 0));
+                io.out_copies++;
                 so = c->sj;
             }
-            KA_CUDA(cudaMemcpyAsync(c->host_out + r * S, c->dev_out + r * S, (size_t)b.rq * S * 4, cudaMemcpyDeviceToHost, so));
-            if (c->host_out_len) KA_CUDA(cudaMemcpyAsync(c->host_out_len + r, c->dev_out_len + r, (size_t)b.rq * 4, cudaMemcpyDeviceToHost, so));
+            if ((rc = enq_copy_out(so, io, S, d.q0 + b.r0, b.rq)) != KA_OK) return rc;
         }
-        if (c->json_job) {   // the sub-block's rows are final: their JSON text can be built and streamed out now
-            const SubBlock b = sub_block(d, j, nsub);
-            if ((rc = enq_json_rows(c, s, d.q0 + b.r0, b.rq, d.topic_base + b.t0, d.P, d.blk == 0 && j == 0,
-                                    d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK) return rc;
+        if (io.json) {   // the sub-block's rows are final: their JSON text can be built and streamed out now
+            if ((rc = enq_json_rows(c, s, io, d, b, d.blk == 0 && j == 0, d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK)
+                return rc;
         }
-        c->chain_used = std::min(c->chain_used + 1, KA_MAX_CHAIN_EVENTS);
+        c->chain_used = std::min(++io.chains, KA_MAX_CHAIN_EVENTS);
     }
     return KA_OK;
 }
@@ -592,9 +657,13 @@ int chain_fork(ka_ctx* c, cudaStream_t s) {
     return KA_OK;
 }
 
-// status words back to pinned host memory (async)
-int enq_flags_readback(ka_ctx* c, cudaStream_t s) {
+// End of a solve on `s`: status words back to pinned host memory (async), end of the timed span.
+int enq_solve_end(ka_ctx* c, cudaStream_t s) {
     KA_CUDA(cudaMemcpyAsync(&c->h_pin->err_topic, c->d_flags.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (c->timing) {
+        KA_CUDA(cudaEventRecord(c->ev[5], s));
+        c->ev_valid = true;
+    }
     return KA_OK;
 }
 
@@ -604,116 +673,89 @@ int pipeline_stages(int T, int64_t Q) {
     // with few topics per chunk A is latency-bound and K chunks cost K times as much — measured on config 5)
     int k = Q >= 262144 ? std::min(4, T / 2048) : 1;
     if (const char* e = std::getenv("KA_PIPELINE_STAGES")) k = std::atoi(e);
-    return std::max(1, std::min(k, std::min(8, std::max(T, 1))));
+    return std::max(1, std::min(k, std::min(KA_MAX_BLOCKS, std::max(T, 1))));
 }
 
-// Whole dense solve on `s_main`, pipelined in K topic super-chunks: the aux stream runs (H2D,) kernel A and the level
-// tables of chunk k+1 while s_main runs the leader-order chain of chunk k (and the D2H of its output); s_main orders the
-// chunks strictly one after the other through the counters in ctr8.
-// h_* non-null = host-buffer form (copies inside); d_* always valid device buffers of the full problem.
-int run_dense(ka_ctx* c, cudaStream_t s_main, int T, int P, int RF, int desired_rf, int S, const int32_t* h_hash, const int32_t* h_cur,
-              int32_t* d_hash, int32_t* d_cur, int32_t* d_out, int32_t* d_out_len, int32_t* h_out, int32_t* h_out_len, ka_status* st) {
-    const int64_t Q = (int64_t)T * P;
-    const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    const int64_t capmax = c->N > 0 ? ((int64_t)P * std::max(rf_t, 0) + c->N - 1) / c->N : 0;
-    const int K = pipeline_stages(T, Q);
-    c->host_out = nullptr;
-    StageDesc ds[8];
-    // Block boundaries: the first block's H2D and the last block's D2H are the only copies that nothing overlaps, so with
-    // host buffers the end blocks get half the weight of the inner ones (1:2:..:2:1).
-    const bool host_io = (h_cur != nullptr || h_out != nullptr) && K >= 3;
-    const int wsum = host_io ? 2 * (K - 1) : K;
-    auto bound = [&](int k) { return k <= 0 ? 0 : (k >= K ? T : (int)((int64_t)T * (host_io ? 2 * k - 1 : k) / wsum)); };
-    for (int k = 0; k < K; ++k) {
-        const int t0 = bound(k), t1 = bound(k + 1);
-        StageDesc& d = ds[k];
-        d.topic_base = t0;
-        d.T = t1 - t0;
-        d.q0 = (int64_t)t0 * P;
-        d.Q = (int64_t)d.T * P;
-        d.d_hash = d_hash + t0;
-        d.P = P;
-        d.RF = RF;
-        d.d_cur = d_cur + d.q0 * RF;
-        d.desired_rf = desired_rf;
-        d.S = S;
-        d.Pmax = P;
-        d.capmax = capmax;
-        d.blk = k;
-        int rc = make_plan(c, d.Q, S, P, capmax, false, d.pl, st);
-        if (rc != KA_OK) return rc;
-    }
-    int rc = reserve_scratch(c, Q, ds[0].pl.rec_bytes, T, K, ds[0].pl.a_levels != 0);
-    if (rc != KA_OK) return set_status(st, rc);
-    c->last_stages = K;
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev[0], s_main));
-    if (K == 1) {
-        cudaStream_t s = s_main;
-        StageDesc& d = ds[0];
-        if (h_hash && T > 0) KA_CUDA(cudaMemcpyAsync(d_hash, h_hash, (size_t)T * 4, cudaMemcpyHostToDevice, s));
-        if (h_cur && Q * RF > 0) KA_CUDA(cudaMemcpyAsync(d_cur, h_cur, (size_t)Q * RF * 4, cudaMemcpyHostToDevice, s));
-        if ((rc = reset_flags(c, s)) != KA_OK) return rc;
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev[1], s));
-        c->ev_mark = c->ev[2];
-        if ((rc = enq_stage(c, s, d)) != KA_OK) return rc;
-        c->ev_mark = nullptr;
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev[3], s));
-        if ((rc = chain_fork(c, s)) != KA_OK) return rc;
-        if ((rc = enq_order_emit(c, s, d, d_out, d_out_len, 1)) != KA_OK) return rc;
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev[4], s));
-
-        if (h_out && Q > 0 && c->N > 0) {
-            KA_CUDA(cudaMemcpyAsync(h_out, d_out, (size_t)Q * S * 4, cudaMemcpyDeviceToHost, s));
-            if (h_out_len) KA_CUDA(cudaMemcpyAsync(h_out_len, d_out_len, (size_t)Q * 4, cudaMemcpyDeviceToHost, s));
-        }
-    } else {
-        cudaStream_t aux = c->aux;
-        const bool stream_out = h_out && ds[0].pl.rec_kind == 3 && !c->json_job;
-        c->host_out = stream_out ? h_out : nullptr;
-        c->host_out_len = stream_out ? h_out_len : nullptr;
-        c->dev_out = d_out;
-        c->dev_out_len = d_out_len;
-        c->out_copies = 0;
-        KA_CUDA(cudaEventRecord(c->ev_in, s_main));           // inputs ready / earlier work on s_main done
-        if (stream_out) KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_in, 0));
-        KA_CUDA(cudaStreamWaitEvent(aux, c->ev_in, 0));
-        if ((rc = reset_flags(c, aux)) != KA_OK) return rc;
-        for (int k = 0; k < K; ++k) {
-            StageDesc& d = ds[k];
-            if (h_hash && d.T > 0) KA_CUDA(cudaMemcpyAsync(d_hash + d.topic_base, h_hash + d.topic_base, (size_t)d.T * 4, cudaMemcpyHostToDevice, aux));
-            if (h_cur && d.Q * RF > 0)
-                KA_CUDA(cudaMemcpyAsync(d_cur + d.q0 * RF, h_cur + d.q0 * RF, (size_t)d.Q * RF * 4, cudaMemcpyHostToDevice, aux));
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][0], aux));
-            c->ev_mark = c->timing ? c->ev_pipe[k][1] : nullptr;
-            if ((rc = enq_stage(c, aux, d)) != KA_OK) return rc;
-            c->ev_mark = nullptr;
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][2], aux));
-            KA_CUDA(cudaEventRecord(c->ev_stage[k], aux));
-            KA_CUDA(cudaStreamWaitEvent(s_main, c->ev_stage[k], 0));
-            KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_stage[k], 0));
-            if (k == 0) KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_in, 0));
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][3], s_main));
-            if ((rc = enq_order_emit(c, s_main, d, d_out + d.q0 * S, d_out_len ? d_out_len + d.q0 : nullptr, K)) != KA_OK) return rc;
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][4], s_main));
-
-            if (h_out && d.Q > 0 && c->N > 0 && !c->host_out) {   // rows of 4..8: one copy per block on the caller's stream
-                KA_CUDA(cudaMemcpyAsync(h_out + d.q0 * S, d_out + d.q0 * S, (size_t)d.Q * S * 4, cudaMemcpyDeviceToHost, s_main));
-                if (h_out_len) KA_CUDA(cudaMemcpyAsync(h_out_len + d.q0, d_out_len + d.q0, (size_t)d.Q * 4, cudaMemcpyDeviceToHost, s_main));
-            }
-        }
-    }
-    if (c->host_out) {   // join the copy-out stream back into the caller's stream
-        KA_CUDA(cudaEventRecord(c->ev_out_done, c->sj));
-        KA_CUDA(cudaStreamWaitEvent(s_main, c->ev_out_done, 0));
-        c->host_out = nullptr;
-    }
-    if ((rc = enq_flags_readback(c, s_main)) != KA_OK) return rc;
-    if (c->timing) { KA_CUDA(cudaEventRecord(c->ev[5], s_main)); c->ev_valid = true; }
+// H2D of the host inputs of block d (ncur current replicas).
+int enq_inputs(cudaStream_t s, const SolveCall& io, const StageDesc& d, int64_t ncur) {
+    // the destinations are the ctx's scratch copies (a host-buffer solve's StageDesc points into them)
+    auto h2d = [&](const void* dst, const void* src, size_t bytes) {
+        return cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, s);
+    };
+    if (io.h_hash && d.T > 0) KA_CUDA(h2d(d.d_hash, io.h_hash + d.topic_base, (size_t)d.T * 4));
+    if (io.h_part_off && d.T > 0) KA_CUDA(h2d(d.d_part_off, io.h_part_off, (size_t)(d.T + 1) * 8));
+    if (io.h_rep_off && d.Q > 0) KA_CUDA(h2d(d.d_rep_off, io.h_rep_off, (size_t)(d.Q + 1) * 8));
+    if (io.h_cur && ncur > 0) KA_CUDA(h2d(d.d_cur, io.h_cur + d.q0 * d.RF, (size_t)ncur * 4));
     return KA_OK;
 }
 
-// Wait for the stream, translate device flags into a ka_status.
-int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st) {
+// A whole solve on the caller's stream `s`: H2D -> flags reset -> stage -> chain fork -> order/emit -> copy-out -> flags
+// readback. Dense problems large enough are pipelined in K topic super-chunks: c->aux runs (the H2D,) kernel A and the
+// level tables of chunk k+1 while `s` runs the leader-order chains of chunk k (and the D2H of its output); `s` orders the
+// chunks strictly one after the other through the counters in ctr8.
+int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_status* st) {
+    c->staged = false;   // the solve reuses the scratch a staged block lives in
+    c->last_was_staged = false;
+    const bool ragged = sh.d_part_off != nullptr;
+    const int T = sh.T;
+    const int K = ragged ? 1 : pipeline_stages(T, (int64_t)T * sh.P);
+    // Block boundaries: the first block's H2D and the last block's D2H are the only copies that nothing overlaps, so with
+    // host buffers the end blocks get half the weight of the inner ones (1:2:..:2:1).
+    const bool host_io = (io.h_cur != nullptr || io.h_out != nullptr) && K >= 3;
+    const int wsum = host_io ? 2 * (K - 1) : K;
+    auto bound = [&](int k) { return k <= 0 ? 0 : (k >= K ? T : (int)((int64_t)T * (host_io ? 2 * k - 1 : k) / wsum)); };
+    StageDesc ds[KA_MAX_BLOCKS];
+    int rc;
+    for (int k = 0; k < K; ++k)
+        if ((rc = describe_block(c, sh, bound(k), bound(k + 1), k, ds[k], st)) != KA_OK) return rc;
+    if ((rc = reserve_scratch(c, ds, K)) != KA_OK) return rc;
+    c->last_stages = K;
+    if (c->timing) KA_CUDA(cudaEventRecord(c->ev[0], s));
+    if (K == 1) {
+        const StageDesc& d = ds[0];
+        if ((rc = enq_inputs(s, io, d, ragged ? sh.R : d.Q * d.RF)) != KA_OK) return rc;
+        if ((rc = reset_flags(c, s)) != KA_OK) return rc;
+        if (c->timing) KA_CUDA(cudaEventRecord(c->ev[1], s));
+        if ((rc = enq_stage(c, s, d, c->ev[2])) != KA_OK) return rc;
+        if (c->timing) KA_CUDA(cudaEventRecord(c->ev[3], s));
+        if ((rc = chain_fork(c, s)) != KA_OK) return rc;
+        if ((rc = enq_order_emit(c, s, d, io, 1)) != KA_OK) return rc;
+        if (c->timing) KA_CUDA(cudaEventRecord(c->ev[4], s));
+        if (io.h_out && d.Q > 0 && c->N > 0 && (rc = enq_copy_out(s, io, d.S, 0, d.Q)) != KA_OK) return rc;
+    } else {
+        cudaStream_t aux = c->aux;
+        io.stream_out = io.h_out && ds[0].pl.rec_kind == 3 && !io.json;
+        KA_CUDA(cudaEventRecord(c->ev_in, s));           // inputs ready / earlier work on s done
+        if (io.stream_out) KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_in, 0));
+        KA_CUDA(cudaStreamWaitEvent(aux, c->ev_in, 0));
+        if ((rc = reset_flags(c, aux)) != KA_OK) return rc;
+        for (int k = 0; k < K; ++k) {
+            const StageDesc& d = ds[k];
+            if ((rc = enq_inputs(aux, io, d, d.Q * d.RF)) != KA_OK) return rc;
+            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][0], aux));
+            if ((rc = enq_stage(c, aux, d, c->ev_pipe[k][1])) != KA_OK) return rc;
+            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][2], aux));
+            KA_CUDA(cudaEventRecord(c->ev_stage[k], aux));
+            KA_CUDA(cudaStreamWaitEvent(s, c->ev_stage[k], 0));
+            KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_stage[k], 0));
+            if (k == 0) KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_in, 0));
+            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][3], s));
+            if ((rc = enq_order_emit(c, s, d, io, K)) != KA_OK) return rc;
+            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][4], s));
+            // rows of 4..8: one copy per block on the caller's stream
+            if (io.h_out && !io.stream_out && d.Q > 0 && c->N > 0 && (rc = enq_copy_out(s, io, d.S, d.q0, d.Q)) != KA_OK) return rc;
+        }
+        if (io.stream_out) {   // join the copy-out stream back into the caller's stream
+            KA_CUDA(cudaEventRecord(c->ev_out_done, c->sj));
+            KA_CUDA(cudaStreamWaitEvent(s, c->ev_out_done, 0));
+        }
+    }
+    return enq_solve_end(c, s);
+}
+
+// Wait for the stream, translate device flags into a ka_status. part_id / part_off (ragged host-buffer solve): the
+// reported partition is the failing partition's id rather than its ordinal inside the topic.
+int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st, const int32_t* part_id = nullptr, const int64_t* part_off = nullptr) {
     KA_CUDA(cudaStreamSynchronize(s));
     c->pending_status = false;
     ka_status r{};
@@ -727,7 +769,7 @@ int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st) {
         r.topic_index = t + (c->last_was_staged ? c->topic_base : 0);
         int ord = c->h_pin->tstatus.y;
         r.partition = ord;
-        if (ord >= 0 && c->last_part_id && c->last_part_off) r.partition = c->last_part_id[c->last_part_off[t] + ord];
+        if (ord >= 0 && part_id && part_off) r.partition = part_id[part_off[t] + ord];
         r.a = c->h_pin->tstatus.z;
         r.b = c->h_pin->tstatus.w;
     }
@@ -769,6 +811,22 @@ int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st) {
     c->last = r;
     if (st) *st = r;
     return r.code;
+}
+
+// Prologue of an entry point: the ctx's device current and, with `collect`, the status of the previous asynchronous solve
+// collected first (it may have run on another stream than this call's).
+int enter(ka_ctx* c, bool collect) {
+    KA_CUDA(cudaSetDevice(c->device));
+    if (collect && c->pending_status) finish_status(c, c->last_stream, nullptr);
+    return KA_OK;
+}
+
+// Everything of a solve is enqueued on `s`: its status is pending until ka_last_status, or collected now when the caller
+// asked for it (st) or the entry point is synchronous.
+int finish(ka_ctx* c, cudaStream_t s, ka_status* st, bool sync, const int32_t* part_id = nullptr, const int64_t* part_off = nullptr) {
+    c->last_stream = s;
+    c->pending_status = true;
+    return st || sync ? finish_status(c, s, st, part_id, part_off) : KA_OK;
 }
 
 }  // namespace
@@ -829,62 +887,44 @@ ka_ctx* ka_ctx_create(int32_t device) {
     c->device = device;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
-    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return nullptr; }
-    if (cudaHostAlloc(reinterpret_cast<void**>(&c->h_pin), sizeof(HostPinned), cudaHostAllocDefault) != cudaSuccess) { delete c; return nullptr; }
-    for (auto& e : c->ev) cudaEventCreate(&e);
-    if (cudaStreamCreateWithFlags(&c->aux, cudaStreamNonBlocking) != cudaSuccess) { delete c; return nullptr; }
-    if (cudaStreamCreateWithFlags(&c->sb1, cudaStreamNonBlocking) != cudaSuccess) { delete c; return nullptr; }
-    if (cudaStreamCreateWithFlags(&c->sj, cudaStreamNonBlocking) != cudaSuccess) { delete c; return nullptr; }
-    if (cudaHostAlloc(reinterpret_cast<void**>(&c->h_frag), 2 * KA_MAX_CHAIN_EVENTS * sizeof(unsigned long long), cudaHostAllocDefault) != cudaSuccess) { delete c; return nullptr; }
-    for (auto& e : c->ev_json_in) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    for (auto& e : c->ev_json_scan) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&c->ev_chain_in, cudaEventDisableTiming);
-    cudaEventCreateWithFlags(&c->ev_out_done, cudaEventDisableTiming);
-    for (auto& e : c->ev_b1) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    for (auto& row : c->ev_chain)
-        for (auto& e : row) cudaEventCreate(&e);
-    cudaEventCreateWithFlags(&c->ev_in, cudaEventDisableTiming);
-    for (auto& e : c->ev_stage) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    for (auto& row : c->ev_pipe)
-        for (auto& e : row) cudaEventCreate(&e);
+    bool ok = cudaHostAlloc(reinterpret_cast<void**>(&c->h_pin), sizeof(HostPinned), cudaHostAllocDefault) == cudaSuccess &&
+              cudaHostAlloc(reinterpret_cast<void**>(&c->h_frag), 2 * KA_MAX_CHAIN_EVENTS * sizeof(unsigned long long),
+                            cudaHostAllocDefault) == cudaSuccess;
+    for (cudaStream_t* s : {&c->stream, &c->aux, &c->sb1, &c->sj})
+        ok = ok && cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
+    for_each_event(c, [&](cudaEvent_t& e, bool timed) {
+        ok = ok && cudaEventCreateWithFlags(&e, timed ? cudaEventDefault : cudaEventDisableTiming) == cudaSuccess;
+    });
+    if (!ok) {   // release whatever was created
+        ka_ctx_destroy(c);
+        return nullptr;
+    }
     return c;
 }
 
 void ka_ctx_destroy(ka_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    if (c->stream) cudaStreamSynchronize(c->stream);
-    for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur, &c->d_rec,
-                      &c->d_perm, &c->d_ntl, &c->d_loff, &c->d_lend, &c->d_lvl_end, &c->d_out, &c->d_out_len, &c->d_tstatus, &c->d_flags})
+    for (cudaStream_t s : {c->stream, c->aux, c->sb1, c->sj})
+        if (s) cudaStreamSynchronize(s);
+    for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
+                      &c->d_out, &c->d_out_len, &c->d_tstatus, &c->d_flags, &c->d_rec, &c->d_perm, &c->d_ntl, &c->d_loff, &c->d_lend,
+                      &c->d_lvl_end, &c->d_json, &c->d_names, &c->d_name_off, &c->d_json_rowlen, &c->d_json_blocksum, &c->d_json_state})
         b->release();
-    for (auto& e : c->ev)
+    for_each_event(c, [](cudaEvent_t& e, bool) {
         if (e) cudaEventDestroy(e);
-    if (c->aux) { cudaStreamSynchronize(c->aux); cudaStreamDestroy(c->aux); }
-    if (c->sb1) { cudaStreamSynchronize(c->sb1); cudaStreamDestroy(c->sb1); }
-    if (c->sj) { cudaStreamSynchronize(c->sj); cudaStreamDestroy(c->sj); }
-    if (c->h_frag) cudaFreeHost(c->h_frag);
-    for (auto& e : c->ev_json_in) if (e) cudaEventDestroy(e);
-    for (auto& e : c->ev_json_scan) if (e) cudaEventDestroy(e);
-    for (DevBuf* b : {&c->d_json, &c->d_names, &c->d_name_off, &c->d_json_rowlen, &c->d_json_blocksum, &c->d_json_state}) b->release();
-    if (c->ev_chain_in) cudaEventDestroy(c->ev_chain_in);
-    if (c->ev_out_done) cudaEventDestroy(c->ev_out_done);
-    for (auto& e : c->ev_b1) if (e) cudaEventDestroy(e);
-    for (auto& row : c->ev_chain)
-        for (auto& e : row) if (e) cudaEventDestroy(e);
-    if (c->ev_in) cudaEventDestroy(c->ev_in);
-    for (auto& e : c->ev_stage) if (e) cudaEventDestroy(e);
-    for (auto& row : c->ev_pipe)
-        for (auto& e : row) if (e) cudaEventDestroy(e);
+    });
+    for (cudaStream_t s : {c->stream, c->aux, c->sb1, c->sj})
+        if (s) cudaStreamDestroy(s);
     if (c->h_pin) cudaFreeHost(c->h_pin);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c->staged_block;
+    if (c->h_frag) cudaFreeHost(c->h_frag);
     delete c;
 }
 
 int32_t ka_ctx_reset(ka_ctx* c) {
     if (!c) return KA_ERR_NO_DEVICE;
-    KA_CUDA(cudaSetDevice(c->device));
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);  // do not race an in-flight asynchronous solve
+    int rc = enter(c, true);   // do not race an in-flight asynchronous solve
+    if (rc != KA_OK) return rc;
     c->parked.clear();
     if (c->N > 0 && c->d_ctr8.p) KA_CUDA(cudaMemset(c->d_ctr8.p, 0, (size_t)c->N * KA_MAX_SLOTS * 4));
     return KA_OK;
@@ -898,14 +938,11 @@ int32_t ka_ctx_set_brokers(ka_ctx* c, int32_t N, const int32_t* broker_id, const
         if (i > 0 && broker_id[i] <= broker_id[i - 1]) return KA_ERR_BAD_ARG;  // strictly ascending
         if (broker_rack[i] < 0 || broker_rack[i] >= 65535) return KA_ERR_BAD_ARG;
     }
-    KA_CUDA(cudaSetDevice(c->device));
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
-    int rc = park_counters(c);
-    if (rc != KA_OK) return rc;
+    int rc = enter(c, true);
+    if (rc != KA_OK || (rc = park_counters(c)) != KA_OK) return rc;
 
     c->N = N;
     c->broker_id.assign(broker_id, broker_id + N);
-    c->broker_rack.assign(broker_rack, broker_rack + N);
     c->min_id = N > 0 ? broker_id[0] : 0;
     const uint64_t range64 = N > 0 ? (uint64_t)((int64_t)broker_id[N - 1] - (int64_t)broker_id[0]) + 1 : 0;
     const size_t npad = align16((size_t)std::max(N, 1) * 2) / 2;  // uint16 elements, 16B multiple
@@ -918,7 +955,6 @@ int32_t ka_ctx_set_brokers(ka_ctx* c, int32_t N, const int32_t* broker_id, const
             if (it == seen.end()) it = seen.emplace(broker_rack[i], (int)seen.size()).first;
             rackc[i] = (uint16_t)it->second;
         }
-        c->R = (int)seen.size();
     }
     std::vector<uint16_t> blob;
     size_t lut_elems = 0;
@@ -937,22 +973,11 @@ int32_t ka_ctx_set_brokers(ka_ctx* c, int32_t N, const int32_t* broker_id, const
         c->lut_mode = KA_LUT_BSEARCH;
         c->range = 0;
     }
-    const size_t roff_elems = align16((size_t)(c->R + 1) * 2) / 2;
     c->lut_off = (int)npad;
-    c->roff_off = (int)(npad + lut_elems);
-    c->memb_off = (int)(npad + lut_elems + roff_elems);
-    blob.assign(npad + lut_elems + roff_elems + npad, (uint16_t)KA_DEAD);
+    blob.assign(npad + lut_elems, (uint16_t)KA_DEAD);
     for (int i = 0; i < N; ++i) {
         blob[i] = rackc[i];
         if (c->lut_mode == KA_LUT_SMEM) blob[npad + (size_t)((int64_t)broker_id[i] - c->min_id)] = (uint16_t)i;
-    }
-    {   // rack member lists (CSR): sorted indices ascending inside each rack
-        std::vector<int> cntr(c->R + 1, 0);
-        for (int i = 0; i < N; ++i) cntr[rackc[i] + 1]++;
-        for (int r = 0; r < c->R; ++r) cntr[r + 1] += cntr[r];
-        for (int r = 0; r <= c->R; ++r) blob[c->roff_off + r] = (uint16_t)cntr[r];
-        std::vector<int> fill(cntr.begin(), cntr.end() - 1);
-        for (int i = 0; i < N; ++i) blob[c->memb_off + fill[rackc[i]]++] = (uint16_t)i;
     }
     c->blob_bytes = (int)(blob.size() * 2);
     KA_CUDA(c->d_blob.reserve(blob.size() * 2));
@@ -975,8 +1000,8 @@ int32_t ka_ctx_counter_slots(ka_ctx*) { return KA_MAX_SLOTS; }
 int32_t ka_ctx_get_counters(ka_ctx* c, int32_t* counter) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!counter) return KA_ERR_BAD_ARG;
-    KA_CUDA(cudaSetDevice(c->device));
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
+    int rc = enter(c, true);
+    if (rc != KA_OK) return rc;
     if (c->N > 0) KA_CUDA(cudaMemcpy(counter, c->d_ctr8.p, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToHost));
     return KA_OK;
 }
@@ -984,8 +1009,8 @@ int32_t ka_ctx_get_counters(ka_ctx* c, int32_t* counter) {
 int32_t ka_ctx_set_counters(ka_ctx* c, const int32_t* counter) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!counter) return KA_ERR_BAD_ARG;
-    KA_CUDA(cudaSetDevice(c->device));
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
+    int rc = enter(c, true);
+    if (rc != KA_OK) return rc;
     if (c->N > 0) KA_CUDA(cudaMemcpy(c->d_ctr8.p, counter, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyHostToDevice));
     return KA_OK;
 }
@@ -993,7 +1018,8 @@ int32_t ka_ctx_set_counters(ka_ctx* c, const int32_t* counter) {
 int32_t ka_ctx_export_counters_device(ka_ctx* c, int32_t* d_counter, void* stream) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!d_counter) return KA_ERR_BAD_ARG;
-    KA_CUDA(cudaSetDevice(c->device));
+    int rc = enter(c, false);
+    if (rc != KA_OK) return rc;
     if (c->N > 0)
         KA_CUDA(cudaMemcpyAsync(d_counter, c->d_ctr8.p, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return KA_OK;
@@ -1002,7 +1028,8 @@ int32_t ka_ctx_export_counters_device(ka_ctx* c, int32_t* d_counter, void* strea
 int32_t ka_ctx_import_counters_device(ka_ctx* c, const int32_t* d_counter, void* stream) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!d_counter) return KA_ERR_BAD_ARG;
-    KA_CUDA(cudaSetDevice(c->device));
+    int rc = enter(c, false);
+    if (rc != KA_OK) return rc;
     if (c->N > 0)
         KA_CUDA(cudaMemcpyAsync(c->d_ctr8.p, d_counter, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return KA_OK;
@@ -1025,7 +1052,8 @@ int64_t ka_ctx_launch_count(ka_ctx* c) { return c ? c->launches : 0; }
 
 int32_t ka_last_status(ka_ctx* c, ka_status* st) {
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    int rc = enter(c, false);
+    if (rc != KA_OK) return set_status(st, rc);
     if (c->pending_status) return finish_status(c, c->last_stream, st);
     if (st) *st = c->last;
     return c->last.code;
@@ -1046,129 +1074,93 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
                               int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
     int rc = validate_dense(c, T, P, RF, desired_rf, out_stride, st);
     if (rc != KA_OK) return rc;
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
     cudaStream_t s = (cudaStream_t)stream;
-    c->last_part_id = nullptr;
-    c->last_part_off = nullptr;
-    c->staged = false;
-    c->last_was_staged = false;
-    rc = run_dense(c, s, T, P, RF, desired_rf, out_stride, nullptr, nullptr, const_cast<int32_t*>(d_topic_hash),
-                   const_cast<int32_t*>(d_cur_broker), d_out_broker, d_out_len, nullptr, nullptr, st);
-    if (rc != KA_OK) { if (st && st->code != rc) set_status(st, rc); return rc; }
-    c->last_stream = s;
-    c->pending_status = true;
-    if (st) return finish_status(c, s, st);
-    return KA_OK;
+    SolveCall io;
+    io.d_out = d_out_broker;
+    io.d_out_len = d_out_len;
+    if ((rc = enter(c, true)) != KA_OK || (rc = run_solve(c, s, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, io, st)) != KA_OK)
+        return failed(st, rc);
+    return finish(c, s, st, false);
 }
 
 int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash, int32_t P, int32_t RF,
                               const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride, void* stream) {
     ka_status lst;
     int rc = validate_dense(c, T, P, RF, desired_rf, out_stride, &lst);
-    if (rc != KA_OK) return rc;
-    if (cudaSetDevice(c->device) != cudaSuccess) return KA_ERR_CUDA;
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
+    if (rc != KA_OK || (rc = enter(c, true)) != KA_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    c->host_out = nullptr;
-    if (!c->staged_block) c->staged_block = new StagedBlock();
-    StageDesc& d = c->staged_block->d;
-    d = StageDesc();
-    d.T = T;
-    d.Q = (int64_t)T * P;
-    d.d_hash = d_topic_hash;
-    d.P = P;
-    d.RF = RF;
-    d.d_cur = d_cur_broker;
-    d.desired_rf = desired_rf;
-    d.S = out_stride;
-    d.Pmax = P;
-    const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    d.capmax = c->N > 0 ? ((int64_t)P * std::max(rf_t, 0) + c->N - 1) / c->N : 0;
+    StageDesc& d = c->staged_block;
     c->staged = false;
-    rc = make_plan(c, d.Q, d.S, d.Pmax, d.capmax, false, d.pl, &lst);
-    if (rc != KA_OK) return rc;
-    if ((rc = reserve_scratch(c, d.Q, d.pl.rec_bytes, T, 1, d.pl.a_levels != 0)) != KA_OK) return rc;
-    c->last_part_id = nullptr;
-    c->last_part_off = nullptr;
+    if ((rc = describe_block(c, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, 0, T, 0, d, &lst)) != KA_OK ||
+        (rc = reserve_scratch(c, &d, 1)) != KA_OK)
+        return rc;
     c->last_stages = 1;
     if (c->timing) { cudaEventRecord(c->ev[0], s); cudaEventRecord(c->ev[1], s); }
-    if ((rc = reset_flags(c, s)) != KA_OK) return rc;
-    c->ev_mark = c->timing ? c->ev[2] : nullptr;
-    rc = enq_stage(c, s, d);
-    c->ev_mark = nullptr;
-    if (rc != KA_OK) return rc;
+    if ((rc = reset_flags(c, s)) != KA_OK || (rc = enq_stage(c, s, d, c->ev[2])) != KA_OK) return rc;
     if (c->timing) cudaEventRecord(c->ev[3], s);   // end of the stage (the chains may wait for another rank after this)
     c->staged = true;
     return KA_OK;
 }
 
 int32_t ka_order_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
+    set_status(st, KA_OK);
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    if (!c->staged || !c->staged_block) return set_status(st, KA_ERR_BAD_ARG);
+    int rc = enter(c, false);
+    if (rc != KA_OK) return failed(st, rc);
+    if (!c->staged) return set_status(st, KA_ERR_BAD_ARG);
     cudaStream_t s = (cudaStream_t)stream;
-    const StageDesc& d = c->staged_block->d;
-    int rc;
-    if ((rc = chain_fork(c, s)) != KA_OK) return set_status(st, rc);
-    if ((rc = enq_order_emit(c, s, d, d_out_broker, d_out_len, 1)) != KA_OK) return set_status(st, rc);
+    SolveCall io;
+    io.d_out = d_out_broker;
+    io.d_out_len = d_out_len;
+    if ((rc = chain_fork(c, s)) != KA_OK || (rc = enq_order_emit(c, s, c->staged_block, io, 1)) != KA_OK) return failed(st, rc);
     if (c->timing) cudaEventRecord(c->ev[4], s);
-    if ((rc = enq_flags_readback(c, s)) != KA_OK) return set_status(st, rc);
-    if (c->timing) { cudaEventRecord(c->ev[5], s); c->ev_valid = true; }
+    if ((rc = enq_solve_end(c, s)) != KA_OK) return failed(st, rc);
     c->staged = false;
     c->last_was_staged = true;
-    c->last_stream = s;
-    c->pending_status = true;
-    if (st) return finish_status(c, s, st);
-    return KA_OK;
+    return finish(c, s, st, false);
 }
 
 int32_t ka_staged_slot_chains(ka_ctx* c) {
-    if (!c || !c->staged || !c->staged_block) return 0;
-    return c->staged_block->d.pl.rec_kind == 3 ? 2 : 0;
+    if (!c || !c->staged) return 0;
+    return c->staged_block.pl.rec_kind == 3 ? 2 : 0;
 }
 
 int32_t ka_order_slot_device(ka_ctx* c, int32_t slot, void* stream) {
     if (!c) return KA_ERR_NO_DEVICE;
-    if (cudaSetDevice(c->device) != cudaSuccess) return KA_ERR_CUDA;
-    if (!c->staged || !c->staged_block || c->staged_block->d.pl.rec_kind != 3 || slot < 0 || slot > 1) return KA_ERR_BAD_ARG;
-    const StageDesc& d = c->staged_block->d;
+    int rc = enter(c, false);
+    if (rc != KA_OK) return rc;
+    if (!c->staged || c->staged_block.pl.rec_kind != 3 || slot < 0 || slot > 1) return KA_ERR_BAD_ARG;
+    const StageDesc& d = c->staged_block;
     cudaStream_t s = (cudaStream_t)stream;
     const int nsub = chain_subblocks(d, 1);
-    cudaEvent_t e0 = c->ev_chain[slot][0], e1 = c->ev_chain[slot][1];
-    if (c->timing) cudaEventRecord(e0, s);
-    for (int j = 0; j < nsub; ++j) {
-        int rc = enq_slot_chain(c, s, d, slot, j, nsub);
-        if (rc != KA_OK) return rc;
-    }
-    if (c->timing) cudaEventRecord(e1, s);
+    if (c->timing) cudaEventRecord(c->ev_chain[slot][0], s);
+    for (int j = 0; j < nsub; ++j)
+        if ((rc = enq_slot_chain(c, s, d, slot, j, nsub)) != KA_OK) return rc;
+    if (c->timing) cudaEventRecord(c->ev_chain[slot][1], s);
     c->slot_timed[slot] = c->timing;
     return KA_OK;
 }
 
 int32_t ka_emit_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
+    set_status(st, KA_OK);
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    if (!c->staged || !c->staged_block || c->staged_block->d.pl.rec_kind != 3 || !d_out_broker) return set_status(st, KA_ERR_BAD_ARG);
-    const StageDesc& d = c->staged_block->d;
+    int rc = enter(c, false);
+    if (rc != KA_OK) return failed(st, rc);
+    if (!c->staged || c->staged_block.pl.rec_kind != 3 || !d_out_broker) return set_status(st, KA_ERR_BAD_ARG);
     cudaStream_t s = (cudaStream_t)stream;
-    int rc;
-    if ((rc = enq_emit_block(c, s, d, 0, 1, d_out_broker, d_out_len)) != KA_OK) return set_status(st, rc);
+    if ((rc = enq_emit_block(c, s, c->staged_block, 0, 1, d_out_broker, d_out_len)) != KA_OK) return failed(st, rc);
     if (c->timing) cudaEventRecord(c->ev[4], s);
-    if ((rc = enq_flags_readback(c, s)) != KA_OK) return set_status(st, rc);
-    if (c->timing) { cudaEventRecord(c->ev[5], s); c->ev_valid = true; }
+    if ((rc = enq_solve_end(c, s)) != KA_OK) return failed(st, rc);
     c->staged = false;
     c->last_was_staged = true;
-    c->last_stream = s;
-    c->pending_status = true;
-    if (st) return finish_status(c, s, st);
-    return KA_OK;
+    return finish(c, s, st, false);
 }
 
 static int copy_counter_column(ka_ctx* c, int slot, int32_t* d_col, const int32_t* d_src, cudaStream_t s) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (slot < 0 || slot >= KA_MAX_SLOTS || (!d_col && !d_src)) return KA_ERR_BAD_ARG;
-    KA_CUDA(cudaSetDevice(c->device));
+    int rc = enter(c, false);
+    if (rc != KA_OK) return rc;
     if (c->N <= 0) return KA_OK;
     int32_t* col = c->d_ctr8.as<int32_t>() + slot;
     if (d_col) KA_CUDA(cudaMemcpy2DAsync(d_col, 4, col, KA_MAX_SLOTS * 4, 4, (size_t)c->N, cudaMemcpyDeviceToDevice, s));
@@ -1196,26 +1188,34 @@ int32_t ka_solve_dense(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t 
                        int32_t* out_len, int32_t* out_broker, ka_status* st) {
     int rc = validate_dense(c, T, P, RF, desired_rf, out_stride, st);
     if (rc != KA_OK) return rc;
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
-    cudaStream_t s = c->stream;
+    if ((rc = enter(c, true)) != KA_OK) return failed(st, rc);
     const int64_t Q = (int64_t)T * P, R = Q * RF;
     if ((T > 0 && !topic_hash) || (R > 0 && !cur_broker) || (Q > 0 && !out_broker)) return set_status(st, KA_ERR_BAD_ARG);
-    KA_CUDA(c->d_hash.reserve((size_t)std::max(T, 1) * 4));
-    KA_CUDA(c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4));
-    KA_CUDA(c->d_out.reserve((size_t)std::max<int64_t>(Q, 1) * out_stride * 4));
-    KA_CUDA(c->d_out_len.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
-    c->last_part_id = nullptr;
-    c->last_part_off = nullptr;
-    c->staged = false;
-    c->last_was_staged = false;
-    rc = run_dense(c, s, T, P, RF, desired_rf, out_stride, topic_hash, cur_broker, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(),
-                   c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>(), out_broker, out_len, st);
-    if (rc != KA_OK) { if (st && st->code != rc) set_status(st, rc); return rc; }
-    c->last_stream = s;
-    c->pending_status = true;
-    ka_status local;
-    return finish_status(c, s, st ? st : &local);
+    if ((rc = reserve_io(c, T, Q, R, out_stride, false)) != KA_OK) return failed(st, rc);
+    SolveCall io;
+    io.h_hash = topic_hash;
+    io.h_cur = cur_broker;
+    io.d_out = c->d_out.as<int32_t>();
+    io.d_out_len = c->d_out_len.as<int32_t>();
+    io.h_out = out_broker;
+    io.h_out_len = out_len;
+    const Shape sh{T, P, RF, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>()};
+    if ((rc = run_solve(c, c->stream, sh, io, st)) != KA_OK) return failed(st, rc);
+    return finish(c, c->stream, st, true);
+}
+
+// Device buffers of a JSON solve, and its topic names H2D (on c->sj, ahead of the first fragment).
+static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, const int64_t* name_off, int64_t name_bytes, int64_t json_cap) {
+    KA_CUDA(c->d_json.reserve((size_t)json_cap));
+    KA_CUDA(c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)));
+    KA_CUDA(c->d_name_off.reserve((size_t)(T + 1) * 8));
+    KA_CUDA(c->d_json_rowlen.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
+    KA_CUDA(c->d_json_blocksum.reserve((size_t)(Q / 256 + 2 * KA_MAX_CHAIN_EVENTS) * 4));
+    KA_CUDA(c->d_json_state.reserve((2 + 2 * KA_MAX_CHAIN_EVENTS) * 8));
+    KA_CUDA(cudaMemsetAsync(c->d_json_state.p, 0, (2 + 2 * KA_MAX_CHAIN_EVENTS) * 8, c->sj));
+    if (name_bytes > 0) KA_CUDA(cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, c->sj));
+    if (T > 0) KA_CUDA(cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, c->sj));
+    return KA_OK;
 }
 
 int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t P, int32_t RF, const int32_t* cur_broker,
@@ -1233,39 +1233,24 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
         const unsigned char ch = (unsigned char)names[i];
         if (ch < 0x20 || ch == '"' || ch == '\\' || ch == '/') return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)ch);
     }
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
+    if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, T, Q, R, S, false)) != KA_OK ||
+        (rc = prepare_json(c, T, Q, names, name_off, name_bytes, json_cap)) != KA_OK)
+        return failed(st, rc);
     cudaStream_t s = c->stream;
-    KA_CUDA(c->d_hash.reserve((size_t)std::max(T, 1) * 4));
-    KA_CUDA(c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4));
-    KA_CUDA(c->d_out.reserve((size_t)std::max<int64_t>(Q, 1) * S * 4));
-    KA_CUDA(c->d_out_len.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
-    KA_CUDA(c->d_json.reserve((size_t)json_cap));
-    KA_CUDA(c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)));
-    KA_CUDA(c->d_name_off.reserve((size_t)(T + 1) * 8));
-    KA_CUDA(c->d_json_rowlen.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
-    KA_CUDA(c->d_json_blocksum.reserve((size_t)(Q / 256 + 2 * KA_MAX_CHAIN_EVENTS) * 4));
-    KA_CUDA(c->d_json_state.reserve((2 + 2 * KA_MAX_CHAIN_EVENTS) * 8));
-    KA_CUDA(cudaMemsetAsync(c->d_json_state.p, 0, (2 + 2 * KA_MAX_CHAIN_EVENTS) * 8, c->sj));
-    if (name_bytes > 0) KA_CUDA(cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, c->sj));
-    if (T > 0) KA_CUDA(cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, c->sj));
-    JsonJob job{c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>(), S, 0};
-    c->json_job = &job;
-    c->last_part_id = nullptr;
-    c->last_part_off = nullptr;
-    c->staged = false;
-    c->last_was_staged = false;
-    rc = T > 0 && c->N > 0 ? run_dense(c, s, T, P, RF, desired_rf, S, topic_hash, cur_broker, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(),
-                                      c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>(), nullptr, nullptr, st)
-                            : KA_ERR_BAD_ARG;
-    c->json_job = nullptr;
-    if (rc != KA_OK) { if (st && st->code != rc) set_status(st, rc); cudaStreamSynchronize(c->sj); return rc; }
-    c->last_stream = s;
-    c->pending_status = true;
+    SolveCall io;
+    io.h_hash = topic_hash;
+    io.h_cur = cur_broker;
+    io.d_out = c->d_out.as<int32_t>();
+    io.d_out_len = c->d_out_len.as<int32_t>();
+    io.json = true;
+    const Shape sh{T, P, RF, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>()};
+    rc = T > 0 && c->N > 0 ? run_solve(c, s, sh, io, st) : KA_ERR_BAD_ARG;
+    if (rc != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
+    finish(c, s, nullptr, false);   // pending: collected below, once the fragments are out
     // every block is enqueued; stream the fragments out as their sizes become known (later blocks are still in the chains)
     int64_t total = 0;
     bool overflow = false;
-    for (int k = 0; k < job.blocks; ++k) {
+    for (int k = 0; k < io.json_blocks; ++k) {
         KA_CUDA(cudaEventSynchronize(c->ev_json_scan[k]));
         const int64_t base = (int64_t)c->h_frag[2 * k], size = (int64_t)c->h_frag[2 * k + 1];
         if (base + size > json_cap) { overflow = true; break; }
@@ -1273,8 +1258,7 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
         total = base + size;
     }
     KA_CUDA(cudaStreamSynchronize(c->sj));
-    ka_status local;
-    rc = finish_status(c, s, st ? st : &local);
+    rc = finish_status(c, s, st);
     if (rc == KA_OK && overflow) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
     if (json_bytes) *json_bytes = rc == KA_OK ? total : 0;
     return rc;
@@ -1289,8 +1273,8 @@ int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t*
     if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return set_status(st, KA_ERR_BAD_ARG);
     const int S = out_stride;
     if (S < 1 || S > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
-    if (cudaSetDevice(c->device) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    if (c->pending_status) finish_status(c, c->last_stream, nullptr);
+    int rc = enter(c, true);
+    if (rc != KA_OK) return failed(st, rc);
     const int64_t Q = T > 0 ? part_off[T] : 0;
     if (Q < 0 || (T > 0 && part_off[0] != 0) || (Q > 0 && (!rep_off || !out_broker))) return set_status(st, KA_ERR_BAD_ARG);
     const int64_t R = Q > 0 ? rep_off[Q] : 0;
@@ -1318,63 +1302,20 @@ int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t*
     }
     if (maxsz > S) return set_status(st, KA_ERR_BAD_ARG, -1, -1, S);
 
-    cudaStream_t s = c->stream;
-    KA_CUDA(c->d_hash.reserve((size_t)std::max(T, 1) * 4));
-    KA_CUDA(c->d_part_off.reserve((size_t)(T + 1) * 8));
-    KA_CUDA(c->d_rep_off.reserve((size_t)(Q + 1) * 8));
-    KA_CUDA(c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4));
-    KA_CUDA(c->d_out.reserve((size_t)std::max<int64_t>(Q, 1) * S * 4));
-    KA_CUDA(c->d_out_len.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
-    c->host_out = nullptr;
-    StageDesc d;
-    d.T = T;
-    d.Q = Q;
-    d.d_hash = c->d_hash.as<int32_t>();
-    d.d_part_off = c->d_part_off.as<int64_t>();
-    d.d_rep_off = c->d_rep_off.as<int64_t>();
-    d.d_cur = c->d_cur.as<int32_t>();
-    d.desired_rf = desired_rf;
-    d.S = S;
-    d.Pmax = Pmax;
-    d.capmax = capmax;
-    c->staged = false;
-    int rc = make_plan(c, Q, S, Pmax, capmax, true, d.pl, st);
-    if (rc != KA_OK) return rc;
-    if ((rc = reserve_scratch(c, Q, d.pl.rec_bytes, T, 1, true)) != KA_OK) return set_status(st, rc);
-    c->last_stages = 1;
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev[0], s));
-    if (T > 0) {
-        KA_CUDA(cudaMemcpyAsync(c->d_hash.p, topic_hash, (size_t)T * 4, cudaMemcpyHostToDevice, s));
-        KA_CUDA(cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s));
-    }
-    if (Q > 0) KA_CUDA(cudaMemcpyAsync(c->d_rep_off.p, rep_off, (size_t)(Q + 1) * 8, cudaMemcpyHostToDevice, s));
-    if (R > 0) KA_CUDA(cudaMemcpyAsync(c->d_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s));
-    if ((rc = reset_flags(c, s)) != KA_OK) return set_status(st, rc);
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev[1], s));
-    c->last_part_id = part_id;
-    c->last_part_off = part_off;
-    c->last_was_staged = false;
-    c->ev_mark = c->timing ? c->ev[2] : nullptr;
-    rc = enq_stage(c, s, d);
-    c->ev_mark = nullptr;
-    if (rc != KA_OK) return set_status(st, rc);
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev[3], s));
-    if ((rc = chain_fork(c, s)) != KA_OK) return set_status(st, rc);
-    if ((rc = enq_order_emit(c, s, d, c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>(), 1)) != KA_OK) return set_status(st, rc);
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev[4], s));
-    if (Q > 0 && c->N > 0) {
-        KA_CUDA(cudaMemcpyAsync(out_broker, c->d_out.p, (size_t)Q * S * 4, cudaMemcpyDeviceToHost, s));
-        if (out_len) KA_CUDA(cudaMemcpyAsync(out_len, c->d_out_len.p, (size_t)Q * 4, cudaMemcpyDeviceToHost, s));
-    }
-    if ((rc = enq_flags_readback(c, s)) != KA_OK) return set_status(st, rc);
-    if (c->timing) { KA_CUDA(cudaEventRecord(c->ev[5], s)); c->ev_valid = true; }
-    c->last_stream = s;
-    c->pending_status = true;
-    ka_status local;
-    rc = finish_status(c, s, st ? st : &local);
-    c->last_part_id = nullptr;
-    c->last_part_off = nullptr;
-    return rc;
+    if ((rc = reserve_io(c, T, Q, R, S, true)) != KA_OK) return failed(st, rc);
+    SolveCall io;
+    io.h_hash = topic_hash;
+    io.h_part_off = part_off;
+    io.h_rep_off = rep_off;
+    io.h_cur = cur_broker;
+    io.d_out = c->d_out.as<int32_t>();
+    io.d_out_len = c->d_out_len.as<int32_t>();
+    io.h_out = out_broker;
+    io.h_out_len = out_len;
+    const Shape sh{T, 0, 0, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
+                   c->d_rep_off.as<int64_t>(), Q, R, Pmax, capmax};
+    if ((rc = run_solve(c, c->stream, sh, io, st)) != KA_OK) return failed(st, rc);
+    return finish(c, c->stream, st, true, part_id, part_off);
 }
 
 }  // extern "C"

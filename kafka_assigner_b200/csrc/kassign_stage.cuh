@@ -21,11 +21,6 @@ struct KaSolveParams {
     const uint16_t* blob;       // global: rack16[Npad] | lut16[range_pad] (16B aligned, multiple of 16B)
     int blob_bytes;             // bytes staged into smem (rack, plus lut when lut_mode == SMEM)
     int lut_off;                // element offset (uint16) of lut16 inside blob
-    int R;                      // number of distinct racks (compact ids 0..R-1 in rack16)
-    int rackptr;                // 1: spread phase uses per-rack first-free pointers (R small); 0: window scan
-    int roff_off;               // element offset of rack_off16[R+1] inside blob
-    int memb_off;               // element offset of members16[N] (sorted indices grouped by rack, ascending) inside blob
-    int rp_bytes;               // per-warp bytes of each of the three rack-pointer arrays
     int lut_mode;
     int min_id;
     uint32_t range;
@@ -48,8 +43,6 @@ struct KaSolveParams {
 struct KaTab {               // CTA-shared views into the staged broker table
     const uint16_t* rack;    // [N] compact rack id of each broker (sorted-index order)
     const uint16_t* lut;     // [range] (lut_mode == SMEM)
-    const uint16_t* roff;    // [R+1] member ranges per rack
-    const uint16_t* memb;    // [N] sorted indices grouped by rack, ascending inside a rack
 };
 
 __device__ __forceinline__ uint32_t ka_lookup(int id, const KaTab& tab, const KaSolveParams& p) {
@@ -83,7 +76,7 @@ struct KaLevelScratch {
 // phase, so that RF = 3 runs 3-wide compares instead of 8-wide ones.
 template <typename LoadT, bool LEVELS, int SM>
 __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, LoadT* load, uint16_t* slab, uint8_t* cnt,
-                               uint16_t* rpos, uint16_t* rst, uint16_t* rkk, const KaLevelScratch& ls) {
+                               const KaLevelScratch& ls) {
     const int lane = threadIdx.x & 31;
     const uint32_t lt = ka_lanemask_lt();
     const int S = p.S;
@@ -237,85 +230,6 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
         const int i0 = (int)(((uint32_t)N - start) % (uint32_t)N);  // sorted index at order position 0
 
         // ---- KAS:133-186 orphans, ascending partition; first-fit from position 0 each time -------
-        if (p.rackptr) {
-            // Exact reformulation of the walk: a position is acceptable iff its node is not full and its rack does
-            // not hold the partition yet, and loads / used racks only grow — so "first acceptable position from
-            // j = 0" == min over the racks not yet used of that rack's first non-full member (in rotated order).
-            // Each rack keeps a monotone pointer into its member list; placing a replica is one warp min-reduction.
-            const int R = p.R;
-            for (int r = lane; r < R; r += 32) {
-                const int o = tab.roff[r], sz = (int)tab.roff[r + 1] - o;
-                int lo = 0, hi = sz;
-                while (lo < hi) {  // first member with sorted index >= i0 starts the rack's rotated order
-                    const int mid = (lo + hi) >> 1;
-                    if ((int)tab.memb[o + mid] < i0) lo = mid + 1; else hi = mid;
-                }
-                const int st = (lo == sz) ? 0 : lo;
-                int kk = 0, pos = 0xFFFF;
-                while (kk < sz) {
-                    const int m = tab.memb[o + (st + kk >= sz ? st + kk - sz : st + kk)];
-                    if ((int)load[m] < cap) { pos = m - i0; if (pos < 0) pos += N; break; }
-                    ++kk;
-                }
-                rst[r] = (uint16_t)st; rkk[r] = (uint16_t)kk; rpos[r] = (uint16_t)pos;
-            }
-            __syncwarp();
-            for (int c0 = 0; c0 < P && !err; c0 += 32) {
-                const int pp0 = c0 + lane;
-                const int need = pp0 < P ? rf - (int)cnt[pp0] : 0;
-                uint32_t ob = __ballot_sync(KA_FULL, need > 0);
-                while (ob && !err) {
-                    const int src = __ffs(ob) - 1;
-                    ob &= ob - 1;
-                    const int pp = c0 + src;
-                    int rem = __shfl_sync(KA_FULL, need, src);
-                    int k = (int)cnt[pp];
-                    uint32_t ur[SM];  // racks already holding this partition (warp-uniform)
-#pragma unroll
-                    for (int i = 0; i < SM; ++i) ur[i] = i < k ? (uint32_t)tab.rack[slab[pp * S + i]] : 0xFFFFFFFFu;
-                    while (rem > 0) {
-                        uint32_t best = 0xFFFFFFFFu;
-                        for (int r = lane; r < R; r += 32) {
-                            bool used = false;
-#pragma unroll
-                            for (int i = 0; i < SM; ++i) used = used || (ur[i] == (uint32_t)r);
-                            const uint32_t cnd = used ? 0xFFFFFFFFu : (((uint32_t)rpos[r] << 16) | (uint32_t)r);
-                            best = min(best, cnd);
-                        }
-                        best = __reduce_min_sync(KA_FULL, best);
-                        if ((best >> 16) == 0xFFFFu) break;  // no rack can take it: stranded (KAS:183-184)
-                        const int pos = (int)(best >> 16), r = (int)(best & 0xFFFFu);
-                        int idx = i0 + pos;
-                        if (idx >= N) idx -= N;
-                        const int nl = (int)load[idx] + 1;
-                        __syncwarp();
-                        if (lane == 0) {
-                            load[idx] = (LoadT)nl;
-                            slab[pp * S + k] = (uint16_t)idx;
-                        }
-#pragma unroll
-                        for (int i = 0; i < SM; ++i)
-                            if (i == k) ur[i] = (uint32_t)r;
-                        ++k;
-                        --rem;
-                        if (nl >= cap) {  // the rack's first-free member just filled up: advance its pointer
-                            const int o = tab.roff[r], sz = (int)tab.roff[r + 1] - o, st = rst[r];
-                            int kk = (int)rkk[r] + 1, np = 0xFFFF;
-                            while (kk < sz) {
-                                const int m = tab.memb[o + (st + kk >= sz ? st + kk - sz : st + kk)];
-                                if ((int)load[m] < cap) { np = m - i0; if (np < 0) np += N; break; }
-                                ++kk;
-                            }
-                            if (lane == 0) { rkk[r] = (uint16_t)kk; rpos[r] = (uint16_t)np; }
-                        }
-                        __syncwarp();
-                    }
-                    if (lane == 0) cnt[pp] = (uint8_t)k;
-                    __syncwarp();
-                    if (rem > 0 && !err) { err = KA_E_UNASSIGNABLE; errp = pp; }  // KAS:183-184
-                }
-            }
-        } else {
         int head = 0;  // all order positions < head hold full nodes (loads never decrease)
         for (int c0 = 0; c0 < P && !err; c0 += 32) {
             const int pp0 = c0 + lane;
@@ -372,8 +286,6 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
                 __syncwarp();
                 if (rem > 0 && !err) { err = KA_E_UNASSIGNABLE; errp = pp; }  // KAS:183-184
             }
-        }
-
         }
 
         // ---- per-partition finalisation: ascending broker order (KAS:205-214) --------------------
@@ -584,23 +496,18 @@ __global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolvePara
     KaTab tab;
     tab.rack = reinterpret_cast<const uint16_t*>(blob);
     tab.lut = reinterpret_cast<const uint16_t*>(blob) + p.lut_off;
-    tab.roff = reinterpret_cast<const uint16_t*>(blob) + p.roff_off;
-    tab.memb = reinterpret_cast<const uint16_t*>(blob) + p.memb_off;
 
     const int warp = threadIdx.x >> 5;
     const int nwarp = blockDim.x >> 5;
     const int lv_bytes = LEVELS ? lv_owner_bytes + lv_last_bytes + 2 * lv_p_bytes : 0;
-    const int per_warp = load_bytes + slab_bytes + cnt_bytes + 3 * p.rp_bytes + lv_bytes;
+    const int per_warp = load_bytes + slab_bytes + cnt_bytes + lv_bytes;
     unsigned char* mine = warp_base + (size_t)warp * per_warp;
     LoadT* load = reinterpret_cast<LoadT*>(mine);
     uint16_t* slab = reinterpret_cast<uint16_t*>(mine + load_bytes);
     uint8_t* cnt = reinterpret_cast<uint8_t*>(mine + load_bytes + slab_bytes);
-    uint16_t* rpos = reinterpret_cast<uint16_t*>(mine + load_bytes + slab_bytes + cnt_bytes);
-    uint16_t* rst = reinterpret_cast<uint16_t*>(mine + load_bytes + slab_bytes + cnt_bytes + p.rp_bytes);
-    uint16_t* rkk = reinterpret_cast<uint16_t*>(mine + load_bytes + slab_bytes + cnt_bytes + 2 * p.rp_bytes);
     KaLevelScratch ls{};
     if (LEVELS) {
-        unsigned char* lvb = mine + load_bytes + slab_bytes + cnt_bytes + 3 * p.rp_bytes;
+        unsigned char* lvb = mine + load_bytes + slab_bytes + cnt_bytes;
         ls.owner = reinterpret_cast<uint32_t*>(lvb);
         ls.last = reinterpret_cast<uint16_t*>(lvb + lv_owner_bytes);
         ls.lvl = reinterpret_cast<uint16_t*>(lvb + lv_owner_bytes + lv_last_bytes);
@@ -609,5 +516,5 @@ __global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolvePara
 
     const int total_warps = gridDim.x * nwarp;
     for (int t = blockIdx.x * nwarp + warp; t < p.T; t += total_warps)
-        ka_solve_topic<LoadT, LEVELS, SM>(p, tab, t, load, slab, cnt, rpos, rst, rkk, ls);
+        ka_solve_topic<LoadT, LEVELS, SM>(p, tab, t, load, slab, cnt, ls);
 }

@@ -484,22 +484,27 @@ def test_degenerate_shapes(native_lib, oracle):
         kab.KafkaTopicAssigner().generate_assignment("big", {0: list(range(1, 10))}, set(range(1, 12)), {}, -1)  # 9 replicas > 8 slots
 
 
-def test_rack_pointer_spread_variant_is_exact(native_lib, oracle, tmp_path):
-    """The opt-in per-rack-pointer spread (KA_SPREAD_RACKPTR=1) must give the same bytes as the default window scan."""
-    import subprocess
-    import sys
-    code = ("import os, numpy as np, kafka_assigner_b200 as kab\n"
-            "d = %r\n"
-            "for key, kind in (('c1','random'), ('c2','mixed')):\n"
-            "    cl = kab.synth.make_config(key, kind)\n"
-            "    out, _, st = kab.Solver(0).solve_cluster(cl)\n"
-            "    np.save(os.path.join(d, '_rp_%%s.npy' %% key), out)\n" % str(tmp_path))
-    env = dict(os.environ, KA_SPREAD_RACKPTR="1", PYTHONPATH=util.os.path.dirname(util.HERE))
-    subprocess.run([sys.executable, "-c", code], check=True, env=env, timeout=300)
-    for key, kind in (("c1", "random"), ("c2", "mixed")):
-        cl = kab.synth.make_config(key, kind)
-        exp, _, _ = util.oracle_dense(oracle, cl)
-        assert np.array_equal(np.load(tmp_path / ("_rp_%s.npy" % key)).reshape(-1, 3), exp)
+def test_solves_before_any_broker_table(native_lib):
+    """A context whose broker table was never set has no brokers: every entry point reports the first topic's
+    replication factor above the broker count (KTA:67-69; KA_ERR_BAD_ARG for the JSON entry), and kernel A stages no
+    broker table."""
+    import torch
+    cl = kab.synth.make_cluster(T=4, P=8, RF=3, N=10, R=3, seed=3, kind="mixed")
+    rf_gt_brokers = (3, 0, -1, 3, 0)   # KA_ERR_RF_GT_BROKERS at topic 0, no partition, a = RF
+    key = lambda st: (st.code, st.topic_index, st.partition, st.a, st.b)
+    assert key(kab.Solver(0).solve_dense(cl.topic_hash, cl.cur, check=False)[2]) == rf_gt_brokers
+    part_off, part_id, rep_off, cur = cl.ragged()
+    assert key(kab.Solver(0).solve_ragged(cl.topic_hash, part_off, part_id, rep_off, cur, -1, 3, check=False)[2]) == rf_gt_brokers
+    assert key(kab.Solver(0).solve_dense_json(cl.topic_names, cl.topic_hash, cl.cur, check=False)[1]) == (-1, -1, -1, 0, 0)
+    d_hash, d_cur = torch.from_numpy(cl.topic_hash).cuda(), torch.from_numpy(cl.cur).cuda()
+    d_out = torch.empty((cl.T, cl.P, 3), dtype=torch.int32, device="cuda")
+    d_len = torch.empty((cl.T, cl.P), dtype=torch.int32, device="cuda")
+    torch.cuda.synchronize()
+    st = kab.Solver(0).solve_dense_device(cl.T, d_hash.data_ptr(), cl.P, cl.RF, d_cur.data_ptr(), -1, 3, d_len.data_ptr(), d_out.data_ptr())
+    assert key(st) == rf_gt_brokers
+    s = kab.Solver(0)
+    s.stage_dense_device(cl.T, d_hash.data_ptr(), cl.P, cl.RF, d_cur.data_ptr(), -1, 3)
+    assert key(s.order_device(d_len.data_ptr(), d_out.data_ptr())) == rf_gt_brokers
 
 
 def test_pipelined_super_chunks_are_exact(native_lib, oracle, tmp_path):
