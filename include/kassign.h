@@ -91,7 +91,7 @@ int32_t ka_java_string_hash(const char* utf8);
  *   topic_hash[T]    String.hashCode of each topic name
  *   part_off[T+1]    partitions of topic t are rows part_off[t] .. part_off[t+1]-1
  *   part_id[ΣP]      partition ids, ascending within a topic (TreeMap order, KAS:107-110); NULL = 0..P-1.
- *                    Only used to report ka_status.partition; the solver works on ordinals.
+ *                    Only used to report ka_status.partition (and printed by ka_solve_json); the solver works on ordinals.
  *   rep_off[ΣP+1]    current replica list of row g is cur_broker[rep_off[g] .. rep_off[g+1]-1] (leader first)
  *   desired_rf       --desired_replication_factor; -1 = keep (KTA:49,55-61)
  *   out_stride       slots per output row; must be >= max(list length, target RF) over all rows
@@ -117,6 +117,19 @@ int32_t ka_solve_dense(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, int32_
 int32_t ka_solve_dense_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, int32_t P, int32_t RF,
                             const int32_t* cur_broker, int32_t desired_rf, const char* names, const int64_t* name_off,
                             char* json, int64_t json_cap, int64_t* json_bytes, ka_status* st);
+
+/* General (ragged) solve + the reference's JSON emitter: the inputs of ka_solve (part_id, NULL = 0..P-1, is what the text
+ * prints as "partition"), the name slab and output contract of ka_solve_dense_json. The row stride is internal:
+ * max(longest current list, desired_rf, 1). The text is cut into fragments of a fixed number of rows, each streamed out as
+ * soon as it is built. json_cap = 64 + sum over rows of (50 + 12*stride + name length of the row's topic) always suffices
+ * (it holds for any int32 partition id); KA_ERR_LIMIT if json_cap is too small. A run without rows (T == 0, or only empty
+ * topics under a desired_rf) gives {"partitions":[],"version":1}. Names needing JSON escapes give KA_ERR_BAD_ARG before
+ * anything is solved (counters untouched). On any error *json_bytes = 0 and *st is what ka_solve reports for the same
+ * input; the ctx counters afterwards equal those after ka_solve. */
+int32_t ka_solve_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                      const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf,
+                      const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                      int64_t* json_bytes, ka_status* st);
 
 /* Dense form on DEVICE buffers (d_* are device pointers on the ctx's device; d_out_len may be NULL),
  * enqueued on `stream` (a cudaStream_t, NULL = the legacy default stream) — inputs already resident in

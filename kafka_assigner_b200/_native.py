@@ -27,6 +27,7 @@ SYMBOLS = {
     "ka_solve": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "ka_solve_dense": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
     "ka_solve_dense_json": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp]),
+    "ka_solve_json": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp]),
     "ka_solve_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
     "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),

@@ -208,6 +208,31 @@ class Solver:
             raise_for_status(st, topic_names)
         return out, out_len, st
 
+    def solve_ragged_json(self, topic_names, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, json_buf=None,
+                          check=True):
+        """ka_solve_json: the ragged solve of solve_ragged + the reassignment JSON built on the device (KAG:169-186);
+        returns (bytes-like view of the text, status). json_buf: optional writable uint8 numpy array (pinned for full
+        PCIe speed); by default one of the documented sufficient size."""
+        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
+        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
+        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
+        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
+        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        names, name_off = self.marshal_names(topic_names)
+        if json_buf is None:
+            sizes = np.diff(rep_off)
+            S = max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+            rows = np.diff(part_off)
+            json_buf = np.empty(64 + int(part_off[-1]) * (50 + 12 * S) + int(np.dot(rows, np.diff(name_off))), dtype=np.uint8)
+        nbytes = ctypes.c_int64(0)
+        st = KaStatus()
+        self._L.ka_solve_json(self._h, len(th), _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker),
+                              int(desired_rf), _ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size),
+                              ctypes.byref(nbytes), ctypes.byref(st))
+        if check:
+            raise_for_status(st, topic_names)
+        return json_buf[:nbytes.value], st
+
     def solve_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, d_out_len, d_out, stream=0,
                            sync=True):
         """Device-pointer form (ints from tensor.data_ptr()); returns KaStatus when sync else None."""

@@ -51,6 +51,11 @@ struct DevBuf {
 constexpr int KA_MAX_BLOCKS = 8;          // topic blocks of a pipelined solve
 constexpr int KA_MAX_CHAIN_BLOCKS = 8;    // slot-chain sub-blocks per staged block
 constexpr int KA_MAX_CHAIN_EVENTS = 64;   // per solve: 8 staged blocks x 8 sub-blocks
+// JSON fragments of one solve: one per chain sub-block of a dense solve; a ragged solve (one block, one sub-block) cuts its
+// rows into fragments of KA_JSON_FRAG_ROWS rows (more per fragment only beyond KA_MAX_JSON_FRAGS of them), so that the text
+// streams out while later fragments are still being built and every fragment stays far below the 4 GiB of its 32-bit offsets.
+constexpr int KA_MAX_JSON_FRAGS = 256;
+constexpr int64_t KA_JSON_FRAG_ROWS = 1 << 18;
 
 struct HostPinned {
     int err_topic;
@@ -112,16 +117,16 @@ struct ka_ctx {
     // scratch
     DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len, d_tstatus, d_flags;
     DevBuf d_rec, d_perm, d_ntl, d_loff, d_lend, d_lvl_end;  // records, chosen positions, schedule permutation, level tables
-    DevBuf d_json, d_names, d_name_off, d_json_rowlen, d_json_blocksum, d_json_state;
+    DevBuf d_json, d_names, d_name_off, d_part_id, d_json_rowlen, d_json_blocksum, d_json_state;
     HostPinned* h_pin = nullptr;
-    unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_CHAIN_EVENTS][2]: {first byte, bytes} of every JSON fragment
+    unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
     cudaEvent_t ev[6] = {};                                // solve: start, inputs in, kernel A done, stage done, chains done, end
     cudaEvent_t ev_pipe[KA_MAX_BLOCKS][5] = {};            // pipelined block: stage start, kernel A done, stage done, chains start / done
     cudaEvent_t ev_chain[KA_MAX_CHAIN_EVENTS][4] = {};     // chain sub-block: slot-0 chain start / done, slot-1 chain + emit start / done
     // cross-stream events
     cudaEvent_t ev_in = nullptr, ev_stage[KA_MAX_BLOCKS] = {}, ev_chain_in = nullptr, ev_b1[KA_MAX_CHAIN_EVENTS] = {};
-    cudaEvent_t ev_json_in[KA_MAX_CHAIN_EVENTS] = {}, ev_json_scan[KA_MAX_CHAIN_EVENTS] = {}, ev_out_done = nullptr;
+    cudaEvent_t ev_json_in[KA_MAX_JSON_FRAGS] = {}, ev_json_scan[KA_MAX_JSON_FRAGS] = {}, ev_out_done = nullptr;
     // timing of the last solve
     bool timing = false;
     float last_ms[8] = {};
@@ -182,8 +187,8 @@ void for_each_event(ka_ctx* c, F f) {
         {c->ev_stage, KA_MAX_BLOCKS, false},
         {&c->ev_chain_in, 1, false},
         {c->ev_b1, KA_MAX_CHAIN_EVENTS, false},
-        {c->ev_json_in, KA_MAX_CHAIN_EVENTS, false},
-        {c->ev_json_scan, KA_MAX_CHAIN_EVENTS, false},
+        {c->ev_json_in, KA_MAX_JSON_FRAGS, false},
+        {c->ev_json_scan, KA_MAX_JSON_FRAGS, false},
         {&c->ev_out_done, 1, false},
     };
     for (const auto& p : pools)
@@ -482,12 +487,14 @@ struct SolveCall {
     const int32_t* h_cur = nullptr;
     const int64_t* h_part_off = nullptr;  // ragged
     const int64_t* h_rep_off = nullptr;
+    const int32_t* h_part_id = nullptr;   // ragged JSON solve: partition ids, copied to d_part_id (the text prints them)
+    int32_t* d_part_id = nullptr;
     // rows of the whole problem on the device, and their host destination (null: they stay on the device)
     int32_t* d_out = nullptr;
     int32_t* d_out_len = nullptr;
     int32_t* h_out = nullptr;
     int32_t* h_out_len = nullptr;
-    bool json = false;        // ka_solve_dense_json: rows -> JSON text on c->sj as soon as they are final
+    bool json = false;        // ka_solve_dense_json / ka_solve_json: rows -> JSON text on c->sj as soon as they are final
     // pipelined host-buffer solve, rows <= 3: every chain sub-block is copied out on c->sj as soon as its emit is done, so
     // that no D2H sits between two slot-1 chains on the caller's stream
     bool stream_out = false;
@@ -511,7 +518,7 @@ SubBlock sub_block(const StageDesc& d, int j, int nsub) {
 // KAG:169-186 for a finished range of rows (sub-block b of block d): rows -> JSON text at the running offset of d_json, on c->sj.
 int enq_json_rows(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc& d, const SubBlock& b, bool first, bool last) {
     const int k = io.json_blocks;
-    if (k >= KA_MAX_CHAIN_EVENTS) return KA_ERR_LIMIT;
+    if (k >= KA_MAX_JSON_FRAGS) return KA_ERR_LIMIT;
     const int64_t row0 = d.q0 + b.r0, rows = b.rq;
     KA_CUDA(cudaEventRecord(c->ev_json_in[k], s_done));
     KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_json_in[k], 0));
@@ -520,6 +527,9 @@ int enq_json_rows(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc
     p.row0 = (uint32_t)row0;
     p.P = std::max(d.P, 1);
     p.topic0 = d.topic_base + b.t0;
+    p.T = d.T;
+    p.part_off = d.d_part_off;
+    p.part_id = io.d_part_id;
     p.name_off = c->d_name_off.as<int64_t>();
     p.names = c->d_names.as<char>();
     p.out = io.d_out + row0 * d.S;
@@ -543,6 +553,29 @@ int enq_json_rows(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc
     KA_CUDA(cudaEventRecord(c->ev_json_scan[k], c->sj));
     c->launches += 3;
     io.json_blocks = k + 1;
+    return KA_OK;
+}
+
+// Rows per JSON fragment of a ragged solve of Q rows (a multiple of 256: fragments own whole blocks of the length pass).
+int64_t json_fragment_rows(int64_t Q) {
+    const int64_t spread = (Q + KA_MAX_JSON_FRAGS - 1) / KA_MAX_JSON_FRAGS;
+    return std::max(KA_JSON_FRAG_ROWS, (spread + 255) / 256 * 256);
+}
+
+// JSON of the finished rows of sub-block b. A ragged block is never cut into chain sub-blocks, so its text is cut into
+// fragments here instead; a ragged run without rows still gets its (empty) text.
+int enq_json(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc& d, const SubBlock& b, bool first, bool last) {
+    if (!d.d_part_off) return enq_json_rows(c, s_done, io, d, b, first, last);
+    const int64_t step = json_fragment_rows(b.rq);
+    int64_t r = 0;
+    do {
+        SubBlock f = b;
+        f.r0 = b.r0 + r;
+        f.rq = std::min(step, b.rq - r);
+        const int rc = enq_json_rows(c, s_done, io, d, f, first && r == 0, last && r + step >= b.rq);
+        if (rc != KA_OK) return rc;
+        r += step;
+    } while (r < b.rq);
     return KA_OK;
 }
 
@@ -602,7 +635,7 @@ int enq_emit_block(ka_ctx* c, cudaStream_t s, const StageDesc& d, int j, int nsu
 int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io, int blocks_in_solve) {
     const int S = d.S;
     const Plan& pl = d.pl;
-    if (d.Q <= 0 || c->N <= 0) return KA_OK;
+    if (d.Q <= 0 || c->N <= 0) return io.json && d.d_part_off && d.Q == 0 ? enq_json(c, s, io, d, sub_block(d, 0, 1), true, true) : KA_OK;
     int32_t* d_out = io.d_out + d.q0 * S;
     int32_t* d_out_len = io.d_out_len ? io.d_out_len + d.q0 : nullptr;
     if (pl.rec_kind != 3) {  // rows of 4..8: one fused chain over all slots, rows written by the kernel
@@ -613,7 +646,7 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io,
         o.out_len = d_out_len;
         KA_CUDA((pl.rec_kind == 4 ? launch_order<4, 512>(s, o, pl) : launch_order<8, 256>(s, o, pl)));
         c->launches++;
-        if (io.json) return enq_json_rows(c, s, io, d, b, d.blk == 0, d.blk == blocks_in_solve - 1);
+        if (io.json) return enq_json(c, s, io, d, b, d.blk == 0, d.blk == blocks_in_solve - 1);
         return KA_OK;
     }
     const int nsub = chain_subblocks(d, blocks_in_solve);
@@ -642,7 +675,7 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io,
             if ((rc = enq_copy_out(so, io, S, d.q0 + b.r0, b.rq)) != KA_OK) return rc;
         }
         if (io.json) {   // the sub-block's rows are final: their JSON text can be built and streamed out now
-            if ((rc = enq_json_rows(c, s, io, d, b, d.blk == 0 && j == 0, d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK)
+            if ((rc = enq_json(c, s, io, d, b, d.blk == 0 && j == 0, d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK)
                 return rc;
         }
         c->chain_used = std::min(++io.chains, KA_MAX_CHAIN_EVENTS);
@@ -685,6 +718,7 @@ int enq_inputs(cudaStream_t s, const SolveCall& io, const StageDesc& d, int64_t 
     if (io.h_hash && d.T > 0) KA_CUDA(h2d(d.d_hash, io.h_hash + d.topic_base, (size_t)d.T * 4));
     if (io.h_part_off && d.T > 0) KA_CUDA(h2d(d.d_part_off, io.h_part_off, (size_t)(d.T + 1) * 8));
     if (io.h_rep_off && d.Q > 0) KA_CUDA(h2d(d.d_rep_off, io.h_rep_off, (size_t)(d.Q + 1) * 8));
+    if (io.h_part_id && d.Q > 0) KA_CUDA(h2d(io.d_part_id, io.h_part_id, (size_t)d.Q * 4));
     if (io.h_cur && ncur > 0) KA_CUDA(h2d(d.d_cur, io.h_cur + d.q0 * d.RF, (size_t)ncur * 4));
     return KA_OK;
 }
@@ -888,7 +922,7 @@ ka_ctx* ka_ctx_create(int32_t device) {
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
     bool ok = cudaHostAlloc(reinterpret_cast<void**>(&c->h_pin), sizeof(HostPinned), cudaHostAllocDefault) == cudaSuccess &&
-              cudaHostAlloc(reinterpret_cast<void**>(&c->h_frag), 2 * KA_MAX_CHAIN_EVENTS * sizeof(unsigned long long),
+              cudaHostAlloc(reinterpret_cast<void**>(&c->h_frag), 2 * KA_MAX_JSON_FRAGS * sizeof(unsigned long long),
                             cudaHostAllocDefault) == cudaSuccess;
     for (cudaStream_t* s : {&c->stream, &c->aux, &c->sb1, &c->sj})
         ok = ok && cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
@@ -909,7 +943,8 @@ void ka_ctx_destroy(ka_ctx* c) {
         if (s) cudaStreamSynchronize(s);
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
                       &c->d_out, &c->d_out_len, &c->d_tstatus, &c->d_flags, &c->d_rec, &c->d_perm, &c->d_ntl, &c->d_loff, &c->d_lend,
-                      &c->d_lvl_end, &c->d_json, &c->d_names, &c->d_name_off, &c->d_json_rowlen, &c->d_json_blocksum, &c->d_json_state})
+                      &c->d_lvl_end, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen, &c->d_json_blocksum,
+                      &c->d_json_state})
         b->release();
     for_each_event(c, [](cudaEvent_t& e, bool) {
         if (e) cudaEventDestroy(e);
@@ -1210,12 +1245,45 @@ static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, cons
     KA_CUDA(c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)));
     KA_CUDA(c->d_name_off.reserve((size_t)(T + 1) * 8));
     KA_CUDA(c->d_json_rowlen.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
-    KA_CUDA(c->d_json_blocksum.reserve((size_t)(Q / 256 + 2 * KA_MAX_CHAIN_EVENTS) * 4));
-    KA_CUDA(c->d_json_state.reserve((2 + 2 * KA_MAX_CHAIN_EVENTS) * 8));
-    KA_CUDA(cudaMemsetAsync(c->d_json_state.p, 0, (2 + 2 * KA_MAX_CHAIN_EVENTS) * 8, c->sj));
+    KA_CUDA(c->d_json_blocksum.reserve((size_t)(Q / 256 + 2 * KA_MAX_JSON_FRAGS) * 4));
+    KA_CUDA(c->d_json_state.reserve((2 + 2 * KA_MAX_JSON_FRAGS) * 8));
+    KA_CUDA(cudaMemsetAsync(c->d_json_state.p, 0, (2 + 2 * KA_MAX_JSON_FRAGS) * 8, c->sj));
     if (name_bytes > 0) KA_CUDA(cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, c->sj));
     if (T > 0) KA_CUDA(cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, c->sj));
     return KA_OK;
+}
+
+// The device emitter copies topic names verbatim: a name that org.json's quote() would escape is refused (KA_ERR_BAD_ARG,
+// a = the byte), and the caller takes the host emitter instead.
+static int check_names(int32_t T, const char* names, const int64_t* name_off, ka_status* st) {
+    const int64_t name_bytes = T > 0 ? name_off[T] : 0;
+    for (int64_t i = 0; i < name_bytes; ++i) {
+        const unsigned char ch = (unsigned char)names[i];
+        if (ch < 0x20 || ch == '"' || ch == '\\' || ch == '/') return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)ch);
+    }
+    return KA_OK;
+}
+
+// Every fragment of a JSON solve is enqueued on c->sj: stream each one into `json` as soon as its size is known (later
+// fragments may still be in the chains or being built), then collect the solve's status. part_id / part_off: as in
+// finish_status. On any error *json_bytes stays 0; a text longer than json_cap is KA_ERR_LIMIT.
+static int stream_json(ka_ctx* c, cudaStream_t s, const SolveCall& io, char* json, int64_t json_cap, int64_t* json_bytes,
+                       ka_status* st, const int32_t* part_id = nullptr, const int64_t* part_off = nullptr) {
+    finish(c, s, nullptr, false);   // pending: collected below, once the fragments are out
+    int64_t total = 0;
+    bool overflow = false;
+    for (int k = 0; k < io.json_blocks; ++k) {
+        KA_CUDA(cudaEventSynchronize(c->ev_json_scan[k]));
+        const int64_t base = (int64_t)c->h_frag[2 * k], size = (int64_t)c->h_frag[2 * k + 1];
+        if (base + size > json_cap) { overflow = true; break; }
+        if (size > 0) KA_CUDA(cudaMemcpyAsync(json + base, c->d_json.as<char>() + base, (size_t)size, cudaMemcpyDeviceToHost, c->sj));
+        total = base + size;
+    }
+    KA_CUDA(cudaStreamSynchronize(c->sj));
+    int rc = finish_status(c, s, st, part_id, part_off);
+    if (rc == KA_OK && overflow) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
+    if (json_bytes) *json_bytes = rc == KA_OK ? total : 0;
+    return rc;
 }
 
 int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t P, int32_t RF, const int32_t* cur_broker,
@@ -1228,13 +1296,9 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     const int64_t Q = (int64_t)T * P, R = Q * RF;
     if ((T > 0 && (!topic_hash || !names || !name_off)) || (R > 0 && !cur_broker) || !json || json_cap < KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN)
         return set_status(st, KA_ERR_BAD_ARG);
-    const int64_t name_bytes = T > 0 ? name_off[T] : 0;
-    for (int64_t i = 0; i < name_bytes; ++i) {  // org.json quote() would escape these: such names take the host emitter
-        const unsigned char ch = (unsigned char)names[i];
-        if (ch < 0x20 || ch == '"' || ch == '\\' || ch == '/') return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)ch);
-    }
+    if ((rc = check_names(T, names, name_off, st)) != KA_OK) return rc;
     if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, T, Q, R, S, false)) != KA_OK ||
-        (rc = prepare_json(c, T, Q, names, name_off, name_bytes, json_cap)) != KA_OK)
+        (rc = prepare_json(c, T, Q, names, name_off, T > 0 ? name_off[T] : 0, json_cap)) != KA_OK)
         return failed(st, rc);
     cudaStream_t s = c->stream;
     SolveCall io;
@@ -1246,40 +1310,31 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     const Shape sh{T, P, RF, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>()};
     rc = T > 0 && c->N > 0 ? run_solve(c, s, sh, io, st) : KA_ERR_BAD_ARG;
     if (rc != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
-    finish(c, s, nullptr, false);   // pending: collected below, once the fragments are out
-    // every block is enqueued; stream the fragments out as their sizes become known (later blocks are still in the chains)
-    int64_t total = 0;
-    bool overflow = false;
-    for (int k = 0; k < io.json_blocks; ++k) {
-        KA_CUDA(cudaEventSynchronize(c->ev_json_scan[k]));
-        const int64_t base = (int64_t)c->h_frag[2 * k], size = (int64_t)c->h_frag[2 * k + 1];
-        if (base + size > json_cap) { overflow = true; break; }
-        if (size > 0) KA_CUDA(cudaMemcpyAsync(json + base, c->d_json.as<char>() + base, (size_t)size, cudaMemcpyDeviceToHost, c->sj));
-        total = base + size;
-    }
-    KA_CUDA(cudaStreamSynchronize(c->sj));
-    rc = finish_status(c, s, st);
-    if (rc == KA_OK && overflow) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
-    if (json_bytes) *json_bytes = rc == KA_OK ? total : 0;
-    return rc;
+    return stream_json(c, s, io, json, json_cap, json_bytes, st);
 }
 
-int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off,
-                 const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker,
-                 int32_t desired_rf, int32_t out_stride, int32_t* out_len, int32_t* out_broker,
-                 ka_status* st) {
+// Validation and host-side sizing scan of a ragged solve (largest topic, largest current list, largest capacity,
+// KAS:65-71), then its device input buffers: the Shape run_solve takes. pick_stride: S is chosen here, as
+// max(longest current list, desired_rf, 1). have_out: the caller has somewhere to put the rows.
+static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
+                        const int32_t* cur_broker, int32_t desired_rf, int32_t S, bool pick_stride, bool have_out, Shape& sh,
+                        ka_status* st) {
     set_status(st, KA_OK);
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return set_status(st, KA_ERR_BAD_ARG);
-    const int S = out_stride;
-    if (S < 1 || S > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
+    if (!pick_stride && (S < 1 || S > KA_MAX_SLOTS)) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
     int rc = enter(c, true);
     if (rc != KA_OK) return failed(st, rc);
     const int64_t Q = T > 0 ? part_off[T] : 0;
-    if (Q < 0 || (T > 0 && part_off[0] != 0) || (Q > 0 && (!rep_off || !out_broker))) return set_status(st, KA_ERR_BAD_ARG);
+    if (Q < 0 || (T > 0 && part_off[0] != 0) || (Q > 0 && (!rep_off || !have_out))) return set_status(st, KA_ERR_BAD_ARG);
     const int64_t R = Q > 0 ? rep_off[Q] : 0;
     if (R < 0 || (Q > 0 && rep_off[0] != 0) || (R > 0 && !cur_broker)) return set_status(st, KA_ERR_BAD_ARG);
-    // host-side sizing scan: largest topic, largest current list, largest capacity (KAS:65-71)
+    if (pick_stride) {
+        int64_t m = std::max(desired_rf, 1);
+        for (int64_t g = 0; g < Q; ++g) m = std::max(m, rep_off[g + 1] - rep_off[g]);
+        if (m > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(m, INT_MAX));
+        S = (int)m;
+    }
     int Pmax = 0;
     int64_t capmax = 0, maxsz = 0;
     for (int t = 0; t < T; ++t) {
@@ -1301,8 +1356,19 @@ int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t*
         maxsz = std::max(maxsz, sz);
     }
     if (maxsz > S) return set_status(st, KA_ERR_BAD_ARG, -1, -1, S);
-
     if ((rc = reserve_io(c, T, Q, R, S, true)) != KA_OK) return failed(st, rc);
+    sh = Shape{T, 0, 0, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
+               c->d_rep_off.as<int64_t>(), Q, R, Pmax, capmax};
+    return KA_OK;
+}
+
+int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off,
+                 const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker,
+                 int32_t desired_rf, int32_t out_stride, int32_t* out_len, int32_t* out_broker,
+                 ka_status* st) {
+    Shape sh;
+    int rc = ragged_shape(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, out_stride, false, out_broker != nullptr, sh, st);
+    if (rc != KA_OK) return rc;
     SolveCall io;
     io.h_hash = topic_hash;
     io.h_part_off = part_off;
@@ -1312,10 +1378,40 @@ int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t*
     io.d_out_len = c->d_out_len.as<int32_t>();
     io.h_out = out_broker;
     io.h_out_len = out_len;
-    const Shape sh{T, 0, 0, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-                   c->d_rep_off.as<int64_t>(), Q, R, Pmax, capmax};
     if ((rc = run_solve(c, c->stream, sh, io, st)) != KA_OK) return failed(st, rc);
     return finish(c, c->stream, st, true, part_id, part_off);
+}
+
+int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                      const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, const char* names,
+                      const int64_t* name_off, char* json, int64_t json_cap, int64_t* json_bytes, ka_status* st) {
+    if (json_bytes) *json_bytes = 0;
+    Shape sh;
+    int rc = ragged_shape(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, 0, true, true, sh, st);
+    if (rc != KA_OK) return rc;
+    if ((T > 0 && (!names || !name_off)) || !json || json_cap < 0) return set_status(st, KA_ERR_BAD_ARG);
+    if ((rc = check_names(T, names, name_off, st)) != KA_OK) return rc;
+    // a fragment's offsets are 32-bit: its rows at their longest (any int32 partition id, S replicas, the longest name)
+    int64_t longest_name = 0;
+    for (int t = 0; t < T; ++t) longest_name = std::max(longest_name, name_off[t + 1] - name_off[t]);
+    const int64_t frag_rows = std::min(json_fragment_rows(sh.Q), std::max<int64_t>(sh.Q, 1));
+    if (64 + frag_rows * (50 + 12 * sh.S + longest_name) > (int64_t)UINT32_MAX)
+        return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(longest_name, INT_MAX));
+    if (c->d_part_id.reserve((size_t)std::max<int64_t>(sh.Q, 1) * 4) != cudaSuccess) return failed(st, KA_ERR_CUDA);
+    if ((rc = prepare_json(c, T, sh.Q, names, name_off, T > 0 ? name_off[T] : 0, json_cap)) != KA_OK) return failed(st, rc);
+    cudaStream_t s = c->stream;
+    SolveCall io;
+    io.h_hash = topic_hash;
+    io.h_part_off = part_off;
+    io.h_rep_off = rep_off;
+    io.h_cur = cur_broker;
+    io.h_part_id = part_id;
+    io.d_part_id = part_id ? c->d_part_id.as<int32_t>() : nullptr;
+    io.d_out = c->d_out.as<int32_t>();
+    io.d_out_len = c->d_out_len.as<int32_t>();
+    io.json = true;
+    if ((rc = run_solve(c, s, sh, io, st)) != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
+    return stream_json(c, s, io, json, json_cap, json_bytes, st, part_id, part_off);
 }
 
 }  // extern "C"

@@ -1,6 +1,7 @@
 // kassign_json.cuh — the reassignment JSON of KafkaAssignmentGenerator.printLeastDisruptiveReassignment (KAG:169-186) built
-// on the device from the solved rows, so that only TEXT crosses PCIe and it can stream out block by block while later topic
-// blocks are still in the leader-order chains.
+// on the device from the solved rows, so that only TEXT crosses PCIe and it can stream out fragment by fragment while later
+// topic blocks are still in the leader-order chains. Rows are those of a dense run (P partitions 0..P-1 per topic) or of a
+// ragged one (part_off / part_id, as ka_solve takes them).
 //
 //   {"partitions":[{"partition":P,"replicas":[a,b,c],"topic":"name"},...],"version":1}
 //
@@ -16,6 +17,9 @@ struct KaJsonParams {
     uint32_t row0;              // index of the fragment's first row in the whole run (row 0 has no leading comma)
     int P;                      // dense shape: partition id = row % P, topic = topic0 + row / P
     int topic0;
+    int T;                      // ragged shape (part_off != null): topics of the run
+    const int64_t* part_off;    // [T+1] rows of topic t are part_off[t] .. part_off[t+1]-1 (run-wide row indices)
+    const int32_t* part_id;     // [rows of the run] partition ids; null = the ordinal inside the topic
     const int64_t* name_off;    // [T+1] byte offsets into names
     const char* names;          // concatenated topic names (UTF-8, no escapes needed)
     const int32_t* out;         // [Q][S] broker ids, leader first
@@ -54,15 +58,34 @@ __device__ __forceinline__ char* ka_put_str(char* p, const char* s, int n) {
     return p + n;
 }
 
+// Topic and partition id of row q of the fragment.
+__device__ __forceinline__ void ka_json_row_key(const KaJsonParams& p, uint32_t q, int& t, int& part) {
+    if (p.part_off) {
+        const int64_t g = (int64_t)p.row0 + q;
+        int lo = 0, hi = p.T;  // part_off[lo] <= g < part_off[hi]; a topic without partitions never satisfies both
+        while (hi - lo > 1) {
+            const int mid = (lo + hi) >> 1;
+            if (p.part_off[mid] <= g) lo = mid; else hi = mid;
+        }
+        t = lo;
+        part = p.part_id ? p.part_id[g] : (int)(g - p.part_off[lo]);
+    } else {
+        t = p.topic0 + (int)(q / (uint32_t)p.P);
+        part = (int)(q % (uint32_t)p.P);
+    }
+}
+
 __device__ __forceinline__ uint32_t ka_json_row_len(const KaJsonParams& p, uint32_t q) {
-    const int t = p.topic0 + (int)(q / (uint32_t)p.P), part = (int)(q % (uint32_t)p.P);
+    int t, part;
+    ka_json_row_key(p, q, t, part);
     const int len = p.out_len[q];
     uint32_t n = (p.row0 + q > 0 ? 1u : 0u) + 13u + ka_ndigits(part) + 13u + 11u + (uint32_t)(p.name_off[t + 1] - p.name_off[t]) + 2u;
     for (int i = 0; i < len; ++i) n += ka_ndigits(p.out[(size_t)q * p.S + i]) + (i ? 1u : 0u);
     return n;
 }
 __device__ __forceinline__ void ka_json_row_put(const KaJsonParams& p, uint32_t q, char* w) {
-    const int t = p.topic0 + (int)(q / (uint32_t)p.P), part = (int)(q % (uint32_t)p.P);
+    int t, part;
+    ka_json_row_key(p, q, t, part);
     const int len = p.out_len[q];
     if (p.row0 + q > 0) *w++ = ',';
     w = ka_put_str(w, "{\"partition\":", 13);

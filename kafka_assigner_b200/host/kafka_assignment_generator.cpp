@@ -357,8 +357,8 @@ int runTool(int argc, char** argv) {
         std::cout << "CURRENT ASSIGNMENT:\n" << kassign::kafkaReassignmentJson(gatherTopics(sn, topics, false)) << "\n";  // KAG:160
         std::vector<kassign::TopicInput> inputs = gatherTopics(sn, topics, true);
         kassign::KafkaTopicAssigner assigner;                                   // ONE assigner for the run, KAG:172
-        std::vector<kassign::TopicOutput> result = assigner.solveTopics(inputs, brokers, rackAssignment, o.desiredReplicationFactor);
-        std::cout << "NEW ASSIGNMENT:\n" << kassign::newAssignmentJson(result) << "\n";  // KAG:186
+        const std::string result = assigner.solveTopicsJson(inputs, brokers, rackAssignment, o.desiredReplicationFactor);
+        std::cout << "NEW ASSIGNMENT:\n" << result << "\n";                    // KAG:186, text built on the device
     }
     return 0;
 }

@@ -5,14 +5,17 @@
 //                                                          (reference KafkaTopicAssigner.java:42-72)
 //   kassign::solveTopics                              <->  the per-topic loop with ONE shared assigner
 //                                                          (reference KafkaAssignmentGenerator.java:172-184)
+//   kassign::solveTopicsJson                          <->  that loop + its org.json text, built on the device (KAG:172-186)
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
 // ArrayIndexOutOfBoundsException with the reference's message texts (KTA:58-60, 65-66, 67-69; KAS:183-184, 190-192).
 // All compute runs in libkassign.so's CUDA kernels; there is no CPU fallback — without a GPU the constructor throws.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <map>
+#include <memory>
 #include <set>
 #include <stdexcept>
 #include <string>
@@ -86,41 +89,62 @@ public:
     std::vector<TopicOutput> solveTopics(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
                                          const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor) {
         setBrokers(brokers, rackAssignment);
+        const Flat f = flatten(topics, desiredReplicationFactor);
         const int T = (int)topics.size();
-        std::vector<int32_t> hash(T), partId, cur;
-        std::vector<int64_t> partOff(T + 1, 0), repOff(1, 0);
-        std::vector<std::string> names(T);
-        int maxLen = 0;
-        for (int t = 0; t < T; ++t) {
-            names[t] = topics[t].name;
-            hash[t] = ka_java_string_hash(topics[t].name.c_str());
-            for (const auto& e : topics[t].current) {  // std::map: ascending partition == TreeMap order (KAS:107-110)
-                partId.push_back(e.first);
-                for (int b : e.second) cur.push_back(b);
-                repOff.push_back((int64_t)cur.size());
-                maxLen = std::max(maxLen, (int)e.second.size());
-            }
-            partOff[t + 1] = (int64_t)partId.size();
-        }
-        const int stride = std::max(1, std::max(maxLen, std::max(desiredReplicationFactor, 0)));
-        const size_t Q = partId.size();
-        std::vector<int32_t> outLen(Q, 0), out(Q * (size_t)stride, -1);
+        const size_t Q = f.partId.size();
+        std::vector<int32_t> outLen(Q, 0), out(Q * (size_t)f.stride, -1);
         ka_status st{};
-        ka_solve(ctx_, T, hash.data(), partOff.data(), partId.data(), repOff.data(), cur.data(), desiredReplicationFactor, stride,
-                 outLen.data(), out.data(), &st);
-        throwForStatus(st, names);
+        ka_solve(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
+                 f.stride, outLen.data(), out.data(), &st);
+        throwForStatus(st, f.names);
         std::vector<TopicOutput> res(T);
         for (int t = 0; t < T; ++t) {
-            res[t].name = names[t];
-            for (int64_t g = partOff[t]; g < partOff[t + 1]; ++g)
-                res[t].assignment[partId[g]] = std::vector<int>(out.begin() + g * stride, out.begin() + g * stride + outLen[g]);
+            res[t].name = f.names[t];
+            for (int64_t g = f.partOff[t]; g < f.partOff[t + 1]; ++g)
+                res[t].assignment[f.partId[g]] =
+                    std::vector<int>(out.begin() + g * f.stride, out.begin() + g * f.stride + outLen[g]);
         }
         return res;
     }
 
+    // The KAG:172-186 loop and its "NEW ASSIGNMENT" text in one device call (ka_solve_json): only the text crosses PCIe.
+    // Same solve and exceptions as solveTopics; the text equals newAssignmentJson(solveTopics(...)). Topic names that
+    // org.json would escape take that host emitter instead.
+    std::string solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
+                                const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor);
+
     ka_ctx* handle() { return ctx_; }
 
 private:
+    // The flat ragged layout of include/kassign.h (ka_solve / ka_solve_json inputs).
+    struct Flat {
+        std::vector<std::string> names;
+        std::vector<int32_t> hash, partId, cur;
+        std::vector<int64_t> partOff, repOff;
+        int stride = 1;
+    };
+    static Flat flatten(const std::vector<TopicInput>& topics, int desiredReplicationFactor) {
+        const int T = (int)topics.size();
+        Flat f;
+        f.names.resize(T);
+        f.hash.resize(T);
+        f.partOff.assign(T + 1, 0);
+        f.repOff.assign(1, 0);
+        int maxLen = 0;
+        for (int t = 0; t < T; ++t) {
+            f.names[t] = topics[t].name;
+            f.hash[t] = ka_java_string_hash(topics[t].name.c_str());
+            for (const auto& e : topics[t].current) {  // std::map: ascending partition == TreeMap order (KAS:107-110)
+                f.partId.push_back(e.first);
+                for (int b : e.second) f.cur.push_back(b);
+                f.repOff.push_back((int64_t)f.cur.size());
+                maxLen = std::max(maxLen, (int)e.second.size());
+            }
+            f.partOff[t + 1] = (int64_t)f.partId.size();
+        }
+        f.stride = std::max(1, std::max(maxLen, std::max(desiredReplicationFactor, 0)));
+        return f;
+    }
     void setBrokers(const std::set<int>& brokers, const std::map<int, std::string>& racks) {
         std::vector<int32_t> ids(brokers.begin(), brokers.end());  // std::set: ascending == TreeMap order (KAS:78)
         if (ids == ids_ && racks == racks_) return;
@@ -196,6 +220,38 @@ inline std::string newAssignmentJson(const std::vector<TopicOutput>& topics) {
         }
     s += "],\"version\":1}";  // KAFKA_FORMAT_VERSION (KAG:49)
     return s;
+}
+
+// Bytes org.json's JSONObject.quote() may rewrite: the device emitter copies names verbatim and refuses these.
+inline bool needsJsonEscape(const std::string& name) {
+    for (unsigned char c : name)
+        if (c < 0x20 || c == '"' || c == '\\' || c == '/') return true;
+    return false;
+}
+
+inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
+                                                       const std::map<int, std::string>& rackAssignment,
+                                                       int desiredReplicationFactor) {
+    for (const auto& t : topics)
+        if (needsJsonEscape(t.name)) return newAssignmentJson(solveTopics(topics, brokers, rackAssignment, desiredReplicationFactor));
+    setBrokers(brokers, rackAssignment);
+    const Flat f = flatten(topics, desiredReplicationFactor);
+    const int T = (int)topics.size();
+    std::string names;
+    std::vector<int64_t> nameOff(T + 1, 0);
+    int64_t cap = 64;  // the sufficient size documented in kassign.h
+    for (int t = 0; t < T; ++t) {
+        names += f.names[t];
+        nameOff[t + 1] = (int64_t)names.size();
+        cap += (f.partOff[t + 1] - f.partOff[t]) * (50 + 12 * (int64_t)f.stride + (int64_t)f.names[t].size());
+    }
+    std::unique_ptr<char[]> json(new char[cap]);
+    int64_t bytes = 0;
+    ka_status st{};
+    ka_solve_json(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
+                  names.data(), nameOff.data(), json.get(), cap, &bytes, &st);
+    throwForStatus(st, f.names);
+    return std::string(json.get(), (size_t)bytes);
 }
 
 // Kafka 0.10 ZkUtils.formatAsReassignmentJson shape (used for "CURRENT ASSIGNMENT:", KAG:103-111): scala Map literals keep

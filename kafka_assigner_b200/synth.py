@@ -163,6 +163,95 @@ def make_cluster(T, P, RF, N, R, seed, kind="mixed", n_old=None, remove_frac=0.0
                    dict(T=T, P=P, RF=RF, N=N, R=R, seed=seed, kind=kind, n_old=n_old, remove_frac=remove_frac))
 
 
+@dataclass
+class RaggedCluster:
+    """A real-cluster-shaped problem in the ragged layout of ka_solve / ka_solve_json: partition counts and replication
+    factors differ from topic to topic."""
+    name: str
+    topic_names: List[str]
+    topic_hash: np.ndarray          # int32 [T]
+    part_off: np.ndarray            # int64 [T+1]
+    part_id: np.ndarray             # int32 [Q] 0..P_t-1 per topic
+    rep_off: np.ndarray             # int64 [Q+1]
+    cur: np.ndarray                 # int32 [R] current replica lists, leader first
+    broker_id: np.ndarray           # int32 [N] ascending — the LIVE set handed to the solver
+    rack_name: List[Optional[str]]  # per live broker (None: no rack defined)
+    rack_index: np.ndarray          # int32 [N]
+    all_broker_id: np.ndarray       # int32 every broker of the cluster, removed ones included (ascending)
+    all_rack_name: List[Optional[str]]
+    desired_rf: int = -1
+    meta: dict = field(default_factory=dict)
+
+    @property
+    def T(self):
+        return len(self.topic_names)
+
+    @property
+    def Q(self):
+        return int(self.part_off[-1])
+
+    @property
+    def N(self):
+        return len(self.broker_id)
+
+    def topics(self):
+        """[(name, {partition: [brokers]})] — the per-topic maps of the reference's generateAssignment loop."""
+        out = []
+        for t, n in enumerate(self.topic_names):
+            a, b = int(self.part_off[t]), int(self.part_off[t + 1])
+            out.append((n, {int(self.part_id[g]): self.cur[self.rep_off[g]:self.rep_off[g + 1]].tolist() for g in range(a, b)}))
+        return out
+
+
+def make_ragged_cluster(T, N=800, R=10, seed=0, max_partitions=256, tail=1.1, rf_weights=(0.15, 0.25, 0.6),
+                        rack_frac=0.8, new_frac=0.1, remove_frac=0.0, desired_rf=-1, topic_prefix="svc."):
+    """A seeded, deterministic real-cluster shape.
+
+    Topic t has P_t = min(max_partitions, floor(u^(-1/tail))) partitions (a Pareto tail: most topics have a handful, a few have
+    hundreds) and replication factor 1, 2 or 3 drawn with rf_weights. Brokers are ids 1..N; broker i is in rack "r<i % R>"
+    with probability rack_frac and has no rack otherwise. The current lists use the first N - round(new_frac * N) brokers
+    (the rest joined empty); remove_frac of the brokers (drawn at random) leave the live set.
+    """
+    t_idx = np.arange(T, dtype=np.uint64)
+    u = (splitmix64(seed, t_idx) >> np.uint64(11)).astype(np.float64) / float(1 << 53)
+    P = np.minimum(max_partitions, np.floor((1.0 - u) ** (-1.0 / tail))).astype(np.int64)
+    w = np.cumsum(np.asarray(rf_weights, dtype=np.float64) / sum(rf_weights))
+    v = (splitmix64(seed + 1, t_idx) >> np.uint64(11)).astype(np.float64) / float(1 << 53)
+    rf = (1 + np.searchsorted(w, v, side="right")).clip(1, len(rf_weights)).astype(np.int64)
+    part_off = np.zeros(T + 1, dtype=np.int64)
+    np.cumsum(P, out=part_off[1:])
+    Q = int(part_off[-1])
+    topic_of = np.repeat(np.arange(T), P)
+    part_id = (np.arange(Q, dtype=np.int64) - part_off[topic_of]).astype(np.int32)
+    rf_row = rf[topic_of]
+    rep_off = np.zeros(Q + 1, dtype=np.int64)
+    np.cumsum(rf_row, out=rep_off[1:])
+    # current lists: RF distinct old brokers base, base + step, base + 2 step (mod n_old; 0 < step < n_old / 2)
+    all_ids = np.arange(1, N + 1, dtype=np.int32)
+    n_old = max(3, N - int(round(new_frac * N)))
+    g = np.arange(Q, dtype=np.uint64)
+    base = (splitmix64(seed + 2, g) % np.uint64(n_old)).astype(np.int64)
+    step = 1 + (splitmix64(seed + 3, g) % np.uint64(max(1, (n_old - 1) // 2))).astype(np.int64)
+    slot = np.arange(int(rep_off[-1]), dtype=np.int64) - np.repeat(rep_off[:-1], rf_row)
+    cur = all_ids[(np.repeat(base, rf_row) + slot * np.repeat(step, rf_row)) % n_old]
+    # racks, removals
+    bi = np.arange(N, dtype=np.uint64)
+    has_rack = (splitmix64(seed + 4, bi) >> np.uint64(11)).astype(np.float64) / float(1 << 53) < rack_frac
+    all_racks = ["r%02d" % (i % R) if has_rack[i] else None for i in range(N)]
+    n_remove = int(round(remove_frac * N))
+    removed = np.argsort(splitmix64(seed + 5, bi))[:n_remove]
+    live = np.ones(N, dtype=bool)
+    live[removed] = False
+    live_ids = all_ids[live]
+    live_racks = [all_racks[i] for i in range(N) if live[i]]
+    names = ["%s%05d" % (topic_prefix, t) for t in range(T)]
+    th = java_string_hash_ascii(names)
+    assert not np.any(th == np.int32(-2**31)), "synthetic topic name hashes to Integer.MIN_VALUE"
+    return RaggedCluster("ragged_T%d_N%d_s%d" % (T, N, seed), names, th, part_off, part_id, rep_off, cur.astype(np.int32),
+                         live_ids, live_racks, rack_indices(live_ids, live_racks), all_ids, all_racks, desired_rf,
+                         dict(T=T, N=N, R=R, seed=seed, max_partitions=max_partitions, tail=tail, remove_frac=remove_frac))
+
+
 # BASELINE.json configs (index = position in `configs`); seeds 0x5EED0000 + config#.
 CONFIGS = {
     "c1": dict(T=10, P=8, RF=3, N=6, R=3, seed=0x5EED0001, n_old=6),
