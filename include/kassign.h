@@ -139,6 +139,28 @@ int32_t ka_solve_dense_device(ka_ctx* ctx, int32_t T, const int32_t* d_topic_has
                               const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride,
                               int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st);
 
+/* The dense problem of ka_solve_dense_device, solved against K candidate broker tables, each on a FRESH Context
+ * (all counters zero) — K independent runs of the reference tool over one cluster (KAG:172, one assigner per run), e.g. the
+ * broker sets of a decommission sweep. The candidates run side by side inside every kernel: the number of kernel launches
+ * does not depend on K.
+ *   cand_off[K+1]      host; table k is broker_id/broker_rack[cand_off[k] .. cand_off[k+1]-1]
+ *   broker_id, broker_rack   host; per table, exactly what ka_ctx_set_brokers takes (ids strictly ascending, rack index)
+ *   d_topic_hash, d_cur_broker   device, shared by all candidates
+ *   d_out_broker       device [K][T*P][out_stride]; d_out_len device [K][T*P] or NULL
+ *   st[K]              host, required; st[k] is candidate k's status
+ * Candidate k gives exactly what ka_ctx_create -> ka_ctx_set_brokers(table k) -> ka_solve_dense_device gives: the same rows,
+ * out_len and status fields. The rows of a failed candidate are unspecified; a failing candidate changes nothing of another.
+ * Limits, checked before anything is enqueued: K <= 128 and out_stride <= 3 (else KA_ERR_LIMIT); out_stride >=
+ * max(RF, desired_rf) (else KA_ERR_BAD_ARG); every table as ka_ctx_set_brokers checks it (same code). K == 0 or T == 0:
+ * KA_OK, nothing written.
+ * Synchronises `stream` before returning. Returns KA_OK when every candidate solved, else st[k].code of the lowest failing k;
+ * library-side failures (bad argument, limit, CUDA) are returned directly and written to every st[k].
+ * Does not read or change ctx's own Context, broker table, parked counters or topic_base. */
+int32_t ka_solve_dense_candidates_device(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                                         const int32_t* broker_rack, int32_t T, const int32_t* d_topic_hash, int32_t P,
+                                         int32_t RF, const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride,
+                                         int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

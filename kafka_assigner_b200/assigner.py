@@ -248,6 +248,26 @@ class Solver:
             return None
         return st
 
+    def solve_dense_candidates_device(self, tables, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, d_out_len, d_out,
+                                      stream=0):
+        """ka_solve_dense_candidates_device: the dense device solve against every broker table of `tables` (a list of
+        (broker_id, rack_index) numpy pairs), each on a fresh Context; this Solver's own Context is untouched. Candidate k's
+        rows are d_out[k] ([K, T, P, out_stride] on the device). Synchronous; returns the K KaStatus."""
+        ids = [np.ascontiguousarray(b, dtype=np.int32) for b, _ in tables]
+        racks = [np.ascontiguousarray(r, dtype=np.int32) for _, r in tables]
+        assert all(len(b) == len(r) for b, r in zip(ids, racks))
+        cand_off = np.zeros(len(tables) + 1, dtype=np.int32)
+        np.cumsum([len(b) for b in ids], out=cand_off[1:])
+        broker_id = np.concatenate(ids) if ids else np.zeros(0, dtype=np.int32)
+        broker_rack = np.concatenate(racks) if racks else np.zeros(0, dtype=np.int32)
+        st = (KaStatus * max(len(tables), 1))()
+        self._L.ka_solve_dense_candidates_device(self._h, len(tables), _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), int(T),
+                                                 ctypes.c_void_p(d_topic_hash), int(P), int(RF), ctypes.c_void_p(d_cur),
+                                                 int(desired_rf), int(out_stride),
+                                                 ctypes.c_void_p(d_out_len) if d_out_len else None, ctypes.c_void_p(d_out),
+                                                 ctypes.c_void_p(stream) if stream else None, st)
+        return [st[k] for k in range(len(tables))]
+
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""
         rc = self._L.ka_stage_dense_device(self._h, int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF),

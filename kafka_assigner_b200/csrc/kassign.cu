@@ -55,6 +55,7 @@ constexpr int KA_MAX_CHAIN_EVENTS = 64;   // per solve: 8 staged blocks x 8 sub-
 // rows into fragments of KA_JSON_FRAG_ROWS rows (more per fragment only beyond KA_MAX_JSON_FRAGS of them), so that the text
 // streams out while later fragments are still being built and every fragment stays far below the 4 GiB of its 32-bit offsets.
 constexpr int KA_MAX_JSON_FRAGS = 256;
+constexpr int KA_MAX_CANDIDATES = 128;    // candidate broker tables of one batched solve
 constexpr int64_t KA_JSON_FRAG_ROWS = 1 << 18;
 
 struct HostPinned {
@@ -118,6 +119,10 @@ struct ka_ctx {
     DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len, d_tstatus, d_flags;
     DevBuf d_rec, d_perm, d_ntl, d_loff, d_lend, d_lvl_end;  // records, chosen positions, schedule permutation, level tables
     DevBuf d_json, d_names, d_name_off, d_part_id, d_json_rowlen, d_json_blocksum, d_json_state;
+    // scratch of ka_solve_dense_candidates_device, apart from the single solve's: descriptors + broker tables, counters,
+    // records, level tables, status
+    DevBuf d_cand_tab, d_cand_ctr, d_cand_rec, d_cand_perm, d_cand_ntl, d_cand_lend, d_cand_loff, d_cand_lvl_end, d_cand_tstatus,
+        d_cand_flags;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -210,10 +215,67 @@ int park_counters(ka_ctx* c) {
     return KA_OK;
 }
 
+// What ka_ctx_set_brokers refuses in a broker table.
+int check_brokers(int N, const int32_t* broker_id, const int32_t* broker_rack) {
+    if (N < 0 || (N > 0 && (!broker_id || !broker_rack))) return KA_ERR_BAD_ARG;
+    if (N > 65535) return KA_ERR_LIMIT;
+    for (int i = 0; i < N; ++i) {
+        if (i > 0 && broker_id[i] <= broker_id[i - 1]) return KA_ERR_BAD_ARG;  // strictly ascending
+        if (broker_rack[i] < 0 || broker_rack[i] >= 65535) return KA_ERR_BAD_ARG;
+    }
+    return KA_OK;
+}
+
+// The device image of a (checked) broker table: the blob kernel A stages (rack16 || lut16; the LUT part only in
+// KA_LUT_SMEM mode) and, in KA_LUT_GLOBAL mode, the id -> index LUT it reads from global memory.
+struct BrokerTable {
+    int lut_mode = KA_LUT_SMEM, min_id = 0, lut_off = 0;
+    uint32_t range = 0;
+    std::vector<uint16_t> blob, glut;
+};
+
+BrokerTable broker_table(int N, const int32_t* broker_id, const int32_t* broker_rack) {
+    BrokerTable t;
+    t.min_id = N > 0 ? broker_id[0] : 0;
+    const uint64_t range64 = N > 0 ? (uint64_t)((int64_t)broker_id[N - 1] - (int64_t)broker_id[0]) + 1 : 0;
+    const size_t npad = align16((size_t)std::max(N, 1) * 2) / 2;  // uint16 elements, 16B multiple
+    // compact rack ids in order of first appearance (rack identity is all that matters, KAS:90-94)
+    std::vector<uint16_t> rackc(std::max(N, 1), 0);
+    {
+        std::unordered_map<int32_t, int> seen;
+        for (int i = 0; i < N; ++i) {
+            auto it = seen.find(broker_rack[i]);
+            if (it == seen.end()) it = seen.emplace(broker_rack[i], (int)seen.size()).first;
+            rackc[i] = (uint16_t)it->second;
+        }
+    }
+    size_t lut_elems = 0;
+    if (range64 <= KA_LUT_SMEM_MAX_RANGE) {
+        t.lut_mode = KA_LUT_SMEM;
+        t.range = (uint32_t)range64;
+        lut_elems = align16((size_t)std::max<uint64_t>(range64, 1) * 2) / 2;
+    } else if (range64 <= KA_LUT_GLOBAL_MAX_RANGE) {
+        t.lut_mode = KA_LUT_GLOBAL;
+        t.range = (uint32_t)range64;
+        t.glut.assign((size_t)range64, (uint16_t)KA_DEAD);
+        for (int i = 0; i < N; ++i) t.glut[(size_t)((int64_t)broker_id[i] - t.min_id)] = (uint16_t)i;
+    } else {
+        t.lut_mode = KA_LUT_BSEARCH;
+        t.range = 0;
+    }
+    t.lut_off = (int)npad;
+    t.blob.assign(npad + lut_elems, (uint16_t)KA_DEAD);
+    for (int i = 0; i < N; ++i) {
+        t.blob[i] = rackc[i];
+        if (t.lut_mode == KA_LUT_SMEM) t.blob[npad + (size_t)((int64_t)broker_id[i] - t.min_id)] = (uint16_t)i;
+    }
+    return t;
+}
+
 constexpr size_t KA_ORDER_SMEM_BUDGET = 226 * 1024;
 
-int make_plan(ka_ctx* c, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged, Plan& pl, ka_status* st) {
-    const int N = c->N;
+// N / blob_bytes: the broker table (the largest one of a batched solve).
+int make_plan(int N, int blob_bytes, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged, Plan& pl, ka_status* st) {
     if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX, 0);
     // ---- kernel A
     pl.a_load_kind = capmax <= 255 ? 0 : (capmax <= 65535 ? 1 : 2);
@@ -229,7 +291,7 @@ int make_plan(ka_ctx* c, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged
     pl.lv_p_bytes = pl.a_levels ? (int)align16((size_t)(std::max(Pmax, 1) + 2) * 2) : 0;
     const size_t per_warp = (size_t)pl.a_load_bytes + pl.a_slab_bytes + pl.a_cnt_bytes + pl.lv_owner_bytes + pl.lv_last_bytes +
                             2 * (size_t)pl.lv_p_bytes;
-    const size_t shared = 16 + (size_t)c->blob_bytes;
+    const size_t shared = 16 + (size_t)blob_bytes;
     if (shared + per_warp > KA_SMEM_BUDGET) return set_status(st, KA_ERR_LIMIT, -1, -1, Pmax, N);
     pl.a_warps = (int)std::min<size_t>(16, (KA_SMEM_BUDGET - shared) / per_warp);
     pl.a_smem = shared + per_warp * pl.a_warps;
@@ -310,7 +372,7 @@ int describe_block(ka_ctx* c, const Shape& sh, int t0, int t1, int blk, StageDes
         d.Pmax = sh.P;
         d.capmax = c->N > 0 ? ((int64_t)sh.P * std::max(rf_t, 0) + c->N - 1) / c->N : 0;
     }
-    return make_plan(c, d.Q, d.S, d.Pmax, d.capmax, ragged, d.pl, st);
+    return make_plan(c->N, c->blob_bytes, d.Q, d.S, d.Pmax, d.capmax, ragged, d.pl, st);
 }
 
 // Scratch of a solve of the blocks ds[0..K) (consecutive: the last one ends the problem).
@@ -354,9 +416,10 @@ int reset_flags(ka_ctx* c, cudaStream_t s) {
     return KA_OK;
 }
 
-template <typename LoadT, bool LEVELS, int SM>
-cudaError_t launch_stage_t(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T) {
-    auto kern = ka_sticky_spread_kernel<LoadT, LEVELS, SM>;
+// ncand > 0: kernel A of a batched solve over ncand candidate tables (p.cand), grid.y = candidate.
+template <typename LoadT, bool LEVELS, int SM, bool CAND>
+cudaError_t launch_stage_t(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand) {
+    auto kern = ka_sticky_spread_kernel<LoadT, LEVELS, SM, CAND>;
     const int threads = pl.a_warps * 32;
     cudaError_t e = allow_smem(kern, pl.a_smem);
     if (e != cudaSuccess) return e;
@@ -364,34 +427,61 @@ cudaError_t launch_stage_t(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, co
     e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, pl.a_smem);
     if (e != cudaSuccess) return e;
     int grid = (T + pl.a_warps - 1) / pl.a_warps;
-    grid = std::min(grid, std::max(1, occ) * c->sm_count);
-    kern<<<grid, threads, pl.a_smem, s>>>(p, pl.a_load_bytes, pl.a_slab_bytes, pl.a_cnt_bytes, pl.lv_owner_bytes, pl.lv_last_bytes, pl.lv_p_bytes);
+    grid = std::min(grid, std::max(1, std::max(1, occ) * c->sm_count / std::max(ncand, 1)));
+    kern<<<dim3(grid, std::max(ncand, 1)), threads, pl.a_smem, s>>>(p, pl.a_load_bytes, pl.a_slab_bytes, pl.a_cnt_bytes, pl.lv_owner_bytes,
+                                                                 pl.lv_last_bytes, pl.lv_p_bytes);
     return cudaGetLastError();
 }
 
-template <typename LoadT, bool LEVELS>
-cudaError_t launch_stage(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T) {
-    return p.S <= 3 ? launch_stage_t<LoadT, LEVELS, 3>(c, s, p, pl, T) : launch_stage_t<LoadT, LEVELS, 8>(c, s, p, pl, T);
+template <typename LoadT, bool LEVELS, bool CAND>
+cudaError_t launch_stage(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand) {
+    return p.S <= 3 ? launch_stage_t<LoadT, LEVELS, 3, CAND>(c, s, p, pl, T, ncand) : launch_stage_t<LoadT, LEVELS, 8, CAND>(c, s, p, pl, T, ncand);
+}
+
+// Kernel A in the instantiation the plan asks for.
+template <bool CAND>
+int launch_stage_plan(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand) {
+    cudaError_t e;
+    if (pl.a_levels) {
+        if (pl.a_load_kind == 0) e = launch_stage<uint8_t, true, CAND>(c, s, p, pl, T, ncand);
+        else if (pl.a_load_kind == 1) e = launch_stage<uint16_t, true, CAND>(c, s, p, pl, T, ncand);
+        else e = launch_stage<uint32_t, true, CAND>(c, s, p, pl, T, ncand);
+    } else {
+        if (pl.a_load_kind == 0) e = launch_stage<uint8_t, false, CAND>(c, s, p, pl, T, ncand);
+        else if (pl.a_load_kind == 1) e = launch_stage<uint16_t, false, CAND>(c, s, p, pl, T, ncand);
+        else e = launch_stage<uint32_t, false, CAND>(c, s, p, pl, T, ncand);
+    }
+    KA_CUDA(e);
+    c->launches++;
+    return KA_OK;
+}
+
+// Kernel A's view of the problem of block d (the broker table and the outputs are set by the caller).
+KaSolveParams stage_params(const StageDesc& d) {
+    KaSolveParams p{};
+    p.T = d.T;
+    p.topic_base = d.topic_base;
+    p.topic_hash = d.d_hash;
+    p.part_off = d.d_part_off;
+    p.P = d.P;
+    p.rep_off = d.d_rep_off;
+    p.RF = d.RF;
+    p.cur = d.d_cur;
+    p.desired_rf = d.desired_rf;
+    p.S = d.S;
+    p.Pmax = d.Pmax;
+    p.rec_kind = d.pl.rec_kind;
+    p.chunk_w = d.pl.b_threads;
+    return p;
 }
 
 // Context-free part of a block (shards across GPUs): kernel A (records in schedule order) + the level tables.
 // a_done is recorded at the end of kernel A when timing is on.
 int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done) {
-    const int N = c->N, S = d.S;
+    const int N = c->N;
     const Plan& pl = d.pl;
     if (d.T > 0) {
-        KaSolveParams p{};
-        p.T = d.T;
-        p.topic_base = d.topic_base;
-        p.topic_hash = d.d_hash;
-        p.part_off = d.d_part_off;
-        p.P = d.P;
-        p.rep_off = d.d_rep_off;
-        p.RF = d.RF;
-        p.cur = d.d_cur;
-        p.desired_rf = d.desired_rf;
-        p.S = S;
-        p.Pmax = d.Pmax;
+        KaSolveParams p = stage_params(d);
         p.N = N;
         p.blob = c->d_blob.as<uint16_t>();
         p.blob_bytes = c->blob_bytes;
@@ -401,26 +491,14 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done)
         p.range = c->range;
         p.glut = c->d_glut.as<uint16_t>();
         p.broker_id = c->d_broker_id.as<int32_t>();
-        p.rec_kind = pl.rec_kind;
         p.rec = c->d_rec.as<unsigned char>() + (size_t)d.q0 * pl.rec_bytes;
         p.perm = pl.a_levels ? c->d_perm.as<uint16_t>() + d.q0 : nullptr;
-        p.chunk_w = pl.b_threads;
         p.ntl = pl.a_levels ? c->d_ntl.as<int32_t>() + d.topic_base : nullptr;
         p.lend = pl.a_levels ? c->d_lend.as<uint32_t>() + d.q0 : nullptr;
         p.tstatus = c->d_tstatus.as<int4>();
         p.err_topic = c->d_flags.as<unsigned>();
-        cudaError_t e;
-        if (pl.a_levels) {
-            if (pl.a_load_kind == 0) e = launch_stage<uint8_t, true>(c, s, p, pl, d.T);
-            else if (pl.a_load_kind == 1) e = launch_stage<uint16_t, true>(c, s, p, pl, d.T);
-            else e = launch_stage<uint32_t, true>(c, s, p, pl, d.T);
-        } else {
-            if (pl.a_load_kind == 0) e = launch_stage<uint8_t, false>(c, s, p, pl, d.T);
-            else if (pl.a_load_kind == 1) e = launch_stage<uint16_t, false>(c, s, p, pl, d.T);
-            else e = launch_stage<uint32_t, false>(c, s, p, pl, d.T);
-        }
-        KA_CUDA(e);
-        c->launches++;
+        const int rc = launch_stage_plan<false>(c, s, p, pl, d.T, 0);
+        if (rc != KA_OK) return rc;
     }
     if (c->timing) KA_CUDA(cudaEventRecord(a_done, s));
     if (pl.a_levels && d.T > 0) {
@@ -436,34 +514,36 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done)
     return KA_OK;
 }
 
-template <int KIND, int MAXNT, bool GCTR, bool SINGLE, bool WARP1, bool FULL>
-cudaError_t launch_order_t(cudaStream_t s, const KaOrderParams& o, const Plan& pl) {
-    auto kern = ka_order_levels_kernel<KIND, GCTR, MAXNT, SINGLE, WARP1, FULL>;
+// CAND: one CTA per candidate of a batched solve (ncand of them), else one CTA.
+template <int KIND, int MAXNT, bool CAND, bool GCTR, bool SINGLE, bool WARP1, bool FULL>
+cudaError_t launch_order_t(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int ncand) {
+    auto kern = ka_order_levels_kernel<KIND, GCTR, MAXNT, SINGLE, WARP1, FULL, CAND>;
     cudaError_t e = allow_smem(kern, pl.b_smem);
     if (e != cudaSuccess) return e;
-    kern<<<1, pl.b_threads, pl.b_smem, s>>>(o);
+    kern<<<CAND ? ncand : 1, pl.b_threads, pl.b_smem, s>>>(o);
     return cudaGetLastError();
 }
 
 // KIND 0 / 1: slot chains of rows <= 3 (chunk arithmetic, barrier flavour, full chunks are compile-time); 4 / 8: rows of 4 / 5..8
-template <int KIND, int MAXNT>
-cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl) {
+template <int KIND, int MAXNT, bool CAND = false>
+cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int ncand = 0) {
     if constexpr (KIND > 1) {
-        return pl.b_gctr ? launch_order_t<KIND, MAXNT, true, false, false, false>(s, o, pl) : launch_order_t<KIND, MAXNT, false, false, false, false>(s, o, pl);
+        return pl.b_gctr ? launch_order_t<KIND, MAXNT, false, true, false, false, false>(s, o, pl, ncand)
+                         : launch_order_t<KIND, MAXNT, false, false, false, false, false>(s, o, pl, ncand);
     } else {
         const bool warp1 = pl.b_threads == 32;                                                          // window mode
         const bool single = !warp1 && o.uniform_width != 0 && o.uniform_width <= (uint32_t)pl.b_threads;   // chunk = topic
         const bool full = single && o.uniform_width == (uint32_t)pl.b_threads;                          // no idle lane
         const int sel = (pl.b_gctr ? 4 : 0) | (warp1 ? 1 : (full ? 3 : (single ? 2 : 0)));
         switch (sel) {
-            case 0: return launch_order_t<KIND, MAXNT, false, false, false, false>(s, o, pl);
-            case 1: return launch_order_t<KIND, MAXNT, false, false, true, false>(s, o, pl);
-            case 2: return launch_order_t<KIND, MAXNT, false, true, false, false>(s, o, pl);
-            case 3: return launch_order_t<KIND, MAXNT, false, true, false, true>(s, o, pl);
-            case 4: return launch_order_t<KIND, MAXNT, true, false, false, false>(s, o, pl);
-            case 5: return launch_order_t<KIND, MAXNT, true, false, true, false>(s, o, pl);
-            case 6: return launch_order_t<KIND, MAXNT, true, true, false, false>(s, o, pl);
-            default: return launch_order_t<KIND, MAXNT, true, true, false, true>(s, o, pl);
+            case 0: return launch_order_t<KIND, MAXNT, CAND, false, false, false, false>(s, o, pl, ncand);
+            case 1: return launch_order_t<KIND, MAXNT, CAND, false, false, true, false>(s, o, pl, ncand);
+            case 2: return launch_order_t<KIND, MAXNT, CAND, false, true, false, false>(s, o, pl, ncand);
+            case 3: return launch_order_t<KIND, MAXNT, CAND, false, true, false, true>(s, o, pl, ncand);
+            case 4: return launch_order_t<KIND, MAXNT, CAND, true, false, false, false>(s, o, pl, ncand);
+            case 5: return launch_order_t<KIND, MAXNT, CAND, true, false, true, false>(s, o, pl, ncand);
+            case 6: return launch_order_t<KIND, MAXNT, CAND, true, true, false, false>(s, o, pl, ncand);
+            default: return launch_order_t<KIND, MAXNT, CAND, true, true, false, true>(s, o, pl, ncand);
         }
     }
 }
@@ -944,7 +1024,8 @@ void ka_ctx_destroy(ka_ctx* c) {
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
                       &c->d_out, &c->d_out_len, &c->d_tstatus, &c->d_flags, &c->d_rec, &c->d_perm, &c->d_ntl, &c->d_loff, &c->d_lend,
                       &c->d_lvl_end, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen, &c->d_json_blocksum,
-                      &c->d_json_state})
+                      &c->d_json_state, &c->d_cand_tab, &c->d_cand_ctr, &c->d_cand_rec, &c->d_cand_perm, &c->d_cand_ntl,
+                      &c->d_cand_lend, &c->d_cand_loff, &c->d_cand_lvl_end, &c->d_cand_tstatus, &c->d_cand_flags})
         b->release();
     for_each_event(c, [](cudaEvent_t& e, bool) {
         if (e) cudaEventDestroy(e);
@@ -967,56 +1048,24 @@ int32_t ka_ctx_reset(ka_ctx* c) {
 
 int32_t ka_ctx_set_brokers(ka_ctx* c, int32_t N, const int32_t* broker_id, const int32_t* broker_rack) {
     if (!c) return KA_ERR_NO_DEVICE;
-    if (N < 0 || (N > 0 && (!broker_id || !broker_rack))) return KA_ERR_BAD_ARG;
-    if (N > 65535) return KA_ERR_LIMIT;
-    for (int i = 0; i < N; ++i) {
-        if (i > 0 && broker_id[i] <= broker_id[i - 1]) return KA_ERR_BAD_ARG;  // strictly ascending
-        if (broker_rack[i] < 0 || broker_rack[i] >= 65535) return KA_ERR_BAD_ARG;
-    }
-    int rc = enter(c, true);
-    if (rc != KA_OK || (rc = park_counters(c)) != KA_OK) return rc;
+    int rc = check_brokers(N, broker_id, broker_rack);
+    if (rc != KA_OK) return rc;
+    if ((rc = enter(c, true)) != KA_OK || (rc = park_counters(c)) != KA_OK) return rc;
 
     c->N = N;
     c->broker_id.assign(broker_id, broker_id + N);
-    c->min_id = N > 0 ? broker_id[0] : 0;
-    const uint64_t range64 = N > 0 ? (uint64_t)((int64_t)broker_id[N - 1] - (int64_t)broker_id[0]) + 1 : 0;
-    const size_t npad = align16((size_t)std::max(N, 1) * 2) / 2;  // uint16 elements, 16B multiple
-    // compact rack ids in order of first appearance (rack identity is all that matters, KAS:90-94)
-    std::vector<uint16_t> rackc(std::max(N, 1), 0);
-    {
-        std::unordered_map<int32_t, int> seen;
-        for (int i = 0; i < N; ++i) {
-            auto it = seen.find(broker_rack[i]);
-            if (it == seen.end()) it = seen.emplace(broker_rack[i], (int)seen.size()).first;
-            rackc[i] = (uint16_t)it->second;
-        }
+    const BrokerTable t = broker_table(N, broker_id, broker_rack);
+    c->min_id = t.min_id;
+    c->lut_mode = t.lut_mode;
+    c->range = t.range;
+    if (t.lut_mode == KA_LUT_GLOBAL) {
+        KA_CUDA(c->d_glut.reserve(t.glut.size() * 2));
+        KA_CUDA(cudaMemcpy(c->d_glut.p, t.glut.data(), t.glut.size() * 2, cudaMemcpyHostToDevice));
     }
-    std::vector<uint16_t> blob;
-    size_t lut_elems = 0;
-    if (range64 <= KA_LUT_SMEM_MAX_RANGE) {
-        c->lut_mode = KA_LUT_SMEM;
-        c->range = (uint32_t)range64;
-        lut_elems = align16((size_t)std::max<uint64_t>(range64, 1) * 2) / 2;
-    } else if (range64 <= KA_LUT_GLOBAL_MAX_RANGE) {
-        c->lut_mode = KA_LUT_GLOBAL;
-        c->range = (uint32_t)range64;
-        std::vector<uint16_t> g((size_t)range64, (uint16_t)KA_DEAD);
-        for (int i = 0; i < N; ++i) g[(size_t)((int64_t)broker_id[i] - c->min_id)] = (uint16_t)i;
-        KA_CUDA(c->d_glut.reserve(g.size() * 2));
-        KA_CUDA(cudaMemcpy(c->d_glut.p, g.data(), g.size() * 2, cudaMemcpyHostToDevice));
-    } else {
-        c->lut_mode = KA_LUT_BSEARCH;
-        c->range = 0;
-    }
-    c->lut_off = (int)npad;
-    blob.assign(npad + lut_elems, (uint16_t)KA_DEAD);
-    for (int i = 0; i < N; ++i) {
-        blob[i] = rackc[i];
-        if (c->lut_mode == KA_LUT_SMEM) blob[npad + (size_t)((int64_t)broker_id[i] - c->min_id)] = (uint16_t)i;
-    }
-    c->blob_bytes = (int)(blob.size() * 2);
-    KA_CUDA(c->d_blob.reserve(blob.size() * 2));
-    KA_CUDA(cudaMemcpy(c->d_blob.p, blob.data(), blob.size() * 2, cudaMemcpyHostToDevice));
+    c->lut_off = t.lut_off;
+    c->blob_bytes = (int)(t.blob.size() * 2);
+    KA_CUDA(c->d_blob.reserve(t.blob.size() * 2));
+    KA_CUDA(cudaMemcpy(c->d_blob.p, t.blob.data(), t.blob.size() * 2, cudaMemcpyHostToDevice));
     KA_CUDA(c->d_broker_id.reserve((size_t)std::max(N, 1) * 4));
     if (N > 0) KA_CUDA(cudaMemcpy(c->d_broker_id.p, broker_id, (size_t)N * 4, cudaMemcpyHostToDevice));
     // counters for the new table
@@ -1116,6 +1165,199 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     if ((rc = enter(c, true)) != KA_OK || (rc = run_solve(c, s, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, io, st)) != KA_OK)
         return failed(st, rc);
     return finish(c, s, st, false);
+}
+
+// Everything of a batched solve over K candidate tables, enqueued on `s` (slot-0 chains on c->sb1): the candidates' tables
+// and descriptors H2D, fresh counters, kernel A with grid.y = candidate, the level tables of all candidates as one table,
+// then per chain sub-block the slot-0 / slot-1 chains (one CTA per candidate) and the emit (grid.y = candidate).
+static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<BrokerTable>& tabs, const int32_t* cand_off,
+                          const int32_t* broker_id, const StageDesc& d, int32_t* d_out_len, int32_t* d_out) {
+    const Plan& pl = d.pl;
+    const int T = d.T, S = d.S;
+    const int64_t Q = d.Q;
+    const size_t q = (size_t)std::max<int64_t>(Q, 1), kq = (size_t)K * q, kt = (size_t)K * T;
+    // descriptors, then every candidate's blob, global LUT and broker ids, in one upload
+    std::vector<size_t> blob_off(K), glut_off(K), bid_off(K), ctr_off(K);
+    size_t bytes = align16((size_t)K * sizeof(KaCandidate)), ctr_ints = 0;
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        blob_off[k] = bytes;
+        bytes += tabs[k].blob.size() * 2;
+        glut_off[k] = bytes;
+        bytes += align16(tabs[k].glut.size() * 2);
+        bid_off[k] = bytes;
+        bytes += align16((size_t)std::max(n, 1) * 4);
+        ctr_off[k] = ctr_ints;
+        ctr_ints += (size_t)(n + 1) * KA_MAX_SLOTS;   // + the chains' dummy row
+    }
+    KA_CUDA(c->d_cand_tab.reserve(bytes));
+    KA_CUDA(c->d_cand_ctr.reserve(ctr_ints * 4));
+    KA_CUDA(c->d_cand_rec.reserve(kq * 16));
+    if (pl.a_levels) {
+        KA_CUDA(c->d_cand_perm.reserve(kq * 2));
+        KA_CUDA(c->d_cand_lend.reserve(kq * 4));
+        KA_CUDA(c->d_cand_lvl_end.reserve(kq * 4));
+        KA_CUDA(c->d_cand_ntl.reserve(kt * 4));
+        KA_CUDA(c->d_cand_loff.reserve((kt + 1) * 4));
+    }
+    KA_CUDA(c->d_cand_tstatus.reserve(kt * sizeof(int4)));
+    KA_CUDA(c->d_cand_flags.reserve((size_t)K * 4));
+    unsigned char* base = c->d_cand_tab.as<unsigned char>();
+    std::vector<unsigned char> h(bytes, 0);
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        const BrokerTable& t = tabs[k];
+        KaCandidate e{};
+        e.N = n;
+        e.lut_mode = t.lut_mode;
+        e.lut_off = t.lut_off;
+        e.blob_bytes = (int)(t.blob.size() * 2);
+        e.min_id = t.min_id;
+        e.range = t.range;
+        e.blob = reinterpret_cast<const uint16_t*>(base + blob_off[k]);
+        e.glut = reinterpret_cast<const uint16_t*>(base + glut_off[k]);
+        e.broker_id = reinterpret_cast<const int32_t*>(base + bid_off[k]);
+        e.ctr8 = c->d_cand_ctr.as<int32_t>() + ctr_off[k];
+        e.rec = c->d_cand_rec.as<unsigned char>() + (size_t)k * q * 16;
+        if (pl.a_levels) {
+            e.perm = c->d_cand_perm.as<uint16_t>() + (size_t)k * q;
+            e.ntl = c->d_cand_ntl.as<int32_t>() + (size_t)k * T;
+            e.lend = c->d_cand_lend.as<uint32_t>() + (size_t)k * q;
+            e.loff = c->d_cand_loff.as<int32_t>() + (size_t)k * T;
+            e.pos0 = (uint32_t)((size_t)k * Q);   // the level tables of the K candidates are one table of K * T topics
+        }
+        e.tstatus = c->d_cand_tstatus.as<int4>() + (size_t)k * T;
+        e.err_topic = c->d_cand_flags.as<unsigned>() + k;
+        std::memcpy(h.data() + (size_t)k * sizeof(KaCandidate), &e, sizeof(e));
+        std::memcpy(h.data() + blob_off[k], t.blob.data(), t.blob.size() * 2);
+        if (!t.glut.empty()) std::memcpy(h.data() + glut_off[k], t.glut.data(), t.glut.size() * 2);
+        if (n > 0) std::memcpy(h.data() + bid_off[k], broker_id + cand_off[k], (size_t)n * 4);
+    }
+    const KaCandidate* cand = c->d_cand_tab.as<KaCandidate>();
+    KA_CUDA(cudaMemcpyAsync(base, h.data(), bytes, cudaMemcpyHostToDevice, s));
+    KA_CUDA(cudaMemsetAsync(c->d_cand_ctr.p, 0, ctr_ints * 4, s));   // every candidate starts from a fresh Context
+    KA_CUDA(cudaMemsetAsync(c->d_cand_flags.p, 0xFF, (size_t)K * 4, s));
+    // kernel A: grid.y = candidate; the shared-memory layout is that of the largest table
+    KaSolveParams p = stage_params(d);
+    p.N = 0;
+    p.blob_bytes = 0;
+    for (const BrokerTable& t : tabs) p.blob_bytes = std::max(p.blob_bytes, (int)(t.blob.size() * 2));
+    p.cand = cand;
+    int rc = launch_stage_plan<true>(c, s, p, pl, T, K);
+    if (rc != KA_OK) return rc;
+    if (pl.a_levels) {
+        ka_level_scan_kernel<<<1, 1024, 0, s>>>(c->d_cand_ntl.as<int32_t>(), (int)kt, c->d_cand_loff.as<int32_t>());
+        KA_CUDA(cudaGetLastError());
+        ka_level_fill_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(c->d_cand_ntl.as<int32_t>(), c->d_cand_loff.as<int32_t>(),
+                                                                      c->d_cand_lend.as<uint32_t>(), nullptr, d.P, (int)kt,
+                                                                      c->d_cand_lvl_end.as<uint32_t>());
+        KA_CUDA(cudaGetLastError());
+        c->launches += 2;
+    }
+    if (Q <= 0) return KA_OK;
+    // the chains: slot 0 of sub-block j+1 (c->sb1) overlaps slot 1 + emit of sub-block j (s), as in the single solve
+    if ((rc = chain_fork(c, s)) != KA_OK) return rc;
+    const int nsub = chain_subblocks(d, 1);
+    for (int j = 0; j < nsub; ++j) {
+        const SubBlock b = sub_block(d, j, nsub);
+        KaOrderParams o{};
+        o.N = 0;
+        o.S = S;
+        o.uniform_width = pl.a_levels ? 0u : (uint32_t)d.P;
+        o.chunk_end = pl.a_levels ? c->d_cand_lvl_end.as<uint32_t>() : nullptr;
+        o.ring_log2 = pl.b_ring_log2;
+        o.Q = (uint32_t)b.rq;
+        o.pos_base = (uint32_t)b.r0;
+        o.cand = cand;
+        o.cand_t0 = b.t0;
+        o.cand_t1 = b.t1;
+        KA_CUDA((launch_order<0, 1024, true>(c->sb1, o, pl, K)));
+        KA_CUDA(cudaEventRecord(c->ev_b1[j], c->sb1));
+        KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[j], 0));
+        KA_CUDA((launch_order<1, 1024, true>(s, o, pl, K)));
+        ka_emit3_candidates_kernel<<<dim3((unsigned)((b.rq + 255) / 256), K), 256, 0, s>>>(cand, (uint32_t)b.r0, b.t1 - b.t0, d.P,
+                                                                                           (uint32_t)b.rq, S, Q, d_out, d_out_len);
+        KA_CUDA(cudaGetLastError());
+        c->launches += 3;
+    }
+    return KA_OK;
+}
+
+int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                                         const int32_t* broker_rack, int32_t T, const int32_t* d_topic_hash, int32_t P,
+                                         int32_t RF, const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride,
+                                         int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
+    auto all = [&](int rc) {   // a library-side failure: every candidate reports it
+        for (int k = 0; k < K; ++k) set_status(st + k, rc);
+        return rc;
+    };
+    if (!c) return all(KA_ERR_NO_DEVICE);
+    if (K > KA_MAX_CANDIDATES || out_stride > 3) return all(KA_ERR_LIMIT);   // wider rows: the fused chain of the single solve
+    if (T < 0 || P < 0 || RF < 0 || out_stride < 1 || out_stride < std::max(RF, desired_rf)) return all(KA_ERR_BAD_ARG);
+    if (K == 0) return KA_OK;
+    if (!cand_off || cand_off[0] != 0) return all(KA_ERR_BAD_ARG);
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        if (cand_off[k + 1] < cand_off[k] || (n > 0 && (!broker_id || !broker_rack))) return all(KA_ERR_BAD_ARG);
+        const int rc = n > 0 ? check_brokers(n, broker_id + cand_off[k], broker_rack + cand_off[k]) : KA_OK;
+        if (rc != KA_OK) return all(rc);
+    }
+    if (T == 0) return KA_OK;
+    const int64_t Q = (int64_t)T * P;
+    if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
+    if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
+    int rc = enter(c, true);
+    if (rc != KA_OK) return all(rc);
+    // the plan of the call: counter placement and loop shape from the largest table, levels if any candidate has capacity > 1
+    std::vector<BrokerTable> tabs(K);
+    int nmax = 0, blob_max = 0;
+    int64_t capmax = 0;
+    const int rf_t = desired_rf >= 0 ? desired_rf : RF;
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        tabs[k] = broker_table(n, broker_id + cand_off[k], broker_rack + cand_off[k]);
+        nmax = std::max(nmax, n);
+        blob_max = std::max(blob_max, (int)(tabs[k].blob.size() * 2));
+        if (n > 0) capmax = std::max<int64_t>(capmax, ((int64_t)P * std::max(rf_t, 0) + n - 1) / n);
+    }
+    StageDesc d;
+    d.T = T;
+    d.Q = Q;
+    d.d_hash = d_topic_hash;
+    d.P = P;
+    d.RF = RF;
+    d.d_cur = d_cur_broker;
+    d.desired_rf = desired_rf;
+    d.S = out_stride;
+    d.Pmax = P;
+    d.capmax = capmax;
+    if ((rc = make_plan(nmax, blob_max, Q, out_stride, P, capmax, false, d.pl, st)) != KA_OK) {
+        for (int k = 1; k < K; ++k) st[k] = st[0];
+        return rc;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    if ((rc = enq_candidates(c, s, K, tabs, cand_off, broker_id, d, d_out_len, d_out_broker)) != KA_OK) {
+        cudaStreamSynchronize(c->sb1);
+        cudaStreamSynchronize(s);
+        return all(rc);
+    }
+    // per-candidate status: the lowest failing topic of each, as finish_status reports it for one solve
+    if (cudaStreamSynchronize(s) != cudaSuccess) return all(KA_ERR_CUDA);
+    std::vector<unsigned> err(K);
+    if (cudaMemcpy(err.data(), c->d_cand_flags.p, (size_t)K * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return all(KA_ERR_CUDA);
+    int first = KA_OK;
+    for (int k = 0; k < K; ++k) {
+        if (err[k] == 0xFFFFFFFFu) continue;
+        const int t = (int)err[k];
+        int4 ts;
+        if (cudaMemcpy(&ts, c->d_cand_tstatus.as<int4>() + (size_t)k * T + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
+            return all(KA_ERR_CUDA);
+        set_status(st + k, ts.x, t, ts.y, ts.z, ts.w);
+        if (first == KA_OK) first = ts.x;
+    }
+    return first;
 }
 
 int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash, int32_t P, int32_t RF,

@@ -29,6 +29,27 @@
 
 enum { KA_LUT_SMEM = 0, KA_LUT_GLOBAL = 1, KA_LUT_BSEARCH = 2 };
 
+// One candidate broker table of a batched solve (ka_solve_dense_candidates_device), in HBM: its broker table, its own
+// fresh Context and its slice of the call's scratch. Every kernel of the batched solve reads the entry of its candidate
+// once, at entry; the kernels of the single solve never see one.
+struct KaCandidate {
+    int N;
+    int lut_mode, lut_off, blob_bytes, min_id;
+    uint32_t range;
+    const uint16_t* blob;       // rack16 || lut16, staged by kernel A (blob_bytes of it)
+    const uint16_t* glut;       // lut_mode == KA_LUT_GLOBAL
+    const int32_t* broker_id;   // [N] ascending
+    int32_t* ctr8;              // [N+1][8] the candidate's Context.counter (+ the chains' dummy row), zero at the call's start
+    unsigned char* rec;         // [Q] records of the candidate (16 B)
+    uint16_t* perm;             // [Q] LEVELS: schedule position -> partition ordinal
+    int32_t* ntl;               // [T] LEVELS: chunks per topic
+    uint32_t* lend;             // [Q] LEVELS: topic-relative chunk ends
+    const int32_t* loff;        // [T+1] LEVELS: first chunk of each topic in the call-wide chunk table
+    uint32_t pos0;              // LEVELS: position of rec[0] in the call-wide chunk table (candidate k: k * Q)
+    int4* tstatus;              // [T] per-topic error record
+    unsigned* err_topic;        // lowest failing topic (unsigned atomicMin, 0xFFFFFFFF = none)
+};
+
 // ------------------------------------------------------------------------------------------------
 // Partition records: what kernel A hands to the leader-order kernel, in SCHEDULE order (topic by topic; inside a
 // topic by conflict level, then partition ascending). Broker indices are positions in the ascending live-id table.

@@ -83,6 +83,10 @@ struct KaOrderParams {
     int32_t* out;
     int32_t* out_len;
     int ring_log2;              // log2(records per ring stage)
+    // batched solve (CAND): CTA k orders candidate k. N / ctr8 / records / chunk table come from cand[k]: the launch walks
+    // records [pos_base, pos_base + Q) of the candidate and chunks [loff[cand_t0], loff[cand_t1]) of its chunk table.
+    const KaCandidate* cand;
+    int cand_t0, cand_t1;
 };
 
 #define KA_RING_STAGES 8
@@ -168,7 +172,9 @@ __device__ __forceinline__ void ka_order_generic(const int (&c)[RS][RS], int len
 //   all threads     chunk by chunk (<= NT records, never spanning two levels): thread i takes record i of the chunk,
 //                   loads its counter rows, decides, stores the bumps; ONE `bar.sync 0` per chunk is the only
 //                   synchronisation on the chain. The next chunk's record is read from the ring before the barrier.
-template <int KIND, bool GCTR, int MAXNT, bool SINGLE, bool WARP1, bool FULL>
+//   CAND            (slot chains only) a batched solve: CTA k orders candidate k, whose values (p.cand[k]) are read once at
+//                   entry; rec / ctr8 then take the same round trip into registers as the other invariants
+template <int KIND, bool GCTR, int MAXNT, bool SINGLE, bool WARP1, bool FULL, bool CAND = false>
 __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrderParams p) {
     constexpr int RS = KIND <= 1 ? 3 : KIND;                 // KIND 0 / 1: slot-0 / slot-1 chain of rows <= 3; 4 / 8: rows of 4 / 5..8
     constexpr int CW = KIND <= 1 ? 1 : (KIND == 4 ? 4 : 8);  // ints per broker in shared memory (one counter column for the slot chains)
@@ -181,12 +187,18 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
     uint64_t* full = reinterpret_cast<uint64_t*>(ka_osmem + ((size_t)NS << p.ring_log2) * RB);
     volatile uint32_t* pin = reinterpret_cast<volatile uint32_t*>(full + 2 * NS);   // 16 words
     int* ctr = reinterpret_cast<int*>(ka_osmem + ((size_t)NS << p.ring_log2) * RB + 256);
+    static_assert(!CAND || KIND <= 1, "batched solves order rows of <= 3 replicas");
+    const KaCandidate* const cd = CAND ? p.cand + blockIdx.x : nullptr;
+    if (CAND && cd->N <= 0) return;   // no broker: every topic of the candidate failed in kernel A
     // Loop invariants take a round trip through shared memory (volatile) so that they live in registers: ptxas otherwise
     // re-reads kernel parameters from the constant bank inside the chain loop, and every such load stalls a branch.
     if (tid == 0) {
+        const void* const rec = CAND ? (const void*)(cd->rec + (size_t)p.pos_base * RB) : p.rec;
+        int32_t* const c8 = CAND ? cd->ctr8 : p.ctr8;
         pin[0] = p.Q; pin[1] = blockDim.x; pin[2] = (uint32_t)p.ring_log2; pin[3] = p.uniform_width;
-        pin[4] = (uint32_t)reinterpret_cast<uintptr_t>(p.rec); pin[5] = (uint32_t)(reinterpret_cast<uintptr_t>(p.rec) >> 32);
-        pin[6] = (uint32_t)reinterpret_cast<uintptr_t>(p.ctr8); pin[7] = (uint32_t)(reinterpret_cast<uintptr_t>(p.ctr8) >> 32);
+        pin[4] = (uint32_t)reinterpret_cast<uintptr_t>(rec); pin[5] = (uint32_t)(reinterpret_cast<uintptr_t>(rec) >> 32);
+        pin[6] = (uint32_t)reinterpret_cast<uintptr_t>(c8); pin[7] = (uint32_t)(reinterpret_cast<uintptr_t>(c8) >> 32);
+        if (CAND) pin[8] = (uint32_t)cd->N;
     }
     __syncthreads();
     const uint32_t Q = pin[0], NT = pin[1];
@@ -201,10 +213,11 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
         ka_fence_mbar_init();
     }
     if (!GCTR)
-        for (uint32_t i = tid; i < (uint32_t)p.N * CW; i += blockDim.x)
+        for (uint32_t i = tid; i < (uint32_t)(CAND ? (int)pin[8] : p.N) * CW; i += blockDim.x)
             ctr[i] = ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))];
     if (KIND <= 1 && tid == 0) {  // the dummy broker (index N) that pads rows shorter than 3: a counter that never wins a comparison
-        if (GCTR) ctr8[(size_t)p.N * KA_MAX_SLOTS + KIND] = 0x3FFFFFFF; else ctr[p.N] = 0x3FFFFFFF;
+        const int N = CAND ? (int)pin[8] : p.N;
+        if (GCTR) ctr8[(size_t)N * KA_MAX_SLOTS + KIND] = 0x3FFFFFFF; else ctr[N] = 0x3FFFFFFF;
     }
     // idle lanes read (and ignore) ring slots past the end of the stream: make those valid records (all zero)
     for (uint32_t i = tid; i < (uint32_t)NS * G * (RB / 16); i += blockDim.x) reinterpret_cast<uint4*>(ring)[i] = make_uint4(0, 0, 0, 0);
@@ -221,7 +234,8 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
         const uint32_t slot = j & (NS - 1);
         const uint32_t bytes = min(G, Q - (j << LG)) * RB;
         ka_mbar_expect_tx(&full[slot], bytes);
-        ka_tma_bulk_g2s(ring + (size_t)slot * G * RB, reinterpret_cast<const unsigned char*>(p.rec) + (size_t)j * G * RB, bytes, &full[slot]);
+        ka_tma_bulk_g2s(ring + (size_t)slot * G * RB, reinterpret_cast<const unsigned char*>(CAND ? (const void*)orec : p.rec) + (size_t)j * G * RB,
+                        bytes, &full[slot]);
     };
     if (tid == 0)
         for (uint32_t j = 0; j < min(nstages_all, (uint32_t)NS); ++j) issue_stage(j);
@@ -232,10 +246,10 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
     uint32_t landed = 0;    // stages this thread has seen complete
     uint32_t released = 0;  // thread 0: stages handed back to the producer
     // chunk boundaries
-    const int chunk_lo = w ? 0 : *p.chunk_lo_ptr;
-    const int nchunk = w ? 0 : *p.chunk_hi_ptr - chunk_lo;
+    const int chunk_lo = w ? 0 : (CAND ? cd->loff[p.cand_t0] : *p.chunk_lo_ptr);
+    const int nchunk = w ? 0 : (CAND ? cd->loff[p.cand_t1] : *p.chunk_hi_ptr) - chunk_lo;
     const uint32_t* const cend = p.chunk_end + chunk_lo;
-    const uint32_t pos_base = p.pos_base;
+    const uint32_t pos_base = CAND ? cd->pos0 + p.pos_base : p.pos_base;
     int wbase = 0;
     uint32_t wcur = Q, wnxt = Q;  // table mode: chunk end of chunk wbase + lane, wbase + 32 + lane
     if (!w) {
@@ -538,7 +552,7 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
 
     if (!GCTR) {
         if (NT == 32) __syncwarp(); else __syncthreads();
-        for (uint32_t i = tid; i < (uint32_t)p.N * CW; i += NT) ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))] = ctr[i];
+        for (uint32_t i = tid; i < (uint32_t)(CAND ? (int)pin[8] : p.N) * CW; i += NT) ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))] = ctr[i];
     }
 }
 
@@ -546,10 +560,10 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
 // Emit (rows of <= 3 replicas): ordered record -> broker ids + list length + the slot-2 counters, one thread per schedule
 // position, fully parallel; keeps the id lookups and the 4 B/replica output stream off the serial chain.
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) ka_emit3_kernel(const uint4* __restrict__ rec, const uint16_t* __restrict__ perm,
-                                                       const int64_t* __restrict__ part_off, int T, int P,
-                                                       const int32_t* __restrict__ broker_id, uint32_t Q, int S, int32_t* __restrict__ out,
-                                                       int32_t* __restrict__ out_len, int32_t* __restrict__ ctr8) {
+__device__ __forceinline__ void ka_emit3(const uint4* __restrict__ rec, const uint16_t* __restrict__ perm,
+                                         const int64_t* __restrict__ part_off, int T, int P, const int32_t* __restrict__ broker_id,
+                                         uint32_t Q, int S, int32_t* __restrict__ out, int32_t* __restrict__ out_len,
+                                         int32_t* __restrict__ ctr8) {
     const uint32_t pos = blockIdx.x * blockDim.x + threadIdx.x;
     if (pos >= Q) return;
     const uint4 r = rec[pos];   // ordered by the slot chains: {o0, o1, o2, f}, o_r = broker index << 2
@@ -576,4 +590,23 @@ __global__ void __launch_bounds__(256) ka_emit3_kernel(const uint4* __restrict__
     if (out_len) out_len[row] = len;
     // counter[list[2]][2] += 1 (KAS:254-261): never compared by a row of <= 3 replicas, i.e. a plain commutative sum
     if (len > 2) atomicAdd(ctr8 + (size_t)(r.z >> 2) * KA_MAX_SLOTS + 2, 1);
+}
+
+__global__ void __launch_bounds__(256) ka_emit3_kernel(const uint4* __restrict__ rec, const uint16_t* __restrict__ perm,
+                                                       const int64_t* __restrict__ part_off, int T, int P,
+                                                       const int32_t* __restrict__ broker_id, uint32_t Q, int S, int32_t* __restrict__ out,
+                                                       int32_t* __restrict__ out_len, int32_t* __restrict__ ctr8) {
+    ka_emit3(rec, perm, part_off, T, P, broker_id, Q, S, out, out_len, ctr8);
+}
+
+// Batched solve: blockIdx.y = candidate k. Rows [r0, r0 + Q) of a dense sub-block of T topics; candidate k's rows are
+// out + k * cand_rows * S (out_len + k * cand_rows), its counters its own ctr8.
+__global__ void __launch_bounds__(256) ka_emit3_candidates_kernel(const KaCandidate* __restrict__ cand, uint32_t r0, int T, int P,
+                                                                  uint32_t Q, int S, int64_t cand_rows, int32_t* __restrict__ out,
+                                                                  int32_t* __restrict__ out_len) {
+    const KaCandidate& c = cand[blockIdx.y];
+    if (c.N <= 0) return;   // no broker: every topic failed in kernel A, its rows are unspecified
+    const int64_t row0 = (int64_t)blockIdx.y * cand_rows + r0;
+    ka_emit3(reinterpret_cast<const uint4*>(c.rec) + r0, c.perm ? c.perm + r0 : nullptr, nullptr, T, P, c.broker_id, Q, S,
+             out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8);
 }

@@ -35,6 +35,7 @@ struct KaSolveParams {
     uint32_t* lend;             // [Q] LEVELS: lend[g0 + i] = topic-relative end of the topic's i-th chunk (first ntl[t] entries)
     int4* tstatus;              // [T] per-topic error record (written only on error)
     unsigned* err_topic;        // unsigned atomicMin of the failing topic index (init = 0xFFFFFFFF)
+    const KaCandidate* cand;    // batched solve: candidate blockIdx.y's broker table, records, level tables and status
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -473,14 +474,12 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
     __syncwarp();
 }
 
+// One CTA of kernel A: stage p's broker table, then its topics, one per warp. warp_base: the per-warp scratch, behind the
+// largest blob of the launch.
 template <typename LoadT, bool LEVELS, int SM>
-__global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolveParams p, int load_bytes, int slab_bytes, int cnt_bytes,
-                                                               int lv_owner_bytes, int lv_last_bytes, int lv_p_bytes) {
-    extern __shared__ __align__(16) unsigned char ka_smem[];
-    uint64_t* bar = reinterpret_cast<uint64_t*>(ka_smem);
-    unsigned char* blob = ka_smem + 16;
-    unsigned char* warp_base = blob + p.blob_bytes;
-
+__device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uint64_t* bar, unsigned char* blob, unsigned char* warp_base,
+                                                     int load_bytes, int slab_bytes, int cnt_bytes, int lv_owner_bytes, int lv_last_bytes,
+                                                     int lv_p_bytes) {
     // TMA bulk-stage the broker table (rack indices + id->index LUT) once per CTA.
     if (threadIdx.x == 0) {
         ka_mbar_init(bar, 1);
@@ -517,4 +516,39 @@ __global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolvePara
     const int total_warps = gridDim.x * nwarp;
     for (int t = blockIdx.x * nwarp + warp; t < p.T; t += total_warps)
         ka_solve_topic<LoadT, LEVELS, SM>(p, tab, t, load, slab, cnt, ls);
+}
+
+// CAND: a batched solve over candidate broker tables, blockIdx.y = candidate. A CTA serves one candidate, so its broker
+// table is still staged once per CTA; p.blob_bytes is the largest blob of the launch (the shared-memory layout).
+template <typename LoadT, bool LEVELS, int SM, bool CAND = false>
+__global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolveParams p, int load_bytes, int slab_bytes, int cnt_bytes,
+                                                               int lv_owner_bytes, int lv_last_bytes, int lv_p_bytes) {
+    extern __shared__ __align__(16) unsigned char ka_smem[];
+    uint64_t* bar = reinterpret_cast<uint64_t*>(ka_smem);
+    unsigned char* blob = ka_smem + 16;
+    unsigned char* warp_base = blob + p.blob_bytes;
+    if constexpr (CAND) {
+        const KaCandidate& c = p.cand[blockIdx.y];
+        KaSolveParams q = p;
+        q.N = c.N;
+        q.blob = c.blob;
+        q.blob_bytes = c.blob_bytes;
+        q.lut_off = c.lut_off;
+        q.lut_mode = c.lut_mode;
+        q.min_id = c.min_id;
+        q.range = c.range;
+        q.glut = c.glut;
+        q.broker_id = c.broker_id;
+        q.rec = c.rec;
+        q.perm = c.perm;
+        q.ntl = c.ntl;
+        q.lend = c.lend;
+        q.tstatus = c.tstatus;
+        q.err_topic = c.err_topic;
+        ka_sticky_spread_cta<LoadT, LEVELS, SM>(q, bar, blob, warp_base, load_bytes, slab_bytes, cnt_bytes, lv_owner_bytes,
+                                                lv_last_bytes, lv_p_bytes);
+    } else {
+        ka_sticky_spread_cta<LoadT, LEVELS, SM>(p, bar, blob, warp_base, load_bytes, slab_bytes, cnt_bytes, lv_owner_bytes,
+                                                lv_last_bytes, lv_p_bytes);
+    }
 }

@@ -92,6 +92,30 @@ def rack_indices(broker_id, rack_name):
     return out
 
 
+def _live_brokers(N, R, remove_frac, rack_aware=True):
+    """make_cluster's live set: brokers 1000+i, rack i % R, minus the round(remove_frac*N/R) highest ordinals of every rack."""
+    ordinal = np.arange(N)
+    per_rack_remove = int(round(remove_frac * N / R))
+    rack_of = ordinal % R
+    rank_in_rack = ordinal // R
+    rack_sizes = np.bincount(rack_of, minlength=R)
+    live_mask = rank_in_rack < (rack_sizes[rack_of] - per_rack_remove)
+    live_ids = (1000 + ordinal[live_mask]).astype(np.int32)
+    return live_ids, ["r%02d" % (i % R) if rack_aware else None for i in ordinal[live_mask]]
+
+
+def decommission_tables(key, fracs, **over):
+    """The live broker tables (broker_id, rack_index) of make_config(key, remove_frac=f) for every f of fracs, without
+    generating the cluster: its current assignment does not depend on remove_frac. For one batched candidate solve."""
+    kw = dict(CONFIGS[key])
+    kw.update(over)
+    out = []
+    for f in fracs:
+        ids, names = _live_brokers(kw["N"], kw["R"], f, kw.get("rack_aware", True))
+        out.append((ids, rack_indices(ids, names)))
+    return out
+
+
 def make_cluster(T, P, RF, N, R, seed, kind="mixed", n_old=None, remove_frac=0.0, name=None,
                  rack_aware=True, topic_prefix="topic-", t_offset=0):
     """Expansion / decommission scenario of SURVEY §8d.
@@ -111,15 +135,7 @@ def make_cluster(T, P, RF, N, R, seed, kind="mixed", n_old=None, remove_frac=0.0
             n_old = N
     n_old = max(R, (n_old // R) * R)
     all_ids = (1000 + np.arange(N)).astype(np.int32)
-    ordinal = np.arange(N)
-    # decommission: drop the highest ordinals of every rack
-    per_rack_remove = int(round(remove_frac * N / R))
-    rack_of = ordinal % R
-    rank_in_rack = ordinal // R
-    rack_sizes = np.bincount(rack_of, minlength=R)
-    live_mask = rank_in_rack < (rack_sizes[rack_of] - per_rack_remove)
-    live_ids = all_ids[live_mask]
-    rack_names = ["r%02d" % (i % R) if rack_aware else None for i in ordinal[live_mask]]
+    live_ids, rack_names = _live_brokers(N, R, remove_frac, rack_aware)
 
     names = ["%s%06d" % (topic_prefix, t) for t in range(t_offset, t_offset + T)]
     th = java_string_hash_ascii(names)
