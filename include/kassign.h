@@ -161,6 +161,29 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* ctx, int32_t K, const int32_t* 
                                          int32_t RF, const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride,
                                          int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st);
 
+/* The general (ragged) problem of ka_solve, in HOST buffers, solved against K candidate broker tables, each on a FRESH
+ * Context: K runs of the reference tool over one real cluster, e.g. the broker sets of a decommission sweep.
+ *   cand_off, broker_id, broker_rack   the candidate tables, as ka_solve_dense_candidates_device takes them
+ *   T .. desired_rf    the inputs of ka_solve (part_id, NULL = 0..P-1, is only used for ka_status.partition)
+ *   out_broker[K][ΣP][out_stride], out_len[K][ΣP] (or NULL)   host; candidate k's rows and list lengths
+ *   st[K]              host, required; st[k] is candidate k's status
+ * Candidate k gives exactly what ka_ctx_create -> ka_ctx_set_brokers(table k) -> ka_solve(same inputs, out_stride) gives: the
+ * same rows, out_len and status fields (partition mapped through part_id). The rows of a failed candidate are unspecified; a
+ * failing candidate changes nothing of another. The problem's inputs are copied to the device once and shared by all
+ * candidates; the number of kernel launches does not depend on K.
+ * Limits, checked before anything is enqueued: K <= 128, out_stride <= 3 and K * ΣP < 2^31 (else KA_ERR_LIMIT); out_stride >=
+ * max(longest current list, desired_rf) (else KA_ERR_BAD_ARG), so that every accepted input is one ka_solve accepts for
+ * every table; every table as ka_ctx_set_brokers checks it and every offset array as ka_solve checks it (same status).
+ * K == 0 or T == 0: KA_OK, nothing written. Topics without partitions are solved (and may fail) as ka_solve solves them.
+ * Synchronous. Returns KA_OK when every candidate solved, else st[k].code of the lowest failing k; library-side failures are
+ * returned directly and written to every st[k]. Does not read or change ctx's own Context, broker table, parked counters,
+ * topic_base or staged block. */
+int32_t ka_solve_candidates(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                            const int32_t* broker_rack, int32_t T, const int32_t* topic_hash, const int64_t* part_off,
+                            const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker,
+                            int32_t desired_rf, int32_t out_stride, int32_t* out_len, int32_t* out_broker,
+                            ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

@@ -31,6 +31,7 @@ SYMBOLS = {
     "ka_solve_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp]),
     "ka_solve_dense_candidates_device": (_i32, [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp,
                                                 _vp]),
+    "ka_solve_candidates": (_i32, [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "ka_ctx_set_topic_base": (_i32, [_vp, _i32]),

@@ -253,13 +253,7 @@ class Solver:
         """ka_solve_dense_candidates_device: the dense device solve against every broker table of `tables` (a list of
         (broker_id, rack_index) numpy pairs), each on a fresh Context; this Solver's own Context is untouched. Candidate k's
         rows are d_out[k] ([K, T, P, out_stride] on the device). Synchronous; returns the K KaStatus."""
-        ids = [np.ascontiguousarray(b, dtype=np.int32) for b, _ in tables]
-        racks = [np.ascontiguousarray(r, dtype=np.int32) for _, r in tables]
-        assert all(len(b) == len(r) for b, r in zip(ids, racks))
-        cand_off = np.zeros(len(tables) + 1, dtype=np.int32)
-        np.cumsum([len(b) for b in ids], out=cand_off[1:])
-        broker_id = np.concatenate(ids) if ids else np.zeros(0, dtype=np.int32)
-        broker_rack = np.concatenate(racks) if racks else np.zeros(0, dtype=np.int32)
+        cand_off, broker_id, broker_rack = self._candidate_tables(tables)
         st = (KaStatus * max(len(tables), 1))()
         self._L.ka_solve_dense_candidates_device(self._h, len(tables), _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), int(T),
                                                  ctypes.c_void_p(d_topic_hash), int(P), int(RF), ctypes.c_void_p(d_cur),
@@ -267,6 +261,42 @@ class Solver:
                                                  ctypes.c_void_p(d_out_len) if d_out_len else None, ctypes.c_void_p(d_out),
                                                  ctypes.c_void_p(stream) if stream else None, st)
         return [st[k] for k in range(len(tables))]
+
+    @staticmethod
+    def _candidate_tables(tables):
+        """(cand_off, broker_id, broker_rack) of a list of (broker_id, rack_index) pairs: the candidate tables of the C ABI."""
+        ids = [np.ascontiguousarray(b, dtype=np.int32) for b, _ in tables]
+        racks = [np.ascontiguousarray(r, dtype=np.int32) for _, r in tables]
+        assert all(len(b) == len(r) for b, r in zip(ids, racks))
+        cand_off = np.zeros(len(tables) + 1, dtype=np.int32)
+        np.cumsum([len(b) for b in ids], out=cand_off[1:])
+        broker_id = np.concatenate(ids) if ids else np.zeros(0, dtype=np.int32)
+        broker_rack = np.concatenate(racks) if racks else np.zeros(0, dtype=np.int32)
+        return cand_off, broker_id, broker_rack
+
+    def solve_ragged_candidates(self, tables, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, out_stride=None):
+        """ka_solve_candidates: the ragged solve of solve_ragged against every broker table of `tables` (a list of
+        (broker_id, rack_index) numpy pairs), each on a fresh Context; this Solver's own Context is untouched. out_stride
+        defaults to max(longest current list, desired_rf, 1). Returns (out [K, ΣP, out_stride], out_len [K, ΣP], [KaStatus] * K);
+        the rows of a failed candidate are unspecified."""
+        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
+        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
+        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
+        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
+        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        if out_stride is None:
+            sizes = np.diff(rep_off)
+            out_stride = max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+        cand_off, broker_id, broker_rack = self._candidate_tables(tables)
+        K = len(tables)
+        Q = int(part_off[-1]) if len(part_off) else 0
+        out = np.full((K, Q, out_stride), -1, dtype=np.int32)
+        out_len = np.zeros((K, Q), dtype=np.int32)
+        st = (KaStatus * max(K, 1))()
+        self._L.ka_solve_candidates(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), len(th), _ptr(th),
+                                    _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker), int(desired_rf),
+                                    int(out_stride), _ptr(out_len), _ptr(out), st)
+        return out, out_len, [st[k] for k in range(K)]
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

@@ -1167,9 +1167,64 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     return finish(c, s, st, false);
 }
 
+// A library-side failure of a batched solve: every candidate reports it.
+static int fail_candidates(ka_status* st, int K, int rc) {
+    for (int k = 0; k < K; ++k) set_status(st + k, rc);
+    return rc;
+}
+
+// What ka_ctx_set_brokers refuses in any of the K candidate tables of a batched solve (the same code).
+static int check_candidates(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack) {
+    if (!cand_off || cand_off[0] != 0) return KA_ERR_BAD_ARG;
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        if (cand_off[k + 1] < cand_off[k] || (n > 0 && (!broker_id || !broker_rack))) return KA_ERR_BAD_ARG;
+        const int rc = n > 0 ? check_brokers(n, broker_id + cand_off[k], broker_rack + cand_off[k]) : KA_OK;
+        if (rc != KA_OK) return rc;
+    }
+    return KA_OK;
+}
+
+// The device images of the (checked) candidate tables; nmax / blob_max: the largest table and blob (the call's plan).
+static void candidate_tables(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                             std::vector<BrokerTable>& tabs, int& nmax, int& blob_max) {
+    tabs.resize(K);
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        tabs[k] = broker_table(n, broker_id + cand_off[k], broker_rack + cand_off[k]);
+        nmax = std::max(nmax, n);
+        blob_max = std::max(blob_max, (int)(tabs[k].blob.size() * 2));
+    }
+}
+
+// Wait for a batched solve enqueued on `s` and fill every candidate's status: its lowest failing topic, as finish_status
+// reports it for one solve (part_id / part_off of a ragged solve: the failing partition's id). Returns the code of the
+// lowest failing candidate.
+static int finish_candidates(ka_ctx* c, cudaStream_t s, int K, int T, ka_status* st, const int32_t* part_id = nullptr,
+                             const int64_t* part_off = nullptr) {
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail_candidates(st, K, KA_ERR_CUDA);
+    std::vector<unsigned> err(K);
+    if (cudaMemcpy(err.data(), c->d_cand_flags.p, (size_t)K * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return fail_candidates(st, K, KA_ERR_CUDA);
+    int first = KA_OK;
+    for (int k = 0; k < K; ++k) {
+        if (err[k] == 0xFFFFFFFFu) continue;
+        const int t = (int)err[k];
+        int4 ts;
+        if (cudaMemcpy(&ts, c->d_cand_tstatus.as<int4>() + (size_t)k * T + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
+            return fail_candidates(st, K, KA_ERR_CUDA);
+        const int part = ts.y >= 0 && part_id && part_off ? part_id[part_off[t] + ts.y] : ts.y;
+        set_status(st + k, ts.x, t, part, ts.z, ts.w);
+        if (first == KA_OK) first = ts.x;
+    }
+    return first;
+}
+
 // Everything of a batched solve over K candidate tables, enqueued on `s` (slot-0 chains on c->sb1): the candidates' tables
 // and descriptors H2D, fresh counters, kernel A with grid.y = candidate, the level tables of all candidates as one table,
-// then per chain sub-block the slot-0 / slot-1 chains (one CTA per candidate) and the emit (grid.y = candidate).
+// then per chain sub-block the slot-0 / slot-1 chains (one CTA per candidate) and the emit (grid.y = candidate). `d` is a
+// dense problem or a ragged one (d.d_part_off set: one chain sub-block, as in a ragged single solve); its inputs are shared by
+// every candidate.
 static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<BrokerTable>& tabs, const int32_t* cand_off,
                           const int32_t* broker_id, const StageDesc& d, int32_t* d_out_len, int32_t* d_out) {
     const Plan& pl = d.pl;
@@ -1248,9 +1303,14 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
     if (pl.a_levels) {
         ka_level_scan_kernel<<<1, 1024, 0, s>>>(c->d_cand_ntl.as<int32_t>(), (int)kt, c->d_cand_loff.as<int32_t>());
         KA_CUDA(cudaGetLastError());
-        ka_level_fill_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(c->d_cand_ntl.as<int32_t>(), c->d_cand_loff.as<int32_t>(),
-                                                                      c->d_cand_lend.as<uint32_t>(), nullptr, d.P, (int)kt,
-                                                                      c->d_cand_lvl_end.as<uint32_t>());
+        if (d.d_part_off)
+            ka_level_fill_candidates_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(
+                c->d_cand_ntl.as<int32_t>(), c->d_cand_loff.as<int32_t>(), c->d_cand_lend.as<uint32_t>(), d.d_part_off, T, (int)kt, Q,
+                c->d_cand_lvl_end.as<uint32_t>());
+        else
+            ka_level_fill_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(c->d_cand_ntl.as<int32_t>(), c->d_cand_loff.as<int32_t>(),
+                                                                          c->d_cand_lend.as<uint32_t>(), nullptr, d.P, (int)kt,
+                                                                          c->d_cand_lvl_end.as<uint32_t>());
         KA_CUDA(cudaGetLastError());
         c->launches += 2;
     }
@@ -1275,8 +1335,12 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
         KA_CUDA(cudaEventRecord(c->ev_b1[j], c->sb1));
         KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[j], 0));
         KA_CUDA((launch_order<1, 1024, true>(s, o, pl, K)));
-        ka_emit3_candidates_kernel<<<dim3((unsigned)((b.rq + 255) / 256), K), 256, 0, s>>>(cand, (uint32_t)b.r0, b.t1 - b.t0, d.P,
-                                                                                           (uint32_t)b.rq, S, Q, d_out, d_out_len);
+        const dim3 grid((unsigned)((b.rq + 255) / 256), K);
+        if (d.d_part_off)
+            ka_emit3_candidates_kernel<true><<<grid, 256, 0, s>>>(cand, 0u, T, 0, d.d_part_off, (uint32_t)b.rq, S, Q, d_out, d_out_len);
+        else
+            ka_emit3_candidates_kernel<<<grid, 256, 0, s>>>(cand, (uint32_t)b.r0, b.t1 - b.t0, d.P, nullptr, (uint32_t)b.rq, S, Q, d_out,
+                                                            d_out_len);
         KA_CUDA(cudaGetLastError());
         c->launches += 3;
     }
@@ -1289,37 +1353,26 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
                                          int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
     if (!st || K < 0) return KA_ERR_BAD_ARG;
     for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
-    auto all = [&](int rc) {   // a library-side failure: every candidate reports it
-        for (int k = 0; k < K; ++k) set_status(st + k, rc);
-        return rc;
-    };
+    auto all = [&](int rc) { return fail_candidates(st, K, rc); };
     if (!c) return all(KA_ERR_NO_DEVICE);
     if (K > KA_MAX_CANDIDATES || out_stride > 3) return all(KA_ERR_LIMIT);   // wider rows: the fused chain of the single solve
     if (T < 0 || P < 0 || RF < 0 || out_stride < 1 || out_stride < std::max(RF, desired_rf)) return all(KA_ERR_BAD_ARG);
     if (K == 0) return KA_OK;
-    if (!cand_off || cand_off[0] != 0) return all(KA_ERR_BAD_ARG);
-    for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        if (cand_off[k + 1] < cand_off[k] || (n > 0 && (!broker_id || !broker_rack))) return all(KA_ERR_BAD_ARG);
-        const int rc = n > 0 ? check_brokers(n, broker_id + cand_off[k], broker_rack + cand_off[k]) : KA_OK;
-        if (rc != KA_OK) return all(rc);
-    }
+    int rc = check_candidates(K, cand_off, broker_id, broker_rack);
+    if (rc != KA_OK) return all(rc);
     if (T == 0) return KA_OK;
     const int64_t Q = (int64_t)T * P;
     if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
     if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
-    int rc = enter(c, true);
-    if (rc != KA_OK) return all(rc);
+    if ((rc = enter(c, true)) != KA_OK) return all(rc);
     // the plan of the call: counter placement and loop shape from the largest table, levels if any candidate has capacity > 1
-    std::vector<BrokerTable> tabs(K);
+    std::vector<BrokerTable> tabs;
     int nmax = 0, blob_max = 0;
+    candidate_tables(K, cand_off, broker_id, broker_rack, tabs, nmax, blob_max);
     int64_t capmax = 0;
     const int rf_t = desired_rf >= 0 ? desired_rf : RF;
     for (int k = 0; k < K; ++k) {
         const int n = cand_off[k + 1] - cand_off[k];
-        tabs[k] = broker_table(n, broker_id + cand_off[k], broker_rack + cand_off[k]);
-        nmax = std::max(nmax, n);
-        blob_max = std::max(blob_max, (int)(tabs[k].blob.size() * 2));
         if (n > 0) capmax = std::max<int64_t>(capmax, ((int64_t)P * std::max(rf_t, 0) + n - 1) / n);
     }
     StageDesc d;
@@ -1343,21 +1396,7 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
         cudaStreamSynchronize(s);
         return all(rc);
     }
-    // per-candidate status: the lowest failing topic of each, as finish_status reports it for one solve
-    if (cudaStreamSynchronize(s) != cudaSuccess) return all(KA_ERR_CUDA);
-    std::vector<unsigned> err(K);
-    if (cudaMemcpy(err.data(), c->d_cand_flags.p, (size_t)K * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return all(KA_ERR_CUDA);
-    int first = KA_OK;
-    for (int k = 0; k < K; ++k) {
-        if (err[k] == 0xFFFFFFFFu) continue;
-        const int t = (int)err[k];
-        int4 ts;
-        if (cudaMemcpy(&ts, c->d_cand_tstatus.as<int4>() + (size_t)k * T + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
-            return all(KA_ERR_CUDA);
-        set_status(st + k, ts.x, t, ts.y, ts.z, ts.w);
-        if (first == KA_OK) first = ts.x;
-    }
-    return first;
+    return finish_candidates(c, s, K, T, st);
 }
 
 int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash, int32_t P, int32_t RF,
@@ -1555,18 +1594,22 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     return stream_json(c, s, io, json, json_cap, json_bytes, st);
 }
 
-// Validation and host-side sizing scan of a ragged solve (largest topic, largest current list, largest capacity,
-// KAS:65-71), then its device input buffers: the Shape run_solve takes. pick_stride: S is chosen here, as
-// max(longest current list, desired_rf, 1). have_out: the caller has somewhere to put the rows.
-static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
-                        const int32_t* cur_broker, int32_t desired_rf, int32_t S, bool pick_stride, bool have_out, Shape& sh,
-                        ka_status* st) {
-    set_status(st, KA_OK);
-    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
-    if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return set_status(st, KA_ERR_BAD_ARG);
-    if (!pick_stride && (S < 1 || S > KA_MAX_SLOTS)) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
-    int rc = enter(c, true);
-    if (rc != KA_OK) return failed(st, rc);
+// Host-side sizing scan of a ragged problem that does not depend on any broker table: offsets, list sizes, the largest
+// topic, and per target RF the largest topic of that RF (the capacity bound of KAS:65-71 for any table follows from those:
+// ragged_capmax). pick_stride: S is chosen here, as max(longest current list, desired_rf, 1). have_out: the caller has
+// somewhere to put the rows. Failures that come before the topic loop are returned; those of the topic and list-size
+// loops are kept in `err` (in the order ka_solve reports them), because a failure that depends on the table — a topic
+// whose target RF exceeds S but not N — takes precedence when it comes from an earlier topic.
+struct RaggedScan {
+    int64_t Q = 0, R = 0, maxsz = 0;
+    int S = 1, Pmax = 0;
+    int64_t pmax_rf[KA_MAX_SLOTS + 1] = {};   // [rf] partitions of the largest topic with target RF rf (rf <= S)
+    std::vector<std::pair<int, int64_t>> over;   // (t, target RF) of topics with target RF > S, each below every earlier one
+    ka_status err{KA_OK, -1, -1, 0, 0};
+};
+
+static int ragged_scan(int32_t T, const int64_t* part_off, const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf,
+                       int32_t S, bool pick_stride, bool have_out, RaggedScan& sc, ka_status* st) {
     const int64_t Q = T > 0 ? part_off[T] : 0;
     if (Q < 0 || (T > 0 && part_off[0] != 0) || (Q > 0 && (!rep_off || !have_out))) return set_status(st, KA_ERR_BAD_ARG);
     const int64_t R = Q > 0 ? rep_off[Q] : 0;
@@ -1577,30 +1620,66 @@ static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const i
         if (m > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(m, INT_MAX));
         S = (int)m;
     }
-    int Pmax = 0;
-    int64_t capmax = 0, maxsz = 0;
+    sc.Q = Q;
+    sc.R = R;
+    sc.S = S;
     for (int t = 0; t < T; ++t) {
         const int64_t a = part_off[t], b = part_off[t + 1];
-        if (b < a) return set_status(st, KA_ERR_BAD_ARG, t);
+        if (b < a) { set_status(&sc.err, KA_ERR_BAD_ARG, t); return KA_OK; }
         const int64_t Pn = b - a;
-        if (Pn > INT_MAX / 16) return set_status(st, KA_ERR_LIMIT, t, -1, (int)std::min<int64_t>(Pn, INT_MAX));
-        Pmax = std::max<int>(Pmax, (int)Pn);
+        if (Pn > INT_MAX / 16) { set_status(&sc.err, KA_ERR_LIMIT, t, -1, (int)std::min<int64_t>(Pn, INT_MAX)); return KA_OK; }
+        sc.Pmax = std::max<int>(sc.Pmax, (int)Pn);
         int64_t rf_t = desired_rf;
         if (rf_t < 0 && Pn > 0) rf_t = rep_off[a + 1] - rep_off[a];
-        if (rf_t > 0 && c->N > 0 && rf_t <= c->N) {
-            capmax = std::max<int64_t>(capmax, (Pn * rf_t + c->N - 1) / c->N);
-            if (rf_t > S) return set_status(st, KA_ERR_BAD_ARG, t, -1, S);
+        if (rf_t > S) {
+            if (sc.over.empty() || rf_t < sc.over.back().second) sc.over.emplace_back(t, rf_t);
+        } else if (rf_t > 0) {
+            sc.pmax_rf[rf_t] = std::max(sc.pmax_rf[rf_t], Pn);
         }
     }
     for (int64_t g = 0; g < Q; ++g) {
         const int64_t sz = rep_off[g + 1] - rep_off[g];
-        if (sz < 0) return set_status(st, KA_ERR_BAD_ARG);
-        maxsz = std::max(maxsz, sz);
+        if (sz < 0) { set_status(&sc.err, KA_ERR_BAD_ARG); return KA_OK; }
+        sc.maxsz = std::max(sc.maxsz, sz);
     }
-    if (maxsz > S) return set_status(st, KA_ERR_BAD_ARG, -1, -1, S);
-    if ((rc = reserve_io(c, T, Q, R, S, true)) != KA_OK) return failed(st, rc);
-    sh = Shape{T, 0, 0, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-               c->d_rep_off.as<int64_t>(), Q, R, Pmax, capmax};
+    if (sc.maxsz > S) set_status(&sc.err, KA_ERR_BAD_ARG, -1, -1, S);
+    return KA_OK;
+}
+
+// The largest capacity (KAS:65-71) of a scanned ragged problem under a table of N brokers — over the topics whose target RF
+// the table can serve — or the failure ka_solve reports for that table.
+static int ragged_capmax(const RaggedScan& sc, int N, int64_t& capmax, ka_status* st) {
+    capmax = 0;
+    if (N > 0)
+        for (const auto& o : sc.over)   // the first topic whose target RF is in (S, N]
+            if (o.second <= N) return set_status(st, KA_ERR_BAD_ARG, o.first, -1, sc.S);
+    if (sc.err.code != KA_OK) {
+        if (st) *st = sc.err;
+        return sc.err.code;
+    }
+    for (int rf = 1; rf <= std::min(sc.S, N); ++rf) capmax = std::max<int64_t>(capmax, (sc.pmax_rf[rf] * rf + N - 1) / N);
+    return KA_OK;
+}
+
+// Validation and sizing of a ragged solve against the ctx's broker table, then its device input buffers: the Shape
+// run_solve takes. pick_stride / have_out: as in ragged_scan.
+static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
+                        const int32_t* cur_broker, int32_t desired_rf, int32_t S, bool pick_stride, bool have_out, Shape& sh,
+                        ka_status* st) {
+    set_status(st, KA_OK);
+    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
+    if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return set_status(st, KA_ERR_BAD_ARG);
+    if (!pick_stride && (S < 1 || S > KA_MAX_SLOTS)) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
+    int rc = enter(c, true);
+    if (rc != KA_OK) return failed(st, rc);
+    RaggedScan sc;
+    int64_t capmax = 0;
+    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, S, pick_stride, have_out, sc, st)) != KA_OK ||
+        (rc = ragged_capmax(sc, c->N, capmax, st)) != KA_OK)
+        return rc;
+    if ((rc = reserve_io(c, T, sc.Q, sc.R, sc.S, true)) != KA_OK) return failed(st, rc);
+    sh = Shape{T, 0, 0, desired_rf, sc.S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
+               c->d_rep_off.as<int64_t>(), sc.Q, sc.R, sc.Pmax, capmax};
     return KA_OK;
 }
 
@@ -1654,6 +1733,86 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
     io.json = true;
     if ((rc = run_solve(c, s, sh, io, st)) != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
     return stream_json(c, s, io, json, json_cap, json_bytes, st, part_id, part_off);
+}
+
+int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                            int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                            const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride,
+                            int32_t* out_len, int32_t* out_broker, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
+    auto all = [&](int rc) { return fail_candidates(st, K, rc); };
+    if (!c) return all(KA_ERR_NO_DEVICE);
+    if (K > KA_MAX_CANDIDATES || out_stride > 3) return all(KA_ERR_LIMIT);   // wider rows: the fused chain of the single solve
+    if (T < 0 || (T > 0 && (!topic_hash || !part_off)) || out_stride < 1) return all(KA_ERR_BAD_ARG);
+    if (K == 0) return KA_OK;
+    int rc = check_candidates(K, cand_off, broker_id, broker_rack);
+    if (rc != KA_OK) return all(rc);
+    if (T == 0) return KA_OK;
+    // malformed offsets: every candidate reports what ka_solve reports for its table
+    RaggedScan sc;
+    ka_status sst{};
+    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, false, out_broker != nullptr, sc, &sst)) != KA_OK) {
+        for (int k = 0; k < K; ++k) st[k] = sst;
+        return rc;
+    }
+    if (sc.err.code != KA_OK) {
+        int64_t cap = 0;
+        for (int k = 0; k < K; ++k) ragged_capmax(sc, cand_off[k + 1] - cand_off[k], cap, st + k);
+        return st[0].code;
+    }
+    // the stride holds every current list and the desired RF: every candidate's ka_solve would accept the call's input
+    if (out_stride < std::max<int64_t>(sc.maxsz, desired_rf)) return all(KA_ERR_BAD_ARG);
+    const int64_t Q = sc.Q;
+    if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
+    if ((rc = enter(c, true)) != KA_OK) return all(rc);
+    // the plan of the call: counter placement and loop shape from the largest table, the largest capacity of any candidate
+    std::vector<BrokerTable> tabs;
+    int nmax = 0, blob_max = 0;
+    candidate_tables(K, cand_off, broker_id, broker_rack, tabs, nmax, blob_max);
+    int64_t capmax = 0;
+    for (int k = 0; k < K; ++k) {
+        int64_t cap = 0;
+        if ((rc = ragged_capmax(sc, cand_off[k + 1] - cand_off[k], cap, nullptr)) != KA_OK) return all(rc);
+        capmax = std::max(capmax, cap);
+    }
+    const size_t q = (size_t)std::max<int64_t>(Q, 1);
+    if ((rc = reserve_io(c, T, Q, sc.R, out_stride, true)) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
+        c->d_out_len.reserve((size_t)K * q * 4) != cudaSuccess)
+        return all(KA_ERR_CUDA);
+    StageDesc d;
+    d.T = T;
+    d.Q = Q;
+    d.d_hash = c->d_hash.as<int32_t>();
+    d.d_part_off = c->d_part_off.as<int64_t>();
+    d.d_rep_off = c->d_rep_off.as<int64_t>();
+    d.d_cur = c->d_cur.as<int32_t>();
+    d.desired_rf = desired_rf;
+    d.S = out_stride;
+    d.Pmax = sc.Pmax;
+    d.capmax = capmax;
+    if ((rc = make_plan(nmax, blob_max, Q, out_stride, sc.Pmax, capmax, true, d.pl, st)) != KA_OK) {
+        for (int k = 1; k < K; ++k) st[k] = st[0];
+        return rc;
+    }
+    // the inputs go up once and are shared by every candidate; the rows of all candidates come back in one copy
+    SolveCall io;
+    io.h_hash = topic_hash;
+    io.h_part_off = part_off;
+    io.h_rep_off = rep_off;
+    io.h_cur = cur_broker;
+    io.d_out = c->d_out.as<int32_t>();
+    io.d_out_len = c->d_out_len.as<int32_t>();
+    io.h_out = out_broker;
+    io.h_out_len = out_len;
+    cudaStream_t s = c->stream;
+    if ((rc = enq_inputs(s, io, d, sc.R)) != KA_OK || (rc = enq_candidates(c, s, K, tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK ||
+        (Q > 0 && (rc = enq_copy_out(s, io, out_stride, 0, (int64_t)K * Q)) != KA_OK)) {
+        cudaStreamSynchronize(c->sb1);
+        cudaStreamSynchronize(s);
+        return all(rc);
+    }
+    return finish_candidates(c, s, K, T, st, part_id, part_off);
 }
 
 }  // extern "C"

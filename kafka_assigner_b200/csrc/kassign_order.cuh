@@ -65,6 +65,21 @@ __global__ void __launch_bounds__(256) ka_level_fill_kernel(const int32_t* __res
     for (int l = lane; l < d; l += 32) lvl_end[o + l] = (uint32_t)g0 + lend[g0 + l];
 }
 
+// The call-wide chunk table of a ragged batched solve: K candidates x T topics, topic u = k * T + t starts at record
+// k * Q + part_off[t] (Q = rows of one candidate). The dense batch uses ka_level_fill_kernel, where that is u * P.
+__global__ void __launch_bounds__(256) ka_level_fill_candidates_kernel(const int32_t* __restrict__ ntl, const int32_t* __restrict__ loff,
+                                                                       const uint32_t* __restrict__ lend,
+                                                                       const int64_t* __restrict__ part_off, int T, int KT, int64_t Q,
+                                                                       uint32_t* __restrict__ lvl_end) {
+    const int lane = threadIdx.x & 31;
+    const int u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (u >= KT) return;
+    const int k = u / T, t = u - k * T;
+    const int64_t g0 = (int64_t)k * Q + part_off[t];
+    const int d = ntl[u], o = loff[u];
+    for (int l = lane; l < d; l += 32) lvl_end[o + l] = (uint32_t)g0 + lend[g0 + l];
+}
+
 // ------------------------------------------------------------------------------------------------
 struct KaOrderParams {
     uint32_t Q;                 // records (partitions) of the block
@@ -599,14 +614,17 @@ __global__ void __launch_bounds__(256) ka_emit3_kernel(const uint4* __restrict__
     ka_emit3(rec, perm, part_off, T, P, broker_id, Q, S, out, out_len, ctr8);
 }
 
-// Batched solve: blockIdx.y = candidate k. Rows [r0, r0 + Q) of a dense sub-block of T topics; candidate k's rows are
-// out + k * cand_rows * S (out_len + k * cand_rows), its counters its own ctr8.
+// Batched solve: blockIdx.y = candidate k. Rows [r0, r0 + Q) of a sub-block of T topics; candidate k's rows are
+// out + k * cand_rows * S (out_len + k * cand_rows), its counters its own ctr8. RAGGED: the whole problem (r0 == 0), each
+// schedule position's topic found in part_off[T+1] as ka_emit3_kernel finds it; else dense, P partitions per topic.
+template <bool RAGGED = false>
 __global__ void __launch_bounds__(256) ka_emit3_candidates_kernel(const KaCandidate* __restrict__ cand, uint32_t r0, int T, int P,
-                                                                  uint32_t Q, int S, int64_t cand_rows, int32_t* __restrict__ out,
+                                                                  const int64_t* __restrict__ part_off, uint32_t Q, int S,
+                                                                  int64_t cand_rows, int32_t* __restrict__ out,
                                                                   int32_t* __restrict__ out_len) {
     const KaCandidate& c = cand[blockIdx.y];
     if (c.N <= 0) return;   // no broker: every topic failed in kernel A, its rows are unspecified
     const int64_t row0 = (int64_t)blockIdx.y * cand_rows + r0;
-    ka_emit3(reinterpret_cast<const uint4*>(c.rec) + r0, c.perm ? c.perm + r0 : nullptr, nullptr, T, P, c.broker_id, Q, S,
-             out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8);
+    ka_emit3(reinterpret_cast<const uint4*>(c.rec) + r0, c.perm ? c.perm + r0 : nullptr, RAGGED ? part_off : nullptr, T, P,
+             c.broker_id, Q, S, out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8);
 }

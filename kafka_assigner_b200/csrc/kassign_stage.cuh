@@ -519,7 +519,9 @@ __device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uin
 }
 
 // CAND: a batched solve over candidate broker tables, blockIdx.y = candidate. A CTA serves one candidate, so its broker
-// table is still staged once per CTA; p.blob_bytes is the largest blob of the launch (the shared-memory layout).
+// table is still staged once per CTA; p.blob_bytes is the largest blob of the launch (the shared-memory layout). Dense or
+// ragged (p.part_off): the candidate's slices (records, perm, lend, ntl, status) take the same rows and topics as a single
+// solve's buffers.
 template <typename LoadT, bool LEVELS, int SM, bool CAND = false>
 __global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolveParams p, int load_bytes, int slab_bytes, int cnt_bytes,
                                                                int lv_owner_bytes, int lv_last_bytes, int lv_p_bytes) {

@@ -6,6 +6,8 @@
 //   kassign::solveTopics                              <->  the per-topic loop with ONE shared assigner
 //                                                          (reference KafkaAssignmentGenerator.java:172-184)
 //   kassign::solveTopicsJson                          <->  that loop + its org.json text, built on the device (KAG:172-186)
+//   kassign::solveTopicsCandidates                    <->  that loop once per candidate broker set, each with a new
+//                                                          assigner, in one device call (a decommission sweep)
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -97,12 +99,45 @@ public:
         ka_solve(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
                  f.stride, outLen.data(), out.data(), &st);
         throwForStatus(st, f.names);
-        std::vector<TopicOutput> res(T);
-        for (int t = 0; t < T; ++t) {
-            res[t].name = f.names[t];
-            for (int64_t g = f.partOff[t]; g < f.partOff[t + 1]; ++g)
-                res[t].assignment[f.partId[g]] =
-                    std::vector<int>(out.begin() + g * f.stride, out.begin() + g * f.stride + outLen[g]);
+        return unflatten(f, out.data(), outLen.data());
+    }
+
+    // One candidate broker set of a batched run: the `brokers` and `rackAssignment` of generateAssignment.
+    struct Candidate {
+        std::set<int> brokers;
+        std::map<int, std::string> rackAssignment;
+    };
+    // What one candidate's run gave: its status (re-throw with throwForStatus) and, when that is KA_OK, the new assignment.
+    struct CandidateResult {
+        ka_status status;
+        std::vector<TopicOutput> topics;
+    };
+
+    // The KAG:172-184 loop once per candidate broker set, each on a fresh Context (one new assigner per run), in ONE device
+    // call (ka_solve_candidates): candidate k equals solveTopics(topics, brokers k, racks k) on a new KafkaTopicAssigner,
+    // with the exception it would throw as its status. This instance's own Context is left alone. Rows of at most 3 replicas.
+    std::vector<CandidateResult> solveTopicsCandidates(const std::vector<TopicInput>& topics, const std::vector<Candidate>& candidates,
+                                                       int desiredReplicationFactor) {
+        const Flat f = flatten(topics, desiredReplicationFactor);
+        const int K = (int)candidates.size(), T = (int)topics.size();
+        std::vector<int32_t> candOff(K + 1, 0), ids, racks;
+        for (int k = 0; k < K; ++k) {
+            std::vector<int32_t> id(candidates[k].brokers.begin(), candidates[k].brokers.end()), rackIdx;
+            const int rc = rackIndices(id, candidates[k].rackAssignment, rackIdx);
+            if (rc != KA_OK) throw KassignError(rc, "ka_rack_indices");
+            ids.insert(ids.end(), id.begin(), id.end());
+            racks.insert(racks.end(), rackIdx.begin(), rackIdx.end());
+            candOff[k + 1] = (int32_t)ids.size();
+        }
+        const size_t Q = f.partId.size();
+        std::vector<int32_t> outLen((size_t)K * Q, 0), out((size_t)K * Q * f.stride, -1);
+        std::vector<ka_status> st(std::max(K, 1));
+        ka_solve_candidates(ctx_, K, candOff.data(), ids.data(), racks.data(), T, f.hash.data(), f.partOff.data(), f.partId.data(),
+                            f.repOff.data(), f.cur.data(), desiredReplicationFactor, f.stride, outLen.data(), out.data(), st.data());
+        std::vector<CandidateResult> res(K);
+        for (int k = 0; k < K; ++k) {
+            res[k].status = st[k];
+            if (st[k].code == KA_OK) res[k].topics = unflatten(f, out.data() + (size_t)k * Q * f.stride, outLen.data() + (size_t)k * Q);
         }
         return res;
     }
@@ -145,16 +180,32 @@ private:
         f.stride = std::max(1, std::max(maxLen, std::max(desiredReplicationFactor, 0)));
         return f;
     }
-    void setBrokers(const std::set<int>& brokers, const std::map<int, std::string>& racks) {
-        std::vector<int32_t> ids(brokers.begin(), brokers.end());  // std::set: ascending == TreeMap order (KAS:78)
-        if (ids == ids_ && racks == racks_) return;
+    // Rows of the flat layout (out[ΣP][stride], outLen[ΣP]) -> per-topic assignments.
+    static std::vector<TopicOutput> unflatten(const Flat& f, const int32_t* out, const int32_t* outLen) {
+        const int T = (int)f.names.size();
+        std::vector<TopicOutput> res(T);
+        for (int t = 0; t < T; ++t) {
+            res[t].name = f.names[t];
+            for (int64_t g = f.partOff[t]; g < f.partOff[t + 1]; ++g)
+                res[t].assignment[f.partId[g]] = std::vector<int>(out + g * f.stride, out + g * f.stride + outLen[g]);
+        }
+        return res;
+    }
+    // Rack index of every broker of `ids` (ascending) from the rack strings (ka_rack_indices, KAS:81-94).
+    static int rackIndices(const std::vector<int32_t>& ids, const std::map<int, std::string>& racks, std::vector<int32_t>& rackIdx) {
         std::vector<const char*> names(ids.size(), nullptr);
         for (size_t i = 0; i < ids.size(); ++i) {
             auto it = racks.find(ids[i]);
             if (it != racks.end()) names[i] = it->second.c_str();
         }
-        std::vector<int32_t> rackIdx(ids.size());
-        int rc = ka_rack_indices((int32_t)ids.size(), ids.data(), names.data(), rackIdx.data());
+        rackIdx.assign(ids.size(), 0);
+        return ka_rack_indices((int32_t)ids.size(), ids.data(), names.data(), rackIdx.data());
+    }
+    void setBrokers(const std::set<int>& brokers, const std::map<int, std::string>& racks) {
+        std::vector<int32_t> ids(brokers.begin(), brokers.end());  // std::set: ascending == TreeMap order (KAS:78)
+        if (ids == ids_ && racks == racks_) return;
+        std::vector<int32_t> rackIdx;
+        int rc = rackIndices(ids, racks, rackIdx);
         if (rc == KA_OK) rc = ka_ctx_set_brokers(ctx_, (int32_t)ids.size(), ids.data(), rackIdx.data());
         if (rc != KA_OK) throw KassignError(rc, "ka_ctx_set_brokers");
         ids_ = ids;

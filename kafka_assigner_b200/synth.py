@@ -219,6 +219,26 @@ class RaggedCluster:
         return out
 
 
+def _ragged_live(all_ids, all_racks, seed, remove_frac):
+    """make_ragged_cluster's live set: round(remove_frac * N) brokers drawn at random (seeded) leave; (ids, rack names)."""
+    N = len(all_ids)
+    removed = np.argsort(splitmix64(seed + 5, np.arange(N, dtype=np.uint64)))[:int(round(remove_frac * N))]
+    live = np.ones(N, dtype=bool)
+    live[removed] = False
+    return all_ids[live], [all_racks[i] for i in range(N) if live[i]]
+
+
+def ragged_decommission_tables(cluster, fracs):
+    """The live broker tables (broker_id, rack_index) that make_ragged_cluster(..., remove_frac=f) with cluster's other
+    arguments would produce, for every f of fracs, without regenerating the cluster (its lists do not depend on remove_frac).
+    For one batched candidate solve."""
+    out = []
+    for f in fracs:
+        ids, racks = _ragged_live(cluster.all_broker_id, cluster.all_rack_name, cluster.meta["seed"], f)
+        out.append((ids, rack_indices(ids, racks)))
+    return out
+
+
 def make_ragged_cluster(T, N=800, R=10, seed=0, max_partitions=256, tail=1.1, rf_weights=(0.15, 0.25, 0.6),
                         rack_frac=0.8, new_frac=0.1, remove_frac=0.0, desired_rf=-1, topic_prefix="svc."):
     """A seeded, deterministic real-cluster shape.
@@ -254,12 +274,7 @@ def make_ragged_cluster(T, N=800, R=10, seed=0, max_partitions=256, tail=1.1, rf
     bi = np.arange(N, dtype=np.uint64)
     has_rack = (splitmix64(seed + 4, bi) >> np.uint64(11)).astype(np.float64) / float(1 << 53) < rack_frac
     all_racks = ["r%02d" % (i % R) if has_rack[i] else None for i in range(N)]
-    n_remove = int(round(remove_frac * N))
-    removed = np.argsort(splitmix64(seed + 5, bi))[:n_remove]
-    live = np.ones(N, dtype=bool)
-    live[removed] = False
-    live_ids = all_ids[live]
-    live_racks = [all_racks[i] for i in range(N) if live[i]]
+    live_ids, live_racks = _ragged_live(all_ids, all_racks, seed, remove_frac)
     names = ["%s%05d" % (topic_prefix, t) for t in range(T)]
     th = java_string_hash_ascii(names)
     assert not np.any(th == np.int32(-2**31)), "synthetic topic name hashes to Integer.MIN_VALUE"
