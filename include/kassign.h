@@ -184,6 +184,42 @@ int32_t ka_solve_candidates(ka_ctx* ctx, int32_t K, const int32_t* cand_off, con
                             int32_t desired_rf, int32_t out_stride, int32_t* out_len, int32_t* out_broker,
                             ka_status* st);
 
+/* What a candidate's rows change against the current lists, and how they spread over its brokers. Every field is int64, so
+ * the layout has no padding. Position counts: a duplicate id in a current list, or a current broker the table lacks, needs
+ * no special case. w[g] is the weight of row g (1 without weights); the rows_* and leaders_changed fields count rows. */
+typedef struct ka_move_summary {
+    int64_t rows_changed;       /* rows whose new list differs from the current one (length or any position) */
+    int64_t rows_moved;         /* rows with at least one added or dropped replica */
+    int64_t leaders_changed;    /* rows whose current list is empty or whose first broker changed */
+    int64_t replicas_added;     /* sum of w[g] x (positions of the new list whose broker is not in the current list) */
+    int64_t replicas_dropped;   /* sum of w[g] x (positions of the current list whose broker is not in the new list) */
+    int64_t max_broker_in;      /* largest per-broker sum of added replicas (the receiving bottleneck) ... */
+    int64_t max_broker_in_id;   /* ... and that broker's id (lowest id on ties; -1 when no broker receives anything) */
+    int64_t max_broker_replicas, min_broker_replicas;   /* sum of w over the replicas each live broker holds after the move */
+    int64_t max_broker_leaders, min_broker_leaders;     /* sum of w over the rows each live broker leads after the move */
+} ka_move_summary;
+
+/* ka_solve_candidates, scored on the device: a few numbers per candidate instead of K copies of the rows, to choose between
+ * the broker sets of a sweep.
+ *   K .. out_stride     exactly as ka_solve_candidates takes them
+ *   part_weight[ΣP]     host, >= 0 per row (e.g. the partition's size in bytes), or NULL = 1 per row
+ *   summary[K]          host, required; summary[k] is a function of candidate k's rows and the current lists only
+ *   broker_replicas, broker_leaders, broker_in   host [cand_off[K]] each, or NULL: entry cand_off[k] + i belongs to broker
+ *                       broker_id[cand_off[k] + i] (replicas held, rows led and replicas added, each weighted)
+ *   out_len, out_broker as ka_solve_candidates takes them, or out_broker == NULL: the rows stay on the device
+ *   st[K]               host, required
+ * st[k], the return code and (when out_broker is given) the rows are exactly what ka_solve_candidates gives for the same inputs.
+ * A failed candidate, and every candidate when T == 0, gets a zero summary with max_broker_in_id = -1 and zero per-broker
+ * entries. Checked after every check of ka_solve_candidates and before anything is enqueued: a negative weight gives
+ * KA_ERR_BAD_ARG, 3 x (sum of weights) > INT64_MAX gives KA_ERR_LIMIT. Adds a fixed number of kernel launches, independent
+ * of K. Synchronous. Does not read or change ctx's own Context, broker table, parked counters, topic_base or staged block. */
+int32_t ka_score_candidates(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                            const int32_t* broker_rack, int32_t T, const int32_t* topic_hash, const int64_t* part_off,
+                            const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf,
+                            int32_t out_stride, const int64_t* part_weight, ka_move_summary* summary,
+                            int64_t* broker_replicas, int64_t* broker_leaders, int64_t* broker_in,
+                            int32_t* out_len, int32_t* out_broker, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

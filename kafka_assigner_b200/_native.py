@@ -11,6 +11,13 @@ class KaStatus(ctypes.Structure):
                 ("a", ctypes.c_int32), ("b", ctypes.c_int32)]
 
 
+class KaMoveSummary(ctypes.Structure):
+    """ka_move_summary: what a candidate's rows change against the current lists (every field int64, no padding)."""
+    _fields_ = [(n, ctypes.c_int64) for n in (
+        "rows_changed", "rows_moved", "leaders_changed", "replicas_added", "replicas_dropped", "max_broker_in", "max_broker_in_id",
+        "max_broker_replicas", "min_broker_replicas", "max_broker_leaders", "min_broker_leaders")]
+
+
 KA_OK = 0
 KA_ERR_RF_MISMATCH, KA_ERR_RF_NOT_POSITIVE, KA_ERR_RF_GT_BROKERS, KA_ERR_UNASSIGNABLE, KA_ERR_HASH_INDEX = 1, 2, 3, 4, 5
 KA_ERR_BAD_ARG, KA_ERR_CUDA, KA_ERR_NO_DEVICE, KA_ERR_LIMIT = -1, -2, -3, -4
@@ -32,6 +39,8 @@ SYMBOLS = {
     "ka_solve_dense_candidates_device": (_i32, [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp,
                                                 _vp]),
     "ka_solve_candidates": (_i32, [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
+    "ka_score_candidates": (_i32, [_vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                   _vp, _vp, _vp]),
     "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "ka_ctx_set_topic_base": (_i32, [_vp, _i32]),

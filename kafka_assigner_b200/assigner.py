@@ -14,7 +14,10 @@ import ctypes
 import numpy as np
 
 from . import _native
-from ._native import KaStatus
+from ._native import KaMoveSummary, KaStatus
+
+# numpy view of ka_move_summary (KaMoveSummary): one record per candidate
+MOVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaMoveSummary._fields_])
 
 
 class IllegalStateException(Exception):
@@ -297,6 +300,40 @@ class Solver:
                                     _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker), int(desired_rf),
                                     int(out_stride), _ptr(out_len), _ptr(out), st)
         return out, out_len, [st[k] for k in range(K)]
+
+    def score_ragged_candidates(self, tables, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, out_stride=None,
+                                weight=None, rows=False, per_broker=False):
+        """ka_score_candidates: solve_ragged_candidates scored on the device. weight: [ΣP] int64 per row (e.g. partition bytes),
+        None = 1 per row. Returns (summary, [KaStatus] * K), summary a numpy structured array [K] with the fields of
+        ka_move_summary; then, with rows=True, (out [K, ΣP, out_stride], out_len [K, ΣP]) as solve_ragged_candidates returns
+        them; then, with per_broker=True, (replicas, leaders, added): one int64 array per table, aligned with its broker ids."""
+        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
+        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
+        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
+        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
+        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
+        if out_stride is None:
+            sizes = np.diff(rep_off)
+            out_stride = max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+        cand_off, broker_id, broker_rack = self._candidate_tables(tables)
+        K = len(tables)
+        Q = int(part_off[-1]) if len(part_off) else 0
+        summary = np.zeros(K, dtype=MOVE_SUMMARY_DTYPE)
+        out = np.full((K, Q, out_stride), -1, dtype=np.int32) if rows else None
+        out_len = np.zeros((K, Q), dtype=np.int32) if rows else None
+        brk = [np.zeros(int(cand_off[-1]), dtype=np.int64) for _ in range(3)] if per_broker else [None] * 3
+        st = (KaStatus * max(K, 1))()
+        self._L.ka_score_candidates(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), len(th), _ptr(th),
+                                    _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker), int(desired_rf),
+                                    int(out_stride), _ptr(weight), _ptr(summary), *[_ptr(a) for a in brk], _ptr(out_len),
+                                    _ptr(out), st)
+        res = (summary, [st[k] for k in range(K)])
+        if rows:
+            res += (out, out_len)
+        if per_broker:
+            res += tuple([a[cand_off[k]:cand_off[k + 1]] for k in range(K)] for a in brk)
+        return res
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

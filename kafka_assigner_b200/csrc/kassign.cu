@@ -5,6 +5,7 @@
 #include "kassign_stage.cuh"
 #include "kassign_order.cuh"
 #include "kassign_json.cuh"
+#include "kassign_score.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -123,6 +124,8 @@ struct ka_ctx {
     // records, level tables, status
     DevBuf d_cand_tab, d_cand_ctr, d_cand_rec, d_cand_perm, d_cand_ntl, d_cand_lend, d_cand_loff, d_cand_lvl_end, d_cand_tstatus,
         d_cand_flags;
+    // scratch of ka_score_candidates: row weights, the K summaries, the per-broker sums [3][ΣN], the tables' offsets [K+1]
+    DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -1025,7 +1028,8 @@ void ka_ctx_destroy(ka_ctx* c) {
                       &c->d_out, &c->d_out_len, &c->d_tstatus, &c->d_flags, &c->d_rec, &c->d_perm, &c->d_ntl, &c->d_loff, &c->d_lend,
                       &c->d_lvl_end, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen, &c->d_json_blocksum,
                       &c->d_json_state, &c->d_cand_tab, &c->d_cand_ctr, &c->d_cand_rec, &c->d_cand_perm, &c->d_cand_ntl,
-                      &c->d_cand_lend, &c->d_cand_loff, &c->d_cand_lvl_end, &c->d_cand_tstatus, &c->d_cand_flags})
+                      &c->d_cand_lend, &c->d_cand_loff, &c->d_cand_lvl_end, &c->d_cand_tstatus, &c->d_cand_flags, &c->d_score_w,
+                      &c->d_score_sum, &c->d_score_brk, &c->d_score_off})
         b->release();
     for_each_event(c, [](cudaEvent_t& e, bool) {
         if (e) cudaEventDestroy(e);
@@ -1735,11 +1739,22 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
     return stream_json(c, s, io, json, json_cap, json_bytes, st, part_id, part_off);
 }
 
-int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
-                            int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
-                            const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride,
-                            int32_t* out_len, int32_t* out_broker, ka_status* st) {
-    if (!st || K < 0) return KA_ERR_BAD_ARG;
+// One ragged batched solve as ka_solve_candidates runs it, up to and including the emit, enqueued on c->stream.
+struct CandidateRun {
+    bool tables_ok = false;   // the candidate tables passed their checks (cand_off may be read)
+    bool enqueued = false;    // false: an error (returned, every st[k] set) or nothing to solve (K == 0 or T == 0)
+    int64_t Q = 0;
+    SolveCall io;             // d_out / d_out_len: the rows of all candidates, [K][Q] on the device
+};
+
+// The checks, the sizing scan and plan, the inputs H2D and the batched solve of ka_solve_candidates, for both entry points.
+// have_out: the caller has somewhere to put the rows. part_weight: ka_score_candidates' weights, checked once every check of
+// ka_solve_candidates has passed and before anything is enqueued (negative: KA_ERR_BAD_ARG; 3 x their sum beyond INT64_MAX:
+// KA_ERR_LIMIT).
+static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                                 int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
+                                 const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride, bool have_out,
+                                 const int64_t* part_weight, CandidateRun& run, ka_status* st) {
     for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
     auto all = [&](int rc) { return fail_candidates(st, K, rc); };
     if (!c) return all(KA_ERR_NO_DEVICE);
@@ -1748,11 +1763,12 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     if (K == 0) return KA_OK;
     int rc = check_candidates(K, cand_off, broker_id, broker_rack);
     if (rc != KA_OK) return all(rc);
+    run.tables_ok = true;
     if (T == 0) return KA_OK;
     // malformed offsets: every candidate reports what ka_solve reports for its table
     RaggedScan sc;
     ka_status sst{};
-    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, false, out_broker != nullptr, sc, &sst)) != KA_OK) {
+    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, false, have_out, sc, &sst)) != KA_OK) {
         for (int k = 0; k < K; ++k) st[k] = sst;
         return rc;
     }
@@ -1795,22 +1811,121 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
         for (int k = 1; k < K; ++k) st[k] = st[0];
         return rc;
     }
-    // the inputs go up once and are shared by every candidate; the rows of all candidates come back in one copy
-    SolveCall io;
+    if (part_weight) {
+        bool negative = false;
+        int64_t sum = 0;   // saturates above INT64_MAX / 3
+        for (int64_t g = 0; g < Q; ++g) {
+            const int64_t w = part_weight[g];
+            negative |= w < 0;
+            sum = w > INT64_MAX / 3 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
+        }
+        if (negative) return all(KA_ERR_BAD_ARG);
+        if (sum > INT64_MAX / 3) return all(KA_ERR_LIMIT);
+    }
+    // the inputs go up once and are shared by every candidate
+    SolveCall& io = run.io;
     io.h_hash = topic_hash;
     io.h_part_off = part_off;
     io.h_rep_off = rep_off;
     io.h_cur = cur_broker;
     io.d_out = c->d_out.as<int32_t>();
     io.d_out_len = c->d_out_len.as<int32_t>();
-    io.h_out = out_broker;
-    io.h_out_len = out_len;
+    run.Q = Q;
+    run.enqueued = true;
+    if ((rc = enq_inputs(c->stream, io, d, sc.R)) != KA_OK ||
+        (rc = enq_candidates(c, c->stream, K, tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK) {
+        run.enqueued = false;
+        cudaStreamSynchronize(c->sb1);
+        cudaStreamSynchronize(c->stream);
+        return all(rc);
+    }
+    return KA_OK;
+}
+
+// The summary of a candidate that has none: failed, or T == 0.
+static ka_move_summary empty_summary() {
+    ka_move_summary e{};
+    e.max_broker_in_id = -1;
+    return e;
+}
+
+int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                            int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                            const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride,
+                            int32_t* out_len, int32_t* out_broker, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    CandidateRun run;
+    int rc = enq_ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, topic_hash, part_off, rep_off, cur_broker, desired_rf,
+                                   out_stride, out_broker != nullptr, nullptr, run, st);
+    if (!run.enqueued) return rc;
+    // the rows of all candidates come back in one copy
+    run.io.h_out = out_broker;
+    run.io.h_out_len = out_len;
+    if (run.Q > 0 && (rc = enq_copy_out(c->stream, run.io, out_stride, 0, (int64_t)K * run.Q)) != KA_OK) {
+        cudaStreamSynchronize(c->sb1);
+        cudaStreamSynchronize(c->stream);
+        return fail_candidates(st, K, rc);
+    }
+    return finish_candidates(c, c->stream, K, T, st, part_id, part_off);
+}
+
+int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                            int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                            const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride,
+                            const int64_t* part_weight, ka_move_summary* summary, int64_t* broker_replicas,
+                            int64_t* broker_leaders, int64_t* broker_in, int32_t* out_len, int32_t* out_broker, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    if (!summary) return fail_candidates(st, K, KA_ERR_BAD_ARG);
+    for (int k = 0; k < K; ++k) summary[k] = empty_summary();
+    CandidateRun run;
+    int rc = enq_ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, topic_hash, part_off, rep_off, cur_broker, desired_rf,
+                                   out_stride, true, part_weight, run, st);
+    int64_t* const brk[3] = {broker_replicas, broker_leaders, broker_in};
+    const size_t nb = run.tables_ok ? (size_t)cand_off[K] : 0;
+    if (!run.enqueued) {
+        for (int64_t* a : brk)
+            if (a && nb > 0) std::memset(a, 0, nb * 8);
+        return rc;
+    }
     cudaStream_t s = c->stream;
-    if ((rc = enq_inputs(s, io, d, sc.R)) != KA_OK || (rc = enq_candidates(c, s, K, tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK ||
-        (Q > 0 && (rc = enq_copy_out(s, io, out_stride, 0, (int64_t)K * Q)) != KA_OK)) {
+    const int64_t Q = run.Q;
+    auto fail = [&](int code) {
         cudaStreamSynchronize(c->sb1);
         cudaStreamSynchronize(s);
-        return all(rc);
+        for (int k = 0; k < K; ++k) summary[k] = empty_summary();
+        for (int64_t* a : brk)
+            if (a && nb > 0) std::memset(a, 0, nb * 8);
+        return fail_candidates(st, K, code);
+    };
+    const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
+    if (c->d_score_sum.reserve(sum_bytes) != cudaSuccess || c->d_score_brk.reserve(std::max<size_t>(3 * nb, 1) * 8) != cudaSuccess ||
+        c->d_score_off.reserve((size_t)(K + 1) * 4) != cudaSuccess ||
+        (part_weight && c->d_score_w.reserve((size_t)std::max<int64_t>(Q, 1) * 8) != cudaSuccess))
+        return fail(KA_ERR_CUDA);
+    ka_move_summary* d_sum = c->d_score_sum.as<ka_move_summary>();
+    long long* d_brk = c->d_score_brk.as<long long>();
+    const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
+    if ((part_weight && Q > 0 && cudaMemcpyAsync(c->d_score_w.p, part_weight, (size_t)Q * 8, cudaMemcpyHostToDevice, s) != cudaSuccess) ||
+        cudaMemcpyAsync(c->d_score_off.p, cand_off, (size_t)(K + 1) * 4, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemsetAsync(d_sum, 0, sum_bytes, s) != cudaSuccess || cudaMemsetAsync(d_brk, 0, std::max<size_t>(3 * nb, 1) * 8, s) != cudaSuccess)
+        return fail(KA_ERR_CUDA);
+    const KaCandidate* cand = c->d_cand_tab.as<KaCandidate>();
+    const int32_t* d_off = c->d_score_off.as<int32_t>();
+    const dim3 grid((unsigned)std::max<int64_t>((Q + 255) / 256, 1), K);
+    ka_score_rows_kernel<<<grid, 256, 0, s>>>(cand, d_off, (uint32_t)Q, out_stride, run.io.d_out, run.io.d_out_len,
+                                              c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), d_w, d_sum, d_brk, d_brk + nb,
+                                              d_brk + 2 * nb);
+    ka_score_finish_kernel<<<K, 256, 0, s>>>(cand, d_off, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb);
+    c->launches += 2;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(summary, d_sum, sum_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess)
+        return fail(KA_ERR_CUDA);
+    for (int i = 0; i < 3; ++i)
+        if (brk[i] && nb > 0 && cudaMemcpyAsync(brk[i], d_brk + i * nb, nb * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess)
+            return fail(KA_ERR_CUDA);
+    if (out_broker && Q > 0) {
+        run.io.h_out = out_broker;
+        run.io.h_out_len = out_len;
+        if (enq_copy_out(s, run.io, out_stride, 0, (int64_t)K * Q) != KA_OK) return fail(KA_ERR_CUDA);
     }
     return finish_candidates(c, s, K, T, st, part_id, part_off);
 }

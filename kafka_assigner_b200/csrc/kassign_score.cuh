@@ -1,0 +1,154 @@
+// kassign_score.cuh — movement and balance summary of every candidate of a batched ragged solve (ka_score_candidates), computed
+// from the emitted rows where they already are, so that a sweep needs K summaries instead of K copies of the rows.
+//
+//   ka_score_rows_kernel    one thread per (row, candidate): the row's flags and added / dropped counts against the current
+//                           list, warp sums into the candidate's summary, per-broker sums into [ΣN] arrays in HBM
+//   ka_score_finish_kernel  one CTA per candidate: max / min over its brokers and the busiest receiving broker
+//
+// Everything is integer and every sum commutative, so the results do not depend on the order of the atomics.
+#pragma once
+#include <climits>
+
+#include "kassign_stage.cuh"
+#include "../../include/kassign.h"
+
+// A candidate that failed (or has no broker) keeps the zero summary and per-broker entries the host cleared.
+__device__ __forceinline__ bool ka_score_ok(const KaCandidate& c) { return c.N > 0 && *c.err_topic == 0xFFFFFFFFu; }
+
+__device__ __forceinline__ long long ka_warp_sum64(long long v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(KA_FULL, v, o);
+    return v;
+}
+
+// grid (ceil(Q / 256), K). Row g of candidate k is out[(k * Q + g) * S ..] / out_len[k * Q + g]; its current list is
+// cur[rep_off[g] .. rep_off[g + 1]), at most S <= 3 long. weight: [Q] or null (1 per row). bro_off[k]: candidate k's first
+// entry in the per-broker arrays (cand_off of the call).
+__global__ void __launch_bounds__(256) ka_score_rows_kernel(const KaCandidate* __restrict__ cand, const int32_t* __restrict__ bro_off,
+                                                            uint32_t Q, int S, const int32_t* __restrict__ out,
+                                                            const int32_t* __restrict__ out_len, const int64_t* __restrict__ rep_off,
+                                                            const int32_t* __restrict__ cur, const int64_t* __restrict__ weight,
+                                                            ka_move_summary* __restrict__ summary, long long* __restrict__ broker_replicas,
+                                                            long long* __restrict__ broker_leaders, long long* __restrict__ broker_in) {
+    const int k = blockIdx.y;
+    const KaCandidate& c = cand[k];
+    if (!ka_score_ok(c)) return;   // CTA-uniform: every lane below reaches the warp sums
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    int changed = 0, moved = 0, leader = 0;
+    long long added = 0, dropped = 0;
+    if (g < Q) {
+        const int64_t row = (int64_t)k * Q + g;
+        const int n = out_len[row];
+        const int64_t a = rep_off[g];
+        const int m = (int)(rep_off[g + 1] - a);
+        int nb[3], cb[3];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            nb[j] = j < n ? out[row * S + j] : 0;
+            cb[j] = j < m ? __ldg(cur + a + j) : 0;
+        }
+        const long long w = weight ? __ldg(weight + g) : 1;
+        // the candidate's id -> index lookup of kernel A, its table read from HBM
+        KaSolveParams p{};
+        p.N = c.N;
+        p.lut_mode = c.lut_mode;
+        p.min_id = c.min_id;
+        p.range = c.range;
+        p.glut = c.glut;
+        p.broker_id = c.broker_id;
+        const KaTab tab{nullptr, c.blob + c.lut_off};
+        const int64_t base = bro_off[k];
+        int n_add = 0, n_drop = 0;
+        bool diff = n != m;
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            if (j < m) {
+                bool kept = false;
+#pragma unroll
+                for (int i = 0; i < 3; ++i) kept |= i < n && nb[i] == cb[j];
+                n_drop += !kept;
+            }
+            if (j < n) {
+                bool held = false;
+#pragma unroll
+                for (int i = 0; i < 3; ++i) held |= i < m && cb[i] == nb[j];
+                n_add += !held;
+                diff |= j < m && nb[j] != cb[j];
+                const int64_t e = base + ka_lookup(nb[j], tab, p);
+                atomicAdd(reinterpret_cast<unsigned long long*>(broker_replicas + e), (unsigned long long)w);
+                if (j == 0) atomicAdd(reinterpret_cast<unsigned long long*>(broker_leaders + e), (unsigned long long)w);
+                if (!held) atomicAdd(reinterpret_cast<unsigned long long*>(broker_in + e), (unsigned long long)w);
+            }
+        }
+        changed = diff;
+        moved = n_add + n_drop > 0;
+        leader = m == 0 || n == 0 || nb[0] != cb[0];
+        added = w * n_add;
+        dropped = w * n_drop;
+    }
+    changed = __reduce_add_sync(KA_FULL, changed);
+    moved = __reduce_add_sync(KA_FULL, moved);
+    leader = __reduce_add_sync(KA_FULL, leader);
+    added = ka_warp_sum64(added);
+    dropped = ka_warp_sum64(dropped);
+    if ((threadIdx.x & 31) == 0) {
+        ka_move_summary& s = summary[k];
+        auto add = [](int64_t& f, long long v) {
+            if (v) atomicAdd(reinterpret_cast<unsigned long long*>(&f), (unsigned long long)v);
+        };
+        add(s.rows_changed, changed);
+        add(s.rows_moved, moved);
+        add(s.leaders_changed, leader);
+        add(s.replicas_added, added);
+        add(s.replicas_dropped, dropped);
+    }
+}
+
+// grid K, 256 threads: the per-broker extremes of candidate k over all N_k of its brokers (brokers left with nothing count),
+// and the busiest receiving broker, the lowest id on ties (indices ascend with ids). A failed candidate: zeros, id -1.
+__global__ void __launch_bounds__(256) ka_score_finish_kernel(const KaCandidate* __restrict__ cand, const int32_t* __restrict__ bro_off,
+                                                              ka_move_summary* __restrict__ summary,
+                                                              const long long* __restrict__ broker_replicas,
+                                                              const long long* __restrict__ broker_leaders,
+                                                              const long long* __restrict__ broker_in) {
+    __shared__ long long sh[8][6];
+    const int k = blockIdx.x;
+    const KaCandidate& c = cand[k];
+    const int n = ka_score_ok(c) ? c.N : 0;
+    const int64_t base = bro_off[k];
+    long long rmax = LLONG_MIN, rmin = LLONG_MAX, lmax = LLONG_MIN, lmin = LLONG_MAX, imax = -1, iarg = INT_MAX;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const long long r = broker_replicas[base + i], l = broker_leaders[base + i], in = broker_in[base + i];
+        rmax = max(rmax, r);
+        rmin = min(rmin, r);
+        lmax = max(lmax, l);
+        lmin = min(lmin, l);
+        if (in > imax) { imax = in; iarg = i; }   // i ascends: the first maximum is the lowest index
+    }
+    auto fold = [&](long long orm, long long orn, long long olm, long long oln, long long oim, long long oia) {
+        rmax = max(rmax, orm);
+        rmin = min(rmin, orn);
+        lmax = max(lmax, olm);
+        lmin = min(lmin, oln);
+        if (oim > imax || (oim == imax && oia < iarg)) { imax = oim; iarg = oia; }
+    };
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1)
+        fold(__shfl_xor_sync(KA_FULL, rmax, o), __shfl_xor_sync(KA_FULL, rmin, o), __shfl_xor_sync(KA_FULL, lmax, o),
+             __shfl_xor_sync(KA_FULL, lmin, o), __shfl_xor_sync(KA_FULL, imax, o), __shfl_xor_sync(KA_FULL, iarg, o));
+    const int wid = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) {
+        sh[wid][0] = rmax; sh[wid][1] = rmin; sh[wid][2] = lmax; sh[wid][3] = lmin; sh[wid][4] = imax; sh[wid][5] = iarg;
+    }
+    __syncthreads();
+    if (threadIdx.x != 0) return;
+    for (int v = 1; v < (int)(blockDim.x >> 5); ++v) fold(sh[v][0], sh[v][1], sh[v][2], sh[v][3], sh[v][4], sh[v][5]);
+    ka_move_summary& s = summary[k];
+    const bool any = n > 0;
+    s.max_broker_in = any ? imax : 0;
+    s.max_broker_in_id = any && imax > 0 ? __ldg(c.broker_id + iarg) : -1;
+    s.max_broker_replicas = any ? rmax : 0;
+    s.min_broker_replicas = any ? rmin : 0;
+    s.max_broker_leaders = any ? lmax : 0;
+    s.min_broker_leaders = any ? lmin : 0;
+}

@@ -8,6 +8,8 @@
 //   kassign::solveTopicsJson                          <->  that loop + its org.json text, built on the device (KAG:172-186)
 //   kassign::solveTopicsCandidates                    <->  that loop once per candidate broker set, each with a new
 //                                                          assigner, in one device call (a decommission sweep)
+//   kassign::scoreTopicsCandidates                    <->  the same sweep, reduced on the device to what each broker set
+//                                                          would move and how evenly it spreads replicas and leaders
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -120,15 +122,8 @@ public:
                                                        int desiredReplicationFactor) {
         const Flat f = flatten(topics, desiredReplicationFactor);
         const int K = (int)candidates.size(), T = (int)topics.size();
-        std::vector<int32_t> candOff(K + 1, 0), ids, racks;
-        for (int k = 0; k < K; ++k) {
-            std::vector<int32_t> id(candidates[k].brokers.begin(), candidates[k].brokers.end()), rackIdx;
-            const int rc = rackIndices(id, candidates[k].rackAssignment, rackIdx);
-            if (rc != KA_OK) throw KassignError(rc, "ka_rack_indices");
-            ids.insert(ids.end(), id.begin(), id.end());
-            racks.insert(racks.end(), rackIdx.begin(), rackIdx.end());
-            candOff[k + 1] = (int32_t)ids.size();
-        }
+        std::vector<int32_t> candOff, ids, racks;
+        candidateTables(candidates, candOff, ids, racks);
         const size_t Q = f.partId.size();
         std::vector<int32_t> outLen((size_t)K * Q, 0), out((size_t)K * Q * f.stride, -1);
         std::vector<ka_status> st(std::max(K, 1));
@@ -138,6 +133,52 @@ public:
         for (int k = 0; k < K; ++k) {
             res[k].status = st[k];
             if (st[k].code == KA_OK) res[k].topics = unflatten(f, out.data() + (size_t)k * Q * f.stride, outLen.data() + (size_t)k * Q);
+        }
+        return res;
+    }
+
+    // What one candidate's run would move, and how it spreads the replicas (ka_move_summary); the per-broker maps are keyed by
+    // broker id and hold every broker of the candidate (filled when asked for).
+    struct CandidateScore {
+        ka_status status;   // re-throw with throwForStatus; a failed candidate has a zero summary (max_broker_in_id = -1)
+        ka_move_summary summary;
+        std::map<int, int64_t> brokerReplicas, brokerLeaders, brokerIn;
+    };
+
+    // solveTopicsCandidates scored on the device (ka_score_candidates): per candidate the summary of what its new assignment
+    // changes against `topics`' current one, instead of the assignment itself. weights: empty (1 per partition) or, per topic,
+    // the weight of every partition (e.g. its size in bytes; a missing partition throws std::out_of_range).
+    std::vector<CandidateScore> scoreTopicsCandidates(const std::vector<TopicInput>& topics, const std::vector<Candidate>& candidates,
+                                                      int desiredReplicationFactor,
+                                                      const std::vector<std::map<int, int64_t>>& weights = {}, bool perBroker = false) {
+        const Flat f = flatten(topics, desiredReplicationFactor);
+        const int K = (int)candidates.size(), T = (int)topics.size();
+        std::vector<int32_t> candOff, ids, racks;
+        candidateTables(candidates, candOff, ids, racks);
+        std::vector<int64_t> w;
+        if (!weights.empty()) {
+            if (weights.size() != topics.size()) throw std::invalid_argument("one weight map per topic");
+            for (int t = 0; t < T; ++t)
+                for (const auto& e : topics[t].current) w.push_back(weights[t].at(e.first));
+        }
+        std::vector<ka_move_summary> summary(std::max(K, 1));
+        std::vector<int64_t> brk[3];
+        for (auto& a : brk) a.assign(perBroker ? ids.size() : 0, 0);
+        std::vector<ka_status> st(std::max(K, 1));
+        ka_score_candidates(ctx_, K, candOff.data(), ids.data(), racks.data(), T, f.hash.data(), f.partOff.data(), f.partId.data(),
+                            f.repOff.data(), f.cur.data(), desiredReplicationFactor, f.stride, w.empty() ? nullptr : w.data(),
+                            summary.data(), perBroker ? brk[0].data() : nullptr, perBroker ? brk[1].data() : nullptr,
+                            perBroker ? brk[2].data() : nullptr, nullptr, nullptr, st.data());
+        std::vector<CandidateScore> res(K);
+        for (int k = 0; k < K; ++k) {
+            res[k].status = st[k];
+            res[k].summary = summary[k];
+            if (perBroker)
+                for (int i = candOff[k]; i < candOff[k + 1]; ++i) {
+                    res[k].brokerReplicas[ids[i]] = brk[0][i];
+                    res[k].brokerLeaders[ids[i]] = brk[1][i];
+                    res[k].brokerIn[ids[i]] = brk[2][i];
+                }
         }
         return res;
     }
@@ -200,6 +241,19 @@ private:
         }
         rackIdx.assign(ids.size(), 0);
         return ka_rack_indices((int32_t)ids.size(), ids.data(), names.data(), rackIdx.data());
+    }
+    // The candidate tables of the C ABI (cand_off, broker_id, broker_rack) of a list of broker sets.
+    static void candidateTables(const std::vector<Candidate>& candidates, std::vector<int32_t>& candOff, std::vector<int32_t>& ids,
+                                std::vector<int32_t>& racks) {
+        candOff.assign(candidates.size() + 1, 0);
+        for (size_t k = 0; k < candidates.size(); ++k) {
+            std::vector<int32_t> id(candidates[k].brokers.begin(), candidates[k].brokers.end()), rackIdx;
+            const int rc = rackIndices(id, candidates[k].rackAssignment, rackIdx);
+            if (rc != KA_OK) throw KassignError(rc, "ka_rack_indices");
+            ids.insert(ids.end(), id.begin(), id.end());
+            racks.insert(racks.end(), rackIdx.begin(), rackIdx.end());
+            candOff[k + 1] = (int32_t)ids.size();
+        }
     }
     void setBrokers(const std::set<int>& brokers, const std::map<int, std::string>& racks) {
         std::vector<int32_t> ids(brokers.begin(), brokers.end());  // std::set: ascending == TreeMap order (KAS:78)
