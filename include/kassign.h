@@ -277,6 +277,15 @@ int32_t ka_ctx_set_timing(ka_ctx* ctx, int32_t enabled);
 int32_t ka_ctx_last_timing(ka_ctx* ctx, float* ms /* [8] */);
 /* Number of kernel launches issued by this ctx since creation (for bench.py's gpu_launches). */
 int64_t ka_ctx_launch_count(ka_ctx* ctx);
+/* The leader-order plan of the LAST solve call on this ctx (any entry point, including the staged and candidate calls):
+ * plan[0] rec_kind (3 / 4 / 8)   plan[1] levels (0/1)   plan[2] chain threads   plan[3] ring_log2
+ * plan[4] gctr (0/1)   plan[5] loop shape (0 general, 1 warp1, 2 single, 3 full)   plan[6] chain launches of the call
+ * plan[7] candidates K (0 for a single solve).
+ * Cleared when a solve call passes its argument checks (ka_stage_dense_device starts a staged solve; its ka_order_device /
+ * ka_order_slot_device calls add to it), so a call that launches no chain (a limit before any launch, or no rows) leaves
+ * all zeros.
+ * KA_ERR_BAD_ARG when ctx or plan is NULL. */
+int32_t ka_ctx_last_order_plan(ka_ctx* ctx, int32_t* plan /* [8] */);
 
 const char* ka_version(void);
 

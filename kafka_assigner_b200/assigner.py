@@ -146,6 +146,15 @@ class Solver:
     def launch_count(self):
         return int(self._L.ka_ctx_launch_count(self._h))
 
+    def last_order_plan(self):
+        """The leader-order plan of the last solve call (ka_ctx_last_order_plan): (rec_kind, levels, chain threads, ring_log2,
+        gctr, loop shape [0 general, 1 warp1, 2 single, 3 full], chain launches, candidates K)."""
+        plan = np.zeros(8, dtype=np.int32)
+        rc = self._L.ka_ctx_last_order_plan(self._h, _ptr(plan))
+        if rc:
+            raise KassignError(rc, "ka_ctx_last_order_plan")
+        return tuple(int(x) for x in plan)
+
     # -- solves --------------------------------------------------------------------------------
     def solve_dense(self, topic_hash, cur, desired_rf=-1, out_stride=None, out=None, out_len=None, check=True,
                     topic_names=None):

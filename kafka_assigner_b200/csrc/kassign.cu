@@ -142,6 +142,7 @@ struct ka_ctx {
     int last_stages = 1;
     int chain_used = 0;                    // ev_chain rows recorded
     bool slot_timed[2] = {false, false};   // ka_order_slot_device recorded ev_chain[slot][0..1]
+    int32_t order_plan[8] = {};            // ka_ctx_last_order_plan: the leader-order chains of the last solve call
     // staged problem (between the context-free stage and the leader-order stage)
     bool staged = false;
     StageDesc staged_block;
@@ -527,18 +528,20 @@ cudaError_t launch_order_t(cudaStream_t s, const KaOrderParams& o, const Plan& p
     return cudaGetLastError();
 }
 
-// KIND 0 / 1: slot chains of rows <= 3 (chunk arithmetic, barrier flavour, full chunks are compile-time); 4 / 8: rows of 4 / 5..8
+// KIND 0 / 1: slot chains of rows <= 3 (chunk arithmetic, barrier flavour, full chunks are compile-time); 4 / 8: rows of 4 / 5..8.
+// *sel: the instantiation launched, (GCTR ? 4 : 0) | loop shape (0 general, 1 WARP1, 2 SINGLE, 3 FULL).
 template <int KIND, int MAXNT, bool CAND = false>
-cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int ncand = 0) {
+cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int* sel, int ncand = 0) {
     if constexpr (KIND > 1) {
+        *sel = pl.b_gctr ? 4 : 0;
         return pl.b_gctr ? launch_order_t<KIND, MAXNT, false, true, false, false, false>(s, o, pl, ncand)
                          : launch_order_t<KIND, MAXNT, false, false, false, false, false>(s, o, pl, ncand);
     } else {
         const bool warp1 = pl.b_threads == 32;                                                          // window mode
         const bool single = !warp1 && o.uniform_width != 0 && o.uniform_width <= (uint32_t)pl.b_threads;   // chunk = topic
         const bool full = single && o.uniform_width == (uint32_t)pl.b_threads;                          // no idle lane
-        const int sel = (pl.b_gctr ? 4 : 0) | (warp1 ? 1 : (full ? 3 : (single ? 2 : 0)));
-        switch (sel) {
+        *sel = (pl.b_gctr ? 4 : 0) | (warp1 ? 1 : (full ? 3 : (single ? 2 : 0)));
+        switch (*sel) {
             case 0: return launch_order_t<KIND, MAXNT, CAND, false, false, false, false>(s, o, pl, ncand);
             case 1: return launch_order_t<KIND, MAXNT, CAND, false, false, true, false>(s, o, pl, ncand);
             case 2: return launch_order_t<KIND, MAXNT, CAND, false, true, false, false>(s, o, pl, ncand);
@@ -549,6 +552,23 @@ cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl,
             default: return launch_order_t<KIND, MAXNT, CAND, true, true, false, true>(s, o, pl, ncand);
         }
     }
+}
+
+// ka_ctx_last_order_plan: a chain launch of the current solve call (sel as launch_order reports it, ncand 0 for a single solve).
+void note_order(ka_ctx* c, const Plan& pl, int sel, int ncand) {
+    int32_t* r = c->order_plan;
+    r[0] = pl.rec_kind;
+    r[1] = pl.a_levels;
+    r[2] = pl.b_threads;
+    r[3] = pl.b_ring_log2;
+    r[4] = (sel >> 2) & 1;
+    r[5] = sel & 3;
+    r[6]++;
+    r[7] = ncand;
+}
+
+void reset_order_plan(ka_ctx* c) {
+    for (int32_t& v : c->order_plan) v = 0;
 }
 
 // How many topic sub-blocks the slot chains of one staged block are cut into: the slot-0 chain of sub-block j+1 runs (on
@@ -693,7 +713,9 @@ int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int 
     const SubBlock b = sub_block(d, j, nsub);
     if (b.rq <= 0 || c->N <= 0) return KA_OK;
     const KaOrderParams o = order_params(c, d, b);
-    KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, d.pl) : launch_order<1, 1024>(s, o, d.pl)));
+    int sel = 0;
+    KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, d.pl, &sel) : launch_order<1, 1024>(s, o, d.pl, &sel)));
+    note_order(c, d.pl, sel, 0);
     c->launches++;
     return KA_OK;
 }
@@ -727,7 +749,9 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io,
         o.broker_id = c->d_broker_id.as<int32_t>();
         o.out = d_out;
         o.out_len = d_out_len;
-        KA_CUDA((pl.rec_kind == 4 ? launch_order<4, 512>(s, o, pl) : launch_order<8, 256>(s, o, pl)));
+        int sel = 0;
+        KA_CUDA((pl.rec_kind == 4 ? launch_order<4, 512>(s, o, pl, &sel) : launch_order<8, 256>(s, o, pl, &sel)));
+        note_order(c, pl, sel, 0);
         c->launches++;
         if (io.json) return enq_json(c, s, io, d, b, d.blk == 0, d.blk == blocks_in_solve - 1);
         return KA_OK;
@@ -813,6 +837,7 @@ int enq_inputs(cudaStream_t s, const SolveCall& io, const StageDesc& d, int64_t 
 int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_status* st) {
     c->staged = false;   // the solve reuses the scratch a staged block lives in
     c->last_was_staged = false;
+    reset_order_plan(c);
     const bool ragged = sh.d_part_off != nullptr;
     const int T = sh.T;
     const int K = ragged ? 1 : pipeline_stages(T, (int64_t)T * sh.P);
@@ -1138,6 +1163,12 @@ int32_t ka_ctx_last_timing(ka_ctx* c, float* ms) {
 
 int64_t ka_ctx_launch_count(ka_ctx* c) { return c ? c->launches : 0; }
 
+int32_t ka_ctx_last_order_plan(ka_ctx* c, int32_t* plan) {
+    if (!c || !plan) return KA_ERR_BAD_ARG;
+    for (int i = 0; i < 8; ++i) plan[i] = c->order_plan[i];
+    return KA_OK;
+}
+
 int32_t ka_last_status(ka_ctx* c, ka_status* st) {
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     int rc = enter(c, false);
@@ -1335,10 +1366,13 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
         o.cand = cand;
         o.cand_t0 = b.t0;
         o.cand_t1 = b.t1;
-        KA_CUDA((launch_order<0, 1024, true>(c->sb1, o, pl, K)));
+        int sel = 0;
+        KA_CUDA((launch_order<0, 1024, true>(c->sb1, o, pl, &sel, K)));
+        note_order(c, pl, sel, K);
         KA_CUDA(cudaEventRecord(c->ev_b1[j], c->sb1));
         KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[j], 0));
-        KA_CUDA((launch_order<1, 1024, true>(s, o, pl, K)));
+        KA_CUDA((launch_order<1, 1024, true>(s, o, pl, &sel, K)));
+        note_order(c, pl, sel, K);
         const dim3 grid((unsigned)((b.rq + 255) / 256), K);
         if (d.d_part_off)
             ka_emit3_candidates_kernel<true><<<grid, 256, 0, s>>>(cand, 0u, T, 0, d.d_part_off, (uint32_t)b.rq, S, Q, d_out, d_out_len);
@@ -1369,6 +1403,7 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
     if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
     if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
     if ((rc = enter(c, true)) != KA_OK) return all(rc);
+    reset_order_plan(c);
     // the plan of the call: counter placement and loop shape from the largest table, levels if any candidate has capacity > 1
     std::vector<BrokerTable> tabs;
     int nmax = 0, blob_max = 0;
@@ -1411,6 +1446,7 @@ int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     cudaStream_t s = (cudaStream_t)stream;
     StageDesc& d = c->staged_block;
     c->staged = false;
+    reset_order_plan(c);
     if ((rc = describe_block(c, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, 0, T, 0, d, &lst)) != KA_OK ||
         (rc = reserve_scratch(c, &d, 1)) != KA_OK)
         return rc;
@@ -1782,6 +1818,7 @@ static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, 
     const int64_t Q = sc.Q;
     if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
     if ((rc = enter(c, true)) != KA_OK) return all(rc);
+    reset_order_plan(c);
     // the plan of the call: counter placement and loop shape from the largest table, the largest capacity of any candidate
     std::vector<BrokerTable> tabs;
     int nmax = 0, blob_max = 0;
