@@ -286,6 +286,14 @@ int64_t ka_ctx_launch_count(ka_ctx* ctx);
  * all zeros.
  * KA_ERR_BAD_ARG when ctx or plan is NULL. */
 int32_t ka_ctx_last_order_plan(ka_ctx* ctx, int32_t* plan /* [8] */);
+/* The sticky/spread plan (kernel A) of the LAST solve call on this ctx, from its last kernel A launch:
+ * plan[0] load bytes per broker (1 / 2)   plan[1] levels (0/1)   plan[2] SM, the compile-time row bound (3 / 8)
+ * plan[3] candidates K (0 for a single solve)   plan[4] warps per CTA   plan[5] grid.x (CTAs per candidate)
+ * plan[6] bit mask of the id lookup modes of the call's broker tables (1: shared-memory LUT, 2: global LUT, 4: binary search)
+ * plan[7] kernel A launches of the call.
+ * Cleared as ka_ctx_last_order_plan is, so a call that launches no kernel A leaves all zeros. KA_ERR_BAD_ARG when ctx or
+ * plan is NULL. */
+int32_t ka_ctx_last_stage_plan(ka_ctx* ctx, int32_t* plan /* [8] */);
 
 const char* ka_version(void);
 

@@ -59,6 +59,7 @@ SYMBOLS = {
     "ka_ctx_last_timing": (_i32, [_vp, _vp]),
     "ka_ctx_launch_count": (_i64, [_vp]),
     "ka_ctx_last_order_plan": (_i32, [_vp, _vp]),
+    "ka_ctx_last_stage_plan": (_i32, [_vp, _vp]),
     "ka_version": (ctypes.c_char_p, []),
 }
 

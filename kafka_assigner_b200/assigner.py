@@ -155,6 +155,15 @@ class Solver:
             raise KassignError(rc, "ka_ctx_last_order_plan")
         return tuple(int(x) for x in plan)
 
+    def last_stage_plan(self):
+        """The sticky/spread plan of the last solve call (ka_ctx_last_stage_plan): (load bytes, levels, SM, candidates K,
+        warps per CTA, grid.x, lookup-mode mask [1 shared LUT, 2 global LUT, 4 binary search], kernel A launches)."""
+        plan = np.zeros(8, dtype=np.int32)
+        rc = self._L.ka_ctx_last_stage_plan(self._h, _ptr(plan))
+        if rc:
+            raise KassignError(rc, "ka_ctx_last_stage_plan")
+        return tuple(int(x) for x in plan)
+
     # -- solves --------------------------------------------------------------------------------
     def solve_dense(self, topic_hash, cur, desired_rf=-1, out_stride=None, out=None, out_len=None, check=True,
                     topic_names=None):

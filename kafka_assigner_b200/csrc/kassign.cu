@@ -67,7 +67,7 @@ struct HostPinned {
 
 struct Plan {
     // kernel A
-    int a_warps, a_load_bytes, a_slab_bytes, a_cnt_bytes, a_load_kind;  // kind 0=u8 1=u16 2=u32
+    int a_warps, a_load_bytes, a_slab_bytes, a_cnt_bytes, a_load_kind;  // kind 0=u8 1=u16
     int a_levels;                                   // 1: some topic may hold a broker twice -> conflict levels + tables
     int lv_owner_bytes, lv_last_bytes, lv_p_bytes;  // per-warp scratch of the level pass
     size_t a_smem;
@@ -143,6 +143,7 @@ struct ka_ctx {
     int chain_used = 0;                    // ev_chain rows recorded
     bool slot_timed[2] = {false, false};   // ka_order_slot_device recorded ev_chain[slot][0..1]
     int32_t order_plan[8] = {};            // ka_ctx_last_order_plan: the leader-order chains of the last solve call
+    int32_t stage_plan[8] = {};            // ka_ctx_last_stage_plan: kernel A of the last solve call
     // staged problem (between the context-free stage and the leader-order stage)
     bool staged = false;
     StageDesc staged_block;
@@ -282,8 +283,11 @@ constexpr size_t KA_ORDER_SMEM_BUDGET = 226 * 1024;
 int make_plan(int N, int blob_bytes, int64_t Q, int S, int Pmax, int64_t capmax, bool ragged, Plan& pl, ka_status* st) {
     if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX, 0);
     // ---- kernel A
-    pl.a_load_kind = capmax <= 255 ? 0 : (capmax <= 65535 ? 1 : 2);
-    const int lsz = pl.a_load_kind == 0 ? 1 : (pl.a_load_kind == 1 ? 2 : 4);
+    // A broker's load never exceeds the capacity. capmax only counts tables that can serve the target RF (dense_capmax,
+    // ragged_capmax), so capmax <= Pmax; capacity > 1 turns the level pass on, whose 15-bit cursors need Pmax <= 32767. So
+    // a plan that passes the level check below has capmax <= 32767, and 16-bit loads always suffice.
+    pl.a_load_kind = capmax <= 255 ? 0 : 1;
+    const int lsz = pl.a_load_kind == 0 ? 1 : 2;
     pl.a_load_bytes = (int)align16((size_t)std::max(N, 1) * lsz);
     pl.a_slab_bytes = (int)align16((size_t)std::max(Pmax, 1) * S * 2);
     pl.a_cnt_bytes = (int)align16((size_t)std::max(Pmax, 1));
@@ -351,6 +355,13 @@ struct Shape {
     int64_t capmax = 0;
 };
 
+// The largest capacity (KAS:65-71) of a dense problem of P partitions per topic and target RF rf_t under a table of n
+// brokers: 0 when the table cannot serve rf_t, whose every topic then fails with KA_ERR_RF_GT_BROKERS before it loads a
+// broker. The dense counterpart of ragged_capmax, which applies the same rule per topic; so capmax <= P.
+int64_t dense_capmax(int P, int rf_t, int n) {
+    return n > 0 && rf_t <= n ? ((int64_t)P * std::max(rf_t, 0) + n - 1) / n : 0;
+}
+
 // The planned StageDesc of topics [t0, t1) of a problem, block `blk` of its solve.
 int describe_block(ka_ctx* c, const Shape& sh, int t0, int t1, int blk, StageDesc& d, ka_status* st) {
     const bool ragged = sh.d_part_off != nullptr;
@@ -372,9 +383,8 @@ int describe_block(ka_ctx* c, const Shape& sh, int t0, int t1, int blk, StageDes
         d.Pmax = sh.Pmax;
         d.capmax = sh.capmax;
     } else {
-        const int rf_t = sh.desired_rf >= 0 ? sh.desired_rf : sh.RF;
         d.Pmax = sh.P;
-        d.capmax = c->N > 0 ? ((int64_t)sh.P * std::max(rf_t, 0) + c->N - 1) / c->N : 0;
+        d.capmax = dense_capmax(sh.P, sh.desired_rf >= 0 ? sh.desired_rf : sh.RF, c->N);
     }
     return make_plan(c->N, c->blob_bytes, d.Q, d.S, d.Pmax, d.capmax, ragged, d.pl, st);
 }
@@ -420,9 +430,10 @@ int reset_flags(ka_ctx* c, cudaStream_t s) {
     return KA_OK;
 }
 
-// ncand > 0: kernel A of a batched solve over ncand candidate tables (p.cand), grid.y = candidate.
+// ncand > 0: kernel A of a batched solve over ncand candidate tables (p.cand), grid.y = candidate. *grid_x: the CTAs per
+// candidate it launched.
 template <typename LoadT, bool LEVELS, int SM, bool CAND>
-cudaError_t launch_stage_t(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand) {
+cudaError_t launch_stage_t(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand, int* grid_x) {
     auto kern = ka_sticky_spread_kernel<LoadT, LEVELS, SM, CAND>;
     const int threads = pl.a_warps * 32;
     cudaError_t e = allow_smem(kern, pl.a_smem);
@@ -432,31 +443,44 @@ cudaError_t launch_stage_t(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, co
     if (e != cudaSuccess) return e;
     int grid = (T + pl.a_warps - 1) / pl.a_warps;
     grid = std::min(grid, std::max(1, std::max(1, occ) * c->sm_count / std::max(ncand, 1)));
+    *grid_x = grid;
     kern<<<dim3(grid, std::max(ncand, 1)), threads, pl.a_smem, s>>>(p, pl.a_load_bytes, pl.a_slab_bytes, pl.a_cnt_bytes, pl.lv_owner_bytes,
                                                                  pl.lv_last_bytes, pl.lv_p_bytes);
     return cudaGetLastError();
 }
 
 template <typename LoadT, bool LEVELS, bool CAND>
-cudaError_t launch_stage(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand) {
-    return p.S <= 3 ? launch_stage_t<LoadT, LEVELS, 3, CAND>(c, s, p, pl, T, ncand) : launch_stage_t<LoadT, LEVELS, 8, CAND>(c, s, p, pl, T, ncand);
+cudaError_t launch_stage(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand, int* grid_x) {
+    return p.S <= 3 ? launch_stage_t<LoadT, LEVELS, 3, CAND>(c, s, p, pl, T, ncand, grid_x)
+                    : launch_stage_t<LoadT, LEVELS, 8, CAND>(c, s, p, pl, T, ncand, grid_x);
 }
 
-// Kernel A in the instantiation the plan asks for.
+void reset_plans(ka_ctx* c) {
+    for (int32_t& v : c->order_plan) v = 0;
+    for (int32_t& v : c->stage_plan) v = 0;
+}
+
+// Kernel A in the instantiation the plan asks for. Loads are 1 or 2 bytes (make_plan); a plan without levels has capacity
+// <= 1 and so 1-byte loads. lut_mask: bit m is set when one of the launch's broker tables looks ids up in mode m (KA_LUT_*);
+// recorded for ka_ctx_last_stage_plan.
 template <bool CAND>
-int launch_stage_plan(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand) {
+int launch_stage_plan(ka_ctx* c, cudaStream_t s, const KaSolveParams& p, const Plan& pl, int T, int ncand, int lut_mask) {
     cudaError_t e;
-    if (pl.a_levels) {
-        if (pl.a_load_kind == 0) e = launch_stage<uint8_t, true, CAND>(c, s, p, pl, T, ncand);
-        else if (pl.a_load_kind == 1) e = launch_stage<uint16_t, true, CAND>(c, s, p, pl, T, ncand);
-        else e = launch_stage<uint32_t, true, CAND>(c, s, p, pl, T, ncand);
-    } else {
-        if (pl.a_load_kind == 0) e = launch_stage<uint8_t, false, CAND>(c, s, p, pl, T, ncand);
-        else if (pl.a_load_kind == 1) e = launch_stage<uint16_t, false, CAND>(c, s, p, pl, T, ncand);
-        else e = launch_stage<uint32_t, false, CAND>(c, s, p, pl, T, ncand);
-    }
+    int grid_x = 0;
+    if (!pl.a_levels) e = launch_stage<uint8_t, false, CAND>(c, s, p, pl, T, ncand, &grid_x);
+    else if (pl.a_load_kind == 0) e = launch_stage<uint8_t, true, CAND>(c, s, p, pl, T, ncand, &grid_x);
+    else e = launch_stage<uint16_t, true, CAND>(c, s, p, pl, T, ncand, &grid_x);
     KA_CUDA(e);
     c->launches++;
+    int32_t* r = c->stage_plan;
+    r[0] = pl.a_load_kind == 0 ? 1 : 2;
+    r[1] = pl.a_levels;
+    r[2] = p.S <= 3 ? 3 : 8;
+    r[3] = ncand;
+    r[4] = pl.a_warps;
+    r[5] = grid_x;
+    r[6] = lut_mask;
+    r[7]++;
     return KA_OK;
 }
 
@@ -501,7 +525,7 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done)
         p.lend = pl.a_levels ? c->d_lend.as<uint32_t>() + d.q0 : nullptr;
         p.tstatus = c->d_tstatus.as<int4>();
         p.err_topic = c->d_flags.as<unsigned>();
-        const int rc = launch_stage_plan<false>(c, s, p, pl, d.T, 0);
+        const int rc = launch_stage_plan<false>(c, s, p, pl, d.T, 0, 1 << c->lut_mode);
         if (rc != KA_OK) return rc;
     }
     if (c->timing) KA_CUDA(cudaEventRecord(a_done, s));
@@ -565,10 +589,6 @@ void note_order(ka_ctx* c, const Plan& pl, int sel, int ncand) {
     r[5] = sel & 3;
     r[6]++;
     r[7] = ncand;
-}
-
-void reset_order_plan(ka_ctx* c) {
-    for (int32_t& v : c->order_plan) v = 0;
 }
 
 // How many topic sub-blocks the slot chains of one staged block are cut into: the slot-0 chain of sub-block j+1 runs (on
@@ -837,7 +857,7 @@ int enq_inputs(cudaStream_t s, const SolveCall& io, const StageDesc& d, int64_t 
 int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_status* st) {
     c->staged = false;   // the solve reuses the scratch a staged block lives in
     c->last_was_staged = false;
-    reset_order_plan(c);
+    reset_plans(c);
     const bool ragged = sh.d_part_off != nullptr;
     const int T = sh.T;
     const int K = ragged ? 1 : pipeline_stages(T, (int64_t)T * sh.P);
@@ -1169,6 +1189,12 @@ int32_t ka_ctx_last_order_plan(ka_ctx* c, int32_t* plan) {
     return KA_OK;
 }
 
+int32_t ka_ctx_last_stage_plan(ka_ctx* c, int32_t* plan) {
+    if (!c || !plan) return KA_ERR_BAD_ARG;
+    for (int i = 0; i < 8; ++i) plan[i] = c->stage_plan[i];
+    return KA_OK;
+}
+
 int32_t ka_last_status(ka_ctx* c, ka_status* st) {
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     int rc = enter(c, false);
@@ -1331,9 +1357,13 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
     KaSolveParams p = stage_params(d);
     p.N = 0;
     p.blob_bytes = 0;
-    for (const BrokerTable& t : tabs) p.blob_bytes = std::max(p.blob_bytes, (int)(t.blob.size() * 2));
+    int lut_mask = 0;
+    for (const BrokerTable& t : tabs) {
+        p.blob_bytes = std::max(p.blob_bytes, (int)(t.blob.size() * 2));
+        lut_mask |= 1 << t.lut_mode;
+    }
     p.cand = cand;
-    int rc = launch_stage_plan<true>(c, s, p, pl, T, K);
+    int rc = launch_stage_plan<true>(c, s, p, pl, T, K, lut_mask);
     if (rc != KA_OK) return rc;
     if (pl.a_levels) {
         ka_level_scan_kernel<<<1, 1024, 0, s>>>(c->d_cand_ntl.as<int32_t>(), (int)kt, c->d_cand_loff.as<int32_t>());
@@ -1403,17 +1433,15 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
     if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
     if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
     if ((rc = enter(c, true)) != KA_OK) return all(rc);
-    reset_order_plan(c);
-    // the plan of the call: counter placement and loop shape from the largest table, levels if any candidate has capacity > 1
+    reset_plans(c);
+    // the plan of the call: counter placement and loop shape from the largest table, levels if any candidate that can serve
+    // the target RF has capacity > 1 (one that cannot fails alone, whatever the plan)
     std::vector<BrokerTable> tabs;
     int nmax = 0, blob_max = 0;
     candidate_tables(K, cand_off, broker_id, broker_rack, tabs, nmax, blob_max);
     int64_t capmax = 0;
     const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        if (n > 0) capmax = std::max<int64_t>(capmax, ((int64_t)P * std::max(rf_t, 0) + n - 1) / n);
-    }
+    for (int k = 0; k < K; ++k) capmax = std::max(capmax, dense_capmax(P, rf_t, cand_off[k + 1] - cand_off[k]));
     StageDesc d;
     d.T = T;
     d.Q = Q;
@@ -1446,7 +1474,7 @@ int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     cudaStream_t s = (cudaStream_t)stream;
     StageDesc& d = c->staged_block;
     c->staged = false;
-    reset_order_plan(c);
+    reset_plans(c);
     if ((rc = describe_block(c, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, 0, T, 0, d, &lst)) != KA_OK ||
         (rc = reserve_scratch(c, &d, 1)) != KA_OK)
         return rc;
@@ -1818,7 +1846,7 @@ static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, 
     const int64_t Q = sc.Q;
     if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
     if ((rc = enter(c, true)) != KA_OK) return all(rc);
-    reset_order_plan(c);
+    reset_plans(c);
     // the plan of the call: counter placement and loop shape from the largest table, the largest capacity of any candidate
     std::vector<BrokerTable> tabs;
     int nmax = 0, blob_max = 0;
