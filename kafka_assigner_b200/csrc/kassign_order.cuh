@@ -333,19 +333,22 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
             const uint32_t a0 = RC.x, a1 = RC.y, a2 = RC.z, f = RC.w;                                                           \
             const int x0 = C::ld1(C::col(cbase, ctr8, a0, 0)), x1 = C::ld1(C::col(cbase, ctr8, a1, 0)), x2 = C::ld1(C::col(cbase, ctr8, a2, 0));
 #define KA_SLOT0_DECIDE(ACTIVE, POS)                                                                                            \
-            /* strict minimum in scan order, ties to the earlier scan position: the record IS in scan order */                 \
-            const bool L10 = x1 < x0, L20 = x2 < x0, L21 = x2 < x1;                                                             \
-            const bool is2 = L10 ? L21 : L20;                                                                                   \
-            const bool is1 = L10 && !L21;                                                                                       \
-            const bool is0 = !(is1 || is2);                                                                                     \
-            const uint32_t oA = is2 ? a2 : (is1 ? a1 : a0);                                                                     \
-            const int vA = is2 ? x2 : (is1 ? x1 : x0);                                                                          \
-            /* remaining pair (p, q), p < q in scan order, and the tie-break e_pq of its slot-1 scan */                        \
-            const uint32_t op = is0 ? a1 : a0, oq = is2 ? a1 : a2;                                                              \
-            const uint32_t esh = is2 ? f : (is1 ? f >> 1 : f >> 2);                                                             \
+            /* strict minimum in scan order, ties to the earlier scan position: the record IS in scan order. Written as a   \
+               min tree (x2 wins iff it is below the winner of x0 / x1): the bump's address and value are three dependent   \
+               steps behind the loads, the rewritten record six; the level barrier waits for both (DESIGN §2 B) */          \
+            const bool L10 = x1 < x0;                                                                                       \
+            const int m01 = min(x0, x1);                                                                                    \
+            const bool is2 = x2 < m01;                                                                                      \
+            const uint32_t oA = is2 ? a2 : (L10 ? a1 : a0);                                                                 \
+            const int vA = min(m01, x2);                                                                                    \
+            /* remaining pair (p, q), p < q in scan order, and f with the tie-break e_pq of its slot-1 scan at bit 2        \
+               (e01 / e02 / e12 at bits 2 / 3 / 4 when 2 / 1 / 0 wins) */                                                   \
+            const uint32_t op = is2 ? a0 : (L10 ? a0 : a1), oq = is2 ? a1 : a2;                                             \
+            const uint32_t fz = f & 0x83u;                                                                                  \
+            const uint32_t fo = is2 ? (fz | (f & 4u)) : (L10 ? (fz | ((f >> 1) & 4u)) : (fz | ((f >> 2) & 4u)));            \
             if (ACTIVE) {                                                                                                       \
                 C::st1(C::col(cbase, ctr8, oA, 0), vA + 1);   /* counter[list[0]][0] += 1 (KAS:254-261) */                       \
-                asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(orec + (POS)), "r"(op), "r"(oq), "r"((f & 0x83u) | (esh & 4u)), "r"(oA) : "memory"); \
+                asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(orec + (POS)), "r"(op), "r"(oq), "r"(fo), "r"(oA) : "memory"); \
             }
 #define KA_SLOT1_CORE(RC, ACTIVE, POS)                                                                                          \
             const uint32_t op = RC.x, oq = RC.y, f = RC.z, oA = RC.w;                                                           \
