@@ -67,6 +67,7 @@ struct HostPinned {
 
 struct Plan {
     // kernel A
+    int a_blob_bytes;                               // shared memory for the broker blob (the largest of a batched solve)
     int a_warps, a_load_bytes, a_slab_bytes, a_cnt_bytes, a_load_kind;  // kind 0=u8 1=u16
     int a_levels;                                   // 1: some topic may hold a broker twice -> conflict levels + tables
     int lv_owner_bytes, lv_last_bytes, lv_p_bytes;  // per-warp scratch of the level pass
@@ -95,6 +96,25 @@ struct StageDesc {
     Plan pl;
 };
 
+// Records, level tables and status of one run of kernel A and the chains.
+struct RunScratch {
+    DevBuf rec, perm, ntl, lend, loff, lvl_end, tstatus, flags;
+    // rec_bytes of records, q partitions and T topics (nloff chunk-table offsets: the level tables only with levels), nflags
+    // status words.
+    cudaError_t reserve(size_t rec_bytes, size_t q, size_t T, size_t nloff, bool levels, size_t nflags) {
+        const struct { DevBuf* b; size_t bytes; } want[] = {
+            {&rec, rec_bytes}, {&perm, levels ? q * 2 : 0}, {&lend, levels ? q * 4 : 0}, {&lvl_end, levels ? q * 4 : 0},
+            {&ntl, levels ? T * 4 : 0}, {&loff, levels ? nloff * 4 : 0}, {&tstatus, T * sizeof(int4)}, {&flags, nflags * 4},
+        };
+        for (const auto& w : want)
+            if (cudaError_t e = w.b->reserve(w.bytes)) return e;
+        return cudaSuccess;
+    }
+    void release() {
+        for (DevBuf* b : {&rec, &perm, &ntl, &lend, &loff, &lvl_end, &tstatus, &flags}) b->release();
+    }
+};
+
 }  // namespace
 
 struct ka_ctx {
@@ -104,26 +124,20 @@ struct ka_ctx {
     cudaStream_t aux = nullptr;     // stage of the pipelined (super-chunk) solve
     cudaStream_t sb1 = nullptr;     // slot-0 chains (the slot-1 chains + emit run on the caller's stream)
     cudaStream_t sj = nullptr;      // device JSON emission, streamed copy-out
-    // broker table
-    int N = 0;
+    // broker table: the kernels' view of it (in d_blob, d_glut, d_broker_id; N = 0 before ka_ctx_set_brokers) and its ids
+    KaBrokers br{};
     std::vector<int32_t> broker_id;
-    int lut_mode = KA_LUT_SMEM;
-    int min_id = 0;
-    uint32_t range = 0;
-    int blob_bytes = 0;    // rack16 || lut16, staged whole into kernel A's shared memory (none before ka_ctx_set_brokers)
-    int lut_off = 0;
     DevBuf d_blob, d_glut, d_broker_id, d_ctr8;
     // counters of brokers not in the current table (Context.counter is keyed by broker id)
     std::unordered_map<int32_t, std::vector<int32_t>> parked;
     int64_t launches = 0;
     // scratch
-    DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len, d_tstatus, d_flags;
-    DevBuf d_rec, d_perm, d_ntl, d_loff, d_lend, d_lvl_end;  // records, chosen positions, schedule permutation, level tables
+    DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len;
+    RunScratch run;   // kernel A and the chains of a single solve (and of a staged block)
     DevBuf d_json, d_names, d_name_off, d_part_id, d_json_rowlen, d_json_blocksum, d_json_state;
-    // scratch of ka_solve_dense_candidates_device, apart from the single solve's: descriptors + broker tables, counters,
-    // records, level tables, status
-    DevBuf d_cand_tab, d_cand_ctr, d_cand_rec, d_cand_perm, d_cand_ntl, d_cand_lend, d_cand_loff, d_cand_lvl_end, d_cand_tstatus,
-        d_cand_flags;
+    // scratch of the batched solves, apart from the single solve's: descriptors + broker tables, counters, and the run
+    DevBuf d_cand_tab, d_cand_ctr;
+    RunScratch cand_run;
     // scratch of ka_score_candidates: row weights, the K summaries, the per-broker sums [3][ΣN], the tables' offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
     HostPinned* h_pin = nullptr;
@@ -207,10 +221,10 @@ void for_each_event(ka_ctx* c, F f) {
 
 // download current device counters into ctx->parked keyed by id
 int park_counters(ka_ctx* c) {
-    if (c->N == 0 || !c->d_ctr8.p) return KA_OK;
-    std::vector<int32_t> h((size_t)c->N * KA_MAX_SLOTS);
+    if (c->br.N == 0 || !c->d_ctr8.p) return KA_OK;
+    std::vector<int32_t> h((size_t)c->br.N * KA_MAX_SLOTS);
     KA_CUDA(cudaMemcpy(h.data(), c->d_ctr8.p, h.size() * 4, cudaMemcpyDeviceToHost));
-    for (int i = 0; i < c->N; ++i) {
+    for (int i = 0; i < c->br.N; ++i) {
         const int32_t* row = h.data() + (size_t)i * KA_MAX_SLOTS;
         bool nz = false;
         for (int r = 0; r < KA_MAX_SLOTS; ++r) nz |= row[r] != 0;
@@ -237,6 +251,11 @@ struct BrokerTable {
     int lut_mode = KA_LUT_SMEM, min_id = 0, lut_off = 0;
     uint32_t range = 0;
     std::vector<uint16_t> blob, glut;
+    int blob_bytes() const { return (int)(blob.size() * 2); }
+    // The kernels' view of this table of N brokers, uploaded to d_blob / d_glut / d_broker_id.
+    KaBrokers device(int N, const uint16_t* d_blob, const uint16_t* d_glut, const int32_t* d_broker_id) const {
+        return KaBrokers{N, lut_mode, lut_off, blob_bytes(), min_id, range, d_blob, d_glut, d_broker_id};
+    }
 };
 
 BrokerTable broker_table(int N, const int32_t* broker_id, const int32_t* broker_rack) {
@@ -286,6 +305,7 @@ int make_plan(int N, int blob_bytes, int64_t Q, int S, int Pmax, int64_t capmax,
     // A broker's load never exceeds the capacity. capmax only counts tables that can serve the target RF (dense_capmax,
     // ragged_capmax), so capmax <= Pmax; capacity > 1 turns the level pass on, whose 15-bit cursors need Pmax <= 32767. So
     // a plan that passes the level check below has capmax <= 32767, and 16-bit loads always suffice.
+    pl.a_blob_bytes = blob_bytes;
     pl.a_load_kind = capmax <= 255 ? 0 : 1;
     const int lsz = pl.a_load_kind == 0 ? 1 : 2;
     pl.a_load_bytes = (int)align16((size_t)std::max(N, 1) * lsz);
@@ -343,7 +363,8 @@ cudaError_t allow_smem(K kernel, size_t bytes) {
 }
 
 // A whole problem with its inputs on the device: dense (P partitions of RF replicas per topic), or ragged (d_part_off /
-// d_rep_off set, with Q, R, Pmax and capmax from the host-side sizing scan; a ragged problem is always one block).
+// d_rep_off set, with Q and R from the host-side sizing scan; a ragged problem is always one block). Pmax / capmax: the
+// largest topic and capacity under the broker table(s) it is solved against (dense: P and dense_capmax).
 struct Shape {
     int T = 0, P = 0, RF = 0, desired_rf = -1, S = 1;
     const int32_t* d_hash = nullptr;
@@ -362,8 +383,17 @@ int64_t dense_capmax(int P, int rf_t, int n) {
     return n > 0 && rf_t <= n ? ((int64_t)P * std::max(rf_t, 0) + n - 1) / n : 0;
 }
 
-// The planned StageDesc of topics [t0, t1) of a problem, block `blk` of its solve.
-int describe_block(ka_ctx* c, const Shape& sh, int t0, int t1, int blk, StageDesc& d, ka_status* st) {
+// A dense problem solved against one table of N brokers.
+Shape dense_shape(int T, int P, int RF, int desired_rf, int S, const int32_t* d_hash, const int32_t* d_cur, int N) {
+    Shape sh{T, P, RF, desired_rf, S, d_hash, d_cur};
+    sh.Pmax = P;
+    sh.capmax = dense_capmax(P, desired_rf >= 0 ? desired_rf : RF, N);
+    return sh;
+}
+
+// The planned StageDesc of topics [t0, t1) of a problem, block `blk` of its solve. N / blob_bytes: the broker table (the
+// largest one of a batched solve).
+int describe_block(const Shape& sh, int t0, int t1, int blk, int N, int blob_bytes, StageDesc& d, ka_status* st) {
     const bool ragged = sh.d_part_off != nullptr;
     d = StageDesc();
     d.topic_base = t0;
@@ -379,31 +409,17 @@ int describe_block(ka_ctx* c, const Shape& sh, int t0, int t1, int blk, StageDes
     d.d_cur = sh.d_cur + d.q0 * sh.RF;
     d.desired_rf = sh.desired_rf;
     d.S = sh.S;
-    if (ragged) {
-        d.Pmax = sh.Pmax;
-        d.capmax = sh.capmax;
-    } else {
-        d.Pmax = sh.P;
-        d.capmax = dense_capmax(sh.P, sh.desired_rf >= 0 ? sh.desired_rf : sh.RF, c->N);
-    }
-    return make_plan(c->N, c->blob_bytes, d.Q, d.S, d.Pmax, d.capmax, ragged, d.pl, st);
+    d.Pmax = sh.Pmax;
+    d.capmax = sh.capmax;
+    return make_plan(N, blob_bytes, d.Q, d.S, d.Pmax, d.capmax, ragged, d.pl, st);
 }
 
 // Scratch of a solve of the blocks ds[0..K) (consecutive: the last one ends the problem).
 int reserve_scratch(ka_ctx* c, const StageDesc* ds, int K) {
     const StageDesc& e = ds[K - 1];
     const size_t q = (size_t)std::max<int64_t>(e.q0 + e.Q, 1);
-    const int T = e.topic_base + e.T;
-    KA_CUDA(c->d_rec.reserve(q * ds[0].pl.rec_bytes + 256));
-    if (ds[0].pl.a_levels) {
-        KA_CUDA(c->d_perm.reserve(q * 2));
-        KA_CUDA(c->d_lend.reserve(q * 4));
-        KA_CUDA(c->d_lvl_end.reserve(q * 4));
-        KA_CUDA(c->d_ntl.reserve((size_t)std::max(T, 1) * 4));
-        KA_CUDA(c->d_loff.reserve((size_t)(std::max(T, 1) + K + 1) * 4));
-    }
-    KA_CUDA(c->d_tstatus.reserve((size_t)std::max(T, 1) * sizeof(int4)));
-    KA_CUDA(c->d_flags.reserve(64));
+    const size_t T = (size_t)std::max(e.topic_base + e.T, 1);
+    KA_CUDA(c->run.reserve(q * ds[0].pl.rec_bytes + 256, q, T, T + K + 1, ds[0].pl.a_levels, 16));
     return KA_OK;
 }
 
@@ -426,7 +442,7 @@ int reset_flags(ka_ctx* c, cudaStream_t s) {
     c->h_pin->spin_flag = -1;
     c->chain_used = 0;
     c->slot_timed[0] = c->slot_timed[1] = false;
-    KA_CUDA(cudaMemsetAsync(c->d_flags.p, 0xFF, 2 * sizeof(int), s));
+    KA_CUDA(cudaMemsetAsync(c->run.flags.p, 0xFF, 2 * sizeof(int), s));
     return KA_OK;
 }
 
@@ -498,6 +514,7 @@ KaSolveParams stage_params(const StageDesc& d) {
     p.desired_rf = d.desired_rf;
     p.S = d.S;
     p.Pmax = d.Pmax;
+    p.blob_space = d.pl.a_blob_bytes;
     p.rec_kind = d.pl.rec_kind;
     p.chunk_w = d.pl.b_threads;
     return p;
@@ -506,36 +523,28 @@ KaSolveParams stage_params(const StageDesc& d) {
 // Context-free part of a block (shards across GPUs): kernel A (records in schedule order) + the level tables.
 // a_done is recorded at the end of kernel A when timing is on.
 int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done) {
-    const int N = c->N;
     const Plan& pl = d.pl;
+    RunScratch& r = c->run;
     if (d.T > 0) {
         KaSolveParams p = stage_params(d);
-        p.N = N;
-        p.blob = c->d_blob.as<uint16_t>();
-        p.blob_bytes = c->blob_bytes;
-        p.lut_off = c->lut_off;
-        p.lut_mode = c->lut_mode;
-        p.min_id = c->min_id;
-        p.range = c->range;
-        p.glut = c->d_glut.as<uint16_t>();
-        p.broker_id = c->d_broker_id.as<int32_t>();
-        p.rec = c->d_rec.as<unsigned char>() + (size_t)d.q0 * pl.rec_bytes;
-        p.perm = pl.a_levels ? c->d_perm.as<uint16_t>() + d.q0 : nullptr;
-        p.ntl = pl.a_levels ? c->d_ntl.as<int32_t>() + d.topic_base : nullptr;
-        p.lend = pl.a_levels ? c->d_lend.as<uint32_t>() + d.q0 : nullptr;
-        p.tstatus = c->d_tstatus.as<int4>();
-        p.err_topic = c->d_flags.as<unsigned>();
-        const int rc = launch_stage_plan<false>(c, s, p, pl, d.T, 0, 1 << c->lut_mode);
+        p.br = c->br;
+        p.out.rec = r.rec.as<unsigned char>() + (size_t)d.q0 * pl.rec_bytes;
+        p.out.perm = pl.a_levels ? r.perm.as<uint16_t>() + d.q0 : nullptr;
+        p.out.ntl = pl.a_levels ? r.ntl.as<int32_t>() + d.topic_base : nullptr;
+        p.out.lend = pl.a_levels ? r.lend.as<uint32_t>() + d.q0 : nullptr;
+        p.out.tstatus = r.tstatus.as<int4>();
+        p.out.err_topic = r.flags.as<unsigned>();
+        const int rc = launch_stage_plan<false>(c, s, p, pl, d.T, 0, 1 << c->br.lut_mode);
         if (rc != KA_OK) return rc;
     }
     if (c->timing) KA_CUDA(cudaEventRecord(a_done, s));
     if (pl.a_levels && d.T > 0) {
-        int32_t* ntl = c->d_ntl.as<int32_t>() + d.topic_base;
-        int32_t* loff = c->d_loff.as<int32_t>() + d.topic_base + d.blk;  // every block keeps T_k + 1 entries
+        int32_t* ntl = r.ntl.as<int32_t>() + d.topic_base;
+        int32_t* loff = r.loff.as<int32_t>() + d.topic_base + d.blk;  // every block keeps T_k + 1 entries
         ka_level_scan_kernel<<<1, 1024, 0, s>>>(ntl, d.T, loff);
         KA_CUDA(cudaGetLastError());
-        ka_level_fill_kernel<<<(d.T + 7) / 8, 256, 0, s>>>(ntl, loff, c->d_lend.as<uint32_t>() + d.q0, d.d_part_off, d.P, d.T,
-                                                            c->d_lvl_end.as<uint32_t>() + d.q0);
+        ka_level_fill_kernel<<<(d.T + 7) / 8, 256, 0, s>>>(ntl, loff, r.lend.as<uint32_t>() + d.q0, d.d_part_off, d.P, d.T, d.T, d.Q,
+                                                            r.lvl_end.as<uint32_t>() + d.q0);
         KA_CUDA(cudaGetLastError());
         c->launches += 2;
     }
@@ -713,15 +722,15 @@ int enq_copy_out(cudaStream_t s, const SolveCall& io, int S, int64_t r0, int64_t
 KaOrderParams order_params(ka_ctx* c, const StageDesc& d, const SubBlock& b) {
     const Plan& pl = d.pl;
     KaOrderParams o{};
-    o.N = c->N;
+    o.N = c->br.N;
     o.S = d.S;
     o.uniform_width = pl.a_levels ? 0u : (uint32_t)d.P;
-    o.chunk_end = pl.a_levels ? c->d_lvl_end.as<uint32_t>() + d.q0 : nullptr;
+    o.chunk_end = pl.a_levels ? c->run.lvl_end.as<uint32_t>() + d.q0 : nullptr;
     o.ctr8 = c->d_ctr8.as<int32_t>();
     o.ring_log2 = pl.b_ring_log2;
-    const int32_t* loff = pl.a_levels ? c->d_loff.as<int32_t>() + d.topic_base + d.blk : nullptr;
+    const int32_t* loff = pl.a_levels ? c->run.loff.as<int32_t>() + d.topic_base + d.blk : nullptr;
     o.Q = (uint32_t)b.rq;
-    o.rec = c->d_rec.as<unsigned char>() + (size_t)(d.q0 + b.r0) * pl.rec_bytes;
+    o.rec = c->run.rec.as<unsigned char>() + (size_t)(d.q0 + b.r0) * pl.rec_bytes;
     o.pos_base = (uint32_t)b.r0;
     o.chunk_lo_ptr = loff ? loff + b.t0 : nullptr;
     o.chunk_hi_ptr = loff ? loff + b.t1 : nullptr;
@@ -731,7 +740,7 @@ KaOrderParams order_params(ka_ctx* c, const StageDesc& d, const SubBlock& b) {
 // One slot chain (rows <= 3) over sub-block j of a staged block.
 int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int j, int nsub) {
     const SubBlock b = sub_block(d, j, nsub);
-    if (b.rq <= 0 || c->N <= 0) return KA_OK;
+    if (b.rq <= 0 || c->br.N <= 0) return KA_OK;
     const KaOrderParams o = order_params(c, d, b);
     int sel = 0;
     KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, d.pl, &sel) : launch_order<1, 1024>(s, o, d.pl, &sel)));
@@ -744,10 +753,10 @@ int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int 
 int enq_emit_block(ka_ctx* c, cudaStream_t s, const StageDesc& d, int j, int nsub, int32_t* d_out, int32_t* d_out_len) {
     const Plan& pl = d.pl;
     const SubBlock b = sub_block(d, j, nsub);
-    if (b.rq <= 0 || c->N <= 0) return KA_OK;
+    if (b.rq <= 0 || c->br.N <= 0) return KA_OK;
     ka_emit3_kernel<<<(unsigned)((b.rq + 255) / 256), 256, 0, s>>>(
-        reinterpret_cast<const uint4*>(c->d_rec.as<unsigned char>() + (size_t)(d.q0 + b.r0) * pl.rec_bytes),
-        pl.a_levels ? c->d_perm.as<uint16_t>() + d.q0 + b.r0 : nullptr, d.d_part_off, b.t1 - b.t0, d.P, c->d_broker_id.as<int32_t>(),
+        reinterpret_cast<const uint4*>(c->run.rec.as<unsigned char>() + (size_t)(d.q0 + b.r0) * pl.rec_bytes),
+        pl.a_levels ? c->run.perm.as<uint16_t>() + d.q0 + b.r0 : nullptr, d.d_part_off, b.t1 - b.t0, d.P, c->d_broker_id.as<int32_t>(),
         (uint32_t)b.rq, d.S, d_out + (size_t)b.r0 * d.S, d_out_len ? d_out_len + b.r0 : nullptr, c->d_ctr8.as<int32_t>());
     KA_CUDA(cudaGetLastError());
     c->launches++;
@@ -760,7 +769,7 @@ int enq_emit_block(ka_ctx* c, cudaStream_t s, const StageDesc& d, int j, int nsu
 int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io, int blocks_in_solve) {
     const int S = d.S;
     const Plan& pl = d.pl;
-    if (d.Q <= 0 || c->N <= 0) return io.json && d.d_part_off && d.Q == 0 ? enq_json(c, s, io, d, sub_block(d, 0, 1), true, true) : KA_OK;
+    if (d.Q <= 0 || c->br.N <= 0) return io.json && d.d_part_off && d.Q == 0 ? enq_json(c, s, io, d, sub_block(d, 0, 1), true, true) : KA_OK;
     int32_t* d_out = io.d_out + d.q0 * S;
     int32_t* d_out_len = io.d_out_len ? io.d_out_len + d.q0 : nullptr;
     if (pl.rec_kind != 3) {  // rows of 4..8: one fused chain over all slots, rows written by the kernel
@@ -819,7 +828,7 @@ int chain_fork(ka_ctx* c, cudaStream_t s) {
 
 // End of a solve on `s`: status words back to pinned host memory (async), end of the timed span.
 int enq_solve_end(ka_ctx* c, cudaStream_t s) {
-    KA_CUDA(cudaMemcpyAsync(&c->h_pin->err_topic, c->d_flags.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
+    KA_CUDA(cudaMemcpyAsync(&c->h_pin->err_topic, c->run.flags.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));
     if (c->timing) {
         KA_CUDA(cudaEventRecord(c->ev[5], s));
         c->ev_valid = true;
@@ -869,7 +878,7 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
     StageDesc ds[KA_MAX_BLOCKS];
     int rc;
     for (int k = 0; k < K; ++k)
-        if ((rc = describe_block(c, sh, bound(k), bound(k + 1), k, ds[k], st)) != KA_OK) return rc;
+        if ((rc = describe_block(sh, bound(k), bound(k + 1), k, c->br.N, c->br.blob_bytes, ds[k], st)) != KA_OK) return rc;
     if ((rc = reserve_scratch(c, ds, K)) != KA_OK) return rc;
     c->last_stages = K;
     if (c->timing) KA_CUDA(cudaEventRecord(c->ev[0], s));
@@ -883,7 +892,7 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
         if ((rc = chain_fork(c, s)) != KA_OK) return rc;
         if ((rc = enq_order_emit(c, s, d, io, 1)) != KA_OK) return rc;
         if (c->timing) KA_CUDA(cudaEventRecord(c->ev[4], s));
-        if (io.h_out && d.Q > 0 && c->N > 0 && (rc = enq_copy_out(s, io, d.S, 0, d.Q)) != KA_OK) return rc;
+        if (io.h_out && d.Q > 0 && c->br.N > 0 && (rc = enq_copy_out(s, io, d.S, 0, d.Q)) != KA_OK) return rc;
     } else {
         cudaStream_t aux = c->aux;
         io.stream_out = io.h_out && ds[0].pl.rec_kind == 3 && !io.json;
@@ -905,7 +914,7 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
             if ((rc = enq_order_emit(c, s, d, io, K)) != KA_OK) return rc;
             if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][4], s));
             // rows of 4..8: one copy per block on the caller's stream
-            if (io.h_out && !io.stream_out && d.Q > 0 && c->N > 0 && (rc = enq_copy_out(s, io, d.S, d.q0, d.Q)) != KA_OK) return rc;
+            if (io.h_out && !io.stream_out && d.Q > 0 && c->br.N > 0 && (rc = enq_copy_out(s, io, d.S, d.q0, d.Q)) != KA_OK) return rc;
         }
         if (io.stream_out) {   // join the copy-out stream back into the caller's stream
             KA_CUDA(cudaEventRecord(c->ev_out_done, c->sj));
@@ -915,25 +924,25 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
     return enq_solve_end(c, s);
 }
 
-// Wait for the stream, translate device flags into a ka_status. part_id / part_off (ragged host-buffer solve): the
-// reported partition is the failing partition's id rather than its ordinal inside the topic.
+// The status a run reports for its lowest failing topic t, whose tstatus entry is ts. part_id / part_off (ragged
+// host-buffer solve): the reported partition is the failing partition's id rather than its ordinal inside the topic.
+ka_status topic_status(int t, const int4& ts, const int32_t* part_id, const int64_t* part_off) {
+    ka_status r;
+    set_status(&r, ts.x, t, ts.y >= 0 && part_id && part_off ? part_id[part_off[t] + ts.y] : ts.y, ts.z, ts.w);
+    return r;
+}
+
+// Wait for the stream, translate device flags into a ka_status. part_id / part_off: as in topic_status.
 int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st, const int32_t* part_id = nullptr, const int64_t* part_off = nullptr) {
     KA_CUDA(cudaStreamSynchronize(s));
     c->pending_status = false;
     ka_status r{};
-    r.code = KA_OK;
-    r.topic_index = -1;
-    r.partition = -1;
+    set_status(&r, KA_OK);
     if (c->h_pin->err_topic != -1) {
         const int t = c->h_pin->err_topic;
-        KA_CUDA(cudaMemcpy(&c->h_pin->tstatus, c->d_tstatus.as<int4>() + t, sizeof(int4), cudaMemcpyDeviceToHost));
-        r.code = c->h_pin->tstatus.x;
-        r.topic_index = t + (c->last_was_staged ? c->topic_base : 0);
-        int ord = c->h_pin->tstatus.y;
-        r.partition = ord;
-        if (ord >= 0 && part_id && part_off) r.partition = part_id[part_off[t] + ord];
-        r.a = c->h_pin->tstatus.z;
-        r.b = c->h_pin->tstatus.w;
+        KA_CUDA(cudaMemcpy(&c->h_pin->tstatus, c->run.tstatus.as<int4>() + t, sizeof(int4), cudaMemcpyDeviceToHost));
+        r = topic_status(t, c->h_pin->tstatus, part_id, part_off);
+        r.topic_index += c->last_was_staged ? c->topic_base : 0;
     }
     if (c->timing && c->ev_valid) {
         for (int i = 0; i < 8; ++i) c->last_ms[i] = 0.f;
@@ -989,6 +998,92 @@ int finish(ka_ctx* c, cudaStream_t s, ka_status* st, bool sync, const int32_t* p
     c->last_stream = s;
     c->pending_status = true;
     return st || sync ? finish_status(c, s, st, part_id, part_off) : KA_OK;
+}
+
+// A library-side failure of a batched solve: every candidate reports it.
+int fail_candidates(ka_status* st, int K, int rc) {
+    for (int k = 0; k < K; ++k) set_status(st + k, rc);
+    return rc;
+}
+
+// A batched solve failed with rc after part of it was enqueued on `s` (slot-0 chains on c->sb1): wait for what was enqueued,
+// then every candidate reports rc.
+int abort_candidates(ka_ctx* c, cudaStream_t s, ka_status* st, int K, int rc) {
+    cudaStreamSynchronize(c->sb1);
+    cudaStreamSynchronize(s);
+    return fail_candidates(st, K, rc);
+}
+
+// What ka_ctx_set_brokers refuses in any of the K candidate tables of a batched solve (the same code).
+int check_candidates(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack) {
+    if (!cand_off || cand_off[0] != 0) return KA_ERR_BAD_ARG;
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        if (cand_off[k + 1] < cand_off[k] || (n > 0 && (!broker_id || !broker_rack))) return KA_ERR_BAD_ARG;
+        const int rc = n > 0 ? check_brokers(n, broker_id + cand_off[k], broker_rack + cand_off[k]) : KA_OK;
+        if (rc != KA_OK) return rc;
+    }
+    return KA_OK;
+}
+
+// The device images of the candidate tables of a batched solve, and what the call's plan takes from them: counter placement
+// and loop shape from the largest table and blob, levels and load width from the largest capacity of any candidate.
+struct CandidateTables {
+    std::vector<BrokerTable> tabs;
+    int nmax = 0, blob_max = 0;
+    int64_t capmax = 0;
+};
+
+// The common part of the candidate front ends, once their own checks have passed (the tables are checked and the problem of
+// Q rows per candidate is sized): the K·Q limit, the ctx's device and the candidates' tables. cap(n, capmax) gives the largest
+// capacity of the problem under a table of n brokers, or the status that table fails with.
+template <typename Cap>
+int candidate_tables(ka_ctx* c, int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack, int64_t Q,
+                     Cap cap, CandidateTables& ct, ka_status* st) {
+    if ((int64_t)K * Q >= ((int64_t)1 << 31)) return fail_candidates(st, K, KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
+    int rc = enter(c, true);
+    if (rc != KA_OK) return fail_candidates(st, K, rc);
+    reset_plans(c);
+    ct.tabs.resize(K);
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        ct.tabs[k] = broker_table(n, broker_id + cand_off[k], broker_rack + cand_off[k]);
+        ct.nmax = std::max(ct.nmax, n);
+        ct.blob_max = std::max(ct.blob_max, ct.tabs[k].blob_bytes());
+        int64_t capk = 0;
+        if ((rc = cap(n, capk)) != KA_OK) return fail_candidates(st, K, rc);
+        ct.capmax = std::max(ct.capmax, capk);
+    }
+    return KA_OK;
+}
+
+// The plan of a batched solve of the problem sh (one block) under the tables ct: a limit it exceeds fails every candidate alike.
+int plan_candidates(const Shape& sh, const CandidateTables& ct, int K, StageDesc& d, ka_status* st) {
+    const int rc = describe_block(sh, 0, sh.T, 0, ct.nmax, ct.blob_max, d, st);
+    for (int k = 1; k < K && rc != KA_OK; ++k) st[k] = st[0];
+    return rc;
+}
+
+// Wait for a batched solve enqueued on `s` and fill every candidate's status: its lowest failing topic, as finish_status
+// reports it for one solve (part_id / part_off of a ragged solve: the failing partition's id). Returns the code of the
+// lowest failing candidate.
+int finish_candidates(ka_ctx* c, cudaStream_t s, int K, int T, ka_status* st, const int32_t* part_id = nullptr,
+                      const int64_t* part_off = nullptr) {
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail_candidates(st, K, KA_ERR_CUDA);
+    std::vector<unsigned> err(K);
+    if (cudaMemcpy(err.data(), c->cand_run.flags.p, (size_t)K * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return fail_candidates(st, K, KA_ERR_CUDA);
+    int first = KA_OK;
+    for (int k = 0; k < K; ++k) {
+        if (err[k] == 0xFFFFFFFFu) continue;
+        const int t = (int)err[k];
+        int4 ts;
+        if (cudaMemcpy(&ts, c->cand_run.tstatus.as<int4>() + (size_t)k * T + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
+            return fail_candidates(st, K, KA_ERR_CUDA);
+        st[k] = topic_status(t, ts, part_id, part_off);
+        if (first == KA_OK) first = ts.x;
+    }
+    return first;
 }
 
 }  // namespace
@@ -1070,12 +1165,12 @@ void ka_ctx_destroy(ka_ctx* c) {
     for (cudaStream_t s : {c->stream, c->aux, c->sb1, c->sj})
         if (s) cudaStreamSynchronize(s);
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
-                      &c->d_out, &c->d_out_len, &c->d_tstatus, &c->d_flags, &c->d_rec, &c->d_perm, &c->d_ntl, &c->d_loff, &c->d_lend,
-                      &c->d_lvl_end, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen, &c->d_json_blocksum,
-                      &c->d_json_state, &c->d_cand_tab, &c->d_cand_ctr, &c->d_cand_rec, &c->d_cand_perm, &c->d_cand_ntl,
-                      &c->d_cand_lend, &c->d_cand_loff, &c->d_cand_lvl_end, &c->d_cand_tstatus, &c->d_cand_flags, &c->d_score_w,
-                      &c->d_score_sum, &c->d_score_brk, &c->d_score_off})
+                      &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
+                      &c->d_json_blocksum, &c->d_json_state, &c->d_cand_tab, &c->d_cand_ctr, &c->d_score_w, &c->d_score_sum,
+                      &c->d_score_brk, &c->d_score_off})
         b->release();
+    c->run.release();
+    c->cand_run.release();
     for_each_event(c, [](cudaEvent_t& e, bool) {
         if (e) cudaEventDestroy(e);
     });
@@ -1091,7 +1186,7 @@ int32_t ka_ctx_reset(ka_ctx* c) {
     int rc = enter(c, true);   // do not race an in-flight asynchronous solve
     if (rc != KA_OK) return rc;
     c->parked.clear();
-    if (c->N > 0 && c->d_ctr8.p) KA_CUDA(cudaMemset(c->d_ctr8.p, 0, (size_t)c->N * KA_MAX_SLOTS * 4));
+    if (c->br.N > 0 && c->d_ctr8.p) KA_CUDA(cudaMemset(c->d_ctr8.p, 0, (size_t)c->br.N * KA_MAX_SLOTS * 4));
     return KA_OK;
 }
 
@@ -1101,22 +1196,17 @@ int32_t ka_ctx_set_brokers(ka_ctx* c, int32_t N, const int32_t* broker_id, const
     if (rc != KA_OK) return rc;
     if ((rc = enter(c, true)) != KA_OK || (rc = park_counters(c)) != KA_OK) return rc;
 
-    c->N = N;
-    c->broker_id.assign(broker_id, broker_id + N);
     const BrokerTable t = broker_table(N, broker_id, broker_rack);
-    c->min_id = t.min_id;
-    c->lut_mode = t.lut_mode;
-    c->range = t.range;
     if (t.lut_mode == KA_LUT_GLOBAL) {
         KA_CUDA(c->d_glut.reserve(t.glut.size() * 2));
         KA_CUDA(cudaMemcpy(c->d_glut.p, t.glut.data(), t.glut.size() * 2, cudaMemcpyHostToDevice));
     }
-    c->lut_off = t.lut_off;
-    c->blob_bytes = (int)(t.blob.size() * 2);
     KA_CUDA(c->d_blob.reserve(t.blob.size() * 2));
     KA_CUDA(cudaMemcpy(c->d_blob.p, t.blob.data(), t.blob.size() * 2, cudaMemcpyHostToDevice));
     KA_CUDA(c->d_broker_id.reserve((size_t)std::max(N, 1) * 4));
     if (N > 0) KA_CUDA(cudaMemcpy(c->d_broker_id.p, broker_id, (size_t)N * 4, cudaMemcpyHostToDevice));
+    c->br = t.device(N, c->d_blob.as<uint16_t>(), c->d_glut.as<uint16_t>(), c->d_broker_id.as<int32_t>());
+    c->broker_id.assign(broker_id, broker_id + N);
     // counters for the new table
     std::vector<int32_t> h((size_t)(std::max(N, 1) + 1) * KA_MAX_SLOTS, 0);  // + the order kernel's dummy row (index N)
     for (int i = 0; i < N; ++i) {
@@ -1135,7 +1225,7 @@ int32_t ka_ctx_get_counters(ka_ctx* c, int32_t* counter) {
     if (!counter) return KA_ERR_BAD_ARG;
     int rc = enter(c, true);
     if (rc != KA_OK) return rc;
-    if (c->N > 0) KA_CUDA(cudaMemcpy(counter, c->d_ctr8.p, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToHost));
+    if (c->br.N > 0) KA_CUDA(cudaMemcpy(counter, c->d_ctr8.p, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToHost));
     return KA_OK;
 }
 
@@ -1144,7 +1234,7 @@ int32_t ka_ctx_set_counters(ka_ctx* c, const int32_t* counter) {
     if (!counter) return KA_ERR_BAD_ARG;
     int rc = enter(c, true);
     if (rc != KA_OK) return rc;
-    if (c->N > 0) KA_CUDA(cudaMemcpy(c->d_ctr8.p, counter, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyHostToDevice));
+    if (c->br.N > 0) KA_CUDA(cudaMemcpy(c->d_ctr8.p, counter, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyHostToDevice));
     return KA_OK;
 }
 
@@ -1153,8 +1243,8 @@ int32_t ka_ctx_export_counters_device(ka_ctx* c, int32_t* d_counter, void* strea
     if (!d_counter) return KA_ERR_BAD_ARG;
     int rc = enter(c, false);
     if (rc != KA_OK) return rc;
-    if (c->N > 0)
-        KA_CUDA(cudaMemcpyAsync(d_counter, c->d_ctr8.p, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    if (c->br.N > 0)
+        KA_CUDA(cudaMemcpyAsync(d_counter, c->d_ctr8.p, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return KA_OK;
 }
 
@@ -1163,8 +1253,8 @@ int32_t ka_ctx_import_counters_device(ka_ctx* c, const int32_t* d_counter, void*
     if (!d_counter) return KA_ERR_BAD_ARG;
     int rc = enter(c, false);
     if (rc != KA_OK) return rc;
-    if (c->N > 0)
-        KA_CUDA(cudaMemcpyAsync(c->d_ctr8.p, d_counter, (size_t)c->N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+    if (c->br.N > 0)
+        KA_CUDA(cudaMemcpyAsync(c->d_ctr8.p, d_counter, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
     return KA_OK;
 }
 
@@ -1210,7 +1300,7 @@ static int validate_dense(ka_ctx* c, int32_t T, int32_t P, int32_t RF, int32_t d
     if (T < 0 || P < 0 || RF < 0) return set_status(st, KA_ERR_BAD_ARG);
     if (S < 1 || S > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
     const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    if (S < RF || (rf_t <= c->N && S < rf_t)) return set_status(st, KA_ERR_BAD_ARG, -1, -1, S);
+    if (S < RF || (rf_t <= c->br.N && S < rf_t)) return set_status(st, KA_ERR_BAD_ARG, -1, -1, S);
     return KA_OK;
 }
 
@@ -1223,62 +1313,9 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     SolveCall io;
     io.d_out = d_out_broker;
     io.d_out_len = d_out_len;
-    if ((rc = enter(c, true)) != KA_OK || (rc = run_solve(c, s, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, io, st)) != KA_OK)
-        return failed(st, rc);
+    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker, c->br.N);
+    if ((rc = enter(c, true)) != KA_OK || (rc = run_solve(c, s, sh, io, st)) != KA_OK) return failed(st, rc);
     return finish(c, s, st, false);
-}
-
-// A library-side failure of a batched solve: every candidate reports it.
-static int fail_candidates(ka_status* st, int K, int rc) {
-    for (int k = 0; k < K; ++k) set_status(st + k, rc);
-    return rc;
-}
-
-// What ka_ctx_set_brokers refuses in any of the K candidate tables of a batched solve (the same code).
-static int check_candidates(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack) {
-    if (!cand_off || cand_off[0] != 0) return KA_ERR_BAD_ARG;
-    for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        if (cand_off[k + 1] < cand_off[k] || (n > 0 && (!broker_id || !broker_rack))) return KA_ERR_BAD_ARG;
-        const int rc = n > 0 ? check_brokers(n, broker_id + cand_off[k], broker_rack + cand_off[k]) : KA_OK;
-        if (rc != KA_OK) return rc;
-    }
-    return KA_OK;
-}
-
-// The device images of the (checked) candidate tables; nmax / blob_max: the largest table and blob (the call's plan).
-static void candidate_tables(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
-                             std::vector<BrokerTable>& tabs, int& nmax, int& blob_max) {
-    tabs.resize(K);
-    for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        tabs[k] = broker_table(n, broker_id + cand_off[k], broker_rack + cand_off[k]);
-        nmax = std::max(nmax, n);
-        blob_max = std::max(blob_max, (int)(tabs[k].blob.size() * 2));
-    }
-}
-
-// Wait for a batched solve enqueued on `s` and fill every candidate's status: its lowest failing topic, as finish_status
-// reports it for one solve (part_id / part_off of a ragged solve: the failing partition's id). Returns the code of the
-// lowest failing candidate.
-static int finish_candidates(ka_ctx* c, cudaStream_t s, int K, int T, ka_status* st, const int32_t* part_id = nullptr,
-                             const int64_t* part_off = nullptr) {
-    if (cudaStreamSynchronize(s) != cudaSuccess) return fail_candidates(st, K, KA_ERR_CUDA);
-    std::vector<unsigned> err(K);
-    if (cudaMemcpy(err.data(), c->d_cand_flags.p, (size_t)K * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
-        return fail_candidates(st, K, KA_ERR_CUDA);
-    int first = KA_OK;
-    for (int k = 0; k < K; ++k) {
-        if (err[k] == 0xFFFFFFFFu) continue;
-        const int t = (int)err[k];
-        int4 ts;
-        if (cudaMemcpy(&ts, c->d_cand_tstatus.as<int4>() + (size_t)k * T + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
-            return fail_candidates(st, K, KA_ERR_CUDA);
-        const int part = ts.y >= 0 && part_id && part_off ? part_id[part_off[t] + ts.y] : ts.y;
-        set_status(st + k, ts.x, t, part, ts.z, ts.w);
-        if (first == KA_OK) first = ts.x;
-    }
-    return first;
 }
 
 // Everything of a batched solve over K candidate tables, enqueued on `s` (slot-0 chains on c->sb1): the candidates' tables
@@ -1306,76 +1343,50 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
         ctr_off[k] = ctr_ints;
         ctr_ints += (size_t)(n + 1) * KA_MAX_SLOTS;   // + the chains' dummy row
     }
+    RunScratch& r = c->cand_run;
     KA_CUDA(c->d_cand_tab.reserve(bytes));
     KA_CUDA(c->d_cand_ctr.reserve(ctr_ints * 4));
-    KA_CUDA(c->d_cand_rec.reserve(kq * 16));
-    if (pl.a_levels) {
-        KA_CUDA(c->d_cand_perm.reserve(kq * 2));
-        KA_CUDA(c->d_cand_lend.reserve(kq * 4));
-        KA_CUDA(c->d_cand_lvl_end.reserve(kq * 4));
-        KA_CUDA(c->d_cand_ntl.reserve(kt * 4));
-        KA_CUDA(c->d_cand_loff.reserve((kt + 1) * 4));
-    }
-    KA_CUDA(c->d_cand_tstatus.reserve(kt * sizeof(int4)));
-    KA_CUDA(c->d_cand_flags.reserve((size_t)K * 4));
+    KA_CUDA(r.reserve(kq * 16, kq, kt, kt + 1, pl.a_levels, K));
     unsigned char* base = c->d_cand_tab.as<unsigned char>();
     std::vector<unsigned char> h(bytes, 0);
+    int lut_mask = 0;
     for (int k = 0; k < K; ++k) {
         const int n = cand_off[k + 1] - cand_off[k];
         const BrokerTable& t = tabs[k];
         KaCandidate e{};
-        e.N = n;
-        e.lut_mode = t.lut_mode;
-        e.lut_off = t.lut_off;
-        e.blob_bytes = (int)(t.blob.size() * 2);
-        e.min_id = t.min_id;
-        e.range = t.range;
-        e.blob = reinterpret_cast<const uint16_t*>(base + blob_off[k]);
-        e.glut = reinterpret_cast<const uint16_t*>(base + glut_off[k]);
-        e.broker_id = reinterpret_cast<const int32_t*>(base + bid_off[k]);
+        e.br = t.device(n, reinterpret_cast<const uint16_t*>(base + blob_off[k]), reinterpret_cast<const uint16_t*>(base + glut_off[k]),
+                        reinterpret_cast<const int32_t*>(base + bid_off[k]));
         e.ctr8 = c->d_cand_ctr.as<int32_t>() + ctr_off[k];
-        e.rec = c->d_cand_rec.as<unsigned char>() + (size_t)k * q * 16;
+        e.out.rec = r.rec.as<unsigned char>() + (size_t)k * q * 16;
         if (pl.a_levels) {
-            e.perm = c->d_cand_perm.as<uint16_t>() + (size_t)k * q;
-            e.ntl = c->d_cand_ntl.as<int32_t>() + (size_t)k * T;
-            e.lend = c->d_cand_lend.as<uint32_t>() + (size_t)k * q;
-            e.loff = c->d_cand_loff.as<int32_t>() + (size_t)k * T;
+            e.out.perm = r.perm.as<uint16_t>() + (size_t)k * q;
+            e.out.ntl = r.ntl.as<int32_t>() + (size_t)k * T;
+            e.out.lend = r.lend.as<uint32_t>() + (size_t)k * q;
+            e.loff = r.loff.as<int32_t>() + (size_t)k * T;
             e.pos0 = (uint32_t)((size_t)k * Q);   // the level tables of the K candidates are one table of K * T topics
         }
-        e.tstatus = c->d_cand_tstatus.as<int4>() + (size_t)k * T;
-        e.err_topic = c->d_cand_flags.as<unsigned>() + k;
+        e.out.tstatus = r.tstatus.as<int4>() + (size_t)k * T;
+        e.out.err_topic = r.flags.as<unsigned>() + k;
         std::memcpy(h.data() + (size_t)k * sizeof(KaCandidate), &e, sizeof(e));
         std::memcpy(h.data() + blob_off[k], t.blob.data(), t.blob.size() * 2);
         if (!t.glut.empty()) std::memcpy(h.data() + glut_off[k], t.glut.data(), t.glut.size() * 2);
         if (n > 0) std::memcpy(h.data() + bid_off[k], broker_id + cand_off[k], (size_t)n * 4);
+        lut_mask |= 1 << t.lut_mode;
     }
     const KaCandidate* cand = c->d_cand_tab.as<KaCandidate>();
     KA_CUDA(cudaMemcpyAsync(base, h.data(), bytes, cudaMemcpyHostToDevice, s));
     KA_CUDA(cudaMemsetAsync(c->d_cand_ctr.p, 0, ctr_ints * 4, s));   // every candidate starts from a fresh Context
-    KA_CUDA(cudaMemsetAsync(c->d_cand_flags.p, 0xFF, (size_t)K * 4, s));
-    // kernel A: grid.y = candidate; the shared-memory layout is that of the largest table
+    KA_CUDA(cudaMemsetAsync(r.flags.p, 0xFF, (size_t)K * 4, s));
+    // kernel A: grid.y = candidate; the plan's shared-memory layout is that of the largest table
     KaSolveParams p = stage_params(d);
-    p.N = 0;
-    p.blob_bytes = 0;
-    int lut_mask = 0;
-    for (const BrokerTable& t : tabs) {
-        p.blob_bytes = std::max(p.blob_bytes, (int)(t.blob.size() * 2));
-        lut_mask |= 1 << t.lut_mode;
-    }
     p.cand = cand;
     int rc = launch_stage_plan<true>(c, s, p, pl, T, K, lut_mask);
     if (rc != KA_OK) return rc;
     if (pl.a_levels) {
-        ka_level_scan_kernel<<<1, 1024, 0, s>>>(c->d_cand_ntl.as<int32_t>(), (int)kt, c->d_cand_loff.as<int32_t>());
+        ka_level_scan_kernel<<<1, 1024, 0, s>>>(r.ntl.as<int32_t>(), (int)kt, r.loff.as<int32_t>());
         KA_CUDA(cudaGetLastError());
-        if (d.d_part_off)
-            ka_level_fill_candidates_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(
-                c->d_cand_ntl.as<int32_t>(), c->d_cand_loff.as<int32_t>(), c->d_cand_lend.as<uint32_t>(), d.d_part_off, T, (int)kt, Q,
-                c->d_cand_lvl_end.as<uint32_t>());
-        else
-            ka_level_fill_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(c->d_cand_ntl.as<int32_t>(), c->d_cand_loff.as<int32_t>(),
-                                                                          c->d_cand_lend.as<uint32_t>(), nullptr, d.P, (int)kt,
-                                                                          c->d_cand_lvl_end.as<uint32_t>());
+        ka_level_fill_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(r.ntl.as<int32_t>(), r.loff.as<int32_t>(), r.lend.as<uint32_t>(),
+                                                                      d.d_part_off, d.P, T, (int)kt, Q, r.lvl_end.as<uint32_t>());
         KA_CUDA(cudaGetLastError());
         c->launches += 2;
     }
@@ -1389,7 +1400,7 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
         o.N = 0;
         o.S = S;
         o.uniform_width = pl.a_levels ? 0u : (uint32_t)d.P;
-        o.chunk_end = pl.a_levels ? c->d_cand_lvl_end.as<uint32_t>() : nullptr;
+        o.chunk_end = pl.a_levels ? r.lvl_end.as<uint32_t>() : nullptr;
         o.ring_log2 = pl.b_ring_log2;
         o.Q = (uint32_t)b.rq;
         o.pos_base = (uint32_t)b.r0;
@@ -1431,38 +1442,22 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
     if (T == 0) return KA_OK;
     const int64_t Q = (int64_t)T * P;
     if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
-    if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
-    if ((rc = enter(c, true)) != KA_OK) return all(rc);
-    reset_plans(c);
-    // the plan of the call: counter placement and loop shape from the largest table, levels if any candidate that can serve
-    // the target RF has capacity > 1 (one that cannot fails alone, whatever the plan)
-    std::vector<BrokerTable> tabs;
-    int nmax = 0, blob_max = 0;
-    candidate_tables(K, cand_off, broker_id, broker_rack, tabs, nmax, blob_max);
-    int64_t capmax = 0;
+    // levels if any candidate that can serve the target RF has capacity > 1 (one that cannot fails alone, whatever the plan)
     const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    for (int k = 0; k < K; ++k) capmax = std::max(capmax, dense_capmax(P, rf_t, cand_off[k + 1] - cand_off[k]));
+    auto cap = [&](int n, int64_t& capmax) {
+        capmax = dense_capmax(P, rf_t, n);
+        return KA_OK;
+    };
+    CandidateTables ct;
+    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, Q, cap, ct, st)) != KA_OK) return rc;
+    Shape sh{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker};
+    sh.Pmax = P;
+    sh.capmax = ct.capmax;
     StageDesc d;
-    d.T = T;
-    d.Q = Q;
-    d.d_hash = d_topic_hash;
-    d.P = P;
-    d.RF = RF;
-    d.d_cur = d_cur_broker;
-    d.desired_rf = desired_rf;
-    d.S = out_stride;
-    d.Pmax = P;
-    d.capmax = capmax;
-    if ((rc = make_plan(nmax, blob_max, Q, out_stride, P, capmax, false, d.pl, st)) != KA_OK) {
-        for (int k = 1; k < K; ++k) st[k] = st[0];
-        return rc;
-    }
+    if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    if ((rc = enq_candidates(c, s, K, tabs, cand_off, broker_id, d, d_out_len, d_out_broker)) != KA_OK) {
-        cudaStreamSynchronize(c->sb1);
-        cudaStreamSynchronize(s);
-        return all(rc);
-    }
+    if ((rc = enq_candidates(c, s, K, ct.tabs, cand_off, broker_id, d, d_out_len, d_out_broker)) != KA_OK)
+        return abort_candidates(c, s, st, K, rc);
     return finish_candidates(c, s, K, T, st);
 }
 
@@ -1475,7 +1470,8 @@ int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     StageDesc& d = c->staged_block;
     c->staged = false;
     reset_plans(c);
-    if ((rc = describe_block(c, Shape{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker}, 0, T, 0, d, &lst)) != KA_OK ||
+    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker, c->br.N);
+    if ((rc = describe_block(sh, 0, T, 0, c->br.N, c->br.blob_bytes, d, &lst)) != KA_OK ||
         (rc = reserve_scratch(c, &d, 1)) != KA_OK)
         return rc;
     c->last_stages = 1;
@@ -1545,10 +1541,10 @@ static int copy_counter_column(ka_ctx* c, int slot, int32_t* d_col, const int32_
     if (slot < 0 || slot >= KA_MAX_SLOTS || (!d_col && !d_src)) return KA_ERR_BAD_ARG;
     int rc = enter(c, false);
     if (rc != KA_OK) return rc;
-    if (c->N <= 0) return KA_OK;
+    if (c->br.N <= 0) return KA_OK;
     int32_t* col = c->d_ctr8.as<int32_t>() + slot;
-    if (d_col) KA_CUDA(cudaMemcpy2DAsync(d_col, 4, col, KA_MAX_SLOTS * 4, 4, (size_t)c->N, cudaMemcpyDeviceToDevice, s));
-    else KA_CUDA(cudaMemcpy2DAsync(col, KA_MAX_SLOTS * 4, d_src, 4, 4, (size_t)c->N, cudaMemcpyDeviceToDevice, s));
+    if (d_col) KA_CUDA(cudaMemcpy2DAsync(d_col, 4, col, KA_MAX_SLOTS * 4, 4, (size_t)c->br.N, cudaMemcpyDeviceToDevice, s));
+    else KA_CUDA(cudaMemcpy2DAsync(col, KA_MAX_SLOTS * 4, d_src, 4, 4, (size_t)c->br.N, cudaMemcpyDeviceToDevice, s));
     return KA_OK;
 }
 
@@ -1583,7 +1579,7 @@ int32_t ka_solve_dense(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t 
     io.d_out_len = c->d_out_len.as<int32_t>();
     io.h_out = out_broker;
     io.h_out_len = out_len;
-    const Shape sh{T, P, RF, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>()};
+    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->br.N);
     if ((rc = run_solve(c, c->stream, sh, io, st)) != KA_OK) return failed(st, rc);
     return finish(c, c->stream, st, true);
 }
@@ -1656,8 +1652,8 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     io.d_out = c->d_out.as<int32_t>();
     io.d_out_len = c->d_out_len.as<int32_t>();
     io.json = true;
-    const Shape sh{T, P, RF, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>()};
-    rc = T > 0 && c->N > 0 ? run_solve(c, s, sh, io, st) : KA_ERR_BAD_ARG;
+    const Shape sh = dense_shape(T, P, RF, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->br.N);
+    rc = T > 0 && c->br.N > 0 ? run_solve(c, s, sh, io, st) : KA_ERR_BAD_ARG;
     if (rc != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
     return stream_json(c, s, io, json, json_cap, json_bytes, st);
 }
@@ -1743,7 +1739,7 @@ static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const i
     RaggedScan sc;
     int64_t capmax = 0;
     if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, S, pick_stride, have_out, sc, st)) != KA_OK ||
-        (rc = ragged_capmax(sc, c->N, capmax, st)) != KA_OK)
+        (rc = ragged_capmax(sc, c->br.N, capmax, st)) != KA_OK)
         return rc;
     if ((rc = reserve_io(c, T, sc.Q, sc.R, sc.S, true)) != KA_OK) return failed(st, rc);
     sh = Shape{T, 0, 0, desired_rf, sc.S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
@@ -1844,38 +1840,18 @@ static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, 
     // the stride holds every current list and the desired RF: every candidate's ka_solve would accept the call's input
     if (out_stride < std::max<int64_t>(sc.maxsz, desired_rf)) return all(KA_ERR_BAD_ARG);
     const int64_t Q = sc.Q;
-    if ((int64_t)K * Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
-    if ((rc = enter(c, true)) != KA_OK) return all(rc);
-    reset_plans(c);
-    // the plan of the call: counter placement and loop shape from the largest table, the largest capacity of any candidate
-    std::vector<BrokerTable> tabs;
-    int nmax = 0, blob_max = 0;
-    candidate_tables(K, cand_off, broker_id, broker_rack, tabs, nmax, blob_max);
-    int64_t capmax = 0;
-    for (int k = 0; k < K; ++k) {
-        int64_t cap = 0;
-        if ((rc = ragged_capmax(sc, cand_off[k + 1] - cand_off[k], cap, nullptr)) != KA_OK) return all(rc);
-        capmax = std::max(capmax, cap);
-    }
+    // the plan of the call: the largest capacity of any candidate
+    auto cap = [&](int n, int64_t& capmax) { return ragged_capmax(sc, n, capmax, nullptr); };
+    CandidateTables ct;
+    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, Q, cap, ct, st)) != KA_OK) return rc;
     const size_t q = (size_t)std::max<int64_t>(Q, 1);
     if ((rc = reserve_io(c, T, Q, sc.R, out_stride, true)) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
         c->d_out_len.reserve((size_t)K * q * 4) != cudaSuccess)
         return all(KA_ERR_CUDA);
+    const Shape sh{T, 0, 0, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
+                   c->d_rep_off.as<int64_t>(), Q, sc.R, sc.Pmax, ct.capmax};
     StageDesc d;
-    d.T = T;
-    d.Q = Q;
-    d.d_hash = c->d_hash.as<int32_t>();
-    d.d_part_off = c->d_part_off.as<int64_t>();
-    d.d_rep_off = c->d_rep_off.as<int64_t>();
-    d.d_cur = c->d_cur.as<int32_t>();
-    d.desired_rf = desired_rf;
-    d.S = out_stride;
-    d.Pmax = sc.Pmax;
-    d.capmax = capmax;
-    if ((rc = make_plan(nmax, blob_max, Q, out_stride, sc.Pmax, capmax, true, d.pl, st)) != KA_OK) {
-        for (int k = 1; k < K; ++k) st[k] = st[0];
-        return rc;
-    }
+    if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
     if (part_weight) {
         bool negative = false;
         int64_t sum = 0;   // saturates above INT64_MAX / 3
@@ -1898,11 +1874,9 @@ static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, 
     run.Q = Q;
     run.enqueued = true;
     if ((rc = enq_inputs(c->stream, io, d, sc.R)) != KA_OK ||
-        (rc = enq_candidates(c, c->stream, K, tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK) {
+        (rc = enq_candidates(c, c->stream, K, ct.tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK) {
         run.enqueued = false;
-        cudaStreamSynchronize(c->sb1);
-        cudaStreamSynchronize(c->stream);
-        return all(rc);
+        return abort_candidates(c, c->stream, st, K, rc);
     }
     return KA_OK;
 }
@@ -1926,11 +1900,8 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     // the rows of all candidates come back in one copy
     run.io.h_out = out_broker;
     run.io.h_out_len = out_len;
-    if (run.Q > 0 && (rc = enq_copy_out(c->stream, run.io, out_stride, 0, (int64_t)K * run.Q)) != KA_OK) {
-        cudaStreamSynchronize(c->sb1);
-        cudaStreamSynchronize(c->stream);
-        return fail_candidates(st, K, rc);
-    }
+    if (run.Q > 0 && (rc = enq_copy_out(c->stream, run.io, out_stride, 0, (int64_t)K * run.Q)) != KA_OK)
+        return abort_candidates(c, c->stream, st, K, rc);
     return finish_candidates(c, c->stream, K, T, st, part_id, part_off);
 }
 
@@ -1955,12 +1926,11 @@ int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     cudaStream_t s = c->stream;
     const int64_t Q = run.Q;
     auto fail = [&](int code) {
-        cudaStreamSynchronize(c->sb1);
-        cudaStreamSynchronize(s);
+        abort_candidates(c, s, st, K, code);
         for (int k = 0; k < K; ++k) summary[k] = empty_summary();
         for (int64_t* a : brk)
             if (a && nb > 0) std::memset(a, 0, nb * 8);
-        return fail_candidates(st, K, code);
+        return code;
     };
     const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
     if (c->d_score_sum.reserve(sum_bytes) != cudaSuccess || c->d_score_brk.reserve(std::max<size_t>(3 * nb, 1) * 8) != cudaSuccess ||

@@ -29,26 +29,55 @@
 
 enum { KA_LUT_SMEM = 0, KA_LUT_GLOBAL = 1, KA_LUT_BSEARCH = 2 };
 
+// One broker table in HBM: what kernel A stages and every id -> index lookup reads.
+struct KaBrokers {
+    int N, lut_mode, lut_off, blob_bytes, min_id;
+    uint32_t range;
+    const uint16_t* blob;       // rack16[Npad] || lut16[range_pad] (lut16 only when lut_mode == SMEM), 16B aligned; blob_bytes long
+    const uint16_t* glut;       // lut_mode == KA_LUT_GLOBAL: lut16[range]
+    const int32_t* broker_id;   // [N] ascending
+};
+
+// What kernel A writes for a run (rows and topics relative to the run's block).
+struct KaStageOut {
+    unsigned char* rec;         // [Q] partition records in schedule order (16 B for rec_kind 3, else 32 B)
+    uint16_t* perm;             // [Q] LEVELS && rec_kind == 3: partition ordinal (inside its topic) of each schedule position
+    int32_t* ntl;               // [T] LEVELS: number of chunks of each topic
+    uint32_t* lend;             // [Q] LEVELS: lend[g0 + i] = topic-relative end of the topic's i-th chunk (first ntl[t] entries)
+    int4* tstatus;              // [T] per-topic error record (written only on error)
+    unsigned* err_topic;        // unsigned atomicMin of the failing topic index (init = 0xFFFFFFFF)
+};
+
 // One candidate broker table of a batched solve (ka_solve_dense_candidates_device), in HBM: its broker table, its own
 // fresh Context and its slice of the call's scratch. Every kernel of the batched solve reads the entry of its candidate
 // once, at entry; the kernels of the single solve never see one.
 struct KaCandidate {
-    int N;
-    int lut_mode, lut_off, blob_bytes, min_id;
-    uint32_t range;
-    const uint16_t* blob;       // rack16 || lut16, staged by kernel A (blob_bytes of it)
-    const uint16_t* glut;       // lut_mode == KA_LUT_GLOBAL
-    const int32_t* broker_id;   // [N] ascending
+    KaBrokers br;
+    KaStageOut out;
     int32_t* ctr8;              // [N+1][8] the candidate's Context.counter (+ the chains' dummy row), zero at the call's start
-    unsigned char* rec;         // [Q] records of the candidate (16 B)
-    uint16_t* perm;             // [Q] LEVELS: schedule position -> partition ordinal
-    int32_t* ntl;               // [T] LEVELS: chunks per topic
-    uint32_t* lend;             // [Q] LEVELS: topic-relative chunk ends
     const int32_t* loff;        // [T+1] LEVELS: first chunk of each topic in the call-wide chunk table
     uint32_t pos0;              // LEVELS: position of rec[0] in the call-wide chunk table (candidate k: k * Q)
-    int4* tstatus;              // [T] per-topic error record
-    unsigned* err_topic;        // lowest failing topic (unsigned atomicMin, 0xFFFFFFFF = none)
 };
+
+// Broker id -> index in the ascending table br (KA_DEAD when absent). lut: br's SMEM-mode LUT, wherever it is read from.
+__device__ __forceinline__ uint32_t ka_lookup(int id, const uint16_t* lut, const KaBrokers& br) {
+    if (br.lut_mode == KA_LUT_SMEM) {
+        uint32_t off = (uint32_t)id - (uint32_t)br.min_id;
+        return off < br.range ? (uint32_t)lut[off] : KA_DEAD;
+    } else if (br.lut_mode == KA_LUT_GLOBAL) {
+        uint32_t off = (uint32_t)id - (uint32_t)br.min_id;
+        return off < br.range ? (uint32_t)__ldg(&br.glut[off]) : KA_DEAD;
+    } else {
+        int lo = 0, hi = br.N - 1;
+        while (lo <= hi) {
+            int mid = (lo + hi) >> 1;
+            int v = __ldg(&br.broker_id[mid]);
+            if (v == id) return (uint32_t)mid;
+            if (v < id) lo = mid + 1; else hi = mid - 1;
+        }
+        return KA_DEAD;
+    }
+}
 
 // ------------------------------------------------------------------------------------------------
 // Partition records: what kernel A hands to the leader-order kernel, in SCHEDULE order (topic by topic; inside a

@@ -54,28 +54,17 @@ __global__ void __launch_bounds__(1024) ka_level_scan_kernel(const int32_t* __re
     if (threadIdx.x == 0) loff[T] = carry;
 }
 
+// Chunk ends of a chunk table of U topics, one warp per topic. Topic u = k * T + t (k > 0 only in a batched solve: the K
+// candidates' tables are one table of K * T topics) starts at record k * rows + part_off[t] (dense: t * P), rows = the
+// records of one candidate.
 __global__ void __launch_bounds__(256) ka_level_fill_kernel(const int32_t* __restrict__ ntl, const int32_t* __restrict__ loff,
                                                             const uint32_t* __restrict__ lend, const int64_t* __restrict__ part_off, int P,
-                                                            int T, uint32_t* __restrict__ lvl_end) {
-    const int lane = threadIdx.x & 31;
-    const int t = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (t >= T) return;
-    const int64_t g0 = part_off ? part_off[t] : (int64_t)t * P;
-    const int d = ntl[t], o = loff[t];
-    for (int l = lane; l < d; l += 32) lvl_end[o + l] = (uint32_t)g0 + lend[g0 + l];
-}
-
-// The call-wide chunk table of a ragged batched solve: K candidates x T topics, topic u = k * T + t starts at record
-// k * Q + part_off[t] (Q = rows of one candidate). The dense batch uses ka_level_fill_kernel, where that is u * P.
-__global__ void __launch_bounds__(256) ka_level_fill_candidates_kernel(const int32_t* __restrict__ ntl, const int32_t* __restrict__ loff,
-                                                                       const uint32_t* __restrict__ lend,
-                                                                       const int64_t* __restrict__ part_off, int T, int KT, int64_t Q,
-                                                                       uint32_t* __restrict__ lvl_end) {
+                                                            int T, int U, int64_t rows, uint32_t* __restrict__ lvl_end) {
     const int lane = threadIdx.x & 31;
     const int u = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (u >= KT) return;
+    if (u >= U) return;
     const int k = u / T, t = u - k * T;
-    const int64_t g0 = (int64_t)k * Q + part_off[t];
+    const int64_t g0 = (int64_t)k * rows + (part_off ? part_off[t] : (int64_t)t * P);
     const int d = ntl[u], o = loff[u];
     for (int l = lane; l < d; l += 32) lvl_end[o + l] = (uint32_t)g0 + lend[g0 + l];
 }
@@ -204,16 +193,16 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
     int* ctr = reinterpret_cast<int*>(ka_osmem + ((size_t)NS << p.ring_log2) * RB + 256);
     static_assert(!CAND || KIND <= 1, "batched solves order rows of <= 3 replicas");
     const KaCandidate* const cd = CAND ? p.cand + blockIdx.x : nullptr;
-    if (CAND && cd->N <= 0) return;   // no broker: every topic of the candidate failed in kernel A
+    if (CAND && cd->br.N <= 0) return;   // no broker: every topic of the candidate failed in kernel A
     // Loop invariants take a round trip through shared memory (volatile) so that they live in registers: ptxas otherwise
     // re-reads kernel parameters from the constant bank inside the chain loop, and every such load stalls a branch.
     if (tid == 0) {
-        const void* const rec = CAND ? (const void*)(cd->rec + (size_t)p.pos_base * RB) : p.rec;
+        const void* const rec = CAND ? (const void*)(cd->out.rec + (size_t)p.pos_base * RB) : p.rec;
         int32_t* const c8 = CAND ? cd->ctr8 : p.ctr8;
         pin[0] = p.Q; pin[1] = blockDim.x; pin[2] = (uint32_t)p.ring_log2; pin[3] = p.uniform_width;
         pin[4] = (uint32_t)reinterpret_cast<uintptr_t>(rec); pin[5] = (uint32_t)(reinterpret_cast<uintptr_t>(rec) >> 32);
         pin[6] = (uint32_t)reinterpret_cast<uintptr_t>(c8); pin[7] = (uint32_t)(reinterpret_cast<uintptr_t>(c8) >> 32);
-        if (CAND) pin[8] = (uint32_t)cd->N;
+        if (CAND) pin[8] = (uint32_t)cd->br.N;
     }
     __syncthreads();
     const uint32_t Q = pin[0], NT = pin[1];
@@ -626,8 +615,8 @@ __global__ void __launch_bounds__(256) ka_emit3_candidates_kernel(const KaCandid
                                                                   int64_t cand_rows, int32_t* __restrict__ out,
                                                                   int32_t* __restrict__ out_len) {
     const KaCandidate& c = cand[blockIdx.y];
-    if (c.N <= 0) return;   // no broker: every topic failed in kernel A, its rows are unspecified
+    if (c.br.N <= 0) return;   // no broker: every topic failed in kernel A, its rows are unspecified
     const int64_t row0 = (int64_t)blockIdx.y * cand_rows + r0;
-    ka_emit3(reinterpret_cast<const uint4*>(c.rec) + r0, c.perm ? c.perm + r0 : nullptr, RAGGED ? part_off : nullptr, T, P,
-             c.broker_id, Q, S, out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8);
+    ka_emit3(reinterpret_cast<const uint4*>(c.out.rec) + r0, c.out.perm ? c.out.perm + r0 : nullptr, RAGGED ? part_off : nullptr, T, P,
+             c.br.broker_id, Q, S, out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8);
 }

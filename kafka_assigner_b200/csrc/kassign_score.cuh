@@ -13,7 +13,7 @@
 #include "../../include/kassign.h"
 
 // A candidate that failed (or has no broker) keeps the zero summary and per-broker entries the host cleared.
-__device__ __forceinline__ bool ka_score_ok(const KaCandidate& c) { return c.N > 0 && *c.err_topic == 0xFFFFFFFFu; }
+__device__ __forceinline__ bool ka_score_ok(const KaCandidate& c) { return c.br.N > 0 && *c.out.err_topic == 0xFFFFFFFFu; }
 
 __device__ __forceinline__ long long ka_warp_sum64(long long v) {
 #pragma unroll
@@ -48,15 +48,7 @@ __global__ void __launch_bounds__(256) ka_score_rows_kernel(const KaCandidate* _
             cb[j] = j < m ? __ldg(cur + a + j) : 0;
         }
         const long long w = weight ? __ldg(weight + g) : 1;
-        // the candidate's id -> index lookup of kernel A, its table read from HBM
-        KaSolveParams p{};
-        p.N = c.N;
-        p.lut_mode = c.lut_mode;
-        p.min_id = c.min_id;
-        p.range = c.range;
-        p.glut = c.glut;
-        p.broker_id = c.broker_id;
-        const KaTab tab{nullptr, c.blob + c.lut_off};
+        const KaBrokers br = c.br;   // read once: the atomics below may alias HBM as far as the compiler knows
         const int64_t base = bro_off[k];
         int n_add = 0, n_drop = 0;
         bool diff = n != m;
@@ -74,7 +66,8 @@ __global__ void __launch_bounds__(256) ka_score_rows_kernel(const KaCandidate* _
                 for (int i = 0; i < 3; ++i) held |= i < m && cb[i] == nb[j];
                 n_add += !held;
                 diff |= j < m && nb[j] != cb[j];
-                const int64_t e = base + ka_lookup(nb[j], tab, p);
+                // the candidate's id -> index lookup of kernel A, its table read from HBM
+                const int64_t e = base + ka_lookup(nb[j], br.blob + br.lut_off, br);
                 atomicAdd(reinterpret_cast<unsigned long long*>(broker_replicas + e), (unsigned long long)w);
                 if (j == 0) atomicAdd(reinterpret_cast<unsigned long long*>(broker_leaders + e), (unsigned long long)w);
                 if (!held) atomicAdd(reinterpret_cast<unsigned long long*>(broker_in + e), (unsigned long long)w);
@@ -114,7 +107,7 @@ __global__ void __launch_bounds__(256) ka_score_finish_kernel(const KaCandidate*
     __shared__ long long sh[8][6];
     const int k = blockIdx.x;
     const KaCandidate& c = cand[k];
-    const int n = ka_score_ok(c) ? c.N : 0;
+    const int n = ka_score_ok(c) ? c.br.N : 0;
     const int64_t base = bro_off[k];
     long long rmax = LLONG_MIN, rmin = LLONG_MAX, lmax = LLONG_MIN, lmin = LLONG_MAX, imax = -1, iarg = INT_MAX;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
@@ -146,7 +139,7 @@ __global__ void __launch_bounds__(256) ka_score_finish_kernel(const KaCandidate*
     ka_move_summary& s = summary[k];
     const bool any = n > 0;
     s.max_broker_in = any ? imax : 0;
-    s.max_broker_in_id = any && imax > 0 ? __ldg(c.broker_id + iarg) : -1;
+    s.max_broker_in_id = any && imax > 0 ? __ldg(c.br.broker_id + iarg) : -1;
     s.max_broker_replicas = any ? rmax : 0;
     s.min_broker_replicas = any ? rmin : 0;
     s.max_broker_leaders = any ? lmax : 0;

@@ -16,25 +16,11 @@ struct KaSolveParams {
     int desired_rf;
     int S;                      // row stride of the slab / output rows
     int Pmax;                   // max partitions of any topic (smem sizing)
-    // broker table
-    int N;
-    const uint16_t* blob;       // global: rack16[Npad] | lut16[range_pad] (16B aligned, multiple of 16B)
-    int blob_bytes;             // bytes staged into smem (rack, plus lut when lut_mode == SMEM)
-    int lut_off;                // element offset (uint16) of lut16 inside blob
-    int lut_mode;
-    int min_id;
-    uint32_t range;
-    const uint16_t* glut;       // global lut16 (lut_mode == GLOBAL)
-    const int32_t* broker_id;   // [N] ascending (global)
-    // outputs (block-relative rows)
+    int blob_space;             // shared memory for the broker blob: the plan's (a batched solve's largest blob)
+    KaBrokers br;               // the broker table (batched solve: taken from cand)
     int rec_kind;               // 3: 16 B records (S <= 3), else 32 B records (see kassign_common.cuh)
-    void* rec;                  // [Q] partition records in schedule order
-    uint16_t* perm;             // [Q] LEVELS && rec_kind == 3: partition ordinal (inside its topic) of each schedule position
     int chunk_w;                // LEVELS: a chunk = at most chunk_w records of one level (the order kernel's consumer threads)
-    int32_t* ntl;               // [T] LEVELS: number of chunks of each topic
-    uint32_t* lend;             // [Q] LEVELS: lend[g0 + i] = topic-relative end of the topic's i-th chunk (first ntl[t] entries)
-    int4* tstatus;              // [T] per-topic error record (written only on error)
-    unsigned* err_topic;        // unsigned atomicMin of the failing topic index (init = 0xFFFFFFFF)
+    KaStageOut out;             // outputs, block-relative rows (batched solve: taken from cand)
     const KaCandidate* cand;    // batched solve: candidate blockIdx.y's broker table, records, level tables and status
 };
 
@@ -45,25 +31,6 @@ struct KaTab {               // CTA-shared views into the staged broker table
     const uint16_t* rack;    // [N] compact rack id of each broker (sorted-index order)
     const uint16_t* lut;     // [range] (lut_mode == SMEM)
 };
-
-__device__ __forceinline__ uint32_t ka_lookup(int id, const KaTab& tab, const KaSolveParams& p) {
-    if (p.lut_mode == KA_LUT_SMEM) {
-        uint32_t off = (uint32_t)id - (uint32_t)p.min_id;
-        return off < p.range ? (uint32_t)tab.lut[off] : KA_DEAD;
-    } else if (p.lut_mode == KA_LUT_GLOBAL) {
-        uint32_t off = (uint32_t)id - (uint32_t)p.min_id;
-        return off < p.range ? (uint32_t)__ldg(&p.glut[off]) : KA_DEAD;
-    } else {
-        int lo = 0, hi = p.N - 1;
-        while (lo <= hi) {
-            int mid = (lo + hi) >> 1;
-            int v = __ldg(&p.broker_id[mid]);
-            if (v == id) return (uint32_t)mid;
-            if (v < id) lo = mid + 1; else hi = mid - 1;
-        }
-        return KA_DEAD;
-    }
-}
 
 // Per-warp scratch of the conflict-level pass (LEVELS only).
 struct KaLevelScratch {
@@ -81,7 +48,7 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
     const int lane = threadIdx.x & 31;
     const uint32_t lt = ka_lanemask_lt();
     const int S = p.S;
-    const int N = p.N;
+    const int N = p.br.N;
 
     int64_t g0;
     int P;
@@ -157,18 +124,18 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
                     const int4* s4 = reinterpret_cast<const int4*>(src);
                     for (int e = lane; e < (n >> 2); e += 32) {
                         int4 v = ka_ldg_stream_v4(s4 + e);
-                        uint32_t a = ka_lookup(v.x, tab, p), b = ka_lookup(v.y, tab, p);
-                        uint32_t c = ka_lookup(v.z, tab, p), d = ka_lookup(v.w, tab, p);
+                        uint32_t a = ka_lookup(v.x, tab.lut, p.br), b = ka_lookup(v.y, tab.lut, p.br);
+                        uint32_t c = ka_lookup(v.z, tab.lut, p.br), d = ka_lookup(v.w, tab.lut, p.br);
                         uint2 pk = make_uint2(a | (b << 16), c | (d << 16));
                         *reinterpret_cast<uint2*>(slab + 4 * e) = pk;
                     }
                 } else {
-                    for (int e = lane; e < n; e += 32) slab[e] = (uint16_t)ka_lookup(__ldg(src + e), tab, p);
+                    for (int e = lane; e < n; e += 32) slab[e] = (uint16_t)ka_lookup(__ldg(src + e), tab.lut, p.br);
                 }
             } else {
                 for (int e = lane; e < n; e += 32) {
                     int pp = e / RF, r = e - pp * RF;
-                    slab[pp * S + r] = (uint16_t)ka_lookup(__ldg(src + e), tab, p);
+                    slab[pp * S + r] = (uint16_t)ka_lookup(__ldg(src + e), tab.lut, p.br);
                 }
                 for (int e = lane; e < P * (S - RF); e += 32) {
                     int pp = e / (S - RF), r = RF + (e - pp * (S - RF));
@@ -181,7 +148,7 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
                 int64_t off = ro[pp];
                 int sz = (int)(ro[pp + 1] - off);
                 for (int r = 0; r < S; ++r)
-                    slab[pp * S + r] = r < sz ? (uint16_t)ka_lookup(__ldg(p.cur + off + r), tab, p) : (uint16_t)KA_DEAD;
+                    slab[pp * S + r] = r < sz ? (uint16_t)ka_lookup(__ldg(p.cur + off + r), tab.lut, p.br) : (uint16_t)KA_DEAD;
             }
         }
         __syncwarp();
@@ -395,7 +362,7 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
             }
             if (l <= D) {
                 const int lstart = run + x - v, cstart = crun + y - nc;
-                for (int i = 0; i < nc; ++i) p.lend[g0 + cstart + i] = (uint32_t)(lstart + min((i + 1) * W, v));
+                for (int i = 0; i < nc; ++i) p.out.lend[g0 + cstart + i] = (uint32_t)(lstart + min((i + 1) * W, v));
                 ls.lcur[l] = (uint16_t)lstart;  // first schedule position of level l
             }
             run += __shfl_sync(KA_FULL, x, 31);
@@ -406,9 +373,9 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
     } else if (LEVELS && P > 0) {
         const int W = p.chunk_w;  // failed topic: one level of empty records
         D = (P + W - 1) / W;
-        for (int i = lane; i < D; i += 32) p.lend[g0 + i] = (uint32_t)min((i + 1) * W, P);
+        for (int i = lane; i < D; i += 32) p.out.lend[g0 + i] = (uint32_t)min((i + 1) * W, P);
     }
-    if (LEVELS && lane == 0) p.ntl[t] = D;
+    if (LEVELS && lane == 0) p.out.ntl[t] = D;
 
     // ---- emit the partition records in schedule order ----------------------------------------------------
     const uint32_t rot = (err || hmin) ? 0u : ka_rot_bits(habs);
@@ -457,10 +424,10 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
                                    e12 = (uint32_t)(i1 < i2 ? s2 : 1 - s2);
                     f |= (e01 << 2) | (e02 << 3) | (e12 << 4);
                 }
-                reinterpret_cast<uint4*>(p.rec)[g0 + pos] = make_uint4(a0, a1, a2, f);
-                if (LEVELS) p.perm[g0 + pos] = (uint16_t)pp;
+                reinterpret_cast<uint4*>(p.out.rec)[g0 + pos] = make_uint4(a0, a1, a2, f);
+                if (LEVELS) p.out.perm[g0 + pos] = (uint16_t)pp;
             } else {
-                uint4* r8 = reinterpret_cast<uint4*>(p.rec) + 2 * (g0 + pos);
+                uint4* r8 = reinterpret_cast<uint4*>(p.out.rec) + 2 * (g0 + pos);
                 r8[0] = make_uint4(ix[0] | (ix[1 % SM] << 16), ix[2 % SM] | (ix[3 % SM] << 16), ix[4 % SM] | (ix[5 % SM] << 16),
                                    ix[6 % SM] | (ix[7 % SM] << 16));   // SM == 8 on this path (S > 3)
                 r8[1] = make_uint4((uint32_t)k | rot, (uint32_t)(g0 + pp), 0u, 0u);
@@ -468,14 +435,14 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
         }
     }
     if (err && lane == 0) {
-        p.tstatus[p.topic_base + t] = make_int4(err, errp, erra, errb);
-        atomicMin(p.err_topic, (unsigned)(p.topic_base + t));
+        p.out.tstatus[p.topic_base + t] = make_int4(err, errp, erra, errb);
+        atomicMin(p.out.err_topic, (unsigned)(p.topic_base + t));
     }
     __syncwarp();
 }
 
 // One CTA of kernel A: stage p's broker table, then its topics, one per warp. warp_base: the per-warp scratch, behind the
-// largest blob of the launch.
+// blob space of the launch.
 template <typename LoadT, bool LEVELS, int SM>
 __device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uint64_t* bar, unsigned char* blob, unsigned char* warp_base,
                                                      int load_bytes, int slab_bytes, int cnt_bytes, int lv_owner_bytes, int lv_last_bytes,
@@ -486,15 +453,15 @@ __device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uin
         ka_fence_mbar_init();
     }
     __syncthreads();
-    if (threadIdx.x == 0 && p.blob_bytes > 0) {
-        ka_mbar_expect_tx(bar, (uint32_t)p.blob_bytes);
-        ka_tma_bulk_g2s(blob, p.blob, (uint32_t)p.blob_bytes, bar);
+    if (threadIdx.x == 0 && p.br.blob_bytes > 0) {
+        ka_mbar_expect_tx(bar, (uint32_t)p.br.blob_bytes);
+        ka_tma_bulk_g2s(blob, p.br.blob, (uint32_t)p.br.blob_bytes, bar);
     }
-    if (p.blob_bytes > 0) ka_mbar_wait(bar, 0);
+    if (p.br.blob_bytes > 0) ka_mbar_wait(bar, 0);
 
     KaTab tab;
     tab.rack = reinterpret_cast<const uint16_t*>(blob);
-    tab.lut = reinterpret_cast<const uint16_t*>(blob) + p.lut_off;
+    tab.lut = reinterpret_cast<const uint16_t*>(blob) + p.br.lut_off;
 
     const int warp = threadIdx.x >> 5;
     const int nwarp = blockDim.x >> 5;
@@ -519,34 +486,23 @@ __device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uin
 }
 
 // CAND: a batched solve over candidate broker tables, blockIdx.y = candidate. A CTA serves one candidate, so its broker
-// table is still staged once per CTA; p.blob_bytes is the largest blob of the launch (the shared-memory layout). Dense or
-// ragged (p.part_off): the candidate's slices (records, perm, lend, ntl, status) take the same rows and topics as a single
-// solve's buffers.
+// table is still staged once per CTA. Dense or ragged (p.part_off): the candidate's slices (records, perm, lend, ntl, status)
+// take the same rows and topics as a single solve's buffers. The per-warp scratch sits behind the plan's blob space
+// (p.blob_space, the largest blob of the launch); the TMA copy is the CTA's own table (p.br.blob_bytes). A single solve's blob
+// space is its table's blob, and reading it from the table keeps ptxas' register allocation of the single-solve instances
+// (from p.blob_space they move by up to 5 registers).
 template <typename LoadT, bool LEVELS, int SM, bool CAND = false>
 __global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolveParams p, int load_bytes, int slab_bytes, int cnt_bytes,
                                                                int lv_owner_bytes, int lv_last_bytes, int lv_p_bytes) {
     extern __shared__ __align__(16) unsigned char ka_smem[];
     uint64_t* bar = reinterpret_cast<uint64_t*>(ka_smem);
     unsigned char* blob = ka_smem + 16;
-    unsigned char* warp_base = blob + p.blob_bytes;
+    unsigned char* warp_base = blob + (CAND ? p.blob_space : p.br.blob_bytes);
     if constexpr (CAND) {
         const KaCandidate& c = p.cand[blockIdx.y];
         KaSolveParams q = p;
-        q.N = c.N;
-        q.blob = c.blob;
-        q.blob_bytes = c.blob_bytes;
-        q.lut_off = c.lut_off;
-        q.lut_mode = c.lut_mode;
-        q.min_id = c.min_id;
-        q.range = c.range;
-        q.glut = c.glut;
-        q.broker_id = c.broker_id;
-        q.rec = c.rec;
-        q.perm = c.perm;
-        q.ntl = c.ntl;
-        q.lend = c.lend;
-        q.tstatus = c.tstatus;
-        q.err_topic = c.err_topic;
+        q.br = c.br;
+        q.out = c.out;
         ka_sticky_spread_cta<LoadT, LEVELS, SM>(q, bar, blob, warp_base, load_bytes, slab_bytes, cnt_bytes, lv_owner_bytes,
                                                 lv_last_bytes, lv_p_bytes);
     } else {
