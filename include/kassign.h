@@ -184,6 +184,35 @@ int32_t ka_solve_candidates(ka_ctx* ctx, int32_t K, const int32_t* cand_off, con
                             int32_t desired_rf, int32_t out_stride, int32_t* out_len, int32_t* out_broker,
                             ka_status* st);
 
+/* A fleet of K independent clusters, each solved against its OWN broker table on a FRESH Context, in one call: K runs of the
+ * reference tool, one per cluster (a fleet-wide host retirement or OS roll, a rack move that touches several clusters). The
+ * clusters run side by side inside every kernel; the number of kernel launches does not depend on K, and the call takes about
+ * as long as its longest cluster's leader-order chain.
+ *   cand_off, broker_id, broker_rack   table k is cluster k's, as ka_solve_candidates takes the candidate tables
+ *   topic_off[K+1]     host; cluster k is topics topic_off[k] .. topic_off[k+1]-1 of the inputs below
+ *   desired_rf[K]      host; cluster k's --desired_replication_factor, or NULL = -1 for every cluster
+ *   topic_hash .. cur_broker   ONE ragged layout (as ka_solve takes it) over all ΣT topics and ΣP rows, host
+ *   out_broker[ΣP][out_stride], out_len[ΣP] (or NULL)   host; every row at its place in the layout
+ *   st[K]              host, required; st[k] is cluster k's status
+ * Cluster k's rows, out_len entries and st[k] are exactly what ka_ctx_create -> ka_ctx_set_brokers(table k) -> ka_solve(its
+ * topics, with part_off / rep_off rebased to 0, desired_rf[k], out_stride) gives: topic_index counts from the cluster's first
+ * topic, partition is mapped through part_id. A failing cluster changes nothing of another; its rows are unspecified. What
+ * ka_solve would report for a cluster's slice (malformed offsets inside it, lists longer than out_stride, a target RF in
+ * (out_stride, N], a table beyond the level plan's broker limit, the five reference exceptions) is that cluster's status,
+ * and the others still solve.
+ * Checked for the whole call (the code in every st[k], and returned): K <= 128 and out_stride <= 3 (else KA_ERR_LIMIT);
+ * out_stride >= 1; every table as ka_ctx_set_brokers checks it (same code); topic_off non-decreasing from 0, and part_off at
+ * every cluster's first topic and rep_off at its first row non-decreasing from 0 (else KA_ERR_BAD_ARG); ΣP < 2^31 (else
+ * KA_ERR_LIMIT). One plan serves the call, sized from its largest table and largest topic: if that plan exceeds shared memory
+ * where no cluster's own does, every st[k] is KA_ERR_LIMIT. K == 0: KA_OK, nothing written.
+ * Synchronous. Returns KA_OK when every cluster solved, else st[k].code of the lowest failing k. Does not read or change ctx's
+ * own Context, broker table, parked counters, topic_base or staged block. */
+int32_t ka_solve_clusters(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                          const int32_t* broker_rack, const int32_t* topic_off, const int32_t* desired_rf,
+                          const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                          const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
+                          int32_t* out_len, int32_t* out_broker, ka_status* st);
+
 /* What a candidate's rows change against the current lists, and how they spread over its brokers. Every field is int64, so
  * the layout has no padding. Position counts: a duplicate id in a current list, or a current broker the table lacks, needs
  * no special case. w[g] is the weight of row g (1 without weights); the rows_* and leaders_changed fields count rows. */
@@ -280,7 +309,7 @@ int64_t ka_ctx_launch_count(ka_ctx* ctx);
 /* The leader-order plan of the LAST solve call on this ctx (any entry point, including the staged and candidate calls):
  * plan[0] rec_kind (3 / 4 / 8)   plan[1] levels (0/1)   plan[2] chain threads   plan[3] ring_log2
  * plan[4] gctr (0/1)   plan[5] loop shape (0 general, 1 warp1, 2 single, 3 full)   plan[6] chain launches of the call
- * plan[7] candidates K (0 for a single solve).
+ * plan[7] candidates K (the clusters K of ka_solve_clusters; 0 for a single solve).
  * Cleared when a solve call passes its argument checks (ka_stage_dense_device starts a staged solve; its ka_order_device /
  * ka_order_slot_device calls add to it), so a call that launches no chain (a limit before any launch, or no rows) leaves
  * all zeros.

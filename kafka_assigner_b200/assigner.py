@@ -353,6 +353,57 @@ class Solver:
             res += tuple([a[cand_off[k]:cand_off[k + 1]] for k in range(K)] for a in brk)
         return res
 
+    @staticmethod
+    def marshal_clusters(clusters):
+        """The shared layout of ka_solve_clusters from a list of clusters, each (broker_id, rack_index, topic_hash, part_off,
+        part_id, rep_off, cur_broker, desired_rf) with its own offsets from 0 (part_id may be None: 0..P-1 per topic). Returns
+        (cand_off, broker_id, broker_rack, topic_off, desired_rf, topic_hash, part_off, part_id, rep_off, cur_broker)."""
+        cand_off, broker_id, broker_rack = Solver._candidate_tables([(c[0], c[1]) for c in clusters])
+        th = [np.ascontiguousarray(c[2], dtype=np.int32) for c in clusters]
+        po = [np.ascontiguousarray(c[3], dtype=np.int64) for c in clusters]
+        ro = [np.ascontiguousarray(c[5], dtype=np.int64) for c in clusters]
+        cur = [np.ascontiguousarray(c[6], dtype=np.int32) for c in clusters]
+        topic_off = np.zeros(len(clusters) + 1, dtype=np.int32)
+        np.cumsum([len(h) for h in th], out=topic_off[1:])
+        rows = [int(p[-1]) if len(p) > 1 else 0 for p in po]          # a cluster without topics may pass part_off = [0] or []
+        reps = [int(r[rows[k]]) if rows[k] > 0 else 0 for k, r in enumerate(ro)]
+        row0 = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
+        rep0 = np.concatenate([[0], np.cumsum(reps)]).astype(np.int64)
+        part_off = np.concatenate([[0]] + [p[1:len(h) + 1] + row0[k] for k, (p, h) in enumerate(zip(po, th))]).astype(np.int64)
+        rep_off = np.concatenate([[0]] + [r[1:rows[k] + 1] + rep0[k] for k, r in enumerate(ro)]).astype(np.int64)
+        none = np.zeros(0, dtype=np.int32)
+
+        def ids(k):   # partition ids of cluster k (ordinals inside each topic when it has none)
+            if clusters[k][4] is not None:
+                return np.ascontiguousarray(clusters[k][4], dtype=np.int32)[:rows[k]]
+            return np.concatenate([none] + [np.arange(int(po[k][t + 1] - po[k][t]), dtype=np.int32) for t in range(len(th[k]))])
+
+        part_id = np.concatenate([none] + [ids(k) for k in range(len(clusters))])
+        desired_rf = np.array([int(c[7]) for c in clusters], dtype=np.int32)
+        return (cand_off, broker_id, broker_rack, topic_off, desired_rf, np.concatenate([none] + th), part_off, part_id, rep_off,
+                np.concatenate([none] + [c[:reps[k]] for k, c in enumerate(cur)]))
+
+    def solve_clusters(self, clusters, out_stride=None):
+        """ka_solve_clusters: every cluster of `clusters` solved against its own broker table, each on a fresh Context, in one
+        device call; this Solver's own Context is untouched. Each entry is (broker_id, rack_index, topic_hash, part_off, part_id,
+        rep_off, cur_broker, desired_rf), e.g. from synth.make_ragged_cluster. out_stride defaults to max(longest current list,
+        largest desired_rf, 1) over the fleet. Returns one (out [P_k, out_stride], out_len [P_k], KaStatus) per cluster; the rows
+        of a failed cluster are unspecified."""
+        K = len(clusters)
+        cand_off, broker_id, broker_rack, topic_off, drf, th, part_off, part_id, rep_off, cur = self.marshal_clusters(clusters)
+        if out_stride is None:
+            sizes = np.diff(rep_off)
+            out_stride = max(int(sizes.max()) if len(sizes) else 0, int(drf.max()) if K else -1, 1)
+        Q = int(part_off[-1])
+        out = np.full((Q, out_stride), -1, dtype=np.int32)
+        out_len = np.zeros(Q, dtype=np.int32)
+        st = (KaStatus * max(K, 1))()
+        self._L.ka_solve_clusters(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), _ptr(topic_off), _ptr(drf),
+                                  _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur), int(out_stride), _ptr(out_len),
+                                  _ptr(out), st)
+        rows = part_off[topic_off]
+        return [(out[rows[k]:rows[k + 1]], out_len[rows[k]:rows[k + 1]], st[k]) for k in range(K)]
+
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""
         rc = self._L.ka_stage_dense_device(self._h, int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF),

@@ -1034,13 +1034,13 @@ struct CandidateTables {
     int64_t capmax = 0;
 };
 
-// The common part of the candidate front ends, once their own checks have passed (the tables are checked and the problem of
-// Q rows per candidate is sized): the K·Q limit, the ctx's device and the candidates' tables. cap(n, capmax) gives the largest
-// capacity of the problem under a table of n brokers, or the status that table fails with.
+// The common part of the batched front ends, once their own checks have passed (the tables are checked and the call's `recs`
+// records are sized: K·Q for K candidates over Q rows, ΣP for a fleet): the records' limit, the ctx's device and the tables.
+// cap(k, n, capmax) gives the largest capacity of table k's problem under its n brokers, or the status that table fails with.
 template <typename Cap>
-int candidate_tables(ka_ctx* c, int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack, int64_t Q,
+int candidate_tables(ka_ctx* c, int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack, int64_t recs,
                      Cap cap, CandidateTables& ct, ka_status* st) {
-    if ((int64_t)K * Q >= ((int64_t)1 << 31)) return fail_candidates(st, K, KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
+    if (recs >= ((int64_t)1 << 31)) return fail_candidates(st, K, KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
     int rc = enter(c, true);
     if (rc != KA_OK) return fail_candidates(st, K, rc);
     reset_plans(c);
@@ -1051,7 +1051,7 @@ int candidate_tables(ka_ctx* c, int K, const int32_t* cand_off, const int32_t* b
         ct.nmax = std::max(ct.nmax, n);
         ct.blob_max = std::max(ct.blob_max, ct.tabs[k].blob_bytes());
         int64_t capk = 0;
-        if ((rc = cap(n, capk)) != KA_OK) return fail_candidates(st, K, rc);
+        if ((rc = cap(k, n, capk)) != KA_OK) return fail_candidates(st, K, rc);
         ct.capmax = std::max(ct.capmax, capk);
     }
     return KA_OK;
@@ -1064,26 +1064,69 @@ int plan_candidates(const Shape& sh, const CandidateTables& ct, int K, StageDesc
     return rc;
 }
 
-// Wait for a batched solve enqueued on `s` and fill every candidate's status: its lowest failing topic, as finish_status
-// reports it for one solve (part_id / part_off of a ragged solve: the failing partition's id). Returns the code of the
-// lowest failing candidate.
-int finish_candidates(ka_ctx* c, cudaStream_t s, int K, int T, ka_status* st, const int32_t* part_id = nullptr,
+// Where one member of a batched solve reads and writes (the host side of its KaCandidate): a candidate table over the whole
+// input, or one cluster of a fleet.
+struct BatchMember {
+    int tab = 0;                 // its broker table cand_off[tab] .. cand_off[tab + 1] - 1, and its status st[tab]
+    int t0 = 0, T = 0;           // its topics [t0, t0 + T) of the shared input
+    int64_t row0 = 0, Q = 0;     // its rows [row0, row0 + Q) of the shared input
+    int desired_rf = -1;
+    int64_t rec0 = 0;            // its first record in the call's records = its first position in the call-wide chunk table
+    int64_t topic0 = 0;          // its first topic in the call's topic tables (ntl, loff, status)
+};
+
+// The members of a batched solve and the call-wide sizes that follow from them.
+struct Batch {
+    int K = 0;                   // the call's K (reported by ka_ctx_last_*_plan; a fleet's refused clusters are no member)
+    std::vector<BatchMember> m;
+    int64_t recs = 0;            // records of the call: K·Q for candidates, ΣP for a fleet
+    int topics = 0;              // topics of the call's topic tables: K·T for candidates, ΣT for a fleet
+    int fill_T = 0;              // ka_level_fill_kernel's view: topic u starts at record (u / fill_T)·fill_rows + part_off[u % fill_T]
+    int64_t fill_rows = 0;
+    int64_t out_rows = 0;        // output rows between two members: Q for candidates, 0 for a fleet (rows at their input rows)
+    int Tmax = 0;                // the largest member
+    int64_t Qmax = 0;
+};
+
+// K candidates over one problem of T topics and Q rows: every member reads the whole input, on its own copy of the records.
+Batch candidate_batch(int K, int T, int64_t Q, int desired_rf) {
+    Batch b;
+    b.K = K;
+    const int64_t q = std::max<int64_t>(Q, 1);
+    for (int k = 0; k < K; ++k) b.m.push_back(BatchMember{k, 0, T, 0, Q, desired_rf, (int64_t)k * q, (int64_t)k * T});
+    b.recs = (int64_t)K * q;
+    b.topics = K * T;
+    b.fill_T = T;
+    b.fill_rows = Q;
+    b.out_rows = Q;
+    b.Tmax = T;
+    b.Qmax = Q;
+    return b;
+}
+
+// Wait for a batched solve enqueued on `s` and fill every member's status: its lowest failing topic, as finish_status
+// reports it for one solve (relative to the member's first topic; part_id / part_off of a ragged solve: the failing
+// partition's id). Statuses already in st (a fleet's refused clusters) stay. Returns the code of the lowest failing st[k].
+int finish_candidates(ka_ctx* c, cudaStream_t s, const Batch& b, ka_status* st, const int32_t* part_id = nullptr,
                       const int64_t* part_off = nullptr) {
+    const int K = b.K, M = (int)b.m.size();
     if (cudaStreamSynchronize(s) != cudaSuccess) return fail_candidates(st, K, KA_ERR_CUDA);
-    std::vector<unsigned> err(K);
-    if (cudaMemcpy(err.data(), c->cand_run.flags.p, (size_t)K * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+    std::vector<unsigned> err(std::max(M, 1));
+    if (M > 0 && cudaMemcpy(err.data(), c->cand_run.flags.p, (size_t)M * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
         return fail_candidates(st, K, KA_ERR_CUDA);
-    int first = KA_OK;
-    for (int k = 0; k < K; ++k) {
+    for (int k = 0; k < M; ++k) {
         if (err[k] == 0xFFFFFFFFu) continue;
-        const int t = (int)err[k];
+        const BatchMember& mb = b.m[k];
+        const int t = (int)err[k] - mb.t0;   // kernel A reports the input topic
         int4 ts;
-        if (cudaMemcpy(&ts, c->cand_run.tstatus.as<int4>() + (size_t)k * T + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
+        if (cudaMemcpy(&ts, c->cand_run.tstatus.as<int4>() + mb.topic0 + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
             return fail_candidates(st, K, KA_ERR_CUDA);
-        st[k] = topic_status(t, ts, part_id, part_off);
-        if (first == KA_OK) first = ts.x;
+        st[mb.tab] = topic_status(mb.t0 + t, ts, part_id, part_off);
+        st[mb.tab].topic_index = t;
     }
-    return first;
+    for (int k = 0; k < K; ++k)
+        if (st[k].code != KA_OK) return st[k].code;
+    return KA_OK;
 }
 
 }  // namespace
@@ -1318,30 +1361,31 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     return finish(c, s, st, false);
 }
 
-// Everything of a batched solve over K candidate tables, enqueued on `s` (slot-0 chains on c->sb1): the candidates' tables
-// and descriptors H2D, fresh counters, kernel A with grid.y = candidate, the level tables of all candidates as one table,
-// then per chain sub-block the slot-0 / slot-1 chains (one CTA per candidate) and the emit (grid.y = candidate). `d` is a
-// dense problem or a ragged one (d.d_part_off set: one chain sub-block, as in a ragged single solve); its inputs are shared by
-// every candidate.
-static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<BrokerTable>& tabs, const int32_t* cand_off,
+// Everything of a batched solve over the members of `bt`, enqueued on `s` (slot-0 chains on c->sb1): the members' tables
+// and descriptors H2D, fresh counters, kernel A with grid.y = member, the level tables of all members as one table, then per
+// chain sub-block the slot-0 / slot-1 chains (one CTA per member) and the emit (grid.y = member). `d` is a dense problem or a
+// ragged one (d.d_part_off set: one chain sub-block, as in a ragged single solve); its inputs are shared by every member, each
+// of which reads its own window of them.
+static int enq_candidates(ka_ctx* c, cudaStream_t s, const Batch& bt, const std::vector<BrokerTable>& tabs, const int32_t* cand_off,
                           const int32_t* broker_id, const StageDesc& d, int32_t* d_out_len, int32_t* d_out) {
     const Plan& pl = d.pl;
-    const int T = d.T, S = d.S;
-    const int64_t Q = d.Q;
-    const size_t q = (size_t)std::max<int64_t>(Q, 1), kq = (size_t)K * q, kt = (size_t)K * T;
-    // descriptors, then every candidate's blob, global LUT and broker ids, in one upload
+    const int S = d.S, K = (int)bt.m.size();
+    const size_t kq = (size_t)bt.recs, kt = (size_t)bt.topics;
+    // descriptors, then every member's blob, global LUT and broker ids, in one upload
     std::vector<size_t> blob_off(K), glut_off(K), bid_off(K), ctr_off(K);
     size_t bytes = align16((size_t)K * sizeof(KaCandidate)), ctr_ints = 0;
+    int64_t covered = 0;   // topics kernel A walks
     for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
+        const int tab = bt.m[k].tab, n = cand_off[tab + 1] - cand_off[tab];
         blob_off[k] = bytes;
-        bytes += tabs[k].blob.size() * 2;
+        bytes += tabs[tab].blob.size() * 2;
         glut_off[k] = bytes;
-        bytes += align16(tabs[k].glut.size() * 2);
+        bytes += align16(tabs[tab].glut.size() * 2);
         bid_off[k] = bytes;
         bytes += align16((size_t)std::max(n, 1) * 4);
         ctr_off[k] = ctr_ints;
         ctr_ints += (size_t)(n + 1) * KA_MAX_SLOTS;   // + the chains' dummy row
+        covered += bt.m[k].T;
     }
     RunScratch& r = c->cand_run;
     KA_CUDA(c->d_cand_tab.reserve(bytes));
@@ -1351,47 +1395,60 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
     std::vector<unsigned char> h(bytes, 0);
     int lut_mask = 0;
     for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        const BrokerTable& t = tabs[k];
+        const BatchMember& mb = bt.m[k];
+        const int n = cand_off[mb.tab + 1] - cand_off[mb.tab];
+        const BrokerTable& t = tabs[mb.tab];
+        // kernel A writes the member's records, perm and lend by input row, its ntl and status by input topic
+        const int64_t shift = mb.rec0 - mb.row0, tshift = mb.topic0 - mb.t0;
         KaCandidate e{};
         e.br = t.device(n, reinterpret_cast<const uint16_t*>(base + blob_off[k]), reinterpret_cast<const uint16_t*>(base + glut_off[k]),
                         reinterpret_cast<const int32_t*>(base + bid_off[k]));
         e.ctr8 = c->d_cand_ctr.as<int32_t>() + ctr_off[k];
-        e.out.rec = r.rec.as<unsigned char>() + (size_t)k * q * 16;
+        e.out.rec = r.rec.as<unsigned char>() + shift * 16;
         if (pl.a_levels) {
-            e.out.perm = r.perm.as<uint16_t>() + (size_t)k * q;
-            e.out.ntl = r.ntl.as<int32_t>() + (size_t)k * T;
-            e.out.lend = r.lend.as<uint32_t>() + (size_t)k * q;
-            e.loff = r.loff.as<int32_t>() + (size_t)k * T;
-            e.pos0 = (uint32_t)((size_t)k * Q);   // the level tables of the K candidates are one table of K * T topics
+            e.out.perm = r.perm.as<uint16_t>() + shift;
+            e.out.ntl = r.ntl.as<int32_t>() + tshift;
+            e.out.lend = r.lend.as<uint32_t>() + shift;
+            e.loff = r.loff.as<int32_t>() + mb.topic0;
+            e.pos0 = (uint32_t)mb.rec0;   // the level tables of the members are one table of bt.topics topics
         }
-        e.out.tstatus = r.tstatus.as<int4>() + (size_t)k * T;
+        e.out.tstatus = r.tstatus.as<int4>() + tshift;
         e.out.err_topic = r.flags.as<unsigned>() + k;
+        e.desired_rf = mb.desired_rf;
+        e.t0 = mb.t0;
+        e.T = mb.T;
+        e.row0 = (uint32_t)mb.row0;
+        e.Q = (uint32_t)mb.Q;
         std::memcpy(h.data() + (size_t)k * sizeof(KaCandidate), &e, sizeof(e));
         std::memcpy(h.data() + blob_off[k], t.blob.data(), t.blob.size() * 2);
         if (!t.glut.empty()) std::memcpy(h.data() + glut_off[k], t.glut.data(), t.glut.size() * 2);
-        if (n > 0) std::memcpy(h.data() + bid_off[k], broker_id + cand_off[k], (size_t)n * 4);
+        if (n > 0) std::memcpy(h.data() + bid_off[k], broker_id + cand_off[mb.tab], (size_t)n * 4);
         lut_mask |= 1 << t.lut_mode;
     }
     const KaCandidate* cand = c->d_cand_tab.as<KaCandidate>();
     KA_CUDA(cudaMemcpyAsync(base, h.data(), bytes, cudaMemcpyHostToDevice, s));
-    KA_CUDA(cudaMemsetAsync(c->d_cand_ctr.p, 0, ctr_ints * 4, s));   // every candidate starts from a fresh Context
+    KA_CUDA(cudaMemsetAsync(c->d_cand_ctr.p, 0, ctr_ints * 4, s));   // every member starts from a fresh Context
     KA_CUDA(cudaMemsetAsync(r.flags.p, 0xFF, (size_t)K * 4, s));
-    // kernel A: grid.y = candidate; the plan's shared-memory layout is that of the largest table
+    // topics no member walks (a fleet's refused clusters) have no chunks
+    if (pl.a_levels && covered < bt.topics) KA_CUDA(cudaMemsetAsync(r.ntl.p, 0, kt * 4, s));
+    // kernel A: grid.y = member, grid.x from the largest member; the plan's shared-memory layout is that of the largest table
     KaSolveParams p = stage_params(d);
     p.cand = cand;
-    int rc = launch_stage_plan<true>(c, s, p, pl, T, K, lut_mask);
+    int rc = launch_stage_plan<true>(c, s, p, pl, bt.Tmax, K, lut_mask);
     if (rc != KA_OK) return rc;
+    c->stage_plan[3] = bt.K;
     if (pl.a_levels) {
         ka_level_scan_kernel<<<1, 1024, 0, s>>>(r.ntl.as<int32_t>(), (int)kt, r.loff.as<int32_t>());
         KA_CUDA(cudaGetLastError());
         ka_level_fill_kernel<<<(unsigned)((kt + 7) / 8), 256, 0, s>>>(r.ntl.as<int32_t>(), r.loff.as<int32_t>(), r.lend.as<uint32_t>(),
-                                                                      d.d_part_off, d.P, T, (int)kt, Q, r.lvl_end.as<uint32_t>());
+                                                                      d.d_part_off, d.P, bt.fill_T, (int)kt, bt.fill_rows,
+                                                                      r.lvl_end.as<uint32_t>());
         KA_CUDA(cudaGetLastError());
         c->launches += 2;
     }
-    if (Q <= 0) return KA_OK;
-    // the chains: slot 0 of sub-block j+1 (c->sb1) overlaps slot 1 + emit of sub-block j (s), as in the single solve
+    if (bt.Qmax <= 0) return KA_OK;
+    // the chains: slot 0 of sub-block j+1 (c->sb1) overlaps slot 1 + emit of sub-block j (s), as in the single solve. A launch
+    // covers the sub-block's rows and topics; every member clips them to its own window.
     if ((rc = chain_fork(c, s)) != KA_OK) return rc;
     const int nsub = chain_subblocks(d, 1);
     for (int j = 0; j < nsub; ++j) {
@@ -1409,17 +1466,19 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, int K, const std::vector<Br
         o.cand_t1 = b.t1;
         int sel = 0;
         KA_CUDA((launch_order<0, 1024, true>(c->sb1, o, pl, &sel, K)));
-        note_order(c, pl, sel, K);
+        note_order(c, pl, sel, bt.K);
         KA_CUDA(cudaEventRecord(c->ev_b1[j], c->sb1));
         KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[j], 0));
         KA_CUDA((launch_order<1, 1024, true>(s, o, pl, &sel, K)));
-        note_order(c, pl, sel, K);
-        const dim3 grid((unsigned)((b.rq + 255) / 256), K);
+        note_order(c, pl, sel, bt.K);
+        const int64_t rq = std::min(b.rq, bt.Qmax);   // the largest member's rows of the sub-block
+        const dim3 grid((unsigned)((rq + 255) / 256), K);
         if (d.d_part_off)
-            ka_emit3_candidates_kernel<true><<<grid, 256, 0, s>>>(cand, 0u, T, 0, d.d_part_off, (uint32_t)b.rq, S, Q, d_out, d_out_len);
+            ka_emit3_candidates_kernel<true><<<grid, 256, 0, s>>>(cand, 0u, d.T, 0, d.d_part_off, (uint32_t)rq, S, bt.out_rows, d_out,
+                                                                  d_out_len);
         else
-            ka_emit3_candidates_kernel<<<grid, 256, 0, s>>>(cand, (uint32_t)b.r0, b.t1 - b.t0, d.P, nullptr, (uint32_t)b.rq, S, Q, d_out,
-                                                            d_out_len);
+            ka_emit3_candidates_kernel<<<grid, 256, 0, s>>>(cand, (uint32_t)b.r0, b.t1 - b.t0, d.P, nullptr, (uint32_t)rq, S, bt.out_rows,
+                                                            d_out, d_out_len);
         KA_CUDA(cudaGetLastError());
         c->launches += 3;
     }
@@ -1444,21 +1503,22 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
     if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
     // levels if any candidate that can serve the target RF has capacity > 1 (one that cannot fails alone, whatever the plan)
     const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    auto cap = [&](int n, int64_t& capmax) {
+    auto cap = [&](int, int n, int64_t& capmax) {
         capmax = dense_capmax(P, rf_t, n);
         return KA_OK;
     };
     CandidateTables ct;
-    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, Q, cap, ct, st)) != KA_OK) return rc;
+    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, cap, ct, st)) != KA_OK) return rc;
     Shape sh{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker};
     sh.Pmax = P;
     sh.capmax = ct.capmax;
     StageDesc d;
     if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    if ((rc = enq_candidates(c, s, K, ct.tabs, cand_off, broker_id, d, d_out_len, d_out_broker)) != KA_OK)
+    const Batch bt = candidate_batch(K, T, Q, desired_rf);
+    if ((rc = enq_candidates(c, s, bt, ct.tabs, cand_off, broker_id, d, d_out_len, d_out_broker)) != KA_OK)
         return abort_candidates(c, s, st, K, rc);
-    return finish_candidates(c, s, K, T, st);
+    return finish_candidates(c, s, bt, st);
 }
 
 int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash, int32_t P, int32_t RF,
@@ -1672,12 +1732,14 @@ struct RaggedScan {
     ka_status err{KA_OK, -1, -1, 0, 0};
 };
 
+// row0 / rep0: the scan reads part_off[t] - row0 and rep_off[g] - rep0, i.e. a slice of a larger layout rebased to 0 (one
+// cluster of ka_solve_clusters' fleet), without copying it.
 static int ragged_scan(int32_t T, const int64_t* part_off, const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf,
-                       int32_t S, bool pick_stride, bool have_out, RaggedScan& sc, ka_status* st) {
-    const int64_t Q = T > 0 ? part_off[T] : 0;
-    if (Q < 0 || (T > 0 && part_off[0] != 0) || (Q > 0 && (!rep_off || !have_out))) return set_status(st, KA_ERR_BAD_ARG);
-    const int64_t R = Q > 0 ? rep_off[Q] : 0;
-    if (R < 0 || (Q > 0 && rep_off[0] != 0) || (R > 0 && !cur_broker)) return set_status(st, KA_ERR_BAD_ARG);
+                       int32_t S, bool pick_stride, bool have_out, RaggedScan& sc, ka_status* st, int64_t row0 = 0, int64_t rep0 = 0) {
+    const int64_t Q = T > 0 ? part_off[T] - row0 : 0;
+    if (Q < 0 || (T > 0 && part_off[0] != row0) || (Q > 0 && (!rep_off || !have_out))) return set_status(st, KA_ERR_BAD_ARG);
+    const int64_t R = Q > 0 ? rep_off[Q] - rep0 : 0;
+    if (R < 0 || (Q > 0 && rep_off[0] != rep0) || (R > 0 && !cur_broker)) return set_status(st, KA_ERR_BAD_ARG);
     if (pick_stride) {
         int64_t m = std::max(desired_rf, 1);
         for (int64_t g = 0; g < Q; ++g) m = std::max(m, rep_off[g + 1] - rep_off[g]);
@@ -1688,7 +1750,7 @@ static int ragged_scan(int32_t T, const int64_t* part_off, const int64_t* rep_of
     sc.R = R;
     sc.S = S;
     for (int t = 0; t < T; ++t) {
-        const int64_t a = part_off[t], b = part_off[t + 1];
+        const int64_t a = part_off[t] - row0, b = part_off[t + 1] - row0;
         if (b < a) { set_status(&sc.err, KA_ERR_BAD_ARG, t); return KA_OK; }
         const int64_t Pn = b - a;
         if (Pn > INT_MAX / 16) { set_status(&sc.err, KA_ERR_LIMIT, t, -1, (int)std::min<int64_t>(Pn, INT_MAX)); return KA_OK; }
@@ -1804,6 +1866,7 @@ struct CandidateRun {
     bool tables_ok = false;   // the candidate tables passed their checks (cand_off may be read)
     bool enqueued = false;    // false: an error (returned, every st[k] set) or nothing to solve (K == 0 or T == 0)
     int64_t Q = 0;
+    Batch bt;                 // the candidates as members of the batched solve
     SolveCall io;             // d_out / d_out_len: the rows of all candidates, [K][Q] on the device
 };
 
@@ -1841,9 +1904,9 @@ static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, 
     if (out_stride < std::max<int64_t>(sc.maxsz, desired_rf)) return all(KA_ERR_BAD_ARG);
     const int64_t Q = sc.Q;
     // the plan of the call: the largest capacity of any candidate
-    auto cap = [&](int n, int64_t& capmax) { return ragged_capmax(sc, n, capmax, nullptr); };
+    auto cap = [&](int, int n, int64_t& capmax) { return ragged_capmax(sc, n, capmax, nullptr); };
     CandidateTables ct;
-    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, Q, cap, ct, st)) != KA_OK) return rc;
+    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, cap, ct, st)) != KA_OK) return rc;
     const size_t q = (size_t)std::max<int64_t>(Q, 1);
     if ((rc = reserve_io(c, T, Q, sc.R, out_stride, true)) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
         c->d_out_len.reserve((size_t)K * q * 4) != cudaSuccess)
@@ -1872,9 +1935,10 @@ static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, 
     io.d_out = c->d_out.as<int32_t>();
     io.d_out_len = c->d_out_len.as<int32_t>();
     run.Q = Q;
+    run.bt = candidate_batch(K, T, Q, desired_rf);
     run.enqueued = true;
     if ((rc = enq_inputs(c->stream, io, d, sc.R)) != KA_OK ||
-        (rc = enq_candidates(c, c->stream, K, ct.tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK) {
+        (rc = enq_candidates(c, c->stream, run.bt, ct.tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK) {
         run.enqueued = false;
         return abort_candidates(c, c->stream, st, K, rc);
     }
@@ -1902,7 +1966,108 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     run.io.h_out_len = out_len;
     if (run.Q > 0 && (rc = enq_copy_out(c->stream, run.io, out_stride, 0, (int64_t)K * run.Q)) != KA_OK)
         return abort_candidates(c, c->stream, st, K, rc);
-    return finish_candidates(c, c->stream, K, T, st, part_id, part_off);
+    return finish_candidates(c, c->stream, run.bt, st, part_id, part_off);
+}
+
+int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                          const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
+                          const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
+                          int32_t* out_len, int32_t* out_broker, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
+    auto all = [&](int rc) { return fail_candidates(st, K, rc); };
+    if (!c) return all(KA_ERR_NO_DEVICE);
+    if (out_stride > 3 || K > KA_MAX_CANDIDATES) return all(KA_ERR_LIMIT);   // rows of <= 3 replicas, as the candidate calls
+    if (out_stride < 1) return all(KA_ERR_BAD_ARG);
+    if (K == 0) return KA_OK;
+    int rc = check_candidates(K, cand_off, broker_id, broker_rack);
+    if (rc != KA_OK) return all(rc);
+    // the clusters' boundaries: topic_off, then part_off at their first topics and rep_off at their first rows, each
+    // non-decreasing from 0
+    if (!topic_off || topic_off[0] != 0) return all(KA_ERR_BAD_ARG);
+    for (int k = 0; k < K; ++k)
+        if (topic_off[k + 1] < topic_off[k]) return all(KA_ERR_BAD_ARG);
+    const int T = topic_off[K];
+    if (T > 0 && (!topic_hash || !part_off)) return all(KA_ERR_BAD_ARG);
+    std::vector<int64_t> row0(K + 1, 0), rep0(K + 1, 0);
+    for (int k = 0; k <= K; ++k) {
+        row0[k] = T > 0 ? part_off[topic_off[k]] : 0;
+        if (row0[k] < (k > 0 ? row0[k - 1] : 0) || row0[0] != 0) return all(KA_ERR_BAD_ARG);
+    }
+    const int64_t Q = row0[K];
+    if (Q > 0 && !rep_off) return all(KA_ERR_BAD_ARG);
+    for (int k = 0; k <= K; ++k) {
+        rep0[k] = Q > 0 ? rep_off[row0[k]] : 0;
+        if (rep0[k] < (k > 0 ? rep0[k - 1] : 0) || rep0[0] != 0) return all(KA_ERR_BAD_ARG);
+    }
+    if (Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);
+    // every cluster's slice, checked and sized as ka_solve checks and sizes it against the cluster's table: a cluster that
+    // fails here reports what ka_solve reports and is left out of the call
+    std::vector<RaggedScan> sc(K);
+    std::vector<int64_t> capk(K, 0);
+    std::vector<char> ok(K, 0);
+    for (int k = 0; k < K; ++k) {
+        const int t0 = topic_off[k];
+        ok[k] = ragged_scan(topic_off[k + 1] - t0, part_off ? part_off + t0 : nullptr, rep_off ? rep_off + row0[k] : nullptr,
+                            cur_broker ? cur_broker + rep0[k] : nullptr, desired_rf ? desired_rf[k] : -1, out_stride, false,
+                            out_broker != nullptr, sc[k], st + k, row0[k], rep0[k]) == KA_OK &&
+                ragged_capmax(sc[k], cand_off[k + 1] - cand_off[k], capk[k], st + k) == KA_OK;
+    }
+    auto cap = [&](int k, int, int64_t& capmax) {
+        capmax = ok[k] ? capk[k] : 0;
+        return KA_OK;
+    };
+    CandidateTables ct;
+    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, Q, cap, ct, st)) != KA_OK) return rc;
+    // the limits of ka_solve's own plan per cluster; the call's plan is sized from the clusters that pass them
+    Batch bt;
+    bt.K = K;
+    ct.nmax = ct.blob_max = 0;
+    ct.capmax = 0;
+    int Pmax = 0;
+    for (int k = 0; k < K; ++k) {
+        const int n = cand_off[k + 1] - cand_off[k];
+        Plan own;
+        if (!ok[k] || make_plan(n, ct.tabs[k].blob_bytes(), sc[k].Q, out_stride, sc[k].Pmax, capk[k], true, own, st + k) != KA_OK)
+            continue;
+        const int t0 = topic_off[k];
+        bt.m.push_back(BatchMember{k, t0, topic_off[k + 1] - t0, row0[k], sc[k].Q, desired_rf ? desired_rf[k] : -1, row0[k], t0});
+        ct.nmax = std::max(ct.nmax, n);
+        ct.blob_max = std::max(ct.blob_max, ct.tabs[k].blob_bytes());
+        ct.capmax = std::max(ct.capmax, capk[k]);
+        Pmax = std::max(Pmax, sc[k].Pmax);
+        bt.Tmax = std::max(bt.Tmax, topic_off[k + 1] - t0);
+        bt.Qmax = std::max(bt.Qmax, sc[k].Q);
+    }
+    // one table of the call's T topics over its Q rows: every record sits at its input row
+    bt.recs = std::max<int64_t>(Q, 1);
+    bt.topics = T;
+    bt.fill_T = std::max(T, 1);
+    bt.out_rows = 0;
+    if (bt.Tmax == 0) bt.m.clear();   // no topic to solve: every cluster that passed has solved (ka_solve with T == 0)
+    if (bt.m.empty()) return finish_candidates(c, c->stream, bt, st);
+    const int64_t R = rep0[K];
+    if (reserve_io(c, T, Q, R, out_stride, true) != KA_OK) return all(KA_ERR_CUDA);
+    const Shape sh{T, 0, 0, -1, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
+                   c->d_rep_off.as<int64_t>(), Q, R, Pmax, ct.capmax};
+    StageDesc d;
+    if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
+    // the inputs of every cluster go up at once; the rows of all clusters come back in one copy
+    SolveCall io;
+    io.h_hash = topic_hash;
+    io.h_part_off = part_off;
+    io.h_rep_off = rep_off;
+    io.h_cur = cur_broker;
+    io.d_out = c->d_out.as<int32_t>();
+    io.d_out_len = c->d_out_len.as<int32_t>();
+    io.h_out = out_broker;
+    io.h_out_len = out_len;
+    cudaStream_t s = c->stream;
+    if ((rc = enq_inputs(s, io, d, R)) != KA_OK ||
+        (rc = enq_candidates(c, s, bt, ct.tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK ||
+        (Q > 0 && out_broker && (rc = enq_copy_out(s, io, out_stride, 0, Q)) != KA_OK))
+        return abort_candidates(c, s, st, K, rc);
+    return finish_candidates(c, s, bt, st, part_id, part_off);
 }
 
 int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
@@ -1962,7 +2127,7 @@ int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
         run.io.h_out_len = out_len;
         if (enq_copy_out(s, run.io, out_stride, 0, (int64_t)K * Q) != KA_OK) return fail(KA_ERR_CUDA);
     }
-    return finish_candidates(c, s, K, T, st, part_id, part_off);
+    return finish_candidates(c, s, run.bt, st, part_id, part_off);
 }
 
 }  // extern "C"

@@ -48,15 +48,20 @@ struct KaStageOut {
     unsigned* err_topic;        // unsigned atomicMin of the failing topic index (init = 0xFFFFFFFF)
 };
 
-// One candidate broker table of a batched solve (ka_solve_dense_candidates_device), in HBM: its broker table, its own
-// fresh Context and its slice of the call's scratch. Every kernel of the batched solve reads the entry of its candidate
-// once, at entry; the kernels of the single solve never see one.
+// One member of a batched solve, in HBM: its broker table, its own fresh Context, its window of the call's shared input and
+// its slice of the call's scratch. A member is a candidate broker table over the whole input (ka_solve_candidates: t0 = 0,
+// T = the call's topics, row0 = 0, records from k * Q) or one cluster of a fleet (ka_solve_clusters: its own topics and rows,
+// records at their input rows). Every kernel of the batched solve reads the entry of its member once, at entry; the kernels of
+// the single solve never see one.
 struct KaCandidate {
     KaBrokers br;
-    KaStageOut out;
-    int32_t* ctr8;              // [N+1][8] the candidate's Context.counter (+ the chains' dummy row), zero at the call's start
-    const int32_t* loff;        // [T+1] LEVELS: first chunk of each topic in the call-wide chunk table
-    uint32_t pos0;              // LEVELS: position of rec[0] in the call-wide chunk table (candidate k: k * Q)
+    KaStageOut out;             // rec / perm / lend indexed by input row, ntl / tstatus / err_topic by input topic
+    int32_t* ctr8;              // [N+1][8] the member's Context.counter (+ the chains' dummy row), zero at the call's start
+    const int32_t* loff;        // [T+1] LEVELS: first chunk of each of the member's topics in the call-wide chunk table
+    uint32_t pos0;              // LEVELS: position of the member's first record in the call-wide chunk table
+    int t0, T;                  // the member's topics: [t0, t0 + T) of the shared input
+    uint32_t row0, Q;           // the member's rows: [row0, row0 + Q) of the shared input (part_off[t0] ..)
+    int desired_rf;             // the member's --desired_replication_factor (-1: keep)
 };
 
 // Broker id -> index in the ascending table br (KA_DEAD when absent). lut: br's SMEM-mode LUT, wherever it is read from.

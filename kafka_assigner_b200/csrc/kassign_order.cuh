@@ -54,9 +54,10 @@ __global__ void __launch_bounds__(1024) ka_level_scan_kernel(const int32_t* __re
     if (threadIdx.x == 0) loff[T] = carry;
 }
 
-// Chunk ends of a chunk table of U topics, one warp per topic. Topic u = k * T + t (k > 0 only in a batched solve: the K
-// candidates' tables are one table of K * T topics) starts at record k * rows + part_off[t] (dense: t * P), rows = the
-// records of one candidate.
+// Chunk ends of a chunk table of U topics, one warp per topic. Topic u = k * T + t (k > 0 only in a batched solve over
+// candidates: the K candidates' tables are one table of K * T topics) starts at record k * rows + part_off[t] (dense: t * P),
+// rows = the records of one candidate. The clusters of a fleet are one table of their U = T topics (rows = 0): topic u's
+// records start at part_off[u].
 __global__ void __launch_bounds__(256) ka_level_fill_kernel(const int32_t* __restrict__ ntl, const int32_t* __restrict__ loff,
                                                             const uint32_t* __restrict__ lend, const int64_t* __restrict__ part_off, int P,
                                                             int T, int U, int64_t rows, uint32_t* __restrict__ lvl_end) {
@@ -87,8 +88,9 @@ struct KaOrderParams {
     int32_t* out;
     int32_t* out_len;
     int ring_log2;              // log2(records per ring stage)
-    // batched solve (CAND): CTA k orders candidate k. N / ctr8 / records / chunk table come from cand[k]: the launch walks
-    // records [pos_base, pos_base + Q) of the candidate and chunks [loff[cand_t0], loff[cand_t1]) of its chunk table.
+    // batched solve (CAND): CTA k orders batch member k. N / ctr8 / records / chunk table come from cand[k]: the launch walks
+    // the member's records [pos_base, pos_base + Q) and chunks [loff[cand_t0], loff[cand_t1]) of its chunk table, both
+    // clipped to the member's window (its cand[k].Q records, cand[k].T topics).
     const KaCandidate* cand;
     int cand_t0, cand_t1;
 };
@@ -193,13 +195,15 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
     int* ctr = reinterpret_cast<int*>(ka_osmem + ((size_t)NS << p.ring_log2) * RB + 256);
     static_assert(!CAND || KIND <= 1, "batched solves order rows of <= 3 replicas");
     const KaCandidate* const cd = CAND ? p.cand + blockIdx.x : nullptr;
-    if (CAND && cd->br.N <= 0) return;   // no broker: every topic of the candidate failed in kernel A
+    // no broker: every topic of the member failed in kernel A; no record of the member in the launch's window: nothing to order
+    if (CAND && (cd->br.N <= 0 || p.pos_base >= cd->Q)) return;
     // Loop invariants take a round trip through shared memory (volatile) so that they live in registers: ptxas otherwise
     // re-reads kernel parameters from the constant bank inside the chain loop, and every such load stalls a branch.
     if (tid == 0) {
-        const void* const rec = CAND ? (const void*)(cd->out.rec + (size_t)p.pos_base * RB) : p.rec;
+        const void* const rec = CAND ? (const void*)(cd->out.rec + ((size_t)cd->row0 + p.pos_base) * RB) : p.rec;
         int32_t* const c8 = CAND ? cd->ctr8 : p.ctr8;
-        pin[0] = p.Q; pin[1] = blockDim.x; pin[2] = (uint32_t)p.ring_log2; pin[3] = p.uniform_width;
+        pin[0] = CAND ? min(p.Q, cd->Q - p.pos_base) : p.Q;   // CAND: the launch's window clipped to the member's rows
+        pin[1] = blockDim.x; pin[2] = (uint32_t)p.ring_log2; pin[3] = p.uniform_width;
         pin[4] = (uint32_t)reinterpret_cast<uintptr_t>(rec); pin[5] = (uint32_t)(reinterpret_cast<uintptr_t>(rec) >> 32);
         pin[6] = (uint32_t)reinterpret_cast<uintptr_t>(c8); pin[7] = (uint32_t)(reinterpret_cast<uintptr_t>(c8) >> 32);
         if (CAND) pin[8] = (uint32_t)cd->br.N;
@@ -250,8 +254,8 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
     uint32_t landed = 0;    // stages this thread has seen complete
     uint32_t released = 0;  // thread 0: stages handed back to the producer
     // chunk boundaries
-    const int chunk_lo = w ? 0 : (CAND ? cd->loff[p.cand_t0] : *p.chunk_lo_ptr);
-    const int nchunk = w ? 0 : (CAND ? cd->loff[p.cand_t1] : *p.chunk_hi_ptr) - chunk_lo;
+    const int chunk_lo = w ? 0 : (CAND ? cd->loff[min(p.cand_t0, cd->T)] : *p.chunk_lo_ptr);
+    const int nchunk = w ? 0 : (CAND ? cd->loff[min(p.cand_t1, cd->T)] : *p.chunk_hi_ptr) - chunk_lo;
     const uint32_t* const cend = p.chunk_end + chunk_lo;
     const uint32_t pos_base = CAND ? cd->pos0 + p.pos_base : p.pos_base;
     int wbase = 0;
@@ -567,10 +571,11 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
 // Emit (rows of <= 3 replicas): ordered record -> broker ids + list length + the slot-2 counters, one thread per schedule
 // position, fully parallel; keeps the id lookups and the 4 B/replica output stream off the serial chain.
 // ------------------------------------------------------------------------------------------------
+// base: the input row of rec[0] and out[0] (part_off counts input rows; 0 but for a cluster of a fleet).
 __device__ __forceinline__ void ka_emit3(const uint4* __restrict__ rec, const uint16_t* __restrict__ perm,
                                          const int64_t* __restrict__ part_off, int T, int P, const int32_t* __restrict__ broker_id,
                                          uint32_t Q, int S, int32_t* __restrict__ out, int32_t* __restrict__ out_len,
-                                         int32_t* __restrict__ ctr8) {
+                                         int32_t* __restrict__ ctr8, uint32_t base = 0) {
     const uint32_t pos = blockIdx.x * blockDim.x + threadIdx.x;
     if (pos >= Q) return;
     const uint4 r = rec[pos];   // ordered by the slot chains: {o0, o1, o2, f}, o_r = broker index << 2
@@ -582,9 +587,9 @@ __device__ __forceinline__ void ka_emit3(const uint4* __restrict__ rec, const ui
             int lo = 0, hi = T;  // last topic with part_off[t] <= pos
             while (hi - lo > 1) {
                 const int mid = (lo + hi) >> 1;
-                if (part_off[mid] <= (int64_t)pos) lo = mid; else hi = mid;
+                if (part_off[mid] <= (int64_t)(base + pos)) lo = mid; else hi = mid;
             }
-            g0 = part_off[lo];
+            g0 = part_off[lo] - base;
         } else {
             g0 = (int64_t)(pos / (uint32_t)P) * P;
         }
@@ -606,17 +611,20 @@ __global__ void __launch_bounds__(256) ka_emit3_kernel(const uint4* __restrict__
     ka_emit3(rec, perm, part_off, T, P, broker_id, Q, S, out, out_len, ctr8);
 }
 
-// Batched solve: blockIdx.y = candidate k. Rows [r0, r0 + Q) of a sub-block of T topics; candidate k's rows are
-// out + k * cand_rows * S (out_len + k * cand_rows), its counters its own ctr8. RAGGED: the whole problem (r0 == 0), each
-// schedule position's topic found in part_off[T+1] as ka_emit3_kernel finds it; else dense, P partitions per topic.
+// Batched solve: blockIdx.y = batch member k. Rows [r0, r0 + Q) of the member's rows (clipped to its window), a sub-block of
+// T topics; member k's rows are out + (k * cand_rows + input row) * S (out_len likewise): cand_rows = Q for candidates,
+// 0 for the clusters of a fleet, whose rows sit at their input rows. Its counters are its own ctr8. RAGGED: the member's
+// whole window (r0 == 0), each schedule position's topic found in the member's part_off[t0 .. t0 + T] as ka_emit3_kernel
+// finds it; else dense, P partitions per topic.
 template <bool RAGGED = false>
 __global__ void __launch_bounds__(256) ka_emit3_candidates_kernel(const KaCandidate* __restrict__ cand, uint32_t r0, int T, int P,
                                                                   const int64_t* __restrict__ part_off, uint32_t Q, int S,
                                                                   int64_t cand_rows, int32_t* __restrict__ out,
                                                                   int32_t* __restrict__ out_len) {
     const KaCandidate& c = cand[blockIdx.y];
-    if (c.br.N <= 0) return;   // no broker: every topic failed in kernel A, its rows are unspecified
-    const int64_t row0 = (int64_t)blockIdx.y * cand_rows + r0;
-    ka_emit3(reinterpret_cast<const uint4*>(c.out.rec) + r0, c.out.perm ? c.out.perm + r0 : nullptr, RAGGED ? part_off : nullptr, T, P,
-             c.br.broker_id, Q, S, out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8);
+    if (c.br.N <= 0 || r0 >= c.Q) return;   // no broker: every topic failed in kernel A, its rows are unspecified
+    const uint32_t base = c.row0 + r0;      // input row of the launch's first record of the member
+    const int64_t row0 = (int64_t)blockIdx.y * cand_rows + base;
+    ka_emit3(reinterpret_cast<const uint4*>(c.out.rec) + base, c.out.perm ? c.out.perm + base : nullptr, RAGGED ? part_off + c.t0 : nullptr,
+             RAGGED ? c.T : T, P, c.br.broker_id, min(Q, c.Q - r0), S, out + row0 * S, out_len ? out_len + row0 : nullptr, c.ctr8, base);
 }

@@ -441,12 +441,12 @@ __device__ void ka_solve_topic(const KaSolveParams& p, const KaTab& tab, int t, 
     __syncwarp();
 }
 
-// One CTA of kernel A: stage p's broker table, then its topics, one per warp. warp_base: the per-warp scratch, behind the
-// blob space of the launch.
+// One CTA of kernel A: stage p's broker table, then its topics t_begin .. p.T - 1, one per warp. warp_base: the per-warp
+// scratch, behind the blob space of the launch.
 template <typename LoadT, bool LEVELS, int SM>
 __device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uint64_t* bar, unsigned char* blob, unsigned char* warp_base,
                                                      int load_bytes, int slab_bytes, int cnt_bytes, int lv_owner_bytes, int lv_last_bytes,
-                                                     int lv_p_bytes) {
+                                                     int lv_p_bytes, int t_begin = 0) {
     // TMA bulk-stage the broker table (rack indices + id->index LUT) once per CTA.
     if (threadIdx.x == 0) {
         ka_mbar_init(bar, 1);
@@ -481,13 +481,14 @@ __device__ __forceinline__ void ka_sticky_spread_cta(const KaSolveParams& p, uin
     }
 
     const int total_warps = gridDim.x * nwarp;
-    for (int t = blockIdx.x * nwarp + warp; t < p.T; t += total_warps)
+    for (int t = t_begin + blockIdx.x * nwarp + warp; t < p.T; t += total_warps)
         ka_solve_topic<LoadT, LEVELS, SM>(p, tab, t, load, slab, cnt, ls);
 }
 
-// CAND: a batched solve over candidate broker tables, blockIdx.y = candidate. A CTA serves one candidate, so its broker
-// table is still staged once per CTA. Dense or ragged (p.part_off): the candidate's slices (records, perm, lend, ntl, status)
-// take the same rows and topics as a single solve's buffers. The per-warp scratch sits behind the plan's blob space
+// CAND: a batched solve, blockIdx.y = batch member (a candidate broker table or a cluster of a fleet). A CTA serves one
+// member, so its broker table is still staged once per CTA; it walks the member's topics [t0, t0 + T) of the shared input.
+// Dense or ragged (p.part_off): the member's slices (records, perm, lend, ntl, status: by input row and topic) take the same
+// rows and topics as a single solve's buffers. The per-warp scratch sits behind the plan's blob space
 // (p.blob_space, the largest blob of the launch); the TMA copy is the CTA's own table (p.br.blob_bytes). A single solve's blob
 // space is its table's blob, and reading it from the table keeps ptxas' register allocation of the single-solve instances
 // (from p.blob_space they move by up to 5 registers).
@@ -498,13 +499,18 @@ __global__ void __launch_bounds__(512) ka_sticky_spread_kernel(const KaSolvePara
     uint64_t* bar = reinterpret_cast<uint64_t*>(ka_smem);
     unsigned char* blob = ka_smem + 16;
     unsigned char* warp_base = blob + (CAND ? p.blob_space : p.br.blob_bytes);
-    if constexpr (CAND) {
+    if constexpr (CAND && SM > 3) {
+        // never launched: the batched calls refuse rows of more than 3 replicas before anything is enqueued, so they run SM 3
+    } else if constexpr (CAND) {
         const KaCandidate& c = p.cand[blockIdx.y];
         KaSolveParams q = p;
         q.br = c.br;
         q.out = c.out;
+        // topics t0 .. t0 + T - 1 by their input index (ntl, status and err_topic too: the host biases the member's slices)
+        q.T = c.t0 + c.T;
+        q.desired_rf = c.desired_rf;
         ka_sticky_spread_cta<LoadT, LEVELS, SM>(q, bar, blob, warp_base, load_bytes, slab_bytes, cnt_bytes, lv_owner_bytes,
-                                                lv_last_bytes, lv_p_bytes);
+                                                lv_last_bytes, lv_p_bytes, c.t0);
     } else {
         ka_sticky_spread_cta<LoadT, LEVELS, SM>(p, bar, blob, warp_base, load_bytes, slab_bytes, cnt_bytes, lv_owner_bytes,
                                                 lv_last_bytes, lv_p_bytes);

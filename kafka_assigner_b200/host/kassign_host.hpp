@@ -10,6 +10,8 @@
 //                                                          assigner, in one device call (a decommission sweep)
 //   kassign::scoreTopicsCandidates                    <->  the same sweep, reduced on the device to what each broker set
 //                                                          would move and how evenly it spreads replicas and leaders
+//   kassign::solveClusters                            <->  that loop once per cluster of a fleet, each with its own broker
+//                                                          set and a new assigner, in one device call
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -133,6 +135,58 @@ public:
         for (int k = 0; k < K; ++k) {
             res[k].status = st[k];
             if (st[k].code == KA_OK) res[k].topics = unflatten(f, out.data() + (size_t)k * Q * f.stride, outLen.data() + (size_t)k * Q);
+        }
+        return res;
+    }
+
+    // One cluster of a fleet: its topics and the arguments of its own run.
+    struct ClusterInput {
+        std::vector<TopicInput> topics;
+        std::set<int> brokers;
+        std::map<int, std::string> rackAssignment;
+        int desiredReplicationFactor = -1;
+    };
+
+    // The KAG:172-184 loop once per cluster of a fleet, each with its own broker set on a fresh Context (one new assigner per
+    // cluster), in ONE device call (ka_solve_clusters): cluster k equals solveTopics(its topics, brokers, racks, desired RF) on a
+    // new KafkaTopicAssigner, with the exception it would throw as its status (topic_index counts from the cluster's first
+    // topic). This instance's own Context is left alone. Rows of at most 3 replicas.
+    std::vector<CandidateResult> solveClusters(const std::vector<ClusterInput>& clusters) {
+        const int K = (int)clusters.size();
+        std::vector<Flat> flat;
+        std::vector<Candidate> tables;
+        std::vector<int32_t> topicOff(1, 0), desired, hash, partId, cur;
+        std::vector<int64_t> partOff(1, 0), repOff(1, 0);
+        int stride = 1;
+        for (const auto& cl : clusters) {
+            flat.push_back(flatten(cl.topics, cl.desiredReplicationFactor));
+            const Flat& f = flat.back();
+            tables.push_back(Candidate{cl.brokers, cl.rackAssignment});
+            desired.push_back(cl.desiredReplicationFactor);
+            const int64_t row0 = partOff.back(), rep0 = repOff.back();
+            hash.insert(hash.end(), f.hash.begin(), f.hash.end());
+            for (size_t t = 1; t < f.partOff.size(); ++t) partOff.push_back(row0 + f.partOff[t]);
+            for (size_t g = 1; g < f.repOff.size(); ++g) repOff.push_back(rep0 + f.repOff[g]);
+            partId.insert(partId.end(), f.partId.begin(), f.partId.end());
+            cur.insert(cur.end(), f.cur.begin(), f.cur.end());
+            topicOff.push_back((int32_t)hash.size());
+            stride = std::max(stride, f.stride);
+        }
+        std::vector<int32_t> candOff, ids, racks;
+        candidateTables(tables, candOff, ids, racks);
+        const size_t Q = partId.size();
+        std::vector<int32_t> outLen(Q, 0), out(Q * stride, -1);
+        std::vector<ka_status> st(std::max(K, 1));
+        ka_solve_clusters(ctx_, K, candOff.data(), ids.data(), racks.data(), topicOff.data(), desired.data(), hash.data(), partOff.data(),
+                          partId.data(), repOff.data(), cur.data(), stride, outLen.data(), out.data(), st.data());
+        std::vector<CandidateResult> res(K);
+        for (int k = 0; k < K; ++k) {
+            res[k].status = st[k];
+            if (st[k].code != KA_OK) continue;
+            Flat f = flat[k];
+            f.stride = stride;
+            const int64_t row0 = partOff[topicOff[k]];
+            res[k].topics = unflatten(f, out.data() + (size_t)row0 * stride, outLen.data() + row0);
         }
         return res;
     }
