@@ -44,6 +44,20 @@ def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
 
 
+def _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker):
+    """The ragged layout as the C ABI takes it: (topic_hash, part_off, part_id, rep_off, cur_broker) as contiguous arrays of
+    its element types; part_id may be None."""
+    return (np.ascontiguousarray(topic_hash, dtype=np.int32), np.ascontiguousarray(part_off, dtype=np.int64),
+            None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32),
+            np.ascontiguousarray(rep_off, dtype=np.int64), np.ascontiguousarray(cur_broker, dtype=np.int32))
+
+
+def _default_stride(rep_off, desired_rf):
+    """The row stride of a ragged solve when the caller gives none: max(longest current list, desired_rf, 1)."""
+    sizes = np.diff(rep_off)
+    return max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+
+
 def raise_for_status(st: KaStatus, topic_names=None):
     """Re-throw a ka_status as the reference's exception with the identical message."""
     if st.code == 0:
@@ -214,11 +228,7 @@ class Solver:
 
     def solve_ragged(self, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, out_stride, check=True,
                      topic_names=None):
-        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
-        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
-        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
-        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
-        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
         Q = int(part_off[-1]) if len(part_off) else 0
         out = np.full((Q, out_stride), -1, dtype=np.int32)
         out_len = np.zeros(Q, dtype=np.int32)
@@ -234,15 +244,10 @@ class Solver:
         """ka_solve_json: the ragged solve of solve_ragged + the reassignment JSON built on the device (KAG:169-186);
         returns (bytes-like view of the text, status). json_buf: optional writable uint8 numpy array (pinned for full
         PCIe speed); by default one of the documented sufficient size."""
-        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
-        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
-        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
-        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
-        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
         names, name_off = self.marshal_names(topic_names)
         if json_buf is None:
-            sizes = np.diff(rep_off)
-            S = max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+            S = _default_stride(rep_off, desired_rf)
             rows = np.diff(part_off)
             json_buf = np.empty(64 + int(part_off[-1]) * (50 + 12 * S) + int(np.dot(rows, np.diff(name_off))), dtype=np.uint8)
         nbytes = ctypes.c_int64(0)
@@ -300,14 +305,9 @@ class Solver:
         (broker_id, rack_index) numpy pairs), each on a fresh Context; this Solver's own Context is untouched. out_stride
         defaults to max(longest current list, desired_rf, 1). Returns (out [K, ΣP, out_stride], out_len [K, ΣP], [KaStatus] * K);
         the rows of a failed candidate are unspecified."""
-        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
-        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
-        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
-        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
-        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
         if out_stride is None:
-            sizes = np.diff(rep_off)
-            out_stride = max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+            out_stride = _default_stride(rep_off, desired_rf)
         cand_off, broker_id, broker_rack = self._candidate_tables(tables)
         K = len(tables)
         Q = int(part_off[-1]) if len(part_off) else 0
@@ -325,15 +325,10 @@ class Solver:
         None = 1 per row. Returns (summary, [KaStatus] * K), summary a numpy structured array [K] with the fields of
         ka_move_summary; then, with rows=True, (out [K, ΣP, out_stride], out_len [K, ΣP]) as solve_ragged_candidates returns
         them; then, with per_broker=True, (replicas, leaders, added): one int64 array per table, aligned with its broker ids."""
-        th = np.ascontiguousarray(topic_hash, dtype=np.int32)
-        part_off = np.ascontiguousarray(part_off, dtype=np.int64)
-        part_id = None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32)
-        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
-        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
         weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
         if out_stride is None:
-            sizes = np.diff(rep_off)
-            out_stride = max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+            out_stride = _default_stride(rep_off, desired_rf)
         cand_off, broker_id, broker_rack = self._candidate_tables(tables)
         K = len(tables)
         Q = int(part_off[-1]) if len(part_off) else 0
@@ -392,8 +387,7 @@ class Solver:
         K = len(clusters)
         cand_off, broker_id, broker_rack, topic_off, drf, th, part_off, part_id, rep_off, cur = self.marshal_clusters(clusters)
         if out_stride is None:
-            sizes = np.diff(rep_off)
-            out_stride = max(int(sizes.max()) if len(sizes) else 0, int(drf.max()) if K else -1, 1)
+            out_stride = _default_stride(rep_off, int(drf.max()) if K else -1)
         Q = int(part_off[-1])
         out = np.full((Q, out_stride), -1, dtype=np.int32)
         out_len = np.zeros(Q, dtype=np.int32)

@@ -136,8 +136,8 @@ struct ka_ctx {
     RunScratch run;   // kernel A and the chains of a single solve (and of a staged block)
     DevBuf d_json, d_names, d_name_off, d_part_id, d_json_rowlen, d_json_blocksum, d_json_state;
     // scratch of the batched solves, apart from the single solve's: descriptors + broker tables, counters, and the run
-    DevBuf d_cand_tab, d_cand_ctr;
-    RunScratch cand_run;
+    DevBuf d_batch_tab, d_batch_ctr;
+    RunScratch batch_run;
     // scratch of ka_score_candidates: row weights, the K summaries, the per-broker sums [3][ΣN], the tables' offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
     HostPinned* h_pin = nullptr;
@@ -1000,22 +1000,34 @@ int finish(ka_ctx* c, cudaStream_t s, ka_status* st, bool sync, const int32_t* p
     return st || sync ? finish_status(c, s, st, part_id, part_off) : KA_OK;
 }
 
-// A library-side failure of a batched solve: every candidate reports it.
-int fail_candidates(ka_status* st, int K, int rc) {
+// A library-side failure of a batched solve: every member reports it.
+int fail_members(ka_status* st, int K, int rc) {
     for (int k = 0; k < K; ++k) set_status(st + k, rc);
     return rc;
 }
 
 // A batched solve failed with rc after part of it was enqueued on `s` (slot-0 chains on c->sb1): wait for what was enqueued,
-// then every candidate reports rc.
-int abort_candidates(ka_ctx* c, cudaStream_t s, ka_status* st, int K, int rc) {
+// then every member reports rc.
+int abort_batch(ka_ctx* c, cudaStream_t s, ka_status* st, int K, int rc) {
     cudaStreamSynchronize(c->sb1);
     cudaStreamSynchronize(s);
-    return fail_candidates(st, K, rc);
+    return fail_members(st, K, rc);
 }
 
-// What ka_ctx_set_brokers refuses in any of the K candidate tables of a batched solve (the same code).
-int check_candidates(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack) {
+// The checks every batched call starts with. Without st or with K < 0 there is nowhere to report; otherwise every st[k] starts
+// at KA_OK and the first of these failures fails every member: no ctx, K beyond the limit or rows wider than 3 (the batched
+// chains are the slot chains of rows <= 3; wider rows take the single solve's fused chain), out_stride < 1.
+int batch_args(ka_ctx* c, int K, int out_stride, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
+    if (!c) return fail_members(st, K, KA_ERR_NO_DEVICE);
+    if (K > KA_MAX_CANDIDATES || out_stride > 3) return fail_members(st, K, KA_ERR_LIMIT);
+    if (out_stride < 1) return fail_members(st, K, KA_ERR_BAD_ARG);
+    return KA_OK;
+}
+
+// What ka_ctx_set_brokers refuses in any of the K broker tables of a batched solve (the same code).
+int check_tables(int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack) {
     if (!cand_off || cand_off[0] != 0) return KA_ERR_BAD_ARG;
     for (int k = 0; k < K; ++k) {
         const int n = cand_off[k + 1] - cand_off[k];
@@ -1026,46 +1038,8 @@ int check_candidates(int K, const int32_t* cand_off, const int32_t* broker_id, c
     return KA_OK;
 }
 
-// The device images of the candidate tables of a batched solve, and what the call's plan takes from them: counter placement
-// and loop shape from the largest table and blob, levels and load width from the largest capacity of any candidate.
-struct CandidateTables {
-    std::vector<BrokerTable> tabs;
-    int nmax = 0, blob_max = 0;
-    int64_t capmax = 0;
-};
-
-// The common part of the batched front ends, once their own checks have passed (the tables are checked and the call's `recs`
-// records are sized: K·Q for K candidates over Q rows, ΣP for a fleet): the records' limit, the ctx's device and the tables.
-// cap(k, n, capmax) gives the largest capacity of table k's problem under its n brokers, or the status that table fails with.
-template <typename Cap>
-int candidate_tables(ka_ctx* c, int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack, int64_t recs,
-                     Cap cap, CandidateTables& ct, ka_status* st) {
-    if (recs >= ((int64_t)1 << 31)) return fail_candidates(st, K, KA_ERR_LIMIT);   // positions of the call-wide level table are 32-bit
-    int rc = enter(c, true);
-    if (rc != KA_OK) return fail_candidates(st, K, rc);
-    reset_plans(c);
-    ct.tabs.resize(K);
-    for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        ct.tabs[k] = broker_table(n, broker_id + cand_off[k], broker_rack + cand_off[k]);
-        ct.nmax = std::max(ct.nmax, n);
-        ct.blob_max = std::max(ct.blob_max, ct.tabs[k].blob_bytes());
-        int64_t capk = 0;
-        if ((rc = cap(k, n, capk)) != KA_OK) return fail_candidates(st, K, rc);
-        ct.capmax = std::max(ct.capmax, capk);
-    }
-    return KA_OK;
-}
-
-// The plan of a batched solve of the problem sh (one block) under the tables ct: a limit it exceeds fails every candidate alike.
-int plan_candidates(const Shape& sh, const CandidateTables& ct, int K, StageDesc& d, ka_status* st) {
-    const int rc = describe_block(sh, 0, sh.T, 0, ct.nmax, ct.blob_max, d, st);
-    for (int k = 1; k < K && rc != KA_OK; ++k) st[k] = st[0];
-    return rc;
-}
-
-// Where one member of a batched solve reads and writes (the host side of its KaCandidate): a candidate table over the whole
-// input, or one cluster of a fleet.
+// Where one member of a batched solve reads and writes (the host side of its KaCandidate), and what its table and its slice
+// need of the call's plan: a candidate table over the whole input, or one cluster of a fleet.
 struct BatchMember {
     int tab = 0;                 // its broker table cand_off[tab] .. cand_off[tab + 1] - 1, and its status st[tab]
     int t0 = 0, T = 0;           // its topics [t0, t0 + T) of the shared input
@@ -1073,54 +1047,115 @@ struct BatchMember {
     int desired_rf = -1;
     int64_t rec0 = 0;            // its first record in the call's records = its first position in the call-wide chunk table
     int64_t topic0 = 0;          // its first topic in the call's topic tables (ntl, loff, status)
+    int n = 0, blob_bytes = 0;   // its table's brokers and blob
+    int Pmax = 0;                // its largest topic
+    int64_t capmax = 0;          // its largest capacity under its table (dense_capmax / ragged_capmax)
 };
 
-// The members of a batched solve and the call-wide sizes that follow from them.
+// A batched solve: its K broker tables, its members and the call-wide sizes that follow from them.
 struct Batch {
     int K = 0;                   // the call's K (reported by ka_ctx_last_*_plan; a fleet's refused clusters are no member)
+    const int32_t* cand_off = nullptr;   // table k: broker_id[cand_off[k] .. cand_off[k + 1]) of the call
+    const int32_t* broker_id = nullptr;
+    std::vector<BrokerTable> tabs;       // their device images
     std::vector<BatchMember> m;
-    int64_t recs = 0;            // records of the call: K·Q for candidates, ΣP for a fleet
+    int64_t recs = 0;            // records of the call, laid out as its output rows: K·Q for candidates, ΣP for a fleet
     int topics = 0;              // topics of the call's topic tables: K·T for candidates, ΣT for a fleet
     int fill_T = 0;              // ka_level_fill_kernel's view: topic u starts at record (u / fill_T)·fill_rows + part_off[u % fill_T]
     int64_t fill_rows = 0;
     int64_t out_rows = 0;        // output rows between two members: Q for candidates, 0 for a fleet (rows at their input rows)
-    int Tmax = 0;                // the largest member
-    int64_t Qmax = 0;
+    // The largest member, which the call's plan and launches are sized for: counter placement and loop shape from the largest
+    // table and blob, levels and load width from the largest capacity, grids from the most topics and rows.
+    int nmax = 0, blob_max = 0, Pmax = 0, Tmax = 0;
+    int64_t capmax = 0, Qmax = 0;
+
+    void add(const BatchMember& mb) {
+        m.push_back(mb);
+        nmax = std::max(nmax, mb.n);
+        blob_max = std::max(blob_max, mb.blob_bytes);
+        Pmax = std::max(Pmax, mb.Pmax);
+        capmax = std::max(capmax, mb.capmax);
+        Tmax = std::max(Tmax, mb.T);
+        Qmax = std::max(Qmax, mb.Q);
+    }
 };
 
-// K candidates over one problem of T topics and Q rows: every member reads the whole input, on its own copy of the records.
-Batch candidate_batch(int K, int T, int64_t Q, int desired_rf) {
-    Batch b;
+// The K tables of a batched call into b, once the call's own checks have passed (check_tables among them): the call's `recs`
+// records (K·Q for K candidates over Q rows, ΣP for a fleet) within the 32-bit positions of the call-wide level table, the
+// ctx's device, fresh plan reports, and each table's device image. A failure here fails every member.
+int batch_tables(ka_ctx* c, int K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack, int64_t recs,
+                 Batch& b, ka_status* st) {
+    if (recs >= ((int64_t)1 << 31)) return fail_members(st, K, KA_ERR_LIMIT);
+    const int rc = enter(c, true);
+    if (rc != KA_OK) return fail_members(st, K, rc);
+    reset_plans(c);
     b.K = K;
+    b.cand_off = cand_off;
+    b.broker_id = broker_id;
+    b.tabs.resize(K);
+    for (int k = 0; k < K; ++k)
+        b.tabs[k] = broker_table(cand_off[k + 1] - cand_off[k], broker_id + cand_off[k], broker_rack + cand_off[k]);
+    return KA_OK;
+}
+
+// The members of K candidates over one problem of T topics and Q rows whose largest topic has Pmax partitions, candidate k
+// with the largest capacity capmax[k] under its table: every member reads the whole input, on its own copy of the records.
+void add_candidates(Batch& b, int T, int64_t Q, int Pmax, int desired_rf, const std::vector<int64_t>& capmax) {
     const int64_t q = std::max<int64_t>(Q, 1);
-    for (int k = 0; k < K; ++k) b.m.push_back(BatchMember{k, 0, T, 0, Q, desired_rf, (int64_t)k * q, (int64_t)k * T});
-    b.recs = (int64_t)K * q;
-    b.topics = K * T;
+    for (int k = 0; k < b.K; ++k)
+        b.add(BatchMember{k, 0, T, 0, Q, desired_rf, (int64_t)k * q, (int64_t)k * T, b.cand_off[k + 1] - b.cand_off[k],
+                          b.tabs[k].blob_bytes(), Pmax, capmax[k]});
+    b.recs = (int64_t)b.K * q;
+    b.topics = b.K * T;
     b.fill_T = T;
     b.fill_rows = Q;
     b.out_rows = Q;
-    b.Tmax = T;
-    b.Qmax = Q;
-    return b;
+}
+
+// The members of a fleet of T topics over Q rows: each cluster of `passed` (those that passed ragged_scan and ragged_capmax,
+// with their slice, n, Pmax and capmax) that also passes the limits of ka_solve's own plan under its table. A cluster refused
+// there reports that limit in st[tab] and is left out, as are all clusters when none has a topic.
+void add_clusters(Batch& b, int T, int64_t Q, int S, const std::vector<BatchMember>& passed, ka_status* st) {
+    for (BatchMember mb : passed) {
+        mb.blob_bytes = b.tabs[mb.tab].blob_bytes();
+        Plan own;
+        if (make_plan(mb.n, mb.blob_bytes, mb.Q, S, mb.Pmax, mb.capmax, true, own, st + mb.tab) == KA_OK) b.add(mb);
+    }
+    // one table of the call's T topics over its Q rows: every record sits at its input row
+    b.recs = std::max<int64_t>(Q, 1);
+    b.topics = T;
+    b.fill_T = std::max(T, 1);
+    b.out_rows = 0;
+    if (b.Tmax == 0) b.m.clear();   // no topic to solve: every cluster that passed has solved (ka_solve with T == 0)
+}
+
+// The plan of a batched solve of the problem sh (one block), sized for the batch's largest member: a limit it exceeds fails
+// every st[k] alike.
+int plan_batch(Shape sh, const Batch& b, StageDesc& d, ka_status* st) {
+    sh.Pmax = b.Pmax;
+    sh.capmax = b.capmax;
+    const int rc = describe_block(sh, 0, sh.T, 0, b.nmax, b.blob_max, d, st);
+    for (int k = 1; k < b.K && rc != KA_OK; ++k) st[k] = st[0];
+    return rc;
 }
 
 // Wait for a batched solve enqueued on `s` and fill every member's status: its lowest failing topic, as finish_status
 // reports it for one solve (relative to the member's first topic; part_id / part_off of a ragged solve: the failing
 // partition's id). Statuses already in st (a fleet's refused clusters) stay. Returns the code of the lowest failing st[k].
-int finish_candidates(ka_ctx* c, cudaStream_t s, const Batch& b, ka_status* st, const int32_t* part_id = nullptr,
-                      const int64_t* part_off = nullptr) {
+int finish_batch(ka_ctx* c, cudaStream_t s, const Batch& b, ka_status* st, const int32_t* part_id = nullptr,
+                 const int64_t* part_off = nullptr) {
     const int K = b.K, M = (int)b.m.size();
-    if (cudaStreamSynchronize(s) != cudaSuccess) return fail_candidates(st, K, KA_ERR_CUDA);
+    if (cudaStreamSynchronize(s) != cudaSuccess) return fail_members(st, K, KA_ERR_CUDA);
     std::vector<unsigned> err(std::max(M, 1));
-    if (M > 0 && cudaMemcpy(err.data(), c->cand_run.flags.p, (size_t)M * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
-        return fail_candidates(st, K, KA_ERR_CUDA);
+    if (M > 0 && cudaMemcpy(err.data(), c->batch_run.flags.p, (size_t)M * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+        return fail_members(st, K, KA_ERR_CUDA);
     for (int k = 0; k < M; ++k) {
         if (err[k] == 0xFFFFFFFFu) continue;
         const BatchMember& mb = b.m[k];
         const int t = (int)err[k] - mb.t0;   // kernel A reports the input topic
         int4 ts;
-        if (cudaMemcpy(&ts, c->cand_run.tstatus.as<int4>() + mb.topic0 + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
-            return fail_candidates(st, K, KA_ERR_CUDA);
+        if (cudaMemcpy(&ts, c->batch_run.tstatus.as<int4>() + mb.topic0 + t, sizeof(int4), cudaMemcpyDeviceToHost) != cudaSuccess)
+            return fail_members(st, K, KA_ERR_CUDA);
         st[mb.tab] = topic_status(mb.t0 + t, ts, part_id, part_off);
         st[mb.tab].topic_index = t;
     }
@@ -1209,11 +1244,11 @@ void ka_ctx_destroy(ka_ctx* c) {
         if (s) cudaStreamSynchronize(s);
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
                       &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
-                      &c->d_json_blocksum, &c->d_json_state, &c->d_cand_tab, &c->d_cand_ctr, &c->d_score_w, &c->d_score_sum,
+                      &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
                       &c->d_score_brk, &c->d_score_off})
         b->release();
     c->run.release();
-    c->cand_run.release();
+    c->batch_run.release();
     for_each_event(c, [](cudaEvent_t& e, bool) {
         if (e) cudaEventDestroy(e);
     });
@@ -1366,8 +1401,7 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
 // chain sub-block the slot-0 / slot-1 chains (one CTA per member) and the emit (grid.y = member). `d` is a dense problem or a
 // ragged one (d.d_part_off set: one chain sub-block, as in a ragged single solve); its inputs are shared by every member, each
 // of which reads its own window of them.
-static int enq_candidates(ka_ctx* c, cudaStream_t s, const Batch& bt, const std::vector<BrokerTable>& tabs, const int32_t* cand_off,
-                          const int32_t* broker_id, const StageDesc& d, int32_t* d_out_len, int32_t* d_out) {
+static int enq_batch(ka_ctx* c, cudaStream_t s, const Batch& bt, const StageDesc& d, int32_t* d_out_len, int32_t* d_out) {
     const Plan& pl = d.pl;
     const int S = d.S, K = (int)bt.m.size();
     const size_t kq = (size_t)bt.recs, kt = (size_t)bt.topics;
@@ -1376,34 +1410,33 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, const Batch& bt, const std:
     size_t bytes = align16((size_t)K * sizeof(KaCandidate)), ctr_ints = 0;
     int64_t covered = 0;   // topics kernel A walks
     for (int k = 0; k < K; ++k) {
-        const int tab = bt.m[k].tab, n = cand_off[tab + 1] - cand_off[tab];
+        const BatchMember& mb = bt.m[k];
         blob_off[k] = bytes;
-        bytes += tabs[tab].blob.size() * 2;
+        bytes += bt.tabs[mb.tab].blob.size() * 2;
         glut_off[k] = bytes;
-        bytes += align16(tabs[tab].glut.size() * 2);
+        bytes += align16(bt.tabs[mb.tab].glut.size() * 2);
         bid_off[k] = bytes;
-        bytes += align16((size_t)std::max(n, 1) * 4);
+        bytes += align16((size_t)std::max(mb.n, 1) * 4);
         ctr_off[k] = ctr_ints;
-        ctr_ints += (size_t)(n + 1) * KA_MAX_SLOTS;   // + the chains' dummy row
-        covered += bt.m[k].T;
+        ctr_ints += (size_t)(mb.n + 1) * KA_MAX_SLOTS;   // + the chains' dummy row
+        covered += mb.T;
     }
-    RunScratch& r = c->cand_run;
-    KA_CUDA(c->d_cand_tab.reserve(bytes));
-    KA_CUDA(c->d_cand_ctr.reserve(ctr_ints * 4));
+    RunScratch& r = c->batch_run;
+    KA_CUDA(c->d_batch_tab.reserve(bytes));
+    KA_CUDA(c->d_batch_ctr.reserve(ctr_ints * 4));
     KA_CUDA(r.reserve(kq * 16, kq, kt, kt + 1, pl.a_levels, K));
-    unsigned char* base = c->d_cand_tab.as<unsigned char>();
+    unsigned char* base = c->d_batch_tab.as<unsigned char>();
     std::vector<unsigned char> h(bytes, 0);
     int lut_mask = 0;
     for (int k = 0; k < K; ++k) {
         const BatchMember& mb = bt.m[k];
-        const int n = cand_off[mb.tab + 1] - cand_off[mb.tab];
-        const BrokerTable& t = tabs[mb.tab];
+        const BrokerTable& t = bt.tabs[mb.tab];
         // kernel A writes the member's records, perm and lend by input row, its ntl and status by input topic
         const int64_t shift = mb.rec0 - mb.row0, tshift = mb.topic0 - mb.t0;
         KaCandidate e{};
-        e.br = t.device(n, reinterpret_cast<const uint16_t*>(base + blob_off[k]), reinterpret_cast<const uint16_t*>(base + glut_off[k]),
-                        reinterpret_cast<const int32_t*>(base + bid_off[k]));
-        e.ctr8 = c->d_cand_ctr.as<int32_t>() + ctr_off[k];
+        e.br = t.device(mb.n, reinterpret_cast<const uint16_t*>(base + blob_off[k]),
+                        reinterpret_cast<const uint16_t*>(base + glut_off[k]), reinterpret_cast<const int32_t*>(base + bid_off[k]));
+        e.ctr8 = c->d_batch_ctr.as<int32_t>() + ctr_off[k];
         e.out.rec = r.rec.as<unsigned char>() + shift * 16;
         if (pl.a_levels) {
             e.out.perm = r.perm.as<uint16_t>() + shift;
@@ -1422,12 +1455,12 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, const Batch& bt, const std:
         std::memcpy(h.data() + (size_t)k * sizeof(KaCandidate), &e, sizeof(e));
         std::memcpy(h.data() + blob_off[k], t.blob.data(), t.blob.size() * 2);
         if (!t.glut.empty()) std::memcpy(h.data() + glut_off[k], t.glut.data(), t.glut.size() * 2);
-        if (n > 0) std::memcpy(h.data() + bid_off[k], broker_id + cand_off[mb.tab], (size_t)n * 4);
+        if (mb.n > 0) std::memcpy(h.data() + bid_off[k], bt.broker_id + bt.cand_off[mb.tab], (size_t)mb.n * 4);
         lut_mask |= 1 << t.lut_mode;
     }
-    const KaCandidate* cand = c->d_cand_tab.as<KaCandidate>();
+    const KaCandidate* cand = c->d_batch_tab.as<KaCandidate>();
     KA_CUDA(cudaMemcpyAsync(base, h.data(), bytes, cudaMemcpyHostToDevice, s));
-    KA_CUDA(cudaMemsetAsync(c->d_cand_ctr.p, 0, ctr_ints * 4, s));   // every member starts from a fresh Context
+    KA_CUDA(cudaMemsetAsync(c->d_batch_ctr.p, 0, ctr_ints * 4, s));   // every member starts from a fresh Context
     KA_CUDA(cudaMemsetAsync(r.flags.p, 0xFF, (size_t)K * 4, s));
     // topics no member walks (a fleet's refused clusters) have no chunks
     if (pl.a_levels && covered < bt.topics) KA_CUDA(cudaMemsetAsync(r.ntl.p, 0, kt * 4, s));
@@ -1485,40 +1518,44 @@ static int enq_candidates(ka_ctx* c, cudaStream_t s, const Batch& bt, const std:
     return KA_OK;
 }
 
+// The batched solve planned as d, enqueued on `s`: the host inputs H2D when io has any (ncur current replicas), the batch, and
+// the rows of every member D2H when io has a host destination. A failure after something was enqueued fails every member.
+static int run_batch(ka_ctx* c, cudaStream_t s, const Batch& bt, const StageDesc& d, int64_t ncur, const SolveCall& io,
+                     ka_status* st) {
+    int rc;
+    if ((rc = enq_inputs(s, io, d, ncur)) != KA_OK || (rc = enq_batch(c, s, bt, d, io.d_out_len, io.d_out)) != KA_OK ||
+        (io.h_out && d.Q > 0 && (rc = enq_copy_out(s, io, d.S, 0, bt.recs)) != KA_OK))
+        return abort_batch(c, s, st, bt.K, rc);
+    return KA_OK;
+}
+
 int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
                                          const int32_t* broker_rack, int32_t T, const int32_t* d_topic_hash, int32_t P,
                                          int32_t RF, const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride,
                                          int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
-    if (!st || K < 0) return KA_ERR_BAD_ARG;
-    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
-    auto all = [&](int rc) { return fail_candidates(st, K, rc); };
-    if (!c) return all(KA_ERR_NO_DEVICE);
-    if (K > KA_MAX_CANDIDATES || out_stride > 3) return all(KA_ERR_LIMIT);   // wider rows: the fused chain of the single solve
-    if (T < 0 || P < 0 || RF < 0 || out_stride < 1 || out_stride < std::max(RF, desired_rf)) return all(KA_ERR_BAD_ARG);
+    int rc = batch_args(c, K, out_stride, st);
+    if (rc != KA_OK) return rc;
+    if (T < 0 || P < 0 || RF < 0 || out_stride < std::max(RF, desired_rf)) return fail_members(st, K, KA_ERR_BAD_ARG);
     if (K == 0) return KA_OK;
-    int rc = check_candidates(K, cand_off, broker_id, broker_rack);
-    if (rc != KA_OK) return all(rc);
+    if ((rc = check_tables(K, cand_off, broker_id, broker_rack)) != KA_OK) return fail_members(st, K, rc);
     if (T == 0) return KA_OK;
     const int64_t Q = (int64_t)T * P;
-    if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return all(KA_ERR_BAD_ARG);
+    if (!d_topic_hash || (Q * RF > 0 && !d_cur_broker) || (Q > 0 && !d_out_broker)) return fail_members(st, K, KA_ERR_BAD_ARG);
+    Batch bt;
+    if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, bt, st)) != KA_OK) return rc;
     // levels if any candidate that can serve the target RF has capacity > 1 (one that cannot fails alone, whatever the plan)
     const int rf_t = desired_rf >= 0 ? desired_rf : RF;
-    auto cap = [&](int, int n, int64_t& capmax) {
-        capmax = dense_capmax(P, rf_t, n);
-        return KA_OK;
-    };
-    CandidateTables ct;
-    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, cap, ct, st)) != KA_OK) return rc;
-    Shape sh{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker};
-    sh.Pmax = P;
-    sh.capmax = ct.capmax;
-    StageDesc d;
-    if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
+    std::vector<int64_t> cap(K);
+    for (int k = 0; k < K; ++k) cap[k] = dense_capmax(P, rf_t, cand_off[k + 1] - cand_off[k]);
+    add_candidates(bt, T, Q, P, desired_rf, cap);
+    const Shape sh{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker};
+    SolveCall io;
+    io.d_out = d_out_broker;
+    io.d_out_len = d_out_len;
     cudaStream_t s = (cudaStream_t)stream;
-    const Batch bt = candidate_batch(K, T, Q, desired_rf);
-    if ((rc = enq_candidates(c, s, bt, ct.tabs, cand_off, broker_id, d, d_out_len, d_out_broker)) != KA_OK)
-        return abort_candidates(c, s, st, K, rc);
-    return finish_candidates(c, s, bt, st);
+    StageDesc d;
+    if ((rc = plan_batch(sh, bt, d, st)) != KA_OK || (rc = run_batch(c, s, bt, d, 0, io, st)) != KA_OK) return rc;
+    return finish_batch(c, s, bt, st);
 }
 
 int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash, int32_t P, int32_t RF,
@@ -1861,87 +1898,52 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
     return stream_json(c, s, io, json, json_cap, json_bytes, st, part_id, part_off);
 }
 
-// One ragged batched solve as ka_solve_candidates runs it, up to and including the emit, enqueued on c->stream.
-struct CandidateRun {
-    bool tables_ok = false;   // the candidate tables passed their checks (cand_off may be read)
-    bool enqueued = false;    // false: an error (returned, every st[k] set) or nothing to solve (K == 0 or T == 0)
-    int64_t Q = 0;
-    Batch bt;                 // the candidates as members of the batched solve
-    SolveCall io;             // d_out / d_out_len: the rows of all candidates, [K][Q] on the device
-};
-
-// The checks, the sizing scan and plan, the inputs H2D and the batched solve of ka_solve_candidates, for both entry points.
-// have_out: the caller has somewhere to put the rows. part_weight: ka_score_candidates' weights, checked once every check of
-// ka_solve_candidates has passed and before anything is enqueued (negative: KA_ERR_BAD_ARG; 3 x their sum beyond INT64_MAX:
-// KA_ERR_LIMIT).
-static int enq_ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
-                                 int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
-                                 const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride, bool have_out,
-                                 const int64_t* part_weight, CandidateRun& run, ka_status* st) {
-    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
-    auto all = [&](int rc) { return fail_candidates(st, K, rc); };
-    if (!c) return all(KA_ERR_NO_DEVICE);
-    if (K > KA_MAX_CANDIDATES || out_stride > 3) return all(KA_ERR_LIMIT);   // wider rows: the fused chain of the single solve
-    if (T < 0 || (T > 0 && (!topic_hash || !part_off)) || out_stride < 1) return all(KA_ERR_BAD_ARG);
-    if (K == 0) return KA_OK;
-    int rc = check_candidates(K, cand_off, broker_id, broker_rack);
-    if (rc != KA_OK) return all(rc);
-    run.tables_ok = true;
-    if (T == 0) return KA_OK;
-    // malformed offsets: every candidate reports what ka_solve reports for its table
-    RaggedScan sc;
-    ka_status sst{};
-    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, false, have_out, sc, &sst)) != KA_OK) {
-        for (int k = 0; k < K; ++k) st[k] = sst;
-        return rc;
-    }
-    if (sc.err.code != KA_OK) {
-        int64_t cap = 0;
-        for (int k = 0; k < K; ++k) ragged_capmax(sc, cand_off[k + 1] - cand_off[k], cap, st + k);
-        return st[0].code;
-    }
-    // the stride holds every current list and the desired RF: every candidate's ka_solve would accept the call's input
-    if (out_stride < std::max<int64_t>(sc.maxsz, desired_rf)) return all(KA_ERR_BAD_ARG);
-    const int64_t Q = sc.Q;
-    // the plan of the call: the largest capacity of any candidate
-    auto cap = [&](int, int n, int64_t& capmax) { return ragged_capmax(sc, n, capmax, nullptr); };
-    CandidateTables ct;
-    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, cap, ct, st)) != KA_OK) return rc;
-    const size_t q = (size_t)std::max<int64_t>(Q, 1);
-    if ((rc = reserve_io(c, T, Q, sc.R, out_stride, true)) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
-        c->d_out_len.reserve((size_t)K * q * 4) != cudaSuccess)
-        return all(KA_ERR_CUDA);
-    const Shape sh{T, 0, 0, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-                   c->d_rep_off.as<int64_t>(), Q, sc.R, sc.Pmax, ct.capmax};
-    StageDesc d;
-    if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
-    if (part_weight) {
-        bool negative = false;
-        int64_t sum = 0;   // saturates above INT64_MAX / 3
-        for (int64_t g = 0; g < Q; ++g) {
-            const int64_t w = part_weight[g];
-            negative |= w < 0;
-            sum = w > INT64_MAX / 3 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
-        }
-        if (negative) return all(KA_ERR_BAD_ARG);
-        if (sum > INT64_MAX / 3) return all(KA_ERR_LIMIT);
-    }
-    // the inputs go up once and are shared by every candidate
-    SolveCall& io = run.io;
+// The host inputs and rows of a ragged batched solve: the ctx's device copies of them, and the caller's buffers.
+static SolveCall batch_io(ka_ctx* c, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
+                          const int32_t* cur_broker, int32_t* out_len, int32_t* out_broker) {
+    SolveCall io;
     io.h_hash = topic_hash;
     io.h_part_off = part_off;
     io.h_rep_off = rep_off;
     io.h_cur = cur_broker;
     io.d_out = c->d_out.as<int32_t>();
     io.d_out_len = c->d_out_len.as<int32_t>();
-    run.Q = Q;
-    run.bt = candidate_batch(K, T, Q, desired_rf);
-    run.enqueued = true;
-    if ((rc = enq_inputs(c->stream, io, d, sc.R)) != KA_OK ||
-        (rc = enq_candidates(c, c->stream, run.bt, ct.tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK) {
-        run.enqueued = false;
-        return abort_candidates(c, c->stream, st, K, rc);
+    io.h_out = out_broker;
+    io.h_out_len = out_len;
+    return io;
+}
+
+// ka_solve_candidates and ka_score_candidates once their tables have passed check_tables, up to their plan: the sizing scan,
+// the stride check, the tables and the candidates (bt), and the call's device inputs and rows (sh). bt has no member when
+// there is nothing to solve (T == 0). have_out: as in ragged_scan.
+static int ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                             int32_t T, const int64_t* part_off, const int64_t* rep_off, const int32_t* cur_broker,
+                             int32_t desired_rf, int32_t out_stride, bool have_out, Batch& bt, Shape& sh, ka_status* st) {
+    if (T == 0) return KA_OK;
+    // malformed offsets: every candidate reports what ka_solve reports for its table
+    RaggedScan sc;
+    ka_status sst{};
+    int rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, false, have_out, sc, &sst);
+    if (rc != KA_OK) {
+        for (int k = 0; k < K; ++k) st[k] = sst;
+        return rc;
     }
+    // each table's capacity bound, or the status ka_solve reports for it; a table fails only with malformed offsets or a topic
+    // whose target RF exceeds the stride, which the stride check below refuses for every candidate
+    std::vector<int64_t> cap(K);
+    for (int k = 0; k < K; ++k) ragged_capmax(sc, cand_off[k + 1] - cand_off[k], cap[k], st + k);
+    if (sc.err.code != KA_OK) return st[0].code;
+    // the stride holds every current list and the desired RF: every candidate's ka_solve would accept the call's input
+    if (out_stride < std::max<int64_t>(sc.maxsz, desired_rf)) return fail_members(st, K, KA_ERR_BAD_ARG);
+    const int64_t Q = sc.Q;
+    if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, bt, st)) != KA_OK) return rc;
+    add_candidates(bt, T, Q, sc.Pmax, desired_rf, cap);
+    const size_t q = (size_t)std::max<int64_t>(Q, 1);
+    if (reserve_io(c, T, Q, sc.R, out_stride, true) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
+        c->d_out_len.reserve((size_t)K * q * 4) != cudaSuccess)
+        return fail_members(st, K, KA_ERR_CUDA);
+    sh = Shape{T, 0, 0, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
+               c->d_rep_off.as<int64_t>(), Q, sc.R};
     return KA_OK;
 }
 
@@ -1956,118 +1958,83 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
                             int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
                             const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride,
                             int32_t* out_len, int32_t* out_broker, ka_status* st) {
-    if (!st || K < 0) return KA_ERR_BAD_ARG;
-    CandidateRun run;
-    int rc = enq_ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, topic_hash, part_off, rep_off, cur_broker, desired_rf,
-                                   out_stride, out_broker != nullptr, nullptr, run, st);
-    if (!run.enqueued) return rc;
-    // the rows of all candidates come back in one copy
-    run.io.h_out = out_broker;
-    run.io.h_out_len = out_len;
-    if (run.Q > 0 && (rc = enq_copy_out(c->stream, run.io, out_stride, 0, (int64_t)K * run.Q)) != KA_OK)
-        return abort_candidates(c, c->stream, st, K, rc);
-    return finish_candidates(c, c->stream, run.bt, st, part_id, part_off);
+    int rc = batch_args(c, K, out_stride, st);
+    if (rc != KA_OK) return rc;
+    if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return fail_members(st, K, KA_ERR_BAD_ARG);
+    if (K == 0) return KA_OK;
+    if ((rc = check_tables(K, cand_off, broker_id, broker_rack)) != KA_OK) return fail_members(st, K, rc);
+    Batch bt;
+    Shape sh;
+    StageDesc d;
+    // the inputs go up once and are shared by every candidate; the rows of all candidates come back in one copy
+    if ((rc = ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, part_off, rep_off, cur_broker, desired_rf, out_stride,
+                                out_broker != nullptr, bt, sh, st)) != KA_OK || bt.m.empty() ||
+        (rc = plan_batch(sh, bt, d, st)) != KA_OK ||
+        (rc = run_batch(c, c->stream, bt, d, sh.R, batch_io(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker), st)) !=
+            KA_OK)
+        return rc;
+    return finish_batch(c, c->stream, bt, st, part_id, part_off);
 }
 
 int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
                           const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
                           const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
                           int32_t* out_len, int32_t* out_broker, ka_status* st) {
-    if (!st || K < 0) return KA_ERR_BAD_ARG;
-    for (int k = 0; k < K; ++k) set_status(st + k, KA_OK);
-    auto all = [&](int rc) { return fail_candidates(st, K, rc); };
-    if (!c) return all(KA_ERR_NO_DEVICE);
-    if (out_stride > 3 || K > KA_MAX_CANDIDATES) return all(KA_ERR_LIMIT);   // rows of <= 3 replicas, as the candidate calls
-    if (out_stride < 1) return all(KA_ERR_BAD_ARG);
+    int rc = batch_args(c, K, out_stride, st);
+    if (rc != KA_OK) return rc;
     if (K == 0) return KA_OK;
-    int rc = check_candidates(K, cand_off, broker_id, broker_rack);
-    if (rc != KA_OK) return all(rc);
+    if ((rc = check_tables(K, cand_off, broker_id, broker_rack)) != KA_OK) return fail_members(st, K, rc);
     // the clusters' boundaries: topic_off, then part_off at their first topics and rep_off at their first rows, each
     // non-decreasing from 0
-    if (!topic_off || topic_off[0] != 0) return all(KA_ERR_BAD_ARG);
+    if (!topic_off || topic_off[0] != 0) return fail_members(st, K, KA_ERR_BAD_ARG);
     for (int k = 0; k < K; ++k)
-        if (topic_off[k + 1] < topic_off[k]) return all(KA_ERR_BAD_ARG);
+        if (topic_off[k + 1] < topic_off[k]) return fail_members(st, K, KA_ERR_BAD_ARG);
     const int T = topic_off[K];
-    if (T > 0 && (!topic_hash || !part_off)) return all(KA_ERR_BAD_ARG);
+    if (T > 0 && (!topic_hash || !part_off)) return fail_members(st, K, KA_ERR_BAD_ARG);
     std::vector<int64_t> row0(K + 1, 0), rep0(K + 1, 0);
     for (int k = 0; k <= K; ++k) {
         row0[k] = T > 0 ? part_off[topic_off[k]] : 0;
-        if (row0[k] < (k > 0 ? row0[k - 1] : 0) || row0[0] != 0) return all(KA_ERR_BAD_ARG);
+        if (row0[k] < (k > 0 ? row0[k - 1] : 0) || row0[0] != 0) return fail_members(st, K, KA_ERR_BAD_ARG);
     }
     const int64_t Q = row0[K];
-    if (Q > 0 && !rep_off) return all(KA_ERR_BAD_ARG);
+    if (Q > 0 && !rep_off) return fail_members(st, K, KA_ERR_BAD_ARG);
     for (int k = 0; k <= K; ++k) {
         rep0[k] = Q > 0 ? rep_off[row0[k]] : 0;
-        if (rep0[k] < (k > 0 ? rep0[k - 1] : 0) || rep0[0] != 0) return all(KA_ERR_BAD_ARG);
+        if (rep0[k] < (k > 0 ? rep0[k - 1] : 0) || rep0[0] != 0) return fail_members(st, K, KA_ERR_BAD_ARG);
     }
-    if (Q >= ((int64_t)1 << 31)) return all(KA_ERR_LIMIT);
+    if (Q >= ((int64_t)1 << 31)) return fail_members(st, K, KA_ERR_LIMIT);
     // every cluster's slice, checked and sized as ka_solve checks and sizes it against the cluster's table: a cluster that
     // fails here reports what ka_solve reports and is left out of the call
-    std::vector<RaggedScan> sc(K);
-    std::vector<int64_t> capk(K, 0);
-    std::vector<char> ok(K, 0);
+    std::vector<BatchMember> passed;
     for (int k = 0; k < K; ++k) {
         const int t0 = topic_off[k];
-        ok[k] = ragged_scan(topic_off[k + 1] - t0, part_off ? part_off + t0 : nullptr, rep_off ? rep_off + row0[k] : nullptr,
-                            cur_broker ? cur_broker + rep0[k] : nullptr, desired_rf ? desired_rf[k] : -1, out_stride, false,
-                            out_broker != nullptr, sc[k], st + k, row0[k], rep0[k]) == KA_OK &&
-                ragged_capmax(sc[k], cand_off[k + 1] - cand_off[k], capk[k], st + k) == KA_OK;
-    }
-    auto cap = [&](int k, int, int64_t& capmax) {
-        capmax = ok[k] ? capk[k] : 0;
-        return KA_OK;
-    };
-    CandidateTables ct;
-    if ((rc = candidate_tables(c, K, cand_off, broker_id, broker_rack, Q, cap, ct, st)) != KA_OK) return rc;
-    // the limits of ka_solve's own plan per cluster; the call's plan is sized from the clusters that pass them
-    Batch bt;
-    bt.K = K;
-    ct.nmax = ct.blob_max = 0;
-    ct.capmax = 0;
-    int Pmax = 0;
-    for (int k = 0; k < K; ++k) {
-        const int n = cand_off[k + 1] - cand_off[k];
-        Plan own;
-        if (!ok[k] || make_plan(n, ct.tabs[k].blob_bytes(), sc[k].Q, out_stride, sc[k].Pmax, capk[k], true, own, st + k) != KA_OK)
+        BatchMember mb{k, t0, topic_off[k + 1] - t0, row0[k], 0, desired_rf ? desired_rf[k] : -1, row0[k], t0};
+        mb.n = cand_off[k + 1] - cand_off[k];
+        RaggedScan sc;
+        if (ragged_scan(mb.T, part_off ? part_off + t0 : nullptr, rep_off ? rep_off + row0[k] : nullptr,
+                        cur_broker ? cur_broker + rep0[k] : nullptr, mb.desired_rf, out_stride, false, out_broker != nullptr, sc,
+                        st + k, row0[k], rep0[k]) != KA_OK ||
+            ragged_capmax(sc, mb.n, mb.capmax, st + k) != KA_OK)
             continue;
-        const int t0 = topic_off[k];
-        bt.m.push_back(BatchMember{k, t0, topic_off[k + 1] - t0, row0[k], sc[k].Q, desired_rf ? desired_rf[k] : -1, row0[k], t0});
-        ct.nmax = std::max(ct.nmax, n);
-        ct.blob_max = std::max(ct.blob_max, ct.tabs[k].blob_bytes());
-        ct.capmax = std::max(ct.capmax, capk[k]);
-        Pmax = std::max(Pmax, sc[k].Pmax);
-        bt.Tmax = std::max(bt.Tmax, topic_off[k + 1] - t0);
-        bt.Qmax = std::max(bt.Qmax, sc[k].Q);
+        mb.Q = sc.Q;
+        mb.Pmax = sc.Pmax;
+        passed.push_back(mb);
     }
-    // one table of the call's T topics over its Q rows: every record sits at its input row
-    bt.recs = std::max<int64_t>(Q, 1);
-    bt.topics = T;
-    bt.fill_T = std::max(T, 1);
-    bt.out_rows = 0;
-    if (bt.Tmax == 0) bt.m.clear();   // no topic to solve: every cluster that passed has solved (ka_solve with T == 0)
-    if (bt.m.empty()) return finish_candidates(c, c->stream, bt, st);
+    Batch bt;
+    if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, Q, bt, st)) != KA_OK) return rc;
+    add_clusters(bt, T, Q, out_stride, passed, st);
+    if (bt.m.empty()) return finish_batch(c, c->stream, bt, st);
     const int64_t R = rep0[K];
-    if (reserve_io(c, T, Q, R, out_stride, true) != KA_OK) return all(KA_ERR_CUDA);
+    if (reserve_io(c, T, Q, R, out_stride, true) != KA_OK) return fail_members(st, K, KA_ERR_CUDA);
     const Shape sh{T, 0, 0, -1, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-                   c->d_rep_off.as<int64_t>(), Q, R, Pmax, ct.capmax};
-    StageDesc d;
-    if ((rc = plan_candidates(sh, ct, K, d, st)) != KA_OK) return rc;
+                   c->d_rep_off.as<int64_t>(), Q, R};
     // the inputs of every cluster go up at once; the rows of all clusters come back in one copy
-    SolveCall io;
-    io.h_hash = topic_hash;
-    io.h_part_off = part_off;
-    io.h_rep_off = rep_off;
-    io.h_cur = cur_broker;
-    io.d_out = c->d_out.as<int32_t>();
-    io.d_out_len = c->d_out_len.as<int32_t>();
-    io.h_out = out_broker;
-    io.h_out_len = out_len;
-    cudaStream_t s = c->stream;
-    if ((rc = enq_inputs(s, io, d, R)) != KA_OK ||
-        (rc = enq_candidates(c, s, bt, ct.tabs, cand_off, broker_id, d, io.d_out_len, io.d_out)) != KA_OK ||
-        (Q > 0 && out_broker && (rc = enq_copy_out(s, io, out_stride, 0, Q)) != KA_OK))
-        return abort_candidates(c, s, st, K, rc);
-    return finish_candidates(c, s, bt, st, part_id, part_off);
+    StageDesc d;
+    if ((rc = plan_batch(sh, bt, d, st)) != KA_OK ||
+        (rc = run_batch(c, c->stream, bt, d, R, batch_io(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker), st)) !=
+            KA_OK)
+        return rc;
+    return finish_batch(c, c->stream, bt, st, part_id, part_off);
 }
 
 int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
@@ -2076,58 +2043,70 @@ int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
                             const int64_t* part_weight, ka_move_summary* summary, int64_t* broker_replicas,
                             int64_t* broker_leaders, int64_t* broker_in, int32_t* out_len, int32_t* out_broker, ka_status* st) {
     if (!st || K < 0) return KA_ERR_BAD_ARG;
-    if (!summary) return fail_candidates(st, K, KA_ERR_BAD_ARG);
+    if (!summary) return fail_members(st, K, KA_ERR_BAD_ARG);
     for (int k = 0; k < K; ++k) summary[k] = empty_summary();
-    CandidateRun run;
-    int rc = enq_ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, topic_hash, part_off, rep_off, cur_broker, desired_rf,
-                                   out_stride, true, part_weight, run, st);
+    int rc = batch_args(c, K, out_stride, st);
+    if (rc != KA_OK) return rc;
+    if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return fail_members(st, K, KA_ERR_BAD_ARG);
+    if (K == 0) return KA_OK;
+    if ((rc = check_tables(K, cand_off, broker_id, broker_rack)) != KA_OK) return fail_members(st, K, rc);
     int64_t* const brk[3] = {broker_replicas, broker_leaders, broker_in};
-    const size_t nb = run.tables_ok ? (size_t)cand_off[K] : 0;
-    if (!run.enqueued) {
-        for (int64_t* a : brk)
-            if (a && nb > 0) std::memset(a, 0, nb * 8);
-        return rc;
-    }
-    cudaStream_t s = c->stream;
-    const int64_t Q = run.Q;
+    const size_t nb = (size_t)cand_off[K];
+    // without a result every summary is empty and every per-broker sum 0
     auto fail = [&](int code) {
-        abort_candidates(c, s, st, K, code);
         for (int k = 0; k < K; ++k) summary[k] = empty_summary();
         for (int64_t* a : brk)
             if (a && nb > 0) std::memset(a, 0, nb * 8);
         return code;
     };
+    Batch bt;
+    Shape sh;
+    StageDesc d;
+    if ((rc = ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, part_off, rep_off, cur_broker, desired_rf, out_stride, true,
+                                bt, sh, st)) != KA_OK || bt.m.empty() || (rc = plan_batch(sh, bt, d, st)) != KA_OK)
+        return fail(rc);
+    const int64_t Q = sh.Q;
+    // the weights, once every check of ka_solve_candidates has passed and before anything is enqueued
+    if (part_weight) {
+        bool negative = false;
+        int64_t sum = 0;   // saturates above INT64_MAX / 3
+        for (int64_t g = 0; g < Q; ++g) {
+            const int64_t w = part_weight[g];
+            negative |= w < 0;
+            sum = w > INT64_MAX / 3 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
+        }
+        if (negative) return fail(fail_members(st, K, KA_ERR_BAD_ARG));
+        if (sum > INT64_MAX / 3) return fail(fail_members(st, K, KA_ERR_LIMIT));
+    }
+    cudaStream_t s = c->stream;
+    const SolveCall io = batch_io(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
+    if ((rc = run_batch(c, s, bt, d, sh.R, io, st)) != KA_OK) return fail(rc);
+    auto abort = [&](int code) { return fail(abort_batch(c, s, st, K, code)); };
     const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
     if (c->d_score_sum.reserve(sum_bytes) != cudaSuccess || c->d_score_brk.reserve(std::max<size_t>(3 * nb, 1) * 8) != cudaSuccess ||
         c->d_score_off.reserve((size_t)(K + 1) * 4) != cudaSuccess ||
         (part_weight && c->d_score_w.reserve((size_t)std::max<int64_t>(Q, 1) * 8) != cudaSuccess))
-        return fail(KA_ERR_CUDA);
+        return abort(KA_ERR_CUDA);
     ka_move_summary* d_sum = c->d_score_sum.as<ka_move_summary>();
     long long* d_brk = c->d_score_brk.as<long long>();
     const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
     if ((part_weight && Q > 0 && cudaMemcpyAsync(c->d_score_w.p, part_weight, (size_t)Q * 8, cudaMemcpyHostToDevice, s) != cudaSuccess) ||
         cudaMemcpyAsync(c->d_score_off.p, cand_off, (size_t)(K + 1) * 4, cudaMemcpyHostToDevice, s) != cudaSuccess ||
         cudaMemsetAsync(d_sum, 0, sum_bytes, s) != cudaSuccess || cudaMemsetAsync(d_brk, 0, std::max<size_t>(3 * nb, 1) * 8, s) != cudaSuccess)
-        return fail(KA_ERR_CUDA);
-    const KaCandidate* cand = c->d_cand_tab.as<KaCandidate>();
+        return abort(KA_ERR_CUDA);
+    const KaCandidate* cand = c->d_batch_tab.as<KaCandidate>();
     const int32_t* d_off = c->d_score_off.as<int32_t>();
     const dim3 grid((unsigned)std::max<int64_t>((Q + 255) / 256, 1), K);
-    ka_score_rows_kernel<<<grid, 256, 0, s>>>(cand, d_off, (uint32_t)Q, out_stride, run.io.d_out, run.io.d_out_len,
-                                              c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), d_w, d_sum, d_brk, d_brk + nb,
-                                              d_brk + 2 * nb);
+    ka_score_rows_kernel<<<grid, 256, 0, s>>>(cand, d_off, (uint32_t)Q, out_stride, io.d_out, io.d_out_len, c->d_rep_off.as<int64_t>(),
+                                              c->d_cur.as<int32_t>(), d_w, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb);
     ka_score_finish_kernel<<<K, 256, 0, s>>>(cand, d_off, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb);
     c->launches += 2;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(summary, d_sum, sum_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-        return fail(KA_ERR_CUDA);
+        return abort(KA_ERR_CUDA);
     for (int i = 0; i < 3; ++i)
         if (brk[i] && nb > 0 && cudaMemcpyAsync(brk[i], d_brk + i * nb, nb * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-            return fail(KA_ERR_CUDA);
-    if (out_broker && Q > 0) {
-        run.io.h_out = out_broker;
-        run.io.h_out_len = out_len;
-        if (enq_copy_out(s, run.io, out_stride, 0, (int64_t)K * Q) != KA_OK) return fail(KA_ERR_CUDA);
-    }
-    return finish_candidates(c, s, run.bt, st, part_id, part_off);
+            return abort(KA_ERR_CUDA);
+    return finish_batch(c, s, bt, st, part_id, part_off);
 }
 
 }  // extern "C"

@@ -262,7 +262,7 @@ ALL_PLANS = [c["plan"] for c in SINGLE_CASES + RAGGED_CASES + CAND_CASES + RCAND
 
 def _dispatch_from_source():
     """Reachable (load bytes, levels, SM, cand) instantiations of kernel A, read from kassign.cu: the launch_stage<...> calls of
-    launch_stage_plan, the SM values of launch_stage, and the out_stride limit of the candidate entry points."""
+    launch_stage_plan, the SM values of launch_stage, and the out_stride limit of the batched entry points."""
     src = open(os.path.join(ROOT, "kafka_assigner_b200", "csrc", "kassign.cu")).read()
     body = re.search(r"int launch_stage_plan\(.*?\n}\n", src, flags=re.S).group(0)
     kinds = re.findall(r"launch_stage<(\w+), (true|false), CAND>", body)
@@ -271,8 +271,14 @@ def _dispatch_from_source():
     sms = sorted(set(int(x) for x in re.findall(r"launch_stage_t<LoadT, LEVELS, (\d+), CAND>", ls)))
     assert sms == [3, 8], sms
     assert "p.S <= 3 ? launch_stage_t<LoadT, LEVELS, 3, CAND>" in ls
-    # both candidate entry points refuse rows wider than 3: CAND only ever runs SM 3
-    assert len(re.findall(r"K > KA_MAX_CANDIDATES \|\| out_stride > 3\) return all\(KA_ERR_LIMIT\)", src)) == 2
+    # every batched entry point starts with the shared prologue, which refuses rows wider than 3: CAND only ever runs SM 3
+    prologue = re.search(r"int batch_args\(.*?\n}\n", src, flags=re.S)
+    assert prologue, "batch_args moved: update this test"
+    assert "if (K > KA_MAX_CANDIDATES || out_stride > 3) return fail_members(st, K, KA_ERR_LIMIT);" in prologue.group(0)
+    for entry in ("ka_solve_dense_candidates_device", "ka_solve_candidates", "ka_score_candidates", "ka_solve_clusters"):
+        fn = re.search(r"int32_t %s\(.*?\n}\n" % entry, src, flags=re.S)
+        assert fn, "%s moved: update this test" % entry
+        assert re.search(r"int rc = batch_args\(c, K, out_stride, st\);\s*if \(rc != KA_OK\) return rc;", fn.group(0)), entry
     nbytes = {"uint8_t": 1, "uint16_t": 2, "uint32_t": 4}
     out = set()
     for load, lv in kinds:
