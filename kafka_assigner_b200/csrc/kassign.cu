@@ -364,7 +364,8 @@ cudaError_t allow_smem(K kernel, size_t bytes) {
 
 // A whole problem with its inputs on the device: dense (P partitions of RF replicas per topic), or ragged (d_part_off /
 // d_rep_off set, with Q and R from the host-side sizing scan; a ragged problem is always one block). Pmax / capmax: the
-// largest topic and capacity under the broker table(s) it is solved against (dense: P and dense_capmax).
+// largest topic and capacity under the broker table(s) it is solved against (dense: P and dense_capmax). Made by
+// dense_shape or ragged_shape; that of a host-buffer solve gets its device pointers from reserve_io.
 struct Shape {
     int T = 0, P = 0, RF = 0, desired_rf = -1, S = 1;
     const int32_t* d_hash = nullptr;
@@ -383,11 +384,23 @@ int64_t dense_capmax(int P, int rf_t, int n) {
     return n > 0 && rf_t <= n ? ((int64_t)P * std::max(rf_t, 0) + n - 1) / n : 0;
 }
 
-// A dense problem solved against one table of N brokers.
-Shape dense_shape(int T, int P, int RF, int desired_rf, int S, const int32_t* d_hash, const int32_t* d_cur, int N) {
+// A dense problem solved against one table of N brokers, its inputs at d_hash / d_cur.
+Shape dense_shape(int T, int P, int RF, int desired_rf, int S, int N, const int32_t* d_hash = nullptr, const int32_t* d_cur = nullptr) {
     Shape sh{T, P, RF, desired_rf, S, d_hash, d_cur};
+    sh.Q = (int64_t)T * P;
+    sh.R = sh.Q * RF;
     sh.Pmax = P;
     sh.capmax = dense_capmax(P, desired_rf >= 0 ? desired_rf : RF, N);
+    return sh;
+}
+
+// A ragged problem of Q partitions and R current replicas.
+Shape ragged_shape(int T, int64_t Q, int64_t R, int desired_rf, int S, int Pmax = 0, int64_t capmax = 0) {
+    Shape sh{T, 0, 0, desired_rf, S};
+    sh.Q = Q;
+    sh.R = R;
+    sh.Pmax = Pmax;
+    sh.capmax = capmax;
     return sh;
 }
 
@@ -423,16 +436,23 @@ int reserve_scratch(ka_ctx* c, const StageDesc* ds, int K) {
     return KA_OK;
 }
 
-// Device copies of the inputs and rows of a host-buffer solve.
-int reserve_io(ka_ctx* c, int T, int64_t Q, int64_t R, int S, bool ragged) {
-    KA_CUDA(c->d_hash.reserve((size_t)std::max(T, 1) * 4));
+// The ctx's device copies of the inputs and rows of a host-buffer solve of sh (a dense_shape or, with `ragged`, a
+// ragged_shape), and sh pointed at them.
+int reserve_io(ka_ctx* c, Shape& sh, bool ragged) {
+    KA_CUDA(c->d_hash.reserve((size_t)std::max(sh.T, 1) * 4));
     if (ragged) {
-        KA_CUDA(c->d_part_off.reserve((size_t)(T + 1) * 8));
-        KA_CUDA(c->d_rep_off.reserve((size_t)(Q + 1) * 8));
+        KA_CUDA(c->d_part_off.reserve((size_t)(sh.T + 1) * 8));
+        KA_CUDA(c->d_rep_off.reserve((size_t)(sh.Q + 1) * 8));
     }
-    KA_CUDA(c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4));
-    KA_CUDA(c->d_out.reserve((size_t)std::max<int64_t>(Q, 1) * S * 4));
-    KA_CUDA(c->d_out_len.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
+    KA_CUDA(c->d_cur.reserve((size_t)std::max<int64_t>(sh.R, 1) * 4));
+    KA_CUDA(c->d_out.reserve((size_t)std::max<int64_t>(sh.Q, 1) * sh.S * 4));
+    KA_CUDA(c->d_out_len.reserve((size_t)std::max<int64_t>(sh.Q, 1) * 4));
+    sh.d_hash = c->d_hash.as<int32_t>();
+    sh.d_cur = c->d_cur.as<int32_t>();
+    if (ragged) {
+        sh.d_part_off = c->d_part_off.as<int64_t>();
+        sh.d_rep_off = c->d_rep_off.as<int64_t>();
+    }
     return KA_OK;
 }
 
@@ -633,7 +653,25 @@ struct SolveCall {
     int out_copies = 0;       // sub-block copies handed to c->sj (ev_json_in)
     int json_blocks = 0;      // JSON fragments enqueued (ev_json_in, ev_json_scan, h_frag)
     int chains = 0;           // chain sub-blocks enqueued (ev_chain, ev_b1)
+
+    SolveCall(int32_t* out, int32_t* out_len) : d_out(out), d_out_len(out_len) {}
 };
+
+// A host-buffer solve: its inputs from these host arrays (part_id: a ragged JSON solve's partition ids), its rows to the ctx's
+// d_out / d_out_len and then to out_broker / out_len (null: no host rows). Made once the ctx's device buffers are reserved.
+SolveCall host_call(ka_ctx* c, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off, const int32_t* cur_broker,
+                    int32_t* out_len, int32_t* out_broker, const int32_t* part_id = nullptr) {
+    SolveCall io(c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>());
+    io.h_hash = topic_hash;
+    io.h_part_off = part_off;
+    io.h_rep_off = rep_off;
+    io.h_cur = cur_broker;
+    io.h_part_id = part_id;
+    io.d_part_id = part_id ? c->d_part_id.as<int32_t>() : nullptr;
+    io.h_out = out_broker;
+    io.h_out_len = out_len;
+    return io;
+}
 
 struct SubBlock { int t0, t1; int64_t r0, rq; };
 
@@ -1388,10 +1426,8 @@ int32_t ka_solve_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     int rc = validate_dense(c, T, P, RF, desired_rf, out_stride, st);
     if (rc != KA_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    SolveCall io;
-    io.d_out = d_out_broker;
-    io.d_out_len = d_out_len;
-    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker, c->br.N);
+    SolveCall io(d_out_broker, d_out_len);
+    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, c->br.N, d_topic_hash, d_cur_broker);
     if ((rc = enter(c, true)) != KA_OK || (rc = run_solve(c, s, sh, io, st)) != KA_OK) return failed(st, rc);
     return finish(c, s, st, false);
 }
@@ -1548,10 +1584,8 @@ int32_t ka_solve_dense_candidates_device(ka_ctx* c, int32_t K, const int32_t* ca
     std::vector<int64_t> cap(K);
     for (int k = 0; k < K; ++k) cap[k] = dense_capmax(P, rf_t, cand_off[k + 1] - cand_off[k]);
     add_candidates(bt, T, Q, P, desired_rf, cap);
-    const Shape sh{T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker};
-    SolveCall io;
-    io.d_out = d_out_broker;
-    io.d_out_len = d_out_len;
+    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, 0, d_topic_hash, d_cur_broker);   // sized by plan_batch
+    const SolveCall io(d_out_broker, d_out_len);
     cudaStream_t s = (cudaStream_t)stream;
     StageDesc d;
     if ((rc = plan_batch(sh, bt, d, st)) != KA_OK || (rc = run_batch(c, s, bt, d, 0, io, st)) != KA_OK) return rc;
@@ -1567,7 +1601,7 @@ int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     StageDesc& d = c->staged_block;
     c->staged = false;
     reset_plans(c);
-    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, d_topic_hash, d_cur_broker, c->br.N);
+    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, c->br.N, d_topic_hash, d_cur_broker);
     if ((rc = describe_block(sh, 0, T, 0, c->br.N, c->br.blob_bytes, d, &lst)) != KA_OK ||
         (rc = reserve_scratch(c, &d, 1)) != KA_OK)
         return rc;
@@ -1579,22 +1613,34 @@ int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     return KA_OK;
 }
 
-int32_t ka_order_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
+// Prologue of the calls that finish the staged block: st cleared, the ctx, its device made current, then a staged block
+// (with slot_chains, one whose leader order is the two slot chains of rows <= 3); the first that fails is reported.
+static int enter_staged(ka_ctx* c, bool slot_chains, ka_status* st) {
     set_status(st, KA_OK);
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
-    int rc = enter(c, false);
+    const int rc = enter(c, false);
     if (rc != KA_OK) return failed(st, rc);
-    if (!c->staged) return set_status(st, KA_ERR_BAD_ARG);
-    cudaStream_t s = (cudaStream_t)stream;
-    SolveCall io;
-    io.d_out = d_out_broker;
-    io.d_out_len = d_out_len;
-    if ((rc = chain_fork(c, s)) != KA_OK || (rc = enq_order_emit(c, s, c->staged_block, io, 1)) != KA_OK) return failed(st, rc);
+    if (!c->staged || (slot_chains && c->staged_block.pl.rec_kind != 3)) return set_status(st, KA_ERR_BAD_ARG);
+    return KA_OK;
+}
+
+// End of the staged block's solve, its rows enqueued on `s`: the block is used up and its status pending on `s`.
+static int end_staged(ka_ctx* c, cudaStream_t s, ka_status* st) {
     if (c->timing) cudaEventRecord(c->ev[4], s);
-    if ((rc = enq_solve_end(c, s)) != KA_OK) return failed(st, rc);
+    const int rc = enq_solve_end(c, s);
+    if (rc != KA_OK) return failed(st, rc);
     c->staged = false;
     c->last_was_staged = true;
     return finish(c, s, st, false);
+}
+
+int32_t ka_order_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
+    int rc = enter_staged(c, false, st);
+    if (rc != KA_OK) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    SolveCall io(d_out_broker, d_out_len);
+    if ((rc = chain_fork(c, s)) != KA_OK || (rc = enq_order_emit(c, s, c->staged_block, io, 1)) != KA_OK) return failed(st, rc);
+    return end_staged(c, s, st);
 }
 
 int32_t ka_staged_slot_chains(ka_ctx* c) {
@@ -1603,10 +1649,9 @@ int32_t ka_staged_slot_chains(ka_ctx* c) {
 }
 
 int32_t ka_order_slot_device(ka_ctx* c, int32_t slot, void* stream) {
-    if (!c) return KA_ERR_NO_DEVICE;
-    int rc = enter(c, false);
+    int rc = enter_staged(c, true, nullptr);
     if (rc != KA_OK) return rc;
-    if (!c->staged || c->staged_block.pl.rec_kind != 3 || slot < 0 || slot > 1) return KA_ERR_BAD_ARG;
+    if (slot < 0 || slot > 1) return KA_ERR_BAD_ARG;
     const StageDesc& d = c->staged_block;
     cudaStream_t s = (cudaStream_t)stream;
     const int nsub = chain_subblocks(d, 1);
@@ -1619,18 +1664,12 @@ int32_t ka_order_slot_device(ka_ctx* c, int32_t slot, void* stream) {
 }
 
 int32_t ka_emit_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
-    set_status(st, KA_OK);
-    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
-    int rc = enter(c, false);
-    if (rc != KA_OK) return failed(st, rc);
-    if (!c->staged || c->staged_block.pl.rec_kind != 3 || !d_out_broker) return set_status(st, KA_ERR_BAD_ARG);
+    int rc = enter_staged(c, true, st);
+    if (rc != KA_OK) return rc;
+    if (!d_out_broker) return set_status(st, KA_ERR_BAD_ARG);
     cudaStream_t s = (cudaStream_t)stream;
     if ((rc = enq_emit_block(c, s, c->staged_block, 0, 1, d_out_broker, d_out_len)) != KA_OK) return failed(st, rc);
-    if (c->timing) cudaEventRecord(c->ev[4], s);
-    if ((rc = enq_solve_end(c, s)) != KA_OK) return failed(st, rc);
-    c->staged = false;
-    c->last_was_staged = true;
-    return finish(c, s, st, false);
+    return end_staged(c, s, st);
 }
 
 static int copy_counter_column(ka_ctx* c, int slot, int32_t* d_col, const int32_t* d_src, cudaStream_t s) {
@@ -1666,23 +1705,17 @@ int32_t ka_solve_dense(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t 
     int rc = validate_dense(c, T, P, RF, desired_rf, out_stride, st);
     if (rc != KA_OK) return rc;
     if ((rc = enter(c, true)) != KA_OK) return failed(st, rc);
-    const int64_t Q = (int64_t)T * P, R = Q * RF;
-    if ((T > 0 && !topic_hash) || (R > 0 && !cur_broker) || (Q > 0 && !out_broker)) return set_status(st, KA_ERR_BAD_ARG);
-    if ((rc = reserve_io(c, T, Q, R, out_stride, false)) != KA_OK) return failed(st, rc);
-    SolveCall io;
-    io.h_hash = topic_hash;
-    io.h_cur = cur_broker;
-    io.d_out = c->d_out.as<int32_t>();
-    io.d_out_len = c->d_out_len.as<int32_t>();
-    io.h_out = out_broker;
-    io.h_out_len = out_len;
-    const Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->br.N);
+    Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, c->br.N);
+    if ((T > 0 && !topic_hash) || (sh.R > 0 && !cur_broker) || (sh.Q > 0 && !out_broker)) return set_status(st, KA_ERR_BAD_ARG);
+    if ((rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
+    SolveCall io = host_call(c, topic_hash, nullptr, nullptr, cur_broker, out_len, out_broker);
     if ((rc = run_solve(c, c->stream, sh, io, st)) != KA_OK) return failed(st, rc);
     return finish(c, c->stream, st, true);
 }
 
 // Device buffers of a JSON solve, and its topic names H2D (on c->sj, ahead of the first fragment).
-static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, const int64_t* name_off, int64_t name_bytes, int64_t json_cap) {
+static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, const int64_t* name_off, int64_t json_cap) {
+    const int64_t name_bytes = T > 0 ? name_off[T] : 0;
     KA_CUDA(c->d_json.reserve((size_t)json_cap));
     KA_CUDA(c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)));
     KA_CUDA(c->d_name_off.reserve((size_t)(T + 1) * 8));
@@ -1706,11 +1739,21 @@ static int check_names(int32_t T, const char* names, const int64_t* name_off, ka
     return KA_OK;
 }
 
-// Every fragment of a JSON solve is enqueued on c->sj: stream each one into `json` as soon as its size is known (later
-// fragments may still be in the chains or being built), then collect the solve's status. part_id / part_off: as in
-// finish_status. On any error *json_bytes stays 0; a text longer than json_cap is KA_ERR_LIMIT.
-static int stream_json(ka_ctx* c, cudaStream_t s, const SolveCall& io, char* json, int64_t json_cap, int64_t* json_bytes,
-                       ka_status* st, const int32_t* part_id = nullptr, const int64_t* part_off = nullptr) {
+// A JSON solve of sh on c->stream, from the host inputs of io (no host rows), once its ctx's device copies are reserved:
+// prepare_json, then the run (refused with KA_ERR_BAD_ARG when not `runnable`). Every fragment is enqueued on c->sj: stream
+// each one into `json` as soon as its size is known (later fragments may still be in the chains or being built), then
+// collect the solve's status (the failing partition's id when io has part ids). On any error *json_bytes stays 0; a text
+// longer than json_cap is KA_ERR_LIMIT.
+static int solve_json(ka_ctx* c, const Shape& sh, SolveCall io, const char* names, const int64_t* name_off, char* json,
+                      int64_t json_cap, int64_t* json_bytes, ka_status* st, bool runnable = true) {
+    int rc = prepare_json(c, sh.T, sh.Q, names, name_off, json_cap);
+    if (rc != KA_OK) return failed(st, rc);
+    cudaStream_t s = c->stream;
+    io.json = true;
+    if ((rc = runnable ? run_solve(c, s, sh, io, st) : KA_ERR_BAD_ARG) != KA_OK) {
+        cudaStreamSynchronize(c->sj);
+        return failed(st, rc);
+    }
     finish(c, s, nullptr, false);   // pending: collected below, once the fragments are out
     int64_t total = 0;
     bool overflow = false;
@@ -1722,7 +1765,7 @@ static int stream_json(ka_ctx* c, cudaStream_t s, const SolveCall& io, char* jso
         total = base + size;
     }
     KA_CUDA(cudaStreamSynchronize(c->sj));
-    int rc = finish_status(c, s, st, part_id, part_off);
+    rc = finish_status(c, s, st, io.h_part_id, io.h_part_off);
     if (rc == KA_OK && overflow) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
     if (json_bytes) *json_bytes = rc == KA_OK ? total : 0;
     return rc;
@@ -1735,24 +1778,14 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     if (json_bytes) *json_bytes = 0;
     int rc = validate_dense(c, T, P, RF, desired_rf, S, st);
     if (rc != KA_OK) return rc;
-    const int64_t Q = (int64_t)T * P, R = Q * RF;
-    if ((T > 0 && (!topic_hash || !names || !name_off)) || (R > 0 && !cur_broker) || !json || json_cap < KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN)
+    Shape sh = dense_shape(T, P, RF, desired_rf, S, c->br.N);
+    if ((T > 0 && (!topic_hash || !names || !name_off)) || (sh.R > 0 && !cur_broker) || !json || json_cap < KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN)
         return set_status(st, KA_ERR_BAD_ARG);
     if ((rc = check_names(T, names, name_off, st)) != KA_OK) return rc;
-    if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, T, Q, R, S, false)) != KA_OK ||
-        (rc = prepare_json(c, T, Q, names, name_off, T > 0 ? name_off[T] : 0, json_cap)) != KA_OK)
-        return failed(st, rc);
-    cudaStream_t s = c->stream;
-    SolveCall io;
-    io.h_hash = topic_hash;
-    io.h_cur = cur_broker;
-    io.d_out = c->d_out.as<int32_t>();
-    io.d_out_len = c->d_out_len.as<int32_t>();
-    io.json = true;
-    const Shape sh = dense_shape(T, P, RF, desired_rf, S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->br.N);
-    rc = T > 0 && c->br.N > 0 ? run_solve(c, s, sh, io, st) : KA_ERR_BAD_ARG;
-    if (rc != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
-    return stream_json(c, s, io, json, json_cap, json_bytes, st);
+    if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
+    // no topics or no brokers: no text to write, refused once its buffers are prepared
+    return solve_json(c, sh, host_call(c, topic_hash, nullptr, nullptr, cur_broker, nullptr, nullptr), names, name_off, json, json_cap,
+                      json_bytes, st, T > 0 && c->br.N > 0);
 }
 
 // Host-side sizing scan of a ragged problem that does not depend on any broker table: offsets, list sizes, the largest
@@ -1826,9 +1859,9 @@ static int ragged_capmax(const RaggedScan& sc, int N, int64_t& capmax, ka_status
 
 // Validation and sizing of a ragged solve against the ctx's broker table, then its device input buffers: the Shape
 // run_solve takes. pick_stride / have_out: as in ragged_scan.
-static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
-                        const int32_t* cur_broker, int32_t desired_rf, int32_t S, bool pick_stride, bool have_out, Shape& sh,
-                        ka_status* st) {
+static int prepare_ragged(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
+                          const int32_t* cur_broker, int32_t desired_rf, int32_t S, bool pick_stride, bool have_out, Shape& sh,
+                          ka_status* st) {
     set_status(st, KA_OK);
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return set_status(st, KA_ERR_BAD_ARG);
@@ -1840,9 +1873,8 @@ static int ragged_shape(ka_ctx* c, int32_t T, const int32_t* topic_hash, const i
     if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, S, pick_stride, have_out, sc, st)) != KA_OK ||
         (rc = ragged_capmax(sc, c->br.N, capmax, st)) != KA_OK)
         return rc;
-    if ((rc = reserve_io(c, T, sc.Q, sc.R, sc.S, true)) != KA_OK) return failed(st, rc);
-    sh = Shape{T, 0, 0, desired_rf, sc.S, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-               c->d_rep_off.as<int64_t>(), sc.Q, sc.R, sc.Pmax, capmax};
+    sh = ragged_shape(T, sc.Q, sc.R, desired_rf, sc.S, sc.Pmax, capmax);
+    if ((rc = reserve_io(c, sh, true)) != KA_OK) return failed(st, rc);
     return KA_OK;
 }
 
@@ -1851,17 +1883,9 @@ int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t*
                  int32_t desired_rf, int32_t out_stride, int32_t* out_len, int32_t* out_broker,
                  ka_status* st) {
     Shape sh;
-    int rc = ragged_shape(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, out_stride, false, out_broker != nullptr, sh, st);
+    int rc = prepare_ragged(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, out_stride, false, out_broker != nullptr, sh, st);
     if (rc != KA_OK) return rc;
-    SolveCall io;
-    io.h_hash = topic_hash;
-    io.h_part_off = part_off;
-    io.h_rep_off = rep_off;
-    io.h_cur = cur_broker;
-    io.d_out = c->d_out.as<int32_t>();
-    io.d_out_len = c->d_out_len.as<int32_t>();
-    io.h_out = out_broker;
-    io.h_out_len = out_len;
+    SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
     if ((rc = run_solve(c, c->stream, sh, io, st)) != KA_OK) return failed(st, rc);
     return finish(c, c->stream, st, true, part_id, part_off);
 }
@@ -1871,7 +1895,7 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
                       const int64_t* name_off, char* json, int64_t json_cap, int64_t* json_bytes, ka_status* st) {
     if (json_bytes) *json_bytes = 0;
     Shape sh;
-    int rc = ragged_shape(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, 0, true, true, sh, st);
+    int rc = prepare_ragged(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, 0, true, true, sh, st);
     if (rc != KA_OK) return rc;
     if ((T > 0 && (!names || !name_off)) || !json || json_cap < 0) return set_status(st, KA_ERR_BAD_ARG);
     if ((rc = check_names(T, names, name_off, st)) != KA_OK) return rc;
@@ -1882,35 +1906,8 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
     if (64 + frag_rows * (50 + 12 * sh.S + longest_name) > (int64_t)UINT32_MAX)
         return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(longest_name, INT_MAX));
     if (c->d_part_id.reserve((size_t)std::max<int64_t>(sh.Q, 1) * 4) != cudaSuccess) return failed(st, KA_ERR_CUDA);
-    if ((rc = prepare_json(c, T, sh.Q, names, name_off, T > 0 ? name_off[T] : 0, json_cap)) != KA_OK) return failed(st, rc);
-    cudaStream_t s = c->stream;
-    SolveCall io;
-    io.h_hash = topic_hash;
-    io.h_part_off = part_off;
-    io.h_rep_off = rep_off;
-    io.h_cur = cur_broker;
-    io.h_part_id = part_id;
-    io.d_part_id = part_id ? c->d_part_id.as<int32_t>() : nullptr;
-    io.d_out = c->d_out.as<int32_t>();
-    io.d_out_len = c->d_out_len.as<int32_t>();
-    io.json = true;
-    if ((rc = run_solve(c, s, sh, io, st)) != KA_OK) { cudaStreamSynchronize(c->sj); return failed(st, rc); }
-    return stream_json(c, s, io, json, json_cap, json_bytes, st, part_id, part_off);
-}
-
-// The host inputs and rows of a ragged batched solve: the ctx's device copies of them, and the caller's buffers.
-static SolveCall batch_io(ka_ctx* c, const int32_t* topic_hash, const int64_t* part_off, const int64_t* rep_off,
-                          const int32_t* cur_broker, int32_t* out_len, int32_t* out_broker) {
-    SolveCall io;
-    io.h_hash = topic_hash;
-    io.h_part_off = part_off;
-    io.h_rep_off = rep_off;
-    io.h_cur = cur_broker;
-    io.d_out = c->d_out.as<int32_t>();
-    io.d_out_len = c->d_out_len.as<int32_t>();
-    io.h_out = out_broker;
-    io.h_out_len = out_len;
-    return io;
+    return solve_json(c, sh, host_call(c, topic_hash, part_off, rep_off, cur_broker, nullptr, nullptr, part_id), names, name_off, json,
+                      json_cap, json_bytes, st);
 }
 
 // ka_solve_candidates and ka_score_candidates once their tables have passed check_tables, up to their plan: the sizing scan,
@@ -1939,11 +1936,10 @@ static int ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, cons
     if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, (int64_t)K * Q, bt, st)) != KA_OK) return rc;
     add_candidates(bt, T, Q, sc.Pmax, desired_rf, cap);
     const size_t q = (size_t)std::max<int64_t>(Q, 1);
-    if (reserve_io(c, T, Q, sc.R, out_stride, true) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
+    sh = ragged_shape(T, Q, sc.R, desired_rf, out_stride);
+    if (reserve_io(c, sh, true) != KA_OK || c->d_out.reserve((size_t)K * q * out_stride * 4) != cudaSuccess ||
         c->d_out_len.reserve((size_t)K * q * 4) != cudaSuccess)
         return fail_members(st, K, KA_ERR_CUDA);
-    sh = Shape{T, 0, 0, desired_rf, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-               c->d_rep_off.as<int64_t>(), Q, sc.R};
     return KA_OK;
 }
 
@@ -1970,7 +1966,7 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     if ((rc = ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, part_off, rep_off, cur_broker, desired_rf, out_stride,
                                 out_broker != nullptr, bt, sh, st)) != KA_OK || bt.m.empty() ||
         (rc = plan_batch(sh, bt, d, st)) != KA_OK ||
-        (rc = run_batch(c, c->stream, bt, d, sh.R, batch_io(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker), st)) !=
+        (rc = run_batch(c, c->stream, bt, d, sh.R, host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker), st)) !=
             KA_OK)
         return rc;
     return finish_batch(c, c->stream, bt, st, part_id, part_off);
@@ -2024,14 +2020,12 @@ int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
     if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, Q, bt, st)) != KA_OK) return rc;
     add_clusters(bt, T, Q, out_stride, passed, st);
     if (bt.m.empty()) return finish_batch(c, c->stream, bt, st);
-    const int64_t R = rep0[K];
-    if (reserve_io(c, T, Q, R, out_stride, true) != KA_OK) return fail_members(st, K, KA_ERR_CUDA);
-    const Shape sh{T, 0, 0, -1, out_stride, c->d_hash.as<int32_t>(), c->d_cur.as<int32_t>(), c->d_part_off.as<int64_t>(),
-                   c->d_rep_off.as<int64_t>(), Q, R};
+    Shape sh = ragged_shape(T, Q, rep0[K], -1, out_stride);
+    if (reserve_io(c, sh, true) != KA_OK) return fail_members(st, K, KA_ERR_CUDA);
     // the inputs of every cluster go up at once; the rows of all clusters come back in one copy
     StageDesc d;
     if ((rc = plan_batch(sh, bt, d, st)) != KA_OK ||
-        (rc = run_batch(c, c->stream, bt, d, R, batch_io(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker), st)) !=
+        (rc = run_batch(c, c->stream, bt, d, sh.R, host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker), st)) !=
             KA_OK)
         return rc;
     return finish_batch(c, c->stream, bt, st, part_id, part_off);
@@ -2079,7 +2073,7 @@ int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
         if (sum > INT64_MAX / 3) return fail(fail_members(st, K, KA_ERR_LIMIT));
     }
     cudaStream_t s = c->stream;
-    const SolveCall io = batch_io(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
+    const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
     if ((rc = run_batch(c, s, bt, d, sh.R, io, st)) != KA_OK) return fail(rc);
     auto abort = [&](int code) { return fail(abort_batch(c, s, st, K, code)); };
     const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
