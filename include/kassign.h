@@ -213,6 +213,38 @@ int32_t ka_solve_clusters(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const
                           const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
                           int32_t* out_len, int32_t* out_broker, ka_status* st);
 
+/* The fleet of ka_solve_clusters, each cluster's rows turned into that cluster's reassignment JSON on the device: one document
+ * per cluster, and only the text crosses PCIe.
+ *   K .. cur_broker    the fleet inputs of ka_solve_clusters (no out_stride: the stride is internal, see below)
+ *   names, name_off    the names of all ΣT topics in input order, as ka_solve_json takes them (name_off[ΣT+1])
+ *   json               host buffer of json_cap bytes (pinned for full PCIe speed)
+ *   json_off[K+1]      host; cluster k's document is json[json_off[k] .. json_off[k+1]), back to back in cluster order, not
+ *                      NUL-terminated; json_off[0] = 0, and a cluster that failed has an empty range
+ *   st[K]              host, required; st[k] is cluster k's status
+ * Cluster k's text and st[k] are exactly what ka_ctx_create -> ka_ctx_set_brokers(table k) -> ka_solve_json(its topics, with
+ * part_off / rep_off rebased to 0 and its names, desired_rf[k]) gives: topic_index counts from the cluster's first topic,
+ * partition is mapped through part_id. A cluster without topics, or with only empty topics under a desired RF, gets
+ * {"partitions":[],"version":1}. Per cluster, in ka_solve_json's order: the sizing scan and capacity checks of ka_solve_clusters;
+ * a name that org.json would escape (KA_ERR_BAD_ARG, a = the byte); the 32-bit fragment limit of ka_solve_json; the cluster's
+ * own plan; the five reference exceptions. A cluster that fails any of them has no text, and the others still solve.
+ * Stride: cluster k's width is max(longest current list, desired_rf[k], 1), and the call runs at the largest width among the
+ * clusters it solves. The batched chains take rows of at most 3, so a cluster wider than 3 gets KA_ERR_LIMIT with a = its
+ * width (the one difference from ka_solve_json, which solves widths 4..8 through its fused chain).
+ * Checked for the whole call (the code in every st[k], and returned): what ka_solve_clusters checks for the whole call (K,
+ * tables, cluster boundaries, ΣP < 2^31); names or name_off NULL when ΣT > 0, json or json_off NULL, json_cap < 0
+ * (KA_ERR_BAD_ARG); a plan or fragment size of the whole call that fails where no cluster's own does (KA_ERR_LIMIT).
+ * Buffer: sum over clusters k of (64 + sum over cluster k's rows of (50 + 12 * width k + name length of the row's topic))
+ * always suffices. If json_cap is too small, every cluster that solved gets KA_ERR_LIMIT with a = min(json_cap, INT_MAX), a
+ * failed cluster keeps its status, and every json_off[k] is 0. K == 0: KA_OK, json_off[0] = 0.
+ * Synchronous. Returns KA_OK when every cluster solved, else st[k].code of the lowest failing k. The number of kernel launches
+ * depends on ΣP and not on K. Does not read or change ctx's own Context, broker table, parked counters, topic_base or staged
+ * block. */
+int32_t ka_solve_clusters_json(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                               const int32_t* broker_rack, const int32_t* topic_off, const int32_t* desired_rf,
+                               const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                               const int64_t* rep_off, const int32_t* cur_broker, const char* names, const int64_t* name_off,
+                               char* json, int64_t json_cap, int64_t* json_off, ka_status* st);
+
 /* What a candidate's rows change against the current lists, and how they spread over its brokers. Every field is int64, so
  * the layout has no padding. Position counts: a duplicate id in a current list, or a current broker the table lacks, needs
  * no special case. w[g] is the weight of row g (1 without weights); the rows_* and leaders_changed fields count rows. */

@@ -398,6 +398,29 @@ class Solver:
         rows = part_off[topic_off]
         return [(out[rows[k]:rows[k + 1]], out_len[rows[k]:rows[k + 1]], st[k]) for k in range(K)]
 
+    def solve_clusters_json(self, clusters, topic_names, json_buf=None):
+        """ka_solve_clusters_json: the fleet of solve_clusters, every cluster's reassignment JSON built on the device.
+        topic_names: one list of names per cluster. json_buf: optional writable uint8 numpy array (pinned for full PCIe speed);
+        by default one of the documented sufficient size. Returns one (bytes-like view of the cluster's text, KaStatus) per
+        cluster; the text of a failed cluster is empty."""
+        K = len(clusters)
+        cand_off, broker_id, broker_rack, topic_off, drf, th, part_off, part_id, rep_off, cur = self.marshal_clusters(clusters)
+        names, name_off = self.marshal_names([n for names_k in topic_names for n in names_k])
+        assert len(name_off) == len(th) + 1
+        if json_buf is None:
+            rows, name_len, cap = np.diff(part_off), np.diff(name_off), 0
+            for k in range(K):
+                t0, t1 = int(topic_off[k]), int(topic_off[k + 1])
+                S = _default_stride(rep_off[part_off[t0]:part_off[t1] + 1], int(drf[k]))
+                cap += 64 + int(part_off[t1] - part_off[t0]) * (50 + 12 * S) + int(np.dot(rows[t0:t1], name_len[t0:t1]))
+            json_buf = np.empty(max(cap, 1), dtype=np.uint8)
+        json_off = np.zeros(K + 1, dtype=np.int64)
+        st = (KaStatus * max(K, 1))()
+        self._L.ka_solve_clusters_json(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), _ptr(topic_off), _ptr(drf),
+                                       _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur), _ptr(names),
+                                       _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(json_off), st)
+        return [(json_buf[json_off[k]:json_off[k + 1]], st[k]) for k in range(K)]
+
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""
         rc = self._L.ka_stage_dense_device(self._h, int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF),

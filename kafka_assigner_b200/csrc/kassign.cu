@@ -57,6 +57,7 @@ constexpr int KA_MAX_CHAIN_EVENTS = 64;   // per solve: 8 staged blocks x 8 sub-
 // streams out while later fragments are still being built and every fragment stays far below the 4 GiB of its 32-bit offsets.
 constexpr int KA_MAX_JSON_FRAGS = 256;
 constexpr int KA_MAX_CANDIDATES = 128;    // candidate broker tables of one batched solve
+static_assert(KA_MAX_CANDIDATES <= KA_JSON_MAX_SEGS, "a fleet's documents are built in one segmented JSON pass");
 constexpr int64_t KA_JSON_FRAG_ROWS = 1 << 18;
 
 struct HostPinned {
@@ -135,6 +136,7 @@ struct ka_ctx {
     DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len;
     RunScratch run;   // kernel A and the chains of a single solve (and of a staged block)
     DevBuf d_json, d_names, d_name_off, d_part_id, d_json_rowlen, d_json_blocksum, d_json_state;
+    DevBuf d_json_seg;   // the document table of ka_solve_clusters_json (the arrays of KaJsonSegs)
     // scratch of the batched solves, apart from the single solve's: descriptors + broker tables, counters, and the run
     DevBuf d_batch_tab, d_batch_ctr;
     RunScratch batch_run;
@@ -714,10 +716,10 @@ int enq_json_rows(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc
     p.first = first;
     p.last = last;
     const int nblocks = (int)((rows + 255) / 256);
-    if (nblocks > 0) ka_json_len_kernel<<<nblocks, 256, 0, c->sj>>>(p);
+    if (nblocks > 0) ka_json_len_kernel<false><<<nblocks, 256, 0, c->sj>>>(p, KaJsonSegs{});
     ka_json_scan_kernel<<<1, 1024, 0, c->sj>>>(p, nblocks);
-    KA_CUDA(allow_smem(ka_json_write_kernel, KA_JSON_SMEM_BYTES + 16));
-    ka_json_write_kernel<<<std::max(nblocks, 1), 256, KA_JSON_SMEM_BYTES + 16, c->sj>>>(p);
+    KA_CUDA(allow_smem(ka_json_write_kernel<false>, KA_JSON_SMEM_BYTES + 16));
+    ka_json_write_kernel<false><<<std::max(nblocks, 1), 256, KA_JSON_SMEM_BYTES + 16, c->sj>>>(p, KaJsonSegs{});
     KA_CUDA(cudaGetLastError());
     KA_CUDA(cudaMemcpyAsync(c->h_frag + 2 * k, p.frag, 16, cudaMemcpyDeviceToHost, c->sj));
     KA_CUDA(cudaEventRecord(c->ev_json_scan[k], c->sj));
@@ -1088,6 +1090,7 @@ struct BatchMember {
     int n = 0, blob_bytes = 0;   // its table's brokers and blob
     int Pmax = 0;                // its largest topic
     int64_t capmax = 0;          // its largest capacity under its table (dense_capmax / ragged_capmax)
+    int S = 1;                   // a fleet cluster's row width, which its own plan is checked with
 };
 
 // A batched solve: its K broker tables, its members and the call-wide sizes that follow from them.
@@ -1151,13 +1154,13 @@ void add_candidates(Batch& b, int T, int64_t Q, int Pmax, int desired_rf, const 
 }
 
 // The members of a fleet of T topics over Q rows: each cluster of `passed` (those that passed ragged_scan and ragged_capmax,
-// with their slice, n, Pmax and capmax) that also passes the limits of ka_solve's own plan under its table. A cluster refused
-// there reports that limit in st[tab] and is left out, as are all clusters when none has a topic.
-void add_clusters(Batch& b, int T, int64_t Q, int S, const std::vector<BatchMember>& passed, ka_status* st) {
+// with their slice, n, Pmax, capmax and width) that also passes the limits of ka_solve's own plan under its table. A cluster
+// refused there reports that limit in st[tab] and is left out, as are all clusters when none has a topic.
+void add_clusters(Batch& b, int T, int64_t Q, const std::vector<BatchMember>& passed, ka_status* st) {
     for (BatchMember mb : passed) {
         mb.blob_bytes = b.tabs[mb.tab].blob_bytes();
         Plan own;
-        if (make_plan(mb.n, mb.blob_bytes, mb.Q, S, mb.Pmax, mb.capmax, true, own, st + mb.tab) == KA_OK) b.add(mb);
+        if (make_plan(mb.n, mb.blob_bytes, mb.Q, mb.S, mb.Pmax, mb.capmax, true, own, st + mb.tab) == KA_OK) b.add(mb);
     }
     // one table of the call's T topics over its Q rows: every record sits at its input row
     b.recs = std::max<int64_t>(Q, 1);
@@ -1283,7 +1286,7 @@ void ka_ctx_destroy(ka_ctx* c) {
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
                       &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
-                      &c->d_score_brk, &c->d_score_off})
+                      &c->d_score_brk, &c->d_score_off, &c->d_json_seg})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -1729,10 +1732,9 @@ static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, cons
 }
 
 // The device emitter copies topic names verbatim: a name that org.json's quote() would escape is refused (KA_ERR_BAD_ARG,
-// a = the byte), and the caller takes the host emitter instead.
-static int check_names(int32_t T, const char* names, const int64_t* name_off, ka_status* st) {
-    const int64_t name_bytes = T > 0 ? name_off[T] : 0;
-    for (int64_t i = 0; i < name_bytes; ++i) {
+// a = the byte), and the caller takes the host emitter instead. Checks the name bytes names[b0 .. b1).
+static int check_names(const char* names, int64_t b0, int64_t b1, ka_status* st) {
+    for (int64_t i = b0; i < b1; ++i) {
         const unsigned char ch = (unsigned char)names[i];
         if (ch < 0x20 || ch == '"' || ch == '\\' || ch == '/') return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)ch);
     }
@@ -1781,7 +1783,7 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     Shape sh = dense_shape(T, P, RF, desired_rf, S, c->br.N);
     if ((T > 0 && (!topic_hash || !names || !name_off)) || (sh.R > 0 && !cur_broker) || !json || json_cap < KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN)
         return set_status(st, KA_ERR_BAD_ARG);
-    if ((rc = check_names(T, names, name_off, st)) != KA_OK) return rc;
+    if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
     if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
     // no topics or no brokers: no text to write, refused once its buffers are prepared
     return solve_json(c, sh, host_call(c, topic_hash, nullptr, nullptr, cur_broker, nullptr, nullptr), names, name_off, json, json_cap,
@@ -1790,7 +1792,8 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
 
 // Host-side sizing scan of a ragged problem that does not depend on any broker table: offsets, list sizes, the largest
 // topic, and per target RF the largest topic of that RF (the capacity bound of KAS:65-71 for any table follows from those:
-// ragged_capmax). pick_stride: S is chosen here, as max(longest current list, desired_rf, 1). have_out: the caller has
+// ragged_capmax). pick_max > 0: S is chosen here, as max(longest current list, desired_rf, 1), and a width above pick_max is
+// KA_ERR_LIMIT (a = the width); pick_max == 0: S is the caller's. have_out: the caller has
 // somewhere to put the rows. Failures that come before the topic loop are returned; those of the topic and list-size
 // loops are kept in `err` (in the order ka_solve reports them), because a failure that depends on the table — a topic
 // whose target RF exceeds S but not N — takes precedence when it comes from an earlier topic.
@@ -1805,15 +1808,15 @@ struct RaggedScan {
 // row0 / rep0: the scan reads part_off[t] - row0 and rep_off[g] - rep0, i.e. a slice of a larger layout rebased to 0 (one
 // cluster of ka_solve_clusters' fleet), without copying it.
 static int ragged_scan(int32_t T, const int64_t* part_off, const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf,
-                       int32_t S, bool pick_stride, bool have_out, RaggedScan& sc, ka_status* st, int64_t row0 = 0, int64_t rep0 = 0) {
+                       int32_t S, int pick_max, bool have_out, RaggedScan& sc, ka_status* st, int64_t row0 = 0, int64_t rep0 = 0) {
     const int64_t Q = T > 0 ? part_off[T] - row0 : 0;
     if (Q < 0 || (T > 0 && part_off[0] != row0) || (Q > 0 && (!rep_off || !have_out))) return set_status(st, KA_ERR_BAD_ARG);
     const int64_t R = Q > 0 ? rep_off[Q] - rep0 : 0;
     if (R < 0 || (Q > 0 && rep_off[0] != rep0) || (R > 0 && !cur_broker)) return set_status(st, KA_ERR_BAD_ARG);
-    if (pick_stride) {
+    if (pick_max > 0) {
         int64_t m = std::max(desired_rf, 1);
         for (int64_t g = 0; g < Q; ++g) m = std::max(m, rep_off[g + 1] - rep_off[g]);
-        if (m > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(m, INT_MAX));
+        if (m > pick_max) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(m, INT_MAX));
         S = (int)m;
     }
     sc.Q = Q;
@@ -1870,7 +1873,7 @@ static int prepare_ragged(ka_ctx* c, int32_t T, const int32_t* topic_hash, const
     if (rc != KA_OK) return failed(st, rc);
     RaggedScan sc;
     int64_t capmax = 0;
-    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, S, pick_stride, have_out, sc, st)) != KA_OK ||
+    if ((rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, S, pick_stride ? KA_MAX_SLOTS : 0, have_out, sc, st)) != KA_OK ||
         (rc = ragged_capmax(sc, c->br.N, capmax, st)) != KA_OK)
         return rc;
     sh = ragged_shape(T, sc.Q, sc.R, desired_rf, sc.S, sc.Pmax, capmax);
@@ -1890,6 +1893,22 @@ int32_t ka_solve(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t*
     return finish(c, c->stream, st, true, part_id, part_off);
 }
 
+// The longest of the names of topics [t0, t1).
+static int64_t longest_name(const int64_t* name_off, int t0, int t1) {
+    int64_t m = 0;
+    for (int t = t0; t < t1; ++t) m = std::max(m, name_off[t + 1] - name_off[t]);
+    return m;
+}
+
+// A fragment's offsets are 32-bit: the rows of a fragment of a Q-row text at their longest (any int32 partition id, S
+// replicas, the longest name) must fit, else KA_ERR_LIMIT with a = the longest name.
+static int check_fragments(int64_t Q, int S, int64_t longest, ka_status* st) {
+    const int64_t frag_rows = std::min(json_fragment_rows(Q), std::max<int64_t>(Q, 1));
+    if (64 + frag_rows * (50 + 12 * S + longest) > (int64_t)UINT32_MAX)
+        return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(longest, INT_MAX));
+    return KA_OK;
+}
+
 int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
                       const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, const char* names,
                       const int64_t* name_off, char* json, int64_t json_cap, int64_t* json_bytes, ka_status* st) {
@@ -1898,13 +1917,8 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
     int rc = prepare_ragged(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, 0, true, true, sh, st);
     if (rc != KA_OK) return rc;
     if ((T > 0 && (!names || !name_off)) || !json || json_cap < 0) return set_status(st, KA_ERR_BAD_ARG);
-    if ((rc = check_names(T, names, name_off, st)) != KA_OK) return rc;
-    // a fragment's offsets are 32-bit: its rows at their longest (any int32 partition id, S replicas, the longest name)
-    int64_t longest_name = 0;
-    for (int t = 0; t < T; ++t) longest_name = std::max(longest_name, name_off[t + 1] - name_off[t]);
-    const int64_t frag_rows = std::min(json_fragment_rows(sh.Q), std::max<int64_t>(sh.Q, 1));
-    if (64 + frag_rows * (50 + 12 * sh.S + longest_name) > (int64_t)UINT32_MAX)
-        return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(longest_name, INT_MAX));
+    if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
+    if ((rc = check_fragments(sh.Q, sh.S, longest_name(name_off, 0, T), st)) != KA_OK) return rc;
     if (c->d_part_id.reserve((size_t)std::max<int64_t>(sh.Q, 1) * 4) != cudaSuccess) return failed(st, KA_ERR_CUDA);
     return solve_json(c, sh, host_call(c, topic_hash, part_off, rep_off, cur_broker, nullptr, nullptr, part_id), names, name_off, json,
                       json_cap, json_bytes, st);
@@ -1920,7 +1934,7 @@ static int ragged_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, cons
     // malformed offsets: every candidate reports what ka_solve reports for its table
     RaggedScan sc;
     ka_status sst{};
-    int rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, false, have_out, sc, &sst);
+    int rc = ragged_scan(T, part_off, rep_off, cur_broker, desired_rf, out_stride, 0, have_out, sc, &sst);
     if (rc != KA_OK) {
         for (int k = 0; k < K; ++k) st[k] = sst;
         return rc;
@@ -1972,22 +1986,38 @@ int32_t ka_solve_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     return finish_batch(c, c->stream, bt, st, part_id, part_off);
 }
 
-int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
-                          const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
-                          const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
-                          int32_t* out_len, int32_t* out_broker, ka_status* st) {
-    int rc = batch_args(c, K, out_stride, st);
-    if (rc != KA_OK) return rc;
-    if (K == 0) return KA_OK;
+// A fleet call past its front end: cluster k's first row and first current replica in the shared input (row0[K] = ΣP, rep0[K]
+// = ΣR), and the batch of the clusters that passed.
+struct Fleet {
+    int T = 0;
+    std::vector<int64_t> row0, rep0;
+    Batch bt;
+};
+
+// The front end of ka_solve_clusters and ka_solve_clusters_json, once batch_args has passed and K > 0: the checks of the whole
+// call (tables, cluster boundaries, ΣP < 2^31), which fail every cluster; then every cluster's slice checked and sized as the
+// single solve checks and sizes it against the cluster's table, and its own plan. A cluster that fails there reports what the
+// single solve reports and is left out of the call. out_stride > 0: the single solve is ka_solve with that stride. out_stride
+// == 0: it is ka_solve_json (names / name_off: the call's name slab); every cluster picks its width, max(longest list,
+// desired RF, 1), which the batched chains take up to 3 (above: KA_ERR_LIMIT, a = the width), then its names are checked
+// and its text's fragment size.
+static int fleet_front(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                       const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
+                       const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride, bool have_out, const char* names,
+                       const int64_t* name_off, Fleet& f, ka_status* st) {
+    int rc;
     if ((rc = check_tables(K, cand_off, broker_id, broker_rack)) != KA_OK) return fail_members(st, K, rc);
     // the clusters' boundaries: topic_off, then part_off at their first topics and rep_off at their first rows, each
     // non-decreasing from 0
     if (!topic_off || topic_off[0] != 0) return fail_members(st, K, KA_ERR_BAD_ARG);
     for (int k = 0; k < K; ++k)
         if (topic_off[k + 1] < topic_off[k]) return fail_members(st, K, KA_ERR_BAD_ARG);
-    const int T = topic_off[K];
+    const int T = f.T = topic_off[K];
     if (T > 0 && (!topic_hash || !part_off)) return fail_members(st, K, KA_ERR_BAD_ARG);
-    std::vector<int64_t> row0(K + 1, 0), rep0(K + 1, 0);
+    std::vector<int64_t>& row0 = f.row0;
+    std::vector<int64_t>& rep0 = f.rep0;
+    row0.assign(K + 1, 0);
+    rep0.assign(K + 1, 0);
     for (int k = 0; k <= K; ++k) {
         row0[k] = T > 0 ? part_off[topic_off[k]] : 0;
         if (row0[k] < (k > 0 ? row0[k - 1] : 0) || row0[0] != 0) return fail_members(st, K, KA_ERR_BAD_ARG);
@@ -1999,8 +2029,8 @@ int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
         if (rep0[k] < (k > 0 ? rep0[k - 1] : 0) || rep0[0] != 0) return fail_members(st, K, KA_ERR_BAD_ARG);
     }
     if (Q >= ((int64_t)1 << 31)) return fail_members(st, K, KA_ERR_LIMIT);
-    // every cluster's slice, checked and sized as ka_solve checks and sizes it against the cluster's table: a cluster that
-    // fails here reports what ka_solve reports and is left out of the call
+    const bool json = out_stride == 0;
+    if (json && T > 0 && (!names || !name_off)) return fail_members(st, K, KA_ERR_BAD_ARG);
     std::vector<BatchMember> passed;
     for (int k = 0; k < K; ++k) {
         const int t0 = topic_off[k];
@@ -2008,19 +2038,37 @@ int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
         mb.n = cand_off[k + 1] - cand_off[k];
         RaggedScan sc;
         if (ragged_scan(mb.T, part_off ? part_off + t0 : nullptr, rep_off ? rep_off + row0[k] : nullptr,
-                        cur_broker ? cur_broker + rep0[k] : nullptr, mb.desired_rf, out_stride, false, out_broker != nullptr, sc,
+                        cur_broker ? cur_broker + rep0[k] : nullptr, mb.desired_rf, out_stride, json ? 3 : 0, have_out, sc,
                         st + k, row0[k], rep0[k]) != KA_OK ||
             ragged_capmax(sc, mb.n, mb.capmax, st + k) != KA_OK)
             continue;
+        if (json && (check_names(names, mb.T > 0 ? name_off[t0] : 0, mb.T > 0 ? name_off[t0 + mb.T] : 0, st + k) != KA_OK ||
+                     check_fragments(sc.Q, sc.S, longest_name(name_off, t0, t0 + mb.T), st + k) != KA_OK))
+            continue;
         mb.Q = sc.Q;
         mb.Pmax = sc.Pmax;
+        mb.S = sc.S;
         passed.push_back(mb);
     }
-    Batch bt;
-    if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, Q, bt, st)) != KA_OK) return rc;
-    add_clusters(bt, T, Q, out_stride, passed, st);
+    if ((rc = batch_tables(c, K, cand_off, broker_id, broker_rack, Q, f.bt, st)) != KA_OK) return rc;
+    add_clusters(f.bt, T, Q, passed, st);
+    return KA_OK;
+}
+
+int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                          const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
+                          const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
+                          int32_t* out_len, int32_t* out_broker, ka_status* st) {
+    int rc = batch_args(c, K, out_stride, st);
+    if (rc != KA_OK) return rc;
+    if (K == 0) return KA_OK;
+    Fleet f;
+    if ((rc = fleet_front(c, K, cand_off, broker_id, broker_rack, topic_off, desired_rf, topic_hash, part_off, rep_off, cur_broker,
+                          out_stride, out_broker != nullptr, nullptr, nullptr, f, st)) != KA_OK)
+        return rc;
+    Batch& bt = f.bt;
     if (bt.m.empty()) return finish_batch(c, c->stream, bt, st);
-    Shape sh = ragged_shape(T, Q, rep0[K], -1, out_stride);
+    Shape sh = ragged_shape(f.T, f.row0[K], f.rep0[K], -1, out_stride);
     if (reserve_io(c, sh, true) != KA_OK) return fail_members(st, K, KA_ERR_CUDA);
     // the inputs of every cluster go up at once; the rows of all clusters come back in one copy
     StageDesc d;
@@ -2029,6 +2077,145 @@ int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
             KA_OK)
         return rc;
     return finish_batch(c, c->stream, bt, st, part_id, part_off);
+}
+
+// The document table of a fleet's segmented JSON pass in d_json_seg: doc_off [K+1] | seg_bytes [K] | seg_row0 [K+1] (8 bytes
+// each) | seg_shift [K] | seg_member [K] (4 bytes each). Bytes, and the offset of seg_shift.
+static size_t fleet_segs_bytes(int K, size_t* shift_at) {
+    *shift_at = (3 * (size_t)K + 2) * 8;
+    return *shift_at + 2 * (size_t)K * 4;
+}
+
+// The K clusters' first rows and batch members (-1: left out) to the document table, seg_bytes zeroed, on `s`.
+static int enq_fleet_segs(ka_ctx* c, cudaStream_t s, const Fleet& f, int K) {
+    size_t shift_at;
+    const size_t bytes = fleet_segs_bytes(K, &shift_at);
+    std::vector<unsigned char> h(bytes, 0);
+    std::memcpy(h.data() + (2 * (size_t)K + 1) * 8, f.row0.data(), (size_t)(K + 1) * 8);
+    int32_t* member = reinterpret_cast<int32_t*>(h.data() + shift_at + (size_t)K * 4);
+    std::fill(member, member + K, -1);
+    for (size_t i = 0; i < f.bt.m.size(); ++i) member[f.bt.m[i].tab] = (int32_t)i;
+    KA_CUDA(c->d_json_seg.reserve(bytes));
+    KA_CUDA(cudaMemcpyAsync(c->d_json_seg.p, h.data(), bytes, cudaMemcpyHostToDevice, s));
+    return KA_OK;
+}
+
+// The segmented JSON pass of a fleet solved as d (its rows in io.d_out, its document table uploaded), on `s` after the last
+// emit: the length pass and the scan over fragments of the call's rows, the document table, then the write pass. doc_off
+// comes back to h_doc.
+static int enq_fleet_json(ka_ctx* c, cudaStream_t s, const StageDesc& d, const SolveCall& io, int K, unsigned long long* h_doc) {
+    size_t shift_at;
+    fleet_segs_bytes(K, &shift_at);
+    unsigned char* seg = c->d_json_seg.as<unsigned char>();
+    KaJsonParams p{};
+    p.part_off = d.d_part_off;
+    p.T = d.T;
+    p.part_id = io.d_part_id;
+    p.name_off = c->d_name_off.as<int64_t>();
+    p.names = c->d_names.as<char>();
+    p.S = d.S;
+    p.total = c->d_json_state.as<unsigned long long>();
+    p.json = c->d_json.as<char>();
+    p.cap = (unsigned long long)c->d_json.cap;
+    KaJsonSegs sg{};
+    sg.K = K;
+    sg.doc_off = reinterpret_cast<unsigned long long*>(seg);
+    sg.bytes = sg.doc_off + K + 1;
+    sg.row0 = reinterpret_cast<const int64_t*>(sg.bytes + K);
+    sg.shift = reinterpret_cast<uint32_t*>(seg + shift_at);
+    sg.member = reinterpret_cast<const int32_t*>(sg.shift + K);
+    sg.flags = c->batch_run.flags.as<unsigned>();
+    // fragments of whole 256-row blocks, as in a ragged single solve; their count depends on the rows alone
+    const int64_t Q = d.Q, step = json_fragment_rows(Q);
+    std::vector<KaJsonParams> frags;
+    for (int64_t r = 0; r < Q; r += step) {
+        const int k = (int)frags.size();
+        KaJsonParams fp = p;
+        fp.Q = (uint32_t)std::min(step, Q - r);
+        fp.row0 = (uint32_t)r;
+        fp.out = io.d_out + r * d.S;
+        fp.out_len = io.d_out_len + r;
+        fp.rowlen = c->d_json_rowlen.as<uint32_t>() + r;
+        fp.blocksum = c->d_json_blocksum.as<uint32_t>() + (r / 256) + k;
+        fp.frag = c->d_json_state.as<unsigned long long>() + 2 + 2 * k;
+        const int nblocks = (int)((fp.Q + 255) / 256);
+        ka_json_len_kernel<true><<<nblocks, 256, 0, s>>>(fp, sg);
+        ka_json_scan_kernel<<<1, 1024, 0, s>>>(fp, nblocks);
+        frags.push_back(fp);
+    }
+    ka_json_docs_kernel<<<1, KA_JSON_MAX_SEGS, 0, s>>>(p, sg);
+    KA_CUDA(allow_smem(ka_json_write_kernel<true>, KA_JSON_SMEM_BYTES + 16));
+    for (const KaJsonParams& fp : frags)
+        ka_json_write_kernel<true><<<(unsigned)((fp.Q + 255) / 256), 256, KA_JSON_SMEM_BYTES + 16, s>>>(fp, sg);
+    KA_CUDA(cudaGetLastError());
+    c->launches += 3 * (int64_t)frags.size() + 1;
+    KA_CUDA(cudaMemcpyAsync(h_doc, sg.doc_off, (size_t)(K + 1) * 8, cudaMemcpyDeviceToHost, s));
+    return KA_OK;
+}
+
+int32_t ka_solve_clusters_json(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                               const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
+                               const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, const char* names,
+                               const int64_t* name_off, char* json, int64_t json_cap, int64_t* json_off, ka_status* st) {
+    if (json_off && K >= 0) std::fill(json_off, json_off + K + 1, 0);
+    int rc = batch_args(c, K, 1, st);
+    if (rc != KA_OK) return rc;
+    if (!json || !json_off || json_cap < 0) return fail_members(st, K, KA_ERR_BAD_ARG);
+    if (K == 0) return KA_OK;
+    Fleet f;
+    if ((rc = fleet_front(c, K, cand_off, broker_id, broker_rack, topic_off, desired_rf, topic_hash, part_off, rep_off, cur_broker, 0,
+                          true, names, name_off, f, st)) != KA_OK)
+        return rc;
+    Batch& bt = f.bt;
+    // every cluster's document, placed as the device places them: a failed cluster's range is empty
+    std::vector<unsigned long long> doc(K + 1, 0);
+    if (bt.m.empty()) {   // no topic to solve: every cluster that passed gets the empty document
+        for (int k = 0; k < K; ++k) doc[k + 1] = doc[k] + (st[k].code == KA_OK ? KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN : 0);
+        if ((int64_t)doc[K] <= json_cap)
+            for (int k = 0; k < K; ++k)
+                if (doc[k + 1] > doc[k]) std::memcpy(json + doc[k], KA_JSON_HEAD KA_JSON_TAIL, KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN);
+    } else {
+        // one plan and one stride for the call, from its largest member; a fragment size that fails where no cluster's own does
+        // fails every cluster
+        int S = 1;
+        int64_t longest = 0;
+        for (const BatchMember& mb : bt.m) {
+            S = std::max(S, mb.S);
+            longest = std::max(longest, longest_name(name_off, mb.t0, mb.t0 + mb.T));
+        }
+        Shape sh = ragged_shape(f.T, f.row0[K], f.rep0[K], -1, S);
+        if ((rc = check_fragments(sh.Q, S, longest, st)) != KA_OK) {
+            for (int k = 1; k < K; ++k) st[k] = st[0];
+            return rc;
+        }
+        if (reserve_io(c, sh, true) != KA_OK || c->d_part_id.reserve((size_t)std::max<int64_t>(sh.Q, 1) * 4) != cudaSuccess)
+            return fail_members(st, K, KA_ERR_CUDA);
+        StageDesc d;
+        if ((rc = plan_batch(sh, bt, d, st)) != KA_OK) return rc;
+        // the names go up on c->sj (prepare_json), which the call's stream waits for before its first fragment
+        if ((rc = prepare_json(c, f.T, sh.Q, names, name_off, json_cap)) != KA_OK ||
+            cudaEventRecord(c->ev_json_in[0], c->sj) != cudaSuccess || cudaStreamWaitEvent(c->stream, c->ev_json_in[0], 0) != cudaSuccess) {
+            cudaStreamSynchronize(c->sj);
+            return fail_members(st, K, KA_ERR_CUDA);
+        }
+        if (enq_fleet_segs(c, c->stream, f, K) != KA_OK) return abort_batch(c, c->stream, st, K, KA_ERR_CUDA);
+        const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, nullptr, nullptr, part_id);
+        if ((rc = run_batch(c, c->stream, bt, d, sh.R, io, st)) != KA_OK) return rc;
+        if ((rc = enq_fleet_json(c, c->stream, d, io, K, doc.data())) != KA_OK ||
+            cudaStreamSynchronize(c->stream) != cudaSuccess ||
+            ((int64_t)doc[K] <= json_cap && doc[K] > 0 && cudaMemcpy(json, c->d_json.p, doc[K], cudaMemcpyDeviceToHost) != cudaSuccess))
+            return abort_batch(c, c->stream, st, K, rc != KA_OK ? rc : KA_ERR_CUDA);
+        finish_batch(c, c->stream, bt, st, part_id, part_off);
+    }
+    // a text beyond json_cap: every cluster that solved reports the buffer, and no cluster has text
+    const bool fits = (int64_t)doc[K] <= json_cap;
+    for (int k = 0; k < K; ++k) {
+        if (!fits && st[k].code == KA_OK) set_status(st + k, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
+        json_off[k + 1] = fits ? (int64_t)doc[k + 1] : 0;
+    }
+    for (int k = 0; k < K; ++k)
+        if (st[k].code != KA_OK) return st[k].code;
+    return KA_OK;
 }
 
 int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,

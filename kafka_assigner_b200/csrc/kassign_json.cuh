@@ -34,10 +34,23 @@ struct KaJsonParams {
     int first, last;            // write the header before / the trailer after this fragment
 };
 
+// The documents of a segmented pass (SEG = true): the rows of a fleet of K clusters, one document per cluster. Row g belongs
+// to the cluster k with row0[k] <= g < row0[k + 1]; cluster k is live when it is a batch member whose run reported no failure.
+struct KaJsonSegs {
+    int K;
+    const int64_t* row0;        // [K+1] first row of every cluster (run-wide), row0[K] = rows of the run
+    const int32_t* member;      // [K] batch member of cluster k, -1 = left out of the run
+    const unsigned* flags;      // [members] lowest failing topic of every member, 0xFFFFFFFF = none
+    unsigned long long* bytes;  // [K] text bytes of cluster k's rows (zeroed by the host, summed by the length pass)
+    unsigned long long* doc_off;  // [K+1] out: cluster k's document is json[doc_off[k] .. doc_off[k+1]) (empty when dead)
+    uint32_t* shift;            // [K] out: bytes of headers / trailers in front of cluster k's rows
+};
+
 #define KA_JSON_HEAD "{\"partitions\":["
 #define KA_JSON_TAIL "],\"version\":1}"
 #define KA_JSON_HEAD_LEN 15
 #define KA_JSON_TAIL_LEN 14
+#define KA_JSON_MAX_SEGS 128   // clusters of one segmented pass (the batched solves' member limit)
 
 __device__ __forceinline__ uint32_t ka_ndigits(int32_t v) {  // characters of Integer.toString(v)
     uint32_t u = v < 0 ? 0u - (uint32_t)v : (uint32_t)v, n = v < 0 ? 2u : 1u;
@@ -75,19 +88,23 @@ __device__ __forceinline__ void ka_json_row_key(const KaJsonParams& p, uint32_t 
     }
 }
 
-__device__ __forceinline__ uint32_t ka_json_row_len(const KaJsonParams& p, uint32_t q) {
+// Text of row q of the fragment. Every row but the first of its document has a leading comma: the first of the run, or with
+// SEG the first of its cluster (`first`).
+template <bool SEG>
+__device__ __forceinline__ uint32_t ka_json_row_len(const KaJsonParams& p, uint32_t q, bool first) {
     int t, part;
     ka_json_row_key(p, q, t, part);
     const int len = p.out_len[q];
-    uint32_t n = (p.row0 + q > 0 ? 1u : 0u) + 13u + ka_ndigits(part) + 13u + 11u + (uint32_t)(p.name_off[t + 1] - p.name_off[t]) + 2u;
+    uint32_t n = ((SEG ? !first : p.row0 + q > 0) ? 1u : 0u) + 13u + ka_ndigits(part) + 13u + 11u + (uint32_t)(p.name_off[t + 1] - p.name_off[t]) + 2u;
     for (int i = 0; i < len; ++i) n += ka_ndigits(p.out[(size_t)q * p.S + i]) + (i ? 1u : 0u);
     return n;
 }
-__device__ __forceinline__ void ka_json_row_put(const KaJsonParams& p, uint32_t q, char* w) {
+template <bool SEG>
+__device__ __forceinline__ void ka_json_row_put(const KaJsonParams& p, uint32_t q, char* w, bool first) {
     int t, part;
     ka_json_row_key(p, q, t, part);
     const int len = p.out_len[q];
-    if (p.row0 + q > 0) *w++ = ',';
+    if (SEG ? !first : p.row0 + q > 0) *w++ = ',';
     w = ka_put_str(w, "{\"partition\":", 13);
     w = ka_put_int(w, part);
     w = ka_put_str(w, ",\"replicas\":[", 13);
@@ -100,11 +117,44 @@ __device__ __forceinline__ void ka_json_row_put(const KaJsonParams& p, uint32_t 
     ka_put_str(w, "\"}", 2);
 }
 
-// pass 1: text length of every row + per-block sums
-__global__ void __launch_bounds__(256) ka_json_len_kernel(const KaJsonParams p) {
+// Segmented passes: the clusters' first rows, and (live != null) whether each cluster is live, in shared memory.
+__device__ __forceinline__ void ka_json_stage_segs(const KaJsonSegs& sg, int64_t* row0, int* live) {
+    for (int k = threadIdx.x; k <= sg.K; k += blockDim.x) {
+        row0[k] = sg.row0[k];
+        if (live && k < sg.K) live[k] = sg.member[k] >= 0 && sg.flags[sg.member[k]] == 0xFFFFFFFFu;
+    }
+}
+// The cluster of run-wide row g < seg_row0[K] (a cluster without rows never satisfies row0[k] <= g < row0[k + 1]).
+__device__ __forceinline__ int ka_json_seg_of(const int64_t* row0, int K, int64_t g) {
+    int lo = 0, hi = K;
+    while (hi - lo > 1) {
+        const int mid = (lo + hi) >> 1;
+        if (row0[mid] <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// pass 1: text length of every row + per-block sums. SEG: the rows of a dead cluster are empty, the first row of every
+// cluster has no leading comma, and every cluster's bytes are summed into sg.bytes (one atomic per warp and cluster).
+template <bool SEG>
+__global__ void __launch_bounds__(256) ka_json_len_kernel(const KaJsonParams p, const KaJsonSegs sg) {
     __shared__ uint32_t wsum[8];
     const uint32_t q = blockIdx.x * 256u + threadIdx.x;
-    uint32_t n = q < p.Q ? ka_json_row_len(p, q) : 0u;
+    uint32_t n;
+    if constexpr (SEG) {
+        __shared__ int64_t row0[KA_JSON_MAX_SEGS + 1];
+        __shared__ int live[KA_JSON_MAX_SEGS];
+        ka_json_stage_segs(sg, row0, live);
+        __syncthreads();
+        const int64_t g = (int64_t)p.row0 + q;
+        const int k = q < p.Q ? ka_json_seg_of(row0, sg.K, g) : -1;
+        n = k >= 0 && live[k] ? ka_json_row_len<true>(p, q, g == row0[k]) : 0u;
+        const unsigned grp = __match_any_sync(KA_FULL, k);
+        const unsigned sum = __reduce_add_sync(grp, n);
+        if (k >= 0 && sum > 0 && (int)(threadIdx.x & 31) == __ffs(grp) - 1) atomicAdd(sg.bytes + k, (unsigned long long)sum);
+    } else {
+        n = q < p.Q ? ka_json_row_len<false>(p, q, false) : 0u;
+    }
     if (q < p.Q) p.rowlen[q] = n;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(KA_FULL, n, o);
@@ -160,14 +210,49 @@ __global__ void __launch_bounds__(1024) ka_json_scan_kernel(const KaJsonParams p
     }
 }
 
+// Segmented passes, after the last fragment's scan (one CTA of KA_JSON_MAX_SEGS threads): the document table. Rows are in
+// cluster order and a dead cluster's rows are empty, so the rows of cluster k start at sum_{j<k} sg.bytes[j] of the row
+// text, and its document 29 bytes per live cluster before it later. Writes doc_off, shift and every live cluster's header
+// and trailer (the whole document of a live cluster without rows); no text when it would end beyond p.cap.
+__global__ void __launch_bounds__(KA_JSON_MAX_SEGS) ka_json_docs_kernel(const KaJsonParams p, const KaJsonSegs sg) {
+    __shared__ int64_t row0[KA_JSON_MAX_SEGS + 1];
+    __shared__ int live[KA_JSON_MAX_SEGS];
+    __shared__ unsigned long long off[KA_JSON_MAX_SEGS + 1];
+    ka_json_stage_segs(sg, row0, live);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long o = 0;
+        uint32_t before = 0;
+        for (int k = 0; k < sg.K; ++k) {
+            off[k] = o;
+            sg.shift[k] = KA_JSON_HEAD_LEN + (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN) * before;
+            if (live[k]) {
+                o += KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + sg.bytes[k];
+                ++before;
+            }
+        }
+        off[sg.K] = o;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k <= sg.K; k += blockDim.x) {
+        sg.doc_off[k] = off[k];
+        if (k < sg.K && live[k] && off[sg.K] <= p.cap) {
+            ka_put_str(p.json + off[k], KA_JSON_HEAD, KA_JSON_HEAD_LEN);
+            ka_put_str(p.json + off[k + 1] - KA_JSON_TAIL_LEN, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
+        }
+    }
+}
+
 // pass 3: every row writes its text at its final position. The 256 rows of a block are assembled in shared memory (at the
 // same 16-byte phase as their destination) and copied out with coalesced 16-byte stores; blocks whose text does not fit
-// (very long topic names) write straight to global memory.
+// (very long topic names) write straight to global memory. SEG: a row's position moves by its cluster's shift, so a block
+// whose rows span documents (the shift differs at its ends) also writes straight to global memory.
 #define KA_JSON_SMEM_BYTES (64 * 1024)
-__global__ void __launch_bounds__(256) ka_json_write_kernel(const KaJsonParams p) {
+template <bool SEG>
+__global__ void __launch_bounds__(256) ka_json_write_kernel(const KaJsonParams p, const KaJsonSegs sg) {
     extern __shared__ __align__(16) unsigned char ka_jsmem[];
     __shared__ uint32_t wsum[8];
-    if (p.frag[0] + p.frag[1] > p.cap) return;   // caller's buffer too small (uniform: the host reports KA_ERR_LIMIT)
+    if (SEG ? sg.doc_off[sg.K] > p.cap : p.frag[0] + p.frag[1] > p.cap) return;   // caller's buffer too small (uniform)
     const uint32_t q = blockIdx.x * 256u + threadIdx.x;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t n = q < p.Q ? p.rowlen[q] : 0u;
@@ -181,13 +266,30 @@ __global__ void __launch_bounds__(256) ka_json_write_kernel(const KaJsonParams p
     __syncthreads();
     uint32_t woff = 0, bt = 0;
     for (int i = 0; i < 8; ++i) { if (i < warp) woff += wsum[i]; bt += wsum[i]; }
+    uint32_t shift = 0, bshift = 0;   // position shift of my row and of the block's first row
+    bool staged = true, first = false;
+    if constexpr (SEG) {
+        __shared__ int64_t row0[KA_JSON_MAX_SEGS + 1];
+        ka_json_stage_segs(sg, row0, nullptr);
+        __syncthreads();
+        const uint32_t q0 = blockIdx.x * 256u, q1 = min(p.Q, q0 + 256u) - 1;
+        bshift = sg.shift[ka_json_seg_of(row0, sg.K, (int64_t)p.row0 + q0)];
+        staged = bshift == sg.shift[ka_json_seg_of(row0, sg.K, (int64_t)p.row0 + q1)];
+        if (q < p.Q) {
+            const int64_t g = (int64_t)p.row0 + q;
+            const int k = ka_json_seg_of(row0, sg.K, g);
+            shift = sg.shift[k];
+            first = g == row0[k];
+        }
+    }
     char* frag = p.json + p.frag[0];
-    char* dst = frag + p.blocksum[blockIdx.x];                 // this block's text
+    char* dst = frag + p.blocksum[blockIdx.x] + bshift;        // this block's text
     const uint32_t loc = woff + x - n;                           // my row inside it
     const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15u);
-    if (mis + bt <= KA_JSON_SMEM_BYTES) {
+    // SEG: a dead cluster's rows are empty and never read
+    if (staged && mis + bt <= KA_JSON_SMEM_BYTES) {
         char* stage = reinterpret_cast<char*>(ka_jsmem) + mis;
-        if (q < p.Q) ka_json_row_put(p, q, stage + loc);
+        if (SEG ? n > 0 : q < p.Q) ka_json_row_put<SEG>(p, q, stage + loc, first);
         __syncthreads();
         const uint32_t head = min(bt, (16u - mis) & 15u);       // bytes up to the first 16-byte boundary of dst
         for (uint32_t i = threadIdx.x; i < head; i += 256) dst[i] = stage[i];
@@ -196,9 +298,11 @@ __global__ void __launch_bounds__(256) ka_json_write_kernel(const KaJsonParams p
         uint4* d4 = reinterpret_cast<uint4*>(dst + head);
         for (uint32_t i = threadIdx.x; i < body; i += 256) d4[i] = s4[i];
         for (uint32_t i = head + (body << 4) + threadIdx.x; i < bt; i += 256) dst[i] = stage[i];
-    } else if (q < p.Q) {
-        ka_json_row_put(p, q, dst + loc);
+    } else if (SEG ? n > 0 : q < p.Q) {
+        ka_json_row_put<SEG>(p, q, dst + loc + (shift - bshift), first);
     }
-    if (q == 0 && p.first) ka_put_str(frag, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
-    if (q == 0 && p.last) ka_put_str(frag + p.frag[1] - KA_JSON_TAIL_LEN, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
+    if constexpr (!SEG) {   // a segmented pass's headers and trailers come from ka_json_docs_kernel
+        if (q == 0 && p.first) ka_put_str(frag, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
+        if (q == 0 && p.last) ka_put_str(frag + p.frag[1] - KA_JSON_TAIL_LEN, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
+    }
 }

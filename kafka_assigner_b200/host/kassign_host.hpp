@@ -12,6 +12,7 @@
 //                                                          would move and how evenly it spreads replicas and leaders
 //   kassign::solveClusters                            <->  that loop once per cluster of a fleet, each with its own broker
 //                                                          set and a new assigner, in one device call
+//   kassign::solveClustersJson                        <->  the same fleet, with each cluster's org.json text built on the device
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -74,10 +75,12 @@ struct TopicOutput {
     Assignment assignment;
 };
 
+inline bool needsJsonEscape(const std::string& name);
+
 class KafkaTopicAssigner {
 public:
     // `new KafkaTopicAssigner()` (KTA:21-23): one Context per instance.
-    explicit KafkaTopicAssigner(int device = 0) : ctx_(ka_ctx_create(device)) {
+    explicit KafkaTopicAssigner(int device = 0) : ctx_(ka_ctx_create(device)), device_(device) {
         if (!ctx_) throw KassignError(KA_ERR_NO_DEVICE, "no usable CUDA device: kassign has no CPU fallback");
     }
     ~KafkaTopicAssigner() { ka_ctx_destroy(ctx_); }
@@ -153,40 +156,68 @@ public:
     // topic). This instance's own Context is left alone. Rows of at most 3 replicas.
     std::vector<CandidateResult> solveClusters(const std::vector<ClusterInput>& clusters) {
         const int K = (int)clusters.size();
-        std::vector<Flat> flat;
-        std::vector<Candidate> tables;
-        std::vector<int32_t> topicOff(1, 0), desired, hash, partId, cur;
-        std::vector<int64_t> partOff(1, 0), repOff(1, 0);
-        int stride = 1;
-        for (const auto& cl : clusters) {
-            flat.push_back(flatten(cl.topics, cl.desiredReplicationFactor));
-            const Flat& f = flat.back();
-            tables.push_back(Candidate{cl.brokers, cl.rackAssignment});
-            desired.push_back(cl.desiredReplicationFactor);
-            const int64_t row0 = partOff.back(), rep0 = repOff.back();
-            hash.insert(hash.end(), f.hash.begin(), f.hash.end());
-            for (size_t t = 1; t < f.partOff.size(); ++t) partOff.push_back(row0 + f.partOff[t]);
-            for (size_t g = 1; g < f.repOff.size(); ++g) repOff.push_back(rep0 + f.repOff[g]);
-            partId.insert(partId.end(), f.partId.begin(), f.partId.end());
-            cur.insert(cur.end(), f.cur.begin(), f.cur.end());
-            topicOff.push_back((int32_t)hash.size());
-            stride = std::max(stride, f.stride);
-        }
-        std::vector<int32_t> candOff, ids, racks;
-        candidateTables(tables, candOff, ids, racks);
-        const size_t Q = partId.size();
+        const Fleet fl = flattenFleet(clusters);
+        const int stride = fl.stride;
+        const size_t Q = fl.partId.size();
         std::vector<int32_t> outLen(Q, 0), out(Q * stride, -1);
         std::vector<ka_status> st(std::max(K, 1));
-        ka_solve_clusters(ctx_, K, candOff.data(), ids.data(), racks.data(), topicOff.data(), desired.data(), hash.data(), partOff.data(),
-                          partId.data(), repOff.data(), cur.data(), stride, outLen.data(), out.data(), st.data());
+        ka_solve_clusters(ctx_, K, fl.candOff.data(), fl.ids.data(), fl.racks.data(), fl.topicOff.data(), fl.desired.data(), fl.hash.data(),
+                          fl.partOff.data(), fl.partId.data(), fl.repOff.data(), fl.cur.data(), stride, outLen.data(), out.data(), st.data());
         std::vector<CandidateResult> res(K);
         for (int k = 0; k < K; ++k) {
             res[k].status = st[k];
             if (st[k].code != KA_OK) continue;
-            Flat f = flat[k];
+            Flat f = fl.flat[k];
             f.stride = stride;
-            const int64_t row0 = partOff[topicOff[k]];
+            const int64_t row0 = fl.partOff[fl.topicOff[k]];
             res[k].topics = unflatten(f, out.data() + (size_t)row0 * stride, outLen.data() + row0);
+        }
+        return res;
+    }
+
+    // What one cluster's JSON run gave: its status (re-throw with throwForStatus) and, when that is KA_OK, its "NEW ASSIGNMENT"
+    // text.
+    struct ClusterJson {
+        ka_status status;
+        std::string json;
+    };
+
+    // solveClusters with every cluster's text built on the device (ka_solve_clusters_json): cluster k equals solveTopicsJson(its
+    // topics, brokers, racks, desired RF) on a new KafkaTopicAssigner, with the exception it would throw as its status. The
+    // device call refuses clusters whose names org.json would escape or whose rows are wider than 3; those take
+    // solveTopicsJson on a new assigner instead. This instance's own Context is left alone.
+    std::vector<ClusterJson> solveClustersJson(const std::vector<ClusterInput>& clusters) {
+        const int K = (int)clusters.size();
+        const Fleet fl = flattenFleet(clusters);
+        std::string names;
+        std::vector<int64_t> nameOff(1, 0);
+        int64_t cap = 0;   // the sufficient size documented in kassign.h
+        for (const Flat& f : fl.flat) {
+            cap += 64;
+            for (size_t t = 0; t < f.names.size(); ++t) {
+                names += f.names[t];
+                nameOff.push_back((int64_t)names.size());
+                cap += (f.partOff[t + 1] - f.partOff[t]) * (50 + 12 * (int64_t)f.stride + (int64_t)f.names[t].size());
+            }
+        }
+        std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
+        std::vector<int64_t> jsonOff(K + 1, 0);
+        std::vector<ka_status> st(std::max(K, 1));
+        ka_solve_clusters_json(ctx_, K, fl.candOff.data(), fl.ids.data(), fl.racks.data(), fl.topicOff.data(), fl.desired.data(),
+                               fl.hash.data(), fl.partOff.data(), fl.partId.data(), fl.repOff.data(), fl.cur.data(), names.data(),
+                               nameOff.data(), json.get(), cap, jsonOff.data(), st.data());
+        std::vector<ClusterJson> res(K);
+        for (int k = 0; k < K; ++k) {
+            bool escape = false;
+            for (const auto& n : fl.flat[k].names) escape = escape || needsJsonEscape(n);
+            if (escape || fl.flat[k].stride > 3) {
+                KafkaTopicAssigner fresh(device_);
+                res[k].json = fresh.solveTopicsJson(clusters[k].topics, clusters[k].brokers, clusters[k].rackAssignment,
+                                                    clusters[k].desiredReplicationFactor, res[k].status);
+                continue;
+            }
+            res[k].status = st[k];
+            res[k].json.assign(json.get() + jsonOff[k], (size_t)(jsonOff[k + 1] - jsonOff[k]));
         }
         return res;
     }
@@ -242,6 +273,9 @@ public:
     // org.json would escape take that host emitter instead.
     std::string solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
                                 const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor);
+    // solveTopicsJson with the exception it would throw as `st` instead (the text is empty then).
+    std::string solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
+                                const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor, ka_status& st);
 
     ka_ctx* handle() { return ctx_; }
 
@@ -319,7 +353,36 @@ private:
         ids_ = ids;
         racks_ = racks;
     }
+    // A fleet in the shared layout of ka_solve_clusters: every cluster's own flat layout, their broker tables, and the offsets
+    // continued from one cluster to the next. stride = the largest cluster's.
+    struct Fleet {
+        std::vector<Flat> flat;
+        std::vector<int32_t> candOff, ids, racks, topicOff{0}, desired, hash, partId, cur;
+        std::vector<int64_t> partOff{0}, repOff{0};
+        int stride = 1;
+    };
+    static Fleet flattenFleet(const std::vector<ClusterInput>& clusters) {
+        Fleet fl;
+        std::vector<Candidate> tables;
+        for (const auto& cl : clusters) {
+            fl.flat.push_back(flatten(cl.topics, cl.desiredReplicationFactor));
+            const Flat& f = fl.flat.back();
+            tables.push_back(Candidate{cl.brokers, cl.rackAssignment});
+            fl.desired.push_back(cl.desiredReplicationFactor);
+            const int64_t row0 = fl.partOff.back(), rep0 = fl.repOff.back();
+            fl.hash.insert(fl.hash.end(), f.hash.begin(), f.hash.end());
+            for (size_t t = 1; t < f.partOff.size(); ++t) fl.partOff.push_back(row0 + f.partOff[t]);
+            for (size_t g = 1; g < f.repOff.size(); ++g) fl.repOff.push_back(rep0 + f.repOff[g]);
+            fl.partId.insert(fl.partId.end(), f.partId.begin(), f.partId.end());
+            fl.cur.insert(fl.cur.end(), f.cur.begin(), f.cur.end());
+            fl.topicOff.push_back((int32_t)fl.hash.size());
+            fl.stride = std::max(fl.stride, f.stride);
+        }
+        candidateTables(tables, fl.candOff, fl.ids, fl.racks);
+        return fl;
+    }
     ka_ctx* ctx_;
+    int device_;
     std::vector<int32_t> ids_;
     std::map<int, std::string> racks_;
 };
@@ -391,11 +454,29 @@ inline bool needsJsonEscape(const std::string& name) {
 inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
                                                        const std::map<int, std::string>& rackAssignment,
                                                        int desiredReplicationFactor) {
-    for (const auto& t : topics)
-        if (needsJsonEscape(t.name)) return newAssignmentJson(solveTopics(topics, brokers, rackAssignment, desiredReplicationFactor));
+    ka_status st{};
+    std::string json = solveTopicsJson(topics, brokers, rackAssignment, desiredReplicationFactor, st);
+    std::vector<std::string> names;
+    for (const auto& t : topics) names.push_back(t.name);
+    throwForStatus(st, names);
+    return json;
+}
+
+inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
+                                                       const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor,
+                                                       ka_status& st) {
     setBrokers(brokers, rackAssignment);
     const Flat f = flatten(topics, desiredReplicationFactor);
     const int T = (int)topics.size();
+    st = ka_status{};
+    for (const auto& t : topics)
+        if (needsJsonEscape(t.name)) {   // the host emitter over the rows of solveTopics
+            const size_t Q = f.partId.size();
+            std::vector<int32_t> outLen(Q, 0), out(Q * (size_t)f.stride, -1);
+            ka_solve(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
+                     f.stride, outLen.data(), out.data(), &st);
+            return st.code == KA_OK ? newAssignmentJson(unflatten(f, out.data(), outLen.data())) : std::string();
+        }
     std::string names;
     std::vector<int64_t> nameOff(T + 1, 0);
     int64_t cap = 64;  // the sufficient size documented in kassign.h
@@ -406,10 +487,8 @@ inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicIn
     }
     std::unique_ptr<char[]> json(new char[cap]);
     int64_t bytes = 0;
-    ka_status st{};
     ka_solve_json(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
                   names.data(), nameOff.data(), json.get(), cap, &bytes, &st);
-    throwForStatus(st, f.names);
     return std::string(json.get(), (size_t)bytes);
 }
 
