@@ -9,6 +9,7 @@ Same names, argument meaning and error behaviour (message texts of KTA:58-60, 65
 KAS:183-184). All compute happens in libkassign.so's CUDA kernels; nothing here falls back to a CPU
 solver — if the library or a GPU is missing, construction raises.
 """
+import collections
 import ctypes
 
 import numpy as np
@@ -44,18 +45,58 @@ def _ptr(a):
     return a.ctypes.data_as(ctypes.c_void_p) if a is not None else None
 
 
-def _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker):
-    """The ragged layout as the C ABI takes it: (topic_hash, part_off, part_id, rep_off, cur_broker) as contiguous arrays of
-    its element types; part_id may be None."""
-    return (np.ascontiguousarray(topic_hash, dtype=np.int32), np.ascontiguousarray(part_off, dtype=np.int64),
-            None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32),
-            np.ascontiguousarray(rep_off, dtype=np.int64), np.ascontiguousarray(cur_broker, dtype=np.int32))
+def _vp(x):
+    """An optional device pointer or stream (an int, 0 for none) as a C ABI argument."""
+    return ctypes.c_void_p(x) if x else None
 
 
-def _default_stride(rep_off, desired_rf):
-    """The row stride of a ragged solve when the caller gives none: max(longest current list, desired_rf, 1)."""
-    sizes = np.diff(rep_off)
-    return max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+def _check(rc, what=""):
+    """Raise KassignError for a nonzero return code."""
+    if rc:
+        raise KassignError(rc, what)
+
+
+def _statuses(K):
+    """The KaStatus array of a batched call (never empty: the C ABI requires st) and the list of its first K, which share its
+    memory and so read what the call wrote."""
+    st = (KaStatus * max(K, 1))()
+    return st, st[:K]
+
+
+def _stride(longest, desired_rf):
+    """The row stride when the caller gives none: max(longest current list, desired_rf, 1)."""
+    return max(longest, desired_rf, 1)
+
+
+def _json_size(rows, name_bytes, stride):
+    """The sufficient buffer size kassign.h documents for one document: 64 + per row (50 + 12·stride + its topic's name
+    length); name_bytes = Σ rows·name length over the topics."""
+    return 64 + rows * (50 + 12 * stride) + name_bytes
+
+
+class _Ragged(collections.namedtuple("_Ragged", "topic_hash part_off part_id rep_off cur_broker Q")):
+    """A ragged problem as the C ABI takes it: (topic_hash, part_off, part_id, rep_off, cur_broker) as contiguous arrays of
+    their element types (part_id may be None), and Q = ΣP, its number of rows."""
+    __slots__ = ()
+
+    def stride(self, desired_rf):
+        sizes = np.diff(self.rep_off)
+        return _stride(int(sizes.max()) if len(sizes) else 0, desired_rf)
+
+    def name_bytes(self, name_len):
+        """Σ rows·name length, name_len holding one length per topic."""
+        return int(np.dot(np.diff(self.part_off), name_len))
+
+    def ptrs(self):
+        return tuple(_ptr(a) for a in self[:5])
+
+
+def _ragged(topic_hash, part_off, part_id, rep_off, cur_broker):
+    part_off = np.ascontiguousarray(part_off, dtype=np.int64)
+    return _Ragged(np.ascontiguousarray(topic_hash, dtype=np.int32), part_off,
+                   None if part_id is None else np.ascontiguousarray(part_id, dtype=np.int32),
+                   np.ascontiguousarray(rep_off, dtype=np.int64), np.ascontiguousarray(cur_broker, dtype=np.int32),
+                   int(part_off[-1]) if len(part_off) else 0)
 
 
 def raise_for_status(st: KaStatus, topic_names=None):
@@ -102,16 +143,12 @@ class Solver:
 
     # -- Context -------------------------------------------------------------------------------
     def reset(self):
-        rc = self._L.ka_ctx_reset(self._h)
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_reset(self._h))
 
     def set_brokers(self, broker_id, rack_index):
         b = np.ascontiguousarray(broker_id, dtype=np.int32)
         r = np.ascontiguousarray(rack_index, dtype=np.int32)
-        rc = self._L.ka_ctx_set_brokers(self._h, len(b), _ptr(b), _ptr(r))
-        if rc:
-            raise KassignError(rc, "ka_ctx_set_brokers")
+        _check(self._L.ka_ctx_set_brokers(self._h, len(b), _ptr(b), _ptr(r)), "ka_ctx_set_brokers")
         self.N = len(b)
         self.broker_id = b
 
@@ -121,26 +158,20 @@ class Solver:
         names = [rack_assignment.get(int(x)) for x in b]
         arr = (ctypes.c_char_p * len(b))(*[(n.encode("utf-8") if n is not None else None) for n in names])
         racks = np.zeros(len(b), dtype=np.int32)
-        rc = self._L.ka_rack_indices(len(b), _ptr(b), ctypes.cast(arr, ctypes.c_void_p), _ptr(racks))
-        if rc:
-            raise KassignError(rc, "ka_rack_indices")
+        _check(self._L.ka_rack_indices(len(b), _ptr(b), ctypes.cast(arr, ctypes.c_void_p), _ptr(racks)), "ka_rack_indices")
         self.set_brokers(b, racks)
         return b
 
     def counters(self):
         slots = self._L.ka_ctx_counter_slots(self._h)
         out = np.zeros((self.N, slots), dtype=np.int32)
-        rc = self._L.ka_ctx_get_counters(self._h, _ptr(out))
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_get_counters(self._h, _ptr(out)))
         return out
 
     def set_counters(self, ctr):
         c = np.ascontiguousarray(ctr, dtype=np.int32)
         assert c.shape == (self.N, self._L.ka_ctx_counter_slots(self._h))
-        rc = self._L.ka_ctx_set_counters(self._h, _ptr(c))
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_set_counters(self._h, _ptr(c)))
 
     def set_timing(self, on=True):
         self._L.ka_ctx_set_timing(self._h, 1 if on else 0)
@@ -153,9 +184,7 @@ class Solver:
 
     def set_topic_base(self, topic_base):
         """Topic-sharded runs: index of this rank's first topic in the whole run (status reporting)."""
-        rc = self._L.ka_ctx_set_topic_base(self._h, int(topic_base))
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_set_topic_base(self._h, int(topic_base)))
 
     def launch_count(self):
         return int(self._L.ka_ctx_launch_count(self._h))
@@ -164,18 +193,14 @@ class Solver:
         """The leader-order plan of the last solve call (ka_ctx_last_order_plan): (rec_kind, levels, chain threads, ring_log2,
         gctr, loop shape [0 general, 1 warp1, 2 single, 3 full], chain launches, candidates K)."""
         plan = np.zeros(8, dtype=np.int32)
-        rc = self._L.ka_ctx_last_order_plan(self._h, _ptr(plan))
-        if rc:
-            raise KassignError(rc, "ka_ctx_last_order_plan")
+        _check(self._L.ka_ctx_last_order_plan(self._h, _ptr(plan)), "ka_ctx_last_order_plan")
         return tuple(int(x) for x in plan)
 
     def last_stage_plan(self):
         """The sticky/spread plan of the last solve call (ka_ctx_last_stage_plan): (load bytes, levels, SM, candidates K,
         warps per CTA, grid.x, lookup-mode mask [1 shared LUT, 2 global LUT, 4 binary search], kernel A launches)."""
         plan = np.zeros(8, dtype=np.int32)
-        rc = self._L.ka_ctx_last_stage_plan(self._h, _ptr(plan))
-        if rc:
-            raise KassignError(rc, "ka_ctx_last_stage_plan")
+        _check(self._L.ka_ctx_last_stage_plan(self._h, _ptr(plan)), "ka_ctx_last_stage_plan")
         return tuple(int(x) for x in plan)
 
     # -- solves --------------------------------------------------------------------------------
@@ -187,7 +212,7 @@ class Solver:
         th = np.ascontiguousarray(topic_hash, dtype=np.int32)
         assert th.shape == (T,)
         if out_stride is None:
-            out_stride = max(RF, desired_rf if desired_rf >= 0 else RF, 1)
+            out_stride = _stride(RF, desired_rf)
         if out is None:
             out = np.full((T, P, out_stride), -1, dtype=np.int32)
         if out_len is None:
@@ -214,10 +239,8 @@ class Solver:
         T, P, RF = cur.shape
         th = np.ascontiguousarray(topic_hash, dtype=np.int32)
         names, name_off = names_slab if names_slab is not None else self.marshal_names(topic_names)
-        S = max(RF, desired_rf, 1)
-        cap = 64 + T * P * (50 + 12 * S) + int(P * name_off[-1])
-        if json_buf is None:
-            json_buf = np.empty(cap, dtype=np.uint8)
+        if json_buf is None:    # every topic has P rows
+            json_buf = np.empty(_json_size(T * P, P * int(name_off[-1]), _stride(RF, desired_rf)), dtype=np.uint8)
         nbytes = ctypes.c_int64(0)
         st = KaStatus()
         self._L.ka_solve_dense_json(self._h, T, _ptr(th), P, RF, _ptr(cur), int(desired_rf), _ptr(names), _ptr(name_off),
@@ -228,13 +251,12 @@ class Solver:
 
     def solve_ragged(self, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, out_stride, check=True,
                      topic_names=None):
-        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
-        Q = int(part_off[-1]) if len(part_off) else 0
-        out = np.full((Q, out_stride), -1, dtype=np.int32)
-        out_len = np.zeros(Q, dtype=np.int32)
+        r = _ragged(topic_hash, part_off, part_id, rep_off, cur_broker)
+        out = np.full((r.Q, out_stride), -1, dtype=np.int32)
+        out_len = np.zeros(r.Q, dtype=np.int32)
         st = KaStatus()
-        self._L.ka_solve(self._h, len(th), _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker),
-                         int(desired_rf), int(out_stride), _ptr(out_len), _ptr(out), ctypes.byref(st))
+        self._L.ka_solve(self._h, len(r.topic_hash), *r.ptrs(), int(desired_rf), int(out_stride), _ptr(out_len), _ptr(out),
+                         ctypes.byref(st))
         if check:
             raise_for_status(st, topic_names)
         return out, out_len, st
@@ -244,35 +266,32 @@ class Solver:
         """ka_solve_json: the ragged solve of solve_ragged + the reassignment JSON built on the device (KAG:169-186);
         returns (bytes-like view of the text, status). json_buf: optional writable uint8 numpy array (pinned for full
         PCIe speed); by default one of the documented sufficient size."""
-        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
+        r = _ragged(topic_hash, part_off, part_id, rep_off, cur_broker)
         names, name_off = self.marshal_names(topic_names)
         if json_buf is None:
-            S = _default_stride(rep_off, desired_rf)
-            rows = np.diff(part_off)
-            json_buf = np.empty(64 + int(part_off[-1]) * (50 + 12 * S) + int(np.dot(rows, np.diff(name_off))), dtype=np.uint8)
+            json_buf = np.empty(_json_size(r.Q, r.name_bytes(np.diff(name_off)), r.stride(desired_rf)), dtype=np.uint8)
         nbytes = ctypes.c_int64(0)
         st = KaStatus()
-        self._L.ka_solve_json(self._h, len(th), _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker),
-                              int(desired_rf), _ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size),
-                              ctypes.byref(nbytes), ctypes.byref(st))
+        self._L.ka_solve_json(self._h, len(r.topic_hash), *r.ptrs(), int(desired_rf), _ptr(names), _ptr(name_off), _ptr(json_buf),
+                              int(json_buf.size), ctypes.byref(nbytes), ctypes.byref(st))
         if check:
             raise_for_status(st, topic_names)
         return json_buf[:nbytes.value], st
 
+    def _synced(self, name, *args, stream, sync):
+        """Call the device-pointer entry `name` on `stream`: with sync, return its KaStatus without raising; otherwise raise
+        on its return code and return None."""
+        st = KaStatus()
+        rc = getattr(self._L, name)(self._h, *args, _vp(stream), ctypes.byref(st) if sync else None)
+        if sync:
+            return st
+        _check(rc, name)
+
     def solve_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, d_out_len, d_out, stream=0,
                            sync=True):
         """Device-pointer form (ints from tensor.data_ptr()); returns KaStatus when sync else None."""
-        st = KaStatus()
-        rc = self._L.ka_solve_dense_device(self._h, int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF),
-                                           ctypes.c_void_p(d_cur), int(desired_rf), int(out_stride),
-                                           ctypes.c_void_p(d_out_len) if d_out_len else None, ctypes.c_void_p(d_out),
-                                           ctypes.c_void_p(stream) if stream else None,
-                                           ctypes.byref(st) if sync else None)
-        if not sync:
-            if rc:
-                raise KassignError(rc, "ka_solve_dense_device")
-            return None
-        return st
+        return self._synced("ka_solve_dense_device", int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF), ctypes.c_void_p(d_cur),
+                            int(desired_rf), int(out_stride), _vp(d_out_len), ctypes.c_void_p(d_out), stream=stream, sync=sync)
 
     def solve_dense_candidates_device(self, tables, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, d_out_len, d_out,
                                       stream=0):
@@ -280,13 +299,12 @@ class Solver:
         (broker_id, rack_index) numpy pairs), each on a fresh Context; this Solver's own Context is untouched. Candidate k's
         rows are d_out[k] ([K, T, P, out_stride] on the device). Synchronous; returns the K KaStatus."""
         cand_off, broker_id, broker_rack = self._candidate_tables(tables)
-        st = (KaStatus * max(len(tables), 1))()
+        st, sts = _statuses(len(tables))
         self._L.ka_solve_dense_candidates_device(self._h, len(tables), _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), int(T),
                                                  ctypes.c_void_p(d_topic_hash), int(P), int(RF), ctypes.c_void_p(d_cur),
-                                                 int(desired_rf), int(out_stride),
-                                                 ctypes.c_void_p(d_out_len) if d_out_len else None, ctypes.c_void_p(d_out),
-                                                 ctypes.c_void_p(stream) if stream else None, st)
-        return [st[k] for k in range(len(tables))]
+                                                 int(desired_rf), int(out_stride), _vp(d_out_len), ctypes.c_void_p(d_out),
+                                                 _vp(stream), st)
+        return sts
 
     @staticmethod
     def _candidate_tables(tables):
@@ -300,24 +318,27 @@ class Solver:
         broker_rack = np.concatenate(racks) if racks else np.zeros(0, dtype=np.int32)
         return cand_off, broker_id, broker_rack
 
+    def _candidates_call(self, tables, ragged, desired_rf, out_stride):
+        """The start both ragged candidate calls share: (Q, the row stride, cand_off, the leading C ABI arguments ctx, K,
+        tables, T, problem, desired_rf, stride) for the ragged problem `ragged` against every table of `tables`."""
+        r = _ragged(*ragged)
+        S = r.stride(desired_rf) if out_stride is None else out_stride
+        cand_off, broker_id, broker_rack = self._candidate_tables(tables)
+        return r.Q, S, cand_off, (self._h, len(tables), _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), len(r.topic_hash),
+                                  *r.ptrs(), int(desired_rf), int(S))
+
     def solve_ragged_candidates(self, tables, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, out_stride=None):
         """ka_solve_candidates: the ragged solve of solve_ragged against every broker table of `tables` (a list of
         (broker_id, rack_index) numpy pairs), each on a fresh Context; this Solver's own Context is untouched. out_stride
         defaults to max(longest current list, desired_rf, 1). Returns (out [K, ΣP, out_stride], out_len [K, ΣP], [KaStatus] * K);
         the rows of a failed candidate are unspecified."""
-        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
-        if out_stride is None:
-            out_stride = _default_stride(rep_off, desired_rf)
-        cand_off, broker_id, broker_rack = self._candidate_tables(tables)
         K = len(tables)
-        Q = int(part_off[-1]) if len(part_off) else 0
-        out = np.full((K, Q, out_stride), -1, dtype=np.int32)
+        Q, S, _, args = self._candidates_call(tables, (topic_hash, part_off, part_id, rep_off, cur_broker), desired_rf, out_stride)
+        out = np.full((K, Q, S), -1, dtype=np.int32)
         out_len = np.zeros((K, Q), dtype=np.int32)
-        st = (KaStatus * max(K, 1))()
-        self._L.ka_solve_candidates(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), len(th), _ptr(th),
-                                    _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker), int(desired_rf),
-                                    int(out_stride), _ptr(out_len), _ptr(out), st)
-        return out, out_len, [st[k] for k in range(K)]
+        st, sts = _statuses(K)
+        self._L.ka_solve_candidates(*args, _ptr(out_len), _ptr(out), st)
+        return out, out_len, sts
 
     def score_ragged_candidates(self, tables, topic_hash, part_off, part_id, rep_off, cur_broker, desired_rf, out_stride=None,
                                 weight=None, rows=False, per_broker=False):
@@ -325,23 +346,17 @@ class Solver:
         None = 1 per row. Returns (summary, [KaStatus] * K), summary a numpy structured array [K] with the fields of
         ka_move_summary; then, with rows=True, (out [K, ΣP, out_stride], out_len [K, ΣP]) as solve_ragged_candidates returns
         them; then, with per_broker=True, (replicas, leaders, added): one int64 array per table, aligned with its broker ids."""
-        th, part_off, part_id, rep_off, cur_broker = _ragged_arrays(topic_hash, part_off, part_id, rep_off, cur_broker)
-        weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
-        if out_stride is None:
-            out_stride = _default_stride(rep_off, desired_rf)
-        cand_off, broker_id, broker_rack = self._candidate_tables(tables)
         K = len(tables)
-        Q = int(part_off[-1]) if len(part_off) else 0
+        Q, S, cand_off, args = self._candidates_call(tables, (topic_hash, part_off, part_id, rep_off, cur_broker), desired_rf,
+                                                     out_stride)
+        weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
         summary = np.zeros(K, dtype=MOVE_SUMMARY_DTYPE)
-        out = np.full((K, Q, out_stride), -1, dtype=np.int32) if rows else None
+        out = np.full((K, Q, S), -1, dtype=np.int32) if rows else None
         out_len = np.zeros((K, Q), dtype=np.int32) if rows else None
         brk = [np.zeros(int(cand_off[-1]), dtype=np.int64) for _ in range(3)] if per_broker else [None] * 3
-        st = (KaStatus * max(K, 1))()
-        self._L.ka_score_candidates(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), len(th), _ptr(th),
-                                    _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur_broker), int(desired_rf),
-                                    int(out_stride), _ptr(weight), _ptr(summary), *[_ptr(a) for a in brk], _ptr(out_len),
-                                    _ptr(out), st)
-        res = (summary, [st[k] for k in range(K)])
+        st, sts = _statuses(K)
+        self._L.ka_score_candidates(*args, _ptr(weight), _ptr(summary), *[_ptr(a) for a in brk], _ptr(out_len), _ptr(out), st)
+        res = (summary, sts)
         if rows:
             res += (out, out_len)
         if per_broker:
@@ -354,29 +369,26 @@ class Solver:
         part_id, rep_off, cur_broker, desired_rf) with its own offsets from 0 (part_id may be None: 0..P-1 per topic). Returns
         (cand_off, broker_id, broker_rack, topic_off, desired_rf, topic_hash, part_off, part_id, rep_off, cur_broker)."""
         cand_off, broker_id, broker_rack = Solver._candidate_tables([(c[0], c[1]) for c in clusters])
-        th = [np.ascontiguousarray(c[2], dtype=np.int32) for c in clusters]
-        po = [np.ascontiguousarray(c[3], dtype=np.int64) for c in clusters]
-        ro = [np.ascontiguousarray(c[5], dtype=np.int64) for c in clusters]
-        cur = [np.ascontiguousarray(c[6], dtype=np.int32) for c in clusters]
+        rg = [_ragged(*c[2:7]) for c in clusters]         # a cluster without topics may pass part_off = [0] or []
         topic_off = np.zeros(len(clusters) + 1, dtype=np.int32)
-        np.cumsum([len(h) for h in th], out=topic_off[1:])
-        rows = [int(p[-1]) if len(p) > 1 else 0 for p in po]          # a cluster without topics may pass part_off = [0] or []
-        reps = [int(r[rows[k]]) if rows[k] > 0 else 0 for k, r in enumerate(ro)]
-        row0 = np.concatenate([[0], np.cumsum(rows)]).astype(np.int64)
+        np.cumsum([len(r.topic_hash) for r in rg], out=topic_off[1:])
+        reps = [int(r.rep_off[r.Q]) if r.Q > 0 else 0 for r in rg]
+        row0 = np.concatenate([[0], np.cumsum([r.Q for r in rg])]).astype(np.int64)
         rep0 = np.concatenate([[0], np.cumsum(reps)]).astype(np.int64)
-        part_off = np.concatenate([[0]] + [p[1:len(h) + 1] + row0[k] for k, (p, h) in enumerate(zip(po, th))]).astype(np.int64)
-        rep_off = np.concatenate([[0]] + [r[1:rows[k] + 1] + rep0[k] for k, r in enumerate(ro)]).astype(np.int64)
+        part_off = np.concatenate([[0]] + [r.part_off[1:len(r.topic_hash) + 1] + row0[k] for k, r in enumerate(rg)]).astype(np.int64)
+        rep_off = np.concatenate([[0]] + [r.rep_off[1:r.Q + 1] + rep0[k] for k, r in enumerate(rg)]).astype(np.int64)
         none = np.zeros(0, dtype=np.int32)
 
-        def ids(k):   # partition ids of cluster k (ordinals inside each topic when it has none)
-            if clusters[k][4] is not None:
-                return np.ascontiguousarray(clusters[k][4], dtype=np.int32)[:rows[k]]
-            return np.concatenate([none] + [np.arange(int(po[k][t + 1] - po[k][t]), dtype=np.int32) for t in range(len(th[k]))])
+        def ids(r):   # partition ids of a cluster (ordinals inside each topic when it has none)
+            if r.part_id is not None:
+                return r.part_id[:r.Q]
+            return np.concatenate([none] + [np.arange(int(r.part_off[t + 1] - r.part_off[t]), dtype=np.int32)
+                                            for t in range(len(r.topic_hash))])
 
-        part_id = np.concatenate([none] + [ids(k) for k in range(len(clusters))])
+        part_id = np.concatenate([none] + [ids(r) for r in rg])
         desired_rf = np.array([int(c[7]) for c in clusters], dtype=np.int32)
-        return (cand_off, broker_id, broker_rack, topic_off, desired_rf, np.concatenate([none] + th), part_off, part_id, rep_off,
-                np.concatenate([none] + [c[:reps[k]] for k, c in enumerate(cur)]))
+        return (cand_off, broker_id, broker_rack, topic_off, desired_rf, np.concatenate([none] + [r.topic_hash for r in rg]), part_off,
+                part_id, rep_off, np.concatenate([none] + [r.cur_broker[:reps[k]] for k, r in enumerate(rg)]))
 
     def solve_clusters(self, clusters, out_stride=None):
         """ka_solve_clusters: every cluster of `clusters` solved against its own broker table, each on a fresh Context, in one
@@ -385,18 +397,17 @@ class Solver:
         largest desired_rf, 1) over the fleet. Returns one (out [P_k, out_stride], out_len [P_k], KaStatus) per cluster; the rows
         of a failed cluster are unspecified."""
         K = len(clusters)
-        cand_off, broker_id, broker_rack, topic_off, drf, th, part_off, part_id, rep_off, cur = self.marshal_clusters(clusters)
+        cand_off, broker_id, broker_rack, topic_off, drf, *fleet = self.marshal_clusters(clusters)
+        fleet = _ragged(*fleet)
         if out_stride is None:
-            out_stride = _default_stride(rep_off, int(drf.max()) if K else -1)
-        Q = int(part_off[-1])
-        out = np.full((Q, out_stride), -1, dtype=np.int32)
-        out_len = np.zeros(Q, dtype=np.int32)
-        st = (KaStatus * max(K, 1))()
+            out_stride = fleet.stride(int(drf.max()) if K else -1)
+        out = np.full((fleet.Q, out_stride), -1, dtype=np.int32)
+        out_len = np.zeros(fleet.Q, dtype=np.int32)
+        st, sts = _statuses(K)
         self._L.ka_solve_clusters(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), _ptr(topic_off), _ptr(drf),
-                                  _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur), int(out_stride), _ptr(out_len),
-                                  _ptr(out), st)
-        rows = part_off[topic_off]
-        return [(out[rows[k]:rows[k + 1]], out_len[rows[k]:rows[k + 1]], st[k]) for k in range(K)]
+                                  *fleet.ptrs(), int(out_stride), _ptr(out_len), _ptr(out), st)
+        rows = fleet.part_off[topic_off]
+        return [(out[rows[k]:rows[k + 1]], out_len[rows[k]:rows[k + 1]], sts[k]) for k in range(K)]
 
     def solve_clusters_json(self, clusters, topic_names, json_buf=None):
         """ka_solve_clusters_json: the fleet of solve_clusters, every cluster's reassignment JSON built on the device.
@@ -404,41 +415,32 @@ class Solver:
         by default one of the documented sufficient size. Returns one (bytes-like view of the cluster's text, KaStatus) per
         cluster; the text of a failed cluster is empty."""
         K = len(clusters)
-        cand_off, broker_id, broker_rack, topic_off, drf, th, part_off, part_id, rep_off, cur = self.marshal_clusters(clusters)
+        cand_off, broker_id, broker_rack, topic_off, drf, *fleet = self.marshal_clusters(clusters)
+        fleet = _ragged(*fleet)
         names, name_off = self.marshal_names([n for names_k in topic_names for n in names_k])
-        assert len(name_off) == len(th) + 1
-        if json_buf is None:
-            rows, name_len, cap = np.diff(part_off), np.diff(name_off), 0
-            for k in range(K):
-                t0, t1 = int(topic_off[k]), int(topic_off[k + 1])
-                S = _default_stride(rep_off[part_off[t0]:part_off[t1] + 1], int(drf[k]))
-                cap += 64 + int(part_off[t1] - part_off[t0]) * (50 + 12 * S) + int(np.dot(rows[t0:t1], name_len[t0:t1]))
+        assert len(name_off) == len(fleet.topic_hash) + 1
+        if json_buf is None:    # one document per cluster, each sized as solve_ragged_json sizes it
+            name_len = np.diff(name_off)
+            cap = 0
+            for k, c in enumerate(clusters):
+                r = _ragged(*c[2:7])
+                cap += _json_size(r.Q, r.name_bytes(name_len[topic_off[k]:topic_off[k + 1]]), r.stride(int(drf[k])))
             json_buf = np.empty(max(cap, 1), dtype=np.uint8)
         json_off = np.zeros(K + 1, dtype=np.int64)
-        st = (KaStatus * max(K, 1))()
+        st, sts = _statuses(K)
         self._L.ka_solve_clusters_json(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), _ptr(topic_off), _ptr(drf),
-                                       _ptr(th), _ptr(part_off), _ptr(part_id), _ptr(rep_off), _ptr(cur), _ptr(names),
-                                       _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(json_off), st)
-        return [(json_buf[json_off[k]:json_off[k + 1]], st[k]) for k in range(K)]
+                                       *fleet.ptrs(), _ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(json_off),
+                                       st)
+        return [(json_buf[json_off[k]:json_off[k + 1]], sts[k]) for k in range(K)]
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""
-        rc = self._L.ka_stage_dense_device(self._h, int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF),
-                                           ctypes.c_void_p(d_cur), int(desired_rf), int(out_stride),
-                                           ctypes.c_void_p(stream) if stream else None)
-        if rc:
-            raise KassignError(rc, "ka_stage_dense_device")
+        _check(self._L.ka_stage_dense_device(self._h, int(T), ctypes.c_void_p(d_topic_hash), int(P), int(RF), ctypes.c_void_p(d_cur),
+                                             int(desired_rf), int(out_stride), _vp(stream)), "ka_stage_dense_device")
 
     def order_device(self, d_out_len, d_out, stream=0, sync=True):
         """Leader-order stage (KAS:202-239) of the staged block against this Context's counters."""
-        st = KaStatus()
-        rc = self._L.ka_order_device(self._h, ctypes.c_void_p(d_out_len) if d_out_len else None, ctypes.c_void_p(d_out),
-                                     ctypes.c_void_p(stream) if stream else None, ctypes.byref(st) if sync else None)
-        if not sync:
-            if rc:
-                raise KassignError(rc, "ka_order_device")
-            return None
-        return st
+        return self._synced("ka_order_device", _vp(d_out_len), ctypes.c_void_p(d_out), stream=stream, sync=sync)
 
     def staged_slot_chains(self):
         """2 when the staged block is ordered by per-slot chains (rows <= 3), else 0."""
@@ -446,29 +448,16 @@ class Solver:
 
     def order_slot_device(self, slot, stream=0):
         """Slot-0 / slot-1 leader-order chain of the staged block (reads and bumps only counter[.][slot])."""
-        rc = self._L.ka_order_slot_device(self._h, int(slot), ctypes.c_void_p(stream) if stream else None)
-        if rc:
-            raise KassignError(rc, "ka_order_slot_device")
+        _check(self._L.ka_order_slot_device(self._h, int(slot), _vp(stream)), "ka_order_slot_device")
 
     def emit_device(self, d_out_len, d_out, stream=0, sync=True):
-        st = KaStatus()
-        rc = self._L.ka_emit_device(self._h, ctypes.c_void_p(d_out_len) if d_out_len else None, ctypes.c_void_p(d_out),
-                                    ctypes.c_void_p(stream) if stream else None, ctypes.byref(st) if sync else None)
-        if not sync:
-            if rc:
-                raise KassignError(rc, "ka_emit_device")
-            return None
-        return st
+        return self._synced("ka_emit_device", _vp(d_out_len), ctypes.c_void_p(d_out), stream=stream, sync=sync)
 
     def export_counter_slot_device(self, slot, d_ptr, stream=0):
-        rc = self._L.ka_ctx_export_counter_slot_device(self._h, int(slot), ctypes.c_void_p(d_ptr), ctypes.c_void_p(stream) if stream else None)
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_export_counter_slot_device(self._h, int(slot), ctypes.c_void_p(d_ptr), _vp(stream)))
 
     def import_counter_slot_device(self, slot, d_ptr, stream=0):
-        rc = self._L.ka_ctx_import_counter_slot_device(self._h, int(slot), ctypes.c_void_p(d_ptr), ctypes.c_void_p(stream) if stream else None)
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_import_counter_slot_device(self._h, int(slot), ctypes.c_void_p(d_ptr), _vp(stream)))
 
     def last_status(self):
         st = KaStatus()
@@ -476,14 +465,10 @@ class Solver:
         return st
 
     def export_counters_device(self, d_ptr, stream=0):
-        rc = self._L.ka_ctx_export_counters_device(self._h, ctypes.c_void_p(d_ptr), ctypes.c_void_p(stream) if stream else None)
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_export_counters_device(self._h, ctypes.c_void_p(d_ptr), _vp(stream)))
 
     def import_counters_device(self, d_ptr, stream=0):
-        rc = self._L.ka_ctx_import_counters_device(self._h, ctypes.c_void_p(d_ptr), ctypes.c_void_p(stream) if stream else None)
-        if rc:
-            raise KassignError(rc)
+        _check(self._L.ka_ctx_import_counters_device(self._h, ctypes.c_void_p(d_ptr), _vp(stream)))
 
     def solve_cluster(self, cluster, check=True):
         """The KAG:172-184 loop for a synth.Cluster: all topics in order through this Context."""
@@ -523,9 +508,7 @@ class KafkaTopicAssigner:
         if parts:
             np.cumsum([len(l) for l in lists], out=rep_off[1:])
         cur = np.array([b for l in lists for b in l], dtype=np.int32)
-        maxlen = max([len(l) for l in lists], default=0)
-        stride = max(1, maxlen, desired_replication_factor if desired_replication_factor >= 0 else 0)
-        th = np.array([java_string_hash(topic)], dtype=np.int32)
-        out, out_len, _ = self._solver.solve_ragged(th, part_off, np.array(parts, dtype=np.int32), rep_off, cur,
-                                                    desired_replication_factor, stride, check=True, topic_names=[topic])
+        r = _ragged([java_string_hash(topic)], part_off, parts, rep_off, cur)
+        out, out_len, _ = self._solver.solve_ragged(*r[:5], desired_replication_factor, r.stride(desired_replication_factor),
+                                                    check=True, topic_names=[topic])
         return {p: [int(x) for x in out[i, :out_len[i]]] for i, p in enumerate(parts)}

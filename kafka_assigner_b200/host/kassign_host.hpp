@@ -99,14 +99,10 @@ public:
                                          const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor) {
         setBrokers(brokers, rackAssignment);
         const Flat f = flatten(topics, desiredReplicationFactor);
-        const int T = (int)topics.size();
-        const size_t Q = f.partId.size();
-        std::vector<int32_t> outLen(Q, 0), out(Q * (size_t)f.stride, -1);
         ka_status st{};
-        ka_solve(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
-                 f.stride, outLen.data(), out.data(), &st);
+        std::vector<TopicOutput> res = solveFlat(f, desiredReplicationFactor, st);
         throwForStatus(st, f.names);
-        return unflatten(f, out.data(), outLen.data());
+        return res;
     }
 
     // One candidate broker set of a batched run: the `brokers` and `rackAssignment` of generateAssignment.
@@ -127,19 +123,14 @@ public:
                                                        int desiredReplicationFactor) {
         const Flat f = flatten(topics, desiredReplicationFactor);
         const int K = (int)candidates.size(), T = (int)topics.size();
-        std::vector<int32_t> candOff, ids, racks;
-        candidateTables(candidates, candOff, ids, racks);
+        std::vector<int32_t> candOff{0}, ids, racks;
+        for (const Candidate& c : candidates) addTable(c.brokers, c.rackAssignment, candOff, ids, racks);
         const size_t Q = f.partId.size();
         std::vector<int32_t> outLen((size_t)K * Q, 0), out((size_t)K * Q * f.stride, -1);
         std::vector<ka_status> st(std::max(K, 1));
         ka_solve_candidates(ctx_, K, candOff.data(), ids.data(), racks.data(), T, f.hash.data(), f.partOff.data(), f.partId.data(),
                             f.repOff.data(), f.cur.data(), desiredReplicationFactor, f.stride, outLen.data(), out.data(), st.data());
-        std::vector<CandidateResult> res(K);
-        for (int k = 0; k < K; ++k) {
-            res[k].status = st[k];
-            if (st[k].code == KA_OK) res[k].topics = unflatten(f, out.data() + (size_t)k * Q * f.stride, outLen.data() + (size_t)k * Q);
-        }
-        return res;
+        return memberResults(st, K, f.stride, out, outLen, [&](int k) { return std::make_pair(&f, (int64_t)(k * Q)); });
     }
 
     // One cluster of a fleet: its topics and the arguments of its own run.
@@ -163,16 +154,7 @@ public:
         std::vector<ka_status> st(std::max(K, 1));
         ka_solve_clusters(ctx_, K, fl.candOff.data(), fl.ids.data(), fl.racks.data(), fl.topicOff.data(), fl.desired.data(), fl.hash.data(),
                           fl.partOff.data(), fl.partId.data(), fl.repOff.data(), fl.cur.data(), stride, outLen.data(), out.data(), st.data());
-        std::vector<CandidateResult> res(K);
-        for (int k = 0; k < K; ++k) {
-            res[k].status = st[k];
-            if (st[k].code != KA_OK) continue;
-            Flat f = fl.flat[k];
-            f.stride = stride;
-            const int64_t row0 = fl.partOff[fl.topicOff[k]];
-            res[k].topics = unflatten(f, out.data() + (size_t)row0 * stride, outLen.data() + row0);
-        }
-        return res;
+        return memberResults(st, K, stride, out, outLen, [&](int k) { return std::make_pair(&fl.flat[k], fl.partOff[fl.topicOff[k]]); });
     }
 
     // What one cluster's JSON run gave: its status (re-throw with throwForStatus) and, when that is KA_OK, its "NEW ASSIGNMENT"
@@ -191,15 +173,8 @@ public:
         const Fleet fl = flattenFleet(clusters);
         std::string names;
         std::vector<int64_t> nameOff(1, 0);
-        int64_t cap = 0;   // the sufficient size documented in kassign.h
-        for (const Flat& f : fl.flat) {
-            cap += 64;
-            for (size_t t = 0; t < f.names.size(); ++t) {
-                names += f.names[t];
-                nameOff.push_back((int64_t)names.size());
-                cap += (f.partOff[t + 1] - f.partOff[t]) * (50 + 12 * (int64_t)f.stride + (int64_t)f.names[t].size());
-            }
-        }
+        int64_t cap = 0;
+        for (const Flat& f : fl.flat) cap += appendNames(f, names, nameOff);
         std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
         std::vector<int64_t> jsonOff(K + 1, 0);
         std::vector<ka_status> st(std::max(K, 1));
@@ -238,8 +213,8 @@ public:
                                                       const std::vector<std::map<int, int64_t>>& weights = {}, bool perBroker = false) {
         const Flat f = flatten(topics, desiredReplicationFactor);
         const int K = (int)candidates.size(), T = (int)topics.size();
-        std::vector<int32_t> candOff, ids, racks;
-        candidateTables(candidates, candOff, ids, racks);
+        std::vector<int32_t> candOff{0}, ids, racks;
+        for (const Candidate& c : candidates) addTable(c.brokers, c.rackAssignment, candOff, ids, racks);
         std::vector<int64_t> w;
         if (!weights.empty()) {
             if (weights.size() != topics.size()) throw std::invalid_argument("one weight map per topic");
@@ -310,15 +285,48 @@ private:
         return f;
     }
     // Rows of the flat layout (out[ΣP][stride], outLen[ΣP]) -> per-topic assignments.
-    static std::vector<TopicOutput> unflatten(const Flat& f, const int32_t* out, const int32_t* outLen) {
+    static std::vector<TopicOutput> unflatten(const Flat& f, int stride, const int32_t* out, const int32_t* outLen) {
         const int T = (int)f.names.size();
         std::vector<TopicOutput> res(T);
         for (int t = 0; t < T; ++t) {
             res[t].name = f.names[t];
             for (int64_t g = f.partOff[t]; g < f.partOff[t + 1]; ++g)
-                res[t].assignment[f.partId[g]] = std::vector<int>(out + g * f.stride, out + g * f.stride + outLen[g]);
+                res[t].assignment[f.partId[g]] = std::vector<int>(out + g * stride, out + g * stride + outLen[g]);
         }
         return res;
+    }
+    // ka_solve of `f` on this instance's Context into fresh rows -> per-topic assignments (none unless st is KA_OK).
+    std::vector<TopicOutput> solveFlat(const Flat& f, int desiredReplicationFactor, ka_status& st) {
+        const size_t Q = f.partId.size();
+        std::vector<int32_t> outLen(Q, 0), out(Q * (size_t)f.stride, -1);
+        ka_solve(ctx_, (int)f.names.size(), f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
+                 desiredReplicationFactor, f.stride, outLen.data(), out.data(), &st);
+        return st.code == KA_OK ? unflatten(f, f.stride, out.data(), outLen.data()) : std::vector<TopicOutput>();
+    }
+    // What each member of a batched call gave: its status and, when that is KA_OK, its rows. member(k) gives the member's flat
+    // layout and its first row in out[.][stride] / outLen.
+    template <class Member>
+    static std::vector<CandidateResult> memberResults(const std::vector<ka_status>& st, int K, int stride, const std::vector<int32_t>& out,
+                                                      const std::vector<int32_t>& outLen, Member member) {
+        std::vector<CandidateResult> res(K);
+        for (int k = 0; k < K; ++k) {
+            res[k].status = st[k];
+            if (st[k].code != KA_OK) continue;
+            const std::pair<const Flat*, int64_t> m = member(k);
+            res[k].topics = unflatten(*m.first, stride, out.data() + m.second * stride, outLen.data() + m.second);
+        }
+        return res;
+    }
+    // Append the names of `f` to a name slab (names, nameOff) and return its document's sufficient size, documented in kassign.h:
+    // 64 + per row (50 + 12·stride + its topic's name length).
+    static int64_t appendNames(const Flat& f, std::string& names, std::vector<int64_t>& nameOff) {
+        int64_t cap = 64;
+        for (size_t t = 0; t < f.names.size(); ++t) {
+            names += f.names[t];
+            nameOff.push_back((int64_t)names.size());
+            cap += (f.partOff[t + 1] - f.partOff[t]) * (50 + 12 * (int64_t)f.stride + (int64_t)f.names[t].size());
+        }
+        return cap;
     }
     // Rack index of every broker of `ids` (ascending) from the rack strings (ka_rack_indices, KAS:81-94).
     static int rackIndices(const std::vector<int32_t>& ids, const std::map<int, std::string>& racks, std::vector<int32_t>& rackIdx) {
@@ -330,18 +338,15 @@ private:
         rackIdx.assign(ids.size(), 0);
         return ka_rack_indices((int32_t)ids.size(), ids.data(), names.data(), rackIdx.data());
     }
-    // The candidate tables of the C ABI (cand_off, broker_id, broker_rack) of a list of broker sets.
-    static void candidateTables(const std::vector<Candidate>& candidates, std::vector<int32_t>& candOff, std::vector<int32_t>& ids,
-                                std::vector<int32_t>& racks) {
-        candOff.assign(candidates.size() + 1, 0);
-        for (size_t k = 0; k < candidates.size(); ++k) {
-            std::vector<int32_t> id(candidates[k].brokers.begin(), candidates[k].brokers.end()), rackIdx;
-            const int rc = rackIndices(id, candidates[k].rackAssignment, rackIdx);
-            if (rc != KA_OK) throw KassignError(rc, "ka_rack_indices");
-            ids.insert(ids.end(), id.begin(), id.end());
-            racks.insert(racks.end(), rackIdx.begin(), rackIdx.end());
-            candOff[k + 1] = (int32_t)ids.size();
-        }
+    // Append one broker set to the candidate tables of the C ABI (cand_off, broker_id, broker_rack); candOff starts as {0}.
+    static void addTable(const std::set<int>& brokers, const std::map<int, std::string>& rackAssignment, std::vector<int32_t>& candOff,
+                         std::vector<int32_t>& ids, std::vector<int32_t>& racks) {
+        std::vector<int32_t> id(brokers.begin(), brokers.end()), rackIdx;
+        const int rc = rackIndices(id, rackAssignment, rackIdx);
+        if (rc != KA_OK) throw KassignError(rc, "ka_rack_indices");
+        ids.insert(ids.end(), id.begin(), id.end());
+        racks.insert(racks.end(), rackIdx.begin(), rackIdx.end());
+        candOff.push_back((int32_t)ids.size());
     }
     void setBrokers(const std::set<int>& brokers, const std::map<int, std::string>& racks) {
         std::vector<int32_t> ids(brokers.begin(), brokers.end());  // std::set: ascending == TreeMap order (KAS:78)
@@ -357,17 +362,16 @@ private:
     // continued from one cluster to the next. stride = the largest cluster's.
     struct Fleet {
         std::vector<Flat> flat;
-        std::vector<int32_t> candOff, ids, racks, topicOff{0}, desired, hash, partId, cur;
+        std::vector<int32_t> candOff{0}, ids, racks, topicOff{0}, desired, hash, partId, cur;
         std::vector<int64_t> partOff{0}, repOff{0};
         int stride = 1;
     };
     static Fleet flattenFleet(const std::vector<ClusterInput>& clusters) {
         Fleet fl;
-        std::vector<Candidate> tables;
         for (const auto& cl : clusters) {
             fl.flat.push_back(flatten(cl.topics, cl.desiredReplicationFactor));
             const Flat& f = fl.flat.back();
-            tables.push_back(Candidate{cl.brokers, cl.rackAssignment});
+            addTable(cl.brokers, cl.rackAssignment, fl.candOff, fl.ids, fl.racks);
             fl.desired.push_back(cl.desiredReplicationFactor);
             const int64_t row0 = fl.partOff.back(), rep0 = fl.repOff.back();
             fl.hash.insert(fl.hash.end(), f.hash.begin(), f.hash.end());
@@ -378,7 +382,6 @@ private:
             fl.topicOff.push_back((int32_t)fl.hash.size());
             fl.stride = std::max(fl.stride, f.stride);
         }
-        candidateTables(tables, fl.candOff, fl.ids, fl.racks);
         return fl;
     }
     ka_ctx* ctx_;
@@ -471,20 +474,12 @@ inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicIn
     st = ka_status{};
     for (const auto& t : topics)
         if (needsJsonEscape(t.name)) {   // the host emitter over the rows of solveTopics
-            const size_t Q = f.partId.size();
-            std::vector<int32_t> outLen(Q, 0), out(Q * (size_t)f.stride, -1);
-            ka_solve(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
-                     f.stride, outLen.data(), out.data(), &st);
-            return st.code == KA_OK ? newAssignmentJson(unflatten(f, out.data(), outLen.data())) : std::string();
+            const std::vector<TopicOutput> rows = solveFlat(f, desiredReplicationFactor, st);
+            return st.code == KA_OK ? newAssignmentJson(rows) : std::string();
         }
     std::string names;
-    std::vector<int64_t> nameOff(T + 1, 0);
-    int64_t cap = 64;  // the sufficient size documented in kassign.h
-    for (int t = 0; t < T; ++t) {
-        names += f.names[t];
-        nameOff[t + 1] = (int64_t)names.size();
-        cap += (f.partOff[t + 1] - f.partOff[t]) * (50 + 12 * (int64_t)f.stride + (int64_t)f.names[t].size());
-    }
+    std::vector<int64_t> nameOff(1, 0);
+    const int64_t cap = appendNames(f, names, nameOff);
     std::unique_ptr<char[]> json(new char[cap]);
     int64_t bytes = 0;
     ka_solve_json(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
