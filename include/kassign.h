@@ -281,6 +281,31 @@ int32_t ka_score_candidates(ka_ctx* ctx, int32_t K, const int32_t* cand_off, con
                             int64_t* broker_replicas, int64_t* broker_leaders, int64_t* broker_in,
                             int32_t* out_len, int32_t* out_broker, ka_status* st);
 
+/* ka_solve_clusters, scored on the device: per cluster of a fleet, how much data its new assignment moves, which broker
+ * receives the most and how evenly it leaves replicas and leaders, before any of the K documents goes to the cluster.
+ *   K .. out_stride     exactly as ka_solve_clusters takes them
+ *   part_weight[ΣP]     host, >= 0 per row of the shared layout (e.g. the partition's size in bytes), or NULL = 1 per row
+ *   summary[K]          host, required; summary[k] is a function of cluster k's rows and current lists only
+ *   broker_replicas, broker_leaders, broker_in   host [cand_off[K]] each, or NULL: entry cand_off[k] + i belongs to broker
+ *                       broker_id[cand_off[k] + i] of cluster k (replicas held, rows led and replicas added, each weighted)
+ *   out_len, out_broker as ka_solve_clusters takes them, or out_broker == NULL: the rows stay on the device
+ *   st[K]               host, required
+ * st[k], the return code and (when out_broker is given) the rows are exactly what ka_solve_clusters gives for the same inputs.
+ * A cluster that failed (refused by the checks of its slice or its own plan, or one of the five reference exceptions) gets a
+ * zero summary with max_broker_in_id = -1 and zero per-broker entries, and so does a cluster that solved without rows. A
+ * call refused as a whole writes zero summaries, and zero per-broker entries once the tables pass ka_ctx_set_brokers' checks.
+ * Checked after every check of ka_solve_clusters and before anything is enqueued, over all ΣP rows, when some cluster is
+ * left to solve: a negative weight gives KA_ERR_BAD_ARG, 3 x (sum of weights) > INT64_MAX gives KA_ERR_LIMIT, in every st[k].
+ * Adds two kernel launches to those of ka_solve_clusters, whatever K is. Synchronous. Does not read or change ctx's own
+ * Context, broker table, parked counters, topic_base or staged block. */
+int32_t ka_score_clusters(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const int32_t* broker_id,
+                          const int32_t* broker_rack, const int32_t* topic_off, const int32_t* desired_rf,
+                          const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
+                          const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
+                          const int64_t* part_weight, ka_move_summary* summary,
+                          int64_t* broker_replicas, int64_t* broker_leaders, int64_t* broker_in,
+                          int32_t* out_len, int32_t* out_broker, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

@@ -409,6 +409,41 @@ class Solver:
         rows = fleet.part_off[topic_off]
         return [(out[rows[k]:rows[k + 1]], out_len[rows[k]:rows[k + 1]], sts[k]) for k in range(K)]
 
+    def score_clusters(self, clusters, out_stride=None, weights=None, rows=False, per_broker=False):
+        """ka_score_clusters: the fleet of solve_clusters scored on the device, one ka_move_summary per cluster. weights: None
+        (1 per row) or one int64 array [P_k] per cluster, in the cluster's row order. Returns one tuple per cluster: (summary
+        record, KaStatus); then, with rows=True, (out [P_k, out_stride], out_len [P_k]) as solve_clusters returns them; then,
+        with per_broker=True, (replicas, leaders, added), int64 arrays aligned with the cluster's broker ids. A failed cluster
+        has a zero summary (max_broker_in_id = -1) and zero per-broker sums; its rows are unspecified."""
+        K = len(clusters)
+        cand_off, broker_id, broker_rack, topic_off, drf, *fleet = self.marshal_clusters(clusters)
+        fleet = _ragged(*fleet)
+        if out_stride is None:
+            out_stride = fleet.stride(int(drf.max()) if K else -1)
+        weight = None
+        if weights is not None:
+            assert len(weights) == K
+            weight = np.concatenate([np.zeros(0, dtype=np.int64)] + [np.asarray(w, dtype=np.int64) for w in weights])
+            assert len(weight) == fleet.Q
+        summary = np.zeros(K, dtype=MOVE_SUMMARY_DTYPE)
+        out = np.full((fleet.Q, out_stride), -1, dtype=np.int32) if rows else None
+        out_len = np.zeros(fleet.Q, dtype=np.int32) if rows else None
+        brk = [np.zeros(int(cand_off[-1]), dtype=np.int64) for _ in range(3)] if per_broker else [None] * 3
+        st, sts = _statuses(K)
+        self._L.ka_score_clusters(self._h, K, _ptr(cand_off), _ptr(broker_id), _ptr(broker_rack), _ptr(topic_off), _ptr(drf),
+                                  *fleet.ptrs(), int(out_stride), _ptr(weight), _ptr(summary), *[_ptr(a) for a in brk], _ptr(out_len),
+                                  _ptr(out), st)
+        row0 = fleet.part_off[topic_off]
+        res = []
+        for k in range(K):
+            r = (summary[k], sts[k])
+            if rows:
+                r += (out[row0[k]:row0[k + 1]], out_len[row0[k]:row0[k + 1]])
+            if per_broker:
+                r += tuple(a[cand_off[k]:cand_off[k + 1]] for a in brk)
+            res.append(r)
+        return res
+
     def solve_clusters_json(self, clusters, topic_names, json_buf=None):
         """ka_solve_clusters_json: the fleet of solve_clusters, every cluster's reassignment JSON built on the device.
         topic_names: one list of names per cluster. json_buf: optional writable uint8 numpy array (pinned for full PCIe speed);

@@ -26,15 +26,16 @@ HOST_CANDIDATES_TEST = os.path.join(_HERE, "bin", "test_candidates")
 HOST_SCORES_TEST = os.path.join(_HERE, "bin", "test_candidate_scores")
 HOST_CLUSTERS_TEST = os.path.join(_HERE, "bin", "test_clusters")
 HOST_CLUSTERS_JSON_TEST = os.path.join(_HERE, "bin", "test_clusters_json")
+HOST_CLUSTER_SCORES_TEST = os.path.join(_HERE, "bin", "test_cluster_scores")
 HOST_SOURCES = ["kafka_assignment_generator.cpp", "kassign_host.hpp", "test_kafka_topic_assigner.cpp", "test_candidates.cpp",
-                "test_candidate_scores.cpp", "test_clusters.cpp", "test_clusters_json.cpp"]
+                "test_candidate_scores.cpp", "test_clusters.cpp", "test_clusters_json.cpp", "test_cluster_scores.cpp"]
 
 
 def build_host(force=False):
     """g++ the C++ host mirror + file-based CLI (reference flag surface) against libkassign.so."""
     deps = [os.path.join(HOST_DIR, f) for f in HOST_SOURCES] + [LIB, os.path.join(_HERE, "..", "include", "kassign.h")]
     if not force and all(os.path.exists(x) for x in (CLI, HOST_TEST, HOST_CANDIDATES_TEST, HOST_SCORES_TEST, HOST_CLUSTERS_TEST,
-                                                                   HOST_CLUSTERS_JSON_TEST)) and all(os.path.getmtime(d) <= os.path.getmtime(CLI) for d in deps if os.path.exists(d)):
+                                                                   HOST_CLUSTERS_JSON_TEST, HOST_CLUSTER_SCORES_TEST)) and all(os.path.getmtime(d) <= os.path.getmtime(CLI) for d in deps if os.path.exists(d)):
         return CLI
     os.makedirs(os.path.dirname(CLI), exist_ok=True)
     cmd = ["g++", "-O2", "-std=c++17", "-Wall", os.path.join(HOST_DIR, "kafka_assignment_generator.cpp"), "-L" + CSRC, "-lkassign",
@@ -42,7 +43,7 @@ def build_host(force=False):
     subprocess.check_call(cmd)
     for src, exe in (("test_kafka_topic_assigner.cpp", HOST_TEST), ("test_candidates.cpp", HOST_CANDIDATES_TEST),
                      ("test_candidate_scores.cpp", HOST_SCORES_TEST), ("test_clusters.cpp", HOST_CLUSTERS_TEST),
-                     ("test_clusters_json.cpp", HOST_CLUSTERS_JSON_TEST)):
+                     ("test_clusters_json.cpp", HOST_CLUSTERS_JSON_TEST), ("test_cluster_scores.cpp", HOST_CLUSTER_SCORES_TEST)):
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wall", os.path.join(HOST_DIR, src), "-L" + CSRC, "-lkassign",
                                "-Wl,-rpath,$ORIGIN/../csrc", "-o", exe])
     return CLI

@@ -136,11 +136,12 @@ struct ka_ctx {
     DevBuf d_hash, d_part_off, d_rep_off, d_cur, d_out, d_out_len;
     RunScratch run;   // kernel A and the chains of a single solve (and of a staged block)
     DevBuf d_json, d_names, d_name_off, d_part_id, d_json_rowlen, d_json_blocksum, d_json_state;
-    DevBuf d_json_seg;   // the document table of ka_solve_clusters_json (the arrays of KaJsonSegs)
+    DevBuf d_json_seg;   // the cluster table of ka_solve_clusters_json and ka_score_clusters (the arrays of KaJsonSegs)
     // scratch of the batched solves, apart from the single solve's: descriptors + broker tables, counters, and the run
     DevBuf d_batch_tab, d_batch_ctr;
     RunScratch batch_run;
-    // scratch of ka_score_candidates: row weights, the K summaries, the per-broker sums [3][ΣN], the tables' offsets [K+1]
+    // scratch of ka_score_candidates / ka_score_clusters: row weights, the K summaries, the per-broker sums [3][ΣN], the tables'
+    // offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
@@ -2100,13 +2101,26 @@ static int enq_fleet_segs(ka_ctx* c, cudaStream_t s, const Fleet& f, int K) {
     return KA_OK;
 }
 
+// The kernels' view of the K clusters' table that enq_fleet_segs uploaded, with the batch's failure words.
+static KaJsonSegs fleet_segs(ka_ctx* c, int K) {
+    size_t shift_at;
+    fleet_segs_bytes(K, &shift_at);
+    unsigned char* seg = c->d_json_seg.as<unsigned char>();
+    KaJsonSegs sg{};
+    sg.K = K;
+    sg.doc_off = reinterpret_cast<unsigned long long*>(seg);
+    sg.bytes = sg.doc_off + K + 1;
+    sg.row0 = reinterpret_cast<const int64_t*>(sg.bytes + K);
+    sg.shift = reinterpret_cast<uint32_t*>(seg + shift_at);
+    sg.member = reinterpret_cast<const int32_t*>(sg.shift + K);
+    sg.flags = c->batch_run.flags.as<unsigned>();
+    return sg;
+}
+
 // The segmented JSON pass of a fleet solved as d (its rows in io.d_out, its document table uploaded), on `s` after the last
 // emit: the length pass and the scan over fragments of the call's rows, the document table, then the write pass. doc_off
 // comes back to h_doc.
 static int enq_fleet_json(ka_ctx* c, cudaStream_t s, const StageDesc& d, const SolveCall& io, int K, unsigned long long* h_doc) {
-    size_t shift_at;
-    fleet_segs_bytes(K, &shift_at);
-    unsigned char* seg = c->d_json_seg.as<unsigned char>();
     KaJsonParams p{};
     p.part_off = d.d_part_off;
     p.T = d.T;
@@ -2117,14 +2131,7 @@ static int enq_fleet_json(ka_ctx* c, cudaStream_t s, const StageDesc& d, const S
     p.total = c->d_json_state.as<unsigned long long>();
     p.json = c->d_json.as<char>();
     p.cap = (unsigned long long)c->d_json.cap;
-    KaJsonSegs sg{};
-    sg.K = K;
-    sg.doc_off = reinterpret_cast<unsigned long long*>(seg);
-    sg.bytes = sg.doc_off + K + 1;
-    sg.row0 = reinterpret_cast<const int64_t*>(sg.bytes + K);
-    sg.shift = reinterpret_cast<uint32_t*>(seg + shift_at);
-    sg.member = reinterpret_cast<const int32_t*>(sg.shift + K);
-    sg.flags = c->batch_run.flags.as<unsigned>();
+    const KaJsonSegs sg = fleet_segs(c, K);
     // fragments of whole 256-row blocks, as in a ragged single solve; their count depends on the rows alone
     const int64_t Q = d.Q, step = json_fragment_rows(Q);
     std::vector<KaJsonParams> frags;
@@ -2218,6 +2225,77 @@ int32_t ka_solve_clusters_json(ka_ctx* c, int32_t K, const int32_t* cand_off, co
     return KA_OK;
 }
 
+// What a scored call hands back when it has no result (it failed, or it has nothing to solve): every summary empty and,
+// once the K tables have passed check_tables (nb = their brokers), every per-broker sum 0. Returns code.
+static int score_empty(int K, ka_move_summary* summary, int64_t* const brk[3], size_t nb, int code) {
+    for (int k = 0; k < K; ++k) summary[k] = empty_summary();
+    for (int i = 0; i < 3; ++i)
+        if (brk[i] && nb > 0) std::memset(brk[i], 0, nb * 8);
+    return code;
+}
+
+// The weights of a scored call's Q rows, once every check of its solve has passed and before anything is enqueued: a
+// negative weight fails every member with KA_ERR_BAD_ARG, 3 x their sum beyond INT64_MAX with KA_ERR_LIMIT.
+static int check_weights(const int64_t* part_weight, int64_t Q, int K, ka_status* st) {
+    if (!part_weight) return KA_OK;
+    bool negative = false;
+    int64_t sum = 0;   // saturates above INT64_MAX / 3
+    for (int64_t g = 0; g < Q; ++g) {
+        const int64_t w = part_weight[g];
+        negative |= w < 0;
+        sum = w > INT64_MAX / 3 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
+    }
+    if (negative) return fail_members(st, K, KA_ERR_BAD_ARG);
+    if (sum > INT64_MAX / 3) return fail_members(st, K, KA_ERR_LIMIT);
+    return KA_OK;
+}
+
+// The tail of ka_score_candidates and ka_score_clusters, once run_batch has enqueued the batch bt on `s` (its rows, Q per
+// candidate or ΣP for a fleet, of stride S in io.d_out): the weights and cand_off up, the accumulators zeroed, the two score
+// kernels (with a fleet f, their FLEET instances over f's cluster table), the summaries and the per-broker sums asked for
+// (brk) back, then finish_batch.
+static int score_batch(ka_ctx* c, cudaStream_t s, const Batch& bt, const int32_t* cand_off, int64_t Q, int S, const SolveCall& io,
+                       const int64_t* part_weight, const Fleet* f, ka_move_summary* summary, int64_t* const brk[3], ka_status* st,
+                       const int32_t* part_id, const int64_t* part_off) {
+    const int K = bt.K;
+    const size_t nb = (size_t)cand_off[K];
+    auto abort = [&](int code) { return score_empty(K, summary, brk, nb, abort_batch(c, s, st, K, code)); };
+    const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
+    if (c->d_score_sum.reserve(sum_bytes) != cudaSuccess || c->d_score_brk.reserve(std::max<size_t>(3 * nb, 1) * 8) != cudaSuccess ||
+        c->d_score_off.reserve((size_t)(K + 1) * 4) != cudaSuccess ||
+        (part_weight && c->d_score_w.reserve((size_t)std::max<int64_t>(Q, 1) * 8) != cudaSuccess))
+        return abort(KA_ERR_CUDA);
+    ka_move_summary* d_sum = c->d_score_sum.as<ka_move_summary>();
+    long long* d_brk = c->d_score_brk.as<long long>();
+    const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
+    if ((part_weight && Q > 0 && cudaMemcpyAsync(c->d_score_w.p, part_weight, (size_t)Q * 8, cudaMemcpyHostToDevice, s) != cudaSuccess) ||
+        cudaMemcpyAsync(c->d_score_off.p, cand_off, (size_t)(K + 1) * 4, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemsetAsync(d_sum, 0, sum_bytes, s) != cudaSuccess || cudaMemsetAsync(d_brk, 0, std::max<size_t>(3 * nb, 1) * 8, s) != cudaSuccess ||
+        (f && enq_fleet_segs(c, s, *f, K) != KA_OK))
+        return abort(KA_ERR_CUDA);
+    const KaCandidate* cand = c->d_batch_tab.as<KaCandidate>();
+    const int32_t* d_off = c->d_score_off.as<int32_t>();
+    const unsigned row_blocks = (unsigned)std::max<int64_t>((Q + 255) / 256, 1);
+    if (f) {   // a fleet's rows are disjoint: one thread per input row, its cluster found in the table
+        const KaJsonSegs sg = fleet_segs(c, K);
+        ka_score_rows_kernel<true><<<row_blocks, 256, 0, s>>>(cand, d_off, (uint32_t)Q, S, io.d_out, io.d_out_len, c->d_rep_off.as<int64_t>(),
+                                                              c->d_cur.as<int32_t>(), d_w, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb, sg);
+        ka_score_finish_kernel<true><<<K, 256, 0, s>>>(cand, d_off, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb, sg);
+    } else {
+        ka_score_rows_kernel<false><<<dim3(row_blocks, K), 256, 0, s>>>(cand, d_off, (uint32_t)Q, S, io.d_out, io.d_out_len,
+                                                                        c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), d_w, d_sum,
+                                                                        d_brk, d_brk + nb, d_brk + 2 * nb, KaJsonSegs{});
+        ka_score_finish_kernel<false><<<K, 256, 0, s>>>(cand, d_off, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb, KaJsonSegs{});
+    }
+    c->launches += 2;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(summary, d_sum, sum_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess)
+        return abort(KA_ERR_CUDA);
+    for (int i = 0; i < 3; ++i)
+        if (brk[i] && nb > 0 && cudaMemcpyAsync(brk[i], d_brk + i * nb, nb * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess)
+            return abort(KA_ERR_CUDA);
+    return finish_batch(c, s, bt, st, part_id, part_off);
+}
+
 int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
                             int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
                             const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf, int32_t out_stride,
@@ -2233,61 +2311,46 @@ int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     if ((rc = check_tables(K, cand_off, broker_id, broker_rack)) != KA_OK) return fail_members(st, K, rc);
     int64_t* const brk[3] = {broker_replicas, broker_leaders, broker_in};
     const size_t nb = (size_t)cand_off[K];
-    // without a result every summary is empty and every per-broker sum 0
-    auto fail = [&](int code) {
-        for (int k = 0; k < K; ++k) summary[k] = empty_summary();
-        for (int64_t* a : brk)
-            if (a && nb > 0) std::memset(a, 0, nb * 8);
-        return code;
-    };
     Batch bt;
     Shape sh;
     StageDesc d;
     if ((rc = ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, part_off, rep_off, cur_broker, desired_rf, out_stride, true,
-                                bt, sh, st)) != KA_OK || bt.m.empty() || (rc = plan_batch(sh, bt, d, st)) != KA_OK)
-        return fail(rc);
-    const int64_t Q = sh.Q;
-    // the weights, once every check of ka_solve_candidates has passed and before anything is enqueued
-    if (part_weight) {
-        bool negative = false;
-        int64_t sum = 0;   // saturates above INT64_MAX / 3
-        for (int64_t g = 0; g < Q; ++g) {
-            const int64_t w = part_weight[g];
-            negative |= w < 0;
-            sum = w > INT64_MAX / 3 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
-        }
-        if (negative) return fail(fail_members(st, K, KA_ERR_BAD_ARG));
-        if (sum > INT64_MAX / 3) return fail(fail_members(st, K, KA_ERR_LIMIT));
-    }
-    cudaStream_t s = c->stream;
+                                bt, sh, st)) != KA_OK || bt.m.empty() || (rc = plan_batch(sh, bt, d, st)) != KA_OK ||
+        (rc = check_weights(part_weight, sh.Q, K, st)) != KA_OK)
+        return score_empty(K, summary, brk, nb, rc);
     const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
-    if ((rc = run_batch(c, s, bt, d, sh.R, io, st)) != KA_OK) return fail(rc);
-    auto abort = [&](int code) { return fail(abort_batch(c, s, st, K, code)); };
-    const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
-    if (c->d_score_sum.reserve(sum_bytes) != cudaSuccess || c->d_score_brk.reserve(std::max<size_t>(3 * nb, 1) * 8) != cudaSuccess ||
-        c->d_score_off.reserve((size_t)(K + 1) * 4) != cudaSuccess ||
-        (part_weight && c->d_score_w.reserve((size_t)std::max<int64_t>(Q, 1) * 8) != cudaSuccess))
-        return abort(KA_ERR_CUDA);
-    ka_move_summary* d_sum = c->d_score_sum.as<ka_move_summary>();
-    long long* d_brk = c->d_score_brk.as<long long>();
-    const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
-    if ((part_weight && Q > 0 && cudaMemcpyAsync(c->d_score_w.p, part_weight, (size_t)Q * 8, cudaMemcpyHostToDevice, s) != cudaSuccess) ||
-        cudaMemcpyAsync(c->d_score_off.p, cand_off, (size_t)(K + 1) * 4, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemsetAsync(d_sum, 0, sum_bytes, s) != cudaSuccess || cudaMemsetAsync(d_brk, 0, std::max<size_t>(3 * nb, 1) * 8, s) != cudaSuccess)
-        return abort(KA_ERR_CUDA);
-    const KaCandidate* cand = c->d_batch_tab.as<KaCandidate>();
-    const int32_t* d_off = c->d_score_off.as<int32_t>();
-    const dim3 grid((unsigned)std::max<int64_t>((Q + 255) / 256, 1), K);
-    ka_score_rows_kernel<<<grid, 256, 0, s>>>(cand, d_off, (uint32_t)Q, out_stride, io.d_out, io.d_out_len, c->d_rep_off.as<int64_t>(),
-                                              c->d_cur.as<int32_t>(), d_w, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb);
-    ka_score_finish_kernel<<<K, 256, 0, s>>>(cand, d_off, d_sum, d_brk, d_brk + nb, d_brk + 2 * nb);
-    c->launches += 2;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(summary, d_sum, sum_bytes, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-        return abort(KA_ERR_CUDA);
-    for (int i = 0; i < 3; ++i)
-        if (brk[i] && nb > 0 && cudaMemcpyAsync(brk[i], d_brk + i * nb, nb * 8, cudaMemcpyDeviceToHost, s) != cudaSuccess)
-            return abort(KA_ERR_CUDA);
-    return finish_batch(c, s, bt, st, part_id, part_off);
+    if ((rc = run_batch(c, c->stream, bt, d, sh.R, io, st)) != KA_OK) return score_empty(K, summary, brk, nb, rc);
+    return score_batch(c, c->stream, bt, cand_off, sh.Q, out_stride, io, part_weight, nullptr, summary, brk, st, part_id, part_off);
+}
+
+int32_t ka_score_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const int32_t* broker_id, const int32_t* broker_rack,
+                          const int32_t* topic_off, const int32_t* desired_rf, const int32_t* topic_hash, const int64_t* part_off,
+                          const int32_t* part_id, const int64_t* rep_off, const int32_t* cur_broker, int32_t out_stride,
+                          const int64_t* part_weight, ka_move_summary* summary, int64_t* broker_replicas, int64_t* broker_leaders,
+                          int64_t* broker_in, int32_t* out_len, int32_t* out_broker, ka_status* st) {
+    if (!st || K < 0) return KA_ERR_BAD_ARG;
+    if (!summary) return fail_members(st, K, KA_ERR_BAD_ARG);
+    for (int k = 0; k < K; ++k) summary[k] = empty_summary();
+    int rc = batch_args(c, K, out_stride, st);
+    if (rc != KA_OK) return rc;
+    if (K == 0) return KA_OK;
+    int64_t* const brk[3] = {broker_replicas, broker_leaders, broker_in};
+    Fleet f;
+    if ((rc = fleet_front(c, K, cand_off, broker_id, broker_rack, topic_off, desired_rf, topic_hash, part_off, rep_off, cur_broker,
+                          out_stride, true, nullptr, nullptr, f, st)) != KA_OK)
+        return check_tables(K, cand_off, broker_id, broker_rack) == KA_OK ? score_empty(K, summary, brk, (size_t)cand_off[K], rc) : rc;
+    const size_t nb = (size_t)cand_off[K];
+    Batch& bt = f.bt;
+    if (bt.m.empty()) return score_empty(K, summary, brk, nb, finish_batch(c, c->stream, bt, st));
+    Shape sh = ragged_shape(f.T, f.row0[K], f.rep0[K], -1, out_stride);
+    if (reserve_io(c, sh, true) != KA_OK) return score_empty(K, summary, brk, nb, fail_members(st, K, KA_ERR_CUDA));
+    // the inputs of every cluster go up at once; the weights are checked over all ΣP rows
+    StageDesc d;
+    if ((rc = plan_batch(sh, bt, d, st)) != KA_OK || (rc = check_weights(part_weight, sh.Q, K, st)) != KA_OK)
+        return score_empty(K, summary, brk, nb, rc);
+    const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
+    if ((rc = run_batch(c, c->stream, bt, d, sh.R, io, st)) != KA_OK) return score_empty(K, summary, brk, nb, rc);
+    return score_batch(c, c->stream, bt, cand_off, sh.Q, out_stride, io, part_weight, &f, summary, brk, st, part_id, part_off);
 }
 
 }  // extern "C"

@@ -13,6 +13,8 @@
 //   kassign::solveClusters                            <->  that loop once per cluster of a fleet, each with its own broker
 //                                                          set and a new assigner, in one device call
 //   kassign::solveClustersJson                        <->  the same fleet, with each cluster's org.json text built on the device
+//   kassign::scoreClusters                            <->  the same fleet, reduced on the device to what each cluster would move
+//                                                          and how evenly it spreads replicas and leaders
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -229,18 +231,35 @@ public:
                             f.repOff.data(), f.cur.data(), desiredReplicationFactor, f.stride, w.empty() ? nullptr : w.data(),
                             summary.data(), perBroker ? brk[0].data() : nullptr, perBroker ? brk[1].data() : nullptr,
                             perBroker ? brk[2].data() : nullptr, nullptr, nullptr, st.data());
-        std::vector<CandidateScore> res(K);
-        for (int k = 0; k < K; ++k) {
-            res[k].status = st[k];
-            res[k].summary = summary[k];
-            if (perBroker)
-                for (int i = candOff[k]; i < candOff[k + 1]; ++i) {
-                    res[k].brokerReplicas[ids[i]] = brk[0][i];
-                    res[k].brokerLeaders[ids[i]] = brk[1][i];
-                    res[k].brokerIn[ids[i]] = brk[2][i];
-                }
+        return memberScores(st, K, summary, perBroker ? brk : nullptr, candOff, ids);
+    }
+
+    // solveClusters scored on the device (ka_score_clusters): per cluster of the fleet the summary of what its new assignment
+    // changes against its topics' current one, instead of the assignment itself. weights: empty (1 per partition) or, per
+    // cluster, one map per topic with the weight of every partition, as scoreTopicsCandidates takes them.
+    std::vector<CandidateScore> scoreClusters(const std::vector<ClusterInput>& clusters,
+                                              const std::vector<std::vector<std::map<int, int64_t>>>& weights = {},
+                                              bool perBroker = false) {
+        const int K = (int)clusters.size();
+        const Fleet fl = flattenFleet(clusters);
+        std::vector<int64_t> w;
+        if (!weights.empty()) {
+            if (weights.size() != clusters.size()) throw std::invalid_argument("one list of weight maps per cluster");
+            for (int k = 0; k < K; ++k) {
+                if (weights[k].size() != clusters[k].topics.size()) throw std::invalid_argument("one weight map per topic");
+                for (size_t t = 0; t < clusters[k].topics.size(); ++t)
+                    for (const auto& e : clusters[k].topics[t].current) w.push_back(weights[k][t].at(e.first));
+            }
         }
-        return res;
+        std::vector<ka_move_summary> summary(std::max(K, 1));
+        std::vector<int64_t> brk[3];
+        for (auto& a : brk) a.assign(perBroker ? fl.ids.size() : 0, 0);
+        std::vector<ka_status> st(std::max(K, 1));
+        ka_score_clusters(ctx_, K, fl.candOff.data(), fl.ids.data(), fl.racks.data(), fl.topicOff.data(), fl.desired.data(), fl.hash.data(),
+                          fl.partOff.data(), fl.partId.data(), fl.repOff.data(), fl.cur.data(), fl.stride, w.empty() ? nullptr : w.data(),
+                          summary.data(), perBroker ? brk[0].data() : nullptr, perBroker ? brk[1].data() : nullptr,
+                          perBroker ? brk[2].data() : nullptr, nullptr, nullptr, st.data());
+        return memberScores(st, K, summary, perBroker ? brk : nullptr, fl.candOff, fl.ids);
     }
 
     // The KAG:172-186 loop and its "NEW ASSIGNMENT" text in one device call (ka_solve_json): only the text crosses PCIe.
@@ -314,6 +333,24 @@ private:
             if (st[k].code != KA_OK) continue;
             const std::pair<const Flat*, int64_t> m = member(k);
             res[k].topics = unflatten(*m.first, stride, out.data() + m.second * stride, outLen.data() + m.second);
+        }
+        return res;
+    }
+    // What each member of a scored call gave: its status, its summary and, when brk (the call's three per-broker arrays) is
+    // given, its per-broker sums keyed by the ids of its table (ids[candOff[k] .. candOff[k + 1])).
+    static std::vector<CandidateScore> memberScores(const std::vector<ka_status>& st, int K, const std::vector<ka_move_summary>& summary,
+                                                    const std::vector<int64_t>* brk, const std::vector<int32_t>& candOff,
+                                                    const std::vector<int32_t>& ids) {
+        std::vector<CandidateScore> res(K);
+        for (int k = 0; k < K; ++k) {
+            res[k].status = st[k];
+            res[k].summary = summary[k];
+            if (brk)
+                for (int i = candOff[k]; i < candOff[k + 1]; ++i) {
+                    res[k].brokerReplicas[ids[i]] = brk[0][i];
+                    res[k].brokerLeaders[ids[i]] = brk[1][i];
+                    res[k].brokerIn[ids[i]] = brk[2][i];
+                }
         }
         return res;
     }
