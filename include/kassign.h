@@ -306,6 +306,49 @@ int32_t ka_score_clusters(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const
                           int64_t* broker_replicas, int64_t* broker_leaders, int64_t* broker_in,
                           int32_t* out_len, int32_t* out_broker, ka_status* st);
 
+/* One wave of a reassignment cut into waves by ka_plan_waves. Every field is int64, so the layout has no padding. */
+typedef struct ka_wave_summary {
+    int64_t rows;               /* rows placed in the wave */
+    int64_t rows_moved;         /* of them, rows with at least one receiver */
+    int64_t replicas_added;     /* sum of w[g] x receivers */
+    int64_t max_broker_in;      /* largest per-broker incoming sum in the wave ... */
+    int64_t max_broker_in_id;   /* ... its broker id (lowest id on ties, -1 when nothing is added) */
+} ka_wave_summary;
+
+/* A reassignment cut into waves, consecutive documents in which no broker receives more than a budget: what an operator runs
+ * one after the other instead of starting every new replica of a cluster at once.
+ *   Q                  rows; row g's current list is cur_broker[rep_off[g] .. rep_off[g + 1]) (rep_off[Q+1], host)
+ *   new_len[Q], new_broker[Q * stride]   host; the proposed lists, laid out as ka_solve's out_len / out_broker (its rows go in
+ *                      unchanged); 1 <= stride <= 8
+ *   part_weight[Q]     host, >= 0 per row (e.g. the partition's size in bytes), or NULL = 1 per row
+ *   max_broker_in      the budget B >= 1
+ *   wave[Q]            host, or NULL; the wave of every row (0 for a row that did not change)
+ *   n_waves            host, required; *n_waves = W, the number of waves
+ *   summary[summary_cap]   host; the first min(W, summary_cap) waves' summaries (NULL is allowed when summary_cap == 0)
+ * The rule, over the broker table of ka_ctx_set_brokers. A row is CHANGED when its new list differs from the current one in
+ * length or in any position (ka_move_summary's rows_changed); its RECEIVERS are the positions of the new list whose broker the
+ * current list does not hold (ka_move_summary's replicas_added counts them). Each broker b of the table starts with
+ * open[b] = 1, load[b] = 0, and the rows are taken in input order (permute the input to move some rows first):
+ *   an unchanged row gets wave 0 and a changed row without receivers wave 1; otherwise, with w = w[g],
+ *   wave[g] = max over its receivers b of (open[b] if load[b] == 0 or load[b] + w <= B, else open[b] + 1), and then every
+ *   receiver b with wave[g] > open[b] gets open[b] = wave[g], load[b] = w, every other receiver load[b] += w.
+ * So the waves are 1..W, none empty (W = 0 when no row changed); in every wave every broker receives at most B, unless a single
+ * row heavier than B is its only incoming row of nonzero weight there; with B >= the sum of the weights everything is in wave 1. A broker's waves
+ * only move forward (two words of state per broker): this is a greedy rule, not an optimal packing — a later row never goes
+ * back to fill an earlier wave.
+ * Checks, in this order, before anything is enqueued: st NULL: KA_ERR_BAD_ARG (nothing written); ctx NULL: KA_ERR_NO_DEVICE;
+ * Q < 0, stride < 1, n_waves NULL, summary_cap < 0, summary NULL with summary_cap > 0, max_broker_in < 1, or rep_off not
+ * non-decreasing from 0 (or a needed array NULL): KA_ERR_BAD_ARG; stride > 8 or Q >= 2^31: KA_ERR_LIMIT; a new_len outside
+ * [0, stride]: KA_ERR_BAD_ARG with a = the lowest such row; a negative weight: KA_ERR_BAD_ARG; 8 x (sum of weights) > INT64_MAX:
+ * KA_ERR_LIMIT. On the device, the lowest failing row wins: a new list naming a broker twice, or a receiver the table lacks,
+ * gives KA_ERR_BAD_ARG with a = the row and b = the broker id at the first such position of its list. On any error *n_waves = 0
+ * and wave / summary are unspecified. Q == 0: KA_OK, W = 0. Duplicate or unknown ids in a current list need no special case.
+ * Synchronous; adds a fixed number of kernel launches, whatever Q and W are. Does not read or change the Context counters,
+ * parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
+int32_t ka_plan_waves(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                      const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
+                      int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

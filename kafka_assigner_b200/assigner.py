@@ -15,10 +15,12 @@ import ctypes
 import numpy as np
 
 from . import _native
-from ._native import KaMoveSummary, KaStatus
+from ._native import KaMoveSummary, KaStatus, KaWaveSummary
 
 # numpy view of ka_move_summary (KaMoveSummary): one record per candidate
 MOVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaMoveSummary._fields_])
+# numpy view of ka_wave_summary (KaWaveSummary): one record per wave of Solver.plan_waves
+WAVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaWaveSummary._fields_])
 
 
 class IllegalStateException(Exception):
@@ -467,6 +469,39 @@ class Solver:
                                        *fleet.ptrs(), _ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(json_off),
                                        st)
         return [(json_buf[json_off[k]:json_off[k + 1]], sts[k]) for k in range(K)]
+
+    # The most summaries plan_waves asks for in its first call (40 bytes each): min(Q, this) covers W (never above Q) in one call
+    # on any cluster of up to 64 k rows and, on larger ones, every plan of up to 64 k waves.
+    WAVE_SUMMARY_CAP = 1 << 16
+
+    def plan_waves(self, rep_off, cur_broker, out, out_len, max_broker_in, weight=None):
+        """ka_plan_waves: the proposed lists out [Q, stride] / out_len [Q] (e.g. solve_ragged's rows) against the current lists
+        cur_broker[rep_off[g] .. rep_off[g + 1]), cut into waves in which no broker of this Solver's table receives more than
+        max_broker_in (weight: [Q] int64 per row, None = 1 per row). Returns (wave [Q] int32, 0 for an unchanged row; summary, a
+        numpy structured array [W] with the fields of ka_wave_summary; KaStatus). On an error wave and summary are empty. A plan
+        of more than min(Q, WAVE_SUMMARY_CAP) waves takes a second call for the rest of the summaries."""
+        out = np.ascontiguousarray(out, dtype=np.int32)
+        Q = len(out)
+        stride = out.shape[1] if out.ndim == 2 else 1
+        out_len = np.ascontiguousarray(out_len, dtype=np.int32)
+        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
+        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
+        assert out_len.shape == (Q,) and rep_off.shape == (Q + 1,) and (weight is None or weight.shape == (Q,))
+        wave = np.zeros(Q, dtype=np.int32)
+        n_waves = ctypes.c_int32(0)
+        st = KaStatus()
+        cap = max(1, min(Q, self.WAVE_SUMMARY_CAP))
+        while True:
+            summary = np.zeros(cap, dtype=WAVE_SUMMARY_DTYPE)
+            self._L.ka_plan_waves(self._h, Q, _ptr(rep_off), _ptr(cur_broker), int(stride), _ptr(out_len), _ptr(out),
+                                  _ptr(weight), int(max_broker_in), _ptr(wave), ctypes.byref(n_waves), _ptr(summary), cap,
+                                  ctypes.byref(st))
+            if st.code != 0:
+                return np.zeros(0, dtype=np.int32), np.zeros(0, dtype=WAVE_SUMMARY_DTYPE), st
+            if n_waves.value <= cap:
+                return wave, summary[:n_waves.value], st
+            cap = n_waves.value
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

@@ -6,6 +6,7 @@
 #include "kassign_order.cuh"
 #include "kassign_json.cuh"
 #include "kassign_score.cuh"
+#include "kassign_waves.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -143,6 +144,10 @@ struct ka_ctx {
     // scratch of ka_score_candidates / ka_score_clusters: row weights, the K summaries, the per-broker sums [3][ΣN], the tables'
     // offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
+    // scratch of ka_plan_waves: its inputs, the rows pass's per-row outputs and records, the packed records, the per-CTA counts
+    // and offsets, the chain's per-broker words when they leave shared memory, the bucket log, the summaries and the meta words
+    DevBuf d_wv_rep_off, d_wv_cur, d_wv_len, d_wv_new, d_wv_w, d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state,
+        d_wv_log, d_wv_sum, d_wv_meta;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -1287,7 +1292,9 @@ void ka_ctx_destroy(ka_ctx* c) {
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
                       &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
-                      &c->d_score_brk, &c->d_score_off, &c->d_json_seg})
+                      &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_rep_off, &c->d_wv_cur, &c->d_wv_len,
+                      &c->d_wv_new, &c->d_wv_w, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec, &c->d_wv_cnt, &c->d_wv_state,
+                      &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -2351,6 +2358,128 @@ int32_t ka_score_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
     const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
     if ((rc = run_batch(c, c->stream, bt, d, sh.R, io, st)) != KA_OK) return score_empty(K, summary, brk, nb, rc);
     return score_batch(c, c->stream, bt, cand_off, sh.Q, out_stride, io, part_weight, &f, summary, brk, st, part_id, part_off);
+}
+
+// The broker id at the first position of row g's new list that the device refused: a broker named twice, or a receiver (a
+// broker the current list lacks) that the table `ids` lacks.
+static int32_t wave_refused_id(const std::vector<int32_t>& ids, const int64_t* rep_off, const int32_t* cur, int32_t stride,
+                               const int32_t* new_len, const int32_t* new_broker, int64_t g) {
+    const int32_t* nb = new_broker + g * stride;
+    const int32_t* cb = cur + rep_off[g];
+    const int64_t m = rep_off[g + 1] - rep_off[g];
+    for (int j = 0; j < new_len[g]; ++j) {
+        if (std::find(nb, nb + j, nb[j]) != nb + j) return nb[j];
+        if (std::find(cb, cb + m, nb[j]) == cb + m && !std::binary_search(ids.begin(), ids.end(), nb[j])) return nb[j];
+    }
+    return 0;
+}
+
+int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                      const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, int32_t* wave, int32_t* n_waves,
+                      ka_wave_summary* summary, int32_t summary_cap, ka_status* st) {
+    if (!st) return KA_ERR_BAD_ARG;
+    if (n_waves) *n_waves = 0;
+    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
+    if (Q < 0 || stride < 1 || !n_waves || summary_cap < 0 || (!summary && summary_cap > 0) || max_broker_in < 1 ||
+        (Q > 0 && (!rep_off || !new_len || !new_broker)) || (rep_off && rep_off[0] != 0))
+        return set_status(st, KA_ERR_BAD_ARG);
+    for (int64_t g = 0; g < Q; ++g)
+        if (rep_off[g + 1] < rep_off[g]) return set_status(st, KA_ERR_BAD_ARG);
+    const int64_t R = Q > 0 ? rep_off[Q] : 0;
+    if (R > 0 && !cur_broker) return set_status(st, KA_ERR_BAD_ARG);
+    if (stride > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, stride);
+    if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX);
+    int64_t positions = 0;   // new-list positions: a bound on the chain's buckets
+    for (int64_t g = 0; g < Q; ++g) {
+        if (new_len[g] < 0 || new_len[g] > stride) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
+        positions += new_len[g];
+    }
+    if (part_weight) {
+        bool negative = false;
+        int64_t sum = 0;   // saturates above INT64_MAX / 8: a row adds at most 8 x its weight to a wave
+        for (int64_t g = 0; g < Q; ++g) {
+            const int64_t w = part_weight[g];
+            negative |= w < 0;
+            sum = w > INT64_MAX / 8 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
+        }
+        if (negative) return set_status(st, KA_ERR_BAD_ARG);
+        if (sum > INT64_MAX / 8) return set_status(st, KA_ERR_LIMIT);
+    }
+    if (Q == 0) return set_status(st, KA_OK);
+
+    cudaStream_t s = c->stream;
+    const int N = c->br.N;
+    const unsigned nblk = (unsigned)((Q + 255) / 256);
+    const bool gstate = (size_t)N * KA_WAVE_BROKER_BYTES > KA_SMEM_BUDGET;   // the chain's per-broker words in global memory
+    const size_t q = (size_t)Q;
+    if (c->d_wv_rep_off.reserve((q + 1) * 8) || c->d_wv_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
+        c->d_wv_len.reserve(q * 4) || c->d_wv_new.reserve(q * stride * 4) || (part_weight && c->d_wv_w.reserve(q * 8)) ||
+        c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
+        c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
+        c->d_wv_state.reserve(gstate ? (size_t)N * KA_WAVE_BROKER_BYTES : 16) ||
+        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveMeta)))
+        return set_status(st, KA_ERR_CUDA);
+    const KaWaveMeta meta0{0xFFFFFFFFu, 0, 0, 0};
+    const int64_t* d_w = part_weight ? c->d_wv_w.as<int64_t>() : nullptr;
+    int32_t* d_cnt = c->d_wv_cnt.as<int32_t>();
+    int32_t* d_off = d_cnt + nblk;
+    KaWaveMeta* d_meta = c->d_wv_meta.as<KaWaveMeta>();
+    if (cudaMemcpyAsync(c->d_wv_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
+        (R > 0 && cudaMemcpyAsync(c->d_wv_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
+        cudaMemcpyAsync(c->d_wv_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
+        cudaMemcpyAsync(c->d_wv_new.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
+        (part_weight && cudaMemcpyAsync(c->d_wv_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)) ||
+        cudaMemcpyAsync(d_meta, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s))
+        return set_status(st, KA_ERR_CUDA);
+    KaWaveRec* d_rec = c->d_wv_rec.as<KaWaveRec>();
+    int32_t* d_wave = c->d_wv_wave.as<int32_t>();
+    int8_t* d_nrecv = c->d_wv_nrecv.as<int8_t>();
+    KaWaveBucket* d_log = c->d_wv_log.as<KaWaveBucket>();
+    ka_wave_rows_kernel<<<nblk, 256, 0, s>>>(c->br, (uint32_t)Q, stride, c->d_wv_rep_off.as<int64_t>(), c->d_wv_cur.as<int32_t>(),
+                                             c->d_wv_len.as<int32_t>(), c->d_wv_new.as<int32_t>(), d_w, d_nrecv,
+                                             c->d_wv_tmp.as<KaWaveRec>(), d_wave, d_cnt, d_meta);
+    ka_level_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, (int)nblk, d_off);
+    ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_off, d_rec);
+    if (gstate) {
+        long long* load = c->d_wv_state.as<long long>();
+        int* open = reinterpret_cast<int*>(load + N);
+        ka_wave_chain_kernel<true><<<1, KA_WAVE_THREADS, 0, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, load, open,
+                                                                reinterpret_cast<unsigned*>(open + N), d_log, d_meta);
+    } else {
+        const size_t smem = (size_t)N * KA_WAVE_BROKER_BYTES;
+        if (allow_smem(ka_wave_chain_kernel<false>, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+        ka_wave_chain_kernel<false><<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, nullptr,
+                                                                     nullptr, nullptr, d_log, d_meta);
+    }
+    c->launches += 4;
+    KaWaveMeta meta;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, d_meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
+        cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    if (meta.err_row != 0xFFFFFFFFu)
+        return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row,
+                          wave_refused_id(c->broker_id, rep_off, cur_broker, stride, new_len, new_broker, meta.err_row));
+    const int W = std::max(meta.waves, meta.changed);
+    const size_t sum_bytes = (size_t)std::max(W, 1) * sizeof(ka_wave_summary);
+    const int out = std::min(W, summary_cap);
+    if (c->d_wv_sum.reserve(sum_bytes)) return set_status(st, KA_ERR_CUDA);
+    ka_wave_summary* d_sum = c->d_wv_sum.as<ka_wave_summary>();
+    const unsigned peak_blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>(((int64_t)meta.nlog + 255) / 256, (int64_t)c->sm_count * 8));
+    if (cudaMemsetAsync(d_sum, 0, sum_bytes, s)) return set_status(st, KA_ERR_CUDA);
+    ka_wave_sum_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, d_wave, d_w, d_sum);
+    ka_wave_peak_kernel<false><<<peak_blocks, 256, 0, s>>>(d_log, meta.nlog, N, d_sum);
+    ka_wave_peak_kernel<true><<<peak_blocks, 256, 0, s>>>(d_log, meta.nlog, N, d_sum);
+    c->launches += 3;
+    if (cudaGetLastError() != cudaSuccess ||
+        (out > 0 && cudaMemcpyAsync(summary, d_sum, (size_t)out * sizeof(ka_wave_summary), cudaMemcpyDeviceToHost, s)) ||
+        (wave && cudaMemcpyAsync(wave, d_wave, q * 4, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    for (int v = 0; v < out; ++v) {   // N - the lowest broker index of the wave's peak, 0 when nothing was added
+        const int64_t f = summary[v].max_broker_in_id;
+        summary[v].max_broker_in_id = f > 0 ? c->broker_id[N - f] : -1;
+    }
+    *n_waves = W;
+    return set_status(st, KA_OK);
 }
 
 }  // extern "C"

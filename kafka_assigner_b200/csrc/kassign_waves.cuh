@@ -1,0 +1,294 @@
+// kassign_waves.cuh — a reassignment cut into waves in which no broker receives more than a budget B (ka_plan_waves).
+//
+// The rule (include/kassign.h): rows in input order; broker b of the table has open[b] = 1, load[b] = 0. A row with receivers
+// (new-list brokers its current list lacks) of weight w takes wave = max over its receivers of (open[b] if load[b] == 0 or
+// load[b] + w <= B, else open[b] + 1); then every receiver b either opens that wave (open[b] = wave, load[b] = w) or, already in
+// it, adds w. A broker's waves only move forward, so its state is two words.
+//
+//   ka_wave_rows_kernel     one thread per row: checks, changed flag, receivers as table indices (kernel A's ka_lookup on the
+//                           table in HBM), a record per moved row, moved rows per CTA
+//   ka_level_scan_kernel    CTA offsets of the moved rows (kassign_order.cuh)
+//   ka_wave_compact_kernel  the records of the moved rows, in row order, packed
+//   ka_wave_chain_kernel    ONE CTA: the serial rule over the records, in rounds (below); logs every (broker, wave, load) bucket
+//   ka_wave_sum_kernel      per wave: rows, rows moved, replicas added
+//   ka_wave_peak_kernel     per wave: the largest bucket, then (ID) the lowest broker index among the largest
+//
+// The chain. Two records depend on each other only through a broker they share, so the chain takes KA_WAVE_CHUNK records at a
+// time and decides them in rounds. In a round every pending record claims each of its receivers with an atomicMax of a key
+// (round, then the earlier record wins); a record that holds all its claims is the earliest pending record on each of its
+// brokers, so every earlier record on them has decided and no other record of the round touches them: it decides and updates
+// open / load alone. The earliest pending record always holds its claims, so every round decides at least one record; a record
+// decides in round 1 + (the latest round among the earlier records of its chunk that share a broker with it).
+//
+// Everything is integer, and every sum and extreme commutative: the plan does not depend on the order of the atomics.
+#pragma once
+#include "kassign_common.cuh"
+#include "kassign_score.cuh"
+
+#define KA_WAVE_THREADS 512
+#define KA_WAVE_PER_THREAD 4
+#define KA_WAVE_CHUNK (KA_WAVE_THREADS * KA_WAVE_PER_THREAD)   // records decided together
+#define KA_WAVE_SLOT_BITS 11                                   // log2(KA_WAVE_CHUNK)
+#define KA_WAVE_MAX_ROUND (1u << (32 - KA_WAVE_SLOT_BITS))      // claim keys are (round << 11) | (CHUNK - 1 - slot)
+static_assert(KA_WAVE_CHUNK == 1 << KA_WAVE_SLOT_BITS, "a claim key holds a slot of the chunk");
+
+// A moved row: its input row, its receivers (table indices, 16 bits each, in list order) and its weight.
+struct KaWaveRec {
+    int32_t row, n;
+    long long w;
+    unsigned long long lo, hi;   // receivers 0..3 and 4..7
+};
+static_assert(sizeof(KaWaveRec) == 32, "two 16-byte loads per record");
+
+// A closed (or, at the end, still open) bucket of incoming load: wave, broker index, load > 0.
+struct KaWaveBucket {
+    int32_t wave, idx;
+    long long load;
+};
+
+struct KaWaveMeta {
+    unsigned err_row;   // lowest failing row (unsigned atomicMin, init 0xFFFFFFFF)
+    int changed;        // some row changed
+    int waves;          // W of the chain (the largest wave of a moved row)
+    unsigned nlog;      // buckets logged
+};
+
+__device__ __forceinline__ uint32_t ka_wave_rcv(const KaWaveRec& r, int j) {
+    return (uint32_t)((j < 4 ? r.lo >> (16 * j) : r.hi >> (16 * (j - 4))) & 0xFFFFu);
+}
+
+// grid ceil(Q / 256), 256 threads. Row g: new list new_broker[g * S .. + new_len[g]) (S <= 8), current list cur[rep_off[g] ..
+// rep_off[g + 1]). Writes nrecv[g] (-1 unchanged, else the receivers), wave[g] for the rows without receivers (0 unchanged, 1
+// changed), tmp[g] for a row with receivers, cnt[CTA] = its moved rows. A new list naming a broker twice, or a receiver the
+// table lacks, fails the row.
+__global__ void __launch_bounds__(256) ka_wave_rows_kernel(const KaBrokers br, uint32_t Q, int S, const int64_t* __restrict__ rep_off,
+                                                           const int32_t* __restrict__ cur, const int32_t* __restrict__ new_len,
+                                                           const int32_t* __restrict__ new_broker, const int64_t* __restrict__ weight,
+                                                           int8_t* __restrict__ nrecv, KaWaveRec* __restrict__ tmp,
+                                                           int32_t* __restrict__ wave, int32_t* __restrict__ cnt, KaWaveMeta* __restrict__ meta) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    bool diff = false;
+    int k = 0;
+    if (g < Q) {
+        const int n = new_len[g];
+        const int64_t a = rep_off[g];
+        const int m = (int)(rep_off[g + 1] - a);
+        int nb[KA_MAX_SLOTS];
+#pragma unroll
+        for (int j = 0; j < KA_MAX_SLOTS; ++j) nb[j] = j < n ? __ldg(new_broker + (int64_t)g * S + j) : 0;
+        diff = n != m;
+        bool bad = false;
+        unsigned long long lo = 0, hi = 0;
+        const uint16_t* lut = br.blob + br.lut_off;
+#pragma unroll
+        for (int j = 0; j < KA_MAX_SLOTS; ++j) {
+            if (j < n) {
+                bool held = false;
+                for (int i = 0; i < m; ++i) held |= __ldg(cur + a + i) == nb[j];
+                if (j < m) diff |= __ldg(cur + a + j) != nb[j];
+                bool dup = false;
+#pragma unroll
+                for (int i = 0; i < j; ++i) dup |= nb[i] == nb[j];
+                if (!held) {
+                    const unsigned long long x = ka_lookup(nb[j], lut, br);
+                    bad |= x == KA_DEAD;
+                    if (k < 4) lo |= x << (16 * k); else hi |= x << (16 * (k - 4));
+                    ++k;
+                }
+                bad |= dup;
+            }
+        }
+        if (bad) atomicMin(&meta->err_row, g);
+        if (!diff) wave[g] = 0;
+        else if (k == 0) wave[g] = 1;
+        else tmp[g] = KaWaveRec{(int32_t)g, k, weight ? __ldg(weight + g) : 1, lo, hi};
+        nrecv[g] = diff ? (int8_t)k : (int8_t)-1;
+    }
+    const int moved = __syncthreads_count(k > 0);
+    if (__syncthreads_or(diff) && threadIdx.x == 0) atomicOr(&meta->changed, 1);
+    if (threadIdx.x == 0) cnt[blockIdx.x] = moved;
+}
+
+// Same grid as the rows pass: the records of its moved rows to rec[off[CTA] + rank among the CTA's moved rows].
+__global__ void __launch_bounds__(256) ka_wave_compact_kernel(uint32_t Q, const int8_t* __restrict__ nrecv, const KaWaveRec* __restrict__ tmp,
+                                                              const int32_t* __restrict__ off, KaWaveRec* __restrict__ rec) {
+    __shared__ int wsum[8];
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool moved = g < Q && nrecv[g] > 0;
+    const unsigned b = __ballot_sync(KA_FULL, moved);
+    if (lane == 0) wsum[warp] = __popc(b);
+    __syncthreads();
+    if (!moved) return;
+    int pos = off[blockIdx.x] + __popc(b & ka_lanemask_lt());
+    for (int v = 0; v < warp; ++v) pos += wsum[v];
+    rec[pos] = tmp[g];
+}
+
+// The chain's per-broker words: shared memory while the table fits (GSTATE = false), else global memory read around L1 (the
+// claims are L2 atomics).
+template <bool GSTATE, typename T>
+__device__ __forceinline__ T ka_wave_ld(const T* p) {
+    if constexpr (GSTATE) return __ldcg(p);
+    else return *p;
+}
+template <bool GSTATE, typename T>
+__device__ __forceinline__ void ka_wave_st(T* p, T v) {
+    if constexpr (GSTATE) __stcg(p, v);
+    else *p = v;
+}
+
+// Bytes of shared memory the chain keeps per broker (load, open, claim).
+#define KA_WAVE_BROKER_BYTES 16
+
+// ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B. Writes wave[row] of every
+// record, the bucket log and meta->waves / nlog. With GSTATE the per-broker words are gload / gopen / gclaim [N]. Does nothing
+// when the rows pass failed a row.
+template <bool GSTATE>
+__global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off,
+                                                                           int nblk, int N, long long B, int32_t* __restrict__ wave,
+                                                                           long long* gload, int* gopen, unsigned* gclaim,
+                                                                           KaWaveBucket* __restrict__ log, KaWaveMeta* __restrict__ meta) {
+    extern __shared__ __align__(16) unsigned char ka_wave_smem[];
+    __shared__ unsigned nlog;
+    __shared__ int wmax;
+    if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;   // CTA-uniform
+    long long* load = gload;
+    int* open = gopen;
+    unsigned* claim = gclaim;
+    if constexpr (!GSTATE) {
+        load = reinterpret_cast<long long*>(ka_wave_smem);
+        open = reinterpret_cast<int*>(load + N);
+        claim = reinterpret_cast<unsigned*>(open + N);
+    }
+    const int tid = threadIdx.x;
+    for (int i = tid; i < N; i += KA_WAVE_THREADS) {
+        ka_wave_st<GSTATE>(load + i, 0LL);
+        ka_wave_st<GSTATE>(open + i, 1);
+        ka_wave_st<GSTATE>(claim + i, 0u);
+    }
+    if (tid == 0) { nlog = 0; wmax = 0; }
+    __syncthreads();
+    auto put = [&](int wv, uint32_t b, long long l) {
+        const unsigned s = atomicAdd(&nlog, 1u);
+        log[s] = KaWaveBucket{wv, (int32_t)b, l};
+    };
+    const int M = off[nblk];
+    unsigned round = 0;
+    int my_max = 0;
+    for (int base = 0; base < M; base += KA_WAVE_CHUNK) {
+        KaWaveRec r[KA_WAVE_PER_THREAD];
+        unsigned pend = 0;
+#pragma unroll
+        for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
+            const int i = base + e * KA_WAVE_THREADS + tid;
+            if (i < M) {
+                r[e] = rec[i];
+                pend |= 1u << e;
+            } else {
+                r[e] = KaWaveRec{0, 0, 0, 0, 0};
+            }
+        }
+        for (;;) {
+            if (++round == KA_WAVE_MAX_ROUND) {   // the key's round field is full: clear the claims and count again
+                for (int i = tid; i < N; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(claim + i, 0u);
+                __syncthreads();
+                round = 1;
+            }
+            unsigned key[KA_WAVE_PER_THREAD];
+#pragma unroll
+            for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
+                key[e] = round << KA_WAVE_SLOT_BITS | (unsigned)(KA_WAVE_CHUNK - 1 - (e * KA_WAVE_THREADS + tid));
+                if (pend >> e & 1u)
+                    for (int j = 0; j < r[e].n; ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
+            }
+            __syncthreads();
+#pragma unroll
+            for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
+                if (!(pend >> e & 1u)) continue;
+                bool own = true;
+                for (int j = 0; j < r[e].n; ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
+                if (!own) continue;
+                const long long w = r[e].w;
+                int wv = 0;
+                for (int j = 0; j < r[e].n; ++j) {
+                    const uint32_t b = ka_wave_rcv(r[e], j);
+                    const int o = ka_wave_ld<GSTATE>(open + b);
+                    const long long l = ka_wave_ld<GSTATE>(load + b);
+                    wv = max(wv, (l == 0 || l + w <= B) ? o : o + 1);
+                }
+                for (int j = 0; j < r[e].n; ++j) {
+                    const uint32_t b = ka_wave_rcv(r[e], j);
+                    const int o = ka_wave_ld<GSTATE>(open + b);
+                    const long long l = ka_wave_ld<GSTATE>(load + b);
+                    if (wv > o) {   // b closes its bucket and opens wave wv
+                        if (l > 0) put(o, b, l);
+                        ka_wave_st<GSTATE>(open + b, wv);
+                        ka_wave_st<GSTATE>(load + b, w);
+                    } else {
+                        ka_wave_st<GSTATE>(load + b, l + w);
+                    }
+                }
+                wave[r[e].row] = wv;
+                my_max = max(my_max, wv);
+                pend &= ~(1u << e);
+            }
+            if (!__syncthreads_or(pend != 0)) break;
+        }
+    }
+    // the buckets still open
+    for (int i = tid; i < N; i += KA_WAVE_THREADS) {
+        const long long l = ka_wave_ld<GSTATE>(load + i);
+        if (l > 0) put(ka_wave_ld<GSTATE>(open + i), (uint32_t)i, l);
+    }
+    atomicMax(&wmax, my_max);
+    __syncthreads();
+    if (tid == 0) {
+        meta->waves = wmax;
+        meta->nlog = nlog;
+    }
+}
+
+// grid ceil(Q / 256), 256 threads, summary[W] zeroed: every changed row adds to its wave's rows, rows_moved and replicas_added.
+// A warp sums each wave among its lanes (the 64-bit sums in three limbs of at most 22 bits, so the 32-bit lane sums cannot
+// carry), one atomic per wave and field.
+__global__ void __launch_bounds__(256) ka_wave_sum_kernel(uint32_t Q, const int8_t* __restrict__ nrecv, const int32_t* __restrict__ wave,
+                                                          const int64_t* __restrict__ weight, ka_wave_summary* __restrict__ summary) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    const int v = g < Q ? wave[g] : 0;
+    const int nr = g < Q ? nrecv[g] : -1;
+    const unsigned long long added = nr > 0 ? (unsigned long long)((weight ? __ldg(weight + g) : 1) * nr) : 0;
+    const unsigned grp = __match_any_sync(KA_FULL, v);
+    const unsigned rows = __reduce_add_sync(grp, (unsigned)(v > 0));
+    const unsigned moved = __reduce_add_sync(grp, (unsigned)(nr > 0));
+    const unsigned long long a0 = __reduce_add_sync(grp, (unsigned)(added & 0x3FFFFFu));
+    const unsigned long long a1 = __reduce_add_sync(grp, (unsigned)(added >> 22 & 0x1FFFFFu));
+    const unsigned long long a2 = __reduce_add_sync(grp, (unsigned)(added >> 43));
+    if (v > 0 && (int)(threadIdx.x & 31) == __ffs(grp) - 1) {
+        ka_wave_summary& s = summary[v - 1];
+        atomicAdd(reinterpret_cast<unsigned long long*>(&s.rows), (unsigned long long)rows);
+        if (moved) atomicAdd(reinterpret_cast<unsigned long long*>(&s.rows_moved), (unsigned long long)moved);
+        const unsigned long long sum = a0 + (a1 << 22) + (a2 << 43);
+        if (sum) atomicAdd(reinterpret_cast<unsigned long long*>(&s.replicas_added), sum);
+    }
+}
+
+// grid-stride over the n logged buckets, summary zeroed beforehand. ID = false: max_broker_in[wave] = the largest bucket of
+// the wave. ID = true (after): max_broker_in_id[wave] = N - the lowest broker index among the buckets equal to that maximum,
+// 0 when the wave has no bucket (the host turns it into the broker's id, or -1).
+template <bool ID>
+__global__ void __launch_bounds__(256) ka_wave_peak_kernel(const KaWaveBucket* __restrict__ log, unsigned n, int N,
+                                                           ka_wave_summary* summary) {
+    for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+        const KaWaveBucket b = log[i];
+        ka_wave_summary& s = summary[b.wave - 1];
+        if constexpr (!ID) {
+            if (b.load > *(volatile long long*)&s.max_broker_in)   // most buckets lose without an atomic
+                atomicMax(reinterpret_cast<unsigned long long*>(&s.max_broker_in), (unsigned long long)b.load);
+        } else {
+            const long long key = N - b.idx;
+            if (b.load == s.max_broker_in && key > *(volatile long long*)&s.max_broker_in_id)
+                atomicMax(reinterpret_cast<unsigned long long*>(&s.max_broker_in_id), (unsigned long long)key);
+        }
+    }
+}

@@ -15,6 +15,8 @@
 //   kassign::solveClustersJson                        <->  the same fleet, with each cluster's org.json text built on the device
 //   kassign::scoreClusters                            <->  the same fleet, reduced on the device to what each cluster would move
 //                                                          and how evenly it spreads replicas and leaders
+//   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
+//                                                          receives more than a budget, one document per wave
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -260,6 +262,70 @@ public:
                           summary.data(), perBroker ? brk[0].data() : nullptr, perBroker ? brk[1].data() : nullptr,
                           perBroker ? brk[2].data() : nullptr, nullptr, nullptr, st.data());
         return memberScores(st, K, summary, perBroker ? brk : nullptr, fl.candOff, fl.ids);
+    }
+
+    // A new assignment cut into waves (ka_plan_waves): consecutive documents in which no broker of this instance's table receives
+    // more than maxBrokerIn (weighted). waves[v] holds the changed partitions of wave v + 1, topics in input order, each
+    // printable with newAssignmentJson; unchanged partitions are in no wave.
+    struct WavePlan {
+        ka_status status;   // re-throw with throwForStatus; on an error summary and waves are empty
+        std::vector<ka_wave_summary> summary;
+        std::vector<std::vector<TopicOutput>> waves;
+    };
+
+    // `topics`' current assignment against `proposed` (the solveTopics output for them: the same topics and partitions, in the
+    // same order), against the broker table of this instance's last solveTopics. weights: empty (1 per partition) or, per topic,
+    // the weight of every partition, as scoreTopicsCandidates takes them.
+    WavePlan planWaves(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                       const std::vector<std::map<int, int64_t>>& weights = {}) {
+        if (proposed.size() != topics.size()) throw std::invalid_argument("one proposed topic per topic");
+        if (!weights.empty() && weights.size() != topics.size()) throw std::invalid_argument("one weight map per topic");
+        const Flat f = flatten(topics, -1);
+        const size_t Q = f.partId.size();
+        int stride = 1;
+        for (const TopicOutput& t : proposed)
+            for (const auto& e : t.assignment) stride = std::max(stride, (int)e.second.size());
+        std::vector<int32_t> newLen(Q, 0), newBroker(Q * stride, -1);
+        std::vector<int64_t> w;
+        size_t g = 0;
+        for (size_t t = 0; t < topics.size(); ++t)
+            for (const auto& e : topics[t].current) {
+                const std::vector<int>& l = proposed[t].assignment.at(e.first);
+                newLen[g] = (int32_t)l.size();
+                std::copy(l.begin(), l.end(), newBroker.begin() + g * stride);
+                if (!weights.empty()) w.push_back(weights[t].at(e.first));
+                ++g;
+            }
+        WavePlan res{};
+        std::vector<int32_t> wave(Q, 0);
+        int32_t W = 0;
+        // W never exceeds Q: min(Q, 64 k) summaries (40 bytes each) hold every plan in one call, but one of more than 64 k waves
+        res.summary.resize(std::max<size_t>(1, std::min<size_t>(Q, 1 << 16)));
+        auto plan = [&](int32_t* waveOut) {
+            return ka_plan_waves(ctx_, (int64_t)Q, f.repOff.data(), f.cur.data(), stride, newLen.data(), newBroker.data(),
+                                 w.empty() ? nullptr : w.data(), maxBrokerIn, waveOut, &W, res.summary.data(),
+                                 (int32_t)res.summary.size(), &res.status);
+        };
+        if (plan(wave.data()) == KA_OK && W > (int32_t)res.summary.size()) {
+            res.summary.resize(W);
+            plan(nullptr);
+        }
+        if (res.status.code != KA_OK) return WavePlan{res.status, {}, {}};
+        res.summary.resize(W);
+        res.waves.resize(W);
+        std::vector<size_t> lastTopic(W, topics.size());   // the topic of each wave's last TopicOutput
+        for (size_t t = 0; t < topics.size(); ++t)
+            for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
+                if (wave[r] == 0) continue;
+                std::vector<TopicOutput>& doc = res.waves[wave[r] - 1];
+                if (lastTopic[wave[r] - 1] != t) {
+                    doc.push_back(TopicOutput{f.names[t], {}});
+                    lastTopic[wave[r] - 1] = t;
+                }
+                doc.back().assignment[f.partId[r]] = std::vector<int>(newBroker.begin() + r * stride,
+                                                                      newBroker.begin() + r * stride + newLen[r]);
+            }
+        return res;
     }
 
     // The KAG:172-186 loop and its "NEW ASSIGNMENT" text in one device call (ka_solve_json): only the text crosses PCIe.
