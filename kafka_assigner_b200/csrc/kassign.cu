@@ -144,10 +144,10 @@ struct ka_ctx {
     // scratch of ka_score_candidates / ka_score_clusters: row weights, the K summaries, the per-broker sums [3][ΣN], the tables'
     // offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
-    // scratch of ka_plan_waves: its inputs, the rows pass's per-row outputs and records, the packed records, the per-CTA counts
-    // and offsets, the chain's per-broker words when they leave shared memory, the bucket log, the summaries and the meta words
-    DevBuf d_wv_rep_off, d_wv_cur, d_wv_len, d_wv_new, d_wv_w, d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state,
-        d_wv_log, d_wv_sum, d_wv_meta;
+    // scratch of ka_plan_waves (its inputs go to d_rep_off, d_cur, d_out_len, d_out and d_score_w): the rows pass's per-row
+    // outputs and records, the packed records, the per-CTA counts and offsets, the chain's per-broker words when they leave
+    // shared memory, the bucket log, the summaries and the meta words
+    DevBuf d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state, d_wv_log, d_wv_sum, d_wv_meta;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -1292,9 +1292,8 @@ void ka_ctx_destroy(ka_ctx* c) {
     for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
                       &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
-                      &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_rep_off, &c->d_wv_cur, &c->d_wv_len,
-                      &c->d_wv_new, &c->d_wv_w, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec, &c->d_wv_cnt, &c->d_wv_state,
-                      &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta})
+                      &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec,
+                      &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -2241,20 +2240,21 @@ static int score_empty(int K, ka_move_summary* summary, int64_t* const brk[3], s
     return code;
 }
 
-// The weights of a scored call's Q rows, once every check of its solve has passed and before anything is enqueued: a
-// negative weight fails every member with KA_ERR_BAD_ARG, 3 x their sum beyond INT64_MAX with KA_ERR_LIMIT.
-static int check_weights(const int64_t* part_weight, int64_t Q, int K, ka_status* st) {
+// The weights of Q rows (null: none), each row adding at most `factor` x its weight to a device sum: KA_ERR_BAD_ARG when a
+// weight is negative, else KA_ERR_LIMIT when factor x their sum is beyond INT64_MAX, else KA_OK. A scored call checks them
+// (factor 3) once every check of its solve has passed and before anything is enqueued, ka_plan_waves (factor 8) last of its
+// argument checks.
+static int weights_code(const int64_t* part_weight, int64_t Q, int64_t factor) {
     if (!part_weight) return KA_OK;
     bool negative = false;
-    int64_t sum = 0;   // saturates above INT64_MAX / 3
+    int64_t sum = 0;   // saturates above INT64_MAX / factor
     for (int64_t g = 0; g < Q; ++g) {
         const int64_t w = part_weight[g];
         negative |= w < 0;
-        sum = w > INT64_MAX / 3 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
+        sum = w > INT64_MAX / factor - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
     }
-    if (negative) return fail_members(st, K, KA_ERR_BAD_ARG);
-    if (sum > INT64_MAX / 3) return fail_members(st, K, KA_ERR_LIMIT);
-    return KA_OK;
+    if (negative) return KA_ERR_BAD_ARG;
+    return sum > INT64_MAX / factor ? KA_ERR_LIMIT : KA_OK;
 }
 
 // The tail of ka_score_candidates and ka_score_clusters, once run_batch has enqueued the batch bt on `s` (its rows, Q per
@@ -2322,9 +2322,9 @@ int32_t ka_score_candidates(ka_ctx* c, int32_t K, const int32_t* cand_off, const
     Shape sh;
     StageDesc d;
     if ((rc = ragged_candidates(c, K, cand_off, broker_id, broker_rack, T, part_off, rep_off, cur_broker, desired_rf, out_stride, true,
-                                bt, sh, st)) != KA_OK || bt.m.empty() || (rc = plan_batch(sh, bt, d, st)) != KA_OK ||
-        (rc = check_weights(part_weight, sh.Q, K, st)) != KA_OK)
+                                bt, sh, st)) != KA_OK || bt.m.empty() || (rc = plan_batch(sh, bt, d, st)) != KA_OK)
         return score_empty(K, summary, brk, nb, rc);
+    if ((rc = weights_code(part_weight, sh.Q, 3)) != KA_OK) return score_empty(K, summary, brk, nb, fail_members(st, K, rc));
     const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
     if ((rc = run_batch(c, c->stream, bt, d, sh.R, io, st)) != KA_OK) return score_empty(K, summary, brk, nb, rc);
     return score_batch(c, c->stream, bt, cand_off, sh.Q, out_stride, io, part_weight, nullptr, summary, brk, st, part_id, part_off);
@@ -2353,8 +2353,8 @@ int32_t ka_score_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
     if (reserve_io(c, sh, true) != KA_OK) return score_empty(K, summary, brk, nb, fail_members(st, K, KA_ERR_CUDA));
     // the inputs of every cluster go up at once; the weights are checked over all ΣP rows
     StageDesc d;
-    if ((rc = plan_batch(sh, bt, d, st)) != KA_OK || (rc = check_weights(part_weight, sh.Q, K, st)) != KA_OK)
-        return score_empty(K, summary, brk, nb, rc);
+    if ((rc = plan_batch(sh, bt, d, st)) != KA_OK) return score_empty(K, summary, brk, nb, rc);
+    if ((rc = weights_code(part_weight, sh.Q, 3)) != KA_OK) return score_empty(K, summary, brk, nb, fail_members(st, K, rc));
     const SolveCall io = host_call(c, topic_hash, part_off, rep_off, cur_broker, out_len, out_broker);
     if ((rc = run_batch(c, c->stream, bt, d, sh.R, io, st)) != KA_OK) return score_empty(K, summary, brk, nb, rc);
     return score_batch(c, c->stream, bt, cand_off, sh.Q, out_stride, io, part_weight, &f, summary, brk, st, part_id, part_off);
@@ -2394,49 +2394,43 @@ int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_
         if (new_len[g] < 0 || new_len[g] > stride) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
         positions += new_len[g];
     }
-    if (part_weight) {
-        bool negative = false;
-        int64_t sum = 0;   // saturates above INT64_MAX / 8: a row adds at most 8 x its weight to a wave
-        for (int64_t g = 0; g < Q; ++g) {
-            const int64_t w = part_weight[g];
-            negative |= w < 0;
-            sum = w > INT64_MAX / 8 - sum ? INT64_MAX : sum + std::max<int64_t>(w, 0);
-        }
-        if (negative) return set_status(st, KA_ERR_BAD_ARG);
-        if (sum > INT64_MAX / 8) return set_status(st, KA_ERR_LIMIT);
-    }
+    int rc = weights_code(part_weight, Q, 8);   // a row adds at most 8 x its weight to a wave
+    if (rc != KA_OK) return set_status(st, rc);
     if (Q == 0) return set_status(st, KA_OK);
+    // the call reads only the broker table: a pending asynchronous status stays pending for ka_last_status
+    if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
 
+    // the inputs go up into the buffers of the host-buffer solve and score calls: every such call is synchronous
     cudaStream_t s = c->stream;
     const int N = c->br.N;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
     const bool gstate = (size_t)N * KA_WAVE_BROKER_BYTES > KA_SMEM_BUDGET;   // the chain's per-broker words in global memory
     const size_t q = (size_t)Q;
-    if (c->d_wv_rep_off.reserve((q + 1) * 8) || c->d_wv_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
-        c->d_wv_len.reserve(q * 4) || c->d_wv_new.reserve(q * stride * 4) || (part_weight && c->d_wv_w.reserve(q * 8)) ||
+    if (c->d_rep_off.reserve((q + 1) * 8) || c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
+        c->d_out_len.reserve(q * 4) || c->d_out.reserve(q * stride * 4) || (part_weight && c->d_score_w.reserve(q * 8)) ||
         c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
         c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
         c->d_wv_state.reserve(gstate ? (size_t)N * KA_WAVE_BROKER_BYTES : 16) ||
         c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveMeta)))
         return set_status(st, KA_ERR_CUDA);
     const KaWaveMeta meta0{0xFFFFFFFFu, 0, 0, 0};
-    const int64_t* d_w = part_weight ? c->d_wv_w.as<int64_t>() : nullptr;
+    const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
     int32_t* d_cnt = c->d_wv_cnt.as<int32_t>();
     int32_t* d_off = d_cnt + nblk;
     KaWaveMeta* d_meta = c->d_wv_meta.as<KaWaveMeta>();
-    if (cudaMemcpyAsync(c->d_wv_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
-        (R > 0 && cudaMemcpyAsync(c->d_wv_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
-        cudaMemcpyAsync(c->d_wv_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
-        cudaMemcpyAsync(c->d_wv_new.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
-        (part_weight && cudaMemcpyAsync(c->d_wv_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)) ||
+    if (cudaMemcpyAsync(c->d_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
+        (R > 0 && cudaMemcpyAsync(c->d_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
+        cudaMemcpyAsync(c->d_out_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
+        cudaMemcpyAsync(c->d_out.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
+        (part_weight && cudaMemcpyAsync(c->d_score_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)) ||
         cudaMemcpyAsync(d_meta, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s))
         return set_status(st, KA_ERR_CUDA);
     KaWaveRec* d_rec = c->d_wv_rec.as<KaWaveRec>();
     int32_t* d_wave = c->d_wv_wave.as<int32_t>();
     int8_t* d_nrecv = c->d_wv_nrecv.as<int8_t>();
     KaWaveBucket* d_log = c->d_wv_log.as<KaWaveBucket>();
-    ka_wave_rows_kernel<<<nblk, 256, 0, s>>>(c->br, (uint32_t)Q, stride, c->d_wv_rep_off.as<int64_t>(), c->d_wv_cur.as<int32_t>(),
-                                             c->d_wv_len.as<int32_t>(), c->d_wv_new.as<int32_t>(), d_w, d_nrecv,
+    ka_wave_rows_kernel<<<nblk, 256, 0, s>>>(c->br, (uint32_t)Q, stride, c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(),
+                                             c->d_out_len.as<int32_t>(), c->d_out.as<int32_t>(), d_w, d_nrecv,
                                              c->d_wv_tmp.as<KaWaveRec>(), d_wave, d_cnt, d_meta);
     ka_level_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, (int)nblk, d_off);
     ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_off, d_rec);

@@ -145,6 +145,17 @@ __device__ __forceinline__ uint32_t ka_lanemask_lt() {
     return m;
 }
 
+// The sum of v over the lanes of `grp` (this lane among them), in every lane of the group. Needs v >= 0 in every lane and a
+// sum <= INT64_MAX. v goes in three limbs of at most 22 bits, so a 32-bit __reduce_add_sync over at most 32 lanes never
+// carries; any group of lanes, the whole warp included.
+__device__ __forceinline__ long long ka_group_sum64(long long v, unsigned grp) {
+    const unsigned long long u = (unsigned long long)v;
+    const unsigned long long a0 = __reduce_add_sync(grp, (unsigned)(u & 0x3FFFFFu));
+    const unsigned long long a1 = __reduce_add_sync(grp, (unsigned)(u >> 22 & 0x1FFFFFu));
+    const unsigned long long a2 = __reduce_add_sync(grp, (unsigned)(u >> 43));
+    return (long long)(a0 + (a1 << 22) + (a2 << 43));
+}
+
 // Rotation bits of one topic: (|hash| % k) for k = 2..8 packed above the 4-bit length (KAS:190 applied
 // to the remaining-set sizes of KAS:267). Layout: len[0:4) k2[4] k3[5:7) k4[7:9) k5[9:12) k6[12:15) k7[15:18) k8[18:21)
 __device__ __forceinline__ uint32_t ka_rot_bits(uint32_t habs) {

@@ -17,26 +17,8 @@
 // A candidate that failed (or has no broker) keeps the zero summary and per-broker entries the host cleared.
 __device__ __forceinline__ bool ka_score_ok(const KaCandidate& c) { return c.br.N > 0 && *c.out.err_topic == 0xFFFFFFFFu; }
 
-__device__ __forceinline__ long long ka_warp_sum64(long long v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(KA_FULL, v, o);
-    return v;
-}
-
-// The sum of v over the lanes of `grp`, a run of consecutive lanes that holds this lane, in the run's first lane (a segmented
-// suffix sum: lane i adds lane i + o while that lane is still in its run). Every lane of the warp calls it.
-__device__ __forceinline__ long long ka_seg_sum64(long long v, unsigned grp) {
-    const int lane = threadIdx.x & 31;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const long long y = __shfl_down_sync(KA_FULL, v, o);
-        if (lane + o < 32 && (grp >> (lane + o) & 1u)) v += y;
-    }
-    return v;
-}
-
 // Row g's flags and weighted added / dropped counts (row: where its emitted list sits in out / out_len), and its per-broker
-// sums into entry bro_off[k] + index of member c's table: the per-row code of the candidates' instance, for a fleet's rows.
+// sums into entry bro_off[k] + index of member c's table.
 __device__ __forceinline__ void ka_score_row(const KaCandidate& c, const int32_t* bro_off, int k, int64_t row, uint32_t g,
                                              int S, const int32_t* out, const int32_t* out_len,
                                              const int64_t* rep_off, const int32_t* cur,
@@ -89,7 +71,8 @@ __device__ __forceinline__ void ka_score_row(const KaCandidate& c, const int32_t
 // FLEET = true: grid (ceil(Q / 256)), Q = ΣP of a fleet. Row g belongs to cluster k with sg.row0[k] <= g < sg.row0[k + 1], and
 // sits at its input row; the cluster is live when it is batch member sg.member[k] and that member solved (ka_score_ok). Rows
 // of dead clusters add nothing.
-// Either way its current list is cur[rep_off[g] .. rep_off[g + 1]), at most S <= 3 long. weight: [Q] or null (1 per row).
+// Either way its current list is cur[rep_off[g] .. rep_off[g + 1]), at most S <= 3 long, and ka_score_row scores it; only
+// finding the row's member differs between the instances. weight: [Q] or null (1 per row).
 // bro_off[k]: member k's (cluster k's) first entry in the per-broker arrays (cand_off of the call); summary: [K].
 template <bool FLEET>
 __global__ void __launch_bounds__(256) ka_score_rows_kernel(const KaCandidate* __restrict__ cand, const int32_t* __restrict__ bro_off,
@@ -99,111 +82,50 @@ __global__ void __launch_bounds__(256) ka_score_rows_kernel(const KaCandidate* _
                                                             ka_move_summary* __restrict__ summary, long long* __restrict__ broker_replicas,
                                                             long long* __restrict__ broker_leaders, long long* __restrict__ broker_in,
                                                             const KaJsonSegs sg) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    int k, member;   // the summary the row adds to; the batch member that scores it, -1: the row adds nothing
+    int64_t row;
+    unsigned grp;    // the lanes that add to summary k
     if constexpr (FLEET) {
         __shared__ int64_t row0[KA_JSON_MAX_SEGS + 1];
         __shared__ int live[KA_JSON_MAX_SEGS];   // cluster k's batch member, -1 = dead
         ka_json_stage_segs(sg, row0, nullptr);
-        for (int k = threadIdx.x; k < sg.K; k += blockDim.x) {
-            const int m = sg.member[k];
-            live[k] = m >= 0 && ka_score_ok(cand[m]) ? m : -1;
+        for (int i = threadIdx.x; i < sg.K; i += blockDim.x) {
+            const int m = sg.member[i];
+            live[i] = m >= 0 && ka_score_ok(cand[m]) ? m : -1;
         }
         __syncthreads();
-        const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-        const int k = g < Q ? ka_json_seg_of(row0, sg.K, g) : -1;
-        int changed = 0, moved = 0, leader = 0;
-        long long added = 0, dropped = 0;
-        if (k >= 0 && live[k] >= 0)
-            ka_score_row(cand[live[k]], bro_off, k, g, g, S, out, out_len, rep_off, cur, weight, broker_replicas, broker_leaders,
-                         broker_in, changed, moved, leader, added, dropped);
-        // a warp may span clusters: sum over each run of lanes of one cluster, one atomic per run and field
-        const unsigned grp = __match_any_sync(KA_FULL, k);
-        changed = __reduce_add_sync(grp, changed);
-        moved = __reduce_add_sync(grp, moved);
-        leader = __reduce_add_sync(grp, leader);
-        if (grp == KA_FULL) {   // warp-uniform
-            added = ka_warp_sum64(added);
-            dropped = ka_warp_sum64(dropped);
-        } else {
-            added = ka_seg_sum64(added, grp);
-            dropped = ka_seg_sum64(dropped, grp);
-        }
-        if (k >= 0 && (int)(threadIdx.x & 31) == __ffs(grp) - 1) {
-            ka_move_summary& s = summary[k];
-            auto add = [](int64_t& f, long long v) {
-                if (v) atomicAdd(reinterpret_cast<unsigned long long*>(&f), (unsigned long long)v);
-            };
-            add(s.rows_changed, changed);
-            add(s.rows_moved, moved);
-            add(s.leaders_changed, leader);
-            add(s.replicas_added, added);
-            add(s.replicas_dropped, dropped);
-        }
-    } else {   // the per-row code inline, as before FLEET existed: ka_score_row would change this instance's register allocation
-        const int k = blockIdx.y;
-        const KaCandidate& c = cand[k];
-        if (!ka_score_ok(c)) return;   // CTA-uniform: every lane below reaches the warp sums
-        const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-        int changed = 0, moved = 0, leader = 0;
-        long long added = 0, dropped = 0;
-        if (g < Q) {
-            const int64_t row = (int64_t)k * Q + g;
-            const int n = out_len[row];
-            const int64_t a = rep_off[g];
-            const int m = (int)(rep_off[g + 1] - a);
-            int nb[3], cb[3];
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                nb[j] = j < n ? out[row * S + j] : 0;
-                cb[j] = j < m ? __ldg(cur + a + j) : 0;
-            }
-            const long long w = weight ? __ldg(weight + g) : 1;
-            const KaBrokers br = c.br;   // read once: the atomics below may alias HBM as far as the compiler knows
-            const int64_t base = bro_off[k];
-            int n_add = 0, n_drop = 0;
-            bool diff = n != m;
-#pragma unroll
-            for (int j = 0; j < 3; ++j) {
-                if (j < m) {
-                    bool kept = false;
-#pragma unroll
-                    for (int i = 0; i < 3; ++i) kept |= i < n && nb[i] == cb[j];
-                    n_drop += !kept;
-                }
-                if (j < n) {
-                    bool held = false;
-#pragma unroll
-                    for (int i = 0; i < 3; ++i) held |= i < m && cb[i] == nb[j];
-                    n_add += !held;
-                    diff |= j < m && nb[j] != cb[j];
-                    // the candidate's id -> index lookup of kernel A, its table read from HBM
-                    const int64_t e = base + ka_lookup(nb[j], br.blob + br.lut_off, br);
-                    atomicAdd(reinterpret_cast<unsigned long long*>(broker_replicas + e), (unsigned long long)w);
-                    if (j == 0) atomicAdd(reinterpret_cast<unsigned long long*>(broker_leaders + e), (unsigned long long)w);
-                    if (!held) atomicAdd(reinterpret_cast<unsigned long long*>(broker_in + e), (unsigned long long)w);
-                }
-            }
-            changed = diff;
-            moved = n_add + n_drop > 0;
-            leader = m == 0 || n == 0 || nb[0] != cb[0];
-            added = w * n_add;
-            dropped = w * n_drop;
-        }
-        changed = __reduce_add_sync(KA_FULL, changed);
-        moved = __reduce_add_sync(KA_FULL, moved);
-        leader = __reduce_add_sync(KA_FULL, leader);
-        added = ka_warp_sum64(added);
-        dropped = ka_warp_sum64(dropped);
-        if ((threadIdx.x & 31) == 0) {
-            ka_move_summary& s = summary[k];
-            auto add = [](int64_t& f, long long v) {
-                if (v) atomicAdd(reinterpret_cast<unsigned long long*>(&f), (unsigned long long)v);
-            };
-            add(s.rows_changed, changed);
-            add(s.rows_moved, moved);
-            add(s.leaders_changed, leader);
-            add(s.replicas_added, added);
-            add(s.replicas_dropped, dropped);
-        }
+        k = g < Q ? ka_json_seg_of(row0, sg.K, g) : -1;
+        member = k >= 0 ? live[k] : -1;
+        row = g;
+        grp = __match_any_sync(KA_FULL, k);   // a warp may span clusters: one group, and one atomic per field, per cluster
+    } else {
+        k = blockIdx.y;
+        if (!ka_score_ok(cand[k])) return;   // CTA-uniform: every lane below reaches the group sums
+        member = g < Q ? k : -1;
+        row = (int64_t)k * Q + g;
+        grp = KA_FULL;
+    }
+    int changed = 0, moved = 0, leader = 0;
+    long long added = 0, dropped = 0;
+    if (member >= 0)
+        ka_score_row(cand[member], bro_off, k, row, g, S, out, out_len, rep_off, cur, weight, broker_replicas, broker_leaders,
+                     broker_in, changed, moved, leader, added, dropped);
+    changed = __reduce_add_sync(grp, changed);
+    moved = __reduce_add_sync(grp, moved);
+    leader = __reduce_add_sync(grp, leader);
+    added = ka_group_sum64(added, grp);   // the host holds 3 x the sum of the weights to INT64_MAX
+    dropped = ka_group_sum64(dropped, grp);
+    if (k >= 0 && (int)(threadIdx.x & 31) == __ffs(grp) - 1) {
+        ka_move_summary& s = summary[k];
+        auto add = [](int64_t& f, long long v) {
+            if (v) atomicAdd(reinterpret_cast<unsigned long long*>(&f), (unsigned long long)v);
+        };
+        add(s.rows_changed, changed);
+        add(s.rows_moved, moved);
+        add(s.leaders_changed, leader);
+        add(s.replicas_added, added);
+        add(s.replicas_dropped, dropped);
     }
 }
 

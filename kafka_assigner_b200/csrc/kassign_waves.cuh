@@ -250,26 +250,23 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
 }
 
 // grid ceil(Q / 256), 256 threads, summary[W] zeroed: every changed row adds to its wave's rows, rows_moved and replicas_added.
-// A warp sums each wave among its lanes (the 64-bit sums in three limbs of at most 22 bits, so the 32-bit lane sums cannot
-// carry), one atomic per wave and field.
+// A warp sums each wave among its lanes (ka_group_sum64: a row adds at most 8 x its weight, and the host holds 8 x the sum of
+// the weights to INT64_MAX), one atomic per wave and field.
 __global__ void __launch_bounds__(256) ka_wave_sum_kernel(uint32_t Q, const int8_t* __restrict__ nrecv, const int32_t* __restrict__ wave,
                                                           const int64_t* __restrict__ weight, ka_wave_summary* __restrict__ summary) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     const int v = g < Q ? wave[g] : 0;
     const int nr = g < Q ? nrecv[g] : -1;
-    const unsigned long long added = nr > 0 ? (unsigned long long)((weight ? __ldg(weight + g) : 1) * nr) : 0;
+    const long long added = nr > 0 ? (weight ? __ldg(weight + g) : 1) * nr : 0;
     const unsigned grp = __match_any_sync(KA_FULL, v);
     const unsigned rows = __reduce_add_sync(grp, (unsigned)(v > 0));
     const unsigned moved = __reduce_add_sync(grp, (unsigned)(nr > 0));
-    const unsigned long long a0 = __reduce_add_sync(grp, (unsigned)(added & 0x3FFFFFu));
-    const unsigned long long a1 = __reduce_add_sync(grp, (unsigned)(added >> 22 & 0x1FFFFFu));
-    const unsigned long long a2 = __reduce_add_sync(grp, (unsigned)(added >> 43));
+    const long long sum = ka_group_sum64(added, grp);
     if (v > 0 && (int)(threadIdx.x & 31) == __ffs(grp) - 1) {
         ka_wave_summary& s = summary[v - 1];
         atomicAdd(reinterpret_cast<unsigned long long*>(&s.rows), (unsigned long long)rows);
         if (moved) atomicAdd(reinterpret_cast<unsigned long long*>(&s.rows_moved), (unsigned long long)moved);
-        const unsigned long long sum = a0 + (a1 << 22) + (a2 << 43);
-        if (sum) atomicAdd(reinterpret_cast<unsigned long long*>(&s.replicas_added), sum);
+        if (sum) atomicAdd(reinterpret_cast<unsigned long long*>(&s.replicas_added), (unsigned long long)sum);
     }
 }
 

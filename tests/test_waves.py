@@ -453,6 +453,25 @@ def test_context_is_untouched_and_launches_are_fixed(native_lib):
 
 
 @pytest.mark.gpu
+def test_plans_on_its_own_device(native_lib):
+    """A Solver plans on its context's device whatever device is current: here another Solver's device 0."""
+    import torch
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs two GPUs")
+    cl = kab.synth.make_ragged_cluster(T=2000, N=200, max_partitions=64, seed=23, remove_frac=0.02)
+    s = kab.Solver(1)
+    s.set_brokers(cl.broker_id, cl.rack_index)
+    out, out_len, st = s.solve_ragged(cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off, cl.cur, -1, 3)
+    assert st.code == 0
+    other = kab.Solver(0)   # leaves device 0 current
+    other.set_brokers(cl.broker_id, cl.rack_index)
+    weight = np.random.default_rng(5).integers(0, 1000, len(out_len)).astype(np.int64)
+    for B, w in ((1, None), (2000, weight)):
+        _, summ, st = _check(s, cl.rep_off, cl.cur, out, out_len, B, w)
+        assert st.code == 0 and len(summ) > 0
+
+
+@pytest.mark.gpu
 def test_cpp_host_mirror(native_lib):
     """host/test_waves.cpp: every wave's document of KafkaTopicAssigner::planWaves, concatenated over the waves, holds exactly the
     changed partitions of newAssignmentJson(solveTopics(...))."""
