@@ -349,6 +349,41 @@ int32_t ka_plan_waves(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int3
                       const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
                       int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap, ka_status* st);
 
+/* ka_plan_waves + the documents it plans, built on the device: one reassignment JSON per wave, what an operator feeds
+ * kafka-reassign-partitions one after the other. Only the text, the waves and the summaries cross PCIe.
+ *   T, part_off[T+1], part_id (NULL = 0..P-1 per topic), names, name_off[T+1]   host; the ragged layout and the name slab
+ *                      exactly as ka_solve_json takes them; Q = part_off[T] rows
+ *   rep_off .. max_broker_in   exactly as ka_plan_waves takes them, over those Q rows
+ *   wave, n_waves, summary, summary_cap   exactly as ka_plan_waves writes them: the same values for the same inputs
+ *   json               host buffer of json_cap bytes (pinned for full PCIe speed)
+ *   doc_off[Q+1]       host, required when Q > 0 (W never exceeds Q, so no second call is ever needed); entries 0..W are written,
+ *                      doc_off[0] = 0
+ * Document v, the one of wave v + 1, is json[doc_off[v] .. doc_off[v+1]): the documents lie back to back and are not
+ * NUL-terminated. It is {"partitions":[ + the records of the rows with wave[g] == v + 1, in input row order, comma separated +
+ * ],"version":1}, a record being byte for byte the one ka_solve_json prints for that row (its topic's name, its partition
+ * through part_id, its new list). Unchanged rows (wave 0) are in no document, a changed row is in exactly one. W == 0 (nothing
+ * changed, or Q == 0) gives no document: doc_off[0] = 0 (when doc_off is given), KA_OK.
+ * json_cap = the sum over rows of (79 + 12*stride + name length of the row's topic) always suffices: the 50 + 12*stride + name
+ * of a record of ka_solve_json, and the 29 bytes of a document's header and trailer charged to every row, because a wave has at
+ * least one row.
+ * Checks, in this order, before anything is enqueued: st NULL: KA_ERR_BAD_ARG (nothing written); ctx NULL: KA_ERR_NO_DEVICE;
+ * everything ka_plan_waves checks, with its codes and operands (T < 0, or part_off NULL with T > 0, leaves no Q to check:
+ * KA_ERR_BAD_ARG); then part_off not non-decreasing from 0, names or name_off NULL with T > 0, json NULL, json_cap < 0, or
+ * doc_off NULL with Q > 0: KA_ERR_BAD_ARG; then a name org.json would escape: KA_ERR_BAD_ARG with a = the byte (take
+ * ka_plan_waves and a host emitter instead). On the device the plan's own row errors come first, with the code, a and b of
+ * ka_plan_waves; a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX). On any error *n_waves = 0 and
+ * nothing else is specified.
+ * Synchronous. The kernel launches it adds depend only on the bit length of W (one stable radix pass over the waves per 8
+ * bits), not on Q or T. Does not read or change the Context counters, parked counters, topic_base, the staged block, or the
+ * last order / stage plans and timings. */
+int32_t ka_plan_waves_json(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                           const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                           const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                           int64_t max_broker_in, const char* names, const int64_t* name_off,
+                           char* json, int64_t json_cap, int64_t* doc_off,
+                           int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap,
+                           ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

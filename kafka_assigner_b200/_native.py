@@ -52,6 +52,8 @@ SYMBOLS = {
     "ka_solve_clusters_json": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp,
                                       _vp]),
     "ka_plan_waves": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp]),
+    "ka_plan_waves_json": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
+                                  _vp, _i32, _vp]),
     "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "ka_ctx_set_topic_base": (_i32, [_vp, _i32]),

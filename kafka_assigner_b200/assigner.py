@@ -76,6 +76,12 @@ def _json_size(rows, name_bytes, stride):
     return 64 + rows * (50 + 12 * stride) + name_bytes
 
 
+def _wave_json_size(rows, name_bytes, stride):
+    """The sufficient buffer size kassign.h documents for the documents of a wave plan: per row 79 + 12·stride + its topic's
+    name length (a record of _json_size, and a document's 29 bytes of header and trailer charged to every row)."""
+    return rows * (79 + 12 * stride) + name_bytes
+
+
 class _Ragged(collections.namedtuple("_Ragged", "topic_hash part_off part_id rep_off cur_broker Q")):
     """A ragged problem as the C ABI takes it: (topic_hash, part_off, part_id, rep_off, cur_broker) as contiguous arrays of
     their element types (part_id may be None), and Q = ΣP, its number of rows."""
@@ -502,6 +508,38 @@ class Solver:
             if n_waves.value <= cap:
                 return wave, summary[:n_waves.value], st
             cap = n_waves.value
+
+    def plan_waves_json(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, weight=None,
+                        json_buf=None):
+        """ka_plan_waves_json: plan_waves over the rows of the ragged layout part_off / part_id (None = 0..P-1 per topic), and
+        every wave's reassignment JSON built on the device. json_buf: optional writable uint8 numpy array (pinned for full PCIe
+        speed); by default one of the documented sufficient size. Returns (docs, wave, summary, KaStatus): docs a list of W
+        bytes-like views of the buffer, docs[v] the document of wave v + 1; wave and summary as plan_waves returns them. On an
+        error docs, wave and summary are empty."""
+        out = np.ascontiguousarray(out, dtype=np.int32)
+        Q = len(out)
+        stride = out.shape[1] if out.ndim == 2 else 1
+        out_len = np.ascontiguousarray(out_len, dtype=np.int32)
+        r = _ragged(np.zeros(len(topic_names), dtype=np.int32), part_off, part_id, rep_off, cur_broker)
+        weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
+        assert r.Q == Q and out_len.shape == (Q,) and r.rep_off.shape == (Q + 1,) and (weight is None or weight.shape == (Q,))
+        names, name_off = self.marshal_names(topic_names)
+        if json_buf is None:
+            json_buf = np.empty(max(_wave_json_size(Q, r.name_bytes(np.diff(name_off)), stride), 1), dtype=np.uint8)
+        doc_off = np.zeros(Q + 1, dtype=np.int64)
+        wave = np.zeros(Q, dtype=np.int32)
+        n_waves = ctypes.c_int32(0)
+        st = KaStatus()
+        cap = max(1, Q)   # W never exceeds Q: one call, so the text is built once
+        summary = np.zeros(cap, dtype=WAVE_SUMMARY_DTYPE)
+        self._L.ka_plan_waves_json(self._h, len(topic_names), _ptr(r.part_off), _ptr(r.part_id), _ptr(r.rep_off), _ptr(r.cur_broker),
+                                   int(stride), _ptr(out_len), _ptr(out), _ptr(weight), int(max_broker_in), _ptr(names),
+                                   _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(doc_off), _ptr(wave),
+                                   ctypes.byref(n_waves), _ptr(summary), cap, ctypes.byref(st))
+        if st.code != 0:
+            return [], np.zeros(0, dtype=np.int32), np.zeros(0, dtype=WAVE_SUMMARY_DTYPE), st
+        W = n_waves.value
+        return [json_buf[doc_off[v]:doc_off[v + 1]] for v in range(W)], wave, summary[:W], st
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

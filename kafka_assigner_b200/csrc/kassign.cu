@@ -7,6 +7,7 @@
 #include "kassign_json.cuh"
 #include "kassign_score.cuh"
 #include "kassign_waves.cuh"
+#include "kassign_waves_json.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -148,6 +149,10 @@ struct ka_ctx {
     // outputs and records, the packed records, the per-CTA counts and offsets, the chain's per-broker words when they leave
     // shared memory, the bucket log, the summaries and the meta words
     DevBuf d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state, d_wv_log, d_wv_sum, d_wv_meta;
+    // scratch of ka_plan_waves_json, beside the plan's and the JSON passes' (d_part_off, d_part_id, d_names, d_name_off, d_json,
+    // d_json_rowlen, d_json_blocksum as 64-bit offsets): the grouped rows (two arrays of Q), the radix passes' (digit, tile)
+    // counts and offsets, and the text total followed by doc_off [W + 1]
+    DevBuf d_wv_perm, d_wv_hist, d_wv_doc;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -1293,7 +1298,7 @@ void ka_ctx_destroy(ka_ctx* c) {
                       &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
                       &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec,
-                      &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta})
+                      &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta, &c->d_wv_perm, &c->d_wv_hist, &c->d_wv_doc})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -2374,33 +2379,36 @@ static int32_t wave_refused_id(const std::vector<int32_t>& ids, const int64_t* r
     return 0;
 }
 
-int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
-                      const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, int32_t* wave, int32_t* n_waves,
-                      ka_wave_summary* summary, int32_t summary_cap, ka_status* st) {
-    if (!st) return KA_ERR_BAD_ARG;
-    if (n_waves) *n_waves = 0;
-    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
+// The argument checks of ka_plan_waves, in its order, once st and the ctx are there. R = the current lists' brokers, positions
+// = the new lists' (a bound on the chain's buckets).
+static int wave_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                     const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, const int32_t* n_waves,
+                     const ka_wave_summary* summary, int32_t summary_cap, int64_t& R, int64_t& positions, ka_status* st) {
     if (Q < 0 || stride < 1 || !n_waves || summary_cap < 0 || (!summary && summary_cap > 0) || max_broker_in < 1 ||
         (Q > 0 && (!rep_off || !new_len || !new_broker)) || (rep_off && rep_off[0] != 0))
         return set_status(st, KA_ERR_BAD_ARG);
     for (int64_t g = 0; g < Q; ++g)
         if (rep_off[g + 1] < rep_off[g]) return set_status(st, KA_ERR_BAD_ARG);
-    const int64_t R = Q > 0 ? rep_off[Q] : 0;
+    R = Q > 0 ? rep_off[Q] : 0;
     if (R > 0 && !cur_broker) return set_status(st, KA_ERR_BAD_ARG);
     if (stride > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, stride);
     if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX);
-    int64_t positions = 0;   // new-list positions: a bound on the chain's buckets
+    positions = 0;
     for (int64_t g = 0; g < Q; ++g) {
         if (new_len[g] < 0 || new_len[g] > stride) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
         positions += new_len[g];
     }
-    int rc = weights_code(part_weight, Q, 8);   // a row adds at most 8 x its weight to a wave
-    if (rc != KA_OK) return set_status(st, rc);
-    if (Q == 0) return set_status(st, KA_OK);
-    // the call reads only the broker table: a pending asynchronous status stays pending for ka_last_status
-    if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
+    const int rc = weights_code(part_weight, Q, 8);   // a row adds at most 8 x its weight to a wave
+    return rc != KA_OK ? set_status(st, rc) : KA_OK;
+}
 
-    // the inputs go up into the buffers of the host-buffer solve and score calls: every such call is synchronous
+// The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the inputs up (into the buffers of the
+// host-buffer solve and score calls: every such call is synchronous), the rows / scan / compact / chain kernels, the meta words
+// back, then the sum and the two peak kernels (enqueued, not awaited). Leaves every row's wave in d_wv_wave, its receivers in
+// d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids still N - index) in d_wv_sum.
+static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, const int64_t* rep_off, const int32_t* cur_broker,
+                            int32_t stride, const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                            int64_t max_broker_in, int& W, ka_status* st) {
     cudaStream_t s = c->stream;
     const int N = c->br.N;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
@@ -2453,9 +2461,8 @@ int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_
     if (meta.err_row != 0xFFFFFFFFu)
         return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row,
                           wave_refused_id(c->broker_id, rep_off, cur_broker, stride, new_len, new_broker, meta.err_row));
-    const int W = std::max(meta.waves, meta.changed);
+    W = std::max(meta.waves, meta.changed);
     const size_t sum_bytes = (size_t)std::max(W, 1) * sizeof(ka_wave_summary);
-    const int out = std::min(W, summary_cap);
     if (c->d_wv_sum.reserve(sum_bytes)) return set_status(st, KA_ERR_CUDA);
     ka_wave_summary* d_sum = c->d_wv_sum.as<ka_wave_summary>();
     const unsigned peak_blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>(((int64_t)meta.nlog + 255) / 256, (int64_t)c->sm_count * 8));
@@ -2464,9 +2471,18 @@ int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_
     ka_wave_peak_kernel<false><<<peak_blocks, 256, 0, s>>>(d_log, meta.nlog, N, d_sum);
     ka_wave_peak_kernel<true><<<peak_blocks, 256, 0, s>>>(d_log, meta.nlog, N, d_sum);
     c->launches += 3;
-    if (cudaGetLastError() != cudaSuccess ||
-        (out > 0 && cudaMemcpyAsync(summary, d_sum, (size_t)out * sizeof(ka_wave_summary), cudaMemcpyDeviceToHost, s)) ||
-        (wave && cudaMemcpyAsync(wave, d_wave, q * 4, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
+    return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
+}
+
+// The plan of wave_plan_device out to the caller: the first min(W, summary_cap) summaries and every row's wave, awaited; then
+// the summaries' broker ids and *n_waves.
+static int wave_plan_out(ka_ctx* c, int64_t Q, int W, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap,
+                         ka_status* st) {
+    cudaStream_t s = c->stream;
+    const int N = c->br.N;
+    const int out = std::min(W, summary_cap);
+    if ((out > 0 && cudaMemcpyAsync(summary, c->d_wv_sum.p, (size_t)out * sizeof(ka_wave_summary), cudaMemcpyDeviceToHost, s)) ||
+        (wave && cudaMemcpyAsync(wave, c->d_wv_wave.p, (size_t)Q * 4, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     for (int v = 0; v < out; ++v) {   // N - the lowest broker index of the wave's peak, 0 when nothing was added
         const int64_t f = summary[v].max_broker_in_id;
@@ -2474,6 +2490,131 @@ int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_
     }
     *n_waves = W;
     return set_status(st, KA_OK);
+}
+
+int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                      const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, int32_t* wave, int32_t* n_waves,
+                      ka_wave_summary* summary, int32_t summary_cap, ka_status* st) {
+    if (!st) return KA_ERR_BAD_ARG;
+    if (n_waves) *n_waves = 0;
+    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
+    int64_t R = 0, positions = 0;
+    int rc = wave_args(Q, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, n_waves, summary, summary_cap, R,
+                       positions, st);
+    if (rc != KA_OK) return rc;
+    if (Q == 0) return set_status(st, KA_OK);
+    // the call reads only the broker table: a pending asynchronous status stays pending for ka_last_status
+    if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
+    int W = 0;
+    if ((rc = wave_plan_device(c, Q, R, positions, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, W,
+                               st)) != KA_OK)
+        return rc;
+    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, st);
+}
+
+// The radix passes of ka_plan_waves_json over the plan's d_wv_wave: d_wv_perm (two arrays of Q rows) ends with the changed
+// rows ordered by (wave, row) in the array returned, and the (digit, tile) offsets end with M, the changed rows, at n_rows.
+static const int32_t* enq_wave_group(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const int32_t*& n_rows) {
+    KaWaveSort p{};
+    p.wave = c->d_wv_wave.as<int32_t>();
+    p.Q = (uint32_t)Q;
+    p.tile = (uint32_t)std::max<int64_t>(KA_WAVE_SORT_MIN_TILE, ((Q + KA_WAVE_SORT_MAX_TILES - 1) / KA_WAVE_SORT_MAX_TILES + 255) / 256 * 256);
+    p.ntiles = (int)((Q + p.tile - 1) / p.tile);
+    const int cells = KA_WAVE_SORT_DIGITS * p.ntiles;
+    int32_t* hist = c->d_wv_hist.as<int32_t>();
+    int32_t* off = hist + cells;
+    int32_t* perm[2] = {c->d_wv_perm.as<int32_t>(), c->d_wv_perm.as<int32_t>() + Q};
+    p.n_ptr = n_rows = off + cells;
+    int pass = 0;
+    for (; pass == 0 || W >> p.shift; ++pass, p.shift += KA_WAVE_SORT_BITS) {
+        p.in = pass ? perm[(pass - 1) & 1] : nullptr;
+        ka_wave_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, hist);
+        ka_level_scan_kernel<<<1, 1024, 0, s>>>(hist, cells, off);
+        ka_wave_sort_scatter_kernel<<<p.ntiles, 256, 0, s>>>(p, off, perm[pass & 1]);
+        c->launches += 3;
+    }
+    return perm[(pass - 1) & 1];
+}
+
+int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
+                           const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
+                           const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
+                           int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
+                           int32_t summary_cap, ka_status* st) {
+    if (!st) return KA_ERR_BAD_ARG;
+    if (n_waves) *n_waves = 0;
+    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
+    if (T < 0 || (T > 0 && !part_off)) return set_status(st, KA_ERR_BAD_ARG);   // no Q to check
+    const int64_t Q = T > 0 ? part_off[T] : 0;
+    int64_t R = 0, positions = 0;
+    int rc = wave_args(Q, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, n_waves, summary, summary_cap, R,
+                       positions, st);
+    if (rc != KA_OK) return rc;
+    if ((T > 0 && (part_off[0] != 0 || !names || !name_off)) || !json || json_cap < 0 || (Q > 0 && !doc_off))
+        return set_status(st, KA_ERR_BAD_ARG);
+    int64_t bound = 0;   // the sufficient size: per row 79 + 12 x stride + its topic's name
+    for (int t = 0; t < T; ++t) {
+        if (part_off[t + 1] < part_off[t]) return set_status(st, KA_ERR_BAD_ARG);
+        bound += (part_off[t + 1] - part_off[t]) * (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + 50 + 12 * (int64_t)stride + name_off[t + 1] - name_off[t]);
+    }
+    if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
+    if (doc_off) doc_off[0] = 0;
+    if (Q == 0) return set_status(st, KA_OK);
+    if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
+    int W = 0;
+    if ((rc = wave_plan_device(c, Q, R, positions, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, W,
+                               st)) != KA_OK)
+        return rc;
+    if (W == 0) return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, st);
+
+    cudaStream_t s = c->stream;
+    const size_t q = (size_t)Q;
+    const unsigned nblk = (unsigned)((Q + 255) / 256);
+    const int64_t name_bytes = name_off[T];
+    const int64_t cap = std::min(json_cap, bound);
+    const size_t tiles = (size_t)(Q + KA_WAVE_SORT_MIN_TILE - 1) / KA_WAVE_SORT_MIN_TILE;   // at least the passes' tiles
+    if (c->d_part_off.reserve((size_t)(T + 1) * 8) || (part_id && c->d_part_id.reserve(q * 4)) ||
+        c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)) || c->d_name_off.reserve((size_t)(T + 1) * 8) ||
+        c->d_json.reserve((size_t)std::max<int64_t>(cap, 1)) || c->d_json_rowlen.reserve(q * 4) ||
+        c->d_json_blocksum.reserve((size_t)nblk * 8) || c->d_wv_perm.reserve(2 * q * 4) ||
+        c->d_wv_hist.reserve((2 * KA_WAVE_SORT_DIGITS * tiles + 1) * 4) || c->d_wv_doc.reserve(((size_t)W + 2) * 8))
+        return set_status(st, KA_ERR_CUDA);
+    if (cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s) ||
+        (part_id && cudaMemcpyAsync(c->d_part_id.p, part_id, q * 4, cudaMemcpyHostToDevice, s)) ||
+        (name_bytes > 0 && cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, s)) ||
+        cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s))
+        return set_status(st, KA_ERR_CUDA);
+    KaWaveDocs d{};
+    d.perm = enq_wave_group(c, s, Q, W, d.n_rows);
+    d.wave = c->d_wv_wave.as<int32_t>();
+    d.blockoff = c->d_json_blocksum.as<unsigned long long>();
+    unsigned long long* d_total = c->d_wv_doc.as<unsigned long long>();
+    d.doc_off = d_total + 1;
+    d.p.Q = (uint32_t)Q;
+    d.p.T = T;
+    d.p.part_off = c->d_part_off.as<int64_t>();
+    d.p.part_id = part_id ? c->d_part_id.as<int32_t>() : nullptr;
+    d.p.name_off = c->d_name_off.as<int64_t>();
+    d.p.names = c->d_names.as<char>();
+    d.p.out = c->d_out.as<int32_t>();
+    d.p.out_len = c->d_out_len.as<int32_t>();
+    d.p.S = stride;
+    d.p.rowlen = c->d_json_rowlen.as<uint32_t>();
+    d.p.json = c->d_json.as<char>();
+    d.p.cap = (unsigned long long)cap;
+    if (allow_smem(ka_wave_doc_write_kernel, KA_JSON_SMEM_BYTES + 16) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    ka_wave_doc_len_kernel<<<nblk, 256, 0, s>>>(d);
+    ka_wave_doc_scan_kernel<<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total);
+    ka_wave_doc_write_kernel<<<nblk, 256, KA_JSON_SMEM_BYTES + 16, s>>>(d, d_total);
+    c->launches += 3;
+    unsigned long long total = 0;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, s) || cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    if (total > (unsigned long long)json_cap) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
+    if (cudaMemcpyAsync(json, c->d_json.p, (size_t)total, cudaMemcpyDeviceToHost, s) ||
+        cudaMemcpyAsync(doc_off, d.doc_off, ((size_t)W + 1) * 8, cudaMemcpyDeviceToHost, s))
+        return set_status(st, KA_ERR_CUDA);
+    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, st);
 }
 
 }  // extern "C"

@@ -1,0 +1,236 @@
+// kassign_waves_json.cuh — one reassignment document per wave of a wave plan (ka_plan_waves_json), built on the device from the
+// rows the plan left there, so that only TEXT crosses PCIe.
+//
+// A wave's rows are scattered over the whole input and there may be as many waves as changed rows, so the documents are not
+// segments of the input. The changed rows are first grouped by wave, stably (perm = the changed rows ordered by (wave, row)), and
+// the document frame is folded into the rows: the first row of a wave carries {"partitions":[ in place of its leading comma, the
+// last one also ],"version":1}. The whole output is then ONE concatenation of the grouped rows' texts, and document v starts
+// where the first row of wave v + 1 does.
+//
+//   ka_wave_sort_hist_kernel     per tile of rows: how many keys have each value of the pass's 8-bit digit
+//   ka_level_scan_kernel         (digit, tile) offsets (kassign_order.cuh); their total is M, the changed rows
+//   ka_wave_sort_scatter_kernel  the tile's rows to their digit's range, in row order (a stable LSD radix pass). The first pass
+//                                reads the rows 0..Q-1 themselves and drops wave 0, so it also compacts.
+//   ka_wave_doc_len_kernel       text bytes of every grouped row + per-CTA sums
+//   ka_wave_doc_scan_kernel      ONE CTA: 64-bit text offsets of the CTAs, and the total
+//   ka_wave_doc_write_kernel     the text (the staging of ka_json_write_kernel) and doc_off[0..W]
+//
+// A pass ranks a row by counting, never by the order of atomics: the text depends on the input alone.
+#pragma once
+#include "kassign_json.cuh"
+#include "kassign_waves.cuh"
+
+#define KA_WAVE_SORT_BITS 8
+#define KA_WAVE_SORT_DIGITS (1 << KA_WAVE_SORT_BITS)
+#define KA_WAVE_SORT_MIN_TILE 2048   // rows per CTA of a pass, at least (a multiple of the 256 threads)
+#define KA_WAVE_SORT_MAX_TILES 1024  // CTAs of a pass, at most: the (digit, tile) table stays within 256 k entries
+static_assert(KA_WAVE_SORT_DIGITS == 256, "one thread per digit value");
+
+// One radix pass over the keys wave[g] >> shift. in == null: the items are the rows 0..Q-1 (first pass); else the *n_ptr rows
+// in[]. A row of wave 0 is no item. Tile b owns items [b * tile, (b + 1) * tile).
+struct KaWaveSort {
+    const int32_t* wave;
+    const int32_t* in;
+    uint32_t Q;
+    const int32_t* n_ptr;
+    int shift;
+    uint32_t tile;
+    int ntiles;
+};
+
+__device__ __forceinline__ bool ka_wave_sort_item(const KaWaveSort& p, uint32_t i, uint32_t hi, int32_t& g, int& digit) {
+    if (i >= hi) return false;
+    g = p.in ? p.in[i] : (int32_t)i;
+    const int v = p.wave[g];
+    digit = (v >> p.shift) & (KA_WAVE_SORT_DIGITS - 1);
+    return v > 0;
+}
+
+// grid ntiles, 256 threads: hist[digit * ntiles + tile] = the tile's items with that digit.
+__global__ void __launch_bounds__(256) ka_wave_sort_hist_kernel(const KaWaveSort p, int32_t* __restrict__ hist) {
+    __shared__ int h[KA_WAVE_SORT_DIGITS];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const uint32_t n = p.in ? (uint32_t)*p.n_ptr : p.Q;
+    const uint64_t lo = (uint64_t)blockIdx.x * p.tile;
+    const uint32_t hi = (uint32_t)min((uint64_t)n, lo + p.tile);
+    for (uint64_t i = lo + threadIdx.x; i < hi; i += 256) {
+        int32_t g;
+        int digit;
+        if (ka_wave_sort_item(p, (uint32_t)i, hi, g, digit)) atomicAdd(&h[digit], 1);   // a count: any order gives it
+    }
+    __syncthreads();
+    hist[threadIdx.x * p.ntiles + blockIdx.x] = h[threadIdx.x];
+}
+
+// Same grid: off = the exclusive scan of hist. Item i of the tile goes to out[off[digit][tile] + its rank among the tile's items
+// of that digit]. The tile is taken 256 items at a time; in a round a lane ranks itself among the lanes of its warp with the
+// same digit (match_any, lanes in item order), then behind the earlier warps' and the earlier rounds' items of that digit.
+__global__ void __launch_bounds__(256) ka_wave_sort_scatter_kernel(const KaWaveSort p, const int32_t* __restrict__ off,
+                                                                   int32_t* __restrict__ out) {
+    __shared__ int base[KA_WAVE_SORT_DIGITS];
+    __shared__ int wcnt[8][KA_WAVE_SORT_DIGITS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    base[threadIdx.x] = off[threadIdx.x * p.ntiles + blockIdx.x];
+    const uint32_t n = p.in ? (uint32_t)*p.n_ptr : p.Q;
+    const uint64_t lo = (uint64_t)blockIdx.x * p.tile;
+    const uint32_t hi = (uint32_t)min((uint64_t)n, lo + p.tile);
+    for (uint64_t r0 = lo; r0 < hi; r0 += 256) {   // CTA-uniform
+#pragma unroll
+        for (int w = 0; w < 8; ++w) wcnt[w][threadIdx.x] = 0;
+        int32_t g = 0;
+        int digit = 0;
+        const bool item = ka_wave_sort_item(p, (uint32_t)(r0 + threadIdx.x), hi, g, digit);
+        const unsigned same = __match_any_sync(KA_FULL, item ? digit : -1);
+        __syncthreads();
+        if (item && lane == __ffs(same) - 1) wcnt[warp][digit] = __popc(same);
+        __syncthreads();
+        if (item) {
+            int pos = base[digit] + __popc(same & ka_lanemask_lt());
+            for (int w = 0; w < warp; ++w) pos += wcnt[w][digit];
+            out[pos] = g;
+        }
+        __syncthreads();
+        int s = 0;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s += wcnt[w][threadIdx.x];
+        base[threadIdx.x] += s;   // column threadIdx.x is this thread's alone until the next round's counts
+    }
+}
+
+// The text passes. Grouped position i < M = *n_rows holds row perm[i]; p describes the run's rows (row0 = 0, so its row q is the
+// run-wide row g: p.out / p.out_len are the proposed lists, p.rowlen is indexed by POSITION here). The grids cover Q rows, M is
+// only known on the device: the CTAs beyond it do nothing.
+struct KaWaveDocs {
+    KaJsonParams p;
+    const int32_t* wave;                 // [Q]
+    const int32_t* perm;                 // [M]
+    const int32_t* n_rows;               // M
+    unsigned long long* blockoff;        // [ceil(Q / 256)] text bytes of every CTA, then (scan) its text offset
+    unsigned long long* doc_off;         // [W + 1] out
+};
+
+// Row, wave and place in its document of grouped position i.
+__device__ __forceinline__ void ka_wave_doc_row(const KaWaveDocs& d, uint32_t i, uint32_t M, uint32_t& g, int& v, bool& first, bool& last) {
+    g = (uint32_t)d.perm[i];
+    v = d.wave[g];
+    first = i == 0 || d.wave[d.perm[i - 1]] != v;
+    last = i + 1 == M || d.wave[d.perm[i + 1]] != v;
+}
+
+// grid ceil(Q / 256), 256 threads.
+__global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d) {
+    __shared__ uint32_t wsum[8];
+    const uint32_t M = (uint32_t)*d.n_rows;
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    uint32_t n = 0;
+    if (i < M) {
+        uint32_t g;
+        int v;
+        bool first, last;
+        ka_wave_doc_row(d, i, M, g, v, first, last);
+        n = ka_json_row_len<true>(d.p, g, first) + (first ? KA_JSON_HEAD_LEN : 0u) + (last ? KA_JSON_TAIL_LEN : 0u);
+        d.p.rowlen[i] = n;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(KA_FULL, n, o);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        unsigned long long s = 0;
+        for (int w = 0; w < 8; ++w) s += wsum[w];
+        d.blockoff[blockIdx.x] = s;
+    }
+}
+
+// ONE CTA of 1024: v[0..n) to its exclusive scan in place, *total = the sum. 64-bit throughout: 8 bytes per 256 rows lift the
+// 4 GiB limit a fragment of ka_json_scan_kernel has.
+__global__ void __launch_bounds__(1024) ka_wave_doc_scan_kernel(unsigned long long* __restrict__ v, int n, unsigned long long* __restrict__ total) {
+    __shared__ unsigned long long wtot[32];
+    __shared__ unsigned long long carry;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int b0 = 0; b0 < n; b0 += 1024) {
+        const int b = b0 + threadIdx.x;
+        const unsigned long long mine = b < n ? v[b] : 0ull;
+        unsigned long long x = mine;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long y = __shfl_up_sync(KA_FULL, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) wtot[warp] = x;
+        __syncthreads();
+        if (warp == 0) {
+            unsigned long long w = wtot[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned long long y = __shfl_up_sync(KA_FULL, w, o);
+                if (lane >= o) w += y;
+            }
+            wtot[lane] = w;
+        }
+        __syncthreads();
+        const unsigned long long base = carry + (warp > 0 ? wtot[warp - 1] : 0ull);
+        if (b < n) v[b] = base + x - mine;
+        __syncthreads();
+        if (threadIdx.x == 1023) carry = base + x;
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) *total = carry;
+}
+
+// grid ceil(Q / 256), 256 threads, KA_JSON_SMEM_BYTES + 16 of dynamic shared memory. Every grouped row writes its text at its
+// final position, as ka_json_write_kernel does: the 256 rows of a CTA are assembled in shared memory at the 16-byte phase of
+// their destination and stored with coalesced 16-byte stores, and a CTA whose text does not fit (very long topic names) writes
+// straight to global memory. The frame travels with the rows, so a CTA that spans many waves is staged like any other. The
+// first row of wave v writes doc_off[v - 1], the last row of all doc_off[W]. Nothing is written when the text exceeds p.cap.
+__global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs d, const unsigned long long* __restrict__ total) {
+    extern __shared__ __align__(16) unsigned char ka_wdmem[];
+    __shared__ uint32_t wsum[8];
+    const uint32_t M = (uint32_t)*d.n_rows;
+    if (*total > d.p.cap || blockIdx.x * 256u >= M) return;   // CTA-uniform
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const uint32_t n = i < M ? d.p.rowlen[i] : 0u;
+    uint32_t x = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(KA_FULL, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    uint32_t woff = 0, bt = 0;
+    for (int w = 0; w < 8; ++w) { if (w < warp) woff += wsum[w]; bt += wsum[w]; }
+    const unsigned long long at = d.blockoff[blockIdx.x];   // this CTA's text
+    char* dst = d.p.json + at;
+    const uint32_t loc = woff + x - n;                       // my row inside it
+    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15u);
+    const bool staged = mis + bt <= KA_JSON_SMEM_BYTES;
+    if (i < M) {
+        uint32_t g;
+        int v;
+        bool first, last;
+        ka_wave_doc_row(d, i, M, g, v, first, last);
+        char* w = (staged ? reinterpret_cast<char*>(ka_wdmem) + mis : dst) + loc;
+        if (first) {
+            ka_put_str(w, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
+            d.doc_off[v - 1] = at + loc;
+        }
+        ka_json_row_put<true>(d.p, g, w + (first ? KA_JSON_HEAD_LEN : 0), first);
+        if (last) ka_put_str(w + n - KA_JSON_TAIL_LEN, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
+        if (i + 1 == M) d.doc_off[v] = at + loc + n;
+    }
+    if (!staged) return;
+    __syncthreads();
+    const char* stage = reinterpret_cast<const char*>(ka_wdmem) + mis;
+    const uint32_t head = min(bt, (16u - mis) & 15u);       // bytes up to the first 16-byte boundary of dst
+    for (uint32_t k = threadIdx.x; k < head; k += 256) dst[k] = stage[k];
+    const uint32_t body = (bt - head) >> 4;
+    const uint4* s4 = reinterpret_cast<const uint4*>(stage + head);
+    uint4* d4 = reinterpret_cast<uint4*>(dst + head);
+    for (uint32_t k = threadIdx.x; k < body; k += 256) d4[k] = s4[k];
+    for (uint32_t k = head + (body << 4) + threadIdx.x; k < bt; k += 256) dst[k] = stage[k];
+}

@@ -15,6 +15,7 @@
 //   kassign::solveClustersJson                        <->  the same fleet, with each cluster's org.json text built on the device
 //   kassign::scoreClusters                            <->  the same fleet, reduced on the device to what each cluster would move
 //                                                          and how evenly it spreads replicas and leaders
+//   kassign::planWavesJson                            <->  planWaves with every wave's document built on the device
 //   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
 //                                                          receives more than a budget, one document per wave
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
@@ -278,32 +279,17 @@ public:
     // the weight of every partition, as scoreTopicsCandidates takes them.
     WavePlan planWaves(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                        const std::vector<std::map<int, int64_t>>& weights = {}) {
-        if (proposed.size() != topics.size()) throw std::invalid_argument("one proposed topic per topic");
-        if (!weights.empty() && weights.size() != topics.size()) throw std::invalid_argument("one weight map per topic");
         const Flat f = flatten(topics, -1);
+        const ProposedRows p = proposedRows(topics, proposed, weights);
         const size_t Q = f.partId.size();
-        int stride = 1;
-        for (const TopicOutput& t : proposed)
-            for (const auto& e : t.assignment) stride = std::max(stride, (int)e.second.size());
-        std::vector<int32_t> newLen(Q, 0), newBroker(Q * stride, -1);
-        std::vector<int64_t> w;
-        size_t g = 0;
-        for (size_t t = 0; t < topics.size(); ++t)
-            for (const auto& e : topics[t].current) {
-                const std::vector<int>& l = proposed[t].assignment.at(e.first);
-                newLen[g] = (int32_t)l.size();
-                std::copy(l.begin(), l.end(), newBroker.begin() + g * stride);
-                if (!weights.empty()) w.push_back(weights[t].at(e.first));
-                ++g;
-            }
         WavePlan res{};
         std::vector<int32_t> wave(Q, 0);
         int32_t W = 0;
         // W never exceeds Q: min(Q, 64 k) summaries (40 bytes each) hold every plan in one call, but one of more than 64 k waves
         res.summary.resize(std::max<size_t>(1, std::min<size_t>(Q, 1 << 16)));
         auto plan = [&](int32_t* waveOut) {
-            return ka_plan_waves(ctx_, (int64_t)Q, f.repOff.data(), f.cur.data(), stride, newLen.data(), newBroker.data(),
-                                 w.empty() ? nullptr : w.data(), maxBrokerIn, waveOut, &W, res.summary.data(),
+            return ka_plan_waves(ctx_, (int64_t)Q, f.repOff.data(), f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(),
+                                 p.w.empty() ? nullptr : p.w.data(), maxBrokerIn, waveOut, &W, res.summary.data(),
                                  (int32_t)res.summary.size(), &res.status);
         };
         if (plan(wave.data()) == KA_OK && W > (int32_t)res.summary.size()) {
@@ -322,11 +308,21 @@ public:
                     doc.push_back(TopicOutput{f.names[t], {}});
                     lastTopic[wave[r] - 1] = t;
                 }
-                doc.back().assignment[f.partId[r]] = std::vector<int>(newBroker.begin() + r * stride,
-                                                                      newBroker.begin() + r * stride + newLen[r]);
+                doc.back().assignment[f.partId[r]] = std::vector<int>(p.newBroker.begin() + r * p.stride,
+                                                                      p.newBroker.begin() + r * p.stride + p.newLen[r]);
             }
         return res;
     }
+
+    // planWaves with every wave's document built on the device (ka_plan_waves_json): docs[v] equals
+    // newAssignmentJson(planWaves(...).waves[v]). Topic names that org.json would escape take exactly that host path instead.
+    struct WaveDocs {
+        ka_status status;   // re-throw with throwForStatus; on an error summary and docs are empty
+        std::vector<ka_wave_summary> summary;
+        std::vector<std::string> docs;
+    };
+    WaveDocs planWavesJson(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                           const std::vector<std::map<int, int64_t>>& weights = {});
 
     // The KAG:172-186 loop and its "NEW ASSIGNMENT" text in one device call (ka_solve_json): only the text crosses PCIe.
     // Same solve and exceptions as solveTopics; the text equals newAssignmentJson(solveTopics(...)). Topic names that
@@ -347,6 +343,36 @@ private:
         std::vector<int64_t> partOff, repOff;
         int stride = 1;
     };
+    // The proposed lists of a wave plan as ka_plan_waves takes them, in the row order of flatten(topics): newLen [Q], newBroker
+    // [Q][stride] (stride = the longest proposed list, at least 1) and w [Q] (empty = 1 per row).
+    struct ProposedRows {
+        int stride = 1;
+        std::vector<int32_t> newLen, newBroker;
+        std::vector<int64_t> w;
+    };
+    static ProposedRows proposedRows(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
+                                     const std::vector<std::map<int, int64_t>>& weights) {
+        if (proposed.size() != topics.size()) throw std::invalid_argument("one proposed topic per topic");
+        if (!weights.empty() && weights.size() != topics.size()) throw std::invalid_argument("one weight map per topic");
+        ProposedRows p;
+        size_t Q = 0;
+        for (size_t t = 0; t < topics.size(); ++t) {
+            Q += topics[t].current.size();
+            for (const auto& e : proposed[t].assignment) p.stride = std::max(p.stride, (int)e.second.size());
+        }
+        p.newLen.assign(Q, 0);
+        p.newBroker.assign(Q * p.stride, -1);
+        size_t g = 0;
+        for (size_t t = 0; t < topics.size(); ++t)
+            for (const auto& e : topics[t].current) {
+                const std::vector<int>& l = proposed[t].assignment.at(e.first);
+                p.newLen[g] = (int32_t)l.size();
+                std::copy(l.begin(), l.end(), p.newBroker.begin() + g * p.stride);
+                if (!weights.empty()) p.w.push_back(weights[t].at(e.first));
+                ++g;
+            }
+        return p;
+    }
     static Flat flatten(const std::vector<TopicInput>& topics, int desiredReplicationFactor) {
         const int T = (int)topics.size();
         Flat f;
@@ -588,6 +614,42 @@ inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicIn
     ka_solve_json(ctx_, T, f.hash.data(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), desiredReplicationFactor,
                   names.data(), nameOff.data(), json.get(), cap, &bytes, &st);
     return std::string(json.get(), (size_t)bytes);
+}
+
+inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJson(const std::vector<TopicInput>& topics,
+                                                                      const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                                                                      const std::vector<std::map<int, int64_t>>& weights) {
+    for (const auto& t : topics)
+        if (needsJsonEscape(t.name)) {   // the host emitter over the waves of planWaves
+            const WavePlan plan = planWaves(topics, proposed, maxBrokerIn, weights);
+            WaveDocs res{plan.status, plan.summary, {}};
+            for (const auto& wave : plan.waves) res.docs.push_back(newAssignmentJson(wave));
+            return res;
+        }
+    const Flat f = flatten(topics, -1);
+    const ProposedRows p = proposedRows(topics, proposed, weights);
+    const size_t Q = f.partId.size();
+    std::string names;
+    std::vector<int64_t> nameOff(1, 0);
+    int64_t cap = 0;   // documented in kassign.h: per row 79 + 12·stride + its topic's name length
+    for (size_t t = 0; t < f.names.size(); ++t) {
+        names += f.names[t];
+        nameOff.push_back((int64_t)names.size());
+        cap += (f.partOff[t + 1] - f.partOff[t]) * (79 + 12 * (int64_t)p.stride + (int64_t)f.names[t].size());
+    }
+    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
+    std::vector<int64_t> docOff(Q + 1, 0);
+    WaveDocs res{};
+    res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
+    int32_t W = 0;
+    ka_plan_waves_json(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), p.stride,
+                       p.newLen.data(), p.newBroker.data(), p.w.empty() ? nullptr : p.w.data(), maxBrokerIn, names.data(),
+                       nameOff.data(), json.get(), cap, docOff.data(), nullptr, &W, res.summary.data(), (int32_t)res.summary.size(),
+                       &res.status);
+    if (res.status.code != KA_OK) return WaveDocs{res.status, {}, {}};
+    res.summary.resize(W);
+    for (int32_t v = 0; v < W; ++v) res.docs.emplace_back(json.get() + docOff[v], (size_t)(docOff[v + 1] - docOff[v]));
+    return res;
 }
 
 // Kafka 0.10 ZkUtils.formatAsReassignmentJson shape (used for "CURRENT ASSIGNMENT:", KAG:103-111): scala Map literals keep
