@@ -698,39 +698,67 @@ SubBlock sub_block(const StageDesc& d, int j, int nsub) {
     return b;
 }
 
+// A text pass over rows [row0, row0 + rows) of out / out_len (stride S), laid out as T topics (ragged: part_off and, when
+// given, part_id), printed with the ctx's name slab into its text buffer, cap bytes of it.
+KaJsonParams json_params(ka_ctx* c, const int32_t* out, const int32_t* out_len, int S, int T, const int64_t* part_off,
+                         const int32_t* part_id, int64_t row0, int64_t rows, unsigned long long cap) {
+    KaJsonParams p{};
+    p.Q = (uint32_t)rows;
+    p.row0 = (uint32_t)row0;
+    p.T = T;
+    p.part_off = part_off;
+    p.part_id = part_id;
+    p.name_off = c->d_name_off.as<int64_t>();
+    p.names = c->d_names.as<char>();
+    p.out = out + row0 * S;
+    p.out_len = out_len + row0;
+    p.S = S;
+    p.rowlen = c->d_json_rowlen.as<uint32_t>() + row0;
+    p.json = c->d_json.as<char>();
+    p.cap = cap;
+    return p;
+}
+
+// Fragment k of a solve's text (block d, rows in io): rows [row0, row0 + rows), their block sums, and slot k of the running
+// text state.
+KaJsonParams json_fragment(ka_ctx* c, const StageDesc& d, const SolveCall& io, int64_t row0, int64_t rows, int k) {
+    KaJsonParams p = json_params(c, io.d_out, io.d_out_len, d.S, d.T, d.d_part_off, io.d_part_id, row0, rows,
+                                 (unsigned long long)c->d_json.cap);
+    p.blocksum = c->d_json_blocksum.as<uint32_t>() + (row0 / 256) + k;
+    p.total = c->d_json_state.as<unsigned long long>();
+    p.frag = p.total + 2 + 2 * k;
+    return p;
+}
+
+// The length pass and the scan of fragment p on s (SEG: of a fleet, with its document table sg).
+template <bool SEG>
+void enq_json_lengths(cudaStream_t s, const KaJsonParams& p, const KaJsonSegs& sg) {
+    const int nblocks = (int)((p.Q + 255) / 256);
+    if (nblocks > 0) ka_json_len_kernel<SEG><<<nblocks, 256, 0, s>>>(p, sg);
+    ka_json_scan_kernel<<<1, 1024, 0, s>>>(p, nblocks);
+}
+
+// A write pass of the text passes: `grid` CTAs of 256 threads with the shared-memory stage, on s.
+template <typename K, typename... A>
+cudaError_t enq_json_write(K kernel, unsigned grid, cudaStream_t s, const A&... args) {
+    const cudaError_t e = allow_smem(kernel, KA_JSON_SMEM_BYTES + 16);
+    if (e == cudaSuccess) kernel<<<grid, 256, KA_JSON_SMEM_BYTES + 16, s>>>(args...);
+    return e;
+}
+
 // KAG:169-186 for a finished range of rows (sub-block b of block d): rows -> JSON text at the running offset of d_json, on c->sj.
 int enq_json_rows(ka_ctx* c, cudaStream_t s_done, SolveCall& io, const StageDesc& d, const SubBlock& b, bool first, bool last) {
     const int k = io.json_blocks;
     if (k >= KA_MAX_JSON_FRAGS) return KA_ERR_LIMIT;
-    const int64_t row0 = d.q0 + b.r0, rows = b.rq;
     KA_CUDA(cudaEventRecord(c->ev_json_in[k], s_done));
     KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_json_in[k], 0));
-    KaJsonParams p{};
-    p.Q = (uint32_t)rows;
-    p.row0 = (uint32_t)row0;
+    KaJsonParams p = json_fragment(c, d, io, d.q0 + b.r0, b.rq, k);
     p.P = std::max(d.P, 1);
     p.topic0 = d.topic_base + b.t0;
-    p.T = d.T;
-    p.part_off = d.d_part_off;
-    p.part_id = io.d_part_id;
-    p.name_off = c->d_name_off.as<int64_t>();
-    p.names = c->d_names.as<char>();
-    p.out = io.d_out + row0 * d.S;
-    p.out_len = io.d_out_len + row0;
-    p.S = d.S;
-    p.rowlen = c->d_json_rowlen.as<uint32_t>() + row0;
-    p.blocksum = c->d_json_blocksum.as<uint32_t>() + (row0 / 256) + k;
-    p.total = c->d_json_state.as<unsigned long long>();
-    p.frag = c->d_json_state.as<unsigned long long>() + 2 + 2 * k;
-    p.json = c->d_json.as<char>();
-    p.cap = (unsigned long long)c->d_json.cap;
     p.first = first;
     p.last = last;
-    const int nblocks = (int)((rows + 255) / 256);
-    if (nblocks > 0) ka_json_len_kernel<false><<<nblocks, 256, 0, c->sj>>>(p, KaJsonSegs{});
-    ka_json_scan_kernel<<<1, 1024, 0, c->sj>>>(p, nblocks);
-    KA_CUDA(allow_smem(ka_json_write_kernel<false>, KA_JSON_SMEM_BYTES + 16));
-    ka_json_write_kernel<false><<<std::max(nblocks, 1), 256, KA_JSON_SMEM_BYTES + 16, c->sj>>>(p, KaJsonSegs{});
+    enq_json_lengths<false>(c->sj, p, KaJsonSegs{});
+    KA_CUDA(enq_json_write(ka_json_write_kernel<false>, std::max((p.Q + 255) / 256, 1u), c->sj, p, KaJsonSegs{}));
     KA_CUDA(cudaGetLastError());
     KA_CUDA(cudaMemcpyAsync(c->h_frag + 2 * k, p.frag, 16, cudaMemcpyDeviceToHost, c->sj));
     KA_CUDA(cudaEventRecord(c->ev_json_scan[k], c->sj));
@@ -1728,18 +1756,29 @@ int32_t ka_solve_dense(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t 
     return finish(c, c->stream, st, true);
 }
 
-// Device buffers of a JSON solve, and its topic names H2D (on c->sj, ahead of the first fragment).
-static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, const int64_t* name_off, int64_t json_cap) {
+// The name slab of a text pass over T topics and Q rows H2D on s: names and name_off, and the rows' partition ids when given.
+static int upload_names(ka_ctx* c, cudaStream_t s, int32_t T, int64_t Q, const char* names, const int64_t* name_off,
+                        const int32_t* part_id) {
     const int64_t name_bytes = T > 0 ? name_off[T] : 0;
-    KA_CUDA(c->d_json.reserve((size_t)json_cap));
     KA_CUDA(c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)));
     KA_CUDA(c->d_name_off.reserve((size_t)(T + 1) * 8));
+    if (part_id) KA_CUDA(c->d_part_id.reserve((size_t)Q * 4));
+    if (name_bytes > 0) KA_CUDA(cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, s));
+    if (T > 0) KA_CUDA(cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s));
+    if (part_id && Q > 0) KA_CUDA(cudaMemcpyAsync(c->d_part_id.p, part_id, (size_t)Q * 4, cudaMemcpyHostToDevice, s));
+    return KA_OK;
+}
+
+// Device buffers of a JSON solve, and its topic names H2D (on c->sj, ahead of the first fragment; the solve uploads the
+// partition ids).
+static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, const int64_t* name_off, int64_t json_cap) {
+    KA_CUDA(c->d_json.reserve((size_t)json_cap));
     KA_CUDA(c->d_json_rowlen.reserve((size_t)std::max<int64_t>(Q, 1) * 4));
     KA_CUDA(c->d_json_blocksum.reserve((size_t)(Q / 256 + 2 * KA_MAX_JSON_FRAGS) * 4));
     KA_CUDA(c->d_json_state.reserve((2 + 2 * KA_MAX_JSON_FRAGS) * 8));
+    const int rc = upload_names(c, c->sj, T, Q, names, name_off, nullptr);
+    if (rc != KA_OK) return rc;
     KA_CUDA(cudaMemsetAsync(c->d_json_state.p, 0, (2 + 2 * KA_MAX_JSON_FRAGS) * 8, c->sj));
-    if (name_bytes > 0) KA_CUDA(cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, c->sj));
-    if (T > 0) KA_CUDA(cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, c->sj));
     return KA_OK;
 }
 
@@ -2132,39 +2171,16 @@ static KaJsonSegs fleet_segs(ka_ctx* c, int K) {
 // emit: the length pass and the scan over fragments of the call's rows, the document table, then the write pass. doc_off
 // comes back to h_doc.
 static int enq_fleet_json(ka_ctx* c, cudaStream_t s, const StageDesc& d, const SolveCall& io, int K, unsigned long long* h_doc) {
-    KaJsonParams p{};
-    p.part_off = d.d_part_off;
-    p.T = d.T;
-    p.part_id = io.d_part_id;
-    p.name_off = c->d_name_off.as<int64_t>();
-    p.names = c->d_names.as<char>();
-    p.S = d.S;
-    p.total = c->d_json_state.as<unsigned long long>();
-    p.json = c->d_json.as<char>();
-    p.cap = (unsigned long long)c->d_json.cap;
     const KaJsonSegs sg = fleet_segs(c, K);
     // fragments of whole 256-row blocks, as in a ragged single solve; their count depends on the rows alone
     const int64_t Q = d.Q, step = json_fragment_rows(Q);
     std::vector<KaJsonParams> frags;
     for (int64_t r = 0; r < Q; r += step) {
-        const int k = (int)frags.size();
-        KaJsonParams fp = p;
-        fp.Q = (uint32_t)std::min(step, Q - r);
-        fp.row0 = (uint32_t)r;
-        fp.out = io.d_out + r * d.S;
-        fp.out_len = io.d_out_len + r;
-        fp.rowlen = c->d_json_rowlen.as<uint32_t>() + r;
-        fp.blocksum = c->d_json_blocksum.as<uint32_t>() + (r / 256) + k;
-        fp.frag = c->d_json_state.as<unsigned long long>() + 2 + 2 * k;
-        const int nblocks = (int)((fp.Q + 255) / 256);
-        ka_json_len_kernel<true><<<nblocks, 256, 0, s>>>(fp, sg);
-        ka_json_scan_kernel<<<1, 1024, 0, s>>>(fp, nblocks);
-        frags.push_back(fp);
+        frags.push_back(json_fragment(c, d, io, r, std::min(step, Q - r), (int)frags.size()));
+        enq_json_lengths<true>(s, frags.back(), sg);
     }
-    ka_json_docs_kernel<<<1, KA_JSON_MAX_SEGS, 0, s>>>(p, sg);
-    KA_CUDA(allow_smem(ka_json_write_kernel<true>, KA_JSON_SMEM_BYTES + 16));
-    for (const KaJsonParams& fp : frags)
-        ka_json_write_kernel<true><<<(unsigned)((fp.Q + 255) / 256), 256, KA_JSON_SMEM_BYTES + 16, s>>>(fp, sg);
+    ka_json_docs_kernel<<<1, KA_JSON_MAX_SEGS, 0, s>>>(json_fragment(c, d, io, 0, Q, 0), sg);   // reads json and cap alone
+    for (const KaJsonParams& fp : frags) KA_CUDA(enq_json_write(ka_json_write_kernel<true>, (fp.Q + 255) / 256, s, fp, sg));
     KA_CUDA(cudaGetLastError());
     c->launches += 3 * (int64_t)frags.size() + 1;
     KA_CUDA(cudaMemcpyAsync(h_doc, sg.doc_off, (size_t)(K + 1) * 8, cudaMemcpyDeviceToHost, s));
@@ -2570,42 +2586,25 @@ int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const 
     cudaStream_t s = c->stream;
     const size_t q = (size_t)Q;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
-    const int64_t name_bytes = name_off[T];
     const int64_t cap = std::min(json_cap, bound);
     const size_t tiles = (size_t)(Q + KA_WAVE_SORT_MIN_TILE - 1) / KA_WAVE_SORT_MIN_TILE;   // at least the passes' tiles
-    if (c->d_part_off.reserve((size_t)(T + 1) * 8) || (part_id && c->d_part_id.reserve(q * 4)) ||
-        c->d_names.reserve((size_t)std::max<int64_t>(name_bytes, 1)) || c->d_name_off.reserve((size_t)(T + 1) * 8) ||
-        c->d_json.reserve((size_t)std::max<int64_t>(cap, 1)) || c->d_json_rowlen.reserve(q * 4) ||
-        c->d_json_blocksum.reserve((size_t)nblk * 8) || c->d_wv_perm.reserve(2 * q * 4) ||
-        c->d_wv_hist.reserve((2 * KA_WAVE_SORT_DIGITS * tiles + 1) * 4) || c->d_wv_doc.reserve(((size_t)W + 2) * 8))
-        return set_status(st, KA_ERR_CUDA);
-    if (cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s) ||
-        (part_id && cudaMemcpyAsync(c->d_part_id.p, part_id, q * 4, cudaMemcpyHostToDevice, s)) ||
-        (name_bytes > 0 && cudaMemcpyAsync(c->d_names.p, names, (size_t)name_bytes, cudaMemcpyHostToDevice, s)) ||
-        cudaMemcpyAsync(c->d_name_off.p, name_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s))
+    if (c->d_part_off.reserve((size_t)(T + 1) * 8) || c->d_json.reserve((size_t)std::max<int64_t>(cap, 1)) ||
+        c->d_json_rowlen.reserve(q * 4) || c->d_json_blocksum.reserve((size_t)nblk * 8) || c->d_wv_perm.reserve(2 * q * 4) ||
+        c->d_wv_hist.reserve((2 * KA_WAVE_SORT_DIGITS * tiles + 1) * 4) || c->d_wv_doc.reserve(((size_t)W + 2) * 8) ||
+        upload_names(c, s, T, Q, names, name_off, part_id) != KA_OK ||
+        cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s))
         return set_status(st, KA_ERR_CUDA);
     KaWaveDocs d{};
+    d.p = json_params(c, c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>(), stride, T, c->d_part_off.as<int64_t>(),
+                      part_id ? c->d_part_id.as<int32_t>() : nullptr, 0, Q, (unsigned long long)cap);
     d.perm = enq_wave_group(c, s, Q, W, d.n_rows);
     d.wave = c->d_wv_wave.as<int32_t>();
     d.blockoff = c->d_json_blocksum.as<unsigned long long>();
     unsigned long long* d_total = c->d_wv_doc.as<unsigned long long>();
     d.doc_off = d_total + 1;
-    d.p.Q = (uint32_t)Q;
-    d.p.T = T;
-    d.p.part_off = c->d_part_off.as<int64_t>();
-    d.p.part_id = part_id ? c->d_part_id.as<int32_t>() : nullptr;
-    d.p.name_off = c->d_name_off.as<int64_t>();
-    d.p.names = c->d_names.as<char>();
-    d.p.out = c->d_out.as<int32_t>();
-    d.p.out_len = c->d_out_len.as<int32_t>();
-    d.p.S = stride;
-    d.p.rowlen = c->d_json_rowlen.as<uint32_t>();
-    d.p.json = c->d_json.as<char>();
-    d.p.cap = (unsigned long long)cap;
-    if (allow_smem(ka_wave_doc_write_kernel, KA_JSON_SMEM_BYTES + 16) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
     ka_wave_doc_len_kernel<<<nblk, 256, 0, s>>>(d);
     ka_wave_doc_scan_kernel<<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total);
-    ka_wave_doc_write_kernel<<<nblk, 256, KA_JSON_SMEM_BYTES + 16, s>>>(d, d_total);
+    if (enq_json_write(ka_wave_doc_write_kernel, nblk, s, d, d_total) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
     c->launches += 3;
     unsigned long long total = 0;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, s) || cudaStreamSynchronize(s))

@@ -156,6 +156,45 @@ __device__ __forceinline__ long long ka_group_sum64(long long v, unsigned grp) {
     return (long long)(a0 + (a1 << 22) + (a2 << 43));
 }
 
+// Exclusive scan of in[0..n) by ONE CTA of 1024 threads, in rounds of 1024 elements: out[i] = carry + in[0] + .. + in[i - 1]
+// (in T, then narrowed to Out). Returns carry + the sum of all n, in every thread. in and out may be the same array.
+template <typename T, typename In, typename Out>
+__device__ __forceinline__ T ka_cta_scan(const In* in, Out* out, int n, T carry) {
+    __shared__ T wtot[32];
+    __shared__ T run;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (threadIdx.x == 0) run = carry;
+    __syncthreads();
+    for (int b0 = 0; b0 < n; b0 += 1024) {
+        const int b = b0 + threadIdx.x;
+        const T v = b < n ? (T)in[b] : (T)0;
+        T x = v;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const T y = __shfl_up_sync(KA_FULL, x, o);
+            if (lane >= o) x += y;
+        }
+        if (lane == 31) wtot[warp] = x;
+        __syncthreads();
+        if (warp == 0) {
+            T w = wtot[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const T y = __shfl_up_sync(KA_FULL, w, o);
+                if (lane >= o) w += y;
+            }
+            wtot[lane] = w;  // inclusive over warps
+        }
+        __syncthreads();
+        const T base = run + (warp > 0 ? wtot[warp - 1] : (T)0);
+        if (b < n) out[b] = (Out)(base + x - v);
+        __syncthreads();
+        if (threadIdx.x == 1023) run = base + x;
+        __syncthreads();
+    }
+    return run;
+}
+
 // Rotation bits of one topic: (|hash| % k) for k = 2..8 packed above the 4-bit length (KAS:190 applied
 // to the remaining-set sizes of KAS:267). Layout: len[0:4) k2[4] k3[5:7) k4[7:9) k5[9:12) k6[12:15) k7[15:18) k8[18:21)
 __device__ __forceinline__ uint32_t ka_rot_bits(uint32_t habs) {

@@ -88,23 +88,21 @@ __device__ __forceinline__ void ka_json_row_key(const KaJsonParams& p, uint32_t 
     }
 }
 
-// Text of row q of the fragment. Every row but the first of its document has a leading comma: the first of the run, or with
-// SEG the first of its cluster (`first`).
-template <bool SEG>
-__device__ __forceinline__ uint32_t ka_json_row_len(const KaJsonParams& p, uint32_t q, bool first) {
+// Text of row q of the fragment, with a leading comma when `comma`: every row but the first of its document has one.
+__device__ __forceinline__ uint32_t ka_json_row_len(const KaJsonParams& p, uint32_t q, bool comma) {
     int t, part;
     ka_json_row_key(p, q, t, part);
     const int len = p.out_len[q];
-    uint32_t n = ((SEG ? !first : p.row0 + q > 0) ? 1u : 0u) + 13u + ka_ndigits(part) + 13u + 11u + (uint32_t)(p.name_off[t + 1] - p.name_off[t]) + 2u;
+    uint32_t n = (comma ? 1u : 0u) + 13u + ka_ndigits(part) + 13u + 11u + (uint32_t)(p.name_off[t + 1] - p.name_off[t]) + 2u;
     for (int i = 0; i < len; ++i) n += ka_ndigits(p.out[(size_t)q * p.S + i]) + (i ? 1u : 0u);
     return n;
 }
-template <bool SEG>
-__device__ __forceinline__ void ka_json_row_put(const KaJsonParams& p, uint32_t q, char* w, bool first) {
+// Writes that text at w; returns its end.
+__device__ __forceinline__ char* ka_json_row_put(const KaJsonParams& p, uint32_t q, char* w, bool comma) {
     int t, part;
     ka_json_row_key(p, q, t, part);
     const int len = p.out_len[q];
-    if (SEG ? !first : p.row0 + q > 0) *w++ = ',';
+    if (comma) *w++ = ',';
     w = ka_put_str(w, "{\"partition\":", 13);
     w = ka_put_int(w, part);
     w = ka_put_str(w, ",\"replicas\":[", 13);
@@ -114,7 +112,55 @@ __device__ __forceinline__ void ka_json_row_put(const KaJsonParams& p, uint32_t 
     }
     w = ka_put_str(w, "],\"topic\":\"", 11);
     w = ka_put_str(w, p.names + p.name_off[t], (int)(p.name_off[t + 1] - p.name_off[t]));
-    ka_put_str(w, "\"}", 2);
+    return ka_put_str(w, "\"}", 2);
+}
+
+// The row texts of a CTA of 256 threads, n bytes per thread. ka_cta256_sum: the CTA's bytes, in thread 0. ka_cta256_prefix:
+// this thread's offset in the CTA's text, and (total) the CTA's bytes, in every thread.
+__device__ __forceinline__ unsigned long long ka_cta256_sum(uint32_t n) {
+    __shared__ uint32_t wsum[8];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(KA_FULL, n, o);
+    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = n;
+    __syncthreads();
+    unsigned long long s = 0;
+    if (threadIdx.x == 0)
+        for (int i = 0; i < 8; ++i) s += wsum[i];
+    return s;
+}
+__device__ __forceinline__ uint32_t ka_cta256_prefix(uint32_t n, uint32_t& total) {
+    __shared__ uint32_t wsum[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    uint32_t x = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t y = __shfl_up_sync(KA_FULL, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    uint32_t woff = 0;
+    total = 0;
+    for (int i = 0; i < 8; ++i) { if (i < warp) woff += wsum[i]; total += wsum[i]; }
+    return woff + x - n;
+}
+
+// The write passes assemble a CTA's text in shared memory (KA_JSON_SMEM_BYTES, + 16 for the phase) at the same 16-byte phase
+// as its destination, then store it with coalesced 16-byte stores; a CTA whose text does not fit (very long topic names)
+// writes straight to global memory instead.
+#define KA_JSON_SMEM_BYTES (64 * 1024)
+
+// Every thread of a CTA of 256, once each has written its row into stage: the bt bytes at stage to dst, as the bytes up to
+// dst's first 16-byte boundary, a uint4 body, then the tail bytes.
+__device__ __forceinline__ void ka_json_store_staged(char* dst, const char* stage, uint32_t bt) {
+    __syncthreads();
+    const uint32_t head = min(bt, (0u - (uint32_t)reinterpret_cast<uintptr_t>(dst)) & 15u);
+    for (uint32_t i = threadIdx.x; i < head; i += 256) dst[i] = stage[i];
+    const uint32_t body = (bt - head) >> 4;
+    const uint4* s4 = reinterpret_cast<const uint4*>(stage + head);
+    uint4* d4 = reinterpret_cast<uint4*>(dst + head);
+    for (uint32_t i = threadIdx.x; i < body; i += 256) d4[i] = s4[i];
+    for (uint32_t i = head + (body << 4) + threadIdx.x; i < bt; i += 256) dst[i] = stage[i];
 }
 
 // Segmented passes: the clusters' first rows, and (live != null) whether each cluster is live, in shared memory.
@@ -134,11 +180,11 @@ __device__ __forceinline__ int ka_json_seg_of(const int64_t* row0, int K, int64_
     return lo;
 }
 
-// pass 1: text length of every row + per-block sums. SEG: the rows of a dead cluster are empty, the first row of every
-// cluster has no leading comma, and every cluster's bytes are summed into sg.bytes (one atomic per warp and cluster).
+// pass 1: text length of every row + per-block sums. The first row of the run has no leading comma; SEG: the first row of
+// every cluster has none, the rows of a dead cluster are empty, and every cluster's bytes are summed into sg.bytes (one atomic
+// per warp and cluster).
 template <bool SEG>
 __global__ void __launch_bounds__(256) ka_json_len_kernel(const KaJsonParams p, const KaJsonSegs sg) {
-    __shared__ uint32_t wsum[8];
     const uint32_t q = blockIdx.x * 256u + threadIdx.x;
     uint32_t n;
     if constexpr (SEG) {
@@ -148,65 +194,28 @@ __global__ void __launch_bounds__(256) ka_json_len_kernel(const KaJsonParams p, 
         __syncthreads();
         const int64_t g = (int64_t)p.row0 + q;
         const int k = q < p.Q ? ka_json_seg_of(row0, sg.K, g) : -1;
-        n = k >= 0 && live[k] ? ka_json_row_len<true>(p, q, g == row0[k]) : 0u;
+        n = k >= 0 && live[k] ? ka_json_row_len(p, q, g != row0[k]) : 0u;
         const unsigned grp = __match_any_sync(KA_FULL, k);
         const unsigned sum = __reduce_add_sync(grp, n);
         if (k >= 0 && sum > 0 && (int)(threadIdx.x & 31) == __ffs(grp) - 1) atomicAdd(sg.bytes + k, (unsigned long long)sum);
     } else {
-        n = q < p.Q ? ka_json_row_len<false>(p, q, false) : 0u;
+        n = q < p.Q ? ka_json_row_len(p, q, p.row0 + q > 0) : 0u;
     }
     if (q < p.Q) p.rowlen[q] = n;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(KA_FULL, n, o);
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = n;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t s = 0;
-        for (int i = 0; i < 8; ++i) s += wsum[i];
-        p.blocksum[blockIdx.x] = s;
-    }
+    const unsigned long long bytes = ka_cta256_sum(n);
+    if (threadIdx.x == 0) p.blocksum[blockIdx.x] = (uint32_t)bytes;
 }
 
-// pass 2 (one CTA): exclusive scan of the block sums, placed after the bytes written so far; reserves header / trailer
+// pass 2 (one CTA): exclusive scan of the block sums, relative to the fragment start (a fragment is < 4 GiB), after the
+// header's reserve; the fragment, with its trailer's, is placed after the bytes written so far
 __global__ void __launch_bounds__(1024) ka_json_scan_kernel(const KaJsonParams p, int nblocks) {
-    __shared__ unsigned long long wtot[32];
-    __shared__ unsigned long long carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = *p.total + (p.first ? KA_JSON_HEAD_LEN : 0);
-    __syncthreads();
-    const unsigned long long base0 = *p.total;
-    for (int b0 = 0; b0 < nblocks; b0 += 1024) {
-        const int b = b0 + threadIdx.x;
-        const unsigned long long v = b < nblocks ? p.blocksum[b] : 0ull;
-        unsigned long long x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(KA_FULL, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) wtot[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            unsigned long long w = wtot[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned long long y = __shfl_up_sync(KA_FULL, w, o);
-                if (lane >= o) w += y;
-            }
-            wtot[lane] = w;
-        }
-        __syncthreads();
-        const unsigned long long base = carry + (warp > 0 ? wtot[warp - 1] : 0ull);
-        if (b < nblocks) p.blocksum[b] = (uint32_t)(base + x - v - base0);   // relative to the fragment start (a fragment is < 4 GiB)
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = base + x;
-        __syncthreads();
-    }
+    const unsigned long long base = *p.total;   // loaded ahead of the scan, off the path to the stores below
+    const unsigned long long bytes =
+        ka_cta_scan(p.blocksum, p.blocksum, nblocks, (unsigned long long)(p.first ? KA_JSON_HEAD_LEN : 0)) + (p.last ? KA_JSON_TAIL_LEN : 0);
     if (threadIdx.x == 0) {
-        const unsigned long long end = carry + (p.last ? KA_JSON_TAIL_LEN : 0);
-        p.frag[0] = base0;
-        p.frag[1] = end - base0;
-        *p.total = end;
+        p.frag[0] = base;
+        p.frag[1] = bytes;
+        *p.total = base + bytes;
     }
 }
 
@@ -243,31 +252,19 @@ __global__ void __launch_bounds__(KA_JSON_MAX_SEGS) ka_json_docs_kernel(const Ka
     }
 }
 
-// pass 3: every row writes its text at its final position. The 256 rows of a block are assembled in shared memory (at the
-// same 16-byte phase as their destination) and copied out with coalesced 16-byte stores; blocks whose text does not fit
-// (very long topic names) write straight to global memory. SEG: a row's position moves by its cluster's shift, so a block
-// whose rows span documents (the shift differs at its ends) also writes straight to global memory.
-#define KA_JSON_SMEM_BYTES (64 * 1024)
+// pass 3: every row writes its text at its final position, the 256 rows of a block through the shared-memory stage.
+// SEG: a row's position moves by its cluster's shift, so a block whose rows span documents (the shift differs at its ends)
+// writes straight to global memory.
 template <bool SEG>
 __global__ void __launch_bounds__(256) ka_json_write_kernel(const KaJsonParams p, const KaJsonSegs sg) {
     extern __shared__ __align__(16) unsigned char ka_jsmem[];
-    __shared__ uint32_t wsum[8];
     if (SEG ? sg.doc_off[sg.K] > p.cap : p.frag[0] + p.frag[1] > p.cap) return;   // caller's buffer too small (uniform)
     const uint32_t q = blockIdx.x * 256u + threadIdx.x;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t n = q < p.Q ? p.rowlen[q] : 0u;
-    uint32_t x = n;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(KA_FULL, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) wsum[warp] = x;
-    __syncthreads();
-    uint32_t woff = 0, bt = 0;
-    for (int i = 0; i < 8; ++i) { if (i < warp) woff += wsum[i]; bt += wsum[i]; }
+    uint32_t bt;
+    const uint32_t loc = ka_cta256_prefix(n, bt);               // my row inside the block's text
     uint32_t shift = 0, bshift = 0;   // position shift of my row and of the block's first row
-    bool staged = true, first = false;
+    bool staged = true, comma = p.row0 + q > 0;
     if constexpr (SEG) {
         __shared__ int64_t row0[KA_JSON_MAX_SEGS + 1];
         ka_json_stage_segs(sg, row0, nullptr);
@@ -279,27 +276,19 @@ __global__ void __launch_bounds__(256) ka_json_write_kernel(const KaJsonParams p
             const int64_t g = (int64_t)p.row0 + q;
             const int k = ka_json_seg_of(row0, sg.K, g);
             shift = sg.shift[k];
-            first = g == row0[k];
+            comma = g != row0[k];
         }
     }
     char* frag = p.json + p.frag[0];
     char* dst = frag + p.blocksum[blockIdx.x] + bshift;        // this block's text
-    const uint32_t loc = woff + x - n;                           // my row inside it
     const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15u);
     // SEG: a dead cluster's rows are empty and never read
     if (staged && mis + bt <= KA_JSON_SMEM_BYTES) {
         char* stage = reinterpret_cast<char*>(ka_jsmem) + mis;
-        if (SEG ? n > 0 : q < p.Q) ka_json_row_put<SEG>(p, q, stage + loc, first);
-        __syncthreads();
-        const uint32_t head = min(bt, (16u - mis) & 15u);       // bytes up to the first 16-byte boundary of dst
-        for (uint32_t i = threadIdx.x; i < head; i += 256) dst[i] = stage[i];
-        const uint32_t body = (bt - head) >> 4;
-        const uint4* s4 = reinterpret_cast<const uint4*>(stage + head);
-        uint4* d4 = reinterpret_cast<uint4*>(dst + head);
-        for (uint32_t i = threadIdx.x; i < body; i += 256) d4[i] = s4[i];
-        for (uint32_t i = head + (body << 4) + threadIdx.x; i < bt; i += 256) dst[i] = stage[i];
+        if (SEG ? n > 0 : q < p.Q) ka_json_row_put(p, q, stage + loc, comma);
+        ka_json_store_staged(dst, stage, bt);
     } else if (SEG ? n > 0 : q < p.Q) {
-        ka_json_row_put<SEG>(p, q, dst + loc + (shift - bshift), first);
+        ka_json_row_put(p, q, dst + loc + (shift - bshift), comma);
     }
     if constexpr (!SEG) {   // a segmented pass's headers and trailers come from ka_json_docs_kernel
         if (q == 0 && p.first) ka_put_str(frag, KA_JSON_HEAD, KA_JSON_HEAD_LEN);

@@ -19,39 +19,8 @@
 //   lend[g0 + i] topic-relative ends     -> chunk_end[loff[t] + i] = g0 + lend[g0 + i]   (block-relative record positions)
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024) ka_level_scan_kernel(const int32_t* __restrict__ ntl, int T, int32_t* __restrict__ loff) {
-    __shared__ int wsum[32];
-    __shared__ int carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int t0 = 0; t0 < T; t0 += 1024) {
-        const int t = t0 + threadIdx.x;
-        const int v = t < T ? ntl[t] : 0;
-        int x = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int y = __shfl_up_sync(KA_FULL, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) wsum[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            int w = wsum[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int y = __shfl_up_sync(KA_FULL, w, o);
-                if (lane >= o) w += y;
-            }
-            wsum[lane] = w;  // inclusive over warps
-        }
-        __syncthreads();
-        const int base = carry + (warp > 0 ? wsum[warp - 1] : 0);
-        if (t < T) loff[t] = base + x - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = base + x;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) loff[T] = carry;
+    const int total = ka_cta_scan(ntl, loff, T, 0);
+    if (threadIdx.x == 0) loff[T] = total;
 }
 
 // Chunk ends of a chunk table of U topics, one warp per topic. Topic u = k * T + t (k > 0 only in a batched solve over

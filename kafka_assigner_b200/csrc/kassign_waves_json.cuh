@@ -13,7 +13,7 @@
 //                                reads the rows 0..Q-1 themselves and drops wave 0, so it also compacts.
 //   ka_wave_doc_len_kernel       text bytes of every grouped row + per-CTA sums
 //   ka_wave_doc_scan_kernel      ONE CTA: 64-bit text offsets of the CTAs, and the total
-//   ka_wave_doc_write_kernel     the text (the staging of ka_json_write_kernel) and doc_off[0..W]
+//   ka_wave_doc_write_kernel     the text (through the JSON passes' shared-memory stage) and doc_off[0..W]
 //
 // A pass ranks a row by counting, never by the order of atomics: the text depends on the input alone.
 #pragma once
@@ -120,7 +120,6 @@ __device__ __forceinline__ void ka_wave_doc_row(const KaWaveDocs& d, uint32_t i,
 
 // grid ceil(Q / 256), 256 threads.
 __global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d) {
-    __shared__ uint32_t wsum[8];
     const uint32_t M = (uint32_t)*d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     uint32_t n = 0;
@@ -129,108 +128,50 @@ __global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d
         int v;
         bool first, last;
         ka_wave_doc_row(d, i, M, g, v, first, last);
-        n = ka_json_row_len<true>(d.p, g, first) + (first ? KA_JSON_HEAD_LEN : 0u) + (last ? KA_JSON_TAIL_LEN : 0u);
+        n = (first ? KA_JSON_HEAD_LEN : 0u) + ka_json_row_len(d.p, g, !first) + (last ? KA_JSON_TAIL_LEN : 0u);
         d.p.rowlen[i] = n;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(KA_FULL, n, o);
-    if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = n;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        unsigned long long s = 0;
-        for (int w = 0; w < 8; ++w) s += wsum[w];
-        d.blockoff[blockIdx.x] = s;
-    }
+    const unsigned long long bytes = ka_cta256_sum(n);
+    if (threadIdx.x == 0) d.blockoff[blockIdx.x] = bytes;
 }
 
 // ONE CTA of 1024: v[0..n) to its exclusive scan in place, *total = the sum. 64-bit throughout: 8 bytes per 256 rows lift the
 // 4 GiB limit a fragment of ka_json_scan_kernel has.
 __global__ void __launch_bounds__(1024) ka_wave_doc_scan_kernel(unsigned long long* __restrict__ v, int n, unsigned long long* __restrict__ total) {
-    __shared__ unsigned long long wtot[32];
-    __shared__ unsigned long long carry;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int b0 = 0; b0 < n; b0 += 1024) {
-        const int b = b0 + threadIdx.x;
-        const unsigned long long mine = b < n ? v[b] : 0ull;
-        unsigned long long x = mine;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned long long y = __shfl_up_sync(KA_FULL, x, o);
-            if (lane >= o) x += y;
-        }
-        if (lane == 31) wtot[warp] = x;
-        __syncthreads();
-        if (warp == 0) {
-            unsigned long long w = wtot[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned long long y = __shfl_up_sync(KA_FULL, w, o);
-                if (lane >= o) w += y;
-            }
-            wtot[lane] = w;
-        }
-        __syncthreads();
-        const unsigned long long base = carry + (warp > 0 ? wtot[warp - 1] : 0ull);
-        if (b < n) v[b] = base + x - mine;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry = base + x;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total = carry;
+    const unsigned long long bytes = ka_cta_scan(v, v, n, 0ull);
+    if (threadIdx.x == 0) *total = bytes;
 }
 
 // grid ceil(Q / 256), 256 threads, KA_JSON_SMEM_BYTES + 16 of dynamic shared memory. Every grouped row writes its text at its
-// final position, as ka_json_write_kernel does: the 256 rows of a CTA are assembled in shared memory at the 16-byte phase of
-// their destination and stored with coalesced 16-byte stores, and a CTA whose text does not fit (very long topic names) writes
-// straight to global memory. The frame travels with the rows, so a CTA that spans many waves is staged like any other. The
-// first row of wave v writes doc_off[v - 1], the last row of all doc_off[W]. Nothing is written when the text exceeds p.cap.
+// final position, the 256 rows of a CTA through the shared-memory stage of the JSON passes. The frame travels with the rows,
+// so a CTA that spans many waves is staged like any other. The first row of wave v writes doc_off[v - 1], the last row of all
+// doc_off[W]. Nothing is written when the text exceeds p.cap.
 __global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs d, const unsigned long long* __restrict__ total) {
-    extern __shared__ __align__(16) unsigned char ka_wdmem[];
-    __shared__ uint32_t wsum[8];
+    extern __shared__ __align__(16) unsigned char ka_jsmem[];
     const uint32_t M = (uint32_t)*d.n_rows;
     if (*total > d.p.cap || blockIdx.x * 256u >= M) return;   // CTA-uniform
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const uint32_t n = i < M ? d.p.rowlen[i] : 0u;
-    uint32_t x = n;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y = __shfl_up_sync(KA_FULL, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) wsum[warp] = x;
-    __syncthreads();
-    uint32_t woff = 0, bt = 0;
-    for (int w = 0; w < 8; ++w) { if (w < warp) woff += wsum[w]; bt += wsum[w]; }
+    uint32_t bt;
+    const uint32_t loc = ka_cta256_prefix(n, bt);           // my row inside the CTA's text
     const unsigned long long at = d.blockoff[blockIdx.x];   // this CTA's text
     char* dst = d.p.json + at;
-    const uint32_t loc = woff + x - n;                       // my row inside it
     const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15u);
+    char* stage = reinterpret_cast<char*>(ka_jsmem) + mis;
     const bool staged = mis + bt <= KA_JSON_SMEM_BYTES;
     if (i < M) {
         uint32_t g;
         int v;
         bool first, last;
         ka_wave_doc_row(d, i, M, g, v, first, last);
-        char* w = (staged ? reinterpret_cast<char*>(ka_wdmem) + mis : dst) + loc;
+        char* w = (staged ? stage : dst) + loc;
         if (first) {
-            ka_put_str(w, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
+            w = ka_put_str(w, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
             d.doc_off[v - 1] = at + loc;
         }
-        ka_json_row_put<true>(d.p, g, w + (first ? KA_JSON_HEAD_LEN : 0), first);
-        if (last) ka_put_str(w + n - KA_JSON_TAIL_LEN, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
+        w = ka_json_row_put(d.p, g, w, !first);
+        if (last) ka_put_str(w, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
         if (i + 1 == M) d.doc_off[v] = at + loc + n;
     }
-    if (!staged) return;
-    __syncthreads();
-    const char* stage = reinterpret_cast<const char*>(ka_wdmem) + mis;
-    const uint32_t head = min(bt, (16u - mis) & 15u);       // bytes up to the first 16-byte boundary of dst
-    for (uint32_t k = threadIdx.x; k < head; k += 256) dst[k] = stage[k];
-    const uint32_t body = (bt - head) >> 4;
-    const uint4* s4 = reinterpret_cast<const uint4*>(stage + head);
-    uint4* d4 = reinterpret_cast<uint4*>(dst + head);
-    for (uint32_t k = threadIdx.x; k < body; k += 256) d4[k] = s4[k];
-    for (uint32_t k = head + (body << 4) + threadIdx.x; k < bt; k += 256) dst[k] = stage[k];
+    if (staged) ka_json_store_staged(dst, stage, bt);
 }
