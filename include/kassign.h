@@ -384,6 +384,64 @@ int32_t ka_plan_waves_json(ka_ctx* ctx, int32_t T, const int64_t* part_off, cons
                            int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap,
                            ka_status* st);
 
+/* What the partitions' leaders send in one wave of ka_plan_waves_send, beside that wave's ka_wave_summary. */
+typedef struct ka_wave_send_summary {
+    int64_t max_broker_out;     /* largest per-broker outgoing sum in the wave ... */
+    int64_t max_broker_out_id;  /* ... its broker id (lowest id on ties, -1 when nothing is sent) */
+} ka_wave_send_summary;
+
+/* ka_plan_waves with a sender budget as well: no broker SENDS more than max_broker_out = C per wave either. A new replica
+ * fetches the whole partition from its leader, so a plan that caps only what each broker receives can still have one leader
+ * (typically a drained broker) send to every receiver of the cluster in one wave; Kafka throttles both sides
+ * (leader.replication.throttled.rate and follower.replication.throttled.rate) for this reason.
+ *   Q .. max_broker_in  exactly as ka_plan_waves takes them
+ *   n_send, send_id[n_send]   host; the SEND TABLE, strictly ascending ids (typically every broker of the cluster before an
+ *                      exclusion: a drained broker sends but is not in the ctx's broker table); 0 <= n_send <= 65535
+ *   max_broker_out     the sender budget C >= 1
+ *   wave, n_waves, summary   as ka_plan_waves writes them, under the rule below
+ *   send_summary[summary_cap]   host; the first min(W, summary_cap) waves' sender summaries, send_summary[v] beside summary[v]
+ *                      (NULL is allowed when summary_cap == 0)
+ * The rule is ka_plan_waves's with one more term and one more update per row with receivers. Its SENDER is the first broker of
+ * its current list (the preferred leader, which leads the partition in a balanced cluster); a row whose current list is empty
+ * has no sender. Each sender s of the send table starts with sopen[s] = 1, sload[s] = 0; a row of weight w with r receivers
+ * sends a = w x r. wave[g] = the max of ka_plan_waves's receiver terms and, for its sender s, (sopen[s] if sload[s] == 0 or
+ * sload[s] + a <= C, else sopen[s] + 1). Then the receivers update as in ka_plan_waves, and the sender likewise: wave[g] >
+ * sopen[s] gives sopen[s] = wave[g], sload[s] = a, else sload[s] += a. Sending and receiving are separate budgets: a broker can
+ * be the sender of one row and a receiver of another.
+ * So in every wave every broker sends at most C, unless a single row with w x r > C is its only outgoing row of nonzero weight
+ * there; every receive bound of ka_plan_waves still holds; the waves are still 1..W and none is empty (every wave value is some
+ * broker's open or open + 1), so doc_off and the json_cap bound of ka_plan_waves_json hold unchanged. Like a receiver, a
+ * leader's waves only move forward: a row never goes to an earlier wave than its leader's open one. With C >= 8 x (sum of the
+ * weights) no leader ever opens a wave, so a row's wave is the larger of ka_plan_waves's receiver terms and its leader's open
+ * wave; where no leader has two moved rows, wave, W, summary and every document are exactly those of ka_plan_waves(_json).
+ * Checks: everything ka_plan_waves checks, in its order, with its codes and operands; then max_broker_out < 1, n_send < 0,
+ * send_id NULL with n_send > 0, send_id not strictly ascending, or send_summary NULL with summary_cap > 0: KA_ERR_BAD_ARG;
+ * n_send > 65535: KA_ERR_LIMIT with a = n_send. On the device, the lowest failing row wins, over ka_plan_waves's row errors and
+ * this one together: a row with receivers whose sender the send table lacks gives KA_ERR_BAD_ARG with a = the row and b = the
+ * sender's id; within a row, the new-list errors come first. On any error *n_waves = 0 and nothing else is specified.
+ * Synchronous; 9 kernel launches (ka_plan_waves's 7 and 2 over the sender buckets), whatever Q, W and n_send are. Does not read
+ * or change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
+int32_t ka_plan_waves_send(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                           const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
+                           int32_t n_send, const int32_t* send_id, int64_t max_broker_out,
+                           int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, ka_wave_send_summary* send_summary,
+                           int32_t summary_cap, ka_status* st);
+
+/* ka_plan_waves_json under the rule of ka_plan_waves_send: the documents of its waves, built on the device.
+ *   T .. max_broker_in, names .. summary   exactly as ka_plan_waves_json takes and writes them
+ *   n_send, send_id, max_broker_out, send_summary   exactly as ka_plan_waves_send takes and writes them
+ * Every wave is non-empty, so doc_off[Q+1] and the json_cap bound of ka_plan_waves_json hold unchanged.
+ * Checks: everything ka_plan_waves_json checks, in its order; then the sender checks of ka_plan_waves_send. On the device the
+ * row errors of ka_plan_waves_send come first; a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX).
+ * Synchronous; the 9 launches of ka_plan_waves_send, then, when W > 0, 3 per 8 bits of W and 3 more. */
+int32_t ka_plan_waves_send_json(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                                const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                                int64_t max_broker_in, int32_t n_send, const int32_t* send_id, int64_t max_broker_out,
+                                const char* names, const int64_t* name_off, char* json, int64_t json_cap, int64_t* doc_off,
+                                int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, ka_wave_send_summary* send_summary,
+                                int32_t summary_cap, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

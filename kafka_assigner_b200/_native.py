@@ -23,6 +23,11 @@ class KaWaveSummary(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int64) for n in ("rows", "rows_moved", "replicas_added", "max_broker_in", "max_broker_in_id")]
 
 
+class KaWaveSendSummary(ctypes.Structure):
+    """ka_wave_send_summary: what the leaders send in one wave of ka_plan_waves_send (every field int64, no padding)."""
+    _fields_ = [(n, ctypes.c_int64) for n in ("max_broker_out", "max_broker_out_id")]
+
+
 KA_OK = 0
 KA_ERR_RF_MISMATCH, KA_ERR_RF_NOT_POSITIVE, KA_ERR_RF_GT_BROKERS, KA_ERR_UNASSIGNABLE, KA_ERR_HASH_INDEX = 1, 2, 3, 4, 5
 KA_ERR_BAD_ARG, KA_ERR_CUDA, KA_ERR_NO_DEVICE, KA_ERR_LIMIT = -1, -2, -3, -4
@@ -54,6 +59,9 @@ SYMBOLS = {
     "ka_plan_waves": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i32, _vp]),
     "ka_plan_waves_json": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _vp, _vp, _vp,
                                   _vp, _i32, _vp]),
+    "ka_plan_waves_send": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "ka_plan_waves_send_json": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp, _vp,
+                                       _i64, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "ka_ctx_set_topic_base": (_i32, [_vp, _i32]),

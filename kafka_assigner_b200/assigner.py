@@ -15,12 +15,15 @@ import ctypes
 import numpy as np
 
 from . import _native
-from ._native import KaMoveSummary, KaStatus, KaWaveSummary
+from ._native import KaMoveSummary, KaStatus, KaWaveSendSummary, KaWaveSummary
 
 # numpy view of ka_move_summary (KaMoveSummary): one record per candidate
 MOVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaMoveSummary._fields_])
 # numpy view of ka_wave_summary (KaWaveSummary): one record per wave of Solver.plan_waves
 WAVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaWaveSummary._fields_])
+# ka_wave_summary followed by ka_wave_send_summary: one record per wave of a plan with a sender budget
+WAVE_SEND_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaWaveSummary._fields_ + KaWaveSendSummary._fields_])
+_SEND_FIELDS = [name for name, _ in KaWaveSendSummary._fields_]
 
 
 class IllegalStateException(Exception):
@@ -74,6 +77,28 @@ def _json_size(rows, name_bytes, stride):
     """The sufficient buffer size kassign.h documents for one document: 64 + per row (50 + 12·stride + its topic's name
     length); name_bytes = Σ rows·name length over the topics."""
     return 64 + rows * (50 + 12 * stride) + name_bytes
+
+
+def _send_part(max_broker_out, send_brokers):
+    """The sender part of a wave plan as the _send entry points take it: None without a sender budget, else (n_send, send_id as
+    contiguous int32, max_broker_out). send_brokers is required with a budget, and only with one."""
+    if max_broker_out is None and send_brokers is None:
+        return None
+    if max_broker_out is None or send_brokers is None:
+        raise ValueError("max_broker_out and send_brokers go together")
+    send_id = np.ascontiguousarray(send_brokers, dtype=np.int32)
+    return len(send_id), send_id, int(max_broker_out)
+
+
+def _with_send(summary, send_summary):
+    """summary [W] (WAVE_SUMMARY_DTYPE) and send_summary [W] (its ka_wave_send_summary fields) as one WAVE_SEND_SUMMARY_DTYPE
+    array."""
+    both = np.zeros(len(summary), dtype=WAVE_SEND_SUMMARY_DTYPE)
+    for name in WAVE_SUMMARY_DTYPE.names:
+        both[name] = summary[name]
+    for j, name in enumerate(_SEND_FIELDS):
+        both[name] = send_summary[:, j]
+    return both
 
 
 def _wave_json_size(rows, name_bytes, stride):
@@ -480,12 +505,15 @@ class Solver:
     # on any cluster of up to 64 k rows and, on larger ones, every plan of up to 64 k waves.
     WAVE_SUMMARY_CAP = 1 << 16
 
-    def plan_waves(self, rep_off, cur_broker, out, out_len, max_broker_in, weight=None):
+    def plan_waves(self, rep_off, cur_broker, out, out_len, max_broker_in, weight=None, max_broker_out=None, send_brokers=None):
         """ka_plan_waves: the proposed lists out [Q, stride] / out_len [Q] (e.g. solve_ragged's rows) against the current lists
         cur_broker[rep_off[g] .. rep_off[g + 1]), cut into waves in which no broker of this Solver's table receives more than
         max_broker_in (weight: [Q] int64 per row, None = 1 per row). Returns (wave [Q] int32, 0 for an unchanged row; summary, a
         numpy structured array [W] with the fields of ka_wave_summary; KaStatus). On an error wave and summary are empty. A plan
-        of more than min(Q, WAVE_SUMMARY_CAP) waves takes a second call for the rest of the summaries."""
+        of more than min(Q, WAVE_SUMMARY_CAP) waves takes a second call for the rest of the summaries.
+        max_broker_out: ka_plan_waves_send instead, which also caps what each row's leader (the first broker of its current
+        list) sends per wave; send_brokers (required then: the ascending send table, e.g. every broker of the cluster before an
+        exclusion) holds every such leader. The summary then has the fields of WAVE_SEND_SUMMARY_DTYPE."""
         out = np.ascontiguousarray(out, dtype=np.int32)
         Q = len(out)
         stride = out.shape[1] if out.ndim == 2 else 1
@@ -494,28 +522,35 @@ class Solver:
         cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
         weight = None if weight is None else np.ascontiguousarray(weight, dtype=np.int64)
         assert out_len.shape == (Q,) and rep_off.shape == (Q + 1,) and (weight is None or weight.shape == (Q,))
+        send = _send_part(max_broker_out, send_brokers)
         wave = np.zeros(Q, dtype=np.int32)
         n_waves = ctypes.c_int32(0)
         st = KaStatus()
         cap = max(1, min(Q, self.WAVE_SUMMARY_CAP))
         while True:
             summary = np.zeros(cap, dtype=WAVE_SUMMARY_DTYPE)
-            self._L.ka_plan_waves(self._h, Q, _ptr(rep_off), _ptr(cur_broker), int(stride), _ptr(out_len), _ptr(out),
-                                  _ptr(weight), int(max_broker_in), _ptr(wave), ctypes.byref(n_waves), _ptr(summary), cap,
-                                  ctypes.byref(st))
+            rows = (self._h, Q, _ptr(rep_off), _ptr(cur_broker), int(stride), _ptr(out_len), _ptr(out), _ptr(weight), int(max_broker_in))
+            if send is None:
+                self._L.ka_plan_waves(*rows, _ptr(wave), ctypes.byref(n_waves), _ptr(summary), cap, ctypes.byref(st))
+            else:
+                send_summary = np.zeros((cap, len(_SEND_FIELDS)), dtype=np.int64)
+                self._L.ka_plan_waves_send(*rows, send[0], _ptr(send[1]), send[2], _ptr(wave), ctypes.byref(n_waves), _ptr(summary),
+                                           _ptr(send_summary), cap, ctypes.byref(st))
             if st.code != 0:
-                return np.zeros(0, dtype=np.int32), np.zeros(0, dtype=WAVE_SUMMARY_DTYPE), st
+                dtype = WAVE_SUMMARY_DTYPE if send is None else WAVE_SEND_SUMMARY_DTYPE
+                return np.zeros(0, dtype=np.int32), np.zeros(0, dtype=dtype), st
             if n_waves.value <= cap:
-                return wave, summary[:n_waves.value], st
+                W = n_waves.value
+                return wave, summary[:W] if send is None else _with_send(summary[:W], send_summary[:W]), st
             cap = n_waves.value
 
     def plan_waves_json(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, weight=None,
-                        json_buf=None):
+                        json_buf=None, max_broker_out=None, send_brokers=None):
         """ka_plan_waves_json: plan_waves over the rows of the ragged layout part_off / part_id (None = 0..P-1 per topic), and
         every wave's reassignment JSON built on the device. json_buf: optional writable uint8 numpy array (pinned for full PCIe
         speed); by default one of the documented sufficient size. Returns (docs, wave, summary, KaStatus): docs a list of W
         bytes-like views of the buffer, docs[v] the document of wave v + 1; wave and summary as plan_waves returns them. On an
-        error docs, wave and summary are empty."""
+        error docs, wave and summary are empty. max_broker_out / send_brokers: ka_plan_waves_send_json, as in plan_waves."""
         out = np.ascontiguousarray(out, dtype=np.int32)
         Q = len(out)
         stride = out.shape[1] if out.ndim == 2 else 1
@@ -532,14 +567,22 @@ class Solver:
         st = KaStatus()
         cap = max(1, Q)   # W never exceeds Q: one call, so the text is built once
         summary = np.zeros(cap, dtype=WAVE_SUMMARY_DTYPE)
-        self._L.ka_plan_waves_json(self._h, len(topic_names), _ptr(r.part_off), _ptr(r.part_id), _ptr(r.rep_off), _ptr(r.cur_broker),
-                                   int(stride), _ptr(out_len), _ptr(out), _ptr(weight), int(max_broker_in), _ptr(names),
-                                   _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(doc_off), _ptr(wave),
-                                   ctypes.byref(n_waves), _ptr(summary), cap, ctypes.byref(st))
+        send = _send_part(max_broker_out, send_brokers)
+        rows = (self._h, len(topic_names), _ptr(r.part_off), _ptr(r.part_id), _ptr(r.rep_off), _ptr(r.cur_broker), int(stride),
+                _ptr(out_len), _ptr(out), _ptr(weight), int(max_broker_in))
+        text = (_ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(doc_off), _ptr(wave), ctypes.byref(n_waves),
+                _ptr(summary))
+        if send is None:
+            self._L.ka_plan_waves_json(*rows, *text, cap, ctypes.byref(st))
+        else:
+            send_summary = np.zeros((cap, len(_SEND_FIELDS)), dtype=np.int64)
+            self._L.ka_plan_waves_send_json(*rows, send[0], _ptr(send[1]), send[2], *text, _ptr(send_summary), cap, ctypes.byref(st))
         if st.code != 0:
-            return [], np.zeros(0, dtype=np.int32), np.zeros(0, dtype=WAVE_SUMMARY_DTYPE), st
+            dtype = WAVE_SUMMARY_DTYPE if send is None else WAVE_SEND_SUMMARY_DTYPE
+            return [], np.zeros(0, dtype=np.int32), np.zeros(0, dtype=dtype), st
         W = n_waves.value
-        return [json_buf[doc_off[v]:doc_off[v + 1]] for v in range(W)], wave, summary[:W], st
+        summary = summary[:W] if send is None else _with_send(summary[:W], send_summary[:W])
+        return [json_buf[doc_off[v]:doc_off[v + 1]] for v in range(W)], wave, summary, st
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

@@ -149,6 +149,9 @@ struct ka_ctx {
     // outputs and records, the packed records, the per-CTA counts and offsets, the chain's per-broker words when they leave
     // shared memory, the bucket log, the summaries and the meta words
     DevBuf d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state, d_wv_log, d_wv_sum, d_wv_meta;
+    // scratch of the sender budget (ka_plan_waves_send and its JSON form): the send table, the sender bucket log and the sender
+    // summaries (the per-sender words share d_wv_state)
+    DevBuf d_wv_send, d_wv_slog, d_wv_ssum;
     // scratch of ka_plan_waves_json, beside the plan's and the JSON passes' (d_part_off, d_part_id, d_names, d_name_off, d_json,
     // d_json_rowlen, d_json_blocksum as 64-bit offsets): the grouped rows (two arrays of Q), the radix passes' (digit, tile)
     // counts and offsets, and the text total followed by doc_off [W + 1]
@@ -1244,6 +1247,15 @@ int finish_batch(ka_ctx* c, cudaStream_t s, const Batch& b, ka_status* st, const
     return KA_OK;
 }
 
+// The two peak kernels over a bucket log of n buckets of indices below N, into the fields F names of sum[W].
+template <typename F>
+void enq_wave_peaks(ka_ctx* c, cudaStream_t s, const KaWaveBucket* log, unsigned n, int N, typename F::S* sum) {
+    const unsigned blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>(((int64_t)n + 255) / 256, (int64_t)c->sm_count * 8));
+    ka_wave_peak_kernel<false, F><<<blocks, 256, 0, s>>>(log, n, N, sum);
+    ka_wave_peak_kernel<true, F><<<blocks, 256, 0, s>>>(log, n, N, sum);
+    c->launches += 2;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -1326,7 +1338,8 @@ void ka_ctx_destroy(ka_ctx* c) {
                       &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
                       &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec,
-                      &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta, &c->d_wv_perm, &c->d_wv_hist, &c->d_wv_doc})
+                      &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta, &c->d_wv_perm, &c->d_wv_hist, &c->d_wv_doc,
+                      &c->d_wv_send, &c->d_wv_slog, &c->d_wv_ssum})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -2381,10 +2394,20 @@ int32_t ka_score_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
     return score_batch(c, c->stream, bt, cand_off, sh.Q, out_stride, io, part_weight, &f, summary, brk, st, part_id, part_off);
 }
 
-// The broker id at the first position of row g's new list that the device refused: a broker named twice, or a receiver (a
-// broker the current list lacks) that the table `ids` lacks.
+// The sender part of a wave plan (ka_plan_waves_send and its JSON form): the send table id[n], the budget C and the caller's
+// sender summaries, one per ka_wave_summary.
+struct WaveSend {
+    int32_t n;
+    const int32_t* id;
+    int64_t C;
+    ka_wave_send_summary* summary;
+};
+
+// The broker id the device refused in row g: at the first position of its new list, a broker named twice or a receiver (a
+// broker the current list lacks) that the table `ids` lacks; with a sender part and no such position, the row's sender (the
+// first of its current list), which the send table lacks.
 static int32_t wave_refused_id(const std::vector<int32_t>& ids, const int64_t* rep_off, const int32_t* cur, int32_t stride,
-                               const int32_t* new_len, const int32_t* new_broker, int64_t g) {
+                               const int32_t* new_len, const int32_t* new_broker, int64_t g, const WaveSend* sd) {
     const int32_t* nb = new_broker + g * stride;
     const int32_t* cb = cur + rep_off[g];
     const int64_t m = rep_off[g + 1] - rep_off[g];
@@ -2392,7 +2415,7 @@ static int32_t wave_refused_id(const std::vector<int32_t>& ids, const int64_t* r
         if (std::find(nb, nb + j, nb[j]) != nb + j) return nb[j];
         if (std::find(cb, cb + m, nb[j]) == cb + m && !std::binary_search(ids.begin(), ids.end(), nb[j])) return nb[j];
     }
-    return 0;
+    return sd ? cb[0] : 0;
 }
 
 // The argument checks of ka_plan_waves, in its order, once st and the ctx are there. R = the current lists' brokers, positions
@@ -2418,26 +2441,58 @@ static int wave_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_broke
     return rc != KA_OK ? set_status(st, rc) : KA_OK;
 }
 
+// The checks a sender part adds, in this order, after every check of the call without one. The 16-bit sender index of a record
+// holds 0 .. 65534; 65535 marks a row without a sender.
+static int wave_send_args(const WaveSend& sd, int32_t summary_cap, ka_status* st) {
+    if (sd.C < 1 || sd.n < 0 || (!sd.id && sd.n > 0) || (!sd.summary && summary_cap > 0)) return set_status(st, KA_ERR_BAD_ARG);
+    for (int32_t i = 1; i < sd.n; ++i)
+        if (sd.id[i] <= sd.id[i - 1]) return set_status(st, KA_ERR_BAD_ARG);
+    if (sd.n > (int32_t)KA_WAVE_NO_SENDER) return set_status(st, KA_ERR_LIMIT, -1, -1, sd.n);
+    return KA_OK;
+}
+
 // The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the inputs up (into the buffers of the
 // host-buffer solve and score calls: every such call is synchronous), the rows / scan / compact / chain kernels, the meta words
 // back, then the sum and the two peak kernels (enqueued, not awaited). Leaves every row's wave in d_wv_wave, its receivers in
-// d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids still N - index) in d_wv_sum.
+// d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids still N - index) in d_wv_sum. A sender part sd (null:
+// none) adds the sender rule and its summaries (ids still n - index) in d_wv_ssum.
 static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, const int64_t* rep_off, const int32_t* cur_broker,
                             int32_t stride, const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
-                            int64_t max_broker_in, int& W, ka_status* st) {
+                            int64_t max_broker_in, const WaveSend* sd, int& W, ka_status* st) {
     cudaStream_t s = c->stream;
     const int N = c->br.N;
+    const int ns = sd ? sd->n : 0;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
-    const bool gstate = (size_t)N * KA_WAVE_BROKER_BYTES > KA_SMEM_BUDGET;   // the chain's per-broker words in global memory
+    // the chain's per-broker and per-sender words in global memory
+    const bool gstate = (size_t)(N + ns) * KA_WAVE_BROKER_BYTES > KA_SMEM_BUDGET;
     const size_t q = (size_t)Q;
     if (c->d_rep_off.reserve((q + 1) * 8) || c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
         c->d_out_len.reserve(q * 4) || c->d_out.reserve(q * stride * 4) || (part_weight && c->d_score_w.reserve(q * 8)) ||
         c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
         c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
-        c->d_wv_state.reserve(gstate ? (size_t)N * KA_WAVE_BROKER_BYTES : 16) ||
-        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveMeta)))
+        c->d_wv_state.reserve(gstate ? (size_t)(N + ns) * KA_WAVE_BROKER_BYTES : 16) ||
+        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveSendMeta)))
         return set_status(st, KA_ERR_CUDA);
-    const KaWaveMeta meta0{0xFFFFFFFFu, 0, 0, 0};
+    // a sender bucket holds at least one moved row: at most Q of them
+    if (sd && (c->d_wv_send.reserve((size_t)std::max(ns, 1) * 4) || c->d_wv_slog.reserve(q * sizeof(KaWaveBucket)) ||
+               (ns > 0 && cudaMemcpyAsync(c->d_wv_send.p, sd->id, (size_t)ns * 4, cudaMemcpyHostToDevice, s))))
+        return set_status(st, KA_ERR_CUDA);
+    KaWaveSendMeta meta0{{0xFFFFFFFFu, 0, 0, 0}, 0, {}};   // the sender part only read with sd
+    KaWaveSend& ks = meta0.snd;   // global words laid out as in shared memory: load, open, claim [N], then the senders' [ns]
+    long long* load = gstate ? c->d_wv_state.as<long long>() : nullptr;
+    int* open = gstate ? reinterpret_cast<int*>(load + N) : nullptr;
+    unsigned* claim = gstate ? reinterpret_cast<unsigned*>(open + N) : nullptr;
+    if (sd) {
+        ks.id = c->d_wv_send.as<int32_t>();
+        ks.n = ns;
+        ks.C = sd->C;
+        ks.log = c->d_wv_slog.as<KaWaveBucket>();
+        if (gstate) {
+            ks.load = reinterpret_cast<long long*>(claim + N);
+            ks.open = reinterpret_cast<int*>(ks.load + ns);
+            ks.claim = reinterpret_cast<unsigned*>(ks.open + ns);
+        }
+    }
     const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
     int32_t* d_cnt = c->d_wv_cnt.as<int32_t>();
     int32_t* d_off = d_cnt + nblk;
@@ -2453,64 +2508,72 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     int32_t* d_wave = c->d_wv_wave.as<int32_t>();
     int8_t* d_nrecv = c->d_wv_nrecv.as<int8_t>();
     KaWaveBucket* d_log = c->d_wv_log.as<KaWaveBucket>();
-    ka_wave_rows_kernel<<<nblk, 256, 0, s>>>(c->br, (uint32_t)Q, stride, c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(),
-                                             c->d_out_len.as<int32_t>(), c->d_out.as<int32_t>(), d_w, d_nrecv,
-                                             c->d_wv_tmp.as<KaWaveRec>(), d_wave, d_cnt, d_meta);
+    const auto rows = sd ? ka_wave_rows_kernel<true> : ka_wave_rows_kernel<false>;
+    rows<<<nblk, 256, 0, s>>>(c->br, (uint32_t)Q, stride, c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), c->d_out_len.as<int32_t>(),
+                              c->d_out.as<int32_t>(), d_w, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_wave, d_cnt, d_meta);
     ka_level_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, (int)nblk, d_off);
     ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_off, d_rec);
     if (gstate) {
-        long long* load = c->d_wv_state.as<long long>();
-        int* open = reinterpret_cast<int*>(load + N);
-        ka_wave_chain_kernel<true><<<1, KA_WAVE_THREADS, 0, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, load, open,
-                                                                reinterpret_cast<unsigned*>(open + N), d_log, d_meta);
+        const auto chain = sd ? ka_wave_chain_kernel<true, true> : ka_wave_chain_kernel<true, false>;
+        chain<<<1, KA_WAVE_THREADS, 0, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, load, open, claim, d_log, d_meta);
     } else {
-        const size_t smem = (size_t)N * KA_WAVE_BROKER_BYTES;
-        if (allow_smem(ka_wave_chain_kernel<false>, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-        ka_wave_chain_kernel<false><<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, nullptr,
-                                                                     nullptr, nullptr, d_log, d_meta);
+        const size_t smem = (size_t)(N + ns) * KA_WAVE_BROKER_BYTES;
+        const auto chain = sd ? ka_wave_chain_kernel<false, true> : ka_wave_chain_kernel<false, false>;
+        if (allow_smem(chain, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+        chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, nullptr, nullptr, nullptr, d_log,
+                                               d_meta);
     }
     c->launches += 4;
-    KaWaveMeta meta;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, d_meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
+    KaWaveSendMeta back;
+    const KaWaveMeta& meta = back.m;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&back, d_meta, sizeof(back), cudaMemcpyDeviceToHost, s) ||
         cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     if (meta.err_row != 0xFFFFFFFFu)
         return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row,
-                          wave_refused_id(c->broker_id, rep_off, cur_broker, stride, new_len, new_broker, meta.err_row));
+                          wave_refused_id(c->broker_id, rep_off, cur_broker, stride, new_len, new_broker, meta.err_row, sd));
     W = std::max(meta.waves, meta.changed);
     const size_t sum_bytes = (size_t)std::max(W, 1) * sizeof(ka_wave_summary);
-    if (c->d_wv_sum.reserve(sum_bytes)) return set_status(st, KA_ERR_CUDA);
+    const size_t ssum_bytes = (size_t)std::max(W, 1) * sizeof(ka_wave_send_summary);
+    if (c->d_wv_sum.reserve(sum_bytes) || (sd && c->d_wv_ssum.reserve(ssum_bytes))) return set_status(st, KA_ERR_CUDA);
     ka_wave_summary* d_sum = c->d_wv_sum.as<ka_wave_summary>();
-    const unsigned peak_blocks = (unsigned)std::max<int64_t>(1, std::min<int64_t>(((int64_t)meta.nlog + 255) / 256, (int64_t)c->sm_count * 8));
-    if (cudaMemsetAsync(d_sum, 0, sum_bytes, s)) return set_status(st, KA_ERR_CUDA);
+    if (cudaMemsetAsync(d_sum, 0, sum_bytes, s) || (sd && cudaMemsetAsync(c->d_wv_ssum.p, 0, ssum_bytes, s)))
+        return set_status(st, KA_ERR_CUDA);
     ka_wave_sum_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, d_wave, d_w, d_sum);
-    ka_wave_peak_kernel<false><<<peak_blocks, 256, 0, s>>>(d_log, meta.nlog, N, d_sum);
-    ka_wave_peak_kernel<true><<<peak_blocks, 256, 0, s>>>(d_log, meta.nlog, N, d_sum);
-    c->launches += 3;
+    c->launches += 1;
+    enq_wave_peaks<KaWaveInPeak>(c, s, d_log, meta.nlog, N, d_sum);
+    if (sd) enq_wave_peaks<KaWaveOutPeak>(c, s, ks.log, back.nslog, ns, c->d_wv_ssum.as<ka_wave_send_summary>());
     return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
 }
 
-// The plan of wave_plan_device out to the caller: the first min(W, summary_cap) summaries and every row's wave, awaited; then
-// the summaries' broker ids and *n_waves.
+// The plan of wave_plan_device out to the caller: the first min(W, summary_cap) summaries (and with a sender part sd, sender
+// summaries) and every row's wave, awaited; then the summaries' broker ids and *n_waves.
 static int wave_plan_out(ka_ctx* c, int64_t Q, int W, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap,
-                         ka_status* st) {
+                         const WaveSend* sd, ka_status* st) {
     cudaStream_t s = c->stream;
     const int N = c->br.N;
     const int out = std::min(W, summary_cap);
     if ((out > 0 && cudaMemcpyAsync(summary, c->d_wv_sum.p, (size_t)out * sizeof(ka_wave_summary), cudaMemcpyDeviceToHost, s)) ||
+        (sd && out > 0 &&
+         cudaMemcpyAsync(sd->summary, c->d_wv_ssum.p, (size_t)out * sizeof(ka_wave_send_summary), cudaMemcpyDeviceToHost, s)) ||
         (wave && cudaMemcpyAsync(wave, c->d_wv_wave.p, (size_t)Q * 4, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     for (int v = 0; v < out; ++v) {   // N - the lowest broker index of the wave's peak, 0 when nothing was added
         const int64_t f = summary[v].max_broker_in_id;
         summary[v].max_broker_in_id = f > 0 ? c->broker_id[N - f] : -1;
+        if (sd) {   // likewise n - the lowest send-table index
+            const int64_t h = sd->summary[v].max_broker_out_id;
+            sd->summary[v].max_broker_out_id = h > 0 ? sd->id[sd->n - h] : -1;
+        }
     }
     *n_waves = W;
     return set_status(st, KA_OK);
 }
 
-int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
-                      const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, int32_t* wave, int32_t* n_waves,
-                      ka_wave_summary* summary, int32_t summary_cap, ka_status* st) {
+// ka_plan_waves, and with a sender part sd ka_plan_waves_send.
+static int32_t plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                          const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, int32_t* wave, int32_t* n_waves,
+                          ka_wave_summary* summary, int32_t summary_cap, const WaveSend* sd, ka_status* st) {
     if (!st) return KA_ERR_BAD_ARG;
     if (n_waves) *n_waves = 0;
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
@@ -2518,14 +2581,31 @@ int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_
     int rc = wave_args(Q, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, n_waves, summary, summary_cap, R,
                        positions, st);
     if (rc != KA_OK) return rc;
+    if (sd && (rc = wave_send_args(*sd, summary_cap, st)) != KA_OK) return rc;
     if (Q == 0) return set_status(st, KA_OK);
     // the call reads only the broker table: a pending asynchronous status stays pending for ka_last_status
     if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
     int W = 0;
-    if ((rc = wave_plan_device(c, Q, R, positions, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, W,
+    if ((rc = wave_plan_device(c, Q, R, positions, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, sd, W,
                                st)) != KA_OK)
         return rc;
-    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, st);
+    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, sd, st);
+}
+
+int32_t ka_plan_waves(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                      const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in, int32_t* wave, int32_t* n_waves,
+                      ka_wave_summary* summary, int32_t summary_cap, ka_status* st) {
+    return plan_waves(c, Q, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, wave, n_waves, summary,
+                      summary_cap, nullptr, st);
+}
+
+int32_t ka_plan_waves_send(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                           const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
+                           int32_t n_send, const int32_t* send_id, int64_t max_broker_out, int32_t* wave, int32_t* n_waves,
+                           ka_wave_summary* summary, ka_wave_send_summary* send_summary, int32_t summary_cap, ka_status* st) {
+    const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
+    return plan_waves(c, Q, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, wave, n_waves, summary,
+                      summary_cap, &sd, st);
 }
 
 // The radix passes of ka_plan_waves_json over the plan's d_wv_wave: d_wv_perm (two arrays of Q rows) ends with the changed
@@ -2552,11 +2632,12 @@ static const int32_t* enq_wave_group(ka_ctx* c, cudaStream_t s, int64_t Q, int W
     return perm[(pass - 1) & 1];
 }
 
-int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
-                           const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
-                           const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
-                           int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
-                           int32_t summary_cap, ka_status* st) {
+// ka_plan_waves_json, and with a sender part sd ka_plan_waves_send_json.
+static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
+                               const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
+                               const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
+                               int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
+                               int32_t summary_cap, const WaveSend* sd, ka_status* st) {
     if (!st) return KA_ERR_BAD_ARG;
     if (n_waves) *n_waves = 0;
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
@@ -2574,14 +2655,15 @@ int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const 
         bound += (part_off[t + 1] - part_off[t]) * (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + 50 + 12 * (int64_t)stride + name_off[t + 1] - name_off[t]);
     }
     if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
+    if (sd && (rc = wave_send_args(*sd, summary_cap, st)) != KA_OK) return rc;
     if (doc_off) doc_off[0] = 0;
     if (Q == 0) return set_status(st, KA_OK);
     if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
     int W = 0;
-    if ((rc = wave_plan_device(c, Q, R, positions, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, W,
+    if ((rc = wave_plan_device(c, Q, R, positions, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, sd, W,
                                st)) != KA_OK)
         return rc;
-    if (W == 0) return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, st);
+    if (W == 0) return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, sd, st);
 
     cudaStream_t s = c->stream;
     const size_t q = (size_t)Q;
@@ -2613,7 +2695,27 @@ int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const 
     if (cudaMemcpyAsync(json, c->d_json.p, (size_t)total, cudaMemcpyDeviceToHost, s) ||
         cudaMemcpyAsync(doc_off, d.doc_off, ((size_t)W + 1) * 8, cudaMemcpyDeviceToHost, s))
         return set_status(st, KA_ERR_CUDA);
-    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, st);
+    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, sd, st);
+}
+
+int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
+                           const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
+                           const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
+                           int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
+                           int32_t summary_cap, ka_status* st) {
+    return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, st);
+}
+
+int32_t ka_plan_waves_send_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
+                                const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
+                                const int64_t* part_weight, int64_t max_broker_in, int32_t n_send, const int32_t* send_id,
+                                int64_t max_broker_out, const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
+                                ka_wave_send_summary* send_summary, int32_t summary_cap, ka_status* st) {
+    const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
+    return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, st);
 }
 
 }  // extern "C"

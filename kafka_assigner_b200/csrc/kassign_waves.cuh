@@ -20,6 +20,12 @@
 // open / load alone. The earliest pending record always holds its claims, so every round decides at least one record; a record
 // decides in round 1 + (the latest round among the earlier records of its chunk that share a broker with it).
 //
+// The sender budget (SEND, ka_plan_waves_send): the first broker of a moved row's current list sends w x receivers; its index in the
+// send table rides in the record's n word, and the chain keeps a second set of per-broker words for the senders (open, load,
+// claim). A pending record claims its sender's words with the same key as its receivers' and decides only when it holds every
+// claim, so the earliest pending record still decides in every round. A record decides in the round after the latest earlier
+// record of its chunk that shares a receiver or its sender with it.
+//
 // Everything is integer, and every sum and extreme commutative: the plan does not depend on the order of the atomics.
 #pragma once
 #include "kassign_common.cuh"
@@ -32,7 +38,8 @@
 #define KA_WAVE_MAX_ROUND (1u << (32 - KA_WAVE_SLOT_BITS))      // claim keys are (round << 11) | (CHUNK - 1 - slot)
 static_assert(KA_WAVE_CHUNK == 1 << KA_WAVE_SLOT_BITS, "a claim key holds a slot of the chunk");
 
-// A moved row: its input row, its receivers (table indices, 16 bits each, in list order) and its weight.
+// A moved row: its input row, its receivers (table indices, 16 bits each, in list order) and its weight. n = the receivers;
+// with SEND, bits 16..31 hold the sender's index in the send table (KA_WAVE_NO_SENDER for an empty current list).
 struct KaWaveRec {
     int32_t row, n;
     long long w;
@@ -46,12 +53,35 @@ struct KaWaveBucket {
     long long load;
 };
 
+#define KA_WAVE_NO_SENDER 0xFFFFu
+
+// The sender part of a plan (SEND): the send table id[n] (strictly ascending, n <= 65535), the budget C, the chain's
+// per-sender words when they leave shared memory (load / open / claim [n], else null) and the sender bucket log.
+struct KaWaveSend {
+    const int32_t* id;
+    int n;
+    long long C;
+    long long* load;
+    int* open;
+    unsigned* claim;
+    KaWaveBucket* log;
+};
+
 struct KaWaveMeta {
     unsigned err_row;   // lowest failing row (unsigned atomicMin, init 0xFFFFFFFF)
     int changed;        // some row changed
     int waves;          // W of the chain (the largest wave of a moved row)
     unsigned nlog;      // buckets logged
 };
+
+// The meta words of a plan with a sender part: the SEND instances take the KaWaveMeta* of the others and reach the sender
+// part behind it (ka_wave_send_meta), so that the instances without a sender keep their parameters and their code.
+struct KaWaveSendMeta {
+    KaWaveMeta m;
+    unsigned nslog;     // sender buckets logged
+    KaWaveSend snd;
+};
+__device__ __forceinline__ KaWaveSendMeta* ka_wave_send_meta(KaWaveMeta* meta) { return reinterpret_cast<KaWaveSendMeta*>(meta); }
 
 __device__ __forceinline__ uint32_t ka_wave_rcv(const KaWaveRec& r, int j) {
     return (uint32_t)((j < 4 ? r.lo >> (16 * j) : r.hi >> (16 * (j - 4))) & 0xFFFFu);
@@ -60,7 +90,8 @@ __device__ __forceinline__ uint32_t ka_wave_rcv(const KaWaveRec& r, int j) {
 // grid ceil(Q / 256), 256 threads. Row g: new list new_broker[g * S .. + new_len[g]) (S <= 8), current list cur[rep_off[g] ..
 // rep_off[g + 1]). Writes nrecv[g] (-1 unchanged, else the receivers), wave[g] for the rows without receivers (0 unchanged, 1
 // changed), tmp[g] for a row with receivers, cnt[CTA] = its moved rows. A new list naming a broker twice, or a receiver the
-// table lacks, fails the row.
+// table lacks, fails the row. SEND: so does a row with receivers whose sender (cur[rep_off[g]]) the send table lacks.
+template <bool SEND>
 __global__ void __launch_bounds__(256) ka_wave_rows_kernel(const KaBrokers br, uint32_t Q, int S, const int64_t* __restrict__ rep_off,
                                                            const int32_t* __restrict__ cur, const int32_t* __restrict__ new_len,
                                                            const int32_t* __restrict__ new_broker, const int64_t* __restrict__ weight,
@@ -98,10 +129,30 @@ __global__ void __launch_bounds__(256) ka_wave_rows_kernel(const KaBrokers br, u
                 bad |= dup;
             }
         }
+        int n_word = k;
+        if constexpr (SEND) {
+            if (k > 0) {
+                uint32_t sx = KA_WAVE_NO_SENDER;
+                if (m > 0) {   // the sender's index: a binary search of the send table
+                    const int id = __ldg(cur + a);
+                    const KaWaveSend& snd = ka_wave_send_meta(meta)->snd;
+                    const int32_t* sid = snd.id;
+                    const int ns = snd.n;
+                    int l = 0, h = ns;
+                    while (l < h) {
+                        const int mid = (l + h) >> 1;
+                        if (__ldg(sid + mid) < id) l = mid + 1; else h = mid;
+                    }
+                    if (l < ns && __ldg(sid + l) == id) sx = (uint32_t)l;
+                    else bad = true;
+                }
+                n_word |= (int)(sx << 16);
+            }
+        }
         if (bad) atomicMin(&meta->err_row, g);
         if (!diff) wave[g] = 0;
         else if (k == 0) wave[g] = 1;
-        else tmp[g] = KaWaveRec{(int32_t)g, k, weight ? __ldg(weight + g) : 1, lo, hi};
+        else tmp[g] = KaWaveRec{(int32_t)g, n_word, weight ? __ldg(weight + g) : 1, lo, hi};
         nrecv[g] = diff ? (int8_t)k : (int8_t)-1;
     }
     const int moved = __syncthreads_count(k > 0);
@@ -138,13 +189,42 @@ __device__ __forceinline__ void ka_wave_st(T* p, T v) {
     else *p = v;
 }
 
-// Bytes of shared memory the chain keeps per broker (load, open, claim).
+// Bytes of shared memory the chain keeps per broker (load, open, claim), and with SEND per sender too.
 #define KA_WAVE_BROKER_BYTES 16
 
-// ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B. Writes wave[row] of every
-// record, the bucket log and meta->waves / nlog. With GSTATE the per-broker words are gload / gopen / gclaim [N]. Does nothing
-// when the rows pass failed a row.
+// The receivers of a record (SEND: the n word also holds the sender).
+template <bool SEND>
+__device__ __forceinline__ int ka_wave_nrcv(const KaWaveRec& r) {
+    if constexpr (SEND) return r.n & 0xFFFF;
+    else return r.n;
+}
+
+// The chain's per-sender words (SEND): after the N broker words in shared memory, or where meta->snd points (GSTATE). Read
+// where they are used, so that the instances without a sender declare nothing more than the plan's own.
+struct KaWaveSendWords {
+    long long* load;
+    int* open;
+    unsigned* claim;
+};
 template <bool GSTATE>
+__device__ __forceinline__ KaWaveSendWords ka_wave_send_words(const KaWaveSendMeta* sm, unsigned* claim, int N) {
+    if constexpr (GSTATE) return KaWaveSendWords{sm->snd.load, sm->snd.open, sm->snd.claim};
+    long long* load = reinterpret_cast<long long*>(claim + N);   // 16 N bytes in: 8-byte aligned
+    int* open = reinterpret_cast<int*>(load + sm->snd.n);
+    return KaWaveSendWords{load, open, reinterpret_cast<unsigned*>(open + sm->snd.n)};
+}
+
+// A closed or still-open sender bucket to the sender log (SEND).
+__device__ __forceinline__ void ka_wave_send_put(KaWaveSendMeta* sm, int wv, uint32_t x, long long l) {
+    const unsigned s = atomicAdd(&sm->nslog, 1u);
+    sm->snd.log[s] = KaWaveBucket{wv, (int32_t)x, l};
+}
+
+// ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B. Writes wave[row] of every
+// record, the bucket log and meta->waves / nlog. With GSTATE the per-broker words are gload / gopen / gclaim [N]. SEND: also
+// the sender rule of ka_wave_send_meta(meta) (its budget C, its words by ka_wave_send_words), the sender buckets in its log
+// and their count in its nslog (zeroed by the host). Does nothing when the rows pass failed a row.
+template <bool GSTATE, bool SEND>
 __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off,
                                                                            int nblk, int N, long long B, int32_t* __restrict__ wave,
                                                                            long long* gload, int* gopen, unsigned* gclaim,
@@ -166,6 +246,15 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
         ka_wave_st<GSTATE>(load + i, 0LL);
         ka_wave_st<GSTATE>(open + i, 1);
         ka_wave_st<GSTATE>(claim + i, 0u);
+    }
+    if constexpr (SEND) {
+        KaWaveSendMeta* sm = ka_wave_send_meta(meta);
+        const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
+        for (int i = tid; i < sm->snd.n; i += KA_WAVE_THREADS) {
+            ka_wave_st<GSTATE>(sw.load + i, 0LL);
+            ka_wave_st<GSTATE>(sw.open + i, 1);
+            ka_wave_st<GSTATE>(sw.claim + i, 0u);
+        }
     }
     if (tid == 0) { nlog = 0; wmax = 0; }
     __syncthreads();
@@ -192,6 +281,11 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
         for (;;) {
             if (++round == KA_WAVE_MAX_ROUND) {   // the key's round field is full: clear the claims and count again
                 for (int i = tid; i < N; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(claim + i, 0u);
+                if constexpr (SEND) {
+                    KaWaveSendMeta* sm = ka_wave_send_meta(meta);
+                    const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
+                    for (int i = tid; i < sm->snd.n; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(sw.claim + i, 0u);
+                }
                 __syncthreads();
                 round = 1;
             }
@@ -200,24 +294,52 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
             for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
                 key[e] = round << KA_WAVE_SLOT_BITS | (unsigned)(KA_WAVE_CHUNK - 1 - (e * KA_WAVE_THREADS + tid));
                 if (pend >> e & 1u)
-                    for (int j = 0; j < r[e].n; ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
+                    for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
+                if constexpr (SEND) {   // and its sender
+                    const uint32_t sx = (uint32_t)r[e].n >> 16;
+                    if ((pend >> e & 1u) && sx != KA_WAVE_NO_SENDER)
+                        atomicMax(ka_wave_send_words<GSTATE>(ka_wave_send_meta(meta), claim, N).claim + sx, key[e]);
+                }
             }
             __syncthreads();
 #pragma unroll
             for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
                 if (!(pend >> e & 1u)) continue;
                 bool own = true;
-                for (int j = 0; j < r[e].n; ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
+                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
+                if constexpr (SEND) {
+                    const uint32_t sx = (uint32_t)r[e].n >> 16;
+                    if (sx != KA_WAVE_NO_SENDER)
+                        own &= ka_wave_ld<GSTATE>(ka_wave_send_words<GSTATE>(ka_wave_send_meta(meta), claim, N).claim + sx) == key[e];
+                }
                 if (!own) continue;
                 const long long w = r[e].w;
                 int wv = 0;
-                for (int j = 0; j < r[e].n; ++j) {
+                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) {
                     const uint32_t b = ka_wave_rcv(r[e], j);
                     const int o = ka_wave_ld<GSTATE>(open + b);
                     const long long l = ka_wave_ld<GSTATE>(load + b);
                     wv = max(wv, (l == 0 || l + w <= B) ? o : o + 1);
                 }
-                for (int j = 0; j < r[e].n; ++j) {
+                if constexpr (SEND) {   // the sender's candidate, and with it the row's wave: the sender updates
+                    const uint32_t sx = (uint32_t)r[e].n >> 16;
+                    if (sx != KA_WAVE_NO_SENDER) {
+                        KaWaveSendMeta* sm = ka_wave_send_meta(meta);
+                        const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
+                        const long long a = w * ka_wave_nrcv<SEND>(r[e]);
+                        const int o = ka_wave_ld<GSTATE>(sw.open + sx);
+                        const long long l = ka_wave_ld<GSTATE>(sw.load + sx);
+                        wv = max(wv, (l == 0 || l + a <= sm->snd.C) ? o : o + 1);
+                        if (wv > o) {   // the sender closes its bucket and opens wave wv
+                            if (l > 0) ka_wave_send_put(sm, o, sx, l);
+                            ka_wave_st<GSTATE>(sw.open + sx, wv);
+                            ka_wave_st<GSTATE>(sw.load + sx, a);
+                        } else {
+                            ka_wave_st<GSTATE>(sw.load + sx, l + a);
+                        }
+                    }
+                }
+                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) {
                     const uint32_t b = ka_wave_rcv(r[e], j);
                     const int o = ka_wave_ld<GSTATE>(open + b);
                     const long long l = ka_wave_ld<GSTATE>(load + b);
@@ -240,6 +362,14 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
     for (int i = tid; i < N; i += KA_WAVE_THREADS) {
         const long long l = ka_wave_ld<GSTATE>(load + i);
         if (l > 0) put(ka_wave_ld<GSTATE>(open + i), (uint32_t)i, l);
+    }
+    if constexpr (SEND) {
+        KaWaveSendMeta* sm = ka_wave_send_meta(meta);
+        const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
+        for (int i = tid; i < sm->snd.n; i += KA_WAVE_THREADS) {
+            const long long l = ka_wave_ld<GSTATE>(sw.load + i);
+            if (l > 0) ka_wave_send_put(sm, ka_wave_ld<GSTATE>(sw.open + i), (uint32_t)i, l);
+        }
     }
     atomicMax(&wmax, my_max);
     __syncthreads();
@@ -270,22 +400,35 @@ __global__ void __launch_bounds__(256) ka_wave_sum_kernel(uint32_t Q, const int8
     }
 }
 
-// grid-stride over the n logged buckets, summary zeroed beforehand. ID = false: max_broker_in[wave] = the largest bucket of
-// the wave. ID = true (after): max_broker_in_id[wave] = N - the lowest broker index among the buckets equal to that maximum,
-// 0 when the wave has no bucket (the host turns it into the broker's id, or -1).
-template <bool ID>
+// The fields a peak pass fills: the incoming peak of ka_wave_summary over the bucket log, and the outgoing peak of
+// ka_wave_send_summary over the sender log.
+struct KaWaveInPeak {
+    using S = ka_wave_summary;
+    static __device__ __forceinline__ int64_t& peak(S& s) { return s.max_broker_in; }
+    static __device__ __forceinline__ int64_t& id(S& s) { return s.max_broker_in_id; }
+};
+struct KaWaveOutPeak {
+    using S = ka_wave_send_summary;
+    static __device__ __forceinline__ int64_t& peak(S& s) { return s.max_broker_out; }
+    static __device__ __forceinline__ int64_t& id(S& s) { return s.max_broker_out_id; }
+};
+
+// grid-stride over the n logged buckets, summary zeroed beforehand, into the fields F names. ID = false: peak[wave] = the
+// largest bucket of the wave. ID = true (after): id[wave] = N - the lowest index among the buckets equal to that maximum, 0
+// when the wave has no bucket (the host turns it into the broker's id, or -1).
+template <bool ID, typename F>
 __global__ void __launch_bounds__(256) ka_wave_peak_kernel(const KaWaveBucket* __restrict__ log, unsigned n, int N,
-                                                           ka_wave_summary* summary) {
+                                                           typename F::S* summary) {
     for (unsigned i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const KaWaveBucket b = log[i];
-        ka_wave_summary& s = summary[b.wave - 1];
+        typename F::S& s = summary[b.wave - 1];
         if constexpr (!ID) {
-            if (b.load > *(volatile long long*)&s.max_broker_in)   // most buckets lose without an atomic
-                atomicMax(reinterpret_cast<unsigned long long*>(&s.max_broker_in), (unsigned long long)b.load);
+            if (b.load > *(volatile long long*)&F::peak(s))   // most buckets lose without an atomic
+                atomicMax(reinterpret_cast<unsigned long long*>(&F::peak(s)), (unsigned long long)b.load);
         } else {
             const long long key = N - b.idx;
-            if (b.load == s.max_broker_in && key > *(volatile long long*)&s.max_broker_in_id)
-                atomicMax(reinterpret_cast<unsigned long long*>(&s.max_broker_in_id), (unsigned long long)key);
+            if (b.load == F::peak(s) && key > *(volatile long long*)&F::id(s))
+                atomicMax(reinterpret_cast<unsigned long long*>(&F::id(s)), (unsigned long long)key);
         }
     }
 }

@@ -272,6 +272,15 @@ public:
         ka_status status;   // re-throw with throwForStatus; on an error summary and waves are empty
         std::vector<ka_wave_summary> summary;
         std::vector<std::vector<TopicOutput>> waves;
+        std::vector<ka_wave_send_summary> sendSummary;   // with a SendBudget: beside summary, one per wave
+    };
+
+    // A sender budget as well (ka_plan_waves_send): no partition leader (the first broker of its current list) sends more than
+    // maxBrokerOut (weight x the partition's new replicas) per wave. sendBrokers, strictly ascending, must hold every such
+    // leader: typically every broker of the cluster before an exclusion, since a drained broker still sends.
+    struct SendBudget {
+        int64_t maxBrokerOut;
+        std::vector<int32_t> sendBrokers;
     };
 
     // `topics`' current assignment against `proposed` (the solveTopics output for them: the same topics and partitions, in the
@@ -279,6 +288,35 @@ public:
     // the weight of every partition, as scoreTopicsCandidates takes them.
     WavePlan planWaves(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                        const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavesWith(topics, proposed, maxBrokerIn, nullptr, weights);
+    }
+    // planWaves under a sender budget too; sendSummary is filled.
+    WavePlan planWaves(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                       const SendBudget& send, const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavesWith(topics, proposed, maxBrokerIn, &send, weights);
+    }
+
+    // planWaves with every wave's document built on the device (ka_plan_waves_json): docs[v] equals
+    // newAssignmentJson(planWaves(...).waves[v]). Topic names that org.json would escape take exactly that host path instead.
+    struct WaveDocs {
+        ka_status status;   // re-throw with throwForStatus; on an error summary and docs are empty
+        std::vector<ka_wave_summary> summary;
+        std::vector<std::string> docs;
+        std::vector<ka_wave_send_summary> sendSummary;   // with a SendBudget: beside summary, one per wave
+    };
+    WaveDocs planWavesJson(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                           const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavesJsonWith(topics, proposed, maxBrokerIn, nullptr, weights);
+    }
+    // planWavesJson under a sender budget too (ka_plan_waves_send_json); sendSummary is filled.
+    WaveDocs planWavesJson(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                           const SendBudget& send, const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavesJsonWith(topics, proposed, maxBrokerIn, &send, weights);
+    }
+
+private:
+    WavePlan planWavesWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                           const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights) {
         const Flat f = flatten(topics, -1);
         const ProposedRows p = proposedRows(topics, proposed, weights);
         const size_t Q = f.partId.size();
@@ -288,16 +326,23 @@ public:
         // W never exceeds Q: min(Q, 64 k) summaries (40 bytes each) hold every plan in one call, but one of more than 64 k waves
         res.summary.resize(std::max<size_t>(1, std::min<size_t>(Q, 1 << 16)));
         auto plan = [&](int32_t* waveOut) {
-            return ka_plan_waves(ctx_, (int64_t)Q, f.repOff.data(), f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(),
-                                 p.w.empty() ? nullptr : p.w.data(), maxBrokerIn, waveOut, &W, res.summary.data(),
-                                 (int32_t)res.summary.size(), &res.status);
+            const int64_t* w = p.w.empty() ? nullptr : p.w.data();
+            if (!send)
+                return ka_plan_waves(ctx_, (int64_t)Q, f.repOff.data(), f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(), w,
+                                     maxBrokerIn, waveOut, &W, res.summary.data(), (int32_t)res.summary.size(), &res.status);
+            res.sendSummary.resize(res.summary.size());
+            return ka_plan_waves_send(ctx_, (int64_t)Q, f.repOff.data(), f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(), w,
+                                      maxBrokerIn, (int32_t)send->sendBrokers.size(), send->sendBrokers.data(), send->maxBrokerOut,
+                                      waveOut, &W, res.summary.data(), res.sendSummary.data(), (int32_t)res.summary.size(),
+                                      &res.status);
         };
         if (plan(wave.data()) == KA_OK && W > (int32_t)res.summary.size()) {
             res.summary.resize(W);
             plan(nullptr);
         }
-        if (res.status.code != KA_OK) return WavePlan{res.status, {}, {}};
+        if (res.status.code != KA_OK) return WavePlan{res.status, {}, {}, {}};
         res.summary.resize(W);
+        if (send) res.sendSummary.resize(W);
         res.waves.resize(W);
         std::vector<size_t> lastTopic(W, topics.size());   // the topic of each wave's last TopicOutput
         for (size_t t = 0; t < topics.size(); ++t)
@@ -313,16 +358,10 @@ public:
             }
         return res;
     }
+    WaveDocs planWavesJsonWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                               const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
 
-    // planWaves with every wave's document built on the device (ka_plan_waves_json): docs[v] equals
-    // newAssignmentJson(planWaves(...).waves[v]). Topic names that org.json would escape take exactly that host path instead.
-    struct WaveDocs {
-        ka_status status;   // re-throw with throwForStatus; on an error summary and docs are empty
-        std::vector<ka_wave_summary> summary;
-        std::vector<std::string> docs;
-    };
-    WaveDocs planWavesJson(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
-                           const std::vector<std::map<int, int64_t>>& weights = {});
+public:
 
     // The KAG:172-186 loop and its "NEW ASSIGNMENT" text in one device call (ka_solve_json): only the text crosses PCIe.
     // Same solve and exceptions as solveTopics; the text equals newAssignmentJson(solveTopics(...)). Topic names that
@@ -616,13 +655,14 @@ inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicIn
     return std::string(json.get(), (size_t)bytes);
 }
 
-inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJson(const std::vector<TopicInput>& topics,
-                                                                      const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
-                                                                      const std::vector<std::map<int, int64_t>>& weights) {
+inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJsonWith(const std::vector<TopicInput>& topics,
+                                                                          const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                                                                          const SendBudget* send,
+                                                                          const std::vector<std::map<int, int64_t>>& weights) {
     for (const auto& t : topics)
         if (needsJsonEscape(t.name)) {   // the host emitter over the waves of planWaves
-            const WavePlan plan = planWaves(topics, proposed, maxBrokerIn, weights);
-            WaveDocs res{plan.status, plan.summary, {}};
+            const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights);
+            WaveDocs res{plan.status, plan.summary, {}, plan.sendSummary};
             for (const auto& wave : plan.waves) res.docs.push_back(newAssignmentJson(wave));
             return res;
         }
@@ -642,12 +682,22 @@ inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJson(const std:
     WaveDocs res{};
     res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
     int32_t W = 0;
-    ka_plan_waves_json(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), p.stride,
-                       p.newLen.data(), p.newBroker.data(), p.w.empty() ? nullptr : p.w.data(), maxBrokerIn, names.data(),
-                       nameOff.data(), json.get(), cap, docOff.data(), nullptr, &W, res.summary.data(), (int32_t)res.summary.size(),
-                       &res.status);
-    if (res.status.code != KA_OK) return WaveDocs{res.status, {}, {}};
+    const int64_t* w = p.w.empty() ? nullptr : p.w.data();
+    if (!send) {
+        ka_plan_waves_json(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), p.stride,
+                           p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, names.data(), nameOff.data(), json.get(), cap,
+                           docOff.data(), nullptr, &W, res.summary.data(), (int32_t)res.summary.size(), &res.status);
+    } else {
+        res.sendSummary.resize(res.summary.size());
+        ka_plan_waves_send_json(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
+                                p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, (int32_t)send->sendBrokers.size(),
+                                send->sendBrokers.data(), send->maxBrokerOut, names.data(), nameOff.data(), json.get(), cap,
+                                docOff.data(), nullptr, &W, res.summary.data(), res.sendSummary.data(), (int32_t)res.summary.size(),
+                                &res.status);
+    }
+    if (res.status.code != KA_OK) return WaveDocs{res.status, {}, {}, {}};
     res.summary.resize(W);
+    if (send) res.sendSummary.resize(W);
     for (int32_t v = 0; v < W; ++v) res.docs.emplace_back(json.get() + docOff[v], (size_t)(docOff[v + 1] - docOff[v]));
     return res;
 }
