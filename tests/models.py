@@ -1,0 +1,222 @@
+"""The plain-Python models the device is checked against, each written once: the move summary, the wave rule (with and
+without a sender budget), the reassignment JSON printers, the schedule model's records and the expected counter histogram.
+Each restates a rule of include/kassign.h. This module imports numpy and the status codes only: it never loads the library
+or the oracle, so CPU tests, GPU tests and tests/tools can all use it."""
+import numpy as np
+
+from kafka_assigner_b200 import _native
+
+BAD = _native.KA_ERR_BAD_ARG
+SLOTS = 8            # counter slots per broker (ka_ctx_counter_slots)
+INF = 0x3FFFFFFF     # the counters of the schedule model's dummy broker
+
+
+# ---- the move summary ----------------------------------------------------------------------------------------------------
+
+def move_summary(out, out_len, rep_off, cur, ids, weight=None):
+    """(summary dict, replicas, leaders, added) of one candidate's rows out [Q, S] / out_len [Q] against the current lists
+    cur[rep_off[g] .. rep_off[g + 1]), for the broker table `ids`. Position counts, as ka_move_summary defines them."""
+    Q, S = out.shape
+    m = np.diff(rep_off).astype(np.int64)
+    n = out_len.astype(np.int64)
+    w = np.ones(Q, dtype=np.int64) if weight is None else np.asarray(weight, dtype=np.int64)
+    pos = np.arange(S)
+    cmask, nmask = pos < m[:, None], pos < n[:, None]
+    cb = np.zeros((Q, S), dtype=np.int64)
+    cb[cmask] = cur[(rep_off[:-1, None] + pos)[cmask]]
+    nb = np.where(nmask, out, 0).astype(np.int64)
+    eq = nb[:, :, None] == cb[:, None, :]                       # [g, new position, current position]
+    added_pos = nmask & ~(eq & cmask[:, None, :]).any(2)
+    dropped_pos = cmask & ~(eq & nmask[:, :, None]).any(1)
+    n_add, n_drop = added_pos.sum(1), dropped_pos.sum(1)
+    changed = (n != m) | (nmask & cmask & (nb != cb)).any(1)
+    leader = (m == 0) | (n == 0) | (nb[:, 0] != cb[:, 0])
+    idx = np.searchsorted(ids, nb)
+    assert np.all(ids[idx[nmask]] == nb[nmask]), "a row holds a broker outside the table"
+    wq = np.broadcast_to(w[:, None], (Q, S))
+    rep, lead, inb = (np.zeros(len(ids), dtype=np.int64) for _ in range(3))
+    np.add.at(rep, idx[nmask], wq[nmask])
+    np.add.at(lead, idx[n > 0, 0], w[n > 0])
+    np.add.at(inb, idx[added_pos], wq[added_pos])
+    s = dict(rows_changed=int(changed.sum()), rows_moved=int(((n_add + n_drop) > 0).sum()), leaders_changed=int(leader.sum()),
+             replicas_added=int((w * n_add).sum()), replicas_dropped=int((w * n_drop).sum()))
+    if len(ids):
+        top = int(np.argmax(inb))   # the first maximum: the lowest id
+        s.update(max_broker_in=int(inb[top]), max_broker_in_id=int(ids[top]) if inb[top] > 0 else -1,
+                 max_broker_replicas=int(rep.max()), min_broker_replicas=int(rep.min()),
+                 max_broker_leaders=int(lead.max()), min_broker_leaders=int(lead.min()))
+    else:
+        s.update(max_broker_in=0, max_broker_in_id=-1, max_broker_replicas=0, min_broker_replicas=0, max_broker_leaders=0,
+                 min_broker_leaders=0)
+    return s, rep, lead, inb
+
+
+# ---- wave plans ----------------------------------------------------------------------------------------------------------
+
+def plan_waves(rep_off, cur, out, out_len, ids, B, weight=None, send=None):
+    """(wave [Q] int32, [summary dict per wave], (code, a, b)) of the wave rule, rows in input order.
+
+    send=None is ka_plan_waves: no broker receives more than B per wave; the five ka_wave_summary fields. send=(send_ids, C) is
+    ka_plan_waves_send: also no leader (the first broker of a row's current list) sends more than C per wave; the seven fields.
+    The lowest failing row wins: a new list naming a broker twice or a receiver missing from the table `ids` (at its first such
+    position), else, with a sender budget, a row with receivers whose leader is missing from `send_ids`: (KA_ERR_BAD_ARG, row,
+    id), and no plan."""
+    Q = len(out_len)
+    table = set(int(x) for x in ids)
+    senders, C = (None, None) if send is None else (set(int(x) for x in send[0]), send[1])
+    opened, load, sopen, sload = {}, {}, {}, {}
+    inb, outb = {}, {}                               # (wave, broker id) -> incoming / outgoing weight
+    wave = np.zeros(Q, dtype=np.int32)
+    recv_of = {}
+    for g in range(Q):
+        new = [int(x) for x in out[g][:int(out_len[g])]]
+        old = [int(x) for x in cur[int(rep_off[g]):int(rep_off[g + 1])]]
+        recv = []
+        for j, b in enumerate(new):
+            if b in new[:j] or (b not in old and b not in table):
+                return None, None, (BAD, g, b)
+            if b not in old:
+                recv.append(b)
+        if new == old:
+            continue
+        if not recv:
+            wave[g] = 1
+            continue
+        s = old[0] if send is not None and old else None
+        if s is not None and s not in senders:
+            return None, None, (BAD, g, s)
+        w = 1 if weight is None else int(weight[g])
+        a = w * len(recv)
+        v = max(opened.get(b, 1) if load.get(b, 0) == 0 or load.get(b, 0) + w <= B else opened.get(b, 1) + 1 for b in recv)
+        if s is not None:
+            o, x = sopen.get(s, 1), sload.get(s, 0)
+            v = max(v, o if x == 0 or x + a <= C else o + 1)
+        for b in recv:
+            if v > opened.get(b, 1):
+                opened[b], load[b] = v, w
+            else:
+                load[b] = load.get(b, 0) + w
+            inb[(v, b)] = inb.get((v, b), 0) + w
+        if s is not None:
+            if v > sopen.get(s, 1):
+                sopen[s], sload[s] = v, a
+            else:
+                sload[s] = sload.get(s, 0) + a
+            outb[(v, s)] = outb.get((v, s), 0) + a
+        wave[g] = v
+        recv_of[g] = (len(recv), w)
+    W = int(wave.max()) if Q else 0
+    empty = dict(rows=0, rows_moved=0, replicas_added=0, max_broker_in=0, max_broker_in_id=-1)
+    peaks = [(inb, "max_broker_in", "max_broker_in_id")]
+    if send is not None:
+        empty.update(max_broker_out=0, max_broker_out_id=-1)
+        peaks.append((outb, "max_broker_out", "max_broker_out_id"))
+    summ = [dict(empty) for _ in range(W)]
+    for g in np.nonzero(wave)[0]:
+        s = summ[wave[g] - 1]
+        s["rows"] += 1
+        if g in recv_of:
+            n, w = recv_of[g]
+            s["rows_moved"] += 1
+            s["replicas_added"] += n * w
+    for bins, peak, pid in peaks:
+        for (v, b), x in sorted(bins.items()):
+            s = summ[v - 1]
+            if x > s[peak]:
+                s[peak], s[pid] = x, b
+    return wave, summ, (0, 0, 0)
+
+
+# ---- reassignment JSON ---------------------------------------------------------------------------------------------------
+# The records of KafkaAssignmentGenerator.java:169-186 in the predicted org.json key order (SURVEY §3.4): "partition",
+# "replicas", "topic" inside {"partitions":[...],"version":1}.
+
+def quote(name):
+    """org.json JSONObject.quote() for the names these tests use."""
+    return '"' + name.replace("\\", "\\\\").replace('"', '\\"') + '"'
+
+
+def record(name, partition, replicas):
+    return '{"partition":%d,"replicas":[%s],"topic":%s}' % (partition, ",".join(str(int(b)) for b in replicas), quote(name))
+
+
+def document(records):
+    """The document of these records (str)."""
+    return '{"partitions":[' + ",".join(records) + '],"version":1}'
+
+
+EMPTY_DOCUMENT = document([])
+
+
+def solve_document(names, part_off, part_id, out, out_len):
+    """The text of ka_solve_json for the rows out [Q, S] / out_len [Q] of the topics `names` (partition ids part_id)."""
+    return document(record(name, part_id[g], out[g, :out_len[g]]) for t, name in enumerate(names)
+                    for g in range(int(part_off[t]), int(part_off[t + 1])))
+
+
+def dense_document(cl, out, out_len):
+    """The text of ka_solve_dense_json for the dense cluster cl's rows out [T * P, S] / out_len [T * P]."""
+    return solve_document(cl.topic_names, np.arange(cl.T + 1) * cl.P, np.tile(np.arange(cl.P), cl.T), out.reshape(cl.T * cl.P, -1),
+                          out_len.reshape(-1))
+
+
+def json_bound(names, part_off, stride):
+    """The sufficient json_cap of include/kassign.h for one document per wave."""
+    return sum(int(part_off[t + 1] - part_off[t]) * (79 + 12 * stride + len(n.encode())) for t, n in enumerate(names))
+
+
+def wave_docs(topic_names, part_off, part_id, rep_off, cur, out, out_len, ids, B, weight=None, send=None):
+    """(docs [bytes per wave], wave, summary, (code, a, b)): the waves of plan_waves, each printed as the device prints it: the
+    records of its rows in input row order; ordinals where part_id is None."""
+    wave, summ, st = plan_waves(rep_off, cur, out, out_len, ids, B, weight, send)
+    if st[0] != 0:
+        return None, wave, summ, st
+    recs = [[] for _ in summ]
+    for t, name in enumerate(topic_names):
+        for g in range(int(part_off[t]), int(part_off[t + 1])):
+            if wave[g]:
+                p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
+                recs[wave[g] - 1].append(record(name, p, out[g][:int(out_len[g])]))
+    return [document(r).encode() for r in recs], wave, summ, st
+
+
+# ---- the leader-order schedule and the counters --------------------------------------------------------------------------
+
+def java_abs_hash(h):
+    return int(np.int64(abs(int(h))) if h != -2**31 else 2**31)
+
+
+def build_records(cl, sets):
+    """What kernel A emits for every row: ([a0, a1, a2] in slot-0 scan order with the dummy N for missing slots, len, e01, e02, e12)."""
+    N = cl.N
+    idx_of = {int(b): i for i, b in enumerate(cl.broker_id)}
+    recs = []
+    for t in range(cl.T):
+        habs = java_abs_hash(cl.topic_hash[t])
+        s2, s3 = habs % 2, habs % 3
+        for p in range(cl.P):
+            ix = sorted(idx_of[int(b)] for b in sets[t][p])          # ascending index == ascending id (KAS:205-214)
+            k = len(ix)
+            a, e = [N, N, N], (0, 0, 0)
+            if k == 1:
+                a[0] = ix[0]
+            elif k == 2:
+                a[0], a[1] = ix[s2], ix[1 - s2]                       # |hash| % 2 == 1: the higher id is scanned first
+            elif k == 3:
+                i = [(3 - s3) % 3, (4 - s3) % 3, (5 - s3) % 3]        # list position at scan position 0, 1, 2
+                a = [ix[i[0]], ix[i[1]], ix[i[2]]]
+                e = tuple(s2 if i[x] < i[y] else 1 - s2 for x, y in ((0, 1), (0, 2), (1, 2)))
+            recs.append((a, k, e))
+    return recs
+
+
+def histogram(ids, out, out_len):
+    """counter[b][r] of a fresh Context after these rows: the number of rows with broker ids[b] at position r."""
+    ids = np.asarray(ids)
+    ctr = np.zeros((len(ids), SLOTS), dtype=np.int64)
+    for r in range(out.shape[1]):
+        sel = out_len > r
+        idx = np.searchsorted(ids, out[sel, r])
+        assert np.all(ids[idx] == out[sel, r])
+        np.add.at(ctr[:, r], idx, 1)
+    return ctr

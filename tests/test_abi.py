@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 import kafka_assigner_b200 as kab
+from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -51,15 +52,7 @@ def test_rack_indices_string_semantics(native_lib):
     assert np.array_equal(out, kab.synth.rack_indices(ids, [None, "13", None, "z"]))
 
 
-def _has_gpu():
-    try:
-        import torch
-        return torch.cuda.is_available()
-    except Exception:
-        return False
-
-
-@pytest.mark.skipif(_has_gpu(), reason="only meaningful on a box without a GPU")
+@pytest.mark.skipif(util.has_gpu(), reason="only meaningful on a box without a GPU")
 def test_no_gpu_fails_loudly(native_lib):
     assert not native_lib.ka_ctx_create(0)
     with pytest.raises(kab.KassignError):

@@ -1,5 +1,5 @@
 """ka_score_candidates: the batched ragged solve of ka_solve_candidates, summarised on the device per candidate (data moved and
-broker balance). Every summary must equal, field for field, the numpy reference below computed from ka_solve_candidates' rows;
+broker balance). Every summary must equal, field for field, the numpy reference models.move_summary computed from ka_solve_candidates' rows;
 statuses and (when asked for) rows must equal ka_solve_candidates' for the same call."""
 import ctypes
 import subprocess
@@ -10,55 +10,10 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import MOVE_SUMMARY_DTYPE
-from tests.test_ragged_candidates import FRACS, Problem, _check_equal, _exception_problem, _mixed_tables, _sparse_with_empty_topics, _table
+from tests import models, util
 
 FIELDS = MOVE_SUMMARY_DTYPE.names
 INT64_MAX = np.iinfo(np.int64).max
-
-
-def reference_summary(out, out_len, rep_off, cur, ids, weight=None):
-    """(summary dict, replicas, leaders, added) of one candidate's rows out [Q, S] / out_len [Q] against the current lists
-    cur[rep_off[g] .. rep_off[g + 1]), for the broker table `ids`. Position counts, as ka_move_summary defines them."""
-    Q, S = out.shape
-    m = np.diff(rep_off).astype(np.int64)
-    n = out_len.astype(np.int64)
-    w = np.ones(Q, dtype=np.int64) if weight is None else np.asarray(weight, dtype=np.int64)
-    pos = np.arange(S)
-    cmask, nmask = pos < m[:, None], pos < n[:, None]
-    cb = np.zeros((Q, S), dtype=np.int64)
-    cb[cmask] = cur[(rep_off[:-1, None] + pos)[cmask]]
-    nb = np.where(nmask, out, 0).astype(np.int64)
-    eq = nb[:, :, None] == cb[:, None, :]                       # [g, new position, current position]
-    added_pos = nmask & ~(eq & cmask[:, None, :]).any(2)
-    dropped_pos = cmask & ~(eq & nmask[:, :, None]).any(1)
-    n_add, n_drop = added_pos.sum(1), dropped_pos.sum(1)
-    changed = (n != m) | (nmask & cmask & (nb != cb)).any(1)
-    leader = (m == 0) | (n == 0) | (nb[:, 0] != cb[:, 0])
-    idx = np.searchsorted(ids, nb)
-    assert np.all(ids[idx[nmask]] == nb[nmask]), "a row holds a broker outside the table"
-    wq = np.broadcast_to(w[:, None], (Q, S))
-    rep, lead, inb = (np.zeros(len(ids), dtype=np.int64) for _ in range(3))
-    np.add.at(rep, idx[nmask], wq[nmask])
-    np.add.at(lead, idx[n > 0, 0], w[n > 0])
-    np.add.at(inb, idx[added_pos], wq[added_pos])
-    s = dict(rows_changed=int(changed.sum()), rows_moved=int(((n_add + n_drop) > 0).sum()), leaders_changed=int(leader.sum()),
-             replicas_added=int((w * n_add).sum()), replicas_dropped=int((w * n_drop).sum()))
-    if len(ids):
-        top = int(np.argmax(inb))   # the first maximum: the lowest id
-        s.update(max_broker_in=int(inb[top]), max_broker_in_id=int(ids[top]) if inb[top] > 0 else -1,
-                 max_broker_replicas=int(rep.max()), min_broker_replicas=int(rep.min()),
-                 max_broker_leaders=int(lead.max()), min_broker_leaders=int(lead.min()))
-    else:
-        s.update(max_broker_in=0, max_broker_in_id=-1, max_broker_replicas=0, min_broker_replicas=0, max_broker_leaders=0,
-                 min_broker_leaders=0)
-    return s, rep, lead, inb
-
-
-def _rec(s):
-    return {f: int(s[f]) for f in FIELDS}
-
-
-EMPTY = dict({f: 0 for f in FIELDS}, max_broker_in_id=-1)
 
 
 # ---- CPU -----------------------------------------------------------------------------------------------------------------
@@ -75,19 +30,19 @@ def test_reference_on_a_hand_written_case():
         out[g, :len(x)] = x
     out_len = np.array([len(x) for x in new_lists], dtype=np.int32)
     w = np.array([1, 10, 100, 1000, 10000], dtype=np.int64)
-    s, rep, lead, inb = reference_summary(out, out_len, rep_off, cur, ids, w)
+    s, rep, lead, inb = models.move_summary(out, out_len, rep_off, cur, ids, w)
     assert s == dict(rows_changed=4, rows_moved=3, leaders_changed=3, replicas_added=21100, replicas_dropped=100,
                      max_broker_in=10000, max_broker_in_id=2, max_broker_replicas=11001, min_broker_replicas=0,
                      max_broker_leaders=10000, min_broker_leaders=0)
     assert rep.tolist() == [111, 10011, 11001, 1100, 0]
     assert lead.tolist() == [11, 10000, 1000, 100, 0]
     assert inb.tolist() == [0, 10000, 10000, 1100, 0]
-    s1, rep1, lead1, inb1 = reference_summary(out, out_len, rep_off, cur, ids)
+    s1, rep1, lead1, inb1 = models.move_summary(out, out_len, rep_off, cur, ids)
     assert s1 == dict(rows_changed=4, rows_moved=3, leaders_changed=3, replicas_added=4, replicas_dropped=1, max_broker_in=2,
                       max_broker_in_id=4, max_broker_replicas=3, min_broker_replicas=0, max_broker_leaders=2, min_broker_leaders=0)
     assert rep1.tolist() == [3, 3, 3, 2, 0] and lead1.tolist() == [2, 1, 1, 1, 0] and inb1.tolist() == [0, 1, 1, 2, 0]
     # nothing added: no receiving broker
-    s2, _, _, _ = reference_summary(out[:1], out_len[:1], rep_off[:2], cur, ids)
+    s2, _, _, _ = models.move_summary(out[:1], out_len[:1], rep_off[:2], cur, ids)
     assert s2["replicas_added"] == 0 and s2["max_broker_in"] == 0 and s2["max_broker_in_id"] == -1
 
 
@@ -110,7 +65,7 @@ def test_without_a_context_is_no_device(native_lib):
                                         None, None, st)
     assert rc == _native.KA_ERR_NO_DEVICE
     assert [st[k].code for k in range(3)] == [_native.KA_ERR_NO_DEVICE] * 3
-    assert [_rec(s) for s in summary] == [EMPTY] * 3
+    assert [util.record_of(s, FIELDS) for s in summary] == [util.EMPTY_SUMMARY] * 3
     assert native_lib.ka_score_candidates(None, 1, None, None, None, 0, None, None, None, None, None, -1, 1, None,
                                           summary.ctypes.data_as(vp), None, None, None, None, None, None) == _native.KA_ERR_BAD_ARG
     assert native_lib.ka_score_candidates(None, 1, None, None, None, 0, None, None, None, None, None, -1, 1, None, None, None, None,
@@ -119,50 +74,18 @@ def test_without_a_context_is_no_device(native_lib):
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------------
 
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
-
-
-def _check_scores(prob, tables, weight=None, oracle=None, solver=None, sequential=True):
-    """One ka_score_candidates call (rows and per-broker arrays asked for) against ka_solve_candidates' rows (checked against
-    fresh single solves and the oracle when `sequential`) and the numpy reference. Returns the statuses and summaries."""
-    s = solver or kab.Solver(0)
-    if sequential:
-        sts = _check_equal(prob, tables, oracle, solver=s)
-        out, ln, _ = prob.batched(tables, s)
-    else:
-        out, ln, sts = prob.batched(tables, s)
-    summary, st, sc_out, sc_len, rep, lead, inb = s.score_ragged_candidates(tables, *prob.args(), out_stride=prob.S, weight=weight,
-                                                                           rows=True, per_broker=True)
-    assert [_fields(x) for x in st] == sts
-    w = np.ones(int(prob.part_off[-1]), dtype=np.int64) if weight is None else weight
-    for k, (ids, _) in enumerate(tables):
-        if sts[k][0] != 0:
-            assert _rec(summary[k]) == EMPTY, k
-            assert not rep[k].any() and not lead[k].any() and not inb[k].any(), k
-            continue
-        assert np.array_equal(sc_out[k], out[k]) and np.array_equal(sc_len[k], ln[k]), k
-        e, e_rep, e_lead, e_in = reference_summary(out[k], ln[k], prob.rep_off, prob.cur, np.asarray(ids, dtype=np.int64), weight)
-        assert _rec(summary[k]) == e, (k, _rec(summary[k]), e)
-        assert np.array_equal(rep[k], e_rep) and np.array_equal(lead[k], e_lead) and np.array_equal(inb[k], e_in), k
-        # identities
-        assert rep[k].sum() == int((w * ln[k]).sum()) and lead[k].sum() == int(w[ln[k] > 0].sum())
-        assert inb[k].sum() == summary[k]["replicas_added"]
-    return sts, summary
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_random_ragged_clusters(native_lib, oracle, seed):
     rng = np.random.default_rng(seed)
     cl = kab.synth.make_ragged_cluster(T=80, N=40, R=5, max_partitions=64, seed=seed, remove_frac=0.1)
-    tables = _mixed_tables(rng, cl)
+    tables = util.ragged_mixed_tables(rng, cl)
     n_ok = 0
     for desired_rf in (-1, 1, 2, 3):
-        prob = Problem(*_sparse_with_empty_topics(cl, rng, desired_rf > 0), desired_rf)
+        prob = util.Problem(*util.sparse_with_empty_topics(cl, rng, desired_rf > 0), desired_rf)
         Q = int(prob.part_off[-1])
         weight = rng.integers(0, 1 << 40, size=Q, dtype=np.int64)
-        sts, _ = _check_scores(prob, tables, weight, oracle if desired_rf in (-1, 2) else None)
+        sts, _ = util.check_scores(prob, tables, weight, oracle if desired_rf in (-1, 2) else None)
         n_ok += sum(st[0] == 0 for st in sts)
         assert sts[-1][0] == _native.KA_ERR_RF_GT_BROKERS
         # no weights == weights of one
@@ -175,18 +98,18 @@ def test_random_ragged_clusters(native_lib, oracle, seed):
 
 @pytest.mark.gpu
 def test_one_exception_per_candidate(native_lib, oracle):
-    A = _table(np.arange(1, 9, dtype=np.int32))
-    B = _table(np.arange(1, 3, dtype=np.int32))            # gamma: RF 3 > 2 brokers
-    C = _table(np.arange(1, 4, dtype=np.int32))            # polygenelubricants: hash index
-    D = _table(np.arange(1, 9, dtype=np.int32), 4)         # gamma: unassignable over two racks
-    E = _table(np.zeros(0, dtype=np.int32))                # no broker
+    A = util.table(np.arange(1, 9, dtype=np.int32))
+    B = util.table(np.arange(1, 3, dtype=np.int32))            # gamma: RF 3 > 2 brokers
+    C = util.table(np.arange(1, 4, dtype=np.int32))            # polygenelubricants: hash index
+    D = util.table(np.arange(1, 9, dtype=np.int32), 4)         # gamma: unassignable over two racks
+    E = util.table(np.zeros(0, dtype=np.int32))                # no broker
     kinds = set()
     for tail in ("mismatch", "empty", None):
-        prob = _exception_problem(tail)
-        sts, summary = _check_scores(prob, [A, B, C, D, E, A], oracle=oracle)
+        prob = util.exception_problem(tail)
+        sts, summary = util.check_scores(prob, [A, B, C, D, E, A], oracle=oracle)
         kinds |= {st[0] for st in sts}
         if tail is None:
-            assert sts[0][0] == sts[5][0] == 0 and _rec(summary[0]) == _rec(summary[5])
+            assert sts[0][0] == sts[5][0] == 0 and util.record_of(summary[0], FIELDS) == util.record_of(summary[5], FIELDS)
             assert summary[0]["rows_changed"] > 0
     assert kinds == {0, 1, 2, 3, 4, 5}
 
@@ -198,9 +121,9 @@ def test_c3_in_the_ragged_layout(native_lib):
     ids = [np.sort(rng.choice(cl.broker_id, len(cl.broker_id) - 20, replace=False)) for _ in range(8)]
     tables = [(i, cl.rack_index[np.searchsorted(cl.broker_id, i)]) for i in ids]
     part_off, part_id, rep_off, cur = cl.ragged()
-    prob = Problem(cl.topic_names, cl.topic_hash, part_off, part_id, rep_off, cur)
+    prob = util.Problem(cl.topic_names, cl.topic_hash, part_off, part_id, rep_off, cur)
     weight = rng.integers(1, 1 << 30, size=int(part_off[-1]), dtype=np.int64)
-    sts, summary = _check_scores(prob, tables, weight, sequential=False)
+    sts, summary = util.check_scores(prob, tables, weight, sequential=False)
     assert all(st[0] == 0 for st in sts) and np.all(summary["replicas_added"] > 0)
 
 
@@ -209,21 +132,21 @@ def test_million_partition_cluster_at_k32(native_lib):
     cl = kab.synth.make_ragged_cluster(T=240000, N=400, max_partitions=128, seed=11)
     assert cl.Q > 1_000_000
     rng = np.random.default_rng(32)
-    tables = kab.synth.ragged_decommission_tables(cl, FRACS)
+    tables = kab.synth.ragged_decommission_tables(cl, util.FRACS)
     tables += [(cl.broker_id[k], cl.rack_index[k]) for k in (np.sort(rng.choice(len(cl.broker_id), 392, replace=False))
                                                                for _ in range(32 - len(tables)))]
-    prob = Problem.of(cl)
+    prob = util.Problem.of(cl)
     s = kab.Solver(0)
     out, ln, sts = prob.batched(tables, s)
     weight = rng.integers(0, 1 << 36, size=cl.Q, dtype=np.int64)
     summary, st = s.score_ragged_candidates(tables, *prob.args(), weight=weight)
-    assert [_fields(x) for x in st] == sts and sum(x[0] == 0 for x in sts) >= 24
+    assert [util.fields(x) for x in st] == sts and sum(x[0] == 0 for x in sts) >= 24
     for k, (ids, _) in enumerate(tables):
         if sts[k][0] == 0:
-            e, _, _, _ = reference_summary(out[k], ln[k], prob.rep_off, prob.cur, np.asarray(ids, dtype=np.int64), weight)
-            assert _rec(summary[k]) == e, k
+            e, _, _, _ = models.move_summary(out[k], ln[k], prob.rep_off, prob.cur, np.asarray(ids, dtype=np.int64), weight)
+            assert util.record_of(summary[k], FIELDS) == e, k
         else:
-            assert _rec(summary[k]) == EMPTY, k
+            assert util.record_of(summary[k], FIELDS) == util.EMPTY_SUMMARY, k
 
 
 @pytest.mark.gpu
@@ -233,12 +156,12 @@ def test_ctx_is_untouched(native_lib):
     s, fresh = kab.Solver(0), kab.Solver(0)
     for x in (s, fresh):
         x.set_brokers(cl.broker_id, cl.rack_index)
-        x.solve_ragged(*Problem.of(half).args(), 3)
+        x.solve_ragged(*util.Problem.of(half).args(), 3)
     before = s.counters()
-    _check_scores(Problem.of(cl), kab.synth.ragged_decommission_tables(cl, (0.1, 0.3)), solver=s, sequential=False)
+    util.check_scores(util.Problem.of(cl), kab.synth.ragged_decommission_tables(cl, (0.1, 0.3)), solver=s, sequential=False)
     assert np.array_equal(s.counters(), before) and np.array_equal(s.broker_id, cl.broker_id)
-    a, al, ast = s.solve_ragged(*Problem.of(cl).args(), 3)
-    b, bl, bst = fresh.solve_ragged(*Problem.of(cl).args(), 3)
+    a, al, ast = s.solve_ragged(*util.Problem.of(cl).args(), 3)
+    b, bl, bst = fresh.solve_ragged(*util.Problem.of(cl).args(), 3)
     assert ast.code == bst.code == 0 and np.array_equal(a, b) and np.array_equal(al, bl)
     assert np.array_equal(s.counters(), fresh.counters())
 
@@ -246,7 +169,7 @@ def test_ctx_is_untouched(native_lib):
 @pytest.mark.gpu
 def test_launches_do_not_depend_on_k(native_lib):
     cl = kab.synth.make_ragged_cluster(T=3000, N=120, R=6, seed=21)
-    prob = Problem.of(cl)
+    prob = util.Problem.of(cl)
     s = kab.Solver(0)
     counts = []
     for K in (1, 8):
@@ -285,7 +208,7 @@ def _call(fn, s, prob, tables, st, K=None, out_stride=None, T=None, part_off=Non
 @pytest.mark.gpu
 def test_arguments_and_limits(native_lib):
     cl = kab.synth.make_ragged_cluster(T=40, N=30, R=5, seed=5)
-    prob = Problem.of(cl)
+    prob = util.Problem.of(cl)
     Q = int(prob.part_off[-1])
     good = [(cl.broker_id, cl.rack_index)]
     s = kab.Solver(0)
@@ -296,7 +219,7 @@ def test_arguments_and_limits(native_lib):
         rc = _call("score", s, *a, st, **kw)
         kw.pop("weight", None)
         assert _call("solve", s, *a, st2, **kw) == rc, (rc, kw)
-        assert [_fields(st[k]) for k in range(len(a[1]))] == [_fields(st2[k]) for k in range(len(a[1]))], kw
+        assert [util.fields(st[k]) for k in range(len(a[1]))] == [util.fields(st2[k]) for k in range(len(a[1]))], kw
         return rc
 
     assert same(prob, []) == 0
@@ -332,18 +255,18 @@ def test_arguments_and_limits(native_lib):
     # at the largest total weight the sums are still exact
     summary, sts = s.score_ragged_candidates(good, *prob.args(), weight=np.where(np.arange(Q) == 3, edge - 1, edge))
     out, ln, _ = prob.batched(good, s)
-    e, _, _, _ = reference_summary(out[0], ln[0], prob.rep_off, prob.cur, cl.broker_id.astype(np.int64),
-                                   np.where(np.arange(Q) == 3, edge - 1, edge))
-    assert sts[0].code == 0 and _rec(summary[0]) == e
+    e, _, _, _ = models.move_summary(out[0], ln[0], prob.rep_off, prob.cur, cl.broker_id.astype(np.int64),
+                                     np.where(np.arange(Q) == 3, edge - 1, edge))
+    assert sts[0].code == 0 and util.record_of(summary[0], FIELDS) == e
     # T == 0: zero summaries and per-broker entries
     summary, sts, rep, lead, inb = s.score_ragged_candidates(good * 2, prob.topic_hash[:0], prob.part_off[:1], None, prob.rep_off[:1],
                                                              prob.cur[:0], -1, out_stride=3, per_broker=True)
-    assert [_rec(x) for x in summary] == [EMPTY] * 2 and all(x.code == 0 for x in sts)
+    assert [util.record_of(x, FIELDS) for x in summary] == [util.EMPTY_SUMMARY] * 2 and all(x.code == 0 for x in sts)
     assert all(len(a) == len(cl.broker_id) and not a.any() for a in rep + lead + inb)
     # K * ΣP at 2^31: refused before anything is written
     big_q = (1 << 31) // 128
-    big = Problem(["t"], prob.topic_hash[:1], np.array([0, big_q], dtype=np.int64), None, np.zeros(big_q + 1, dtype=np.int64),
-                  np.zeros(0, dtype=np.int32), 1, 1)
+    big = util.Problem(["t"], prob.topic_hash[:1], np.array([0, big_q], dtype=np.int64), None, np.zeros(big_q + 1, dtype=np.int64),
+                       np.zeros(0, dtype=np.int32), 1, 1)
     assert same(big, good * 128, out_elems=1) == _native.KA_ERR_LIMIT
 
 

@@ -10,88 +10,21 @@ import pytest
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
+from tests import util
 
 pytestmark = pytest.mark.gpu
 
 DECOMMISSION_FRACS = (0.01, 0.02, 0.05, 0.10, 0.20, 0.30, 0.40, 0.50)
 
 
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
-
-
-class Problem:
-    """A dense problem on the device: topic hashes, current lists, and room for K candidates' rows."""
-
-    def __init__(self, topic_hash, cur, desired_rf=-1, out_stride=None):
-        import torch
-        self.T, self.P, self.RF = cur.shape
-        self.desired_rf = desired_rf
-        self.S = out_stride or max(self.RF, desired_rf, 1)
-        self.topic_hash, self.cur = topic_hash, cur
-        self.d_hash = torch.from_numpy(np.ascontiguousarray(topic_hash, dtype=np.int32)).cuda()
-        self.d_cur = torch.from_numpy(np.ascontiguousarray(cur, dtype=np.int32)).cuda()
-
-    def sequential(self, tables):
-        """The contract's reference: a fresh context per table, ka_ctx_set_brokers + ka_solve_dense_device."""
-        import torch
-        rows = []
-        for ids, racks in tables:
-            s = kab.Solver(0)
-            s.set_brokers(ids, racks)
-            out = torch.full((self.T, self.P, self.S), -7, dtype=torch.int32, device="cuda")
-            ln = torch.full((self.T, self.P), -7, dtype=torch.int32, device="cuda")
-            st = s.solve_dense_device(self.T, self.d_hash.data_ptr(), self.P, self.RF, self.d_cur.data_ptr(), self.desired_rf,
-                                      self.S, ln.data_ptr(), out.data_ptr())
-            rows.append((out.cpu().numpy(), ln.cpu().numpy(), _fields(st)))
-            s.close()
-        return rows
-
-    def batched(self, tables, solver=None):
-        import torch
-        K = len(tables)
-        out = torch.full((K, self.T, self.P, self.S), -7, dtype=torch.int32, device="cuda")
-        ln = torch.full((K, self.T, self.P), -7, dtype=torch.int32, device="cuda")
-        s = solver or kab.Solver(0)
-        sts = s.solve_dense_candidates_device(tables, self.T, self.d_hash.data_ptr(), self.P, self.RF, self.d_cur.data_ptr(),
-                                              self.desired_rf, self.S, ln.data_ptr(), out.data_ptr())
-        return out.cpu().numpy(), ln.cpu().numpy(), [_fields(st) for st in sts]
-
-
-def _check_equal(prob, tables, oracle=None, solver=None):
-    out, ln, sts = prob.batched(tables, solver)
-    seq = prob.sequential(tables)
-    for k, (e_out, e_len, e_st) in enumerate(seq):
-        assert sts[k] == e_st, (k, sts[k], e_st)
-        if e_st[0] != 0:
-            continue   # the rows of a failed candidate are unspecified
-        assert np.array_equal(out[k], e_out), k
-        assert np.array_equal(ln[k], e_len), k
-        if oracle is not None:
-            ids, racks = tables[k]
-            exp, exp_len, est = oracle.fast_run_dense(oracle.FastContext(), prob.topic_hash, prob.cur, ids, racks, prob.desired_rf,
-                                                      prob.S)
-            assert est.code == 0, k
-            assert np.array_equal(out[k].reshape(-1, prob.S), exp), k
-            assert np.array_equal(ln[k].reshape(-1), exp_len), k
-    return sts
-
-
-def _table(ids, racks_per=None):
-    """(ids, rack_index): racks_per = brokers per rack (contiguous), or None: no broker has a rack."""
-    ids = np.asarray(ids, dtype=np.int32)
-    names = [None] * len(ids) if racks_per is None else ["k%d" % (i // racks_per) for i in range(len(ids))]
-    return ids, kab.synth.rack_indices(ids, names)
-
-
 def _mixed_tables(rng, cl):
     old = cl.broker_id
     return [
-        _table(np.sort(rng.choice(old, len(old) - 3, replace=False)), 2),                  # capacity > 1, racks
-        _table(np.sort(rng.choice(old, len(old) - 5, replace=False))),                     # capacity > 1, no racks
-        _table(np.arange(1000, 1000 + 4000, dtype=np.int32), 40),                          # capacity 1, racks
-        _table(np.arange(900, 900 + 3000, dtype=np.int32)),                                # capacity 1, no racks
-        _table(1000 + 2 * np.arange(20000, dtype=np.int32), 500),                          # 20 000 brokers, global id LUT
+        util.table(np.sort(rng.choice(old, len(old) - 3, replace=False)), 2),                  # capacity > 1, racks
+        util.table(np.sort(rng.choice(old, len(old) - 5, replace=False))),                     # capacity > 1, no racks
+        util.table(np.arange(1000, 1000 + 4000, dtype=np.int32), 40),                          # capacity 1, racks
+        util.table(np.arange(900, 900 + 3000, dtype=np.int32)),                                # capacity 1, no racks
+        util.table(1000 + 2 * np.arange(20000, dtype=np.int32), 500),                          # 20 000 brokers, global id LUT
     ]
 
 
@@ -100,18 +33,18 @@ def test_random_dense_clusters_match_sequential_and_oracle(native_lib, oracle, s
     rng = np.random.default_rng(seed)
     for RF, desired_rf in ((1, -1), (2, -1), (3, -1), (2, 3), (3, 2), (1, 2)):
         cl = kab.synth.make_cluster(T=40, P=16, RF=RF, N=24, R=4, seed=seed * 101 + RF, kind="mixed")
-        prob = Problem(cl.topic_hash, cl.cur, desired_rf)
+        prob = util.DenseProblem(cl.topic_hash, cl.cur, desired_rf)
         tables = _mixed_tables(rng, cl)
-        _check_equal(prob, tables, oracle)
+        util.check_dense_equal(prob, tables, oracle)
         if RF == 3 and desired_rf == -1:   # the same call with every counter column in global memory
             with mock.patch.dict(os.environ, {"KA_ORDER_GLOBAL_CTR": "1"}):
-                _check_equal(prob, tables, oracle)
+                util.check_dense_equal(prob, tables, oracle)
 
 
 def test_baseline_c2_k4(native_lib, oracle):
     cl = kab.synth.make_config("c2", "mixed")
     tables = kab.synth.decommission_tables("c2", (0.0, 0.05, 0.1, 0.2))
-    _check_equal(Problem(cl.topic_hash, cl.cur), tables, oracle)
+    util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), tables, oracle)
 
 
 def test_baseline_c3_k8(native_lib):
@@ -119,23 +52,23 @@ def test_baseline_c3_k8(native_lib):
     rng = np.random.default_rng(3)
     tables = [(np.sort(rng.choice(cl.broker_id, len(cl.broker_id) - 20, replace=False)),) for _ in range(8)]
     tables = [(ids, cl.rack_index[np.searchsorted(cl.broker_id, ids)]) for (ids,) in tables]
-    assert all(st[0] == 0 for st in _check_equal(Problem(cl.topic_hash, cl.cur), tables))
+    assert all(st[0] == 0 for st in util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), tables))
 
 
 def test_baseline_c5_decommission_sweep(native_lib):
     cl = kab.synth.make_config("c5", "mixed")
     tables = kab.synth.decommission_tables("c5", DECOMMISSION_FRACS)
-    assert all(st[0] == 0 for st in _check_equal(Problem(cl.topic_hash, cl.cur), tables))
+    assert all(st[0] == 0 for st in util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), tables))
 
 
 def test_per_candidate_failures(native_lib):
     cl = kab.synth.make_cluster(T=30, P=12, RF=3, N=24, R=4, seed=77, kind="mixed")
     good = (cl.broker_id, cl.rack_index)
-    too_small = _table(cl.broker_id[:2], 1)                 # fewer brokers than RF
-    two_racks = _table(cl.broker_id, 12)                    # RF 3 over two racks
-    tables = [good, too_small, good, two_racks, _table(np.zeros(0, dtype=np.int32)), good]
-    prob = Problem(cl.topic_hash, cl.cur)
-    sts = _check_equal(prob, tables)
+    too_small = util.table(cl.broker_id[:2], 1)                 # fewer brokers than RF
+    two_racks = util.table(cl.broker_id, 12)                    # RF 3 over two racks
+    tables = [good, too_small, good, two_racks, util.table(np.zeros(0, dtype=np.int32)), good]
+    prob = util.DenseProblem(cl.topic_hash, cl.cur)
+    sts = util.check_dense_equal(prob, tables)
     assert sts[1][0] == _native.KA_ERR_RF_GT_BROKERS and sts[3][0] == _native.KA_ERR_UNASSIGNABLE
     assert sts[0][0] == sts[2][0] == sts[5][0] == 0
     # return code: the status of the lowest failing candidate
@@ -166,7 +99,7 @@ def test_ctx_is_untouched(native_lib):
         x.set_brokers(cl.broker_id, cl.rack_index)
         x.solve_dense(half.topic_hash, half.cur)   # some counters in the Context
     before = s.counters()
-    prob = Problem(cl.topic_hash, cl.cur)
+    prob = util.DenseProblem(cl.topic_hash, cl.cur)
     prob.batched(kab.synth.decommission_tables("c2", (0.1, 0.3)), solver=s)
     assert np.array_equal(s.counters(), before) and np.array_equal(s.broker_id, cl.broker_id)
     a, al, ast = s.solve_dense(cl.topic_hash, cl.cur)
@@ -177,7 +110,7 @@ def test_ctx_is_untouched(native_lib):
 
 def test_launches_do_not_depend_on_k(native_lib):
     cl = kab.synth.make_config("c2", "mixed")
-    prob = Problem(cl.topic_hash, cl.cur)
+    prob = util.DenseProblem(cl.topic_hash, cl.cur)
     s = kab.Solver(0)
     counts = []
     for K in (1, 8):
@@ -189,7 +122,7 @@ def test_launches_do_not_depend_on_k(native_lib):
 
 def test_arguments(native_lib):
     cl = kab.synth.make_cluster(T=10, P=8, RF=3, N=12, R=4, seed=5, kind="mixed")
-    prob = Problem(cl.topic_hash, cl.cur)
+    prob = util.DenseProblem(cl.topic_hash, cl.cur)
     good = [(cl.broker_id, cl.rack_index)]
     s = kab.Solver(0)
     st = (kab.KaStatus * 200)()

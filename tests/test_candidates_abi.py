@@ -5,10 +5,10 @@ import numpy as np
 import pytest
 
 import kafka_assigner_b200 as kab
-from tests.test_abi import _has_gpu
+from tests import util
 
 
-@pytest.mark.skipif(_has_gpu(), reason="only meaningful on a box without a GPU")
+@pytest.mark.skipif(util.has_gpu(), reason="only meaningful on a box without a GPU")
 def test_candidates_without_a_context_is_no_device(native_lib):
     st = (kab.KaStatus * 2)()
     cand_off = np.array([0, 1, 2], dtype=np.int32)

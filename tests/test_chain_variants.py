@@ -24,12 +24,11 @@ import pytest
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
-from tests import util
+from tests import models, util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 GENERAL, WARP1, SINGLE, FULL = 0, 1, 2, 3
-SLOTS = 8   # counter slots per broker (ka_ctx_counter_slots)
 GCTR = {"KA_ORDER_GLOBAL_CTR": "1"}
 
 
@@ -250,18 +249,6 @@ def test_last_order_plan_null_arguments(native_lib):
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------------
 
-def _histogram(ids, out, out_len):
-    """counter[b][r] of a fresh Context after these rows: the number of rows with broker ids[b] at position r."""
-    ids = np.asarray(ids)
-    ctr = np.zeros((len(ids), SLOTS), dtype=np.int64)
-    for r in range(out.shape[1]):
-        sel = out_len > r
-        idx = np.searchsorted(ids, out[sel, r])
-        assert np.all(ids[idx] == out[sel, r])
-        np.add.at(ctr[:, r], idx, 1)
-    return ctr
-
-
 def _cluster(g, seed):
     cl = kab.synth.make_cluster(T=g["T"], P=g["P"], RF=g["RF"], N=g["N"], R=g["R"], seed=seed, kind="mixed")
     cl.desired_rf = g.get("desired_rf", -1)
@@ -284,28 +271,26 @@ def test_single_solve_variant(native_lib, oracle, case):
     assert st.code == 0, (st.code, st.topic_index, st.a, st.b)
     assert np.array_equal(out.reshape(-1, S), exp)
     assert np.array_equal(out_len.reshape(-1), exp_len)
-    assert np.array_equal(s.counters(), _histogram(cl.broker_id, exp, exp_len))
+    assert np.array_equal(s.counters(), models.histogram(cl.broker_id, exp, exp_len))
 
 
 def _cand_tables(cl, g, base):
-    from tests.test_candidates import _table
     tables = [(cl.broker_id, cl.rack_index)]
     for spec in g["tables"]:
         n, per, step = (tuple(spec) + (1,))[:3]
-        tables.append(_table(base + step * np.arange(n, dtype=np.int32), per))
+        tables.append(util.table(base + step * np.arange(n, dtype=np.int32), per))
     return tables
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CAND_CASES, ids=[c["id"] for c in CAND_CASES])
 def test_dense_candidates_variant(native_lib, oracle, case):
-    from tests.test_candidates import Problem, _check_equal
     g = case["gen"]
     cl = _cluster(g, _seed(case["id"]))
     tables = _cand_tables(cl, g, 1000)
     s = kab.Solver(0)
     with mock.patch.dict(os.environ, case["env"]):
-        sts = _check_equal(Problem(cl.topic_hash, cl.cur), tables, oracle, solver=s)
+        sts = util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), tables, oracle, solver=s)
     assert s.last_order_plan() == case["plan"]
     assert all(st[0] == 0 for st in sts), sts
 
@@ -313,13 +298,12 @@ def test_dense_candidates_variant(native_lib, oracle, case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", RAGGED_CAND_CASES, ids=[c["id"] for c in RAGGED_CAND_CASES])
 def test_ragged_candidates_variant(native_lib, oracle, case):
-    from tests.test_ragged_candidates import Problem, _check_equal
     g = case["gen"]
     cl = kab.synth.make_ragged_cluster(T=80, N=40, R=5, max_partitions=64, seed=g["seed"], remove_frac=0.1)
     tables = _cand_tables(cl, g, 1)
     s = kab.Solver(0)
     with mock.patch.dict(os.environ, case["env"]):
-        sts = _check_equal(Problem.of(cl), tables, oracle, solver=s)
+        sts = util.check_equal(util.Problem.of(cl), tables, oracle, solver=s)
     assert s.last_order_plan() == case["plan"]
     assert all(st[0] == 0 for st in sts), sts
 
@@ -336,7 +320,7 @@ def test_one_context_across_variants(native_lib, oracle):
         cl = kab.synth.make_cluster(T=g["T"], P=g["P"], RF=g["RF"], N=SEQUENCE_N, R=SEQUENCE_R, seed=0x5E0 + i, kind="mixed")
         if ids is None:
             ids = cl.broker_id
-            total = np.zeros((len(ids), SLOTS), dtype=np.int64)
+            total = np.zeros((len(ids), models.SLOTS), dtype=np.int64)
         assert np.array_equal(cl.broker_id, ids)
         exp, exp_len, est = oracle.fast_run_dense(fctx, cl.topic_hash, cl.cur, cl.broker_id, cl.rack_index)
         assert est.code == 0
@@ -346,7 +330,7 @@ def test_one_context_across_variants(native_lib, oracle):
         assert st.code == 0, case["id"]
         assert np.array_equal(out.reshape(-1, cl.RF), exp), case["id"]
         assert np.array_equal(out_len.reshape(-1), exp_len), case["id"]
-        total += _histogram(ids, exp, exp_len)
+        total += models.histogram(ids, exp, exp_len)
         assert np.array_equal(s.counters(), total), case["id"]
 
 
@@ -390,9 +374,8 @@ def _lut_universe():
 
 
 def _lut_tables(universe, small):
-    from tests.test_candidates import _table
     mid = universe[(universe > -40001) & (universe < 40001)]
-    tables = [_table(small, 5), _table(mid), _table(universe, 7), _table(universe[universe < 0])]
+    tables = [util.table(small, 5), util.table(mid), util.table(universe, 7), util.table(universe[universe < 0])]
     modes = []
     for ids, _ in tables:
         rng_ = int(ids[-1]) - int(ids[0]) + 1
@@ -405,27 +388,24 @@ def _lut_tables(universe, small):
 def test_lookup_modes_in_one_batch(native_lib, oracle):
     """Candidate tables in the shared-memory LUT, global LUT and binary-search modes, alone and mixed in one batch, through
     the dense and ragged candidate solves and the candidate score (which looks the per-broker sums up by id)."""
-    from tests import test_candidates as tc
-    from tests import test_ragged_candidates as trc
-    from tests.test_candidate_scores import _check_scores
     universe, small = _lut_universe()
     tables = _lut_tables(universe, small)
     # dense: make_cluster's brokers 1000 + i renamed to the universe's ids (ascending: rack order is kept)
     cl = kab.synth.make_cluster(T=30, P=30, RF=3, N=len(universe), R=6, seed=41, kind="mixed")
     cur = universe[cl.cur - 1000]
-    prob = tc.Problem(cl.topic_hash, cur)
+    prob = util.DenseProblem(cl.topic_hash, cur)
     for batch in ([tables[0]], [tables[1]], [tables[2]], tables):
         s = kab.Solver(0)
-        sts = tc._check_equal(prob, batch, oracle, solver=s)
+        sts = util.check_dense_equal(prob, batch, oracle, solver=s)
         assert all(st[0] == 0 for st in sts), sts
         if len(batch) == 4:
             assert s.last_order_plan() == LUT_DENSE_PLAN
     # ragged: brokers 1..N renamed
     rc = kab.synth.make_ragged_cluster(T=60, N=len(universe), R=6, max_partitions=40, seed=43)
-    rprob = trc.Problem(rc.topic_names, rc.topic_hash, rc.part_off, rc.part_id, rc.rep_off, universe[rc.cur - 1])
+    rprob = util.Problem(rc.topic_names, rc.topic_hash, rc.part_off, rc.part_id, rc.rep_off, universe[rc.cur - 1])
     for batch in ([tables[0]], [tables[1]], [tables[2]], tables):
         s = kab.Solver(0)
-        sts, _ = _check_scores(rprob, batch, oracle=oracle, solver=s)
+        sts, _ = util.check_scores(rprob, batch, oracle=oracle, solver=s)
         assert all(st[0] == 0 for st in sts), sts
         if len(batch) == 4:
             assert s.last_order_plan() == LUT_RAGGED_PLAN
@@ -435,9 +415,8 @@ def test_lookup_modes_in_one_batch(native_lib, oracle):
 def test_level_scratch_limit_is_a_clean_error(native_lib, oracle):
     """A ragged table beyond kernel A's level scratch (30 000 brokers) is refused with KA_ERR_LIMIT, b = N, by every ragged
     entry point, before anything runs."""
-    from tests import test_ragged_candidates as trc
     cl = kab.synth.make_ragged_cluster(T=20, N=30000, R=10, max_partitions=32, seed=9)
-    prob = trc.Problem.of(cl)
+    prob = util.Problem.of(cl)
     key = lambda st: (st.code, st.topic_index, st.partition, st.a, st.b)   # noqa: E731
     s = kab.Solver(0)
     s.set_brokers(cl.broker_id, cl.rack_index)

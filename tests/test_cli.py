@@ -9,6 +9,7 @@ import pytest
 
 import kafka_assigner_b200 as kab
 from oracle import py_oracle as po
+from tests import models
 
 BROKERS = [dict(id=10 + i, host="h%d" % (10 + i), port=9092, rack="abcd"[i % 4]) for i in range(8)] + [dict(id=18, host="h18", port=9093)]
 TOPICS = {"test": {0: [10, 11], 1: [11, 12], 2: [12, 10], 3: [10, 12]},
@@ -37,8 +38,7 @@ def run(cli, *args):
 
 def expected_new_assignment(topic_names, brokers, racks, desired=-1):
     recs = po.run_topics([(t, TOPICS[t]) for t in topic_names], brokers, racks, desired)
-    body = ",".join('{"partition":%d,"replicas":[%s],"topic":"%s"}' % (p, ",".join(map(str, r)), t) for t, p, r in recs)
-    return '{"partitions":[' + body + '],"version":1}'
+    return models.document(models.record(t, p, r) for t, p, r in recs)
 
 
 def expected_current(topic_names):

@@ -1,5 +1,5 @@
 """ka_score_clusters: the fleet of ka_solve_clusters, summarised on the device per cluster (data moved and broker balance). Every
-cluster's summary and per-broker sums must equal the numpy reference of tests/test_candidate_scores.py over that cluster's rows
+cluster's summary and per-broker sums must equal the numpy reference (models.move_summary) over that cluster's rows
 from ka_solve_clusters, and what ka_score_candidates gives for the cluster alone with its one table; statuses and (when asked
 for) rows must equal ka_solve_clusters' for the same call."""
 import ctypes
@@ -13,21 +13,12 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import MOVE_SUMMARY_DTYPE
-from tests.test_candidate_scores import reference_summary
-from tests.test_clusters import MIN_HASH, Member, _bsearch_table, _min_hash_cluster, _stride, _table
+from tests import models, util
+from tests.util import MIN_HASH, Member
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 FIELDS = MOVE_SUMMARY_DTYPE.names
-EMPTY = dict({f: 0 for f in FIELDS}, max_broker_in_id=-1)
 INT64_MAX = np.iinfo(np.int64).max
-
-
-def _rec(s):
-    return {f: int(s[f]) for f in FIELDS}
-
-
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
 
 
 # ---- CPU -----------------------------------------------------------------------------------------------------------------
@@ -52,7 +43,7 @@ def test_without_a_context_is_no_device(native_lib):
                              p(summary), None, None, None, None, None, st)
     assert rc == _native.KA_ERR_NO_DEVICE
     assert [st[k].code for k in range(3)] == [_native.KA_ERR_NO_DEVICE] * 3
-    assert [_rec(s) for s in summary] == [EMPTY] * 3
+    assert [util.record_of(s, FIELDS) for s in summary] == [util.EMPTY_SUMMARY] * 3
     assert L.ka_score_clusters(None, 1, None, None, None, None, None, None, None, None, None, None, 1, None, p(summary), None, None,
                                None, None, None, None) == _native.KA_ERR_BAD_ARG          # st is required
     assert L.ka_score_clusters(None, 1, None, None, None, None, None, None, None, None, None, None, 1, None, None, None, None, None,
@@ -79,7 +70,7 @@ def _check_scores(fleet, weights=None, S=None, solver=None, single=True):
     """One score_clusters call (rows and per-broker sums asked for) against solve_clusters' statuses and rows, the numpy
     reference of each cluster's rows, and (single) score_ragged_candidates of each cluster alone with its one table. Returns
     the statuses and summaries."""
-    S = S or _stride(fleet)
+    S = S or util.fleet_stride(fleet)
     s = solver or kab.Solver(0)
     entries = [m.entry() for m in fleet]
     solved = s.solve_clusters(entries, out_stride=S)
@@ -87,24 +78,24 @@ def _check_scores(fleet, weights=None, S=None, solver=None, single=True):
     assert len(res) == len(fleet)
     sts = []
     for k, (m, (out, ln, st), (summ, sst, sc_out, sc_len, rep, lead, inb)) in enumerate(zip(fleet, solved, res)):
-        assert _fields(sst) == _fields(st), (k, _fields(sst), _fields(st))
-        sts.append(_fields(st))
+        assert util.fields(sst) == util.fields(st), (k, util.fields(sst), util.fields(st))
+        sts.append(util.fields(st))
         ids = np.asarray(m.ids, dtype=np.int64)
         assert len(rep) == len(lead) == len(inb) == len(ids)
         if st.code != 0:
-            assert _rec(summ) == EMPTY, k
+            assert util.record_of(summ, FIELDS) == util.EMPTY_SUMMARY, k
             assert not rep.any() and not lead.any() and not inb.any(), k
             continue
         assert np.array_equal(sc_out, out) and np.array_equal(sc_len, ln), k
         w = None if weights is None else weights[k]
         rep_off = np.asarray(m.rep_off, dtype=np.int64) if len(m.rep_off) else np.zeros(1, dtype=np.int64)
-        e, e_rep, e_lead, e_in = reference_summary(out, ln, rep_off, np.asarray(m.cur), ids, w)
-        assert _rec(summ) == e, (k, _rec(summ), e)
+        e, e_rep, e_lead, e_in = models.move_summary(out, ln, rep_off, np.asarray(m.cur), ids, w)
+        assert util.record_of(summ, FIELDS) == e, (k, util.record_of(summ, FIELDS), e)
         assert np.array_equal(rep, e_rep) and np.array_equal(lead, e_lead) and np.array_equal(inb, e_in), k
         if single:
             one, ost, *brk = kab.Solver(0).score_ragged_candidates([(m.ids, m.racks)], m.topic_hash, m.part_off, m.part_id, m.rep_off,
                                                                   m.cur, m.desired_rf, out_stride=S, weight=w, per_broker=True)
-            assert _fields(ost[0]) == _fields(st) and _rec(one[0]) == _rec(summ), k
+            assert util.fields(ost[0]) == util.fields(st) and util.record_of(one[0], FIELDS) == util.record_of(summ, FIELDS), k
             assert all(np.array_equal(a[0], b) for a, b in zip(brk, (rep, lead, inb))), k
     return sts, [r[0] for r in res]
 
@@ -121,10 +112,10 @@ def test_heterogeneous_fleet(native_lib, seed):
         Member.of(mk(T=25, N=20, R=3, seed=seed + 30, rf_weights=(0.5, 0.5))),                                 # rows of 1 and 2
         Member.of(mk(T=50, N=30, R=5, seed=seed + 40, max_partitions=1)),                                      # 1 partition per topic
         Member.of(mk(T=12, N=60, R=6, seed=seed + 50, max_partitions=600, tail=0.4)),                          # topics of hundreds
-        Member.of(mk(T=30, N=40, R=5, seed=seed + 60), table=_table(np.arange(1, 41))),                        # no racks
-        Member.of(mk(T=30, N=30, R=5, seed=seed + 70), table=_table(1 + 2 * np.arange(20000), 500)),           # global id LUT
-        Member.of(mk(T=30, N=30, R=5, seed=seed + 80), table=_bsearch_table(30)),                              # binary search
-        _min_hash_cluster(_table(np.arange(1, 7))),
+        Member.of(mk(T=30, N=40, R=5, seed=seed + 60), table=util.table(np.arange(1, 41))),                    # no racks
+        Member.of(mk(T=30, N=30, R=5, seed=seed + 70), table=util.table(1 + 2 * np.arange(20000), 500)),       # global id LUT
+        Member.of(mk(T=30, N=30, R=5, seed=seed + 80), table=util.bsearch_table(30)),                          # binary search
+        util.min_hash_cluster(util.table(np.arange(1, 7))),
         Member.of(mk(T=20, N=24, R=4, seed=seed + 90), desired_rf=3),
     ]
     fleet = [fleet[i] for i in rng.permutation(len(fleet))]
@@ -141,12 +132,12 @@ def test_exceptions_and_refusals_are_isolated(native_lib):
     ok = [Member.of(kab.synth.make_ragged_cluster(T=40, N=30, R=5, seed=s)) for s in (3, 4, 5)]
     rf3 = {11: [1, 2, 3], 12: [2, 3, 4], 13: [3, 4, 5]}
     fails = [
-        Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2], 9: [3]})]),                          # RF mismatch
-        Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2]}), ("none", {})]),                    # no positive RF
-        Member.of_topics(_table(np.arange(1, 3)), [("gamma", rf3)]),                                      # RF 3 > 2 brokers
-        Member.of_topics(_table(np.arange(1, 9), 4), [("gamma", rf3)]),                                   # two racks
-        Member.of_topics(_table(np.arange(1, 4)), [(MIN_HASH, {5: [1, 2, 3]})]),                           # hash index
-        Member.of_topics(_table(np.zeros(0)), [("alpha", {0: [1, 2]})]),                                   # no broker at all
+        Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2], 9: [3]})]),                      # RF mismatch
+        Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2]}), ("none", {})]),                # no positive RF
+        Member.of_topics(util.table(np.arange(1, 3)), [("gamma", rf3)]),                                  # RF 3 > 2 brokers
+        Member.of_topics(util.table(np.arange(1, 9), 4), [("gamma", rf3)]),                               # two racks
+        Member.of_topics(util.table(np.arange(1, 4)), [(MIN_HASH, {5: [1, 2, 3]})]),                       # hash index
+        Member.of_topics(util.table(np.zeros(0)), [("alpha", {0: [1, 2]})]),                               # no broker at all
     ]
     bad_part = Member.of(kab.synth.make_ragged_cluster(T=20, N=30, R=5, seed=6))
     bad_part.part_off = bad_part.part_off.copy()
@@ -154,7 +145,7 @@ def test_exceptions_and_refusals_are_isolated(native_lib):
     bad_rep = Member.of(kab.synth.make_ragged_cluster(T=20, N=30, R=5, seed=7))
     bad_rep.rep_off = bad_rep.rep_off.copy()
     bad_rep.rep_off[7] = bad_rep.rep_off[8] + 1
-    huge = Member.of(kab.synth.make_ragged_cluster(T=20, N=40, R=5, seed=8), table=_table(np.arange(1, 40001), 100))
+    huge = Member.of(kab.synth.make_ragged_cluster(T=20, N=40, R=5, seed=8), table=util.table(np.arange(1, 40001), 100))
     fleet = [ok[0]] + fails[:3] + [bad_part, ok[1], bad_rep] + fails[3:] + [huge, ok[2]]
     rng = np.random.default_rng(9)
     sts, _ = _check_scores(fleet, _weights(fleet, rng), S=3, single=False)
@@ -163,7 +154,7 @@ def test_exceptions_and_refusals_are_isolated(native_lib):
     assert set(codes) >= {1, 2, 3, 4, 5, _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT}, codes
     assert sts[-2][0] == _native.KA_ERR_LIMIT and sts[-2][4] == 40000
     two = [Member.of(kab.synth.make_ragged_cluster(T=20, N=20, R=4, seed=9, rf_weights=(0.5, 0.5)))]
-    long_list = Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2, 3]})])                          # longer than the stride
+    long_list = Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2, 3]})])                      # longer than the stride
     sts, _ = _check_scores(two + [long_list] + two, S=2)
     assert [st[0] for st in sts] == [0, _native.KA_ERR_BAD_ARG, 0]
 
@@ -177,28 +168,28 @@ def test_segment_edges(native_lib):
     for k in range(128):
         P = int(rng.integers(1, 41))
         topics = [("t%d" % k, {p: [int(x) for x in rng.choice(np.arange(1, 13), 3, replace=False)] for p in range(P)})]
-        tiny.append(Member.of_topics(_table(np.arange(1, 13), 3), topics))
+        tiny.append(Member.of_topics(util.table(np.arange(1, 13), 3), topics))
     sts, _ = _check_scores(tiny, _weights(tiny, rng), single=False)
     assert sum(st[0] == 0 for st in sts) >= 64   # random lists over 4 racks: some clusters are unassignable
     # clusters with no topics, or only empty topics under a desired RF, between non-empty ones
     empty = Member([np.arange(1, 5, dtype=np.int32), np.zeros(4, dtype=np.int32)], [], [], np.zeros(1, dtype=np.int64),
                    np.zeros(0, dtype=np.int32), np.zeros(1, dtype=np.int64), np.zeros(0, dtype=np.int32))
-    no_rows = Member.of_topics(_table(np.arange(1, 5)), [("e1", {}), ("e2", {})], desired_rf=2)
+    no_rows = Member.of_topics(util.table(np.arange(1, 5)), [("e1", {}), ("e2", {})], desired_rf=2)
     one = Member.of(mk(T=300, N=60, R=6, seed=31))
     fleet = [empty, one, empty, no_rows, Member.of(mk(T=50, N=30, R=5, seed=32)), empty]
     sts, summ = _check_scores(fleet, _weights(fleet, rng))
-    assert all(st[0] == 0 for st in sts) and [_rec(summ[k]) for k in (0, 2, 3, 5)] == [EMPTY] * 4
+    assert all(st[0] == 0 for st in sts) and [util.record_of(summ[k], FIELDS) for k in (0, 2, 3, 5)] == [util.EMPTY_SUMMARY] * 4
     sts, summ = _check_scores([empty, no_rows])                                  # nothing to solve at all
-    assert all(st[0] == 0 for st in sts) and [_rec(x) for x in summ] == [EMPTY] * 2
+    assert all(st[0] == 0 for st in sts) and [util.record_of(x, FIELDS) for x in summ] == [util.EMPTY_SUMMARY] * 2
     # a cluster whose rows start exactly at a multiple of 256
-    first = Member.of_topics(_table(np.arange(1, 9), 1), [("a", {p: [1 + p % 8, 1 + (p + 3) % 8] for p in range(200)}),
+    first = Member.of_topics(util.table(np.arange(1, 9), 1), [("a", {p: [1 + p % 8, 1 + (p + 3) % 8] for p in range(200)}),
                                                            ("b", {p: [1 + p % 7, 1 + (p + 2) % 7] for p in range(312)})])
     assert int(first.part_off[-1]) == 512
     mid = Member.of(mk(T=40, N=30, R=5, seed=33))
     sts, _ = _check_scores([first, mid, first], _weights([first, mid, first], rng))
     assert all(st[0] == 0 for st in sts)
     # current lists with duplicate ids and with brokers missing from the cluster's table
-    dup = Member.of_topics(_table(np.arange(1, 7), 2), [("d", {0: [3, 3], 1: [9, 1], 2: [2, 2], 3: [40, 41], 4: [1, 2]})])
+    dup = Member.of_topics(util.table(np.arange(1, 7), 2), [("d", {0: [3, 3], 1: [9, 1], 2: [2, 2], 3: [40, 41], 4: [1, 2]})])
     sts, summ = _check_scores([one, dup, first], _weights([one, dup, first], rng))
     assert sts[1][0] == 0 and summ[1]["replicas_dropped"] > 0 and summ[1]["replicas_added"] > 0
 
@@ -213,7 +204,7 @@ def test_weights(native_lib):
     s = kab.Solver(0)
     a = s.score_clusters(entries)
     b = s.score_clusters(entries, weights=[np.ones(n, dtype=np.int64) for n in sizes])
-    assert [_rec(x[0]) for x in a] == [_rec(x[0]) for x in b] and all(x[1].code == 0 for x in a)
+    assert [util.record_of(x[0], FIELDS) for x in a] == [util.record_of(x[0], FIELDS) for x in b] and all(x[1].code == 0 for x in a)
 
     def split(flat):
         return [flat[o:o + n] for o, n in zip(np.cumsum([0] + sizes[:-1]), sizes)]
@@ -223,13 +214,13 @@ def test_weights(native_lib):
     res = s.score_clusters(entries, weights=split(edge))
     assert all(x[1].code == 0 for x in res)
     solved = s.solve_clusters(entries)
-    e, _, _, _ = reference_summary(solved[0][0], solved[0][1], fleet[0].rep_off, fleet[0].cur, fleet[0].ids.astype(np.int64),
-                                   split(edge)[0])
-    assert _rec(res[0][0]) == e
+    e, _, _, _ = models.move_summary(solved[0][0], solved[0][1], fleet[0].rep_off, fleet[0].cur, fleet[0].ids.astype(np.int64),
+                                     split(edge)[0])
+    assert util.record_of(res[0][0], FIELDS) == e
     over = edge.copy()
     over[Q - 1] += 1                                                          # in the last cluster: the whole call is refused
     res = s.score_clusters(entries, weights=split(over))
-    assert all(x[1].code == _native.KA_ERR_LIMIT for x in res) and all(_rec(x[0]) == EMPTY for x in res)
+    assert all(x[1].code == _native.KA_ERR_LIMIT for x in res) and all(util.record_of(x[0], FIELDS) == util.EMPTY_SUMMARY for x in res)
     neg = np.ones(Q, dtype=np.int64)
     neg[sizes[0] + 3] = -1
     res = s.score_clusters(entries, weights=split(neg), per_broker=True)
@@ -277,12 +268,12 @@ def test_launches_state_and_optional_outputs(native_lib):
     again = s.score_clusters(entries, weights=w, rows=True, per_broker=True)
     assert np.array_equal(s.counters(), before) and np.array_equal(s.broker_id, cl.broker_id)
     for x, y in zip(full, again):
-        assert _rec(x[0]) == _rec(y[0]) and _fields(x[1]) == _fields(y[1])
+        assert util.record_of(x[0], FIELDS) == util.record_of(y[0], FIELDS) and util.fields(x[1]) == util.fields(y[1])
         assert all(np.array_equal(a, b) for a, b in zip(x[2:], y[2:]))
     # rows=False and per_broker=False give the summaries of the full call
     for kw in (dict(), dict(rows=True), dict(per_broker=True)):
         part = s.score_clusters(entries, weights=w, **kw)
-        assert [_rec(x[0]) for x in part] == [_rec(x[0]) for x in full], kw
+        assert [util.record_of(x[0], FIELDS) for x in part] == [util.record_of(x[0], FIELDS) for x in full], kw
         assert len(part[0]) == 2 + 2 * bool(kw.get("rows")) + 3 * bool(kw.get("per_broker"))
 
 

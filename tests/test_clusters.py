@@ -10,62 +10,12 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from tests import util
+from tests.util import MIN_HASH, Member
 
 pytestmark = pytest.mark.gpu
 
-MIN_HASH = "polygenelubricants"   # String.hashCode == Integer.MIN_VALUE (KAS:190-192)
-
-
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
-
-
-def _table(ids, racks_per=None):
-    """(ids, rack_index): racks_per = brokers per rack (contiguous), or None: no broker has a rack."""
-    ids = np.asarray(ids, dtype=np.int32)
-    names = [None] * len(ids) if racks_per is None else ["k%d" % (i // racks_per) for i in range(len(ids))]
-    return ids, kab.synth.rack_indices(ids, names)
-
-
-class Member:
-    """One cluster of a fleet: its table, its ka_solve inputs (offsets from 0) and its topic names."""
-
-    def __init__(self, table, names, topic_hash, part_off, part_id, rep_off, cur, desired_rf=-1):
-        self.ids, self.racks = table
-        self.names = list(names)
-        self.topic_hash = np.asarray(topic_hash, dtype=np.int32)
-        self.part_off, self.part_id, self.rep_off, self.cur = part_off, part_id, rep_off, cur
-        self.desired_rf = desired_rf
-
-    @classmethod
-    def of(cls, cl, table=None, desired_rf=-1):
-        return cls(table or (cl.broker_id, cl.rack_index), cl.topic_names, cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off,
-                   cl.cur, desired_rf)
-
-    @classmethod
-    def of_topics(cls, table, topics, desired_rf=-1):
-        names, part_off, part_id, rep_off, cur = util.flatten(topics)
-        return cls(table, names, [kab.java_string_hash(n) for n in names], part_off, part_id, rep_off, cur, desired_rf)
-
-    def entry(self):
-        return (self.ids, self.racks, self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur, self.desired_rf)
-
-    def sequential(self, s, S):
-        """The contract's reference: a fresh Context with this cluster's table, then ka_solve."""
-        s.reset()
-        s.set_brokers(self.ids, self.racks)
-        out, ln, st = s.solve_ragged(self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur, self.desired_rf, S,
-                                     check=False)
-        return out, ln, _fields(st)
-
-
-def _stride(fleet):
-    sizes = [int(np.diff(m.rep_off).max()) for m in fleet if len(m.rep_off) > 1]
-    return max(sizes + [m.desired_rf for m in fleet] + [1])
-
-
 def _check_fleet(fleet, oracle=None, solver=None, S=None):
-    S = S or _stride(fleet)
+    S = S or util.fleet_stride(fleet)
     s = solver or kab.Solver(0)
     res = s.solve_clusters([m.entry() for m in fleet], out_stride=S)
     assert len(res) == len(fleet)
@@ -73,7 +23,7 @@ def _check_fleet(fleet, oracle=None, solver=None, S=None):
     sts = []
     for k, (m, (out, ln, st)) in enumerate(zip(fleet, res)):
         e_out, e_len, e_st = m.sequential(ref, S)
-        assert _fields(st) == e_st, (k, _fields(st), e_st)
+        assert util.fields(st) == e_st, (k, util.fields(st), e_st)
         sts.append(e_st)
         if e_st[0] != 0:
             continue   # the rows of a failed cluster are unspecified
@@ -84,17 +34,6 @@ def _check_fleet(fleet, oracle=None, solver=None, S=None):
             assert o_st.code == 0, k
             assert np.array_equal(out, o_out) and np.array_equal(ln, o_len), k
     return sts
-
-
-def _min_hash_cluster(table):
-    """Topics around one whose hashCode is Integer.MIN_VALUE, with lists of 2 (|hash| % 2 == 0: it solves)."""
-    topics = [("a", {0: [1, 2], 1: [2, 3]}), (MIN_HASH, {3: [1, 2], 5: [2, 3], 6: [3, 1]}), ("z", {0: [3, 4]})]
-    return Member.of_topics(table, topics)
-
-
-def _bsearch_table(N):
-    """Brokers 1..N plus one id far away: an id range beyond the global LUT, so ids are looked up by binary search."""
-    return _table(np.concatenate([np.arange(1, N + 1), [1 << 27]]).astype(np.int32), 4)
 
 
 @pytest.mark.parametrize("seed", [1, 2])
@@ -108,10 +47,10 @@ def test_heterogeneous_fleet_matches_sequential_and_oracle(native_lib, oracle, s
         Member.of(mk(T=25, N=20, R=3, seed=seed + 30, rf_weights=(0.5, 0.5))),                                 # rows of 1 and 2
         Member.of(mk(T=50, N=30, R=5, seed=seed + 40, max_partitions=1)),                                      # 1 partition per topic
         Member.of(mk(T=12, N=60, R=6, seed=seed + 50, max_partitions=600, tail=0.4)),                          # topics of hundreds
-        Member.of(mk(T=30, N=40, R=5, seed=seed + 60), table=_table(np.arange(1, 41))),                        # no racks
-        Member.of(mk(T=30, N=30, R=5, seed=seed + 70), table=_table(1 + 2 * np.arange(20000), 500)),           # global id LUT
-        Member.of(mk(T=30, N=30, R=5, seed=seed + 80), table=_bsearch_table(30)),                              # binary search
-        _min_hash_cluster(_table(np.arange(1, 7))),
+        Member.of(mk(T=30, N=40, R=5, seed=seed + 60), table=util.table(np.arange(1, 41))),                    # no racks
+        Member.of(mk(T=30, N=30, R=5, seed=seed + 70), table=util.table(1 + 2 * np.arange(20000), 500)),       # global id LUT
+        Member.of(mk(T=30, N=30, R=5, seed=seed + 80), table=util.bsearch_table(30)),                          # binary search
+        util.min_hash_cluster(util.table(np.arange(1, 7))),
         Member.of(mk(T=20, N=24, R=4, seed=seed + 90), desired_rf=3),
     ]
     order = rng.permutation(len(fleet))
@@ -127,12 +66,12 @@ def test_exceptions_and_refusals_are_isolated(native_lib, oracle):
     ok = [Member.of(kab.synth.make_ragged_cluster(T=40, N=30, R=5, seed=s)) for s in (3, 4, 5)]
     rf3 = {11: [1, 2, 3], 12: [2, 3, 4], 13: [3, 4, 5]}
     fails = [
-        Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2], 9: [3]})]),                          # RF mismatch (KTA:58-60)
-        Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2]}), ("none", {})]),                    # no positive RF (KTA:65-66)
-        Member.of_topics(_table(np.arange(1, 3)), [("gamma", rf3)]),                                      # RF 3 > 2 brokers (KTA:67-69)
-        Member.of_topics(_table(np.arange(1, 9), 4), [("gamma", rf3)]),                                   # two racks (KAS:183-184)
-        Member.of_topics(_table(np.arange(1, 4)), [(MIN_HASH, {5: [1, 2, 3]})]),                           # 2^31 % 3 (KAS:190-192)
-        Member.of_topics(_table(np.zeros(0)), [("alpha", {0: [1, 2]})]),                                   # no broker at all
+        Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2], 9: [3]})]),                      # RF mismatch (KTA:58-60)
+        Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2]}), ("none", {})]),                # no positive RF (KTA:65-66)
+        Member.of_topics(util.table(np.arange(1, 3)), [("gamma", rf3)]),                                  # RF 3 > 2 brokers (KTA:67-69)
+        Member.of_topics(util.table(np.arange(1, 9), 4), [("gamma", rf3)]),                               # two racks (KAS:183-184)
+        Member.of_topics(util.table(np.arange(1, 4)), [(MIN_HASH, {5: [1, 2, 3]})]),                       # 2^31 % 3 (KAS:190-192)
+        Member.of_topics(util.table(np.zeros(0)), [("alpha", {0: [1, 2]})]),                               # no broker at all
     ]
     bad_part = Member.of(kab.synth.make_ragged_cluster(T=20, N=30, R=5, seed=6))
     bad_part.part_off = bad_part.part_off.copy()
@@ -140,8 +79,8 @@ def test_exceptions_and_refusals_are_isolated(native_lib, oracle):
     bad_rep = Member.of(kab.synth.make_ragged_cluster(T=20, N=30, R=5, seed=7))
     bad_rep.rep_off = bad_rep.rep_off.copy()
     bad_rep.rep_off[7] = bad_rep.rep_off[8] + 1                                                            # a list of negative size
-    long_list = Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2, 3]})])                          # longer than the stride 2
-    huge = Member.of(kab.synth.make_ragged_cluster(T=20, N=40, R=5, seed=8), table=_table(np.arange(1, 40001), 100))  # level-plan limit
+    long_list = Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2, 3]})])                      # longer than the stride 2
+    huge = Member.of(kab.synth.make_ragged_cluster(T=20, N=40, R=5, seed=8), table=util.table(np.arange(1, 40001), 100))  # level-plan limit
     fleet = [ok[0]] + fails[:3] + [bad_part, ok[1], bad_rep] + fails[3:] + [huge, ok[2]]
     sts = _check_fleet(fleet, oracle, S=3)   # (the malformed rep_off has a list longer than 3)
     codes = [st[0] for st in sts]
@@ -164,7 +103,7 @@ def test_edges(native_lib):
     _check_fleet([one])                                                       # K = 1 is ka_solve
     empty = Member([np.arange(1, 5, dtype=np.int32), np.zeros(4, dtype=np.int32)], [], [], np.zeros(1, dtype=np.int64),
                    np.zeros(0, dtype=np.int32), np.zeros(1, dtype=np.int64), np.zeros(0, dtype=np.int32))
-    no_rows = Member.of_topics(_table(np.arange(1, 5)), [("e1", {}), ("e2", {})], desired_rf=2)
+    no_rows = Member.of_topics(util.table(np.arange(1, 5)), [("e1", {}), ("e2", {})], desired_rf=2)
     sts = _check_fleet([empty, one, empty, no_rows, Member.of(mk(T=50, N=30, R=5, seed=32)), empty])
     assert all(st[0] == 0 for st in sts), sts
     assert all(st[0] == 0 for st in _check_fleet([empty, empty]))            # nothing to solve at all
@@ -185,7 +124,7 @@ def _call(s, fleet, st, K=None, S=None, topic_off=None, part_off=None, rep_off=N
     t_off = t_off if topic_off is None else topic_off
     p_off = p_off if part_off is None else part_off
     r_off = r_off if rep_off is None else rep_off
-    S = _stride(fleet) if S is None else S
+    S = util.fleet_stride(fleet) if S is None else S
     out = np.zeros(max(int(p_off[-1]), 1) * max(S, 1), dtype=np.int32)
     vp = lambda a: None if a is None else a.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
     return s._L.ka_solve_clusters(s._h, len(fleet) if K is None else K, vp(cand_off), vp(ids), vp(racks), vp(t_off),

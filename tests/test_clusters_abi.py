@@ -6,7 +6,7 @@ import os
 import numpy as np
 
 import kafka_assigner_b200 as kab
-from tests.test_solver_abi import fake_solver, view
+from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -41,16 +41,16 @@ class _FakeLib:
         self.seen = None
 
     def ka_solve_clusters(self, h, K, cand_off, ids, racks, topic_off, drf, th, part_off, part_id, rep_off, cur, S, out_len, out, st):
-        c_off = view(cand_off, K + 1, np.int32)
-        t_off = view(topic_off, K + 1, np.int32)
+        c_off = util.view(cand_off, K + 1, np.int32)
+        t_off = util.view(topic_off, K + 1, np.int32)
         T = int(t_off[-1])
-        p_off = view(part_off, T + 1, np.int64)
+        p_off = util.view(part_off, T + 1, np.int64)
         Q = int(p_off[-1])
-        r_off = view(rep_off, Q + 1, np.int64)
-        self.seen = dict(K=K, S=S, cand_off=c_off, broker_id=view(ids, int(c_off[-1]), np.int32),
-                         broker_rack=view(racks, int(c_off[-1]), np.int32), topic_off=t_off, desired_rf=view(drf, K, np.int32),
-                         topic_hash=view(th, T, np.int32), part_off=p_off, part_id=view(part_id, Q, np.int32), rep_off=r_off,
-                         cur=view(cur, int(r_off[-1]), np.int32))
+        r_off = util.view(rep_off, Q + 1, np.int64)
+        self.seen = dict(K=K, S=S, cand_off=c_off, broker_id=util.view(ids, int(c_off[-1]), np.int32),
+                         broker_rack=util.view(racks, int(c_off[-1]), np.int32), topic_off=t_off, desired_rf=util.view(drf, K, np.int32),
+                         topic_hash=util.view(th, T, np.int32), part_off=p_off, part_id=util.view(part_id, Q, np.int32), rep_off=r_off,
+                         cur=util.view(cur, int(r_off[-1]), np.int32))
         rows = np.ctypeslib.as_array(ctypes.cast(out, ctypes.POINTER(ctypes.c_int32)), shape=(Q * S,))
         rows[:] = np.arange(Q * S, dtype=np.int32)
         lens = np.ctypeslib.as_array(ctypes.cast(out_len, ctypes.POINTER(ctypes.c_int32)), shape=(Q,))
@@ -67,7 +67,7 @@ def test_solve_clusters_marshals_the_shared_layout():
              np.array([0], np.int64), np.zeros(0, np.int32), 2)
     b = (np.array([5, 6], np.int32), np.array([0, 1], np.int32), np.array([21], np.int32), np.array([0, 2], np.int64), None,
          np.array([0, 3, 6], np.int64), np.array([5, 6, 7, 6, 5, 7], np.int32), 3)
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     res = s.solve_clusters([a, empty, b])
     got = s._L.seen
     # by hand: the three clusters one after the other, offsets continued from where the previous cluster ends
@@ -90,7 +90,7 @@ def test_solve_clusters_marshals_the_shared_layout():
 def test_solve_clusters_takes_an_explicit_stride():
     c = (np.array([1, 2], np.int32), np.array([0, 1], np.int32), np.array([5], np.int32), np.array([0, 1], np.int64), None,
          np.array([0, 1], np.int64), np.array([2], np.int32), -1)
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     out, ln, st = s.solve_clusters([c, c], out_stride=2)[1]
     assert s._L.seen["S"] == 2 and out.shape == (1, 2)
     assert s._L.seen["part_off"].tolist() == [0, 1, 2] and s._L.seen["rep_off"].tolist() == [0, 1, 2]

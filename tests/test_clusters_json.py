@@ -9,53 +9,10 @@ import pytest
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
-from tests.test_clusters import MIN_HASH, Member, _bsearch_table, _min_hash_cluster, _table
-from tests.test_ragged_json import EMPTY, _oracle_text
+from tests import models, util
+from tests.util import MIN_HASH, Member
 
 pytestmark = pytest.mark.gpu
-
-
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
-
-
-def _width(m):
-    sizes = np.diff(m.rep_off)
-    return max(int(sizes.max()) if len(sizes) else 0, m.desired_rf, 1)
-
-
-def _sequential(m, s):
-    """The contract's reference: a fresh Context with this cluster's table, then ka_solve_json; a cluster wider than the batched
-    chains' 3 is refused with its width instead."""
-    if _width(m) > 3:
-        return b"", (_native.KA_ERR_LIMIT, -1, -1, _width(m), 0)
-    s.reset()
-    s.set_brokers(m.ids, m.racks)
-    text, st = s.solve_ragged_json(m.names, m.topic_hash, m.part_off, m.part_id, m.rep_off, m.cur, m.desired_rf, check=False)
-    return bytes(text), _fields(st)
-
-
-def _check_fleet(fleet, oracle=None, solver=None):
-    """Every cluster against its sequential ka_solve_json (and the oracle's text); the documents back to back in cluster order."""
-    s = solver or kab.Solver(0)
-    res = s.solve_clusters_json([m.entry() for m in fleet], [m.names for m in fleet])
-    assert len(res) == len(fleet)
-    ref = kab.Solver(0)
-    sts, texts = [], []
-    for k, (m, (text, st)) in enumerate(zip(fleet, res)):
-        e_text, e_st = _sequential(m, ref)
-        assert _fields(st) == e_st, (k, _fields(st), e_st)
-        assert bytes(text) == e_text, k
-        sts.append(e_st)
-        texts.append(bytes(text))
-        if oracle is not None and e_st[0] == 0:
-            exp, o_st = _oracle_text(oracle, m.names, m.part_off, m.part_id, m.rep_off, m.cur, m.ids, ["k%d" % r for r in m.racks],
-                                     m.desired_rf)
-            assert o_st.code == 0 and bytes(text).decode() == exp, k
-    # the documents back to back in cluster order, in one buffer (a failed cluster's range is empty)
-    starts = [t.__array_interface__["data"][0] for t, _ in res if len(t)]
-    assert all(b - a == len(t) for a, b, t in zip(starts, starts[1:], [t for t in texts if t]))
-    return sts, texts
 
 
 def _raw(s, fleet, cap=1 << 22, K=None, names=True, json=True, json_off=True, part_id=True, topic_off=None, tables=None):
@@ -87,15 +44,15 @@ def test_heterogeneous_fleet_matches_sequential_and_oracle(native_lib, oracle, s
         Member.of(mk(T=25, N=20, R=3, seed=seed + 30, rf_weights=(0.5, 0.5))),                                 # rows of 1 and 2
         Member.of(mk(T=50, N=30, R=5, seed=seed + 40, max_partitions=1)),                                      # 1 partition per topic
         Member.of(mk(T=12, N=60, R=6, seed=seed + 50, max_partitions=600, tail=0.4)),                          # topics of hundreds
-        Member.of(mk(T=30, N=40, R=5, seed=seed + 60), table=_table(np.arange(1, 41))),                        # no racks
-        Member.of(mk(T=30, N=30, R=5, seed=seed + 70), table=_table(1 + 2 * np.arange(20000), 500)),           # global id LUT
-        Member.of(mk(T=30, N=30, R=5, seed=seed + 80), table=_bsearch_table(30)),                              # binary search
-        _min_hash_cluster(_table(np.arange(1, 7))),                                                            # hashCode MIN_VALUE
+        Member.of(mk(T=30, N=40, R=5, seed=seed + 60), table=util.table(np.arange(1, 41))),                    # no racks
+        Member.of(mk(T=30, N=30, R=5, seed=seed + 70), table=util.table(1 + 2 * np.arange(20000), 500)),       # global id LUT
+        Member.of(mk(T=30, N=30, R=5, seed=seed + 80), table=util.bsearch_table(30)),                          # binary search
+        util.min_hash_cluster(util.table(np.arange(1, 7))),                                                    # hashCode MIN_VALUE
         Member.of(mk(T=20, N=24, R=4, seed=seed + 90), desired_rf=3),
     ]
     fleet = [fleet[i] for i in rng.permutation(len(fleet))]
     s = kab.Solver(0)
-    sts, texts = _check_fleet(fleet, oracle, solver=s)
+    sts, texts = util.check_fleet(fleet, oracle, solver=s)
     assert sum(st[0] == 0 for st in sts) >= 8, sts
     assert s.last_stage_plan()[6] == 7   # all three id lookup modes in one call
     assert s.last_order_plan()[7] == len(fleet)
@@ -106,42 +63,42 @@ def test_exceptions_refusals_and_edges_are_isolated(native_lib, oracle):
     ok = [Member.of(mk(T=40, N=30, R=5, seed=s)) for s in (3, 4, 5)]
     rf3 = {11: [1, 2, 3], 12: [2, 3, 4], 13: [3, 4, 5]}
     fails = [
-        Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2], 9: [3]})]),                          # RF mismatch (KTA:58-60)
-        Member.of_topics(_table(np.arange(1, 9)), [("t", {0: [1, 2]}), ("none", {})]),                    # no positive RF (KTA:65-66)
-        Member.of_topics(_table(np.arange(1, 3)), [("gamma", rf3)]),                                      # RF 3 > 2 brokers (KTA:67-69)
-        Member.of_topics(_table(np.arange(1, 9), 4), [("gamma", rf3)]),                                   # two racks (KAS:183-184)
-        Member.of_topics(_table(np.arange(1, 4)), [(MIN_HASH, {5: [1, 2, 3]})]),                           # 2^31 % 3 (KAS:190-192)
+        Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2], 9: [3]})]),                      # RF mismatch (KTA:58-60)
+        Member.of_topics(util.table(np.arange(1, 9)), [("t", {0: [1, 2]}), ("none", {})]),                # no positive RF (KTA:65-66)
+        Member.of_topics(util.table(np.arange(1, 3)), [("gamma", rf3)]),                                  # RF 3 > 2 brokers (KTA:67-69)
+        Member.of_topics(util.table(np.arange(1, 9), 4), [("gamma", rf3)]),                               # two racks (KAS:183-184)
+        Member.of_topics(util.table(np.arange(1, 4)), [(MIN_HASH, {5: [1, 2, 3]})]),                       # 2^31 % 3 (KAS:190-192)
     ]
-    wide = Member.of_topics(_table(np.arange(1, 9)), [("w", {0: [1, 2, 3, 4], 1: [2, 3, 4, 5]})])           # width 4
+    wide = Member.of_topics(util.table(np.arange(1, 9)), [("w", {0: [1, 2, 3, 4], 1: [2, 3, 4, 5]})])       # width 4
     quoted = Member.of(mk(T=20, N=30, R=5, seed=9))
     quoted.names[4] = "a/b"                                                                                 # org.json escapes '/'
     empty = Member([np.arange(1, 5, dtype=np.int32), np.zeros(4, dtype=np.int32)], [], [], np.zeros(1, dtype=np.int64),
                    np.zeros(0, dtype=np.int32), np.zeros(1, dtype=np.int64), np.zeros(0, dtype=np.int32))
-    no_rows = Member.of_topics(_table(np.arange(1, 5)), [("e1", {}), ("e2", {})], desired_rf=2)
+    no_rows = Member.of_topics(util.table(np.arange(1, 5)), [("e1", {}), ("e2", {})], desired_rf=2)
     fleet = [fails[0], empty, ok[0], fails[1], wide, no_rows, fails[2], ok[1], quoted, fails[3], empty, ok[2], fails[4]]
-    sts, texts = _check_fleet(fleet, oracle)
+    sts, texts = util.check_fleet(fleet, oracle)
     codes = [st[0] for st in sts]
     assert codes == [1, 0, 0, 2, _native.KA_ERR_LIMIT, 0, 3, 0, _native.KA_ERR_BAD_ARG, 4, 0, 0, 5], codes
     assert sts[4][3] == 4 and sts[8][3] == ord("/")
-    assert texts[1] == texts[5] == texts[10] == EMPTY.encode()
+    assert texts[1] == texts[5] == texts[10] == models.EMPTY_DOCUMENT.encode()
     # the failing clusters first and last, and a fleet where only the empty documents are left
-    _check_fleet([wide, ok[0], quoted])
-    assert [st[0] for st in _check_fleet([empty, quoted, no_rows])[0]] == [0, _native.KA_ERR_BAD_ARG, 0]
-    assert [st[0] for st in _check_fleet([empty, empty])[0]] == [0, 0]
+    util.check_fleet([wide, ok[0], quoted])
+    assert [st[0] for st in util.check_fleet([empty, quoted, no_rows])[0]] == [0, _native.KA_ERR_BAD_ARG, 0]
+    assert [st[0] for st in util.check_fleet([empty, empty])[0]] == [0, 0]
 
 
 def test_many_documents_per_block_and_fragments_per_document(native_lib):
     # one row per cluster: a 256-row block of the length and write passes spans 128 documents
-    tiny = [Member.of_topics(_table(np.arange(1, 4 + k % 5)), [("t%d" % k, {k: [1 + k % 3, 2 + k % 2]})], desired_rf=k % 3 - 1)
+    tiny = [Member.of_topics(util.table(np.arange(1, 4 + k % 5)), [("t%d" % k, {k: [1 + k % 3, 2 + k % 2]})], desired_rf=k % 3 - 1)
             for k in range(128)]
-    sts, _ = _check_fleet(tiny)
+    sts, _ = util.check_fleet(tiny)
     assert sum(st[0] == 0 for st in sts) >= 80
     mk = kab.synth.make_ragged_cluster
-    _check_fleet([Member.of(mk(T=8, N=24, R=4, seed=100 + k, max_partitions=32)) for k in range(128)])   # 128 tiny clusters
+    util.check_fleet([Member.of(mk(T=8, N=24, R=4, seed=100 + k, max_partitions=32)) for k in range(128)])   # 128 tiny clusters
     # clusters large enough that the fragments of 2^18 rows cut through a document
     big = [Member.of(mk(T=30000, N=400, max_partitions=128, seed=100 + k)) for k in range(3)]
     assert sum(int(m.part_off[-1]) for m in big) > 1 << 18
-    assert all(st[0] == 0 for st in _check_fleet([big[0], Member.of(mk(T=20, N=20, R=4, seed=74)), big[1], big[2]])[0])
+    assert all(st[0] == 0 for st in util.check_fleet([big[0], Member.of(mk(T=20, N=20, R=4, seed=74)), big[1], big[2]])[0])
 
 
 def test_part_id_null_and_sparse(native_lib):
@@ -154,13 +111,13 @@ def test_part_id_null_and_sparse(native_lib):
     ref = kab.Solver(0)
     assert rc == next((st[k].code for k in range(3) if st[k].code), 0)
     for k, m in enumerate(fleet):
-        e_text, e_st = _sequential(m, ref)
-        assert _fields(st[k]) == e_st and bytes(buf[off[k]:off[k + 1]]) == e_text
+        e_text, e_st = util.sequential_json(m, ref)
+        assert util.fields(st[k]) == e_st and bytes(buf[off[k]:off[k + 1]]) == e_text
 
 
 def test_buffer_size_and_arguments(native_lib):
     mk = kab.synth.make_ragged_cluster
-    bad = Member.of_topics(_table(np.arange(1, 3)), [("gamma", {0: [1, 2, 3]})])
+    bad = Member.of_topics(util.table(np.arange(1, 3)), [("gamma", {0: [1, 2, 3]})])
     fleet = [Member.of(mk(T=20, N=30, R=5, seed=s)) for s in (51, 52)] + [bad]
     s = kab.Solver(0)
     rc, off, buf, st = _raw(s, fleet)
@@ -171,7 +128,7 @@ def test_buffer_size_and_arguments(native_lib):
     assert rc == 3 and np.array_equal(off, off2) and bytes(buf2[:need]) == text
     rc, off2, _, st2 = _raw(s, fleet, cap=need - 1)
     assert rc == _native.KA_ERR_LIMIT and not off2.any()
-    assert [_fields(st2[k]) for k in range(3)] == [(_native.KA_ERR_LIMIT, -1, -1, need - 1, 0)] * 2 + [_fields(st[2])]
+    assert [util.fields(st2[k]) for k in range(3)] == [(_native.KA_ERR_LIMIT, -1, -1, need - 1, 0)] * 2 + [util.fields(st[2])]
     # the documented sufficient size is what Solver.solve_clusters_json allocates
     assert all(bytes(t) == bytes(buf[off[k]:off[k + 1]])
                for k, (t, _) in enumerate(s.solve_clusters_json([m.entry() for m in fleet], [m.names for m in fleet])))
@@ -206,7 +163,7 @@ def test_ctx_state_and_launches(native_lib):
         x.solve_ragged(half.topic_hash, half.part_off, half.part_id, half.rep_off, half.cur, -1, 3)   # counters in the Context
     before = s.counters()
     fleet = [Member.of(mk(T=300, N=40 + 10 * k, R=5, seed=63 + k)) for k in range(4)]
-    _check_fleet(fleet, solver=s)
+    util.check_fleet(fleet, solver=s)
     assert s.last_order_plan()[7] == len(fleet) and s.last_stage_plan()[3] == len(fleet)
     assert np.array_equal(s.counters(), before) and np.array_equal(s.broker_id, cl.broker_id)
     a, al, ast = s.solve_ragged(cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off, cl.cur, -1, 3)

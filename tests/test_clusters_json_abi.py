@@ -7,7 +7,7 @@ import os
 import numpy as np
 
 import kafka_assigner_b200 as kab
-from tests.test_solver_abi import fake_solver, view
+from tests import util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -48,16 +48,16 @@ class _FakeLib:
 
     def ka_solve_clusters_json(self, h, K, cand_off, ids, racks, topic_off, drf, th, part_off, part_id, rep_off, cur, names, name_off,
                                json, json_cap, json_off, st):
-        c_off = view(cand_off, K + 1, np.int32)
-        t_off = view(topic_off, K + 1, np.int32)
+        c_off = util.view(cand_off, K + 1, np.int32)
+        t_off = util.view(topic_off, K + 1, np.int32)
         T = int(t_off[-1])
-        p_off = view(part_off, T + 1, np.int64)
+        p_off = util.view(part_off, T + 1, np.int64)
         Q = int(p_off[-1])
-        r_off = view(rep_off, Q + 1, np.int64)
-        n_off = view(name_off, T + 1, np.int64)
-        self.seen = dict(K=K, cap=json_cap, cand_off=c_off, topic_off=t_off, desired_rf=view(drf, K, np.int32), topic_hash=view(th, T, np.int32),
-                         part_off=p_off, part_id=view(part_id, Q, np.int32), rep_off=r_off, cur=view(cur, int(r_off[-1]), np.int32),
-                         name_off=n_off, names=bytes(view(names, int(n_off[-1]), np.uint8)))
+        r_off = util.view(rep_off, Q + 1, np.int64)
+        n_off = util.view(name_off, T + 1, np.int64)
+        self.seen = dict(K=K, cap=json_cap, cand_off=c_off, topic_off=t_off, desired_rf=util.view(drf, K, np.int32), topic_hash=util.view(th, T, np.int32),
+                         part_off=p_off, part_id=util.view(part_id, Q, np.int32), rep_off=r_off, cur=util.view(cur, int(r_off[-1]), np.int32),
+                         name_off=n_off, names=bytes(util.view(names, int(n_off[-1]), np.uint8)))
         buf = np.ctypeslib.as_array(ctypes.cast(json, ctypes.POINTER(ctypes.c_uint8)), shape=(json_cap,))
         offs = np.ctypeslib.as_array(ctypes.cast(json_off, ctypes.POINTER(ctypes.c_int64)), shape=(K + 1,))
         offs[0] = 0
@@ -76,7 +76,7 @@ def test_solve_clusters_json_marshals_the_layout_and_names():
              np.array([0], np.int64), np.zeros(0, np.int32), 2)
     b = (np.array([5, 6], np.int32), np.array([0, 1], np.int32), np.array([21], np.int32), np.array([0, 2], np.int64), None,
          np.array([0, 3, 6], np.int64), np.array([5, 6, 7, 6, 5, 7], np.int32), 3)
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     res = s.solve_clusters_json([a, empty, b], [["alpha", "be"], [], ["c.d"]])
     got = s._L.seen
     assert got["K"] == 3
@@ -95,7 +95,7 @@ def test_solve_clusters_json_marshals_the_layout_and_names():
 def test_solve_clusters_json_takes_a_buffer():
     c = (np.array([1, 2], np.int32), np.array([0, 1], np.int32), np.array([5], np.int32), np.array([0, 1], np.int64), None,
          np.array([0, 1], np.int64), np.array([2], np.int32), -1)
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     buf = np.zeros(100, dtype=np.uint8)
     res = s.solve_clusters_json([c, c, c], [["x"], ["y"], ["z"]], json_buf=buf)
     assert s._L.seen["cap"] == 100 and bytes(buf[:7]) == b"<doc 0>"

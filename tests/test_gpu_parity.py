@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 import kafka_assigner_b200 as kab
-from tests import util
+from tests import models, util
 
 pytestmark = pytest.mark.gpu
 
@@ -362,17 +362,6 @@ def test_per_slot_ring_on_one_gpu(native_lib, oracle):
                 assert final[i, slot] == octx.counter(int(bid), slot), (shape, int(bid), slot)
 
 
-def _expected_json(cl, out, out_len):
-    """KafkaAssignmentGenerator.java:169-186 in the predicted org.json key order (SURVEY §3.4), built on the host."""
-    rows = out.reshape(cl.T, cl.P, -1)
-    lens = out_len.reshape(cl.T, cl.P)
-    parts = []
-    for t, name in enumerate(cl.topic_names):
-        for p in range(cl.P):
-            parts.append('{"partition":%d,"replicas":[%s],"topic":"%s"}' % (p, ",".join(str(int(b)) for b in rows[t, p, :lens[t, p]]), name))
-    return '{"partitions":[' + ",".join(parts) + '],"version":1}'
-
-
 def test_device_json_emitter_byte_for_byte(native_lib, oracle):
     """ka_solve_dense_json: solve + JSON text on the device, streamed per pipeline block — byte-for-byte against the text built
     from the oracle's rows, on BASELINE config 2 in full, a pipelined run (3 blocks), odd shapes, and the empty run."""
@@ -384,7 +373,7 @@ def test_device_json_emitter_byte_for_byte(native_lib, oracle):
         s.set_brokers(cl.broker_id, cl.rack_index)
         text, st = s.solve_dense_json(cl.topic_names, cl.topic_hash, cl.cur)
         assert st.code == 0
-        assert bytes(text).decode() == _expected_json(cl, exp_out, exp_len), cl.name
+        assert bytes(text).decode() == models.dense_document(cl, exp_out, exp_len), cl.name
     # a failing topic: the reference prints no NEW ASSIGNMENT at all (KAG:186 is never reached)
     bad = kab.synth.make_cluster(T=6, P=4, RF=3, N=9, R=3, seed=8, kind="random")
     s = kab.Solver(0)
@@ -398,12 +387,12 @@ def test_device_json_emitter_pipelined_blocks(native_lib, oracle):
     code = ("import numpy as np, kafka_assigner_b200 as kab\n"
             "from oracle import oracle_lib as ol\n"
             "from tests import util\n"
-            "from tests.test_gpu_parity import _expected_json\n"
+            "from tests import models\n"
             "cl = kab.synth.make_cluster(T=300, P=24, RF=3, N=40, R=5, seed=77, kind='mixed')\n"
             "exp, ln, st = util.oracle_dense(ol, cl)\n"
             "s = kab.Solver(0); s.set_brokers(cl.broker_id, cl.rack_index)\n"
             "text, st = s.solve_dense_json(cl.topic_names, cl.topic_hash, cl.cur)\n"
-            "assert bytes(text).decode() == _expected_json(cl, exp, ln)\n"
+            "assert bytes(text).decode() == models.dense_document(cl, exp, ln)\n"
             "print('OK')\n")
     env = dict(os.environ, KA_PIPELINE_STAGES="3", PYTHONPATH=util.os.path.dirname(util.HERE))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, env=env)

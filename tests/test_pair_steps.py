@@ -16,8 +16,7 @@ import random
 import pytest
 
 import kafka_assigner_b200 as kab
-from tests import util
-from tests.test_schedule_model import INF, build_records
+from tests import models, util
 
 
 def holders_of(recs, N, P, t):
@@ -45,7 +44,7 @@ def run_pair_model(cl, sets, launches, c0, c1, c2):
     """Both slot chains as pair steps over the topic ranges `launches` (each cut into (t, t+1) steps, a single step at the
     end of an odd range). Updates the counter lists in place; returns the ordered rows (broker indices)."""
     N, P = cl.N, cl.P
-    recs = build_records(cl, sets)
+    recs = models.build_records(cl, sets)
     hold = {t: holders_of(recs, N, P, t) for t in range(1, cl.T)}
     mid, out = {}, {}
 
@@ -147,7 +146,7 @@ def test_pair_steps_reproduce_the_reference(oracle, shape):
         octx = oracle.OracleContext()
         sets = _sets(oracle, cl, octx)
         N = cl.N
-        c0, c1, c2 = [0] * N + [INF], [0] * N + [INF], [0] * (N + 1)
+        c0, c1, c2 = [0] * N + [models.INF], [0] * N + [models.INF], [0] * (N + 1)
         out = run_pair_model(cl, sets, _cuts(cl.T, rng), c0, c1, c2)
         for t in range(cl.T):
             for p in range(cl.P):
@@ -161,7 +160,7 @@ def test_pair_steps_carry_one_context_across_runs(oracle):
     octx = oracle.OracleContext()
     first = kab.synth.make_cluster(T=9, P=60, RF=3, N=200, R=8, seed=31, kind="mixed")
     N = first.N
-    c0, c1, c2 = [0] * N + [INF], [0] * N + [INF], [0] * (N + 1)
+    c0, c1, c2 = [0] * N + [models.INF], [0] * N + [models.INF], [0] * (N + 1)
     for seed, T in ((31, 9), (32, 6)):
         cl = kab.synth.make_cluster(T=T, P=60, RF=3, N=200, R=8, seed=seed, kind="mixed")
         assert list(cl.broker_id) == list(first.broker_id)

@@ -15,149 +15,36 @@ from tests import util
 
 pytestmark = pytest.mark.gpu
 
-FRACS = (0.01, 0.02, 0.05, 0.10, 0.20, 0.30, 0.40, 0.50)
-
-
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
-
-
-class Problem:
-    """The ka_solve inputs of one run (host arrays)."""
-
-    def __init__(self, names, topic_hash, part_off, part_id, rep_off, cur, desired_rf=-1, out_stride=None):
-        self.names, self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur = names, topic_hash, part_off, part_id, rep_off, cur
-        self.desired_rf = desired_rf
-        sizes = np.diff(rep_off)
-        self.S = out_stride or max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
-
-    @classmethod
-    def of(cls, cl, desired_rf=-1):
-        return cls(cl.topic_names, cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off, cl.cur, desired_rf)
-
-    def args(self):
-        return self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur, self.desired_rf
-
-    def sequential(self, tables):
-        """The contract's reference: a fresh context per table, ka_ctx_set_brokers + ka_solve."""
-        rows = []
-        for ids, racks in tables:
-            s = kab.Solver(0)
-            s.set_brokers(ids, racks)
-            out, ln, st = s.solve_ragged(*self.args(), self.S, check=False)
-            rows.append((out, ln, _fields(st)))
-            s.close()
-        return rows
-
-    def batched(self, tables, solver=None):
-        s = solver or kab.Solver(0)
-        out, ln, sts = s.solve_ragged_candidates(tables, *self.args(), out_stride=self.S)
-        return out, ln, [_fields(st) for st in sts]
-
-
-def _check_equal(prob, tables, oracle=None, solver=None):
-    out, ln, sts = prob.batched(tables, solver)
-    seq = prob.sequential(tables)
-    assert len(sts) == len(tables)
-    for k, (e_out, e_len, e_st) in enumerate(seq):
-        assert sts[k] == e_st, (k, sts[k], e_st)
-        if e_st[0] != 0:
-            continue   # the rows of a failed candidate are unspecified
-        assert np.array_equal(out[k], e_out), k
-        assert np.array_equal(ln[k], e_len), k
-        if oracle is not None:
-            ids, racks = tables[k]
-            o_len, _, o_out, o_st = oracle.run(oracle.OracleContext(), prob.names, prob.part_off, prob.part_id, prob.rep_off, prob.cur,
-                                               ids, ["k%d" % r for r in racks], prob.desired_rf, prob.S, raise_on_error=False)
-            assert o_st.code == 0, k
-            assert np.array_equal(out[k], o_out) and np.array_equal(ln[k], o_len), k
-    return sts
-
-
-def _table(ids, racks_per=None):
-    """(ids, rack_index): racks_per = brokers per rack (contiguous), or None: no broker has a rack."""
-    ids = np.asarray(ids, dtype=np.int32)
-    names = [None] * len(ids) if racks_per is None else ["k%d" % (i // racks_per) for i in range(len(ids))]
-    return ids, kab.synth.rack_indices(ids, names)
-
-
-def _sparse_with_empty_topics(cl, rng, empty):
-    """cl's topics with sparse (ascending, gapped) partition ids and, with `empty`, a topic without partitions after every
-    seventh one."""
-    names, th, P, pid = [], [], [], []
-    for t in range(cl.T):
-        a, b = int(cl.part_off[t]), int(cl.part_off[t + 1])
-        names.append(cl.topic_names[t])
-        th.append(cl.topic_hash[t])
-        P.append(b - a)
-        pid.append(np.cumsum(rng.integers(1, 9, size=b - a)).astype(np.int32) - 1)
-        if empty and t % 7 == 3:
-            names.append("empty.%d" % t)
-            th.append(kab.java_string_hash("empty.%d" % t))
-            P.append(0)
-            pid.append(np.zeros(0, dtype=np.int32))
-    part_off = np.zeros(len(P) + 1, dtype=np.int64)
-    np.cumsum(P, out=part_off[1:])
-    return names, np.array(th, dtype=np.int32), part_off, np.concatenate(pid), cl.rep_off, cl.cur
-
-
-def _mixed_tables(rng, cl):
-    live = cl.broker_id
-    return [
-        (cl.broker_id, cl.rack_index),                                                        # capacity > 1, the cluster's racks
-        _table(np.sort(rng.choice(live, len(live) - 4, replace=False))),                      # capacity > 1, no racks
-        _table(np.sort(rng.choice(live, len(live) - 6, replace=False)), 3),                   # capacity > 1, other racks
-        _table(np.arange(1, 1 + 4000, dtype=np.int32), 40),                                   # capacity 1, racks
-        _table(np.arange(1, 1 + 3000, dtype=np.int32)),                                       # capacity 1, no racks
-        _table(1 + 2 * np.arange(20000, dtype=np.int32), 500),                                # 20 000 brokers, global id LUT
-        _table(np.zeros(0, dtype=np.int32)),                                                  # no broker
-    ]
-
-
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_random_ragged_clusters_match_sequential_and_oracle(native_lib, oracle, seed):
     rng = np.random.default_rng(seed)
     cl = kab.synth.make_ragged_cluster(T=80, N=40, R=5, max_partitions=64, seed=seed, remove_frac=0.1)
-    tables = _mixed_tables(rng, cl)
+    tables = util.ragged_mixed_tables(rng, cl)
     n_ok = 0
     for desired_rf in (-1, 1, 2, 3):
         # topics without partitions fail every run without a desired RF (KTA:65-66): only with one
-        prob = Problem(*_sparse_with_empty_topics(cl, rng, desired_rf > 0), desired_rf)
+        prob = util.Problem(*util.sparse_with_empty_topics(cl, rng, desired_rf > 0), desired_rf)
         assert desired_rf < 0 or np.any(np.diff(prob.part_off) == 0)
-        sts = _check_equal(prob, tables, oracle)
+        sts = util.check_equal(prob, tables, oracle)
         n_ok += sum(st[0] == 0 for st in sts)
         assert sts[-1][0] == _native.KA_ERR_RF_GT_BROKERS
         if seed == 1 and desired_rf == -1:   # the same call with every counter column in global memory
             with mock.patch.dict(os.environ, {"KA_ORDER_GLOBAL_CTR": "1"}):
-                _check_equal(prob, tables, oracle)
+                util.check_equal(prob, tables, oracle)
     assert n_ok >= 16, n_ok
 
 
-def _exception_problem(tail):
-    """Three topics whose failure depends on the table, then `tail`: a list-size mismatch, or a topic without partitions."""
-    topics = [("alpha", {3: [1, 2], 7: [2, 3], 8: [3, 4], 40: [4, 5], 41: [5, 6]}),
-              ("polygenelubricants", {5: [1, 2], 6: [2, 1]}),       # String.hashCode == Integer.MIN_VALUE (KAS:190-192)
-              ("gamma", {11: [1, 2, 3], 12: [2, 3, 4], 13: [3, 4, 5]})]
-    if tail == "mismatch":
-        topics.append(("delta", {0: [1, 2], 9: [3]}))
-    elif tail == "empty":
-        topics.append(("none", {}))
-    names, part_off, part_id, rep_off, cur = util.flatten(topics)
-    th = np.array([kab.java_string_hash(n) for n in names], dtype=np.int32)
-    return Problem(names, th, part_off, part_id, rep_off, cur, -1, 3)
-
-
 def test_one_exception_per_candidate(native_lib, oracle):
-    A = _table(np.arange(1, 9, dtype=np.int32))            # solves the three topics
-    B = _table(np.arange(1, 3, dtype=np.int32))            # gamma: RF 3 > 2 brokers (KTA:67-69)
-    C = _table(np.arange(1, 4, dtype=np.int32))            # polygenelubricants: 2^31 % 3 != 0 (KAS:190-192)
-    D = _table(np.arange(1, 9, dtype=np.int32), 4)         # gamma: RF 3 over two racks (KAS:183-184)
-    E = _table(np.zeros(0, dtype=np.int32))                # alpha: no broker at all
+    A = util.table(np.arange(1, 9, dtype=np.int32))            # solves the three topics
+    B = util.table(np.arange(1, 3, dtype=np.int32))            # gamma: RF 3 > 2 brokers (KTA:67-69)
+    C = util.table(np.arange(1, 4, dtype=np.int32))            # polygenelubricants: 2^31 % 3 != 0 (KAS:190-192)
+    D = util.table(np.arange(1, 9, dtype=np.int32), 4)         # gamma: RF 3 over two racks (KAS:183-184)
+    E = util.table(np.zeros(0, dtype=np.int32))                # alpha: no broker at all
     tables = [A, B, C, D, E]
     kinds = {}
     for tail, first in (("mismatch", _native.KA_ERR_RF_MISMATCH), ("empty", _native.KA_ERR_RF_NOT_POSITIVE)):
-        prob = _exception_problem(tail)
-        sts = _check_equal(prob, tables, oracle)
+        prob = util.exception_problem(tail)
+        sts = util.check_equal(prob, tables, oracle)
         assert sts[0][:2] == (first, 3)
         assert sts[1][:2] == (_native.KA_ERR_RF_GT_BROKERS, 2) and sts[1][3] == 3
         assert sts[2][0] == _native.KA_ERR_HASH_INDEX and sts[2][1] == 1 and sts[2][3:] == (-2, 3)
@@ -169,7 +56,7 @@ def test_one_exception_per_candidate(native_lib, oracle):
             kinds[st[0]] = st
     assert set(kinds) == {1, 2, 3, 4, 5}
     # the return code is the status of the lowest failing candidate
-    prob = _exception_problem(None)
+    prob = util.exception_problem(None)
     st = (kab.KaStatus * 3)()
     assert _call(kab.Solver(0), prob, [A, C, B], st) == _native.KA_ERR_HASH_INDEX
     assert st[0].code == 0 and st[1].code == _native.KA_ERR_HASH_INDEX and st[2].code == _native.KA_ERR_RF_GT_BROKERS
@@ -185,7 +72,7 @@ def _dense_rows(cl, tables):
     ln = torch.full((K, cl.T, cl.P), -7, dtype=torch.int32, device="cuda")
     sts = kab.Solver(0).solve_dense_candidates_device(tables, cl.T, d_hash.data_ptr(), cl.P, cl.RF, d_cur.data_ptr(), -1, cl.RF,
                                                       ln.data_ptr(), out.data_ptr())
-    return out.cpu().numpy().reshape(K, -1, cl.RF), ln.cpu().numpy().reshape(K, -1), [_fields(st) for st in sts]
+    return out.cpu().numpy().reshape(K, -1, cl.RF), ln.cpu().numpy().reshape(K, -1), [util.fields(st) for st in sts]
 
 
 @pytest.mark.parametrize("key", ["c2", "c3"])
@@ -201,17 +88,17 @@ def test_baseline_configs_in_the_ragged_layout_match_the_dense_batch(native_lib,
     s = kab.Solver(0)
     out, ln, sts = s.solve_ragged_candidates(tables, cl.topic_hash, part_off, part_id, rep_off, cur, -1)
     d_out, d_ln, d_sts = _dense_rows(cl, tables)
-    assert [_fields(st) for st in sts] == d_sts and all(st[0] == 0 for st in d_sts)
+    assert [util.fields(st) for st in sts] == d_sts and all(st[0] == 0 for st in d_sts)
     assert np.array_equal(out, d_out) and np.array_equal(ln, d_ln)
     if key == "c2":   # and the sequential single solves
-        _check_equal(Problem(cl.topic_names, cl.topic_hash, part_off, part_id, rep_off, cur), tables)
+        util.check_equal(util.Problem(cl.topic_names, cl.topic_hash, part_off, part_id, rep_off, cur), tables)
 
 
 def test_million_partition_ragged_cluster_decommission_sweep(native_lib):
     cl = kab.synth.make_ragged_cluster(T=240000, N=400, max_partitions=128, seed=11)
     assert cl.Q > 1_000_000
-    tables = kab.synth.ragged_decommission_tables(cl, FRACS)
-    sts = _check_equal(Problem.of(cl), tables)
+    tables = kab.synth.ragged_decommission_tables(cl, util.FRACS)
+    sts = util.check_equal(util.Problem.of(cl), tables)
     assert all(st[0] == 0 for st in sts[:6]), sts   # up to 30 % removed; beyond, some partition may find no rack left
 
 
@@ -237,19 +124,19 @@ def test_ctx_is_untouched(native_lib):
     s, fresh = kab.Solver(0), kab.Solver(0)
     for x in (s, fresh):
         x.set_brokers(cl.broker_id, cl.rack_index)
-        x.solve_ragged(*Problem.of(half).args(), 3)   # some counters in the Context
+        x.solve_ragged(*util.Problem.of(half).args(), 3)   # some counters in the Context
     before = s.counters()
-    _check_equal(Problem.of(cl), kab.synth.ragged_decommission_tables(cl, (0.1, 0.3)), solver=s)
+    util.check_equal(util.Problem.of(cl), kab.synth.ragged_decommission_tables(cl, (0.1, 0.3)), solver=s)
     assert np.array_equal(s.counters(), before) and np.array_equal(s.broker_id, cl.broker_id)
-    a, al, ast = s.solve_ragged(*Problem.of(cl).args(), 3)
-    b, bl, bst = fresh.solve_ragged(*Problem.of(cl).args(), 3)
+    a, al, ast = s.solve_ragged(*util.Problem.of(cl).args(), 3)
+    b, bl, bst = fresh.solve_ragged(*util.Problem.of(cl).args(), 3)
     assert ast.code == bst.code == 0 and np.array_equal(a, b) and np.array_equal(al, bl)
     assert np.array_equal(s.counters(), fresh.counters())
 
 
 def test_launches_do_not_depend_on_k(native_lib):
     cl = kab.synth.make_ragged_cluster(T=3000, N=120, R=6, seed=21)
-    prob = Problem.of(cl)
+    prob = util.Problem.of(cl)
     s = kab.Solver(0)
     counts = []
     for K in (1, 8):
@@ -261,7 +148,7 @@ def test_launches_do_not_depend_on_k(native_lib):
 
 def test_arguments_and_limits(native_lib):
     cl = kab.synth.make_ragged_cluster(T=40, N=30, R=5, seed=5)
-    prob = Problem.of(cl)
+    prob = util.Problem.of(cl)
     good = [(cl.broker_id, cl.rack_index)]
     s = kab.Solver(0)
     st = (kab.KaStatus * 200)()
@@ -272,9 +159,9 @@ def test_arguments_and_limits(native_lib):
     assert _call(s, prob, good, st, out_stride=2) == _native.KA_ERR_BAD_ARG   # lists of 3
     assert _call(s, prob, good, st, out_stride=0) == _native.KA_ERR_BAD_ARG
     two = kab.synth.make_ragged_cluster(T=40, N=30, R=5, seed=5, rf_weights=(0.5, 0.5))   # lists of 1 and 2
-    p2 = Problem.of(two)
+    p2 = util.Problem.of(two)
     assert p2.S == 2 and _call(s, p2, good, st) == 0
-    p3 = Problem(p2.names, p2.topic_hash, p2.part_off, p2.part_id, p2.rep_off, p2.cur, 3, 2)
+    p3 = util.Problem(p2.names, p2.topic_hash, p2.part_off, p2.part_id, p2.rep_off, p2.cur, 3, 2)
     assert _call(s, p3, good, st) == _native.KA_ERR_BAD_ARG                      # desired RF above the stride
     unsorted = [(cl.broker_id[::-1].copy(), cl.rack_index[::-1].copy())]
     assert _call(s, prob, good + unsorted, st) == _native.KA_ERR_BAD_ARG and st[0].code == st[1].code == _native.KA_ERR_BAD_ARG
@@ -292,11 +179,11 @@ def test_arguments_and_limits(native_lib):
         _, _, rst = ref.solve_ragged(prob.topic_hash, p_off, prob.part_id, r_off, prob.cur, -1, 3, check=False)
         assert rst.code == _native.KA_ERR_BAD_ARG
         assert _call(s, prob, good * 2, st, **kw) == _native.KA_ERR_BAD_ARG
-        assert _fields(st[0]) == _fields(st[1]) == _fields(rst), kw
+        assert util.fields(st[0]) == util.fields(st[1]) == util.fields(rst), kw
     # K * ΣP at 2^31: the call-wide level table's positions are 32-bit (refused before anything is written)
     Q = (1 << 31) // 128
-    big = Problem(["t"], prob.topic_hash[:1], np.array([0, Q], dtype=np.int64), None, np.zeros(Q + 1, dtype=np.int64),
-                  np.zeros(0, dtype=np.int32), 1, 1)
+    big = util.Problem(["t"], prob.topic_hash[:1], np.array([0, Q], dtype=np.int64), None, np.zeros(Q + 1, dtype=np.int64),
+                       np.zeros(0, dtype=np.int32), 1, 1)
     assert _call(s, big, good * 128, st, out_elems=1) == _native.KA_ERR_LIMIT and st[127].code == _native.KA_ERR_LIMIT
 
 

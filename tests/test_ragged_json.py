@@ -10,38 +10,7 @@ import numpy as np
 import pytest
 
 import kafka_assigner_b200 as kab
-from tests import util
-
-EMPTY = '{"partitions":[],"version":1}'
-KEY = lambda st: (st.code, st.topic_index, st.partition, st.a, st.b)  # noqa: E731
-
-
-def _quote(name):
-    """org.json JSONObject.quote() for the names these tests use."""
-    return '"' + name.replace("\\", "\\\\").replace('"', '\\"') + '"'
-
-
-def _text(names, part_off, part_id, out, out_len):
-    parts = []
-    for t, name in enumerate(names):
-        q = _quote(name)
-        for g in range(int(part_off[t]), int(part_off[t + 1])):
-            parts.append('{"partition":%d,"replicas":[%s],"topic":%s}' % (part_id[g], ",".join(map(str, out[g, :out_len[g]])), q))
-    return '{"partitions":[' + ",".join(parts) + '],"version":1}'
-
-
-def _stride(rep_off, desired):
-    sizes = np.diff(rep_off)
-    return max(int(sizes.max()) if len(sizes) else 0, desired, 1)
-
-
-def _oracle_text(ol, names, part_off, part_id, rep_off, cur, brokers, rack_names, desired, ctx=None):
-    """(text or None, oracle status) of one run through the C++ oracle."""
-    pid = part_id if part_id is not None else np.concatenate(
-        [np.arange(part_off[t + 1] - part_off[t], dtype=np.int32) for t in range(len(names))] + [np.zeros(0, np.int32)])
-    ln, opid, out, st = ol.run(ctx or ol.OracleContext(), names, part_off, pid, rep_off, cur, brokers, rack_names, desired,
-                               _stride(rep_off, desired), raise_on_error=False)
-    return (None if st.code else _text(names, part_off, opid, out, ln)), st
+from tests import models, util
 
 
 def _json(solver, names, th, part_off, part_id, rep_off, cur, desired, **kw):
@@ -114,7 +83,7 @@ def test_random_ragged_cases_json_vs_oracle(native_lib, oracle):
         names, part_off, part_id, rep_off, cur = util.flatten(case["topics"])
         brokers = sorted(case["brokers"])
         desired = case["desired_rf"]
-        exp, est = _oracle_text(oracle, names, part_off, part_id, rep_off, cur, brokers, [case["racks"].get(b) for b in brokers], desired)
+        exp, est = util.oracle_text(oracle, names, part_off, part_id, rep_off, cur, brokers, [case["racks"].get(b) for b in brokers], desired)
         th = np.array([kab.java_string_hash(n) for n in names], dtype=np.int32)
         if all(np.array_equal(part_id[part_off[t]:part_off[t + 1]], np.arange(part_off[t + 1] - part_off[t])) for t in range(len(names))) \
                 and it % 2:
@@ -123,8 +92,8 @@ def test_random_ragged_cases_json_vs_oracle(native_lib, oracle):
             solver.reset()
             solver.set_brokers_with_racks(brokers, case["racks"])
         text, st = _json(s, names, th, part_off, part_id, rep_off, cur, desired)
-        _, _, rst = ref.solve_ragged(th, part_off, part_id, rep_off, cur, desired, _stride(rep_off, desired), check=False)
-        assert KEY(st) == KEY(rst), (it, case)
+        _, _, rst = ref.solve_ragged(th, part_off, part_id, rep_off, cur, desired, util.row_width(rep_off, desired), check=False)
+        assert util.fields(st) == util.fields(rst), (it, case)
         if exp is None:
             assert text == "" and (st.code, st.topic_index, st.partition, st.a, st.b) == (est.code, est.topic_index, est.partition, est.a, est.b), (it, case)
             kinds.add(st.code)
@@ -132,7 +101,7 @@ def test_random_ragged_cases_json_vs_oracle(native_lib, oracle):
             assert st.code == 0 and text == exp, (it, case)
             assert np.array_equal(s.counters(), ref.counters()), it
             n_ok += 1
-            n_wide += _stride(rep_off, desired) >= 4
+            n_wide += util.row_width(rep_off, desired) >= 4
     assert kinds == {1, 2, 3, 4, 5} and n_ok > 60 and n_wide > 20, (kinds, n_ok, n_wide)
 
 
@@ -140,7 +109,7 @@ def _fast_text(oracle, cl):
     out, ln, est = oracle.fast_run_dense(oracle.FastContext(), cl.topic_hash, cl.cur, cl.broker_id, cl.rack_index)
     assert est.code == 0
     part_off, part_id, _, _ = cl.ragged()
-    return _text(cl.topic_names, part_off, part_id, out, ln)
+    return models.solve_document(cl.topic_names, part_off, part_id, out, ln)
 
 
 @pytest.mark.gpu
@@ -174,7 +143,7 @@ def test_million_partition_ragged_cluster(native_lib, oracle):
     cl = kab.synth.make_ragged_cluster(T=240000, N=400, max_partitions=128, seed=11, remove_frac=0.05)
     assert cl.Q > 1_000_000
     octx = oracle.OracleContext()
-    exp, est = _oracle_text(oracle, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, cl.broker_id, cl.rack_name, -1, octx)
+    exp, est = util.oracle_text(oracle, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, cl.broker_id, cl.rack_name, -1, octx)
     assert est.code == 0
     s = kab.Solver(0)
     s.set_brokers(cl.broker_id, cl.rack_index)
@@ -198,9 +167,9 @@ def test_edge_cases(native_lib, oracle):
     part_off, part_id, rep_off, cur = (np.array([0, 2, 3], dtype=np.int64), np.array([0, 4, 1], dtype=np.int32),
                                        np.array([0, 2, 4, 6], dtype=np.int64), np.array([1, 2, 2, 3, 4, 1], dtype=np.int32))
     # the empty run: no topics, or only topics without partitions under a desired RF
-    assert _json(s, [], np.zeros(0, np.int32), np.zeros(1, np.int64), None, np.zeros(1, np.int64), np.zeros(0, np.int32), -1)[0] == EMPTY
+    assert _json(s, [], np.zeros(0, np.int32), np.zeros(1, np.int64), None, np.zeros(1, np.int64), np.zeros(0, np.int32), -1)[0] == models.EMPTY_DOCUMENT
     text, st = _json(s, names, th, np.zeros(3, np.int64), None, np.zeros(1, np.int64), np.zeros(0, np.int32), 2)
-    assert st.code == 0 and text == EMPTY
+    assert st.code == 0 and text == models.EMPTY_DOCUMENT
     text, st = _json(s, names, th, np.zeros(3, np.int64), None, np.zeros(1, np.int64), np.zeros(0, np.int32), -1)
     assert (st.code, st.topic_index, text) == (2, 0, "")                  # KTA:65-66 without a desired RF
     # a name the device emitter would have to escape: refused before anything is solved
@@ -220,7 +189,7 @@ def test_edge_cases(native_lib, oracle):
         buf = np.zeros(cap, dtype=np.uint8)
         text, st = _json(s, names, th, part_off, part_id, rep_off, cur, -1, json_buf=buf)
         assert st.code == code and text == (exp if code == 0 else "")
-    buf = np.zeros(len(EMPTY) - 1, dtype=np.uint8)
+    buf = np.zeros(len(models.EMPTY_DOCUMENT) - 1, dtype=np.uint8)
     assert _json(s, [], np.zeros(0, np.int32), np.zeros(1, np.int64), None, np.zeros(1, np.int64), np.zeros(0, np.int32), -1,
                  json_buf=buf)[1].code == kab._native.KA_ERR_LIMIT
 
@@ -238,9 +207,9 @@ def _snapshot(tmp_path, cl, topics, fname="cluster.json"):
 def _cli_expected(oracle, cl, topics, live, desired):
     names, part_off, part_id, rep_off, cur = util.flatten(topics)
     racks = dict(zip(cl.all_broker_id.tolist(), cl.all_rack_name))
-    new, st = _oracle_text(oracle, names, part_off, part_id, rep_off, cur, live, [racks[b] for b in live], desired)
+    new, st = util.oracle_text(oracle, names, part_off, part_id, rep_off, cur, live, [racks[b] for b in live], desired)
     assert st.code == 0
-    current = ",".join('{"topic":%s,"partition":%d,"replicas":[%s]}' % (_quote(n), p, ",".join(map(str, asg[p])))
+    current = ",".join('{"topic":%s,"partition":%d,"replicas":[%s]}' % (models.quote(n), p, ",".join(map(str, asg[p])))
                        for n, asg in topics for p in sorted(asg))
     return "CURRENT ASSIGNMENT:\n" + '{"version":1,"partitions":[' + current + ']}' + "\nNEW ASSIGNMENT:\n" + new + "\n"
 

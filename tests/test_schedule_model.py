@@ -13,41 +13,10 @@ processed in a scrambled order and the whole slot-0 chain runs before the slot-1
 """
 import random
 
-import numpy as np
 import pytest
 
 import kafka_assigner_b200 as kab
-from tests import util
-
-INF = 0x3FFFFFFF
-
-
-def java_abs_hash(h):
-    return int(np.int64(abs(int(h))) if h != -2**31 else 2**31)
-
-
-def build_records(cl, sets):
-    """What kernel A emits for every row: ([a0, a1, a2] in slot-0 scan order with the dummy N for missing slots, len, e01, e02, e12)."""
-    N = cl.N
-    idx_of = {int(b): i for i, b in enumerate(cl.broker_id)}
-    recs = []
-    for t in range(cl.T):
-        habs = java_abs_hash(cl.topic_hash[t])
-        s2, s3 = habs % 2, habs % 3
-        for p in range(cl.P):
-            ix = sorted(idx_of[int(b)] for b in sets[t][p])          # ascending index == ascending id (KAS:205-214)
-            k = len(ix)
-            a, e = [N, N, N], (0, 0, 0)
-            if k == 1:
-                a[0] = ix[0]
-            elif k == 2:
-                a[0], a[1] = ix[s2], ix[1 - s2]                       # |hash| % 2 == 1: the higher id is scanned first
-            elif k == 3:
-                i = [(3 - s3) % 3, (4 - s3) % 3, (5 - s3) % 3]        # list position at scan position 0, 1, 2
-                a = [ix[i[0]], ix[i[1]], ix[i[2]]]
-                e = tuple(s2 if i[x] < i[y] else 1 - s2 for x, y in ((0, 1), (0, 2), (1, 2)))
-            recs.append((a, k, e))
-    return recs
+from tests import models, util
 
 
 def levels_of_topic(rows):
@@ -64,7 +33,7 @@ def levels_of_topic(rows):
 
 def run_model(cl, sets, rng):
     N, P = cl.N, cl.P
-    recs = build_records(cl, sets)
+    recs = models.build_records(cl, sets)
     # schedule: topic by topic, inside a topic by level; inside a level ANY order (scrambled here)
     order = []
     for t in range(cl.T):
@@ -77,8 +46,8 @@ def run_model(cl, sets, rng):
             rng.shuffle(members)
             order.extend(members)
     assert sorted(order) == list(range(cl.T * P))
-    c0 = [0] * N + [INF]
-    c1 = [0] * N + [INF]
+    c0 = [0] * N + [models.INF]
+    c1 = [0] * N + [models.INF]
     c2 = [0] * (N + 1)
     # ---- slot-0 chain over ALL rows first (it never needs a slot-1 decision) ----
     mid = {}

@@ -21,12 +21,8 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
-from tests.test_clusters import Member, _table
-from tests.test_clusters_json import _check_fleet
-from tests.test_ragged_json import _text
-from tests.test_waves import _cur, _rec, _rows
-from tests.test_waves_json import _raw, bound, reference_wave_docs
-from tests.test_waves_send import reference_send_docs
+from tests import models, util
+from tests.util import Member
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIMIT = _native.KA_ERR_LIMIT
@@ -147,13 +143,13 @@ def test_a_path_is_serial():
 def test_unchanged_and_receiverless_rows_are_not_records():
     cur_lists = [[1], [1, 2], [1, 2], [1, 2], [3], [], [4]]
     new_lists = [[2], [1, 2], [2, 1], [1], [2], [], [4, 2]]
-    rcv, snd = wave_records(*_cur(cur_lists), *_rows(new_lists))
+    rcv, snd = wave_records(*util.cur_lists(cur_lists), *util.rows(new_lists))
     assert rcv == [[2], [], [], [], [2], [], [2]] and snd == [1, 1, 1, 1, 3, None, 4]
     assert chain_rounds(rcv).tolist() == [1, 0, 0, 0, 2, 0, 3]
     # rows that are no record take no slot of a chunk: 2 047 serial records, 500 other rows, then the chunk's last record
     cur_lists = [[1]] * (CHUNK - 1) + [[1, 2]] * 500 + [[1], [1]]
     new_lists = [[2]] * (CHUNK - 1) + [[2, 1] if g % 2 else [1, 2] for g in range(500)] + [[2], [2]]
-    rcv, _ = wave_records(*_cur(cur_lists), *_rows(new_lists))
+    rcv, _ = wave_records(*util.cur_lists(cur_lists), *util.rows(new_lists))
     rounds = chain_rounds(rcv)
     assert rounds[CHUNK - 1:CHUNK + 499].tolist() == [0] * 500
     assert rounds[-2:].tolist() == [CHUNK, CHUNK + 1]
@@ -213,14 +209,14 @@ def reset_input(send, seed=5):
                     new.append(b)
         cur_lists.append(c)
         new_lists.append(new)
-    t_off, t_cur = _cur(cur_lists)
-    t_out, t_len = _rows(new_lists, 3)
+    t_off, t_cur = util.cur_lists(cur_lists)
+    t_out, t_len = util.rows(new_lists, 3)
     bound = C if send else B
     weight = np.concatenate([np.full(n_pre, bound), rng.integers(0, 2 * bound + 1, len(t_len))]).astype(np.int64)
     rep_off = np.concatenate([np.arange(n_pre + 1, dtype=np.int64) * pre_rep, n_pre * pre_rep + t_off[1:]])
     Q = len(weight)
     part_off = np.concatenate([[0], np.sort(rng.choice(np.arange(1, Q), 999, replace=False)), [Q]]).astype(np.int64)
-    ids, racks = _table(np.arange(1, NB + 1), 8)
+    ids, racks = util.table(np.arange(1, NB + 1), 8)
     inp = dict(rep_off=rep_off, cur=np.concatenate([pre_cur, t_cur]).astype(np.int32),
                out=np.concatenate([pre_new, t_out]).astype(np.int32), out_len=np.concatenate([pre_len, t_len]).astype(np.int32),
                weight=weight, B=np.int64(B), part_off=part_off, names=np.array(["reset.%d" % t for t in range(1000)]),
@@ -228,7 +224,7 @@ def reset_input(send, seed=5):
     if send:   # N + n_send: 12 800 words of chain state in shared memory, 12 801 in global memory
         inp.update(C=np.int64(C), send_smem=np.arange(1, NB + 1, dtype=np.int32), send_global=np.arange(1, NB + 2, dtype=np.int32))
     else:
-        gids, gracks = _table(np.arange(1, NB + 2), 8)
+        gids, gracks = util.table(np.arange(1, NB + 2), 8)
         inp.update(ids_global=gids, racks_global=gracks)
     return inp
 
@@ -291,10 +287,10 @@ def reset_plans(request, tmp_path_factory, native_lib):
         rounds = chain_rounds(records, senders if send else None)
         names, part_off = list(inp["names"]), inp["part_off"]
         if send:
-            e_docs, e_wave, e_summ, e_st = reference_send_docs(names, part_off, None, *args, inp["ids"], inp["send_smem"], int(inp["B"]),
-                                                               int(inp["C"]), inp["weight"])
+            e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, None, *args, inp["ids"], int(inp["B"]), inp["weight"],
+                                                            send=(inp["send_smem"], int(inp["C"])))
         else:
-            e_docs, e_wave, e_summ, e_st = reference_wave_docs(names, part_off, None, *args, inp["ids"], int(inp["B"]), inp["weight"])
+            e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, None, *args, inp["ids"], int(inp["B"]), inp["weight"])
         assert e_st == (0, 0, 0)
         e_summ = _summary_array(e_summ, WAVE_SEND_SUMMARY_DTYPE if send else WAVE_SUMMARY_DTYPE)
         out, _ = child.communicate(timeout=max(1.0, CHILD_TIMEOUT - (time.monotonic() - t0)))
@@ -355,7 +351,7 @@ def test_scattered_documents_over_large_tiles(native_lib):
     rows are scattered over the whole input. Every tile of a pass (2 560 rows) holds many digit values, and the first pass
     drops the 60 % of unchanged rows."""
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 61), 4))
+    s.set_brokers(*util.table(np.arange(1, 61), 4))
     rng = np.random.default_rng(14)
     Q = 2_500_000
     first = rng.integers(0, 40, Q)
@@ -369,7 +365,7 @@ def test_scattered_documents_over_large_tiles(native_lib):
     names = ["scatter-%d" % t for t in range(2000)]
     assert Q > 2048 * 1024
     docs, wave, summ, st = s.plan_waves_json(names, part_off, None, rep_off, cur, out, out_len, 1)
-    e_docs, e_wave, e_summ, e_st = reference_wave_docs(names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 1)
+    e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 1)
     assert st.code == 0 and e_st == (0, 0, 0) and 256 <= len(e_docs) <= 65535
     assert np.array_equal(wave, e_wave)
     e_summ = _summary_array(e_summ, WAVE_SUMMARY_DTYPE)
@@ -386,7 +382,7 @@ def test_wave_documents_past_4_gib(native_lib):
     the staged store path past 2^32. Every document is compared on its own, against the model's documents printed with
     placeholder names that are then replaced by the real ones; the whole expected text is never built."""
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 41), 4))
+    s.set_brokers(*util.table(np.arange(1, 41), 4))
     rng = np.random.default_rng(15)
     lens = rng.integers(65000, 65537, 68)
     names = ["L%02d-" % t + "n" * (int(n) - 4) for t, n in enumerate(lens)] + ["s%d" % t for t in range(3)]
@@ -396,10 +392,10 @@ def test_wave_documents_past_4_gib(native_lib):
     g = np.arange(Q)
     cur_lists = [[1, 2]] * Q
     new_lists = [[1, 2] if x % 50 == 0 else [1, 3 + x % 4] for x in g.tolist()]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 2)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 2)
     ph = ["@%d@" % t for t in range(len(names))]
-    e_docs, e_wave, e_summ, e_st = reference_wave_docs(ph, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)
+    e_docs, e_wave, e_summ, e_st = models.wave_docs(ph, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)
     assert e_st == (0, 0, 0)
     real = [n.encode() for n in names]
     topic = re.compile(rb'"topic":"@(\d+)@"')
@@ -408,14 +404,14 @@ def test_wave_documents_past_4_gib(native_lib):
         return topic.sub(lambda m: b'"topic":"' + real[int(m.group(1))] + b'"', doc)
 
     slab, name_off = kab.Solver.marshal_names(names)
-    cap = bound(names, part_off, 2)
+    cap = models.json_bound(names, part_off, 2)
     js = np.empty(cap, dtype=np.uint8)
     doc_off, wave = np.zeros(Q + 1, dtype=np.int64), np.zeros(Q, dtype=np.int32)
     summ = np.zeros(Q, dtype=WAVE_SUMMARY_DTYPE)
-    rc, st, n = _raw(s, len(names), part_off, None, rep_off, cur, 2, out_len, out, None, 2, slab, name_off, js, cap, doc_off, wave,
-                     summ, Q)
+    rc, st, n = util.raw_plan_waves_json(s, len(names), part_off, None, rep_off, cur, 2, out_len, out, None, 2, slab, name_off, js,
+                                         cap, doc_off, wave, summ, Q)
     W = n.value
-    assert rc == 0 and W == len(e_docs) and np.array_equal(wave, e_wave) and [_rec(x) for x in summ[:W]] == e_summ
+    assert rc == 0 and W == len(e_docs) and np.array_equal(wave, e_wave) and [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in summ[:W]] == e_summ
     assert doc_off[W] > 1 << 32
     at = 0
     straddle = 0
@@ -459,7 +455,7 @@ def test_solve_json_at_the_fragment_limit(native_lib, oracle):
     L0 = _l0(Q)
     c = _fragment_cluster(Q, T, L0, 16)
     s = kab.Solver(0)
-    s.set_brokers(*_table(c["ids"], 4))
+    s.set_brokers(*util.table(c["ids"], 4))
     args = (c["part_off"], c["part_id"], c["rep_off"], c["cur"], -1)
     text, st = s.solve_ragged_json(c["names"], c["th"], *args, check=False)
     assert st.code == 0
@@ -472,7 +468,7 @@ def test_solve_json_at_the_fragment_limit(native_lib, oracle):
     assert text[:at].tobytes() == b'{"partitions":['
     for t in range(T):   # record by record, one topic's slice at a time
         a, b = int(c["part_off"][t]), int(c["part_off"][t + 1])
-        e = ("," if t else "") + _text([c["names"][t]], [0, b - a], o_pid[a:b], o_out[a:b], o_len[a:b])[15:-14]
+        e = ("," if t else "") + models.solve_document([c["names"][t]], [0, b - a], o_pid[a:b], o_out[a:b], o_len[a:b])[15:-14]
         assert text[at:at + len(e)].tobytes() == e.encode(), t
         at += len(e)
     assert text[at:].tobytes() == b'],"version":1}'
@@ -500,8 +496,8 @@ def test_solve_clusters_json_applies_the_limit_per_cluster(native_lib, oracle):
     c = _fragment_cluster(Q, 32, 20, 17)
     c["names"][0] = "f000-" + "q" * (L0 + 1 - 5)
     c["th"][0] = kab.java_string_hash(c["names"][0])
-    middle = Member(_table(c["ids"], 4), c["names"], c["th"], c["part_off"], c["part_id"], c["rep_off"], c["cur"])
+    middle = Member(util.table(c["ids"], 4), c["names"], c["th"], c["part_off"], c["part_id"], c["rep_off"], c["cur"])
     fleet = [Member.of(mk(T=60, N=40, R=5, max_partitions=64, seed=31)), middle, Member.of(mk(T=40, N=30, R=4, seed=32))]
-    sts, texts = _check_fleet(fleet, oracle)
+    sts, texts = util.check_fleet(fleet, oracle)
     assert sts[1] == (LIMIT, -1, -1, L0 + 1, 0) and texts[1] == b""
     assert sts[0][0] == sts[2][0] == 0 and texts[0] and texts[2]

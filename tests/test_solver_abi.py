@@ -1,44 +1,23 @@
 """What the Python Solver hands the C ABI, without a device: the library is a fake object that records every argument and writes
 recognisable rows, texts and statuses. Pins the arrays, the row stride, the JSON buffer size, K and the sliced results of the
-single, JSON, candidate and score calls, generate_assignment's stride, and the return contract of the device-pointer calls.
-view / fake_solver are shared with the fleet ABI tests."""
-import ctypes
+single, JSON, candidate and score calls, generate_assignment's stride, and the return contract of the device-pointer calls."""
 
 import numpy as np
 import pytest
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import assigner
+from tests import util
 
 I32, I64 = np.int32, np.int64
 
 
-def view(p, n, ctype):
-    """A copy of the n elements of `ctype` at the C pointer p (None for a NULL pointer)."""
-    if p is None:
-        return None
-    if n == 0:
-        return np.zeros(0, dtype=ctype)
-    return np.ctypeslib.as_array(ctypes.cast(p, ctypes.POINTER(np.ctypeslib.as_ctypes_type(ctype))), shape=(n,)).copy()
-
-
-def fake_solver(lib):
-    s = object.__new__(kab.Solver)
-    s._L = lib
-    s._h = ctypes.c_void_p(1)
-    return s
-
-
-def _writable(p, n, ctype):
-    return np.ctypeslib.as_array(ctypes.cast(p, ctypes.POINTER(np.ctypeslib.as_ctypes_type(ctype))), shape=(n,))
-
-
 def _ragged(th, part_off, part_id, rep_off, cur, T):
-    p_off = view(part_off, T + 1, I64)
+    p_off = util.view(part_off, T + 1, I64)
     Q = int(p_off[-1])
-    r_off = view(rep_off, Q + 1, I64)
-    return dict(T=T, topic_hash=view(th, T, I32), part_off=p_off, part_id=view(part_id, Q, I32), rep_off=r_off,
-                cur=view(cur, int(r_off[-1]), I32)), Q
+    r_off = util.view(rep_off, Q + 1, I64)
+    return dict(T=T, topic_hash=util.view(th, T, I32), part_off=p_off, part_id=util.view(part_id, Q, I32), rep_off=r_off,
+                cur=util.view(cur, int(r_off[-1]), I32)), Q
 
 
 class _FakeLib:
@@ -50,9 +29,9 @@ class _FakeLib:
 
     def _rows(self, out, out_len, n, S):
         if out is not None:
-            _writable(out, n * S, I32)[:] = np.arange(n * S, dtype=I32)
+            util.writable(out, n * S, I32)[:] = np.arange(n * S, dtype=I32)
         if out_len is not None:
-            _writable(out_len, n, I32)[:] = np.arange(n, dtype=I32) % 4
+            util.writable(out_len, n, I32)[:] = np.arange(n, dtype=I32) % 4
 
     def _status(self, st):
         st._obj.code, st._obj.topic_index = self.code, 1
@@ -62,13 +41,13 @@ class _FakeLib:
             st[k].code, st[k].topic_index = (3 if k == 1 else 0), k
 
     def _text(self, json, cap, nbytes, doc=b"<doc>"):
-        _writable(json, cap, np.uint8)[:len(doc)] = np.frombuffer(doc, dtype=np.uint8)
+        util.writable(json, cap, np.uint8)[:len(doc)] = np.frombuffer(doc, dtype=np.uint8)
         nbytes._obj.value = len(doc)
 
     def ka_solve_dense_json(self, h, T, th, P, RF, cur, drf, names, name_off, json, cap, nbytes, st):
-        n_off = view(name_off, T + 1, I64)
-        self.seen = dict(T=T, P=P, RF=RF, topic_hash=view(th, T, I32), cur=view(cur, T * P * RF, I32), desired_rf=drf,
-                         name_off=n_off, names=bytes(view(names, int(n_off[-1]), np.uint8)), cap=cap)
+        n_off = util.view(name_off, T + 1, I64)
+        self.seen = dict(T=T, P=P, RF=RF, topic_hash=util.view(th, T, I32), cur=util.view(cur, T * P * RF, I32), desired_rf=drf,
+                         name_off=n_off, names=bytes(util.view(names, int(n_off[-1]), np.uint8)), cap=cap)
         self._text(json, cap, nbytes)
         self._status(st)
         return self.rc
@@ -82,15 +61,15 @@ class _FakeLib:
 
     def ka_solve_json(self, h, T, th, part_off, part_id, rep_off, cur, drf, names, name_off, json, cap, nbytes, st):
         self.seen, Q = _ragged(th, part_off, part_id, rep_off, cur, T)
-        n_off = view(name_off, T + 1, I64)
-        self.seen.update(desired_rf=drf, name_off=n_off, names=bytes(view(names, int(n_off[-1]), np.uint8)), cap=cap)
+        n_off = util.view(name_off, T + 1, I64)
+        self.seen.update(desired_rf=drf, name_off=n_off, names=bytes(util.view(names, int(n_off[-1]), np.uint8)), cap=cap)
         self._text(json, cap, nbytes)
         self._status(st)
         return self.rc
 
     def _tables(self, K, cand_off, ids, racks):
-        c_off = view(cand_off, K + 1, I32)
-        return dict(K=K, cand_off=c_off, broker_id=view(ids, int(c_off[-1]), I32), broker_rack=view(racks, int(c_off[-1]), I32))
+        c_off = util.view(cand_off, K + 1, I32)
+        return dict(K=K, cand_off=c_off, broker_id=util.view(ids, int(c_off[-1]), I32), broker_rack=util.view(racks, int(c_off[-1]), I32))
 
     def ka_solve_candidates(self, h, K, cand_off, ids, racks, T, th, part_off, part_id, rep_off, cur, drf, S, out_len, out, st):
         self.seen, Q = _ragged(th, part_off, part_id, rep_off, cur, T)
@@ -102,21 +81,21 @@ class _FakeLib:
     def ka_score_candidates(self, h, K, cand_off, ids, racks, T, th, part_off, part_id, rep_off, cur, drf, S, weight, summary,
                             b_rep, b_lead, b_in, out_len, out, st):
         self.seen, Q = _ragged(th, part_off, part_id, rep_off, cur, T)
-        self.seen.update(self._tables(K, cand_off, ids, racks), desired_rf=drf, S=S, weight=view(weight, Q, I64),
+        self.seen.update(self._tables(K, cand_off, ids, racks), desired_rf=drf, S=S, weight=util.view(weight, Q, I64),
                          per_broker=[b is not None for b in (b_rep, b_lead, b_in)], rows=out is not None)
-        sm = _writable(summary, K * len(assigner.MOVE_SUMMARY_DTYPE.names), I64).reshape(K, -1)
+        sm = util.writable(summary, K * len(assigner.MOVE_SUMMARY_DTYPE.names), I64).reshape(K, -1)
         sm[:, 0] = 100 + np.arange(K)                                            # rows_changed
         nb = int(self.seen["cand_off"][-1])
         for i, b in enumerate((b_rep, b_lead, b_in)):
             if b is not None:
-                _writable(b, nb, I64)[:] = 10 * (i + 1) + np.arange(nb)
+                util.writable(b, nb, I64)[:] = 10 * (i + 1) + np.arange(nb)
         self._rows(out, out_len, K * Q, S)
         self._statuses(st, K)
         return self.rc
 
     def ka_rack_indices(self, n, ids, names, racks):
-        self.brokers = view(ids, n, I32).tolist()
-        _writable(racks, n, I32)[:] = 0
+        self.brokers = util.view(ids, n, I32).tolist()
+        util.writable(racks, n, I32)[:] = 0
         return 0
 
     def ka_ctx_set_brokers(self, h, n, ids, racks):
@@ -160,7 +139,7 @@ def _check_tables(got):
 
 @pytest.mark.parametrize("desired_rf, S", [(-1, 2), (1, 2), (3, 3)])
 def test_solve_dense_json_marshals_names_and_the_sufficient_buffer(desired_rf, S):
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     cur = np.arange(12).reshape(2, 3, 2)                                     # T = 2, P = 3, RF = 2 (int64: coerced to int32)
     text, st = s.solve_dense_json(["ab", "cde"], [5, 6], cur, desired_rf)
     got = s._L.seen
@@ -173,7 +152,7 @@ def test_solve_dense_json_marshals_names_and_the_sufficient_buffer(desired_rf, S
 
 
 def test_solve_dense_json_takes_a_buffer_and_a_name_slab():
-    s = fake_solver(_FakeLib(code=kab._native.KA_ERR_RF_MISMATCH))
+    s = util.fake_solver(_FakeLib(code=kab._native.KA_ERR_RF_MISMATCH))
     buf = np.zeros(40, dtype=np.uint8)
     slab = kab.Solver.marshal_names(["x", "yz"])
     text, st = s.solve_dense_json(None, [5, 6], np.ones((2, 1, 1), I32), -1, json_buf=buf, check=False, names_slab=slab)
@@ -185,7 +164,7 @@ def test_solve_dense_json_takes_a_buffer_and_a_name_slab():
 
 @pytest.mark.parametrize("desired_rf, S", [(-1, 3), (2, 3), (4, 4)])
 def test_solve_ragged_json_marshals_the_layout_and_the_sufficient_buffer(desired_rf, S):
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     text, st = s.solve_ragged_json(["alpha", "be"], *RAGGED, desired_rf)
     got = s._L.seen
     _check_ragged(got)
@@ -196,7 +175,7 @@ def test_solve_ragged_json_marshals_the_layout_and_the_sufficient_buffer(desired
 
 
 def test_solve_ragged_json_without_ids_or_topics():
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     s.solve_ragged_json([], [], [0], None, [0], [], -1)
     assert s._L.seen["part_id"] is None and s._L.seen["cap"] == 64
     buf = np.zeros(30, dtype=np.uint8)
@@ -205,7 +184,7 @@ def test_solve_ragged_json_without_ids_or_topics():
 
 
 def test_solve_ragged_passes_the_stride_and_slices_nothing():
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     out, ln, st = s.solve_ragged(*RAGGED, -1, 4)
     _check_ragged(s._L.seen)
     assert s._L.seen["S"] == 4 and out.shape == (3, 4) and out[2].tolist() == [8, 9, 10, 11] and ln.tolist() == [0, 1, 2]
@@ -213,7 +192,7 @@ def test_solve_ragged_passes_the_stride_and_slices_nothing():
 
 @pytest.mark.parametrize("desired_rf, out_stride, S", [(-1, None, 3), (4, None, 4), (-1, 2, 2)])
 def test_solve_ragged_candidates_marshals_tables_and_slices_rows(desired_rf, out_stride, S):
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     out, ln, st = s.solve_ragged_candidates(TABLES, *RAGGED, desired_rf, out_stride)
     got = s._L.seen
     _check_ragged(got)
@@ -225,7 +204,7 @@ def test_solve_ragged_candidates_marshals_tables_and_slices_rows(desired_rf, out
 
 
 def test_solve_ragged_candidates_without_tables():
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     out, ln, st = s.solve_ragged_candidates([], *RAGGED, -1)
     assert s._L.seen["K"] == 0 and s._L.seen["cand_off"].tolist() == [0]
     assert out.shape == (0, 3, 3) and ln.shape == (0, 3) and st == []
@@ -233,7 +212,7 @@ def test_solve_ragged_candidates_without_tables():
 
 @pytest.mark.parametrize("rows, per_broker", [(False, False), (True, False), (False, True), (True, True)])
 def test_score_ragged_candidates_marshals_and_returns_what_was_asked(rows, per_broker):
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     res = s.score_ragged_candidates(TABLES, *RAGGED, -1, weight=[5, 6, 7], rows=rows, per_broker=per_broker)
     got = s._L.seen
     _check_ragged(got)
@@ -255,7 +234,7 @@ def test_score_ragged_candidates_marshals_and_returns_what_was_asked(rows, per_b
 
 
 def test_score_ragged_candidates_default_weight_and_stride():
-    s = fake_solver(_FakeLib())
+    s = util.fake_solver(_FakeLib())
     s.score_ragged_candidates(TABLES, *RAGGED, 4, out_stride=None)
     assert s._L.seen["weight"] is None and s._L.seen["S"] == 4
     s.score_ragged_candidates(TABLES, *RAGGED, -1, out_stride=2)
@@ -267,7 +246,7 @@ def test_score_ragged_candidates_default_weight_and_stride():
 def test_generate_assignment_stride(monkeypatch, current, desired_rf, S):
     monkeypatch.setattr(assigner, "java_string_hash", lambda s: 77)
     kta = object.__new__(kab.KafkaTopicAssigner)
-    kta._solver, kta._brokers_key = fake_solver(_FakeLib()), None
+    kta._solver, kta._brokers_key = util.fake_solver(_FakeLib()), None
     res = kta.generate_assignment("t", current, {3, 1, 2}, {}, desired_rf)
     got = kta._solver._L.seen
     assert kta._solver._L.brokers == [1, 2, 3]
@@ -287,7 +266,7 @@ _DEVICE_CALLS = [
 
 @pytest.mark.parametrize("name, args, passed, args0, passed0", _DEVICE_CALLS)
 def test_device_calls_sync_contract(name, args, passed, args0, passed0):
-    s = fake_solver(_FakeLib(code=4, rc=-2))
+    s = util.fake_solver(_FakeLib(code=4, rc=-2))
     st = getattr(s, name)(*args, stream=0x500)                              # sync: the status, never a raise
     assert s._L.seen == dict(args=passed + (0x500,), st=True) and st.code == 4
     with pytest.raises(kab.KassignError) as e:                              # async: rc raises, no status
@@ -298,7 +277,7 @@ def test_device_calls_sync_contract(name, args, passed, args0, passed0):
 
 
 def test_nonzero_rc_raises():
-    s = fake_solver(_FakeLib(rc=-1))
+    s = util.fake_solver(_FakeLib(rc=-1))
     with pytest.raises(kab.KassignError) as e:
         s.set_topic_base(3)
     assert e.value.code == -1

@@ -23,7 +23,7 @@ import pytest
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
-from tests.test_chain_variants import _histogram
+from tests import models, util
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PERSIST = None
@@ -434,10 +434,6 @@ def test_min_value_oracles_agree(oracle):
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------------
 
-def _fields(st):
-    return (st.code, st.topic_index, st.partition, st.a, st.b)
-
-
 def _check_plan(s, want, T, cid, warps=None):
     """The stage plan of s's last call is `want`; warps = make_plan's count where want names None."""
     got = s.last_stage_plan()
@@ -487,12 +483,12 @@ def _check_single(oracle, s, th, cur, ids, racks, desired, S, path="host", cid="
     s.reset()   # a fresh Context: the counters must come from this solve alone
     s.set_brokers(ids, racks)
     out, ln, st = _solve_dense(s, th, cur, desired, S, path)
-    assert _fields(st) == _fields(est), (cid, _fields(st), _fields(est))
+    assert util.fields(st) == util.fields(est), (cid, util.fields(st), util.fields(est))
     if est.code == 0:
         assert np.array_equal(out, exp), cid
         assert np.array_equal(ln, exp_len), cid
-        assert np.array_equal(s.counters(), _histogram(ids, exp, exp_len)), cid
-    return _fields(st)
+        assert np.array_equal(s.counters(), models.histogram(ids, exp, exp_len)), cid
+    return util.fields(st)
 
 
 @pytest.mark.gpu
@@ -539,7 +535,7 @@ def test_budget_edge(native_lib, oracle, edge):
         cl = kab.synth.make_cluster(T=2, P=p, RF=RF, N=N, R=R, seed=0xED6 + p, kind="structured")
         cur = _respace(cl.broker_id, cl.cur, lut)[1]
         st = _check_single(oracle, s, cl.topic_hash, cur, ids, racks, -1, RF, cid="edge P=%d" % p) if ok else \
-            _fields(s.solve_dense(cl.topic_hash, cur, -1, RF, check=False)[2])
+            util.fields(s.solve_dense(cl.topic_hash, cur, -1, RF, check=False)[2])
         if ok:
             assert st[0] == 0, st
             _check_plan(s, (1 if cap <= 255 else 2, int(cap > 1), 3 if RF <= 3 else 8, 0, 1, 2, 1 << lut, 1), 2, "edge")
@@ -586,9 +582,9 @@ def test_ragged_stage_variant(native_lib, oracle, case):
     s = kab.Solver(0)
     s.set_brokers(ids, racks)
     out, ln, st = s.solve_ragged(th, part_off, part_id, rep_off, cur, -1, S, check=False)
-    assert _fields(st) == est == (0, -1, -1, 0, 0), (_fields(st), est)
+    assert util.fields(st) == est == (0, -1, -1, 0, 0), (util.fields(st), est)
     assert np.array_equal(out, exp) and np.array_equal(ln, exp_len)
-    assert np.array_equal(s.counters(), _histogram(ids, exp, exp_len))
+    assert np.array_equal(s.counters(), models.histogram(ids, exp, exp_len))
     _check_plan(s, case["plan"], len(th), case["id"], _ragged_warps([(ids,)], part_off, rep_off, S))
 
 
@@ -599,12 +595,11 @@ def _lut_tables(ids, racks):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", CAND_CASES, ids=[c["id"] for c in CAND_CASES])
 def test_dense_candidates_stage_variant(native_lib, oracle, case):
-    from tests import test_candidates as tc
     g = case["gen"]
     cl, th, cur, ids, racks, desired, S = _dense(g, _seed(case["id"]))
     s = kab.Solver(0)
     tables = _lut_tables(ids, racks)
-    sts = tc._check_equal(tc.Problem(th, cur, desired, S), tables, oracle, solver=s)
+    sts = util.check_dense_equal(util.DenseProblem(th, cur, desired, S), tables, oracle, solver=s)
     assert all(st[0] == 0 for st in (sts[:1] if g.get("own_only") else sts)), sts
     rf = desired if desired >= 0 else g["RF"]
     _check_plan(s, case["plan"], g["T"], case["id"], _dense_warps(tables, g["P"], rf, S))
@@ -613,12 +608,11 @@ def test_dense_candidates_stage_variant(native_lib, oracle, case):
 @pytest.mark.gpu
 @pytest.mark.parametrize("case", RCAND_CASES, ids=[c["id"] for c in RCAND_CASES])
 def test_ragged_candidates_stage_variant(native_lib, oracle, case):
-    from tests import test_ragged_candidates as trc
     names, th, part_off, part_id, rep_off, cur, ids, racks, _, S = _ragged_problem(case)
     s = kab.Solver(0)
-    prob = trc.Problem(names, th, part_off, part_id, rep_off, cur, out_stride=S)
+    prob = util.Problem(names, th, part_off, part_id, rep_off, cur, out_stride=S)
     tables = _lut_tables(ids, racks)
-    sts = trc._check_equal(prob, tables, oracle, solver=s)
+    sts = util.check_equal(prob, tables, oracle, solver=s)
     assert all(st[0] == 0 for st in (sts[:1] if case["gen"].get("own_only") else sts)), sts
     _check_plan(s, case["plan"], len(th), case["id"], _ragged_warps(tables, part_off, rep_off, S))
 
@@ -627,7 +621,6 @@ def test_ragged_candidates_stage_variant(native_lib, oracle, case):
 def test_candidates_k128_persistent_topics(native_lib, oracle):
     """K = 128 (the limit) over 3 000 topics: a CTA or two per candidate, each warp looping over many topics. Tables in all
     three lookup modes, some without the cluster's brokers, and one too small for the RF."""
-    from tests import test_candidates as tc
     cl = kab.synth.make_cluster(T=3000, P=8, RF=3, N=60, R=6, seed=0x128, kind="mixed")
     rng = np.random.default_rng(128)
     tables = []
@@ -636,7 +629,7 @@ def test_candidates_k128_persistent_topics(native_lib, oracle):
         tables.append(_ext(cl.broker_id[keep], cl.rack_index[keep], k % 3))
     tables.append(_ext(cl.broker_id[:2], cl.rack_index[:2], 0))
     s = kab.Solver(0)
-    sts = tc._check_equal(tc.Problem(cl.topic_hash, cl.cur), tables, oracle, solver=s)
+    sts = util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), tables, oracle, solver=s)
     assert all(st[0] == 0 for st in sts[:127]), sts
     assert sts[127] == (_native.KA_ERR_RF_GT_BROKERS, 0, -1, 3, 0)
     assert _dense_warps(tables, cl.P, 3, 3) == K128_PLAN[4]
@@ -674,39 +667,37 @@ def test_min_value_ragged(native_lib, oracle):
         s.reset()
         s.set_brokers(cl.broker_id, cl.rack_index)
         out, ln, st = s.solve_ragged(th, part_off, part_id, rep_off, cur, -1, rf, check=False)
-        assert _fields(st) == est == (_expected_min_status(N, rf) or (0, -1, -1, 0, 0)), (N, rf, _fields(st), est)
+        assert util.fields(st) == est == (_expected_min_status(N, rf) or (0, -1, -1, 0, 0)), (N, rf, util.fields(st), est)
         if est[0] == 0:
             assert np.array_equal(out, exp) and np.array_equal(ln, exp_len), (N, rf)
-            assert np.array_equal(s.counters(), _histogram(cl.broker_id, exp, exp_len)), (N, rf)
+            assert np.array_equal(s.counters(), models.histogram(cl.broker_id, exp, exp_len)), (N, rf)
 
 
 @pytest.mark.gpu
 def test_min_value_candidates(native_lib, oracle):
     """Batched: tables on which the MIN_VALUE topic solves (N divides 2^31, rows of 2), fails early (N does not) and fails late
     (rows of 3), in the dense and the ragged batch."""
-    from tests import test_candidates as tc
-    from tests import test_ragged_candidates as trc
     names = _min_names(3)
     for rf, sizes in ((2, (2, 4, 16, 1024, 3, 6, 12)), (3, (4, 16, 1024, 3, 6, 12, 2))):
         cl = _min_cluster(1024, rf, names[rf - 1], P=12)
         # every broker in a rack of its own: a table of n >= rf brokers never leaves a partition unassignable
-        tables = [tc._table(np.sort(np.random.default_rng(n).choice(cl.broker_id, n, replace=False))) for n in sizes]
+        tables = [util.table(np.sort(np.random.default_rng(n).choice(cl.broker_id, n, replace=False))) for n in sizes]
         s = kab.Solver(0)
-        sts = tc._check_equal(tc.Problem(cl.topic_hash, cl.cur), tables, oracle, solver=s)
+        sts = util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), tables, oracle, solver=s)
         seen = set()
         for (ids, racks), st in zip(tables, sts):
             n = len(ids)
             _, _, est = oracle.fast_run_dense(oracle.FastContext(), cl.topic_hash, cl.cur, ids, racks)
-            assert st == _fields(est), (rf, n, st, _fields(est))
+            assert st == util.fields(est), (rf, n, st, util.fields(est))
             if st[0] in (0, _native.KA_ERR_HASH_INDEX):
                 assert st == (_expected_min_status(n, rf) or (0, -1, -1, 0, 0)), (rf, n, st)
                 seen.add("solve" if st[0] == 0 else ("early" if 2**31 % n else "late"))
         assert seen == ({"solve", "early"} if rf == 2 else {"early", "late"}), (rf, seen)
         assert s.last_stage_plan()[3] == len(tables)
         part_off, part_id, rep_off, cur = cl.ragged()
-        prob = trc.Problem(cl.topic_names, np.array([kab.java_string_hash(x) for x in cl.topic_names], dtype=np.int32), part_off,
-                           part_id, rep_off, cur)
-        assert trc._check_equal(prob, tables, oracle) == sts
+        prob = util.Problem(cl.topic_names, np.array([kab.java_string_hash(x) for x in cl.topic_names], dtype=np.int32), part_off,
+                            part_id, rep_off, cur)
+        assert util.check_equal(prob, tables, oracle) == sts
 
 
 # ---- the dense capacity bound counts only tables that can serve the target RF ----------------------------------------------
@@ -720,12 +711,11 @@ def _ab_problem():
 def test_small_table_does_not_change_the_dense_batch_plan(native_lib, oracle):
     """Table A (52 000 brokers, capacity 1) and table B (2 brokers, RF 3): B fails alone with KA_ERR_RF_GT_BROKERS, and A
     solves under A's own plan (no levels, 1-byte loads) instead of the level scratch B's bound would ask for."""
-    from tests import test_candidates as tc
     cl = _ab_problem()
-    A = tc._table(1000 + np.arange(52000, dtype=np.int32), 500)
-    B = tc._table(cl.broker_id[:2], 1)
+    A = util.table(1000 + np.arange(52000, dtype=np.int32), 500)
+    B = util.table(cl.broker_id[:2], 1)
     s = kab.Solver(0)
-    sts = tc._check_equal(tc.Problem(cl.topic_hash, cl.cur), [A, B], oracle, solver=s)
+    sts = util.check_dense_equal(util.DenseProblem(cl.topic_hash, cl.cur), [A, B], oracle, solver=s)
     assert sts == [(0, -1, -1, 0, 0), (_native.KA_ERR_RF_GT_BROKERS, 0, -1, 3, 0)], sts
     _check_plan(s, AB_PLAN, cl.T, "A+B")
     assert s.last_order_plan()[1] == 0
@@ -735,21 +725,19 @@ def test_small_table_does_not_change_the_dense_batch_plan(native_lib, oracle):
 def test_dense_and_ragged_batches_agree_with_a_small_table(native_lib, oracle):
     """The same cluster and tables through the dense and the ragged candidate solves: identical statuses and rows. Table A
     has 20 000 brokers (global id LUT), which fits the ragged layout's level scratch but not levels with 2-byte loads."""
-    from tests import test_candidates as tc
-    from tests import test_ragged_candidates as trc
     cl = _ab_problem()
-    A = tc._table(1000 + 2 * np.arange(20000, dtype=np.int32), 500)
-    B = tc._table(cl.broker_id[:2], 1)
+    A = util.table(1000 + 2 * np.arange(20000, dtype=np.int32), 500)
+    B = util.table(cl.broker_id[:2], 1)
     s = kab.Solver(0)
-    dprob = tc.Problem(cl.topic_hash, cl.cur)
+    dprob = util.DenseProblem(cl.topic_hash, cl.cur)
     d_out, d_len, d_sts = dprob.batched([A, B], s)
     part_off, part_id, rep_off, cur = cl.ragged()
-    rprob = trc.Problem(cl.topic_names, cl.topic_hash, part_off, part_id, rep_off, cur)
+    rprob = util.Problem(cl.topic_names, cl.topic_hash, part_off, part_id, rep_off, cur)
     r_out, r_len, r_sts = rprob.batched([A, B])
     assert d_sts == r_sts == [(0, -1, -1, 0, 0), (_native.KA_ERR_RF_GT_BROKERS, 0, -1, 3, 0)], (d_sts, r_sts)
     assert np.array_equal(d_out[0].reshape(-1, 3), r_out[0]) and np.array_equal(d_len[0].reshape(-1), r_len[0])
-    assert trc._check_equal(rprob, [A, B], oracle) == r_sts
-    assert tc._check_equal(dprob, [A, B], oracle) == d_sts
+    assert util.check_equal(rprob, [A, B], oracle) == r_sts
+    assert util.check_dense_equal(dprob, [A, B], oracle) == d_sts
     _check_plan(s, AB20K_PLAN, cl.T, "A20k+B")
 
 
@@ -763,6 +751,6 @@ def test_rf_above_a_one_broker_table_is_the_reference_error(native_lib, oracle):
     _, _, est = oracle.fast_run_dense(oracle.FastContext(), th, cur, ids, racks)
     s = kab.Solver(0)
     s.set_brokers(ids, racks)
-    st = _fields(s.solve_dense(th, cur, check=False)[2])
+    st = util.fields(s.solve_dense(th, cur, check=False)[2])
     assert st == (est.code, est.topic_index, est.partition, est.a, est.b) == (_native.KA_ERR_RF_GT_BROKERS, 0, -1, 2, 0), st
     _check_plan(s, P33000_PLAN, 1, "P33000")

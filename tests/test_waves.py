@@ -1,5 +1,5 @@
-"""ka_plan_waves: a reassignment cut into waves in which no broker receives more than a budget. `reference_waves` restates the rule
-of include/kassign.h as a plain loop; every wave, summary and W of the device must equal it. The CPU tests pin the model on
+"""ka_plan_waves: a reassignment cut into waves in which no broker receives more than a budget. `models.plan_waves` restates the
+rule of include/kassign.h as a plain loop; every wave, summary and W of the device must equal it. The CPU tests pin the model on
 hand-worked cases and its invariants on random inputs, and what Solver.plan_waves hands the C ABI."""
 import ctypes
 import os
@@ -11,87 +11,17 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE
-from tests.test_candidate_scores import reference_summary
-from tests.test_clusters import _bsearch_table, _table
-from tests.test_solver_abi import fake_solver, view
+from tests import models, util
 
 FIELDS = WAVE_SUMMARY_DTYPE.names
 INT64_MAX = np.iinfo(np.int64).max
 BAD, LIMIT = _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT
 
 
-def reference_waves(rep_off, cur, out, out_len, ids, B, weight=None):
-    """(wave [Q] int32, [summary dict per wave], (code, a, b)) of the rule, rows in input order. A new list naming a broker twice,
-    or a receiver missing from the table `ids`, fails at its lowest row: (KA_ERR_BAD_ARG, row, broker id), and no plan."""
-    Q = len(out_len)
-    table = set(int(x) for x in ids)
-    opened, load = {}, {}
-    inb = {}                                        # (wave, broker id) -> incoming weight
-    wave = np.zeros(Q, dtype=np.int32)
-    recv_of = {}
-    for g in range(Q):
-        new = [int(x) for x in out[g][:int(out_len[g])]]
-        old = [int(x) for x in cur[int(rep_off[g]):int(rep_off[g + 1])]]
-        recv = []
-        for j, b in enumerate(new):
-            if b in new[:j] or (b not in old and b not in table):
-                return None, None, (BAD, g, b)
-            if b not in old:
-                recv.append(b)
-        if new == old:
-            continue
-        if not recv:
-            wave[g] = 1
-            continue
-        w = 1 if weight is None else int(weight[g])
-        v = max(opened.get(b, 1) if load.get(b, 0) == 0 or load.get(b, 0) + w <= B else opened.get(b, 1) + 1 for b in recv)
-        for b in recv:
-            if v > opened.get(b, 1):
-                opened[b], load[b] = v, w
-            else:
-                load[b] = load.get(b, 0) + w
-            inb[(v, b)] = inb.get((v, b), 0) + w
-        wave[g] = v
-        recv_of[g] = (len(recv), w)
-    W = int(wave.max()) if Q else 0
-    summ = [dict(rows=0, rows_moved=0, replicas_added=0, max_broker_in=0, max_broker_in_id=-1) for _ in range(W)]
-    for g in np.nonzero(wave)[0]:
-        s = summ[wave[g] - 1]
-        s["rows"] += 1
-        if g in recv_of:
-            n, w = recv_of[g]
-            s["rows_moved"] += 1
-            s["replicas_added"] += n * w
-    for (v, b), x in sorted(inb.items()):
-        s = summ[v - 1]
-        if x > s["max_broker_in"]:
-            s["max_broker_in"], s["max_broker_in_id"] = x, b
-    return wave, summ, (0, 0, 0)
-
-
-def _rec(s):
-    return {f: int(s[f]) for f in FIELDS}
-
-
-def _rows(lists, stride=None):
-    """(out [Q, stride], out_len [Q]) from a list of new lists; unused slots -1."""
-    stride = stride or max([len(x) for x in lists] + [1])
-    out = np.full((len(lists), stride), -1, dtype=np.int32)
-    for g, x in enumerate(lists):
-        out[g, :len(x)] = x
-    return out, np.array([len(x) for x in lists], dtype=np.int32)
-
-
-def _cur(lists):
-    rep_off = np.zeros(len(lists) + 1, dtype=np.int64)
-    np.cumsum([len(x) for x in lists], out=rep_off[1:])
-    return rep_off, np.array([b for x in lists for b in x], dtype=np.int32)
-
-
 def _model(cur_lists, new_lists, B, weight=None, ids=range(1, 100)):
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists)
-    return reference_waves(rep_off, cur, out, out_len, np.asarray(list(ids)), B, weight)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists)
+    return models.plan_waves(rep_off, cur, out, out_len, np.asarray(list(ids)), B, weight)
 
 
 # ---- CPU -----------------------------------------------------------------------------------------------------------------
@@ -116,35 +46,12 @@ def test_without_a_context_is_no_device(native_lib):
     assert L.ka_plan_waves(None, 0, None, None, 1, None, None, None, 1, None, ctypes.byref(n), None, 0, None) == BAD
 
 
-class _FakeLib:
-    """Stands in for libkassign.so: records what ka_plan_waves is handed, plans W waves (wave[g] = 1 + g % W) and writes
-    recognisable summaries, at most summary_cap of them."""
-
-    def __init__(self, W):
-        self.W, self.calls = W, []
-
-    def ka_plan_waves(self, h, Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave, n_waves, summary, cap, st):
-        r_off = view(rep_off, Q + 1, np.int64)
-        self.calls.append(dict(Q=Q, stride=stride, rep_off=r_off, cur=view(cur, int(r_off[-1]), np.int32),
-                               new_len=view(new_len, Q, np.int32), new_broker=view(new_broker, Q * stride, np.int32),
-                               weight=view(weight, Q, np.int64), B=B, cap=cap, wave=wave is not None))
-        if wave is not None and Q:
-            np.ctypeslib.as_array(ctypes.cast(wave, ctypes.POINTER(ctypes.c_int32)), shape=(Q,))[:] = 1 + np.arange(Q) % self.W
-        if cap:
-            s = np.ctypeslib.as_array(ctypes.cast(summary, ctypes.POINTER(ctypes.c_int64)), shape=(cap * 5,)).reshape(cap, 5)
-            n = min(cap, self.W)
-            s[:n] = np.arange(n)[:, None] * 10 + np.arange(5)
-        n_waves._obj.value = self.W
-        st._obj.code = 0
-        return 0
-
-
 @pytest.mark.parametrize("W", [3, 100])
 def test_plan_waves_marshals_its_arguments(W):
-    lib = _FakeLib(W)
-    s = fake_solver(lib)
-    out, out_len = _rows([[1, 2], [3], [4, 5, 6], []])
-    rep_off, cur = _cur([[1], [2, 3], [4], [7, 8]])
+    lib = util.FakeWaveLib(W)
+    s = util.fake_solver(lib)
+    out, out_len = util.rows([[1, 2], [3], [4, 5, 6], []])
+    rep_off, cur = util.cur_lists([[1], [2, 3], [4], [7, 8]])
     weight = np.array([5, 0, 7, 1], dtype=np.int64)
     wave, summ, st = s.plan_waves(rep_off.astype(np.int32), cur.astype(np.int64), out, out_len, 9, weight=weight)
     assert st.code == 0
@@ -194,19 +101,6 @@ def test_model_hand_worked_weights():
     assert _model([[200]], [[200]], 1)[2] == (0, 0, 0)   # a kept broker need not be in the table
 
 
-def _random_case(rng, Q, N, stride=3):
-    cur_lists, new_lists = [], []
-    for _ in range(Q):
-        m = int(rng.integers(0, stride + 1))
-        cur_lists.append([int(x) for x in rng.choice(np.arange(1, N + 1), m, replace=False)])
-        if rng.random() < 0.3:
-            new_lists.append(list(cur_lists[-1]))
-        else:
-            n = int(rng.integers(0, stride + 1))
-            new_lists.append([int(x) for x in rng.choice(np.arange(1, N + 1), n, replace=False)])
-    return cur_lists, new_lists
-
-
 def check_invariants(cur_lists, new_lists, wave, summ, B, weight, ids):
     """The budget rule, contiguous non-empty waves, and the per-wave replicas_added summing to ka_move_summary's."""
     W = len(summ)
@@ -221,9 +115,9 @@ def check_invariants(cur_lists, new_lists, wave, summ, B, weight, ids):
                 inb.setdefault((int(wave[g]), b), []).append(int(w[g]))
     for ws in inb.values():   # beyond B only through one heavier row, with nothing else but zero weights
         assert sum(ws) <= B or sum(x > 0 for x in ws) == 1, ws
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
-    e = reference_summary(out, out_len, rep_off, cur, np.asarray(ids, dtype=np.int64), weight)[0]
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
+    e = models.move_summary(out, out_len, rep_off, cur, np.asarray(ids, dtype=np.int64), weight)[0]
     assert sum(s["replicas_added"] for s in summ) == e["replicas_added"]
     if w.sum() <= B:
         assert W <= 1
@@ -233,7 +127,7 @@ def check_invariants(cur_lists, new_lists, wave, summ, B, weight, ids):
 def test_model_invariants(seed):
     rng = np.random.default_rng(seed)
     ids = np.arange(1, 13)
-    cur_lists, new_lists = _random_case(rng, 300, 12)
+    cur_lists, new_lists = util.random_wave_case(rng, 300, 12)
     for B, weight in ((1, None), (4, None), (10 ** 6, None), (50, rng.integers(0, 40, 300)), (30, rng.integers(0, 80, 300))):
         wave, summ, st = _model(cur_lists, new_lists, B, weight, ids)
         assert st == (0, 0, 0)
@@ -246,29 +140,19 @@ def _check(s, rep_off, cur, out, out_len, B, weight=None, ids=None):
     """plan_waves against the model, every field. Returns (wave, summary, status)."""
     ids = s.broker_id if ids is None else ids
     wave, summ, st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight)
-    e_wave, e_summ, e_st = reference_waves(rep_off, cur, out, out_len, ids, B, weight)
+    e_wave, e_summ, e_st = models.plan_waves(rep_off, cur, out, out_len, ids, B, weight)
     assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
     if st.code == 0:
         assert np.array_equal(wave, e_wave), np.nonzero(wave != e_wave)[0][:10]
-        assert [_rec(x) for x in summ] == e_summ
+        assert [util.record_of(x, FIELDS) for x in summ] == e_summ
     return wave, summ, st
-
-
-def _solved(cl, desired_rf=-1):
-    """A fresh Solver on the cluster's table and the rows ka_solve gives for it."""
-    s = kab.Solver(0)
-    s.set_brokers(cl.broker_id, cl.rack_index)
-    S = max(int(np.diff(cl.rep_off).max()), desired_rf, 1)
-    out, out_len, st = s.solve_ragged(cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off, cl.cur, desired_rf, S)
-    assert st.code == 0
-    return s, out, out_len, S
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("remove", [0.0, 0.02, 0.2])
 def test_solve_rows(native_lib, remove):
     cl = kab.synth.make_ragged_cluster(T=4000, N=400, max_partitions=128, seed=7, remove_frac=remove)
-    s, out, out_len, S = _solved(cl)
+    s, out, out_len, S = util.solved(cl)
     rng = np.random.default_rng(3)
     Q = len(out_len)
     weight = rng.integers(0, 1 << 30, Q).astype(np.int64)
@@ -290,7 +174,7 @@ def test_solve_rows(native_lib, remove):
 def test_growing_rf_rows_of_4_to_8(native_lib):
     for drf, shape in ((5, dict(N=60, seed=16)), (8, dict(N=200, seed=19, max_partitions=64))):   # no racks: RF 8 is assignable
         cl = kab.synth.make_ragged_cluster(T=600, R=6, rack_frac=0.0, desired_rf=drf, **shape)
-        s, out, out_len, S = _solved(cl, drf)
+        s, out, out_len, S = util.solved(cl, drf)
         assert S == drf and out_len.max() == drf
         for B in (1, 7, 1000):
             _check(s, cl.rep_off, cl.cur, out, out_len, B)
@@ -300,11 +184,11 @@ def test_growing_rf_rows_of_4_to_8(native_lib):
 @pytest.mark.gpu
 def test_hand_built_rows(native_lib):
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 41), 4))
+    s.set_brokers(*util.table(np.arange(1, 41), 4))
 
     def run(cur_lists, new_lists, B, weight=None, stride=None):
-        rep_off, cur = _cur(cur_lists)
-        out, out_len = _rows(new_lists, stride)
+        rep_off, cur = util.cur_lists(cur_lists)
+        out, out_len = util.rows(new_lists, stride)
         return _check(s, rep_off, cur, out, out_len, B, None if weight is None else np.asarray(weight, dtype=np.int64))
 
     assert run([[1, 2], [3, 4]], [[2, 1], [4, 3]], 1)[0].tolist() == [1, 1]                   # reorder only
@@ -320,7 +204,7 @@ def test_hand_built_rows(native_lib):
     run([[]] * 3000, eight, 1)
     run([[]] * 3000, eight, 5, np.arange(3000) % 4)
     rng = np.random.default_rng(2)
-    cur_lists, new_lists = _random_case(rng, 20000, 40, 8)
+    cur_lists, new_lists = util.random_wave_case(rng, 20000, 40, 8)
     for B in (1, 2, 9):
         run(cur_lists, new_lists, B, stride=8)
         run(cur_lists, new_lists, B * 10, rng.integers(0, 30, 20000), stride=8)
@@ -331,11 +215,11 @@ def test_hand_built_rows(native_lib):
 def test_lookup_modes_and_chain_state(native_lib, table):
     N = dict(smem_lut=50, global_lut=50, bsearch=50, state_in_smem=12800, state_in_global=12801)[table]
     if table == "global_lut":
-        ids, racks = _table(1 + 700 * np.arange(N), 5)
+        ids, racks = util.table(1 + 700 * np.arange(N), 5)
     elif table == "bsearch":
-        ids, racks = _bsearch_table(N)
+        ids, racks = util.bsearch_table(N)
     else:
-        ids, racks = _table(np.arange(1, N + 1), 8)
+        ids, racks = util.table(np.arange(1, N + 1), 8)
     s = kab.Solver(0)
     s.set_brokers(ids, racks)
     rng = np.random.default_rng(N)
@@ -343,8 +227,8 @@ def test_lookup_modes_and_chain_state(native_lib, table):
     cur_lists = [[int(x) for x in rng.choice(ids, int(rng.integers(0, 4)), replace=False)] for _ in range(Q)]
     hot = ids[-5:]   # receivers crowd on a few brokers (the chain's conflicts)
     new_lists = [[int(x) for x in rng.choice(hot if g % 3 == 0 else ids, int(rng.integers(1, 4)), replace=False)] for g in range(Q)]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     for B, w in ((1, None), (16, None), (500, rng.integers(0, 100, Q).astype(np.int64))):
         _check(s, rep_off, cur, out, out_len, B, w)
 
@@ -361,11 +245,11 @@ def _raw(s, Q, rep_off, cur, stride, new_len, new, weight, B, wave, summary, cap
 @pytest.mark.gpu
 def test_errors(native_lib):
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 21), 4))
+    s.set_brokers(*util.table(np.arange(1, 21), 4))
     rng = np.random.default_rng(4)
-    cur_lists, new_lists = _random_case(rng, 1000, 20)
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    cur_lists, new_lists = util.random_wave_case(rng, 1000, 20)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     wave, summ = np.zeros(1000, dtype=np.int32), np.zeros(8, dtype=WAVE_SUMMARY_DTYPE)
     ok = (s, 1000, rep_off, cur, 3, out_len, out, None, 2, wave, summ, 8)
 
@@ -408,18 +292,18 @@ def test_errors(native_lib):
             o[g, :len(x)] = x
             ln[g] = len(x)
         assert call(new=o, new_len=ln) == expect
-        e = reference_waves(rep_off, cur, o, ln, s.broker_id, 2)[2]
+        e = models.plan_waves(rep_off, cur, o, ln, s.broker_id, 2)[2]
         assert e == expect
     # Q == 0 and a cap below W
     assert call(Q=0)[0] == 0
     n = ctypes.c_int32(0)
     _check(s, rep_off, cur, out, out_len, 1)
-    e_wave, e_summ, _ = reference_waves(rep_off, cur, out, out_len, s.broker_id, 1)
+    e_wave, e_summ, _ = models.plan_waves(rep_off, cur, out, out_len, s.broker_id, 1)
     W = len(e_summ)
     assert W > 3
     few = np.zeros(3, dtype=WAVE_SUMMARY_DTYPE)
     rc, _, n = _raw(s, 1000, rep_off, cur, 3, out_len, out, None, 1, wave, few, 3)
-    assert rc == 0 and n.value == W and [_rec(x) for x in few] == e_summ[:3] and np.array_equal(wave, e_wave)
+    assert rc == 0 and n.value == W and [util.record_of(x, FIELDS) for x in few] == e_summ[:3] and np.array_equal(wave, e_wave)
     rc, _, n = _raw(s, 1000, rep_off, cur, 3, out_len, out, None, 1, None, None, 0)
     assert rc == 0 and n.value == W
 
@@ -446,7 +330,7 @@ def test_context_is_untouched_and_launches_are_fixed(native_lib):
     assert np.array_equal(again, ref_out) and np.array_equal(again_len, ref_len)
     # the same launches at another size
     big = kab.synth.make_ragged_cluster(T=40000, N=400, max_partitions=128, seed=22, remove_frac=0.2)
-    s2, bout, blen, _ = _solved(big)
+    s2, bout, blen, _ = util.solved(big)
     m0 = s2.launch_count()   # one C call each: Solver.plan_waves makes a second one for a plan of many waves
     rc, _, n = _raw(s2, len(blen), big.rep_off, big.cur, 3, blen, bout, None, 1, np.zeros(len(blen), dtype=np.int32), None, 0)
     assert rc == 0 and n.value > 64 and s2.launch_count() - m0 == n1 - n0

@@ -1,5 +1,5 @@
-"""ka_plan_waves_json: one reassignment document per wave of a wave plan, built on the device. `reference_wave_docs` prints the
-waves of `reference_waves` (tests/test_waves.py) record by record in the key order of the device emitter; every document, wave,
+"""ka_plan_waves_json: one reassignment document per wave of a wave plan, built on the device. `models.wave_docs` prints the
+waves of `models.plan_waves` record by record in the key order of the device emitter; every document, wave,
 summary and W of the device must equal it byte for byte. The CPU tests pin the model and what Solver.plan_waves_json hands the
 C ABI."""
 import ctypes
@@ -13,33 +13,10 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE
-from tests.test_clusters import _bsearch_table, _table
-from tests.test_solver_abi import fake_solver, view
-from tests.test_waves import _cur, _rec, _rows, _solved, reference_waves
+from tests import models, util
 
 BAD, LIMIT = _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT
 INT64_MAX = np.iinfo(np.int64).max
-
-
-def reference_wave_docs(topic_names, part_off, part_id, rep_off, cur, out, out_len, ids, B, weight=None):
-    """(docs [bytes per wave], wave, summary, (code, a, b)): the waves of reference_waves, each printed as the device prints it:
-    the records of its rows in input row order, keys "partition", "replicas", "topic"."""
-    wave, summ, st = reference_waves(rep_off, cur, out, out_len, ids, B, weight)
-    if st[0] != 0:
-        return None, wave, summ, st
-    recs = [[] for _ in summ]
-    for t, name in enumerate(topic_names):
-        for g in range(int(part_off[t]), int(part_off[t + 1])):
-            if wave[g]:
-                p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
-                recs[wave[g] - 1].append('{"partition":%d,"replicas":[%s],"topic":"%s"}'
-                                         % (p, ",".join(str(int(b)) for b in out[g][:int(out_len[g])]), name))
-    return [('{"partitions":[' + ",".join(r) + '],"version":1}').encode() for r in recs], wave, summ, st
-
-
-def bound(topic_names, part_off, stride):
-    """The sufficient json_cap of include/kassign.h."""
-    return sum(int(part_off[t + 1] - part_off[t]) * (79 + 12 * stride + len(n.encode())) for t, n in enumerate(topic_names))
 
 
 def _one_topic(Q, name="t"):
@@ -67,45 +44,11 @@ def test_without_a_context_is_no_device(native_lib):
     assert L.ka_plan_waves_json(*args, None) == BAD
 
 
-class _FakeLib:
-    """Stands in for libkassign.so: records what ka_plan_waves_json is handed, plans W waves (wave[g] = 1 + g % W), and writes
-    document v as b"<v>" and recognisable summaries."""
-
-    def __init__(self, W):
-        self.W, self.calls = W, []
-
-    def ka_plan_waves_json(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, names, name_off,
-                           js, json_cap, doc_off, wave, n_waves, summary, cap, st):
-        p_off = view(part_off, T + 1, np.int64)
-        Q = int(p_off[-1])
-        r_off = view(rep_off, Q + 1, np.int64)
-        n_off = view(name_off, T + 1, np.int64)
-        self.calls.append(dict(T=T, part_off=p_off, part_id=view(part_id, Q, np.int32), stride=stride, rep_off=r_off,
-                               cur=view(cur, int(r_off[-1]), np.int32), new_len=view(new_len, Q, np.int32),
-                               new_broker=view(new_broker, Q * stride, np.int32), weight=view(weight, Q, np.int64), B=B,
-                               names=bytes(view(names, int(n_off[-1]), np.uint8)), name_off=n_off, json_cap=json_cap, cap=cap))
-        np.ctypeslib.as_array(ctypes.cast(wave, ctypes.POINTER(ctypes.c_int32)), shape=(Q,))[:] = 1 + np.arange(Q) % self.W
-        s = np.ctypeslib.as_array(ctypes.cast(summary, ctypes.POINTER(ctypes.c_int64)), shape=(cap * 5,)).reshape(cap, 5)
-        s[:self.W] = np.arange(self.W)[:, None] * 10 + np.arange(5)
-        text = np.ctypeslib.as_array(ctypes.cast(js, ctypes.POINTER(ctypes.c_uint8)), shape=(json_cap,))
-        off = np.ctypeslib.as_array(ctypes.cast(doc_off, ctypes.POINTER(ctypes.c_int64)), shape=(Q + 1,))
-        at = 0
-        for v in range(self.W):
-            doc = b"<%d>" % v
-            off[v] = at
-            text[at:at + len(doc)] = np.frombuffer(doc, dtype=np.uint8)
-            at += len(doc)
-        off[self.W] = at
-        n_waves._obj.value = self.W
-        st._obj.code = 0
-        return 0
-
-
 def test_plan_waves_json_marshals_its_arguments():
-    lib = _FakeLib(3)
-    s = fake_solver(lib)
-    out, out_len = _rows([[1, 2], [3], [4, 5, 6], []])
-    rep_off, cur = _cur([[1], [2, 3], [4], [7, 8]])
+    lib = util.FakeWaveLib(3)
+    s = util.fake_solver(lib)
+    out, out_len = util.rows([[1, 2], [3], [4, 5, 6], []])
+    rep_off, cur = util.cur_lists([[1], [2, 3], [4], [7, 8]])
     weight = np.array([5, 0, 7, 1], dtype=np.int64)
     names = ["alpha", "", "bc"]
     part_off, part_id = [0, 3, 3, 4], [4, 9, -2, 0]
@@ -119,7 +62,7 @@ def test_plan_waves_json_marshals_its_arguments():
     assert np.array_equal(c["new_len"], out_len) and np.array_equal(c["new_broker"], out.ravel())
     assert np.array_equal(c["weight"], weight)
     assert c["names"] == b"alphabc" and c["name_off"].tolist() == [0, 5, 5, 7]
-    assert c["json_cap"] == bound(names, part_off, 3) == 3 * (79 + 36 + 5) + (79 + 36 + 2)
+    assert c["json_cap"] == models.json_bound(names, part_off, 3) == 3 * (79 + 36 + 5) + (79 + 36 + 2)
     assert [bytes(d) for d in docs] == [b"<0>", b"<1>", b"<2>"]
     assert wave.tolist() == [1, 2, 3, 1] and [list(x) for x in summ] == [[v * 10 + f for f in range(5)] for v in range(3)]
     buf = np.zeros(50, dtype=np.uint8)
@@ -131,10 +74,10 @@ def test_plan_waves_json_marshals_its_arguments():
 def test_model_hand_worked():
     cur = [[1, 2], [1, 2], [1], [2], [1, 2], [1, 2], [5], [1], [2]]
     new = [[1, 3], [3, 4], [3], [4], [2, 1], [1, 2], [4, 5], [3, 4], [3]]
-    rep_off, cur_flat = _cur(cur)
-    out, out_len = _rows(new)
-    docs, wave, summ, st = reference_wave_docs(["a", "empty", "b.c"], [0, 4, 4, 9], [0, 1, 5, 7, 2, 3, 4, -6, 8], rep_off, cur_flat, out,
-                                               out_len, np.arange(1, 100), 2)
+    rep_off, cur_flat = util.cur_lists(cur)
+    out, out_len = util.rows(new)
+    docs, wave, summ, st = models.wave_docs(["a", "empty", "b.c"], [0, 4, 4, 9], [0, 1, 5, 7, 2, 3, 4, -6, 8], rep_off, cur_flat, out,
+                                            out_len, np.arange(1, 100), 2)
     assert st == (0, 0, 0) and wave.tolist() == [1, 1, 2, 1, 1, 0, 2, 2, 3]
     assert docs == [
         b'{"partitions":[{"partition":0,"replicas":[1,3],"topic":"a"},{"partition":1,"replicas":[3,4],"topic":"a"},'
@@ -143,11 +86,11 @@ def test_model_hand_worked():
         b'{"partition":-6,"replicas":[3,4],"topic":"b.c"}],"version":1}',
         b'{"partitions":[{"partition":8,"replicas":[3],"topic":"b.c"}],"version":1}']
     # ordinals without part_id; nothing changed gives no document; a refused plan none either
-    docs, _, _, _ = reference_wave_docs(["a", "b"], [0, 1, 3], None, *_cur([[1], [1], [1]]), *_rows([[2], [1], [2]]), [1, 2], 1)
+    docs, _, _, _ = models.wave_docs(["a", "b"], [0, 1, 3], None, *util.cur_lists([[1], [1], [1]]), *util.rows([[2], [1], [2]]), [1, 2], 1)
     assert docs == [b'{"partitions":[{"partition":0,"replicas":[2],"topic":"a"}],"version":1}',
                     b'{"partitions":[{"partition":1,"replicas":[2],"topic":"b"}],"version":1}']
-    assert reference_wave_docs(["a"], [0, 1], None, *_cur([[1]]), *_rows([[1]]), [1], 1)[0] == []
-    assert reference_wave_docs(["a"], [0, 1], None, *_cur([[1]]), *_rows([[2, 2]]), [1, 2], 1)[::3] == (None, (BAD, 0, 2))
+    assert models.wave_docs(["a"], [0, 1], None, *util.cur_lists([[1]]), *util.rows([[1]]), [1], 1)[0] == []
+    assert models.wave_docs(["a"], [0, 1], None, *util.cur_lists([[1]]), *util.rows([[2, 2]]), [1, 2], 1)[::3] == (None, (BAD, 0, 2))
 
 
 @pytest.mark.parametrize("seed", range(4))
@@ -163,11 +106,11 @@ def test_model_invariants(seed):
     cur_lists = [[int(x) for x in rng.choice(np.arange(1, 13), int(rng.integers(0, 4)), replace=False)] for _ in range(Q)]
     new_lists = [c if rng.random() < 0.3 else [int(x) for x in rng.choice(np.arange(1, 13), int(rng.integers(0, 4)), replace=False)]
                  for c in cur_lists]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     topic_of = np.repeat(np.arange(T), sizes)
     for B, weight in ((1, None), (3, None), (40, rng.integers(0, 30, Q))):
-        docs, wave, summ, st = reference_wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, np.arange(1, 13), B, weight)
+        docs, wave, summ, st = models.wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, np.arange(1, 13), B, weight)
         assert st == (0, 0, 0) and len(docs) == len(summ)
         seen = []
         for v, doc in enumerate(docs):
@@ -176,7 +119,7 @@ def test_model_invariants(seed):
             seen += [(r["topic"], r["partition"], tuple(r["replicas"])) for r in parsed["partitions"]]
         want = [(names[topic_of[g]], int(part_id[g]), tuple(new_lists[g])) for g in range(Q) if new_lists[g] != cur_lists[g]]
         assert sorted(seen) == sorted(want) and len(set(seen)) == len(seen)
-        assert sum(len(d) for d in docs) <= bound(names, part_off, 3)
+        assert sum(len(d) for d in docs) <= models.json_bound(names, part_off, 3)
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------------
@@ -184,13 +127,13 @@ def test_model_invariants(seed):
 def _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, weight=None, json_buf=None):
     """plan_waves_json against the model and against plan_waves on the same inputs. Returns (docs, wave, summary, status)."""
     docs, wave, summ, st = s.plan_waves_json(names, part_off, part_id, rep_off, cur, out, out_len, B, weight=weight, json_buf=json_buf)
-    e_docs, e_wave, e_summ, e_st = reference_wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, weight)
+    e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, weight)
     assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
     p_wave, p_summ, p_st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight)
     assert (p_st.code, p_st.a, p_st.b) == e_st
     if st.code == 0:
         assert np.array_equal(wave, e_wave) and np.array_equal(wave, p_wave)
-        assert [_rec(x) for x in summ] == e_summ and np.array_equal(summ, p_summ)
+        assert [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in summ] == e_summ and np.array_equal(summ, p_summ)
         assert len(docs) == len(e_docs)
         for v, (d, e) in enumerate(zip(docs, e_docs)):
             assert bytes(d) == e, (v, bytes(d)[:200], e[:200])
@@ -201,7 +144,7 @@ def _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, weight=No
 @pytest.mark.parametrize("remove", [0.0, 0.02, 0.2])
 def test_solve_rows(native_lib, remove):
     cl = kab.synth.make_ragged_cluster(T=4000, N=400, max_partitions=128, seed=7, remove_frac=remove)
-    s, out, out_len, S = _solved(cl)
+    s, out, out_len, S = util.solved(cl)
     Q = len(out_len)
     weight = np.random.default_rng(3).integers(0, 1 << 20, Q).astype(np.int64)
     sparse = (cl.part_id.astype(np.int64) * 7 - 50).astype(np.int32)   # sparse and negative ids
@@ -217,7 +160,7 @@ def test_solve_rows(native_lib, remove):
 def test_growing_rf_rows_of_4_to_8(native_lib):
     for drf, shape in ((5, dict(N=60, seed=16)), (8, dict(N=200, seed=19, max_partitions=64))):
         cl = kab.synth.make_ragged_cluster(T=600, R=6, rack_frac=0.0, desired_rf=drf, **shape)
-        s, out, out_len, S = _solved(cl, drf)
+        s, out, out_len, S = util.solved(cl, drf)
         assert S == drf and out_len.max() == drf
         for B in (1, 1000):
             _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B)
@@ -226,11 +169,11 @@ def test_growing_rf_rows_of_4_to_8(native_lib):
 @pytest.mark.gpu
 def test_hand_built_rows(native_lib):
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 41), 4))
+    s.set_brokers(*util.table(np.arange(1, 41), 4))
 
     def run(names, part_off, part_id, cur_lists, new_lists, B, weight=None, stride=None):
-        rep_off, cur = _cur(cur_lists)
-        out, out_len = _rows(new_lists, stride)
+        rep_off, cur = util.cur_lists(cur_lists)
+        out, out_len = util.rows(new_lists, stride)
         return _check(s, names, np.asarray(part_off, dtype=np.int64), None if part_id is None else np.asarray(part_id, dtype=np.int32),
                       rep_off, cur, out, out_len, B, None if weight is None else np.asarray(weight, dtype=np.int64))
 
@@ -261,12 +204,12 @@ def test_fully_serial_plans_cross_every_sort_pass(native_lib, Q):
     """Every row receives the same broker with B = 1: W = Q, one row per document. W on both sides of 128 and of 256 (one 8-bit
     pass or two), above 2 048, and above 65 536 (three passes)."""
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 41), 4))
+    s.set_brokers(*util.table(np.arange(1, 41), 4))
     T = 7
     part_off = (np.arange(T + 1) * Q) // T
     names = ["serial-%d" % t for t in range(T)]
-    rep_off, cur = _cur([[1]] * Q)
-    out, out_len = _rows([[2]] * Q)
+    rep_off, cur = util.cur_lists([[1]] * Q)
+    out, out_len = util.rows([[2]] * Q)
     docs, wave, _, st = _check(s, names, part_off, None, rep_off, cur, out, out_len, 1)
     assert st.code == 0 and len(docs) == Q and wave.tolist() == list(range(1, Q + 1))
 
@@ -275,13 +218,13 @@ def test_fully_serial_plans_cross_every_sort_pass(native_lib, Q):
 def test_scattered_waves_in_two_passes(native_lib):
     """A few hot brokers with B = 1: hundreds of waves whose rows are scattered over the whole input."""
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 61), 4))
+    s.set_brokers(*util.table(np.arange(1, 61), 4))
     rng = np.random.default_rng(8)
     Q = 30000
     cur_lists = [[int(x) for x in rng.choice(np.arange(1, 41), 2, replace=False)] for _ in range(Q)]
     new_lists = [[c[0], int(rng.integers(41, 61))] if rng.random() < 0.4 else c for c in cur_lists]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 2)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 2)
     part_off = np.concatenate([[0], np.sort(rng.choice(np.arange(1, Q), 499, replace=False)), [Q]])
     names = ["t.%d" % t for t in range(500)]
     docs, _, _, _ = _check(s, names, part_off, None, rep_off, cur, out, out_len, 1)
@@ -295,15 +238,15 @@ def test_long_names_take_the_direct_path(native_lib):
     """Names of about 400 bytes: the text of 256 rows exceeds the 64 KiB staging area, and those CTAs write straight to global
     memory; short names beside them keep other CTAs staged."""
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 41), 4))
+    s.set_brokers(*util.table(np.arange(1, 41), 4))
     rng = np.random.default_rng(9)
     T, Q = 40, 4000
     names = [("long-%02d-" % t) + "x" * int(rng.integers(380, 420)) if t % 4 else "s%d" % t for t in range(T)]
     part_off = np.arange(T + 1) * (Q // T)
     cur_lists = [[int(x) for x in rng.choice(np.arange(1, 31), 3, replace=False)] for _ in range(Q)]
     new_lists = [[c[0], c[1], int(rng.integers(31, 41))] if rng.random() < 0.8 else c for c in cur_lists]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     for B in (1, 50, 10 ** 6):
         docs, _, _, _ = _check(s, names, part_off, None, rep_off, cur, out, out_len, B)
     assert len(docs) == 1 and len(docs[0]) > 256 * 400
@@ -314,11 +257,11 @@ def test_long_names_take_the_direct_path(native_lib):
 def test_lookup_modes_and_chain_state(native_lib, table):
     N = dict(smem_lut=50, global_lut=50, bsearch=50, state_in_smem=12800, state_in_global=12801)[table]
     if table == "global_lut":
-        ids, racks = _table(1 + 700 * np.arange(N), 5)
+        ids, racks = util.table(1 + 700 * np.arange(N), 5)
     elif table == "bsearch":
-        ids, racks = _bsearch_table(N)
+        ids, racks = util.bsearch_table(N)
     else:
-        ids, racks = _table(np.arange(1, N + 1), 8)
+        ids, racks = util.table(np.arange(1, N + 1), 8)
     s = kab.Solver(0)
     s.set_brokers(ids, racks)
     rng = np.random.default_rng(N)
@@ -326,40 +269,29 @@ def test_lookup_modes_and_chain_state(native_lib, table):
     cur_lists = [[int(x) for x in rng.choice(ids, int(rng.integers(0, 4)), replace=False)] for _ in range(Q)]
     hot = ids[-5:]
     new_lists = [[int(x) for x in rng.choice(hot if g % 3 == 0 else ids, int(rng.integers(1, 4)), replace=False)] for g in range(Q)]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     part_off = np.arange(61) * 200
     names = ["m%d" % t for t in range(60)]
     for B, w in ((1, None), (500, rng.integers(0, 100, Q).astype(np.int64))):
         _check(s, names, part_off, None, rep_off, cur, out, out_len, B, w)
 
 
-def _raw(s, T, part_off, part_id, rep_off, cur, stride, new_len, new, weight, B, names, name_off, js, json_cap, doc_off, wave, summary,
-         cap, n=None):
-    st = kab.KaStatus()
-    n = ctypes.c_int32(-7) if n is None else n
-    p = lambda a: None if a is None else a.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
-    rc = s._L.ka_plan_waves_json(s._h, T, p(part_off), p(part_id), p(rep_off), p(cur), stride, p(new_len), p(new), p(weight), B,
-                                 p(names), p(name_off), p(js), json_cap, p(doc_off), p(wave),
-                                 ctypes.byref(n) if n is not False else None, p(summary), cap, ctypes.byref(st))
-    return rc, st, n
-
-
 @pytest.mark.gpu
 def test_errors(native_lib):
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 21), 4))
+    s.set_brokers(*util.table(np.arange(1, 21), 4))
     rng = np.random.default_rng(4)
     Q, T = 1000, 10
     cur_lists = [[int(x) for x in rng.choice(np.arange(1, 21), int(rng.integers(0, 4)), replace=False)] for _ in range(Q)]
     new_lists = [c if rng.random() < 0.3 else [int(x) for x in rng.choice(np.arange(1, 21), int(rng.integers(0, 4)), replace=False)]
                  for c in cur_lists]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     topic_names = ["err-%d" % t for t in range(T)]
     names, name_off = kab.Solver.marshal_names(topic_names)
     part_off = np.arange(T + 1, dtype=np.int64) * 100
-    cap = bound(topic_names, part_off, 3)
+    cap = models.json_bound(topic_names, part_off, 3)
     js, doc_off = np.zeros(cap, dtype=np.uint8), np.zeros(Q + 1, dtype=np.int64)
     wave, summ = np.zeros(Q, dtype=np.int32), np.zeros(Q, dtype=WAVE_SUMMARY_DTYPE)
     keys = ("s", "T", "part_off", "part_id", "rep_off", "cur", "stride", "new_len", "new", "weight", "B", "names", "name_off", "js",
@@ -369,7 +301,7 @@ def test_errors(native_lib):
     def call(n=None, **kw):
         a = dict(zip(keys, ok))
         a.update(kw)
-        rc, st, n = _raw(*a.values(), n=n)
+        rc, st, n = util.raw_plan_waves_json(*a.values(), n=n)
         assert rc == st.code
         if n is not False:
             assert rc == 0 or n.value == 0
@@ -417,12 +349,12 @@ def test_errors(native_lib):
         assert call(new=o, new_len=ln) == expect
         assert call(new=o, new_len=ln, json_cap=0) == expect
     # the text's exact size succeeds, one byte less is KA_ERR_LIMIT with a = json_cap; the bound always succeeds
-    e_docs = reference_wave_docs(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)[0]
+    e_docs = models.wave_docs(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)[0]
     size = sum(len(d) for d in e_docs)
     assert 0 < size <= cap
     assert call(json_cap=size - 1)[:2] == (LIMIT, size - 1) and call(json_cap=0)[:2] == (LIMIT, 0)
     js[:] = 0
-    rc, _, n = _raw(*ok[:14], size, *ok[15:])
+    rc, _, n = util.raw_plan_waves_json(*ok[:14], size, *ok[15:])
     assert rc == 0 and n.value == len(e_docs) and bytes(js[:size]) == b"".join(e_docs) and not js[size:].any()
     assert doc_off[:n.value + 1].tolist() == np.concatenate([[0], np.cumsum([len(d) for d in e_docs])]).tolist()
     # Q == 0: no document, doc_off[0] = 0 when given
@@ -432,9 +364,9 @@ def test_errors(native_lib):
     # a summary capacity below W, and no wave array: the documents all the same
     few = np.zeros(2, dtype=WAVE_SUMMARY_DTYPE)
     js[:] = 0
-    rc, _, n = _raw(*ok[:16], None, few, 2)
+    rc, _, n = util.raw_plan_waves_json(*ok[:16], None, few, 2)
     assert rc == 0 and n.value == len(e_docs) > 2 and bytes(js[:size]) == b"".join(e_docs)
-    assert [_rec(x) for x in few] == [_rec(x) for x in summ[:2]]
+    assert [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in few] == [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in summ[:2]]
 
 
 @pytest.mark.gpu
@@ -481,8 +413,8 @@ def test_context_is_untouched_and_launches_follow_the_bits_of_w(native_lib):
     # launches: the plan's 7, then 3 per radix pass (8 bits of W each) and the 3 text kernels; none of the latter when W = 0
     def launches(Q, same=False):
         names, part_off = _one_topic(Q)
-        rep_off, cur = _cur([[1]] * Q)
-        o, ln = _rows([[1 if same else 2]] * Q)
+        rep_off, cur = util.cur_lists([[1]] * Q)
+        o, ln = util.rows([[1 if same else 2]] * Q)
         n0 = s.launch_count()
         docs, _, _, st = s.plan_waves_json(names, part_off, None, rep_off, cur, o, ln, 1)
         assert st.code == 0 and len(docs) == (0 if same else Q)

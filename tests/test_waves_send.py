@@ -1,7 +1,7 @@
 """ka_plan_waves_send and ka_plan_waves_send_json: a wave plan that caps what each partition's leader sends per wave as well as
-what each broker receives. `reference_waves_send` restates the rule of include/kassign.h as a plain loop; every wave, W, summary
-and document of the device must equal it. The CPU tests pin the model on hand-worked cases and its invariants on random inputs,
-the declarations, and what Solver.plan_waves / plan_waves_json hand the C ABI."""
+what each broker receives. `models.plan_waves` with `send` restates the rule of include/kassign.h as a plain loop; every wave,
+W, summary and document of the device must equal it. The CPU tests pin the model on hand-worked cases and its invariants on
+random inputs, the declarations, and what Solver.plan_waves / plan_waves_json hand the C ABI."""
 import ctypes
 import os
 import subprocess
@@ -12,104 +12,17 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
-from tests.test_clusters import _bsearch_table, _table
-from tests.test_solver_abi import fake_solver, view
-from tests.test_waves import _cur, _random_case, _rows, _solved, reference_waves
-from tests.test_waves_json import bound
+from tests import models, util
 
 FIELDS = WAVE_SEND_SUMMARY_DTYPE.names
 INT64_MAX = np.iinfo(np.int64).max
 BAD, LIMIT = _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT
 
 
-def reference_waves_send(rep_off, cur, out, out_len, ids, send_ids, B, C, weight=None):
-    """(wave [Q] int32, [summary dict per wave, the seven fields], (code, a, b)) of the rule, rows in input order. The lowest
-    failing row wins: a new list naming a broker twice or a receiver missing from `ids` (at its first such position), else a row
-    with receivers whose sender (the first broker of its current list) is missing from `send_ids`; (KA_ERR_BAD_ARG, row, id)."""
-    Q = len(out_len)
-    table, senders = set(int(x) for x in ids), set(int(x) for x in send_ids)
-    opened, load, sopen, sload = {}, {}, {}, {}
-    inb, outb = {}, {}                               # (wave, broker id) -> incoming / outgoing weight
-    wave = np.zeros(Q, dtype=np.int32)
-    recv_of = {}
-    for g in range(Q):
-        new = [int(x) for x in out[g][:int(out_len[g])]]
-        old = [int(x) for x in cur[int(rep_off[g]):int(rep_off[g + 1])]]
-        recv = []
-        for j, b in enumerate(new):
-            if b in new[:j] or (b not in old and b not in table):
-                return None, None, (BAD, g, b)
-            if b not in old:
-                recv.append(b)
-        if new == old:
-            continue
-        if not recv:
-            wave[g] = 1
-            continue
-        s = old[0] if old else None
-        if s is not None and s not in senders:
-            return None, None, (BAD, g, s)
-        w = 1 if weight is None else int(weight[g])
-        a = w * len(recv)
-        v = max(opened.get(b, 1) if load.get(b, 0) == 0 or load.get(b, 0) + w <= B else opened.get(b, 1) + 1 for b in recv)
-        if s is not None:
-            o, x = sopen.get(s, 1), sload.get(s, 0)
-            v = max(v, o if x == 0 or x + a <= C else o + 1)
-        for b in recv:
-            if v > opened.get(b, 1):
-                opened[b], load[b] = v, w
-            else:
-                load[b] = load.get(b, 0) + w
-            inb[(v, b)] = inb.get((v, b), 0) + w
-        if s is not None:
-            if v > sopen.get(s, 1):
-                sopen[s], sload[s] = v, a
-            else:
-                sload[s] = sload.get(s, 0) + a
-            outb[(v, s)] = outb.get((v, s), 0) + a
-        wave[g] = v
-        recv_of[g] = (len(recv), w)
-    W = int(wave.max()) if Q else 0
-    summ = [dict(rows=0, rows_moved=0, replicas_added=0, max_broker_in=0, max_broker_in_id=-1, max_broker_out=0, max_broker_out_id=-1)
-            for _ in range(W)]
-    for g in np.nonzero(wave)[0]:
-        s = summ[wave[g] - 1]
-        s["rows"] += 1
-        if g in recv_of:
-            n, w = recv_of[g]
-            s["rows_moved"] += 1
-            s["replicas_added"] += n * w
-    for bins, peak, pid in ((inb, "max_broker_in", "max_broker_in_id"), (outb, "max_broker_out", "max_broker_out_id")):
-        for (v, b), x in sorted(bins.items()):
-            s = summ[v - 1]
-            if x > s[peak]:
-                s[peak], s[pid] = x, b
-    return wave, summ, (0, 0, 0)
-
-
-def reference_send_docs(topic_names, part_off, part_id, rep_off, cur, out, out_len, ids, send_ids, B, C, weight=None):
-    """(docs, wave, summary, status): the waves of reference_waves_send printed as reference_wave_docs prints them."""
-    wave, summ, st = reference_waves_send(rep_off, cur, out, out_len, ids, send_ids, B, C, weight)
-    if st[0] != 0:
-        return None, wave, summ, st
-    recs = [[] for _ in summ]
-    for t, name in enumerate(topic_names):
-        for g in range(int(part_off[t]), int(part_off[t + 1])):
-            if wave[g]:
-                p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
-                recs[wave[g] - 1].append('{"partition":%d,"replicas":[%s],"topic":"%s"}'
-                                         % (p, ",".join(str(int(b)) for b in out[g][:int(out_len[g])]), name))
-    return [('{"partitions":[' + ",".join(r) + '],"version":1}').encode() for r in recs], wave, summ, st
-
-
-def _rec(s):
-    return {f: int(s[f]) for f in FIELDS}
-
-
 def _model(cur_lists, new_lists, B, C, weight=None, ids=range(1, 100), send_ids=range(1, 100)):
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists)
-    return reference_waves_send(rep_off, cur, out, out_len, list(ids), list(send_ids), B, C, weight)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists)
+    return models.plan_waves(rep_off, cur, out, out_len, list(ids), B, weight, send=(list(send_ids), C))
 
 
 def send_loads(cur_lists, new_lists, wave, weight=None):
@@ -157,7 +70,7 @@ def test_model_drained_leader_is_split():
     budget of 5 cuts them into waves of 5."""
     cur = [[1, 2]] * 12
     new = [[2, 10 + g] for g in range(12)]
-    wave, summ, st = reference_waves(*_cur(cur), *_rows(new), list(range(2, 40)), 1)
+    wave, summ, st = models.plan_waves(*util.cur_lists(cur), *util.rows(new), list(range(2, 40)), 1)
     assert st == (0, 0, 0) and wave.tolist() == [1] * 12
     wave, summ, st = _model(cur, new, 1, 5)
     assert st == (0, 0, 0) and wave.tolist() == [1] * 5 + [2] * 5 + [3] * 2
@@ -193,12 +106,12 @@ def test_model_hand_worked_cases():
 def test_model_invariants(seed):
     rng = np.random.default_rng(seed)
     ids = np.arange(1, 13)
-    cur_lists, new_lists = _random_case(rng, 300, 12)
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    cur_lists, new_lists = util.random_wave_case(rng, 300, 12)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     for B, C, weight in ((1, 1, None), (2, 5, None), (10 ** 6, 3, None), (4, 10 ** 6, None), (50, 60, rng.integers(0, 40, 300)),
                          (30, 200, rng.integers(0, 80, 300))):
-        wave, summ, st = reference_waves_send(rep_off, cur, out, out_len, ids, ids, B, C, weight)
+        wave, summ, st = models.plan_waves(rep_off, cur, out, out_len, ids, B, weight, send=(ids, C))
         assert st == (0, 0, 0)
         W = len(summ)
         assert W == (int(wave.max()) if len(wave) else 0)
@@ -216,7 +129,7 @@ def test_model_invariants(seed):
         # a send budget no plan reaches: no leader opens a wave, so a row's wave is the larger of ka_plan_waves's receiver term
         # and its leader's open wave (the wave of the leader's previous moved row)
         big = 8 * int(w.sum())
-        wave, summ, _ = reference_waves_send(rep_off, cur, out, out_len, ids, ids, B, big, weight)
+        wave, summ, _ = models.plan_waves(rep_off, cur, out, out_len, ids, B, weight, send=(ids, big))
         last = {}
         for g in range(300):
             r = [b for b in new_lists[g] if b not in cur_lists[g]]
@@ -227,64 +140,20 @@ def test_model_invariants(seed):
     cur_lists = [[g + 1] + c[1:] if rng.random() < 0.7 else [] for g, c in enumerate(cur_lists)]
     new_lists = [[b for b in x if b not in c[:1]] for x, c in zip(new_lists, cur_lists)]
     ids = np.arange(1, 301)
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     for B, weight in ((1, None), (3, None), (40, rng.integers(0, 30, 300))):
-        wave, summ, _ = reference_waves_send(rep_off, cur, out, out_len, ids, ids, B, INT64_MAX, weight)
-        e_wave, e_summ, _ = reference_waves(rep_off, cur, out, out_len, ids, B, weight)
+        wave, summ, _ = models.plan_waves(rep_off, cur, out, out_len, ids, B, weight, send=(ids, INT64_MAX))
+        e_wave, e_summ, _ = models.plan_waves(rep_off, cur, out, out_len, ids, B, weight)
         assert np.array_equal(wave, e_wave) and [{k: s[k] for k in WAVE_SUMMARY_DTYPE.names} for s in summ] == e_summ
-
-
-class _FakeLib:
-    """Stands in for libkassign.so: records what the _send entry points are handed, plans W waves (wave[g] = 1 + g % W) and
-    writes recognisable summaries and sender summaries."""
-
-    def __init__(self, W):
-        self.W, self.calls = W, []
-
-    def _fill(self, Q, wave, summary, send_summary, cap, n_waves, st):
-        if wave is not None and Q:
-            np.ctypeslib.as_array(ctypes.cast(wave, ctypes.POINTER(ctypes.c_int32)), shape=(Q,))[:] = 1 + np.arange(Q) % self.W
-        n = min(cap, self.W)
-        s = np.ctypeslib.as_array(ctypes.cast(summary, ctypes.POINTER(ctypes.c_int64)), shape=(cap * 5,)).reshape(cap, 5)
-        s[:n] = np.arange(n)[:, None] * 10 + np.arange(5)
-        o = np.ctypeslib.as_array(ctypes.cast(send_summary, ctypes.POINTER(ctypes.c_int64)), shape=(cap * 2,)).reshape(cap, 2)
-        o[:n] = np.arange(n)[:, None] * 10 + 5 + np.arange(2)
-        n_waves._obj.value = self.W
-        st._obj.code = 0
-        return 0
-
-    def ka_plan_waves_send(self, h, Q, rep_off, cur, stride, new_len, new_broker, weight, B, n_send, send_id, C, wave, n_waves, summary,
-                           send_summary, cap, st):
-        r_off = view(rep_off, Q + 1, np.int64)
-        self.calls.append(dict(Q=Q, stride=stride, rep_off=r_off, cur=view(cur, int(r_off[-1]), np.int32),
-                               new_len=view(new_len, Q, np.int32), new_broker=view(new_broker, Q * stride, np.int32),
-                               weight=view(weight, Q, np.int64), B=B, send_id=view(send_id, n_send, np.int32), C=C, cap=cap))
-        return self._fill(Q, wave, summary, send_summary, cap, n_waves, st)
-
-    def ka_plan_waves_send_json(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, n_send, send_id, C,
-                                names, name_off, js, json_cap, doc_off, wave, n_waves, summary, send_summary, cap, st):
-        p_off = view(part_off, T + 1, np.int64)
-        Q = int(p_off[-1])
-        self.calls.append(dict(T=T, Q=Q, stride=stride, B=B, send_id=view(send_id, n_send, np.int32), C=C, json_cap=json_cap, cap=cap))
-        text = np.ctypeslib.as_array(ctypes.cast(js, ctypes.POINTER(ctypes.c_uint8)), shape=(json_cap,))
-        off = np.ctypeslib.as_array(ctypes.cast(doc_off, ctypes.POINTER(ctypes.c_int64)), shape=(Q + 1,))
-        at = 0
-        for v in range(self.W):
-            doc = b"<%d>" % v
-            off[v] = at
-            text[at:at + len(doc)] = np.frombuffer(doc, dtype=np.uint8)
-            at += len(doc)
-        off[self.W] = at
-        return self._fill(Q, wave, summary, send_summary, cap, n_waves, st)
 
 
 @pytest.mark.parametrize("W", [3, 100])
 def test_plan_waves_with_a_send_budget_marshals_its_arguments(W):
-    lib = _FakeLib(W)
-    s = fake_solver(lib)
-    out, out_len = _rows([[1, 2], [3], [4, 5, 6], []])
-    rep_off, cur = _cur([[1], [2, 3], [4], [7, 8]])
+    lib = util.FakeWaveLib(W)
+    s = util.fake_solver(lib)
+    out, out_len = util.rows([[1, 2], [3], [4, 5, 6], []])
+    rep_off, cur = util.cur_lists([[1], [2, 3], [4], [7, 8]])
     weight = np.array([5, 0, 7, 1], dtype=np.int64)
     wave, summ, st = s.plan_waves(rep_off, cur, out, out_len, 9, weight=weight, max_broker_out=11, send_brokers=[1, 2, 4, 7])
     assert st.code == 0
@@ -303,17 +172,17 @@ def test_plan_waves_with_a_send_budget_marshals_its_arguments(W):
 
 
 def test_plan_waves_json_with_a_send_budget_marshals_its_arguments():
-    lib = _FakeLib(3)
-    s = fake_solver(lib)
-    out, out_len = _rows([[1, 2], [3], [4, 5, 6], []])
-    rep_off, cur = _cur([[1], [2, 3], [4], [7, 8]])
+    lib = util.FakeWaveLib(3)
+    s = util.fake_solver(lib)
+    out, out_len = util.rows([[1, 2], [3], [4, 5, 6], []])
+    rep_off, cur = util.cur_lists([[1], [2, 3], [4], [7, 8]])
     names, part_off = ["alpha", "", "bc"], [0, 3, 3, 4]
     docs, wave, summ, st = s.plan_waves_json(names, part_off, None, rep_off, cur, out, out_len, 9, max_broker_out=12,
                                              send_brokers=np.array([1, 2, 4, 7], dtype=np.int64))
     assert st.code == 0 and len(lib.calls) == 1
     c = lib.calls[0]
     assert c["T"] == 3 and c["B"] == 9 and c["C"] == 12 and c["cap"] == 4 and c["send_id"].tolist() == [1, 2, 4, 7]
-    assert c["json_cap"] == bound(names, part_off, 3)
+    assert c["json_cap"] == models.json_bound(names, part_off, 3)
     assert [bytes(d) for d in docs] == [b"<0>", b"<1>", b"<2>"] and wave.tolist() == [1, 2, 3, 1]
     assert summ.dtype == WAVE_SEND_SUMMARY_DTYPE and [list(x) for x in summ] == [[v * 10 + f for f in range(7)] for v in range(3)]
 
@@ -323,11 +192,11 @@ def test_plan_waves_json_with_a_send_budget_marshals_its_arguments():
 def _check(s, rep_off, cur, out, out_len, B, C, send_ids, weight=None):
     """plan_waves with a send budget against the model, every field. Returns (wave, summary, status)."""
     wave, summ, st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight, max_broker_out=C, send_brokers=send_ids)
-    e_wave, e_summ, e_st = reference_waves_send(rep_off, cur, out, out_len, s.broker_id, send_ids, B, C, weight)
+    e_wave, e_summ, e_st = models.plan_waves(rep_off, cur, out, out_len, s.broker_id, B, weight, send=(send_ids, C))
     assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
     if st.code == 0:
         assert np.array_equal(wave, e_wave), np.nonzero(wave != e_wave)[0][:10]
-        assert [_rec(x) for x in summ] == e_summ
+        assert [util.record_of(x, FIELDS) for x in summ] == e_summ
     return wave, summ, st
 
 
@@ -335,13 +204,13 @@ def _check_docs(s, names, part_off, part_id, rep_off, cur, out, out_len, B, C, s
     """plan_waves_json with a send budget against the model and against plan_waves with the same budget."""
     docs, wave, summ, st = s.plan_waves_json(names, part_off, part_id, rep_off, cur, out, out_len, B, weight=weight, json_buf=json_buf,
                                              max_broker_out=C, send_brokers=send_ids)
-    e_docs, e_wave, e_summ, e_st = reference_send_docs(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, send_ids, B,
-                                                       C, weight)
+    e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, weight,
+                                                    send=(send_ids, C))
     assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
     if st.code == 0:
         p_wave, p_summ, _ = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight, max_broker_out=C, send_brokers=send_ids)
         assert np.array_equal(wave, e_wave) and np.array_equal(wave, p_wave)
-        assert [_rec(x) for x in summ] == e_summ and np.array_equal(summ, p_summ)
+        assert [util.record_of(x, FIELDS) for x in summ] == e_summ and np.array_equal(summ, p_summ)
         assert len(docs) == len(e_docs)
         for v, (d, e) in enumerate(zip(docs, e_docs)):
             assert bytes(d) == e, (v, bytes(d)[:200], e[:200])
@@ -352,7 +221,7 @@ def _check_docs(s, names, part_off, part_id, rep_off, cur, out, out_len, B, C, s
 @pytest.mark.parametrize("remove", [0.0, 0.03])
 def test_solve_rows(native_lib, remove):
     cl = kab.synth.make_ragged_cluster(T=4000, N=400, max_partitions=128, seed=7, remove_frac=remove)
-    s, out, out_len, S = _solved(cl)
+    s, out, out_len, S = util.solved(cl)
     Q = len(out_len)
     weight = np.random.default_rng(3).integers(0, 1 << 30, Q).astype(np.int64)
     mean = int(weight.mean())
@@ -368,7 +237,7 @@ def test_drained_brokers_send_within_the_budget(native_lib):
     """With brokers removed, a receive budget alone lets the drained leaders send far beyond C in one wave; the send budget holds
     every leader to C."""
     cl = kab.synth.make_ragged_cluster(T=4000, N=400, max_partitions=128, seed=9, remove_frac=0.03)
-    s, out, out_len, S = _solved(cl)
+    s, out, out_len, S = util.solved(cl)
     B, C = 8, 8
     wave, _, st = s.plan_waves(cl.rep_off, cl.cur, out, out_len, B)
     assert st.code == 0
@@ -386,15 +255,15 @@ def test_a_huge_send_budget(native_lib):
     ka_plan_waves / ka_plan_waves_json; on a solved cluster the device still equals the model."""
     s = kab.Solver(0)
     N = 3000
-    s.set_brokers(*_table(np.arange(1, N + 1), 8))
+    s.set_brokers(*util.table(np.arange(1, N + 1), 8))
     rng = np.random.default_rng(12)
     Q = N
     cur_lists = [[g + 1] + [int(x) for x in rng.choice(np.arange(1, N + 1), 1)] if g % 5 else [] for g in range(Q)]
     cur_lists = [c[:1] if len(c) == 2 and c[0] == c[1] else c for c in cur_lists]
     hot = np.arange(N - 20, N + 1)
     new_lists = [[int(x) for x in rng.choice(hot if g % 2 else np.arange(1, N + 1), 2, replace=False)] for g in range(Q)]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 2)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 2)
     weight = rng.integers(0, 1 << 20, Q).astype(np.int64)
     names, part_off = ["h%d" % t for t in range(30)], np.arange(31) * (Q // 30)
     send_ids = np.arange(1, N + 1, dtype=np.int32)
@@ -409,7 +278,7 @@ def test_a_huge_send_budget(native_lib):
         e_docs, _, _, _ = s.plan_waves_json(names, part_off, None, rep_off, cur, out, out_len, B, weight=w)
         assert st.code == 0 and [bytes(d) for d in docs] == [bytes(d) for d in e_docs]
     cl = kab.synth.make_ragged_cluster(T=3000, N=300, max_partitions=128, seed=13, remove_frac=0.02)
-    s, out, out_len, S = _solved(cl)
+    s, out, out_len, S = util.solved(cl)
     _check(s, cl.rep_off, cl.cur, out, out_len, 2, INT64_MAX, cl.all_broker_id)
 
 
@@ -420,11 +289,11 @@ def test_lookup_modes_and_chain_state(native_lib, table):
     6 400 + 6 400 in shared memory, 6 400 + 6 401 in global memory."""
     N = 6400 if table.startswith("state") else 50
     if table == "global_lut":
-        ids, racks = _table(1 + 700 * np.arange(N), 5)
+        ids, racks = util.table(1 + 700 * np.arange(N), 5)
     elif table == "bsearch":
-        ids, racks = _bsearch_table(N)
+        ids, racks = util.bsearch_table(N)
     else:
-        ids, racks = _table(np.arange(1, N + 1), 8)
+        ids, racks = util.table(np.arange(1, N + 1), 8)
     # the send table: the broker table and senders outside it (a drained set), n_send = N or N + 1 for the state cases
     extra = {"state_in_smem": 0, "state_in_global": 1}.get(table, 7)
     gone = np.arange(1, extra + 1) + int(ids.max())
@@ -440,8 +309,8 @@ def test_lookup_modes_and_chain_state(native_lib, table):
     for g, c in enumerate(cur_lists):
         pool = np.setdiff1d(hot if g % 3 == 0 else ids, c)
         new_lists.append([int(x) for x in rng.choice(pool, int(rng.integers(1, 4)), replace=False)])
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     for B, C, w in ((1, 1, None), (16, 5, None), (500, 700, rng.integers(0, 100, Q).astype(np.int64))):
         _check(s, rep_off, cur, out, out_len, B, C, send_ids, w)
     names, part_off = ["m%d" % t for t in range(40)], np.arange(41) * (Q // 40)
@@ -453,12 +322,12 @@ def test_one_leader_is_fully_serial(native_lib):
     """Every moved row comes from broker 1, each to a receiver of its own: with C = 1 every row is a wave of its own, across the
     chain's chunks; the documents cross two radix passes."""
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 41), 4))
+    s.set_brokers(*util.table(np.arange(1, 41), 4))
     Q = 5000
     cur_lists = [[1]] * Q
     new_lists = [[1, 2 + g % 39] for g in range(Q)]
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists)
     wave, summ, st = _check(s, rep_off, cur, out, out_len, 10 ** 6, 1, [1])
     assert st.code == 0 and wave.tolist() == list(range(1, Q + 1)) and set(summ["max_broker_out_id"].tolist()) == {1}
     names, part_off = ["serial-%d" % t for t in range(7)], (np.arange(8) * Q) // 7
@@ -489,12 +358,12 @@ def _raw_json(s, T, part_off, rep_off, cur, stride, new_len, new, B, n_send, sen
 @pytest.mark.gpu
 def test_errors_and_buffers(native_lib):
     s = kab.Solver(0)
-    s.set_brokers(*_table(np.arange(1, 21), 4))
+    s.set_brokers(*util.table(np.arange(1, 21), 4))
     rng = np.random.default_rng(4)
     Q = 1000
-    cur_lists, new_lists = _random_case(rng, Q, 20)
-    rep_off, cur = _cur(cur_lists)
-    out, out_len = _rows(new_lists, 3)
+    cur_lists, new_lists = util.random_wave_case(rng, Q, 20)
+    rep_off, cur = util.cur_lists(cur_lists)
+    out, out_len = util.rows(new_lists, 3)
     send = np.arange(1, 21, dtype=np.int32)
     wave, summ, ssum = np.zeros(Q, dtype=np.int32), np.zeros(Q, dtype=WAVE_SUMMARY_DTYPE), np.zeros((Q, 2), dtype=np.int64)
     keys = ("s", "Q", "rep_off", "cur", "stride", "new_len", "new", "weight", "B", "n_send", "send_id", "C", "wave", "summary",
@@ -533,17 +402,17 @@ def test_errors_and_buffers(native_lib):
             o[g, :] = -1
             o[g, :len(x)] = x
             ln[g] = len(x)
-        e = reference_waves_send(rep_off, cur, o, ln, s.broker_id, sids, 2, 3)[2]
+        e = models.plan_waves(rep_off, cur, o, ln, s.broker_id, 2, send=(sids, 3))[2]
         assert e[0] == BAD and (expect is None or e == expect)
         assert call(new=o, new_len=ln, n_send=len(sids), send_id=sids) == e
-    g = int(reference_waves_send(rep_off, cur, out, out_len, s.broker_id, send[send != 5], 2, 3)[2][1])
+    g = int(models.plan_waves(rep_off, cur, out, out_len, s.broker_id, 2, send=(send[send != 5], 3))[2][1])
     o, ln = out.copy(), out_len.copy()
     o[g, :] = -1
     o[g, :2] = [7, 7]
     ln[g] = 2
     assert call(new=o, new_len=ln, n_send=19, send_id=send[send != 5]) == (BAD, g, 7)   # its own new list comes first
     # a summary capacity below W
-    e_wave, e_summ, _ = reference_waves_send(rep_off, cur, out, out_len, s.broker_id, send, 1, 1)
+    e_wave, e_summ, _ = models.plan_waves(rep_off, cur, out, out_len, s.broker_id, 1, send=(send, 1))
     W = len(e_summ)
     assert W > 3
     few, few_s = np.zeros(3, dtype=WAVE_SUMMARY_DTYPE), np.zeros((3, 2), dtype=np.int64)
@@ -556,7 +425,7 @@ def test_errors_and_buffers(native_lib):
     topic_names = ["err-%d" % t for t in range(T)]
     names, name_off = kab.Solver.marshal_names(topic_names)
     part_off = np.arange(T + 1, dtype=np.int64) * 100
-    cap = bound(topic_names, part_off, 3)
+    cap = models.json_bound(topic_names, part_off, 3)
     js, doc_off = np.zeros(cap, dtype=np.uint8), np.zeros(Q + 1, dtype=np.int64)
     jok = dict(s=s, T=T, part_off=part_off, rep_off=rep_off, cur=cur, stride=3, new_len=out_len, new=out, B=2, n_send=20, send_id=send,
                C=3, names=names, name_off=name_off, js=js, json_cap=cap, doc_off=doc_off, wave=wave, summary=summ, send_summary=ssum,
@@ -571,7 +440,7 @@ def test_errors_and_buffers(native_lib):
 
     assert jcall(js=None, C=0)[0] == BAD and jcall(doc_off=None, n_send=70000)[0] == BAD
     assert jcall(C=0)[0] == BAD and jcall(n_send=70000, send_id=np.arange(70000, dtype=np.int32))[:2] == (LIMIT, 70000)
-    e_docs = reference_send_docs(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, send, 2, 3)[0]
+    e_docs = models.wave_docs(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, send=(send, 3))[0]
     size = sum(len(d) for d in e_docs)
     assert 0 < size <= cap
     assert jcall(json_cap=size - 1)[:2] == (LIMIT, size - 1)
@@ -605,8 +474,8 @@ def test_context_is_untouched_and_launches_are_fixed(native_lib):
 
     # the plan's 9 whatever Q, W and n_send; the documents add 3 per radix pass (8 bits of W each) and 3, none when W = 0
     def launches(Q, same=False, n_send=1):
-        rep_off, cur = _cur([[1]] * Q)
-        o, ln = _rows([[1 if same else 2]] * Q)
+        rep_off, cur = util.cur_lists([[1]] * Q)
+        o, ln = util.rows([[1 if same else 2]] * Q)
         send_ids = np.arange(1, n_send + 1, dtype=np.int32)
         n0 = s.launch_count()
         _, _, st = s.plan_waves(rep_off, cur, o, ln, 10 ** 9, max_broker_out=1, send_brokers=send_ids)

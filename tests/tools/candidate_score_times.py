@@ -4,7 +4,7 @@ that each remove a different seeded random 2 % of the brokers, and a seeded rand
 the host:
 
   (a) ka_solve_candidates (every candidate's rows and list lengths copied back) + the numpy summary of
-      tests/test_candidate_scores.py per candidate on the host;
+      tests/models.py per candidate on the host;
   (b) ka_score_candidates without rows (K summaries come back);
   (c) ka_score_candidates with rows (the summaries and the rows of (a)).
 
@@ -25,7 +25,7 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import MOVE_SUMMARY_DTYPE  # noqa: E402
-from tests.test_candidate_scores import reference_summary  # noqa: E402
+from tests import models  # noqa: E402
 from tests.tools.ragged_candidate_times import gpu_info, random_tables  # noqa: E402
 
 
@@ -62,7 +62,7 @@ def measure(name, prob, tables, weight, steps, warmup):
         for k, (ids, _) in enumerate(tabs):
             if st_a[k].code != 0:
                 continue
-            e, rep, lead, inb = reference_summary(out[k], out_len[k], rep_off, cur, ids.astype(np.int64), weight)
+            e, rep, lead, inb = models.move_summary(out[k], out_len[k], rep_off, cur, ids.astype(np.int64), weight)
             for f, v in e.items():
                 sum_a[k][f] = v
             for i, a in enumerate((rep, lead, inb)):

@@ -4,7 +4,7 @@ topics each; a skewed fleet, one 240 k-topic cluster and 31 of 2 k topics; K = 1
 weight per partition. Arms, all buffers on the host:
 
   (a) ka_solve_clusters (every cluster's rows and list lengths copied back) + the numpy summary of
-      tests/test_candidate_scores.py per cluster on the host; in brackets, the ka_solve_clusters call alone;
+      tests/models.py per cluster on the host; in brackets, the ka_solve_clusters call alone;
   (b) ka_score_clusters without rows (K summaries come back);
   (c) ka_score_clusters with rows (the summaries and the rows of (a)).
 
@@ -24,7 +24,7 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import MOVE_SUMMARY_DTYPE  # noqa: E402
-from tests.test_candidate_scores import reference_summary  # noqa: E402
+from tests import models  # noqa: E402
 from tests.tools.cluster_batch_times import gpu_info  # noqa: E402
 
 
@@ -63,8 +63,8 @@ def measure(name, clusters, steps, warmup, seed):
             if st_a[k].code != 0:
                 continue
             r0, r1 = row0[k], row0[k + 1]
-            e, rep, lead, inb = reference_summary(out[r0:r1], out_len[r0:r1], c.rep_off, c.cur, c.broker_id.astype(np.int64),
-                                                  weight[r0:r1])
+            e, rep, lead, inb = models.move_summary(out[r0:r1], out_len[r0:r1], c.rep_off, c.cur, c.broker_id.astype(np.int64),
+                                                    weight[r0:r1])
             for f, v in e.items():
                 sum_a[k][f] = v
             for i, a in enumerate((rep, lead, inb)):

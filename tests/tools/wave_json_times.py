@@ -11,8 +11,8 @@ Two arms, both starting from the rows in host memory and ending with every docum
             wave) and Python string formatting of every record. It is what a script around Solver.plan_waves would do, NOT a
             tuned emitter: a compiled one would be much faster.
 Every step is synchronous and timed with the host clock, the L2 flushed (256 MiB written) before it; the median of --steps steps
-after --warmup warm-up steps. Before timing, the documents of both arms are checked equal, byte for byte, to reference_wave_docs
-of tests/test_waves_json.py. Prints the GPU, its power limit and SM clock, and a markdown table."""
+after --warmup warm-up steps. Before timing, the documents of both arms are checked equal, byte for byte, to models.wave_docs
+of tests/models.py. Prints the GPU, its power limit and SM clock, and a markdown table."""
 import argparse
 import ctypes
 import os
@@ -26,7 +26,7 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE  # noqa: E402
-from tests.test_waves_json import bound, reference_wave_docs  # noqa: E402
+from tests import models  # noqa: E402
 from tests.tools.cluster_batch_times import gpu_info  # noqa: E402
 from tests.tools.wave_plan_times import _vp, plan_once  # noqa: E402
 
@@ -37,9 +37,9 @@ def host_docs(names, part_off, part_id, out, out_len, wave, W):
     order = changed[np.argsort(wave[changed], kind="stable")]
     topic_of = np.searchsorted(part_off, order, side="right") - 1
     ends = np.cumsum(np.bincount(wave[changed], minlength=W + 1)[1:]).tolist()
-    recs = ['{"partition":%d,"replicas":[%s],"topic":"%s"}' % (p, ",".join(map(str, row[:n])), names[t])
+    recs = [models.record(names[t], p, row[:n])
             for p, row, n, t in zip(part_id[order].tolist(), out[order].tolist(), out_len[order].tolist(), topic_of.tolist())]
-    return [('{"partitions":[' + ",".join(recs[a:b]) + '],"version":1}').encode() for a, b in zip([0] + ends[:-1], ends)]
+    return [models.document(recs[a:b]).encode() for a, b in zip([0] + ends[:-1], ends)]
 
 
 def measure(name, cl, steps, warmup, flush):
@@ -49,7 +49,7 @@ def measure(name, cl, steps, warmup, flush):
     assert st.code == 0
     Q, T = len(out_len), len(cl.topic_names)
     names, name_off = s.marshal_names(cl.topic_names)
-    cap = bound(cl.topic_names, cl.part_off, 3)
+    cap = models.json_bound(cl.topic_names, cl.part_off, 3)
     text = torch.empty(cap, dtype=torch.uint8).pin_memory().numpy()
     doc_off, wave = np.zeros(Q + 1, dtype=np.int64), np.zeros(Q, dtype=np.int32)
     weight = np.random.default_rng(0x5EED).integers(1, 1 << 34, size=Q, dtype=np.int64)
@@ -67,8 +67,8 @@ def measure(name, cl, steps, warmup, flush):
         return float(np.median(ms))
 
     for label, B, w in (("unit, B = 1", 1, None), ("weighted, B = 16 x mean", 16 * int(weight.mean()), weight)):
-        e_docs, e_wave, e_summ, e_st = reference_wave_docs(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len,
-                                                           cl.broker_id, B, w)
+        e_docs, e_wave, e_summ, e_st = models.wave_docs(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len,
+                                                        cl.broker_id, B, w)
         assert e_st[0] == 0, name + ": refused"
         W = len(e_docs)
         summ = np.zeros(W, dtype=WAVE_SUMMARY_DTYPE)

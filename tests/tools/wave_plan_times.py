@@ -7,8 +7,8 @@ planned
 
 Two arms: ONE ka_plan_waves C call with a summary buffer of W entries, and Solver.plan_waves (which asks for min(Q, 64 k)
 summaries, so here it also makes one C call; the tool checks that W fits). Every step is synchronous and timed with the host clock, the L2 flushed (256 MiB written) before it; the median of --steps
-steps after --warmup warm-up steps. Before timing, every wave and summary is checked equal to reference_waves of
-tests/test_waves.py. The chain's rounds are counted from the records in the chain's own chunks (a record decides in round
+steps after --warmup warm-up steps. Before timing, every wave and summary is checked equal to models.plan_waves of
+tests/models.py. The chain's rounds are counted from the records in the chain's own chunks (a record decides in round
 1 + the latest round of the earlier records of its chunk that share a receiver with it). Prints the GPU, its power limit and SM
 clock, and a markdown table."""
 import argparse
@@ -24,7 +24,7 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE  # noqa: E402
-from tests.test_waves import _rec, reference_waves  # noqa: E402
+from tests import models, util  # noqa: E402
 from tests.tools.cluster_batch_times import gpu_info  # noqa: E402
 
 CHUNK = 2048   # KA_WAVE_CHUNK of kassign_waves.cuh: records the chain decides together
@@ -91,9 +91,9 @@ def measure(name, cl, steps, warmup, flush):
     rounds, moved = chain_rounds(cl.rep_off, cl.cur, out, out_len)
     for label, B, w in (("unit, B = 1", 1, None), ("weighted, B = 16 x mean", 16 * int(weight.mean()), weight)):
         wave, summ, st = s.plan_waves(cl.rep_off, cl.cur, out, out_len, B, weight=w)
-        e_wave, e_summ, e_st = reference_waves(cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
+        e_wave, e_summ, e_st = models.plan_waves(cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
         assert st.code == 0 and e_st[0] == 0, name + ": refused"
-        assert np.array_equal(wave, e_wave) and [_rec(x) for x in summ] == e_summ, name + ": plan differs from the model"
+        assert np.array_equal(wave, e_wave) and [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in summ] == e_summ, name + ": plan differs from the model"
         W = len(summ)
         assert W <= min(Q, s.WAVE_SUMMARY_CAP), name + ": Solver.plan_waves would make a second call"
         wave1, summ1 = np.zeros(Q, dtype=np.int32), np.zeros(W, dtype=WAVE_SUMMARY_DTYPE)

@@ -6,8 +6,8 @@ rows (all buffers on the host) then planned with unit weights and B = 1, and wit
 For each: the largest per-wave sender load of ka_plan_waves's plan (computed here from its waves: what a receive budget alone
 lets one leader send), then ka_plan_waves_send with C = B and C = 4 B: W, the chain's rounds (a record decides in round 1 + the
 latest round of the earlier records of its chunk that share a receiver or its sender with it) and the time of one C call, with
-ka_plan_waves's on the same rows beside it. Every plan is checked equal to its model (reference_waves /
-reference_waves_send) before it is timed. Each step is synchronous and timed with the host clock, the L2 flushed (256 MiB
+ka_plan_waves's on the same rows beside it. Every plan is checked equal to its model (models.plan_waves,
+without and with a sender) before it is timed. Each step is synchronous and timed with the host clock, the L2 flushed (256 MiB
 written) before it; the median of --steps steps after --warmup. Prints the GPU, its power limit and SM clock, and a markdown
 table."""
 import argparse
@@ -23,8 +23,7 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE  # noqa: E402
-from tests.test_waves import _rec, reference_waves  # noqa: E402
-from tests.test_waves_send import reference_waves_send  # noqa: E402
+from tests import models, util  # noqa: E402
 from tests.tools.cluster_batch_times import gpu_info  # noqa: E402
 
 CHUNK = 2048   # KA_WAVE_CHUNK of kassign_waves.cuh: records the chain decides together
@@ -108,15 +107,15 @@ def measure(name, cl, steps, warmup, flush):
 
     for label, B, w in (("unit, B = 1", 1, None), ("weighted, B = 16 x mean", 16 * int(weight.mean()), weight)):
         assert plan(B, w) == 0
-        e_wave, e_summ, _ = reference_waves(cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
-        assert np.array_equal(wave, e_wave) and [_rec(x) for x in summ[:n.value]] == e_summ, name + ": plan differs from the model"
+        e_wave, e_summ, _ = models.plan_waves(cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
+        assert np.array_equal(wave, e_wave) and [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in summ[:n.value]] == e_summ, name + ": plan differs from the model"
         W0, open_send = n.value, max_send(moved, wave, w)
         t0 = timed(lambda: plan(B, w))
         for cm in (1, 4):
             C = cm * B
             assert plan_send(B, C, w) == 0
-            e_wave, e_summ, _ = reference_waves_send(cl.rep_off, cl.cur, out, out_len, cl.broker_id, send_id, B, C, w)
-            got = [dict(_rec(x), max_broker_out=int(y[0]), max_broker_out_id=int(y[1])) for x, y in zip(summ[:n.value], ssum)]
+            e_wave, e_summ, _ = models.plan_waves(cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w, send=(send_id, C))
+            got = [dict(util.record_of(x, WAVE_SUMMARY_DTYPE.names), max_broker_out=int(y[0]), max_broker_out_id=int(y[1])) for x, y in zip(summ[:n.value], ssum)]
             assert np.array_equal(wave, e_wave) and got == e_summ, name + ": send plan differs from the model"
             W, peak = n.value, max_send(moved, wave, w)
             t1 = timed(lambda: plan_send(B, C, w))

@@ -1,11 +1,19 @@
-"""Shared helpers for the parity tests: flatten {topic: {partition: [brokers]}} cases into the flat
-layout of include/kassign.h, and run them through the C++ oracle or the CUDA library."""
+"""Shared helpers of the test suite, each written once: flatten {topic: {partition: [brokers]}} cases into the flat layout of
+include/kassign.h and run them through the C++ oracle or the CUDA library; broker tables, problems, fleets and wave inputs;
+the checks and fakes more than one test module uses. The plain-Python models live in tests/models.py."""
+import ctypes
 import json
 import os
 
 import numpy as np
 
+import kafka_assigner_b200 as kab
+from kafka_assigner_b200 import _native
+from tests import models
+
 HERE = os.path.dirname(os.path.abspath(__file__))
+FRACS = (0.01, 0.02, 0.05, 0.10, 0.20, 0.30, 0.40, 0.50)
+MIN_HASH = "polygenelubricants"   # String.hashCode == Integer.MIN_VALUE (KAS:190-192)
 
 
 def load_golden():
@@ -80,3 +88,465 @@ def oracle_dense(ol, cl, ctx=None):
     ln, _, out, st = ol.run(ctx or ol.OracleContext(), cl.topic_names, part_off, part_id, rep_off, cur, cl.broker_id,
                             cl.rack_name, cl.desired_rf, max(cl.RF, cl.desired_rf, 1), raise_on_error=False)
     return out, ln, st
+
+
+def fields(st):
+    """A KaStatus as a comparable tuple."""
+    return (st.code, st.topic_index, st.partition, st.a, st.b)
+
+
+def record_of(s, names):
+    """The fields `names` of one structured-array summary as a dict of ints."""
+    return {f: int(s[f]) for f in names}
+
+
+EMPTY_SUMMARY = dict({f: 0 for f in kab.assigner.MOVE_SUMMARY_DTYPE.names}, max_broker_in_id=-1)   # a refused candidate's
+
+
+def row_width(rep_off, desired_rf):
+    """The narrowest row stride for these lists and desired RF."""
+    sizes = np.diff(rep_off)
+    return max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+
+
+def has_gpu():
+    try:
+        import torch
+        return torch.cuda.is_available()
+    except Exception:
+        return False
+
+
+# ---- fakes of the library ------------------------------------------------------------------------------------------------
+
+def view(p, n, ctype):
+    """A copy of the n elements of `ctype` at the C pointer p (None for a NULL pointer)."""
+    if p is None:
+        return None
+    if n == 0:
+        return np.zeros(0, dtype=ctype)
+    return np.ctypeslib.as_array(ctypes.cast(p, ctypes.POINTER(np.ctypeslib.as_ctypes_type(ctype))), shape=(n,)).copy()
+
+
+def writable(p, n, ctype):
+    return np.ctypeslib.as_array(ctypes.cast(p, ctypes.POINTER(np.ctypeslib.as_ctypes_type(ctype))), shape=(n,))
+
+
+def fake_solver(lib):
+    s = object.__new__(kab.Solver)
+    s._L = lib
+    s._h = ctypes.c_void_p(1)
+    return s
+
+
+class FakeWaveLib:
+    """Stands in for libkassign.so's four wave entry points: records what each call is handed, plans W waves
+    (wave[g] = 1 + g % W), writes recognisable summaries (field f of summary v: 10 v + f, the sender fields as f = 5, 6), at most
+    `cap` of them, and writes document v as b"<v>"."""
+
+    def __init__(self, W):
+        self.W, self.calls = W, []
+
+    @staticmethod
+    def _rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave):
+        r_off = view(rep_off, Q + 1, np.int64)
+        return dict(Q=Q, stride=stride, rep_off=r_off, cur=view(cur, int(r_off[-1]), np.int32), new_len=view(new_len, Q, np.int32),
+                    new_broker=view(new_broker, Q * stride, np.int32), weight=view(weight, Q, np.int64), B=B, wave=wave is not None)
+
+    def _docs(self, T, part_off, part_id, names, name_off, js, json_cap, doc_off):
+        """Writes the W documents; returns Q and what the text arguments were."""
+        p_off = view(part_off, T + 1, np.int64)
+        Q = int(p_off[-1])
+        n_off = view(name_off, T + 1, np.int64)
+        text, off = writable(js, json_cap, np.uint8), writable(doc_off, Q + 1, np.int64)
+        at = 0
+        for v in range(self.W):
+            doc = b"<%d>" % v
+            off[v] = at
+            text[at:at + len(doc)] = np.frombuffer(doc, dtype=np.uint8)
+            at += len(doc)
+        off[self.W] = at
+        return Q, dict(T=T, part_off=p_off, part_id=view(part_id, Q, np.int32), names=bytes(view(names, int(n_off[-1]), np.uint8)),
+                       name_off=n_off, json_cap=json_cap)
+
+    def _fill(self, Q, wave, n_waves, summary, send_summary, cap, st):
+        if wave is not None and Q:
+            writable(wave, Q, np.int32)[:] = 1 + np.arange(Q) % self.W
+        n = min(cap, self.W)
+        if cap:
+            writable(summary, cap * 5, np.int64).reshape(cap, 5)[:n] = np.arange(n)[:, None] * 10 + np.arange(5)
+            if send_summary is not None:
+                writable(send_summary, cap * 2, np.int64).reshape(cap, 2)[:n] = np.arange(n)[:, None] * 10 + 5 + np.arange(2)
+        n_waves._obj.value = self.W
+        st._obj.code = 0
+        return 0
+
+    def ka_plan_waves(self, h, Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave, n_waves, summary, cap, st):
+        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), cap=cap))
+        return self._fill(Q, wave, n_waves, summary, None, cap, st)
+
+    def ka_plan_waves_send(self, h, Q, rep_off, cur, stride, new_len, new_broker, weight, B, n_send, send_id, C, wave, n_waves, summary,
+                           send_summary, cap, st):
+        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave),
+                               send_id=view(send_id, n_send, np.int32), C=C, cap=cap))
+        return self._fill(Q, wave, n_waves, summary, send_summary, cap, st)
+
+    def ka_plan_waves_json(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, names, name_off,
+                           js, json_cap, doc_off, wave, n_waves, summary, cap, st):
+        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off)
+        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), **text, cap=cap))
+        return self._fill(Q, wave, n_waves, summary, None, cap, st)
+
+    def ka_plan_waves_send_json(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, n_send, send_id, C,
+                                names, name_off, js, json_cap, doc_off, wave, n_waves, summary, send_summary, cap, st):
+        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off)
+        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), **text,
+                               send_id=view(send_id, n_send, np.int32), C=C, cap=cap))
+        return self._fill(Q, wave, n_waves, summary, send_summary, cap, st)
+
+
+# ---- broker tables -------------------------------------------------------------------------------------------------------
+
+def table(ids, racks_per=None):
+    """(ids, rack_index): racks_per = brokers per rack (contiguous), or None: no broker has a rack."""
+    ids = np.asarray(ids, dtype=np.int32)
+    names = [None] * len(ids) if racks_per is None else ["k%d" % (i // racks_per) for i in range(len(ids))]
+    return ids, kab.synth.rack_indices(ids, names)
+
+
+def bsearch_table(N):
+    """Brokers 1..N plus one id far away: an id range beyond the global LUT, so ids are looked up by binary search."""
+    return table(np.concatenate([np.arange(1, N + 1), [1 << 27]]).astype(np.int32), 4)
+
+
+def ragged_mixed_tables(rng, cl):
+    """Candidate tables for a make_ragged_cluster: every capacity and lookup mode, and one without brokers (the last)."""
+    live = cl.broker_id
+    return [
+        (cl.broker_id, cl.rack_index),                                                        # capacity > 1, the cluster's racks
+        table(np.sort(rng.choice(live, len(live) - 4, replace=False))),                       # capacity > 1, no racks
+        table(np.sort(rng.choice(live, len(live) - 6, replace=False)), 3),                    # capacity > 1, other racks
+        table(np.arange(1, 1 + 4000, dtype=np.int32), 40),                                    # capacity 1, racks
+        table(np.arange(1, 1 + 3000, dtype=np.int32)),                                        # capacity 1, no racks
+        table(1 + 2 * np.arange(20000, dtype=np.int32), 500),                                 # 20 000 brokers, global id LUT
+        table(np.zeros(0, dtype=np.int32)),                                                   # no broker
+    ]
+
+
+# ---- candidate problems --------------------------------------------------------------------------------------------------
+
+class DenseProblem:
+    """A dense problem on the device: topic hashes, current lists, and room for K candidates' rows."""
+
+    def __init__(self, topic_hash, cur, desired_rf=-1, out_stride=None):
+        import torch
+        self.T, self.P, self.RF = cur.shape
+        self.desired_rf = desired_rf
+        self.S = out_stride or max(self.RF, desired_rf, 1)
+        self.topic_hash, self.cur = topic_hash, cur
+        self.d_hash = torch.from_numpy(np.ascontiguousarray(topic_hash, dtype=np.int32)).cuda()
+        self.d_cur = torch.from_numpy(np.ascontiguousarray(cur, dtype=np.int32)).cuda()
+
+    def sequential(self, tables):
+        """The contract's reference: a fresh context per table, ka_ctx_set_brokers + ka_solve_dense_device."""
+        import torch
+        rows = []
+        for ids, racks in tables:
+            s = kab.Solver(0)
+            s.set_brokers(ids, racks)
+            out = torch.full((self.T, self.P, self.S), -7, dtype=torch.int32, device="cuda")
+            ln = torch.full((self.T, self.P), -7, dtype=torch.int32, device="cuda")
+            st = s.solve_dense_device(self.T, self.d_hash.data_ptr(), self.P, self.RF, self.d_cur.data_ptr(), self.desired_rf,
+                                      self.S, ln.data_ptr(), out.data_ptr())
+            rows.append((out.cpu().numpy(), ln.cpu().numpy(), fields(st)))
+            s.close()
+        return rows
+
+    def batched(self, tables, solver=None):
+        import torch
+        K = len(tables)
+        out = torch.full((K, self.T, self.P, self.S), -7, dtype=torch.int32, device="cuda")
+        ln = torch.full((K, self.T, self.P), -7, dtype=torch.int32, device="cuda")
+        s = solver or kab.Solver(0)
+        sts = s.solve_dense_candidates_device(tables, self.T, self.d_hash.data_ptr(), self.P, self.RF, self.d_cur.data_ptr(),
+                                              self.desired_rf, self.S, ln.data_ptr(), out.data_ptr())
+        return out.cpu().numpy(), ln.cpu().numpy(), [fields(st) for st in sts]
+
+
+def check_dense_equal(prob, tables, oracle=None, solver=None):
+    """ka_solve_dense_candidates_device against a fresh context per table (and the oracle). Returns the statuses."""
+    out, ln, sts = prob.batched(tables, solver)
+    seq = prob.sequential(tables)
+    for k, (e_out, e_len, e_st) in enumerate(seq):
+        assert sts[k] == e_st, (k, sts[k], e_st)
+        if e_st[0] != 0:
+            continue   # the rows of a failed candidate are unspecified
+        assert np.array_equal(out[k], e_out), k
+        assert np.array_equal(ln[k], e_len), k
+        if oracle is not None:
+            ids, racks = tables[k]
+            exp, exp_len, est = oracle.fast_run_dense(oracle.FastContext(), prob.topic_hash, prob.cur, ids, racks, prob.desired_rf,
+                                                      prob.S)
+            assert est.code == 0, k
+            assert np.array_equal(out[k].reshape(-1, prob.S), exp), k
+            assert np.array_equal(ln[k].reshape(-1), exp_len), k
+    return sts
+
+
+class Problem:
+    """The ka_solve inputs of one run (host arrays)."""
+
+    def __init__(self, names, topic_hash, part_off, part_id, rep_off, cur, desired_rf=-1, out_stride=None):
+        self.names, self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur = names, topic_hash, part_off, part_id, rep_off, cur
+        self.desired_rf = desired_rf
+        self.S = out_stride or row_width(rep_off, desired_rf)
+
+    @classmethod
+    def of(cls, cl, desired_rf=-1):
+        return cls(cl.topic_names, cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off, cl.cur, desired_rf)
+
+    def args(self):
+        return self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur, self.desired_rf
+
+    def sequential(self, tables):
+        """The contract's reference: a fresh context per table, ka_ctx_set_brokers + ka_solve."""
+        rows = []
+        for ids, racks in tables:
+            s = kab.Solver(0)
+            s.set_brokers(ids, racks)
+            out, ln, st = s.solve_ragged(*self.args(), self.S, check=False)
+            rows.append((out, ln, fields(st)))
+            s.close()
+        return rows
+
+    def batched(self, tables, solver=None):
+        s = solver or kab.Solver(0)
+        out, ln, sts = s.solve_ragged_candidates(tables, *self.args(), out_stride=self.S)
+        return out, ln, [fields(st) for st in sts]
+
+
+def check_equal(prob, tables, oracle=None, solver=None):
+    """ka_solve_candidates against a fresh context per table (and the oracle). Returns the statuses."""
+    out, ln, sts = prob.batched(tables, solver)
+    seq = prob.sequential(tables)
+    assert len(sts) == len(tables)
+    for k, (e_out, e_len, e_st) in enumerate(seq):
+        assert sts[k] == e_st, (k, sts[k], e_st)
+        if e_st[0] != 0:
+            continue   # the rows of a failed candidate are unspecified
+        assert np.array_equal(out[k], e_out), k
+        assert np.array_equal(ln[k], e_len), k
+        if oracle is not None:
+            ids, racks = tables[k]
+            o_len, _, o_out, o_st = oracle.run(oracle.OracleContext(), prob.names, prob.part_off, prob.part_id, prob.rep_off, prob.cur,
+                                               ids, ["k%d" % r for r in racks], prob.desired_rf, prob.S, raise_on_error=False)
+            assert o_st.code == 0, k
+            assert np.array_equal(out[k], o_out) and np.array_equal(ln[k], o_len), k
+    return sts
+
+
+def check_scores(prob, tables, weight=None, oracle=None, solver=None, sequential=True):
+    """One ka_score_candidates call (rows and per-broker arrays asked for) against ka_solve_candidates' rows (checked against
+    fresh single solves and the oracle when `sequential`) and the numpy reference. Returns the statuses and summaries."""
+    s = solver or kab.Solver(0)
+    if sequential:
+        sts = check_equal(prob, tables, oracle, solver=s)
+        out, ln, _ = prob.batched(tables, s)
+    else:
+        out, ln, sts = prob.batched(tables, s)
+    summary, st, sc_out, sc_len, rep, lead, inb = s.score_ragged_candidates(tables, *prob.args(), out_stride=prob.S, weight=weight,
+                                                                           rows=True, per_broker=True)
+    assert [fields(x) for x in st] == sts
+    names = kab.assigner.MOVE_SUMMARY_DTYPE.names
+    w = np.ones(int(prob.part_off[-1]), dtype=np.int64) if weight is None else weight
+    for k, (ids, _) in enumerate(tables):
+        if sts[k][0] != 0:
+            assert record_of(summary[k], names) == EMPTY_SUMMARY, k
+            assert not rep[k].any() and not lead[k].any() and not inb[k].any(), k
+            continue
+        assert np.array_equal(sc_out[k], out[k]) and np.array_equal(sc_len[k], ln[k]), k
+        e, e_rep, e_lead, e_in = models.move_summary(out[k], ln[k], prob.rep_off, prob.cur, np.asarray(ids, dtype=np.int64), weight)
+        assert record_of(summary[k], names) == e, (k, record_of(summary[k], names), e)
+        assert np.array_equal(rep[k], e_rep) and np.array_equal(lead[k], e_lead) and np.array_equal(inb[k], e_in), k
+        # identities
+        assert rep[k].sum() == int((w * ln[k]).sum()) and lead[k].sum() == int(w[ln[k] > 0].sum())
+        assert inb[k].sum() == summary[k]["replicas_added"]
+    return sts, summary
+
+
+def sparse_with_empty_topics(cl, rng, empty):
+    """cl's topics with sparse (ascending, gapped) partition ids and, with `empty`, a topic without partitions after every
+    seventh one."""
+    names, th, P, pid = [], [], [], []
+    for t in range(cl.T):
+        a, b = int(cl.part_off[t]), int(cl.part_off[t + 1])
+        names.append(cl.topic_names[t])
+        th.append(cl.topic_hash[t])
+        P.append(b - a)
+        pid.append(np.cumsum(rng.integers(1, 9, size=b - a)).astype(np.int32) - 1)
+        if empty and t % 7 == 3:
+            names.append("empty.%d" % t)
+            th.append(kab.java_string_hash("empty.%d" % t))
+            P.append(0)
+            pid.append(np.zeros(0, dtype=np.int32))
+    part_off = np.zeros(len(P) + 1, dtype=np.int64)
+    np.cumsum(P, out=part_off[1:])
+    return names, np.array(th, dtype=np.int32), part_off, np.concatenate(pid), cl.rep_off, cl.cur
+
+
+def exception_problem(tail):
+    """Three topics whose failure depends on the table, then `tail`: a list-size mismatch, or a topic without partitions."""
+    topics = [("alpha", {3: [1, 2], 7: [2, 3], 8: [3, 4], 40: [4, 5], 41: [5, 6]}),
+              ("polygenelubricants", {5: [1, 2], 6: [2, 1]}),       # String.hashCode == Integer.MIN_VALUE (KAS:190-192)
+              ("gamma", {11: [1, 2, 3], 12: [2, 3, 4], 13: [3, 4, 5]})]
+    if tail == "mismatch":
+        topics.append(("delta", {0: [1, 2], 9: [3]}))
+    elif tail == "empty":
+        topics.append(("none", {}))
+    names, part_off, part_id, rep_off, cur = flatten(topics)
+    th = np.array([kab.java_string_hash(n) for n in names], dtype=np.int32)
+    return Problem(names, th, part_off, part_id, rep_off, cur, -1, 3)
+
+
+# ---- fleets --------------------------------------------------------------------------------------------------------------
+
+class Member:
+    """One cluster of a fleet: its table, its ka_solve inputs (offsets from 0) and its topic names."""
+
+    def __init__(self, table, names, topic_hash, part_off, part_id, rep_off, cur, desired_rf=-1):
+        self.ids, self.racks = table
+        self.names = list(names)
+        self.topic_hash = np.asarray(topic_hash, dtype=np.int32)
+        self.part_off, self.part_id, self.rep_off, self.cur = part_off, part_id, rep_off, cur
+        self.desired_rf = desired_rf
+
+    @classmethod
+    def of(cls, cl, table=None, desired_rf=-1):
+        return cls(table or (cl.broker_id, cl.rack_index), cl.topic_names, cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off,
+                   cl.cur, desired_rf)
+
+    @classmethod
+    def of_topics(cls, table, topics, desired_rf=-1):
+        names, part_off, part_id, rep_off, cur = flatten(topics)
+        return cls(table, names, [kab.java_string_hash(n) for n in names], part_off, part_id, rep_off, cur, desired_rf)
+
+    def entry(self):
+        return (self.ids, self.racks, self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur, self.desired_rf)
+
+    def sequential(self, s, S):
+        """The contract's reference: a fresh Context with this cluster's table, then ka_solve."""
+        s.reset()
+        s.set_brokers(self.ids, self.racks)
+        out, ln, st = s.solve_ragged(self.topic_hash, self.part_off, self.part_id, self.rep_off, self.cur, self.desired_rf, S,
+                                     check=False)
+        return out, ln, fields(st)
+
+
+def fleet_stride(fleet):
+    """The narrowest row stride for every cluster of the fleet."""
+    return max([row_width(m.rep_off, m.desired_rf) for m in fleet] + [1])
+
+
+def min_hash_cluster(table):
+    """Topics around one whose hashCode is Integer.MIN_VALUE, with lists of 2 (|hash| % 2 == 0: it solves)."""
+    topics = [("a", {0: [1, 2], 1: [2, 3]}), (MIN_HASH, {3: [1, 2], 5: [2, 3], 6: [3, 1]}), ("z", {0: [3, 4]})]
+    return Member.of_topics(table, topics)
+
+
+def oracle_text(ol, names, part_off, part_id, rep_off, cur, brokers, rack_names, desired, ctx=None):
+    """(text or None, oracle status) of one run through the C++ oracle."""
+    pid = part_id if part_id is not None else np.concatenate(
+        [np.arange(part_off[t + 1] - part_off[t], dtype=np.int32) for t in range(len(names))] + [np.zeros(0, np.int32)])
+    ln, opid, out, st = ol.run(ctx or ol.OracleContext(), names, part_off, pid, rep_off, cur, brokers, rack_names, desired,
+                               row_width(rep_off, desired), raise_on_error=False)
+    return (None if st.code else models.solve_document(names, part_off, opid, out, ln)), st
+
+
+def sequential_json(m, s):
+    """The contract's reference: a fresh Context with this cluster's table, then ka_solve_json; a cluster wider than the batched
+    chains' 3 is refused with its width instead."""
+    width = row_width(m.rep_off, m.desired_rf)
+    if width > 3:
+        return b"", (_native.KA_ERR_LIMIT, -1, -1, width, 0)
+    s.reset()
+    s.set_brokers(m.ids, m.racks)
+    text, st = s.solve_ragged_json(m.names, m.topic_hash, m.part_off, m.part_id, m.rep_off, m.cur, m.desired_rf, check=False)
+    return bytes(text), fields(st)
+
+
+def check_fleet(fleet, oracle=None, solver=None):
+    """ka_solve_clusters_json: every cluster against its sequential ka_solve_json (and the oracle's text); the documents back to
+    back in cluster order."""
+    s = solver or kab.Solver(0)
+    res = s.solve_clusters_json([m.entry() for m in fleet], [m.names for m in fleet])
+    assert len(res) == len(fleet)
+    ref = kab.Solver(0)
+    sts, texts = [], []
+    for k, (m, (text, st)) in enumerate(zip(fleet, res)):
+        e_text, e_st = sequential_json(m, ref)
+        assert fields(st) == e_st, (k, fields(st), e_st)
+        assert bytes(text) == e_text, k
+        sts.append(e_st)
+        texts.append(bytes(text))
+        if oracle is not None and e_st[0] == 0:
+            exp, o_st = oracle_text(oracle, m.names, m.part_off, m.part_id, m.rep_off, m.cur, m.ids, ["k%d" % r for r in m.racks],
+                                    m.desired_rf)
+            assert o_st.code == 0 and bytes(text).decode() == exp, k
+    # the documents back to back in cluster order, in one buffer (a failed cluster's range is empty)
+    starts = [t.__array_interface__["data"][0] for t, _ in res if len(t)]
+    assert all(b - a == len(t) for a, b, t in zip(starts, starts[1:], [t for t in texts if t]))
+    return sts, texts
+
+
+# ---- wave plans ----------------------------------------------------------------------------------------------------------
+
+def rows(lists, stride=None):
+    """(out [Q, stride], out_len [Q]) from a list of new lists; unused slots -1."""
+    stride = stride or max([len(x) for x in lists] + [1])
+    out = np.full((len(lists), stride), -1, dtype=np.int32)
+    for g, x in enumerate(lists):
+        out[g, :len(x)] = x
+    return out, np.array([len(x) for x in lists], dtype=np.int32)
+
+
+def cur_lists(lists):
+    """(rep_off, cur) from a list of current lists."""
+    rep_off = np.zeros(len(lists) + 1, dtype=np.int64)
+    np.cumsum([len(x) for x in lists], out=rep_off[1:])
+    return rep_off, np.array([b for x in lists for b in x], dtype=np.int32)
+
+
+def random_wave_case(rng, Q, N, stride=3):
+    """Q random (current, new) list pairs over brokers 1..N, 30 % of them unchanged."""
+    cur, new = [], []
+    for _ in range(Q):
+        m = int(rng.integers(0, stride + 1))
+        cur.append([int(x) for x in rng.choice(np.arange(1, N + 1), m, replace=False)])
+        if rng.random() < 0.3:
+            new.append(list(cur[-1]))
+        else:
+            n = int(rng.integers(0, stride + 1))
+            new.append([int(x) for x in rng.choice(np.arange(1, N + 1), n, replace=False)])
+    return cur, new
+
+
+def solved(cl, desired_rf=-1):
+    """A fresh Solver on the cluster's table and the rows ka_solve gives for it."""
+    s = kab.Solver(0)
+    s.set_brokers(cl.broker_id, cl.rack_index)
+    S = max(int(np.diff(cl.rep_off).max()), desired_rf, 1)
+    out, out_len, st = s.solve_ragged(cl.topic_hash, cl.part_off, cl.part_id, cl.rep_off, cl.cur, desired_rf, S)
+    assert st.code == 0
+    return s, out, out_len, S
+
+
+def raw_plan_waves_json(s, T, part_off, part_id, rep_off, cur, stride, new_len, new, weight, B, names, name_off, js, json_cap, doc_off,
+                        wave, summary, cap, n=None):
+    """ka_plan_waves_json through ctypes: (rc, status, W)."""
+    st = kab.KaStatus()
+    n = ctypes.c_int32(-7) if n is None else n
+    p = lambda a: None if a is None else a.ctypes.data_as(ctypes.c_void_p)  # noqa: E731
+    rc = s._L.ka_plan_waves_json(s._h, T, p(part_off), p(part_id), p(rep_off), p(cur), stride, p(new_len), p(new), p(weight), B,
+                                 p(names), p(name_off), p(js), json_cap, p(doc_off), p(wave),
+                                 ctypes.byref(n) if n is not False else None, p(summary), cap, ctypes.byref(st))
+    return rc, st, n
