@@ -442,6 +442,60 @@ int32_t ka_plan_waves_send_json(ka_ctx* ctx, int32_t T, const int64_t* part_off,
                                 int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, ka_wave_send_summary* send_summary,
                                 int32_t summary_cap, ka_status* st);
 
+/* ka_plan_waves_json with every document under a size limit: each wave cut on the device into PARTS of at most L =
+ * max_doc_bytes bytes, documents that run one after the other. Kafka 0.10's kafka-reassign-partitions writes a whole document
+ * into one ZooKeeper znode, and ZooKeeper refuses znode data above jute.maxbuffer (0xfffff bytes by default): L = 1048575 gives
+ * documents it accepts. Any subset of a wave keeps every receive (and send) budget of that wave, so cutting a wave weakens no
+ * guarantee of the plan.
+ *   T .. json_cap, wave, n_waves, summary, summary_cap   exactly as ka_plan_waves_json takes and writes them: wave, W and the
+ *                      summaries are those of ka_plan_waves for the same inputs
+ *   max_doc_bytes      the limit L >= 1
+ *   doc_off[Q+1]       host, required when Q > 0; entries 0..D are written, doc_off[0] = 0
+ *   doc_wave[Q]        host, required when Q > 0; doc_wave[d] = the wave (1..W) of part d, for d < D
+ *   n_docs             host, required when Q > 0; *n_docs = D, the number of parts
+ * The rule. Take the rows of wave v in input row order, and let b_i be the byte length of row i's record: exactly the record
+ * ka_solve_json prints, without its comma. A part is a run of consecutive rows of one wave; its document is {"partitions":[ +
+ * the records, comma separated, + ],"version":1}, 29 + sum(b_i) + (rows - 1) bytes. The cut is greedy: the first row of a
+ * wave opens a part, and each next row joins the current part if the part stays <= L, else it opens a new part. So the parts
+ * are unique, and no two consecutive parts of a wave could be merged within L. The parts are ordered by (wave, place in the
+ * wave); document d is json[doc_off[d] .. doc_off[d+1]), back to back and not NUL-terminated. Every wave has at least one part,
+ * and D <= the changed rows <= Q. With L >= the longest wave document, D = W, doc_wave[d] = d + 1, and json and doc_off are
+ * byte for byte those of ka_plan_waves_json. json_cap = the bound of ka_plan_waves_json still suffices: every part holds at
+ * least one row.
+ * One document under a limit for a whole solve needs no other call: with max_broker_in >= the sum of the weights every changed
+ * row is in wave 1, and wave 1 is cut into parts. Unchanged rows are in no part, which an operator does not submit anyway.
+ * Checks, in this order: everything ka_plan_waves_json checks, in its order, with its codes and operands; then max_doc_bytes < 1,
+ * or doc_wave or n_docs NULL with Q > 0: KA_ERR_BAD_ARG. On the device, after the plan's own row errors: a changed row whose
+ * one-record document (29 + b_i bytes) exceeds L gives KA_ERR_LIMIT with a = the lowest such row (input order) and b = that
+ * length clipped to INT_MAX; then a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX). On any error
+ * *n_waves = *n_docs = 0 (when given) and nothing else is specified. W == 0 gives D = 0 and doc_off[0] = 0.
+ * Synchronous; two synchronisations. The launches of ka_plan_waves_json, then, when W > 0, 4 more, and 2K - 1 more when the
+ * widest wave has m >= 2 rows, K = the bit length of m - 1 (a pointer-doubling level per bit): they depend only on the bit
+ * lengths of W and of m. Does not read or change the Context counters, parked counters, topic_base, the staged block, or the
+ * last order / stage plans and timings. */
+int32_t ka_plan_waves_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                 const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                                 const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                                 int64_t max_broker_in, const char* names, const int64_t* name_off,
+                                 char* json, int64_t json_cap, int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave,
+                                 int32_t* n_docs, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
+                                 int32_t summary_cap, ka_status* st);
+
+/* ka_plan_waves_json_parts under the rule of ka_plan_waves_send: the waves of ka_plan_waves_send_json, each cut into parts.
+ *   T .. json_cap       exactly as ka_plan_waves_send_json takes them
+ *   max_doc_bytes .. n_docs   exactly as ka_plan_waves_json_parts takes and writes them
+ *   wave .. summary_cap   exactly as ka_plan_waves_send_json writes them
+ * Checks: everything ka_plan_waves_send_json checks, in its order; then those ka_plan_waves_json_parts adds, in its order. The
+ * launches of ka_plan_waves_send_json, and those ka_plan_waves_json_parts adds. */
+int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                      const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                                      const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                                      int64_t max_broker_in, int32_t n_send, const int32_t* send_id, int64_t max_broker_out,
+                                      const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                      int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave, int32_t* n_docs,
+                                      int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
+                                      ka_wave_send_summary* send_summary, int32_t summary_cap, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

@@ -551,6 +551,25 @@ class Solver:
         speed); by default one of the documented sufficient size. Returns (docs, wave, summary, KaStatus): docs a list of W
         bytes-like views of the buffer, docs[v] the document of wave v + 1; wave and summary as plan_waves returns them. On an
         error docs, wave and summary are empty. max_broker_out / send_brokers: ka_plan_waves_send_json, as in plan_waves."""
+        docs, _, wave, summary, st = self._wave_documents(topic_names, part_off, part_id, rep_off, cur_broker, out, out_len,
+                                                          max_broker_in, weight, json_buf, max_broker_out, send_brokers, None)
+        return docs, wave, summary, st
+
+    def plan_wave_parts_json(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, max_doc_bytes,
+                             weight=None, json_buf=None, max_broker_out=None, send_brokers=None):
+        """ka_plan_waves_json_parts: plan_waves_json with every wave cut on the device into parts whose documents are at most
+        max_doc_bytes bytes (1048575 fits ZooKeeper's default jute.maxbuffer). Returns (parts, part_wave, wave, summary,
+        KaStatus): parts a list of D bytes-like views of the buffer in (wave, place in the wave) order, part_wave [D] int32 the
+        wave (1..W) of each; the other arguments and results as plan_waves_json takes and returns them. On an error parts,
+        part_wave, wave and summary are empty. With max_broker_in >= the sum of the weights every changed row is in wave 1: the
+        whole reassignment under the limit."""
+        return self._wave_documents(topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, weight,
+                                    json_buf, max_broker_out, send_brokers, int(max_doc_bytes))
+
+    def _wave_documents(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, weight, json_buf,
+                        max_broker_out, send_brokers, max_doc_bytes):
+        """One call of the four wave document entry points: with max_doc_bytes None ka_plan_waves(_send)_json, else their
+        _parts forms. Returns (docs, doc_wave, wave, summary, KaStatus); doc_wave is 1..W without a limit."""
         out = np.ascontiguousarray(out, dtype=np.int32)
         Q = len(out)
         stride = out.shape[1] if out.ndim == 2 else 1
@@ -570,19 +589,28 @@ class Solver:
         send = _send_part(max_broker_out, send_brokers)
         rows = (self._h, len(topic_names), _ptr(r.part_off), _ptr(r.part_id), _ptr(r.rep_off), _ptr(r.cur_broker), int(stride),
                 _ptr(out_len), _ptr(out), _ptr(weight), int(max_broker_in))
-        text = (_ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(doc_off), _ptr(wave), ctypes.byref(n_waves),
-                _ptr(summary))
+        if max_doc_bytes is None:
+            text = (_ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), _ptr(doc_off), _ptr(wave), ctypes.byref(n_waves),
+                    _ptr(summary))
+            entry = self._L.ka_plan_waves_json if send is None else self._L.ka_plan_waves_send_json
+        else:
+            doc_wave = np.zeros(Q, dtype=np.int32)
+            n_docs = ctypes.c_int32(0)
+            text = (_ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), max_doc_bytes, _ptr(doc_off), _ptr(doc_wave),
+                    ctypes.byref(n_docs), _ptr(wave), ctypes.byref(n_waves), _ptr(summary))
+            entry = self._L.ka_plan_waves_json_parts if send is None else self._L.ka_plan_waves_send_json_parts
         if send is None:
-            self._L.ka_plan_waves_json(*rows, *text, cap, ctypes.byref(st))
+            entry(*rows, *text, cap, ctypes.byref(st))
         else:
             send_summary = np.zeros((cap, len(_SEND_FIELDS)), dtype=np.int64)
-            self._L.ka_plan_waves_send_json(*rows, send[0], _ptr(send[1]), send[2], *text, _ptr(send_summary), cap, ctypes.byref(st))
+            entry(*rows, send[0], _ptr(send[1]), send[2], *text, _ptr(send_summary), cap, ctypes.byref(st))
         if st.code != 0:
             dtype = WAVE_SUMMARY_DTYPE if send is None else WAVE_SEND_SUMMARY_DTYPE
-            return [], np.zeros(0, dtype=np.int32), np.zeros(0, dtype=dtype), st
+            return [], np.zeros(0, dtype=np.int32), np.zeros(0, dtype=np.int32), np.zeros(0, dtype=dtype), st
         W = n_waves.value
         summary = summary[:W] if send is None else _with_send(summary[:W], send_summary[:W])
-        return [json_buf[doc_off[v]:doc_off[v + 1]] for v in range(W)], wave, summary, st
+        D, doc_wave = (W, np.arange(1, W + 1, dtype=np.int32)) if max_doc_bytes is None else (n_docs.value, doc_wave[:n_docs.value])
+        return [json_buf[doc_off[d]:doc_off[d + 1]] for d in range(D)], doc_wave, wave, summary, st
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

@@ -154,8 +154,11 @@ struct ka_ctx {
     DevBuf d_wv_send, d_wv_slog, d_wv_ssum;
     // scratch of ka_plan_waves_json, beside the plan's and the JSON passes' (d_part_off, d_part_id, d_names, d_name_off, d_json,
     // d_json_rowlen, d_json_blocksum as 64-bit offsets): the grouped rows (two arrays of Q), the radix passes' (digit, tile)
-    // counts and offsets, and the text total followed by doc_off [W + 1]
+    // counts and offsets, and the text total followed by doc_off [W + 1] (with a size limit: the total, D, then doc_off [D + 1])
     DevBuf d_wv_perm, d_wv_hist, d_wv_doc;
+    // scratch of a size limit (ka_plan_waves_json_parts): the prefix S, the meta words, J_0, the waves' first positions, the
+    // parts per CTA, the parts' waves and the start flags; then the jump tables J_1 .. J_{K-1}
+    DevBuf d_wv_part, d_wv_jump;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -1339,7 +1342,7 @@ void ka_ctx_destroy(ka_ctx* c) {
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
                       &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec,
                       &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta, &c->d_wv_perm, &c->d_wv_hist, &c->d_wv_doc,
-                      &c->d_wv_send, &c->d_wv_slog, &c->d_wv_ssum})
+                      &c->d_wv_part, &c->d_wv_jump, &c->d_wv_send, &c->d_wv_slog, &c->d_wv_ssum})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -2632,14 +2635,70 @@ static const int32_t* enq_wave_group(ka_ctx* c, cudaStream_t s, int64_t Q, int W
     return perm[(pass - 1) & 1];
 }
 
-// ka_plan_waves_json, and with a sender part sd ka_plan_waves_send_json.
+// The size limit of ka_plan_waves_json_parts: L = max_doc_bytes, and the caller's doc_wave and n_docs.
+struct WaveParts {
+    int64_t L;
+    int32_t* doc_wave;
+    int32_t* n_docs;
+};
+
+// The part passes of a size limit pt over the grouped rows of d, on s: every part start flagged in pd.start, pd.part_cnt and
+// pd.doc_wave placed, or KA_ERR_LIMIT for the lowest row whose one-record document exceeds pt.L. Q rows, W > 0 waves.
+static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const WaveParts& pt, const KaWaveDocs& d, KaWaveDocParts& pd,
+                          ka_status* st) {
+    const size_t q = (size_t)Q;
+    const unsigned nblk = (unsigned)((Q + 255) / 256);
+    // S [Q + 1] u64, err and widest, J_0 [Q], first_pos [W + 1], part_cnt [nblk], doc_wave [Q], start [Q + 1]
+    const size_t o_meta = (q + 1) * 8, o_next = o_meta + 16, o_first = o_next + q * 4, o_cnt = o_first + ((size_t)W + 1) * 4,
+                 o_dw = o_cnt + (size_t)nblk * 4, o_start = o_dw + q * 4;
+    if (c->d_wv_part.reserve(o_start + q + 1)) return set_status(st, KA_ERR_CUDA);
+    char* base = static_cast<char*>(c->d_wv_part.p);
+    KaWaveParts pp{};
+    pp.d = d;
+    pp.room = std::min<int64_t>(pt.L - 28, (int64_t)1 << 62);   // S[i] + room never overflows
+    pp.S = reinterpret_cast<unsigned long long*>(base);
+    pp.err = reinterpret_cast<unsigned long long*>(base + o_meta);
+    pp.widest = pp.err + 1;
+    pp.next = reinterpret_cast<int32_t*>(base + o_next);
+    pp.first_pos = reinterpret_cast<int32_t*>(base + o_first);
+    pp.start = reinterpret_cast<uint8_t*>(base + o_start);
+    const unsigned long long meta0[2] = {~0ull, 0ull};
+    if (cudaMemcpyAsync(pp.err, meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
+    ka_wave_part_len_kernel<<<nblk, 256, 0, s>>>(pp);
+    ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, pp.S, nullptr);   // S[0] is rewritten next
+    ka_wave_part_prefix_kernel<<<nblk, 256, 0, s>>>(pp);
+    ka_wave_part_next_kernel<<<nblk, 256, 0, s>>>(pp);
+    c->launches += 4;
+    unsigned long long back[2];
+    int32_t M = 0;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(back, pp.err, sizeof(back), cudaMemcpyDeviceToHost, s) ||
+        cudaMemcpyAsync(&M, d.n_rows, 4, cudaMemcpyDeviceToHost, s) || cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    if (back[0] != ~0ull)
+        return set_status(st, KA_ERR_LIMIT, -1, -1, (int)(back[0] >> 32), (int)std::min<unsigned long long>(back[0] & 0xFFFFFFFFull, INT_MAX));
+    int K = 0;   // 2^K >= the most rows, so the most parts, of a wave
+    while ((1ull << K) < back[1]) ++K;
+    const unsigned mblk = (unsigned)((M + 255) / 256);
+    if (K > 1 && c->d_wv_jump.reserve((size_t)(K - 1) * M * 4)) return set_status(st, KA_ERR_CUDA);
+    auto level = [&](int k) { return k == 0 ? pp.next : c->d_wv_jump.as<int32_t>() + (size_t)(k - 1) * M; };
+    for (int k = 1; k < K; ++k) ka_wave_part_jump_kernel<<<mblk, 256, 0, s>>>(level(k - 1), level(k), (uint32_t)M);
+    for (int k = K - 1; k >= 0; --k) ka_wave_part_mark_kernel<<<mblk, 256, 0, s>>>(level(k), pp.start, (uint32_t)M);
+    c->launches += K > 0 ? 2 * K - 1 : 0;
+    pd.start = pp.start;
+    pd.part_cnt = reinterpret_cast<int*>(base + o_cnt);
+    pd.doc_wave = reinterpret_cast<int32_t*>(base + o_dw);
+    return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
+}
+
+// ka_plan_waves_json, with a sender part sd ka_plan_waves_send_json, and with a size limit pt their _parts forms.
 static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
                                const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
                                const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
                                int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
-                               int32_t summary_cap, const WaveSend* sd, ka_status* st) {
+                               int32_t summary_cap, const WaveSend* sd, const WaveParts* pt, ka_status* st) {
     if (!st) return KA_ERR_BAD_ARG;
     if (n_waves) *n_waves = 0;
+    if (pt && pt->n_docs) *pt->n_docs = 0;
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     if (T < 0 || (T > 0 && !part_off)) return set_status(st, KA_ERR_BAD_ARG);   // no Q to check
     const int64_t Q = T > 0 ? part_off[T] : 0;
@@ -2656,6 +2715,7 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     }
     if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
     if (sd && (rc = wave_send_args(*sd, summary_cap, st)) != KA_OK) return rc;
+    if (pt && (pt->L < 1 || (Q > 0 && (!pt->doc_wave || !pt->n_docs)))) return set_status(st, KA_ERR_BAD_ARG);
     if (doc_off) doc_off[0] = 0;
     if (Q == 0) return set_status(st, KA_OK);
     if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
@@ -2672,7 +2732,7 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     const size_t tiles = (size_t)(Q + KA_WAVE_SORT_MIN_TILE - 1) / KA_WAVE_SORT_MIN_TILE;   // at least the passes' tiles
     if (c->d_part_off.reserve((size_t)(T + 1) * 8) || c->d_json.reserve((size_t)std::max<int64_t>(cap, 1)) ||
         c->d_json_rowlen.reserve(q * 4) || c->d_json_blocksum.reserve((size_t)nblk * 8) || c->d_wv_perm.reserve(2 * q * 4) ||
-        c->d_wv_hist.reserve((2 * KA_WAVE_SORT_DIGITS * tiles + 1) * 4) || c->d_wv_doc.reserve(((size_t)W + 2) * 8) ||
+        c->d_wv_hist.reserve((2 * KA_WAVE_SORT_DIGITS * tiles + 1) * 4) || c->d_wv_doc.reserve((pt ? q + 3 : (size_t)W + 2) * 8) ||
         upload_names(c, s, T, Q, names, name_off, part_id) != KA_OK ||
         cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s))
         return set_status(st, KA_ERR_CUDA);
@@ -2683,19 +2743,32 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     d.wave = c->d_wv_wave.as<int32_t>();
     d.blockoff = c->d_json_blocksum.as<unsigned long long>();
     unsigned long long* d_total = c->d_wv_doc.as<unsigned long long>();
-    d.doc_off = d_total + 1;
-    ka_wave_doc_len_kernel<<<nblk, 256, 0, s>>>(d);
-    ka_wave_doc_scan_kernel<<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total);
-    if (enq_json_write(ka_wave_doc_write_kernel, nblk, s, d, d_total) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    d.doc_off = d_total + (pt ? 2 : 1);
+    KaWaveDocParts pd{};
+    if (!pt) {
+        ka_wave_doc_len_kernel<false><<<nblk, 256, 0, s>>>(d, pd);
+        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total, nullptr);
+        if (enq_json_write(ka_wave_doc_write_kernel<false>, nblk, s, d, d_total, pd) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    } else {
+        if ((rc = enq_wave_parts(c, s, Q, W, *pt, d, pd, st)) != KA_OK) return rc;
+        ka_wave_doc_len_kernel<true><<<nblk, 256, 0, s>>>(d, pd);
+        ka_wave_doc_scan_kernel<true><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total, pd.part_cnt);
+        if (enq_json_write(ka_wave_doc_write_kernel<true>, nblk, s, d, d_total, pd) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    }
     c->launches += 3;
-    unsigned long long total = 0;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&total, d_total, 8, cudaMemcpyDeviceToHost, s) || cudaStreamSynchronize(s))
+    unsigned long long total[2] = {0, (unsigned long long)W};   // the text's bytes and the documents D
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(total, d_total, pt ? 16 : 8, cudaMemcpyDeviceToHost, s) ||
+        cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
-    if (total > (unsigned long long)json_cap) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
-    if (cudaMemcpyAsync(json, c->d_json.p, (size_t)total, cudaMemcpyDeviceToHost, s) ||
-        cudaMemcpyAsync(doc_off, d.doc_off, ((size_t)W + 1) * 8, cudaMemcpyDeviceToHost, s))
+    if (total[0] > (unsigned long long)json_cap) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
+    const size_t D = (size_t)total[1];
+    if (cudaMemcpyAsync(json, c->d_json.p, (size_t)total[0], cudaMemcpyDeviceToHost, s) ||
+        cudaMemcpyAsync(doc_off, d.doc_off, (D + 1) * 8, cudaMemcpyDeviceToHost, s) ||
+        (pt && cudaMemcpyAsync(pt->doc_wave, pd.doc_wave, D * 4, cudaMemcpyDeviceToHost, s)))
         return set_status(st, KA_ERR_CUDA);
-    return wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, sd, st);
+    if ((rc = wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, sd, st)) != KA_OK) return rc;
+    if (pt) *pt->n_docs = (int32_t)D;
+    return KA_OK;
 }
 
 int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
@@ -2704,7 +2777,7 @@ int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const 
                            int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
                            int32_t summary_cap, ka_status* st) {
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, st);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, nullptr, st);
 }
 
 int32_t ka_plan_waves_send_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
@@ -2715,7 +2788,31 @@ int32_t ka_plan_waves_send_json(ka_ctx* c, int32_t T, const int64_t* part_off, c
                                 ka_wave_send_summary* send_summary, int32_t summary_cap, ka_status* st) {
     const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, st);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, nullptr, st);
+}
+
+int32_t ka_plan_waves_json_parts(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
+                                 const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
+                                 const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off,
+                                 char* json, int64_t json_cap, int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave,
+                                 int32_t* n_docs, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap,
+                                 ka_status* st) {
+    const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
+    return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, &pt, st);
+}
+
+int32_t ka_plan_waves_send_json_parts(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
+                                      const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
+                                      const int64_t* part_weight, int64_t max_broker_in, int32_t n_send, const int32_t* send_id,
+                                      int64_t max_broker_out, const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                      int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave, int32_t* n_docs, int32_t* wave,
+                                      int32_t* n_waves, ka_wave_summary* summary, ka_wave_send_summary* send_summary,
+                                      int32_t summary_cap, ka_status* st) {
+    const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
+    const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
+    return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, st);
 }
 
 }  // extern "C"

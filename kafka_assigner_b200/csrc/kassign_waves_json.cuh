@@ -15,6 +15,22 @@
 //   ka_wave_doc_scan_kernel      ONE CTA: 64-bit text offsets of the CTAs, and the total
 //   ka_wave_doc_write_kernel     the text (through the JSON passes' shared-memory stage) and doc_off[0..W]
 //
+// A size limit L (ka_plan_waves_json_parts) cuts every wave into PARTS, runs of consecutive grouped rows, greedily: a row joins
+// its wave's current part while that part's document stays <= L. With c_i = a record's bytes + 1 (its comma) and S the 64-bit
+// exclusive prefix of c over the grouped positions, positions i..j-1 of one wave make a document of S[j] - S[i] + 28 bytes.
+//
+//   ka_wave_part_len_kernel      c_i, per-CTA sums, the first position of every wave, the wave starts as part starts
+//   ka_wave_doc_scan_kernel      ONE CTA: the CTA sums to offsets
+//   ka_wave_part_prefix_kernel   S[0..M]
+//   ka_wave_part_next_kernel     J_0[i] = where a part opened at i ends (binary search over S within the wave; M = the wave's
+//                                end); a record that alone exceeds L reports its row; the most rows of a wave
+//   ka_wave_part_jump_kernel     J_k = J_{k-1} o J_{k-1}, k = 1 .. K-1, with 2^K >= the most rows of a wave
+//   ka_wave_part_mark_kernel     k = K-1 .. 0: every part start i marks J_k[i]. Starting from the wave starts, level k adds the
+//                                starts 2^k parts further on, so after level 0 every start is marked. A mark only ever sets a
+//                                start, and every start is set by some level: the flags do not depend on the order of stores.
+// The text passes then run with PARTS = true: the frame goes at part boundaries and doc_off is indexed by part. They add the
+// parts starting in every CTA, and the scan numbers the parts (D, the parts of all waves).
+//
 // A pass ranks a row by counting, never by the order of atomics: the text depends on the input alone.
 #pragma once
 #include "kassign_json.cuh"
@@ -107,46 +123,77 @@ struct KaWaveDocs {
     const int32_t* perm;                 // [M]
     const int32_t* n_rows;               // M
     unsigned long long* blockoff;        // [ceil(Q / 256)] text bytes of every CTA, then (scan) its text offset
-    unsigned long long* doc_off;         // [W + 1] out
+    unsigned long long* doc_off;         // [W + 1] out, with PARTS [D + 1]
+};
+
+// What the text passes read and write only with PARTS = true, which places the frame at part boundaries instead of wave
+// boundaries. A separate (last) kernel argument, so that the PARTS = false instances keep the parameter layout of KaWaveDocs.
+struct KaWaveDocParts {
+    const uint8_t* start;                // [M] 1 where a part starts
+    int* part_cnt;                       // [ceil(Q / 256)] parts starting in every CTA, then (scan) the parts before it
+    int32_t* doc_wave;                   // [D] out: the wave of every part
 };
 
 // Row, wave and place in its document of grouped position i.
-__device__ __forceinline__ void ka_wave_doc_row(const KaWaveDocs& d, uint32_t i, uint32_t M, uint32_t& g, int& v, bool& first, bool& last) {
+template <bool PARTS>
+__device__ __forceinline__ void ka_wave_doc_row(const KaWaveDocs& d, const KaWaveDocParts& pd, uint32_t i, uint32_t M, uint32_t& g, int& v,
+                                                bool& first, bool& last) {
     g = (uint32_t)d.perm[i];
     v = d.wave[g];
-    first = i == 0 || d.wave[d.perm[i - 1]] != v;
-    last = i + 1 == M || d.wave[d.perm[i + 1]] != v;
+    if constexpr (PARTS) {
+        first = pd.start[i];
+        last = i + 1 == M || pd.start[i + 1];
+    } else {
+        first = i == 0 || d.wave[d.perm[i - 1]] != v;
+        last = i + 1 == M || d.wave[d.perm[i + 1]] != v;
+    }
 }
 
 // grid ceil(Q / 256), 256 threads.
-__global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d) {
+template <bool PARTS>
+__global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d, const KaWaveDocParts pd) {
     const uint32_t M = (uint32_t)*d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     uint32_t n = 0;
+    bool opens = false;
     if (i < M) {
         uint32_t g;
         int v;
         bool first, last;
-        ka_wave_doc_row(d, i, M, g, v, first, last);
+        ka_wave_doc_row<PARTS>(d, pd, i, M, g, v, first, last);
         n = (first ? KA_JSON_HEAD_LEN : 0u) + ka_json_row_len(d.p, g, !first) + (last ? KA_JSON_TAIL_LEN : 0u);
         d.p.rowlen[i] = n;
+        opens = first;
     }
     const unsigned long long bytes = ka_cta256_sum(n);
     if (threadIdx.x == 0) d.blockoff[blockIdx.x] = bytes;
+    if constexpr (PARTS) {
+        const int parts = __syncthreads_count(opens);
+        if (threadIdx.x == 0) pd.part_cnt[blockIdx.x] = parts;
+    }
 }
 
 // ONE CTA of 1024: v[0..n) to its exclusive scan in place, *total = the sum. 64-bit throughout: 8 bytes per 256 rows lift the
-// 4 GiB limit a fragment of ka_json_scan_kernel has.
-__global__ void __launch_bounds__(1024) ka_wave_doc_scan_kernel(unsigned long long* __restrict__ v, int n, unsigned long long* __restrict__ total) {
+// 4 GiB limit a fragment of ka_json_scan_kernel has. PARTS: cnt[0..n) likewise, total[1] = D.
+template <bool PARTS>
+__global__ void __launch_bounds__(1024) ka_wave_doc_scan_kernel(unsigned long long* __restrict__ v, int n, unsigned long long* __restrict__ total,
+                                                                int* __restrict__ cnt) {
     const unsigned long long bytes = ka_cta_scan(v, v, n, 0ull);
     if (threadIdx.x == 0) *total = bytes;
+    if constexpr (PARTS) {
+        const int parts = ka_cta_scan(cnt, cnt, n, 0);
+        if (threadIdx.x == 0) total[1] = (unsigned long long)parts;
+    }
 }
 
 // grid ceil(Q / 256), 256 threads, KA_JSON_SMEM_BYTES + 16 of dynamic shared memory. Every grouped row writes its text at its
 // final position, the 256 rows of a CTA through the shared-memory stage of the JSON passes. The frame travels with the rows,
 // so a CTA that spans many waves is staged like any other. The first row of wave v writes doc_off[v - 1], the last row of all
-// doc_off[W]. Nothing is written when the text exceeds p.cap.
-__global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs d, const unsigned long long* __restrict__ total) {
+// doc_off[W]; PARTS: the first row of part r writes doc_off[r] and doc_wave[r], the last row of all doc_off[D]. Nothing is
+// written when the text exceeds p.cap.
+template <bool PARTS>
+__global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs d, const unsigned long long* __restrict__ total,
+                                                                const KaWaveDocParts pd) {
     extern __shared__ __align__(16) unsigned char ka_jsmem[];
     const uint32_t M = (uint32_t)*d.n_rows;
     if (*total > d.p.cap || blockIdx.x * 256u >= M) return;   // CTA-uniform
@@ -154,6 +201,15 @@ __global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs
     const uint32_t n = i < M ? d.p.rowlen[i] : 0u;
     uint32_t bt;
     const uint32_t loc = ka_cta256_prefix(n, bt);           // my row inside the CTA's text
+    uint32_t part = 0;                                      // PARTS: my part, when I open one
+    if constexpr (PARTS) {
+        __shared__ int wparts[8];
+        const unsigned opens = __ballot_sync(KA_FULL, i < M && pd.start[i]);
+        if ((threadIdx.x & 31) == 0) wparts[threadIdx.x >> 5] = __popc(opens);
+        __syncthreads();
+        part = (uint32_t)pd.part_cnt[blockIdx.x] + __popc(opens & ka_lanemask_lt());
+        for (int w = 0; w < (int)(threadIdx.x >> 5); ++w) part += wparts[w];
+    }
     const unsigned long long at = d.blockoff[blockIdx.x];   // this CTA's text
     char* dst = d.p.json + at;
     const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(dst) & 15u);
@@ -163,15 +219,110 @@ __global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs
         uint32_t g;
         int v;
         bool first, last;
-        ka_wave_doc_row(d, i, M, g, v, first, last);
+        ka_wave_doc_row<PARTS>(d, pd, i, M, g, v, first, last);
         char* w = (staged ? stage : dst) + loc;
         if (first) {
             w = ka_put_str(w, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
-            d.doc_off[v - 1] = at + loc;
+            if constexpr (PARTS) {
+                d.doc_off[part] = at + loc;
+                pd.doc_wave[part] = v;
+            } else {
+                d.doc_off[v - 1] = at + loc;
+            }
         }
         w = ka_json_row_put(d.p, g, w, !first);
         if (last) ka_put_str(w, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
-        if (i + 1 == M) d.doc_off[v] = at + loc + n;
+        if (i + 1 == M) {
+            if constexpr (PARTS) d.doc_off[total[1]] = at + loc + n;
+            else d.doc_off[v] = at + loc + n;
+        }
     }
     if (staged) ka_json_store_staged(dst, stage, bt);
+}
+
+// The part passes of a size limit, over the grouped positions of d (d.p.rowlen holds c_i, d.blockoff their CTA sums and then
+// offsets). Positions i..j-1 of one wave make one part iff S[j] - S[i] <= room = L - 28.
+struct KaWaveParts {
+    KaWaveDocs d;
+    long long room;
+    unsigned long long* S;          // [M + 1]
+    int32_t* first_pos;             // [W + 1] first position of every wave, M at W
+    int32_t* next;                  // [M] J_0
+    uint8_t* start;                 // [M] 1 at the wave starts (then, by the mark passes, at every part start)
+    unsigned long long* err;        // (row << 32) | its one-record document's bytes (clipped), of the lowest row that exceeds L
+    unsigned long long* widest;     // the most rows of a wave
+};
+
+// grid ceil(Q / 256), 256 threads.
+__global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts pp) {
+    const KaWaveDocs& d = pp.d;
+    const uint32_t M = (uint32_t)*d.n_rows;
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    uint32_t c = 0;
+    if (i < M) {
+        uint32_t g;
+        int v;
+        bool first, last;
+        ka_wave_doc_row<false>(d, KaWaveDocParts{}, i, M, g, v, first, last);
+        c = ka_json_row_len(d.p, g, true);   // the record and its comma
+        d.p.rowlen[i] = c;
+        pp.start[i] = first;
+        if (first) pp.first_pos[v - 1] = (int32_t)i;
+        if (i + 1 == M) pp.first_pos[v] = (int32_t)M;
+    }
+    const unsigned long long bytes = ka_cta256_sum(c);
+    if (threadIdx.x == 0) d.blockoff[blockIdx.x] = bytes;
+}
+
+// grid ceil(Q / 256), 256 threads: S[i] = the CTA's offset + the in-CTA prefix; the last position also writes S[M].
+__global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWaveParts pp) {
+    const uint32_t M = (uint32_t)*pp.d.n_rows;
+    if (blockIdx.x * 256u >= M) return;   // CTA-uniform
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    const uint32_t c = i < M ? pp.d.p.rowlen[i] : 0u;
+    uint32_t bt;
+    const unsigned long long s = pp.d.blockoff[blockIdx.x] + ka_cta256_prefix(c, bt);
+    if (i < M) pp.S[i] = s;
+    if (i + 1 == M) pp.S[M] = s + c;
+}
+
+// grid ceil(Q / 256), 256 threads: J_0[i] = the last j in (i, e] with S[j] - S[i] <= room, e the end of i's wave, and M in
+// place of e. A position whose own record does not fit reports its ROW, so the lowest input row wins.
+__global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWaveParts pp) {
+    const uint32_t M = (uint32_t)*pp.d.n_rows;
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    if (i >= M) return;
+    const uint32_t g = (uint32_t)pp.d.perm[i];
+    const int v = pp.d.wave[g];
+    const uint32_t e = (uint32_t)pp.first_pos[v];
+    if (pp.start[i]) atomicMax(pp.widest, (unsigned long long)(e - i));
+    const long long lim = (long long)pp.S[i] + pp.room;
+    if ((long long)pp.S[i + 1] > lim) {
+        const unsigned long long bytes = min(28ull + (pp.S[i + 1] - pp.S[i]), 0xFFFFFFFFull);
+        atomicMin(pp.err, (unsigned long long)g << 32 | bytes);
+        return;
+    }
+    uint32_t lo = i + 1, hi = e;   // S[lo] <= lim
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if ((long long)pp.S[mid] <= lim) lo = mid; else hi = mid - 1;
+    }
+    pp.next[i] = (int32_t)(lo == e ? M : lo);
+}
+
+// grid ceil(M / 256), 256 threads: J_k from J_{k-1}; M stays M.
+__global__ void __launch_bounds__(256) ka_wave_part_jump_kernel(const int32_t* __restrict__ J, int32_t* __restrict__ J2, uint32_t M) {
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    if (i >= M) return;
+    const int32_t j = J[i];
+    J2[i] = (uint32_t)j == M ? j : J[j];
+}
+
+// grid ceil(M / 256), 256 threads: one level of the top-down marking. A start read here may have been set in this same pass;
+// its image is a start all the same.
+__global__ void __launch_bounds__(256) ka_wave_part_mark_kernel(const int32_t* __restrict__ J, uint8_t* start, uint32_t M) {
+    const uint32_t i = blockIdx.x * 256u + threadIdx.x;
+    if (i >= M || !start[i]) return;
+    const int32_t j = J[i];
+    if ((uint32_t)j != M) start[j] = 1;
 }

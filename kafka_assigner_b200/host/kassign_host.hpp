@@ -16,6 +16,8 @@
 //   kassign::scoreClusters                            <->  the same fleet, reduced on the device to what each cluster would move
 //                                                          and how evenly it spreads replicas and leaders
 //   kassign::planWavesJson                            <->  planWaves with every wave's document built on the device
+//   kassign::planWaveParts                            <->  planWavesJson with every wave cut into documents of at most a
+//                                                          size limit (ZooKeeper's znode limit), cut on the device
 //   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
 //                                                          receives more than a budget, one document per wave
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
@@ -314,9 +316,35 @@ public:
         return planWavesJsonWith(topics, proposed, maxBrokerIn, &send, weights);
     }
 
+    // planWavesJson with every wave cut into parts of at most maxDocBytes bytes (ka_plan_waves_json_parts): documents that run
+    // one after the other, each small enough for the znode Kafka 0.10 writes it into (maxDocBytes = 1048575 under ZooKeeper's
+    // default jute.maxbuffer). The cut is greedy: a wave's first partition opens a part, and each next partition of the wave
+    // joins the current part while its document stays <= maxDocBytes, else it opens a new part. parts are in (wave, place in
+    // the wave) order, partWave[d] the wave (1..W) of parts[d]; with maxDocBytes >= the longest wave document, parts equals
+    // planWavesJson(...).docs. A partition whose one-record document exceeds maxDocBytes gives KA_ERR_LIMIT with a = its row
+    // and b = that length. Topic names that org.json would escape take the host emitter and the same cut on the host.
+    struct WaveParts {
+        ka_status status;   // re-throw with throwForStatus; on an error summary, parts and partWave are empty
+        std::vector<ka_wave_summary> summary;
+        std::vector<std::string> parts;
+        std::vector<int32_t> partWave;
+        std::vector<ka_wave_send_summary> sendSummary;   // with a SendBudget: beside summary, one per wave
+    };
+    WaveParts planWaveParts(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                            int64_t maxDocBytes, const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavePartsWith(topics, proposed, maxBrokerIn, maxDocBytes, nullptr, weights);
+    }
+    // planWaveParts under a sender budget too (ka_plan_waves_send_json_parts); sendSummary is filled.
+    WaveParts planWaveParts(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                            int64_t maxDocBytes, const SendBudget& send, const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavePartsWith(topics, proposed, maxBrokerIn, maxDocBytes, &send, weights);
+    }
+
 private:
+    // rowWave (when given) receives every row's wave, in the row order of flatten(topics).
     WavePlan planWavesWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
-                           const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights) {
+                           const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights,
+                           std::vector<int32_t>* rowWave = nullptr) {
         const Flat f = flatten(topics, -1);
         const ProposedRows p = proposedRows(topics, proposed, weights);
         const size_t Q = f.partId.size();
@@ -343,6 +371,7 @@ private:
         if (res.status.code != KA_OK) return WavePlan{res.status, {}, {}, {}};
         res.summary.resize(W);
         if (send) res.sendSummary.resize(W);
+        if (rowWave) *rowWave = wave;
         res.waves.resize(W);
         std::vector<size_t> lastTopic(W, topics.size());   // the topic of each wave's last TopicOutput
         for (size_t t = 0; t < topics.size(); ++t)
@@ -360,6 +389,8 @@ private:
     }
     WaveDocs planWavesJsonWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                                const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
+    WaveParts planWavePartsWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                                int64_t maxDocBytes, const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
 
 public:
 
@@ -389,6 +420,17 @@ private:
         std::vector<int32_t> newLen, newBroker;
         std::vector<int64_t> w;
     };
+    // The name slab of f for the wave document calls (names, nameOff [T+1]); returns the json_cap kassign.h documents as
+    // sufficient: per row 79 + 12·stride + its topic's name length.
+    static int64_t waveNames(const Flat& f, int stride, std::string& names, std::vector<int64_t>& nameOff) {
+        int64_t cap = 0;
+        for (size_t t = 0; t < f.names.size(); ++t) {
+            names += f.names[t];
+            nameOff.push_back((int64_t)names.size());
+            cap += (f.partOff[t + 1] - f.partOff[t]) * (79 + 12 * (int64_t)stride + (int64_t)f.names[t].size());
+        }
+        return cap;
+    }
     static ProposedRows proposedRows(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
                                      const std::vector<std::map<int, int64_t>>& weights) {
         if (proposed.size() != topics.size()) throw std::invalid_argument("one proposed topic per topic");
@@ -593,6 +635,19 @@ inline void appendQuoted(std::string& s, const std::string& v) {
 // Key order of org.json 20131018 objects == java.util.HashMap iteration order of the keys (SURVEY §3.4; predicted for
 // JDK >= 8, unverified without a JVM — isolated here so it can be corrected in one place):
 //   top level: "partitions" (bucket 0) before "version" (13); per record: "partition" (3), "replicas" (6), "topic" (9).
+inline void appendRecord(std::string& s, const std::string& topic, int partition, const int* replicas, size_t n) {
+    s += "{\"partition\":";
+    appendInt(s, partition);
+    s += ",\"replicas\":[";
+    for (size_t i = 0; i < n; ++i) {
+        if (i) s.push_back(',');
+        appendInt(s, replicas[i]);
+    }
+    s += "],\"topic\":";
+    appendQuoted(s, topic);
+    s.push_back('}');
+}
+
 inline std::string newAssignmentJson(const std::vector<TopicOutput>& topics) {
     std::string s = "{\"partitions\":[";
     bool first = true;
@@ -600,16 +655,7 @@ inline std::string newAssignmentJson(const std::vector<TopicOutput>& topics) {
         for (const auto& e : t.assignment) {  // ascending partition, topics in loop order (KAG:173-183)
             if (!first) s.push_back(',');
             first = false;
-            s += "{\"partition\":";
-            appendInt(s, e.first);
-            s += ",\"replicas\":[";
-            for (size_t i = 0; i < e.second.size(); ++i) {
-                if (i) s.push_back(',');
-                appendInt(s, e.second[i]);
-            }
-            s += "],\"topic\":";
-            appendQuoted(s, t.name);
-            s.push_back('}');
+            appendRecord(s, t.name, e.first, e.second.data(), e.second.size());
         }
     s += "],\"version\":1}";  // KAFKA_FORMAT_VERSION (KAG:49)
     return s;
@@ -671,12 +717,7 @@ inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJsonWith(const 
     const size_t Q = f.partId.size();
     std::string names;
     std::vector<int64_t> nameOff(1, 0);
-    int64_t cap = 0;   // documented in kassign.h: per row 79 + 12·stride + its topic's name length
-    for (size_t t = 0; t < f.names.size(); ++t) {
-        names += f.names[t];
-        nameOff.push_back((int64_t)names.size());
-        cap += (f.partOff[t + 1] - f.partOff[t]) * (79 + 12 * (int64_t)p.stride + (int64_t)f.names[t].size());
-    }
+    const int64_t cap = waveNames(f, p.stride, names, nameOff);
     std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
     std::vector<int64_t> docOff(Q + 1, 0);
     WaveDocs res{};
@@ -699,6 +740,82 @@ inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJsonWith(const 
     res.summary.resize(W);
     if (send) res.sendSummary.resize(W);
     for (int32_t v = 0; v < W; ++v) res.docs.emplace_back(json.get() + docOff[v], (size_t)(docOff[v + 1] - docOff[v]));
+    return res;
+}
+
+inline KafkaTopicAssigner::WaveParts KafkaTopicAssigner::planWavePartsWith(const std::vector<TopicInput>& topics,
+                                                                           const std::vector<TopicOutput>& proposed,
+                                                                           int64_t maxBrokerIn, int64_t maxDocBytes,
+                                                                           const SendBudget* send,
+                                                                           const std::vector<std::map<int, int64_t>>& weights) {
+    const Flat f = flatten(topics, -1);
+    const ProposedRows p = proposedRows(topics, proposed, weights);
+    const size_t Q = f.partId.size();
+    for (const auto& t : topics)
+        if (needsJsonEscape(t.name)) {   // the host emitter over the rows of planWaves, cut by the rule of planWaveParts
+            std::vector<int32_t> rowWave;
+            const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights, &rowWave);
+            WaveParts res{plan.status, plan.summary, {}, {}, plan.sendSummary};
+            if (res.status.code == KA_OK && maxDocBytes < 1) res.status.code = KA_ERR_BAD_ARG;
+            if (res.status.code != KA_OK) return WaveParts{res.status, {}, {}, {}, {}};
+            std::vector<std::vector<std::string>> recs(plan.summary.size());
+            for (size_t t = 0; t < f.names.size(); ++t)
+                for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
+                    if (rowWave[r] == 0) continue;
+                    std::string rec;
+                    appendRecord(rec, f.names[t], f.partId[r], p.newBroker.data() + r * p.stride, (size_t)p.newLen[r]);
+                    if (29 + (int64_t)rec.size() > maxDocBytes) {
+                        ka_status st{};
+                        st.code = KA_ERR_LIMIT;
+                        st.a = (int32_t)r;
+                        st.b = (int32_t)std::min<int64_t>(29 + (int64_t)rec.size(), INT32_MAX);
+                        return WaveParts{st, {}, {}, {}, {}};
+                    }
+                    recs[rowWave[r] - 1].push_back(std::move(rec));
+                }
+            for (size_t v = 0; v < recs.size(); ++v) {
+                int64_t size = 0;   // of the current part, 0 before the wave's first
+                for (const std::string& rec : recs[v]) {
+                    if (size > 0 && size + 1 + (int64_t)rec.size() <= maxDocBytes) {
+                        res.parts.back().insert(res.parts.back().size() - 14, "," + rec);
+                        size += 1 + (int64_t)rec.size();
+                    } else {
+                        res.parts.push_back("{\"partitions\":[" + rec + "],\"version\":1}");
+                        res.partWave.push_back((int32_t)v + 1);
+                        size = 29 + (int64_t)rec.size();
+                    }
+                }
+            }
+            return res;
+        }
+    std::string names;
+    std::vector<int64_t> nameOff(1, 0);
+    const int64_t cap = waveNames(f, p.stride, names, nameOff);
+    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
+    std::vector<int64_t> docOff(Q + 1, 0);
+    std::vector<int32_t> docWave(std::max<size_t>(Q, 1), 0);
+    WaveParts res{};
+    res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
+    int32_t W = 0, D = 0;
+    const int64_t* w = p.w.empty() ? nullptr : p.w.data();
+    if (!send) {
+        ka_plan_waves_json_parts(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
+                                 p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, names.data(), nameOff.data(),
+                                 json.get(), cap, maxDocBytes, docOff.data(), docWave.data(), &D, nullptr, &W, res.summary.data(),
+                                 (int32_t)res.summary.size(), &res.status);
+    } else {
+        res.sendSummary.resize(res.summary.size());
+        ka_plan_waves_send_json_parts(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
+                                      p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, (int32_t)send->sendBrokers.size(),
+                                      send->sendBrokers.data(), send->maxBrokerOut, names.data(), nameOff.data(), json.get(), cap,
+                                      maxDocBytes, docOff.data(), docWave.data(), &D, nullptr, &W, res.summary.data(),
+                                      res.sendSummary.data(), (int32_t)res.summary.size(), &res.status);
+    }
+    if (res.status.code != KA_OK) return WaveParts{res.status, {}, {}, {}, {}};
+    res.summary.resize(W);
+    if (send) res.sendSummary.resize(W);
+    for (int32_t d = 0; d < D; ++d) res.parts.emplace_back(json.get() + docOff[d], (size_t)(docOff[d + 1] - docOff[d]));
+    res.partWave.assign(docWave.begin(), docWave.begin() + D);
     return res;
 }
 
