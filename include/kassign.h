@@ -496,6 +496,63 @@ int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* par
                                       int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
                                       ka_wave_send_summary* send_summary, int32_t summary_cap, ka_status* st);
 
+/* ka_plan_waves_json_parts with every part's ROLLBACK document beside it: the document that puts exactly that part's partitions
+ * back on their current lists, as kafka-reassign-partitions and the reference tool print them "in case a rollback is needed".
+ * If part d stalls, rollback document d undoes it, however far the other parts have run: every changed row is in exactly one
+ * part.
+ *   T .. n_docs        exactly as ka_plan_waves_json_parts takes them
+ *   back[back_cap]     host, required: the rollback text
+ *   back_off[Q+1]      host, required when Q > 0; entries 0..D are written, back_off[0] = 0: rollback document d is
+ *                      back[back_off[d] .. back_off[d+1]), back to back and not NUL-terminated
+ *   wave .. summary_cap   exactly as ka_plan_waves_json_parts writes them
+ * The rollback record of a changed row g is exactly the record the host's CURRENT ASSIGNMENT prints for that partition (Kafka
+ * 0.10's ZkUtils.formatAsReassignmentJson key order): {"topic":"<name>","partition":<id>,"replicas":[<list>]}, the list being
+ * cur_broker[rep_off[g] .. rep_off[g+1]) as given (duplicates, ids missing from the table and an empty list [] included); the
+ * partition id and topic name as in the forward record. It is 39 + name + partition digits + list bytes, like the forward
+ * record: the two differ only by the printed list. Rollback document d is {"version":1,"partitions":[ + the rollback records
+ * of part d's rows, in part d's order, comma separated, + ]}: a 29-byte frame, like the forward one.
+ * The paired cut: the greedy cut of ka_plan_waves_json_parts with one more condition, a row joins the current part only if BOTH
+ * the part's document and its rollback document stay <= L. With S and R the exclusive prefixes of (record + comma) and
+ * (rollback record + comma) over a wave's rows, rows i..j-1 make a part iff S[j] - S[i] <= L - 28 and R[j] - R[i] <= L - 28.
+ * Both conditions are monotone in j, so the parts are unique and no two consecutive parts of a wave could be merged within L
+ * on both sides. When no changed row's current list prints longer than its new list, the cut, json, doc_off and doc_wave are
+ * exactly those of ka_plan_waves_json_parts; it differs where the rollback side is longer (a replication-factor reduction, a
+ * move to shorter broker ids). With L >= the longest wave document on both sides, D = W and json is that of
+ * ka_plan_waves_json. The plan, W, wave and the summaries are those of ka_plan_waves.
+ * Sufficient back_cap: the sum over rows of (79 + the name length of the row's topic), + 12 x rep_off[Q]. json_cap as before.
+ * Checks, in this order: everything ka_plan_waves_json_parts checks, in its order; then back NULL, back_cap < 0, or back_off
+ * NULL with Q > 0: KA_ERR_BAD_ARG. On the device: the plan's row errors; a changed row with 29 + max(record, rollback record)
+ * > L: KA_ERR_LIMIT, a = the lowest such row (input order), b = that length clipped to INT_MAX; a text above json_cap:
+ * KA_ERR_LIMIT, a = min(json_cap, INT_MAX); a rollback text above back_cap: KA_ERR_LIMIT, a = min(back_cap, INT_MAX). On any
+ * error *n_waves = *n_docs = 0 (when given). W == 0 gives D = 0 and back_off[0] = 0.
+ * Synchronous. The launches of ka_plan_waves_json_parts on the same inputs, and, when W > 0, 3 more (the rollback text's
+ * length, scan and write passes; the part passes carry the rollback side without a launch of their own). Does not read or
+ * change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
+int32_t ka_plan_waves_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                          const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                                          const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
+                                          const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                          int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave, int32_t* n_docs, char* back,
+                                          int64_t back_cap, int64_t* back_off, int32_t* wave, int32_t* n_waves,
+                                          ka_wave_summary* summary, int32_t summary_cap, ka_status* st);
+
+/* ka_plan_waves_json_parts_rollback under the rule of ka_plan_waves_send: ka_plan_waves_send_json_parts with the rollback
+ * documents.
+ *   T .. n_docs        exactly as ka_plan_waves_send_json_parts takes them
+ *   back .. back_off   exactly as ka_plan_waves_json_parts_rollback takes and writes them
+ *   wave .. summary_cap   exactly as ka_plan_waves_send_json_parts writes them
+ * Checks: everything ka_plan_waves_send_json_parts checks, in its order; then those ka_plan_waves_json_parts_rollback adds, in
+ * its order. The launches of ka_plan_waves_send_json_parts, and the 3 ka_plan_waves_json_parts_rollback adds. */
+int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                               const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                                               const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                                               int64_t max_broker_in, int32_t n_send, const int32_t* send_id, int64_t max_broker_out,
+                                               const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                               int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave, int32_t* n_docs,
+                                               char* back, int64_t back_cap, int64_t* back_off, int32_t* wave, int32_t* n_waves,
+                                               ka_wave_summary* summary, ka_wave_send_summary* send_summary, int32_t summary_cap,
+                                               ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

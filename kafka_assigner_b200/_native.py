@@ -66,6 +66,11 @@ SYMBOLS = {
                                         _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
     "ka_plan_waves_send_json_parts": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp, _vp,
                                              _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "ka_plan_waves_json_parts_rollback": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _i64, _i64,
+                                                 _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _i32, _vp]),
+    "ka_plan_waves_send_json_parts_rollback": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp,
+                                                      _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i32,
+                                                      _vp]),
     "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "ka_ctx_set_topic_base": (_i32, [_vp, _i32]),

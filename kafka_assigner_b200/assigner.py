@@ -551,8 +551,8 @@ class Solver:
         speed); by default one of the documented sufficient size. Returns (docs, wave, summary, KaStatus): docs a list of W
         bytes-like views of the buffer, docs[v] the document of wave v + 1; wave and summary as plan_waves returns them. On an
         error docs, wave and summary are empty. max_broker_out / send_brokers: ka_plan_waves_send_json, as in plan_waves."""
-        docs, _, wave, summary, st = self._wave_documents(topic_names, part_off, part_id, rep_off, cur_broker, out, out_len,
-                                                          max_broker_in, weight, json_buf, max_broker_out, send_brokers, None)
+        docs, _, _, wave, summary, st = self._wave_documents(topic_names, part_off, part_id, rep_off, cur_broker, out, out_len,
+                                                             max_broker_in, weight, json_buf, max_broker_out, send_brokers, None)
         return docs, wave, summary, st
 
     def plan_wave_parts_json(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, max_doc_bytes,
@@ -563,13 +563,27 @@ class Solver:
         wave (1..W) of each; the other arguments and results as plan_waves_json takes and returns them. On an error parts,
         part_wave, wave and summary are empty. With max_broker_in >= the sum of the weights every changed row is in wave 1: the
         whole reassignment under the limit."""
+        parts, _, part_wave, wave, summary, st = self._wave_documents(topic_names, part_off, part_id, rep_off, cur_broker, out,
+                                                                      out_len, max_broker_in, weight, json_buf, max_broker_out,
+                                                                      send_brokers, int(max_doc_bytes))
+        return parts, part_wave, wave, summary, st
+
+    def plan_wave_parts_rollback_json(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in,
+                                      max_doc_bytes, weight=None, json_buf=None, back_buf=None, max_broker_out=None, send_brokers=None):
+        """ka_plan_waves_json_parts_rollback: plan_wave_parts_json with every part's rollback document, the document that puts
+        exactly that part's partitions back on their current lists (cur_broker). A row joins a part only while both documents
+        stay <= max_doc_bytes. back_buf: optional writable uint8 numpy array for the rollback text; by default one of the
+        documented sufficient size. Returns (parts, rollback, part_wave, wave, summary, KaStatus): rollback[d] a bytes-like view
+        of back_buf, the rollback document of parts[d]; the rest as plan_wave_parts_json returns them. On an error every result
+        is empty."""
         return self._wave_documents(topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, weight,
-                                    json_buf, max_broker_out, send_brokers, int(max_doc_bytes))
+                                    json_buf, max_broker_out, send_brokers, int(max_doc_bytes), True, back_buf)
 
     def _wave_documents(self, topic_names, part_off, part_id, rep_off, cur_broker, out, out_len, max_broker_in, weight, json_buf,
-                        max_broker_out, send_brokers, max_doc_bytes):
-        """One call of the four wave document entry points: with max_doc_bytes None ka_plan_waves(_send)_json, else their
-        _parts forms. Returns (docs, doc_wave, wave, summary, KaStatus); doc_wave is 1..W without a limit."""
+                        max_broker_out, send_brokers, max_doc_bytes, rollback=False, back_buf=None):
+        """One call of the six wave document entry points: with max_doc_bytes None ka_plan_waves(_send)_json, else their
+        _parts forms, and with rollback their _parts_rollback forms. Returns (docs, backs, doc_wave, wave, summary, KaStatus);
+        doc_wave is 1..W without a limit, backs the rollback documents (None without rollback)."""
         out = np.ascontiguousarray(out, dtype=np.int32)
         Q = len(out)
         stride = out.shape[1] if out.ndim == 2 else 1
@@ -580,6 +594,8 @@ class Solver:
         names, name_off = self.marshal_names(topic_names)
         if json_buf is None:
             json_buf = np.empty(max(_wave_json_size(Q, r.name_bytes(np.diff(name_off)), stride), 1), dtype=np.uint8)
+        if rollback and back_buf is None:   # per row 79 + its topic's name, 12 per current broker
+            back_buf = np.empty(max(_wave_json_size(Q, r.name_bytes(np.diff(name_off)), 0) + 12 * len(r.cur_broker), 1), dtype=np.uint8)
         doc_off = np.zeros(Q + 1, dtype=np.int64)
         wave = np.zeros(Q, dtype=np.int32)
         n_waves = ctypes.c_int32(0)
@@ -596,9 +612,16 @@ class Solver:
         else:
             doc_wave = np.zeros(Q, dtype=np.int32)
             n_docs = ctypes.c_int32(0)
+            back = ()
+            if rollback:
+                back_off = np.zeros(Q + 1, dtype=np.int64)
+                back = (_ptr(back_buf), int(back_buf.size), _ptr(back_off))
             text = (_ptr(names), _ptr(name_off), _ptr(json_buf), int(json_buf.size), max_doc_bytes, _ptr(doc_off), _ptr(doc_wave),
-                    ctypes.byref(n_docs), _ptr(wave), ctypes.byref(n_waves), _ptr(summary))
-            entry = self._L.ka_plan_waves_json_parts if send is None else self._L.ka_plan_waves_send_json_parts
+                    ctypes.byref(n_docs), *back, _ptr(wave), ctypes.byref(n_waves), _ptr(summary))
+            if rollback:
+                entry = self._L.ka_plan_waves_json_parts_rollback if send is None else self._L.ka_plan_waves_send_json_parts_rollback
+            else:
+                entry = self._L.ka_plan_waves_json_parts if send is None else self._L.ka_plan_waves_send_json_parts
         if send is None:
             entry(*rows, *text, cap, ctypes.byref(st))
         else:
@@ -606,11 +629,12 @@ class Solver:
             entry(*rows, send[0], _ptr(send[1]), send[2], *text, _ptr(send_summary), cap, ctypes.byref(st))
         if st.code != 0:
             dtype = WAVE_SUMMARY_DTYPE if send is None else WAVE_SEND_SUMMARY_DTYPE
-            return [], np.zeros(0, dtype=np.int32), np.zeros(0, dtype=np.int32), np.zeros(0, dtype=dtype), st
+            return [], [] if rollback else None, np.zeros(0, dtype=np.int32), np.zeros(0, dtype=np.int32), np.zeros(0, dtype=dtype), st
         W = n_waves.value
         summary = summary[:W] if send is None else _with_send(summary[:W], send_summary[:W])
         D, doc_wave = (W, np.arange(1, W + 1, dtype=np.int32)) if max_doc_bytes is None else (n_docs.value, doc_wave[:n_docs.value])
-        return [json_buf[doc_off[d]:doc_off[d + 1]] for d in range(D)], doc_wave, wave, summary, st
+        backs = [back_buf[back_off[d]:back_off[d + 1]] for d in range(D)] if rollback else None
+        return [json_buf[doc_off[d]:doc_off[d + 1]] for d in range(D)], backs, doc_wave, wave, summary, st
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

@@ -159,6 +159,9 @@ struct ka_ctx {
     // scratch of a size limit (ka_plan_waves_json_parts): the prefix S, the meta words, J_0, the waves' first positions, the
     // parts per CTA, the parts' waves and the start flags; then the jump tables J_1 .. J_{K-1}
     DevBuf d_wv_part, d_wv_jump;
+    // scratch of the rollback documents (ka_plan_waves_json_parts_rollback): the text, then the rollback side's row bytes, CTA
+    // sums, prefix R, text total and back_off [D + 1]
+    DevBuf d_wv_back, d_wv_bscr;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -2642,10 +2645,18 @@ struct WaveParts {
     int32_t* n_docs;
 };
 
+// The rollback documents of ka_plan_waves_json_parts_rollback: the caller's text buffer, its size and back_off.
+struct WaveBack {
+    char* back;
+    int64_t cap;
+    int64_t* back_off;
+};
+
 // The part passes of a size limit pt over the grouped rows of d, on s: every part start flagged in pd.start, pd.part_cnt and
-// pd.doc_wave placed, or KA_ERR_LIMIT for the lowest row whose one-record document exceeds pt.L. Q rows, W > 0 waves.
+// pd.doc_wave placed, or KA_ERR_LIMIT for the lowest row whose one-record document exceeds pt.L. Q rows, W > 0 waves. With the
+// rollback side's bk (bk.R != null) the cut is the paired cut, and a row over-long on either side is the error.
 static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const WaveParts& pt, const KaWaveDocs& d, KaWaveDocParts& pd,
-                          ka_status* st) {
+                          const KaWaveBack& bk, ka_status* st) {
     const size_t q = (size_t)Q;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
     // S [Q + 1] u64, err and widest, J_0 [Q], first_pos [W + 1], part_cnt [nblk], doc_wave [Q], start [Q + 1]
@@ -2664,10 +2675,17 @@ static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const Wav
     pp.start = reinterpret_cast<uint8_t*>(base + o_start);
     const unsigned long long meta0[2] = {~0ull, 0ull};
     if (cudaMemcpyAsync(pp.err, meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
-    ka_wave_part_len_kernel<<<nblk, 256, 0, s>>>(pp);
-    ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, pp.S, nullptr);   // S[0] is rewritten next
-    ka_wave_part_prefix_kernel<<<nblk, 256, 0, s>>>(pp);
-    ka_wave_part_next_kernel<<<nblk, 256, 0, s>>>(pp);
+    if (!bk.R) {
+        ka_wave_part_len_kernel<false><<<nblk, 256, 0, s>>>(pp, bk);
+        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, pp.S, nullptr);   // S[0] is rewritten next
+        ka_wave_part_prefix_kernel<false><<<nblk, 256, 0, s>>>(pp, bk);
+        ka_wave_part_next_kernel<false><<<nblk, 256, 0, s>>>(pp, bk);
+    } else {
+        ka_wave_part_len_kernel<true><<<nblk, 256, 0, s>>>(pp, bk);
+        ka_wave_part_scan2_kernel<<<1, 1024, 0, s>>>(d.blockoff, bk.blockoff, (int)nblk);
+        ka_wave_part_prefix_kernel<true><<<nblk, 256, 0, s>>>(pp, bk);
+        ka_wave_part_next_kernel<true><<<nblk, 256, 0, s>>>(pp, bk);
+    }
     c->launches += 4;
     unsigned long long back[2];
     int32_t M = 0;
@@ -2690,12 +2708,14 @@ static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const Wav
     return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
 }
 
-// ka_plan_waves_json, with a sender part sd ka_plan_waves_send_json, and with a size limit pt their _parts forms.
+// ka_plan_waves_json, with a sender part sd ka_plan_waves_send_json, with a size limit pt their _parts forms, and with the
+// rollback documents bk (only with pt) the _parts_rollback forms.
 static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
                                const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
                                const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
                                int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
-                               int32_t summary_cap, const WaveSend* sd, const WaveParts* pt, ka_status* st) {
+                               int32_t summary_cap, const WaveSend* sd, const WaveParts* pt, ka_status* st,
+                               const WaveBack* bk = nullptr) {
     if (!st) return KA_ERR_BAD_ARG;
     if (n_waves) *n_waves = 0;
     if (pt && pt->n_docs) *pt->n_docs = 0;
@@ -2709,14 +2729,18 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     if ((T > 0 && (part_off[0] != 0 || !names || !name_off)) || !json || json_cap < 0 || (Q > 0 && !doc_off))
         return set_status(st, KA_ERR_BAD_ARG);
     int64_t bound = 0;   // the sufficient size: per row 79 + 12 x stride + its topic's name
+    int64_t back_bound = 12 * R;   // of the rollback text: per row 79 + its topic's name, 12 per current broker
     for (int t = 0; t < T; ++t) {
         if (part_off[t + 1] < part_off[t]) return set_status(st, KA_ERR_BAD_ARG);
         bound += (part_off[t + 1] - part_off[t]) * (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + 50 + 12 * (int64_t)stride + name_off[t + 1] - name_off[t]);
+        back_bound += (part_off[t + 1] - part_off[t]) * (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + 50 + name_off[t + 1] - name_off[t]);
     }
     if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
     if (sd && (rc = wave_send_args(*sd, summary_cap, st)) != KA_OK) return rc;
     if (pt && (pt->L < 1 || (Q > 0 && (!pt->doc_wave || !pt->n_docs)))) return set_status(st, KA_ERR_BAD_ARG);
+    if (bk && (!bk->back || bk->cap < 0 || (Q > 0 && !bk->back_off))) return set_status(st, KA_ERR_BAD_ARG);
     if (doc_off) doc_off[0] = 0;
+    if (bk && bk->back_off) bk->back_off[0] = 0;
     if (Q == 0) return set_status(st, KA_OK);
     if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
     int W = 0;
@@ -2745,26 +2769,61 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     unsigned long long* d_total = c->d_wv_doc.as<unsigned long long>();
     d.doc_off = d_total + (pt ? 2 : 1);
     KaWaveDocParts pd{};
+    KaWaveBack kb{};   // the rollback side: scratch of Q row bytes, nblk CTA sums, R [Q + 1], the text total, back_off [Q + 1]
+    const int64_t back_cap = bk ? std::min(bk->cap, back_bound) : 0;
+    unsigned long long* d_back_total = nullptr;
+    if (bk) {
+        const size_t o_blk = (q * 4 + 7) / 8 * 8, o_R = o_blk + (size_t)nblk * 8, o_tot = o_R + (q + 1) * 8;
+        if (c->d_wv_back.reserve((size_t)std::max<int64_t>(back_cap, 1)) || c->d_wv_bscr.reserve(o_tot + (q + 2) * 8))
+            return set_status(st, KA_ERR_CUDA);
+        char* base = static_cast<char*>(c->d_wv_bscr.p);
+        kb.rep_off = c->d_rep_off.as<int64_t>();
+        kb.cur = c->d_cur.as<int32_t>();
+        kb.rowlen = reinterpret_cast<uint32_t*>(base);
+        kb.blockoff = reinterpret_cast<unsigned long long*>(base + o_blk);
+        kb.R = reinterpret_cast<unsigned long long*>(base + o_R);
+        d_back_total = reinterpret_cast<unsigned long long*>(base + o_tot);
+    }
     if (!pt) {
-        ka_wave_doc_len_kernel<false><<<nblk, 256, 0, s>>>(d, pd);
+        ka_wave_doc_len_kernel<false, false><<<nblk, 256, 0, s>>>(d, pd, kb);
         ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total, nullptr);
-        if (enq_json_write(ka_wave_doc_write_kernel<false>, nblk, s, d, d_total, pd) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+        if (enq_json_write(ka_wave_doc_write_kernel<false, false>, nblk, s, d, d_total, pd, kb) != cudaSuccess)
+            return set_status(st, KA_ERR_CUDA);
     } else {
-        if ((rc = enq_wave_parts(c, s, Q, W, *pt, d, pd, st)) != KA_OK) return rc;
-        ka_wave_doc_len_kernel<true><<<nblk, 256, 0, s>>>(d, pd);
+        if ((rc = enq_wave_parts(c, s, Q, W, *pt, d, pd, kb, st)) != KA_OK) return rc;
+        ka_wave_doc_len_kernel<true, false><<<nblk, 256, 0, s>>>(d, pd, kb);
         ka_wave_doc_scan_kernel<true><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total, pd.part_cnt);
-        if (enq_json_write(ka_wave_doc_write_kernel<true>, nblk, s, d, d_total, pd) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+        if (enq_json_write(ka_wave_doc_write_kernel<true, false>, nblk, s, d, d_total, pd, kb) != cudaSuccess)
+            return set_status(st, KA_ERR_CUDA);
     }
     c->launches += 3;
+    KaWaveDocs db = d;   // the rollback text: the same positions and part starts, its own bytes, offsets, buffer and back_off
+    if (bk) {
+        db.p.json = c->d_wv_back.as<char>();
+        db.p.cap = (unsigned long long)back_cap;
+        db.p.rowlen = kb.rowlen;
+        db.blockoff = kb.blockoff;
+        db.doc_off = d_back_total + 1;
+        ka_wave_doc_len_kernel<true, true><<<nblk, 256, 0, s>>>(db, pd, kb);
+        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(db.blockoff, (int)nblk, d_back_total, nullptr);
+        if (enq_json_write(ka_wave_doc_write_kernel<true, true>, nblk, s, db, d_back_total, pd, kb) != cudaSuccess)
+            return set_status(st, KA_ERR_CUDA);
+        c->launches += 3;
+    }
     unsigned long long total[2] = {0, (unsigned long long)W};   // the text's bytes and the documents D
+    unsigned long long back_total = 0;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(total, d_total, pt ? 16 : 8, cudaMemcpyDeviceToHost, s) ||
-        cudaStreamSynchronize(s))
+        (bk && cudaMemcpyAsync(&back_total, d_back_total, 8, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     if (total[0] > (unsigned long long)json_cap) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
+    if (bk && back_total > (unsigned long long)bk->cap)
+        return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(bk->cap, INT_MAX));
     const size_t D = (size_t)total[1];
     if (cudaMemcpyAsync(json, c->d_json.p, (size_t)total[0], cudaMemcpyDeviceToHost, s) ||
         cudaMemcpyAsync(doc_off, d.doc_off, (D + 1) * 8, cudaMemcpyDeviceToHost, s) ||
-        (pt && cudaMemcpyAsync(pt->doc_wave, pd.doc_wave, D * 4, cudaMemcpyDeviceToHost, s)))
+        (pt && cudaMemcpyAsync(pt->doc_wave, pd.doc_wave, D * 4, cudaMemcpyDeviceToHost, s)) ||
+        (bk && (cudaMemcpyAsync(bk->back, db.p.json, (size_t)back_total, cudaMemcpyDeviceToHost, s) ||
+                cudaMemcpyAsync(bk->back_off, db.doc_off, (D + 1) * 8, cudaMemcpyDeviceToHost, s))))
         return set_status(st, KA_ERR_CUDA);
     if ((rc = wave_plan_out(c, Q, W, wave, n_waves, summary, summary_cap, sd, st)) != KA_OK) return rc;
     if (pt) *pt->n_docs = (int32_t)D;
@@ -2813,6 +2872,35 @@ int32_t ka_plan_waves_send_json_parts(ka_ctx* c, int32_t T, const int64_t* part_
     const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
                            name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, st);
+}
+
+int32_t ka_plan_waves_json_parts_rollback(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                          const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                                          const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
+                                          const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                          int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave, int32_t* n_docs, char* back,
+                                          int64_t back_cap, int64_t* back_off, int32_t* wave, int32_t* n_waves,
+                                          ka_wave_summary* summary, int32_t summary_cap, ka_status* st) {
+    const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
+    const WaveBack bk{back, back_cap, back_off};
+    return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, &pt, st, &bk);
+}
+
+int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id,
+                                               const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                                               const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
+                                               int64_t max_broker_in, int32_t n_send, const int32_t* send_id, int64_t max_broker_out,
+                                               const char* names, const int64_t* name_off, char* json, int64_t json_cap,
+                                               int64_t max_doc_bytes, int64_t* doc_off, int32_t* doc_wave, int32_t* n_docs,
+                                               char* back, int64_t back_cap, int64_t* back_off, int32_t* wave, int32_t* n_waves,
+                                               ka_wave_summary* summary, ka_wave_send_summary* send_summary, int32_t summary_cap,
+                                               ka_status* st) {
+    const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
+    const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
+    const WaveBack bk{back, back_cap, back_off};
+    return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, st, &bk);
 }
 
 }  // extern "C"

@@ -115,6 +115,43 @@ __device__ __forceinline__ char* ka_json_row_put(const KaJsonParams& p, uint32_t
     return ka_put_str(w, "\"}", 2);
 }
 
+// The rollback record of row q: the row's CURRENT list cur[rep_off[g] .. rep_off[g + 1]) (g the run-wide row) as given, in the
+// key order of Kafka 0.10's ZkUtils.formatAsReassignmentJson, which prints the "CURRENT ASSIGNMENT" (KAG:103-111):
+//   {"topic":"name","partition":P,"replicas":[a,b,c]}
+// 39 bytes + name + partition digits + list, as the record of ka_json_row_len: only the list differs. Its document frame is
+// {"version":1,"partitions":[ ... ]}, 29 bytes like the other.
+#define KA_BACK_HEAD "{\"version\":1,\"partitions\":["
+#define KA_BACK_TAIL "]}"
+#define KA_BACK_HEAD_LEN 27
+#define KA_BACK_TAIL_LEN 2
+
+__device__ __forceinline__ uint32_t ka_json_back_len(const KaJsonParams& p, const int64_t* rep_off, const int32_t* cur, uint32_t q,
+                                                     bool comma) {
+    int t, part;
+    ka_json_row_key(p, q, t, part);
+    const int64_t g = (int64_t)p.row0 + q, a = rep_off[g], b = rep_off[g + 1];
+    uint32_t n = (comma ? 1u : 0u) + 10u + (uint32_t)(p.name_off[t + 1] - p.name_off[t]) + 14u + ka_ndigits(part) + 13u + 2u;
+    for (int64_t i = a; i < b; ++i) n += ka_ndigits(cur[i]) + (i > a ? 1u : 0u);
+    return n;
+}
+__device__ __forceinline__ char* ka_json_back_put(const KaJsonParams& p, const int64_t* rep_off, const int32_t* cur, uint32_t q,
+                                                  char* w, bool comma) {
+    int t, part;
+    ka_json_row_key(p, q, t, part);
+    const int64_t g = (int64_t)p.row0 + q, a = rep_off[g], b = rep_off[g + 1];
+    if (comma) *w++ = ',';
+    w = ka_put_str(w, "{\"topic\":\"", 10);
+    w = ka_put_str(w, p.names + p.name_off[t], (int)(p.name_off[t + 1] - p.name_off[t]));
+    w = ka_put_str(w, "\",\"partition\":", 14);
+    w = ka_put_int(w, part);
+    w = ka_put_str(w, ",\"replicas\":[", 13);
+    for (int64_t i = a; i < b; ++i) {
+        if (i > a) *w++ = ',';
+        w = ka_put_int(w, cur[i]);
+    }
+    return ka_put_str(w, "]}", 2);
+}
+
 // The row texts of a CTA of 256 threads, n bytes per thread. ka_cta256_sum: the CTA's bytes, in thread 0. ka_cta256_prefix:
 // this thread's offset in the CTA's text, and (total) the CTA's bytes, in every thread.
 __device__ __forceinline__ unsigned long long ka_cta256_sum(uint32_t n) {

@@ -31,6 +31,13 @@
 // The text passes then run with PARTS = true: the frame goes at part boundaries and doc_off is indexed by part. They add the
 // parts starting in every CTA, and the scan numbers the parts (D, the parts of all waves).
 //
+// The rollback documents (ka_plan_waves_json_parts_rollback) print every part's rows with their CURRENT lists
+// (ka_json_back_len / ka_json_back_put). The paired cut takes the rollback record's c'_i beside c_i and its prefix R beside S:
+// positions i..j-1 of one wave make a part iff both S[j] - S[i] and R[j] - R[i] are <= L - 28. The part passes' BACK = true
+// instances carry R (the pair scan ka_wave_part_scan2_kernel takes the place of ka_wave_doc_scan_kernel); the jump and mark
+// passes are the same. The rollback text is then one more length / scan / write trio (BACK = true, over the same positions and
+// part starts), into its own buffer, with the frame {"version":1,"partitions":[ ... ]}.
+//
 // A pass ranks a row by counting, never by the order of atomics: the text depends on the input alone.
 #pragma once
 #include "kassign_json.cuh"
@@ -134,6 +141,16 @@ struct KaWaveDocParts {
     int32_t* doc_wave;                   // [D] out: the wave of every part
 };
 
+// What the passes read and write only for the rollback documents (BACK = true): the current lists, and the rollback side's row
+// bytes, CTA sums / offsets and (part passes) prefix R. A separate (last) kernel argument, like KaWaveDocParts.
+struct KaWaveBack {
+    const int64_t* rep_off;              // [Q + 1]
+    const int32_t* cur;                  // [rep_off[Q]]
+    uint32_t* rowlen;                    // [M] c'_i in the part passes, then the rollback text bytes of every position
+    unsigned long long* blockoff;        // [ceil(Q / 256)] CTA sums, then (scan) their offsets
+    unsigned long long* R;               // [M + 1] the part passes' prefix of c'
+};
+
 // Row, wave and place in its document of grouped position i.
 template <bool PARTS>
 __device__ __forceinline__ void ka_wave_doc_row(const KaWaveDocs& d, const KaWaveDocParts& pd, uint32_t i, uint32_t M, uint32_t& g, int& v,
@@ -149,9 +166,9 @@ __device__ __forceinline__ void ka_wave_doc_row(const KaWaveDocs& d, const KaWav
     }
 }
 
-// grid ceil(Q / 256), 256 threads.
-template <bool PARTS>
-__global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d, const KaWaveDocParts pd) {
+// grid ceil(Q / 256), 256 threads. BACK (with PARTS): the rollback text, whose parts the PARTS = true pass has counted already.
+template <bool PARTS, bool BACK>
+__global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d, const KaWaveDocParts pd, const KaWaveBack bk) {
     const uint32_t M = (uint32_t)*d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     uint32_t n = 0;
@@ -161,13 +178,16 @@ __global__ void __launch_bounds__(256) ka_wave_doc_len_kernel(const KaWaveDocs d
         int v;
         bool first, last;
         ka_wave_doc_row<PARTS>(d, pd, i, M, g, v, first, last);
-        n = (first ? KA_JSON_HEAD_LEN : 0u) + ka_json_row_len(d.p, g, !first) + (last ? KA_JSON_TAIL_LEN : 0u);
+        if constexpr (BACK)
+            n = (first ? KA_BACK_HEAD_LEN : 0u) + ka_json_back_len(d.p, bk.rep_off, bk.cur, g, !first) + (last ? KA_BACK_TAIL_LEN : 0u);
+        else
+            n = (first ? KA_JSON_HEAD_LEN : 0u) + ka_json_row_len(d.p, g, !first) + (last ? KA_JSON_TAIL_LEN : 0u);
         d.p.rowlen[i] = n;
         opens = first;
     }
     const unsigned long long bytes = ka_cta256_sum(n);
     if (threadIdx.x == 0) d.blockoff[blockIdx.x] = bytes;
-    if constexpr (PARTS) {
+    if constexpr (PARTS && !BACK) {
         const int parts = __syncthreads_count(opens);
         if (threadIdx.x == 0) pd.part_cnt[blockIdx.x] = parts;
     }
@@ -189,11 +209,11 @@ __global__ void __launch_bounds__(1024) ka_wave_doc_scan_kernel(unsigned long lo
 // grid ceil(Q / 256), 256 threads, KA_JSON_SMEM_BYTES + 16 of dynamic shared memory. Every grouped row writes its text at its
 // final position, the 256 rows of a CTA through the shared-memory stage of the JSON passes. The frame travels with the rows,
 // so a CTA that spans many waves is staged like any other. The first row of wave v writes doc_off[v - 1], the last row of all
-// doc_off[W]; PARTS: the first row of part r writes doc_off[r] and doc_wave[r], the last row of all doc_off[D]. Nothing is
-// written when the text exceeds p.cap.
-template <bool PARTS>
+// doc_off[W]; PARTS: the first row of part r writes doc_off[r] and doc_wave[r], the last row of all doc_off[D]. BACK: the
+// rollback text, whose doc_off is back_off and which writes no doc_wave. Nothing is written when the text exceeds p.cap.
+template <bool PARTS, bool BACK>
 __global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs d, const unsigned long long* __restrict__ total,
-                                                                const KaWaveDocParts pd) {
+                                                                const KaWaveDocParts pd, const KaWaveBack bk) {
     extern __shared__ __align__(16) unsigned char ka_jsmem[];
     const uint32_t M = (uint32_t)*d.n_rows;
     if (*total > d.p.cap || blockIdx.x * 256u >= M) return;   // CTA-uniform
@@ -221,20 +241,30 @@ __global__ void __launch_bounds__(256) ka_wave_doc_write_kernel(const KaWaveDocs
         bool first, last;
         ka_wave_doc_row<PARTS>(d, pd, i, M, g, v, first, last);
         char* w = (staged ? stage : dst) + loc;
-        if (first) {
-            w = ka_put_str(w, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
-            if constexpr (PARTS) {
+        if constexpr (BACK) {   // part is the number of parts opened before i: with i's own, D at the last row
+            if (first) {
+                w = ka_put_str(w, KA_BACK_HEAD, KA_BACK_HEAD_LEN);
                 d.doc_off[part] = at + loc;
-                pd.doc_wave[part] = v;
-            } else {
-                d.doc_off[v - 1] = at + loc;
             }
-        }
-        w = ka_json_row_put(d.p, g, w, !first);
-        if (last) ka_put_str(w, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
-        if (i + 1 == M) {
-            if constexpr (PARTS) d.doc_off[total[1]] = at + loc + n;
-            else d.doc_off[v] = at + loc + n;
+            w = ka_json_back_put(d.p, bk.rep_off, bk.cur, g, w, !first);
+            if (last) ka_put_str(w, KA_BACK_TAIL, KA_BACK_TAIL_LEN);
+            if (i + 1 == M) d.doc_off[part + (first ? 1u : 0u)] = at + loc + n;
+        } else {
+            if (first) {
+                w = ka_put_str(w, KA_JSON_HEAD, KA_JSON_HEAD_LEN);
+                if constexpr (PARTS) {
+                    d.doc_off[part] = at + loc;
+                    pd.doc_wave[part] = v;
+                } else {
+                    d.doc_off[v - 1] = at + loc;
+                }
+            }
+            w = ka_json_row_put(d.p, g, w, !first);
+            if (last) ka_put_str(w, KA_JSON_TAIL, KA_JSON_TAIL_LEN);
+            if (i + 1 == M) {
+                if constexpr (PARTS) d.doc_off[total[1]] = at + loc + n;
+                else d.doc_off[v] = at + loc + n;
+            }
         }
     }
     if (staged) ka_json_store_staged(dst, stage, bt);
@@ -253,12 +283,13 @@ struct KaWaveParts {
     unsigned long long* widest;     // the most rows of a wave
 };
 
-// grid ceil(Q / 256), 256 threads.
-__global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts pp) {
+// grid ceil(Q / 256), 256 threads. BACK: c'_i and its CTA sums too.
+template <bool BACK>
+__global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts pp, const KaWaveBack bk) {
     const KaWaveDocs& d = pp.d;
     const uint32_t M = (uint32_t)*d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
-    uint32_t c = 0;
+    uint32_t c = 0, cb = 0;
     if (i < M) {
         uint32_t g;
         int v;
@@ -266,16 +297,35 @@ __global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts
         ka_wave_doc_row<false>(d, KaWaveDocParts{}, i, M, g, v, first, last);
         c = ka_json_row_len(d.p, g, true);   // the record and its comma
         d.p.rowlen[i] = c;
+        if constexpr (BACK) {
+            cb = ka_json_back_len(d.p, bk.rep_off, bk.cur, g, true);
+            bk.rowlen[i] = cb;
+        }
         pp.start[i] = first;
         if (first) pp.first_pos[v - 1] = (int32_t)i;
         if (i + 1 == M) pp.first_pos[v] = (int32_t)M;
     }
     const unsigned long long bytes = ka_cta256_sum(c);
     if (threadIdx.x == 0) d.blockoff[blockIdx.x] = bytes;
+    if constexpr (BACK) {
+        __syncthreads();   // thread 0 has read the warp sums: the second sum may write them
+        const unsigned long long back = ka_cta256_sum(cb);
+        if (threadIdx.x == 0) bk.blockoff[blockIdx.x] = back;
+    }
 }
 
-// grid ceil(Q / 256), 256 threads: S[i] = the CTA's offset + the in-CTA prefix; the last position also writes S[M].
-__global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWaveParts pp) {
+// ONE CTA of 1024: both sides' CTA sums of the paired cut to their offsets, in place.
+__global__ void __launch_bounds__(1024) ka_wave_part_scan2_kernel(unsigned long long* __restrict__ v, unsigned long long* __restrict__ w,
+                                                                  int n) {
+    ka_cta_scan(v, v, n, 0ull);
+    __syncthreads();   // every thread has read the first scan's total: the second may reset it
+    ka_cta_scan(w, w, n, 0ull);
+}
+
+// grid ceil(Q / 256), 256 threads: S[i] = the CTA's offset + the in-CTA prefix; the last position also writes S[M]. BACK: R
+// likewise.
+template <bool BACK>
+__global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWaveParts pp, const KaWaveBack bk) {
     const uint32_t M = (uint32_t)*pp.d.n_rows;
     if (blockIdx.x * 256u >= M) return;   // CTA-uniform
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
@@ -284,11 +334,21 @@ __global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWavePa
     const unsigned long long s = pp.d.blockoff[blockIdx.x] + ka_cta256_prefix(c, bt);
     if (i < M) pp.S[i] = s;
     if (i + 1 == M) pp.S[M] = s + c;
+    if constexpr (BACK) {
+        __syncthreads();   // every thread has read the warp sums
+        const uint32_t cb = i < M ? bk.rowlen[i] : 0u;
+        const unsigned long long r = bk.blockoff[blockIdx.x] + ka_cta256_prefix(cb, bt);
+        if (i < M) bk.R[i] = r;
+        if (i + 1 == M) bk.R[M] = r + cb;
+    }
 }
 
 // grid ceil(Q / 256), 256 threads: J_0[i] = the last j in (i, e] with S[j] - S[i] <= room, e the end of i's wave, and M in
-// place of e. A position whose own record does not fit reports its ROW, so the lowest input row wins.
-__global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWaveParts pp) {
+// place of e. A position whose own record does not fit reports its ROW, so the lowest input row wins. BACK: the last j that
+// also keeps R[j] - R[i] <= room (both conditions are monotone in j); a record that does not fit on either side reports the
+// longer one-record document.
+template <bool BACK>
+__global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWaveParts pp, const KaWaveBack bk) {
     const uint32_t M = (uint32_t)*pp.d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     if (i >= M) return;
@@ -297,6 +357,21 @@ __global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWavePart
     const uint32_t e = (uint32_t)pp.first_pos[v];
     if (pp.start[i]) atomicMax(pp.widest, (unsigned long long)(e - i));
     const long long lim = (long long)pp.S[i] + pp.room;
+    if constexpr (BACK) {
+        const long long lim_r = (long long)bk.R[i] + pp.room;
+        if ((long long)pp.S[i + 1] > lim || (long long)bk.R[i + 1] > lim_r) {
+            const unsigned long long rec = max(pp.S[i + 1] - pp.S[i], bk.R[i + 1] - bk.R[i]);
+            atomicMin(pp.err, (unsigned long long)g << 32 | min(28ull + rec, 0xFFFFFFFFull));
+            return;
+        }
+        uint32_t lo = i + 1, hi = e;   // S[lo] <= lim and R[lo] <= lim_r
+        while (lo < hi) {
+            const uint32_t mid = (lo + hi + 1) >> 1;
+            if ((long long)pp.S[mid] <= lim && (long long)bk.R[mid] <= lim_r) lo = mid; else hi = mid - 1;
+        }
+        pp.next[i] = (int32_t)(lo == e ? M : lo);
+        return;
+    }
     if ((long long)pp.S[i + 1] > lim) {
         const unsigned long long bytes = min(28ull + (pp.S[i + 1] - pp.S[i]), 0xFFFFFFFFull);
         atomicMin(pp.err, (unsigned long long)g << 32 | bytes);

@@ -18,6 +18,8 @@
 //   kassign::planWavesJson                            <->  planWaves with every wave's document built on the device
 //   kassign::planWaveParts                            <->  planWavesJson with every wave cut into documents of at most a
 //                                                          size limit (ZooKeeper's znode limit), cut on the device
+//   kassign::planWavePartsRollback                    <->  planWaveParts with every part's rollback document (its partitions
+//                                                          on their current lists), both sides under the limit
 //   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
 //                                                          receives more than a budget, one document per wave
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
@@ -340,6 +342,31 @@ public:
         return planWavePartsWith(topics, proposed, maxBrokerIn, maxDocBytes, &send, weights);
     }
 
+    // planWaveParts with every part's rollback document beside it (ka_plan_waves_json_parts_rollback): rollback[d] equals
+    // kafkaReassignmentJson of parts[d]'s partitions, in parts[d]'s order, with their current lists, the document that undoes
+    // part d whatever else has run. A partition joins a part only while both its document and its rollback document stay <=
+    // maxDocBytes; when no current list prints longer than its new one, parts and partWave are those of planWaveParts. A
+    // partition whose one-record document on either side exceeds maxDocBytes gives KA_ERR_LIMIT with a = its row and b = the
+    // longer length. Topic names that org.json would escape take the host emitters and the same cut on the host.
+    struct WaveRollback {
+        ka_status status;   // re-throw with throwForStatus; on an error summary, parts, rollback and partWave are empty
+        std::vector<ka_wave_summary> summary;
+        std::vector<std::string> parts;
+        std::vector<std::string> rollback;
+        std::vector<int32_t> partWave;
+        std::vector<ka_wave_send_summary> sendSummary;   // with a SendBudget: beside summary, one per wave
+    };
+    WaveRollback planWavePartsRollback(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
+                                       int64_t maxBrokerIn, int64_t maxDocBytes, const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavePartsRollbackWith(topics, proposed, maxBrokerIn, maxDocBytes, nullptr, weights);
+    }
+    // planWavePartsRollback under a sender budget too (ka_plan_waves_send_json_parts_rollback); sendSummary is filled.
+    WaveRollback planWavePartsRollback(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
+                                       int64_t maxBrokerIn, int64_t maxDocBytes, const SendBudget& send,
+                                       const std::vector<std::map<int, int64_t>>& weights = {}) {
+        return planWavePartsRollbackWith(topics, proposed, maxBrokerIn, maxDocBytes, &send, weights);
+    }
+
 private:
     // rowWave (when given) receives every row's wave, in the row order of flatten(topics).
     WavePlan planWavesWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
@@ -391,6 +418,9 @@ private:
                                const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
     WaveParts planWavePartsWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                                 int64_t maxDocBytes, const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
+    WaveRollback planWavePartsRollbackWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
+                                           int64_t maxBrokerIn, int64_t maxDocBytes, const SendBudget* send,
+                                           const std::vector<std::map<int, int64_t>>& weights);
 
 public:
 
@@ -648,6 +678,21 @@ inline void appendRecord(std::string& s, const std::string& topic, int partition
     s.push_back('}');
 }
 
+// A partition's record in Kafka 0.10 ZkUtils.formatAsReassignmentJson order (the "CURRENT ASSIGNMENT" and rollback records):
+// scala Map literals keep insertion order for <= 4 entries: topic, partition, replicas.
+inline void appendCurrentRecord(std::string& s, const std::string& topic, int partition, const int* replicas, size_t n) {
+    s += "{\"topic\":";
+    appendQuoted(s, topic);
+    s += ",\"partition\":";
+    appendInt(s, partition);
+    s += ",\"replicas\":[";
+    for (size_t i = 0; i < n; ++i) {
+        if (i) s.push_back(',');
+        appendInt(s, replicas[i]);
+    }
+    s += "]}";
+}
+
 inline std::string newAssignmentJson(const std::vector<TopicOutput>& topics) {
     std::string s = "{\"partitions\":[";
     bool first = true;
@@ -828,19 +873,99 @@ inline std::string kafkaReassignmentJson(const std::vector<TopicInput>& topics) 
         for (const auto& e : t.current) {
             if (!first) s.push_back(',');
             first = false;
-            s += "{\"topic\":";
-            appendQuoted(s, t.name);
-            s += ",\"partition\":";
-            appendInt(s, e.first);
-            s += ",\"replicas\":[";
-            for (size_t i = 0; i < e.second.size(); ++i) {
-                if (i) s.push_back(',');
-                appendInt(s, e.second[i]);
-            }
-            s += "]}";
+            appendCurrentRecord(s, t.name, e.first, e.second.data(), e.second.size());
         }
     s += "]}";
     return s;
+}
+
+inline KafkaTopicAssigner::WaveRollback KafkaTopicAssigner::planWavePartsRollbackWith(const std::vector<TopicInput>& topics,
+                                                                                      const std::vector<TopicOutput>& proposed,
+                                                                                      int64_t maxBrokerIn, int64_t maxDocBytes,
+                                                                                      const SendBudget* send,
+                                                                                      const std::vector<std::map<int, int64_t>>& weights) {
+    const Flat f = flatten(topics, -1);
+    const ProposedRows p = proposedRows(topics, proposed, weights);
+    const size_t Q = f.partId.size();
+    for (const auto& t : topics)
+        if (needsJsonEscape(t.name)) {   // the host emitters over the rows of planWaves, cut by the rule of planWavePartsRollback
+            std::vector<int32_t> rowWave;
+            const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights, &rowWave);
+            WaveRollback res{plan.status, plan.summary, {}, {}, {}, plan.sendSummary};
+            if (res.status.code == KA_OK && maxDocBytes < 1) res.status.code = KA_ERR_BAD_ARG;
+            if (res.status.code != KA_OK) return WaveRollback{res.status, {}, {}, {}, {}, {}};
+            std::vector<std::vector<std::pair<std::string, std::string>>> recs(plan.summary.size());
+            for (size_t t = 0; t < f.names.size(); ++t)
+                for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
+                    if (rowWave[r] == 0) continue;
+                    std::string rec, back;
+                    appendRecord(rec, f.names[t], f.partId[r], p.newBroker.data() + r * p.stride, (size_t)p.newLen[r]);
+                    appendCurrentRecord(back, f.names[t], f.partId[r], f.cur.data() + f.repOff[r], (size_t)(f.repOff[r + 1] - f.repOff[r]));
+                    const int64_t longest = 29 + (int64_t)std::max(rec.size(), back.size());
+                    if (longest > maxDocBytes) {
+                        ka_status st{};
+                        st.code = KA_ERR_LIMIT;
+                        st.a = (int32_t)r;
+                        st.b = (int32_t)std::min<int64_t>(longest, INT32_MAX);
+                        return WaveRollback{st, {}, {}, {}, {}, {}};
+                    }
+                    recs[rowWave[r] - 1].emplace_back(std::move(rec), std::move(back));
+                }
+            for (size_t v = 0; v < recs.size(); ++v) {
+                int64_t size = 0, backSize = 0;   // of the current part's two documents, 0 before the wave's first
+                for (const auto& rb : recs[v]) {
+                    const int64_t n = (int64_t)rb.first.size(), m = (int64_t)rb.second.size();
+                    if (size > 0 && size + 1 + n <= maxDocBytes && backSize + 1 + m <= maxDocBytes) {
+                        res.parts.back().insert(res.parts.back().size() - 14, "," + rb.first);
+                        res.rollback.back().insert(res.rollback.back().size() - 2, "," + rb.second);
+                        size += 1 + n;
+                        backSize += 1 + m;
+                    } else {
+                        res.parts.push_back("{\"partitions\":[" + rb.first + "],\"version\":1}");
+                        res.rollback.push_back("{\"version\":1,\"partitions\":[" + rb.second + "]}");
+                        res.partWave.push_back((int32_t)v + 1);
+                        size = 29 + n;
+                        backSize = 29 + m;
+                    }
+                }
+            }
+            return res;
+        }
+    std::string names;
+    std::vector<int64_t> nameOff(1, 0);
+    const int64_t cap = waveNames(f, p.stride, names, nameOff);
+    int64_t backCap = 12 * (int64_t)f.cur.size();   // per row 79 + its topic's name, 12 per current broker
+    for (size_t t = 0; t < f.names.size(); ++t) backCap += (f.partOff[t + 1] - f.partOff[t]) * (79 + (int64_t)f.names[t].size());
+    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]), back(new char[std::max<int64_t>(backCap, 1)]);
+    std::vector<int64_t> docOff(Q + 1, 0), backOff(Q + 1, 0);
+    std::vector<int32_t> docWave(std::max<size_t>(Q, 1), 0);
+    WaveRollback res{};
+    res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
+    int32_t W = 0, D = 0;
+    const int64_t* w = p.w.empty() ? nullptr : p.w.data();
+    if (!send) {
+        ka_plan_waves_json_parts_rollback(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
+                                          p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, names.data(), nameOff.data(),
+                                          json.get(), cap, maxDocBytes, docOff.data(), docWave.data(), &D, back.get(), backCap,
+                                          backOff.data(), nullptr, &W, res.summary.data(), (int32_t)res.summary.size(), &res.status);
+    } else {
+        res.sendSummary.resize(res.summary.size());
+        ka_plan_waves_send_json_parts_rollback(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(),
+                                               f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn,
+                                               (int32_t)send->sendBrokers.size(), send->sendBrokers.data(), send->maxBrokerOut,
+                                               names.data(), nameOff.data(), json.get(), cap, maxDocBytes, docOff.data(),
+                                               docWave.data(), &D, back.get(), backCap, backOff.data(), nullptr, &W,
+                                               res.summary.data(), res.sendSummary.data(), (int32_t)res.summary.size(), &res.status);
+    }
+    if (res.status.code != KA_OK) return WaveRollback{res.status, {}, {}, {}, {}, {}};
+    res.summary.resize(W);
+    if (send) res.sendSummary.resize(W);
+    for (int32_t d = 0; d < D; ++d) {
+        res.parts.emplace_back(json.get() + docOff[d], (size_t)(docOff[d + 1] - docOff[d]));
+        res.rollback.emplace_back(back.get() + backOff[d], (size_t)(backOff[d + 1] - backOff[d]));
+    }
+    res.partWave.assign(docWave.begin(), docWave.begin() + D);
+    return res;
 }
 
 }  // namespace kassign
