@@ -590,7 +590,12 @@ int32_t ka_last_status(ka_ctx* ctx, ka_status* st);
 /* ---- counters (Context.counter) -----------------------------------------------------------------
  * counter[i*slots + r] = Context.counter[broker_id[i]][r] for the CURRENT broker table (KAS:289-301:
  * absent == 0). slots = ka_ctx_counter_slots(). Used by tests and by the multi-GPU ring hand-off
- * (rank g imports what rank g-1 exported before ordering its own topics — S5 is a serial chain). */
+ * (rank g imports what rank g-1 exported before ordering its own topics — S5 is a serial chain).
+ * Values: any int32 may be set or imported. The rows and counters equal the reference's (whose counters are Java ints) as
+ * long as every counter a run reads is below INT_MAX, e.g. every value at most INT_MAX minus the run's rows when it starts;
+ * a bump past INT_MAX wraps, as the reference's does. Rows shorter than 3 are padded inside the chains with a dummy broker
+ * whose counter is INT_MAX, listed after every real broker of the row and never bumped, so the dummy cannot win a slot
+ * from a real broker at any counter value. */
 int32_t ka_ctx_counter_slots(ka_ctx* ctx);
 int32_t ka_ctx_get_counters(ka_ctx* ctx, int32_t* counter /* [N*slots] host */);
 int32_t ka_ctx_set_counters(ka_ctx* ctx, const int32_t* counter /* [N*slots] host */);

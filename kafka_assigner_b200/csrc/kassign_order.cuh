@@ -193,8 +193,11 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
         for (uint32_t i = tid; i < (uint32_t)(CAND ? (int)pin[8] : p.N) * CW; i += blockDim.x)
             ctr[i] = ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))];
     if (KIND <= 1 && tid == 0) {  // the dummy broker (index N) that pads rows shorter than 3: a counter that never wins a comparison
+        // INT_MAX, and every record lists the dummy after its real brokers: a real counter is at most INT_MAX, so it wins both
+        // the slot-0 minimum and the slot-1 pair (e = 0 there) in scan order. The dummy is never bumped (the bumps below are
+        // skipped for rows too short to fill the slot), so its counter stays INT_MAX for the whole launch.
         const int N = CAND ? (int)pin[8] : p.N;
-        if (GCTR) ctr8[(size_t)N * KA_MAX_SLOTS + KIND] = 0x3FFFFFFF; else ctr[N] = 0x3FFFFFFF;
+        if (GCTR) ctr8[(size_t)N * KA_MAX_SLOTS + KIND] = 0x7FFFFFFF; else ctr[N] = 0x7FFFFFFF;
     }
     // idle lanes read (and ignore) ring slots past the end of the stream: make those valid records (all zero)
     for (uint32_t i = tid; i < (uint32_t)NS * G * (RB / 16); i += blockDim.x) reinterpret_cast<uint4*>(ring)[i] = make_uint4(0, 0, 0, 0);
@@ -309,7 +312,7 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
             const uint32_t fz = f & 0x83u;                                                                                  \
             const uint32_t fo = is2 ? (fz | (f & 4u)) : (L10 ? (fz | ((f >> 1) & 4u)) : (fz | ((f >> 2) & 4u)));            \
             if (ACTIVE) {                                                                                                       \
-                C::st1(C::col(cbase, ctr8, oA, 0), vA + 1);   /* counter[list[0]][0] += 1 (KAS:254-261) */                       \
+                if (f & 3u) C::st1(C::col(cbase, ctr8, oA, 0), vA + 1);   /* counter[list[0]][0] += 1 (KAS:254-261); never the dummy */ \
                 asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(orec + (POS)), "r"(op), "r"(oq), "r"(fo), "r"(oA) : "memory"); \
             }
 #define KA_SLOT1_CORE(RC, ACTIVE, POS)                                                                                          \
@@ -319,7 +322,8 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
             const bool pickq = yq < yp + (int)((f >> 2) & 1u);                                                                  \
             const uint32_t o1 = pickq ? oq : op, o2 = pickq ? op : oq;                                                          \
             if (ACTIVE) {                                                                                                       \
-                C::st1(C::col(cbase, ctr8, o1, 1), (pickq ? yq : yp) + 1);   /* counter[list[1]][1] += 1 (KAS:254-261) */        \
+                /* counter[list[1]][1] += 1 (KAS:254-261), for rows of >= 2: a shorter row's pair is the dummy twice */          \
+                if (f & 2u) C::st1(C::col(cbase, ctr8, o1, 1), (pickq ? yq : yp) + 1);                                          \
                 /* the ordered list replaces the record (ka_emit3_kernel reads it) */                                           \
                 asm volatile("st.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(orec + (POS)), "r"(oA), "r"(o1), "r"(o2), "r"(f) : "memory"); \
             }
@@ -350,7 +354,7 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
                         const bool L10 = x1 < x0, L20 = x2 < x0, L21 = x2 < x1;   // scan order: strict '<', ties to the earlier
                         is2 = L10 ? L21 : L20;
                         is1 = L10 && !L21;
-                        C::st1(C::col(cbase, ctr8, is2 ? a2 : (is1 ? a1 : a0), 0), (is2 ? x2 : (is1 ? x1 : x0)) + 1);   // KAS:254-261
+                        if (f & 3u) C::st1(C::col(cbase, ctr8, is2 ? a2 : (is1 ? a1 : a0), 0), (is2 ? x2 : (is1 ? x1 : x0)) + 1);   // KAS:254-261
                     }
                     __syncwarp();   // level barrier
                 }
@@ -365,7 +369,7 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
                     if (grp == g && active) {
                         const int yp = C::ld1(C::col(cbase, ctr8, op, 1)), yq = C::ld1(C::col(cbase, ctr8, oq, 1));
                         pickq = yq < yp + (int)((f >> 2) & 1u);
-                        C::st1(C::col(cbase, ctr8, pickq ? oq : op, 1), (pickq ? yq : yp) + 1);   // KAS:254-261
+                        if (f & 2u) C::st1(C::col(cbase, ctr8, pickq ? oq : op, 1), (pickq ? yq : yp) + 1);   // KAS:254-261
                     }
                     __syncwarp();
                 }

@@ -130,6 +130,10 @@ class OracleContext:
     def counter(self, broker_id, slot):
         return lib().oracle_ctx_get_counter(self._h, int(broker_id), int(slot))
 
+    def set_counter(self, broker_id, slot, value):
+        """Preload Context.counter[broker_id][slot] (a Context carried over from earlier runs)."""
+        lib().oracle_ctx_set_counter(self._h, int(broker_id), int(slot), int(value))
+
     def __del__(self):
         try:
             lib().oracle_ctx_destroy(self._h)

@@ -1,5 +1,6 @@
 """The plain-Python models the device is checked against, each written once: the move summary, the wave rule (with and
-without a sender budget), the reassignment JSON printers, the schedule model's records and the expected counter histogram.
+without a sender budget), the reassignment JSON printers, the schedule model's records, slot chains and the expected counter
+histogram, and kernel A's shared-memory budget.
 Each restates a rule of include/kassign.h. This module imports numpy and the status codes only: it never loads the library
 or the oracle, so CPU tests, GPU tests and tests/tools can all use it."""
 import numpy as np
@@ -8,7 +9,7 @@ from kafka_assigner_b200 import _native
 
 BAD = _native.KA_ERR_BAD_ARG
 SLOTS = 8            # counter slots per broker (ka_ctx_counter_slots)
-INF = 0x3FFFFFFF     # the counters of the schedule model's dummy broker
+INF = 0x7FFFFFFF     # the counter of the slot chains' dummy broker (index N): INT_MAX, never bumped
 
 
 # ---- the move summary ----------------------------------------------------------------------------------------------------
@@ -187,15 +188,16 @@ def java_abs_hash(h):
 
 
 def build_records(cl, sets):
-    """What kernel A emits for every row: ([a0, a1, a2] in slot-0 scan order with the dummy N for missing slots, len, e01, e02, e12)."""
+    """What kernel A emits for every row: ([a0, a1, a2] in slot-0 scan order with the dummy N for missing slots, len, e01, e02, e12).
+    sets[t]: the rows of topic t (a dense cluster's P rows, or a ragged topic's)."""
     N = cl.N
     idx_of = {int(b): i for i, b in enumerate(cl.broker_id)}
     recs = []
     for t in range(cl.T):
         habs = java_abs_hash(cl.topic_hash[t])
         s2, s3 = habs % 2, habs % 3
-        for p in range(cl.P):
-            ix = sorted(idx_of[int(b)] for b in sets[t][p])          # ascending index == ascending id (KAS:205-214)
+        for row in sets[t]:
+            ix = sorted(idx_of[int(b)] for b in row)                 # ascending index == ascending id (KAS:205-214)
             k = len(ix)
             a, e = [N, N, N], (0, 0, 0)
             if k == 1:
@@ -210,6 +212,72 @@ def build_records(cl, sets):
     return recs
 
 
+def i32(v):
+    """v as a Java int (two's complement wrap)."""
+    return (int(v) + 2**31) % 2**32 - 2**31
+
+
+def conflict_levels(rows):
+    """Conflict level of every record of one topic (kernel A's LEVELS pass)."""
+    last, lv = {}, []
+    for a, k, _ in rows:
+        real = [b for b in a[:max(k, 0)]]
+        lvl = 1 + max([last.get(b, 0) for b in real] or [0])
+        for b in real:
+            last[b] = lvl
+        lv.append(lvl)
+    return lv
+
+
+def slot_chains(cl, sets, rng, c0, c1, c2):
+    """The leader order of the CUDA path for rows of <= 3, as kassign_stage.cuh / kassign_order.cuh run it: the records of
+    build_records in a level schedule (topic by topic, level by level, in a scrambled order inside a level), the whole slot-0
+    chain first, then the slot-1 chain; slot 2 a plain sum. c0 / c1 / c2: counter[.][0 / 1 / 2] by broker index, each with
+    the dummy's entry at index N (INF for c0 and c1); updated in place with int32 arithmetic, as the device adds. A row of k
+    replicas bumps slot r only when r < k, so the dummy is never bumped. Returns {record: ordered broker indices}."""
+    N = cl.N
+    recs = build_records(cl, sets)
+    order, g0 = [], 0
+    for t in range(cl.T):
+        rows = recs[g0:g0 + len(sets[t])]
+        lv = conflict_levels(rows)
+        for level in range(1, max(lv + [0]) + 1):
+            members = [g0 + p for p in range(len(rows)) if lv[p] == level]
+            used = [b for q in members for b in recs[q][0][:recs[q][1]]]
+            assert len(used) == len(set(used)), "partitions of one level must not share a broker"
+            rng.shuffle(members)
+            order.extend(members)
+        g0 += len(rows)
+    assert sorted(order) == list(range(len(recs)))
+    assert c0[N] == INF and c1[N] == INF
+    # ---- slot-0 chain over ALL rows first (it never needs a slot-1 decision) ----
+    mid = {}
+    for q in order:
+        a, k, e = recs[q]
+        x = [c0[a[0]], c0[a[1]], c0[a[2]]]
+        L10, L20, L21 = x[1] < x[0], x[2] < x[0], x[2] < x[1]       # strict '<' in scan order: ties to the earlier position
+        is2 = L21 if L10 else L20
+        is1 = L10 and not L21
+        w = 2 if is2 else (1 if is1 else 0)
+        if k > 0:
+            c0[a[w]] = i32(c0[a[w]] + 1)
+        p_, q_ = (1, 2) if w == 0 else ((0, 2) if w == 1 else (0, 1))
+        mid[q] = (a[p_], a[q_], e[{(0, 1): 0, (0, 2): 1, (1, 2): 2}[(p_, q_)]], a[w], k)
+    # ---- slot-1 chain ----
+    out = {}
+    for q in order:
+        op, oq, e, oA, k = mid[q]
+        pick = c1[oq] < i32(c1[op] + e)
+        o1, o2 = (oq, op) if pick else (op, oq)
+        if k > 1:
+            c1[o1] = i32(c1[o1] + 1)
+        if k > 2:
+            c2[o2] = i32(c2[o2] + 1)                                 # slot 2: a plain sum (the emit kernel's atomicAdd)
+        out[q] = [oA, o1, o2][:k]
+    assert c0[N] == INF and c1[N] == INF
+    return out
+
+
 def histogram(ids, out, out_len):
     """counter[b][r] of a fresh Context after these rows: the number of rows with broker ids[b] at position r."""
     ids = np.asarray(ids)
@@ -220,3 +288,29 @@ def histogram(ids, out, out_len):
         assert np.all(ids[idx] == out[sel, r])
         np.add.at(ctr[:, r], idx, 1)
     return ctr
+
+
+# ---- kernel A's shared-memory budget (make_plan, kassign.cu) --------------------------------------------------------------
+
+def a16(v):
+    return (v + 15) & ~15
+
+
+def blob_bytes(ids):
+    """Bytes of the broker blob kernel A stages: rack indices, plus the id LUT when the id range fits shared memory."""
+    n = len(ids)
+    rng_ = int(ids[-1]) - int(ids[0]) + 1 if n else 0
+    lut = a16(max(rng_, 1) * 2) if rng_ <= 32768 else 0
+    return a16(max(n, 1) * 2) + lut
+
+
+def stage_warps(N, blob, Pmax, S, capmax, levels):
+    """Warps per CTA of make_plan, or 0 when the layout exceeds the 200 KB budget (KA_ERR_LIMIT, a = Pmax, b = N)."""
+    lsz = 1 if capmax <= 255 else 2
+    per_warp = a16(max(N, 1) * lsz) + a16(max(Pmax, 1) * S * 2) + a16(max(Pmax, 1))
+    if levels:
+        per_warp += a16(max(N, 1) * 4) + a16(max(N, 1) * 2) + 2 * a16((max(Pmax, 1) + 2) * 2)
+    shared = 16 + blob
+    if shared + per_warp > 200 * 1024:
+        return 0
+    return min(16, (200 * 1024 - shared) // per_warp)

@@ -75,7 +75,8 @@ def run_pair_model(cl, sets, launches, c0, c1, c2):
                     win[(t + 1, i)] = slot0_pick(a, x)
             for (u, i), w in win.items():
                 a, k, e = recs[u * P + i]
-                c0[a[w]] += 1
+                if k > 0:                                    # the dummy is never bumped (models.slot_chains)
+                    c0[a[w]] += 1
                 p_, q_ = (1, 2) if w == 0 else ((0, 2) if w == 1 else (0, 1))
                 mid[u * P + i] = (a[p_], a[q_], e[{(0, 1): 0, (0, 2): 1, (1, 2): 2}[(p_, q_)]], a[w], k)
         for t in range(t0, t1, 2):
@@ -96,8 +97,9 @@ def run_pair_model(cl, sets, launches, c0, c1, c2):
                         c[b] = S[b] + int(h is not None and decide1(t, h, S) == b)
                     pick[(t + 1, i)] = oq if c[oq] < c[op] + e else op
             for (u, i), o1 in pick.items():
-                c1[o1] += 1
                 op, oq, e, oA, k = mid[u * P + i]
+                if k > 1:
+                    c1[o1] += 1
                 o2 = op if o1 == oq else oq
                 if k > 2:
                     c2[o2] += 1

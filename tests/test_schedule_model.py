@@ -7,9 +7,10 @@ The CUDA path replaces the reference's single pass over all partitions (KafkaAss
      precomputed tie-breaks e_pq of the slot-1 scan, short rows padded with a dummy broker whose counters are "infinite",
   3. ONE CHAIN PER REPLICA SLOT: slot 0 only reads/bumps counter[.][0], slot 1 counter[.][1] (given the slot-0 winner), and
      counter[.][2] is a plain sum for rows of <= 3 replicas.
-This file restates exactly that in Python — the same record layout and decision rules as kassign_stage.cuh / kassign_order.cuh —
-and asserts that it reproduces the oracle's ordered lists AND its final Context, even when the partitions of a level are
-processed in a scrambled order and the whole slot-0 chain runs before the slot-1 chain starts.
+tests/models.py (build_records, slot_chains) restates exactly that in Python — the same record layout and decision rules as
+kassign_stage.cuh / kassign_order.cuh — and this file asserts that it reproduces the oracle's ordered lists AND its final
+Context, even when the partitions of a level are processed in a scrambled order and the whole slot-0 chain runs before the
+slot-1 chain starts.
 """
 import random
 
@@ -19,58 +20,10 @@ import kafka_assigner_b200 as kab
 from tests import models, util
 
 
-def levels_of_topic(rows):
-    """Conflict level of every partition of one topic (kernel A's LEVELS pass)."""
-    last, lv = {}, []
-    for a, k, _ in rows:
-        real = [b for b in a[:max(k, 0)]]
-        l = 1 + max([last.get(b, 0) for b in real] or [0])
-        for b in real:
-            last[b] = l
-        lv.append(l)
-    return lv
-
-
 def run_model(cl, sets, rng):
-    N, P = cl.N, cl.P
-    recs = models.build_records(cl, sets)
-    # schedule: topic by topic, inside a topic by level; inside a level ANY order (scrambled here)
-    order = []
-    for t in range(cl.T):
-        rows = recs[t * P:(t + 1) * P]
-        lv = levels_of_topic(rows)
-        for level in range(1, max(lv + [0]) + 1):
-            members = [t * P + p for p in range(P) if lv[p] == level]
-            used = [b for q in members for b in recs[q][0][:recs[q][1]]]
-            assert len(used) == len(set(used)), "partitions of one level must not share a broker"
-            rng.shuffle(members)
-            order.extend(members)
-    assert sorted(order) == list(range(cl.T * P))
-    c0 = [0] * N + [models.INF]
-    c1 = [0] * N + [models.INF]
-    c2 = [0] * (N + 1)
-    # ---- slot-0 chain over ALL rows first (it never needs a slot-1 decision) ----
-    mid = {}
-    for q in order:
-        a, k, e = recs[q]
-        x = [c0[a[0]], c0[a[1]], c0[a[2]]]
-        L10, L20, L21 = x[1] < x[0], x[2] < x[0], x[2] < x[1]       # strict '<' in scan order: ties to the earlier position
-        is2 = L21 if L10 else L20
-        is1 = L10 and not L21
-        w = 2 if is2 else (1 if is1 else 0)
-        c0[a[w]] += 1
-        p_, q_ = (1, 2) if w == 0 else ((0, 2) if w == 1 else (0, 1))
-        mid[q] = (a[p_], a[q_], e[{(0, 1): 0, (0, 2): 1, (1, 2): 2}[(p_, q_)]], a[w], k)
-    # ---- slot-1 chain ----
-    out = {}
-    for q in order:
-        op, oq, e, oA, k = mid[q]
-        pick = c1[oq] < c1[op] + e
-        o1, o2 = (oq, op) if pick else (op, oq)
-        c1[o1] += 1
-        if k > 2:
-            c2[o2] += 1                                              # slot 2: a plain sum (the emit kernel's atomicAdd)
-        out[q] = [oA, o1, o2][:k]
+    N = cl.N
+    c0, c1, c2 = [0] * N + [models.INF], [0] * N + [models.INF], [0] * (N + 1)
+    out = models.slot_chains(cl, sets, rng, c0, c1, c2)
     return out, c0, c1, c2
 
 

@@ -12,7 +12,7 @@ Stage plan tuples: (load bytes, levels, SM, candidates K, warps per CTA, grid.x,
 Lookup-mode mask: 1 shared-memory id LUT, 2 global LUT, 4 binary search. grid.x = PERSIST: the grid is capped by occupancy,
 so that the topics outnumber grid.x x warps and the persistent topic loop runs (asserted as grid.x x warps < T); grid.x =
 AUTO: one CTA per `warps` topics, ceil(T / warps). Warps per CTA = None: make_plan's count for the case's layout, computed by
-_warps below (the budget edges and deep-level cases pin it at 1, the small cases at 16).
+models.stage_warps (the budget edges and deep-level cases pin it at 1, the small cases at 16).
 """
 import ctypes
 import os
@@ -31,42 +31,18 @@ AUTO = -1
 INT_MIN = -2**31
 
 
-# ---- make_plan's kernel A arithmetic (kassign.cu): the budget edges below are computed with it -----------------------------
-
-def _a16(v):
-    return (v + 15) & ~15
-
-
-def _blob_bytes(ids):
-    """Bytes of the broker blob kernel A stages: rack indices, plus the id LUT when the id range fits shared memory."""
-    n = len(ids)
-    rng_ = int(ids[-1]) - int(ids[0]) + 1 if n else 0
-    lut = _a16(max(rng_, 1) * 2) if rng_ <= 32768 else 0
-    return _a16(max(n, 1) * 2) + lut
-
+# ---- make_plan's kernel A arithmetic (kassign.cu, restated by models.stage_warps): the budget edges below are computed with it
 
 def _lut_mode(ids):
     rng_ = int(ids[-1]) - int(ids[0]) + 1 if len(ids) else 0
     return 0 if rng_ <= 32768 else (1 if rng_ <= 1 << 25 else 2)
 
 
-def _warps(N, blob, Pmax, S, capmax, levels):
-    """Warps per CTA of make_plan, or 0 when the layout exceeds the 200 KB budget (KA_ERR_LIMIT, a = Pmax, b = N)."""
-    lsz = 1 if capmax <= 255 else 2
-    per_warp = _a16(max(N, 1) * lsz) + _a16(max(Pmax, 1) * S * 2) + _a16(max(Pmax, 1))
-    if levels:
-        per_warp += _a16(max(N, 1) * 4) + _a16(max(N, 1) * 2) + 2 * _a16((max(Pmax, 1) + 2) * 2)
-    shared = 16 + blob
-    if shared + per_warp > 200 * 1024:
-        return 0
-    return min(16, (200 * 1024 - shared) // per_warp)
-
-
 def _largest_p(N, S, rf, blob):
     """The largest P of a dense single solve (rf = S) that kernel A's layout holds for a table of N brokers."""
     def fits(P):
         cap = -(-P * rf // N)
-        return _warps(N, blob, P, S, cap, cap > 1) > 0 and not (cap > 1 and P > 32767)
+        return models.stage_warps(N, blob, P, S, cap, cap > 1) > 0 and not (cap > 1 and P > 32767)
     lo, hi = 1, 32767
     while lo < hi:
         mid = (lo + hi + 1) // 2
@@ -94,13 +70,13 @@ def _ragged_cap(part_off, rep_off, S, n):
 def _dense_warps(tables, P, rf, S):
     """make_plan's warps for a dense call over `tables` (its layout follows the largest table and blob)."""
     cap = max(_dense_cap(P, rf, len(t[0])) for t in tables)
-    return _warps(max(len(t[0]) for t in tables), max(_blob_bytes(t[0]) for t in tables), P, S, cap, cap > 1)
+    return models.stage_warps(max(len(t[0]) for t in tables), max(models.blob_bytes(t[0]) for t in tables), P, S, cap, cap > 1)
 
 
 def _ragged_warps(tables, part_off, rep_off, S):
     cap = max(_ragged_cap(part_off, rep_off, S, len(t[0])) for t in tables)
     Pmax = int(np.diff(part_off).max())
-    return _warps(max(len(t[0]) for t in tables), max(_blob_bytes(t[0]) for t in tables), Pmax, S, cap, True)
+    return models.stage_warps(max(len(t[0]) for t in tables), max(models.blob_bytes(t[0]) for t in tables), Pmax, S, cap, True)
 
 
 # ---- broker tables and current lists ---------------------------------------------------------------------------------------
@@ -333,10 +309,10 @@ def test_regression_plans_follow_make_plan():
     assert _dense_warps([A20, B], 1000, 3, 3) == AB20K_PLAN[4]
     assert _dense_warps([(np.array([7]),)], 33000, 2, 2) == P33000_PLAN[4]
     # the bound of the parent: B's 1 500 turns levels on, and neither layout fits
-    assert _warps(52000, _blob_bytes(A52[0]), 1000, 3, 1500, True) == 0
-    assert _warps(20000, _blob_bytes(A20[0]), 1000, 3, 1500, True) == 0
+    assert models.stage_warps(52000, models.blob_bytes(A52[0]), 1000, 3, 1500, True) == 0
+    assert models.stage_warps(20000, models.blob_bytes(A20[0]), 1000, 3, 1500, True) == 0
     # the ragged layout of A20 (levels, capacity 1) fits
-    assert _warps(20000, _blob_bytes(A20[0]), 1000, 3, 1, True) > 0
+    assert models.stage_warps(20000, models.blob_bytes(A20[0]), 1000, 3, 1, True) > 0
 
 
 def test_last_stage_plan_null_arguments(native_lib):
@@ -504,7 +480,7 @@ def test_single_solve_stage_variant(native_lib, oracle, case):
 
 
 def _deep_p(S):
-    return _largest_p(S, S, S, _blob_bytes(np.arange(S)))
+    return _largest_p(S, S, S, models.blob_bytes(np.arange(S)))
 
 
 @pytest.mark.gpu
@@ -528,7 +504,7 @@ def test_budget_edge(native_lib, oracle, edge):
     N, RF, R, lut = edge
     cl0 = kab.synth.make_cluster(T=1, P=1, RF=RF, N=N, R=R, seed=1)
     ids, racks = _respace(cl0.broker_id, cl0.broker_id, lut)[0], cl0.rack_index
-    P = _largest_p(len(ids), RF, RF, _blob_bytes(ids))
+    P = _largest_p(len(ids), RF, RF, models.blob_bytes(ids))
     cap = -(-P * RF // len(ids))
     s = kab.Solver(0)
     for p, ok in ((P, True), (P + 1, False)):
