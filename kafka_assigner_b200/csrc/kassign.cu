@@ -2652,9 +2652,11 @@ struct WaveBack {
     int64_t* back_off;
 };
 
+extern "C++" {   // the templates of the wave text passes
 // The part passes of a size limit pt over the grouped rows of d, on s: every part start flagged in pd.start, pd.part_cnt and
-// pd.doc_wave placed, or KA_ERR_LIMIT for the lowest row whose one-record document exceeds pt.L. Q rows, W > 0 waves. With the
-// rollback side's bk (bk.R != null) the cut is the paired cut, and a row over-long on either side is the error.
+// pd.doc_wave placed, or KA_ERR_LIMIT for the lowest row whose one-record document exceeds pt.L. Q rows, W > 0 waves. With BACK
+// the cut is the paired cut over the rollback side's bk, and a row over-long on either side is the error.
+template <bool BACK>
 static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const WaveParts& pt, const KaWaveDocs& d, KaWaveDocParts& pd,
                           const KaWaveBack& bk, ka_status* st) {
     const size_t q = (size_t)Q;
@@ -2675,17 +2677,13 @@ static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const Wav
     pp.start = reinterpret_cast<uint8_t*>(base + o_start);
     const unsigned long long meta0[2] = {~0ull, 0ull};
     if (cudaMemcpyAsync(pp.err, meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
-    if (!bk.R) {
-        ka_wave_part_len_kernel<false><<<nblk, 256, 0, s>>>(pp, bk);
-        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, pp.S, nullptr);   // S[0] is rewritten next
-        ka_wave_part_prefix_kernel<false><<<nblk, 256, 0, s>>>(pp, bk);
-        ka_wave_part_next_kernel<false><<<nblk, 256, 0, s>>>(pp, bk);
-    } else {
-        ka_wave_part_len_kernel<true><<<nblk, 256, 0, s>>>(pp, bk);
+    ka_wave_part_len_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
+    if constexpr (BACK)
         ka_wave_part_scan2_kernel<<<1, 1024, 0, s>>>(d.blockoff, bk.blockoff, (int)nblk);
-        ka_wave_part_prefix_kernel<true><<<nblk, 256, 0, s>>>(pp, bk);
-        ka_wave_part_next_kernel<true><<<nblk, 256, 0, s>>>(pp, bk);
-    }
+    else
+        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, pp.S, nullptr);   // S[0] is rewritten next
+    ka_wave_part_prefix_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
+    ka_wave_part_next_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
     c->launches += 4;
     unsigned long long back[2];
     int32_t M = 0;
@@ -2708,14 +2706,25 @@ static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const Wav
     return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
 }
 
+// The length / scan / write passes of one wave text: per wave, per part of pd (PARTS), or the parts' rollback text (BACK).
+template <bool PARTS, bool BACK>
+static cudaError_t enq_wave_text(ka_ctx* c, cudaStream_t s, unsigned nblk, const KaWaveDocs& d, unsigned long long* total,
+                                 const KaWaveDocParts& pd, const KaWaveBack& kb) {
+    ka_wave_doc_len_kernel<PARTS, BACK><<<nblk, 256, 0, s>>>(d, pd, kb);
+    ka_wave_doc_scan_kernel<PARTS && !BACK><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, total, PARTS && !BACK ? pd.part_cnt : nullptr);
+    const cudaError_t e = enq_json_write(ka_wave_doc_write_kernel<PARTS, BACK>, nblk, s, d, total, pd, kb);
+    if (e == cudaSuccess) c->launches += 3;
+    return e;
+}
+}  // extern "C++"
+
 // ka_plan_waves_json, with a sender part sd ka_plan_waves_send_json, with a size limit pt their _parts forms, and with the
 // rollback documents bk (only with pt) the _parts_rollback forms.
 static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
                                const int32_t* cur_broker, int32_t stride, const int32_t* new_len, const int32_t* new_broker,
                                const int64_t* part_weight, int64_t max_broker_in, const char* names, const int64_t* name_off, char* json,
                                int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
-                               int32_t summary_cap, const WaveSend* sd, const WaveParts* pt, ka_status* st,
-                               const WaveBack* bk = nullptr) {
+                               int32_t summary_cap, const WaveSend* sd, const WaveParts* pt, const WaveBack* bk, ka_status* st) {
     if (!st) return KA_ERR_BAD_ARG;
     if (n_waves) *n_waves = 0;
     if (pt && pt->n_docs) *pt->n_docs = 0;
@@ -2784,19 +2793,13 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
         kb.R = reinterpret_cast<unsigned long long*>(base + o_R);
         d_back_total = reinterpret_cast<unsigned long long*>(base + o_tot);
     }
-    if (!pt) {
-        ka_wave_doc_len_kernel<false, false><<<nblk, 256, 0, s>>>(d, pd, kb);
-        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total, nullptr);
-        if (enq_json_write(ka_wave_doc_write_kernel<false, false>, nblk, s, d, d_total, pd, kb) != cudaSuccess)
-            return set_status(st, KA_ERR_CUDA);
-    } else {
-        if ((rc = enq_wave_parts(c, s, Q, W, *pt, d, pd, kb, st)) != KA_OK) return rc;
-        ka_wave_doc_len_kernel<true, false><<<nblk, 256, 0, s>>>(d, pd, kb);
-        ka_wave_doc_scan_kernel<true><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, d_total, pd.part_cnt);
-        if (enq_json_write(ka_wave_doc_write_kernel<true, false>, nblk, s, d, d_total, pd, kb) != cudaSuccess)
-            return set_status(st, KA_ERR_CUDA);
+    if (pt) {
+        rc = bk ? enq_wave_parts<true>(c, s, Q, W, *pt, d, pd, kb, st) : enq_wave_parts<false>(c, s, Q, W, *pt, d, pd, kb, st);
+        if (rc != KA_OK) return rc;
     }
-    c->launches += 3;
+    const cudaError_t e = pt ? enq_wave_text<true, false>(c, s, nblk, d, d_total, pd, kb)
+                             : enq_wave_text<false, false>(c, s, nblk, d, d_total, pd, kb);
+    if (e != cudaSuccess) return set_status(st, KA_ERR_CUDA);
     KaWaveDocs db = d;   // the rollback text: the same positions and part starts, its own bytes, offsets, buffer and back_off
     if (bk) {
         db.p.json = c->d_wv_back.as<char>();
@@ -2804,11 +2807,7 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
         db.p.rowlen = kb.rowlen;
         db.blockoff = kb.blockoff;
         db.doc_off = d_back_total + 1;
-        ka_wave_doc_len_kernel<true, true><<<nblk, 256, 0, s>>>(db, pd, kb);
-        ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(db.blockoff, (int)nblk, d_back_total, nullptr);
-        if (enq_json_write(ka_wave_doc_write_kernel<true, true>, nblk, s, db, d_back_total, pd, kb) != cudaSuccess)
-            return set_status(st, KA_ERR_CUDA);
-        c->launches += 3;
+        if (enq_wave_text<true, true>(c, s, nblk, db, d_back_total, pd, kb) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
     }
     unsigned long long total[2] = {0, (unsigned long long)W};   // the text's bytes and the documents D
     unsigned long long back_total = 0;
@@ -2836,7 +2835,7 @@ int32_t ka_plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, const 
                            int64_t json_cap, int64_t* doc_off, int32_t* wave, int32_t* n_waves, ka_wave_summary* summary,
                            int32_t summary_cap, ka_status* st) {
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, nullptr, st);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, nullptr, nullptr, st);
 }
 
 int32_t ka_plan_waves_send_json(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
@@ -2847,7 +2846,7 @@ int32_t ka_plan_waves_send_json(ka_ctx* c, int32_t T, const int64_t* part_off, c
                                 ka_wave_send_summary* send_summary, int32_t summary_cap, ka_status* st) {
     const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, nullptr, st);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, nullptr, nullptr, st);
 }
 
 int32_t ka_plan_waves_json_parts(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
@@ -2858,7 +2857,7 @@ int32_t ka_plan_waves_json_parts(ka_ctx* c, int32_t T, const int64_t* part_off, 
                                  ka_status* st) {
     const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, &pt, st);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, &pt, nullptr, st);
 }
 
 int32_t ka_plan_waves_send_json_parts(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id, const int64_t* rep_off,
@@ -2871,7 +2870,7 @@ int32_t ka_plan_waves_send_json_parts(ka_ctx* c, int32_t T, const int64_t* part_
     const WaveSend sd{n_send, send_id, max_broker_out, send_summary};
     const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, st);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, nullptr, st);
 }
 
 int32_t ka_plan_waves_json_parts_rollback(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id,
@@ -2884,7 +2883,7 @@ int32_t ka_plan_waves_json_parts_rollback(ka_ctx* c, int32_t T, const int64_t* p
     const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
     const WaveBack bk{back, back_cap, back_off};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, &pt, st, &bk);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, nullptr, &pt, &bk, st);
 }
 
 int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* c, int32_t T, const int64_t* part_off, const int32_t* part_id,
@@ -2900,7 +2899,7 @@ int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* c, int32_t T, const int64
     const WaveParts pt{max_doc_bytes, doc_wave, n_docs};
     const WaveBack bk{back, back_cap, back_off};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
-                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, st, &bk);
+                           name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, &bk, st);
 }
 
 }  // extern "C"

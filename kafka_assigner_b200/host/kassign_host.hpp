@@ -301,7 +301,7 @@ public:
     }
 
     // planWaves with every wave's document built on the device (ka_plan_waves_json): docs[v] equals
-    // newAssignmentJson(planWaves(...).waves[v]). Topic names that org.json would escape take exactly that host path instead.
+    // newAssignmentJson(planWaves(...).waves[v]). Topic names that org.json would escape take the host emitter instead.
     struct WaveDocs {
         ka_status status;   // re-throw with throwForStatus; on an error summary and docs are empty
         std::vector<ka_wave_summary> summary;
@@ -310,12 +310,12 @@ public:
     };
     WaveDocs planWavesJson(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                            const std::vector<std::map<int, int64_t>>& weights = {}) {
-        return planWavesJsonWith(topics, proposed, maxBrokerIn, nullptr, weights);
+        return docsOf(waveDocuments(topics, proposed, maxBrokerIn, nullptr, false, nullptr, weights));
     }
     // planWavesJson under a sender budget too (ka_plan_waves_send_json); sendSummary is filled.
     WaveDocs planWavesJson(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                            const SendBudget& send, const std::vector<std::map<int, int64_t>>& weights = {}) {
-        return planWavesJsonWith(topics, proposed, maxBrokerIn, &send, weights);
+        return docsOf(waveDocuments(topics, proposed, maxBrokerIn, nullptr, false, &send, weights));
     }
 
     // planWavesJson with every wave cut into parts of at most maxDocBytes bytes (ka_plan_waves_json_parts): documents that run
@@ -334,12 +334,12 @@ public:
     };
     WaveParts planWaveParts(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                             int64_t maxDocBytes, const std::vector<std::map<int, int64_t>>& weights = {}) {
-        return planWavePartsWith(topics, proposed, maxBrokerIn, maxDocBytes, nullptr, weights);
+        return partsOf(waveDocuments(topics, proposed, maxBrokerIn, &maxDocBytes, false, nullptr, weights));
     }
     // planWaveParts under a sender budget too (ka_plan_waves_send_json_parts); sendSummary is filled.
     WaveParts planWaveParts(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
                             int64_t maxDocBytes, const SendBudget& send, const std::vector<std::map<int, int64_t>>& weights = {}) {
-        return planWavePartsWith(topics, proposed, maxBrokerIn, maxDocBytes, &send, weights);
+        return partsOf(waveDocuments(topics, proposed, maxBrokerIn, &maxDocBytes, false, &send, weights));
     }
 
     // planWaveParts with every part's rollback document beside it (ka_plan_waves_json_parts_rollback): rollback[d] equals
@@ -358,13 +358,13 @@ public:
     };
     WaveRollback planWavePartsRollback(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
                                        int64_t maxBrokerIn, int64_t maxDocBytes, const std::vector<std::map<int, int64_t>>& weights = {}) {
-        return planWavePartsRollbackWith(topics, proposed, maxBrokerIn, maxDocBytes, nullptr, weights);
+        return waveDocuments(topics, proposed, maxBrokerIn, &maxDocBytes, true, nullptr, weights);
     }
     // planWavePartsRollback under a sender budget too (ka_plan_waves_send_json_parts_rollback); sendSummary is filled.
     WaveRollback planWavePartsRollback(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
                                        int64_t maxBrokerIn, int64_t maxDocBytes, const SendBudget& send,
                                        const std::vector<std::map<int, int64_t>>& weights = {}) {
-        return planWavePartsRollbackWith(topics, proposed, maxBrokerIn, maxDocBytes, &send, weights);
+        return waveDocuments(topics, proposed, maxBrokerIn, &maxDocBytes, true, &send, weights);
     }
 
 private:
@@ -414,13 +414,17 @@ private:
             }
         return res;
     }
-    WaveDocs planWavesJsonWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
-                               const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
-    WaveParts planWavePartsWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
-                                int64_t maxDocBytes, const SendBudget* send, const std::vector<std::map<int, int64_t>>& weights);
-    WaveRollback planWavePartsRollbackWith(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed,
-                                           int64_t maxBrokerIn, int64_t maxDocBytes, const SendBudget* send,
-                                           const std::vector<std::map<int, int64_t>>& weights);
+    // The one path of the six wave document entry points, each step once: with no maxDocBytes ka_plan_waves(_send)_json (parts
+    // are the wave documents, partWave 1..W), else their _parts forms, and with rollback their _parts_rollback forms.
+    WaveRollback waveDocuments(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                               const int64_t* maxDocBytes, bool rollback, const SendBudget* send,
+                               const std::vector<std::map<int, int64_t>>& weights);
+    static WaveDocs docsOf(WaveRollback&& r) {
+        return WaveDocs{r.status, std::move(r.summary), std::move(r.parts), std::move(r.sendSummary)};
+    }
+    static WaveParts partsOf(WaveRollback&& r) {
+        return WaveParts{r.status, std::move(r.summary), std::move(r.parts), std::move(r.partWave), std::move(r.sendSummary)};
+    }
 
 public:
 
@@ -746,124 +750,6 @@ inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicIn
     return std::string(json.get(), (size_t)bytes);
 }
 
-inline KafkaTopicAssigner::WaveDocs KafkaTopicAssigner::planWavesJsonWith(const std::vector<TopicInput>& topics,
-                                                                          const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
-                                                                          const SendBudget* send,
-                                                                          const std::vector<std::map<int, int64_t>>& weights) {
-    for (const auto& t : topics)
-        if (needsJsonEscape(t.name)) {   // the host emitter over the waves of planWaves
-            const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights);
-            WaveDocs res{plan.status, plan.summary, {}, plan.sendSummary};
-            for (const auto& wave : plan.waves) res.docs.push_back(newAssignmentJson(wave));
-            return res;
-        }
-    const Flat f = flatten(topics, -1);
-    const ProposedRows p = proposedRows(topics, proposed, weights);
-    const size_t Q = f.partId.size();
-    std::string names;
-    std::vector<int64_t> nameOff(1, 0);
-    const int64_t cap = waveNames(f, p.stride, names, nameOff);
-    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
-    std::vector<int64_t> docOff(Q + 1, 0);
-    WaveDocs res{};
-    res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
-    int32_t W = 0;
-    const int64_t* w = p.w.empty() ? nullptr : p.w.data();
-    if (!send) {
-        ka_plan_waves_json(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(), p.stride,
-                           p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, names.data(), nameOff.data(), json.get(), cap,
-                           docOff.data(), nullptr, &W, res.summary.data(), (int32_t)res.summary.size(), &res.status);
-    } else {
-        res.sendSummary.resize(res.summary.size());
-        ka_plan_waves_send_json(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
-                                p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, (int32_t)send->sendBrokers.size(),
-                                send->sendBrokers.data(), send->maxBrokerOut, names.data(), nameOff.data(), json.get(), cap,
-                                docOff.data(), nullptr, &W, res.summary.data(), res.sendSummary.data(), (int32_t)res.summary.size(),
-                                &res.status);
-    }
-    if (res.status.code != KA_OK) return WaveDocs{res.status, {}, {}, {}};
-    res.summary.resize(W);
-    if (send) res.sendSummary.resize(W);
-    for (int32_t v = 0; v < W; ++v) res.docs.emplace_back(json.get() + docOff[v], (size_t)(docOff[v + 1] - docOff[v]));
-    return res;
-}
-
-inline KafkaTopicAssigner::WaveParts KafkaTopicAssigner::planWavePartsWith(const std::vector<TopicInput>& topics,
-                                                                           const std::vector<TopicOutput>& proposed,
-                                                                           int64_t maxBrokerIn, int64_t maxDocBytes,
-                                                                           const SendBudget* send,
-                                                                           const std::vector<std::map<int, int64_t>>& weights) {
-    const Flat f = flatten(topics, -1);
-    const ProposedRows p = proposedRows(topics, proposed, weights);
-    const size_t Q = f.partId.size();
-    for (const auto& t : topics)
-        if (needsJsonEscape(t.name)) {   // the host emitter over the rows of planWaves, cut by the rule of planWaveParts
-            std::vector<int32_t> rowWave;
-            const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights, &rowWave);
-            WaveParts res{plan.status, plan.summary, {}, {}, plan.sendSummary};
-            if (res.status.code == KA_OK && maxDocBytes < 1) res.status.code = KA_ERR_BAD_ARG;
-            if (res.status.code != KA_OK) return WaveParts{res.status, {}, {}, {}, {}};
-            std::vector<std::vector<std::string>> recs(plan.summary.size());
-            for (size_t t = 0; t < f.names.size(); ++t)
-                for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
-                    if (rowWave[r] == 0) continue;
-                    std::string rec;
-                    appendRecord(rec, f.names[t], f.partId[r], p.newBroker.data() + r * p.stride, (size_t)p.newLen[r]);
-                    if (29 + (int64_t)rec.size() > maxDocBytes) {
-                        ka_status st{};
-                        st.code = KA_ERR_LIMIT;
-                        st.a = (int32_t)r;
-                        st.b = (int32_t)std::min<int64_t>(29 + (int64_t)rec.size(), INT32_MAX);
-                        return WaveParts{st, {}, {}, {}, {}};
-                    }
-                    recs[rowWave[r] - 1].push_back(std::move(rec));
-                }
-            for (size_t v = 0; v < recs.size(); ++v) {
-                int64_t size = 0;   // of the current part, 0 before the wave's first
-                for (const std::string& rec : recs[v]) {
-                    if (size > 0 && size + 1 + (int64_t)rec.size() <= maxDocBytes) {
-                        res.parts.back().insert(res.parts.back().size() - 14, "," + rec);
-                        size += 1 + (int64_t)rec.size();
-                    } else {
-                        res.parts.push_back("{\"partitions\":[" + rec + "],\"version\":1}");
-                        res.partWave.push_back((int32_t)v + 1);
-                        size = 29 + (int64_t)rec.size();
-                    }
-                }
-            }
-            return res;
-        }
-    std::string names;
-    std::vector<int64_t> nameOff(1, 0);
-    const int64_t cap = waveNames(f, p.stride, names, nameOff);
-    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]);
-    std::vector<int64_t> docOff(Q + 1, 0);
-    std::vector<int32_t> docWave(std::max<size_t>(Q, 1), 0);
-    WaveParts res{};
-    res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
-    int32_t W = 0, D = 0;
-    const int64_t* w = p.w.empty() ? nullptr : p.w.data();
-    if (!send) {
-        ka_plan_waves_json_parts(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
-                                 p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, names.data(), nameOff.data(),
-                                 json.get(), cap, maxDocBytes, docOff.data(), docWave.data(), &D, nullptr, &W, res.summary.data(),
-                                 (int32_t)res.summary.size(), &res.status);
-    } else {
-        res.sendSummary.resize(res.summary.size());
-        ka_plan_waves_send_json_parts(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
-                                      p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, (int32_t)send->sendBrokers.size(),
-                                      send->sendBrokers.data(), send->maxBrokerOut, names.data(), nameOff.data(), json.get(), cap,
-                                      maxDocBytes, docOff.data(), docWave.data(), &D, nullptr, &W, res.summary.data(),
-                                      res.sendSummary.data(), (int32_t)res.summary.size(), &res.status);
-    }
-    if (res.status.code != KA_OK) return WaveParts{res.status, {}, {}, {}, {}};
-    res.summary.resize(W);
-    if (send) res.sendSummary.resize(W);
-    for (int32_t d = 0; d < D; ++d) res.parts.emplace_back(json.get() + docOff[d], (size_t)(docOff[d + 1] - docOff[d]));
-    res.partWave.assign(docWave.begin(), docWave.begin() + D);
-    return res;
-}
-
 // Kafka 0.10 ZkUtils.formatAsReassignmentJson shape (used for "CURRENT ASSIGNMENT:", KAG:103-111): scala Map literals keep
 // insertion order for <= 4 entries: version, partitions / topic, partition, replicas.
 inline std::string kafkaReassignmentJson(const std::vector<TopicInput>& topics) {
@@ -879,90 +765,115 @@ inline std::string kafkaReassignmentJson(const std::vector<TopicInput>& topics) 
     return s;
 }
 
-inline KafkaTopicAssigner::WaveRollback KafkaTopicAssigner::planWavePartsRollbackWith(const std::vector<TopicInput>& topics,
-                                                                                      const std::vector<TopicOutput>& proposed,
-                                                                                      int64_t maxBrokerIn, int64_t maxDocBytes,
-                                                                                      const SendBudget* send,
-                                                                                      const std::vector<std::map<int, int64_t>>& weights) {
+inline KafkaTopicAssigner::WaveRollback KafkaTopicAssigner::waveDocuments(const std::vector<TopicInput>& topics,
+                                                                          const std::vector<TopicOutput>& proposed, int64_t maxBrokerIn,
+                                                                          const int64_t* maxDocBytes, bool rollback,
+                                                                          const SendBudget* send,
+                                                                          const std::vector<std::map<int, int64_t>>& weights) {
     const Flat f = flatten(topics, -1);
     const ProposedRows p = proposedRows(topics, proposed, weights);
     const size_t Q = f.partId.size();
-    for (const auto& t : topics)
-        if (needsJsonEscape(t.name)) {   // the host emitters over the rows of planWaves, cut by the rule of planWavePartsRollback
-            std::vector<int32_t> rowWave;
-            const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights, &rowWave);
-            WaveRollback res{plan.status, plan.summary, {}, {}, {}, plan.sendSummary};
-            if (res.status.code == KA_OK && maxDocBytes < 1) res.status.code = KA_ERR_BAD_ARG;
-            if (res.status.code != KA_OK) return WaveRollback{res.status, {}, {}, {}, {}, {}};
-            std::vector<std::vector<std::pair<std::string, std::string>>> recs(plan.summary.size());
-            for (size_t t = 0; t < f.names.size(); ++t)
-                for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
-                    if (rowWave[r] == 0) continue;
-                    std::string rec, back;
-                    appendRecord(rec, f.names[t], f.partId[r], p.newBroker.data() + r * p.stride, (size_t)p.newLen[r]);
+    WaveRollback res{};
+    if (std::any_of(topics.begin(), topics.end(), [](const TopicInput& t) { return needsJsonEscape(t.name); })) {
+        // the host emitters over the rows of planWaves, cut by the same greedy rule; no limit: every wave one part
+        std::vector<int32_t> rowWave;
+        const WavePlan plan = planWavesWith(topics, proposed, maxBrokerIn, send, weights, &rowWave);
+        const int64_t L = maxDocBytes ? *maxDocBytes : INT64_MAX;
+        res = WaveRollback{plan.status, plan.summary, {}, {}, {}, plan.sendSummary};
+        if (res.status.code == KA_OK && L < 1) res.status.code = KA_ERR_BAD_ARG;
+        if (res.status.code != KA_OK) return WaveRollback{res.status, {}, {}, {}, {}, {}};
+        std::vector<std::vector<std::pair<std::string, std::string>>> recs(plan.summary.size());   // (record, rollback record)
+        for (size_t t = 0; t < f.names.size(); ++t)
+            for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
+                if (rowWave[r] == 0) continue;
+                std::string rec, back;
+                appendRecord(rec, f.names[t], f.partId[r], p.newBroker.data() + r * p.stride, (size_t)p.newLen[r]);
+                if (rollback)
                     appendCurrentRecord(back, f.names[t], f.partId[r], f.cur.data() + f.repOff[r], (size_t)(f.repOff[r + 1] - f.repOff[r]));
-                    const int64_t longest = 29 + (int64_t)std::max(rec.size(), back.size());
-                    if (longest > maxDocBytes) {
-                        ka_status st{};
-                        st.code = KA_ERR_LIMIT;
-                        st.a = (int32_t)r;
-                        st.b = (int32_t)std::min<int64_t>(longest, INT32_MAX);
-                        return WaveRollback{st, {}, {}, {}, {}, {}};
-                    }
-                    recs[rowWave[r] - 1].emplace_back(std::move(rec), std::move(back));
+                const int64_t longest = 29 + (int64_t)std::max(rec.size(), back.size());
+                if (longest > L) {
+                    ka_status st{};
+                    st.code = KA_ERR_LIMIT;
+                    st.a = (int32_t)r;
+                    st.b = (int32_t)std::min<int64_t>(longest, INT32_MAX);
+                    return WaveRollback{st, {}, {}, {}, {}, {}};
                 }
-            for (size_t v = 0; v < recs.size(); ++v) {
-                int64_t size = 0, backSize = 0;   // of the current part's two documents, 0 before the wave's first
-                for (const auto& rb : recs[v]) {
-                    const int64_t n = (int64_t)rb.first.size(), m = (int64_t)rb.second.size();
-                    if (size > 0 && size + 1 + n <= maxDocBytes && backSize + 1 + m <= maxDocBytes) {
-                        res.parts.back().insert(res.parts.back().size() - 14, "," + rb.first);
-                        res.rollback.back().insert(res.rollback.back().size() - 2, "," + rb.second);
-                        size += 1 + n;
-                        backSize += 1 + m;
-                    } else {
-                        res.parts.push_back("{\"partitions\":[" + rb.first + "],\"version\":1}");
-                        res.rollback.push_back("{\"version\":1,\"partitions\":[" + rb.second + "]}");
-                        res.partWave.push_back((int32_t)v + 1);
-                        size = 29 + n;
-                        backSize = 29 + m;
-                    }
+                recs[rowWave[r] - 1].emplace_back(std::move(rec), std::move(back));
+            }
+        for (size_t v = 0; v < recs.size(); ++v) {
+            // the current part's two document sizes, 0 before the wave's first; without rollback the empty back side never binds
+            int64_t size = 0, backSize = 0;
+            for (const auto& rb : recs[v]) {
+                const int64_t n = (int64_t)rb.first.size(), m = (int64_t)rb.second.size();
+                if (size > 0 && size + 1 + n <= L && backSize + 1 + m <= L) {
+                    res.parts.back().insert(res.parts.back().size() - 14, "," + rb.first);
+                    if (rollback) res.rollback.back().insert(res.rollback.back().size() - 2, "," + rb.second);
+                    size += 1 + n;
+                    backSize += 1 + m;
+                } else {
+                    res.parts.push_back("{\"partitions\":[" + rb.first + "],\"version\":1}");
+                    if (rollback) res.rollback.push_back("{\"version\":1,\"partitions\":[" + rb.second + "]}");
+                    res.partWave.push_back((int32_t)v + 1);
+                    size = 29 + n;
+                    backSize = 29 + m;
                 }
             }
-            return res;
         }
+        return res;
+    }
     std::string names;
     std::vector<int64_t> nameOff(1, 0);
     const int64_t cap = waveNames(f, p.stride, names, nameOff);
-    int64_t backCap = 12 * (int64_t)f.cur.size();   // per row 79 + its topic's name, 12 per current broker
-    for (size_t t = 0; t < f.names.size(); ++t) backCap += (f.partOff[t + 1] - f.partOff[t]) * (79 + (int64_t)f.names[t].size());
-    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]), back(new char[std::max<int64_t>(backCap, 1)]);
+    int64_t backCap = 0;
+    if (rollback) {   // per row 79 + its topic's name, 12 per current broker
+        backCap = 12 * (int64_t)f.cur.size();
+        for (size_t t = 0; t < f.names.size(); ++t) backCap += (f.partOff[t + 1] - f.partOff[t]) * (79 + (int64_t)f.names[t].size());
+    }
+    std::unique_ptr<char[]> json(new char[std::max<int64_t>(cap, 1)]), back(rollback ? new char[std::max<int64_t>(backCap, 1)] : nullptr);
     std::vector<int64_t> docOff(Q + 1, 0), backOff(Q + 1, 0);
     std::vector<int32_t> docWave(std::max<size_t>(Q, 1), 0);
-    WaveRollback res{};
     res.summary.resize(std::max<size_t>(Q, 1));   // W never exceeds Q: one call
+    if (send) res.sendSummary.resize(res.summary.size());
     int32_t W = 0, D = 0;
-    const int64_t* w = p.w.empty() ? nullptr : p.w.data();
-    if (!send) {
-        ka_plan_waves_json_parts_rollback(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(), f.cur.data(),
-                                          p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn, names.data(), nameOff.data(),
-                                          json.get(), cap, maxDocBytes, docOff.data(), docWave.data(), &D, back.get(), backCap,
-                                          backOff.data(), nullptr, &W, res.summary.data(), (int32_t)res.summary.size(), &res.status);
-    } else {
-        res.sendSummary.resize(res.summary.size());
-        ka_plan_waves_send_json_parts_rollback(ctx_, (int32_t)topics.size(), f.partOff.data(), f.partId.data(), f.repOff.data(),
-                                               f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(), w, maxBrokerIn,
-                                               (int32_t)send->sendBrokers.size(), send->sendBrokers.data(), send->maxBrokerOut,
-                                               names.data(), nameOff.data(), json.get(), cap, maxDocBytes, docOff.data(),
-                                               docWave.data(), &D, back.get(), backCap, backOff.data(), nullptr, &W,
-                                               res.summary.data(), res.sendSummary.data(), (int32_t)res.summary.size(), &res.status);
-    }
+    const int32_t T = (int32_t)topics.size(), S = (int32_t)res.summary.size();
+    const int64_t *po = f.partOff.data(), *ro = f.repOff.data(), *w = p.w.empty() ? nullptr : p.w.data();
+    const int32_t *pid = f.partId.data(), *cu = f.cur.data(), *nl = p.newLen.data(), *nb = p.newBroker.data();
+    const int32_t nSend = send ? (int32_t)send->sendBrokers.size() : 0;
+    const int32_t* sendId = send ? send->sendBrokers.data() : nullptr;
+    const int64_t C = send ? send->maxBrokerOut : 0;
+    ka_wave_summary* sum = res.summary.data();
+    ka_wave_send_summary* sendSum = res.sendSummary.data();
+    if (!maxDocBytes && !send)
+        ka_plan_waves_json(ctx_, T, po, pid, ro, cu, p.stride, nl, nb, w, maxBrokerIn, names.data(), nameOff.data(), json.get(), cap,
+                           docOff.data(), nullptr, &W, sum, S, &res.status);
+    else if (!maxDocBytes)
+        ka_plan_waves_send_json(ctx_, T, po, pid, ro, cu, p.stride, nl, nb, w, maxBrokerIn, nSend, sendId, C, names.data(), nameOff.data(),
+                                json.get(), cap, docOff.data(), nullptr, &W, sum, sendSum, S, &res.status);
+    else if (!rollback && !send)
+        ka_plan_waves_json_parts(ctx_, T, po, pid, ro, cu, p.stride, nl, nb, w, maxBrokerIn, names.data(), nameOff.data(), json.get(), cap,
+                                 *maxDocBytes, docOff.data(), docWave.data(), &D, nullptr, &W, sum, S, &res.status);
+    else if (!rollback)
+        ka_plan_waves_send_json_parts(ctx_, T, po, pid, ro, cu, p.stride, nl, nb, w, maxBrokerIn, nSend, sendId, C, names.data(),
+                                      nameOff.data(), json.get(), cap, *maxDocBytes, docOff.data(), docWave.data(), &D, nullptr, &W, sum,
+                                      sendSum, S, &res.status);
+    else if (!send)
+        ka_plan_waves_json_parts_rollback(ctx_, T, po, pid, ro, cu, p.stride, nl, nb, w, maxBrokerIn, names.data(), nameOff.data(),
+                                          json.get(), cap, *maxDocBytes, docOff.data(), docWave.data(), &D, back.get(), backCap,
+                                          backOff.data(), nullptr, &W, sum, S, &res.status);
+    else
+        ka_plan_waves_send_json_parts_rollback(ctx_, T, po, pid, ro, cu, p.stride, nl, nb, w, maxBrokerIn, nSend, sendId, C, names.data(),
+                                               nameOff.data(), json.get(), cap, *maxDocBytes, docOff.data(), docWave.data(), &D,
+                                               back.get(), backCap, backOff.data(), nullptr, &W, sum, sendSum, S, &res.status);
     if (res.status.code != KA_OK) return WaveRollback{res.status, {}, {}, {}, {}, {}};
+    if (!maxDocBytes) {   // one document per wave
+        D = W;
+        for (int32_t v = 0; v < W; ++v) docWave[v] = v + 1;
+    }
     res.summary.resize(W);
     if (send) res.sendSummary.resize(W);
     for (int32_t d = 0; d < D; ++d) {
         res.parts.emplace_back(json.get() + docOff[d], (size_t)(docOff[d + 1] - docOff[d]));
-        res.rollback.emplace_back(back.get() + backOff[d], (size_t)(backOff[d + 1] - backOff[d]));
+        if (rollback) res.rollback.emplace_back(back.get() + backOff[d], (size_t)(backOff[d + 1] - backOff[d]));
     }
     res.partWave.assign(docWave.begin(), docWave.begin() + D);
     return res;

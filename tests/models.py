@@ -1,6 +1,6 @@
 """The plain-Python models the device is checked against, each written once: the move summary, the wave rule (with and
-without a sender budget), the reassignment JSON printers, the schedule model's records, slot chains and the expected counter
-histogram, and kernel A's shared-memory budget.
+without a sender budget), the reassignment JSON printers, the wave documents and their greedy cut, the schedule model's records,
+slot chains and the expected counter histogram, and kernel A's shared-memory budget.
 Each restates a rule of include/kassign.h. This module imports numpy and the status codes only: it never loads the library
 or the oracle, so CPU tests, GPU tests and tests/tools can all use it."""
 import numpy as np
@@ -146,6 +146,17 @@ def document(records):
     return '{"partitions":[' + ",".join(records) + '],"version":1}'
 
 
+def current_record(name, partition, replicas):
+    """The rollback record: the host's CURRENT ASSIGNMENT record (Kafka 0.10 ZkUtils.formatAsReassignmentJson key order) of a
+    partition on its current list `replicas`, printed as given."""
+    return '{"topic":%s,"partition":%d,"replicas":[%s]}' % (quote(name), partition, ",".join(str(int(b)) for b in replicas))
+
+
+def rollback_document(records):
+    """The rollback document of these current records (str)."""
+    return '{"version":1,"partitions":[' + ",".join(records) + ']}'
+
+
 EMPTY_DOCUMENT = document([])
 
 
@@ -166,19 +177,52 @@ def json_bound(names, part_off, stride):
     return sum(int(part_off[t + 1] - part_off[t]) * (79 + 12 * stride + len(n.encode())) for t, n in enumerate(names))
 
 
-def wave_docs(topic_names, part_off, part_id, rep_off, cur, out, out_len, ids, B, weight=None, send=None):
-    """(docs [bytes per wave], wave, summary, (code, a, b)): the waves of plan_waves, each printed as the device prints it: the
-    records of its rows in input row order; ordinals where part_id is None."""
+def cut_parts(sides, L):
+    """The greedy cut of ka_plan_waves_json_parts(_rollback) over one wave's records, in order: [(first, end)] runs. `sides`
+    holds one list of record byte lengths, or two with the rollback records'. A part of n records is 29 + their bytes + (n - 1)
+    long on each side; a record joins the current part while every side stays <= L."""
+    runs, size = [], [0] * len(sides)
+    for i, lens in enumerate(zip(*sides)):
+        if runs and all(s + 1 + b <= L for s, b in zip(size, lens)):
+            runs[-1] = (runs[-1][0], i + 1)
+            size = [s + 1 + b for s, b in zip(size, lens)]
+        else:
+            runs.append((i, i + 1))
+            size = [29 + b for b in lens]
+    return runs
+
+
+def wave_documents(topic_names, part_off, part_id, rep_off, cur, out, out_len, ids, B, weight=None, send=None, L=None,
+                   rollback=False):
+    """(docs [bytes], backs [bytes] or None, doc_wave, wave, summary, (code, a, b)) of the six wave document entry points, the
+    shape Solver._wave_documents returns: the records of every wave of plan_waves in input row order (ordinals where part_id is
+    None), one document per wave with L None (ka_plan_waves(_send)_json), else cut by cut_parts (their _parts forms), and with
+    rollback backs[d] the current records of docs[d]'s rows (their _parts_rollback forms). A changed row whose one-record
+    document on either side exceeds L, the lowest in input order, gives (KA_ERR_LIMIT, row, the longer length) and no docs."""
     wave, summ, st = plan_waves(rep_off, cur, out, out_len, ids, B, weight, send)
     if st[0] != 0:
-        return None, wave, summ, st
+        return None, None, None, wave, summ, st
     recs = [[] for _ in summ]
     for t, name in enumerate(topic_names):
         for g in range(int(part_off[t]), int(part_off[t + 1])):
             if wave[g]:
                 p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
-                recs[wave[g] - 1].append(record(name, p, out[g][:int(out_len[g])]))
-    return [document(r).encode() for r in recs], wave, summ, st
+                sides = [record(name, p, out[g][:int(out_len[g])])]
+                if rollback:
+                    sides.append(current_record(name, p, cur[int(rep_off[g]):int(rep_off[g + 1])]))
+                longest = 29 + max(len(x.encode()) for x in sides)
+                if L is not None and longest > L:
+                    return None, None, None, wave, summ, (_native.KA_ERR_LIMIT, g, min(longest, 2 ** 31 - 1))
+                recs[wave[g] - 1].append(sides)
+    docs, backs, doc_wave = [], [] if rollback else None, []
+    for v, rs in enumerate(recs, 1):
+        runs = [(0, len(rs))] if L is None else cut_parts([[len(r[k].encode()) for r in rs] for k in range(len(rs[0]))], L)
+        for a, b in runs:
+            docs.append(document([r[0] for r in rs[a:b]]).encode())
+            if rollback:
+                backs.append(rollback_document([r[1] for r in rs[a:b]]).encode())
+            doc_wave.append(v)
+    return docs, backs, doc_wave, wave, summ, st
 
 
 # ---- the leader-order schedule and the counters --------------------------------------------------------------------------

@@ -287,10 +287,11 @@ def reset_plans(request, tmp_path_factory, native_lib):
         rounds = chain_rounds(records, senders if send else None)
         names, part_off = list(inp["names"]), inp["part_off"]
         if send:
-            e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, None, *args, inp["ids"], int(inp["B"]), inp["weight"],
-                                                            send=(inp["send_smem"], int(inp["C"])))
+            e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(names, part_off, None, *args, inp["ids"], int(inp["B"]),
+                                                                       inp["weight"], send=(inp["send_smem"], int(inp["C"])))
         else:
-            e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, None, *args, inp["ids"], int(inp["B"]), inp["weight"])
+            e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(names, part_off, None, *args, inp["ids"], int(inp["B"]),
+                                                                       inp["weight"])
         assert e_st == (0, 0, 0)
         e_summ = _summary_array(e_summ, WAVE_SEND_SUMMARY_DTYPE if send else WAVE_SUMMARY_DTYPE)
         out, _ = child.communicate(timeout=max(1.0, CHILD_TIMEOUT - (time.monotonic() - t0)))
@@ -365,7 +366,7 @@ def test_scattered_documents_over_large_tiles(native_lib):
     names = ["scatter-%d" % t for t in range(2000)]
     assert Q > 2048 * 1024
     docs, wave, summ, st = s.plan_waves_json(names, part_off, None, rep_off, cur, out, out_len, 1)
-    e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 1)
+    e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 1)
     assert st.code == 0 and e_st == (0, 0, 0) and 256 <= len(e_docs) <= 65535
     assert np.array_equal(wave, e_wave)
     e_summ = _summary_array(e_summ, WAVE_SUMMARY_DTYPE)
@@ -395,7 +396,7 @@ def test_wave_documents_past_4_gib(native_lib):
     rep_off, cur = util.cur_lists(cur_lists)
     out, out_len = util.rows(new_lists, 2)
     ph = ["@%d@" % t for t in range(len(names))]
-    e_docs, e_wave, e_summ, e_st = models.wave_docs(ph, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)
+    e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(ph, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)
     assert e_st == (0, 0, 0)
     real = [n.encode() for n in names]
     topic = re.compile(rb'"topic":"@(\d+)@"')

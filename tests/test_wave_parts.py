@@ -1,5 +1,5 @@
 """ka_plan_waves_json_parts and ka_plan_waves_send_json_parts on the GPU: every part, its wave, D, wave and the summaries of the
-device must equal `part_models.wave_parts` byte for byte; with a limit above every wave the text and doc_off must be those of
+device must equal `models.wave_documents` byte for byte; with a limit above every wave the text and doc_off must be those of
 ka_plan_waves(_send)_json."""
 import ctypes
 import json
@@ -11,43 +11,11 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
-from tests import models, part_models, util
+from tests import models, util
 
 pytestmark = pytest.mark.gpu
 BAD, LIMIT = _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT
 ZNODE = 0xFFFFF   # ZooKeeper's default jute.maxbuffer
-
-
-def _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, L, weight=None, C=None, send_ids=None):
-    """plan_wave_parts_json against the model; with C a sender budget over send_ids (None: the Solver's table). Returns
-    (parts, part_wave, st)."""
-    send_ids = list(np.asarray(s.broker_id if send_ids is None else send_ids))
-    send = None if C is None else dict(max_broker_out=C, send_brokers=send_ids)
-    parts, part_wave, wave, summ, st = s.plan_wave_parts_json(names, part_off, part_id, rep_off, cur, out, out_len, B, L, weight=weight,
-                                                              **(send or {}))
-    m_send = None if C is None else (send_ids, C)
-    e_parts, e_wave_of, e_wave, e_summ, e_st = part_models.wave_parts(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, L,
-                                                                 weight, m_send)
-    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
-    if st.code == 0:
-        dtype = WAVE_SUMMARY_DTYPE if C is None else WAVE_SEND_SUMMARY_DTYPE
-        assert np.array_equal(wave, e_wave)
-        assert [util.record_of(x, dtype.names) for x in summ] == e_summ
-        assert part_wave.tolist() == e_wave_of and len(parts) == len(e_parts)
-        for d, (p, e) in enumerate(zip(parts, e_parts)):
-            assert bytes(p) == e, (d, bytes(p)[:200], e[:200])
-    return parts, part_wave, st
-
-
-def _smallest(names, part_off, part_id, out, out_len, wave):
-    """The smallest L that fits every changed row: its longest one-record document."""
-    best = 0
-    for t, name in enumerate(names):
-        for g in range(int(part_off[t]), int(part_off[t + 1])):
-            if wave[g]:
-                p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
-                best = max(best, 29 + len(models.record(name, p, out[g][:int(out_len[g])]).encode()))
-    return best
 
 
 @pytest.mark.parametrize("seed", range(3))
@@ -55,23 +23,15 @@ def test_random_ragged_cases(native_lib, seed):
     s = kab.Solver(0)
     s.set_brokers(*util.table(np.arange(1, 31), 4))
     rng = np.random.default_rng(100 + seed)
-    T = 300
-    sizes = rng.integers(0, 30, T)
-    part_off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-    Q = int(part_off[-1])
-    names = ["ragged.%d.%s" % (t, "y" * int(rng.integers(0, 40))) for t in range(T)]
-    part_id = np.concatenate([np.sort(rng.choice(5000, n, replace=False)) for n in sizes]).astype(np.int32)
-    cur_l, new_l = util.random_wave_case(rng, Q, 30)
-    rep_off, cur = util.cur_lists(cur_l)
-    out, out_len = util.rows(new_l, 3)
-    weight = rng.integers(0, 50, Q).astype(np.int64)
+    names, part_off, part_id, rep_off, cur, out, out_len = util.ragged_wave_case(rng, 300, 30)
+    weight = rng.integers(0, 50, len(out_len)).astype(np.int64)
     for B, w, C in ((1, None, None), (4, None, None), (10 ** 9, None, None), (60, weight, None), (2, None, 3), (80, weight, 200)):
         wave = s.plan_waves(rep_off, cur, out, out_len, B, weight=w)[0]
-        small = _smallest(names, part_off, part_id, out, out_len, wave)
+        small = util.smallest_limit(names, part_off, part_id, rep_off, cur, out, out_len, wave)
         for L in (small, small + 1, 500, 3000, 70000, ZNODE):
-            parts, part_wave, st = _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, L, w, C)
+            st = util.check_wave_documents(s, names, part_off, part_id, rep_off, cur, out, out_len, B, L, weight=w, C=C)[5]
             assert st.code == 0
-        parts, _, _ = _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, small, w, C)
+        parts = util.check_wave_documents(s, names, part_off, part_id, rep_off, cur, out, out_len, B, small, weight=w, C=C)[0]
         assert len(parts) >= len(set(wave[wave > 0].tolist()))
 
 
@@ -92,8 +52,8 @@ def test_a_limit_above_every_wave_gives_the_wave_documents(native_lib, send):
         # doc_off: the parts lie back to back from the buffer's start
         text = b"".join(bytes(d) for d in docs)
         assert bytes(buf[:len(text)]) == text
-        _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, 4096, None, 5 if send else None,
-               cl.all_broker_id)
+        util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, 4096,
+                                  C=5 if send else None, send_ids=cl.all_broker_id)
 
 
 def test_parts_straddle_ctas_and_the_staging_limit(native_lib):
@@ -111,7 +71,7 @@ def test_parts_straddle_ctas_and_the_staging_limit(native_lib):
     out, out_len = util.rows(new_l, 3)
     for B in (50, 10 ** 6):
         for L in (1000, 5000, 64 * 1024, 200 * 1024, ZNODE):
-            parts, _, st = _check(s, names, part_off, None, rep_off, cur, out, out_len, B, L)
+            parts, _, _, _, _, st = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, B, L)
             assert st.code == 0
     assert len(parts) > 1
 
@@ -129,11 +89,12 @@ def test_one_wave_of_more_than_65536_parts(native_lib, weighted):
     w = np.arange(Q, dtype=np.int64) % 5 if weighted else None
     L = 29 + len(models.record("w", 7, [2, 1]))
     n0 = s.launch_count()
-    parts, part_wave, st = _check(s, names, part_off, part_id, rep_off, cur, out, out_len, 1, L, w)
-    assert st.code == 0 and len(parts) == Q and set(part_wave.tolist()) == {1}
+    st = s.plan_wave_parts_json(names, part_off, part_id, rep_off, cur, out, out_len, 1, L, weight=w)[4]
     # launches: the plan's 7, one radix pass, 4, 2 x 17 - 1 doubling, the 3 text passes
-    assert s.launch_count() - n0 == 7 + 3 + 4 + 33 + 3
-    parts, _, _ = _check(s, names, part_off, part_id, rep_off, cur, out, out_len, 1, 3 * L, w)
+    assert st.code == 0 and s.launch_count() - n0 == 7 + 3 + 4 + 33 + 3
+    parts, _, part_wave, _, _, st = util.check_wave_documents(s, names, part_off, part_id, rep_off, cur, out, out_len, 1, L, weight=w)
+    assert st.code == 0 and len(parts) == Q and set(part_wave.tolist()) == {1}
+    parts = util.check_wave_documents(s, names, part_off, part_id, rep_off, cur, out, out_len, 1, 3 * L, weight=w)[0]
     assert Q // 4 <= len(parts) < Q // 2
 
 
@@ -208,7 +169,7 @@ def test_errors(native_lib):
     o[999, :2], ln[999] = [4, 4], 2
     assert call(L=1, new=o, new_len=ln)[:3] == (BAD, 999, 4)
     # over-long rows come before json_cap; then a text above json_cap is KA_ERR_LIMIT with a = json_cap
-    e_parts = part_models.wave_parts(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, 300)[0]
+    e_parts = models.wave_documents(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, L=300)[0]
     size = sum(len(p) for p in e_parts)
     assert call(L=300, json_cap=size - 1)[:2] == (LIMIT, size - 1)
     assert call(L=longest - 1, json_cap=0)[:3] == (LIMIT, low, longest)
@@ -223,7 +184,8 @@ def test_million_partition_cluster_under_the_znode_limit(native_lib, remove):
     cl = kab.synth.make_ragged_cluster(T=240000, N=400, max_partitions=128, seed=11, remove_frac=remove)
     s, out, out_len, S = util.solved(cl)
     B = len(out_len) if remove == 0.0 else 4000   # everything in wave 1 (one solve's document under the limit), or waves
-    parts, part_wave, st = _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, ZNODE)
+    parts, _, part_wave, _, _, st = util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out,
+                                                              out_len, B, ZNODE)
     assert st.code == 0
     assert (part_wave == 1).sum() >= 25   # the reorder-only rows of wave 1 alone are about 25 MB
     for p in parts:

@@ -1,5 +1,5 @@
 """ka_plan_waves_json_parts_rollback and ka_plan_waves_send_json_parts_rollback on the GPU: every part, every rollback document,
-D, part_wave, wave and the summaries of the device must equal `rollback_models.wave_rollback_parts` byte for byte; every rollback
+D, part_wave, wave and the summaries of the device must equal `models.wave_documents` byte for byte; every rollback
 document must name exactly its part's partitions, in order, on their current lists; where no current list prints longer than
 its new list the results must be those of ka_plan_waves(_send)_json_parts."""
 import ctypes
@@ -13,36 +13,11 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
-from tests import models, part_models, rollback_models, util
+from tests import models, util
 
 pytestmark = pytest.mark.gpu
 BAD, LIMIT = _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT
 ZNODE = 0xFFFFF   # ZooKeeper's default jute.maxbuffer
-
-
-def _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, L, weight=None, C=None, send_ids=None):
-    """plan_wave_parts_rollback_json against the model; with C a sender budget over send_ids (None: the Solver's table).
-    Returns (parts, rollback, part_wave, st)."""
-    send_ids = list(np.asarray(s.broker_id if send_ids is None else send_ids))
-    send = None if C is None else dict(max_broker_out=C, send_brokers=send_ids)
-    parts, rollback, part_wave, wave, summ, st = s.plan_wave_parts_rollback_json(names, part_off, part_id, rep_off, cur, out, out_len, B,
-                                                                                 L, weight=weight, **(send or {}))
-    m_send = None if C is None else (send_ids, C)
-    e_parts, e_back, e_wave_of, e_wave, e_summ, e_st = rollback_models.wave_rollback_parts(names, part_off, part_id, rep_off, cur, out,
-                                                                                       out_len, s.broker_id, B, L, weight, m_send)
-    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
-    if st.code == 0:
-        dtype = WAVE_SUMMARY_DTYPE if C is None else WAVE_SEND_SUMMARY_DTYPE
-        assert np.array_equal(wave, e_wave)
-        assert [util.record_of(x, dtype.names) for x in summ] == e_summ
-        assert part_wave.tolist() == e_wave_of and len(parts) == len(e_parts) and len(rollback) == len(e_back)
-        for d, (p, e) in enumerate(zip(parts, e_parts)):
-            assert bytes(p) == e, (d, bytes(p)[:200], e[:200])
-        for d, (p, e) in enumerate(zip(rollback, e_back)):
-            assert bytes(p) == e, (d, bytes(p)[:200], e[:200])
-    else:
-        assert parts == [] and rollback == [] and len(part_wave) == len(wave) == len(summ) == 0
-    return parts, rollback, part_wave, st
 
 
 def _current(names, part_off, part_id, rep_off, cur):
@@ -65,49 +40,20 @@ def _check_pairs(parts, rollback, current, L):
         assert all(r["replicas"] == current[(r["topic"], r["partition"])] for r in back["partitions"])
 
 
-def _smallest(names, part_off, part_id, rep_off, cur, out, out_len, wave):
-    """The smallest L that fits every changed row: its longest one-record document on either side."""
-    best = 0
-    for t, name in enumerate(names):
-        for g in range(int(part_off[t]), int(part_off[t + 1])):
-            if wave[g]:
-                p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
-                fwd = models.record(name, p, out[g][:int(out_len[g])])
-                back = rollback_models.current_record(name, p, cur[int(rep_off[g]):int(rep_off[g + 1])])
-                best = max(best, 29 + len(fwd.encode()), 29 + len(back.encode()))
-    return best
-
-
-def _ragged(rng, T, N, shrink=0.0):
-    sizes = rng.integers(0, 30, T)
-    part_off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-    Q = int(part_off[-1])
-    names = ["ragged.%d.%s" % (t, "y" * int(rng.integers(0, 40))) for t in range(T)]
-    part_id = np.concatenate([np.sort(rng.choice(5000, n, replace=False)) for n in sizes]).astype(np.int32)
-    cur_l, new_l = util.random_wave_case(rng, Q, N)
-    for g in range(Q):   # some replication-factor reductions: a 3-broker list onto its first one or two
-        if rng.random() < shrink:
-            cur_l[g] = [int(x) for x in rng.choice(np.arange(1, N + 1), 3, replace=False)]
-            new_l[g] = cur_l[g][:int(rng.integers(1, 3))]
-    rep_off, cur = util.cur_lists(cur_l)
-    out, out_len = util.rows(new_l, 3)
-    return names, part_off, part_id, rep_off, cur, out, out_len
-
-
 @pytest.mark.parametrize("seed", range(3))
 def test_random_ragged_cases(native_lib, seed):
     s = kab.Solver(0)
     s.set_brokers(*util.table(np.arange(1, 31), 4))
     rng = np.random.default_rng(200 + seed)
-    case = _ragged(rng, 300, 30, shrink=0.3)
+    case = util.ragged_wave_case(rng, 300, 30, shrink=0.3)
     names, part_off, part_id, rep_off, cur, out, out_len = case
     current = _current(names, part_off, part_id, rep_off, cur)
     weight = rng.integers(0, 50, len(out_len)).astype(np.int64)
     for B, w, C in ((1, None, None), (4, None, None), (10 ** 9, None, None), (60, weight, None), (2, None, 3), (80, weight, 200)):
         wave = s.plan_waves(rep_off, cur, out, out_len, B, weight=w)[0]
-        small = _smallest(names, part_off, part_id, rep_off, cur, out, out_len, wave)
+        small = util.smallest_limit(*case, wave, rollback=True)
         for L in (small, small + 1, 500, 3000, 70000, ZNODE):
-            parts, rollback, part_wave, st = _check(s, *case, B, L, w, C)
+            parts, rollback, _, _, _, st = util.check_wave_documents(s, *case, B, L, True, weight=w, C=C)
             assert st.code == 0
             _check_pairs(parts, rollback, current, L)
         assert len(parts) >= len(set(wave[wave > 0].tolist()))
@@ -148,7 +94,8 @@ def test_a_replication_factor_reduction_takes_more_parts(native_lib):
     for L in (4000, 65536, ZNODE):
         parts, _, _, _, st = s.plan_wave_parts_json(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, 10 ** 9, L)
         assert st.code == 0
-        r_parts, rollback, _, st = _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, 10 ** 9, L)
+        r_parts, rollback, _, _, _, st = util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out,
+                                                                   out_len, 10 ** 9, L, True)
         assert st.code == 0 and len(r_parts) >= len(parts) and (L > 4000 or len(r_parts) > len(parts))
         _check_pairs(r_parts, rollback, current, L)
 
@@ -169,8 +116,8 @@ def test_a_limit_above_every_document_gives_the_wave_documents(native_lib, send)
         assert np.array_equal(p_wave, wave) and np.array_equal(p_summ, summ)
         assert [bytes(p) for p in parts] == [bytes(d) for d in docs]
         _check_pairs(parts, rollback, current, L)
-        _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, 4096, None, 5 if send else None,
-               cl.all_broker_id)
+        util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, 4096, True,
+                                  C=5 if send else None, send_ids=cl.all_broker_id)
 
 
 def test_parts_straddle_ctas_and_the_staging_limit(native_lib):
@@ -190,7 +137,7 @@ def test_parts_straddle_ctas_and_the_staging_limit(native_lib):
     current = _current(names, part_off, None, rep_off, cur)
     for B in (50, 10 ** 6):
         for L in (1000, 5000, 64 * 1024, 200 * 1024, ZNODE):
-            parts, rollback, _, st = _check(s, names, part_off, None, rep_off, cur, out, out_len, B, L)
+            parts, rollback, _, _, _, st = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, B, L, True)
             assert st.code == 0
             _check_pairs(parts, rollback, current, L)
     assert len(parts) > 1
@@ -201,9 +148,9 @@ def test_launches_are_those_of_the_parts_call_and_three(native_lib):
     s.set_brokers(*util.table(np.arange(1, 31), 4))
     rng = np.random.default_rng(5)
     for T, B, L in ((300, 1, 500), (300, 10 ** 9, 3000), (40, 4, ZNODE), (600, 2, 300)):
-        case = _ragged(rng, T, 30, shrink=0.3)
+        case = util.ragged_wave_case(rng, T, 30, shrink=0.3)
         wave = s.plan_waves(*case[3:7], B)[0]
-        L = max(L, _smallest(*case, wave))
+        L = max(L, util.smallest_limit(*case, wave, rollback=True))
         n0 = s.launch_count()
         st = s.plan_wave_parts_json(*case, B, L)[4]
         n1 = s.launch_count()
@@ -274,7 +221,7 @@ def test_errors(native_lib):
         if wave[g]:
             t = g // 100
             lens[g] = 29 + max(len(models.record(topic_names[t], g - 100 * t, new_l[g])),
-                               len(rollback_models.current_record(topic_names[t], g - 100 * t, cur_l[g])))
+                               len(models.current_record(topic_names[t], g - 100 * t, cur_l[g])))
     longest = max(lens.values())
     low = min(g for g, n in lens.items() if n == longest)
     assert call(L=longest - 1)[:3] == (LIMIT, low, longest)
@@ -284,7 +231,8 @@ def test_errors(native_lib):
     o[999, :2], ln[999] = [4, 4], 2
     assert call(L=1, new=o, new_len=ln)[:3] == (BAD, 999, 4)
     # over-long rows, then json_cap, then back_cap; each cap one byte short is refused and exact is taken
-    e_parts, e_back = rollback_models.wave_rollback_parts(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, 400)[:2]
+    e_parts, e_back = models.wave_documents(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, L=400,
+                                            rollback=True)[:2]
     size, bsize = sum(len(p) for p in e_parts), sum(len(p) for p in e_back)
     assert call(L=400, json_cap=size - 1)[:2] == (LIMIT, size - 1)
     assert call(L=400, json_cap=size - 1, back_cap=0)[:2] == (LIMIT, size - 1)
@@ -304,7 +252,8 @@ def test_million_partition_cluster_under_the_znode_limit(native_lib, remove):
     cl = kab.synth.make_ragged_cluster(T=240000, N=400, max_partitions=128, seed=11, remove_frac=remove)
     s, out, out_len, S = util.solved(cl)
     B = len(out_len) if remove == 0.0 else 4000
-    parts, rollback, part_wave, st = _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, ZNODE)
+    parts, rollback, part_wave, _, _, st = util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out,
+                                                                     out_len, B, ZNODE, True)
     assert st.code == 0 and (part_wave == 1).sum() >= 25
     _check_pairs(parts, rollback, _current(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur), ZNODE)
 
@@ -333,7 +282,7 @@ def test_rollback_text_past_4_gib(native_lib):
         for r in range(int(part_off[t]), int(part_off[t + 1])):
             if wave[r]:
                 f = models.record(ph[t], r - int(part_off[t]), out[r][:int(out_len[r])]).encode()
-                b = rollback_models.current_record(ph[t], r - int(part_off[t]), cur[3 * r:3 * r + 3]).encode()
+                b = models.current_record(ph[t], r - int(part_off[t]), cur[3 * r:3 * r + 3]).encode()
                 grow = len(real[t]) - len(ph[t])
                 recs.setdefault(int(wave[r]), []).append((f, b, len(f) + grow, len(b) + grow))
     topic = re.compile(rb'"topic":"@(\d+)@"')
@@ -344,7 +293,7 @@ def test_rollback_text_past_4_gib(native_lib):
     e_back = []
     for v in sorted(recs):
         rs = recs[v]
-        for a, b in rollback_models.cut_parts_paired([x[2] for x in rs], [x[3] for x in rs], L):
+        for a, b in models.cut_parts([[x[2] for x in rs], [x[3] for x in rs]], L):
             e_back.append((b'{"version":1,"partitions":[' + b",".join(x[1] for x in rs[a:b]) + b"]}", b - a))
     slab, name_off = kab.Solver.marshal_names(names)
     cap = models.json_bound(names, part_off, 3)

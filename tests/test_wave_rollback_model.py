@@ -1,7 +1,6 @@
-"""ka_plan_waves_json_parts_rollback on the CPU: the paired cut of `rollback_models.cut_parts_paired` against a brute force over every
-cut of random length pairs and against `part_models.cut_parts`; the rollback documents of `rollback_models.wave_rollback_parts`; the
-record-length identity of the two key orders; the declarations; and what Solver.plan_wave_parts_rollback_json hands the C ABI
-and makes of what it gets back, through a fake library."""
+"""ka_plan_waves_json_parts_rollback on the CPU: the rollback documents of `models.wave_documents`; the record-length identity
+of the two key orders; the declarations; and what Solver.plan_wave_parts_rollback_json hands the C ABI and makes of what it gets
+back, through a fake library. The paired cut itself is tested beside the one-sided cut, in tests/test_wave_parts_model.py."""
 import ctypes
 import json
 import os
@@ -12,51 +11,10 @@ import pytest
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
-from tests import models, part_models, rollback_models, util
+from tests import models, util
 
 BAD, LIMIT = _native.KA_ERR_BAD_ARG, _native.KA_ERR_LIMIT
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _size(lengths):
-    return 29 + sum(lengths) + len(lengths) - 1
-
-
-def _fits(fwd, back, a, b, L):
-    return _size(fwd[a:b]) <= L and _size(back[a:b]) <= L
-
-
-def _brute(fwd, back, L):
-    """Every cut into consecutive runs in which each run fits on both sides and each run but the last could not take the next
-    record on at least one side."""
-    n = len(fwd)
-    found = []
-    for mask in range(1 << max(n - 1, 0)):
-        bounds = [0] + [i + 1 for i in range(n - 1) if mask >> i & 1] + [n]
-        runs = list(zip(bounds, bounds[1:]))
-        if all(_fits(fwd, back, a, b, L) for a, b in runs) and not any(_fits(fwd, back, a, b + 1, L) for a, b in runs[:-1]):
-            found.append(runs)
-    return found
-
-
-@pytest.mark.parametrize("seed", range(6))
-def test_paired_cut_is_the_only_greedy_cut(seed):
-    rng = np.random.default_rng(seed)
-    for _ in range(60):
-        n = int(rng.integers(1, 11))
-        fwd = [int(x) for x in rng.integers(40, 120, n)]
-        back = [int(x) for x in rng.integers(40, 120, n)]
-        L = int(rng.integers(29 + max(fwd + back), 29 + max(sum(fwd), sum(back)) + n + 20))
-        runs = rollback_models.cut_parts_paired(fwd, back, L)
-        assert _brute(fwd, back, L) == [runs], (fwd, back, L)
-        # every part fits on both sides; a part and the next part's first record exceed L on at least one side
-        assert all(_fits(fwd, back, a, b, L) for a, b in runs)
-        assert not any(_fits(fwd, back, a, b + 1, L) for a, b in runs[:-1])
-        # the same lengths on both sides: the one-sided cut
-        assert rollback_models.cut_parts_paired(fwd, fwd, L) == part_models.cut_parts(fwd, L)
-        # a rollback side never longer than the forward side: the one-sided cut too
-        shorter = [max(1, f - int(d)) for f, d in zip(fwd, rng.integers(0, 30, n))]
-        assert rollback_models.cut_parts_paired(fwd, shorter, L) == part_models.cut_parts(fwd, L)
 
 
 @pytest.mark.parametrize("seed", range(20))
@@ -69,43 +27,28 @@ def test_record_lengths_differ_only_by_the_list(seed):
     a = [int(x) for x in rng.integers(-2 ** 31, 2 ** 31, int(rng.integers(0, 5)))]
     b = [int(x) for x in rng.integers(-2 ** 31, 2 ** 31, int(rng.integers(0, 5)))]
     lst = lambda x: len(",".join(str(v) for v in x))  # noqa: E731
-    fwd, back = models.record(name, part, a), rollback_models.current_record(name, part, b)
+    fwd, back = models.record(name, part, a), models.current_record(name, part, b)
     assert len(fwd) == 39 + len(name) + len(str(part)) + lst(a)
     assert len(back) == 39 + len(name) + len(str(part)) + lst(b)
-    assert len(models.document([])) == len(rollback_models.rollback_document([])) == 29
+    assert len(models.document([])) == len(models.rollback_document([])) == 29
     assert json.loads(back) == {"topic": name, "partition": part, "replicas": b}
     assert list(json.loads(back)) == ["topic", "partition", "replicas"]
-
-
-def _random_case(rng, T=30, N=12, shrink=False):
-    sizes = rng.integers(0, 9, T)
-    part_off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-    Q = int(part_off[-1])
-    names = ["topic.%d-%s" % (t, "x" * int(rng.integers(0, 30))) for t in range(T)]
-    part_id = np.concatenate([np.sort(rng.choice(1000, n, replace=False)) for n in sizes]).astype(np.int32)
-    cur, new = util.random_wave_case(rng, Q, N)
-    if shrink:   # a replication-factor reduction: RF-3 current lists onto 1 or 2 of their brokers
-        cur = [[int(x) for x in rng.choice(np.arange(1, N + 1), 3, replace=False)] for _ in range(Q)]
-        new = [c[:int(rng.integers(1, 3))] for c in cur]
-    rep_off, cur_flat = util.cur_lists(cur)
-    out, out_len = util.rows(new, 3)
-    return names, part_off, part_id, rep_off, cur_flat, out, out_len, np.arange(1, N + 1)
 
 
 @pytest.mark.parametrize("seed", range(4))
 def test_rollback_documents_hold_each_part_on_its_current_lists(seed):
     rng = np.random.default_rng(20 + seed)
-    for shrink in (False, True):
-        case = _random_case(rng, shrink=shrink)
+    for shrink in (0.0, 1.0):
+        case = (*util.ragged_wave_case(rng, 30, 12, shrink), np.arange(1, 13))
         names, part_off, part_id, rep_off, cur = case[:5]
         current = {}
         for t, name in enumerate(names):
             for g in range(int(part_off[t]), int(part_off[t + 1])):
                 current[(name, int(part_id[g]))] = cur[int(rep_off[g]):int(rep_off[g + 1])].tolist()
         for B, send in ((1, None), (3, None), (2, (list(range(1, 13)), 4)), (10 ** 6, None)):
-            parts, p_wave, e_wave, summ, st = part_models.wave_parts(*case, B, 10 ** 9, send=send)
+            parts, _, p_wave, e_wave, summ, st = models.wave_documents(*case, B, send=send, L=10 ** 9)
             for L in (700, 2000, 10 ** 9):
-                r = rollback_models.wave_rollback_parts(*case, B, L, send=send)
+                r = models.wave_documents(*case, B, send=send, L=L, rollback=True)
                 if r[5][0]:
                     continue
                 fwd, back, part_wave, wave, r_summ, r_st = r
@@ -126,13 +69,13 @@ def test_rollback_documents_hold_each_part_on_its_current_lists(seed):
 
 def test_shorter_current_lists_give_the_one_sided_cut_and_longer_ones_more_parts():
     rng = np.random.default_rng(7)
-    case = _random_case(rng, T=40, shrink=True)
+    case = (*util.ragged_wave_case(rng, 40, 12, 1.0), np.arange(1, 13))
     B = 10 ** 6
     smallest = max(29 + len(models.record(n, 0, [12, 12, 12])) for n in case[0])
     more = []
     for L in (smallest + 100, 900, 3000):
-        parts, _, _, _, _ = part_models.wave_parts(*case, B, L)
-        fwd, back, _, _, _, _ = rollback_models.wave_rollback_parts(*case, B, L)
+        parts = models.wave_documents(*case, B, L=L)[0]
+        fwd, back = models.wave_documents(*case, B, L=L, rollback=True)[:2]
         assert len(fwd) >= len(parts) and max(len(b) for b in back) <= L
         more.append(len(fwd) > len(parts))
     assert any(more)
@@ -144,8 +87,8 @@ def test_shorter_current_lists_give_the_one_sided_cut_and_longer_ones_more_parts
     o, o_len = util.rows(new_lists, 3)
     swapped = (names, part_off, part_id, r_off, c_flat, o, o_len, ids)
     for L in (smallest + 100, 900, 3000):
-        parts, part_wave, wave, summ, st = part_models.wave_parts(*swapped, B, L)
-        fwd, back, r_wave, r_plan, r_summ, r_st = rollback_models.wave_rollback_parts(*swapped, B, L)
+        parts, _, part_wave, wave, summ, st = models.wave_documents(*swapped, B, L=L)
+        fwd, back, r_wave, r_plan, r_summ, r_st = models.wave_documents(*swapped, B, L=L, rollback=True)
         assert (fwd, r_wave, r_summ, r_st) == (parts, part_wave, summ, st) and np.array_equal(r_plan, wave)
 
 
@@ -156,20 +99,20 @@ def test_over_long_rows_and_plan_errors():
     out, out_len = util.rows(new)
     case = (["abc"], np.array([0, 4]), None, rep_off, cur_flat, out, out_len, np.arange(1, 20))
     fwd = [29 + len(models.record("abc", g, new[g])) for g in range(4)]
-    back = [29 + len(rollback_models.current_record("abc", g, cur[g])) for g in range(4)]
+    back = [29 + len(models.current_record("abc", g, cur[g])) for g in range(4)]
     lens = [max(f, b) for f, b in zip(fwd, back)]
     assert back[1] > fwd[1] and fwd[2] > back[2]
     # the lowest over-long row on either side, with the longer one-record document's length
-    assert rollback_models.wave_rollback_parts(*case, 10, max(lens) - 1)[5] == (LIMIT, 1, lens[1])
-    assert rollback_models.wave_rollback_parts(*case, 10, min(lens) - 1)[5] == (LIMIT, 0, lens[0])
-    assert rollback_models.wave_rollback_parts(*case, 10, fwd[1])[5] == (LIMIT, 1, back[1])
-    assert rollback_models.wave_rollback_parts(*case, 10, max(lens))[5] == (0, 0, 0)
+    assert models.wave_documents(*case, 10, rollback=True, L=max(lens) - 1)[5] == (LIMIT, 1, lens[1])
+    assert models.wave_documents(*case, 10, rollback=True, L=min(lens) - 1)[5] == (LIMIT, 0, lens[0])
+    assert models.wave_documents(*case, 10, rollback=True, L=fwd[1])[5] == (LIMIT, 1, back[1])
+    assert models.wave_documents(*case, 10, rollback=True, L=max(lens))[5] == (0, 0, 0)
     # the plan's own errors come first
     bad = util.rows([[5, 5], [1], [1], [1]])
-    assert rollback_models.wave_rollback_parts(*case[:5], *bad, case[7], 10, 1)[5] == (BAD, 0, 5)
+    assert models.wave_documents(*case[:5], *bad, case[7], 10, L=1, rollback=True)[5] == (BAD, 0, 5)
     # nothing changed: no part
     same = util.rows(cur, 6)
-    assert rollback_models.wave_rollback_parts(*case[:5], *same, case[7], 10, 100)[:3] == ([], [], [])
+    assert models.wave_documents(*case[:5], *same, case[7], 10, L=100, rollback=True)[:3] == ([], [], [])
 
 
 # ---- the C ABI --------------------------------------------------------------------------------------------------------------
@@ -199,67 +142,10 @@ def test_without_a_context_is_no_device(native_lib):
     assert n.value == 0 and d.value == 0
 
 
-class FakeRollbackLib(util.FakeWaveLib):
-    """FakeWaveLib with the two _parts_rollback entry points: records what each call is handed; writes D = 2 W parts (2 W <= Q),
-    part d as b"[d]" of wave 1 + d // 2 and its rollback document as b"(d)"; or, with `fail` = (code, a, b), refuses the call
-    with that status."""
-
-    def __init__(self, W, fail=None):
-        super().__init__(W)
-        self.fail = fail
-
-    def _parts(self, T, part_off, part_id, names, name_off, js, json_cap, L, doc_off, doc_wave, n_docs, back, back_cap, back_off):
-        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off)
-        text.update(L=L, doc_wave=doc_wave is not None, back_cap=back_cap)
-        if self.fail:
-            return Q, text, False
-        D = 2 * self.W
-        for buf, off, fmt in ((util.writable(js, json_cap, np.uint8), util.writable(doc_off, Q + 1, np.int64), b"[%d]"),
-                              (util.writable(back, back_cap, np.uint8), util.writable(back_off, Q + 1, np.int64), b"(%d)")):
-            at = 0
-            for d in range(D):
-                p = fmt % d
-                off[d] = at
-                buf[at:at + len(p)] = np.frombuffer(p, dtype=np.uint8)
-                at += len(p)
-            off[D] = at
-        util.writable(doc_wave, Q, np.int32)[:D] = 1 + np.arange(D) // 2
-        n_docs._obj.value = D
-        return Q, text, True
-
-    def _refuse(self, st, n_waves, n_docs):
-        st._obj.code, st._obj.a, st._obj.b = self.fail
-        n_waves._obj.value = n_docs._obj.value = 0
-        return self.fail[0]
-
-    def ka_plan_waves_json_parts_rollback(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, names,
-                                          name_off, js, json_cap, L, doc_off, doc_wave, n_docs, back, back_cap, back_off, wave,
-                                          n_waves, summary, cap, st):
-        Q, text, ok = self._parts(T, part_off, part_id, names, name_off, js, json_cap, L, doc_off, doc_wave, n_docs, back, back_cap,
-                                  back_off)
-        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), **text, cap=cap))
-        return self._fill(Q, wave, n_waves, summary, None, cap, st) if ok else self._refuse(st, n_waves, n_docs)
-
-    def ka_plan_waves_send_json_parts_rollback(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B,
-                                               n_send, send_id, C, names, name_off, js, json_cap, L, doc_off, doc_wave, n_docs,
-                                               back, back_cap, back_off, wave, n_waves, summary, send_summary, cap, st):
-        Q, text, ok = self._parts(T, part_off, part_id, names, name_off, js, json_cap, L, doc_off, doc_wave, n_docs, back, back_cap,
-                                  back_off)
-        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), **text,
-                               send_id=util.view(send_id, n_send, np.int32), C=C, cap=cap))
-        return self._fill(Q, wave, n_waves, summary, send_summary, cap, st) if ok else self._refuse(st, n_waves, n_docs)
-
-
-def _inputs():
-    out, out_len = util.rows([[1, 2], [3], [4, 5, 6], []])
-    rep_off, cur = util.cur_lists([[1], [2, 3], [4], [7, 8]])
-    return ["alpha", "", "bc"], [0, 3, 3, 4], [4, 9, -2, 0], rep_off, cur, out, out_len
-
-
 def test_plan_wave_parts_rollback_json_marshals_its_arguments():
-    lib = FakeRollbackLib(2)
+    lib = util.FakeWaveLib(2)
     s = util.fake_solver(lib)
-    names, part_off, part_id, rep_off, cur, out, out_len = _inputs()
+    names, part_off, part_id, rep_off, cur, out, out_len = util.wave_inputs()
     weight = np.array([5, 0, 7, 1], dtype=np.int64)
     parts, rollback, part_wave, wave, summ, st = s.plan_wave_parts_rollback_json(
         names, part_off, part_id, rep_off.astype(np.int32), cur.astype(np.int64), out, out_len, 9, 1 << 20, weight=weight)
@@ -291,8 +177,8 @@ def test_plan_wave_parts_rollback_json_marshals_its_arguments():
 
 @pytest.mark.parametrize("fail", [(BAD, 0, 0), (LIMIT, 2, 123), (LIMIT, 4000, 0)])
 def test_a_refused_call_gives_empty_results_and_its_status(fail):
-    s = util.fake_solver(FakeRollbackLib(3, fail))
-    names, part_off, part_id, rep_off, cur, out, out_len = _inputs()
+    s = util.fake_solver(util.FakeWaveLib(3, fail))
+    names, part_off, part_id, rep_off, cur, out, out_len = util.wave_inputs()
     for send in ({}, dict(max_broker_out=7, send_brokers=[1, 2])):
         parts, rollback, part_wave, wave, summ, st = s.plan_wave_parts_rollback_json(names, part_off, part_id, rep_off, cur, out,
                                                                                      out_len, 9, 0, **send)

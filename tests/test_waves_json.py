@@ -1,5 +1,5 @@
-"""ka_plan_waves_json: one reassignment document per wave of a wave plan, built on the device. `models.wave_docs` prints the
-waves of `models.plan_waves` record by record in the key order of the device emitter; every document, wave,
+"""ka_plan_waves_json: one reassignment document per wave of a wave plan, built on the device. `models.wave_documents` prints
+the waves of `models.plan_waves` record by record in the key order of the device emitter; every document, wave,
 summary and W of the device must equal it byte for byte. The CPU tests pin the model and what Solver.plan_waves_json hands the
 C ABI."""
 import ctypes
@@ -76,8 +76,8 @@ def test_model_hand_worked():
     new = [[1, 3], [3, 4], [3], [4], [2, 1], [1, 2], [4, 5], [3, 4], [3]]
     rep_off, cur_flat = util.cur_lists(cur)
     out, out_len = util.rows(new)
-    docs, wave, summ, st = models.wave_docs(["a", "empty", "b.c"], [0, 4, 4, 9], [0, 1, 5, 7, 2, 3, 4, -6, 8], rep_off, cur_flat, out,
-                                            out_len, np.arange(1, 100), 2)
+    docs, _, _, wave, summ, st = models.wave_documents(["a", "empty", "b.c"], [0, 4, 4, 9], [0, 1, 5, 7, 2, 3, 4, -6, 8], rep_off,
+                                                       cur_flat, out, out_len, np.arange(1, 100), 2)
     assert st == (0, 0, 0) and wave.tolist() == [1, 1, 2, 1, 1, 0, 2, 2, 3]
     assert docs == [
         b'{"partitions":[{"partition":0,"replicas":[1,3],"topic":"a"},{"partition":1,"replicas":[3,4],"topic":"a"},'
@@ -86,11 +86,11 @@ def test_model_hand_worked():
         b'{"partition":-6,"replicas":[3,4],"topic":"b.c"}],"version":1}',
         b'{"partitions":[{"partition":8,"replicas":[3],"topic":"b.c"}],"version":1}']
     # ordinals without part_id; nothing changed gives no document; a refused plan none either
-    docs, _, _, _ = models.wave_docs(["a", "b"], [0, 1, 3], None, *util.cur_lists([[1], [1], [1]]), *util.rows([[2], [1], [2]]), [1, 2], 1)
+    docs = models.wave_documents(["a", "b"], [0, 1, 3], None, *util.cur_lists([[1], [1], [1]]), *util.rows([[2], [1], [2]]), [1, 2], 1)[0]
     assert docs == [b'{"partitions":[{"partition":0,"replicas":[2],"topic":"a"}],"version":1}',
                     b'{"partitions":[{"partition":1,"replicas":[2],"topic":"b"}],"version":1}']
-    assert models.wave_docs(["a"], [0, 1], None, *util.cur_lists([[1]]), *util.rows([[1]]), [1], 1)[0] == []
-    assert models.wave_docs(["a"], [0, 1], None, *util.cur_lists([[1]]), *util.rows([[2, 2]]), [1, 2], 1)[::3] == (None, (BAD, 0, 2))
+    assert models.wave_documents(["a"], [0, 1], None, *util.cur_lists([[1]]), *util.rows([[1]]), [1], 1)[0] == []
+    assert models.wave_documents(["a"], [0, 1], None, *util.cur_lists([[1]]), *util.rows([[2, 2]]), [1, 2], 1)[::5] == (None, (BAD, 0, 2))
 
 
 @pytest.mark.parametrize("seed", range(4))
@@ -110,7 +110,8 @@ def test_model_invariants(seed):
     out, out_len = util.rows(new_lists, 3)
     topic_of = np.repeat(np.arange(T), sizes)
     for B, weight in ((1, None), (3, None), (40, rng.integers(0, 30, Q))):
-        docs, wave, summ, st = models.wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, np.arange(1, 13), B, weight)
+        docs, _, _, wave, summ, st = models.wave_documents(names, part_off, part_id, rep_off, cur, out, out_len, np.arange(1, 13), B,
+                                                           weight)
         assert st == (0, 0, 0) and len(docs) == len(summ)
         seen = []
         for v, doc in enumerate(docs):
@@ -124,22 +125,6 @@ def test_model_invariants(seed):
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------------
 
-def _check(s, names, part_off, part_id, rep_off, cur, out, out_len, B, weight=None, json_buf=None):
-    """plan_waves_json against the model and against plan_waves on the same inputs. Returns (docs, wave, summary, status)."""
-    docs, wave, summ, st = s.plan_waves_json(names, part_off, part_id, rep_off, cur, out, out_len, B, weight=weight, json_buf=json_buf)
-    e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, weight)
-    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
-    p_wave, p_summ, p_st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight)
-    assert (p_st.code, p_st.a, p_st.b) == e_st
-    if st.code == 0:
-        assert np.array_equal(wave, e_wave) and np.array_equal(wave, p_wave)
-        assert [util.record_of(x, WAVE_SUMMARY_DTYPE.names) for x in summ] == e_summ and np.array_equal(summ, p_summ)
-        assert len(docs) == len(e_docs)
-        for v, (d, e) in enumerate(zip(docs, e_docs)):
-            assert bytes(d) == e, (v, bytes(d)[:200], e[:200])
-    return docs, wave, summ, st
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("remove", [0.0, 0.02, 0.2])
 def test_solve_rows(native_lib, remove):
@@ -149,7 +134,8 @@ def test_solve_rows(native_lib, remove):
     weight = np.random.default_rng(3).integers(0, 1 << 20, Q).astype(np.int64)
     sparse = (cl.part_id.astype(np.int64) * 7 - 50).astype(np.int32)   # sparse and negative ids
     for B, w, pid in ((1, None, cl.part_id), (3, None, None), (INT64_MAX, None, sparse), (int(weight.mean()), weight, sparse)):
-        docs, _, summ, st = _check(s, cl.topic_names, cl.part_off, pid, cl.rep_off, cl.cur, out, out_len, B, w)
+        docs, _, _, _, summ, st = util.check_wave_documents(s, cl.topic_names, cl.part_off, pid, cl.rep_off, cl.cur, out, out_len, B,
+                                                            weight=w)
         assert st.code == 0
         if B == INT64_MAX:   # a single wave
             assert len(docs) == 1
@@ -163,7 +149,7 @@ def test_growing_rf_rows_of_4_to_8(native_lib):
         s, out, out_len, S = util.solved(cl, drf)
         assert S == drf and out_len.max() == drf
         for B in (1, 1000):
-            _check(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B)
+            util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B)
 
 
 @pytest.mark.gpu
@@ -174,8 +160,10 @@ def test_hand_built_rows(native_lib):
     def run(names, part_off, part_id, cur_lists, new_lists, B, weight=None, stride=None):
         rep_off, cur = util.cur_lists(cur_lists)
         out, out_len = util.rows(new_lists, stride)
-        return _check(s, names, np.asarray(part_off, dtype=np.int64), None if part_id is None else np.asarray(part_id, dtype=np.int32),
-                      rep_off, cur, out, out_len, B, None if weight is None else np.asarray(weight, dtype=np.int64))
+        docs, _, _, wave, summ, st = util.check_wave_documents(
+            s, names, np.asarray(part_off, dtype=np.int64), None if part_id is None else np.asarray(part_id, dtype=np.int32), rep_off,
+            cur, out, out_len, B, weight=None if weight is None else np.asarray(weight, dtype=np.int64))
+        return docs, wave, summ, st
 
     # reorder only (changed without a receiver: wave 1), drops only, and topics without partitions at both ends and inside
     docs, wave, _, _ = run(["none", "a", "gap", "b", "end"], [0, 0, 2, 2, 4, 4], [3, 9, -1, 0],
@@ -210,7 +198,7 @@ def test_fully_serial_plans_cross_every_sort_pass(native_lib, Q):
     names = ["serial-%d" % t for t in range(T)]
     rep_off, cur = util.cur_lists([[1]] * Q)
     out, out_len = util.rows([[2]] * Q)
-    docs, wave, _, st = _check(s, names, part_off, None, rep_off, cur, out, out_len, 1)
+    docs, _, _, wave, _, st = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, 1)
     assert st.code == 0 and len(docs) == Q and wave.tolist() == list(range(1, Q + 1))
 
 
@@ -227,9 +215,9 @@ def test_scattered_waves_in_two_passes(native_lib):
     out, out_len = util.rows(new_lists, 2)
     part_off = np.concatenate([[0], np.sort(rng.choice(np.arange(1, Q), 499, replace=False)), [Q]])
     names = ["t.%d" % t for t in range(500)]
-    docs, _, _, _ = _check(s, names, part_off, None, rep_off, cur, out, out_len, 1)
+    docs = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, 1)[0]
     assert len(docs) > 256
-    docs, _, _, _ = _check(s, names, part_off, None, rep_off, cur, out, out_len, 3)
+    docs = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, 3)[0]
     assert 128 < len(docs) < 256
 
 
@@ -248,7 +236,7 @@ def test_long_names_take_the_direct_path(native_lib):
     rep_off, cur = util.cur_lists(cur_lists)
     out, out_len = util.rows(new_lists, 3)
     for B in (1, 50, 10 ** 6):
-        docs, _, _, _ = _check(s, names, part_off, None, rep_off, cur, out, out_len, B)
+        docs = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, B)[0]
     assert len(docs) == 1 and len(docs[0]) > 256 * 400
 
 
@@ -274,7 +262,7 @@ def test_lookup_modes_and_chain_state(native_lib, table):
     part_off = np.arange(61) * 200
     names = ["m%d" % t for t in range(60)]
     for B, w in ((1, None), (500, rng.integers(0, 100, Q).astype(np.int64))):
-        _check(s, names, part_off, None, rep_off, cur, out, out_len, B, w)
+        util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, B, weight=w)
 
 
 @pytest.mark.gpu
@@ -349,7 +337,7 @@ def test_errors(native_lib):
         assert call(new=o, new_len=ln) == expect
         assert call(new=o, new_len=ln, json_cap=0) == expect
     # the text's exact size succeeds, one byte less is KA_ERR_LIMIT with a = json_cap; the bound always succeeds
-    e_docs = models.wave_docs(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)[0]
+    e_docs = models.wave_documents(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2)[0]
     size = sum(len(d) for d in e_docs)
     assert 0 < size <= cap
     assert call(json_cap=size - 1)[:2] == (LIMIT, size - 1) and call(json_cap=0)[:2] == (LIMIT, 0)

@@ -200,23 +200,6 @@ def _check(s, rep_off, cur, out, out_len, B, C, send_ids, weight=None):
     return wave, summ, st
 
 
-def _check_docs(s, names, part_off, part_id, rep_off, cur, out, out_len, B, C, send_ids, weight=None, json_buf=None):
-    """plan_waves_json with a send budget against the model and against plan_waves with the same budget."""
-    docs, wave, summ, st = s.plan_waves_json(names, part_off, part_id, rep_off, cur, out, out_len, B, weight=weight, json_buf=json_buf,
-                                             max_broker_out=C, send_brokers=send_ids)
-    e_docs, e_wave, e_summ, e_st = models.wave_docs(names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, weight,
-                                                    send=(send_ids, C))
-    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
-    if st.code == 0:
-        p_wave, p_summ, _ = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight, max_broker_out=C, send_brokers=send_ids)
-        assert np.array_equal(wave, e_wave) and np.array_equal(wave, p_wave)
-        assert [util.record_of(x, FIELDS) for x in summ] == e_summ and np.array_equal(summ, p_summ)
-        assert len(docs) == len(e_docs)
-        for v, (d, e) in enumerate(zip(docs, e_docs)):
-            assert bytes(d) == e, (v, bytes(d)[:200], e[:200])
-    return docs, wave, summ, st
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("remove", [0.0, 0.03])
 def test_solve_rows(native_lib, remove):
@@ -229,7 +212,8 @@ def test_solve_rows(native_lib, remove):
                     (mean, 16 * mean, weight)):
         _check(s, cl.rep_off, cl.cur, out, out_len, B, C, cl.all_broker_id, w)
     for B, C, w in ((2, 2, None), (8 * mean, 2 * mean, weight)):
-        _check_docs(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, C, cl.all_broker_id, w)
+        util.check_wave_documents(s, cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, B, weight=w, C=C,
+                                  send_ids=cl.all_broker_id)
 
 
 @pytest.mark.gpu
@@ -274,7 +258,8 @@ def test_a_huge_send_budget(native_lib):
             e_wave, e_summ, e_st = s.plan_waves(rep_off, cur, out, out_len, B, weight=w)
             assert st.code == e_st.code == 0 and len(e_summ) > 1 and np.array_equal(wave, e_wave)
             assert all(np.array_equal(summ[f], e_summ[f]) for f in WAVE_SUMMARY_DTYPE.names)
-        docs, _, _, st = _check_docs(s, names, part_off, None, rep_off, cur, out, out_len, B, big, send_ids, w)
+        docs, _, _, _, _, st = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, B, weight=w, C=big,
+                                                         send_ids=send_ids)
         e_docs, _, _, _ = s.plan_waves_json(names, part_off, None, rep_off, cur, out, out_len, B, weight=w)
         assert st.code == 0 and [bytes(d) for d in docs] == [bytes(d) for d in e_docs]
     cl = kab.synth.make_ragged_cluster(T=3000, N=300, max_partitions=128, seed=13, remove_frac=0.02)
@@ -314,7 +299,7 @@ def test_lookup_modes_and_chain_state(native_lib, table):
     for B, C, w in ((1, 1, None), (16, 5, None), (500, 700, rng.integers(0, 100, Q).astype(np.int64))):
         _check(s, rep_off, cur, out, out_len, B, C, send_ids, w)
     names, part_off = ["m%d" % t for t in range(40)], np.arange(41) * (Q // 40)
-    _check_docs(s, names, part_off, None, rep_off, cur, out, out_len, 16, 5, send_ids)
+    util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, 16, C=5, send_ids=send_ids)
 
 
 @pytest.mark.gpu
@@ -331,7 +316,7 @@ def test_one_leader_is_fully_serial(native_lib):
     wave, summ, st = _check(s, rep_off, cur, out, out_len, 10 ** 6, 1, [1])
     assert st.code == 0 and wave.tolist() == list(range(1, Q + 1)) and set(summ["max_broker_out_id"].tolist()) == {1}
     names, part_off = ["serial-%d" % t for t in range(7)], (np.arange(8) * Q) // 7
-    docs, _, _, st = _check_docs(s, names, part_off, None, rep_off, cur, out, out_len, 10 ** 6, 1, [1])
+    docs, _, _, _, _, st = util.check_wave_documents(s, names, part_off, None, rep_off, cur, out, out_len, 10 ** 6, C=1, send_ids=[1])
     assert st.code == 0 and len(docs) == Q
 
 
@@ -440,7 +425,7 @@ def test_errors_and_buffers(native_lib):
 
     assert jcall(js=None, C=0)[0] == BAD and jcall(doc_off=None, n_send=70000)[0] == BAD
     assert jcall(C=0)[0] == BAD and jcall(n_send=70000, send_id=np.arange(70000, dtype=np.int32))[:2] == (LIMIT, 70000)
-    e_docs = models.wave_docs(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, send=(send, 3))[0]
+    e_docs = models.wave_documents(topic_names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 2, send=(send, 3))[0]
     size = sum(len(d) for d in e_docs)
     assert 0 < size <= cap
     assert jcall(json_cap=size - 1)[:2] == (LIMIT, size - 1)

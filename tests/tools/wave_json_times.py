@@ -11,7 +11,7 @@ Two arms, both starting from the rows in host memory and ending with every docum
             wave) and Python string formatting of every record. It is what a script around Solver.plan_waves would do, NOT a
             tuned emitter: a compiled one would be much faster.
 Every step is synchronous and timed with the host clock, the L2 flushed (256 MiB written) before it; the median of --steps steps
-after --warmup warm-up steps. Before timing, the documents of both arms are checked equal, byte for byte, to models.wave_docs
+after --warmup warm-up steps. Before timing, the documents of both arms are checked equal, byte for byte, to models.wave_documents
 of tests/models.py. Prints the GPU, its power limit and SM clock, and a markdown table."""
 import argparse
 import ctypes
@@ -67,8 +67,8 @@ def measure(name, cl, steps, warmup, flush):
         return float(np.median(ms))
 
     for label, B, w in (("unit, B = 1", 1, None), ("weighted, B = 16 x mean", 16 * int(weight.mean()), weight)):
-        e_docs, e_wave, e_summ, e_st = models.wave_docs(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len,
-                                                        cl.broker_id, B, w)
+        e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out,
+                                                                   out_len, cl.broker_id, B, w)
         assert e_st[0] == 0, name + ": refused"
         W = len(e_docs)
         summ = np.zeros(W, dtype=WAVE_SUMMARY_DTYPE)

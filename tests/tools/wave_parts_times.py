@@ -7,8 +7,8 @@ document: every part then holds as few rows as any cut can give).
 Both arms start from the rows in host memory and end with every document's text in host memory (a pinned buffer of the
 documented sufficient size): ONE ka_plan_waves_json C call, and ONE ka_plan_waves_json_parts C call. Every step is synchronous
 and timed with the host clock, the L2 flushed (256 MiB written) before it; the median of --steps steps after --warmup warm-up
-steps. Before timing, every document of both arms is checked equal, byte for byte, to the model: models.wave_docs, and the
-part_models.cut_parts of its records. Prints the GPU, its power limit and SM clock, and a markdown table."""
+steps. Before timing, every document of both arms is checked equal, byte for byte, to the model, models.wave_documents without
+and with the limit. Prints the GPU, its power limit and SM clock, and a markdown table."""
 import argparse
 import ctypes
 import os
@@ -22,29 +22,11 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE  # noqa: E402
-from tests import models, part_models  # noqa: E402
+from tests import models, util  # noqa: E402
 from tests.tools.cluster_batch_times import gpu_info  # noqa: E402
 from tests.tools.wave_plan_times import _vp  # noqa: E402
 
 ZNODE = 0xFFFFF
-HEAD, TAIL = b'{"partitions":[', b'],"version":1}'
-
-
-def records(doc):
-    """The records of a document, without their commas (names of this cluster hold no "},{")."""
-    recs = doc[len(HEAD):-len(TAIL)].split(b"},{")
-    return [(b"" if i == 0 else b"{") + r + (b"" if i == len(recs) - 1 else b"}") for i, r in enumerate(recs)]
-
-
-def model_parts(docs, L):
-    """(parts, part_wave) of the model: each wave document's records cut by part_models.cut_parts."""
-    parts, part_wave = [], []
-    for v, doc in enumerate(docs, 1):
-        recs = records(doc)
-        for a, b in part_models.cut_parts([len(r) for r in recs], L):
-            parts.append(HEAD + b",".join(recs[a:b]) + TAIL)
-            part_wave.append(v)
-    return parts, part_wave
 
 
 def measure(name, cl, steps, warmup, flush):
@@ -72,8 +54,8 @@ def measure(name, cl, steps, warmup, flush):
         return float(np.median(ms))
 
     for label, B, w in (("unit, B = 1", 1, None), ("weighted, B = 16 x mean", 16 * int(weight.mean()), weight)):
-        e_docs, e_wave, _, e_st = models.wave_docs(cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len,
-                                                   cl.broker_id, B, w)
+        case = (cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
+        e_docs, _, _, e_wave, _, e_st = models.wave_documents(*case)
         assert e_st[0] == 0, name + ": refused"
         W = len(e_docs)
         summ = np.zeros(W, dtype=WAVE_SUMMARY_DTYPE)
@@ -95,9 +77,9 @@ def measure(name, cl, steps, warmup, flush):
         for v, e in enumerate(e_docs):
             assert bytes(text[doc_off[v]:doc_off[v + 1]]) == e, "%s: document %d differs from the model" % (name, v)
         t_docs = timed(docs)
-        smallest = max(29 + len(r) for doc in e_docs for r in records(doc))
+        smallest = util.smallest_limit(*case[:7], e_wave)
         for L_label, L in (("1 048 575", ZNODE), ("smallest, %d" % smallest, smallest)):
-            e_parts, e_part_wave = model_parts(e_docs, L)
+            e_parts, _, e_part_wave = models.wave_documents(*case, L=L)[:3]
             D = len(e_parts)
             assert parts(L) == (0, W, D) and np.array_equal(wave, e_wave), name + ": device parts plan differs"
             assert doc_wave[:D].tolist() == e_part_wave, name + ": part waves differ from the model"

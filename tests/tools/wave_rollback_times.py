@@ -14,10 +14,11 @@ sufficient sizes):
   rollback   ONE ka_plan_waves_json_parts_rollback call
 Every step is synchronous and timed with the host clock, the L2 flushed (256 MiB written) before it; the median of --steps steps
 after --warmup warm-up steps (--host-steps for the host arm). Before timing, every document of every arm is checked equal, byte
-for byte, to the model: the records of models.plan_waves cut by part_models.cut_parts and rollback_models.cut_parts_paired. Prints the GPU, its
-power limit and SM clock, and a markdown table."""
+for byte, to the model, models.wave_documents with the limit, one-sided and paired; the host arm's documents to the rollback
+documents of the one-sided parts. Prints the GPU, its power limit and SM clock, and a markdown table."""
 import argparse
 import ctypes
+import json
 import os
 import sys
 import time
@@ -29,25 +30,25 @@ import torch  # noqa: E402
 
 import kafka_assigner_b200 as kab  # noqa: E402
 from kafka_assigner_b200.assigner import WAVE_SUMMARY_DTYPE  # noqa: E402
-from tests import models, part_models, rollback_models  # noqa: E402
+from tests import models, util  # noqa: E402
 from tests.tools.cluster_batch_times import gpu_info  # noqa: E402
 from tests.tools.wave_plan_times import _vp  # noqa: E402
 
 ZNODE = 0xFFFFF
 
 
-def model_records(cl, out, out_len, B, w):
-    """(wave, [per wave: [(record, rollback record)]]) of the model, rows in input order."""
-    wave, summ, st = models.plan_waves(cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
-    assert st[0] == 0
-    recs = [[] for _ in summ]
-    for t, name in enumerate(cl.topic_names):
-        for g in range(int(cl.part_off[t]), int(cl.part_off[t + 1])):
-            if wave[g]:
-                p = int(cl.part_id[g])
-                recs[wave[g] - 1].append((models.record(name, p, out[g][:int(out_len[g])]).encode(),
-                                          rollback_models.current_record(name, p, cl.cur[int(cl.rep_off[g]):int(cl.rep_off[g + 1])]).encode()))
-    return wave, recs
+def rollback_of(cl, parts):
+    """The rollback document of each forward part: its records' partitions on their current lists, in its order."""
+    row = {(name, int(cl.part_id[g])): g for t, name in enumerate(cl.topic_names)
+           for g in range(int(cl.part_off[t]), int(cl.part_off[t + 1]))}
+    docs = []
+    for p in parts:
+        recs = []
+        for r in json.loads(p)["partitions"]:
+            g = row[(r["topic"], r["partition"])]
+            recs.append(models.current_record(r["topic"], r["partition"], cl.cur[int(cl.rep_off[g]):int(cl.rep_off[g + 1])]))
+        docs.append(models.rollback_document(recs).encode())
+    return docs
 
 
 def host_rollback(cl, wave, fwd_text, doc_off, D):
@@ -97,8 +98,10 @@ def measure(name, cl, desired_rf, steps, warmup, host_steps, flush):
         return float(np.median(ms))
 
     for label, B, w in (("unit, B = 1", 1, None), ("weighted, B = 16 x mean", 16 * int(weight.mean()), weight)):
-        e_wave, recs = model_records(cl, out, out_len, B, w)
-        W = len(recs)
+        case = (cl.topic_names, cl.part_off, cl.part_id, cl.rep_off, cl.cur, out, out_len, cl.broker_id, B, w)
+        _, _, _, e_wave, e_summ, e_st = models.wave_documents(*case)
+        assert e_st[0] == 0, name + ": refused"
+        W = len(e_summ)
         summ = np.zeros(W, dtype=WAVE_SUMMARY_DTYPE)
         rows = (s._h, T, _vp(cl.part_off), _vp(cl.part_id), _vp(cl.rep_off), _vp(cl.cur), S, _vp(out_len), _vp(out), _vp(w), int(B),
                 _vp(names), _vp(name_off), _vp(text), cap)
@@ -119,16 +122,11 @@ def measure(name, cl, desired_rf, steps, warmup, host_steps, flush):
                                                         _vp(back_off), _vp(wave), ctypes.byref(n), _vp(summ), W, ctypes.byref(st))
             return rc, n.value, d.value
 
-        smallest = max(29 + max(len(f), len(b)) for rs in recs for f, b in rs)
+        smallest = util.smallest_limit(*case[:7], e_wave, rollback=True)
         for L_label, L in (("1 048 575", ZNODE), ("smallest, %d" % smallest, smallest)):
-            e_fwd, e_one_back, e_pair, e_pair_back = [], [], [], []
-            for rs in recs:
-                for a, b in part_models.cut_parts([len(f) for f, _ in rs], L):
-                    e_fwd.append(b'{"partitions":[' + b",".join(f for f, _ in rs[a:b]) + b'],"version":1}')
-                    e_one_back.append(b'{"version":1,"partitions":[' + b",".join(r for _, r in rs[a:b]) + b"]}")
-                for a, b in rollback_models.cut_parts_paired([len(f) for f, _ in rs], [len(r) for _, r in rs], L):
-                    e_pair.append(b'{"partitions":[' + b",".join(f for f, _ in rs[a:b]) + b'],"version":1}')
-                    e_pair_back.append(b'{"version":1,"partitions":[' + b",".join(r for _, r in rs[a:b]) + b"]}")
+            e_fwd = models.wave_documents(*case, L=L)[0]
+            e_one_back = rollback_of(cl, e_fwd)
+            e_pair, e_pair_back = models.wave_documents(*case, L=L, rollback=True)[:2]
             D1, D2 = len(e_fwd), len(e_pair)
             # arm 1 and arm 2 against the model
             host = parts_host(L)

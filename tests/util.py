@@ -9,6 +9,7 @@ import numpy as np
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
+from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
 from tests import models
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -140,12 +141,14 @@ def fake_solver(lib):
 
 
 class FakeWaveLib:
-    """Stands in for libkassign.so's four wave entry points: records what each call is handed, plans W waves
+    """Stands in for libkassign.so's eight wave entry points: records what each call is handed, plans W waves
     (wave[g] = 1 + g % W), writes recognisable summaries (field f of summary v: 10 v + f, the sender fields as f = 5, 6), at most
-    `cap` of them, and writes document v as b"<v>"."""
+    `cap` of them, and writes document v of the per-wave calls as b"<v>"; the _parts calls write D = 2 W parts (2 W <= Q), part d
+    as b"[d]" of wave 1 + d // 2, and the _parts_rollback calls part d's rollback document as b"(d)". With `fail` = (code, a, b)
+    every call is refused with that status."""
 
-    def __init__(self, W):
-        self.W, self.calls = W, []
+    def __init__(self, W, fail=None):
+        self.W, self.fail, self.calls = W, fail, []
 
     @staticmethod
     def _rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave):
@@ -153,23 +156,55 @@ class FakeWaveLib:
         return dict(Q=Q, stride=stride, rep_off=r_off, cur=view(cur, int(r_off[-1]), np.int32), new_len=view(new_len, Q, np.int32),
                     new_broker=view(new_broker, Q * stride, np.int32), weight=view(weight, Q, np.int64), B=B, wave=wave is not None)
 
-    def _docs(self, T, part_off, part_id, names, name_off, js, json_cap, doc_off):
-        """Writes the W documents; returns Q and what the text arguments were."""
+    @staticmethod
+    def _write(buf, cap, offsets, Q, docs):
+        text, off = writable(buf, cap, np.uint8), writable(offsets, Q + 1, np.int64)
+        at = 0
+        for d, doc in enumerate(docs):
+            off[d] = at
+            text[at:at + len(doc)] = np.frombuffer(doc, dtype=np.uint8)
+            at += len(doc)
+        off[len(docs)] = at
+
+    def _docs(self, T, part_off, part_id, names, name_off, js, json_cap, doc_off, parts=None, back=None):
+        """Writes the documents: the W per-wave ones, or with parts = (L, doc_wave, n_docs) the 2 W parts and with
+        back = (back, back_cap, back_off) their rollback documents; nothing for a refused call. Returns Q and what the text
+        arguments were."""
         p_off = view(part_off, T + 1, np.int64)
         Q = int(p_off[-1])
         n_off = view(name_off, T + 1, np.int64)
-        text, off = writable(js, json_cap, np.uint8), writable(doc_off, Q + 1, np.int64)
-        at = 0
-        for v in range(self.W):
-            doc = b"<%d>" % v
-            off[v] = at
-            text[at:at + len(doc)] = np.frombuffer(doc, dtype=np.uint8)
-            at += len(doc)
-        off[self.W] = at
-        return Q, dict(T=T, part_off=p_off, part_id=view(part_id, Q, np.int32), names=bytes(view(names, int(n_off[-1]), np.uint8)),
-                       name_off=n_off, json_cap=json_cap)
+        text = dict(T=T, part_off=p_off, part_id=view(part_id, Q, np.int32), names=bytes(view(names, int(n_off[-1]), np.uint8)),
+                    name_off=n_off, json_cap=json_cap)
+        if parts is not None:
+            text.update(L=parts[0], doc_wave=parts[1] is not None)
+        if back is not None:
+            text.update(back_cap=back[1])
+        if self.fail:
+            return Q, text
+        if parts is None:
+            self._write(js, json_cap, doc_off, Q, [b"<%d>" % v for v in range(self.W)])
+            return Q, text
+        D = 2 * self.W
+        self._write(js, json_cap, doc_off, Q, [b"[%d]" % d for d in range(D)])
+        if back is not None:
+            self._write(*back, Q, [b"(%d)" % d for d in range(D)])
+        writable(parts[1], Q, np.int32)[:D] = 1 + np.arange(D) // 2
+        parts[2]._obj.value = D
+        return Q, text
 
-    def _fill(self, Q, wave, n_waves, summary, send_summary, cap, st):
+    def _call(self, Q, rows, text, send, cap):
+        call = dict(self._rows(Q, *rows), **text)
+        if send is not None:
+            call.update(send_id=view(send[1], send[0], np.int32), C=send[2])
+        self.calls.append(dict(call, cap=cap))
+
+    def _fill(self, Q, wave, n_waves, summary, send_summary, cap, st, n_docs=None):
+        if self.fail:
+            st._obj.code, st._obj.a, st._obj.b = self.fail
+            n_waves._obj.value = 0
+            if n_docs is not None:
+                n_docs._obj.value = 0
+            return self.fail[0]
         if wave is not None and Q:
             writable(wave, Q, np.int32)[:] = 1 + np.arange(Q) % self.W
         n = min(cap, self.W)
@@ -182,27 +217,54 @@ class FakeWaveLib:
         return 0
 
     def ka_plan_waves(self, h, Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave, n_waves, summary, cap, st):
-        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), cap=cap))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), {}, None, cap)
         return self._fill(Q, wave, n_waves, summary, None, cap, st)
 
     def ka_plan_waves_send(self, h, Q, rep_off, cur, stride, new_len, new_broker, weight, B, n_send, send_id, C, wave, n_waves, summary,
                            send_summary, cap, st):
-        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave),
-                               send_id=view(send_id, n_send, np.int32), C=C, cap=cap))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), {}, (n_send, send_id, C), cap)
         return self._fill(Q, wave, n_waves, summary, send_summary, cap, st)
 
     def ka_plan_waves_json(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, names, name_off,
                            js, json_cap, doc_off, wave, n_waves, summary, cap, st):
         Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off)
-        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), **text, cap=cap))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), text, None, cap)
         return self._fill(Q, wave, n_waves, summary, None, cap, st)
 
     def ka_plan_waves_send_json(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, n_send, send_id, C,
                                 names, name_off, js, json_cap, doc_off, wave, n_waves, summary, send_summary, cap, st):
         Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off)
-        self.calls.append(dict(self._rows(Q, rep_off, cur, stride, new_len, new_broker, weight, B, wave), **text,
-                               send_id=view(send_id, n_send, np.int32), C=C, cap=cap))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), text, (n_send, send_id, C), cap)
         return self._fill(Q, wave, n_waves, summary, send_summary, cap, st)
+
+    def ka_plan_waves_json_parts(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, names,
+                                 name_off, js, json_cap, L, doc_off, doc_wave, n_docs, wave, n_waves, summary, cap, st):
+        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off, (L, doc_wave, n_docs))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), text, None, cap)
+        return self._fill(Q, wave, n_waves, summary, None, cap, st, n_docs)
+
+    def ka_plan_waves_send_json_parts(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, n_send,
+                                      send_id, C, names, name_off, js, json_cap, L, doc_off, doc_wave, n_docs, wave, n_waves,
+                                      summary, send_summary, cap, st):
+        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off, (L, doc_wave, n_docs))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), text, (n_send, send_id, C), cap)
+        return self._fill(Q, wave, n_waves, summary, send_summary, cap, st, n_docs)
+
+    def ka_plan_waves_json_parts_rollback(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B, names,
+                                          name_off, js, json_cap, L, doc_off, doc_wave, n_docs, back, back_cap, back_off, wave,
+                                          n_waves, summary, cap, st):
+        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off, (L, doc_wave, n_docs),
+                             (back, back_cap, back_off))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), text, None, cap)
+        return self._fill(Q, wave, n_waves, summary, None, cap, st, n_docs)
+
+    def ka_plan_waves_send_json_parts_rollback(self, h, T, part_off, part_id, rep_off, cur, stride, new_len, new_broker, weight, B,
+                                               n_send, send_id, C, names, name_off, js, json_cap, L, doc_off, doc_wave, n_docs,
+                                               back, back_cap, back_off, wave, n_waves, summary, send_summary, cap, st):
+        Q, text = self._docs(T, part_off, part_id, names, name_off, js, json_cap, doc_off, (L, doc_wave, n_docs),
+                             (back, back_cap, back_off))
+        self._call(Q, (rep_off, cur, stride, new_len, new_broker, weight, B, wave), text, (n_send, send_id, C), cap)
+        return self._fill(Q, wave, n_waves, summary, send_summary, cap, st, n_docs)
 
 
 # ---- broker tables -------------------------------------------------------------------------------------------------------
@@ -528,6 +590,83 @@ def random_wave_case(rng, Q, N, stride=3):
             n = int(rng.integers(0, stride + 1))
             new.append([int(x) for x in rng.choice(np.arange(1, N + 1), n, replace=False)])
     return cur, new
+
+
+def ragged_wave_case(rng, T, N, shrink=0.0):
+    """(names, part_off, part_id, rep_off, cur, out, out_len): T topics of 0..29 partitions (sparse ids below 5000, names of up to
+    50 bytes) with the rows of random_wave_case over brokers 1..N; with probability `shrink` a row is a replication-factor
+    reduction instead: a 3-broker current list onto its first one or two."""
+    sizes = rng.integers(0, 30, T)
+    part_off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    Q = int(part_off[-1])
+    names = ["ragged.%d.%s" % (t, "y" * int(rng.integers(0, 40))) for t in range(T)]
+    part_id = np.concatenate([np.sort(rng.choice(5000, n, replace=False)) for n in sizes]).astype(np.int32)
+    cur_l, new_l = random_wave_case(rng, Q, N)
+    for g in range(Q if shrink else 0):
+        if rng.random() < shrink:
+            cur_l[g] = [int(x) for x in rng.choice(np.arange(1, N + 1), 3, replace=False)]
+            new_l[g] = cur_l[g][:int(rng.integers(1, 3))]
+    rep_off, cur = cur_lists(cur_l)
+    out, out_len = rows(new_l, 3)
+    return names, part_off, part_id, rep_off, cur, out, out_len
+
+
+def wave_inputs():
+    """(names, part_off, part_id, rep_off, cur, out, out_len): four rows in three topics, one empty, for the marshalling tests."""
+    out, out_len = rows([[1, 2], [3], [4, 5, 6], []])
+    rep_off, cur = cur_lists([[1], [2, 3], [4], [7, 8]])
+    return ["alpha", "", "bc"], [0, 3, 3, 4], [4, 9, -2, 0], rep_off, cur, out, out_len
+
+
+def smallest_limit(names, part_off, part_id, rep_off, cur, out, out_len, wave, rollback=False):
+    """The smallest L that fits every changed row: its longest one-record document, on either side with rollback."""
+    best = 0
+    for t, name in enumerate(names):
+        for g in range(int(part_off[t]), int(part_off[t + 1])):
+            if wave[g]:
+                p = int(part_id[g]) if part_id is not None else g - int(part_off[t])
+                best = max(best, 29 + len(models.record(name, p, out[g][:int(out_len[g])]).encode()))
+                if rollback:
+                    best = max(best, 29 + len(models.current_record(name, p, cur[int(rep_off[g]):int(rep_off[g + 1])]).encode()))
+    return best
+
+
+def check_wave_documents(s, names, part_off, part_id, rep_off, cur, out, out_len, B, L=None, rollback=False, weight=None, C=None,
+                         send_ids=None, json_buf=None):
+    """plan_waves_json (L None), plan_wave_parts_json or, with rollback, plan_wave_parts_rollback_json against
+    models.wave_documents and against plan_waves on the same inputs; with C a sender budget over send_ids (None: the Solver's
+    table). Returns (docs, backs, doc_wave, wave, summary, status), the shape of models.wave_documents."""
+    send_ids = list(np.asarray(s.broker_id if send_ids is None else send_ids))
+    send = {} if C is None else dict(max_broker_out=C, send_brokers=send_ids)
+    args = (names, part_off, part_id, rep_off, cur, out, out_len, B)
+    if L is None:
+        docs, wave, summ, st = s.plan_waves_json(*args, weight=weight, json_buf=json_buf, **send)
+        got = (docs, None, np.arange(1, len(docs) + 1, dtype=np.int32), wave, summ, st)
+    elif not rollback:
+        docs, doc_wave, wave, summ, st = s.plan_wave_parts_json(*args, L, weight=weight, json_buf=json_buf, **send)
+        got = (docs, None, doc_wave, wave, summ, st)
+    else:
+        got = s.plan_wave_parts_rollback_json(*args, L, weight=weight, json_buf=json_buf, **send)
+    docs, backs, doc_wave, wave, summ, st = got
+    e_docs, e_backs, e_doc_wave, e_wave, e_summ, e_st = models.wave_documents(
+        names, part_off, part_id, rep_off, cur, out, out_len, s.broker_id, B, weight, None if C is None else (send_ids, C), L, rollback)
+    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
+    p_wave, p_summ, p_st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight, **send)
+    assert (p_st.code, p_st.a, p_st.b) == (e_st if e_st[0] != _native.KA_ERR_LIMIT else (0, 0, 0))
+    if st.code == 0:
+        dtype = WAVE_SUMMARY_DTYPE if C is None else WAVE_SEND_SUMMARY_DTYPE
+        assert np.array_equal(wave, e_wave) and np.array_equal(wave, p_wave)
+        assert [record_of(x, dtype.names) for x in summ] == e_summ and np.array_equal(summ, p_summ)
+        assert doc_wave.tolist() == e_doc_wave and len(docs) == len(e_docs)
+        for d, (x, e) in enumerate(zip(docs, e_docs)):
+            assert bytes(x) == e, (d, bytes(x)[:200], e[:200])
+        if rollback:
+            assert len(backs) == len(e_backs)
+            for d, (x, e) in enumerate(zip(backs, e_backs)):
+                assert bytes(x) == e, (d, bytes(x)[:200], e[:200])
+    else:
+        assert docs == [] and backs in (None, []) and len(doc_wave) == len(wave) == len(summ) == 0
+    return got
 
 
 def solved(cl, desired_rf=-1):
