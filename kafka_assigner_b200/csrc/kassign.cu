@@ -52,8 +52,8 @@ struct DevBuf {
 };
 
 constexpr int KA_MAX_BLOCKS = 8;          // topic blocks of a pipelined solve
-constexpr int KA_MAX_CHAIN_BLOCKS = 8;    // slot-chain sub-blocks per staged block
-constexpr int KA_MAX_CHAIN_EVENTS = 64;   // per solve: 8 staged blocks x 8 sub-blocks
+constexpr int KA_MAX_CHAIN_BLOCKS = 16;   // slot-chain sub-blocks per staged block
+constexpr int KA_MAX_CHAIN_EVENTS = KA_MAX_BLOCKS * KA_MAX_CHAIN_BLOCKS;   // chain sub-blocks per solve
 // JSON fragments of one solve: one per chain sub-block of a dense solve; a ragged solve (one block, one sub-block) cuts its
 // rows into fragments of KA_JSON_FRAG_ROWS rows (more per fragment only beyond KA_MAX_JSON_FRAGS of them), so that the text
 // streams out while later fragments are still being built and every fragment stays far below the 4 GiB of its 32-bit offsets.
@@ -167,16 +167,17 @@ struct ka_ctx {
     // timing events (recorded only with timing on)
     cudaEvent_t ev[6] = {};                                // solve: start, inputs in, kernel A done, stage done, chains done, end
     cudaEvent_t ev_pipe[KA_MAX_BLOCKS][5] = {};            // pipelined block: stage start, kernel A done, stage done, chains start / done
-    cudaEvent_t ev_chain[KA_MAX_CHAIN_EVENTS][4] = {};     // chain sub-block: slot-0 chain start / done, slot-1 chain + emit start / done
-    // cross-stream events
+    cudaEvent_t ev_chain[KA_MAX_BLOCKS][4] = {};           // chains of a block: slot-0 chains start / done, slot-1 chains + emits start / done
+    // cross-stream events: ev_b1 / ev_b2 = slot-0 / slot-1 chain of a sub-block done, ev_emit_done = a block's emits done
     cudaEvent_t ev_in = nullptr, ev_stage[KA_MAX_BLOCKS] = {}, ev_chain_in = nullptr, ev_b1[KA_MAX_CHAIN_EVENTS] = {};
+    cudaEvent_t ev_b2[KA_MAX_CHAIN_EVENTS] = {}, ev_emit_done = nullptr;
     cudaEvent_t ev_json_in[KA_MAX_JSON_FRAGS] = {}, ev_json_scan[KA_MAX_JSON_FRAGS] = {}, ev_out_done = nullptr;
     // timing of the last solve
     bool timing = false;
     float last_ms[8] = {};
     bool ev_valid = false;
     int last_stages = 1;
-    int chain_used = 0;                    // ev_chain rows recorded
+    int chain_used = 0;                    // ev_chain rows recorded (one per block of a solve)
     bool slot_timed[2] = {false, false};   // ka_order_slot_device recorded ev_chain[slot][0..1]
     int32_t order_plan[8] = {};            // ka_ctx_last_order_plan: the leader-order chains of the last solve call
     int32_t stage_plan[8] = {};            // ka_ctx_last_stage_plan: kernel A of the last solve call
@@ -233,6 +234,8 @@ void for_each_event(ka_ctx* c, F f) {
         {c->ev_stage, KA_MAX_BLOCKS, false},
         {&c->ev_chain_in, 1, false},
         {c->ev_b1, KA_MAX_CHAIN_EVENTS, false},
+        {c->ev_b2, KA_MAX_CHAIN_EVENTS, false},
+        {&c->ev_emit_done, 1, false},
         {c->ev_json_in, KA_MAX_JSON_FRAGS, false},
         {c->ev_json_scan, KA_MAX_JSON_FRAGS, false},
         {&c->ev_out_done, 1, false},
@@ -593,38 +596,49 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done)
     return KA_OK;
 }
 
-// CAND: one CTA per candidate of a batched solve (ncand of them), else one CTA.
+// CAND: one CTA per candidate of a batched solve (ncand of them), else one CTA. behind: launched behind the kernel before it
+// on s (programmatic dependent launch): the chain's prologue overlaps that kernel's end, and only its counter load waits for
+// it. Only for a predecessor that writes none of the records the chain reads.
 template <int KIND, int MAXNT, bool CAND, bool GCTR, bool SINGLE, bool WARP1, bool FULL>
-cudaError_t launch_order_t(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int ncand) {
+cudaError_t launch_order_t(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int ncand, bool behind) {
     auto kern = ka_order_levels_kernel<KIND, GCTR, MAXNT, SINGLE, WARP1, FULL, CAND>;
     cudaError_t e = allow_smem(kern, pl.b_smem);
     if (e != cudaSuccess) return e;
-    kern<<<CAND ? ncand : 1, pl.b_threads, pl.b_smem, s>>>(o);
-    return cudaGetLastError();
+    cudaLaunchAttribute attr{};
+    attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr.val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(CAND ? ncand : 1);
+    cfg.blockDim = dim3(pl.b_threads);
+    cfg.dynamicSmemBytes = pl.b_smem;
+    cfg.stream = s;
+    cfg.attrs = &attr;
+    cfg.numAttrs = behind ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, kern, o);
 }
 
 // KIND 0 / 1: slot chains of rows <= 3 (chunk arithmetic, barrier flavour, full chunks are compile-time); 4 / 8: rows of 4 / 5..8.
 // *sel: the instantiation launched, (GCTR ? 4 : 0) | loop shape (0 general, 1 WARP1, 2 SINGLE, 3 FULL).
 template <int KIND, int MAXNT, bool CAND = false>
-cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int* sel, int ncand = 0) {
+cudaError_t launch_order(cudaStream_t s, const KaOrderParams& o, const Plan& pl, int* sel, int ncand = 0, bool behind = false) {
     if constexpr (KIND > 1) {
         *sel = pl.b_gctr ? 4 : 0;
-        return pl.b_gctr ? launch_order_t<KIND, MAXNT, false, true, false, false, false>(s, o, pl, ncand)
-                         : launch_order_t<KIND, MAXNT, false, false, false, false, false>(s, o, pl, ncand);
+        return pl.b_gctr ? launch_order_t<KIND, MAXNT, false, true, false, false, false>(s, o, pl, ncand, behind)
+                         : launch_order_t<KIND, MAXNT, false, false, false, false, false>(s, o, pl, ncand, behind);
     } else {
         const bool warp1 = pl.b_threads == 32;                                                          // window mode
         const bool single = !warp1 && o.uniform_width != 0 && o.uniform_width <= (uint32_t)pl.b_threads;   // chunk = topic
         const bool full = single && o.uniform_width == (uint32_t)pl.b_threads;                          // no idle lane
         *sel = (pl.b_gctr ? 4 : 0) | (warp1 ? 1 : (full ? 3 : (single ? 2 : 0)));
         switch (*sel) {
-            case 0: return launch_order_t<KIND, MAXNT, CAND, false, false, false, false>(s, o, pl, ncand);
-            case 1: return launch_order_t<KIND, MAXNT, CAND, false, false, true, false>(s, o, pl, ncand);
-            case 2: return launch_order_t<KIND, MAXNT, CAND, false, true, false, false>(s, o, pl, ncand);
-            case 3: return launch_order_t<KIND, MAXNT, CAND, false, true, false, true>(s, o, pl, ncand);
-            case 4: return launch_order_t<KIND, MAXNT, CAND, true, false, false, false>(s, o, pl, ncand);
-            case 5: return launch_order_t<KIND, MAXNT, CAND, true, false, true, false>(s, o, pl, ncand);
-            case 6: return launch_order_t<KIND, MAXNT, CAND, true, true, false, false>(s, o, pl, ncand);
-            default: return launch_order_t<KIND, MAXNT, CAND, true, true, false, true>(s, o, pl, ncand);
+            case 0: return launch_order_t<KIND, MAXNT, CAND, false, false, false, false>(s, o, pl, ncand, behind);
+            case 1: return launch_order_t<KIND, MAXNT, CAND, false, false, true, false>(s, o, pl, ncand, behind);
+            case 2: return launch_order_t<KIND, MAXNT, CAND, false, true, false, false>(s, o, pl, ncand, behind);
+            case 3: return launch_order_t<KIND, MAXNT, CAND, false, true, false, true>(s, o, pl, ncand, behind);
+            case 4: return launch_order_t<KIND, MAXNT, CAND, true, false, false, false>(s, o, pl, ncand, behind);
+            case 5: return launch_order_t<KIND, MAXNT, CAND, true, false, true, false>(s, o, pl, ncand, behind);
+            case 6: return launch_order_t<KIND, MAXNT, CAND, true, true, false, false>(s, o, pl, ncand, behind);
+            default: return launch_order_t<KIND, MAXNT, CAND, true, true, false, true>(s, o, pl, ncand, behind);
         }
     }
 }
@@ -642,13 +656,24 @@ void note_order(ka_ctx* c, const Plan& pl, int sel, int ncand) {
     r[7] = ncand;
 }
 
+// Topics per chain sub-block of a large block (at least KA_CHAIN_LARGE_BLOCK topics) of a single solve, whose chain launches
+// overlap (enq_order_emit). A solve ends about one sub-block's slot-1 chain after its slot-0 chain ends, so smaller sub-blocks
+// shorten that tail; but a slot-1 chain launch waits for its slot-0 chain (an event), which keeps it from overlapping the
+// slot-1 chain before it: measured at C3 on H100, a slot-1 boundary costs about 7 us against 3 us for a slot-0 one, while a
+// slot-1 level is about 7 ns faster. Below about 650 levels per sub-block the slot-1 chain falls further behind at every
+// boundary (DESIGN §2 "Pipelining").
+constexpr int KA_CHAIN_SUB_TOPICS = 512;
+constexpr int KA_CHAIN_LARGE_BLOCK = 1024;
+
 // How many topic sub-blocks the slot chains of one staged block are cut into: the slot-0 chain of sub-block j+1 runs (on
 // its own SM) while the slot-1 chain + emit of sub-block j run. A chain launch is one CTA, so sub-blocks are cheap; each
-// should still hold a few hundred levels to amortise the launch + ring fill.
-int chain_subblocks(const StageDesc& d, int blocks_in_solve) {
+// should still hold a few hundred levels to amortise the launch + ring fill. overlapped: the chain launches of the
+// sub-blocks overlap their predecessors (the single solve), which makes a boundary cheap enough for many sub-blocks.
+int chain_subblocks(const StageDesc& d, int blocks_in_solve, bool overlapped = false) {
     if (d.d_part_off || d.pl.rec_kind != 3 || d.T < 2) return 1;
     int n = std::max(1, 8 / std::max(1, blocks_in_solve));
     n = std::min(n, std::max(1, d.T / 128));
+    if (overlapped && d.T >= KA_CHAIN_LARGE_BLOCK) n = std::max(n, d.T / KA_CHAIN_SUB_TOPICS);
     if (const char* e = std::getenv("KA_CHAIN_SUBBLOCKS")) n = std::max(1, std::min(std::atoi(e), d.T));
     return std::min(n, KA_MAX_CHAIN_BLOCKS);
 }
@@ -672,9 +697,9 @@ struct SolveCall {
     // pipelined host-buffer solve, rows <= 3: every chain sub-block is copied out on c->sj as soon as its emit is done, so
     // that no D2H sits between two slot-1 chains on the caller's stream
     bool stream_out = false;
-    int out_copies = 0;       // sub-block copies handed to c->sj (ev_json_in)
     int json_blocks = 0;      // JSON fragments enqueued (ev_json_in, ev_json_scan, h_frag)
-    int chains = 0;           // chain sub-blocks enqueued (ev_chain, ev_b1)
+    int chains = 0;           // chain sub-blocks enqueued (ev_b1, ev_b2)
+    bool emits = false;       // emits enqueued on c->sj (ev_emit_done)
 
     SolveCall(int32_t* out, int32_t* out_len) : d_out(out), d_out_len(out_len) {}
 };
@@ -825,13 +850,13 @@ KaOrderParams order_params(ka_ctx* c, const StageDesc& d, const SubBlock& b) {
     return o;
 }
 
-// One slot chain (rows <= 3) over sub-block j of a staged block.
-int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int j, int nsub) {
+// One slot chain (rows <= 3) over sub-block j of a staged block; behind: as launch_order_t.
+int enq_slot_chain(ka_ctx* c, cudaStream_t s, const StageDesc& d, int slot, int j, int nsub, bool behind = false) {
     const SubBlock b = sub_block(d, j, nsub);
     if (b.rq <= 0 || c->br.N <= 0) return KA_OK;
     const KaOrderParams o = order_params(c, d, b);
     int sel = 0;
-    KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, d.pl, &sel) : launch_order<1, 1024>(s, o, d.pl, &sel)));
+    KA_CUDA((slot == 0 ? launch_order<0, 1024>(s, o, d.pl, &sel, 0, behind) : launch_order<1, 1024>(s, o, d.pl, &sel, 0, behind)));
     note_order(c, d.pl, sel, 0);
     c->launches++;
     return KA_OK;
@@ -852,8 +877,9 @@ int enq_emit_block(ka_ctx* c, cudaStream_t s, const StageDesc& d, int j, int nsu
 }
 
 // The serial chains through Context.counter (KAS:202-239) for a staged block + the parallel emit into the block's rows of
-// io.d_out. Rows <= 3: slot-0 chain on c->sb1, slot-1 chain + emit on `s`; the caller has made c->sb1 wait for the stage
-// (c->ev_chain_in recorded after kernel A / the counter import). Everything is joined back into `s`.
+// io.d_out. Rows <= 3: slot-0 chains on c->sb1, slot-1 chains on `s`, emits (and the rows' copy-out or text) on c->sj; the
+// caller has made c->sb1 wait for the stage (c->ev_chain_in recorded after kernel A / the counter import), and joins the
+// emits back into `s` (join_emits) once every block is enqueued.
 int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io, int blocks_in_solve) {
     const int S = d.S;
     const Plan& pl = d.pl;
@@ -873,37 +899,45 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io,
         if (io.json) return enq_json(c, s, io, d, b, d.blk == 0, d.blk == blocks_in_solve - 1);
         return KA_OK;
     }
-    const int nsub = chain_subblocks(d, blocks_in_solve);
-    cudaStream_t s1 = c->sb1;
+    const int nsub = chain_subblocks(d, blocks_in_solve, true);
+    const int e = c->chain_used;
+    if (e >= KA_MAX_BLOCKS || io.chains + nsub > KA_MAX_CHAIN_EVENTS) return KA_ERR_LIMIT;
+    // Each chain stream runs the chains of the block back to back, every one launched behind the one before it: its prologue
+    // overlaps that chain's end. The slot-1 chains read records the slot-0 chains rewrote, and the emits read the slot-1
+    // chains' records, so each hands over through an event (ev_b1, ev_b2); the emits run on c->sj, off the slot-1 path.
+    cudaStream_t s1 = c->sb1, se = c->sj;
+    if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][0], s1));
     for (int j = 0; j < nsub; ++j) {
-        const int e = io.chains % KA_MAX_CHAIN_EVENTS;
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][0], s1));
-        int rc = enq_slot_chain(c, s1, d, 0, j, nsub);                    // slot-0 chain
+        const int k = io.chains + j;
+        int rc = enq_slot_chain(c, s1, d, 0, j, nsub, true);              // slot-0 chain
         if (rc != KA_OK) return rc;
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][1], s1));
-        KA_CUDA(cudaEventRecord(c->ev_b1[e], s1));
-        KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[e], 0));
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][2], s));
-        if ((rc = enq_slot_chain(c, s, d, 1, j, nsub)) != KA_OK) return rc;   // slot-1 chain
-        if ((rc = enq_emit_block(c, s, d, j, nsub, d_out, d_out_len)) != KA_OK) return rc;
-        if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][3], s));
+        KA_CUDA(cudaEventRecord(c->ev_b1[k], s1));
+        KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[k], 0));
+        if (c->timing && j == 0) KA_CUDA(cudaEventRecord(c->ev_chain[e][2], s));
+        if ((rc = enq_slot_chain(c, s, d, 1, j, nsub, true)) != KA_OK) return rc;   // slot-1 chain
+        KA_CUDA(cudaEventRecord(c->ev_b2[k], s));
+        KA_CUDA(cudaStreamWaitEvent(se, c->ev_b2[k], 0));
+        if ((rc = enq_emit_block(c, se, d, j, nsub, d_out, d_out_len)) != KA_OK) return rc;
+        if (j == nsub - 1) {   // the block's emits are done: join_emits hands them to `s`
+            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][3], se));
+            KA_CUDA(cudaEventRecord(c->ev_emit_done, se));
+            io.emits = true;
+        }
         const SubBlock b = sub_block(d, j, nsub);
-        if (io.stream_out) {   // rows of this sub-block are final: copy them out on c->sj (on `s` itself once the events run out)
-            cudaStream_t so = s;
-            if (io.out_copies < KA_MAX_CHAIN_EVENTS) {
-                KA_CUDA(cudaEventRecord(c->ev_json_in[io.out_copies], s));
-                KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_json_in[io.out_copies], 0));
-                io.out_copies++;
-                so = c->sj;
-            }
-            if ((rc = enq_copy_out(so, io, S, d.q0 + b.r0, b.rq)) != KA_OK) return rc;
-        }
-        if (io.json) {   // the sub-block's rows are final: their JSON text can be built and streamed out now
-            if ((rc = enq_json(c, s, io, d, b, d.blk == 0 && j == 0, d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK)
-                return rc;
-        }
-        c->chain_used = std::min(++io.chains, KA_MAX_CHAIN_EVENTS);
+        // the rows of this sub-block are final: copy them out, or build and stream out their JSON text
+        if (io.stream_out && (rc = enq_copy_out(se, io, S, d.q0 + b.r0, b.rq)) != KA_OK) return rc;
+        if (io.json && (rc = enq_json(c, se, io, d, b, d.blk == 0 && j == 0, d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK)
+            return rc;
     }
+    if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][1], s1));
+    io.chains += nsub;
+    c->chain_used = e + 1;
+    return KA_OK;
+}
+
+// `s` waits for every emit enq_order_emit put on c->sj (not for the copies and text behind them).
+int join_emits(ka_ctx* c, cudaStream_t s, const SolveCall& io) {
+    if (io.emits) KA_CUDA(cudaStreamWaitEvent(s, c->ev_emit_done, 0));
     return KA_OK;
 }
 
@@ -978,7 +1012,7 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
         if ((rc = enq_stage(c, s, d, c->ev[2])) != KA_OK) return rc;
         if (c->timing) KA_CUDA(cudaEventRecord(c->ev[3], s));
         if ((rc = chain_fork(c, s)) != KA_OK) return rc;
-        if ((rc = enq_order_emit(c, s, d, io, 1)) != KA_OK) return rc;
+        if ((rc = enq_order_emit(c, s, d, io, 1)) != KA_OK || (rc = join_emits(c, s, io)) != KA_OK) return rc;
         if (c->timing) KA_CUDA(cudaEventRecord(c->ev[4], s));
         if (io.h_out && d.Q > 0 && c->br.N > 0 && (rc = enq_copy_out(s, io, d.S, 0, d.Q)) != KA_OK) return rc;
     } else {
@@ -988,6 +1022,8 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
         if (io.stream_out) KA_CUDA(cudaStreamWaitEvent(c->sj, c->ev_in, 0));
         KA_CUDA(cudaStreamWaitEvent(aux, c->ev_in, 0));
         if ((rc = reset_flags(c, aux)) != KA_OK) return rc;
+        // every block's stage is enqueued before the chains: enqueueing a block's chains takes the host longer than kernel A
+        // of the next block takes the GPU, so a stage enqueued behind them would start late and hold up the next block's chains
         for (int k = 0; k < K; ++k) {
             const StageDesc& d = ds[k];
             if ((rc = enq_inputs(aux, io, d, d.Q * d.RF)) != KA_OK) return rc;
@@ -995,6 +1031,9 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
             if ((rc = enq_stage(c, aux, d, c->ev_pipe[k][1])) != KA_OK) return rc;
             if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][2], aux));
             KA_CUDA(cudaEventRecord(c->ev_stage[k], aux));
+        }
+        for (int k = 0; k < K; ++k) {
+            const StageDesc& d = ds[k];
             KA_CUDA(cudaStreamWaitEvent(s, c->ev_stage[k], 0));
             KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_stage[k], 0));
             if (k == 0) KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_in, 0));
@@ -1004,6 +1043,7 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
             // rows of 4..8: one copy per block on the caller's stream
             if (io.h_out && !io.stream_out && d.Q > 0 && c->br.N > 0 && (rc = enq_copy_out(s, io, d.S, d.q0, d.Q)) != KA_OK) return rc;
         }
+        if ((rc = join_emits(c, s, io)) != KA_OK) return rc;
         if (io.stream_out) {   // join the copy-out stream back into the caller's stream
             KA_CUDA(cudaEventRecord(c->ev_out_done, c->sj));
             KA_CUDA(cudaStreamWaitEvent(s, c->ev_out_done, 0));
@@ -1052,7 +1092,7 @@ int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st, const int32_t* part_
                 c->last_ms[7] += b;
             }
         }
-        if (c->chain_used > 0) {  // rows <= 3: per-slot chains (sums over the sub-blocks; the two chains overlap in time)
+        if (c->chain_used > 0) {  // rows <= 3: per-slot chains (sums over the blocks; the two chains overlap in time)
             for (int e = 0; e < c->chain_used; ++e) {
                 float b1 = 0.f, b2 = 0.f;
                 cudaEventElapsedTime(&b1, c->ev_chain[e][0], c->ev_chain[e][1]);
@@ -1701,7 +1741,9 @@ int32_t ka_order_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, vo
     if (rc != KA_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     SolveCall io(d_out_broker, d_out_len);
-    if ((rc = chain_fork(c, s)) != KA_OK || (rc = enq_order_emit(c, s, c->staged_block, io, 1)) != KA_OK) return failed(st, rc);
+    if ((rc = chain_fork(c, s)) != KA_OK || (rc = enq_order_emit(c, s, c->staged_block, io, 1)) != KA_OK ||
+        (rc = join_emits(c, s, io)) != KA_OK)
+        return failed(st, rc);
     return end_staged(c, s, st);
 }
 

@@ -72,6 +72,10 @@ __device__ __forceinline__ void ka_mbar_arrive(uint64_t* bar) {
 __device__ __forceinline__ void ka_named_bar_sync(uint32_t id, uint32_t nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Programmatic dependent launch: wait until the grid this one was launched behind has completed and its writes are visible
+// (returns at once without such a predecessor); let the grid launched behind this one start its prologue.
+__device__ __forceinline__ void ka_grid_dependency_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void ka_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 // counter-row access: shared memory (byte address = base + idx*16 .. the record's precomputed offset) or global memory
 // (ctr8 rows of 8 ints, L2-resident; for broker tables beyond shared memory)
@@ -189,18 +193,10 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
         for (int i = 0; i < NS; ++i) ka_mbar_init(&full[i], 1);
         ka_fence_mbar_init();
     }
-    if (!GCTR)
-        for (uint32_t i = tid; i < (uint32_t)(CAND ? (int)pin[8] : p.N) * CW; i += blockDim.x)
-            ctr[i] = ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))];
-    if (KIND <= 1 && tid == 0) {  // the dummy broker (index N) that pads rows shorter than 3: a counter that never wins a comparison
-        // INT_MAX, and every record lists the dummy after its real brokers: a real counter is at most INT_MAX, so it wins both
-        // the slot-0 minimum and the slot-1 pair (e = 0 there) in scan order. The dummy is never bumped (the bumps below are
-        // skipped for rows too short to fill the slot), so its counter stays INT_MAX for the whole launch.
-        const int N = CAND ? (int)pin[8] : p.N;
-        if (GCTR) ctr8[(size_t)N * KA_MAX_SLOTS + KIND] = 0x7FFFFFFF; else ctr[N] = 0x7FFFFFFF;
-    }
-    // idle lanes read (and ignore) ring slots past the end of the stream: make those valid records (all zero)
-    for (uint32_t i = tid; i < (uint32_t)NS * G * (RB / 16); i += blockDim.x) reinterpret_cast<uint4*>(ring)[i] = make_uint4(0, 0, 0, 0);
+    // idle lanes read (and ignore) ring slots past the end of the stream: make those valid records (all zero). Every lane of
+    // the FULL shape is active on every chunk, and its one read past the end (the last chunk's prefetch) is never used.
+    if (!FULL)
+        for (uint32_t i = tid; i < (uint32_t)NS * G * (RB / 16); i += blockDim.x) reinterpret_cast<uint4*>(ring)[i] = make_uint4(0, 0, 0, 0);
     ka_fence_proxy_async();   // generic-proxy writes above vs the async-proxy (TMA) writes that follow
     __syncthreads();
 
@@ -219,6 +215,22 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
     };
     if (tid == 0)
         for (uint32_t j = 0; j < min(nstages_all, (uint32_t)NS); ++j) issue_stage(j);
+
+    // Everything above reads only parameters and records, which kernel A or the slot-0 chain wrote and the stream has joined
+    // through events. The counters are the output of the chain launch before this one on the stream, which may still be
+    // running when this grid was launched behind it (programmatic dependent launch): only their load waits for it.
+    ka_grid_dependency_wait();
+    if (!GCTR)
+        for (uint32_t i = tid; i < (uint32_t)(CAND ? (int)pin[8] : p.N) * CW; i += blockDim.x)
+            ctr[i] = ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))];
+    if (KIND <= 1 && tid == 0) {  // the dummy broker (index N) that pads rows shorter than 3: a counter that never wins a comparison
+        // INT_MAX, and every record lists the dummy after its real brokers: a real counter is at most INT_MAX, so it wins both
+        // the slot-0 minimum and the slot-1 pair (e = 0 there) in scan order. The dummy is never bumped (the bumps below are
+        // skipped for rows too short to fill the slot), so its counter stays INT_MAX for the whole launch.
+        const int N = CAND ? (int)pin[8] : p.N;
+        if (GCTR) ctr8[(size_t)N * KA_MAX_SLOTS + KIND] = 0x7FFFFFFF; else ctr[N] = 0x7FFFFFFF;
+    }
+    __syncthreads();
 
     // ---- consumers ------------------------------------------------------------------------------------------------------
     const uint32_t rmask = (uint32_t)NS * G - 1u;
@@ -534,6 +546,8 @@ __global__ void __launch_bounds__(MAXNT, 1) ka_order_levels_kernel(const KaOrder
         }
     }
 
+    // the next chain launch may run its prologue now; its counter load still waits for this grid to complete
+    ka_launch_dependents();
     if (!GCTR) {
         if (NT == 32) __syncwarp(); else __syncthreads();
         for (uint32_t i = tid; i < (uint32_t)(CAND ? (int)pin[8] : p.N) * CW; i += NT) ctr8[(i / CW) * KA_MAX_SLOTS + (KIND <= 1 ? KIND : (int)(i % CW))] = ctr[i];
