@@ -608,8 +608,8 @@ int32_t ka_ctx_import_counters_device(ka_ctx* ctx, const int32_t* d_counter, voi
 /* ---- instrumentation ----------------------------------------------------------------------------
  * Per-phase device times of the LAST solve, measured with CUDA events on the solve's stream.
  * ms[0]=sticky+spread kernel (S0-S4)  ms[1]=chunk tables of the level schedule (scan + fill; 0 when capacity is 1)
- * ms[2]=slot-0 leader-order chain (S5; sum over sub-blocks)   ms[3]=H2D   ms[4]=D2H   ms[5]=total on stream
- * ms[6]=slot-1 chain + emit (sum over sub-blocks; overlaps ms[2] in time)   ms[7]=wall time of all chains + emit
+ * ms[2]=slot-0 leader-order chains (S5; first start .. last end)   ms[3]=H2D   ms[4]=D2H   ms[5]=total on stream
+ * ms[6]=slot-1 chains + emits (first start .. last end; overlaps ms[2] in time)   ms[7]=wall time of all chains + emit
  * Enabled with ka_ctx_set_timing(ctx, 1); costs a few event records per solve. */
 int32_t ka_ctx_set_timing(ka_ctx* ctx, int32_t enabled);
 int32_t ka_ctx_last_timing(ka_ctx* ctx, float* ms /* [8] */);

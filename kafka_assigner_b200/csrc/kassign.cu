@@ -167,7 +167,7 @@ struct ka_ctx {
     // timing events (recorded only with timing on)
     cudaEvent_t ev[6] = {};                                // solve: start, inputs in, kernel A done, stage done, chains done, end
     cudaEvent_t ev_pipe[KA_MAX_BLOCKS][5] = {};            // pipelined block: stage start, kernel A done, stage done, chains start / done
-    cudaEvent_t ev_chain[KA_MAX_BLOCKS][4] = {};           // chains of a block: slot-0 chains start / done, slot-1 chains + emits start / done
+    cudaEvent_t ev_chain[KA_MAX_BLOCKS][4] = {};           // chains of a block: slot-0 chains start / done (a solve: [0] only), slot-1 chains + emits start / done
     // cross-stream events: ev_b1 / ev_b2 = slot-0 / slot-1 chain of a sub-block done, ev_emit_done = a block's emits done
     cudaEvent_t ev_in = nullptr, ev_stage[KA_MAX_BLOCKS] = {}, ev_chain_in = nullptr, ev_b1[KA_MAX_CHAIN_EVENTS] = {};
     cudaEvent_t ev_b2[KA_MAX_CHAIN_EVENTS] = {}, ev_emit_done = nullptr;
@@ -566,8 +566,10 @@ KaSolveParams stage_params(const StageDesc& d) {
 }
 
 // Context-free part of a block (shards across GPUs): kernel A (records in schedule order) + the level tables.
-// a_done is recorded at the end of kernel A when timing is on.
-int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done) {
+// a_done is recorded at the end of kernel A when timing is on; `done` (if given) when the stage is complete. When kernel A
+// ends the stage, `done` goes ahead of a_done, so that the chains waiting for it do not also wait for a timed event record,
+// which holds its stream for a few µs.
+int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done, cudaEvent_t done = nullptr) {
     const Plan& pl = d.pl;
     RunScratch& r = c->run;
     if (d.T > 0) {
@@ -582,8 +584,10 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done)
         const int rc = launch_stage_plan<false>(c, s, p, pl, d.T, 0, 1 << c->br.lut_mode);
         if (rc != KA_OK) return rc;
     }
+    const bool tables = pl.a_levels && d.T > 0;
+    if (done && !tables) KA_CUDA(cudaEventRecord(done, s));
     if (c->timing) KA_CUDA(cudaEventRecord(a_done, s));
-    if (pl.a_levels && d.T > 0) {
+    if (tables) {
         int32_t* ntl = r.ntl.as<int32_t>() + d.topic_base;
         int32_t* loff = r.loff.as<int32_t>() + d.topic_base + d.blk;  // every block keeps T_k + 1 entries
         ka_level_scan_kernel<<<1, 1024, 0, s>>>(ntl, d.T, loff);
@@ -592,6 +596,7 @@ int enq_stage(ka_ctx* c, cudaStream_t s, const StageDesc& d, cudaEvent_t a_done)
                                                             r.lvl_end.as<uint32_t>() + d.q0);
         KA_CUDA(cudaGetLastError());
         c->launches += 2;
+        if (done) KA_CUDA(cudaEventRecord(done, s));
     }
     return KA_OK;
 }
@@ -879,10 +884,13 @@ int enq_emit_block(ka_ctx* c, cudaStream_t s, const StageDesc& d, int j, int nsu
 // The serial chains through Context.counter (KAS:202-239) for a staged block + the parallel emit into the block's rows of
 // io.d_out. Rows <= 3: slot-0 chains on c->sb1, slot-1 chains on `s`, emits (and the rows' copy-out or text) on c->sj; the
 // caller has made c->sb1 wait for the stage (c->ev_chain_in recorded after kernel A / the counter import), and joins the
-// emits back into `s` (join_emits) once every block is enqueued.
-int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io, int blocks_in_solve) {
+// emits back into `s` (join_emits) once every block is enqueued. next_stage (a pipelined solve's next block: its kernel A
+// is done): c->sb1 waits for it before this block's last slot-0 chain rather than before the next block's first one, so
+// that one is launched behind its stream predecessor like the chains inside a block. That kernel A ends long before.
+int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io, int blocks_in_solve, cudaEvent_t next_stage = nullptr) {
     const int S = d.S;
     const Plan& pl = d.pl;
+    if (next_stage && (d.Q <= 0 || c->br.N <= 0 || pl.rec_kind != 3)) KA_CUDA(cudaStreamWaitEvent(c->sb1, next_stage, 0));
     if (d.Q <= 0 || c->br.N <= 0) return io.json && d.d_part_off && d.Q == 0 ? enq_json(c, s, io, d, sub_block(d, 0, 1), true, true) : KA_OK;
     int32_t* d_out = io.d_out + d.q0 * S;
     int32_t* d_out_len = io.d_out_len ? io.d_out_len + d.q0 : nullptr;
@@ -906,20 +914,24 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io,
     // overlaps that chain's end. The slot-1 chains read records the slot-0 chains rewrote, and the emits read the slot-1
     // chains' records, so each hands over through an event (ev_b1, ev_b2); the emits run on c->sj, off the slot-1 path.
     cudaStream_t s1 = c->sb1, se = c->sj;
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][0], s1));
+    const int jw = nsub > 1 ? nsub - 1 : nsub;   // next_stage is waited for before slot-0 chain jw (nsub: after the block)
+    // The slot-0 chains are timed from the first block's start to the last block's end (ev_chain[0][0..1]): a timed event
+    // record between two blocks' chains would keep the second from launching behind the first.
+    if (c->timing && e == 0) KA_CUDA(cudaEventRecord(c->ev_chain[0][0], s1));
     for (int j = 0; j < nsub; ++j) {
         const int k = io.chains + j;
+        if (next_stage && j == jw) KA_CUDA(cudaStreamWaitEvent(s1, next_stage, 0));
         int rc = enq_slot_chain(c, s1, d, 0, j, nsub, true);              // slot-0 chain
         if (rc != KA_OK) return rc;
         KA_CUDA(cudaEventRecord(c->ev_b1[k], s1));
         KA_CUDA(cudaStreamWaitEvent(s, c->ev_b1[k], 0));
-        if (c->timing && j == 0) KA_CUDA(cudaEventRecord(c->ev_chain[e][2], s));
+        if (c->timing && j == 0 && e == 0) KA_CUDA(cudaEventRecord(c->ev_chain[0][2], s));   // as slot 0: one span per solve
         if ((rc = enq_slot_chain(c, s, d, 1, j, nsub, true)) != KA_OK) return rc;   // slot-1 chain
         KA_CUDA(cudaEventRecord(c->ev_b2[k], s));
         KA_CUDA(cudaStreamWaitEvent(se, c->ev_b2[k], 0));
         if ((rc = enq_emit_block(c, se, d, j, nsub, d_out, d_out_len)) != KA_OK) return rc;
         if (j == nsub - 1) {   // the block's emits are done: join_emits hands them to `s`
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][3], se));
+            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[0][3], se));   // the last block's record ends the span
             KA_CUDA(cudaEventRecord(c->ev_emit_done, se));
             io.emits = true;
         }
@@ -929,7 +941,8 @@ int enq_order_emit(ka_ctx* c, cudaStream_t s, const StageDesc& d, SolveCall& io,
         if (io.json && (rc = enq_json(c, se, io, d, b, d.blk == 0 && j == 0, d.blk == blocks_in_solve - 1 && j == nsub - 1)) != KA_OK)
             return rc;
     }
-    if (c->timing) KA_CUDA(cudaEventRecord(c->ev_chain[e][1], s1));
+    if (next_stage && jw == nsub) KA_CUDA(cudaStreamWaitEvent(s1, next_stage, 0));
+    if (c->timing && !next_stage) KA_CUDA(cudaEventRecord(c->ev_chain[0][1], s1));
     io.chains += nsub;
     c->chain_used = e + 1;
     return KA_OK;
@@ -1028,18 +1041,20 @@ int run_solve(ka_ctx* c, cudaStream_t s, const Shape& sh, SolveCall& io, ka_stat
             const StageDesc& d = ds[k];
             if ((rc = enq_inputs(aux, io, d, d.Q * d.RF)) != KA_OK) return rc;
             if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][0], aux));
-            if ((rc = enq_stage(c, aux, d, c->ev_pipe[k][1])) != KA_OK) return rc;
+            if ((rc = enq_stage(c, aux, d, c->ev_pipe[k][1], c->ev_stage[k])) != KA_OK) return rc;
             if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][2], aux));
-            KA_CUDA(cudaEventRecord(c->ev_stage[k], aux));
         }
         for (int k = 0; k < K; ++k) {
             const StageDesc& d = ds[k];
             KA_CUDA(cudaStreamWaitEvent(s, c->ev_stage[k], 0));
-            KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_stage[k], 0));
-            if (k == 0) KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_in, 0));
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][3], s));
-            if ((rc = enq_order_emit(c, s, d, io, K)) != KA_OK) return rc;
-            if (c->timing) KA_CUDA(cudaEventRecord(c->ev_pipe[k][4], s));
+            if (k == 0) {   // c->sb1 waits for the later blocks' stages inside enq_order_emit
+                KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_stage[0], 0));
+                KA_CUDA(cudaStreamWaitEvent(c->sb1, c->ev_in, 0));
+            }
+            // chains of all blocks timed as one span: a timed record between two blocks' slot-1 chains delays the second
+            if (c->timing && k == 0) KA_CUDA(cudaEventRecord(c->ev_pipe[0][3], s));
+            if ((rc = enq_order_emit(c, s, d, io, K, k + 1 < K ? c->ev_stage[k + 1] : nullptr)) != KA_OK) return rc;
+            if (c->timing && k == K - 1) KA_CUDA(cudaEventRecord(c->ev_pipe[K - 1][4], s));
             // rows of 4..8: one copy per block on the caller's stream
             if (io.h_out && !io.stream_out && d.Q > 0 && c->br.N > 0 && (rc = enq_copy_out(s, io, d.S, d.q0, d.Q)) != KA_OK) return rc;
         }
@@ -1083,23 +1098,17 @@ int finish_status(ka_ctx* c, cudaStream_t s, ka_status* st, const int32_t* part_
             cudaEventElapsedTime(&c->last_ms[4], c->ev[4], c->ev[5]);  // D2H
         } else {  // pipelined: phases of different chunks overlap; report the per-phase sums
             for (int k = 0; k < c->last_stages; ++k) {
-                float a = 0.f, t = 0.f, b = 0.f;
+                float a = 0.f, t = 0.f;
                 cudaEventElapsedTime(&a, c->ev_pipe[k][0], c->ev_pipe[k][1]);
                 cudaEventElapsedTime(&t, c->ev_pipe[k][1], c->ev_pipe[k][2]);
-                cudaEventElapsedTime(&b, c->ev_pipe[k][3], c->ev_pipe[k][4]);
                 c->last_ms[0] += a;
                 c->last_ms[1] += t;
-                c->last_ms[7] += b;
             }
+            cudaEventElapsedTime(&c->last_ms[7], c->ev_pipe[0][3], c->ev_pipe[c->last_stages - 1][4]);
         }
-        if (c->chain_used > 0) {  // rows <= 3: per-slot chains (sums over the blocks; the two chains overlap in time)
-            for (int e = 0; e < c->chain_used; ++e) {
-                float b1 = 0.f, b2 = 0.f;
-                cudaEventElapsedTime(&b1, c->ev_chain[e][0], c->ev_chain[e][1]);
-                cudaEventElapsedTime(&b2, c->ev_chain[e][2], c->ev_chain[e][3]);
-                c->last_ms[2] += b1;
-                c->last_ms[6] += b2;
-            }
+        if (c->chain_used > 0) {  // rows <= 3: each slot's chains, first start .. last end (slot 1 with its emits)
+            cudaEventElapsedTime(&c->last_ms[2], c->ev_chain[0][0], c->ev_chain[0][1]);
+            cudaEventElapsedTime(&c->last_ms[6], c->ev_chain[0][2], c->ev_chain[0][3]);
         } else if (c->slot_timed[0] || c->slot_timed[1]) {  // per-slot entry points (topic-sharded runs)
             if (c->slot_timed[0]) cudaEventElapsedTime(&c->last_ms[2], c->ev_chain[0][0], c->ev_chain[0][1]);
             if (c->slot_timed[1]) cudaEventElapsedTime(&c->last_ms[6], c->ev_chain[1][0], c->ev_chain[1][1]);
