@@ -553,6 +553,56 @@ int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* ctx, int32_t T, const int
                                                ka_wave_summary* summary, ka_wave_send_summary* send_summary, int32_t summary_cap,
                                                ka_status* st);
 
+/* What one broker holds across a wave plan, in the weight's unit (ka_wave_broker_usage). Every field is int64, so the layout has
+ * no padding. */
+typedef struct ka_broker_usage {
+    int64_t before;      /* before the plan starts: its base + the rows whose current list holds it */
+    int64_t peak;        /* the most it holds at any wave 0..W ... */
+    int64_t peak_wave;   /* ... and the lowest such wave (0 = before the plan starts) */
+    int64_t after;       /* once every wave has run */
+    int64_t over_wave;   /* the lowest wave in which it holds more than its capacity (0: already before), -1 when none */
+} ka_broker_usage;
+
+/* Every broker's disk usage across a wave plan: whether some broker runs out of disk PARTWAY through a plan, although it fits
+ * both before and after. Kafka adds a new replica when a partition's reassignment starts and deletes the old one only when it
+ * completes, so a broker that receives in one wave and drops in a later one holds both copies in between.
+ *   Q .. part_weight   the rows exactly as ka_plan_waves takes them (1 <= stride <= 8; part_weight >= 0, or NULL = 1 per row)
+ *   wave[Q]            host, required when Q > 0: every row's wave >= 0, e.g. the wave array of ka_plan_waves(_send), a plan the
+ *                      caller reordered, or a whole solve as one document (changed ? 1 : 0). W = the largest entry (0 when Q == 0)
+ *   n_use, use_id[n_use]   host; the USAGE TABLE, strictly ascending ids, 0 <= n_use <= 65535 (typically every broker of the
+ *                      cluster before an exclusion: a drained broker holds data until its waves have run)
+ *   use_base[n_use]    host, >= 0 per broker, or NULL = 0: what each broker holds beside the rows (e.g. topics outside the plan)
+ *   use_cap[n_use]     host, >= 0 per broker, or NULL = no capacity
+ *   usage[n_use]       host; usage[i] reports broker use_id[i]
+ *   n_waves_out        host, required; *n_waves_out = W
+ * The rule. Row g's RECEIVERS are the brokers of its new list that its current list lacks; its DROPPERS are the distinct
+ * brokers of its current list that its new list lacks (a broker stores one copy: a duplicate id in a current list counts once).
+ * For table broker b, with w_g the weight of row g:
+ *   before[b]   = base[b] + sum of w_g over the rows whose current list holds b
+ *   usage_b(v)  = before[b] + sum of w_g over the rows with 1 <= wave[g] <= v that b receives
+ *                           - sum of w_g over the rows with 1 <= wave[g] < v that b drops,   v = 0 .. W
+ * A receiver holds the new copy from the start of the row's wave, a dropper frees its copy only after that wave has ended: the
+ * worst case inside a wave, so usage_b bounds what b holds under any order of the wave's parts. A row with wave 0 is not run:
+ * it counts in before only. Then usage[i] = {before, peak = max_v usage(v), peak_wave = the lowest such v, after = usage(W) minus
+ * the drops of wave W, over_wave = the lowest v with usage(v) > cap (-1 when none, or use_cap NULL)}. Ids outside the table are
+ * not tracked.
+ * Checks, in this order, before anything is enqueued: st NULL: KA_ERR_BAD_ARG (nothing written); ctx NULL: KA_ERR_NO_DEVICE;
+ * Q < 0, stride < 1, n_use < 0, usage NULL with n_use > 0, n_waves_out NULL, rep_off not non-decreasing from 0, or a needed
+ * array NULL: KA_ERR_BAD_ARG; stride > 8 (a = stride), Q >= 2^31 (a = INT_MAX) or n_use > 65535 (a = n_use): KA_ERR_LIMIT; use_id
+ * not strictly ascending: KA_ERR_BAD_ARG; a negative weight, base or cap: KA_ERR_BAD_ARG; a new_len outside [0, stride] or a
+ * negative wave: KA_ERR_BAD_ARG with a = the lowest such row; sum of the bases + sum over rows of w_g x (current + new list
+ * lengths) > INT64_MAX, or Q x stride + rep_off[Q] > 2^31 - 1 (the replica events): KA_ERR_LIMIT. On the device, the lowest
+ * failing row wins: a new list naming a broker twice, or a receiver of a row with wave[g] > 0 that the usage table lacks, gives
+ * KA_ERR_BAD_ARG with a = the row and b = the broker id at the first such position of its list. On any error *n_waves_out = 0 and
+ * usage is unspecified.
+ * Synchronous; 2 kernel launches, and 3 per radix pass when W > 0: one per 8 bits of W + 1 and one per 8 bits of n_use - 1. Does
+ * not read or change the Context counters, the broker table, parked counters, topic_base, the staged block, or the last order /
+ * stage plans and timings. */
+int32_t ka_wave_broker_usage(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                             const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, const int32_t* wave,
+                             int32_t n_use, const int32_t* use_id, const int64_t* use_base, const int64_t* use_cap,
+                             ka_broker_usage* usage, int32_t* n_waves_out, ka_status* st);
+
 /* The same solve split at the only point where topics stop being independent, for topic-sharded
  * multi-GPU runs (SURVEY.md §8e):
  *   ka_stage_dense_device  capacity, sticky fill, orphan spread (KAS:65-200) + per-broker histograms —

@@ -28,6 +28,11 @@ class KaWaveSendSummary(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int64) for n in ("max_broker_out", "max_broker_out_id")]
 
 
+class KaBrokerUsage(ctypes.Structure):
+    """ka_broker_usage: what one broker holds across a wave plan (every field int64, no padding)."""
+    _fields_ = [(n, ctypes.c_int64) for n in ("before", "peak", "peak_wave", "after", "over_wave")]
+
+
 KA_OK = 0
 KA_ERR_RF_MISMATCH, KA_ERR_RF_NOT_POSITIVE, KA_ERR_RF_GT_BROKERS, KA_ERR_UNASSIGNABLE, KA_ERR_HASH_INDEX = 1, 2, 3, 4, 5
 KA_ERR_BAD_ARG, KA_ERR_CUDA, KA_ERR_NO_DEVICE, KA_ERR_LIMIT = -1, -2, -3, -4
@@ -71,7 +76,8 @@ SYMBOLS = {
     "ka_plan_waves_send_json_parts_rollback": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _i64, _i32, _vp, _i64, _vp,
                                                       _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _i32,
                                                       _vp]),
-    "ka_stage_dense_device": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
+    "ka_wave_broker_usage": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "ka_stage_dense_device":(_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp]),
     "ka_order_device": (_i32, [_vp, _vp, _vp, _vp, _vp]),
     "ka_ctx_set_topic_base": (_i32, [_vp, _i32]),
     "ka_staged_slot_chains": (_i32, [_vp]),

@@ -15,7 +15,7 @@ import ctypes
 import numpy as np
 
 from . import _native
-from ._native import KaMoveSummary, KaStatus, KaWaveSendSummary, KaWaveSummary
+from ._native import KaBrokerUsage, KaMoveSummary, KaStatus, KaWaveSendSummary, KaWaveSummary
 
 # numpy view of ka_move_summary (KaMoveSummary): one record per candidate
 MOVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaMoveSummary._fields_])
@@ -24,6 +24,8 @@ WAVE_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaWaveSummary._fi
 # ka_wave_summary followed by ka_wave_send_summary: one record per wave of a plan with a sender budget
 WAVE_SEND_SUMMARY_DTYPE = np.dtype([(name, np.int64) for name, _ in KaWaveSummary._fields_ + KaWaveSendSummary._fields_])
 _SEND_FIELDS = [name for name, _ in KaWaveSendSummary._fields_]
+# numpy view of ka_broker_usage (KaBrokerUsage): one record per broker of Solver.broker_usage's usage table
+BROKER_USAGE_DTYPE = np.dtype([(name, np.int64) for name, _ in KaBrokerUsage._fields_])
 
 
 class IllegalStateException(Exception):
@@ -635,6 +637,35 @@ class Solver:
         D, doc_wave = (W, np.arange(1, W + 1, dtype=np.int32)) if max_doc_bytes is None else (n_docs.value, doc_wave[:n_docs.value])
         backs = [back_buf[back_off[d]:back_off[d + 1]] for d in range(D)] if rollback else None
         return [json_buf[doc_off[d]:doc_off[d + 1]] for d in range(D)], backs, doc_wave, wave, summary, st
+
+    def broker_usage(self, rep_off, cur_broker, out, out_len, wave, use_brokers, weight=None, base=None, capacity=None):
+        """ka_wave_broker_usage: what every broker of use_brokers (strictly ascending ids, e.g. every broker of the cluster before
+        an exclusion) holds across the wave plan `wave` [Q] (plan_waves' wave unchanged, or any waves >= 0) of the proposed lists
+        out [Q, stride] / out_len [Q] against the current lists cur_broker[rep_off[g] .. rep_off[g + 1]). weight: [Q] int64 per
+        row, None = 1 per row; base, capacity: int64 per broker of use_brokers, None = 0 / no capacity. Returns (usage, a numpy
+        structured array [len(use_brokers)] with the fields of ka_broker_usage, aligned with use_brokers; W; KaStatus). On an
+        error usage is empty and W = 0."""
+        out = np.ascontiguousarray(out, dtype=np.int32)
+        Q = len(out)
+        stride = out.shape[1] if out.ndim == 2 else 1
+        out_len = np.ascontiguousarray(out_len, dtype=np.int32)
+        rep_off = np.ascontiguousarray(rep_off, dtype=np.int64)
+        cur_broker = np.ascontiguousarray(cur_broker, dtype=np.int32)
+        wave = np.ascontiguousarray(wave, dtype=np.int32)
+        use_id = np.ascontiguousarray(use_brokers, dtype=np.int32)
+        n = len(use_id)
+        weight, base, capacity = (None if a is None else np.ascontiguousarray(a, dtype=np.int64) for a in (weight, base, capacity))
+        assert out_len.shape == wave.shape == (Q,) and rep_off.shape == (Q + 1,) and (weight is None or weight.shape == (Q,))
+        assert (base is None or base.shape == (n,)) and (capacity is None or capacity.shape == (n,))
+        usage = np.zeros(n, dtype=BROKER_USAGE_DTYPE)
+        n_waves = ctypes.c_int32(0)
+        st = KaStatus()
+        self._L.ka_wave_broker_usage(self._h, Q, _ptr(rep_off), _ptr(cur_broker), int(stride), _ptr(out_len), _ptr(out), _ptr(weight),
+                                     _ptr(wave), n, _ptr(use_id), _ptr(base), _ptr(capacity), _ptr(usage), ctypes.byref(n_waves),
+                                     ctypes.byref(st))
+        if st.code != 0:
+            return np.zeros(0, dtype=BROKER_USAGE_DTYPE), 0, st
+        return usage, n_waves.value, st
 
     def stage_dense_device(self, T, d_topic_hash, P, RF, d_cur, desired_rf, out_stride, stream=0):
         """Context-free stage (KAS:65-200) of a topic block — shards across GPUs."""

@@ -8,6 +8,7 @@
 #include "kassign_score.cuh"
 #include "kassign_waves.cuh"
 #include "kassign_waves_json.cuh"
+#include "kassign_usage.cuh"
 
 #include <algorithm>
 #include <climits>
@@ -162,6 +163,10 @@ struct ka_ctx {
     // scratch of the rollback documents (ka_plan_waves_json_parts_rollback): the text, then the rollback side's row bytes, CTA
     // sums, prefix R, text total and back_off [D + 1]
     DevBuf d_wv_back, d_wv_bscr;
+    // scratch of ka_wave_broker_usage (its rows go to d_rep_off, d_cur, d_out_len, d_out, d_score_w and d_wv_wave): the usage
+    // table's ids, bases and capacities, before[], the event list twice (the radix passes' two sides), the (digit, tile) counts
+    // and offsets, the report and the meta words
+    DevBuf d_us_id, d_us_base, d_us_cap, d_us_before, d_us_ev, d_us_hist, d_us_out, d_us_meta;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -1394,7 +1399,8 @@ void ka_ctx_destroy(ka_ctx* c) {
                       &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
                       &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec,
                       &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta, &c->d_wv_perm, &c->d_wv_hist, &c->d_wv_doc,
-                      &c->d_wv_part, &c->d_wv_jump, &c->d_wv_send, &c->d_wv_slog, &c->d_wv_ssum})
+                      &c->d_wv_part, &c->d_wv_jump, &c->d_wv_send, &c->d_wv_slog, &c->d_wv_ssum, &c->d_us_id, &c->d_us_base,
+                      &c->d_us_cap, &c->d_us_before, &c->d_us_ev, &c->d_us_hist, &c->d_us_out, &c->d_us_meta})
         b->release();
     c->run.release();
     c->batch_run.release();
@@ -2951,6 +2957,156 @@ int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* c, int32_t T, const int64
     const WaveBack bk{back, back_cap, back_off};
     return plan_waves_json(c, T, part_off, part_id, rep_off, cur_broker, stride, new_len, new_broker, part_weight, max_broker_in, names,
                            name_off, json, json_cap, doc_off, wave, n_waves, summary, summary_cap, &sd, &pt, &bk, st);
+}
+
+// The argument checks of ka_wave_broker_usage, in its order, once st and the ctx are there. R = the current lists' brokers, E =
+// the bound Q x stride + R on the events, W = the largest wave.
+static int usage_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
+                      const int32_t* new_broker, const int64_t* part_weight, const int32_t* wave, int32_t n_use, const int32_t* use_id,
+                      const int64_t* use_base, const int64_t* use_cap, const ka_broker_usage* usage, const int32_t* n_waves_out,
+                      int64_t& R, int64_t& E, int& W, ka_status* st) {
+    if (Q < 0 || stride < 1 || n_use < 0 || (!usage && n_use > 0) || !n_waves_out ||
+        (Q > 0 && (!rep_off || !new_len || !new_broker || !wave)) || (n_use > 0 && !use_id) || (rep_off && rep_off[0] != 0))
+        return set_status(st, KA_ERR_BAD_ARG);
+    for (int64_t g = 0; g < Q; ++g)
+        if (rep_off[g + 1] < rep_off[g]) return set_status(st, KA_ERR_BAD_ARG);
+    R = Q > 0 ? rep_off[Q] : 0;
+    if (R > 0 && !cur_broker) return set_status(st, KA_ERR_BAD_ARG);
+    if (stride > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, stride);
+    if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX);
+    if (n_use > 65535) return set_status(st, KA_ERR_LIMIT, -1, -1, n_use);
+    for (int32_t i = 1; i < n_use; ++i)
+        if (use_id[i] <= use_id[i - 1]) return set_status(st, KA_ERR_BAD_ARG);
+    bool negative = false;
+    for (int64_t g = 0; part_weight && g < Q; ++g) negative |= part_weight[g] < 0;
+    for (int32_t i = 0; i < n_use; ++i) negative |= (use_base && use_base[i] < 0) || (use_cap && use_cap[i] < 0);
+    if (negative) return set_status(st, KA_ERR_BAD_ARG);
+    W = 0;
+    for (int64_t g = 0; g < Q; ++g) {
+        if (new_len[g] < 0 || new_len[g] > stride || wave[g] < 0) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
+        W = std::max(W, (int)wave[g]);
+    }
+    // every usage is a sum of some of these terms: sum base + sum over rows of w x (current + new list lengths)
+    int64_t total = 0;
+    bool over = false;
+    for (int32_t i = 0; use_base && i < n_use; ++i) {
+        over |= use_base[i] > INT64_MAX - total;
+        total = over ? INT64_MAX : total + use_base[i];
+    }
+    for (int64_t g = 0; g < Q && !over; ++g) {
+        const int64_t w = part_weight ? part_weight[g] : 1, k = rep_off[g + 1] - rep_off[g] + new_len[g];
+        over |= w > 0 && k > (INT64_MAX - total) / w;
+        total = over ? INT64_MAX : total + w * k;
+    }
+    E = Q * stride + R;
+    if (over || E > INT_MAX) return set_status(st, KA_ERR_LIMIT);
+    return KA_OK;
+}
+
+// The broker id the device refused in row g: at the first position of its new list, a broker named twice or, for a row with a
+// wave, a receiver (a broker the current list lacks) that the ascending table id[n] lacks.
+static int32_t usage_refused_id(const int32_t* id, int32_t n, const int64_t* rep_off, const int32_t* cur, int32_t stride,
+                                const int32_t* new_len, const int32_t* new_broker, const int32_t* wave, int64_t g) {
+    const int32_t* nb = new_broker + g * stride;
+    const int32_t* cb = cur + rep_off[g];
+    const int64_t m = rep_off[g + 1] - rep_off[g];
+    for (int j = 0; j < new_len[g]; ++j) {
+        if (std::find(nb, nb + j, nb[j]) != nb + j) return nb[j];
+        if (wave[g] > 0 && std::find(cb, cb + m, nb[j]) == cb + m && !std::binary_search(id, id + n, nb[j])) return nb[j];
+    }
+    return 0;
+}
+
+int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                             const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, const int32_t* wave,
+                             int32_t n_use, const int32_t* use_id, const int64_t* use_base, const int64_t* use_cap,
+                             ka_broker_usage* usage, int32_t* n_waves_out, ka_status* st) {
+    if (!st) return KA_ERR_BAD_ARG;
+    if (n_waves_out) *n_waves_out = 0;
+    if (!c) return set_status(st, KA_ERR_NO_DEVICE);
+    int64_t R = 0, E = 0;
+    int W = 0;
+    int rc = usage_args(Q, rep_off, cur_broker, stride, new_len, new_broker, part_weight, wave, n_use, use_id, use_base, use_cap, usage,
+                        n_waves_out, R, E, W, st);
+    if (rc != KA_OK) return rc;
+    // the call reads no Context state: a pending asynchronous status stays pending for ka_last_status
+    if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
+    cudaStream_t s = c->stream;
+    const size_t q = (size_t)Q, nu = (size_t)n_use;
+    const unsigned nblk = (unsigned)std::max<int64_t>((Q + 255) / 256, 1);
+    const size_t ev_bytes = (size_t)std::max<int64_t>(E, 1) * sizeof(KaUseEvent);
+    const size_t tiles = (size_t)(E + KA_USAGE_SORT_MIN_TILE - 1) / KA_USAGE_SORT_MIN_TILE + 1;   // at least the passes' tiles
+    if ((Q > 0 && (c->d_rep_off.reserve((q + 1) * 8) || c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
+                   c->d_out_len.reserve(q * 4) || c->d_out.reserve(q * stride * 4) || c->d_wv_wave.reserve(q * 4) ||
+                   (part_weight && c->d_score_w.reserve(q * 8)))) ||
+        c->d_us_id.reserve(std::max<size_t>(nu, 1) * 4) || (use_base && c->d_us_base.reserve(nu * 8 + 8)) ||
+        (use_cap && c->d_us_cap.reserve(nu * 8 + 8)) || c->d_us_before.reserve(std::max<size_t>(nu, 1) * 8) ||
+        c->d_us_ev.reserve(2 * ev_bytes) || c->d_us_hist.reserve(2 * KA_USAGE_SORT_DIGITS * tiles * 4) ||
+        c->d_us_out.reserve(std::max<size_t>(nu, 1) * sizeof(ka_broker_usage)) || c->d_us_meta.reserve(sizeof(KaUsageMeta)))
+        return set_status(st, KA_ERR_CUDA);
+    const KaUsageMeta meta0{0xFFFFFFFFu, 0u};
+    if ((Q > 0 && (cudaMemcpyAsync(c->d_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
+                   (R > 0 && cudaMemcpyAsync(c->d_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
+                   cudaMemcpyAsync(c->d_out_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
+                   cudaMemcpyAsync(c->d_out.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
+                   cudaMemcpyAsync(c->d_wv_wave.p, wave, q * 4, cudaMemcpyHostToDevice, s) ||
+                   (part_weight && cudaMemcpyAsync(c->d_score_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)))) ||
+        (nu > 0 && cudaMemcpyAsync(c->d_us_id.p, use_id, nu * 4, cudaMemcpyHostToDevice, s)) ||
+        (use_base && nu > 0 && cudaMemcpyAsync(c->d_us_base.p, use_base, nu * 8, cudaMemcpyHostToDevice, s)) ||
+        (use_cap && nu > 0 && cudaMemcpyAsync(c->d_us_cap.p, use_cap, nu * 8, cudaMemcpyHostToDevice, s)) ||
+        (nu > 0 && cudaMemsetAsync(c->d_us_before.p, 0, nu * 8, s)) ||
+        cudaMemcpyAsync(c->d_us_meta.p, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s))
+        return set_status(st, KA_ERR_CUDA);
+    KaUseEvent* ev[2] = {c->d_us_ev.as<KaUseEvent>(), c->d_us_ev.as<KaUseEvent>() + std::max<int64_t>(E, 1)};
+    long long* d_before = c->d_us_before.as<long long>();
+    KaUsageMeta* d_meta = c->d_us_meta.as<KaUsageMeta>();
+    ka_usage_rows_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, stride, c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(),
+                                              c->d_out_len.as<int32_t>(), c->d_out.as<int32_t>(),
+                                              part_weight ? c->d_score_w.as<int64_t>() : nullptr, c->d_wv_wave.as<int32_t>(),
+                                              c->d_us_id.as<int32_t>(), n_use, d_before, ev[0], d_meta);
+    c->launches += 1;
+    KaUsageMeta meta;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, d_meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
+        cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    if (meta.err_row != 0xFFFFFFFFu)
+        return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row,
+                          usage_refused_id(use_id, n_use, rep_off, cur_broker, stride, new_len, new_broker, wave, meta.err_row));
+    // the radix passes: the digits of the wave (1 .. W + 1), then those of the table index (0 .. n_use - 1); none without a wave
+    KaUsageSort p{};
+    p.ne = meta.nev;
+    p.tile = (uint32_t)std::max<int64_t>(KA_USAGE_SORT_MIN_TILE,
+                                         ((int64_t)p.ne + KA_USAGE_SORT_MAX_TILES - 1) / KA_USAGE_SORT_MAX_TILES + 255) / 256 * 256;
+    p.ntiles = (int)std::max<int64_t>(((int64_t)p.ne + p.tile - 1) / p.tile, 1);
+    const int cells = KA_USAGE_SORT_DIGITS * p.ntiles;
+    int32_t* hist = c->d_us_hist.as<int32_t>();
+    int32_t* off = hist + cells;
+    auto bits = [](uint64_t x) { int b = 0; while (x >> b) ++b; return b; };   // x <= 2^31: the shift stays below 64
+    std::vector<int> shifts;
+    if (W > 0) {
+        for (int b = 0; b < bits((uint64_t)W + 1); b += KA_USAGE_SORT_BITS) shifts.push_back(b);
+        for (int b = 0; b < bits((uint64_t)std::max(n_use - 1, 0)); b += KA_USAGE_SORT_BITS) shifts.push_back(32 + b);
+    }
+    int side = 0;
+    for (int shift : shifts) {
+        p.in = ev[side];
+        p.shift = shift;
+        ka_usage_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, hist);
+        ka_level_scan_kernel<<<1, 1024, 0, s>>>(hist, cells, off);
+        ka_usage_sort_scatter_kernel<<<p.ntiles, 256, 0, s>>>(p, off, ev[side ^ 1]);
+        side ^= 1;
+        c->launches += 3;
+    }
+    ka_broker_usage* d_out = c->d_us_out.as<ka_broker_usage>();
+    ka_usage_broker_kernel<<<(unsigned)std::max<int64_t>(((int64_t)n_use + 7) / 8, 1), 256, 0, s>>>(
+        ev[side], p.ne, n_use, W, d_before, use_base ? c->d_us_base.as<int64_t>() : nullptr, use_cap ? c->d_us_cap.as<int64_t>() : nullptr,
+        d_out);
+    c->launches += 1;
+    if (cudaGetLastError() != cudaSuccess ||
+        (nu > 0 && cudaMemcpyAsync(usage, d_out, nu * sizeof(ka_broker_usage), cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    *n_waves_out = W;
+    return set_status(st, KA_OK);
 }
 
 }  // extern "C"

@@ -22,6 +22,8 @@
 //                                                          on their current lists), both sides under the limit
 //   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
 //                                                          receives more than a budget, one document per wave
+//   kassign::brokerUsage                              <->  what every broker holds across a wave plan: its peak, the wave of
+//                                                          the peak and the first wave over its capacity
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
 //
 // Same argument meaning and error behaviour: failures are re-thrown as IllegalStateException /
@@ -365,6 +367,45 @@ public:
                                        int64_t maxBrokerIn, int64_t maxDocBytes, const SendBudget& send,
                                        const std::vector<std::map<int, int64_t>>& weights = {}) {
         return waveDocuments(topics, proposed, maxBrokerIn, &maxDocBytes, true, &send, weights);
+    }
+
+    // What every broker of usageBrokers holds across a wave plan (ka_wave_broker_usage): its peak and the wave of the peak, and
+    // the first wave in which it is over its capacity. `plan` is a planWaves result for these topics and proposed lists (or one
+    // the caller built or reordered): each partition of plan.waves[v] runs in wave v + 1, every other partition is not run.
+    // usageBrokers: strictly ascending (typically every broker of the cluster before an exclusion); base and capacity: empty (0 /
+    // no capacity) or one entry per broker of usageBrokers; weights as planWaves takes them. usage is keyed by broker id and waves
+    // = W; on an error usage is empty.
+    struct BrokerUsage {
+        ka_status status;   // re-throw with throwForStatus
+        int32_t waves = 0;
+        std::map<int32_t, ka_broker_usage> usage;
+    };
+    BrokerUsage brokerUsage(const std::vector<TopicInput>& topics, const std::vector<TopicOutput>& proposed, const WavePlan& plan,
+                            const std::vector<int32_t>& usageBrokers, const std::vector<int64_t>& base = {},
+                            const std::vector<int64_t>& capacity = {}, const std::vector<std::map<int, int64_t>>& weights = {}) {
+        if ((!base.empty() && base.size() != usageBrokers.size()) || (!capacity.empty() && capacity.size() != usageBrokers.size()))
+            throw std::invalid_argument("one base and one capacity per usage broker");
+        const Flat f = flatten(topics, -1);
+        const ProposedRows p = proposedRows(topics, proposed, weights);
+        std::map<std::pair<std::string, int>, int32_t> waveOf;   // (topic, partition) -> its wave
+        for (size_t v = 0; v < plan.waves.size(); ++v)
+            for (const TopicOutput& t : plan.waves[v])
+                for (const auto& e : t.assignment) waveOf[{t.name, e.first}] = (int32_t)v + 1;
+        std::vector<int32_t> wave(f.partId.size(), 0);
+        for (size_t t = 0; t < topics.size(); ++t)
+            for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
+                const auto it = waveOf.find({f.names[t], f.partId[r]});
+                if (it != waveOf.end()) wave[r] = it->second;
+            }
+        BrokerUsage res{};
+        std::vector<ka_broker_usage> usage(usageBrokers.size());
+        ka_wave_broker_usage(ctx_, (int64_t)f.partId.size(), f.repOff.data(), f.cur.data(), p.stride, p.newLen.data(), p.newBroker.data(),
+                             p.w.empty() ? nullptr : p.w.data(), wave.data(), (int32_t)usageBrokers.size(), usageBrokers.data(),
+                             base.empty() ? nullptr : base.data(), capacity.empty() ? nullptr : capacity.data(), usage.data(), &res.waves,
+                             &res.status);
+        if (res.status.code != KA_OK) return res;
+        for (size_t i = 0; i < usageBrokers.size(); ++i) res.usage[usageBrokers[i]] = usage[i];
+        return res;
     }
 
 private:
