@@ -11,6 +11,7 @@
 #include "kassign_usage.cuh"
 
 #include <algorithm>
+#include <array>
 #include <climits>
 #include <cmath>
 #include <cstdio>
@@ -18,6 +19,7 @@
 #include <cstring>
 #include <map>
 #include <new>
+#include <optional>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -31,14 +33,17 @@ constexpr size_t KA_SMEM_BUDGET = 200 * 1024;   // per-CTA dynamic smem we allow
 constexpr uint32_t KA_LUT_SMEM_MAX_RANGE = 32768;
 constexpr uint32_t KA_LUT_GLOBAL_MAX_RANGE = 1u << 25;
 
+// A device allocation that only grows, freed with its owner (ka_ctx_destroy deletes the ctx with its device current).
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     cudaError_t reserve(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
+        release();
         size_t want = bytes + bytes / 8 + 256;
         cudaError_t e = cudaMalloc(&p, want);
         if (e == cudaSuccess) cap = want;
@@ -114,9 +119,6 @@ struct RunScratch {
             if (cudaError_t e = w.b->reserve(w.bytes)) return e;
         return cudaSuccess;
     }
-    void release() {
-        for (DevBuf* b : {&rec, &perm, &ntl, &lend, &loff, &lvl_end, &tstatus, &flags}) b->release();
-    }
 };
 
 }  // namespace
@@ -128,6 +130,7 @@ struct ka_ctx {
     cudaStream_t aux = nullptr;     // stage of the pipelined (super-chunk) solve
     cudaStream_t sb1 = nullptr;     // slot-0 chains (the slot-1 chains + emit run on the caller's stream)
     cudaStream_t sj = nullptr;      // device JSON emission, streamed copy-out
+    std::array<cudaStream_t*, 4> streams() { return {&stream, &aux, &sb1, &sj}; }
     // broker table: the kernels' view of it (in d_blob, d_glut, d_broker_id; N = 0 before ka_ctx_set_brokers) and its ids
     KaBrokers br{};
     std::vector<int32_t> broker_id;
@@ -146,9 +149,9 @@ struct ka_ctx {
     // scratch of ka_score_candidates / ka_score_clusters: row weights, the K summaries, the per-broker sums [3][ΣN], the tables'
     // offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
-    // scratch of ka_plan_waves (its inputs go to d_rep_off, d_cur, d_out_len, d_out and d_score_w): the rows pass's per-row
-    // outputs and records, the packed records, the per-CTA counts and offsets, the chain's per-broker words when they leave
-    // shared memory, the bucket log, the summaries and the meta words
+    // scratch of ka_plan_waves (its rows: upload_wave_rows): the rows pass's per-row outputs and records, the packed records, the
+    // per-CTA counts and offsets, the chain's per-broker words when they leave shared memory, the bucket log, the summaries and
+    // the meta words
     DevBuf d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state, d_wv_log, d_wv_sum, d_wv_meta;
     // scratch of the sender budget (ka_plan_waves_send and its JSON form): the send table, the sender bucket log and the sender
     // summaries (the per-sender words share d_wv_state)
@@ -163,9 +166,8 @@ struct ka_ctx {
     // scratch of the rollback documents (ka_plan_waves_json_parts_rollback): the text, then the rollback side's row bytes, CTA
     // sums, prefix R, text total and back_off [D + 1]
     DevBuf d_wv_back, d_wv_bscr;
-    // scratch of ka_wave_broker_usage (its rows go to d_rep_off, d_cur, d_out_len, d_out, d_score_w and d_wv_wave): the usage
-    // table's ids, bases and capacities, before[], the event list twice (the radix passes' two sides), the (digit, tile) counts
-    // and offsets, the report and the meta words
+    // scratch of ka_wave_broker_usage (its rows: upload_wave_rows): the usage table's ids, bases and capacities, before[], the
+    // event list twice (the radix passes' two sides), the (digit, tile) counts and offsets, the report and the meta words
     DevBuf d_us_id, d_us_base, d_us_cap, d_us_before, d_us_ev, d_us_hist, d_us_out, d_us_meta;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
@@ -1377,7 +1379,7 @@ ka_ctx* ka_ctx_create(int32_t device) {
     bool ok = cudaHostAlloc(reinterpret_cast<void**>(&c->h_pin), sizeof(HostPinned), cudaHostAllocDefault) == cudaSuccess &&
               cudaHostAlloc(reinterpret_cast<void**>(&c->h_frag), 2 * KA_MAX_JSON_FRAGS * sizeof(unsigned long long),
                             cudaHostAllocDefault) == cudaSuccess;
-    for (cudaStream_t* s : {&c->stream, &c->aux, &c->sb1, &c->sj})
+    for (cudaStream_t* s : c->streams())
         ok = ok && cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) == cudaSuccess;
     for_each_event(c, [&](cudaEvent_t& e, bool timed) {
         ok = ok && cudaEventCreateWithFlags(&e, timed ? cudaEventDefault : cudaEventDisableTiming) == cudaSuccess;
@@ -1392,26 +1394,14 @@ ka_ctx* ka_ctx_create(int32_t device) {
 void ka_ctx_destroy(ka_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    for (cudaStream_t s : {c->stream, c->aux, c->sb1, c->sj})
-        if (s) cudaStreamSynchronize(s);
-    for (DevBuf* b : {&c->d_blob, &c->d_glut, &c->d_broker_id, &c->d_ctr8, &c->d_hash, &c->d_part_off, &c->d_rep_off, &c->d_cur,
-                      &c->d_out, &c->d_out_len, &c->d_json, &c->d_names, &c->d_name_off, &c->d_part_id, &c->d_json_rowlen,
-                      &c->d_json_blocksum, &c->d_json_state, &c->d_batch_tab, &c->d_batch_ctr, &c->d_score_w, &c->d_score_sum,
-                      &c->d_score_brk, &c->d_score_off, &c->d_json_seg, &c->d_wv_nrecv, &c->d_wv_wave, &c->d_wv_tmp, &c->d_wv_rec,
-                      &c->d_wv_cnt, &c->d_wv_state, &c->d_wv_log, &c->d_wv_sum, &c->d_wv_meta, &c->d_wv_perm, &c->d_wv_hist, &c->d_wv_doc,
-                      &c->d_wv_part, &c->d_wv_jump, &c->d_wv_send, &c->d_wv_slog, &c->d_wv_ssum, &c->d_us_id, &c->d_us_base,
-                      &c->d_us_cap, &c->d_us_before, &c->d_us_ev, &c->d_us_hist, &c->d_us_out, &c->d_us_meta})
-        b->release();
-    c->run.release();
-    c->batch_run.release();
-    for_each_event(c, [](cudaEvent_t& e, bool) {
-        if (e) cudaEventDestroy(e);
-    });
-    for (cudaStream_t s : {c->stream, c->aux, c->sb1, c->sj})
-        if (s) cudaStreamDestroy(s);
+    for (cudaStream_t* s : c->streams())
+        if (*s) cudaStreamSynchronize(*s);
+    for_each_event(c, [](cudaEvent_t& e, bool) { if (e) cudaEventDestroy(e); });
+    for (cudaStream_t* s : c->streams())
+        if (*s) cudaStreamDestroy(*s);
     if (c->h_pin) cudaFreeHost(c->h_pin);
     if (c->h_frag) cudaFreeHost(c->h_frag);
-    delete c;
+    delete c;   // the DevBufs free themselves, on c->device
 }
 
 int32_t ka_ctx_reset(ka_ctx* c) {
@@ -2466,19 +2456,41 @@ struct WaveSend {
     ka_wave_send_summary* summary;
 };
 
-// The broker id the device refused in row g: at the first position of its new list, a broker named twice or a receiver (a
-// broker the current list lacks) that the table `ids` lacks; with a sender part and no such position, the row's sender (the
-// first of its current list), which the send table lacks.
-static int32_t wave_refused_id(const std::vector<int32_t>& ids, const int64_t* rep_off, const int32_t* cur, int32_t stride,
-                               const int32_t* new_len, const int32_t* new_broker, int64_t g, const WaveSend* sd) {
+// The row checks of a wave-row call (ka_plan_waves* and ka_wave_broker_usage) that follow its own first argument check, in this
+// order: rep_off never decreases, cur_broker is there for R = rep_off[Q] > 0 brokers, stride <= KA_MAX_SLOTS, Q < 2^31.
+static int wave_rows_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, int64_t& R, ka_status* st) {
+    for (int64_t g = 0; g < Q; ++g)
+        if (rep_off[g + 1] < rep_off[g]) return set_status(st, KA_ERR_BAD_ARG);
+    R = Q > 0 ? rep_off[Q] : 0;
+    if (R > 0 && !cur_broker) return set_status(st, KA_ERR_BAD_ARG);
+    if (stride > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, stride);
+    if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX);
+    return KA_OK;
+}
+
+// Every row's new_len[g] in 0 .. stride and, with wave, wave[g] >= 0; the lowest row g that fails is refused (st.a = g).
+// W = the largest wave (0 without wave).
+static int wave_lens_args(int64_t Q, int32_t stride, const int32_t* new_len, const int32_t* wave, int& W, ka_status* st) {
+    W = 0;
+    for (int64_t g = 0; g < Q; ++g) {
+        if (new_len[g] < 0 || new_len[g] > stride || (wave && wave[g] < 0)) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
+        if (wave) W = std::max(W, (int)wave[g]);
+    }
+    return KA_OK;
+}
+
+// The broker id the device refused in row g, if any: at the first failing position of its new list, a broker named twice or,
+// with `receivers`, a receiver (a broker the current list lacks) that the ascending table id[n] lacks.
+static std::optional<int32_t> refused_id(const int32_t* id, size_t n, const int64_t* rep_off, const int32_t* cur, int32_t stride,
+                                         const int32_t* new_len, const int32_t* new_broker, int64_t g, bool receivers) {
     const int32_t* nb = new_broker + g * stride;
     const int32_t* cb = cur + rep_off[g];
     const int64_t m = rep_off[g + 1] - rep_off[g];
     for (int j = 0; j < new_len[g]; ++j) {
         if (std::find(nb, nb + j, nb[j]) != nb + j) return nb[j];
-        if (std::find(cb, cb + m, nb[j]) == cb + m && !std::binary_search(ids.begin(), ids.end(), nb[j])) return nb[j];
+        if (receivers && std::find(cb, cb + m, nb[j]) == cb + m && !std::binary_search(id, id + n, nb[j])) return nb[j];
     }
-    return sd ? cb[0] : 0;
+    return std::nullopt;
 }
 
 // The argument checks of ka_plan_waves, in its order, once st and the ctx are there. R = the current lists' brokers, positions
@@ -2489,18 +2501,13 @@ static int wave_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_broke
     if (Q < 0 || stride < 1 || !n_waves || summary_cap < 0 || (!summary && summary_cap > 0) || max_broker_in < 1 ||
         (Q > 0 && (!rep_off || !new_len || !new_broker)) || (rep_off && rep_off[0] != 0))
         return set_status(st, KA_ERR_BAD_ARG);
-    for (int64_t g = 0; g < Q; ++g)
-        if (rep_off[g + 1] < rep_off[g]) return set_status(st, KA_ERR_BAD_ARG);
-    R = Q > 0 ? rep_off[Q] : 0;
-    if (R > 0 && !cur_broker) return set_status(st, KA_ERR_BAD_ARG);
-    if (stride > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, stride);
-    if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX);
+    int rc, W;   // the rows have no waves yet: W stays 0
+    if ((rc = wave_rows_args(Q, rep_off, cur_broker, stride, R, st)) != KA_OK ||
+        (rc = wave_lens_args(Q, stride, new_len, nullptr, W, st)) != KA_OK)
+        return rc;
     positions = 0;
-    for (int64_t g = 0; g < Q; ++g) {
-        if (new_len[g] < 0 || new_len[g] > stride) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
-        positions += new_len[g];
-    }
-    const int rc = weights_code(part_weight, Q, 8);   // a row adds at most 8 x its weight to a wave
+    for (int64_t g = 0; g < Q; ++g) positions += new_len[g];
+    rc = weights_code(part_weight, Q, 8);   // a row adds at most 8 x its weight to a wave
     return rc != KA_OK ? set_status(st, rc) : KA_OK;
 }
 
@@ -2514,11 +2521,31 @@ static int wave_send_args(const WaveSend& sd, int32_t summary_cap, ka_status* st
     return KA_OK;
 }
 
-// The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the inputs up (into the buffers of the
-// host-buffer solve and score calls: every such call is synchronous), the rows / scan / compact / chain kernels, the meta words
-// back, then the sum and the two peak kernels (enqueued, not awaited). Leaves every row's wave in d_wv_wave, its receivers in
-// d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids still N - index) in d_wv_sum. A sender part sd (null:
-// none) adds the sender rule and its summaries (ids still n - index) in d_wv_ssum.
+// The Q > 0 rows of a wave-row call (ka_plan_waves*, ka_wave_broker_usage) up on c->stream, into d_rep_off, d_cur (R brokers),
+// d_out_len, d_out, d_score_w (weights, null: none) and d_wv_wave (waves, null: none). These buffers belong to the synchronous
+// host-buffer calls (solves, scores, wave plans, broker usage): one call may overwrite what another left there, because each
+// awaits its own work before it returns.
+static int upload_wave_rows(ka_ctx* c, int64_t Q, int64_t R, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
+                            const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, const int32_t* wave) {
+    cudaStream_t s = c->stream;
+    const size_t q = (size_t)Q;
+    if (c->d_rep_off.reserve((q + 1) * 8) || c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) || c->d_out_len.reserve(q * 4) ||
+        c->d_out.reserve(q * stride * 4) || (part_weight && c->d_score_w.reserve(q * 8)) || (wave && c->d_wv_wave.reserve(q * 4)) ||
+        cudaMemcpyAsync(c->d_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
+        (R > 0 && cudaMemcpyAsync(c->d_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
+        cudaMemcpyAsync(c->d_out_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
+        cudaMemcpyAsync(c->d_out.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
+        (part_weight && cudaMemcpyAsync(c->d_score_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)) ||
+        (wave && cudaMemcpyAsync(c->d_wv_wave.p, wave, q * 4, cudaMemcpyHostToDevice, s)))
+        return KA_ERR_CUDA;
+    return KA_OK;
+}
+
+// The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the rows up (upload_wave_rows), the
+// rows / scan / compact / chain kernels, the meta words back, then the sum and the two peak kernels (enqueued, not awaited).
+// Leaves every row's wave in d_wv_wave, its receivers in d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids
+// still N - index) in d_wv_sum. A sender part sd (null: none) adds the sender rule and its summaries (ids still n - index) in
+// d_wv_ssum.
 static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, const int64_t* rep_off, const int32_t* cur_broker,
                             int32_t stride, const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
                             int64_t max_broker_in, const WaveSend* sd, int& W, ka_status* st) {
@@ -2529,8 +2556,7 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     // the chain's per-broker and per-sender words in global memory
     const bool gstate = (size_t)(N + ns) * KA_WAVE_BROKER_BYTES > KA_SMEM_BUDGET;
     const size_t q = (size_t)Q;
-    if (c->d_rep_off.reserve((q + 1) * 8) || c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
-        c->d_out_len.reserve(q * 4) || c->d_out.reserve(q * stride * 4) || (part_weight && c->d_score_w.reserve(q * 8)) ||
+    if (upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, nullptr) != KA_OK ||
         c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
         c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
         c->d_wv_state.reserve(gstate ? (size_t)(N + ns) * KA_WAVE_BROKER_BYTES : 16) ||
@@ -2560,13 +2586,7 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     int32_t* d_cnt = c->d_wv_cnt.as<int32_t>();
     int32_t* d_off = d_cnt + nblk;
     KaWaveMeta* d_meta = c->d_wv_meta.as<KaWaveMeta>();
-    if (cudaMemcpyAsync(c->d_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
-        (R > 0 && cudaMemcpyAsync(c->d_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
-        cudaMemcpyAsync(c->d_out_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
-        cudaMemcpyAsync(c->d_out.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
-        (part_weight && cudaMemcpyAsync(c->d_score_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)) ||
-        cudaMemcpyAsync(d_meta, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s))
-        return set_status(st, KA_ERR_CUDA);
+    if (cudaMemcpyAsync(d_meta, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
     KaWaveRec* d_rec = c->d_wv_rec.as<KaWaveRec>();
     int32_t* d_wave = c->d_wv_wave.as<int32_t>();
     int8_t* d_nrecv = c->d_wv_nrecv.as<int8_t>();
@@ -2592,9 +2612,11 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&back, d_meta, sizeof(back), cudaMemcpyDeviceToHost, s) ||
         cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
-    if (meta.err_row != 0xFFFFFFFFu)
-        return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row,
-                          wave_refused_id(c->broker_id, rep_off, cur_broker, stride, new_len, new_broker, meta.err_row, sd));
+    if (meta.err_row != 0xFFFFFFFFu) {   // no refused position: with a sender part, the row's sender, which the send table lacks
+        const auto id = refused_id(c->broker_id.data(), c->broker_id.size(), rep_off, cur_broker, stride, new_len, new_broker,
+                                   meta.err_row, true);
+        return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row, id ? *id : sd ? cur_broker[rep_off[meta.err_row]] : 0);
+    }
     W = std::max(meta.waves, meta.changed);
     const size_t sum_bytes = (size_t)std::max(W, 1) * sizeof(ka_wave_summary);
     const size_t ssum_bytes = (size_t)std::max(W, 1) * sizeof(ka_wave_send_summary);
@@ -2671,21 +2693,32 @@ int32_t ka_plan_waves_send(ka_ctx* c, int64_t Q, const int64_t* rep_off, const i
                       summary_cap, &sd, st);
 }
 
+// The tiling of a radix pass over n items: `tile` items per CTA, ntiles >= 1 CTAs. Returns the (digit, tile) cells: the pass's
+// hist buffer holds their counts, then their offsets at hist + cells, then the offsets' total.
+static int radix_tiles(int64_t n, uint32_t& tile, int& ntiles) {
+    tile = (uint32_t)std::max<int64_t>(KA_RADIX_MIN_TILE, ((n + KA_RADIX_MAX_TILES - 1) / KA_RADIX_MAX_TILES + 255) / 256 * 256);
+    ntiles = (int)std::max<int64_t>((n + tile - 1) / tile, 1);
+    return KA_RADIX_DIGITS * ntiles;
+}
+
+// Bytes of a hist buffer for the passes over at most n items (a tile holds at least KA_RADIX_MIN_TILE of them).
+static size_t radix_hist_bytes(int64_t n) {
+    return (2 * (size_t)KA_RADIX_DIGITS * std::max<int64_t>((n + KA_RADIX_MIN_TILE - 1) / KA_RADIX_MIN_TILE, 1) + 1) * 4;
+}
+
 // The radix passes of ka_plan_waves_json over the plan's d_wv_wave: d_wv_perm (two arrays of Q rows) ends with the changed
 // rows ordered by (wave, row) in the array returned, and the (digit, tile) offsets end with M, the changed rows, at n_rows.
 static const int32_t* enq_wave_group(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const int32_t*& n_rows) {
     KaWaveSort p{};
     p.wave = c->d_wv_wave.as<int32_t>();
     p.Q = (uint32_t)Q;
-    p.tile = (uint32_t)std::max<int64_t>(KA_WAVE_SORT_MIN_TILE, ((Q + KA_WAVE_SORT_MAX_TILES - 1) / KA_WAVE_SORT_MAX_TILES + 255) / 256 * 256);
-    p.ntiles = (int)((Q + p.tile - 1) / p.tile);
-    const int cells = KA_WAVE_SORT_DIGITS * p.ntiles;
+    const int cells = radix_tiles(Q, p.tile, p.ntiles);
     int32_t* hist = c->d_wv_hist.as<int32_t>();
     int32_t* off = hist + cells;
     int32_t* perm[2] = {c->d_wv_perm.as<int32_t>(), c->d_wv_perm.as<int32_t>() + Q};
     p.n_ptr = n_rows = off + cells;
     int pass = 0;
-    for (; pass == 0 || W >> p.shift; ++pass, p.shift += KA_WAVE_SORT_BITS) {
+    for (; pass == 0 || W >> p.shift; ++pass, p.shift += KA_RADIX_BITS) {
         p.in = pass ? perm[(pass - 1) & 1] : nullptr;
         ka_wave_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, hist);
         ka_level_scan_kernel<<<1, 1024, 0, s>>>(hist, cells, off);
@@ -2819,10 +2852,9 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     const size_t q = (size_t)Q;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
     const int64_t cap = std::min(json_cap, bound);
-    const size_t tiles = (size_t)(Q + KA_WAVE_SORT_MIN_TILE - 1) / KA_WAVE_SORT_MIN_TILE;   // at least the passes' tiles
     if (c->d_part_off.reserve((size_t)(T + 1) * 8) || c->d_json.reserve((size_t)std::max<int64_t>(cap, 1)) ||
         c->d_json_rowlen.reserve(q * 4) || c->d_json_blocksum.reserve((size_t)nblk * 8) || c->d_wv_perm.reserve(2 * q * 4) ||
-        c->d_wv_hist.reserve((2 * KA_WAVE_SORT_DIGITS * tiles + 1) * 4) || c->d_wv_doc.reserve((pt ? q + 3 : (size_t)W + 2) * 8) ||
+        c->d_wv_hist.reserve(radix_hist_bytes(Q)) || c->d_wv_doc.reserve((pt ? q + 3 : (size_t)W + 2) * 8) ||
         upload_names(c, s, T, Q, names, name_off, part_id) != KA_OK ||
         cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s))
         return set_status(st, KA_ERR_CUDA);
@@ -2968,12 +3000,8 @@ static int usage_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_brok
     if (Q < 0 || stride < 1 || n_use < 0 || (!usage && n_use > 0) || !n_waves_out ||
         (Q > 0 && (!rep_off || !new_len || !new_broker || !wave)) || (n_use > 0 && !use_id) || (rep_off && rep_off[0] != 0))
         return set_status(st, KA_ERR_BAD_ARG);
-    for (int64_t g = 0; g < Q; ++g)
-        if (rep_off[g + 1] < rep_off[g]) return set_status(st, KA_ERR_BAD_ARG);
-    R = Q > 0 ? rep_off[Q] : 0;
-    if (R > 0 && !cur_broker) return set_status(st, KA_ERR_BAD_ARG);
-    if (stride > KA_MAX_SLOTS) return set_status(st, KA_ERR_LIMIT, -1, -1, stride);
-    if (Q >= (int64_t)1 << 31) return set_status(st, KA_ERR_LIMIT, -1, -1, INT_MAX);
+    int rc = wave_rows_args(Q, rep_off, cur_broker, stride, R, st);
+    if (rc != KA_OK) return rc;
     if (n_use > 65535) return set_status(st, KA_ERR_LIMIT, -1, -1, n_use);
     for (int32_t i = 1; i < n_use; ++i)
         if (use_id[i] <= use_id[i - 1]) return set_status(st, KA_ERR_BAD_ARG);
@@ -2981,11 +3009,7 @@ static int usage_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_brok
     for (int64_t g = 0; part_weight && g < Q; ++g) negative |= part_weight[g] < 0;
     for (int32_t i = 0; i < n_use; ++i) negative |= (use_base && use_base[i] < 0) || (use_cap && use_cap[i] < 0);
     if (negative) return set_status(st, KA_ERR_BAD_ARG);
-    W = 0;
-    for (int64_t g = 0; g < Q; ++g) {
-        if (new_len[g] < 0 || new_len[g] > stride || wave[g] < 0) return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)g);
-        W = std::max(W, (int)wave[g]);
-    }
+    if ((rc = wave_lens_args(Q, stride, new_len, wave, W, st)) != KA_OK) return rc;
     // every usage is a sum of some of these terms: sum base + sum over rows of w x (current + new list lengths)
     int64_t total = 0;
     bool over = false;
@@ -3003,20 +3027,6 @@ static int usage_args(int64_t Q, const int64_t* rep_off, const int32_t* cur_brok
     return KA_OK;
 }
 
-// The broker id the device refused in row g: at the first position of its new list, a broker named twice or, for a row with a
-// wave, a receiver (a broker the current list lacks) that the ascending table id[n] lacks.
-static int32_t usage_refused_id(const int32_t* id, int32_t n, const int64_t* rep_off, const int32_t* cur, int32_t stride,
-                                const int32_t* new_len, const int32_t* new_broker, const int32_t* wave, int64_t g) {
-    const int32_t* nb = new_broker + g * stride;
-    const int32_t* cb = cur + rep_off[g];
-    const int64_t m = rep_off[g + 1] - rep_off[g];
-    for (int j = 0; j < new_len[g]; ++j) {
-        if (std::find(nb, nb + j, nb[j]) != nb + j) return nb[j];
-        if (wave[g] > 0 && std::find(cb, cb + m, nb[j]) == cb + m && !std::binary_search(id, id + n, nb[j])) return nb[j];
-    }
-    return 0;
-}
-
 int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                              const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, const int32_t* wave,
                              int32_t n_use, const int32_t* use_id, const int64_t* use_base, const int64_t* use_cap,
@@ -3032,26 +3042,17 @@ int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const
     // the call reads no Context state: a pending asynchronous status stays pending for ka_last_status
     if ((rc = enter(c, false)) != KA_OK) return set_status(st, rc);
     cudaStream_t s = c->stream;
-    const size_t q = (size_t)Q, nu = (size_t)n_use;
+    const size_t nu = (size_t)n_use;
     const unsigned nblk = (unsigned)std::max<int64_t>((Q + 255) / 256, 1);
     const size_t ev_bytes = (size_t)std::max<int64_t>(E, 1) * sizeof(KaUseEvent);
-    const size_t tiles = (size_t)(E + KA_USAGE_SORT_MIN_TILE - 1) / KA_USAGE_SORT_MIN_TILE + 1;   // at least the passes' tiles
-    if ((Q > 0 && (c->d_rep_off.reserve((q + 1) * 8) || c->d_cur.reserve((size_t)std::max<int64_t>(R, 1) * 4) ||
-                   c->d_out_len.reserve(q * 4) || c->d_out.reserve(q * stride * 4) || c->d_wv_wave.reserve(q * 4) ||
-                   (part_weight && c->d_score_w.reserve(q * 8)))) ||
+    if ((Q > 0 && upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, wave) != KA_OK) ||
         c->d_us_id.reserve(std::max<size_t>(nu, 1) * 4) || (use_base && c->d_us_base.reserve(nu * 8 + 8)) ||
         (use_cap && c->d_us_cap.reserve(nu * 8 + 8)) || c->d_us_before.reserve(std::max<size_t>(nu, 1) * 8) ||
-        c->d_us_ev.reserve(2 * ev_bytes) || c->d_us_hist.reserve(2 * KA_USAGE_SORT_DIGITS * tiles * 4) ||
+        c->d_us_ev.reserve(2 * ev_bytes) || c->d_us_hist.reserve(radix_hist_bytes(E)) ||
         c->d_us_out.reserve(std::max<size_t>(nu, 1) * sizeof(ka_broker_usage)) || c->d_us_meta.reserve(sizeof(KaUsageMeta)))
         return set_status(st, KA_ERR_CUDA);
     const KaUsageMeta meta0{0xFFFFFFFFu, 0u};
-    if ((Q > 0 && (cudaMemcpyAsync(c->d_rep_off.p, rep_off, (q + 1) * 8, cudaMemcpyHostToDevice, s) ||
-                   (R > 0 && cudaMemcpyAsync(c->d_cur.p, cur_broker, (size_t)R * 4, cudaMemcpyHostToDevice, s)) ||
-                   cudaMemcpyAsync(c->d_out_len.p, new_len, q * 4, cudaMemcpyHostToDevice, s) ||
-                   cudaMemcpyAsync(c->d_out.p, new_broker, q * stride * 4, cudaMemcpyHostToDevice, s) ||
-                   cudaMemcpyAsync(c->d_wv_wave.p, wave, q * 4, cudaMemcpyHostToDevice, s) ||
-                   (part_weight && cudaMemcpyAsync(c->d_score_w.p, part_weight, q * 8, cudaMemcpyHostToDevice, s)))) ||
-        (nu > 0 && cudaMemcpyAsync(c->d_us_id.p, use_id, nu * 4, cudaMemcpyHostToDevice, s)) ||
+    if ((nu > 0 && cudaMemcpyAsync(c->d_us_id.p, use_id, nu * 4, cudaMemcpyHostToDevice, s)) ||
         (use_base && nu > 0 && cudaMemcpyAsync(c->d_us_base.p, use_base, nu * 8, cudaMemcpyHostToDevice, s)) ||
         (use_cap && nu > 0 && cudaMemcpyAsync(c->d_us_cap.p, use_cap, nu * 8, cudaMemcpyHostToDevice, s)) ||
         (nu > 0 && cudaMemsetAsync(c->d_us_before.p, 0, nu * 8, s)) ||
@@ -3069,23 +3070,21 @@ int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, d_meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
         cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
-    if (meta.err_row != 0xFFFFFFFFu)
-        return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row,
-                          usage_refused_id(use_id, n_use, rep_off, cur_broker, stride, new_len, new_broker, wave, meta.err_row));
+    if (meta.err_row != 0xFFFFFFFFu) {
+        const auto id = refused_id(use_id, nu, rep_off, cur_broker, stride, new_len, new_broker, meta.err_row, wave[meta.err_row] > 0);
+        return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)meta.err_row, id.value_or(0));
+    }
     // the radix passes: the digits of the wave (1 .. W + 1), then those of the table index (0 .. n_use - 1); none without a wave
     KaUsageSort p{};
     p.ne = meta.nev;
-    p.tile = (uint32_t)std::max<int64_t>(KA_USAGE_SORT_MIN_TILE,
-                                         ((int64_t)p.ne + KA_USAGE_SORT_MAX_TILES - 1) / KA_USAGE_SORT_MAX_TILES + 255) / 256 * 256;
-    p.ntiles = (int)std::max<int64_t>(((int64_t)p.ne + p.tile - 1) / p.tile, 1);
-    const int cells = KA_USAGE_SORT_DIGITS * p.ntiles;
+    const int cells = radix_tiles(p.ne, p.tile, p.ntiles);
     int32_t* hist = c->d_us_hist.as<int32_t>();
     int32_t* off = hist + cells;
     auto bits = [](uint64_t x) { int b = 0; while (x >> b) ++b; return b; };   // x <= 2^31: the shift stays below 64
     std::vector<int> shifts;
     if (W > 0) {
-        for (int b = 0; b < bits((uint64_t)W + 1); b += KA_USAGE_SORT_BITS) shifts.push_back(b);
-        for (int b = 0; b < bits((uint64_t)std::max(n_use - 1, 0)); b += KA_USAGE_SORT_BITS) shifts.push_back(32 + b);
+        for (int b = 0; b < bits((uint64_t)W + 1); b += KA_RADIX_BITS) shifts.push_back(b);
+        for (int b = 0; b < bits((uint64_t)std::max(n_use - 1, 0)); b += KA_RADIX_BITS) shifts.push_back(32 + b);
     }
     int side = 0;
     for (int shift : shifts) {

@@ -20,6 +20,13 @@
 #define KA_DEAD 0xFFFFu     // "broker not in the live set" marker in 16-bit index space
 #define KA_FULL 0xFFFFFFFFu
 
+// The stable LSD radix passes (the wave documents' row grouping, the broker usage's event sort): 8-bit digits.
+#define KA_RADIX_BITS 8
+#define KA_RADIX_DIGITS (1 << KA_RADIX_BITS)
+#define KA_RADIX_MIN_TILE 2048   // items per CTA of a pass, at least (a multiple of the 256 threads)
+#define KA_RADIX_MAX_TILES 1024  // CTAs of a pass, at most: the (digit, tile) table stays within 256 k entries
+static_assert(KA_RADIX_DIGITS == 256, "one thread per digit value");
+
 // Error codes (mirror include/kassign.h)
 #define KA_E_RF_MISMATCH 1
 #define KA_E_RF_NOT_POSITIVE 2

@@ -23,12 +23,6 @@
 #include "kassign_common.cuh"
 #include "../../include/kassign.h"
 
-#define KA_USAGE_SORT_BITS 8
-#define KA_USAGE_SORT_DIGITS (1 << KA_USAGE_SORT_BITS)
-#define KA_USAGE_SORT_MIN_TILE 2048   // events per CTA of a pass, at least (a multiple of the 256 threads)
-#define KA_USAGE_SORT_MAX_TILES 1024  // CTAs of a pass, at most: the (digit, tile) table stays within 256 k entries
-static_assert(KA_USAGE_SORT_DIGITS == 256, "one thread per digit value");
-
 // One event: from wave `wave` on, broker index `idx` holds w more (w < 0: a freed copy). Sorted by the 64-bit key
 // idx << 32 | wave.
 struct __align__(16) KaUseEvent {
@@ -173,12 +167,12 @@ struct KaUsageSort {
 };
 
 __device__ __forceinline__ int ka_usage_digit(const KaUsageSort& p, const KaUseEvent& e) {
-    return (int)(ka_usage_key(e) >> p.shift) & (KA_USAGE_SORT_DIGITS - 1);
+    return (int)(ka_usage_key(e) >> p.shift) & (KA_RADIX_DIGITS - 1);
 }
 
 // grid ntiles, 256 threads: hist[digit * ntiles + tile] = the tile's events with that digit.
 __global__ void __launch_bounds__(256) ka_usage_sort_hist_kernel(const KaUsageSort p, int32_t* __restrict__ hist) {
-    __shared__ int h[KA_USAGE_SORT_DIGITS];
+    __shared__ int h[KA_RADIX_DIGITS];
     h[threadIdx.x] = 0;
     __syncthreads();
     const uint64_t lo = (uint64_t)blockIdx.x * p.tile;
@@ -193,8 +187,8 @@ __global__ void __launch_bounds__(256) ka_usage_sort_hist_kernel(const KaUsageSo
 // same digit (match_any, lanes in event order), then behind the earlier warps' and the earlier rounds' events of that digit.
 __global__ void __launch_bounds__(256) ka_usage_sort_scatter_kernel(const KaUsageSort p, const int32_t* __restrict__ off,
                                                                     KaUseEvent* __restrict__ out) {
-    __shared__ int base[KA_USAGE_SORT_DIGITS];
-    __shared__ int wcnt[8][KA_USAGE_SORT_DIGITS];
+    __shared__ int base[KA_RADIX_DIGITS];
+    __shared__ int wcnt[8][KA_RADIX_DIGITS];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     base[threadIdx.x] = off[threadIdx.x * p.ntiles + blockIdx.x];
     const uint64_t lo = (uint64_t)blockIdx.x * p.tile;

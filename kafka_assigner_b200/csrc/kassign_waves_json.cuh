@@ -43,12 +43,6 @@
 #include "kassign_json.cuh"
 #include "kassign_waves.cuh"
 
-#define KA_WAVE_SORT_BITS 8
-#define KA_WAVE_SORT_DIGITS (1 << KA_WAVE_SORT_BITS)
-#define KA_WAVE_SORT_MIN_TILE 2048   // rows per CTA of a pass, at least (a multiple of the 256 threads)
-#define KA_WAVE_SORT_MAX_TILES 1024  // CTAs of a pass, at most: the (digit, tile) table stays within 256 k entries
-static_assert(KA_WAVE_SORT_DIGITS == 256, "one thread per digit value");
-
 // One radix pass over the keys wave[g] >> shift. in == null: the items are the rows 0..Q-1 (first pass); else the *n_ptr rows
 // in[]. A row of wave 0 is no item. Tile b owns items [b * tile, (b + 1) * tile).
 struct KaWaveSort {
@@ -65,13 +59,13 @@ __device__ __forceinline__ bool ka_wave_sort_item(const KaWaveSort& p, uint32_t 
     if (i >= hi) return false;
     g = p.in ? p.in[i] : (int32_t)i;
     const int v = p.wave[g];
-    digit = (v >> p.shift) & (KA_WAVE_SORT_DIGITS - 1);
+    digit = (v >> p.shift) & (KA_RADIX_DIGITS - 1);
     return v > 0;
 }
 
 // grid ntiles, 256 threads: hist[digit * ntiles + tile] = the tile's items with that digit.
 __global__ void __launch_bounds__(256) ka_wave_sort_hist_kernel(const KaWaveSort p, int32_t* __restrict__ hist) {
-    __shared__ int h[KA_WAVE_SORT_DIGITS];
+    __shared__ int h[KA_RADIX_DIGITS];
     h[threadIdx.x] = 0;
     __syncthreads();
     const uint32_t n = p.in ? (uint32_t)*p.n_ptr : p.Q;
@@ -91,8 +85,8 @@ __global__ void __launch_bounds__(256) ka_wave_sort_hist_kernel(const KaWaveSort
 // same digit (match_any, lanes in item order), then behind the earlier warps' and the earlier rounds' items of that digit.
 __global__ void __launch_bounds__(256) ka_wave_sort_scatter_kernel(const KaWaveSort p, const int32_t* __restrict__ off,
                                                                    int32_t* __restrict__ out) {
-    __shared__ int base[KA_WAVE_SORT_DIGITS];
-    __shared__ int wcnt[8][KA_WAVE_SORT_DIGITS];
+    __shared__ int base[KA_RADIX_DIGITS];
+    __shared__ int wcnt[8][KA_RADIX_DIGITS];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     base[threadIdx.x] = off[threadIdx.x * p.ntiles + blockIdx.x];
     const uint32_t n = p.in ? (uint32_t)*p.n_ptr : p.Q;
