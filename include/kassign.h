@@ -333,9 +333,21 @@ typedef struct ka_wave_summary {
  *   wave[g] = max over its receivers b of (open[b] if load[b] == 0 or load[b] + w <= B, else open[b] + 1), and then every
  *   receiver b with wave[g] > open[b] gets open[b] = wave[g], load[b] = w, every other receiver load[b] += w.
  * So the waves are 1..W, none empty (W = 0 when no row changed); in every wave every broker receives at most B, unless a single
- * row heavier than B is its only incoming row of nonzero weight there; with B >= the sum of the weights everything is in wave 1. A broker's waves
- * only move forward (two words of state per broker): this is a greedy rule, not an optimal packing — a later row never goes
- * back to fill an earlier wave.
+ * row heavier than B is its only incoming row of nonzero weight there; with B >= the sum of the weights everything is in wave 1. Under
+ * this rule (KA_WAVE_GREEDY, a Context's default) a broker's waves only move forward (two words of state per broker): this is
+ * a greedy rule, not an optimal packing — a later row never goes back to fill an earlier wave.
+ * FIRST FIT (KA_WAVE_FIRST_FIT, chosen with ka_ctx_set_wave_rule) puts each row in the earliest wave where its receivers still
+ * have room. Every (broker, wave) pair starts with load[b][v] = 0; unchanged rows and changed rows without receivers are as
+ * above; any other row g takes wave[g] = the smallest v >= 1 in which every receiver b has load[b][v] == 0 or
+ * load[b][v] + w <= B, then load[b][v] += w for every receiver. A broker's waves no longer only move forward: a later row fills
+ * an earlier wave wherever every one of its receivers has room there. Every budget above holds exactly as under the greedy rule;
+ * no wave is empty (a row takes wave v > 1 only when wave v - 1 is refused by a bucket with nonzero load), so W <= the changed
+ * rows and every bound of the document calls holds unchanged; where no broker receives two moved rows the plan equals the
+ * greedy one. With M the rows with receivers and R_b the moved rows b receives, W <= Wb = min(M, 1 + max over those rows of
+ * the sum over their receivers of (R_b - 1)): a wave below a row's is refused only by a bucket holding an earlier row that
+ * shares a receiver, and b has at most R_b - 1 of them. The device keeps a load table of Wb x N int64 words: after the row
+ * errors, Wb x N x 8 > 2^30 bytes gives KA_ERR_LIMIT with a = Wb, before the plan runs. First fit adds 3 kernel launches and
+ * one synchronisation (the bound, read back to size the table), whatever Q and W are.
  * Checks, in this order, before anything is enqueued: st NULL: KA_ERR_BAD_ARG (nothing written); ctx NULL: KA_ERR_NO_DEVICE;
  * Q < 0, stride < 1, n_waves NULL, summary_cap < 0, summary NULL with summary_cap > 0, max_broker_in < 1, or rep_off not
  * non-decreasing from 0 (or a needed array NULL): KA_ERR_BAD_ARG; stride > 8 or Q >= 2^31: KA_ERR_LIMIT; a new_len outside
@@ -343,11 +355,24 @@ typedef struct ka_wave_summary {
  * KA_ERR_LIMIT. On the device, the lowest failing row wins: a new list naming a broker twice, or a receiver the table lacks,
  * gives KA_ERR_BAD_ARG with a = the row and b = the broker id at the first such position of its list. On any error *n_waves = 0
  * and wave / summary are unspecified. Q == 0: KA_OK, W = 0. Duplicate or unknown ids in a current list need no special case.
- * Synchronous; adds a fixed number of kernel launches, whatever Q and W are. Does not read or change the Context counters,
- * parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
+ * Synchronous; adds a fixed number of kernel launches, whatever Q and W are. Follows the Context's wave rule
+ * (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the
+ * last order / stage plans and timings. */
 int32_t ka_plan_waves(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                       const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
                       int32_t* wave, int32_t* n_waves, ka_wave_summary* summary, int32_t summary_cap, ka_status* st);
+
+/* The wave rule every plan call of this Context follows: ka_plan_waves, ka_plan_waves_send and their _json, _json_parts and
+ * _json_parts_rollback forms. Their checks, error codes and outputs keep their contracts under either rule; only wave[] (and
+ * so W, the summaries and the documents) changes. Configuration like ka_ctx_set_timing: ka_ctx_reset leaves it alone. */
+enum {
+    KA_WAVE_GREEDY = 0,      /* the default: a broker's waves only move forward (ka_plan_waves, ka_plan_waves_send) */
+    KA_WAVE_FIRST_FIT = 1    /* each row in the earliest wave where its receivers and its sender still have room */
+};
+/* KA_OK; any other rule: KA_ERR_BAD_ARG (the rule stays); ctx NULL: KA_ERR_NO_DEVICE. */
+int32_t ka_ctx_set_wave_rule(ka_ctx* ctx, int32_t rule);
+/* The Context's wave rule; ctx NULL: KA_ERR_NO_DEVICE. */
+int32_t ka_ctx_wave_rule(ka_ctx* ctx);
 
 /* ka_plan_waves + the documents it plans, built on the device: one reassignment JSON per wave, what an operator feeds
  * kafka-reassign-partitions one after the other. Only the text, the waves and the summaries cross PCIe.
@@ -374,7 +399,7 @@ int32_t ka_plan_waves(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int3
  * ka_plan_waves; a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX). On any error *n_waves = 0 and
  * nothing else is specified.
  * Synchronous. The kernel launches it adds depend only on the bit length of W (one stable radix pass over the waves per 8
- * bits), not on Q or T. Does not read or change the Context counters, parked counters, topic_base, the staged block, or the
+ * bits), not on Q or T. Follows the Context's wave rule (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the
  * last order / stage plans and timings. */
 int32_t ka_plan_waves_json(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                            const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
@@ -411,7 +436,12 @@ typedef struct ka_wave_send_summary {
  * So in every wave every broker sends at most C, unless a single row with w x r > C is its only outgoing row of nonzero weight
  * there; every receive bound of ka_plan_waves still holds; the waves are still 1..W and none is empty (every wave value is some
  * broker's open or open + 1), so doc_off and the json_cap bound of ka_plan_waves_json hold unchanged. Like a receiver, a
- * leader's waves only move forward: a row never goes to an earlier wave than its leader's open one. With C >= 8 x (sum of the
+ * leader's waves only move forward under the greedy rule: a row never goes to an earlier wave than its leader's open one.
+ * Under KA_WAVE_FIRST_FIT the sender is one more bucket per wave: wave[g] = the smallest v >= 1 in which every receiver fits as
+ * in ka_plan_waves and its sender s has sload[s][v] == 0 or sload[s][v] + a <= C; then sload[s][v] += a. Every bound above
+ * holds; where no broker receives two moved rows and no sender sends two, the plan equals the greedy one. Wb adds
+ * (S_s - 1) to each row's sum, S_s the moved rows s sends, and the load table is Wb x (N + n_send) words: Wb x (N + n_send) x
+ * 8 > 2^30 gives KA_ERR_LIMIT with a = Wb. With C >= 8 x (sum of the
  * weights) no leader ever opens a wave, so a row's wave is the larger of ka_plan_waves's receiver terms and its leader's open
  * wave; where no leader has two moved rows, wave, W, summary and every document are exactly those of ka_plan_waves(_json).
  * Checks: everything ka_plan_waves checks, in its order, with its codes and operands; then max_broker_out < 1, n_send < 0,
@@ -419,8 +449,8 @@ typedef struct ka_wave_send_summary {
  * n_send > 65535: KA_ERR_LIMIT with a = n_send. On the device, the lowest failing row wins, over ka_plan_waves's row errors and
  * this one together: a row with receivers whose sender the send table lacks gives KA_ERR_BAD_ARG with a = the row and b = the
  * sender's id; within a row, the new-list errors come first. On any error *n_waves = 0 and nothing else is specified.
- * Synchronous; 9 kernel launches (ka_plan_waves's 7 and 2 over the sender buckets), whatever Q, W and n_send are. Does not read
- * or change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
+ * Synchronous; 9 kernel launches (ka_plan_waves's 7 and 2 over the sender buckets), whatever Q, W and n_send are, and the 3 of
+ * first fit. Follows the Context's wave rule; does not read or change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
 int32_t ka_plan_waves_send(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                            const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
                            int32_t n_send, const int32_t* send_id, int64_t max_broker_out,
@@ -433,7 +463,7 @@ int32_t ka_plan_waves_send(ka_ctx* ctx, int64_t Q, const int64_t* rep_off, const
  * Every wave is non-empty, so doc_off[Q+1] and the json_cap bound of ka_plan_waves_json hold unchanged.
  * Checks: everything ka_plan_waves_json checks, in its order; then the sender checks of ka_plan_waves_send. On the device the
  * row errors of ka_plan_waves_send come first; a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX).
- * Synchronous; the 9 launches of ka_plan_waves_send, then, when W > 0, 3 per 8 bits of W and 3 more. */
+ * Follows the Context's wave rule (ka_ctx_set_wave_rule). Synchronous; the launches of ka_plan_waves_send, then, when W > 0, 3 per 8 bits of W and 3 more. */
 int32_t ka_plan_waves_send_json(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                 const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                                 const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
@@ -471,7 +501,7 @@ int32_t ka_plan_waves_send_json(ka_ctx* ctx, int32_t T, const int64_t* part_off,
  * *n_waves = *n_docs = 0 (when given) and nothing else is specified. W == 0 gives D = 0 and doc_off[0] = 0.
  * Synchronous; two synchronisations. The launches of ka_plan_waves_json, then, when W > 0, 4 more, and 2K - 1 more when the
  * widest wave has m >= 2 rows, K = the bit length of m - 1 (a pointer-doubling level per bit): they depend only on the bit
- * lengths of W and of m. Does not read or change the Context counters, parked counters, topic_base, the staged block, or the
+ * lengths of W and of m. Follows the Context's wave rule (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the
  * last order / stage plans and timings. */
 int32_t ka_plan_waves_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                  const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
@@ -486,7 +516,7 @@ int32_t ka_plan_waves_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off
  *   max_doc_bytes .. n_docs   exactly as ka_plan_waves_json_parts takes and writes them
  *   wave .. summary_cap   exactly as ka_plan_waves_send_json writes them
  * Checks: everything ka_plan_waves_send_json checks, in its order; then those ka_plan_waves_json_parts adds, in its order. The
- * launches of ka_plan_waves_send_json, and those ka_plan_waves_json_parts adds. */
+ * launches of ka_plan_waves_send_json, and those ka_plan_waves_json_parts adds. Follows the Context's wave rule. */
 int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                       const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                                       const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
@@ -526,8 +556,8 @@ int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* par
  * KA_ERR_LIMIT, a = min(json_cap, INT_MAX); a rollback text above back_cap: KA_ERR_LIMIT, a = min(back_cap, INT_MAX). On any
  * error *n_waves = *n_docs = 0 (when given). W == 0 gives D = 0 and back_off[0] = 0.
  * Synchronous. The launches of ka_plan_waves_json_parts on the same inputs, and, when W > 0, 3 more (the rollback text's
- * length, scan and write passes; the part passes carry the rollback side without a launch of their own). Does not read or
- * change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
+ * length, scan and write passes; the part passes carry the rollback side without a launch of their own). Follows the
+ * Context's wave rule (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
 int32_t ka_plan_waves_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                           const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
                                           const int32_t* new_broker, const int64_t* part_weight, int64_t max_broker_in,
@@ -542,7 +572,8 @@ int32_t ka_plan_waves_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t*
  *   back .. back_off   exactly as ka_plan_waves_json_parts_rollback takes and writes them
  *   wave .. summary_cap   exactly as ka_plan_waves_send_json_parts writes them
  * Checks: everything ka_plan_waves_send_json_parts checks, in its order; then those ka_plan_waves_json_parts_rollback adds, in
- * its order. The launches of ka_plan_waves_send_json_parts, and the 3 ka_plan_waves_json_parts_rollback adds. */
+ * its order. The launches of ka_plan_waves_send_json_parts, and the 3 ka_plan_waves_json_parts_rollback adds. Follows the
+ * Context's wave rule. */
 int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                                const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                                                const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,

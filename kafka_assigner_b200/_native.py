@@ -36,6 +36,7 @@ class KaBrokerUsage(ctypes.Structure):
 KA_OK = 0
 KA_ERR_RF_MISMATCH, KA_ERR_RF_NOT_POSITIVE, KA_ERR_RF_GT_BROKERS, KA_ERR_UNASSIGNABLE, KA_ERR_HASH_INDEX = 1, 2, 3, 4, 5
 KA_ERR_BAD_ARG, KA_ERR_CUDA, KA_ERR_NO_DEVICE, KA_ERR_LIMIT = -1, -2, -3, -4
+KA_WAVE_GREEDY, KA_WAVE_FIRST_FIT = 0, 1
 
 # every symbol include/kassign.h declares: (restype, argtypes)
 _vp, _i32, _i64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64
@@ -92,6 +93,8 @@ SYMBOLS = {
     "ka_ctx_export_counters_device": (_i32, [_vp, _vp, _vp]),
     "ka_ctx_import_counters_device": (_i32, [_vp, _vp, _vp]),
     "ka_ctx_set_timing": (_i32, [_vp, _i32]),
+    "ka_ctx_set_wave_rule": (_i32, [_vp, _i32]),
+    "ka_ctx_wave_rule": (_i32, [_vp]),
     "ka_ctx_last_timing": (_i32, [_vp, _vp]),
     "ka_ctx_launch_count": (_i64, [_vp]),
     "ka_ctx_last_order_plan": (_i32, [_vp, _vp]),

@@ -211,6 +211,23 @@ class Solver:
     def set_timing(self, on=True):
         self._L.ka_ctx_set_timing(self._h, 1 if on else 0)
 
+    WAVE_RULES = {"greedy": _native.KA_WAVE_GREEDY, "first_fit": _native.KA_WAVE_FIRST_FIT}
+
+    def set_wave_rule(self, rule):
+        """The wave rule of every plan_waves / plan_waves_json / plan_wave_parts_json / plan_wave_parts_rollback_json call of this
+        Solver (ka_ctx_set_wave_rule): "greedy" (the default: a broker's waves only move forward) or "first_fit" (each row in the
+        earliest wave where its receivers and its leader still have room, which often needs fewer waves). reset() keeps it."""
+        if rule not in self.WAVE_RULES:
+            raise ValueError("wave rule must be one of %s, not %r" % (sorted(self.WAVE_RULES), rule))
+        _check(self._L.ka_ctx_set_wave_rule(self._h, self.WAVE_RULES[rule]), "ka_ctx_set_wave_rule")
+
+    @property
+    def wave_rule(self):
+        """The wave rule set_wave_rule chose: "greedy" or "first_fit"."""
+        code = self._L.ka_ctx_wave_rule(self._h)
+        _check(min(code, 0), "ka_ctx_wave_rule")
+        return {v: k for k, v in self.WAVE_RULES.items()}[code]
+
     def last_timing(self):
         ms = np.zeros(8, dtype=np.float32)
         self._L.ka_ctx_last_timing(self._h, _ptr(ms))
@@ -512,7 +529,8 @@ class Solver:
         cur_broker[rep_off[g] .. rep_off[g + 1]), cut into waves in which no broker of this Solver's table receives more than
         max_broker_in (weight: [Q] int64 per row, None = 1 per row). Returns (wave [Q] int32, 0 for an unchanged row; summary, a
         numpy structured array [W] with the fields of ka_wave_summary; KaStatus). On an error wave and summary are empty. A plan
-        of more than min(Q, WAVE_SUMMARY_CAP) waves takes a second call for the rest of the summaries.
+        of more than min(Q, WAVE_SUMMARY_CAP) waves takes a second call for the rest of the summaries. The waves follow this
+        Solver's wave rule (set_wave_rule), as do those of every wave document call.
         max_broker_out: ka_plan_waves_send instead, which also caps what each row's leader (the first broker of its current
         list) sends per wave; send_brokers (required then: the ascending send table, e.g. every broker of the cluster before an
         exclusion) holds every such leader. The summary then has the fields of WAVE_SEND_SUMMARY_DTYPE."""

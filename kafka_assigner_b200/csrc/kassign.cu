@@ -156,6 +156,10 @@ struct ka_ctx {
     // scratch of the sender budget (ka_plan_waves_send and its JSON form): the send table, the sender bucket log and the sender
     // summaries (the per-sender words share d_wv_state)
     DevBuf d_wv_send, d_wv_slog, d_wv_ssum;
+    // the wave rule of every plan call (ka_ctx_set_wave_rule) and, under KA_WAVE_FIRST_FIT, the load table [N + ns][Wb] (the
+    // counts and the chain's per-row words share d_wv_state)
+    int32_t wave_rule = KA_WAVE_GREEDY;
+    DevBuf d_wv_fit;
     // scratch of ka_plan_waves_json, beside the plan's and the JSON passes' (d_part_off, d_part_id, d_names, d_name_off, d_json,
     // d_json_rowlen, d_json_blocksum as 64-bit offsets): the grouped rows (two arrays of Q), the radix passes' (digit, tile)
     // counts and offsets, and the text total followed by doc_off [W + 1] (with a size limit: the total, D, then doc_off [D + 1])
@@ -1487,6 +1491,15 @@ int32_t ka_ctx_set_timing(ka_ctx* c, int32_t enabled) {
     return KA_OK;
 }
 
+int32_t ka_ctx_set_wave_rule(ka_ctx* c, int32_t rule) {
+    if (!c) return KA_ERR_NO_DEVICE;
+    if (rule != KA_WAVE_GREEDY && rule != KA_WAVE_FIRST_FIT) return KA_ERR_BAD_ARG;
+    c->wave_rule = rule;
+    return KA_OK;
+}
+
+int32_t ka_ctx_wave_rule(ka_ctx* c) { return c ? c->wave_rule : KA_ERR_NO_DEVICE; }
+
 int32_t ka_ctx_last_timing(ka_ctx* c, float* ms) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!ms) return KA_ERR_BAD_ARG;
@@ -2541,8 +2554,51 @@ static int upload_wave_rows(ka_ctx* c, int64_t Q, int64_t R, const int64_t* rep_
     return KA_OK;
 }
 
+// The most bytes the load table of a first-fit plan may take: Wb x (N + n_send) x 8 (kassign_waves.cuh).
+constexpr size_t KA_WAVE_FIT_MAX_BYTES = size_t(1) << 30;
+
+// The first-fit chain of wave_plan_device (KA_WAVE_FIRST_FIT), after its rows / scan / compact kernels: the counts and the
+// bound Wb, awaited; unless the rows pass failed a row (left for the caller to report), KA_ERR_LIMIT with a = Wb when the load
+// table exceeds KA_WAVE_FIT_MAX_BYTES, else the zeroed table, the chain and the bucket logs (the meta words' nlog / nslog).
+static int wave_fit_chain(ka_ctx* c, cudaStream_t s, unsigned nblk, int N, int ns, int64_t B, bool gstate, bool send,
+                          const KaWaveRec* d_rec, const int32_t* d_off, int32_t* d_wave, KaWaveBucket* d_log, KaWaveMeta* d_meta,
+                          ka_status* st) {
+    const size_t rows = (size_t)(N + ns);
+    int* d_cnt = c->d_wv_state.as<int>();   // R_b, S_s; then, with gstate, the chain's claim and hint words
+    if (cudaMemsetAsync(d_cnt, 0, rows * 4, s)) return set_status(st, KA_ERR_CUDA);
+    const auto count = send ? ka_wave_fit_count_kernel<true> : ka_wave_fit_count_kernel<false>;
+    const auto bound = send ? ka_wave_fit_bound_kernel<true> : ka_wave_fit_bound_kernel<false>;
+    count<<<nblk, 256, 0, s>>>(d_rec, d_off, (int)nblk, N, d_cnt, d_meta);
+    bound<<<nblk, 256, 0, s>>>(d_rec, d_off, (int)nblk, N, d_cnt, d_meta);
+    c->launches += 2;
+    KaWaveFitMeta fm;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&fm, d_meta, sizeof(fm), cudaMemcpyDeviceToHost, s) ||
+        cudaStreamSynchronize(s))
+        return set_status(st, KA_ERR_CUDA);
+    if (fm.sm.m.err_row != 0xFFFFFFFFu) return KA_OK;
+    const int Wb = fm.bound;
+    const size_t bytes = (size_t)Wb * rows * 8;
+    if (bytes > KA_WAVE_FIT_MAX_BYTES) return set_status(st, KA_ERR_LIMIT, -1, -1, Wb);
+    if (c->d_wv_fit.reserve(std::max<size_t>(bytes, 16)) || cudaMemsetAsync(c->d_wv_fit.p, 0, bytes, s)) return set_status(st, KA_ERR_CUDA);
+    long long* table = c->d_wv_fit.as<long long>();
+    unsigned* claim = gstate ? c->d_wv_state.as<unsigned>() : nullptr;
+    int* hint = gstate ? reinterpret_cast<int*>(claim + rows) : nullptr;
+    const size_t smem = gstate ? 0 : rows * KA_WAVE_FIT_ROW_BYTES;
+    const auto chain = gstate ? (send ? ka_wave_fit_chain_kernel<true, true> : ka_wave_fit_chain_kernel<true, false>)
+                              : (send ? ka_wave_fit_chain_kernel<false, true> : ka_wave_fit_chain_kernel<false, false>);
+    if (!gstate && allow_smem(chain, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, B, Wb, d_wave, table, claim, hint, d_meta);
+    const size_t n = (size_t)Wb * rows;
+    const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
+    const auto log = send ? ka_wave_fit_log_kernel<true> : ka_wave_fit_log_kernel<false>;
+    log<<<blocks, 256, 0, s>>>(table, Wb, N, n, d_log, d_meta);
+    c->launches += 2;
+    return KA_OK;
+}
+
 // The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the rows up (upload_wave_rows), the
-// rows / scan / compact / chain kernels, the meta words back, then the sum and the two peak kernels (enqueued, not awaited).
+// rows / scan / compact / chain kernels under the ctx's wave rule (KA_WAVE_FIRST_FIT: wave_fit_chain), the meta words back,
+// then the sum and the two peak kernels (enqueued, not awaited).
 // Leaves every row's wave in d_wv_wave, its receivers in d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids
 // still N - index) in d_wv_sum. A sender part sd (null: none) adds the sender rule and its summaries (ids still n - index) in
 // d_wv_ssum.
@@ -2553,30 +2609,33 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     const int N = c->br.N;
     const int ns = sd ? sd->n : 0;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
+    const bool fit = c->wave_rule == KA_WAVE_FIRST_FIT;
+    const size_t row_bytes = fit ? KA_WAVE_FIT_ROW_BYTES : KA_WAVE_BROKER_BYTES;
     // the chain's per-broker and per-sender words in global memory
-    const bool gstate = (size_t)(N + ns) * KA_WAVE_BROKER_BYTES > KA_SMEM_BUDGET;
+    const bool gstate = (size_t)(N + ns) * row_bytes > KA_SMEM_BUDGET;
     const size_t q = (size_t)Q;
     if (upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, nullptr) != KA_OK ||
         c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
         c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
-        c->d_wv_state.reserve(gstate ? (size_t)(N + ns) * KA_WAVE_BROKER_BYTES : 16) ||
-        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveSendMeta)))
+        c->d_wv_state.reserve(gstate || fit ? (size_t)(N + ns) * row_bytes : 16) ||
+        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveFitMeta)))
         return set_status(st, KA_ERR_CUDA);
     // a sender bucket holds at least one moved row: at most Q of them
     if (sd && (c->d_wv_send.reserve((size_t)std::max(ns, 1) * 4) || c->d_wv_slog.reserve(q * sizeof(KaWaveBucket)) ||
                (ns > 0 && cudaMemcpyAsync(c->d_wv_send.p, sd->id, (size_t)ns * 4, cudaMemcpyHostToDevice, s))))
         return set_status(st, KA_ERR_CUDA);
-    KaWaveSendMeta meta0{{0xFFFFFFFFu, 0, 0, 0}, 0, {}};   // the sender part only read with sd
-    KaWaveSend& ks = meta0.snd;   // global words laid out as in shared memory: load, open, claim [N], then the senders' [ns]
-    long long* load = gstate ? c->d_wv_state.as<long long>() : nullptr;
-    int* open = gstate ? reinterpret_cast<int*>(load + N) : nullptr;
-    unsigned* claim = gstate ? reinterpret_cast<unsigned*>(open + N) : nullptr;
+    KaWaveFitMeta meta0{{{0xFFFFFFFFu, 0, 0, 0}, 0, {}}, 0};   // the sender part only read with sd, the bound only by first fit
+    KaWaveSend& ks = meta0.sm.snd;   // global words laid out as in shared memory: load, open, claim [N], then the senders' [ns]
+    const bool gwords = gstate && !fit;   // the greedy chain's
+    long long* load = gwords ? c->d_wv_state.as<long long>() : nullptr;
+    int* open = gwords ? reinterpret_cast<int*>(load + N) : nullptr;
+    unsigned* claim = gwords ? reinterpret_cast<unsigned*>(open + N) : nullptr;
     if (sd) {
         ks.id = c->d_wv_send.as<int32_t>();
         ks.n = ns;
         ks.C = sd->C;
         ks.log = c->d_wv_slog.as<KaWaveBucket>();
-        if (gstate) {
+        if (gwords) {
             ks.load = reinterpret_cast<long long*>(claim + N);
             ks.open = reinterpret_cast<int*>(ks.load + ns);
             ks.claim = reinterpret_cast<unsigned*>(ks.open + ns);
@@ -2596,7 +2655,11 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
                               c->d_out.as<int32_t>(), d_w, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_wave, d_cnt, d_meta);
     ka_level_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, (int)nblk, d_off);
     ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_off, d_rec);
-    if (gstate) {
+    c->launches += 3;   // rows, scan, compact
+    if (fit) {
+        int rc = wave_fit_chain(c, s, nblk, N, ns, max_broker_in, gstate, sd != nullptr, d_rec, d_off, d_wave, d_log, d_meta, st);
+        if (rc != KA_OK) return rc;
+    } else if (gstate) {
         const auto chain = sd ? ka_wave_chain_kernel<true, true> : ka_wave_chain_kernel<true, false>;
         chain<<<1, KA_WAVE_THREADS, 0, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, load, open, claim, d_log, d_meta);
     } else {
@@ -2606,7 +2669,7 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
         chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, nullptr, nullptr, nullptr, d_log,
                                                d_meta);
     }
-    c->launches += 4;
+    if (!fit) c->launches += 1;   // the greedy chain
     KaWaveSendMeta back;
     const KaWaveMeta& meta = back.m;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&back, d_meta, sizeof(back), cudaMemcpyDeviceToHost, s) ||

@@ -432,3 +432,213 @@ __global__ void __launch_bounds__(256) ka_wave_peak_kernel(const KaWaveBucket* _
         }
     }
 }
+
+// ---- first fit (KA_WAVE_FIRST_FIT, include/kassign.h) --------------------------------------------------------------------------
+// A row with receivers takes the SMALLEST wave v >= 1 in which every receiver's bucket (b, v) is empty or takes w within B, and
+// (SEND) its sender's bucket takes a = w x receivers within C. A broker's waves no longer only move forward, so its state is a
+// row of loads, one per wave: the table [N + ns][Wb] of int64, the senders' rows after the brokers' (sender x is row N + x).
+// Wb bounds W: a wave below a row's is refused only by a bucket with nonzero load, which holds an earlier row sharing a receiver
+// or the sender, so with R_b / S_s the moved rows b receives / s sends, W <= Wb = min(M, 1 + max over rows of
+// sum over its receivers (R_b - 1) + (S_s - 1)).
+//
+//   ka_wave_fit_count_kernel  R_b and S_s over the packed records (after the compact pass)
+//   ka_wave_fit_bound_kernel  Wb, to the meta words the host reads before it sizes the table
+//   ka_wave_fit_chain_kernel  ONE CTA: the rows pass's claim rounds, with the first-fit decision
+//   ka_wave_fit_log_kernel    every nonzero bucket of the table into the bucket logs, for the peak passes
+//
+// The chain keeps a hint per row of the table: every wave below it has load >= the budget, so it refuses any row of weight >= 1.
+// A row of weight >= 1 starts at the largest hint among its receivers and sender and walks up; a row of weight 0 starts at wave 1.
+
+// Bytes of shared memory the first-fit chain keeps per table row (claim, hint).
+#define KA_WAVE_FIT_ROW_BYTES 8
+
+// The meta words of a first-fit plan: the others', then Wb (atomicMax, init 0).
+struct KaWaveFitMeta {
+    KaWaveSendMeta sm;
+    int bound;
+};
+__device__ __forceinline__ KaWaveFitMeta* ka_wave_fit_meta(KaWaveMeta* meta) { return reinterpret_cast<KaWaveFitMeta*>(meta); }
+
+// The sender's row of the table (N + its send-table index), or -1 for a record without one or a plan without a sender part.
+template <bool SEND>
+__device__ __forceinline__ int ka_wave_fit_sender(const KaWaveRec& r, int N) {
+    if constexpr (SEND) {
+        const uint32_t sx = (uint32_t)r.n >> 16;
+        return sx != KA_WAVE_NO_SENDER ? N + (int)sx : -1;
+    }
+    return -1;
+}
+
+// Same grid as the rows pass: cnt[N + ns] (zeroed) gets R_b, then S_s at N + s. Does nothing when the rows pass failed a row.
+template <bool SEND>
+__global__ void __launch_bounds__(256) ka_wave_fit_count_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off, int nblk,
+                                                                int N, int* __restrict__ cnt, KaWaveMeta* __restrict__ meta) {
+    if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= off[nblk]) return;
+    const KaWaveRec r = rec[i];
+    for (int j = 0; j < ka_wave_nrcv<SEND>(r); ++j) atomicAdd(cnt + ka_wave_rcv(r, j), 1);
+    const int s = ka_wave_fit_sender<SEND>(r, N);
+    if (s >= 0) atomicAdd(cnt + s, 1);
+}
+
+// Same grid: ka_wave_fit_meta(meta)->bound = Wb over the counts of ka_wave_fit_count_kernel.
+template <bool SEND>
+__global__ void __launch_bounds__(256) ka_wave_fit_bound_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off, int nblk,
+                                                                int N, const int* __restrict__ cnt, KaWaveMeta* __restrict__ meta) {
+    if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;
+    const int M = off[nblk];
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned v = 0;
+    if (i < M) {
+        const KaWaveRec r = rec[i];
+        long long x = 0;   // up to 8 x (M - 1) + M - 1: beyond int32 for large M
+        for (int j = 0; j < ka_wave_nrcv<SEND>(r); ++j) x += cnt[ka_wave_rcv(r, j)] - 1;
+        const int s = ka_wave_fit_sender<SEND>(r, N);
+        if (s >= 0) x += cnt[s] - 1;
+        v = (unsigned)(1 + min(x, (long long)M - 1));
+    }
+    v = __reduce_max_sync(KA_FULL, v);
+    if ((threadIdx.x & 31) == 0 && v) atomicMax(&ka_wave_fit_meta(meta)->bound, (int)v);
+}
+
+// ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B, the zeroed table [N + ns][Wb].
+// Writes wave[row] of every record and meta->waves. With GSTATE the per-row words are gclaim / ghint [N + ns], else shared
+// memory. SEND: ns, C and the senders' rows as ka_wave_send_meta(meta) gives them. Does nothing when the rows pass failed a row.
+template <bool GSTATE, bool SEND>
+__global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_fit_chain_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off,
+                                                                               int nblk, int N, long long B, int Wb, int32_t* __restrict__ wave,
+                                                                               long long* __restrict__ table, unsigned* gclaim, int* ghint,
+                                                                               KaWaveMeta* __restrict__ meta) {
+    extern __shared__ __align__(16) unsigned char ka_wave_smem[];
+    __shared__ int wmax;
+    if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;   // CTA-uniform
+    int rows = N;
+    long long C = 0;
+    if constexpr (SEND) {
+        rows += ka_wave_send_meta(meta)->snd.n;
+        C = ka_wave_send_meta(meta)->snd.C;
+    }
+    unsigned* claim = gclaim;
+    int* hint = ghint;
+    if constexpr (!GSTATE) {
+        claim = reinterpret_cast<unsigned*>(ka_wave_smem);
+        hint = reinterpret_cast<int*>(claim + rows);
+    }
+    const int tid = threadIdx.x;
+    for (int i = tid; i < rows; i += KA_WAVE_THREADS) {
+        ka_wave_st<GSTATE>(claim + i, 0u);
+        ka_wave_st<GSTATE>(hint + i, 1);
+    }
+    if (tid == 0) wmax = 0;
+    __syncthreads();
+    const int M = off[nblk];
+    unsigned round = 0;
+    int my_max = 0;
+    for (int base = 0; base < M; base += KA_WAVE_CHUNK) {
+        KaWaveRec r[KA_WAVE_PER_THREAD];
+        unsigned pend = 0;
+#pragma unroll
+        for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
+            const int i = base + e * KA_WAVE_THREADS + tid;
+            if (i < M) {
+                r[e] = rec[i];
+                pend |= 1u << e;
+            } else {
+                r[e] = KaWaveRec{0, 0, 0, 0, 0};
+            }
+        }
+        for (;;) {
+            if (++round == KA_WAVE_MAX_ROUND) {   // the key's round field is full: clear the claims and count again
+                for (int i = tid; i < rows; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(claim + i, 0u);
+                __syncthreads();
+                round = 1;
+            }
+            unsigned key[KA_WAVE_PER_THREAD];
+#pragma unroll
+            for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
+                key[e] = round << KA_WAVE_SLOT_BITS | (unsigned)(KA_WAVE_CHUNK - 1 - (e * KA_WAVE_THREADS + tid));
+                if (!(pend >> e & 1u)) continue;
+                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
+                const int s = ka_wave_fit_sender<SEND>(r[e], N);
+                if (s >= 0) atomicMax(claim + s, key[e]);
+            }
+            __syncthreads();
+#pragma unroll
+            for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
+                if (!(pend >> e & 1u)) continue;
+                const int k = ka_wave_nrcv<SEND>(r[e]);
+                const int s = ka_wave_fit_sender<SEND>(r[e], N);
+                bool own = s < 0 || ka_wave_ld<GSTATE>(claim + s) == key[e];
+                for (int j = 0; j < k; ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
+                if (!own) continue;
+                const long long w = r[e].w, a = w * k;
+                int v = 1;
+                if (w > 0) {
+                    for (int j = 0; j < k; ++j) v = max(v, ka_wave_ld<GSTATE>(hint + ka_wave_rcv(r[e], j)));
+                    if (s >= 0) v = max(v, ka_wave_ld<GSTATE>(hint + s));
+                }
+                for (; v < Wb; ++v) {   // Wb itself always fits (the bound above)
+                    bool fit = true;
+                    for (int j = 0; j < k && fit; ++j) {
+                        const long long l = table[(size_t)ka_wave_rcv(r[e], j) * Wb + v - 1];
+                        fit = l == 0 || l + w <= B;
+                    }
+                    if (fit && s >= 0) {
+                        const long long l = table[(size_t)s * Wb + v - 1];
+                        fit = l == 0 || l + a <= C;
+                    }
+                    if (fit) break;
+                }
+                // add to every bucket, and move each row's hint past the waves that are now full
+                auto add = [&](int x, long long amount, long long cap) {
+                    long long* row = table + (size_t)x * Wb;
+                    row[v - 1] += amount;
+                    int h = ka_wave_ld<GSTATE>(hint + x);
+                    if (h != v) return;
+                    while (h < Wb && row[h - 1] >= cap) ++h;
+                    ka_wave_st<GSTATE>(hint + x, h);
+                };
+                for (int j = 0; j < k; ++j) add((int)ka_wave_rcv(r[e], j), w, B);
+                if (s >= 0) add(s, a, C);
+                wave[r[e].row] = v;
+                my_max = max(my_max, v);
+                pend &= ~(1u << e);
+            }
+            if (!__syncthreads_or(pend != 0)) break;
+        }
+    }
+    atomicMax(&wmax, my_max);
+    __syncthreads();
+    if (tid == 0) meta->waves = wmax;
+}
+
+// grid-stride over the table [N + ns][Wb]: every bucket with nonzero load to the bucket log (meta->nlog, zeroed) or, a sender's
+// row (SEND), to the sender log (its nslog, zeroed) with the send-table index. The peak passes read the logs in any order.
+template <bool SEND>
+__global__ void __launch_bounds__(256) ka_wave_fit_log_kernel(const long long* __restrict__ table, int Wb, int N, size_t n,
+                                                              KaWaveBucket* __restrict__ log, KaWaveMeta* __restrict__ meta) {
+    const int lane = threadIdx.x & 31;
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    for (size_t base = (size_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); base < n; base += stride) {   // warp-uniform
+        const size_t i = base + lane;
+        const long long l = i < n ? table[i] : 0;
+        const int x = (int)(i / (size_t)Wb);
+        const int v = (int)(i % (size_t)Wb) + 1;
+        const bool in = l > 0 && x < N;
+        const unsigned mi = __ballot_sync(KA_FULL, in);
+        unsigned at = 0;
+        if (lane == 0 && mi) at = atomicAdd(&meta->nlog, (unsigned)__popc(mi));
+        at = __shfl_sync(KA_FULL, at, 0) + __popc(mi & ka_lanemask_lt());
+        if (in) log[at] = KaWaveBucket{v, x, l};
+        if constexpr (SEND) {
+            KaWaveSendMeta* sm = ka_wave_send_meta(meta);
+            const bool out = l > 0 && x >= N;
+            const unsigned mo = __ballot_sync(KA_FULL, out);
+            unsigned so = 0;
+            if (lane == 0 && mo) so = atomicAdd(&sm->nslog, (unsigned)__popc(mo));
+            so = __shfl_sync(KA_FULL, so, 0) + __popc(mo & ka_lanemask_lt());
+            if (out) sm->snd.log[so] = KaWaveBucket{v, x - N, l};
+        }
+    }
+}

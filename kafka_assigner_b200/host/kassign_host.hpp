@@ -22,6 +22,7 @@
 //                                                          on their current lists), both sides under the limit
 //   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
 //                                                          receives more than a budget, one document per wave
+//   kassign::setWaveRule                              <->  the wave rule of those plans: greedy, or first fit
 //   kassign::brokerUsage                              <->  what every broker holds across a wave plan: its peak, the wave of
 //                                                          the peak and the first wave over its capacity
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
@@ -270,6 +271,15 @@ public:
                           perBroker ? brk[2].data() : nullptr, nullptr, nullptr, st.data());
         return memberScores(st, K, summary, perBroker ? brk : nullptr, fl.candOff, fl.ids);
     }
+
+    // The wave rule of every planWaves* call of this instance (ka_ctx_set_wave_rule): KA_WAVE_GREEDY (the default: a broker's
+    // waves only move forward) or KA_WAVE_FIRST_FIT (each partition in the earliest wave where its receivers and its leader still
+    // have room, often fewer waves). Any other value throws KassignError(KA_ERR_BAD_ARG).
+    void setWaveRule(int32_t rule) {
+        const int32_t rc = ka_ctx_set_wave_rule(ctx_, rule);
+        if (rc != KA_OK) throw KassignError(rc, "(wave rule " + std::to_string(rule) + ")");
+    }
+    int32_t waveRule() const { return ka_ctx_wave_rule(ctx_); }
 
     // A new assignment cut into waves (ka_plan_waves): consecutive documents in which no broker of this instance's table receives
     // more than maxBrokerIn (weighted). waves[v] holds the changed partitions of wave v + 1, topics in input order, each
