@@ -150,7 +150,7 @@ struct ka_ctx {
     // offsets [K+1]
     DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
     // scratch of ka_plan_waves (its rows: upload_wave_rows): the rows pass's per-row outputs and records, the packed records, the
-    // per-CTA counts and offsets, the chain's per-broker words when they leave shared memory, the bucket log, the summaries and
+    // per-CTA counts and offsets, the chain's per-row words when they leave shared memory, the bucket log, the summaries and
     // the meta words
     DevBuf d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state, d_wv_log, d_wv_sum, d_wv_meta;
     // scratch of the sender budget (ka_plan_waves_send and its JSON form): the send table, the sender bucket log and the sender
@@ -2559,35 +2559,33 @@ constexpr size_t KA_WAVE_FIT_MAX_BYTES = size_t(1) << 30;
 
 // The first-fit chain of wave_plan_device (KA_WAVE_FIRST_FIT), after its rows / scan / compact kernels: the counts and the
 // bound Wb, awaited; unless the rows pass failed a row (left for the caller to report), KA_ERR_LIMIT with a = Wb when the load
-// table exceeds KA_WAVE_FIT_MAX_BYTES, else the zeroed table, the chain and the bucket logs (the meta words' nlog / nslog).
-static int wave_fit_chain(ka_ctx* c, cudaStream_t s, unsigned nblk, int N, int ns, int64_t B, bool gstate, bool send,
-                          const KaWaveRec* d_rec, const int32_t* d_off, int32_t* d_wave, KaWaveBucket* d_log, KaWaveMeta* d_meta,
-                          ka_status* st) {
+// table exceeds KA_WAVE_FIT_MAX_BYTES, else the zeroed table, the chain (its per-row words at state, or when state is null in
+// smem bytes of shared memory) and the bucket logs (the meta words' nlog / nslog).
+static int wave_fit_chain(ka_ctx* c, cudaStream_t s, unsigned nblk, int N, int ns, int64_t B, bool send, unsigned char* state,
+                          size_t smem, const KaWaveRec* d_rec, const int32_t* d_off, int32_t* d_wave, KaWaveBucket* d_log,
+                          KaWaveMeta* d_meta, ka_status* st) {
     const size_t rows = (size_t)(N + ns);
-    int* d_cnt = c->d_wv_state.as<int>();   // R_b, S_s; then, with gstate, the chain's claim and hint words
+    int* d_cnt = c->d_wv_state.as<int>();   // R_b, S_s; then, with the state in global memory, the chain's claim and hint words
     if (cudaMemsetAsync(d_cnt, 0, rows * 4, s)) return set_status(st, KA_ERR_CUDA);
     const auto count = send ? ka_wave_fit_count_kernel<true> : ka_wave_fit_count_kernel<false>;
     const auto bound = send ? ka_wave_fit_bound_kernel<true> : ka_wave_fit_bound_kernel<false>;
     count<<<nblk, 256, 0, s>>>(d_rec, d_off, (int)nblk, N, d_cnt, d_meta);
     bound<<<nblk, 256, 0, s>>>(d_rec, d_off, (int)nblk, N, d_cnt, d_meta);
     c->launches += 2;
-    KaWaveFitMeta fm;
+    KaWaveMeta fm;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&fm, d_meta, sizeof(fm), cudaMemcpyDeviceToHost, s) ||
         cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
-    if (fm.sm.m.err_row != 0xFFFFFFFFu) return KA_OK;
+    if (fm.err_row != 0xFFFFFFFFu) return KA_OK;
     const int Wb = fm.bound;
     const size_t bytes = (size_t)Wb * rows * 8;
     if (bytes > KA_WAVE_FIT_MAX_BYTES) return set_status(st, KA_ERR_LIMIT, -1, -1, Wb);
     if (c->d_wv_fit.reserve(std::max<size_t>(bytes, 16)) || cudaMemsetAsync(c->d_wv_fit.p, 0, bytes, s)) return set_status(st, KA_ERR_CUDA);
     long long* table = c->d_wv_fit.as<long long>();
-    unsigned* claim = gstate ? c->d_wv_state.as<unsigned>() : nullptr;
-    int* hint = gstate ? reinterpret_cast<int*>(claim + rows) : nullptr;
-    const size_t smem = gstate ? 0 : rows * KA_WAVE_FIT_ROW_BYTES;
-    const auto chain = gstate ? (send ? ka_wave_fit_chain_kernel<true, true> : ka_wave_fit_chain_kernel<true, false>)
-                              : (send ? ka_wave_fit_chain_kernel<false, true> : ka_wave_fit_chain_kernel<false, false>);
-    if (!gstate && allow_smem(chain, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-    chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, B, Wb, d_wave, table, claim, hint, d_meta);
+    const auto chain = state ? (send ? ka_wave_fit_chain_kernel<true, true> : ka_wave_fit_chain_kernel<true, false>)
+                             : (send ? ka_wave_fit_chain_kernel<false, true> : ka_wave_fit_chain_kernel<false, false>);
+    if (!state && allow_smem(chain, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+    chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, (int)rows, B, Wb, d_wave, table, state, d_meta);
     const size_t n = (size_t)Wb * rows;
     const unsigned blocks = (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)c->sm_count * 8));
     const auto log = send ? ka_wave_fit_log_kernel<true> : ka_wave_fit_log_kernel<false>;
@@ -2610,37 +2608,24 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     const int ns = sd ? sd->n : 0;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
     const bool fit = c->wave_rule == KA_WAVE_FIRST_FIT;
-    const size_t row_bytes = fit ? KA_WAVE_FIT_ROW_BYTES : KA_WAVE_BROKER_BYTES;
-    // the chain's per-broker and per-sender words in global memory
-    const bool gstate = (size_t)(N + ns) * row_bytes > KA_SMEM_BUDGET;
+    // the chain's per-row words (the brokers', then the senders'): in shared memory while they fit, else in d_wv_state
+    const size_t state_bytes = (size_t)(N + ns) * (fit ? KA_WAVE_FIT_ROW_BYTES : KA_WAVE_ROW_BYTES);
+    const bool gstate = state_bytes > KA_SMEM_BUDGET;
     const size_t q = (size_t)Q;
     if (upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, nullptr) != KA_OK ||
         c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
         c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
-        c->d_wv_state.reserve(gstate || fit ? (size_t)(N + ns) * row_bytes : 16) ||
-        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveFitMeta)))
+        c->d_wv_state.reserve(gstate || fit ? state_bytes : 16) ||
+        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveMeta)))
         return set_status(st, KA_ERR_CUDA);
+    unsigned char* state = gstate ? c->d_wv_state.as<unsigned char>() : nullptr;
+    const size_t smem = gstate ? 0 : state_bytes;
     // a sender bucket holds at least one moved row: at most Q of them
     if (sd && (c->d_wv_send.reserve((size_t)std::max(ns, 1) * 4) || c->d_wv_slog.reserve(q * sizeof(KaWaveBucket)) ||
                (ns > 0 && cudaMemcpyAsync(c->d_wv_send.p, sd->id, (size_t)ns * 4, cudaMemcpyHostToDevice, s))))
         return set_status(st, KA_ERR_CUDA);
-    KaWaveFitMeta meta0{{{0xFFFFFFFFu, 0, 0, 0}, 0, {}}, 0};   // the sender part only read with sd, the bound only by first fit
-    KaWaveSend& ks = meta0.sm.snd;   // global words laid out as in shared memory: load, open, claim [N], then the senders' [ns]
-    const bool gwords = gstate && !fit;   // the greedy chain's
-    long long* load = gwords ? c->d_wv_state.as<long long>() : nullptr;
-    int* open = gwords ? reinterpret_cast<int*>(load + N) : nullptr;
-    unsigned* claim = gwords ? reinterpret_cast<unsigned*>(open + N) : nullptr;
-    if (sd) {
-        ks.id = c->d_wv_send.as<int32_t>();
-        ks.n = ns;
-        ks.C = sd->C;
-        ks.log = c->d_wv_slog.as<KaWaveBucket>();
-        if (gwords) {
-            ks.load = reinterpret_cast<long long*>(claim + N);
-            ks.open = reinterpret_cast<int*>(ks.load + ns);
-            ks.claim = reinterpret_cast<unsigned*>(ks.open + ns);
-        }
-    }
+    KaWaveMeta meta0{0xFFFFFFFFu, 0, 0, 0, 0, 0, {}};   // the sender part only read with sd
+    if (sd) meta0.snd = KaWaveSend{c->d_wv_send.as<int32_t>(), ns, sd->C, c->d_wv_slog.as<KaWaveBucket>()};
     const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
     int32_t* d_cnt = c->d_wv_cnt.as<int32_t>();
     int32_t* d_off = d_cnt + nblk;
@@ -2657,22 +2642,17 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_off, d_rec);
     c->launches += 3;   // rows, scan, compact
     if (fit) {
-        int rc = wave_fit_chain(c, s, nblk, N, ns, max_broker_in, gstate, sd != nullptr, d_rec, d_off, d_wave, d_log, d_meta, st);
+        int rc = wave_fit_chain(c, s, nblk, N, ns, max_broker_in, sd != nullptr, state, smem, d_rec, d_off, d_wave, d_log, d_meta, st);
         if (rc != KA_OK) return rc;
-    } else if (gstate) {
-        const auto chain = sd ? ka_wave_chain_kernel<true, true> : ka_wave_chain_kernel<true, false>;
-        chain<<<1, KA_WAVE_THREADS, 0, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, load, open, claim, d_log, d_meta);
     } else {
-        const size_t smem = (size_t)(N + ns) * KA_WAVE_BROKER_BYTES;
-        const auto chain = sd ? ka_wave_chain_kernel<false, true> : ka_wave_chain_kernel<false, false>;
-        if (allow_smem(chain, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
-        chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, max_broker_in, d_wave, nullptr, nullptr, nullptr, d_log,
-                                               d_meta);
+        const auto chain = gstate ? (sd ? ka_wave_chain_kernel<true, true> : ka_wave_chain_kernel<true, false>)
+                                  : (sd ? ka_wave_chain_kernel<false, true> : ka_wave_chain_kernel<false, false>);
+        if (!gstate && allow_smem(chain, smem) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+        chain<<<1, KA_WAVE_THREADS, smem, s>>>(d_rec, d_off, (int)nblk, N, N + ns, max_broker_in, d_wave, state, d_log, d_meta);
+        c->launches += 1;
     }
-    if (!fit) c->launches += 1;   // the greedy chain
-    KaWaveSendMeta back;
-    const KaWaveMeta& meta = back.m;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&back, d_meta, sizeof(back), cudaMemcpyDeviceToHost, s) ||
+    KaWaveMeta meta;
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, d_meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
         cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     if (meta.err_row != 0xFFFFFFFFu) {   // no refused position: with a sender part, the row's sender, which the send table lacks
@@ -2690,7 +2670,7 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     ka_wave_sum_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, d_wave, d_w, d_sum);
     c->launches += 1;
     enq_wave_peaks<KaWaveInPeak>(c, s, d_log, meta.nlog, N, d_sum);
-    if (sd) enq_wave_peaks<KaWaveOutPeak>(c, s, ks.log, back.nslog, ns, c->d_wv_ssum.as<ka_wave_send_summary>());
+    if (sd) enq_wave_peaks<KaWaveOutPeak>(c, s, c->d_wv_slog.as<KaWaveBucket>(), meta.nslog, ns, c->d_wv_ssum.as<ka_wave_send_summary>());
     return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
 }
 

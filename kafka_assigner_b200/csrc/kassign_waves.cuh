@@ -20,11 +20,13 @@
 // open / load alone. The earliest pending record always holds its claims, so every round decides at least one record; a record
 // decides in round 1 + (the latest round among the earlier records of its chunk that share a broker with it).
 //
-// The sender budget (SEND, ka_plan_waves_send): the first broker of a moved row's current list sends w x receivers; its index in the
-// send table rides in the record's n word, and the chain keeps a second set of per-broker words for the senders (open, load,
-// claim). A pending record claims its sender's words with the same key as its receivers' and decides only when it holds every
-// claim, so the earliest pending record still decides in every round. A record decides in the round after the latest earlier
-// record of its chunk that shares a receiver or its sender with it.
+// The sender budget (SEND, ka_plan_waves_send): the first broker of a moved row's current list sends w x receivers; its index x in
+// the send table rides in the record's n word, and the chain keeps its words (open, load, claim) as row N + x, after the N
+// brokers' rows. A pending record claims its sender's row with the same key as its receivers' and decides only when it holds
+// every claim, so the earliest pending record still decides in every round. A record decides in the round after the latest
+// earlier record of its chunk that shares a receiver or its sender with it.
+//
+// The claim rounds exist once (ka_wave_rounds); each rule's chain passes them its decision.
 //
 // Everything is integer, and every sum and extreme commutative: the plan does not depend on the order of the atomics.
 #pragma once
@@ -55,33 +57,25 @@ struct KaWaveBucket {
 
 #define KA_WAVE_NO_SENDER 0xFFFFu
 
-// The sender part of a plan (SEND): the send table id[n] (strictly ascending, n <= 65535), the budget C, the chain's
-// per-sender words when they leave shared memory (load / open / claim [n], else null) and the sender bucket log.
+// The sender part of a plan (SEND): the send table id[n] (strictly ascending, n <= 65535), the budget C and the sender bucket
+// log.
 struct KaWaveSend {
     const int32_t* id;
     int n;
     long long C;
-    long long* load;
-    int* open;
-    unsigned* claim;
     KaWaveBucket* log;
 };
 
+// The meta words of a plan, zeroed by the host but for err_row. Kernels without a sender part never read snd.
 struct KaWaveMeta {
     unsigned err_row;   // lowest failing row (unsigned atomicMin, init 0xFFFFFFFF)
     int changed;        // some row changed
     int waves;          // W of the chain (the largest wave of a moved row)
     unsigned nlog;      // buckets logged
-};
-
-// The meta words of a plan with a sender part: the SEND instances take the KaWaveMeta* of the others and reach the sender
-// part behind it (ka_wave_send_meta), so that the instances without a sender keep their parameters and their code.
-struct KaWaveSendMeta {
-    KaWaveMeta m;
     unsigned nslog;     // sender buckets logged
+    int bound;          // first fit: Wb (atomicMax)
     KaWaveSend snd;
 };
-__device__ __forceinline__ KaWaveSendMeta* ka_wave_send_meta(KaWaveMeta* meta) { return reinterpret_cast<KaWaveSendMeta*>(meta); }
 
 __device__ __forceinline__ uint32_t ka_wave_rcv(const KaWaveRec& r, int j) {
     return (uint32_t)((j < 4 ? r.lo >> (16 * j) : r.hi >> (16 * (j - 4))) & 0xFFFFu);
@@ -135,7 +129,7 @@ __global__ void __launch_bounds__(256) ka_wave_rows_kernel(const KaBrokers br, u
                 uint32_t sx = KA_WAVE_NO_SENDER;
                 if (m > 0) {   // the sender's index: a binary search of the send table
                     const int id = __ldg(cur + a);
-                    const KaWaveSend& snd = ka_wave_send_meta(meta)->snd;
+                    const KaWaveSend& snd = meta->snd;
                     const int32_t* sid = snd.id;
                     const int ns = snd.n;
                     int l = 0, h = ns;
@@ -176,8 +170,8 @@ __global__ void __launch_bounds__(256) ka_wave_compact_kernel(uint32_t Q, const 
     rec[pos] = tmp[g];
 }
 
-// The chain's per-broker words: shared memory while the table fits (GSTATE = false), else global memory read around L1 (the
-// claims are L2 atomics).
+// The chains' per-row words: shared memory while they fit (GSTATE = false), else global memory read around L1 (the claims are
+// L2 atomics).
 template <bool GSTATE, typename T>
 __device__ __forceinline__ T ka_wave_ld(const T* p) {
     if constexpr (GSTATE) return __ldcg(p);
@@ -189,8 +183,8 @@ __device__ __forceinline__ void ka_wave_st(T* p, T v) {
     else *p = v;
 }
 
-// Bytes of shared memory the chain keeps per broker (load, open, claim), and with SEND per sender too.
-#define KA_WAVE_BROKER_BYTES 16
+// Bytes the greedy chain keeps per row (load, open, claim): a broker, or with SEND a sender.
+#define KA_WAVE_ROW_BYTES 16
 
 // The receivers of a record (SEND: the n word also holds the sender).
 template <bool SEND>
@@ -199,70 +193,24 @@ __device__ __forceinline__ int ka_wave_nrcv(const KaWaveRec& r) {
     else return r.n;
 }
 
-// The chain's per-sender words (SEND): after the N broker words in shared memory, or where meta->snd points (GSTATE). Read
-// where they are used, so that the instances without a sender declare nothing more than the plan's own.
-struct KaWaveSendWords {
-    long long* load;
-    int* open;
-    unsigned* claim;
-};
-template <bool GSTATE>
-__device__ __forceinline__ KaWaveSendWords ka_wave_send_words(const KaWaveSendMeta* sm, unsigned* claim, int N) {
-    if constexpr (GSTATE) return KaWaveSendWords{sm->snd.load, sm->snd.open, sm->snd.claim};
-    long long* load = reinterpret_cast<long long*>(claim + N);   // 16 N bytes in: 8-byte aligned
-    int* open = reinterpret_cast<int*>(load + sm->snd.n);
-    return KaWaveSendWords{load, open, reinterpret_cast<unsigned*>(open + sm->snd.n)};
-}
-
-// A closed or still-open sender bucket to the sender log (SEND).
-__device__ __forceinline__ void ka_wave_send_put(KaWaveSendMeta* sm, int wv, uint32_t x, long long l) {
-    const unsigned s = atomicAdd(&sm->nslog, 1u);
-    sm->snd.log[s] = KaWaveBucket{wv, (int32_t)x, l};
-}
-
-// ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B. Writes wave[row] of every
-// record, the bucket log and meta->waves / nlog. With GSTATE the per-broker words are gload / gopen / gclaim [N]. SEND: also
-// the sender rule of ka_wave_send_meta(meta) (its budget C, its words by ka_wave_send_words), the sender buckets in its log
-// and their count in its nslog (zeroed by the host). Does nothing when the rows pass failed a row.
-template <bool GSTATE, bool SEND>
-__global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off,
-                                                                           int nblk, int N, long long B, int32_t* __restrict__ wave,
-                                                                           long long* gload, int* gopen, unsigned* gclaim,
-                                                                           KaWaveBucket* __restrict__ log, KaWaveMeta* __restrict__ meta) {
-    extern __shared__ __align__(16) unsigned char ka_wave_smem[];
-    __shared__ unsigned nlog;
-    __shared__ int wmax;
-    if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;   // CTA-uniform
-    long long* load = gload;
-    int* open = gopen;
-    unsigned* claim = gclaim;
-    if constexpr (!GSTATE) {
-        load = reinterpret_cast<long long*>(ka_wave_smem);
-        open = reinterpret_cast<int*>(load + N);
-        claim = reinterpret_cast<unsigned*>(open + N);
-    }
-    const int tid = threadIdx.x;
-    for (int i = tid; i < N; i += KA_WAVE_THREADS) {
-        ka_wave_st<GSTATE>(load + i, 0LL);
-        ka_wave_st<GSTATE>(open + i, 1);
-        ka_wave_st<GSTATE>(claim + i, 0u);
-    }
+// The sender's row (N + its send-table index), or -1 for a record without one or a plan without a sender part.
+template <bool SEND>
+__device__ __forceinline__ int ka_wave_sender(const KaWaveRec& r, int N) {
     if constexpr (SEND) {
-        KaWaveSendMeta* sm = ka_wave_send_meta(meta);
-        const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
-        for (int i = tid; i < sm->snd.n; i += KA_WAVE_THREADS) {
-            ka_wave_st<GSTATE>(sw.load + i, 0LL);
-            ka_wave_st<GSTATE>(sw.open + i, 1);
-            ka_wave_st<GSTATE>(sw.claim + i, 0u);
-        }
+        const uint32_t sx = (uint32_t)r.n >> 16;
+        return sx != KA_WAVE_NO_SENDER ? N + (int)sx : -1;
     }
-    if (tid == 0) { nlog = 0; wmax = 0; }
-    __syncthreads();
-    auto put = [&](int wv, uint32_t b, long long l) {
-        const unsigned s = atomicAdd(&nlog, 1u);
-        log[s] = KaWaveBucket{wv, (int32_t)b, l};
-    };
-    const int M = off[nblk];
+    return -1;
+}
+
+// The claim rounds of both chains, run by their ONE CTA of KA_WAVE_THREADS over the M records in rec, with claim[rows] zeroed
+// (rows = N + ns: the brokers, then the senders). A record that holds the claims of its k receivers and of its sender's row s
+// (-1: none) gets its wave from decide(r, k, s), which also makes the rule's updates. Writes wave[row] of every record and
+// returns the largest wave this thread decided.
+template <bool GSTATE, bool SEND, typename Decide>
+__device__ __forceinline__ int ka_wave_rounds(const KaWaveRec* __restrict__ rec, int M, int N, int rows, unsigned* claim,
+                                              int32_t* __restrict__ wave, Decide&& decide) {
+    const int tid = threadIdx.x;
     unsigned round = 0;
     int my_max = 0;
     for (int base = 0; base < M; base += KA_WAVE_CHUNK) {
@@ -279,13 +227,12 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
             }
         }
         for (;;) {
+            // N, opaque to the compiler: each round derives the records' sender rows again rather than holding them in
+            // registers across the rounds, where the SEND chains would spill
+            int n0 = N;
+            asm volatile("" : "+r"(n0));
             if (++round == KA_WAVE_MAX_ROUND) {   // the key's round field is full: clear the claims and count again
-                for (int i = tid; i < N; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(claim + i, 0u);
-                if constexpr (SEND) {
-                    KaWaveSendMeta* sm = ka_wave_send_meta(meta);
-                    const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
-                    for (int i = tid; i < sm->snd.n; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(sw.claim + i, 0u);
-                }
+                for (int i = tid; i < rows; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(claim + i, 0u);
                 __syncthreads();
                 round = 1;
             }
@@ -293,83 +240,93 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const
 #pragma unroll
             for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
                 key[e] = round << KA_WAVE_SLOT_BITS | (unsigned)(KA_WAVE_CHUNK - 1 - (e * KA_WAVE_THREADS + tid));
-                if (pend >> e & 1u)
-                    for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
-                if constexpr (SEND) {   // and its sender
-                    const uint32_t sx = (uint32_t)r[e].n >> 16;
-                    if ((pend >> e & 1u) && sx != KA_WAVE_NO_SENDER)
-                        atomicMax(ka_wave_send_words<GSTATE>(ka_wave_send_meta(meta), claim, N).claim + sx, key[e]);
-                }
+                if (!(pend >> e & 1u)) continue;
+                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
+                const int s = ka_wave_sender<SEND>(r[e], n0);
+                if (s >= 0) atomicMax(claim + s, key[e]);
             }
             __syncthreads();
 #pragma unroll
             for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
                 if (!(pend >> e & 1u)) continue;
-                bool own = true;
-                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
-                if constexpr (SEND) {
-                    const uint32_t sx = (uint32_t)r[e].n >> 16;
-                    if (sx != KA_WAVE_NO_SENDER)
-                        own &= ka_wave_ld<GSTATE>(ka_wave_send_words<GSTATE>(ka_wave_send_meta(meta), claim, N).claim + sx) == key[e];
-                }
+                const int k = ka_wave_nrcv<SEND>(r[e]);
+                const int s = ka_wave_sender<SEND>(r[e], n0);
+                bool own = s < 0 || ka_wave_ld<GSTATE>(claim + s) == key[e];
+                for (int j = 0; j < k; ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
                 if (!own) continue;
-                const long long w = r[e].w;
-                int wv = 0;
-                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) {
-                    const uint32_t b = ka_wave_rcv(r[e], j);
-                    const int o = ka_wave_ld<GSTATE>(open + b);
-                    const long long l = ka_wave_ld<GSTATE>(load + b);
-                    wv = max(wv, (l == 0 || l + w <= B) ? o : o + 1);
-                }
-                if constexpr (SEND) {   // the sender's candidate, and with it the row's wave: the sender updates
-                    const uint32_t sx = (uint32_t)r[e].n >> 16;
-                    if (sx != KA_WAVE_NO_SENDER) {
-                        KaWaveSendMeta* sm = ka_wave_send_meta(meta);
-                        const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
-                        const long long a = w * ka_wave_nrcv<SEND>(r[e]);
-                        const int o = ka_wave_ld<GSTATE>(sw.open + sx);
-                        const long long l = ka_wave_ld<GSTATE>(sw.load + sx);
-                        wv = max(wv, (l == 0 || l + a <= sm->snd.C) ? o : o + 1);
-                        if (wv > o) {   // the sender closes its bucket and opens wave wv
-                            if (l > 0) ka_wave_send_put(sm, o, sx, l);
-                            ka_wave_st<GSTATE>(sw.open + sx, wv);
-                            ka_wave_st<GSTATE>(sw.load + sx, a);
-                        } else {
-                            ka_wave_st<GSTATE>(sw.load + sx, l + a);
-                        }
-                    }
-                }
-                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) {
-                    const uint32_t b = ka_wave_rcv(r[e], j);
-                    const int o = ka_wave_ld<GSTATE>(open + b);
-                    const long long l = ka_wave_ld<GSTATE>(load + b);
-                    if (wv > o) {   // b closes its bucket and opens wave wv
-                        if (l > 0) put(o, b, l);
-                        ka_wave_st<GSTATE>(open + b, wv);
-                        ka_wave_st<GSTATE>(load + b, w);
-                    } else {
-                        ka_wave_st<GSTATE>(load + b, l + w);
-                    }
-                }
-                wave[r[e].row] = wv;
-                my_max = max(my_max, wv);
+                const int v = decide(r[e], k, s);
+                wave[r[e].row] = v;
+                my_max = max(my_max, v);
                 pend &= ~(1u << e);
             }
             if (!__syncthreads_or(pend != 0)) break;
         }
     }
-    // the buckets still open
-    for (int i = tid; i < N; i += KA_WAVE_THREADS) {
-        const long long l = ka_wave_ld<GSTATE>(load + i);
-        if (l > 0) put(ka_wave_ld<GSTATE>(open + i), (uint32_t)i, l);
+    return my_max;
+}
+
+// ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B. Writes wave[row] of every
+// record, the bucket log and meta->waves / nlog. The state is load / open / claim [rows = N + ns] in shared memory, or from
+// state on (GSTATE). SEND: also the sender rule of meta->snd (budget C), the sender buckets in its log and their count in meta->nslog.
+// Does nothing when the rows pass failed a row.
+template <bool GSTATE, bool SEND>
+__global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_chain_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off,
+                                                                           int nblk, int N, int rows, long long B, int32_t* __restrict__ wave,
+                                                                           unsigned char* state, KaWaveBucket* __restrict__ log,
+                                                                           KaWaveMeta* __restrict__ meta) {
+    extern __shared__ __align__(16) unsigned char ka_wave_smem[];
+    __shared__ unsigned nlog;
+    __shared__ int wmax;
+    if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;   // CTA-uniform
+    long long* load = reinterpret_cast<long long*>(GSTATE ? state : ka_wave_smem);
+    int* open = reinterpret_cast<int*>(load + rows);
+    unsigned* claim = reinterpret_cast<unsigned*>(open + rows);
+    const int tid = threadIdx.x;
+    for (int i = tid; i < rows; i += KA_WAVE_THREADS) {
+        ka_wave_st<GSTATE>(load + i, 0LL);
+        ka_wave_st<GSTATE>(open + i, 1);
+        ka_wave_st<GSTATE>(claim + i, 0u);
     }
-    if constexpr (SEND) {
-        KaWaveSendMeta* sm = ka_wave_send_meta(meta);
-        const KaWaveSendWords sw = ka_wave_send_words<GSTATE>(sm, claim, N);
-        for (int i = tid; i < sm->snd.n; i += KA_WAVE_THREADS) {
-            const long long l = ka_wave_ld<GSTATE>(sw.load + i);
-            if (l > 0) ka_wave_send_put(sm, ka_wave_ld<GSTATE>(sw.open + i), (uint32_t)i, l);
+    if (tid == 0) { nlog = 0; wmax = 0; }
+    __syncthreads();
+    // a closed or still-open bucket of row x: a broker's to the bucket log, a sender's (snd) to the sender log
+    auto put = [&](bool snd, int wv, int x, long long l) {
+        if (!snd) {
+            const unsigned i = atomicAdd(&nlog, 1u);
+            log[i] = KaWaveBucket{wv, x, l};
+        } else {
+            const unsigned i = atomicAdd(&meta->nslog, 1u);
+            meta->snd.log[i] = KaWaveBucket{wv, x - N, l};
         }
+    };
+    const int my_max = ka_wave_rounds<GSTATE, SEND>(rec, off[nblk], N, rows, claim, wave, [&](const KaWaveRec& r, int k, int s) {
+        const long long w = r.w;
+        int wv = 0;
+        auto want = [&](int x, long long amount, long long cap) {   // the record's wave: the latest any of its rows asks for
+            const int o = ka_wave_ld<GSTATE>(open + x);
+            const long long l = ka_wave_ld<GSTATE>(load + x);
+            wv = max(wv, (l == 0 || l + amount <= cap) ? o : o + 1);
+        };
+        for (int j = 0; j < k; ++j) want((int)ka_wave_rcv(r, j), w, B);
+        if (s >= 0) want(s, w * k, meta->snd.C);
+        auto take = [&](int x, long long amount, bool snd) {
+            const int o = ka_wave_ld<GSTATE>(open + x);
+            const long long l = ka_wave_ld<GSTATE>(load + x);
+            if (wv > o) {   // x closes its bucket and opens wave wv
+                if (l > 0) put(snd, o, x, l);
+                ka_wave_st<GSTATE>(open + x, wv);
+                ka_wave_st<GSTATE>(load + x, amount);
+            } else {
+                ka_wave_st<GSTATE>(load + x, l + amount);
+            }
+        };
+        for (int j = 0; j < k; ++j) take((int)ka_wave_rcv(r, j), w, false);
+        if (s >= 0) take(s, w * k, true);
+        return wv;
+    });
+    for (int i = tid; i < rows; i += KA_WAVE_THREADS) {   // the buckets still open
+        const long long l = ka_wave_ld<GSTATE>(load + i);
+        if (l > 0) put(SEND && i >= N, ka_wave_ld<GSTATE>(open + i), i, l);
     }
     atomicMax(&wmax, my_max);
     __syncthreads();
@@ -443,31 +400,14 @@ __global__ void __launch_bounds__(256) ka_wave_peak_kernel(const KaWaveBucket* _
 //
 //   ka_wave_fit_count_kernel  R_b and S_s over the packed records (after the compact pass)
 //   ka_wave_fit_bound_kernel  Wb, to the meta words the host reads before it sizes the table
-//   ka_wave_fit_chain_kernel  ONE CTA: the rows pass's claim rounds, with the first-fit decision
+//   ka_wave_fit_chain_kernel  ONE CTA: the claim rounds of ka_wave_rounds, with the first-fit decision
 //   ka_wave_fit_log_kernel    every nonzero bucket of the table into the bucket logs, for the peak passes
 //
 // The chain keeps a hint per row of the table: every wave below it has load >= the budget, so it refuses any row of weight >= 1.
 // A row of weight >= 1 starts at the largest hint among its receivers and sender and walks up; a row of weight 0 starts at wave 1.
 
-// Bytes of shared memory the first-fit chain keeps per table row (claim, hint).
+// Bytes the first-fit chain keeps per table row (claim, hint).
 #define KA_WAVE_FIT_ROW_BYTES 8
-
-// The meta words of a first-fit plan: the others', then Wb (atomicMax, init 0).
-struct KaWaveFitMeta {
-    KaWaveSendMeta sm;
-    int bound;
-};
-__device__ __forceinline__ KaWaveFitMeta* ka_wave_fit_meta(KaWaveMeta* meta) { return reinterpret_cast<KaWaveFitMeta*>(meta); }
-
-// The sender's row of the table (N + its send-table index), or -1 for a record without one or a plan without a sender part.
-template <bool SEND>
-__device__ __forceinline__ int ka_wave_fit_sender(const KaWaveRec& r, int N) {
-    if constexpr (SEND) {
-        const uint32_t sx = (uint32_t)r.n >> 16;
-        return sx != KA_WAVE_NO_SENDER ? N + (int)sx : -1;
-    }
-    return -1;
-}
 
 // Same grid as the rows pass: cnt[N + ns] (zeroed) gets R_b, then S_s at N + s. Does nothing when the rows pass failed a row.
 template <bool SEND>
@@ -478,11 +418,11 @@ __global__ void __launch_bounds__(256) ka_wave_fit_count_kernel(const KaWaveRec*
     if (i >= off[nblk]) return;
     const KaWaveRec r = rec[i];
     for (int j = 0; j < ka_wave_nrcv<SEND>(r); ++j) atomicAdd(cnt + ka_wave_rcv(r, j), 1);
-    const int s = ka_wave_fit_sender<SEND>(r, N);
+    const int s = ka_wave_sender<SEND>(r, N);
     if (s >= 0) atomicAdd(cnt + s, 1);
 }
 
-// Same grid: ka_wave_fit_meta(meta)->bound = Wb over the counts of ka_wave_fit_count_kernel.
+// Same grid: meta->bound = Wb over the counts of ka_wave_fit_count_kernel.
 template <bool SEND>
 __global__ void __launch_bounds__(256) ka_wave_fit_bound_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off, int nblk,
                                                                 int N, const int* __restrict__ cnt, KaWaveMeta* __restrict__ meta) {
@@ -494,37 +434,29 @@ __global__ void __launch_bounds__(256) ka_wave_fit_bound_kernel(const KaWaveRec*
         const KaWaveRec r = rec[i];
         long long x = 0;   // up to 8 x (M - 1) + M - 1: beyond int32 for large M
         for (int j = 0; j < ka_wave_nrcv<SEND>(r); ++j) x += cnt[ka_wave_rcv(r, j)] - 1;
-        const int s = ka_wave_fit_sender<SEND>(r, N);
+        const int s = ka_wave_sender<SEND>(r, N);
         if (s >= 0) x += cnt[s] - 1;
         v = (unsigned)(1 + min(x, (long long)M - 1));
     }
     v = __reduce_max_sync(KA_FULL, v);
-    if ((threadIdx.x & 31) == 0 && v) atomicMax(&ka_wave_fit_meta(meta)->bound, (int)v);
+    if ((threadIdx.x & 31) == 0 && v) atomicMax(&meta->bound, (int)v);
 }
 
 // ONE CTA of KA_WAVE_THREADS. The M = off[nblk] records in rec, the table's N brokers, budget B, the zeroed table [N + ns][Wb].
-// Writes wave[row] of every record and meta->waves. With GSTATE the per-row words are gclaim / ghint [N + ns], else shared
-// memory. SEND: ns, C and the senders' rows as ka_wave_send_meta(meta) gives them. Does nothing when the rows pass failed a row.
+// Writes wave[row] of every record and meta->waves. The state is claim / hint [rows = N + ns] in shared memory, or from state
+// on (GSTATE). SEND: also the senders' rows and budget C of meta->snd. Does nothing when the rows pass failed a row.
 template <bool GSTATE, bool SEND>
 __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_fit_chain_kernel(const KaWaveRec* __restrict__ rec, const int32_t* __restrict__ off,
-                                                                               int nblk, int N, long long B, int Wb, int32_t* __restrict__ wave,
-                                                                               long long* __restrict__ table, unsigned* gclaim, int* ghint,
+                                                                               int nblk, int N, int rows, long long B, int Wb, int32_t* __restrict__ wave,
+                                                                               long long* __restrict__ table, unsigned char* state,
                                                                                KaWaveMeta* __restrict__ meta) {
     extern __shared__ __align__(16) unsigned char ka_wave_smem[];
     __shared__ int wmax;
     if (*(volatile unsigned*)&meta->err_row != 0xFFFFFFFFu) return;   // CTA-uniform
-    int rows = N;
     long long C = 0;
-    if constexpr (SEND) {
-        rows += ka_wave_send_meta(meta)->snd.n;
-        C = ka_wave_send_meta(meta)->snd.C;
-    }
-    unsigned* claim = gclaim;
-    int* hint = ghint;
-    if constexpr (!GSTATE) {
-        claim = reinterpret_cast<unsigned*>(ka_wave_smem);
-        hint = reinterpret_cast<int*>(claim + rows);
-    }
+    if constexpr (SEND) C = meta->snd.C;
+    unsigned* claim = reinterpret_cast<unsigned*>(GSTATE ? state : ka_wave_smem);
+    int* hint = reinterpret_cast<int*>(claim + rows);
     const int tid = threadIdx.x;
     for (int i = tid; i < rows; i += KA_WAVE_THREADS) {
         ka_wave_st<GSTATE>(claim + i, 0u);
@@ -532,82 +464,38 @@ __global__ void __launch_bounds__(KA_WAVE_THREADS, 1) ka_wave_fit_chain_kernel(c
     }
     if (tid == 0) wmax = 0;
     __syncthreads();
-    const int M = off[nblk];
-    unsigned round = 0;
-    int my_max = 0;
-    for (int base = 0; base < M; base += KA_WAVE_CHUNK) {
-        KaWaveRec r[KA_WAVE_PER_THREAD];
-        unsigned pend = 0;
-#pragma unroll
-        for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
-            const int i = base + e * KA_WAVE_THREADS + tid;
-            if (i < M) {
-                r[e] = rec[i];
-                pend |= 1u << e;
-            } else {
-                r[e] = KaWaveRec{0, 0, 0, 0, 0};
-            }
+    const int my_max = ka_wave_rounds<GSTATE, SEND>(rec, off[nblk], N, rows, claim, wave, [&](const KaWaveRec& r, int k, int s) {
+        const long long w = r.w, a = w * k;
+        int v = 1;
+        if (w > 0) {
+            for (int j = 0; j < k; ++j) v = max(v, ka_wave_ld<GSTATE>(hint + ka_wave_rcv(r, j)));
+            if (s >= 0) v = max(v, ka_wave_ld<GSTATE>(hint + s));
         }
-        for (;;) {
-            if (++round == KA_WAVE_MAX_ROUND) {   // the key's round field is full: clear the claims and count again
-                for (int i = tid; i < rows; i += KA_WAVE_THREADS) ka_wave_st<GSTATE>(claim + i, 0u);
-                __syncthreads();
-                round = 1;
+        for (; v < Wb; ++v) {   // Wb itself always fits (the bound above)
+            bool fit = true;
+            for (int j = 0; j < k && fit; ++j) {
+                const long long l = table[(size_t)ka_wave_rcv(r, j) * Wb + v - 1];
+                fit = l == 0 || l + w <= B;
             }
-            unsigned key[KA_WAVE_PER_THREAD];
-#pragma unroll
-            for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
-                key[e] = round << KA_WAVE_SLOT_BITS | (unsigned)(KA_WAVE_CHUNK - 1 - (e * KA_WAVE_THREADS + tid));
-                if (!(pend >> e & 1u)) continue;
-                for (int j = 0; j < ka_wave_nrcv<SEND>(r[e]); ++j) atomicMax(claim + ka_wave_rcv(r[e], j), key[e]);
-                const int s = ka_wave_fit_sender<SEND>(r[e], N);
-                if (s >= 0) atomicMax(claim + s, key[e]);
+            if (fit && s >= 0) {
+                const long long l = table[(size_t)s * Wb + v - 1];
+                fit = l == 0 || l + a <= C;
             }
-            __syncthreads();
-#pragma unroll
-            for (int e = 0; e < KA_WAVE_PER_THREAD; ++e) {
-                if (!(pend >> e & 1u)) continue;
-                const int k = ka_wave_nrcv<SEND>(r[e]);
-                const int s = ka_wave_fit_sender<SEND>(r[e], N);
-                bool own = s < 0 || ka_wave_ld<GSTATE>(claim + s) == key[e];
-                for (int j = 0; j < k; ++j) own &= ka_wave_ld<GSTATE>(claim + ka_wave_rcv(r[e], j)) == key[e];
-                if (!own) continue;
-                const long long w = r[e].w, a = w * k;
-                int v = 1;
-                if (w > 0) {
-                    for (int j = 0; j < k; ++j) v = max(v, ka_wave_ld<GSTATE>(hint + ka_wave_rcv(r[e], j)));
-                    if (s >= 0) v = max(v, ka_wave_ld<GSTATE>(hint + s));
-                }
-                for (; v < Wb; ++v) {   // Wb itself always fits (the bound above)
-                    bool fit = true;
-                    for (int j = 0; j < k && fit; ++j) {
-                        const long long l = table[(size_t)ka_wave_rcv(r[e], j) * Wb + v - 1];
-                        fit = l == 0 || l + w <= B;
-                    }
-                    if (fit && s >= 0) {
-                        const long long l = table[(size_t)s * Wb + v - 1];
-                        fit = l == 0 || l + a <= C;
-                    }
-                    if (fit) break;
-                }
-                // add to every bucket, and move each row's hint past the waves that are now full
-                auto add = [&](int x, long long amount, long long cap) {
-                    long long* row = table + (size_t)x * Wb;
-                    row[v - 1] += amount;
-                    int h = ka_wave_ld<GSTATE>(hint + x);
-                    if (h != v) return;
-                    while (h < Wb && row[h - 1] >= cap) ++h;
-                    ka_wave_st<GSTATE>(hint + x, h);
-                };
-                for (int j = 0; j < k; ++j) add((int)ka_wave_rcv(r[e], j), w, B);
-                if (s >= 0) add(s, a, C);
-                wave[r[e].row] = v;
-                my_max = max(my_max, v);
-                pend &= ~(1u << e);
-            }
-            if (!__syncthreads_or(pend != 0)) break;
+            if (fit) break;
         }
-    }
+        // add to every bucket, and move each row's hint past the waves that are now full
+        auto add = [&](int x, long long amount, long long cap) {
+            long long* row = table + (size_t)x * Wb;
+            row[v - 1] += amount;
+            int h = ka_wave_ld<GSTATE>(hint + x);
+            if (h != v) return;
+            while (h < Wb && row[h - 1] >= cap) ++h;
+            ka_wave_st<GSTATE>(hint + x, h);
+        };
+        for (int j = 0; j < k; ++j) add((int)ka_wave_rcv(r, j), w, B);
+        if (s >= 0) add(s, a, C);
+        return v;
+    });
     atomicMax(&wmax, my_max);
     __syncthreads();
     if (tid == 0) meta->waves = wmax;
@@ -632,13 +520,12 @@ __global__ void __launch_bounds__(256) ka_wave_fit_log_kernel(const long long* _
         at = __shfl_sync(KA_FULL, at, 0) + __popc(mi & ka_lanemask_lt());
         if (in) log[at] = KaWaveBucket{v, x, l};
         if constexpr (SEND) {
-            KaWaveSendMeta* sm = ka_wave_send_meta(meta);
             const bool out = l > 0 && x >= N;
             const unsigned mo = __ballot_sync(KA_FULL, out);
             unsigned so = 0;
-            if (lane == 0 && mo) so = atomicAdd(&sm->nslog, (unsigned)__popc(mo));
+            if (lane == 0 && mo) so = atomicAdd(&meta->nslog, (unsigned)__popc(mo));
             so = __shfl_sync(KA_FULL, so, 0) + __popc(mo & ka_lanemask_lt());
-            if (out) sm->snd.log[so] = KaWaveBucket{v, x - N, l};
+            if (out) meta->snd.log[so] = KaWaveBucket{v, x - N, l};
         }
     }
 }
