@@ -1,6 +1,6 @@
-"""The plain-Python model of the first-fit wave rule (KA_WAVE_FIRST_FIT of include/kassign.h) and of the documents built from
-its plan, beside the greedy rule's in tests/models.py. Like that module it imports numpy and the status codes only, so CPU
-tests, GPU tests and tests/tools can all use it."""
+"""The plain-Python model of the first-fit wave rule (KA_WAVE_FIRST_FIT of include/kassign.h), its bound Wb on the waves, and
+the documents built from its plan, beside the greedy rule's in tests/models.py. Like that module it imports numpy and the
+status codes only, so CPU tests, GPU tests and tests/tools can all use it."""
 import numpy as np
 
 from kafka_assigner_b200 import _native
@@ -71,6 +71,30 @@ def plan_waves(rep_off, cur, out, out_len, ids, B, weight=None, send=None):
             if k == kind and x > s[peak]:
                 s[peak], s[pid] = x, b
     return wave, summ, (0, 0, 0)
+
+
+def moved(cur_lists, new_lists, weight, send):
+    """[(row, receivers, w, sender or None)] of the rows with receivers (the chain's records), from the current and new lists."""
+    res = []
+    for g, (old, new) in enumerate(zip(cur_lists, new_lists)):
+        recv = [b for b in new if b not in old]
+        if old != new and recv:
+            res.append((g, recv, 1 if weight is None else int(weight[g]), old[0] if send is not None and old else None))
+    return res
+
+
+def bound(moved):
+    """Wb of include/kassign.h over the records of `moved`: min(M, 1 + max over moved rows of sum (R_b - 1) + (S_s - 1))."""
+    R, S = {}, {}
+    for _, recv, _, s in moved:
+        for b in recv:
+            R[b] = R.get(b, 0) + 1
+        if s is not None:
+            S[s] = S.get(s, 0) + 1
+    if not moved:
+        return 0
+    worst = max(sum(R[b] - 1 for b in recv) + (S[s] - 1 if s is not None else 0) for _, recv, _, s in moved)
+    return min(len(moved), 1 + worst)
 
 
 def wave_documents(topic_names, part_off, part_id, rep_off, cur, out, out_len, ids, B, weight=None, send=None, L=None,

@@ -1,5 +1,5 @@
 """The plain-Python models the device is checked against, each written once: the move summary, the wave rule (with and
-without a sender budget), the reassignment JSON printers, the wave documents and their greedy cut, the schedule model's records,
+without a sender budget), the wave chain's claim rounds, the reassignment JSON printers, the wave documents and their greedy cut, the schedule model's records,
 slot chains and the expected counter histogram, and kernel A's shared-memory budget.
 Each restates a rule of include/kassign.h. This module imports numpy and the status codes only: it never loads the library
 or the oracle, so CPU tests, GPU tests and tests/tools can all use it."""
@@ -126,6 +126,76 @@ def plan_waves(rep_off, cur, out, out_len, ids, B, weight=None, send=None):
             if x > s[peak]:
                 s[peak], s[pid] = x, b
     return wave, summ, (0, 0, 0)
+
+
+# ---- the wave chain's rounds (both rules) ----------------------------------------------------------------------------------
+# The device does not report its rounds, so these restatements of the round rule of kassign_waves.cuh are the evidence that a
+# plan reaches the chain's claim reset.
+
+WAVE_CHUNK = 2048            # KA_WAVE_CHUNK: records the chain decides together
+WAVE_RESET = 1 << 21         # KA_WAVE_MAX_ROUND: the round at which the chain clears its claims and counts from 1 again
+
+
+def wave_records(rep_off, cur, out, out_len):
+    """(receivers, senders) per row: the new-list brokers its current list lacks, in list order, and the first broker of its
+    current list (None when it is empty). A row with receivers is a record of the chain; the others are not."""
+    rcv, snd = [], []
+    for g in range(len(out_len)):
+        old = cur[int(rep_off[g]):int(rep_off[g + 1])].tolist()
+        rcv.append([b for b in out[g, :int(out_len[g])].tolist() if b not in old])
+        snd.append(old[0] if old else None)
+    return rcv, snd
+
+
+def chain_keys(records, senders, g):
+    """The chain's words a record claims: its receivers', and with a send table its sender's (a separate set of words)."""
+    keys = [("r", b) for b in records[g]]
+    if senders is not None and senders[g] is not None:
+        keys.append(("s", senders[g]))
+    return keys
+
+
+def chain_rounds(records, senders=None):
+    """The global round in which the chain decides every record (int64 per row, 0 for a row without receivers). records: the
+    receivers of every row; senders (the send form): the sender of every row, or None. The records, in row order, are cut into
+    chunks of 2 048. A record decides in round 1 + the latest round among the earlier records of its chunk that share a receiver
+    with it, or its sender; a chunk takes as many rounds as its latest record, and the count runs on across chunks."""
+    rounds = np.zeros(len(records), dtype=np.int64)
+    base = top = n = 0
+    last = {}
+    for g, rcv in enumerate(records):
+        if not rcv:
+            continue
+        if n == WAVE_CHUNK:
+            base, top, n, last = base + top, 0, 0, {}
+        keys = chain_keys(records, senders, g)
+        r = 1 + max(last.get(k, 0) for k in keys)
+        for k in keys:
+            last[k] = r
+        top = max(top, r)
+        n += 1
+        rounds[g] = base + r
+    return rounds
+
+
+def crossing_chunk(records, senders, rounds):
+    """The chunk in which round 2^21 falls: (records decided before the reset, after it, keys (receivers or senders) with records
+    on both sides, chunks after it). Fails unless exactly one chunk has records on both sides."""
+    rows = np.nonzero(rounds)[0]
+    chunk = np.arange(len(rows)) // WAVE_CHUNK
+    starts = np.arange(0, len(rows), WAVE_CHUNK)
+    lo, hi = np.minimum.reduceat(rounds[rows], starts), np.maximum.reduceat(rounds[rows], starts)
+    mixed = np.nonzero((lo < WAVE_RESET) & (hi >= WAVE_RESET))[0]
+    assert len(mixed) == 1, mixed
+    c = int(mixed[0])
+    mine = rows[chunk == c]
+    before = rounds[mine] < WAVE_RESET
+    sides = {}
+    for g, b in zip(mine, before):
+        for k in chain_keys(records, senders, g):
+            sides.setdefault(k, set()).add(bool(b))
+    shared = sum(len(v) == 2 for v in sides.values())
+    return int(before.sum()), int((~before).sum()), shared, len(starts) - 1 - c
 
 
 # ---- reassignment JSON ---------------------------------------------------------------------------------------------------

@@ -6,14 +6,10 @@
 - wave documents whose text passes 2^32 bytes (64-bit document offsets);
 - the 32-bit fragment limit of ka_solve_json and ka_solve_clusters_json, on both sides.
 
-`chain_rounds` restates the chain's round rule (kassign_waves.cuh). The device does not report its rounds, so this model is the
-evidence that a plan reaches the reset. The plans that cross it run in a child process with a timeout: a chain that stopped
+`models.chain_rounds` restates the chain's round rule (kassign_waves.cuh). The device does not report its rounds, so this model is
+the evidence that a plan reaches the reset. The plans that cross it run in a child process with a timeout: a chain that stopped
 finishing would fail its test and go away with the process."""
-import os
 import re
-import subprocess
-import sys
-import time
 
 import numpy as np
 import pytest
@@ -24,73 +20,9 @@ from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_D
 from tests import models, util
 from tests.util import Member
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIMIT = _native.KA_ERR_LIMIT
-CHUNK = 2048                 # KA_WAVE_CHUNK: records the chain decides together
-RESET = 1 << 21              # KA_WAVE_MAX_ROUND: the round at which the chain clears its claims and counts from 1 again
+CHUNK, RESET = models.WAVE_CHUNK, models.WAVE_RESET
 UINT32_MAX = (1 << 32) - 1
-
-
-def wave_records(rep_off, cur, out, out_len):
-    """(receivers, senders) per row: the new-list brokers its current list lacks, in list order, and the first broker of its
-    current list (None when it is empty). A row with receivers is a record of the chain; the others are not."""
-    rcv, snd = [], []
-    for g in range(len(out_len)):
-        old = cur[int(rep_off[g]):int(rep_off[g + 1])].tolist()
-        rcv.append([b for b in out[g, :int(out_len[g])].tolist() if b not in old])
-        snd.append(old[0] if old else None)
-    return rcv, snd
-
-
-def _keys(records, senders, g):
-    """The chain's words a record claims: its receivers', and with a send table its sender's (a separate set of words)."""
-    keys = [("r", b) for b in records[g]]
-    if senders is not None and senders[g] is not None:
-        keys.append(("s", senders[g]))
-    return keys
-
-
-def chain_rounds(records, senders=None):
-    """The global round in which the chain decides every record (int64 per row, 0 for a row without receivers). records: the
-    receivers of every row; senders (the send form): the sender of every row, or None. The records, in row order, are cut into
-    chunks of 2 048. A record decides in round 1 + the latest round among the earlier records of its chunk that share a receiver
-    with it, or its sender; a chunk takes as many rounds as its latest record, and the count runs on across chunks."""
-    rounds = np.zeros(len(records), dtype=np.int64)
-    base = top = n = 0
-    last = {}
-    for g, rcv in enumerate(records):
-        if not rcv:
-            continue
-        if n == CHUNK:
-            base, top, n, last = base + top, 0, 0, {}
-        keys = _keys(records, senders, g)
-        r = 1 + max(last.get(k, 0) for k in keys)
-        for k in keys:
-            last[k] = r
-        top = max(top, r)
-        n += 1
-        rounds[g] = base + r
-    return rounds
-
-
-def crossing_chunk(records, senders, rounds):
-    """The chunk in which round 2^21 falls: (records decided before the reset, after it, brokers with records on both sides,
-    chunks after it). Fails unless exactly one chunk has records on both sides."""
-    rows = np.nonzero(rounds)[0]
-    chunk = np.arange(len(rows)) // CHUNK
-    starts = np.arange(0, len(rows), CHUNK)
-    lo, hi = np.minimum.reduceat(rounds[rows], starts), np.maximum.reduceat(rounds[rows], starts)
-    mixed = np.nonzero((lo < RESET) & (hi >= RESET))[0]
-    assert len(mixed) == 1, mixed
-    c = int(mixed[0])
-    mine = rows[chunk == c]
-    before = rounds[mine] < RESET
-    sides = {}
-    for g, b in zip(mine, before):
-        for k in _keys(records, senders, g):
-            sides.setdefault(k, set()).add(bool(b))
-    shared = sum(len(v) == 2 for v in sides.values())
-    return int(before.sum()), int((~before).sum()), shared, len(starts) - 1 - c
 
 
 # ---- CPU: the round model ------------------------------------------------------------------------------------------------
@@ -107,9 +39,9 @@ def _claims(records, senders=None):
         while pend:
             rnd += 1
             for slot, g in pend:
-                for k in _keys(records, senders, g):
+                for k in models.chain_keys(records, senders, g):
                     claim[k] = max(claim.get(k, (0, 0)), (rnd, -slot))
-            won = {g for slot, g in pend if all(claim[k] == (rnd, -slot) for k in _keys(records, senders, g))}
+            won = {g for slot, g in pend if all(claim[k] == (rnd, -slot) for k in models.chain_keys(records, senders, g))}
             for g in won:
                 rounds[g] = rnd
             pend = [(slot, g) for slot, g in pend if g not in won]
@@ -117,40 +49,40 @@ def _claims(records, senders=None):
 
 
 def test_a_fully_serial_chunk_takes_2048_rounds():
-    rounds = chain_rounds([[7]] * (CHUNK + 3))
+    rounds = models.chain_rounds([[7]] * (CHUNK + 3))
     assert rounds.tolist() == list(range(1, CHUNK + 4))
     # a sender alone makes records serial, as a shared receiver does
-    rounds = chain_rounds([[100 + g] for g in range(CHUNK + 1)], [1] * (CHUNK + 1))
+    rounds = models.chain_rounds([[100 + g] for g in range(CHUNK + 1)], [1] * (CHUNK + 1))
     assert rounds.tolist() == list(range(1, CHUNK + 2))
     # without a send table the sender is no link
-    assert chain_rounds([[100 + g] for g in range(CHUNK + 1)]).tolist() == [1] * CHUNK + [2]
+    assert models.chain_rounds([[100 + g] for g in range(CHUNK + 1)]).tolist() == [1] * CHUNK + [2]
 
 
 def test_a_chunk_of_independent_records_takes_one_round():
-    rounds = chain_rounds([[g, g + 50000] for g in range(3 * CHUNK)])
+    rounds = models.chain_rounds([[g, g + 50000] for g in range(3 * CHUNK)])
     assert rounds.tolist() == [1] * CHUNK + [2] * CHUNK + [3] * CHUNK
-    assert chain_rounds([[g] for g in range(10)], [None] * 10).tolist() == [1] * 10
+    assert models.chain_rounds([[g] for g in range(10)], [None] * 10).tolist() == [1] * 10
 
 
 def test_a_path_is_serial():
     L = CHUNK + 1
     records = [[1 + i % L, 1 + (i + 1) % L] for i in range(2 * CHUNK + 5)]
-    assert chain_rounds(records).tolist() == list(range(1, 2 * CHUNK + 6))
+    assert models.chain_rounds(records).tolist() == list(range(1, 2 * CHUNK + 6))
     # two interleaved paths (record i receives i and i + 2) are two chains: half the rounds
-    assert chain_rounds([[i, i + 2] for i in range(CHUNK)]).tolist() == [1 + i // 2 for i in range(CHUNK)]
+    assert models.chain_rounds([[i, i + 2] for i in range(CHUNK)]).tolist() == [1 + i // 2 for i in range(CHUNK)]
 
 
 def test_unchanged_and_receiverless_rows_are_not_records():
     cur_lists = [[1], [1, 2], [1, 2], [1, 2], [3], [], [4]]
     new_lists = [[2], [1, 2], [2, 1], [1], [2], [], [4, 2]]
-    rcv, snd = wave_records(*util.cur_lists(cur_lists), *util.rows(new_lists))
+    rcv, snd = models.wave_records(*util.cur_lists(cur_lists), *util.rows(new_lists))
     assert rcv == [[2], [], [], [], [2], [], [2]] and snd == [1, 1, 1, 1, 3, None, 4]
-    assert chain_rounds(rcv).tolist() == [1, 0, 0, 0, 2, 0, 3]
+    assert models.chain_rounds(rcv).tolist() == [1, 0, 0, 0, 2, 0, 3]
     # rows that are no record take no slot of a chunk: 2 047 serial records, 500 other rows, then the chunk's last record
     cur_lists = [[1]] * (CHUNK - 1) + [[1, 2]] * 500 + [[1], [1]]
     new_lists = [[2]] * (CHUNK - 1) + [[2, 1] if g % 2 else [1, 2] for g in range(500)] + [[2], [2]]
-    rcv, _ = wave_records(*util.cur_lists(cur_lists), *util.rows(new_lists))
-    rounds = chain_rounds(rcv)
+    rcv, _ = models.wave_records(*util.cur_lists(cur_lists), *util.rows(new_lists))
+    rounds = models.chain_rounds(rcv)
     assert rounds[CHUNK - 1:CHUNK + 499].tolist() == [0] * 500
     assert rounds[-2:].tolist() == [CHUNK, CHUNK + 1]
 
@@ -164,7 +96,7 @@ def test_the_rule_is_the_claims_mechanism(seed):
                for g in range(n)]
     senders = [None if rng.random() < 0.2 else int(rng.integers(1, 60)) for _ in range(n)]
     for s in (None, senders):
-        assert np.array_equal(chain_rounds(records, s), _claims(records, s))
+        assert np.array_equal(models.chain_rounds(records, s), _claims(records, s))
 
 
 # ---- GPU: plans that cross round 2^21, and their documents ---------------------------------------------------------------
@@ -229,8 +161,8 @@ def reset_input(send, seed=5):
     return inp
 
 
-# Run in a child process: both plans (chain state in shared and in global memory) and the documents, written back to the
-# directory given. A chain that never finished would take the child, not the test session, with it.
+# Run in a child process (util.run_child): both plans (chain state in shared and in global memory) and the documents, written
+# back to the directory given.
 _CHILD = r"""
 import sys
 import time
@@ -263,10 +195,6 @@ np.savez(d + "/out.npz", **res)
 CHILD_TIMEOUT = 300   # seconds: about five times what the child takes on an H100
 
 
-def _summary_array(summ, dtype):
-    return np.array([tuple(s[f] for f in dtype.names) for s in summ], dtype=dtype)
-
-
 @pytest.fixture(scope="module", params=["receive", "send"])
 def reset_plans(request, tmp_path_factory, native_lib):
     """The device's plans and documents for reset_input (from the child) with the models of the same input, each computed once:
@@ -275,16 +203,11 @@ def reset_plans(request, tmp_path_factory, native_lib):
     d = tmp_path_factory.mktemp(request.param)
     inp = reset_input(send)
     np.savez(d / "in.npz", **inp)
-    env = dict(os.environ, PYTHONPATH=ROOT + os.pathsep + os.environ.get("PYTHONPATH", ""))
-    flags = ["-s"] if sys.flags.no_user_site else []
-    t0 = time.monotonic()
-    child = subprocess.Popen([sys.executable] + flags + ["-c", _CHILD, str(d)], cwd=ROOT, env=env, stdout=subprocess.PIPE,
-                             stderr=subprocess.STDOUT, text=True)
-    try:
-        # the models, while the device plans
-        args = (inp["rep_off"], inp["cur"], inp["out"], inp["out_len"])
-        records, senders = wave_records(*args)
-        rounds = chain_rounds(records, senders if send else None)
+    args = (inp["rep_off"], inp["cur"], inp["out"], inp["out_len"])
+
+    def expected():   # the models, while the device plans
+        records, senders = models.wave_records(*args)
+        rounds = models.chain_rounds(records, senders if send else None)
         names, part_off = list(inp["names"]), inp["part_off"]
         if send:
             e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(names, part_off, None, *args, inp["ids"], int(inp["B"]),
@@ -293,18 +216,12 @@ def reset_plans(request, tmp_path_factory, native_lib):
             e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(names, part_off, None, *args, inp["ids"], int(inp["B"]),
                                                                        inp["weight"])
         assert e_st == (0, 0, 0)
-        e_summ = _summary_array(e_summ, WAVE_SEND_SUMMARY_DTYPE if send else WAVE_SUMMARY_DTYPE)
-        out, _ = child.communicate(timeout=max(1.0, CHILD_TIMEOUT - (time.monotonic() - t0)))
-    except subprocess.TimeoutExpired:
-        child.kill()
-        child.communicate()
-        pytest.fail("the plans of %s did not finish within %d s" % (request.param, CHILD_TIMEOUT))
-    finally:
-        if child.poll() is None:
-            child.kill()
-            child.communicate()
-    print("%s: child and models %.1f s\n%s" % (request.param, time.monotonic() - t0, out))
-    assert child.returncode == 0, out
+        e_summ = util.summary_array(e_summ, WAVE_SEND_SUMMARY_DTYPE if send else WAVE_SUMMARY_DTYPE)
+        return records, senders, rounds, e_docs, e_wave, e_summ
+
+    (records, senders, rounds, e_docs, e_wave, e_summ), out, secs = util.run_child(_CHILD, d, CHILD_TIMEOUT, expected,
+                                                                                   "the plans of " + request.param)
+    print("%s: child and models %.1f s\n%s" % (request.param, secs, out))
     dev = dict(np.load(d / "out.npz"))
     return inp, dev, e_docs, e_wave, e_summ, rounds, records, senders if send else None
 
@@ -314,7 +231,7 @@ def test_plans_cross_round_2_21(reset_plans):
     """All four chain instances: every wave, W and summary field of both state placements equal the model, and the chain really
     crossed round 2^21 inside a chunk, with records of that chunk on both sides of the reset and brokers they share across it."""
     inp, dev, _, e_wave, e_summ, rounds, records, senders = reset_plans
-    before, after, shared, later = crossing_chunk(records, senders, rounds)
+    before, after, shared, later = models.crossing_chunk(records, senders, rounds)
     assert before >= 300 and after >= 300 and shared >= 4 and later >= 5, (before, after, shared, later)
     assert int(rounds.max()) > RESET
     W = len(e_summ)
@@ -369,7 +286,7 @@ def test_scattered_documents_over_large_tiles(native_lib):
     e_docs, _, _, e_wave, e_summ, e_st = models.wave_documents(names, part_off, None, rep_off, cur, out, out_len, s.broker_id, 1)
     assert st.code == 0 and e_st == (0, 0, 0) and 256 <= len(e_docs) <= 65535
     assert np.array_equal(wave, e_wave)
-    e_summ = _summary_array(e_summ, WAVE_SUMMARY_DTYPE)
+    e_summ = util.summary_array(e_summ, WAVE_SUMMARY_DTYPE)
     assert all(np.array_equal(summ[f], e_summ[f]) for f in WAVE_SUMMARY_DTYPE.names)
     _compare_docs(docs, e_docs)
 

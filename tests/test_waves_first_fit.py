@@ -25,30 +25,6 @@ def _model(cur_lists, new_lists, B, weight=None, ids=range(1, 100), send=None, f
     return plan(rep_off, cur, out, out_len, np.asarray(list(ids)), B, weight, send)
 
 
-def _moved(cur_lists, new_lists, weight, send):
-    """[(row, receivers, w, sender or None)] of the rows with receivers."""
-    res = []
-    for g, (old, new) in enumerate(zip(cur_lists, new_lists)):
-        recv = [b for b in new if b not in old]
-        if old != new and recv:
-            res.append((g, recv, 1 if weight is None else int(weight[g]), old[0] if send is not None and old else None))
-    return res
-
-
-def _bound(moved):
-    """Wb of include/kassign.h: min(M, 1 + max over moved rows of sum (R_b - 1) + (S_s - 1))."""
-    R, S = {}, {}
-    for _, recv, _, s in moved:
-        for b in recv:
-            R[b] = R.get(b, 0) + 1
-        if s is not None:
-            S[s] = S.get(s, 0) + 1
-    if not moved:
-        return 0
-    worst = max(sum(R[b] - 1 for b in recv) + (S[s] - 1 if s is not None else 0) for _, recv, _, s in moved)
-    return min(len(moved), 1 + worst)
-
-
 def check_first_fit(cur_lists, new_lists, wave, summ, B, weight=None, send=None):
     """Every invariant include/kassign.h states for a first-fit plan: non-empty waves 1..W, every row's wave the smallest that
     fits beside the earlier rows (a search from wave 1), so every budget holds, and W <= Wb."""
@@ -57,7 +33,7 @@ def check_first_fit(cur_lists, new_lists, wave, summ, B, weight=None, send=None)
     assert all(s["rows"] > 0 for s in summ) and set(wave.tolist()) - {0} == set(range(1, W + 1))
     C = None if send is None else send[1]
     inb, outb = {}, {}
-    moved = _moved(cur_lists, new_lists, weight, send)
+    moved = fit_models.moved(cur_lists, new_lists, weight, send)
     for g, recv, w, s in moved:
         a = w * len(recv)
 
@@ -72,7 +48,7 @@ def check_first_fit(cur_lists, new_lists, wave, summ, B, weight=None, send=None)
             inb[(b, v)] = inb.get((b, v), 0) + w
         if s is not None:
             outb[(s, v)] = outb.get((s, v), 0) + a
-    assert W <= max(_bound(moved), 1 if any(o != n for o, n in zip(cur_lists, new_lists)) else 0)
+    assert W <= max(fit_models.bound(moved), 1 if any(o != n for o, n in zip(cur_lists, new_lists)) else 0)
     if weight is None:   # unit weights: no rule can use fewer waves than the busiest receiver needs
         R = {}
         for _, recv, _, _ in moved:
@@ -196,21 +172,6 @@ def test_model_equals_greedy_without_repeats(seed):
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------------
 
-def _check(s, rep_off, cur, out, out_len, B, weight=None, send_ids=None, C=None):
-    """plan_waves under first fit against the model, every field. Returns (wave, summary, status)."""
-    s.set_wave_rule("first_fit")
-    send = {} if C is None else dict(max_broker_out=C, send_brokers=send_ids)
-    wave, summ, st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight, **send)
-    e_wave, e_summ, e_st = fit_models.plan_waves(rep_off, cur, out, out_len, s.broker_id, B, weight,
-                                                 None if C is None else (list(send_ids), C))
-    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
-    if st.code == 0:
-        assert np.array_equal(wave, e_wave), np.nonzero(wave != e_wave)[0][:10]
-        names = (WAVE_SUMMARY_DTYPE if C is None else WAVE_SEND_SUMMARY_DTYPE).names
-        assert [util.record_of(x, names) for x in summ] == e_summ
-    return wave, summ, st
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("remove", [0.0, 0.02])
 def test_solve_rows(native_lib, remove):
@@ -221,7 +182,7 @@ def test_solve_rows(native_lib, remove):
     mean = int(weight.mean())
     for B, w in ((1, None), (3, None), (INT64_MAX, None), (16 * mean, weight), (1, weight)):
         for C in (None, min(2 * B, INT64_MAX) if w is None else 16 * mean):
-            wave, summ, st = _check(s, cl.rep_off, cl.cur, out, out_len, B, w, cl.all_broker_id, C)
+            wave, summ, st = util.check_plan(s, cl.rep_off, cl.cur, out, out_len, B, w, cl.all_broker_id, C)
             assert st.code == 0 and len(summ) > 0
             s.set_wave_rule("greedy")
             g_wave, g_summ, _ = s.plan_waves(cl.rep_off, cl.cur, out, out_len, B, weight=w,
@@ -252,14 +213,14 @@ def test_lookup_modes_and_claim_state(native_lib, table):
     rep_off, cur = util.cur_lists(cur_lists)
     out, out_len = util.rows(new_lists, 3)
     for B, w in ((1, None), (16, None), (500, rng.integers(0, 100, Q).astype(np.int64))):
-        _check(s, rep_off, cur, out, out_len, B, w)
+        util.check_plan(s, rep_off, cur, out, out_len, B, w)
     # with a sender part: the send table is the brokers, then padded with ids no row names so that the words of brokers and
     # senders leave shared memory (fewer rows: the load table grows with the senders)
     for pad, q in ((0, Q), (25600, 3000)):
         send_ids = np.union1d(ids, 10 ** 8 + np.arange(pad)).astype(np.int32)
         rep_off, cur = util.cur_lists(cur_lists[:q])
         out, out_len = util.rows(new_lists[:q], 3)
-        _check(s, rep_off, cur, out, out_len, 4, None, send_ids, 6)
+        util.check_plan(s, rep_off, cur, out, out_len, 4, None, send_ids, 6)
 
 
 @pytest.mark.gpu
@@ -270,7 +231,7 @@ def test_hand_built_rows(native_lib):
     def run(cur_lists, new_lists, B, weight=None, stride=None):
         rep_off, cur = util.cur_lists(cur_lists)
         out, out_len = util.rows(new_lists, stride)
-        return _check(s, rep_off, cur, out, out_len, B, None if weight is None else np.asarray(weight, dtype=np.int64))
+        return util.check_plan(s, rep_off, cur, out, out_len, B, None if weight is None else np.asarray(weight, dtype=np.int64))
 
     assert run([[1], [1], [1]], [[2], [2, 3], [3]], 1)[0].tolist() == [1, 2, 1]                 # the hole greedy leaves
     assert run([[1]] * 5, [[2]] * 5, 3, [5, 1, 4, 2, 0])[0].tolist() == [1, 2, 3, 2, 2]          # heavier, zero
@@ -332,7 +293,7 @@ def test_documents_parts_and_rollback(native_lib, seed):
 def test_broker_usage_of_a_first_fit_plan(native_lib):
     cl = kab.synth.make_ragged_cluster(T=3000, N=400, max_partitions=128, seed=21, remove_frac=0.02)
     s, out, out_len, _ = util.solved(cl)
-    wave, _, st = _check(s, cl.rep_off, cl.cur, out, out_len, 1)
+    wave, _, st = util.check_plan(s, cl.rep_off, cl.cur, out, out_len, 1)
     assert st.code == 0
     usage, W, ust = s.broker_usage(cl.rep_off, cl.cur, out, out_len, wave, cl.all_broker_id)
     assert ust.code == 0 and W == int(wave.max())
@@ -347,7 +308,7 @@ def test_the_rule_is_context_configuration(native_lib):
     s, out, out_len, _ = util.solved(cl)
     assert s.wave_rule == "greedy"
     greedy = s.plan_waves(cl.rep_off, cl.cur, out, out_len, 1)
-    fit = _check(s, cl.rep_off, cl.cur, out, out_len, 1)
+    fit = util.check_plan(s, cl.rep_off, cl.cur, out, out_len, 1)
     assert not np.array_equal(fit[0], greedy[0])
     s.reset()   # keeps the rule
     assert s.wave_rule == "first_fit"

@@ -4,13 +4,17 @@ the checks and fakes more than one test module uses. The plain-Python models liv
 import ctypes
 import json
 import os
+import subprocess
+import sys
+import time
 
 import numpy as np
+import pytest
 
 import kafka_assigner_b200 as kab
 from kafka_assigner_b200 import _native
 from kafka_assigner_b200.assigner import WAVE_SEND_SUMMARY_DTYPE, WAVE_SUMMARY_DTYPE
-from tests import models
+from tests import fit_models, models
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 FRACS = (0.01, 0.02, 0.05, 0.10, 0.20, 0.30, 0.40, 0.50)
@@ -108,6 +112,30 @@ def row_width(rep_off, desired_rf):
     """The narrowest row stride for these lists and desired RF."""
     sizes = np.diff(rep_off)
     return max(int(sizes.max()) if len(sizes) else 0, desired_rf, 1)
+
+
+def run_child(code, d, timeout, meanwhile, what):
+    """Runs the Python source `code` in a child process, from the repository root with the package importable and argv[1] = d,
+    while the parent calls meanwhile(). A child that is not done `timeout` seconds after its start is killed and fails the test
+    ("<what> did not finish"): device calls that never finished go away with the child, not the test session. Returns
+    (meanwhile's result, the child's output, seconds from its start to its end)."""
+    root = os.path.dirname(HERE)
+    env = dict(os.environ, PYTHONPATH=root + os.pathsep + os.environ.get("PYTHONPATH", ""))
+    flags = ["-s"] if sys.flags.no_user_site else []
+    t0 = time.monotonic()
+    child = subprocess.Popen([sys.executable] + flags + ["-c", code, str(d)], cwd=root, env=env, stdout=subprocess.PIPE,
+                             stderr=subprocess.STDOUT, text=True)
+    try:
+        res = meanwhile()
+        out, _ = child.communicate(timeout=max(1.0, timeout - (time.monotonic() - t0)))
+    except subprocess.TimeoutExpired:
+        pytest.fail("%s did not finish within %d s" % (what, timeout))
+    finally:
+        if child.poll() is None:
+            child.kill()
+            child.communicate()
+    assert child.returncode == 0, out
+    return res, out, time.monotonic() - t0
 
 
 def has_gpu():
@@ -667,6 +695,27 @@ def check_wave_documents(s, names, part_off, part_id, rep_off, cur, out, out_len
     else:
         assert docs == [] and backs in (None, []) and len(doc_wave) == len(wave) == len(summ) == 0
     return got
+
+
+def summary_array(summ, dtype):
+    """A model's summary dicts as a structured array of `dtype`."""
+    return np.array([tuple(s[f] for f in dtype.names) for s in summ], dtype=dtype)
+
+
+def check_plan(s, rep_off, cur, out, out_len, B, weight=None, send_ids=None, C=None, rule="first_fit"):
+    """plan_waves under `rule` against its model (fit_models.plan_waves or models.plan_waves), every field; with C a sender
+    budget over send_ids. Returns (wave, summary, status)."""
+    s.set_wave_rule(rule)
+    send = {} if C is None else dict(max_broker_out=C, send_brokers=send_ids)
+    wave, summ, st = s.plan_waves(rep_off, cur, out, out_len, B, weight=weight, **send)
+    plan = fit_models.plan_waves if rule == "first_fit" else models.plan_waves
+    e_wave, e_summ, e_st = plan(rep_off, cur, out, out_len, s.broker_id, B, weight, None if C is None else (list(send_ids), C))
+    assert (st.code, st.a, st.b) == e_st, ((st.code, st.a, st.b), e_st)
+    if st.code == 0:
+        assert np.array_equal(wave, e_wave), np.nonzero(wave != e_wave)[0][:10]
+        names = (WAVE_SUMMARY_DTYPE if C is None else WAVE_SEND_SUMMARY_DTYPE).names
+        assert [record_of(x, names) for x in summ] == e_summ
+    return wave, summ, st
 
 
 def solved(cl, desired_rf=-1):
