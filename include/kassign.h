@@ -26,7 +26,10 @@ extern "C" {
 /* One ka_ctx == one `KafkaTopicAssigner` instance == one `KafkaAssignmentStrategy.Context`
  * (KTA:19-23, KAS:360-369): it owns the cross-topic leader-preference counters counter[broker][slot],
  * keyed by BROKER ID (so successive calls may use different broker sets, as the reference's tests do),
- * plus the device scratch. One in-flight call per ctx (the reference is single-threaded, KAS:361-368). */
+ * plus the device scratch. One in-flight call per ctx (the reference is single-threaded, KAS:361-368); different
+ * ctxs may be used at the same time, from different host threads, and may have asynchronous calls in flight at once.
+ * A call that takes a `stream` reads its device inputs, and writes its device outputs, in that stream's order: it sees
+ * whatever was enqueued on `stream` before it, and work enqueued on `stream` after it sees its outputs. */
 typedef struct ka_ctx ka_ctx;
 
 /* Error report. `code` > 0 are the reference's exceptions; `topic_index` is the LOWEST failing topic in
@@ -64,6 +67,8 @@ enum {
 
 /* `new KafkaTopicAssigner()` (KTA:21-23). device = CUDA ordinal. NULL if no CUDA device/driver. */
 ka_ctx* ka_ctx_create(int32_t device);
+/* Waits for a pending asynchronous call of the ctx (on the stream it was enqueued on, which must still exist), then frees
+ * the ctx. The call's outputs are complete in its stream's order. */
 void ka_ctx_destroy(ka_ctx* ctx);
 /* Drop all counters: a fresh Context (KAS:365-368). */
 int32_t ka_ctx_reset(ka_ctx* ctx);
@@ -134,7 +139,8 @@ int32_t ka_solve_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, const i
 /* Dense form on DEVICE buffers (d_* are device pointers on the ctx's device; d_out_len may be NULL),
  * enqueued on `stream` (a cudaStream_t, NULL = the legacy default stream) — inputs already resident in
  * HBM, outputs left in HBM. If st != NULL the call synchronises the stream and fills *st; with
- * st == NULL it is fully asynchronous and the status is fetched later with ka_last_status(). */
+ * st == NULL it is fully asynchronous and the status is fetched later with ka_last_status(); work enqueued on `stream`
+ * after the call may read the outputs without any host synchronisation. */
 int32_t ka_solve_dense_device(ka_ctx* ctx, int32_t T, const int32_t* d_topic_hash, int32_t P, int32_t RF,
                               const int32_t* d_cur_broker, int32_t desired_rf, int32_t out_stride,
                               int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st);

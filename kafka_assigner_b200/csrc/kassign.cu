@@ -18,6 +18,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <mutex>
 #include <new>
 #include <optional>
 #include <string>
@@ -393,9 +394,27 @@ int make_plan(int N, int blob_bytes, int64_t Q, int S, int Pmax, int64_t capmax,
     return KA_OK;
 }
 
+// A kernel's dynamic shared-memory cap belongs to the kernel on its device, not to a ka_ctx: every Context of the process
+// sets the same attribute, from any host thread. So the cap only ever rises, under one lock: lowering it to one Context's
+// size between another Context's raise and its launch would fail that launch. A cap is no reservation; a launch still gets
+// the shared memory it asks for, and occupancy follows from that.
+cudaError_t allow_smem_of(const void* kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> cap;   // (device, kernel) -> the cap set so far
+    int dev = 0;
+    const cudaError_t e = cudaGetDevice(&dev);
+    if (e != cudaSuccess) return e;
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& have = cap[{dev, kernel}];
+    if (bytes <= have) return cudaSuccess;
+    const cudaError_t r = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (r == cudaSuccess) have = bytes;
+    return r;
+}
+
 template <typename K>
 cudaError_t allow_smem(K kernel, size_t bytes) {
-    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    return allow_smem_of((const void*)kernel, bytes);
 }
 
 // A whole problem with its inputs on the device: dense (P partitions of RF replicas per topic), or ragged (d_part_off /
@@ -1397,7 +1416,7 @@ ka_ctx* ka_ctx_create(int32_t device) {
 
 void ka_ctx_destroy(ka_ctx* c) {
     if (!c) return;
-    cudaSetDevice(c->device);
+    enter(c, true);   // a pending asynchronous call still uses the buffers on the caller's stream: wait for it first
     for (cudaStream_t* s : c->streams())
         if (*s) cudaStreamSynchronize(*s);
     for_each_event(c, [](cudaEvent_t& e, bool) { if (e) cudaEventDestroy(e); });
