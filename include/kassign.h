@@ -90,6 +90,13 @@ int32_t ka_rack_indices(int32_t N, const int32_t* broker_id, const char* const* 
 /* java.lang.String.hashCode of a UTF-8 encoded topic name (UTF-16 code units, int32 wrap) — KAS:190. */
 int32_t ka_java_string_hash(const char* utf8);
 
+/* The name rule of every _json entry point: the device emitters copy topic names verbatim, so a name holding a character
+ * that org.json 20131018's JSONObject.quote() rewrites is refused (KA_ERR_BAD_ARG with a = that character's code point; take
+ * a host emitter instead). Over the len bytes of the UTF-8 name (NULs included), the first of: a byte below 0x20, '"', '\\'
+ * or '/' (org.json escapes '/' only after '<'; every '/' is refused); the UTF-8 form of U+0080..U+009F (C2 80 .. C2 9F) or
+ * of U+2000..U+20FF (E2 80 80 .. E2 83 BF). Returns its code point, or -1 when the name passes. Host only; needs no device. */
+int32_t ka_json_name_refused(const char* name, int64_t len);
+
 /* ---- the solve ----------------------------------------------------------------------------------
  * General (ragged) form, HOST buffers; copies in, runs the kernels, copies out, synchronises.
  *   T                topics, solved in index order through this ctx (KAG:173)
@@ -116,7 +123,8 @@ int32_t ka_solve_dense(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, int32_
 /* Dense solve + the reference's JSON emitter (KAG:169-186) in one call: the rows never leave the device, only the TEXT
  *   {"partitions":[{"partition":p,"replicas":[..],"topic":"name"},...],"version":1}
  * crosses PCIe, streamed block by block while later topic blocks are still being ordered. names = the T topic names
- * concatenated (UTF-8, none needing JSON escapes — else KA_ERR_BAD_ARG: use the host emitter), name_off[T+1] their offsets;
+ * concatenated (UTF-8; a name ka_json_name_refused refuses gives KA_ERR_BAD_ARG with a = the refused character's code
+ * point: use the host emitter), name_off[T+1] their offsets;
  * json = host buffer of json_cap bytes (pinned for full PCIe speed; KA_ERR_LIMIT if too small: 64 + sum over rows of
  * (50 + 12*out_stride + name length) always suffices); *json_bytes = length of the text (not NUL-terminated). */
 int32_t ka_solve_dense_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, int32_t P, int32_t RF,
@@ -128,9 +136,9 @@ int32_t ka_solve_dense_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, i
  * max(longest current list, desired_rf, 1). The text is cut into fragments of a fixed number of rows, each streamed out as
  * soon as it is built. json_cap = 64 + sum over rows of (50 + 12*stride + name length of the row's topic) always suffices
  * (it holds for any int32 partition id); KA_ERR_LIMIT if json_cap is too small. A run without rows (T == 0, or only empty
- * topics under a desired_rf) gives {"partitions":[],"version":1}. Names needing JSON escapes give KA_ERR_BAD_ARG before
- * anything is solved (counters untouched). On any error *json_bytes = 0 and *st is what ka_solve reports for the same
- * input; the ctx counters afterwards equal those after ka_solve. */
+ * topics under a desired_rf) gives {"partitions":[],"version":1}. A name ka_json_name_refused refuses gives KA_ERR_BAD_ARG
+ * with a = the refused character's code point before anything is solved (counters untouched). On any error *json_bytes = 0
+ * and *st is what ka_solve reports for the same input; the ctx counters afterwards equal those after ka_solve. */
 int32_t ka_solve_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, const int64_t* part_off, const int32_t* part_id,
                       const int64_t* rep_off, const int32_t* cur_broker, int32_t desired_rf,
                       const char* names, const int64_t* name_off, char* json, int64_t json_cap,
@@ -231,8 +239,8 @@ int32_t ka_solve_clusters(ka_ctx* ctx, int32_t K, const int32_t* cand_off, const
  * part_off / rep_off rebased to 0 and its names, desired_rf[k]) gives: topic_index counts from the cluster's first topic,
  * partition is mapped through part_id. A cluster without topics, or with only empty topics under a desired RF, gets
  * {"partitions":[],"version":1}. Per cluster, in ka_solve_json's order: the sizing scan and capacity checks of ka_solve_clusters;
- * a name that org.json would escape (KA_ERR_BAD_ARG, a = the byte); the 32-bit fragment limit of ka_solve_json; the cluster's
- * own plan; the five reference exceptions. A cluster that fails any of them has no text, and the others still solve.
+ * a name ka_json_name_refused refuses (KA_ERR_BAD_ARG, a = its code point); the 32-bit fragment limit of ka_solve_json; the
+ * cluster's own plan; the five reference exceptions. A cluster that fails any of them has no text, and the others still solve.
  * Stride: cluster k's width is max(longest current list, desired_rf[k], 1), and the call runs at the largest width among the
  * clusters it solves. The batched chains take rows of at most 3, so a cluster wider than 3 gets KA_ERR_LIMIT with a = its
  * width (the one difference from ka_solve_json, which solves widths 4..8 through its fused chain).
@@ -400,9 +408,9 @@ int32_t ka_ctx_wave_rule(ka_ctx* ctx);
  * Checks, in this order, before anything is enqueued: st NULL: KA_ERR_BAD_ARG (nothing written); ctx NULL: KA_ERR_NO_DEVICE;
  * everything ka_plan_waves checks, with its codes and operands (T < 0, or part_off NULL with T > 0, leaves no Q to check:
  * KA_ERR_BAD_ARG); then part_off not non-decreasing from 0, names or name_off NULL with T > 0, json NULL, json_cap < 0, or
- * doc_off NULL with Q > 0: KA_ERR_BAD_ARG; then a name org.json would escape: KA_ERR_BAD_ARG with a = the byte (take
- * ka_plan_waves and a host emitter instead). On the device the plan's own row errors come first, with the code, a and b of
- * ka_plan_waves; a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX). On any error *n_waves = 0 and
+ * doc_off NULL with Q > 0: KA_ERR_BAD_ARG; then a name ka_json_name_refused refuses: KA_ERR_BAD_ARG with a = the
+ * refused character's code point (take ka_plan_waves and a host emitter instead). On the device the plan's own row errors
+ * come first, with the code, a and b of ka_plan_waves; a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX). On any error *n_waves = 0 and
  * nothing else is specified.
  * Synchronous. The kernel launches it adds depend only on the bit length of W (one stable radix pass over the waves per 8
  * bits), not on Q or T. Follows the Context's wave rule (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the

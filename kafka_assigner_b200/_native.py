@@ -47,6 +47,7 @@ SYMBOLS = {
     "ka_ctx_set_brokers": (_i32, [_vp, _i32, _vp, _vp]),
     "ka_rack_indices": (_i32, [_i32, _vp, _vp, _vp]),
     "ka_java_string_hash": (_i32, [ctypes.c_char_p]),
+    "ka_json_name_refused": (_i32, [ctypes.c_char_p, _i64]),
     "ka_solve": (_i32, [_vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "ka_solve_dense": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp]),
     "ka_solve_dense_json": (_i32, [_vp, _i32, _vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, _i64, _vp, _vp]),

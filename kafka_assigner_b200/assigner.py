@@ -45,6 +45,10 @@ class KassignError(RuntimeError):
 
 
 def java_string_hash(s: str) -> int:
+    """String.hashCode of s (ka_java_string_hash). A name holding U+0000 is a ValueError: the C string would end there, and
+    the topic would be solved with the hash of its prefix."""
+    if "\0" in s:
+        raise ValueError("topic name %r holds U+0000" % s)
     return _native.load().ka_java_string_hash(s.encode("utf-8"))
 
 

@@ -1373,6 +1373,31 @@ int32_t ka_java_string_hash(const char* s) {
     return (int32_t)h;
 }
 
+// The bytes at which a character ka_json_name_refused refuses can start: one table lookup per byte of a name that passes.
+struct NameStops {
+    bool at[256];
+    constexpr NameStops() : at() {
+        for (int b = 0; b < 0x20; ++b) at[b] = true;
+        at[(int)'"'] = at[(int)'\\'] = at[(int)'/'] = at[0xC2] = at[0xE2] = true;
+    }
+};
+static constexpr NameStops kNameStops{};
+
+int32_t ka_json_name_refused(const char* name, int64_t len) {
+    // org.json 20131018 JSONObject.quote rewrites ", \, "</", chars below 0x20 and those in [0x80, 0xA0) and [0x2000, 0x2100);
+    // the device emitter copies names verbatim, so it refuses all of them, and every '/'
+    const unsigned char* u = reinterpret_cast<const unsigned char*>(name);
+    for (int64_t i = 0; i < len; ++i) {
+        const unsigned char b = u[i];
+        if (!kNameStops.at[b]) continue;
+        if (b < 0x20 || b == '"' || b == '\\' || b == '/') return b;
+        if (b == 0xC2 && i + 1 < len && u[i + 1] >= 0x80 && u[i + 1] < 0xA0) return u[i + 1];   // U+0080..U+009F
+        if (b == 0xE2 && i + 2 < len && u[i + 1] >= 0x80 && u[i + 1] < 0x84 && (u[i + 2] & 0xC0) == 0x80)
+            return 0x2000 | ((u[i + 1] & 0x3F) << 6) | (u[i + 2] & 0x3F);                     // U+2000..U+20FF
+    }
+    return -1;
+}
+
 int32_t ka_rack_indices(int32_t N, const int32_t* broker_id, const char* const* rack_name, int32_t* broker_rack) {
     if (N < 0 || (N > 0 && (!broker_id || !broker_rack))) return KA_ERR_BAD_ARG;
     // rack key = the rack string, or Integer.toString(id) when no rack is defined (KAS:81-86); brokers
@@ -1880,12 +1905,13 @@ static int prepare_json(ka_ctx* c, int32_t T, int64_t Q, const char* names, cons
     return KA_OK;
 }
 
-// The device emitter copies topic names verbatim: a name that org.json's quote() would escape is refused (KA_ERR_BAD_ARG,
-// a = the byte), and the caller takes the host emitter instead. Checks the name bytes names[b0 .. b1).
-static int check_names(const char* names, int64_t b0, int64_t b1, ka_status* st) {
-    for (int64_t i = b0; i < b1; ++i) {
-        const unsigned char ch = (unsigned char)names[i];
-        if (ch < 0x20 || ch == '"' || ch == '\\' || ch == '/') return set_status(st, KA_ERR_BAD_ARG, -1, -1, (int)ch);
+// The device emitter copies topic names verbatim: a name with a character ka_json_name_refused refuses is refused
+// (KA_ERR_BAD_ARG, a = that character's code point), and the caller takes the host emitter instead. Checks the names of
+// topics [t0, t1), each on its own.
+static int check_names(const char* names, const int64_t* name_off, int t0, int t1, ka_status* st) {
+    for (int t = t0; t < t1; ++t) {
+        const int32_t cp = ka_json_name_refused(names + name_off[t], name_off[t + 1] - name_off[t]);
+        if (cp >= 0) return set_status(st, KA_ERR_BAD_ARG, -1, -1, cp);
     }
     return KA_OK;
 }
@@ -1932,7 +1958,7 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     Shape sh = dense_shape(T, P, RF, desired_rf, S, c->br.N);
     if ((T > 0 && (!topic_hash || !names || !name_off)) || (sh.R > 0 && !cur_broker) || !json || json_cap < KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN)
         return set_status(st, KA_ERR_BAD_ARG);
-    if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
+    if ((rc = check_names(names, name_off, 0, T, st)) != KA_OK) return rc;
     if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
     // no topics or no brokers: no text to write, refused once its buffers are prepared
     return solve_json(c, sh, host_call(c, topic_hash, nullptr, nullptr, cur_broker, nullptr, nullptr), names, name_off, json, json_cap,
@@ -2066,7 +2092,7 @@ int32_t ka_solve_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, const int
     int rc = prepare_ragged(c, T, topic_hash, part_off, rep_off, cur_broker, desired_rf, 0, true, true, sh, st);
     if (rc != KA_OK) return rc;
     if ((T > 0 && (!names || !name_off)) || !json || json_cap < 0) return set_status(st, KA_ERR_BAD_ARG);
-    if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
+    if ((rc = check_names(names, name_off, 0, T, st)) != KA_OK) return rc;
     if ((rc = check_fragments(sh.Q, sh.S, longest_name(name_off, 0, T), st)) != KA_OK) return rc;
     if (c->d_part_id.reserve((size_t)std::max<int64_t>(sh.Q, 1) * 4) != cudaSuccess) return failed(st, KA_ERR_CUDA);
     return solve_json(c, sh, host_call(c, topic_hash, part_off, rep_off, cur_broker, nullptr, nullptr, part_id), names, name_off, json,
@@ -2191,7 +2217,7 @@ static int fleet_front(ka_ctx* c, int32_t K, const int32_t* cand_off, const int3
                         st + k, row0[k], rep0[k]) != KA_OK ||
             ragged_capmax(sc, mb.n, mb.capmax, st + k) != KA_OK)
             continue;
-        if (json && (check_names(names, mb.T > 0 ? name_off[t0] : 0, mb.T > 0 ? name_off[t0 + mb.T] : 0, st + k) != KA_OK ||
+        if (json && (check_names(names, name_off, t0, t0 + mb.T, st + k) != KA_OK ||
                      check_fragments(sc.Q, sc.S, longest_name(name_off, t0, t0 + mb.T), st + k) != KA_OK))
             continue;
         mb.Q = sc.Q;
@@ -2896,8 +2922,8 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
         bound += (part_off[t + 1] - part_off[t]) * (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + 50 + 12 * (int64_t)stride + name_off[t + 1] - name_off[t]);
         back_bound += (part_off[t + 1] - part_off[t]) * (KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN + 50 + name_off[t + 1] - name_off[t]);
     }
-    if ((rc = check_names(names, 0, T > 0 ? name_off[T] : 0, st)) != KA_OK) return rc;
-    if (sd && (rc = wave_send_args(*sd, summary_cap, st)) != KA_OK) return rc;
+    if ((rc = check_names(names, name_off, 0, T, st)) != KA_OK) return rc;
+    if (sd &&(rc = wave_send_args(*sd, summary_cap, st)) != KA_OK) return rc;
     if (pt && (pt->L < 1 || (Q > 0 && (!pt->doc_wave || !pt->n_docs)))) return set_status(st, KA_ERR_BAD_ARG);
     if (bk && (!bk->back || bk->cap < 0 || (Q > 0 && !bk->back_off))) return set_status(st, KA_ERR_BAD_ARG);
     if (doc_off) doc_off[0] = 0;

@@ -45,6 +45,13 @@ struct JParser {
     explicit JParser(const std::string& src) : s(src) {}
     [[noreturn]] void fail(const char* what) { throw std::runtime_error(std::string("snapshot JSON: ") + what + " at byte " + std::to_string(i)); }
     void ws() { while (i < s.size() && (s[i] == ' ' || s[i] == '\n' || s[i] == '\t' || s[i] == '\r')) ++i; }
+    // the four hex digits of a \u escape at i
+    unsigned hex4() {
+        if (i + 4 > s.size()) fail("bad \\u escape");
+        const unsigned cp = (unsigned)std::stoul(s.substr(i, 4), nullptr, 16);
+        i += 4;
+        return cp;
+    }
     JVal parse() {
         ws();
         if (i >= s.size()) fail("unexpected end");
@@ -92,12 +99,25 @@ struct JParser {
                     case 'b': v.str.push_back('\b'); break;
                     case 'f': v.str.push_back('\f'); break;
                     case 'u': {
-                        if (i + 4 > s.size()) fail("bad \\u escape");
-                        unsigned cp = (unsigned)std::stoul(s.substr(i, 4), nullptr, 16);
-                        i += 4;
+                        unsigned cp = hex4();
+                        // a high surrogate followed by a low one is one character (json.dumps writes every character above
+                        // U+FFFF so); a lone surrogate keeps its own 3-byte form, which ka_java_string_hash reads as that unit
+                        if (cp >= 0xD800 && cp < 0xDC00 && s.compare(i, 2, "\\u") == 0) {
+                            const size_t at = i;
+                            i += 2;
+                            const unsigned lo = hex4();
+                            if (lo >= 0xDC00 && lo < 0xE000) cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
+                            else i = at;
+                        }
                         if (cp < 0x80) v.str.push_back((char)cp);
                         else if (cp < 0x800) { v.str.push_back((char)(0xC0 | (cp >> 6))); v.str.push_back((char)(0x80 | (cp & 0x3F))); }
-                        else { v.str.push_back((char)(0xE0 | (cp >> 12))); v.str.push_back((char)(0x80 | ((cp >> 6) & 0x3F))); v.str.push_back((char)(0x80 | (cp & 0x3F))); }
+                        else if (cp < 0x10000) { v.str.push_back((char)(0xE0 | (cp >> 12))); v.str.push_back((char)(0x80 | ((cp >> 6) & 0x3F))); v.str.push_back((char)(0x80 | (cp & 0x3F))); }
+                        else {
+                            v.str.push_back((char)(0xF0 | (cp >> 18)));
+                            v.str.push_back((char)(0x80 | ((cp >> 12) & 0x3F)));
+                            v.str.push_back((char)(0x80 | ((cp >> 6) & 0x3F)));
+                            v.str.push_back((char)(0x80 | (cp & 0x3F)));
+                        }
                         break;
                     }
                     default: v.str.push_back(e);
@@ -146,6 +166,11 @@ Snapshot loadSnapshot(const std::string& path) {
     const std::string text = ss.str();
     JVal root = JParser(text).parse();
     Snapshot sn;
+    // String.hashCode of a topic is taken over a C string: a name with a NUL would be solved with the hash of its prefix
+    auto topicName = [](const JVal& t) -> const std::string& {
+        if (t.str.find('\0') != std::string::npos) throw std::runtime_error("snapshot JSON: a topic name holds \\u0000");
+        return t.str;
+    };
     if (const JVal* bs = root.get("brokers"))
         for (const JVal& b : bs->arr) {
             Broker br{};
@@ -163,7 +188,7 @@ Snapshot loadSnapshot(const std::string& path) {
         for (const JVal& p : ps->arr) {
             const JVal *t = p.get("topic"), *pi = p.get("partition"), *rs = p.get("replicas");
             if (!t || !pi || !rs) throw std::runtime_error("snapshot partition record needs topic/partition/replicas");
-            auto& asg = sn.assignment[t->str];
+            auto& asg = sn.assignment[topicName(*t)];
             if (sn.assignment.size() > sn.topics.size() && !root.get("topics")) sn.topics.push_back(t->str);  // first-seen order
             std::vector<int>& reps = asg[(int)pi->num];
             reps.clear();
@@ -171,7 +196,7 @@ Snapshot loadSnapshot(const std::string& path) {
         }
     if (const JVal* ts = root.get("topics")) {
         sn.topics.clear();
-        for (const JVal& t : ts->arr) sn.topics.push_back(t.str);
+        for (const JVal& t : ts->arr) sn.topics.push_back(topicName(t));
     }
     return sn;
 }

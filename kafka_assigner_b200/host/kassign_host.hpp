@@ -178,7 +178,7 @@ public:
 
     // solveClusters with every cluster's text built on the device (ka_solve_clusters_json): cluster k equals solveTopicsJson(its
     // topics, brokers, racks, desired RF) on a new KafkaTopicAssigner, with the exception it would throw as its status. The
-    // device call refuses clusters whose names org.json would escape or whose rows are wider than 3; those take
+    // device call refuses clusters with a name ka_json_name_refused refuses or whose rows are wider than 3; those take
     // solveTopicsJson on a new assigner instead. This instance's own Context is left alone.
     std::vector<ClusterJson> solveClustersJson(const std::vector<ClusterInput>& clusters) {
         const int K = (int)clusters.size();
@@ -313,7 +313,7 @@ public:
     }
 
     // planWaves with every wave's document built on the device (ka_plan_waves_json): docs[v] equals
-    // newAssignmentJson(planWaves(...).waves[v]). Topic names that org.json would escape take the host emitter instead.
+    // newAssignmentJson(planWaves(...).waves[v]). Topic names the device refuses (ka_json_name_refused) take the host emitter instead.
     struct WaveDocs {
         ka_status status;   // re-throw with throwForStatus; on an error summary and docs are empty
         std::vector<ka_wave_summary> summary;
@@ -336,7 +336,7 @@ public:
     // joins the current part while its document stays <= maxDocBytes, else it opens a new part. parts are in (wave, place in
     // the wave) order, partWave[d] the wave (1..W) of parts[d]; with maxDocBytes >= the longest wave document, parts equals
     // planWavesJson(...).docs. A partition whose one-record document exceeds maxDocBytes gives KA_ERR_LIMIT with a = its row
-    // and b = that length. Topic names that org.json would escape take the host emitter and the same cut on the host.
+    // and b = that length. Topic names the device refuses (ka_json_name_refused) take the host emitter and the same cut on the host.
     struct WaveParts {
         ka_status status;   // re-throw with throwForStatus; on an error summary, parts and partWave are empty
         std::vector<ka_wave_summary> summary;
@@ -359,7 +359,7 @@ public:
     // part d whatever else has run. A partition joins a part only while both its document and its rollback document stay <=
     // maxDocBytes; when no current list prints longer than its new one, parts and partWave are those of planWaveParts. A
     // partition whose one-record document on either side exceeds maxDocBytes gives KA_ERR_LIMIT with a = its row and b = the
-    // longer length. Topic names that org.json would escape take the host emitters and the same cut on the host.
+    // longer length. Topic names the device refuses (ka_json_name_refused) take the host emitters and the same cut on the host.
     struct WaveRollback {
         ka_status status;   // re-throw with throwForStatus; on an error summary, parts, rollback and partWave are empty
         std::vector<ka_wave_summary> summary;
@@ -480,8 +480,8 @@ private:
 public:
 
     // The KAG:172-186 loop and its "NEW ASSIGNMENT" text in one device call (ka_solve_json): only the text crosses PCIe.
-    // Same solve and exceptions as solveTopics; the text equals newAssignmentJson(solveTopics(...)). Topic names that
-    // org.json would escape take that host emitter instead.
+    // Same solve and exceptions as solveTopics; the text equals newAssignmentJson(solveTopics(...)). Topic names the
+    // device refuses (ka_json_name_refused) take that host emitter instead.
     std::string solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
                                 const std::map<int, std::string>& rackAssignment, int desiredReplicationFactor);
     // solveTopicsJson with the exception it would throw as `st` instead (the text is empty then).
@@ -549,6 +549,9 @@ private:
         int maxLen = 0;
         for (int t = 0; t < T; ++t) {
             f.names[t] = topics[t].name;
+            // the hash reads a C string: a NUL would leave it the hash of the name's prefix
+            if (topics[t].name.find('\0') != std::string::npos)
+                throw std::invalid_argument("topic " + std::to_string(t) + "'s name holds U+0000");
             f.hash[t] = ka_java_string_hash(topics[t].name.c_str());
             for (const auto& e : topics[t].current) {  // std::map: ascending partition == TreeMap order (KAS:107-110)
                 f.partId.push_back(e.first);
@@ -695,27 +698,47 @@ inline void appendInt(std::string& s, long long v) {
     while (n) s.push_back(buf[--n]);
 }
 
-// org.json JSONObject.quote(): escapes ", \, control chars and "</" (Kafka topic names never need it).
-inline void appendQuoted(std::string& s, const std::string& v) {
+// The quote of a UTF-8 string: escapes ", \, control chars and "</" (Kafka topic names never need it); with `wide`, also the
+// chars org.json 20131018 JSONObject.quote() writes as \u plus four lowercase hex digits above ASCII: U+0080..U+009F and
+// U+2000..U+20FF, whose UTF-8 forms ka_json_name_refused refuses. Every other byte is copied.
+inline void appendQuotedAs(std::string& s, const std::string& v, bool wide) {
+    static const char* hx = "0123456789abcdef";
+    auto hex4 = [&](unsigned cp) { s += "\\u"; for (int k = 12; k >= 0; k -= 4) s.push_back(hx[(cp >> k) & 15]); };
     s.push_back('"');
     char prev = 0;
-    for (unsigned char c : v) {
-        switch (c) {
-        case '\\': case '"': s.push_back('\\'); s.push_back((char)c); break;
-        case '/': if (prev == '<') s.push_back('\\'); s.push_back('/'); break;
-        case '\b': s += "\\b"; break;
-        case '\t': s += "\\t"; break;
-        case '\n': s += "\\n"; break;
-        case '\f': s += "\\f"; break;
-        case '\r': s += "\\r"; break;
-        default:
-            if (c < 0x20) { static const char* hx = "0123456789abcdef"; s += "\\u00"; s.push_back(hx[c >> 4]); s.push_back(hx[c & 15]); }
-            else s.push_back((char)c);
+    for (size_t i = 0; i < v.size(); ++i) {
+        const unsigned char c = (unsigned char)v[i];
+        const unsigned char c1 = i + 1 < v.size() ? (unsigned char)v[i + 1] : 0, c2 = i + 2 < v.size() ? (unsigned char)v[i + 2] : 0;
+        if (wide && c == 0xC2 && c1 >= 0x80 && c1 < 0xA0) {
+            hex4(c1);
+            ++i;
+        } else if (wide && c == 0xE2 && c1 >= 0x80 && c1 < 0x84 && (c2 & 0xC0) == 0x80) {
+            hex4(0x2000 | ((c1 & 0x3F) << 6) | (c2 & 0x3F));
+            i += 2;
+        } else {
+            switch (c) {
+            case '\\': case '"': s.push_back('\\'); s.push_back((char)c); break;
+            case '/': if (prev == '<') s.push_back('\\'); s.push_back('/'); break;
+            case '\b': s += "\\b"; break;
+            case '\t': s += "\\t"; break;
+            case '\n': s += "\\n"; break;
+            case '\f': s += "\\f"; break;
+            case '\r': s += "\\r"; break;
+            default:
+                if (c < 0x20) hex4(c);
+                else s.push_back((char)c);
+            }
         }
         prev = (char)c;
     }
     s.push_back('"');
 }
+
+// org.json JSONObject.quote(), for the records of KafkaAssignmentGenerator and the rack and host names of the broker list.
+inline void appendQuoted(std::string& s, const std::string& v) { appendQuotedAs(s, v, true); }
+
+// The quote of the CURRENT ASSIGNMENT and rollback records (Kafka's own encoder, not org.json): only the ASCII rewrites.
+inline void appendKafkaQuoted(std::string& s, const std::string& v) { appendQuotedAs(s, v, false); }
 
 // Key order of org.json 20131018 objects == java.util.HashMap iteration order of the keys (SURVEY §3.4; predicted for
 // JDK >= 8, unverified without a JVM — isolated here so it can be corrected in one place):
@@ -737,7 +760,7 @@ inline void appendRecord(std::string& s, const std::string& topic, int partition
 // scala Map literals keep insertion order for <= 4 entries: topic, partition, replicas.
 inline void appendCurrentRecord(std::string& s, const std::string& topic, int partition, const int* replicas, size_t n) {
     s += "{\"topic\":";
-    appendQuoted(s, topic);
+    appendKafkaQuoted(s, topic);
     s += ",\"partition\":";
     appendInt(s, partition);
     s += ",\"replicas\":[";
@@ -761,12 +784,9 @@ inline std::string newAssignmentJson(const std::vector<TopicOutput>& topics) {
     return s;
 }
 
-// Bytes org.json's JSONObject.quote() may rewrite: the device emitter copies names verbatim and refuses these.
-inline bool needsJsonEscape(const std::string& name) {
-    for (unsigned char c : name)
-        if (c < 0x20 || c == '"' || c == '\\' || c == '/') return true;
-    return false;
-}
+// A name the device emitters refuse (ka_json_name_refused: a character org.json's JSONObject.quote() may rewrite, or '/'):
+// such names take the host emitter, appendQuoted.
+inline bool needsJsonEscape(const std::string& name) { return ka_json_name_refused(name.data(), (int64_t)name.size()) >= 0; }
 
 inline std::string KafkaTopicAssigner::solveTopicsJson(const std::vector<TopicInput>& topics, const std::set<int>& brokers,
                                                        const std::map<int, std::string>& rackAssignment,

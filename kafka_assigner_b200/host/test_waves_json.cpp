@@ -1,11 +1,12 @@
 // test_waves_json.cpp — KafkaTopicAssigner::planWavesJson over the rows of solveTopics: every document built on the device equals
 // newAssignmentJson of the same wave of planWaves, byte for byte, with the same summaries, unit and weighted; topic names that
-// org.json escapes take the host emitter and give the same text; a refused proposal carries its status. Needs a GPU (kassign has
-// no CPU fallback). Exit code 0 = all passed.
+// org.json escapes take the host emitter and give the same text (with argv[1], a file of such names and their quotes, every one of
+// them); a refused proposal carries its status. Needs a GPU (kassign has no CPU fallback). Exit code 0 = all passed.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <fstream>
 
 #include "kassign_host.hpp"
 
@@ -52,7 +53,13 @@ static void compare(KafkaTopicAssigner& a, const std::vector<TopicInput>& topics
     }
 }
 
-int main() {
+static std::string unhex(const std::string& h) {
+    std::string s;
+    for (size_t i = 0; i + 1 < h.size(); i += 2) s.push_back((char)std::stoi(h.substr(i, 2), nullptr, 16));
+    return s;
+}
+
+int main(int argc, char** argv) {
     std::vector<TopicInput> topics = makeTopics(7, 400, 30, 12);
     std::set<int> brokers;
     std::map<int, std::string> racks;
@@ -76,6 +83,36 @@ int main() {
     compare(a, odd, oddProposed, 2, {});
     const KafkaTopicAssigner::WaveDocs escaped = a.planWavesJson(odd, oddProposed, 1000000);
     CHECK(escaped.docs.size() == 1 && escaped.docs[0].find("\"a\\\"b<\\/c\\\\d\"") != std::string::npos);
+
+    // argv[1]: a file of names the device refuses, one per line as "<hex of the name's UTF-8> <hex of its org.json quote>": each
+    // takes the host emitter, and every record of its topic prints that quote
+    if (argc > 1) {
+        std::ifstream in(argv[1]);
+        std::string nameHex, quoteHex;
+        int n = 0;
+        while (in >> nameHex >> quoteHex) {
+            odd[5].name = oddProposed[5].name = unhex(nameHex);
+            CHECK(kassign::needsJsonEscape(odd[5].name));
+            compare(a, odd, oddProposed, 2, {});
+            const KafkaTopicAssigner::WaveDocs one = a.planWavesJson(odd, oddProposed, 1000000);
+            const std::string rec = ",\"topic\":" + unhex(quoteHex) + "}";
+            size_t hits = 0;
+            for (size_t at = one.docs.empty() ? std::string::npos : one.docs[0].find(rec); at != std::string::npos;
+                 at = one.docs[0].find(rec, at + 1))
+                ++hits;
+            size_t moved = 0;
+            for (const auto& e : oddProposed[5].assignment) moved += e.second != odd[5].current.at(e.first);
+            CHECK(one.status.code == KA_OK && one.docs.size() == 1 && moved > 0 && hits == moved);
+            ++n;
+        }
+        CHECK(n > 0);
+    }
+    // a NUL in a name would cut its hash short: refused before anything runs
+    std::vector<TopicInput> nul = topics;
+    nul[3].name = std::string("t\0x", 3);
+    bool threw = false;
+    try { a.planWavesJson(nul, proposed, 2); } catch (const std::invalid_argument&) { threw = true; }
+    CHECK(threw);
 
     // nothing changed: no document
     std::vector<TopicOutput> same;

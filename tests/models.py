@@ -202,9 +202,49 @@ def crossing_chunk(records, senders, rounds):
 # The records of KafkaAssignmentGenerator.java:169-186 in the predicted org.json key order (SURVEY §3.4): "partition",
 # "replicas", "topic" inside {"partitions":[...],"version":1}.
 
+_SHORT = {"\b": "\\b", "\t": "\\t", "\n": "\\n", "\f": "\\f", "\r": "\\r", '"': '\\"', "\\": "\\\\"}
+
+
+def _quote(name, wide):
+    """org.json 20131018 JSONObject.quote() over the UTF-16 code units of `name`: '"' and '\\' escaped, '/' only right after
+    '<', \\b \\t \\n \\f \\r short, every other unit below 0x20 (and with `wide` every unit in [0x80, 0xA0) or [0x2000, 0x2100))
+    as \\u plus four lowercase hex digits; the rest kept. No escaped unit is a surrogate, so walking the code points of `name`
+    visits the same units: a char above U+FFFF (two surrogates) is kept whole and is never the '<' before a '/'."""
+    out, prev = [], ""
+    for ch in name:
+        c = ord(ch)
+        if ch in _SHORT:
+            out.append(_SHORT[ch])
+        elif ch == "/":
+            out.append("\\/" if prev == "<" else "/")
+        elif c < 0x20 or (wide and (0x80 <= c < 0xA0 or 0x2000 <= c < 0x2100)):
+            out.append("\\u%04x" % c)
+        else:
+            out.append(ch)
+        prev = ch
+    return '"' + "".join(out) + '"'
+
+
 def quote(name):
-    """org.json JSONObject.quote() for the names these tests use."""
-    return '"' + name.replace("\\", "\\\\").replace('"', '\\"') + '"'
+    """org.json 20131018 JSONObject.quote() of a topic name (the records of the reassignment JSON): the ASCII escapes, and
+    every char in [0x80, 0xA0) or [0x2000, 0x2100) as \\u%04x. U+007F and U+00A0 are kept; "" gives '""'."""
+    return _quote(name, True)
+
+
+def kafka_quote(name):
+    """The quote of the CURRENT ASSIGNMENT and rollback records (Kafka's own encoder, not org.json): the ASCII escapes of quote
+    only; every char above 0x7F is kept."""
+    return _quote(name, False)
+
+
+def device_refuses(name):
+    """(char, a) of the first char of `name` the device emitters refuse (ka_json_name_refused), a its code point, or None:
+    a char quote() rewrites, or '/' (quote() escapes it only after '<'; the device refuses every one)."""
+    for ch in name:
+        c = ord(ch)
+        if c < 0x20 or ch in '"\\/' or 0x80 <= c < 0xA0 or 0x2000 <= c < 0x2100:
+            return ch, c
+    return None
 
 
 def record(name, partition, replicas):
@@ -219,7 +259,7 @@ def document(records):
 def current_record(name, partition, replicas):
     """The rollback record: the host's CURRENT ASSIGNMENT record (Kafka 0.10 ZkUtils.formatAsReassignmentJson key order) of a
     partition on its current list `replicas`, printed as given."""
-    return '{"topic":%s,"partition":%d,"replicas":[%s]}' % (quote(name), partition, ",".join(str(int(b)) for b in replicas))
+    return '{"topic":%s,"partition":%d,"replicas":[%s]}' % (kafka_quote(name), partition, ",".join(str(int(b)) for b in replicas))
 
 
 def rollback_document(records):

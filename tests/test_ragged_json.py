@@ -209,7 +209,7 @@ def _cli_expected(oracle, cl, topics, live, desired):
     racks = dict(zip(cl.all_broker_id.tolist(), cl.all_rack_name))
     new, st = util.oracle_text(oracle, names, part_off, part_id, rep_off, cur, live, [racks[b] for b in live], desired)
     assert st.code == 0
-    current = ",".join('{"topic":%s,"partition":%d,"replicas":[%s]}' % (models.quote(n), p, ",".join(map(str, asg[p])))
+    current = ",".join('{"topic":%s,"partition":%d,"replicas":[%s]}' % (models.kafka_quote(n), p, ",".join(map(str, asg[p])))
                        for n, asg in topics for p in sorted(asg))
     return "CURRENT ASSIGNMENT:\n" + '{"version":1,"partitions":[' + current + ']}' + "\nNEW ASSIGNMENT:\n" + new + "\n"
 
