@@ -666,6 +666,7 @@ int32_t ka_order_device(ka_ctx* ctx, int32_t* d_out_len, int32_t* d_out_broker, 
  *   ka_staged_slot_chains()   2 if the staged block is ordered by per-slot chains (all rows <= 3), else 0 (use ka_order_device)
  *   ka_order_slot_device()    the slot-0 (slot = 0) or slot-1 (slot = 1) chain of the staged block; slot 1 after slot 0
  *   ka_emit_device()          ordered records -> d_out_broker / d_out_len, adds counter[.][2]; ends the staged solve
+ *                             (d_out_broker may be NULL only when the staged block has no rows; else KA_ERR_BAD_ARG)
  *   ka_ctx_{export,import}_counter_slot_device()  one counter column, d_column = N int32 on the device
  * ka_order_device == slot 0 (internal stream) overlapped with slot 1 + emit, sub-block by sub-block. */
 int32_t ka_staged_slot_chains(ka_ctx* ctx);

@@ -1832,7 +1832,7 @@ int32_t ka_order_slot_device(ka_ctx* c, int32_t slot, void* stream) {
 int32_t ka_emit_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
     int rc = enter_staged(c, true, st);
     if (rc != KA_OK) return rc;
-    if (!d_out_broker) return set_status(st, KA_ERR_BAD_ARG);
+    if (!d_out_broker && c->staged_block.Q > 0) return set_status(st, KA_ERR_BAD_ARG);   // a block without rows writes none
     cudaStream_t s = (cudaStream_t)stream;
     if ((rc = enq_emit_block(c, s, c->staged_block, 0, 1, d_out_broker, d_out_len)) != KA_OK) return failed(st, rc);
     return end_staged(c, s, st);

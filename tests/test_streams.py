@@ -30,8 +30,6 @@ from tests import fit_models, models, usage_models, util
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "kafka_assigner_b200", "csrc")
 
-# About 0.1 s at the H100's 1.98 GHz SM clock: far longer than the host's enqueue of any call here (checked per call).
-SLEEP_CYCLES = 200_000_000
 LEGACY = "legacy"     # the legacy default stream, passed to the library as 0
 SIDE = "side"         # a torch.cuda.Stream of its own
 
@@ -77,14 +75,11 @@ def _dev(a):
 def late_inputs(stream, pairs):
     """On `stream`: a device sleep, then dst.copy_(src) for every (dst, src). Returns the sleep's (start, end) events."""
     import torch
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    sleep = util.device_sleep(stream)
     with torch.cuda.stream(stream):
-        a.record()
-        torch.cuda._sleep(SLEEP_CYCLES)
-        b.record()
         for dst, src in pairs:
             dst.copy_(src, non_blocking=True)
-    return a, b
+    return sleep
 
 
 def early_read(stream, *tensors):
@@ -94,13 +89,6 @@ def early_read(stream, *tensors):
         got = [t.clone() for t in tensors]
     stream.synchronize()
     return [g.cpu().numpy() for g in got]
-
-
-def enqueued_behind(sleep, t_call):
-    """The call was enqueued (t_call seconds on the host) well inside the sleep ahead of its inputs."""
-    ms = sleep[0].elapsed_time(sleep[1])
-    print("device sleep %.1f ms, host enqueue %.3f ms" % (ms, 1e3 * t_call))
-    assert 1e3 * t_call < ms / 2, ("the call's enqueue outlasted half the sleep: the test would not see an early read", t_call, ms)
 
 
 def decoy_of(cl):
@@ -214,7 +202,7 @@ def test_dense_device_solve_follows_the_stream(native_lib, oracle, case, kind):
         s.solve_dense_device(*p.solve_args(), stream=h, sync=False)
         t_call = time.perf_counter() - t0
         out, ln = early_read(stream, p.d_out, p.d_len)
-    enqueued_behind(sleep, t_call)
+    util.enqueued_behind(sleep, t_call)
     assert util.fields(s.last_status()) == exp[2]
     got_plan = s.last_order_plan()
     assert (got_plan[0], got_plan[1], got_plan[6]) == plan, (cid, got_plan)
@@ -288,7 +276,7 @@ def test_staged_slot_chains_on_one_stream(native_lib, oracle):
     s.export_counter_slot_device(2, got[2].data_ptr(), stream=h)
     t_call = time.perf_counter() - t0
     out, ln, c0, c1, c2 = early_read(stream, p.d_out, p.d_len, *got)
-    enqueued_behind(sleep, t_call)
+    util.enqueued_behind(sleep, t_call)
     assert util.fields(s.last_status()) == exp_st
     check_rows(out, ln, (exp_out, exp_ln), "staged-slots")
     for slot, c in enumerate((c0, c1, c2)):
@@ -314,7 +302,7 @@ def test_staged_slot_chains_back_to_back(native_lib, oracle):
     s.emit_device(p.d_len.data_ptr(), p.d_out.data_ptr(), stream=h, sync=False)
     t_call = time.perf_counter() - t0
     out, ln = early_read(stream, p.d_out, p.d_len)
-    enqueued_behind(sleep, t_call)
+    util.enqueued_behind(sleep, t_call)
     assert util.fields(s.last_status()) == exp[2]
     check_rows(out, ln, exp, "back-to-back")
     assert np.array_equal(s.counters(), exp[3])
@@ -346,7 +334,7 @@ def test_staged_order_with_device_counters(native_lib, oracle, RF):
     s.export_counters_device(d_exp.data_ptr(), stream=h)
     t_call = time.perf_counter() - t0
     out, ln, got_ctr = early_read(stream, p.d_out, p.d_len, d_exp)
-    enqueued_behind(sleep, t_call)
+    util.enqueued_behind(sleep, t_call)
     assert util.fields(s.last_status()) == exp_st
     assert s.last_order_plan()[0] == (3 if RF == 3 else 4)
     check_rows(out, ln, (exp_out, exp_ln), ("staged-order", RF))
@@ -378,7 +366,7 @@ def test_two_contexts_in_flight_on_one_stream(native_lib, oracle, failing_first)
         s.solve_dense_device(*p.solve_args(), stream=h, sync=False)
     t_call = time.perf_counter() - t0
     out, ln = early_read(stream, good.d_out, good.d_len)
-    enqueued_behind(sleep, t_call)
+    util.enqueued_behind(sleep, t_call)
     assert util.fields(s_bad.last_status()) == bad_exp[2]
     assert util.fields(s_good.last_status()) == exp[2]
     check_rows(out, ln, exp, "good")
@@ -403,7 +391,7 @@ def test_destroy_waits_for_the_pending_call(native_lib, oracle):
     t_call = time.perf_counter() - t0
     s.close()
     out, ln = early_read(stream, p.d_out, p.d_len)
-    enqueued_behind(sleep, t_call)
+    util.enqueued_behind(sleep, t_call)
     check_rows(out, ln, exp, "destroy")
 
 

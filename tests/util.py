@@ -146,6 +146,30 @@ def has_gpu():
         return False
 
 
+# ---- work held behind a device sleep -------------------------------------------------------------------------------------
+
+# About 0.1 s at the H100's 1.98 GHz SM clock: far longer than the host's enqueue of any call the tests hold behind it.
+SLEEP_CYCLES = 200_000_000
+
+
+def device_sleep(stream, cycles=SLEEP_CYCLES):
+    """A device sleep on `stream`, enqueued at once. Returns its (start, end) events."""
+    import torch
+    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    with torch.cuda.stream(stream):
+        a.record()
+        torch.cuda._sleep(cycles)
+        b.record()
+    return a, b
+
+
+def enqueued_behind(sleep, t_call):
+    """The call was enqueued (t_call seconds on the host) well inside the sleep ahead of its inputs."""
+    ms = sleep[0].elapsed_time(sleep[1])
+    print("device sleep %.1f ms, host enqueue %.3f ms" % (ms, 1e3 * t_call))
+    assert 1e3 * t_call < ms / 2, ("the call's enqueue outlasted half the sleep: the test would not see an early read", t_call, ms)
+
+
 # ---- fakes of the library ------------------------------------------------------------------------------------------------
 
 def view(p, n, ctype):
