@@ -29,7 +29,12 @@ extern "C" {
  * plus the device scratch. One in-flight call per ctx (the reference is single-threaded, KAS:361-368); different
  * ctxs may be used at the same time, from different host threads, and may have asynchronous calls in flight at once.
  * A call that takes a `stream` reads its device inputs, and writes its device outputs, in that stream's order: it sees
- * whatever was enqueued on `stream` before it, and work enqueued on `stream` after it sees its outputs. */
+ * whatever was enqueued on `stream` before it, and work enqueued on `stream` after it sees its outputs.
+ * A host call sees every earlier call of the same ctx: ka_ctx_get_counters, ka_ctx_set_counters, ka_ctx_reset,
+ * ka_ctx_set_brokers, the host-buffer solves (ka_solve, ka_solve_dense and their _json forms), ka_last_status and
+ * ka_ctx_destroy first wait on the host for the ctx's earlier asynchronous calls to finish on their streams, so a read sees
+ * what they wrote and a write cannot reach what they still read. This rule adds no host wait to the calls that take a
+ * `stream`. */
 typedef struct ka_ctx ka_ctx;
 
 /* Error report. `code` > 0 are the reference's exceptions; `topic_index` is the LOWEST failing topic in

@@ -184,6 +184,10 @@ struct ka_ctx {
     cudaEvent_t ev_in = nullptr, ev_stage[KA_MAX_BLOCKS] = {}, ev_chain_in = nullptr, ev_b1[KA_MAX_CHAIN_EVENTS] = {};
     cudaEvent_t ev_b2[KA_MAX_CHAIN_EVENTS] = {}, ev_emit_done = nullptr;
     cudaEvent_t ev_json_in[KA_MAX_JSON_FRAGS] = {}, ev_json_scan[KA_MAX_JSON_FRAGS] = {}, ev_out_done = nullptr;
+    // end of the last asynchronous call that leaves no status pending (stage, slot chain, counter import / export), recorded on
+    // its stream; the next host call waits for it (enter_host)
+    cudaEvent_t ev_tail = nullptr;
+    bool tail_pending = false;
     // timing of the last solve
     bool timing = false;
     float last_ms[8] = {};
@@ -251,6 +255,7 @@ void for_each_event(ka_ctx* c, F f) {
         {c->ev_json_in, KA_MAX_JSON_FRAGS, false},
         {c->ev_json_scan, KA_MAX_JSON_FRAGS, false},
         {&c->ev_out_done, 1, false},
+        {&c->ev_tail, 1, false},
     };
     for (const auto& p : pools)
         for (size_t i = 0; i < p.n; ++i) f(p.e[i], p.timed);
@@ -1159,6 +1164,30 @@ int enter(ka_ctx* c, bool collect) {
     return KA_OK;
 }
 
+// Wait for the last asynchronous call that left no status pending (end_untracked).
+int wait_untracked(ka_ctx* c) {
+    if (!c->tail_pending) return KA_OK;
+    KA_CUDA(cudaEventSynchronize(c->ev_tail));
+    c->tail_pending = false;
+    return KA_OK;
+}
+
+// Prologue of a host call, whose work runs on the ctx's own streams, the legacy stream or the host, none of which is ordered
+// after the caller's stream: enter(c, true), then wait_untracked. So the host call sees every earlier call of the ctx, and
+// nothing it writes reaches what such a call still has to read.
+int enter_host(ka_ctx* c) {
+    const int rc = enter(c, true);
+    return rc != KA_OK ? rc : wait_untracked(c);
+}
+
+// End of an asynchronous call that leaves no status pending, its work enqueued on `s`: recorded there for the next host call
+// to wait for. The call itself does not wait.
+int end_untracked(ka_ctx* c, cudaStream_t s) {
+    KA_CUDA(cudaEventRecord(c->ev_tail, s));
+    c->tail_pending = true;
+    return KA_OK;
+}
+
 // Everything of a solve is enqueued on `s`: its status is pending until ka_last_status, or collected now when the caller
 // asked for it (st) or the entry point is synchronous.
 int finish(ka_ctx* c, cudaStream_t s, ka_status* st, bool sync, const int32_t* part_id = nullptr, const int64_t* part_off = nullptr) {
@@ -1441,7 +1470,7 @@ ka_ctx* ka_ctx_create(int32_t device) {
 
 void ka_ctx_destroy(ka_ctx* c) {
     if (!c) return;
-    enter(c, true);   // a pending asynchronous call still uses the buffers on the caller's stream: wait for it first
+    enter_host(c);   // a pending asynchronous call still uses the buffers on the caller's stream: wait for it first
     for (cudaStream_t* s : c->streams())
         if (*s) cudaStreamSynchronize(*s);
     for_each_event(c, [](cudaEvent_t& e, bool) { if (e) cudaEventDestroy(e); });
@@ -1454,7 +1483,7 @@ void ka_ctx_destroy(ka_ctx* c) {
 
 int32_t ka_ctx_reset(ka_ctx* c) {
     if (!c) return KA_ERR_NO_DEVICE;
-    int rc = enter(c, true);   // do not race an in-flight asynchronous solve
+    int rc = enter_host(c);   // do not race an in-flight asynchronous call
     if (rc != KA_OK) return rc;
     c->parked.clear();
     if (c->br.N > 0 && c->d_ctr8.p) KA_CUDA(cudaMemset(c->d_ctr8.p, 0, (size_t)c->br.N * KA_MAX_SLOTS * 4));
@@ -1465,7 +1494,7 @@ int32_t ka_ctx_set_brokers(ka_ctx* c, int32_t N, const int32_t* broker_id, const
     if (!c) return KA_ERR_NO_DEVICE;
     int rc = check_brokers(N, broker_id, broker_rack);
     if (rc != KA_OK) return rc;
-    if ((rc = enter(c, true)) != KA_OK || (rc = park_counters(c)) != KA_OK) return rc;
+    if ((rc = enter_host(c)) != KA_OK || (rc = park_counters(c)) != KA_OK) return rc;
 
     const BrokerTable t = broker_table(N, broker_id, broker_rack);
     if (t.lut_mode == KA_LUT_GLOBAL) {
@@ -1494,7 +1523,7 @@ int32_t ka_ctx_counter_slots(ka_ctx*) { return KA_MAX_SLOTS; }
 int32_t ka_ctx_get_counters(ka_ctx* c, int32_t* counter) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!counter) return KA_ERR_BAD_ARG;
-    int rc = enter(c, true);
+    int rc = enter_host(c);
     if (rc != KA_OK) return rc;
     if (c->br.N > 0) KA_CUDA(cudaMemcpy(counter, c->d_ctr8.p, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToHost));
     return KA_OK;
@@ -1503,7 +1532,7 @@ int32_t ka_ctx_get_counters(ka_ctx* c, int32_t* counter) {
 int32_t ka_ctx_set_counters(ka_ctx* c, const int32_t* counter) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!counter) return KA_ERR_BAD_ARG;
-    int rc = enter(c, true);
+    int rc = enter_host(c);
     if (rc != KA_OK) return rc;
     if (c->br.N > 0) KA_CUDA(cudaMemcpy(c->d_ctr8.p, counter, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyHostToDevice));
     return KA_OK;
@@ -1516,7 +1545,7 @@ int32_t ka_ctx_export_counters_device(ka_ctx* c, int32_t* d_counter, void* strea
     if (rc != KA_OK) return rc;
     if (c->br.N > 0)
         KA_CUDA(cudaMemcpyAsync(d_counter, c->d_ctr8.p, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-    return KA_OK;
+    return end_untracked(c, (cudaStream_t)stream);
 }
 
 int32_t ka_ctx_import_counters_device(ka_ctx* c, const int32_t* d_counter, void* stream) {
@@ -1526,7 +1555,7 @@ int32_t ka_ctx_import_counters_device(ka_ctx* c, const int32_t* d_counter, void*
     if (rc != KA_OK) return rc;
     if (c->br.N > 0)
         KA_CUDA(cudaMemcpyAsync(c->d_ctr8.p, d_counter, (size_t)c->br.N * KA_MAX_SLOTS * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-    return KA_OK;
+    return end_untracked(c, (cudaStream_t)stream);
 }
 
 int32_t ka_ctx_set_timing(ka_ctx* c, int32_t enabled) {
@@ -1568,7 +1597,7 @@ int32_t ka_ctx_last_stage_plan(ka_ctx* c, int32_t* plan) {
 int32_t ka_last_status(ka_ctx* c, ka_status* st) {
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     int rc = enter(c, false);
-    if (rc != KA_OK) return set_status(st, rc);
+    if (rc != KA_OK || (rc = wait_untracked(c)) != KA_OK) return set_status(st, rc);
     if (c->pending_status) return finish_status(c, c->last_stream, st);
     if (st) *st = c->last;
     return c->last.code;
@@ -1774,7 +1803,7 @@ int32_t ka_stage_dense_device(ka_ctx* c, int32_t T, const int32_t* d_topic_hash,
     if ((rc = reset_flags(c, s)) != KA_OK || (rc = enq_stage(c, s, d, c->ev[2])) != KA_OK) return rc;
     if (c->timing) cudaEventRecord(c->ev[3], s);   // end of the stage (the chains may wait for another rank after this)
     c->staged = true;
-    return KA_OK;
+    return end_untracked(c, s);
 }
 
 // Prologue of the calls that finish the staged block: st cleared, the ctx, its device made current, then a staged block
@@ -1826,7 +1855,7 @@ int32_t ka_order_slot_device(ka_ctx* c, int32_t slot, void* stream) {
         if ((rc = enq_slot_chain(c, s, d, slot, j, nsub)) != KA_OK) return rc;
     if (c->timing) cudaEventRecord(c->ev_chain[slot][1], s);
     c->slot_timed[slot] = c->timing;
-    return KA_OK;
+    return end_untracked(c, s);
 }
 
 int32_t ka_emit_device(ka_ctx* c, int32_t* d_out_len, int32_t* d_out_broker, void* stream, ka_status* st) {
@@ -1847,7 +1876,7 @@ static int copy_counter_column(ka_ctx* c, int slot, int32_t* d_col, const int32_
     int32_t* col = c->d_ctr8.as<int32_t>() + slot;
     if (d_col) KA_CUDA(cudaMemcpy2DAsync(d_col, 4, col, KA_MAX_SLOTS * 4, 4, (size_t)c->br.N, cudaMemcpyDeviceToDevice, s));
     else KA_CUDA(cudaMemcpy2DAsync(col, KA_MAX_SLOTS * 4, d_src, 4, 4, (size_t)c->br.N, cudaMemcpyDeviceToDevice, s));
-    return KA_OK;
+    return end_untracked(c, s);
 }
 
 int32_t ka_ctx_export_counter_slot_device(ka_ctx* c, int32_t slot, int32_t* d_column, void* stream) {
@@ -1870,7 +1899,7 @@ int32_t ka_solve_dense(ka_ctx* c, int32_t T, const int32_t* topic_hash, int32_t 
                        int32_t* out_len, int32_t* out_broker, ka_status* st) {
     int rc = validate_dense(c, T, P, RF, desired_rf, out_stride, st);
     if (rc != KA_OK) return rc;
-    if ((rc = enter(c, true)) != KA_OK) return failed(st, rc);
+    if ((rc = enter_host(c)) != KA_OK) return failed(st, rc);
     Shape sh = dense_shape(T, P, RF, desired_rf, out_stride, c->br.N);
     if ((T > 0 && !topic_hash) || (sh.R > 0 && !cur_broker) || (sh.Q > 0 && !out_broker)) return set_status(st, KA_ERR_BAD_ARG);
     if ((rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
@@ -1959,7 +1988,7 @@ int32_t ka_solve_dense_json(ka_ctx* c, int32_t T, const int32_t* topic_hash, int
     if ((T > 0 && (!topic_hash || !names || !name_off)) || (sh.R > 0 && !cur_broker) || !json || json_cap < KA_JSON_HEAD_LEN + KA_JSON_TAIL_LEN)
         return set_status(st, KA_ERR_BAD_ARG);
     if ((rc = check_names(names, name_off, 0, T, st)) != KA_OK) return rc;
-    if ((rc = enter(c, true)) != KA_OK || (rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
+    if ((rc = enter_host(c)) != KA_OK || (rc = reserve_io(c, sh, false)) != KA_OK) return failed(st, rc);
     // no topics or no brokers: no text to write, refused once its buffers are prepared
     return solve_json(c, sh, host_call(c, topic_hash, nullptr, nullptr, cur_broker, nullptr, nullptr), names, name_off, json, json_cap,
                       json_bytes, st, T > 0 && c->br.N > 0);
@@ -2044,7 +2073,7 @@ static int prepare_ragged(ka_ctx* c, int32_t T, const int32_t* topic_hash, const
     if (!c) return set_status(st, KA_ERR_NO_DEVICE);
     if (T < 0 || (T > 0 && (!topic_hash || !part_off))) return set_status(st, KA_ERR_BAD_ARG);
     if (!pick_stride && (S < 1 || S > KA_MAX_SLOTS)) return set_status(st, KA_ERR_LIMIT, -1, -1, S);
-    int rc = enter(c, true);
+    int rc = enter_host(c);
     if (rc != KA_OK) return failed(st, rc);
     RaggedScan sc;
     int64_t capmax = 0;
