@@ -131,7 +131,9 @@ int32_t ka_solve_dense(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, int32_
  * concatenated (UTF-8; a name ka_json_name_refused refuses gives KA_ERR_BAD_ARG with a = the refused character's code
  * point: use the host emitter), name_off[T+1] their offsets;
  * json = host buffer of json_cap bytes (pinned for full PCIe speed; KA_ERR_LIMIT if too small: 64 + sum over rows of
- * (50 + 12*out_stride + name length) always suffices); *json_bytes = length of the text (not NUL-terminated). */
+ * (50 + 12*out_stride + name length) always suffices); *json_bytes = length of the text (not NUL-terminated).
+ * A topic's exception wins over KA_ERR_LIMIT: when a topic fails, *st is what ka_solve_dense reports, whatever json_cap is, and
+ * *json_bytes = 0. */
 int32_t ka_solve_dense_json(ka_ctx* ctx, int32_t T, const int32_t* topic_hash, int32_t P, int32_t RF,
                             const int32_t* cur_broker, int32_t desired_rf, const char* names, const int64_t* name_off,
                             char* json, int64_t json_cap, int64_t* json_bytes, ka_status* st);
