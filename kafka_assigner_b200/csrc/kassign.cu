@@ -147,13 +147,11 @@ struct ka_ctx {
     // scratch of the batched solves, apart from the single solve's: descriptors + broker tables, counters, and the run
     DevBuf d_batch_tab, d_batch_ctr;
     RunScratch batch_run;
-    // scratch of ka_score_candidates / ka_score_clusters: row weights, the K summaries, the per-broker sums [3][ΣN], the tables'
-    // offsets [K+1]
-    DevBuf d_score_w, d_score_sum, d_score_brk, d_score_off;
-    // scratch of ka_plan_waves (its rows: upload_wave_rows): the rows pass's per-row outputs and records, the packed records, the
-    // per-CTA counts and offsets, the chain's per-row words when they leave shared memory, the bucket log, the summaries and
-    // the meta words
-    DevBuf d_wv_nrecv, d_wv_wave, d_wv_tmp, d_wv_rec, d_wv_cnt, d_wv_state, d_wv_log, d_wv_sum, d_wv_meta;
+    // scratch of ka_score_candidates / ka_score_clusters: row weights, and the score passes' arrays (score_batch)
+    DevBuf d_score_w, d_score;
+    // scratch of ka_plan_waves (its rows: upload_wave_rows): every row's wave, the plan passes' arrays (wave_plan_device), the
+    // chain's per-row words when they leave shared memory and the summaries
+    DevBuf d_wv_wave, d_wv_plan, d_wv_state, d_wv_sum;
     // scratch of the sender budget (ka_plan_waves_send and its JSON form): the send table, the sender bucket log and the sender
     // summaries (the per-sender words share d_wv_state)
     DevBuf d_wv_send, d_wv_slog, d_wv_ssum;
@@ -162,18 +160,15 @@ struct ka_ctx {
     int32_t wave_rule = KA_WAVE_GREEDY;
     DevBuf d_wv_fit;
     // scratch of ka_plan_waves_json, beside the plan's and the JSON passes' (d_part_off, d_part_id, d_names, d_name_off, d_json,
-    // d_json_rowlen, d_json_blocksum as 64-bit offsets): the grouped rows (two arrays of Q), the radix passes' (digit, tile)
-    // counts and offsets, and the text total followed by doc_off [W + 1] (with a size limit: the total, D, then doc_off [D + 1])
-    DevBuf d_wv_perm, d_wv_hist, d_wv_doc;
-    // scratch of a size limit (ka_plan_waves_json_parts): the prefix S, the meta words, J_0, the waves' first positions, the
-    // parts per CTA, the parts' waves and the start flags; then the jump tables J_1 .. J_{K-1}
+    // d_json_rowlen, d_json_blocksum as 64-bit offsets): the radix passes' arrays (enq_wave_group), and the text total followed
+    // by doc_off [W + 1] (with a size limit: the total, D, then doc_off [D + 1])
+    DevBuf d_wv_sort, d_wv_doc;
+    // scratch of a size limit (ka_plan_waves_json_parts): the part passes' arrays (enq_wave_parts) and the jump tables J_k, k > 0
     DevBuf d_wv_part, d_wv_jump;
-    // scratch of the rollback documents (ka_plan_waves_json_parts_rollback): the text, then the rollback side's row bytes, CTA
-    // sums, prefix R, text total and back_off [D + 1]
+    // scratch of the rollback documents (ka_plan_waves_json_parts_rollback): the text, then the rollback side's arrays
     DevBuf d_wv_back, d_wv_bscr;
-    // scratch of ka_wave_broker_usage (its rows: upload_wave_rows): the usage table's ids, bases and capacities, before[], the
-    // event list twice (the radix passes' two sides), the (digit, tile) counts and offsets, the report and the meta words
-    DevBuf d_us_id, d_us_base, d_us_cap, d_us_before, d_us_ev, d_us_hist, d_us_out, d_us_meta;
+    // scratch of ka_wave_broker_usage (its rows: upload_wave_rows): the usage passes' arrays
+    DevBuf d_usage;
     HostPinned* h_pin = nullptr;
     unsigned long long* h_frag = nullptr;  // pinned [KA_MAX_JSON_FRAGS][2]: {first byte, bytes} of every JSON fragment
     // timing events (recorded only with timing on)
@@ -238,6 +233,26 @@ int failed(ka_status* st, int rc) {
 }
 
 inline size_t align16(size_t v) { return (v + 15) & ~size_t(15); }
+
+// The arrays of one scratch, each at a 16-byte boundary, listed once by a function that takes them in order (braced
+// initializers evaluate in order, function arguments do not). Run over a Layout without a base, the function sums their bytes
+// (layout_bytes); over one at the scratch's memory, a DevBuf's or a host image's, it returns their pointers (place).
+struct Layout {
+    unsigned char* base = nullptr;
+    size_t bytes = 0;
+    template <typename T> T* take(size_t n) {
+        T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+        bytes += align16(n * sizeof(T));
+        return p;
+    }
+};
+template <typename F> size_t layout_bytes(const F& lay) { Layout l; lay(l); return l.bytes; }
+template <typename F> auto place(const F& lay, void* base) { Layout l{static_cast<unsigned char*>(base)}; return lay(l); }
+// `buf` reserved for the scratch `lay` lists, and the scratch placed there; nullopt when the reserve fails.
+template <typename F> auto reserve_layout(DevBuf& buf, const F& lay) -> std::optional<decltype(place(lay, nullptr))> {
+    if (buf.reserve(layout_bytes(lay)) != cudaSuccess) return std::nullopt;
+    return place(lay, buf.p);
+}
 
 // Every event of the ctx, with whether it is timed.
 template <typename F>
@@ -1634,38 +1649,40 @@ static int enq_batch(ka_ctx* c, cudaStream_t s, const Batch& bt, const StageDesc
     const Plan& pl = d.pl;
     const int S = d.S, K = (int)bt.m.size();
     const size_t kq = (size_t)bt.recs, kt = (size_t)bt.topics;
-    // descriptors, then every member's blob, global LUT and broker ids, in one upload
-    std::vector<size_t> blob_off(K), glut_off(K), bid_off(K), ctr_off(K);
-    size_t bytes = align16((size_t)K * sizeof(KaCandidate)), ctr_ints = 0;
-    int64_t covered = 0;   // topics kernel A walks
-    for (int k = 0; k < K; ++k) {
-        const BatchMember& mb = bt.m[k];
-        blob_off[k] = bytes;
-        bytes += bt.tabs[mb.tab].blob.size() * 2;
-        glut_off[k] = bytes;
-        bytes += align16(bt.tabs[mb.tab].glut.size() * 2);
-        bid_off[k] = bytes;
-        bytes += align16((size_t)std::max(mb.n, 1) * 4);
-        ctr_off[k] = ctr_ints;
-        ctr_ints += (size_t)(mb.n + 1) * KA_MAX_SLOTS;   // + the chains' dummy row
-        covered += mb.T;
-    }
+    // the members' tables, in one upload: the descriptors (first: score_batch reads them at d_batch_tab), then every member's
+    // blob, global LUT and broker ids
+    struct MemberTab { uint16_t *blob, *glut; int32_t* bid; };
+    struct Tables { KaCandidate* cand; std::vector<MemberTab> m; };
+    const auto tables = [&](Layout& l) {
+        Tables o{l.take<KaCandidate>(K), {}};
+        for (const BatchMember& mb : bt.m)
+            o.m.push_back({l.take<uint16_t>(bt.tabs[mb.tab].blob.size()), l.take<uint16_t>(bt.tabs[mb.tab].glut.size()),
+                           l.take<int32_t>(std::max(mb.n, 1))});
+        return o;
+    };
+    const auto counters = [&](Layout& l) {   // every member's counters, + the chains' dummy row
+        std::vector<int32_t*> ctr8;
+        for (const BatchMember& mb : bt.m) ctr8.push_back(l.take<int32_t>((size_t)(mb.n + 1) * KA_MAX_SLOTS));
+        return ctr8;
+    };
+    std::vector<unsigned char> h(layout_bytes(tables), 0);
+    const size_t ctr_bytes = layout_bytes(counters);
     RunScratch& r = c->batch_run;
-    KA_CUDA(c->d_batch_tab.reserve(bytes));
-    KA_CUDA(c->d_batch_ctr.reserve(ctr_ints * 4));
+    KA_CUDA(c->d_batch_tab.reserve(h.size()));
+    KA_CUDA(c->d_batch_ctr.reserve(ctr_bytes));
     KA_CUDA(r.reserve(kq * 16, kq, kt, kt + 1, pl.a_levels, K));
-    unsigned char* base = c->d_batch_tab.as<unsigned char>();
-    std::vector<unsigned char> h(bytes, 0);
+    const Tables host = place(tables, h.data()), dev = place(tables, c->d_batch_tab.p);
+    const std::vector<int32_t*> ctr8 = place(counters, c->d_batch_ctr.p);
     int lut_mask = 0;
+    int64_t covered = 0;   // topics kernel A walks
     for (int k = 0; k < K; ++k) {
         const BatchMember& mb = bt.m[k];
         const BrokerTable& t = bt.tabs[mb.tab];
         // kernel A writes the member's records, perm and lend by input row, its ntl and status by input topic
         const int64_t shift = mb.rec0 - mb.row0, tshift = mb.topic0 - mb.t0;
         KaCandidate e{};
-        e.br = t.device(mb.n, reinterpret_cast<const uint16_t*>(base + blob_off[k]),
-                        reinterpret_cast<const uint16_t*>(base + glut_off[k]), reinterpret_cast<const int32_t*>(base + bid_off[k]));
-        e.ctr8 = c->d_batch_ctr.as<int32_t>() + ctr_off[k];
+        e.br = t.device(mb.n, dev.m[k].blob, dev.m[k].glut, dev.m[k].bid);
+        e.ctr8 = ctr8[k];
         e.out.rec = r.rec.as<unsigned char>() + shift * 16;
         if (pl.a_levels) {
             e.out.perm = r.perm.as<uint16_t>() + shift;
@@ -1681,15 +1698,16 @@ static int enq_batch(ka_ctx* c, cudaStream_t s, const Batch& bt, const StageDesc
         e.T = mb.T;
         e.row0 = (uint32_t)mb.row0;
         e.Q = (uint32_t)mb.Q;
-        std::memcpy(h.data() + (size_t)k * sizeof(KaCandidate), &e, sizeof(e));
-        std::memcpy(h.data() + blob_off[k], t.blob.data(), t.blob.size() * 2);
-        if (!t.glut.empty()) std::memcpy(h.data() + glut_off[k], t.glut.data(), t.glut.size() * 2);
-        if (mb.n > 0) std::memcpy(h.data() + bid_off[k], bt.broker_id + bt.cand_off[mb.tab], (size_t)mb.n * 4);
+        std::memcpy(host.cand + k, &e, sizeof(e));
+        std::memcpy(host.m[k].blob, t.blob.data(), t.blob.size() * 2);
+        if (!t.glut.empty()) std::memcpy(host.m[k].glut, t.glut.data(), t.glut.size() * 2);
+        if (mb.n > 0) std::memcpy(host.m[k].bid, bt.broker_id + bt.cand_off[mb.tab], (size_t)mb.n * 4);
         lut_mask |= 1 << t.lut_mode;
+        covered += mb.T;
     }
-    const KaCandidate* cand = c->d_batch_tab.as<KaCandidate>();
-    KA_CUDA(cudaMemcpyAsync(base, h.data(), bytes, cudaMemcpyHostToDevice, s));
-    KA_CUDA(cudaMemsetAsync(c->d_batch_ctr.p, 0, ctr_ints * 4, s));   // every member starts from a fresh Context
+    const KaCandidate* cand = dev.cand;
+    KA_CUDA(cudaMemcpyAsync(c->d_batch_tab.p, h.data(), h.size(), cudaMemcpyHostToDevice, s));
+    KA_CUDA(cudaMemsetAsync(c->d_batch_ctr.p, 0, ctr_bytes, s));   // every member starts from a fresh Context
     KA_CUDA(cudaMemsetAsync(r.flags.p, 0xFF, (size_t)K * 4, s));
     // topics no member walks (a fleet's refused clusters) have no chunks
     if (pl.a_levels && covered < bt.topics) KA_CUDA(cudaMemsetAsync(r.ntl.p, 0, kt * 4, s));
@@ -2283,41 +2301,31 @@ int32_t ka_solve_clusters(ka_ctx* c, int32_t K, const int32_t* cand_off, const i
     return finish_batch(c, c->stream, bt, st, part_id, part_off);
 }
 
-// The document table of a fleet's segmented JSON pass in d_json_seg: doc_off [K+1] | seg_bytes [K] | seg_row0 [K+1] (8 bytes
-// each) | seg_shift [K] | seg_member [K] (4 bytes each). Bytes, and the offset of seg_shift.
-static size_t fleet_segs_bytes(int K, size_t* shift_at) {
-    *shift_at = (3 * (size_t)K + 2) * 8;
-    return *shift_at + 2 * (size_t)K * 4;
+// The document table of a fleet's segmented JSON pass in d_json_seg: the arrays of KaJsonSegs.
+struct FleetSegs { unsigned long long *doc_off, *bytes; int64_t* row0; uint32_t* shift; int32_t* member; };
+static auto fleet_segs_layout(int K) {
+    return [K](Layout& l) {
+        return FleetSegs{l.take<unsigned long long>(K + 1), l.take<unsigned long long>(K), l.take<int64_t>(K + 1), l.take<uint32_t>(K),
+                         l.take<int32_t>(K)};
+    };
 }
 
-// The K clusters' first rows and batch members (-1: left out) to the document table, seg_bytes zeroed, on `s`.
+// The K clusters' first rows and batch members (-1: left out) to the document table, bytes zeroed, on `s`.
 static int enq_fleet_segs(ka_ctx* c, cudaStream_t s, const Fleet& f, int K) {
-    size_t shift_at;
-    const size_t bytes = fleet_segs_bytes(K, &shift_at);
-    std::vector<unsigned char> h(bytes, 0);
-    std::memcpy(h.data() + (2 * (size_t)K + 1) * 8, f.row0.data(), (size_t)(K + 1) * 8);
-    int32_t* member = reinterpret_cast<int32_t*>(h.data() + shift_at + (size_t)K * 4);
-    std::fill(member, member + K, -1);
-    for (size_t i = 0; i < f.bt.m.size(); ++i) member[f.bt.m[i].tab] = (int32_t)i;
-    KA_CUDA(c->d_json_seg.reserve(bytes));
-    KA_CUDA(cudaMemcpyAsync(c->d_json_seg.p, h.data(), bytes, cudaMemcpyHostToDevice, s));
+    std::vector<unsigned char> h(layout_bytes(fleet_segs_layout(K)), 0);
+    const FleetSegs hs = place(fleet_segs_layout(K), h.data());
+    std::copy(f.row0.begin(), f.row0.begin() + K + 1, hs.row0);
+    std::fill(hs.member, hs.member + K, -1);
+    for (size_t i = 0; i < f.bt.m.size(); ++i) hs.member[f.bt.m[i].tab] = (int32_t)i;
+    KA_CUDA(c->d_json_seg.reserve(h.size()));
+    KA_CUDA(cudaMemcpyAsync(c->d_json_seg.p, h.data(), h.size(), cudaMemcpyHostToDevice, s));
     return KA_OK;
 }
 
 // The kernels' view of the K clusters' table that enq_fleet_segs uploaded, with the batch's failure words.
 static KaJsonSegs fleet_segs(ka_ctx* c, int K) {
-    size_t shift_at;
-    fleet_segs_bytes(K, &shift_at);
-    unsigned char* seg = c->d_json_seg.as<unsigned char>();
-    KaJsonSegs sg{};
-    sg.K = K;
-    sg.doc_off = reinterpret_cast<unsigned long long*>(seg);
-    sg.bytes = sg.doc_off + K + 1;
-    sg.row0 = reinterpret_cast<const int64_t*>(sg.bytes + K);
-    sg.shift = reinterpret_cast<uint32_t*>(seg + shift_at);
-    sg.member = reinterpret_cast<const int32_t*>(sg.shift + K);
-    sg.flags = c->batch_run.flags.as<unsigned>();
-    return sg;
+    const FleetSegs sg = place(fleet_segs_layout(K), c->d_json_seg.p);
+    return KaJsonSegs{K, sg.row0, sg.member, c->batch_run.flags.as<unsigned>(), sg.bytes, sg.doc_off, sg.shift};
 }
 
 // The segmented JSON pass of a fleet solved as d (its rows in io.d_out, its document table uploaded), on `s` after the last
@@ -2441,21 +2449,21 @@ static int score_batch(ka_ctx* c, cudaStream_t s, const Batch& bt, const int32_t
     const int K = bt.K;
     const size_t nb = (size_t)cand_off[K];
     auto abort = [&](int code) { return score_empty(K, summary, brk, nb, abort_batch(c, s, st, K, code)); };
-    const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary);
-    if (c->d_score_sum.reserve(sum_bytes) != cudaSuccess || c->d_score_brk.reserve(std::max<size_t>(3 * nb, 1) * 8) != cudaSuccess ||
-        c->d_score_off.reserve((size_t)(K + 1) * 4) != cudaSuccess ||
-        (part_weight && c->d_score_w.reserve((size_t)std::max<int64_t>(Q, 1) * 8) != cudaSuccess))
-        return abort(KA_ERR_CUDA);
-    ka_move_summary* d_sum = c->d_score_sum.as<ka_move_summary>();
-    long long* d_brk = c->d_score_brk.as<long long>();
+    const size_t sum_bytes = (size_t)K * sizeof(ka_move_summary), brk_n = std::max<size_t>(3 * nb, 1);
+    // the K summaries, the per-broker sums [3][ΣN] and the tables' offsets [K+1]
+    struct Scores { ka_move_summary* sum; long long* brk; int32_t* off; };
+    const auto sc = reserve_layout(c->d_score, [&](Layout& l) {
+        return Scores{l.take<ka_move_summary>(K), l.take<long long>(brk_n), l.take<int32_t>(K + 1)};
+    });
+    if (!sc || (part_weight && c->d_score_w.reserve((size_t)std::max<int64_t>(Q, 1) * 8) != cudaSuccess)) return abort(KA_ERR_CUDA);
+    const auto [d_sum, d_brk, d_off] = *sc;
     const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
     if ((part_weight && Q > 0 && cudaMemcpyAsync(c->d_score_w.p, part_weight, (size_t)Q * 8, cudaMemcpyHostToDevice, s) != cudaSuccess) ||
-        cudaMemcpyAsync(c->d_score_off.p, cand_off, (size_t)(K + 1) * 4, cudaMemcpyHostToDevice, s) != cudaSuccess ||
-        cudaMemsetAsync(d_sum, 0, sum_bytes, s) != cudaSuccess || cudaMemsetAsync(d_brk, 0, std::max<size_t>(3 * nb, 1) * 8, s) != cudaSuccess ||
+        cudaMemcpyAsync(d_off, cand_off, (size_t)(K + 1) * 4, cudaMemcpyHostToDevice, s) != cudaSuccess ||
+        cudaMemsetAsync(d_sum, 0, sum_bytes, s) != cudaSuccess || cudaMemsetAsync(d_brk, 0, brk_n * 8, s) != cudaSuccess ||
         (f && enq_fleet_segs(c, s, *f, K) != KA_OK))
         return abort(KA_ERR_CUDA);
     const KaCandidate* cand = c->d_batch_tab.as<KaCandidate>();
-    const int32_t* d_off = c->d_score_off.as<int32_t>();
     const unsigned row_blocks = (unsigned)std::max<int64_t>((Q + 255) / 256, 1);
     if (f) {   // a fleet's rows are disjoint: one thread per input row, its cluster found in the table
         const KaJsonSegs sg = fleet_segs(c, K);
@@ -2671,7 +2679,7 @@ static int wave_fit_chain(ka_ctx* c, cudaStream_t s, unsigned nblk, int N, int n
 // The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the rows up (upload_wave_rows), the
 // rows / scan / compact / chain kernels under the ctx's wave rule (KA_WAVE_FIRST_FIT: wave_fit_chain), the meta words back,
 // then the sum and the two peak kernels (enqueued, not awaited).
-// Leaves every row's wave in d_wv_wave, its receivers in d_wv_nrecv, the new lists in d_out / d_out_len and the W summaries (ids
+// Leaves every row's wave in d_wv_wave, its receivers in d_wv_plan, the new lists in d_out / d_out_len and the W summaries (ids
 // still N - index) in d_wv_sum. A sender part sd (null: none) adds the sender rule and its summaries (ids still n - index) in
 // d_wv_ssum.
 static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, const int64_t* rep_off, const int32_t* cur_broker,
@@ -2686,11 +2694,15 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     const size_t state_bytes = (size_t)(N + ns) * (fit ? KA_WAVE_FIT_ROW_BYTES : KA_WAVE_ROW_BYTES);
     const bool gstate = state_bytes > KA_SMEM_BUDGET;
     const size_t q = (size_t)Q;
-    if (upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, nullptr) != KA_OK ||
-        c->d_wv_nrecv.reserve(q) || c->d_wv_wave.reserve(q * 4) || c->d_wv_tmp.reserve(q * sizeof(KaWaveRec)) ||
-        c->d_wv_rec.reserve(q * sizeof(KaWaveRec)) || c->d_wv_cnt.reserve((size_t)(2 * nblk + 1) * 4) ||
-        c->d_wv_state.reserve(gstate || fit ? state_bytes : 16) ||
-        c->d_wv_log.reserve((size_t)std::max<int64_t>(positions, 1) * sizeof(KaWaveBucket)) || c->d_wv_meta.reserve(sizeof(KaWaveMeta)))
+    // the rows pass's receiver counts and records, the packed records, the per-CTA counts, their offsets followed by their
+    // total, the bucket log and the meta words
+    struct PlanScratch { int8_t* nrecv; KaWaveRec *tmp, *rec; int32_t *cnt, *off; KaWaveBucket* log; KaWaveMeta* meta; };
+    const auto sc = reserve_layout(c->d_wv_plan, [&](Layout& l) {
+        return PlanScratch{l.take<int8_t>(q), l.take<KaWaveRec>(q), l.take<KaWaveRec>(q), l.take<int32_t>(nblk), l.take<int32_t>(nblk + 1),
+                           l.take<KaWaveBucket>((size_t)std::max<int64_t>(positions, 1)), l.take<KaWaveMeta>(1)};
+    });
+    if (upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, nullptr) != KA_OK || !sc ||
+        c->d_wv_wave.reserve(q * 4) || c->d_wv_state.reserve(gstate || fit ? state_bytes : 16))
         return set_status(st, KA_ERR_CUDA);
     unsigned char* state = gstate ? c->d_wv_state.as<unsigned char>() : nullptr;
     const size_t smem = gstate ? 0 : state_bytes;
@@ -2701,19 +2713,14 @@ static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, 
     KaWaveMeta meta0{0xFFFFFFFFu, 0, 0, 0, 0, 0, {}};   // the sender part only read with sd
     if (sd) meta0.snd = KaWaveSend{c->d_wv_send.as<int32_t>(), ns, sd->C, c->d_wv_slog.as<KaWaveBucket>()};
     const int64_t* d_w = part_weight ? c->d_score_w.as<int64_t>() : nullptr;
-    int32_t* d_cnt = c->d_wv_cnt.as<int32_t>();
-    int32_t* d_off = d_cnt + nblk;
-    KaWaveMeta* d_meta = c->d_wv_meta.as<KaWaveMeta>();
+    const auto [d_nrecv, d_tmp, d_rec, d_cnt, d_off, d_log, d_meta] = *sc;
     if (cudaMemcpyAsync(d_meta, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
-    KaWaveRec* d_rec = c->d_wv_rec.as<KaWaveRec>();
     int32_t* d_wave = c->d_wv_wave.as<int32_t>();
-    int8_t* d_nrecv = c->d_wv_nrecv.as<int8_t>();
-    KaWaveBucket* d_log = c->d_wv_log.as<KaWaveBucket>();
     const auto rows = sd ? ka_wave_rows_kernel<true> : ka_wave_rows_kernel<false>;
     rows<<<nblk, 256, 0, s>>>(c->br, (uint32_t)Q, stride, c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), c->d_out_len.as<int32_t>(),
-                              c->d_out.as<int32_t>(), d_w, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_wave, d_cnt, d_meta);
+                              c->d_out.as<int32_t>(), d_w, d_nrecv, d_tmp, d_wave, d_cnt, d_meta);
     ka_level_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, (int)nblk, d_off);
-    ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, c->d_wv_tmp.as<KaWaveRec>(), d_off, d_rec);
+    ka_wave_compact_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, d_nrecv, d_tmp, d_off, d_rec);
     c->launches += 3;   // rows, scan, compact
     if (fit) {
         int rc = wave_fit_chain(c, s, nblk, N, ns, max_broker_in, sd != nullptr, state, smem, d_rec, d_off, d_wave, d_log, d_meta, st);
@@ -2810,39 +2817,41 @@ int32_t ka_plan_waves_send(ka_ctx* c, int64_t Q, const int64_t* rep_off, const i
                       summary_cap, &sd, st);
 }
 
-// The tiling of a radix pass over n items: `tile` items per CTA, ntiles >= 1 CTAs. Returns the (digit, tile) cells: the pass's
-// hist buffer holds their counts, then their offsets at hist + cells, then the offsets' total.
+// The tiling of a radix pass over n items: `tile` items per CTA, ntiles >= 1 CTAs. Returns the (digit, tile) cells: the pass
+// counts them, then scans the counts to their offsets followed by the offsets' total.
 static int radix_tiles(int64_t n, uint32_t& tile, int& ntiles) {
     tile = (uint32_t)std::max<int64_t>(KA_RADIX_MIN_TILE, ((n + KA_RADIX_MAX_TILES - 1) / KA_RADIX_MAX_TILES + 255) / 256 * 256);
     ntiles = (int)std::max<int64_t>((n + tile - 1) / tile, 1);
     return KA_RADIX_DIGITS * ntiles;
 }
 
-// Bytes of a hist buffer for the passes over at most n items (a tile holds at least KA_RADIX_MIN_TILE of them).
-static size_t radix_hist_bytes(int64_t n) {
-    return (2 * (size_t)KA_RADIX_DIGITS * std::max<int64_t>((n + KA_RADIX_MIN_TILE - 1) / KA_RADIX_MIN_TILE, 1) + 1) * 4;
+// The most cells of the passes over at most n items (a tile holds at least KA_RADIX_MIN_TILE of them).
+static size_t radix_cells_max(int64_t n) {
+    return (size_t)KA_RADIX_DIGITS * std::max<int64_t>((n + KA_RADIX_MIN_TILE - 1) / KA_RADIX_MIN_TILE, 1);
 }
 
-// The radix passes of ka_plan_waves_json over the plan's d_wv_wave: d_wv_perm (two arrays of Q rows) ends with the changed
-// rows ordered by (wave, row) in the array returned, and the (digit, tile) offsets end with M, the changed rows, at n_rows.
+// The radix passes of ka_plan_waves_json over the plan's d_wv_wave, in d_wv_sort: the changed rows end ordered by (wave, row)
+// in the array returned, and the (digit, tile) offsets end with M, the changed rows, at n_rows. Null when d_wv_sort fails.
 static const int32_t* enq_wave_group(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const int32_t*& n_rows) {
     KaWaveSort p{};
     p.wave = c->d_wv_wave.as<int32_t>();
     p.Q = (uint32_t)Q;
     const int cells = radix_tiles(Q, p.tile, p.ntiles);
-    int32_t* hist = c->d_wv_hist.as<int32_t>();
-    int32_t* off = hist + cells;
-    int32_t* perm[2] = {c->d_wv_perm.as<int32_t>(), c->d_wv_perm.as<int32_t>() + Q};
-    p.n_ptr = n_rows = off + cells;
+    struct Sort { int32_t *perm[2], *hist, *off; };
+    const auto sc = reserve_layout(c->d_wv_sort, [&](Layout& l) {
+        return Sort{{l.take<int32_t>(Q), l.take<int32_t>(Q)}, l.take<int32_t>(cells), l.take<int32_t>(cells + 1)};
+    });
+    if (!sc) return nullptr;
+    p.n_ptr = n_rows = sc->off + cells;
     int pass = 0;
     for (; pass == 0 || W >> p.shift; ++pass, p.shift += KA_RADIX_BITS) {
-        p.in = pass ? perm[(pass - 1) & 1] : nullptr;
-        ka_wave_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, hist);
-        ka_level_scan_kernel<<<1, 1024, 0, s>>>(hist, cells, off);
-        ka_wave_sort_scatter_kernel<<<p.ntiles, 256, 0, s>>>(p, off, perm[pass & 1]);
+        p.in = pass ? sc->perm[(pass - 1) & 1] : nullptr;
+        ka_wave_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, sc->hist);
+        ka_level_scan_kernel<<<1, 1024, 0, s>>>(sc->hist, cells, sc->off);
+        ka_wave_sort_scatter_kernel<<<p.ntiles, 256, 0, s>>>(p, sc->off, sc->perm[pass & 1]);
         c->launches += 3;
     }
-    return perm[(pass - 1) & 1];
+    return sc->perm[(pass - 1) & 1];
 }
 
 // The size limit of ka_plan_waves_json_parts: L = max_doc_bytes, and the caller's doc_wave and n_docs.
@@ -2868,20 +2877,16 @@ static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const Wav
                           const KaWaveBack& bk, ka_status* st) {
     const size_t q = (size_t)Q;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
-    // S [Q + 1] u64, err and widest, J_0 [Q], first_pos [W + 1], part_cnt [nblk], doc_wave [Q], start [Q + 1]
-    const size_t o_meta = (q + 1) * 8, o_next = o_meta + 16, o_first = o_next + q * 4, o_cnt = o_first + ((size_t)W + 1) * 4,
-                 o_dw = o_cnt + (size_t)nblk * 4, o_start = o_dw + q * 4;
-    if (c->d_wv_part.reserve(o_start + q + 1)) return set_status(st, KA_ERR_CUDA);
-    char* base = static_cast<char*>(c->d_wv_part.p);
-    KaWaveParts pp{};
-    pp.d = d;
-    pp.room = std::min<int64_t>(pt.L - 28, (int64_t)1 << 62);   // S[i] + room never overflows
-    pp.S = reinterpret_cast<unsigned long long*>(base);
-    pp.err = reinterpret_cast<unsigned long long*>(base + o_meta);
-    pp.widest = pp.err + 1;
-    pp.next = reinterpret_cast<int32_t*>(base + o_next);
-    pp.first_pos = reinterpret_cast<int32_t*>(base + o_first);
-    pp.start = reinterpret_cast<uint8_t*>(base + o_start);
+    // S [Q + 1], err and widest (one pair: set and read back in one copy), J_0 [Q], first_pos [W + 1], part_cnt [nblk],
+    // doc_wave [Q], start [Q + 1]
+    struct Parts { unsigned long long *S, *meta; int32_t *next, *first_pos, *part_cnt, *doc_wave; uint8_t* start; };
+    const auto sc = reserve_layout(c->d_wv_part, [&](Layout& l) {
+        return Parts{l.take<unsigned long long>(q + 1), l.take<unsigned long long>(2), l.take<int32_t>(q), l.take<int32_t>((size_t)W + 1),
+                     l.take<int32_t>(nblk), l.take<int32_t>(q), l.take<uint8_t>(q + 1)};
+    });
+    if (!sc) return set_status(st, KA_ERR_CUDA);
+    const long long room = std::min<int64_t>(pt.L - 28, (int64_t)1 << 62);   // S[i] + room never overflows
+    const KaWaveParts pp{d, room, sc->S, sc->first_pos, sc->next, sc->start, sc->meta, sc->meta + 1};
     const unsigned long long meta0[2] = {~0ull, 0ull};
     if (cudaMemcpyAsync(pp.err, meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
     ka_wave_part_len_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
@@ -2908,8 +2913,8 @@ static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const Wav
     for (int k = K - 1; k >= 0; --k) ka_wave_part_mark_kernel<<<mblk, 256, 0, s>>>(level(k), pp.start, (uint32_t)M);
     c->launches += K > 0 ? 2 * K - 1 : 0;
     pd.start = pp.start;
-    pd.part_cnt = reinterpret_cast<int*>(base + o_cnt);
-    pd.doc_wave = reinterpret_cast<int32_t*>(base + o_dw);
+    pd.part_cnt = sc->part_cnt;
+    pd.doc_wave = sc->doc_wave;
     return cudaGetLastError() != cudaSuccess ? set_status(st, KA_ERR_CUDA) : KA_OK;
 }
 
@@ -2970,35 +2975,32 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
     const unsigned nblk = (unsigned)((Q + 255) / 256);
     const int64_t cap = std::min(json_cap, bound);
     if (c->d_part_off.reserve((size_t)(T + 1) * 8) || c->d_json.reserve((size_t)std::max<int64_t>(cap, 1)) ||
-        c->d_json_rowlen.reserve(q * 4) || c->d_json_blocksum.reserve((size_t)nblk * 8) || c->d_wv_perm.reserve(2 * q * 4) ||
-        c->d_wv_hist.reserve(radix_hist_bytes(Q)) || c->d_wv_doc.reserve((pt ? q + 3 : (size_t)W + 2) * 8) ||
-        upload_names(c, s, T, Q, names, name_off, part_id) != KA_OK ||
+        c->d_json_rowlen.reserve(q * 4) || c->d_json_blocksum.reserve((size_t)nblk * 8) ||
+        c->d_wv_doc.reserve((pt ? q + 3 : (size_t)W + 2) * 8) || upload_names(c, s, T, Q, names, name_off, part_id) != KA_OK ||
         cudaMemcpyAsync(c->d_part_off.p, part_off, (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s))
         return set_status(st, KA_ERR_CUDA);
     KaWaveDocs d{};
     d.p = json_params(c, c->d_out.as<int32_t>(), c->d_out_len.as<int32_t>(), stride, T, c->d_part_off.as<int64_t>(),
                       part_id ? c->d_part_id.as<int32_t>() : nullptr, 0, Q, (unsigned long long)cap);
-    d.perm = enq_wave_group(c, s, Q, W, d.n_rows);
+    if (!(d.perm = enq_wave_group(c, s, Q, W, d.n_rows))) return set_status(st, KA_ERR_CUDA);
     d.wave = c->d_wv_wave.as<int32_t>();
     d.blockoff = c->d_json_blocksum.as<unsigned long long>();
     unsigned long long* d_total = c->d_wv_doc.as<unsigned long long>();
     d.doc_off = d_total + (pt ? 2 : 1);
     KaWaveDocParts pd{};
-    KaWaveBack kb{};   // the rollback side: scratch of Q row bytes, nblk CTA sums, R [Q + 1], the text total, back_off [Q + 1]
+    // the rollback side: its row bytes [Q], CTA sums [nblk], prefix R [Q + 1], text total and back_off [Q + 1]
+    struct Back { uint32_t* rowlen; unsigned long long *blockoff, *R, *total, *back_off; };
+    Back bs{};
     const int64_t back_cap = bk ? std::min(bk->cap, back_bound) : 0;
-    unsigned long long* d_back_total = nullptr;
     if (bk) {
-        const size_t o_blk = (q * 4 + 7) / 8 * 8, o_R = o_blk + (size_t)nblk * 8, o_tot = o_R + (q + 1) * 8;
-        if (c->d_wv_back.reserve((size_t)std::max<int64_t>(back_cap, 1)) || c->d_wv_bscr.reserve(o_tot + (q + 2) * 8))
-            return set_status(st, KA_ERR_CUDA);
-        char* base = static_cast<char*>(c->d_wv_bscr.p);
-        kb.rep_off = c->d_rep_off.as<int64_t>();
-        kb.cur = c->d_cur.as<int32_t>();
-        kb.rowlen = reinterpret_cast<uint32_t*>(base);
-        kb.blockoff = reinterpret_cast<unsigned long long*>(base + o_blk);
-        kb.R = reinterpret_cast<unsigned long long*>(base + o_R);
-        d_back_total = reinterpret_cast<unsigned long long*>(base + o_tot);
+        const auto sc = reserve_layout(c->d_wv_bscr, [&](Layout& l) {
+            return Back{l.take<uint32_t>(q), l.take<unsigned long long>(nblk), l.take<unsigned long long>(q + 1),
+                        l.take<unsigned long long>(1), l.take<unsigned long long>(q + 1)};
+        });
+        if (c->d_wv_back.reserve((size_t)std::max<int64_t>(back_cap, 1)) || !sc) return set_status(st, KA_ERR_CUDA);
+        bs = *sc;
     }
+    const KaWaveBack kb{c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), bs.rowlen, bs.blockoff, bs.R};
     if (pt) {
         rc = bk ? enq_wave_parts<true>(c, s, Q, W, *pt, d, pd, kb, st) : enq_wave_parts<false>(c, s, Q, W, *pt, d, pd, kb, st);
         if (rc != KA_OK) return rc;
@@ -3012,13 +3014,13 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
         db.p.cap = (unsigned long long)back_cap;
         db.p.rowlen = kb.rowlen;
         db.blockoff = kb.blockoff;
-        db.doc_off = d_back_total + 1;
-        if (enq_wave_text<true, true>(c, s, nblk, db, d_back_total, pd, kb) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
+        db.doc_off = bs.back_off;
+        if (enq_wave_text<true, true>(c, s, nblk, db, bs.total, pd, kb) != cudaSuccess) return set_status(st, KA_ERR_CUDA);
     }
     unsigned long long total[2] = {0, (unsigned long long)W};   // the text's bytes and the documents D
     unsigned long long back_total = 0;
     if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(total, d_total, pt ? 16 : 8, cudaMemcpyDeviceToHost, s) ||
-        (bk && cudaMemcpyAsync(&back_total, d_back_total, 8, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
+        (bk && cudaMemcpyAsync(&back_total, bs.total, 8, cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     if (total[0] > (unsigned long long)json_cap) return set_status(st, KA_ERR_LIMIT, -1, -1, (int)std::min<int64_t>(json_cap, INT_MAX));
     if (bk && back_total > (unsigned long long)bk->cap)
@@ -3161,30 +3163,31 @@ int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const
     cudaStream_t s = c->stream;
     const size_t nu = (size_t)n_use;
     const unsigned nblk = (unsigned)std::max<int64_t>((Q + 255) / 256, 1);
-    const size_t ev_bytes = (size_t)std::max<int64_t>(E, 1) * sizeof(KaUseEvent);
-    if ((Q > 0 && upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, wave) != KA_OK) ||
-        c->d_us_id.reserve(std::max<size_t>(nu, 1) * 4) || (use_base && c->d_us_base.reserve(nu * 8 + 8)) ||
-        (use_cap && c->d_us_cap.reserve(nu * 8 + 8)) || c->d_us_before.reserve(std::max<size_t>(nu, 1) * 8) ||
-        c->d_us_ev.reserve(2 * ev_bytes) || c->d_us_hist.reserve(radix_hist_bytes(E)) ||
-        c->d_us_out.reserve(std::max<size_t>(nu, 1) * sizeof(ka_broker_usage)) || c->d_us_meta.reserve(sizeof(KaUsageMeta)))
+    const size_t nu1 = std::max<size_t>(nu, 1), ne = (size_t)std::max<int64_t>(E, 1), cells_max = radix_cells_max(E);
+    // the usage table's ids, bases and capacities (those given), before[], the event list twice (the radix passes' two sides),
+    // the (digit, tile) counts, their offsets followed by their total, the report and the meta words
+    struct Usage { int32_t* id; int64_t *base, *cap; long long* before; KaUseEvent* ev[2]; int32_t *hist, *off; ka_broker_usage* out;
+                   KaUsageMeta* meta; };
+    const auto u = reserve_layout(c->d_usage, [&](Layout& l) {
+        return Usage{l.take<int32_t>(nu1), use_base ? l.take<int64_t>(nu + 1) : nullptr, use_cap ? l.take<int64_t>(nu + 1) : nullptr,
+                     l.take<long long>(nu1), {l.take<KaUseEvent>(ne), l.take<KaUseEvent>(ne)}, l.take<int32_t>(cells_max),
+                     l.take<int32_t>(cells_max + 1), l.take<ka_broker_usage>(nu1), l.take<KaUsageMeta>(1)};
+    });
+    if ((Q > 0 && upload_wave_rows(c, Q, R, rep_off, cur_broker, stride, new_len, new_broker, part_weight, wave) != KA_OK) || !u)
         return set_status(st, KA_ERR_CUDA);
     const KaUsageMeta meta0{0xFFFFFFFFu, 0u};
-    if ((nu > 0 && cudaMemcpyAsync(c->d_us_id.p, use_id, nu * 4, cudaMemcpyHostToDevice, s)) ||
-        (use_base && nu > 0 && cudaMemcpyAsync(c->d_us_base.p, use_base, nu * 8, cudaMemcpyHostToDevice, s)) ||
-        (use_cap && nu > 0 && cudaMemcpyAsync(c->d_us_cap.p, use_cap, nu * 8, cudaMemcpyHostToDevice, s)) ||
-        (nu > 0 && cudaMemsetAsync(c->d_us_before.p, 0, nu * 8, s)) ||
-        cudaMemcpyAsync(c->d_us_meta.p, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s))
+    if ((nu > 0 && cudaMemcpyAsync(u->id, use_id, nu * 4, cudaMemcpyHostToDevice, s)) ||
+        (use_base && nu > 0 && cudaMemcpyAsync(u->base, use_base, nu * 8, cudaMemcpyHostToDevice, s)) ||
+        (use_cap && nu > 0 && cudaMemcpyAsync(u->cap, use_cap, nu * 8, cudaMemcpyHostToDevice, s)) ||
+        (nu > 0 && cudaMemsetAsync(u->before, 0, nu * 8, s)) || cudaMemcpyAsync(u->meta, &meta0, sizeof(meta0), cudaMemcpyHostToDevice, s))
         return set_status(st, KA_ERR_CUDA);
-    KaUseEvent* ev[2] = {c->d_us_ev.as<KaUseEvent>(), c->d_us_ev.as<KaUseEvent>() + std::max<int64_t>(E, 1)};
-    long long* d_before = c->d_us_before.as<long long>();
-    KaUsageMeta* d_meta = c->d_us_meta.as<KaUsageMeta>();
     ka_usage_rows_kernel<<<nblk, 256, 0, s>>>((uint32_t)Q, stride, c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(),
                                               c->d_out_len.as<int32_t>(), c->d_out.as<int32_t>(),
-                                              part_weight ? c->d_score_w.as<int64_t>() : nullptr, c->d_wv_wave.as<int32_t>(),
-                                              c->d_us_id.as<int32_t>(), n_use, d_before, ev[0], d_meta);
+                                              part_weight ? c->d_score_w.as<int64_t>() : nullptr, c->d_wv_wave.as<int32_t>(), u->id, n_use,
+                                              u->before, u->ev[0], u->meta);
     c->launches += 1;
     KaUsageMeta meta;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, d_meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
+    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&meta, u->meta, sizeof(meta), cudaMemcpyDeviceToHost, s) ||
         cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     if (meta.err_row != 0xFFFFFFFFu) {
@@ -3195,8 +3198,6 @@ int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const
     KaUsageSort p{};
     p.ne = meta.nev;
     const int cells = radix_tiles(p.ne, p.tile, p.ntiles);
-    int32_t* hist = c->d_us_hist.as<int32_t>();
-    int32_t* off = hist + cells;
     auto bits = [](uint64_t x) { int b = 0; while (x >> b) ++b; return b; };   // x <= 2^31: the shift stays below 64
     std::vector<int> shifts;
     if (W > 0) {
@@ -3205,21 +3206,19 @@ int32_t ka_wave_broker_usage(ka_ctx* c, int64_t Q, const int64_t* rep_off, const
     }
     int side = 0;
     for (int shift : shifts) {
-        p.in = ev[side];
+        p.in = u->ev[side];
         p.shift = shift;
-        ka_usage_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, hist);
-        ka_level_scan_kernel<<<1, 1024, 0, s>>>(hist, cells, off);
-        ka_usage_sort_scatter_kernel<<<p.ntiles, 256, 0, s>>>(p, off, ev[side ^ 1]);
+        ka_usage_sort_hist_kernel<<<p.ntiles, 256, 0, s>>>(p, u->hist);
+        ka_level_scan_kernel<<<1, 1024, 0, s>>>(u->hist, cells, u->off);
+        ka_usage_sort_scatter_kernel<<<p.ntiles, 256, 0, s>>>(p, u->off, u->ev[side ^ 1]);
         side ^= 1;
         c->launches += 3;
     }
-    ka_broker_usage* d_out = c->d_us_out.as<ka_broker_usage>();
-    ka_usage_broker_kernel<<<(unsigned)std::max<int64_t>(((int64_t)n_use + 7) / 8, 1), 256, 0, s>>>(
-        ev[side], p.ne, n_use, W, d_before, use_base ? c->d_us_base.as<int64_t>() : nullptr, use_cap ? c->d_us_cap.as<int64_t>() : nullptr,
-        d_out);
+    ka_usage_broker_kernel<<<(unsigned)std::max<int64_t>(((int64_t)n_use + 7) / 8, 1), 256, 0, s>>>(u->ev[side], p.ne, n_use, W,
+                                                                                                  u->before, u->base, u->cap, u->out);
     c->launches += 1;
     if (cudaGetLastError() != cudaSuccess ||
-        (nu > 0 && cudaMemcpyAsync(usage, d_out, nu * sizeof(ka_broker_usage), cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
+        (nu > 0 && cudaMemcpyAsync(usage, u->out, nu * sizeof(ka_broker_usage), cudaMemcpyDeviceToHost, s)) || cudaStreamSynchronize(s))
         return set_status(st, KA_ERR_CUDA);
     *n_waves_out = W;
     return set_status(st, KA_OK);

@@ -1,6 +1,6 @@
 """Small end-to-end cases for compute-sanitizer (memcheck): dense + ragged + error + 8-slot rows + pipelined, a wave plan with its
-rollback documents and the broker usage of that plan. Every Solver is closed, so that --leak-check full sees each Context's
-buffers freed."""
+rollback documents, the broker usage of that plan, a fleet's documents and a scored candidate batch. Every Solver is closed, so
+that --leak-check full sees each Context's buffers freed."""
 import os
 import sys
 
@@ -49,6 +49,14 @@ parts, rollback, part_wave, wave, summary, st = w.plan_wave_parts_rollback_json(
 print(st.code, len(parts), len(rollback))
 usage, W, st = w.broker_usage(rg.rep_off, rg.cur, new, new_len, wave, rg.all_broker_id)
 print(st.code, W, len(usage))
+fleet = [kab.synth.make_ragged_cluster(T=30, N=20, max_partitions=8, seed=11 + k) for k in range(3)]
+docs = solver().solve_clusters_json([(f.broker_id, f.rack_index, f.topic_hash, f.part_off, f.part_id, f.rep_off, f.cur, -1)
+                                     for f in fleet], [f.topic_names for f in fleet])   # the batch table image + the fleet segments
+print([(st.code, len(text)) for text, st in docs])
+tables = [(rg.broker_id, rg.rack_index), (rg.broker_id[::2], rg.rack_index[::2])]
+summary, sts, rep, lead, added = w.score_ragged_candidates(tables, rg.topic_hash, rg.part_off, rg.part_id, rg.rep_off, rg.cur, -1,
+                                                           weight=np.arange(rg.Q), per_broker=True)
+print([st.code for st in sts], summary["rows_moved"].tolist(), [len(a) for a in rep])
 for s in solvers:
     s.close()
 print("sanitize cases done")
