@@ -395,6 +395,28 @@ int32_t ka_ctx_set_wave_rule(ka_ctx* ctx, int32_t rule);
 /* The Context's wave rule; ctx NULL: KA_ERR_NO_DEVICE. */
 int32_t ka_ctx_wave_rule(ka_ctx* ctx);
 
+/* The PART CAPS every _parts call of this Context follows: ka_plan_waves_json_parts, ka_plan_waves_send_json_parts and their
+ * _rollback forms. The parts of a wave run one after the other, so one part is everything in flight at a time; the caps bound
+ * it beside the byte limit L of those calls:
+ *   max_part_rows = Lr   the most rows one part holds (0: no row cap)
+ *   max_part_in = Lx     the most data one part moves (0: no data cap): with a_g = w[g] x the receivers of row g, exactly what
+ *                        ka_wave_summary.replicas_added adds for the row (0 for a row that only reorders, w = 1 without
+ *                        weights), a part's rows hold sum(a) <= Lx unless the part is a single row
+ * The rule. Within one wave, rows i..j-1 (input order) make a part iff every byte condition of the call holds (S, and R on the
+ * rollback side), j - i <= Lr when Lr is set, and sum over i..j-1 of a <= Lx or j - i == 1 when Lx is set. Every condition is
+ * monotone in j, so the greedy cut stays unique, and no two consecutive parts of a wave could be merged under all of them. A
+ * row with a_g > Lx makes a part of its own, as a row heavier than max_broker_in has a wave to itself; it is not an error, and
+ * the caps add no error code (sum(a) <= 8 x the sum of the weights <= INT64_MAX is checked already). Any subset of a wave keeps
+ * every budget of that wave, so the plan, wave[], W and the summaries are those of the uncapped call; D <= the changed rows <=
+ * Q still holds, so doc_off[Q+1], doc_wave[Q] and the json_cap / back_cap bounds are unchanged. With both caps 0 every output
+ * is byte for byte that of a Context that never set them. The caps add no kernel launch and no synchronisation.
+ * ka_plan_waves(_send)(_json) make no parts and ignore the caps. Configuration like the wave rule: ka_ctx_reset leaves it alone.
+ * KA_OK; a negative value: KA_ERR_BAD_ARG (the caps stay as they were); ctx NULL: KA_ERR_NO_DEVICE. */
+int32_t ka_ctx_set_part_caps(ka_ctx* ctx, int64_t max_part_rows, int64_t max_part_in);
+/* The Context's part caps into *max_part_rows and *max_part_in (0 = no cap); ctx NULL: KA_ERR_NO_DEVICE; an output NULL:
+ * KA_ERR_BAD_ARG. */
+int32_t ka_ctx_part_caps(ka_ctx* ctx, int64_t* max_part_rows, int64_t* max_part_in);
+
 /* ka_plan_waves + the documents it plans, built on the device: one reassignment JSON per wave, what an operator feeds
  * kafka-reassign-partitions one after the other. Only the text, the waves and the summaries cross PCIe.
  *   T, part_off[T+1], part_id (NULL = 0..P-1 per topic), names, name_off[T+1]   host; the ragged layout and the name slab
@@ -520,9 +542,12 @@ int32_t ka_plan_waves_send_json(ka_ctx* ctx, int32_t T, const int64_t* part_off,
  * one-record document (29 + b_i bytes) exceeds L gives KA_ERR_LIMIT with a = the lowest such row (input order) and b = that
  * length clipped to INT_MAX; then a text longer than json_cap gives KA_ERR_LIMIT with a = min(json_cap, INT_MAX). On any error
  * *n_waves = *n_docs = 0 (when given) and nothing else is specified. W == 0 gives D = 0 and doc_off[0] = 0.
+ * The Context's part caps (ka_ctx_set_part_caps) cut the parts finer: a row also opens a new part when the current one would
+ * exceed Lr rows or, past its first row, Lx of data. The error checks and codes stay those above.
  * Synchronous; two synchronisations. The launches of ka_plan_waves_json, then, when W > 0, 4 more, and 2K - 1 more when the
  * widest wave has m >= 2 rows, K = the bit length of m - 1 (a pointer-doubling level per bit): they depend only on the bit
- * lengths of W and of m. Follows the Context's wave rule (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the
+ * lengths of W and of m, and are the same with the part caps set or not. Follows the Context's wave rule
+ * (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the
  * last order / stage plans and timings. */
 int32_t ka_plan_waves_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                  const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
@@ -537,7 +562,8 @@ int32_t ka_plan_waves_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off
  *   max_doc_bytes .. n_docs   exactly as ka_plan_waves_json_parts takes and writes them
  *   wave .. summary_cap   exactly as ka_plan_waves_send_json writes them
  * Checks: everything ka_plan_waves_send_json checks, in its order; then those ka_plan_waves_json_parts adds, in its order. The
- * launches of ka_plan_waves_send_json, and those ka_plan_waves_json_parts adds. Follows the Context's wave rule. */
+ * launches of ka_plan_waves_send_json, and those ka_plan_waves_json_parts adds, with the part caps set or not. Follows the
+ * Context's wave rule and its part caps (ka_ctx_set_part_caps), as ka_plan_waves_json_parts does. */
 int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                       const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                                       const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
@@ -569,7 +595,8 @@ int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* par
  * on both sides. When no changed row's current list prints longer than its new list, the cut, json, doc_off and doc_wave are
  * exactly those of ka_plan_waves_json_parts; it differs where the rollback side is longer (a replication-factor reduction, a
  * move to shorter broker ids). With L >= the longest wave document on both sides, D = W and json is that of
- * ka_plan_waves_json. The plan, W, wave and the summaries are those of ka_plan_waves.
+ * ka_plan_waves_json. The plan, W, wave and the summaries are those of ka_plan_waves. The Context's part caps
+ * (ka_ctx_set_part_caps) add their conditions to the paired cut; the rollback documents follow the parts.
  * Sufficient back_cap: the sum over rows of (79 + the name length of the row's topic), + 12 x rep_off[Q]. json_cap as before.
  * Checks, in this order: everything ka_plan_waves_json_parts checks, in its order; then back NULL, back_cap < 0, or back_off
  * NULL with Q > 0: KA_ERR_BAD_ARG. On the device: the plan's row errors; a changed row with 29 + max(record, rollback record)
@@ -577,7 +604,8 @@ int32_t ka_plan_waves_send_json_parts(ka_ctx* ctx, int32_t T, const int64_t* par
  * KA_ERR_LIMIT, a = min(json_cap, INT_MAX); a rollback text above back_cap: KA_ERR_LIMIT, a = min(back_cap, INT_MAX). On any
  * error *n_waves = *n_docs = 0 (when given). W == 0 gives D = 0 and back_off[0] = 0.
  * Synchronous. The launches of ka_plan_waves_json_parts on the same inputs, and, when W > 0, 3 more (the rollback text's
- * length, scan and write passes; the part passes carry the rollback side without a launch of their own). Follows the
+ * length, scan and write passes; the part passes carry the rollback side without a launch of their own), with the part caps
+ * set or not. Follows the
  * Context's wave rule (ka_ctx_set_wave_rule); does not read or change the Context counters, parked counters, topic_base, the staged block, or the last order / stage plans and timings. */
 int32_t ka_plan_waves_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                           const int64_t* rep_off, const int32_t* cur_broker, int32_t stride, const int32_t* new_len,
@@ -593,8 +621,8 @@ int32_t ka_plan_waves_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t*
  *   back .. back_off   exactly as ka_plan_waves_json_parts_rollback takes and writes them
  *   wave .. summary_cap   exactly as ka_plan_waves_send_json_parts writes them
  * Checks: everything ka_plan_waves_send_json_parts checks, in its order; then those ka_plan_waves_json_parts_rollback adds, in
- * its order. The launches of ka_plan_waves_send_json_parts, and the 3 ka_plan_waves_json_parts_rollback adds. Follows the
- * Context's wave rule. */
+ * its order. The launches of ka_plan_waves_send_json_parts, and the 3 ka_plan_waves_json_parts_rollback adds, with the part
+ * caps set or not. Follows the Context's wave rule and its part caps (ka_ctx_set_part_caps). */
 int32_t ka_plan_waves_send_json_parts_rollback(ka_ctx* ctx, int32_t T, const int64_t* part_off, const int32_t* part_id,
                                                const int64_t* rep_off, const int32_t* cur_broker, int32_t stride,
                                                const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,

@@ -96,6 +96,8 @@ SYMBOLS = {
     "ka_ctx_set_timing": (_i32, [_vp, _i32]),
     "ka_ctx_set_wave_rule": (_i32, [_vp, _i32]),
     "ka_ctx_wave_rule": (_i32, [_vp]),
+    "ka_ctx_set_part_caps": (_i32, [_vp, _i64, _i64]),
+    "ka_ctx_part_caps": (_i32, [_vp, _vp, _vp]),
     "ka_ctx_last_timing": (_i32, [_vp, _vp]),
     "ka_ctx_launch_count": (_i64, [_vp]),
     "ka_ctx_last_order_plan": (_i32, [_vp, _vp]),

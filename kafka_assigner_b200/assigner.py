@@ -232,6 +232,23 @@ class Solver:
         _check(min(code, 0), "ka_ctx_wave_rule")
         return {v: k for k, v in self.WAVE_RULES.items()}[code]
 
+    def set_part_caps(self, max_rows=None, max_in=None):
+        """The part caps of every plan_wave_parts_json / plan_wave_parts_rollback_json call of this Solver
+        (ka_ctx_set_part_caps): a part holds at most max_rows rows, and moves at most max_in of data (weight x the row's new
+        replicas, summed over the part's rows) unless it is a single row. None (or 0) is no cap. The cut only gets finer: the
+        plan, wave and the summaries stay those of the uncapped call. reset() keeps them. A negative cap raises ValueError and
+        leaves the caps as they were."""
+        rows, data = (0 if x is None else int(x) for x in (max_rows, max_in))
+        if rows < 0 or data < 0:
+            raise ValueError("part caps must be >= 0 (0 or None: no cap), not %r, %r" % (max_rows, max_in))
+        _check(self._L.ka_ctx_set_part_caps(self._h, rows, data), "ka_ctx_set_part_caps")
+
+    def part_caps(self):
+        """(max_rows, max_in) as set_part_caps set them, None where there is no cap."""
+        rows, data = ctypes.c_int64(0), ctypes.c_int64(0)
+        _check(self._L.ka_ctx_part_caps(self._h, ctypes.byref(rows), ctypes.byref(data)), "ka_ctx_part_caps")
+        return tuple(x.value or None for x in (rows, data))
+
     def last_timing(self):
         ms = np.zeros(8, dtype=np.float32)
         self._L.ka_ctx_last_timing(self._h, _ptr(ms))

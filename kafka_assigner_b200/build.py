@@ -34,16 +34,18 @@ HOST_WAVE_PARTS_TEST = os.path.join(_HERE, "bin", "test_wave_parts")
 HOST_WAVE_ROLLBACK_TEST = os.path.join(_HERE, "bin", "test_wave_rollback")
 HOST_BROKER_USAGE_TEST = os.path.join(_HERE, "bin", "test_broker_usage")
 HOST_WAVES_FIRST_FIT_TEST = os.path.join(_HERE, "bin", "test_waves_first_fit")
+HOST_PART_CAPS_TEST = os.path.join(_HERE, "bin", "test_part_caps")
 HOST_SOURCES = ["kafka_assignment_generator.cpp", "kassign_host.hpp", "test_kafka_topic_assigner.cpp", "test_candidates.cpp",
                 "test_candidate_scores.cpp", "test_clusters.cpp", "test_clusters_json.cpp", "test_cluster_scores.cpp", "test_waves.cpp", "test_waves_json.cpp",
-                "test_waves_send.cpp", "test_wave_parts.cpp", "test_wave_rollback.cpp", "test_broker_usage.cpp", "test_waves_first_fit.cpp"]
+                "test_waves_send.cpp", "test_wave_parts.cpp", "test_wave_rollback.cpp", "test_broker_usage.cpp", "test_waves_first_fit.cpp",
+                "test_part_caps.cpp"]
 
 
 def build_host(force=False):
     """g++ the C++ host mirror + file-based CLI (reference flag surface) against libkassign.so."""
     deps = [os.path.join(HOST_DIR, f) for f in HOST_SOURCES] + [LIB, os.path.join(_HERE, "..", "include", "kassign.h")]
     if not force and all(os.path.exists(x) for x in (CLI, HOST_TEST, HOST_CANDIDATES_TEST, HOST_SCORES_TEST, HOST_CLUSTERS_TEST,
-                                                                   HOST_CLUSTERS_JSON_TEST, HOST_CLUSTER_SCORES_TEST, HOST_WAVES_TEST, HOST_WAVES_JSON_TEST, HOST_WAVES_SEND_TEST, HOST_WAVE_PARTS_TEST, HOST_WAVE_ROLLBACK_TEST, HOST_BROKER_USAGE_TEST, HOST_WAVES_FIRST_FIT_TEST)) and all(os.path.getmtime(d) <= os.path.getmtime(CLI) for d in deps if os.path.exists(d)):
+                                                                   HOST_CLUSTERS_JSON_TEST, HOST_CLUSTER_SCORES_TEST, HOST_WAVES_TEST, HOST_WAVES_JSON_TEST, HOST_WAVES_SEND_TEST, HOST_WAVE_PARTS_TEST, HOST_WAVE_ROLLBACK_TEST, HOST_BROKER_USAGE_TEST, HOST_WAVES_FIRST_FIT_TEST, HOST_PART_CAPS_TEST)) and all(os.path.getmtime(d) <= os.path.getmtime(CLI) for d in deps if os.path.exists(d)):
         return CLI
     os.makedirs(os.path.dirname(CLI), exist_ok=True)
     cmd = ["g++", "-O2", "-std=c++17", "-Wall", os.path.join(HOST_DIR, "kafka_assignment_generator.cpp"), "-L" + CSRC, "-lkassign",
@@ -55,7 +57,7 @@ def build_host(force=False):
                      ("test_waves.cpp", HOST_WAVES_TEST), ("test_waves_json.cpp", HOST_WAVES_JSON_TEST),
                      ("test_waves_send.cpp", HOST_WAVES_SEND_TEST), ("test_wave_parts.cpp", HOST_WAVE_PARTS_TEST),
                      ("test_wave_rollback.cpp", HOST_WAVE_ROLLBACK_TEST), ("test_broker_usage.cpp", HOST_BROKER_USAGE_TEST),
-                     ("test_waves_first_fit.cpp", HOST_WAVES_FIRST_FIT_TEST)):
+                     ("test_waves_first_fit.cpp", HOST_WAVES_FIRST_FIT_TEST), ("test_part_caps.cpp", HOST_PART_CAPS_TEST)):
         subprocess.check_call(["g++", "-O2", "-std=c++17", "-Wall", os.path.join(HOST_DIR, src), "-L" + CSRC, "-lkassign",
                                "-Wl,-rpath,$ORIGIN/../csrc", "-o", exe])
     return CLI

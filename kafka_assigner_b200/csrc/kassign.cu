@@ -165,6 +165,8 @@ struct ka_ctx {
     DevBuf d_wv_sort, d_wv_doc;
     // scratch of a size limit (ka_plan_waves_json_parts): the part passes' arrays (enq_wave_parts) and the jump tables J_k, k > 0
     DevBuf d_wv_part, d_wv_jump;
+    // the part caps of every _parts call (ka_ctx_set_part_caps): the most rows and the most data of one part, 0 = no cap
+    int64_t part_rows = 0, part_in = 0;
     // scratch of the rollback documents (ka_plan_waves_json_parts_rollback): the text, then the rollback side's arrays
     DevBuf d_wv_back, d_wv_bscr;
     // scratch of ka_wave_broker_usage (its rows: upload_wave_rows): the usage passes' arrays
@@ -1588,6 +1590,22 @@ int32_t ka_ctx_set_wave_rule(ka_ctx* c, int32_t rule) {
 
 int32_t ka_ctx_wave_rule(ka_ctx* c) { return c ? c->wave_rule : KA_ERR_NO_DEVICE; }
 
+int32_t ka_ctx_set_part_caps(ka_ctx* c, int64_t max_part_rows, int64_t max_part_in) {
+    if (!c) return KA_ERR_NO_DEVICE;
+    if (max_part_rows < 0 || max_part_in < 0) return KA_ERR_BAD_ARG;
+    c->part_rows = max_part_rows;
+    c->part_in = max_part_in;
+    return KA_OK;
+}
+
+int32_t ka_ctx_part_caps(ka_ctx* c, int64_t* max_part_rows, int64_t* max_part_in) {
+    if (!c) return KA_ERR_NO_DEVICE;
+    if (!max_part_rows || !max_part_in) return KA_ERR_BAD_ARG;
+    *max_part_rows = c->part_rows;
+    *max_part_in = c->part_in;
+    return KA_OK;
+}
+
 int32_t ka_ctx_last_timing(ka_ctx* c, float* ms) {
     if (!c) return KA_ERR_NO_DEVICE;
     if (!ms) return KA_ERR_BAD_ARG;
@@ -2679,9 +2697,9 @@ static int wave_fit_chain(ka_ctx* c, cudaStream_t s, unsigned nblk, int N, int n
 // The device part of a wave plan of Q > 0 checked rows, on c->stream of the entered ctx: the rows up (upload_wave_rows), the
 // rows / scan / compact / chain kernels under the ctx's wave rule (KA_WAVE_FIRST_FIT: wave_fit_chain), the meta words back,
 // then the sum and the two peak kernels (enqueued, not awaited).
-// Leaves every row's wave in d_wv_wave, its receivers in d_wv_plan, the new lists in d_out / d_out_len and the W summaries (ids
-// still N - index) in d_wv_sum. A sender part sd (null: none) adds the sender rule and its summaries (ids still n - index) in
-// d_wv_ssum.
+// Leaves every row's wave in d_wv_wave, its receivers (int8, -1 unchanged) at the start of d_wv_plan, where the part caps read
+// them (enq_wave_parts), the new lists in d_out / d_out_len and the W summaries (ids still N - index) in d_wv_sum. A sender part
+// sd (null: none) adds the sender rule and its summaries (ids still n - index) in d_wv_ssum.
 static int wave_plan_device(ka_ctx* c, int64_t Q, int64_t R, int64_t positions, const int64_t* rep_off, const int32_t* cur_broker,
                             int32_t stride, const int32_t* new_len, const int32_t* new_broker, const int64_t* part_weight,
                             int64_t max_broker_in, const WaveSend* sd, int& W, ka_status* st) {
@@ -2871,31 +2889,39 @@ struct WaveBack {
 extern "C++" {   // the templates of the wave text passes
 // The part passes of a size limit pt over the grouped rows of d, on s: every part start flagged in pd.start, pd.part_cnt and
 // pd.doc_wave placed, or KA_ERR_LIMIT for the lowest row whose one-record document exceeds pt.L. Q rows, W > 0 waves. With BACK
-// the cut is the paired cut over the rollback side's bk, and a row over-long on either side is the error.
-template <bool BACK>
+// the cut is the paired cut over the rollback side's bk, and a row over-long on either side is the error. With CAPS the cut
+// also keeps the ctx's part caps, over the receivers the plan left first in d_wv_plan (wave_plan_device) and the weights d_w
+// (null: 1 per row).
+template <bool BACK, bool CAPS>
 static int enq_wave_parts(ka_ctx* c, cudaStream_t s, int64_t Q, int W, const WaveParts& pt, const KaWaveDocs& d, KaWaveDocParts& pd,
-                          const KaWaveBack& bk, ka_status* st) {
+                          const KaWaveBack& bk, const int64_t* d_w, ka_status* st) {
     const size_t q = (size_t)Q;
     const unsigned nblk = (unsigned)((Q + 255) / 256);
     // S [Q + 1], err and widest (one pair: set and read back in one copy), J_0 [Q], first_pos [W + 1], part_cnt [nblk],
-    // doc_wave [Q], start [Q + 1]
-    struct Parts { unsigned long long *S, *meta; int32_t *next, *first_pos, *part_cnt, *doc_wave; uint8_t* start; };
+    // doc_wave [Q], start [Q + 1]; with CAPS A [Q + 1] and its CTA sums [nblk]
+    struct Parts { unsigned long long *S, *meta; int32_t *next, *first_pos, *part_cnt, *doc_wave; uint8_t* start; unsigned long long *A, *ablk; };
     const auto sc = reserve_layout(c->d_wv_part, [&](Layout& l) {
         return Parts{l.take<unsigned long long>(q + 1), l.take<unsigned long long>(2), l.take<int32_t>(q), l.take<int32_t>((size_t)W + 1),
-                     l.take<int32_t>(nblk), l.take<int32_t>(q), l.take<uint8_t>(q + 1)};
+                     l.take<int32_t>(nblk), l.take<int32_t>(q), l.take<uint8_t>(q + 1), l.take<unsigned long long>(CAPS ? q + 1 : 0),
+                     l.take<unsigned long long>(CAPS ? nblk : 0)};
     });
     if (!sc) return set_status(st, KA_ERR_CUDA);
     const long long room = std::min<int64_t>(pt.L - 28, (int64_t)1 << 62);   // S[i] + room never overflows
     const KaWaveParts pp{d, room, sc->S, sc->first_pos, sc->next, sc->start, sc->meta, sc->meta + 1};
+    // M < 2^31, so i + 2^32 is past every wave's end
+    const KaWaveCaps cp{c->d_wv_plan.as<int8_t>(), d_w, sc->ablk, sc->A, c->part_rows > 0 ? (unsigned long long)c->part_rows : 1ull << 32,
+                        c->part_in > 0 ? (unsigned long long)c->part_in : ~0ull};
     const unsigned long long meta0[2] = {~0ull, 0ull};
     if (cudaMemcpyAsync(pp.err, meta0, sizeof(meta0), cudaMemcpyHostToDevice, s)) return set_status(st, KA_ERR_CUDA);
-    ka_wave_part_len_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
-    if constexpr (BACK)
-        ka_wave_part_scan2_kernel<<<1, 1024, 0, s>>>(d.blockoff, bk.blockoff, (int)nblk);
+    ka_wave_part_len_kernel<BACK, CAPS><<<nblk, 256, 0, s>>>(pp, bk, cp);
+    if constexpr (BACK && CAPS)
+        ka_wave_part_scan_kernel<3><<<1, 1024, 0, s>>>(d.blockoff, bk.blockoff, (int)nblk, cp.blockoff);
+    else if constexpr (BACK || CAPS)
+        ka_wave_part_scan_kernel<2><<<1, 1024, 0, s>>>(d.blockoff, BACK ? bk.blockoff : cp.blockoff, (int)nblk, nullptr);
     else
         ka_wave_doc_scan_kernel<false><<<1, 1024, 0, s>>>(d.blockoff, (int)nblk, pp.S, nullptr);   // S[0] is rewritten next
-    ka_wave_part_prefix_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
-    ka_wave_part_next_kernel<BACK><<<nblk, 256, 0, s>>>(pp, bk);
+    ka_wave_part_prefix_kernel<BACK, CAPS><<<nblk, 256, 0, s>>>(pp, bk, cp);
+    ka_wave_part_next_kernel<BACK, CAPS><<<nblk, 256, 0, s>>>(pp, bk, cp);
     c->launches += 4;
     unsigned long long back[2];
     int32_t M = 0;
@@ -3001,9 +3027,11 @@ static int32_t plan_waves_json(ka_ctx* c, int32_t T, const int64_t* part_off, co
         bs = *sc;
     }
     const KaWaveBack kb{c->d_rep_off.as<int64_t>(), c->d_cur.as<int32_t>(), bs.rowlen, bs.blockoff, bs.R};
-    if (pt) {
-        rc = bk ? enq_wave_parts<true>(c, s, Q, W, *pt, d, pd, kb, st) : enq_wave_parts<false>(c, s, Q, W, *pt, d, pd, kb, st);
-        if (rc != KA_OK) return rc;
+    if (pt) {   // the caps off: the uncapped passes
+        const bool caps = c->part_rows > 0 || c->part_in > 0;
+        const auto parts = bk ? (caps ? enq_wave_parts<true, true> : enq_wave_parts<true, false>)
+                              : (caps ? enq_wave_parts<false, true> : enq_wave_parts<false, false>);
+        if ((rc = parts(c, s, Q, W, *pt, d, pd, kb, part_weight ? c->d_score_w.as<int64_t>() : nullptr, st)) != KA_OK) return rc;
     }
     const cudaError_t e = pt ? enq_wave_text<true, false>(c, s, nblk, d, d_total, pd, kb)
                              : enq_wave_text<false, false>(c, s, nblk, d, d_total, pd, kb);

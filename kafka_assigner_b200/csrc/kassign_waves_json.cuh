@@ -34,9 +34,17 @@
 // The rollback documents (ka_plan_waves_json_parts_rollback) print every part's rows with their CURRENT lists
 // (ka_json_back_len / ka_json_back_put). The paired cut takes the rollback record's c'_i beside c_i and its prefix R beside S:
 // positions i..j-1 of one wave make a part iff both S[j] - S[i] and R[j] - R[i] are <= L - 28. The part passes' BACK = true
-// instances carry R (the pair scan ka_wave_part_scan2_kernel takes the place of ka_wave_doc_scan_kernel); the jump and mark
+// instances carry R (the pair scan ka_wave_part_scan_kernel<2> takes the place of ka_wave_doc_scan_kernel); the jump and mark
 // passes are the same. The rollback text is then one more length / scan / write trio (BACK = true, over the same positions and
 // part starts), into its own buffer, with the frame {"version":1,"partitions":[ ... ]}.
+//
+// The part caps (ka_ctx_set_part_caps) bound what one part holds: at most Lr rows, and at most Lx of data, a_i = w[g] x the
+// receivers of row g = perm[i] (0 for a row that only reorders), unless the part is a single row. The CAPS = true instances of
+// the length, prefix and next passes carry A, the 64-bit exclusive prefix of a, beside S (and R): the length pass writes a_i
+// and its CTA sums, the one-CTA scan takes them as one more array (ka_wave_part_scan_kernel<2> or <3>), the prefix pass turns
+// a_i into A[i], and the next pass ends its search at i + Lr and tests A[j] - A[i] <= Lx beside the bytes. j = i + 1 is never
+// tested: a single row always makes a part, so only the byte limit can refuse a row. The launches are those of the uncapped
+// call.
 //
 // A pass ranks a row by counting, never by the order of atomics: the text depends on the input alone.
 #pragma once
@@ -144,6 +152,35 @@ struct KaWaveBack {
     unsigned long long* blockoff;        // [ceil(Q / 256)] CTA sums, then (scan) their offsets
     unsigned long long* R;               // [M + 1] the part passes' prefix of c'
 };
+
+// What the part passes read and write only under the part caps (CAPS = true). A separate (last) kernel argument, like
+// KaWaveBack.
+struct KaWaveCaps {
+    const int8_t* nrecv;                 // [Q] the plan's receivers of every row (-1 for an unchanged row)
+    const int64_t* weight;               // [Q], or null: 1 per row
+    unsigned long long* blockoff;        // [ceil(Q / 256)] the CTA sums of a, then (scan) their offsets
+    unsigned long long* A;               // [M + 1] a_i (length pass), then (prefix pass) the exclusive prefix of a
+    unsigned long long rows;             // Lr, or 2^32 without a row cap
+    unsigned long long in;               // Lx, or ~0 without a data cap
+};
+
+// ka_cta256_prefix over 64-bit values: this thread's offset in the CTA's sum, and (total) that sum, in every thread.
+__device__ __forceinline__ unsigned long long ka_cta256_prefix64(unsigned long long n, unsigned long long& total) {
+    __shared__ unsigned long long wsum[8];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long x = n;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned long long y = __shfl_up_sync(KA_FULL, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) wsum[warp] = x;
+    __syncthreads();
+    unsigned long long woff = 0;
+    total = 0;
+    for (int i = 0; i < 8; ++i) { if (i < warp) woff += wsum[i]; total += wsum[i]; }
+    return woff + x - n;
+}
 
 // Row, wave and place in its document of grouped position i.
 template <bool PARTS>
@@ -277,13 +314,14 @@ struct KaWaveParts {
     unsigned long long* widest;     // the most rows of a wave
 };
 
-// grid ceil(Q / 256), 256 threads. BACK: c'_i and its CTA sums too.
-template <bool BACK>
-__global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts pp, const KaWaveBack bk) {
+// grid ceil(Q / 256), 256 threads. BACK: c'_i and its CTA sums too. CAPS: a_i and its CTA sums too.
+template <bool BACK, bool CAPS>
+__global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts pp, const KaWaveBack bk, const KaWaveCaps cp) {
     const KaWaveDocs& d = pp.d;
     const uint32_t M = (uint32_t)*d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     uint32_t c = 0, cb = 0;
+    unsigned long long a = 0;
     if (i < M) {
         uint32_t g;
         int v;
@@ -294,6 +332,11 @@ __global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts
         if constexpr (BACK) {
             cb = ka_json_back_len(d.p, bk.rep_off, bk.cur, g, true);
             bk.rowlen[i] = cb;
+        }
+        if constexpr (CAPS) {   // what ka_wave_sum_kernel adds to replicas_added for the row
+            const int nr = cp.nrecv[g];
+            a = nr > 0 ? (unsigned long long)nr * (unsigned long long)(cp.weight ? __ldg(cp.weight + g) : 1) : 0ull;
+            cp.A[i] = a;
         }
         pp.start[i] = first;
         if (first) pp.first_pos[v - 1] = (int32_t)i;
@@ -306,20 +349,31 @@ __global__ void __launch_bounds__(256) ka_wave_part_len_kernel(const KaWaveParts
         const unsigned long long back = ka_cta256_sum(cb);
         if (threadIdx.x == 0) bk.blockoff[blockIdx.x] = back;
     }
+    if constexpr (CAPS) {   // its own shared words: no barrier needed before it
+        unsigned long long sum;
+        ka_cta256_prefix64(a, sum);
+        if (threadIdx.x == 0) cp.blockoff[blockIdx.x] = sum;
+    }
 }
 
-// ONE CTA of 1024: both sides' CTA sums of the paired cut to their offsets, in place.
-__global__ void __launch_bounds__(1024) ka_wave_part_scan2_kernel(unsigned long long* __restrict__ v, unsigned long long* __restrict__ w,
-                                                                  int n) {
+// ONE CTA of 1024: K arrays of CTA sums to their offsets, in place: v and w (K = 2: S and R, or S and A), and x (K = 3: A
+// beside S and R).
+template <int K>
+__global__ void __launch_bounds__(1024) ka_wave_part_scan_kernel(unsigned long long* __restrict__ v, unsigned long long* __restrict__ w,
+                                                                 int n, unsigned long long* __restrict__ x) {
     ka_cta_scan(v, v, n, 0ull);
     __syncthreads();   // every thread has read the first scan's total: the second may reset it
     ka_cta_scan(w, w, n, 0ull);
+    if constexpr (K == 3) {
+        __syncthreads();
+        ka_cta_scan(x, x, n, 0ull);
+    }
 }
 
 // grid ceil(Q / 256), 256 threads: S[i] = the CTA's offset + the in-CTA prefix; the last position also writes S[M]. BACK: R
-// likewise.
-template <bool BACK>
-__global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWaveParts pp, const KaWaveBack bk) {
+// likewise. CAPS: A likewise, over the a_i the length pass left in A (each thread reads only its own).
+template <bool BACK, bool CAPS>
+__global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWaveParts pp, const KaWaveBack bk, const KaWaveCaps cp) {
     const uint32_t M = (uint32_t)*pp.d.n_rows;
     if (blockIdx.x * 256u >= M) return;   // CTA-uniform
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
@@ -335,14 +389,28 @@ __global__ void __launch_bounds__(256) ka_wave_part_prefix_kernel(const KaWavePa
         if (i < M) bk.R[i] = r;
         if (i + 1 == M) bk.R[M] = r + cb;
     }
+    if constexpr (CAPS) {
+        const unsigned long long a = i < M ? cp.A[i] : 0ull;
+        unsigned long long sum;
+        const unsigned long long x = cp.blockoff[blockIdx.x] + ka_cta256_prefix64(a, sum);
+        if (i < M) cp.A[i] = x;
+        if (i + 1 == M) cp.A[M] = x + a;
+    }
+}
+
+// CAPS: whether a part opened at a position with A = a0 may end at j (j > that position + 1) within the data cap.
+template <bool CAPS>
+__device__ __forceinline__ bool ka_wave_part_in(const KaWaveCaps& cp, uint32_t j, unsigned long long a0) {
+    if constexpr (CAPS) return cp.A[j] - a0 <= cp.in;
+    return true;
 }
 
 // grid ceil(Q / 256), 256 threads: J_0[i] = the last j in (i, e] with S[j] - S[i] <= room, e the end of i's wave, and M in
 // place of e. A position whose own record does not fit reports its ROW, so the lowest input row wins. BACK: the last j that
 // also keeps R[j] - R[i] <= room (both conditions are monotone in j); a record that does not fit on either side reports the
-// longer one-record document.
-template <bool BACK>
-__global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWaveParts pp, const KaWaveBack bk) {
+// longer one-record document. CAPS: j also at most i + Lr, and A[j] - A[i] <= Lx for j > i + 1 (monotone too: a >= 0).
+template <bool BACK, bool CAPS>
+__global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWaveParts pp, const KaWaveBack bk, const KaWaveCaps cp) {
     const uint32_t M = (uint32_t)*pp.d.n_rows;
     const uint32_t i = blockIdx.x * 256u + threadIdx.x;
     if (i >= M) return;
@@ -359,9 +427,11 @@ __global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWavePart
             return;
         }
         uint32_t lo = i + 1, hi = e;   // S[lo] <= lim and R[lo] <= lim_r
+        unsigned long long a0 = 0;   // CAPS: the search ends at i + Lr, and a run holds at most Lx above A[i]
+        if constexpr (CAPS) hi = (uint32_t)min((unsigned long long)e, (unsigned long long)i + cp.rows), a0 = cp.A[i];
         while (lo < hi) {
             const uint32_t mid = (lo + hi + 1) >> 1;
-            if ((long long)pp.S[mid] <= lim && (long long)bk.R[mid] <= lim_r) lo = mid; else hi = mid - 1;
+            if ((long long)pp.S[mid] <= lim && (long long)bk.R[mid] <= lim_r && ka_wave_part_in<CAPS>(cp, mid, a0)) lo = mid; else hi = mid - 1;
         }
         pp.next[i] = (int32_t)(lo == e ? M : lo);
         return;
@@ -372,9 +442,11 @@ __global__ void __launch_bounds__(256) ka_wave_part_next_kernel(const KaWavePart
         return;
     }
     uint32_t lo = i + 1, hi = e;   // S[lo] <= lim
+    unsigned long long a0 = 0;   // CAPS: the search ends at i + Lr, and a run holds at most Lx above A[i]
+    if constexpr (CAPS) hi = (uint32_t)min((unsigned long long)e, (unsigned long long)i + cp.rows), a0 = cp.A[i];
     while (lo < hi) {
         const uint32_t mid = (lo + hi + 1) >> 1;
-        if ((long long)pp.S[mid] <= lim) lo = mid; else hi = mid - 1;
+        if ((long long)pp.S[mid] <= lim && (!CAPS || ka_wave_part_in<CAPS>(cp, mid, a0))) lo = mid; else hi = mid - 1;
     }
     pp.next[i] = (int32_t)(lo == e ? M : lo);
 }

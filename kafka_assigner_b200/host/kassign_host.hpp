@@ -23,6 +23,7 @@
 //   kassign::planWaves                                <->  a new assignment cut on the device into waves in which no broker
 //                                                          receives more than a budget, one document per wave
 //   kassign::setWaveRule                              <->  the wave rule of those plans: greedy, or first fit
+//   kassign::setPartCaps                              <->  the most partitions and the most data one part of a wave holds
 //   kassign::brokerUsage                              <->  what every broker holds across a wave plan: its peak, the wave of
 //                                                          the peak and the first wave over its capacity
 //   kassign::newAssignmentJson                        <->  the org.json emitter (KafkaAssignmentGenerator.java:169-186)
@@ -281,6 +282,22 @@ public:
     }
     int32_t waveRule() const { return ka_ctx_wave_rule(ctx_); }
 
+    // The part caps of every planWaveParts / planWavePartsRollback call of this instance (ka_ctx_set_part_caps): a part holds at
+    // most maxPartRows partitions, and moves at most maxPartIn (weight x the partition's new replicas, summed over the part)
+    // unless it is a single partition; 0 is no cap. The plan and its summaries stay those of the uncapped call. A negative
+    // value throws KassignError(KA_ERR_BAD_ARG) and leaves the caps as they were.
+    void setPartCaps(int64_t maxPartRows, int64_t maxPartIn) {
+        const int32_t rc = ka_ctx_set_part_caps(ctx_, maxPartRows, maxPartIn);
+        if (rc != KA_OK)
+            throw KassignError(rc, "(part caps " + std::to_string(maxPartRows) + ", " + std::to_string(maxPartIn) + ")");
+    }
+    // {maxPartRows, maxPartIn}, 0 where there is no cap.
+    std::pair<int64_t, int64_t> partCaps() const {
+        std::pair<int64_t, int64_t> caps{0, 0};
+        ka_ctx_part_caps(ctx_, &caps.first, &caps.second);
+        return caps;
+    }
+
     // A new assignment cut into waves (ka_plan_waves): consecutive documents in which no broker of this instance's table receives
     // more than maxBrokerIn (weighted). waves[v] holds the changed partitions of wave v + 1, topics in input order, each
     // printable with newAssignmentJson; unchanged partitions are in no wave.
@@ -337,6 +354,8 @@ public:
     // the wave) order, partWave[d] the wave (1..W) of parts[d]; with maxDocBytes >= the longest wave document, parts equals
     // planWavesJson(...).docs. A partition whose one-record document exceeds maxDocBytes gives KA_ERR_LIMIT with a = its row
     // and b = that length. Topic names the device refuses (ka_json_name_refused) take the host emitter and the same cut on the host.
+    // The part caps of setPartCaps cut finer on both paths: a partition also opens a new part when the current one holds
+    // maxPartRows partitions, or would move more than maxPartIn.
     struct WaveParts {
         ka_status status;   // re-throw with throwForStatus; on an error summary, parts and partWave are empty
         std::vector<ka_wave_summary> summary;
@@ -360,6 +379,7 @@ public:
     // maxDocBytes; when no current list prints longer than its new one, parts and partWave are those of planWaveParts. A
     // partition whose one-record document on either side exceeds maxDocBytes gives KA_ERR_LIMIT with a = its row and b = the
     // longer length. Topic names the device refuses (ka_json_name_refused) take the host emitters and the same cut on the host.
+    // The part caps of setPartCaps apply as in planWaveParts.
     struct WaveRollback {
         ka_status status;   // re-throw with throwForStatus; on an error summary, parts, rollback and partWave are empty
         std::vector<ka_wave_summary> summary;
@@ -853,10 +873,19 @@ inline KafkaTopicAssigner::WaveRollback KafkaTopicAssigner::waveDocuments(const 
         res = WaveRollback{plan.status, plan.summary, {}, {}, {}, plan.sendSummary};
         if (res.status.code == KA_OK && L < 1) res.status.code = KA_ERR_BAD_ARG;
         if (res.status.code != KA_OK) return WaveRollback{res.status, {}, {}, {}, {}, {}};
+        // the part caps of ka_ctx_set_part_caps: the most records of a part, the most data it moves (past its first record)
+        const std::pair<int64_t, int64_t> caps = maxDocBytes ? partCaps() : std::pair<int64_t, int64_t>{0, 0};
+        const int64_t maxRows = caps.first > 0 ? caps.first : INT64_MAX, maxIn = caps.second > 0 ? caps.second : INT64_MAX;
         std::vector<std::vector<std::pair<std::string, std::string>>> recs(plan.summary.size());   // (record, rollback record)
+        std::vector<std::vector<int64_t>> moved(plan.summary.size());   // every record's weight x its receivers
         for (size_t t = 0; t < f.names.size(); ++t)
             for (int64_t r = f.partOff[t]; r < f.partOff[t + 1]; ++r) {
                 if (rowWave[r] == 0) continue;
+                int64_t receivers = 0;
+                for (int32_t j = 0; j < p.newLen[r]; ++j)
+                    receivers += std::find(f.cur.begin() + f.repOff[r], f.cur.begin() + f.repOff[r + 1], p.newBroker[r * p.stride + j]) ==
+                                 f.cur.begin() + f.repOff[r + 1];
+                moved[rowWave[r] - 1].push_back(receivers * (p.w.empty() ? 1 : p.w[r]));
                 std::string rec, back;
                 appendRecord(rec, f.names[t], f.partId[r], p.newBroker.data() + r * p.stride, (size_t)p.newLen[r]);
                 if (rollback)
@@ -872,21 +901,27 @@ inline KafkaTopicAssigner::WaveRollback KafkaTopicAssigner::waveDocuments(const 
                 recs[rowWave[r] - 1].emplace_back(std::move(rec), std::move(back));
             }
         for (size_t v = 0; v < recs.size(); ++v) {
-            // the current part's two document sizes, 0 before the wave's first; without rollback the empty back side never binds
-            int64_t size = 0, backSize = 0;
-            for (const auto& rb : recs[v]) {
-                const int64_t n = (int64_t)rb.first.size(), m = (int64_t)rb.second.size();
-                if (size > 0 && size + 1 + n <= L && backSize + 1 + m <= L) {
+            // the current part's two document sizes, 0 before the wave's first; without rollback the empty back side never binds;
+            // its records and the data they move
+            int64_t size = 0, backSize = 0, rows = 0, in = 0;
+            for (size_t k = 0; k < recs[v].size(); ++k) {
+                const auto& rb = recs[v][k];
+                const int64_t n = (int64_t)rb.first.size(), m = (int64_t)rb.second.size(), a = moved[v][k];
+                if (size > 0 && size + 1 + n <= L && backSize + 1 + m <= L && rows < maxRows && in + a <= maxIn) {
                     res.parts.back().insert(res.parts.back().size() - 14, "," + rb.first);
                     if (rollback) res.rollback.back().insert(res.rollback.back().size() - 2, "," + rb.second);
                     size += 1 + n;
                     backSize += 1 + m;
+                    rows += 1;
+                    in += a;
                 } else {
                     res.parts.push_back("{\"partitions\":[" + rb.first + "],\"version\":1}");
                     if (rollback) res.rollback.push_back("{\"version\":1,\"partitions\":[" + rb.second + "]}");
                     res.partWave.push_back((int32_t)v + 1);
                     size = 29 + n;
                     backSize = 29 + m;
+                    rows = 1;
+                    in = a;
                 }
             }
         }
